@@ -238,10 +238,11 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
     };
     if (!kSelf) {
         // ============================ producer warp =============================================
+        // after its last claim it skips the consumer loop but does not return: every warp of the CTA must reach the
+        // final __syncthreads() (a CTA barrier that some threads never reach is undefined)
         if (warp == kConsumerWarps) {
             for (int it = 0;; ++it)
                 if (!claim_stage(it, std::true_type{})) break;
-            return;
         }
     } else if (warp < kAhead) {                            // prologue: utterances 0 .. kAhead-1
         claim_stage(warp, std::false_type{});
@@ -272,7 +273,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
     const int4 *dctk4 = sm.dct + 3 * (lane < 24 ? lane : 0);
 
     u32 gidx = 0;   // frames of this CTA's stream before the current utterance
-    for (int it = 0;; ++it) {
+    for (int it = 0; kSelf || warp < kConsumerWarps; ++it) {           // w15's producer warp never enters
         if (kSelf && warp == it % kConsumerWarps) claim_stage(it + kAhead, std::false_type{});
         const int s = it % kNBuf;
         mbar_wait(&sm.full[s], (it / kNBuf) & 1);
@@ -462,7 +463,8 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
 // Variants (one persistent CTA per SM; threads per CTA are capped at floor(65536 / regs / 128) * 128):
 //   s16: 16 warps, all consumers, staging as a rotating side job, 3-deep ring   (default)
 //   w15: 15 consumers + 1 dedicated producer warp, 3-deep ring   (SR_MFCC_WARPS=15; 5 % slower: one scheduler
-//        carries only 3 working warps)
+//        carries only 3 working warps). Its producer warp used to return after its last claim, leaving the final
+//        __syncthreads() to the consumers alone, which is undefined; it now skips the consumer loop and joins it.
 // Measured and dropped: the asm's 3-multiply twiddle form (one IMAD traded for a subtract: 4.91 ms vs 4.76), forcing the
 // C+-D sums of the butterflies onto the ALU pipe as three-input adds (4.86 vs 4.76), two 16-bit
 // stores instead of PRMT + one 32-bit store in block A (4.86 vs 4.80), 20 warps @ 96 regs (5.29 ms vs 5.31), 24 warps @ 80 regs (5.48 ms) -- the half-rate ALU and

@@ -115,24 +115,74 @@ def test_mfcc_unaligned_utterance_stride(handle, ora, U):
     assert ob.ftr_equal(handle.mfcc(pcm, seg, atap), ora.mfcc_batch(pcm, seg, atap))
 
 
-@pytest.mark.parametrize("B", [1, 2, 37, 131, 132, 133, 147, 148, 149, 263, 264, 265, 295, 296, 297, 395, 396, 397, 445, 1000])
-def test_mfcc_batch_sizes_around_the_cta_count(handle, ora, B):
+_MFCC_SIZES = [1, 2, 37, 131, 132, 133, 147, 148, 149, 263, 264, 265, 295, 296, 297, 395, 396, 397, 445, 1000]
+_MFCC_MIXES = ["rejected_runs", "all_rejected", "all_1", "all_119", "alt_1_119"]
+
+
+def _mfcc_mix_segments(mix, B, U, rng):
+    """segments of one skewed mix; U >= 9839 leaves room for 120-frame segments after a start of up to 79"""
+    one, f119, f120 = 160, 118 * 80 + 160, 119 * 80 + 160
+    st = rng.integers(1, 80, B)
+    if mix == "all_1":
+        ln = np.full(B, one)
+    elif mix == "all_119":
+        ln = np.full(B, f119)
+    elif mix == "alt_1_119":
+        ln = np.where(np.arange(B) % 2 == 0, one, f119)
+    else:
+        ln = 160 + 80 * rng.integers(0, 119, B) + rng.integers(0, 80, B)      # 1..119 frames
+        rej = np.ones(B, bool)
+        if mix == "rejected_runs":                     # 1..3 valid utterances, then 20..30 rejected ones, and so on
+            i = 0
+            while i < B:
+                n_ok = int(rng.integers(1, 4))
+                rej[i:i + n_ok] = False
+                i += n_ok + int(rng.integers(20, 31))
+        kind = np.arange(B) % 3                        # rejected: 120 frames (MFCC.C:103-107), < one frame, NULL
+        ln = np.where(rej & (kind == 0), f120 + rng.integers(0, 80, B), ln)
+        ln = np.where(rej & (kind == 1), rng.integers(0, 160, B), ln)
+    seg = np.stack([st, st + ln], 1).astype(np.uint32)
+    if mix in ("rejected_runs", "all_rejected"):
+        seg[rej & (kind == 2)] = [ob.NULL, ob.NULL]
+        assert rej.sum() >= min(B, 20) or (mix == "rejected_runs" and B <= 3)     # a run starts with 1..3 valid ones
+    assert (seg[seg[:, 1] != ob.NULL, 1] <= U).all()
+    return seg
+
+
+@pytest.mark.parametrize("B,mix", [pytest.param(B, "ragged", id=str(B)) for B in _MFCC_SIZES] +
+                         [pytest.param(B, m, id="%s-%d" % (m, B)) for m in _MFCC_MIXES for B in _MFCC_SIZES])
+def test_mfcc_batch_sizes_around_the_cta_count(handle, ora, B, mix):
     """mfcc_kernel hands utterances out with an atomic counter and ends a CTA's walk with an end marker in its staging
     ring; batch sizes around 1x / 2x / 3x the CTA count make every mix of (utterance, marker) land in a CTA's first
     ring slots, in either claim order (the first version lost an utterance that sat behind a marker); 132 is the H100's
-    CTA count. Run twice: the
-    last CTA out re-arms the counter for the next launch."""
-    U = 4003
-    pcm = sr_b200.synth_pcm_host(B, U, 0x4A00 + B)
-    rng = np.random.default_rng(B)
-    st = rng.integers(1, 900, B)
-    en = np.minimum(st + rng.integers(160, 3000, B), U)
-    seg = np.stack([st, en], 1).astype(np.uint32)
+    CTA count. The mixes skew the work per ring slot: a rejected utterance (F = 0) passes the ring without a frame loop,
+    yet every consumer warp must still arrive on its `empty` barrier; runs of 20+ of them, all rejected, all 1 frame, all
+    119 frames, 1 / 119 alternating. Run twice: the last CTA out re-arms the counter for the next launch; an all-NULL
+    launch in between overwrites every frm_num, so an utterance the second launch lost cannot show the first launch's rows."""
+    if mix == "ragged":
+        U = 4003
+        pcm = sr_b200.synth_pcm_host(B, U, 0x4A00 + B)
+        rng = np.random.default_rng(B)
+        st = rng.integers(1, 900, B)
+        en = np.minimum(st + rng.integers(160, 3000, B), U)
+        seg = np.stack([st, en], 1).astype(np.uint32)
+    else:
+        U = 9843
+        pcm = sr_b200.synth_pcm_host(B, U, 0x4B00 + B, 2)
+        seg = _mfcc_mix_segments(mix, B, U, np.random.default_rng(0x4B00 + B))
     atap = np.zeros(B, sr_b200.ATAP_DTYPE)
     atap["mid_val"] = 2000
-    want = ora.mfcc_batch(pcm, seg, atap)
+    valid = (seg != ob.NULL).all(axis=1)
+    want = ora.mfcc_batch(pcm[valid], seg[valid], atap[valid])
+    if mix == "all_rejected":
+        assert (want["frm_num"] == 0).all()
+    elif mix != "ragged":
+        assert (want["frm_num"] > 0).any()
+    nulls = np.full((B, 2), ob.NULL, np.uint32)
     for _ in range(2):
-        assert ob.ftr_equal(handle.mfcc(pcm, seg, atap), want)
+        got = handle.mfcc(pcm, seg, atap)
+        assert ob.ftr_equal(got[valid], want) and (got["frm_num"][~valid] == 0).all()
+        assert (handle.mfcc(pcm, nulls, atap)["frm_num"] == 0).all()
 
 
 def test_mfcc_segment_at_sample_zero_reads_previous_utterance(handle, ora):
@@ -150,6 +200,88 @@ def test_mfcc_segment_at_sample_zero_reads_previous_utterance(handle, ora):
         view = flat[b * U: b * U + 1 + U].copy().reshape(1, -1)
         want = ora.mfcc_batch(view, np.array([[1, 1601]], np.uint32), atap[b:b + 1])
         assert ob.ftr_equal(got[b:b + 1], want), b
+
+
+def _windowed(x, prv, mid, hamm):
+    """vc_temp of MFCC.C:118-121 in the C types: (x - mid) - (prv - mid)*95/100 in s32 with truncating division, times
+    hamm[i], / 1000 truncating, cast to s16 (no intermediate here leaves s32)"""
+    def cdiv(a, d):                                        # C division: truncates toward zero
+        return np.sign(a) * (np.abs(a) // d)
+    cur, p = x.astype(np.int64) - mid, prv.astype(np.int64) - mid
+    t = cur - cdiv(p * 95, 100)
+    return cdiv(t * hamm, 1000).astype(np.int16)
+
+
+def _full_scale_frames(targets, mids, prv0, hamm):
+    """one 160-sample frame per row of `targets`: sample n is the u16 (0..65535) whose windowed value is closest to
+    targets[:, n], given the sample chosen before it (prv0 for n = 0)"""
+    cand = np.arange(65536, dtype=np.int64)[None, :]
+    mid = np.asarray(mids, np.int64)[:, None]
+    prv = np.asarray(prv0, np.int64)[:, None]
+    out = np.zeros(targets.shape, np.uint16)
+    for n in range(160):
+        w = _windowed(cand, prv, mid, int(hamm[n])).astype(np.int64)
+        out[:, n] = np.argmin(np.abs(w - targets[:, n:n + 1]), axis=1)
+        prv = out[:, n:n + 1].astype(np.int64)
+    return out
+
+
+def test_mfcc_largest_magnitude_frames(handle, ora):
+    """one-frame segments whose windowed samples sit at +-full scale: constants, the +-alternation, and
+    +-32767*sign(cos(2 pi k n / 1024 + phi)) for a spread of bins k. They reach the largest stage-0 values (+-8192) and
+    final FFT components near the bound 160*32768/1024 = 5120 that the pruned FFT's no-wrap proof (sr_mfcc.cu header)
+    rests on -- synthetic speech and random PCM stay far below it"""
+    hamm = np.load(os.path.join(HERE, "golden", "ref_tables.npz"))["hamm"].astype(np.int64)
+    n = np.arange(160)
+    tg = [np.full(160, 32767), np.full(160, -32768), np.where(n % 2 == 0, 32767, -32768), np.where(n % 2 == 0, -32768, 32767)]
+    for k in (0, 1, 2, 3, 5, 8, 13, 21, 34, 55, 89, 144, 233, 256, 377, 448, 500, 511):
+        for phi in (0.0, np.pi / 3):
+            tg.append(np.where(np.cos(2 * np.pi * k * n / 1024 + phi) >= 0, 32767, -32768))
+    targets = np.stack(tg).astype(np.int64)
+    B, U = targets.shape[0], 173
+    rng = np.random.default_rng(5120)
+    mids = rng.choice([0, 2048, 32768, 65535], B)
+    mids[:4] = 2048
+    prv0 = rng.integers(0, 65536, B)
+    frames = _full_scale_frames(targets, mids, prv0, hamm)
+    pcm = rng.integers(0, 65536, (B, U)).astype(np.uint16)
+    pcm[:, 2] = prv0                                       # x[-1] of the segment [3, 163)
+    pcm[:, 3:163] = frames
+    seg = np.tile(np.array([3, 163], np.uint32), (B, 1))
+    atap = np.zeros(B, sr_b200.ATAP_DTYPE)
+    atap["mid_val"] = mids
+    # the frames reach what they are built for, on the oracle's FFT of the same windowed samples
+    w = np.stack([_windowed(pcm[b, 3:163], pcm[b, 2:162], int(mids[b]), hamm) for b in range(B)])
+    assert (np.abs(w.astype(np.int64)) >= 32000).mean() > 0.9
+    st0 = w.astype(np.int32) >> 2                          # stage 0 of a real frame: w >> 2
+    assert (st0 == -8192).any() and (st0 == 8191).any()
+    packed = np.zeros((B, 1024), np.uint32)
+    packed[:, :160] = w.view(np.uint16)
+    raw = ora.fft_raw(packed)
+    comp = np.maximum(np.abs(raw.view(np.int16)[:, 0::2].astype(np.int32)), np.abs(raw.view(np.int16)[:, 1::2].astype(np.int32)))
+    assert 0.9 * 5120 <= comp.max() <= 8209
+    assert np.array_equal(handle.fft_raw(packed), raw)
+    got = handle.mfcc(pcm, seg, atap)
+    assert (got["frm_num"] == 1).all()
+    assert ob.ftr_equal(got, ora.mfcc_batch(pcm, seg, atap))
+
+
+def test_mfcc_tests_under_the_w15_variant():
+    """SR_MFCC_WARPS=15 selects mfcc_kernel_w15 (15 consumer warps + a dedicated producer warp, relaxed barrier waits).
+    The library reads the switch once per process, so this file's MFCC tests run again in a child pytest"""
+    import re
+    import subprocess
+    import sys
+    if os.environ.get("SR_MFCC_WARPS"):
+        pytest.skip("already running under a chosen MFCC variant")
+    env = dict(os.environ, SR_MFCC_WARPS="15", SR_NO_BUILD="1")
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
+        "-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.abspath(__file__), "-k", "mfcc and not geom"]
+    r = subprocess.run(cmd, cwd=os.path.dirname(HERE), env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
+                       timeout=1800)
+    assert r.returncode == 0, r.stdout[-4000:]
+    m = re.search(r"(\d+) passed", r.stdout)
+    assert m and int(m.group(1)) >= 100 and " failed" not in r.stdout, r.stdout[-4000:]
 
 
 # ---- noise_atap + VAD ---------------------------------------------------------------------------------
@@ -216,6 +348,61 @@ def test_noise_atap_windows_longer_than_one_chunk(handle, ora):
             a = ora.noise_atap(pcm[b], n_len)
             assert a.tobytes() == atap[b:b + 1].tobytes(), (n_len, b)
             assert ora.vad(pcm[b], U, a).tolist() == seg[b].reshape(-1).tolist(), (n_len, b)
+
+
+def _first_bad_rows(got, want):
+    return np.nonzero((got != want).reshape(got.shape[0], -1).any(axis=1))[0][:8].tolist()
+
+
+@pytest.mark.parametrize("U,sized_for", [(8000, "vad"), (16000, "vad"), (40000, "vad"), (65535, "vad"), (16000, "noise_atap")])
+def test_vad_handout_around_sms_times_warps(ora, U, sized_for):
+    """vad_kernel: one CTA per SM, one warp per utterance, the next utterance claimed early from an atomic counter that
+    the last warp out re-arms. Batch sizes n*W - 1, n*W, n*W + 1 (n = 1, 2) for W = SMs x warps per CTA, where the warps
+    per CTA shrink with U (20 at 8 000 and for noise_atap alone, 18 at 16 000, 15 at 40 000, 13 at 65 535): noise_atap
+    then VAD, each launched twice on the same handle into outputs refilled with a sentinel, against the oracle"""
+    import torch
+    dev = torch.device("cuda:0")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+
+    def warps_per_cta(buf_len):                        # the formula of launch_vad (sr_vad.cu); noise_atap alone: buf_len 0
+        max_frames = 2 * ((((buf_len - 160 + 79) // 80) if buf_len > 160 else 0) + 2)
+        per_warp = 2 * (2560 * 2 + 32) + max_frames * 4
+        return min(220 * 1024 // per_warp, 20)
+
+    W = sms * warps_per_cta(U if sized_for == "vad" else 0)
+    assert warps_per_cta(0) == 20 and warps_per_cta(U) == {8000: 20, 16000: 18, 40000: 15, 65535: 13}[U]
+    sizes = [n * W + d for n in (1, 2) for d in (-1, 0, 1)]
+    Bmax = sizes[-1]
+    pcm = sr_b200.synth_pcm_host(Bmax, U, 0x7AD00000 + U, max(1, (U - 3200) // 5000))
+    rng = np.random.default_rng(U)
+    for r in (0, W - 1, W, 2 * W):
+        pcm[r] = 2048                                  # silence: no segment
+    for r in (1, W + 1, 2 * W - 1):
+        pcm[r] = rng.integers(0, 65536, U)             # full range
+    want_a = np.concatenate([ora.noise_atap(pcm[b], 2400) for b in range(Bmax)])
+    want_s = np.stack([ora.vad(pcm[b], U, want_a[b:b + 1]) for b in range(Bmax)])
+    assert (want_s[:, 1] != ob.NULL).mean() > 0.9
+    h = sr_b200.Handle(0)
+    st = torch.cuda.Stream(dev)
+    h.set_stream(st.cuda_stream)
+    with torch.cuda.stream(st):
+        pcm_d = torch.from_numpy(pcm.view(np.int16)).to(dev)
+        at = torch.empty(Bmax * 12, dtype=torch.uint8, device=dev)
+        sg = torch.empty(Bmax * 6, dtype=torch.int32, device=dev)
+        for B in sizes:
+            for run in range(2):
+                at.fill_(0xA5 + run)
+                sg.fill_(0x5A5A5A5A + run)
+                h.noise_atap_dev(pcm_d.data_ptr(), U, B, 2400, at.data_ptr())
+                h.vad_dev(pcm_d.data_ptr(), U, B, U, at.data_ptr(), sg.data_ptr())
+                st.synchronize()
+                got_a = at.cpu().numpy()
+                got_s = sg.cpu().numpy().view(np.uint32).reshape(Bmax, 6)
+                assert (got_a[B * 12:] == 0xA5 + run).all() and (got_s[B:] == 0x5A5A5A5A + run).all(), (B, run)
+                ga = got_a[:B * 12].view(np.uint8).reshape(B, 12)
+                assert np.array_equal(ga, want_a[:B].view(np.uint8).reshape(B, 12)), (B, run, _first_bad_rows(ga, want_a[:B].view(np.uint8).reshape(B, 12)))
+                assert np.array_equal(got_s[:B], want_s[:B]), (B, run, _first_bad_rows(got_s[:B], want_s[:B]))
+    h.close()
 
 
 def test_vad_and_mfcc_fuzz_with_arbitrary_atap(handle, ora):
@@ -627,6 +814,165 @@ def test_device_pointer_api_on_torch_stream(ora):
     h.close()
 
 
+def _to_dev(a):
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).to("cuda:0")
+
+
+@pytest.mark.parametrize("U", [8000, 8003, 16000])
+def test_unaligned_device_pcm_vad_mfcc_recognise(ora, U):
+    """the _dev entry points take pcm with 2-byte alignment (speech_recog.h). A batch base that is not 16-byte aligned makes
+    vad_kernel stage with plain loads (chunk_issue) and mfcc_kernel with its cooperative copy (stage_utterance), which
+    pins x[-1] of a segment at sample 0 of row 0 to mid_val on its own; noise windows past 2 560 samples read global
+    memory from the unaligned base"""
+    import torch
+    dev = torch.device("cuda:0")
+    B, T = 40, 8
+    pcm = sr_b200.synth_pcm_host(B, U, 0xA1160000 + U, 1 if U < 16000 else 2)
+    rng = np.random.default_rng(U)
+    pcm[3] = 2048                                      # VAD fails
+    pcm[5] = rng.integers(0, 65536, U)                 # full range
+    # MFCC segments: ragged, 1 frame, < 1 frame, 119 and 120 frames where U allows, NULL, ending at the batch end
+    st_ = rng.integers(1, 900, B)
+    seg = np.stack([st_, np.minimum(st_ + rng.integers(160, 4000, B), U)], 1).astype(np.uint32)
+    seg[0] = (0, 1600)                                 # x[-1] of the whole batch: pinned to mid_val
+    seg[1] = (1, 161)
+    seg[2] = (7, 7 + 159)
+    seg[4] = (ob.NULL, ob.NULL)
+    if U >= 2 + 119 * 80 + 160:
+        seg[6] = (1, 1 + 118 * 80 + 160)
+        seg[7] = (2, 2 + 119 * 80 + 160)
+    seg[B - 1] = (U - 1999, U)
+    atm = np.zeros(B, sr_b200.ATAP_DTYPE)
+    atm["mid_val"] = rng.integers(0, 4096, B)
+    atm["mid_val"][0] = 2100
+    valid = (seg != ob.NULL).all(axis=1)
+    # oracle rows of U + 1 samples: row b's own samples after the sample before them in the contiguous batch (mid_val for
+    # row 0), i.e. x[-1] as the kernel sees it
+    flat = np.concatenate([[np.uint16(2100)], pcm.reshape(-1)])
+    rows1 = np.stack([flat[b * U: b * U + U + 1] for b in range(B)])
+    want_f = ora.mfcc_batch(rows1[valid], seg[valid] + 1, atm[valid])
+    fv = want_f["frm_num"]
+    assert fv[0] == 19 and fv[1] == 1 and fv[2] == 0 and (U < 2 + 119 * 80 + 160 or (fv[5] == 119 and fv[6] == 0))
+    want_a = {n_len: np.concatenate([ora.noise_atap(pcm[b], n_len) for b in range(B)]) for n_len in (2400, 4800)}
+    want_s = np.stack([ora.vad(pcm[b], U, want_a[2400][b:b + 1]) for b in range(B)])
+    tpl = sr_b200.synth_pcm_host(T, 8000, 0x7E3A0000)
+    h = sr_b200.Handle(0)
+    bank, est = h.enrol(tpl, 2400)
+    assert (est == 0).all()
+    h.set_bank(bank, T, 4096)
+    want_r = ora.recognise_batch(pcm, 2400, bank, T, 4096)
+    assert set(want_r["status"].tolist()) >= {0, 1}
+    st = torch.cuda.Stream(dev)
+    h.set_stream(st.cuda_stream)
+    with torch.cuda.stream(st):
+        buf = torch.zeros(B * U + 16, dtype=torch.int16, device=dev)
+        seg_d, atm_d = _to_dev(seg), _to_dev(atm)
+        for k in (1, 3, 7):
+            buf.zero_()
+            buf[k:k + B * U] = torch.from_numpy(pcm.view(np.int16).reshape(-1)).to(dev)
+            ptr = buf.data_ptr() + 2 * k
+            assert ptr % 16 != 0
+            for n_len in (2400, 4800):
+                at = torch.full((B * 12,), 0xA5, dtype=torch.uint8, device=dev)
+                h.noise_atap_dev(ptr, U, B, n_len, at.data_ptr())
+                st.synchronize()
+                assert at.cpu().numpy().tobytes() == want_a[n_len].tobytes(), (k, n_len)
+            sg = torch.full((B * 6,), 0x5A5A5A5A, dtype=torch.int32, device=dev)
+            h.vad_dev(ptr, U, B, U, at.data_ptr(), sg.data_ptr())        # atap of the 4 800-sample window
+            st.synchronize()
+            want_s48 = np.stack([ora.vad(pcm[b], U, want_a[4800][b:b + 1]) for b in range(B)])
+            assert np.array_equal(sg.cpu().numpy().view(np.uint32).reshape(B, 6), want_s48), k
+            ft = torch.full((B * sr_b200.FTR_BYTES,), 0x5A, dtype=torch.uint8, device=dev)
+            h.mfcc_dev(ptr, U, B, seg_d.data_ptr(), 2, atm_d.data_ptr(), ft.data_ptr())
+            st.synchronize()
+            got_f = ft.cpu().numpy().view(sr_b200.FTR_DTYPE)
+            assert ob.ftr_equal(got_f[valid], want_f) and (got_f["frm_num"][~valid] == 0).all(), k
+            out = {"atap": torch.full((B * 12,), 0xA5, dtype=torch.uint8, device=dev),
+                   "seg_off": torch.full((B * 6,), 0x5A5A5A5A, dtype=torch.int32, device=dev),
+                   "ftr": torch.full((B * sr_b200.FTR_BYTES,), 0x5A, dtype=torch.uint8, device=dev),
+                   "score": torch.full((B * T,), 0x5A5A5A5A, dtype=torch.int32, device=dev),
+                   "status": torch.full((B,), 0x5A, dtype=torch.uint8, device=dev)}
+            for key in ("best_idx", "best_dis", "cmd"):
+                out[key] = torch.full((B,), 0x5A5A5A5A, dtype=torch.int32, device=dev)
+            h.recognise_dev(ptr, U, B, 2400, **{key: v.data_ptr() for key, v in out.items()})
+            st.synchronize()
+            got = {key: v.cpu().numpy() for key, v in out.items()}
+            assert got["atap"].tobytes() == want_a[2400].tobytes(), k
+            assert np.array_equal(got["seg_off"].view(np.uint32).reshape(B, 6), want_s), k
+            got["ftr"] = got["ftr"].view(sr_b200.FTR_DTYPE)
+            got["seg_off"] = got["seg_off"].view(np.uint32)
+            for key in ("score", "best_idx", "best_dis", "cmd"):
+                got[key] = got[key].view(np.uint32)
+            _cmp_recog(got, want_r)
+    h.close()
+
+
+@pytest.mark.parametrize("stride", [4096, 2860])
+def test_device_bank_wider_than_one_tile_rewritten_in_place(ora, stride):
+    """sr_set_bank_dev with T = 70 > 32: the headers come back with a strided D2H copy and the slots are walked in
+    ascending frm_num order. Rewriting the bank in place (slots permuted, frm_num changed, signs erased) and setting the same
+    pointer again keeps the stale order, which may only cost speed: results equal the oracle on the new contents"""
+    import torch
+    dev = torch.device("cuda:0")
+    B, U, T = 96, 8000, 70
+    h = sr_b200.Handle(0)
+    bank, est = h.enrol(sr_b200.synth_pcm_host(T, U, 0x7E3A0000 + stride), 2400, slot_stride=stride)
+    assert (est == 0).all()
+    rng = np.random.default_rng(stride)
+    bad = rng.random(T) < 0.25
+    bank[bad, 0:2] = 0xFF                              # erased flash: save_sign != 12345
+    bank[np.nonzero(~bad)[0][:3], 0:2] = 0             # another wrong sign
+    pcm = sr_b200.synth_pcm_host(B, U, 0xBA2C0000 + stride)
+    pcm[::11] = 2048                                   # VAD fails
+    fin = sr_b200.synth_ftr_host(B, 0xBA2D0000 + stride, 1, 119).view(sr_b200.FTR_DTYPE).reshape(-1)
+
+    def order(b):                                      # the walk order sr_set_bank_dev derives from the headers
+        f = b[:, 2].astype(np.int64) | (b[:, 3].astype(np.int64) << 8)
+        return np.argsort(np.where(f > 119, 0xFFFF, f), kind="stable")
+
+    def check(bank_h):
+        out = {"score": torch.zeros((B, T), dtype=torch.int32, device=dev)}
+        for key in ("best_idx", "best_dis", "cmd"):
+            out[key] = torch.zeros(B, dtype=torch.int32, device=dev)
+        out["status"] = torch.zeros(B, dtype=torch.uint8, device=dev)
+        h.recognise_dev(pcm_d.data_ptr(), U, B, 2400, **{key: v.data_ptr() for key, v in out.items()})
+        st.synchronize()
+        ref = ora.recognise_batch(pcm, 2400, bank_h, T, stride)
+        for key, v in out.items():
+            assert np.array_equal(v.cpu().numpy().view(ref[key].dtype).reshape(ref[key].shape), ref[key]), key
+        assert (ref["status"] == 0).sum() > B // 2 and (ref["score"][ref["status"] == 0] != ob.NULL).any()
+        score, bi, bd = h.dtw(fin, flags=sr_b200.DTW_CHECK_SIGN)
+        want, _ = ora.dtw_batch(fin, bank_h, T, stride, check_sign=1)
+        assert np.array_equal(score, want)
+        key64 = (want.astype(np.uint64) << np.uint64(32)) | np.arange(T, dtype=np.uint64)[None, :]
+        kmin = key64.min(axis=1)
+        assert np.array_equal(bi, (kmin & np.uint64(0xFFFFFFFF)).astype(np.uint32))
+        assert np.array_equal(bd, (kmin >> np.uint64(32)).astype(np.uint32))
+
+    st = torch.cuda.Stream(dev)
+    h.set_stream(st.cuda_stream)
+    with torch.cuda.stream(st):
+        pcm_d = torch.from_numpy(pcm.view(np.int16)).to(dev)
+        bank_d = _to_dev(bank)
+        ptr = bank_d.data_ptr()
+        assert T > 32
+        h.set_bank_dev(ptr, T, stride)
+        check(bank)
+        # in place: permute the slots, shorten / lengthen some templates (rows past the old end are erased flash), erase signs
+        new = bank[rng.permutation(T)].copy()
+        for t in rng.choice(T, 12, replace=False):
+            f = int(rng.integers(1, 120))
+            new[t, 2], new[t, 3] = f & 0xFF, f >> 8
+        new[rng.choice(T, 5, replace=False), 0:2] = 0xFF
+        assert not np.array_equal(order(new), order(bank))
+        bank_d.copy_(_to_dev(new))
+        assert bank_d.data_ptr() == ptr
+        h.set_bank_dev(ptr, T, stride)                 # the same buffer: the order of the old contents is kept
+        check(new)
+    h.close()
+
+
 def test_enrol_and_get_mdl(handle, ora):
     """save_mdl (main.c:121-138 + Flash.C:17-67) as a batch, and the reference's template averaging get_mdl"""
     B, U = 40, 8000
@@ -859,6 +1205,65 @@ def test_geom_b_extension_vs_own_oracle():
     assert ob.ftr_equal(out["ftr"][ok], f[ok])
     sc, _ = po.dtw_batch(f, bank, T, 4096, check_sign=1)
     assert np.array_equal(out["score"][ok], sc[ok]) and ok.sum() >= 30
+    h.close()
+
+
+@pytest.mark.parametrize("arrival", ["lockstep", "ragged"])
+def test_geom_b_streaming_vs_own_oracle(ora, arrival):
+    """streaming pushes on a handle in GEOM_B go to mfcc_geomb_kernel with a row map and a batch size produced on the
+    device: every event equals the port's VAD, then GEOM_B get_mfcc, dtw and argmin of that segment (parity unpinned, as
+    for the batch GEOM_B test)"""
+    po = ob.port()
+    h = sr_b200.Handle(0)
+    h.set_geometry(1)
+    S, L, T = 24, 40000, 6
+    pcm = sr_b200.synth_pcm_host(S, L, 0x5EEDB000, 3)
+    pcm[3] = 2048                                      # a silent stream: no event
+    bank, est = h.enrol(sr_b200.synth_pcm_host(T, 8000, 0x7E3A0000), 2400)
+    assert (est == 0).all()
+    h.set_bank(bank, T, 4096)
+    pool = sr_b200.StreamPool(h, S, L, 2400)
+    events = []
+    if arrival == "lockstep":
+        for n0 in range(0, L, 800):
+            events += pool.push(np.ascontiguousarray(pcm[:, n0:n0 + 800]))
+    else:
+        rng = np.random.default_rng(0xB5)
+        pos = np.zeros(S, np.int64)
+        while (pos < L).any():
+            lens = np.minimum(rng.choice([0, 1, 79, 81, 160, 333, 1601, 4000], S), L - pos)
+            w = int(lens.max())
+            if w == 0:
+                continue
+            chunk = np.zeros((S, w), np.uint16)
+            for s in range(S):
+                chunk[s, :lens[s]] = pcm[s, pos[s]:pos[s] + lens[s]]
+            events += pool.push_ragged(chunk, lens)
+            pos += lens
+    seg, atap = pool.segments()
+    pool.close()
+    for s in range(S):
+        a = po.noise_atap(pcm[s], 2400)
+        assert a.tobytes() == atap[s:s + 1].tobytes(), s
+        assert po.vad(pcm[s], L, a).tolist() == seg[s].reshape(-1).tolist(), s
+    closed = [(s, k) for s in range(S) for k in range(3) if seg[s, k, 1] != ob.NULL]
+    assert sorted((e["stream"], e["segment"]) for e in events) == closed and len(closed) >= 2 * S
+    geometry_differs = 0
+    for e in events:
+        s, k = e["stream"], e["segment"]
+        assert (e["start"], e["end"]) == tuple(seg[s, k])
+        f = po.mfcc_geom_b_batch(pcm[s:s + 1], seg[s, k].reshape(1, 2), atap[s:s + 1])
+        assert e["frm_num"] == int(f["frm_num"][0]), e
+        if e["frm_num"] == 0:
+            assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (2, 0, ob.NULL, 0), e
+            continue
+        sc, _ = po.dtw_batch(f, bank, T, 4096, check_sign=1)
+        kmin = ((sc[0].astype(np.uint64) << np.uint64(32)) | np.arange(T, dtype=np.uint64)).min()
+        assert e["status"] == 0 and e["best_dis"] == int(kmin >> np.uint64(32)), e
+        assert e["best_idx"] == int(kmin & np.uint64(0xFFFFFFFF)) and e["cmd"] == e["best_idx"] // 4, e
+        ref_geom = ora.mfcc_batch(pcm[s:s + 1], seg[s, k].reshape(1, 2), atap[s:s + 1])
+        geometry_differs += int(ref_geom["frm_num"][0]) != e["frm_num"]
+    assert geometry_differs > 0                        # the 200-sample framing ran, not the reference's 160
     h.close()
 
 
