@@ -4,74 +4,81 @@
 //
 // Mapping: one thread per (utterance, template) pair -- the walk is inherently sequential and data
 // dependent; parallelism is across the B x T pairs. A CTA keeps a tile of up to 32 templates in shared
-// memory (loaded once, reused for every utterance the CTA visits). Its 16 warps are split into groups
+// memory (loaded once, reused for every utterance the CTA visits). Its 32 warps are split into groups
 // of Wg warps; a group stages NU utterances at a time and its 32*Wg lanes walk the NU x Tt pairs
 // (flattened), so lanes stay busy when Tt < 32 (the host picks NU/Wg for the tile width).
-// Rows are staged as BYTE PLANES (low bytes | high bytes of the 12 s16), so that
-//   sum (a-b)^2 = |a|^2 + |b|^2 - 2 a.b        (exact in Z/2^32, the ring the reference accumulates in)
-// costs 12 IDP.4A per local distance on packed registers: a.b = 65536*HH + 256*(HL+LH) + LL.
-// dtw_limit is evaluated as a per-column y interval (ya, yb) updated only when x moves.
-#include "sr_common.cuh"
+// dtw_limit is evaluated as a per-column y interval (ya, yb) updated only when x moves. Rows, header decode, the walk and
+// the epilogue are the shared core of sr_dtw_core.cuh.
+#include "sr_dtw_core.cuh"
 
 namespace srk {
 
 constexpr int kDtwWarps = 16;
-constexpr int kK2Warps = 32;                // dtw_kernel: 1024 threads x 64 registers, more walks in flight per SM
-constexpr int kTileT = 32;
+constexpr int kK2Warps = 32;                // lane-packed kernels: 1024 threads x 64 registers, more walks in flight per SM
+constexpr int kTileHdr = 256;               // after the tile: [32] frame counts, then [32] bank slot numbers
 
-// ---- byte-plane rows: 6 words = lo bytes of dims 0..11 (3 words) then hi bytes (3 words) -----------------
-constexpr int kSlotBytes = 119 * 24 + 120 * 4;            // rows + squared norms = 3336
-struct PRow { u32 lo[3], hi[3]; u32 n; };
-
-__device__ __forceinline__ void load_prow(PRow &r, const unsigned char *slot, int idx) {
-    const uint2 *p = reinterpret_cast<const uint2 *>(slot + idx * 24);
-    const uint2 a = p[0], b = p[1], c = p[2];
-    r.lo[0] = a.x; r.lo[1] = a.y; r.lo[2] = b.x; r.hi[0] = b.y; r.hi[1] = c.x; r.hi[2] = c.y;
-    r.n = reinterpret_cast<const u32 *>(slot + 119 * 24)[idx];
-}
-__device__ __forceinline__ u32 dp4a_uu(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-__device__ __forceinline__ u32 dp4a_ss(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.s32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-__device__ __forceinline__ u32 dp4a_su(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-__device__ __forceinline__ u32 dp4a_us(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-// get_dis, DTW.C:45-62
-__device__ __forceinline__ u32 pdist(const PRow &a, const PRow &b) {
-    u32 ll = 0, hh = 0, mx = 0;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-        ll = dp4a_uu(a.lo[j], b.lo[j], ll);
-        hh = dp4a_ss(a.hi[j], b.hi[j], hh);
-        mx = dp4a_su(a.hi[j], b.lo[j], mx);
-        mx = dp4a_us(a.lo[j], b.hi[j], mx);
-    }
-    const u32 dot = hh * 65536u + mx * 256u + ll;
-    return usqrt_trunc(a.n + b.n - 2u * dot);
-}
-// convert one v_ftr_tag's rows [0,nrows) into the byte-plane slot; threads tid, tid+nthr, ... of the caller
-__device__ __forceinline__ void stage_planes(unsigned char *slot, const unsigned char *src_ftr, int nrows, int tid, int nthr) {
-    for (int r = tid; r < nrows; r += nthr) {
-        const u32 *s = reinterpret_cast<const u32 *>(src_ftr + 4 + r * 24);
-        u32 w[6];
-#pragma unroll
-        for (int j = 0; j < 6; ++j) w[j] = s[j];
-        u32 lo[3], hi[3], nrm = 0;
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {                      // words 2j, 2j+1 hold dims 4j..4j+3
-            lo[j] = __byte_perm(w[2 * j], w[2 * j + 1], 0x6420);
-            hi[j] = __byte_perm(w[2 * j], w[2 * j + 1], 0x7531);
-        }
-#pragma unroll
-        for (int j = 0; j < 6; ++j) {
-            const u32 a = lo16s(w[j]), b = hi16s(w[j]);
-            nrm += a * a + b * b;
-        }
-        u32 *d = reinterpret_cast<u32 *>(slot + r * 24);
-        d[0] = lo[0]; d[1] = lo[1]; d[2] = lo[2]; d[3] = hi[0]; d[4] = hi[1]; d[5] = hi[2];
-        reinterpret_cast<u32 *>(slot + 119 * 24)[r] = nrm;
-    }
-}
 __device__ __forceinline__ void group_barrier(int id, int nthreads) {
     if (nthreads == 32) __syncwarp();
     else asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// The lane-packed tile scan of dtw_kernel and dtw_band_thread_kernel. A CTA stages a tile of Tt <= 32 templates; its
+// warps, in G groups of Wg, stage NU utterances at a time, and each lane of a group scores one fixed (utterance slot,
+// template) pair of the NU x Tt (flattened), so lanes stay busy when Tt < 32. pair(I, M, urow, trow) scores a pair
+// that passed pair_walks.
+template <class Pair>
+__device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
+                                                 u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status, int Wg,
+                                                 int NU, int G, u32 tile0, int tslots, const u32 *B_dev, const u32 *perm,
+                                                 Pair pair) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    if (B_dev) B = min(B, *B_dev);
+    if (B == 0) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const u32 t0 = (blockIdx.x + tile0) * kTileT;
+    const int Tt = (int)min((u32)kTileT, T - t0);
+    unsigned char *tile = smem_raw;                                                // Tt slots
+    u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)tslots * kSlotBytes);
+    unsigned char *uslots = smem_raw + (size_t)tslots * kSlotBytes + kTileHdr;     // G*NU slots
+    u32 *ufrm = reinterpret_cast<u32 *>(uslots + (size_t)G * NU * kSlotBytes);     // [G*NU]
+
+    stage_tile(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kK2Warps);
+    __syncthreads();
+
+    const int group = warp / Wg, wig = warp - group * Wg;
+    if (group >= G) return;                                            // idle warps (32 not divisible by Wg)
+    const int gthreads = Wg * 32, gtid = wig * 32 + lane;
+    const int ul = gtid / Tt, tl = gtid - ul * Tt;                     // this lane's (utterance slot, template) -- fixed
+    const bool lane_has_pair = ul < NU;
+    unsigned char *gslots = uslots + (size_t)group * NU * kSlotBytes;
+    u32 *gfrm = ufrm + group * NU;
+    const unsigned char *trow = tile + (size_t)tl * kSlotBytes;
+    const u32 Mraw = lane_has_pair ? tfrm[tl] : kNoWalk;
+
+    for (u32 ubase = (blockIdx.y * G + group) * NU; ubase < B; ubase += gridDim.y * G * NU) {
+        // ---- stage NU utterances of this group ---------------------------------------------------------
+        for (int s = 0; s < NU; ++s) {
+            const u32 u = ubase + s;
+            u32 frm = kNoWalk;
+            if (u < B && !(status && status[u] != SR_ST_OK)) {        // VAD/MFCC failed: spch_recg returns before dtw
+                const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
+                frm = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
+                stage_planes(gslots + (size_t)s * kSlotBytes, kNrm119, uf, staged_rows(frm), gtid, gthreads);
+            }
+            if (gtid == 0) gfrm[s] = frm;
+        }
+        group_barrier(1 + group, gthreads);
+
+        const u32 u = ubase + (u32)ul;
+        if (lane_has_pair && u < B) {
+            const u32 Iraw = gfrm[ul];
+            const u32 result = pair_walks(Iraw, Mraw) ? pair((int)Iraw, (int)Mraw, gslots + (size_t)ul * kSlotBytes, trow)
+                                                      : SR_DIS_ERR;
+            const u32 t = perm ? tfrm[kTileT + tl] : t0 + (u32)tl;   // the original slot number: score column, argmin key
+            emit_pair(score, best, T, u, t, result);
+        }
+        group_barrier(1 + group, gthreads);                                                          // before restaging
+    }
 }
 
 __global__ void __launch_bounds__(kK2Warps * 32)
@@ -82,102 +89,17 @@ dtw_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char 
            const u32 *__restrict__ B_dev /* optional: batch size produced on the device (streaming) */,
            const u32 *__restrict__ perm /* optional: bank slots in ascending frm_num order (templates of a tile then have
                                            similar walk lengths); results are indexed by the ORIGINAL slot number */) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    if (B_dev) B = min(B, *B_dev);
-    if (B == 0) return;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const u32 t0 = (blockIdx.x + tile0) * kTileT;
-    const int Tt = (int)min((u32)kTileT, T - t0);
-    unsigned char *tile = smem_raw;                                   // Tt slots
-    u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)tslots * kSlotBytes);   // [32] frame counts, then [32] bank slot numbers
-    unsigned char *uslots = smem_raw + (size_t)tslots * kSlotBytes + 256;          // G*NU slots
-    u32 *ufrm = reinterpret_cast<u32 *>(uslots + (size_t)G * NU * kSlotBytes);     // [G*NU]
-
-    // ---- template tile: byte-plane rows + norms + frame counts ----------------------------------------
-    for (int tt = warp; tt < Tt; tt += kK2Warps) {
-        const u32 ts = perm ? perm[t0 + tt] : t0 + (u32)tt;
-        const unsigned char *slot = bank + (size_t)ts * slot_stride;
-        const u32 hdr = *reinterpret_cast<const u32 *>(slot);
-        u32 frm = hdr >> 16;
-        if ((flags & SR_DTW_CHECK_SIGN) && (hdr & 0xFFFFu) != SR_SAVE_MASK) frm = 0xFFFFFFFFu;   // main.c:283
-        if (frm > 119u && frm != 0xFFFFFFFFu) frm = 0xFFFFFFFEu;                                    // garbage header: no walk
-        const int nrows = (frm >= 0xFFFFFFFEu) ? 0 : (int)min(max(frm + 1u, 2u), 119u);   // +1: the do-while may touch row frm; rows 0 and 1 are always read (DTW.C:146-160), also when frm_num == 0
-        stage_planes(tile + (size_t)tt * kSlotBytes, slot, nrows, lane, 32);
-        if (lane == 0) { tfrm[tt] = frm; tfrm[32 + tt] = ts; }
-    }
-    __syncthreads();
-
-    const int group = warp / Wg, wig = warp - group * Wg;
-    if (group >= G) return;                                            // idle warps (16 not divisible by Wg)
-    const int gthreads = Wg * 32, gtid = wig * 32 + lane;
-    const int ul = gtid / Tt, tl = gtid - ul * Tt;                     // this lane's (utterance slot, template) -- fixed
-    const bool lane_has_pair = ul < NU;
-    unsigned char *gslots = uslots + (size_t)group * NU * kSlotBytes;
-    u32 *gfrm = ufrm + group * NU;
-    const unsigned char *trow = tile + (size_t)tl * kSlotBytes;
-    const u32 Mraw = lane_has_pair ? tfrm[tl] : 0xFFFFFFFFu;
-    const u32 t = lane_has_pair ? tfrm[32 + tl] : 0u;                  // original slot number: score column and argmin key
-
-    for (u32 ubase = (blockIdx.y * G + group) * NU; ubase < B; ubase += gridDim.y * G * NU) {
-        // ---- stage NU utterances of this group ---------------------------------------------------------
-        for (int s = 0; s < NU; ++s) {
-            const u32 u = ubase + s;
-            u32 frm = 0xFFFFFFFFu;
-            if (u < B && !(status && status[u] != SR_ST_OK)) {        // VAD/MFCC failed: spch_recg returns before dtw
-                const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
-                frm = (*reinterpret_cast<const u32 *>(uf)) >> 16;
-                if (frm > 119u) frm = 0xFFFFFFFEu;
-                else stage_planes(gslots + (size_t)s * kSlotBytes, uf, (int)min(max(frm + 1u, 2u), 119u), gtid, gthreads);
-            }
-            if (gtid == 0) gfrm[s] = frm;
-        }
-        group_barrier(1 + group, gthreads);
-
-        const u32 u = ubase + (u32)ul;
-        if (lane_has_pair && u < B) {
-            const u32 Iraw = gfrm[ul];
-            u32 result = SR_DIS_ERR;
-            const int I = (int)Iraw, M = (int)Mraw;
-            if (Iraw < 0xFFFFFFFEu && Mraw < 0xFFFFFFFEu && !(I > M * 2 || 2 * I < M)) {             // DTW.C:133
-                const unsigned char *urow = gslots + (size_t)ul * kSlotBytes;
-                const int X1 = (2 * M - I) / 3, X2 = (4 * I - 2 * M) / 3;                             // DTW.C:141-142
-                // dtw_limit (DTW.C:76-109) as an open y interval per column: ins(x,y) <=> yb(x) < y < ya(x)
-                const int ca = 4 - I + 2 * M + 1, cb = M - 2 * I - 4;
-                auto ya = [&](int x) { return x < X1 ? 2 * x + 2 : (x + ca) >> 1; };
-                auto yb = [&](int x) { return x < X2 ? (x - 2) >> 1 : 2 * x + cb; };
-                PRow i0, i1, m0, m1;
-                load_prow(i0, urow, 0); load_prow(m0, trow, 0);
-                load_prow(i1, urow, 1); load_prow(m1, trow, 1);
-                u32 dis = pdist(i0, m0);                                                             // DTW.C:146
-                int x = 1, y = 1;
-                int ya0 = ya(1), yb0 = yb(1), ya1 = ya(2), yb1 = yb(2);
-                u32 step = 1;
-                while (true) {                                                                       // DTW.C:150-188
-                    const u32 d_up = pdist(m1, i0), d_right = pdist(m0, i1), d_ru = pdist(m1, i1);
-                    const u32 up = (y + 1 < ya0 && y + 1 > yb0) ? d_up : SR_DIS_ERR;
-                    const u32 right = (y < ya1 && y > yb1) ? d_right : SR_DIS_ERR;
-                    const u32 ru = (y + 1 < ya1 && y + 1 > yb1) ? d_ru : SR_DIS_ERR;
-                    u32 mn = ru;
-                    if (mn > right) mn = right;
-                    if (mn > up) mn = up;
-                    dis += mn;
-                    const bool mv_x = (mn == ru) || (mn != up);                                       // diag, else up, else right
-                    const bool mv_y = (mn == ru) || (mn == up);
-                    ++step;
-                    if (mv_x) { i0 = i1; ++x; ya0 = ya1; yb0 = yb1; ya1 = ya(x + 1); yb1 = yb(x + 1); }
-                    if (mv_y) { m0 = m1; ++y; }
-                    if (!(x < I && y < M)) break;
-                    if (mv_x) load_prow(i1, urow, x);
-                    if (mv_y) load_prow(m1, trow, y);
-                }
-                result = dis / (step & 0xFFFFu);                                                     // DTW.C:191 (step is u16)
-            }
-            if (score) score[(size_t)u * T + t] = result;
-            if (best) atomicMin(reinterpret_cast<unsigned long long *>(&best[u]),
-                                (unsigned long long)(((u64)result << 32) | (u64)t));   // strict '<', first wins == lexicographic min
-        }
-        group_barrier(1 + group, gthreads);                                                          // before restaging
-    }
+    lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
+                     [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+                         PRow i0, i1, m0, m1;
+                         u32 dis, steps;
+                         int X1, X2, x, y, ya0, yb0, ya1, yb1;
+                         greedy_start(I, M, X1, X2, i0, i1, m0, m1, dis, steps, x, y, ya0, yb0, ya1, yb1, urow, kNrm119, trow,
+                                      kNrm119);
+                         while (greedy_step(I, M, X1, X2, i0, i1, m0, m1, dis, steps, x, y, ya0, yb0, ya1, yb1, urow, kNrm119,
+                                            trow, kNrm119)) {}
+                         return dis / (steps & 0xFFFFu);                                         // DTW.C:191 (step is u16)
+                     });
 }
 
 // best[] initialiser and finaliser (main.c:276-278 min_comm=0, min_dis=dis_max; main.c:292-294)
@@ -315,22 +237,17 @@ cudaError_t launch_dtw_limit(const u16 *x, const u16 *y, const u16 *I, const u16
 __global__ void get_dis_kernel(const s16 *a, const s16 *b, u32 n, u32 *out) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    u32 d = 0;
-    for (int j = 0; j < 12; ++j) {
-        const s32 dif = (s32)a[(size_t)i * 12 + j] - (s32)b[(size_t)i * 12 + j];
-        d += (u32)dif * (u32)dif;
-    }
-    out[i] = usqrt_trunc(d);
+    out[i] = get_dis_rows(a + (size_t)i * 12, b + (size_t)i * 12);
 }
 
-// one launch for `ntiles` template tiles of width Tt starting at tile `tile0`
-static cudaError_t launch_dtw_tiles(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags,
-                                    u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st, u32 tile0,
-                                    u32 ntiles, int Tt, const u32 *B_dev, const u32 *perm) {
-    // lane packing: groups of Wg warps walk NU utterances x Tt templates; pick the best (Wg, NU, G)
-    const size_t budget = 224 * 1024 - (size_t)Tt * kSlotBytes - 256 - 512;
+// lane packing of a tile of width Tt for lane_packed_scan: groups of Wg warps walk NU utterances x Tt templates; the
+// (Wg, NU, G) with the most busy lanes, and the shared memory it takes
+struct LanePlan { int Wg, NU, G; size_t smem; };
+static LanePlan plan_lanes(int Tt) {
+    constexpr int kSmemMax = 224 * 1024;
+    const size_t budget = kSmemMax - (size_t)Tt * kSlotBytes - kTileHdr - 512;
     const int slots_max = (int)(budget / kSlotBytes);
-    int bestWg = 1, bestNU = 1, bestG = 1;
+    LanePlan p{1, 1, 1, 0};
     double best_util = -1.0;
     for (int Wg = 1; Wg <= 8; ++Wg) {
         const int NU = (32 * Wg) / Tt;
@@ -340,33 +257,24 @@ static cudaError_t launch_dtw_tiles(const void *in_ftr, u32 B, const void *bank,
         if (Wg > 1 && G > 15) G = 15;                       // named barriers 1..15
         if (G < 1) continue;
         const double util = ((double)NU * Tt / (32.0 * Wg)) * ((double)G * Wg / kK2Warps);
-        if (util > best_util + 1e-9) { best_util = util; bestWg = Wg; bestNU = NU; bestG = G; }
+        if (util > best_util + 1e-9) { best_util = util; p.Wg = Wg; p.NU = NU; p.G = G; }
     }
-    const size_t smem = (size_t)Tt * kSlotBytes + 256 + (size_t)bestG * bestNU * kSlotBytes + (size_t)bestG * bestNU * 4 + 64;
-    cudaError_t e = cudaFuncSetAttribute(dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e != cudaSuccess) return e;
-    u32 gy = (u32)num_sms / ntiles;                      // floor: one CTA per SM, never a second partial wave
-    const u32 ugroups = (B + (u32)(bestG * bestNU) - 1) / (u32)(bestG * bestNU);
-    if (gy > ugroups) gy = ugroups;
-    if (gy < 1) gy = 1;
-    if (gy > 65535) gy = 65535;
-    dim3 grid(ntiles, gy);
-    dtw_kernel<<<grid, kK2Warps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
-                                                 static_cast<const unsigned char *>(bank), T, slot_stride, flags,
-                                                 score, best, status, bestWg, bestNU, bestG, tile0, Tt, B_dev, perm);
-    return cudaGetLastError();
+    p.smem = (size_t)Tt * kSlotBytes + kTileHdr + (size_t)p.G * p.NU * kSlotBytes + (size_t)p.G * p.NU * 4 + 64;
+    return p;
 }
 
 cudaError_t launch_dtw(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
                        u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev, const u32 *perm) {
     if (B == 0 || T == 0) return cudaSuccess;
-    const u32 full = T / kTileT, rem = T % kTileT;
-    if (full) {
-        cudaError_t e = launch_dtw_tiles(in_ftr, B, bank, T, slot_stride, flags, score, best, status, num_sms, st, 0, full, kTileT, B_dev, perm);
-        if (e != cudaSuccess) return e;
-    }
-    if (rem) return launch_dtw_tiles(in_ftr, B, bank, T, slot_stride, flags, score, best, status, num_sms, st, full, 1, (int)rem, B_dev, perm);
-    return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    if (e != cudaSuccess) return e;
+    return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
+        const LanePlan p = plan_lanes(Tt);
+        dtw_kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32, p.smem, st>>>(
+            static_cast<const unsigned char *>(in_ftr), B, static_cast<const unsigned char *>(bank), T, slot_stride, flags,
+            score, best, status, p.Wg, p.NU, p.G, tile0, Tt, B_dev, perm);
+        return cudaGetLastError();
+    });
 }
 cudaError_t launch_best_init(u64 *best, u32 B, cudaStream_t st) {
     if (B == 0) return cudaSuccess;
@@ -413,28 +321,20 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
     unsigned char *tile = smem_raw;                                               // byte-plane slots, as in dtw_kernel
     u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)kTileT * kSlotBytes);
     unsigned char *uslot = smem_raw + (size_t)kTileT * kSlotBytes + 128 + (size_t)warp * kSlotBytes;
-    for (int tt = warp; tt < Tt; tt += kDtwWarps) {
-        const unsigned char *slot = bank + (size_t)(t0 + tt) * slot_stride;
-        const u32 hdr = *reinterpret_cast<const u32 *>(slot);
-        u32 frm = hdr >> 16;
-        if ((flags & SR_DTW_CHECK_SIGN) && (hdr & 0xFFFFu) != SR_SAVE_MASK) frm = 0xFFFFFFFFu;
-        if (frm > 119u) frm = 0xFFFFFFFFu;
-        stage_planes(tile + (size_t)tt * kSlotBytes, slot, frm == 0xFFFFFFFFu ? 0 : (int)frm, lane, 32);
-        if (lane == 0) tfrm[tt] = frm;
-    }
+    stage_tile(tile, kSlotBytes, kNrm119, tfrm, nullptr, bank, slot_stride, flags, nullptr, t0, Tt, warp, lane, kDtwWarps);
     __syncthreads();
     for (u32 u = blockIdx.y * kDtwWarps + warp; u < B; u += gridDim.y * kDtwWarps) {
         const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
         const int I = (int)((*reinterpret_cast<const u32 *>(uf)) >> 16);
         __syncwarp();
-        if (I <= 119) stage_planes(uslot, uf, I, lane, 32);
+        if (I <= 119) stage_planes(uslot, kNrm119, uf, I, lane, 32);
         __syncwarp();
         u32 my_result = SR_DIS_ERR;                       // lane tt keeps the result of template tt
         for (int tt = 0; tt < Tt; ++tt) {
             const u32 Mraw = tfrm[tt];
             const int M = (int)Mraw;
             u32 result = SR_DIS_ERR;
-            if (Mraw != 0xFFFFFFFFu && I >= 1 && M >= 1 && I <= 119 && !(I > M * 2 || 2 * I < M)) {
+            if (I >= 1 && I <= 119 && pair_walks((u32)I, Mraw)) {
                 const unsigned char *trow = tile + (size_t)tt * kSlotBytes;
                 s32 Dprev = kInf;
                 int cprev = 0;
@@ -442,8 +342,8 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
                     const int c = (i * M) / I, j = c - r + lane;
                     const bool valid = lane <= 2 * r && j >= 0 && j < M;
                     PRow a, b;
-                    load_prow(a, uslot, i);                                   // broadcast read
-                    load_prow(b, trow, valid ? j : 0);
+                    load_row(a, uslot, kNrm119, i);                            // broadcast read
+                    load_row(b, trow, kNrm119, valid ? j : 0);
                     const s32 d = valid ? (s32)pdist(a, b) : 0;
                     const int sft = c - cprev;
                     const int su = lane + sft, sd = lane + sft - 1;
@@ -483,8 +383,8 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 }
 
 // ---- K3b: the same banded DP, one THREAD per pair, band in registers (compile-time radius) -----------------------
-// 3.7x fewer issue slots per lattice cell than the warp-scan form: no scans, no idle lanes (21 of 32), lane packing
-// and byte-plane dp4a distances exactly like dtw_kernel. The band of row i sits at columns c_i-R..c_i+R with
+// 3.7x fewer issue slots per lattice cell than the warp-scan form: no scans, no idle lanes (21 of 32), and the
+// lane-packed tile scan of dtw_kernel. The band of row i sits at columns c_i-R..c_i+R with
 // c_i = floor(i*M/I); it slides by s = c_i - c_{i-1} in {0,1,2} per row, realised as two predicated shift-by-one
 // passes over the register array (no divergence between lanes whose templates have different lengths).
 template <int R>
@@ -492,138 +392,57 @@ __global__ void __launch_bounds__(kK2Warps * 32)
 dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                        u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best, int Wg, int NU, int G,
                        u32 tile0, int tslots) {
-    constexpr int W = 2 * R + 1;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const u32 t0 = (blockIdx.x + tile0) * kTileT;
-    const int Tt = (int)min((u32)kTileT, T - t0);
-    unsigned char *tile = smem_raw;
-    u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)tslots * kSlotBytes);
-    unsigned char *uslots = smem_raw + (size_t)tslots * kSlotBytes + 128;
-    u32 *ufrm = reinterpret_cast<u32 *>(uslots + (size_t)G * NU * kSlotBytes);
-    for (int tt = warp; tt < Tt; tt += kK2Warps) {
-        const unsigned char *slot = bank + (size_t)(t0 + tt) * slot_stride;
-        const u32 hdr = *reinterpret_cast<const u32 *>(slot);
-        u32 frm = hdr >> 16;
-        if ((flags & SR_DTW_CHECK_SIGN) && (hdr & 0xFFFFu) != SR_SAVE_MASK) frm = 0xFFFFFFFFu;
-        if (frm > 119u) frm = 0xFFFFFFFFu;
-        stage_planes(tile + (size_t)tt * kSlotBytes, slot, frm == 0xFFFFFFFFu ? 0 : (int)frm, lane, 32);
-        if (lane == 0) tfrm[tt] = frm;
-    }
-    __syncthreads();
-    const int group = warp / Wg, wig = warp - group * Wg;
-    if (group >= G) return;
-    const int gthreads = Wg * 32, gtid = wig * 32 + lane;
-    const int ul = gtid / Tt, tl = gtid - ul * Tt;
-    const bool lane_has_pair = ul < NU;
-    unsigned char *gslots = uslots + (size_t)group * NU * kSlotBytes;
-    u32 *gfrm = ufrm + group * NU;
-    const unsigned char *trow = tile + (size_t)tl * kSlotBytes;
-    const u32 Mraw = lane_has_pair ? tfrm[tl] : 0xFFFFFFFFu;
-    const u32 t = t0 + (u32)tl;
-    for (u32 ubase = (blockIdx.y * G + group) * NU; ubase < B; ubase += gridDim.y * G * NU) {
-        for (int sl = 0; sl < NU; ++sl) {
-            const u32 u = ubase + sl;
-            u32 frm = 0xFFFFFFFFu;
-            if (u < B) {
-                const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
-                frm = (*reinterpret_cast<const u32 *>(uf)) >> 16;
-                if (frm > 119u) frm = 0xFFFFFFFFu;
-                else stage_planes(gslots + (size_t)sl * kSlotBytes, uf, (int)frm, gtid, gthreads);
+    lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, nullptr, Wg, NU, G, tile0, tslots, nullptr, nullptr,
+                     [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+        constexpr int W = 2 * R + 1;
+        if (I == 0) return SR_DIS_ERR;                     // empty feature sets (M == 0 too, by the 2:1 guard): no cell
+        s32 D[W];
+#pragma unroll
+        for (int k = 0; k < W; ++k) D[k] = kInf;
+        int c = 0, cprev = 0, err = 0;                     // c = floor(i*M/I) kept incrementally: i*M = c*I + err
+        for (int i = 0; i < I; ++i) {
+            const int sft = c - cprev;                     // 0, 1 or 2 (M <= 2I)
+            // diag source of cell k=0 is the old element at index sft-1
+            s32 dm1 = sft == 2 ? D[1] : (sft == 1 ? D[0] : kInf);
+            if (sft >= 1) {
+#pragma unroll
+                for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
+                D[W - 1] = kInf;
             }
-            if (gtid == 0) gfrm[sl] = frm;
-        }
-        group_barrier(1 + group, gthreads);
-        const u32 u = ubase + (u32)ul;
-        if (lane_has_pair && u < B) {
-            const u32 Iraw = gfrm[ul];
-            const int I = (int)Iraw, M = (int)Mraw;
-            u32 result = SR_DIS_ERR;
-            if (Iraw != 0xFFFFFFFFu && Mraw != 0xFFFFFFFFu && I >= 1 && M >= 1 && !(I > M * 2 || 2 * I < M)) {
-                const unsigned char *urow = gslots + (size_t)ul * kSlotBytes;
-                s32 D[W];
+            if (sft >= 2) {
 #pragma unroll
-                for (int k = 0; k < W; ++k) D[k] = kInf;
-                int c = 0, cprev = 0, err = 0;                     // c = floor(i*M/I) kept incrementally: i*M = c*I + err
-                for (int i = 0; i < I; ++i) {
-                    const int sft = c - cprev;                     // 0, 1 or 2 (M <= 2I)
-                    // diag source of cell k=0 is the old element at index sft-1
-                    s32 dm1 = sft == 2 ? D[1] : (sft == 1 ? D[0] : kInf);
-                    if (sft >= 1) {
-#pragma unroll
-                        for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
-                        D[W - 1] = kInf;
-                    }
-                    if (sft >= 2) {
-#pragma unroll
-                        for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
-                        D[W - 1] = kInf;
-                    }
-                    PRow a;
-                    load_prow(a, urow, i);
-                    s32 left = kInf;
-#pragma unroll
-                    for (int k = 0; k < W; ++k) {
-                        const int j = c - R + k;
-                        const bool valid = j >= 0 && j < M;
-                        const s32 up = D[k];
-                        s32 bst = min(min(up, dm1), left);
-                        if (i == 0 && j == 0) bst = 0;
-                        PRow b;
-                        load_prow(b, trow, valid ? j : 0);
-                        const s32 d = (s32)pdist(a, b);
-                        const s32 x = (valid && bst < kInf / 2) ? bst + d : kInf;
-                        dm1 = up;                                  // becomes the diagonal source of cell k+1
-                        D[k] = x;
-                        left = x;
-                    }
-                    cprev = c;
-                    err += M;                                      // advance c to floor((i+1)*M/I)
-                    if (err >= I) { err -= I; ++c; }
-                    if (err >= I) { err -= I; ++c; }
-                }
-                const int kend = (M - 1) - (cprev - R);            // cell holding column M-1 in the last row
-                s32 fin = kInf;
-#pragma unroll
-                for (int k = 0; k < W; ++k) if (k == kend) fin = D[k];
-                if (fin < kInf / 2) result = (u32)fin / (u32)(I + M);
+                for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
+                D[W - 1] = kInf;
             }
-            if (score) score[(size_t)u * T + t] = result;
-            if (best) atomicMin(reinterpret_cast<unsigned long long *>(&best[u]), (unsigned long long)(((u64)result << 32) | (u64)t));
+            PRow a;
+            load_row(a, urow, kNrm119, i);
+            s32 left = kInf;
+#pragma unroll
+            for (int k = 0; k < W; ++k) {
+                const int j = c - R + k;
+                const bool valid = j >= 0 && j < M;
+                const s32 up = D[k];
+                s32 bst = min(min(up, dm1), left);
+                if (i == 0 && j == 0) bst = 0;
+                PRow b;
+                load_row(b, trow, kNrm119, valid ? j : 0);
+                const s32 d = (s32)pdist(a, b);
+                const s32 x = (valid && bst < kInf / 2) ? bst + d : kInf;
+                dm1 = up;                                  // becomes the diagonal source of cell k+1
+                D[k] = x;
+                left = x;
+            }
+            cprev = c;
+            err += M;                                      // advance c to floor((i+1)*M/I)
+            if (err >= I) { err -= I; ++c; }
+            if (err >= I) { err -= I; ++c; }
         }
-        group_barrier(1 + group, gthreads);
-    }
-}
-
-static cudaError_t launch_band_thread_tiles(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags,
-                                            u32 *score, u64 *best, int num_sms, cudaStream_t st, u32 tile0, u32 ntiles, int Tt) {
-    const size_t budget = 224 * 1024 - (size_t)Tt * kSlotBytes - 128 - 512;
-    const int slots_max = (int)(budget / kSlotBytes);
-    int bestWg = 1, bestNU = 1, bestG = 1;
-    double best_util = -1.0;
-    for (int Wg = 1; Wg <= 8; ++Wg) {
-        const int NU = (32 * Wg) / Tt;
-        if (NU < 1) continue;
-        int G = kK2Warps / Wg;
-        if (G > slots_max / NU) G = slots_max / NU;
-        if (Wg > 1 && G > 15) G = 15;
-        if (G < 1) continue;
-        const double util = ((double)NU * Tt / (32.0 * Wg)) * ((double)G * Wg / kK2Warps);
-        if (util > best_util + 1e-9) { best_util = util; bestWg = Wg; bestNU = NU; bestG = G; }
-    }
-    const size_t smem = (size_t)Tt * kSlotBytes + 128 + (size_t)bestG * bestNU * kSlotBytes + (size_t)bestG * bestNU * 4 + 64;
-    cudaError_t e = cudaFuncSetAttribute(dtw_band_thread_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e != cudaSuccess) return e;
-    u32 gy = (u32)num_sms / ntiles;                      // floor: one CTA per SM, never a second partial wave
-    const u32 ugroups = (B + (u32)(bestG * bestNU) - 1) / (u32)(bestG * bestNU);
-    if (gy > ugroups) gy = ugroups;
-    if (gy < 1) gy = 1;
-    if (gy > 65535) gy = 65535;
-    dim3 grid(ntiles, gy);
-    dtw_band_thread_kernel<10><<<grid, kK2Warps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
-                                                                  static_cast<const unsigned char *>(bank), T, slot_stride,
-                                                                  flags, score, best, bestWg, bestNU, bestG, tile0, Tt);
-    return cudaGetLastError();
+        const int kend = (M - 1) - (cprev - R);            // cell holding column M-1 in the last row
+        s32 fin = kInf;
+#pragma unroll
+        for (int k = 0; k < W; ++k) if (k == kend) fin = D[k];
+        return fin < kInf / 2 ? (u32)fin / (u32)(I + M) : SR_DIS_ERR;
+    });
 }
 
 cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
@@ -631,24 +450,22 @@ cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, 
     if (B == 0 || T == 0) return cudaSuccess;
     if (band_r < 0 || band_r > 15) return cudaErrorInvalidValue;               // 2r+1 lanes of one warp
     if (band_r == 10) {                                                       // the BASELINE radius: thread-per-pair form
-        const u32 full = T / kTileT, rem = T % kTileT;
-        if (full) {
-            cudaError_t e1 = launch_band_thread_tiles(in_ftr, B, bank, T, slot_stride, flags, score, best, num_sms, st, 0, full, kTileT);
-            if (e1 != cudaSuccess) return e1;
-        }
-        if (rem) return launch_band_thread_tiles(in_ftr, B, bank, T, slot_stride, flags, score, best, num_sms, st, full, 1, (int)rem);
-        return cudaSuccess;
+        cudaError_t e = cudaFuncSetAttribute(dtw_band_thread_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+        if (e != cudaSuccess) return e;
+        return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
+            const LanePlan p = plan_lanes(Tt);
+            dtw_band_thread_kernel<10><<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32,
+                                         p.smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
+                                                       static_cast<const unsigned char *>(bank), T, slot_stride, flags,
+                                                       score, best, p.Wg, p.NU, p.G, tile0, Tt);
+            return cudaGetLastError();
+        });
     }
     const size_t band_smem = (size_t)kTileT * kSlotBytes + 128 + (size_t)kDtwWarps * kSlotBytes;
     cudaError_t e = cudaFuncSetAttribute(dtw_band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)band_smem);
     if (e != cudaSuccess) return e;
     const u32 tiles = (T + kTileT - 1) / kTileT;
-    u32 gy = (u32)num_sms / tiles;                       // floor: never a second partial wave
-    const u32 ugroups = (B + kDtwWarps - 1) / kDtwWarps;
-    if (gy > ugroups) gy = ugroups;
-    if (gy < 1) gy = 1;
-    if (gy > 65535) gy = 65535;
-    dim3 grid(tiles, gy);
+    dim3 grid(tiles, grid_rows(num_sms, tiles, B, kDtwWarps));
     dtw_band_kernel<<<grid, kDtwWarps * 32, band_smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
                                                                   static_cast<const unsigned char *>(bank), T,
                                                                   slot_stride, flags, band_r, score, best);

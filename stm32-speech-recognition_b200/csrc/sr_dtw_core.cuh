@@ -1,0 +1,181 @@
+// sr_dtw_core.cuh -- the template scan's shared core, used by the static kernels (sr_dtw.cu: greedy dtw_kernel, banded
+// dtw_band_kernel and dtw_band_thread_kernel) and the dynamic-pair kernel (sr_dtw_dyn.cu): byte-plane rows and their
+// get_dis, the slot header decode, the template tile stager, the greedy walk step, the score/argmin epilogue and the
+// launch geometry.
+//
+// Rows are staged as BYTE PLANES (low bytes | high bytes of the 12 s16), so that
+//   sum (a-b)^2 = |a|^2 + |b|^2 - 2 a.b        (exact in Z/2^32, the ring the reference accumulates in)
+// costs 12 IDP.4A per local distance on packed registers: a.b = 65536*HH + 256*(HL+LH) + LL.
+// A slot holds 24 bytes of planes per row, then one u32 squared norm per row from byte `nrm` on. The static kernels
+// size every slot for vv_frm_max rows (nrm = kNrm119); the dynamic kernel sizes them for the longest feature set present.
+#pragma once
+#include "sr_common.cuh"
+
+namespace srk {
+
+constexpr int kTileT = 32;                                // templates per tile: one CTA column
+constexpr u32 kMaxFrm = 119;                              // vv_frm_max
+constexpr u32 kNrm119 = kMaxFrm * 24;                     // norm offset of a vv_frm_max-row slot
+constexpr int kSlotBytes = kMaxFrm * 24 + 120 * 4;        // rows + squared norms = 3336
+constexpr u32 kNoWalk = 0xFFFFFFFFu;                      // frame count of a feature set that is never walked
+
+// ---- byte-plane rows: 6 words = lo bytes of dims 0..11 (3 words) then hi bytes (3 words), plus the squared norm ------
+struct PRow { u32 lo[3], hi[3]; u32 n; };
+
+__device__ __forceinline__ void load_row(PRow &r, const unsigned char *slot, u32 nrm, int idx) {
+    const uint2 *p = reinterpret_cast<const uint2 *>(slot + idx * 24);
+    const uint2 a = p[0], b = p[1], c = p[2];
+    r.lo[0] = a.x; r.lo[1] = a.y; r.lo[2] = b.x; r.hi[0] = b.y; r.hi[1] = c.x; r.hi[2] = c.y;
+    r.n = reinterpret_cast<const u32 *>(slot + nrm)[idx];
+}
+__device__ __forceinline__ u32 dp4a_uu(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
+__device__ __forceinline__ u32 dp4a_ss(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.s32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
+__device__ __forceinline__ u32 dp4a_su(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
+__device__ __forceinline__ u32 dp4a_us(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
+// get_dis, DTW.C:45-62
+__device__ __forceinline__ u32 pdist(const PRow &a, const PRow &b) {
+    u32 ll = 0, hh = 0, mx = 0;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        ll = dp4a_uu(a.lo[j], b.lo[j], ll);
+        hh = dp4a_ss(a.hi[j], b.hi[j], hh);
+        mx = dp4a_su(a.hi[j], b.lo[j], mx);
+        mx = dp4a_us(a.lo[j], b.hi[j], mx);
+    }
+    const u32 dot = hh * 65536u + mx * 256u + ll;
+    return usqrt_trunc(a.n + b.n - 2u * dot);
+}
+// convert one v_ftr_tag's rows [0,nrows) into the byte-plane slot; threads tid, tid+nthr, ... of the caller
+__device__ __forceinline__ void stage_planes(unsigned char *slot, u32 nrm, const unsigned char *src_ftr, int nrows, int tid,
+                                             int nthr) {
+    for (int r = tid; r < nrows; r += nthr) {
+        const u32 *s = reinterpret_cast<const u32 *>(src_ftr + 4 + r * 24);
+        u32 w[6];
+#pragma unroll
+        for (int j = 0; j < 6; ++j) w[j] = s[j];
+        u32 lo[3], hi[3], n = 0;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {                      // words 2j, 2j+1 hold dims 4j..4j+3
+            lo[j] = __byte_perm(w[2 * j], w[2 * j + 1], 0x6420);
+            hi[j] = __byte_perm(w[2 * j], w[2 * j + 1], 0x7531);
+        }
+#pragma unroll
+        for (int j = 0; j < 6; ++j) {
+            const u32 a = lo16s(w[j]), b = hi16s(w[j]);
+            n += a * a + b * b;
+        }
+        u32 *d = reinterpret_cast<u32 *>(slot + r * 24);
+        d[0] = lo[0]; d[1] = lo[1]; d[2] = lo[2]; d[3] = hi[0]; d[4] = hi[1]; d[5] = hi[2];
+        reinterpret_cast<u32 *>(slot + nrm)[r] = n;
+    }
+}
+
+// ---- headers ----------------------------------------------------------------------------------------------------
+// frame count from a feature set's first word (save_sign | frm_num << 16), or kNoWalk: a bank slot that is unsigned or
+// erased under SR_DTW_CHECK_SIGN (main.c:283), or a frm_num > vv_frm_max, whose rows would lie past the struct.
+// Utterances pass flags = 0.
+__device__ __forceinline__ u32 decode_frm(u32 hdr, u32 flags) {
+    const u32 frm = hdr >> 16;
+    const bool unsigned_slot = (flags & SR_DTW_CHECK_SIGN) && (hdr & 0xFFFFu) != SR_SAVE_MASK;
+    return (unsigned_slot || frm > kMaxFrm) ? kNoWalk : frm;
+}
+// rows to stage: the greedy do-while may touch row frm, and rows 0 and 1 are always read (DTW.C:146-160), also when
+// frm_num == 0. The banded DP reads rows [0, frm) only.
+__device__ __forceinline__ int staged_rows(u32 frm) { return frm == kNoWalk ? 0 : (int)min(max(frm + 1u, 2u), kMaxFrm); }
+// both sides walkable and within the 2:1 length ratio (DTW.C:133)
+__device__ __forceinline__ bool pair_walks(u32 Iraw, u32 Mraw) {
+    const int I = (int)Iraw, M = (int)Mraw;
+    return Iraw != kNoWalk && Mraw != kNoWalk && !(I > M * 2 || 2 * I < M);
+}
+
+// stage bank templates t0 .. t0+Tt-1 (bank slot perm[t] when a bank order is given) into tile slots of slot_bytes each:
+// planes and norms, frame counts to tfrm[], bank slot numbers to tslot[] unless it is NULL. Warp w of nwarps stages
+// templates w, w+nwarps, ...
+__device__ __forceinline__ void stage_tile(unsigned char *tile, u32 slot_bytes, u32 nrm, u32 *tfrm, u32 *tslot,
+                                           const unsigned char *bank, u32 slot_stride, u32 flags, const u32 *perm, u32 t0,
+                                           int Tt, int warp, int lane, int nwarps) {
+    for (int tt = warp; tt < Tt; tt += nwarps) {
+        const u32 ts = perm ? perm[t0 + tt] : t0 + (u32)tt;
+        const unsigned char *slot = bank + (size_t)ts * slot_stride;
+        const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), flags);
+        stage_planes(tile + (size_t)tt * slot_bytes, nrm, slot, staged_rows(frm), lane, 32);
+        if (lane == 0) {
+            tfrm[tt] = frm;
+            if (tslot) tslot[tt] = ts;
+        }
+    }
+}
+
+// ---- the reference's greedy walk (DTW.C:141-191) over a staged utterance and template -----------------------------
+// The walk state lives in the caller's locals, passed by reference: i0/i1 are the utterance rows x-1 and x, m0/m1 the
+// template rows y-1 and y, (ya0, yb0) and (ya1, yb1) the dtw_limit intervals of columns x and x+1. (Held in a struct
+// across dtw_dyn_kernel's claim/poll loop, the same state compiled to 13 more instructions per step, mostly moves.)
+// dtw_limit (DTW.C:76-109) as an open y interval per column: ins(x,y) <=> yb(x) < y < ya(x)
+__device__ __forceinline__ int walk_ya(int x, int I, int M, int X1) { return x < X1 ? 2 * x + 2 : (x + (4 - I + 2 * M + 1)) >> 1; }
+__device__ __forceinline__ int walk_yb(int x, int I, int M, int X2) { return x < X2 ? (x - 2) >> 1 : 2 * x + (M - 2 * I - 4); }
+
+// first point of the walk of a pair that passed pair_walks (DTW.C:141-146)
+__device__ __forceinline__ void greedy_start(int I, int M, int &X1, int &X2, PRow &i0, PRow &i1, PRow &m0, PRow &m1, u32 &dis,
+                                             u32 &steps, int &x, int &y, int &ya0, int &yb0, int &ya1, int &yb1,
+                                             const unsigned char *urow, u32 unrm, const unsigned char *trow, u32 tnrm) {
+    X1 = (2 * M - I) / 3; X2 = (4 * I - 2 * M) / 3;                                              // DTW.C:141-142
+    load_row(i0, urow, unrm, 0); load_row(m0, trow, tnrm, 0);
+    load_row(i1, urow, unrm, 1); load_row(m1, trow, tnrm, 1);
+    dis = pdist(i0, m0);                                                                         // DTW.C:146
+    x = 1; y = 1; steps = 1;
+    ya0 = walk_ya(1, I, M, X1); yb0 = walk_yb(1, I, M, X2); ya1 = walk_ya(2, I, M, X1); yb1 = walk_yb(2, I, M, X2);
+}
+// one step of DTW.C:150-188; false once the walk has ended, and its score is then dis / (steps & 0xFFFF) (DTW.C:191,
+// step is a u16)
+__device__ __forceinline__ bool greedy_step(int I, int M, int X1, int X2, PRow &i0, PRow &i1, PRow &m0, PRow &m1, u32 &dis,
+                                            u32 &steps, int &x, int &y, int &ya0, int &yb0, int &ya1, int &yb1,
+                                            const unsigned char *urow, u32 unrm, const unsigned char *trow, u32 tnrm) {
+    const u32 d_up = pdist(m1, i0), d_right = pdist(m0, i1), d_ru = pdist(m1, i1);
+    const u32 up = (y + 1 < ya0 && y + 1 > yb0) ? d_up : SR_DIS_ERR;
+    const u32 right = (y < ya1 && y > yb1) ? d_right : SR_DIS_ERR;
+    const u32 ru = (y + 1 < ya1 && y + 1 > yb1) ? d_ru : SR_DIS_ERR;
+    u32 mn = ru;
+    if (mn > right) mn = right;
+    if (mn > up) mn = up;
+    dis += mn;
+    const bool mv_x = (mn == ru) || (mn != up);                                                   // diag, else up, else right
+    const bool mv_y = (mn == ru) || (mn == up);
+    ++steps;
+    if (mv_x) { i0 = i1; ++x; ya0 = ya1; yb0 = yb1; ya1 = walk_ya(x + 1, I, M, X1); yb1 = walk_yb(x + 1, I, M, X2); }
+    if (mv_y) { m0 = m1; ++y; }
+    if (!(x < I && y < M)) return false;
+    if (mv_x) load_row(i1, urow, unrm, x);
+    if (mv_y) load_row(m1, trow, tnrm, y);
+    return true;
+}
+
+// score[u][t] and the spch_recg argmin (main.c:276-291) as one 64-bit atomicMin of (result, bank slot t):
+// strict '<', first wins == lexicographic min
+__device__ __forceinline__ void emit_pair(u32 *score, u64 *best, u32 T, u32 u, u32 t, u32 result) {
+    if (score) score[(size_t)u * T + t] = result;
+    if (best) atomicMin(reinterpret_cast<unsigned long long *>(&best[u]), (unsigned long long)(((u64)result << 32) | (u64)t));
+}
+
+// ---- launch geometry --------------------------------------------------------------------------------------------
+// CTA rows per tile column: one CTA per SM over all columns (never a second partial wave), no more than the batch needs
+inline u32 grid_rows(int num_sms, u32 ntiles, u32 B, u32 utt_per_cta) {
+    u32 gy = (u32)num_sms / ntiles;
+    const u32 need = (B + utt_per_cta - 1) / utt_per_cta;
+    if (gy > need) gy = need;
+    if (gy < 1) gy = 1;
+    if (gy > 65535) gy = 65535;
+    return gy;
+}
+// T templates as one launch of the full kTileT-wide tiles and one of the remainder tile: launch(tile0, ntiles, Tt)
+template <class Launch>
+inline cudaError_t launch_tiles(u32 T, Launch launch) {
+    const u32 full = T / kTileT, rem = T % kTileT;
+    if (full) {
+        cudaError_t e = launch(0u, full, kTileT);
+        if (e != cudaSuccess) return e;
+    }
+    if (rem) return launch(full, 1u, (int)rem);
+    return cudaSuccess;
+}
+
+}  // namespace srk

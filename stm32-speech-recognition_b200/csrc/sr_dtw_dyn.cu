@@ -16,8 +16,9 @@
 //   flag[slot] = seq + 1   (producer, release)  -> the consumer that was handed a pair of utterance `seq` waits for it;
 //   done[slot] += 1        (consumer, release, after its last read of the slot) -> the producer reuses the slot for
 //                           utterance seq when done[slot] == (seq / R) * Tt.
-// Arithmetic, tie-breaking and the argmin epilogue are exactly those of dtw_kernel (sr_dtw.cu); results are identical.
-#include "sr_common.cuh"
+// Rows, header decode, the tile stager, the walk step and the argmin epilogue are those of dtw_kernel (sr_dtw_core.cuh);
+// results are identical.
+#include "sr_dtw_core.cuh"
 
 namespace srk {
 
@@ -25,8 +26,6 @@ constexpr int kDynWarps = 32;
 constexpr int kDynProducers = 2;
 constexpr int kDynRMax = 192;               // ring slots the control arrays are sized for
 constexpr int kDynRefill = 8;               // idle lanes of a warp that trigger a claim
-
-struct QRow { u32 lo[3], hi[3]; u32 n; };
 
 __device__ __forceinline__ u32 ld_acquire_s(const u32 *p) {
     u32 v;
@@ -40,62 +39,12 @@ __device__ __forceinline__ void red_release_add_s(u32 *p, u32 v) {
     asm volatile("red.release.cta.shared.add.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
 }
 
-__device__ __forceinline__ void load_qrow(QRow &r, u32 slot_s /* shared address */, u32 nrm_off, int idx) {
-    u32 a0, a1, b0, b1, c0, c1;
-    const u32 p = slot_s + (u32)idx * 24u;
-    asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(a0), "=r"(a1) : "r"(p));
-    asm volatile("ld.shared.v2.u32 {%0,%1}, [%2+8];" : "=r"(b0), "=r"(b1) : "r"(p));
-    asm volatile("ld.shared.v2.u32 {%0,%1}, [%2+16];" : "=r"(c0), "=r"(c1) : "r"(p));
-    r.lo[0] = a0; r.lo[1] = a1; r.lo[2] = b0; r.hi[0] = b1; r.hi[1] = c0; r.hi[2] = c1;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.n) : "r"(slot_s + nrm_off + (u32)idx * 4u));
-}
-__device__ __forceinline__ u32 qdp_uu(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-__device__ __forceinline__ u32 qdp_ss(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.s32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-__device__ __forceinline__ u32 qdp_su(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.s32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-__device__ __forceinline__ u32 qdp_us(u32 a, u32 b, u32 c) { u32 d; asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
-// get_dis, DTW.C:45-62: sum (a-b)^2 = |a|^2 + |b|^2 - 2 a.b in Z/2^32, a.b from byte planes (see sr_dtw.cu)
-__device__ __forceinline__ u32 qdist(const QRow &a, const QRow &b) {
-    u32 ll = 0, hh = 0, mx = 0;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-        ll = qdp_uu(a.lo[j], b.lo[j], ll);
-        hh = qdp_ss(a.hi[j], b.hi[j], hh);
-        mx = qdp_su(a.hi[j], b.lo[j], mx);
-        mx = qdp_us(a.lo[j], b.hi[j], mx);
-    }
-    const u32 dot = hh * 65536u + mx * 256u + ll;
-    return usqrt_trunc(a.n + b.n - 2u * dot);
-}
-// rows [0,nrows) of one v_ftr_tag -> byte planes + squared norms; lanes tid, tid+nthr, ..
-__device__ __forceinline__ void stage_qplanes(unsigned char *slot, u32 nrm_off, const unsigned char *src_ftr, int nrows, int tid, int nthr) {
-    for (int r = tid; r < nrows; r += nthr) {
-        const u32 *s = reinterpret_cast<const u32 *>(src_ftr + 4 + r * 24);
-        u32 w[6];
-#pragma unroll
-        for (int j = 0; j < 6; ++j) w[j] = s[j];
-        u32 lo[3], hi[3], nrm = 0;
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            lo[j] = __byte_perm(w[2 * j], w[2 * j + 1], 0x6420);
-            hi[j] = __byte_perm(w[2 * j], w[2 * j + 1], 0x7531);
-        }
-#pragma unroll
-        for (int j = 0; j < 6; ++j) {
-            const u32 a = lo16s(w[j]), b = hi16s(w[j]);
-            nrm += a * a + b * b;
-        }
-        u32 *d = reinterpret_cast<u32 *>(slot + r * 24);
-        d[0] = lo[0]; d[1] = lo[1]; d[2] = lo[2]; d[3] = hi[0]; d[4] = hi[1]; d[5] = hi[2];
-        reinterpret_cast<u32 *>(slot + nrm_off)[r] = nrm;
-    }
-}
-
 struct DynCtrl {
     u32 next_pair;
     u32 tmax;
     u32 pad[2];
-    u32 tfrm[32];
-    u32 tslot_id[32];
+    u32 tfrm[kTileT];
+    u32 tslot_id[kTileT];
     u32 flag[kDynRMax];
     u32 done[kDynRMax];
     u32 ufrm[kDynRMax];
@@ -114,28 +63,22 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (B_dev) B = min(B, *B_dev);
     if (B == 0 || blockIdx.y >= B) return;
-    const u32 t0 = (blockIdx.x + tile0) * 32u;
-    const int Tt = (int)min(32u, T - t0);
+    const u32 t0 = (blockIdx.x + tile0) * kTileT;
+    const int Tt = (int)min((u32)kTileT, T - t0);
 
-    // ---- template headers, slot sizes ---------------------------------------------------------------------------
+    // ---- slot sizes from the longest template of the tile --------------------------------------------------------
     if (threadIdx.x == 0) { c.next_pair = 0; c.tmax = 0; }
     for (int i = threadIdx.x; i < kDynRMax; i += blockDim.x) { c.flag[i] = 0; c.done[i] = 0; }
     __syncthreads();
     if (threadIdx.x < Tt) {
         const u32 ts = perm ? perm[t0 + threadIdx.x] : t0 + threadIdx.x;
-        c.tslot_id[threadIdx.x] = ts;
-        const u32 hdr = *reinterpret_cast<const u32 *>(bank + (size_t)ts * slot_stride);
-        u32 frm = hdr >> 16;
-        if ((flags & SR_DTW_CHECK_SIGN) && (hdr & 0xFFFFu) != SR_SAVE_MASK) frm = 0xFFFFFFFFu;   // main.c:283
-        if (frm > 119u && frm != 0xFFFFFFFFu) frm = 0xFFFFFFFEu;                                    // garbage header: no walk
-        c.tfrm[threadIdx.x] = frm;
-        if (frm < 0xFFFFFFFEu) atomicMax(&c.tmax, frm);
+        const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(bank + (size_t)ts * slot_stride), flags);
+        if (frm != kNoWalk) atomicMax(&c.tmax, frm);
     }
     __syncthreads();
-    // +1: the do-while may touch row frm; rows 0 and 1 are always read (DTW.C:146-160)
-    const u32 trows = min(max(c.tmax + 1u, 2u), 119u);
-    u32 umax = max_frm_dev ? *max_frm_dev : 119u;
-    const u32 urows = min(max(min(umax, 119u) + 1u, 2u), 119u);
+    const u32 trows = (u32)staged_rows(c.tmax);
+    u32 umax = max_frm_dev ? *max_frm_dev : kMaxFrm;
+    const u32 urows = (u32)staged_rows(min(umax, kMaxFrm));
     const u32 tslot = dyn_slot_bytes(trows), uslot = dyn_slot_bytes(urows);
     const u32 tnrm = trows * 24u, unrm = urows * 24u;
     unsigned char *tile = smem_raw + ((sizeof(DynCtrl) + 127) & ~127u);
@@ -144,12 +87,7 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
     u32 R = ring_cap / uslot;
     if (R > (u32)kDynRMax) R = kDynRMax;
 
-    // ---- template tile ------------------------------------------------------------------------------------------
-    for (int tt = warp; tt < Tt; tt += kDynWarps) {
-        const u32 frm = c.tfrm[tt];
-        const int nrows = (frm >= 0xFFFFFFFEu) ? 0 : (int)min(max(frm + 1u, 2u), 119u);
-        stage_qplanes(tile + (size_t)tt * tslot, tnrm, bank + (size_t)c.tslot_id[tt] * slot_stride, nrows, lane, 32);
-    }
+    stage_tile(tile, tslot, tnrm, c.tfrm, c.tslot_id, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kDynWarps);
     __syncthreads();
 
     const u32 nseq = (B - blockIdx.y + gridDim.y - 1) / gridDim.y;       // utterances of this CTA: blockIdx.y + seq*gridDim.y
@@ -163,12 +101,11 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
             if (lane == 0) while (ld_acquire_s(&c.done[slot]) != want) __nanosleep(64);
             __syncwarp();
             const u32 u = blockIdx.y + seq * gridDim.y;
-            u32 frm = 0xFFFFFFFFu;
+            u32 frm = kNoWalk;
             if (!(status && status[u] != SR_ST_OK)) {                    // VAD/MFCC failed: spch_recg returns before dtw
                 const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
-                frm = (*reinterpret_cast<const u32 *>(uf)) >> 16;
-                if (frm > 119u) frm = 0xFFFFFFFEu;
-                else stage_qplanes(ring + (size_t)slot * uslot, unrm, uf, (int)min(max(frm + 1u, 2u), urows), lane, 32);
+                frm = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
+                stage_planes(ring + (size_t)slot * uslot, unrm, uf, min(staged_rows(frm), (int)urows), lane, 32);
             }
             __syncwarp();
             if (lane == 0) { c.ufrm[slot] = frm; st_release_s(&c.flag[slot], seq + 1u); }
@@ -177,18 +114,13 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
     }
 
     // ================================ consumers: pull pairs, walk ===================================================
-    const u32 tile_s = smem_u32(tile), ring_s = smem_u32(ring);
     bool active = false, exhausted = false;
-    QRow i0, i1, m0, m1;
-    u32 dis = 0, step = 0, urow_s = 0, trow_s = 0, slot = 0, out_u = 0, out_t = 0;
+    PRow i0, i1, m0, m1;
+    const unsigned char *urow = ring, *trow = tile;   // shared from the start: kept as 32-bit shared addresses
+    u32 dis = 0, step = 0, slot = 0, out_u = 0, out_t = 0;
     int x = 0, y = 0, I = 0, M = 0, X1 = 0, X2 = 0, ya0 = 0, yb0 = 0, ya1 = 0, yb1 = 0;
-    // dtw_limit (DTW.C:76-109) as an open y interval per column: ins(x,y) <=> yb(x) < y < ya(x)
-    auto ya = [&](int xx) { return xx < X1 ? 2 * xx + 2 : (xx + (4 - I + 2 * M + 1)) >> 1; };
-    auto yb = [&](int xx) { return xx < X2 ? (xx - 2) >> 1 : 2 * xx + (M - 2 * I - 4); };
     auto finish = [&](u32 result) {
-        if (score) score[(size_t)out_u * T + out_t] = result;
-        if (best) atomicMin(reinterpret_cast<unsigned long long *>(&best[out_u]),
-                            (unsigned long long)(((u64)result << 32) | (u64)out_t));   // strict '<', first wins == lexicographic min
+        emit_pair(score, best, T, out_u, out_t, result);
         red_release_add_s(&c.done[slot], 1u);
         active = false;
     };
@@ -220,38 +152,17 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
                 pending = false;
                 out_u = blockIdx.y + pend_seq * gridDim.y; out_t = c.tslot_id[pend_tl];
                 const u32 Iraw = c.ufrm[slot], Mraw = c.tfrm[pend_tl];
-                I = (int)Iraw; M = (int)Mraw;
-                if (Iraw >= 0xFFFFFFFEu || Mraw >= 0xFFFFFFFEu || I > M * 2 || 2 * I < M) finish(SR_DIS_ERR);       // DTW.C:133
+                if (!pair_walks(Iraw, Mraw)) finish(SR_DIS_ERR);
                 else {
-                    urow_s = ring_s + slot * uslot; trow_s = tile_s + pend_tl * tslot;
-                    X1 = (2 * M - I) / 3; X2 = (4 * I - 2 * M) / 3;                                     // DTW.C:141-142
-                    load_qrow(i0, urow_s, unrm, 0); load_qrow(m0, trow_s, tnrm, 0);
-                    load_qrow(i1, urow_s, unrm, 1); load_qrow(m1, trow_s, tnrm, 1);
-                    dis = qdist(i0, m0);                                                             // DTW.C:146
-                    x = 1; y = 1; step = 1;
-                    ya0 = ya(1); yb0 = yb(1); ya1 = ya(2); yb1 = yb(2);
+                    urow = ring + slot * uslot; trow = tile + pend_tl * tslot;
+                    I = (int)Iraw; M = (int)Mraw;
+                    greedy_start(I, M, X1, X2, i0, i1, m0, m1, dis, step, x, y, ya0, yb0, ya1, yb1, urow, unrm, trow, tnrm);
                     active = true;
                 }
             } else if (act == 0) __nanosleep(100);                        // nothing to walk meanwhile: do not hammer the flag
-        } else if (active) {                                              // one step of DTW.C:150-188
-            const u32 d_up = qdist(m1, i0), d_right = qdist(m0, i1), d_ru = qdist(m1, i1);
-            const u32 up = (y + 1 < ya0 && y + 1 > yb0) ? d_up : SR_DIS_ERR;
-            const u32 right = (y < ya1 && y > yb1) ? d_right : SR_DIS_ERR;
-            const u32 ru = (y + 1 < ya1 && y + 1 > yb1) ? d_ru : SR_DIS_ERR;
-            u32 mn = ru;
-            if (mn > right) mn = right;
-            if (mn > up) mn = up;
-            dis += mn;
-            const bool mv_x = (mn == ru) || (mn != up);                   // diag, else up, else right
-            const bool mv_y = (mn == ru) || (mn == up);
-            ++step;
-            if (mv_x) { i0 = i1; ++x; ya0 = ya1; yb0 = yb1; ya1 = ya(x + 1); yb1 = yb(x + 1); }
-            if (mv_y) { m0 = m1; ++y; }
-            if (!(x < I && y < M)) finish(dis / (step & 0xFFFFu));        // DTW.C:191 (step is u16)
-            else {
-                if (mv_x) load_qrow(i1, urow_s, unrm, x);
-                if (mv_y) load_qrow(m1, trow_s, tnrm, y);
-            }
+        } else if (active) {
+            if (!greedy_step(I, M, X1, X2, i0, i1, m0, m1, dis, step, x, y, ya0, yb0, ya1, yb1, urow, unrm, trow, tnrm))
+                finish(dis / (step & 0xFFFFu));                           // DTW.C:191 (step is u16)
         }
     }
 }
@@ -271,22 +182,6 @@ __global__ void frm_max_kernel(const unsigned char *__restrict__ ftr, u32 B, con
     if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
 }
 
-static cudaError_t launch_dyn_tiles(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
-                                    u64 *best, const u8 *status, int num_sms, cudaStream_t st, u32 tile0, u32 ntiles,
-                                    const u32 *max_frm_dev, const u32 *B_dev, const u32 *perm) {
-    const u32 smem = 226 * 1024;
-    cudaError_t e = cudaFuncSetAttribute(dtw_dyn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    u32 gy = (u32)num_sms / ntiles;                      // one CTA per SM, never a second partial wave
-    if (gy < 1) gy = 1;
-    if (gy > B) gy = B;
-    if (gy > 65535) gy = 65535;
-    dtw_dyn_kernel<<<dim3(ntiles, gy), kDynWarps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
-                                                                 static_cast<const unsigned char *>(bank), T, slot_stride, flags,
-                                                                 score, best, status, tile0, smem, max_frm_dev, B_dev, perm);
-    return cudaGetLastError();
-}
-
 // scratch: one device word for the maximum frame count (owned by the caller's handle)
 cudaError_t launch_dtw_dyn(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
                            u64 *best, const u8 *status, int num_sms, cudaStream_t st, u32 *max_frm_scratch, const u32 *B_dev,
@@ -301,13 +196,15 @@ cudaError_t launch_dtw_dyn(const void *in_ftr, u32 B, const void *bank, u32 T, u
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    const u32 full = T / 32u, rem = T % 32u;
-    if (full) {
-        cudaError_t e = launch_dyn_tiles(in_ftr, B, bank, T, slot_stride, flags, score, best, status, num_sms, st, 0, full, max_frm_scratch, B_dev, perm);
-        if (e != cudaSuccess) return e;
-    }
-    if (rem) return launch_dyn_tiles(in_ftr, B, bank, T, slot_stride, flags, score, best, status, num_sms, st, full, 1, max_frm_scratch, B_dev, perm);
-    return cudaSuccess;
+    const u32 smem = 226 * 1024;
+    cudaError_t e = cudaFuncSetAttribute(dtw_dyn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    return launch_tiles(T, [&](u32 tile0, u32 ntiles, int) {
+        dtw_dyn_kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, 1u)), kDynWarps * 32, smem, st>>>(
+            static_cast<const unsigned char *>(in_ftr), B, static_cast<const unsigned char *>(bank), T, slot_stride, flags,
+            score, best, status, tile0, smem, max_frm_scratch, B_dev, perm);
+        return cudaGetLastError();
+    });
 }
 
 }  // namespace srk

@@ -663,6 +663,31 @@ def test_dtw_band_extension_vs_own_dp_oracle(handle, r):
     assert (want != ob.NULL).any() and (want == ob.NULL).any()
     key = (want.astype(np.uint64) << np.uint64(32)) | np.arange(T, dtype=np.uint64)[None, :]
     assert np.array_equal(bd, (key.min(axis=1) >> np.uint64(32)).astype(np.uint32))
+    # headers the banded kernels decode: unsigned and erased slots under the save_sign check, frm_num == 0 on both sides,
+    # and one template with frm_num > vv_frm_max (never walked; the oracle would read past the struct, so its column is
+    # checked directly and left out of the comparison)
+    fin = ftr.copy()
+    fin["frm_num"][:2] = 0
+    bank2 = bank.copy()
+    erased = np.random.default_rng(r).random(T) < 0.2
+    erased[[3, 5]] = False
+    bank2[erased, 0:2] = 0xFF
+    bank2[1, 0:2] = 0                                      # unsigned
+    bank2[3, 2:4] = 0                                      # frm_num 0
+    bank2[5, 2:4] = (200, 0)                               # frm_num 200 > vv_frm_max
+    handle.set_bank(bank2, T, 4096)
+    score, bi, bd = handle.dtw(fin, flags=sr_b200.DTW_BAND | sr_b200.DTW_CHECK_SIGN, band_r=r)
+    bank_o = bank2.copy()
+    bank_o[5, 0:2] = 0xFF                                  # the oracle skips it under the save_sign check
+    want, _ = ob.port().dtw_batch(fin, bank_o, T, 4096, check_sign=1, band_r=r, nthreads=4)
+    cols = np.arange(T) != 5
+    assert np.array_equal(score[:, cols], want[:, cols])
+    assert (score[:, 5] == ob.NULL).all() and (score[:, erased | (np.arange(T) == 1)] == ob.NULL).all()
+    assert (score[:2, 3] == ob.NULL).all() and (score[2:][:, cols] != ob.NULL).any()
+    want[:, 5] = ob.NULL
+    key = (want.astype(np.uint64) << np.uint64(32)) | np.arange(T, dtype=np.uint64)[None, :]
+    k = key.min(axis=1)
+    assert np.array_equal(bi, (k & np.uint64(0xFFFFFFFF)).astype(np.uint32)) and np.array_equal(bd, (k >> np.uint64(32)).astype(np.uint32))
 
 
 # ---- spch_recg ---------------------------------------------------------------------------------------
