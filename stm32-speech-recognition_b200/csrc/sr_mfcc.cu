@@ -27,11 +27,11 @@
 // stage maps complex magnitudes <= M to magnitudes <= (M + 3*1.00015*M)/4 + 3 (twiddle rounding
 // |W| <= 1.00015, a few LSB of floor rounding), so after four stages every component is <= 8209 << 32767
 // and the sign-extending truncation is the identity (also no 32-bit overflow: 2*8209*16385 < 2^31).
-// The generic kernel below keeps the wrap because it accepts arbitrary complex input.
+// The generic kernel below runs the shared core's FFT, which keeps the wrap because it accepts arbitrary complex input.
 #include <stdio.h>
 #include <stdlib.h>
 #include <type_traits>
-#include "sr_common.cuh"
+#include "sr_mfcc_core.cuh"
 
 #ifndef SR_MFCC_DEFAULT_WARPS
 #define SR_MFCC_DEFAULT_WARPS 16
@@ -62,25 +62,6 @@ struct __align__(16) MfccSmem {
     int turn;                                // dynamic hand-out: number of the CTA's next claim (claims are made in ring order)
 };
 
-// (u32)(log((double)v)*100) via the exact threshold table (MFCC.C:168; log(0) pinned to 0)
-__device__ __forceinline__ u32 log100(u32 v, const u32 *thr) {
-    if (v == 0) return 0;
-    int L = (int)(__log2f(__uint2float_rn(v)) * 69.31471805599453f);
-    L = max(0, min(L, 2218));
-    while (v < thr[L]) --L;                       // thr[0] = 1 <= v, so this stops at L >= 0
-    while (L < 2218 && v >= thr[L + 1]) ++L;
-    return (u32)L;
-}
-
-// frame count of a segment, MFCC.C:102-107 (u32 wrap, u16 truncation); 0 = rejected / empty
-__device__ __forceinline__ int mfcc_frames(u32 start, u32 end, u32 U) {
-    if (start == SR_SEG_NULL || end == SR_SEG_NULL || end > U || start > end) return 0;
-    u32 len = end - start;
-    if (len < SR_FRAME_LEN) return 0;             // loop MFCC.C:113 never runs
-    u32 n = (len - SR_FRAME_LEN) / SR_FRAME_MOV + 1u;
-    return n > SR_VV_FRM_MAX ? 0 : (int)n;
-}
-
 static_assert(sizeof(MfccSmem<16, 3>) <= 232448, "s16 variant exceeds the 227 KB shared-memory opt-in limit");
 static_assert(sizeof(MfccSmem<15, 3>) <= 232448, "w15 variant exceeds the 227 KB shared-memory opt-in limit");
 
@@ -100,7 +81,7 @@ __device__ __forceinline__ void stage_utterance(MfccSmem<kConsumerWarps, kNBuf> 
         if (kRelaxedWait) mbar_wait_relaxed(&sm.empty[s], ((it / kNBuf) - 1) & 1);
         else mbar_wait(&sm.empty[s], ((it / kNBuf) - 1) & 1);
     }
-    const int F = mfcc_frames(st, en, U);
+    const int F = mfcc_frames<SR_FRAME_LEN>(st, en, U);
     if (lane == 0) *reinterpret_cast<u16 *>(ftr + (size_t)b * kFtrBytes + 2) = (u16)F;   // MFCC.C:106,189
     if (F == 0) {
         if (lane == 0) { sm.meta[s][0] = 0; sm.meta[s][1] = 0; sm.meta[s][2] = (s32)mid; sm.meta[s][3] = (s32)b; mbar_arrive(&sm.full[s]); }
@@ -291,10 +272,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
 #pragma unroll
             for (int k = 0; k < 5; ++k) {
                 const int i = lane + 32 * k;
-                const s32 cur = (s32)((u32)xf[i + 1] - (u32)mid), prv = (s32)((u32)xf[i] - (u32)mid);
-                const s32 t = (s32)((u32)cur - (u32)((s32)((u32)prv * 95u) / 100));
-                const s32 w = (s32)(s16)((s32)((u32)t * hm[k]) / 1000);
-                wq[i] = w >> 2;                                           // BUTFLY4ZERO_OPT with B=C=D=0
+                wq[i] = preemph_hamm(xf[i + 1], xf[i], (u32)mid, hm[k]) >> 2;   // BUTFLY4ZERO_OPT with B=C=D=0
             }
         };
         for (int f = (int)((warp - (int)(gidx % kConsumerWarps) + kConsumerWarps) % kConsumerWarps); f < F;
@@ -438,17 +416,11 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
                 sm.lg[warp][lane] = (lane < 24) ? log100(acc, sm.log_thr) : 0u;
             }
             __syncwarp();
-            // ---- DCT, MFCC.C:173-183: each term truncated toward zero, s16 accumulate ----------
+            // ---- DCT, MFCC.C:173-183 ---------------------------------------------------------
             {
-                const u32 *lgp = &sm.lg[warp][(lane & 1) * 12];
                 const int4 d0 = dctk4[0], d1 = dctk4[1], d2 = dctk4[2];
                 const s32 dctk[12] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w, d2.x, d2.y, d2.z, d2.w};
-                s32 acc = 0;
-#pragma unroll
-                for (int i = 0; i < 12; ++i) acc += ((s32)lgp[i] * dctk[i]) / 100;
-                acc += __shfl_xor_sync(0xFFFFFFFFu, acc, 1);
-                if (lane < 24 && (lane & 1) == 0)
-                    *reinterpret_cast<s16 *>(out_rows + (size_t)f * kRowBytes + (lane >> 1) * 2) = (s16)acc;
+                dct_row(sm.lg[warp], dctk, out_rows + (size_t)f * kRowBytes, lane);
             }
             __syncwarp();
         }
@@ -505,33 +477,7 @@ fft_generic_kernel(const u32 *__restrict__ in /*[n][1024] packed or NULL*/, cons
         x[i] = v;
     }
     __syncwarp();
-    for (int idx = lane; idx < 256; idx += 32) {                                 // .s:226-232
-        const int j = (int)(__brev((u32)idx) >> 24);
-        const u32 A = x[j], C = x[j + 256], Bv = x[j + 512], D = x[j + 768];
-        u32 o[8];
-        cxadda4<0>(lo16s(A), hi16s(A), lo16s(Bv), hi16s(Bv), lo16s(C), hi16s(C), lo16s(D), hi16s(D),
-                   o[0], o[1], o[2], o[3], o[4], o[5], o[6], o[7]);
-#pragma unroll
-        for (int m = 0; m < 4; ++m) y[4 * idx + m] = pack16(o[2 * m], o[2 * m + 1]);
-    }
-    __syncwarp();
-    int toff = 0;
-    for (int s = 4; s <= 256; s <<= 2) {                                         // .s:254-279
-        for (int t = lane; t < 256; t += 32) {
-            const int q = t % s, base = (t / s) * 4 * s;
-            const int2 k3 = tab->tw[(toff + q) * 3], k2 = tab->tw[(toff + q) * 3 + 1], k1 = tab->tw[(toff + q) * 3 + 2];
-            const u32 p0 = y[base + q], p1 = y[base + q + s], p2 = y[base + q + 2 * s], p3 = y[base + q + 3 * s];
-            u32 Dr, Di, Cr, Ci, Br, Bi, o[8];
-            cxmul(Dr, Di, lo16s(p3), hi16s(p3), (u32)k3.x, (u32)k3.y);
-            cxmul(Cr, Ci, lo16s(p2), hi16s(p2), (u32)k2.x, (u32)k2.y);
-            cxmul(Br, Bi, lo16s(p1), hi16s(p1), (u32)k1.x, (u32)k1.y);
-            cxadda4<14>(lo16s(p0), hi16s(p0), Br, Bi, Cr, Ci, Dr, Di, o[0], o[1], o[2], o[3], o[4], o[5], o[6], o[7]);
-#pragma unroll
-            for (int m = 0; m < 4; ++m) y[base + q + m * s] = pack16(o[2 * m], o[2 * m + 1]);
-        }
-        __syncwarp();
-        toff += s;
-    }
+    fft_radix4<1024>(x, y, tab, lane);
     if (raw_out) for (int i = lane; i < 1024; i += 32) raw_out[(size_t)fr * 1024 + i] = y[i];
     if (mag) for (int i = lane; i < 512; i += 32) mag[(size_t)fr * 512 + i] = mag10(lo16s(y[i]), hi16s(y[i]));
 }

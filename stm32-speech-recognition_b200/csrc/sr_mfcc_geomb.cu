@@ -9,25 +9,16 @@
 // integer rule of MFCC.C (pre-emphasis 95/100, hamm/1000, sqrtf*10, u32 energies, tri/100, log*100, DCT/100 into an
 // s16) is kept. Its only checker is oracle/sr_oracle.c::sro_mfcc_geom_b.
 //
-// One CTA per utterance (persistent over the batch), one frame per warp; the FFT runs in shared memory with the
-// generic butterflies (s16 wrap on every store kept: a 200-sample frame does not enjoy the stage-0 collapse of the
-// reference geometry). Not the benchmarked path: simple and exact rather than tuned.
-#include "sr_common.cuh"
+// One CTA per utterance (persistent over the batch), one frame per warp. The FFT is the N = 256 instance of the shared
+// core's fft_radix4 (sr_mfcc_core.cuh), the device code the drop-in fft runs at N = 1024 (s16 wrap on every store kept:
+// a 200-sample frame does not enjoy the stage-0 collapse of the reference geometry). Not the benchmarked path: simple
+// and exact rather than tuned.
+#include "sr_mfcc_core.cuh"
 
 namespace srk {
 
 constexpr int kGbWarps = 8;
 constexpr int kGbFrame = 200, kGbN = 256, kGbBins = 128;
-
-// log table lookup shared with sr_mfcc.cu (same exact threshold table)
-__device__ __forceinline__ u32 log100_gb(u32 v, const u32 *thr) {
-    if (v == 0) return 0;
-    int L = (int)(__log2f(__uint2float_rn(v)) * 69.31471805599453f);
-    L = max(0, min(L, 2218));
-    while (v < thr[L]) --L;
-    while (L < 2218 && v >= thr[L + 1]) ++L;
-    return (u32)L;
-}
 
 __global__ void __launch_bounds__(kGbWarps * 32)
 mfcc_geomb_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restrict__ seg, u32 seg_stride,
@@ -50,12 +41,7 @@ mfcc_geomb_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
         const u32 st = seg[(size_t)b * seg_stride], en = seg[(size_t)b * seg_stride + 1];
         const s32 mid = (s32)atap[b].mid_val;
         const size_t row = row_map ? row_map[b] : b;
-        // frame count, MFCC.C:102-107 with frame_len = 200
-        int F = 0;
-        if (st != SR_SEG_NULL && en != SR_SEG_NULL && en <= U && st <= en && en - st >= (u32)kGbFrame) {
-            const u32 n = (en - st - (u32)kGbFrame) / SR_FRAME_MOV + 1u;
-            F = n > SR_VV_FRM_MAX ? 0 : (int)n;
-        }
+        const int F = mfcc_frames<kGbFrame>(st, en, U);
         if (threadIdx.x == 0) *reinterpret_cast<u16 *>(ftr + (size_t)b * kFtrBytes + 2) = (u16)F;
         const u16 *xs = pcm + row * U + st;                        // xs[-1] is read (MFCC.C:119); pinned to mid at the very start
         const bool at_origin = (row == 0 && st == 0);
@@ -68,43 +54,13 @@ mfcc_geomb_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
                 const int i = lane + 32 * k;
                 u32 v = 0;
                 if (i < kGbFrame) {
-                    const u32 c = xf[i];
                     const u32 p = (i == 0 && f == 0 && at_origin) ? (u32)mid : (u32)xf[i - 1];
-                    const s32 cur = (s32)(c - (u32)mid), prv = (s32)(p - (u32)mid);
-                    const s32 t = (s32)((u32)cur - (u32)((s32)((u32)prv * 95u) / 100));
-                    v = (u32)(u16)(s16)((s32)((u32)t * (u32)tab->b_hamm[i]) / 1000);
+                    v = (u32)(u16)preemph_hamm(xf[i], p, (u32)mid, tab->b_hamm[i]);
                 }
                 x[i] = v;
             }
             __syncwarp();
-            // first pass: 64 x BUTFLY4ZERO_OPT, 6-bit reversed gather (.s:132-178, 226-232 for N = 256)
-            for (int idx = lane; idx < 64; idx += 32) {
-                const int j = (int)(__brev((u32)idx) >> 26);
-                const u32 A = x[j], Cv = x[j + 64], Bv = x[j + 128], D = x[j + 192];
-                u32 o[8];
-                cxadda4<0>(lo16s(A), hi16s(A), lo16s(Bv), hi16s(Bv), lo16s(Cv), hi16s(Cv), lo16s(D), hi16s(D),
-                           o[0], o[1], o[2], o[3], o[4], o[5], o[6], o[7]);
-#pragma unroll
-                for (int m = 0; m < 4; ++m) y[4 * idx + m] = pack16(o[2 * m], o[2 * m + 1]);
-            }
-            __syncwarp();
-            int toff = 0;
-            for (int s = 4; s <= 64; s <<= 2) {                       // .s:254-279, strides 4, 16, 64
-                for (int t = lane; t < 64; t += 32) {
-                    const int q = t % s, base = (t / s) * 4 * s;
-                    const int2 k3 = tab->tw[(toff + q) * 3], k2 = tab->tw[(toff + q) * 3 + 1], k1 = tab->tw[(toff + q) * 3 + 2];
-                    const u32 p0 = y[base + q], p1 = y[base + q + s], p2 = y[base + q + 2 * s], p3 = y[base + q + 3 * s];
-                    u32 Dr, Di, Cr, Ci, Br, Bi, o[8];
-                    cxmul(Dr, Di, lo16s(p3), hi16s(p3), (u32)k3.x, (u32)k3.y);
-                    cxmul(Cr, Ci, lo16s(p2), hi16s(p2), (u32)k2.x, (u32)k2.y);
-                    cxmul(Br, Bi, lo16s(p1), hi16s(p1), (u32)k1.x, (u32)k1.y);
-                    cxadda4<14>(lo16s(p0), hi16s(p0), Br, Bi, Cr, Ci, Dr, Di, o[0], o[1], o[2], o[3], o[4], o[5], o[6], o[7]);
-#pragma unroll
-                    for (int m = 0; m < 4; ++m) y[base + q + m * s] = pack16(o[2 * m], o[2 * m + 1]);
-                }
-                __syncwarp();
-                toff += s;
-            }
+            fft_radix4<kGbN>(x, y, tab, lane);
             // magnitude (MFCC.C:49-60) and energy (MFCC.C:128-133) of bins 0..127 -> x[0..127]
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
@@ -117,19 +73,10 @@ mfcc_geomb_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
             {
                 u32 acc = 0;
                 for (int i = flo; i < fhi; ++i) acc += (x[i] * (u32)tri[i]) / 100u;
-                lg[warp][lane] = (lane < 24) ? log100_gb(acc, tab->log_thr) : 0u;
+                lg[warp][lane] = (lane < 24) ? log100(acc, tab->log_thr) : 0u;
             }
             __syncwarp();
-            // DCT, MFCC.C:173-183
-            {
-                const u32 *lgp = &lg[warp][(lane & 1) * 12];
-                s32 acc = 0;
-#pragma unroll
-                for (int i = 0; i < 12; ++i) acc += ((s32)lgp[i] * dctk[i]) / 100;
-                acc += __shfl_xor_sync(0xFFFFFFFFu, acc, 1);
-                if (lane < 24 && (lane & 1) == 0)
-                    *reinterpret_cast<s16 *>(out_rows + (size_t)f * kRowBytes + (lane >> 1) * 2) = (s16)acc;
-            }
+            dct_row(lg[warp], dctk, out_rows + (size_t)f * kRowBytes, lane);   // MFCC.C:173-183
             __syncwarp();
         }
     }

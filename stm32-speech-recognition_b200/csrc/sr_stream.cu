@@ -89,9 +89,7 @@ stream_step_kernel(u16 *__restrict__ pcm, u32 L, u32 S, const u16 *__restrict__ 
         if (n_len != 0 && n_len % 240u == 0) {                        // else atap stays untouched (VAD.C:33-36)
             u32 m, max_sum, abs_sum;
             atap_stats(x, vec_ok, n_len, lane, m, max_sum, abs_sum);
-            abs_sum /= (n_len / SR_FRAME_LEN);                        // VAD.C:65
-            max_sum /= (n_len / 240u);                                // VAD.C:66
-            at.mid_val = m; at.n_thl = (u16)max_sum; at.s_thl = abs_sum * 11u / 10u; at.z_thl = 2;
+            atap_finish(at, n_len, m, max_sum, abs_sum);
         }
     }
     const u32 mid = at.mid_val, a_thl = mid + at.n_thl, b_thl = mid - at.n_thl;          // VAD.C:112-113 (u32 wrap)

@@ -111,9 +111,7 @@ vad_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, u32 n_len, u32 buf_len, in
         if (atap_on && !atap_staged) {
             u32 m, max_sum, abs_sum;
             atap_stats(pcm + ubase, false, n_len, lane, m, max_sum, abs_sum);
-            abs_sum /= (n_len / SR_FRAME_LEN);                             // VAD.C:65
-            max_sum /= (n_len / 240u);                                     // VAD.C:66
-            at.mid_val = m; at.n_thl = (u16)max_sum; at.s_thl = abs_sum * 11u / 10u; at.z_thl = 2;
+            atap_finish(at, n_len, m, max_sum, abs_sum);
             if (lane == 0) atap[b] = at;
         }
         u32 mid = at.mid_val, a_thl = mid + at.n_thl, b_thl = mid - at.n_thl;            // VAD.C:112-113 (u32 wrap)
@@ -139,12 +137,7 @@ vad_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, u32 n_len, u32 buf_len, in
             if (c0 == 0 && atap_staged) {
                 u32 m, max_sum, abs_sum;
                 atap_stats(v.x, v.vec_ok, n_len, lane, m, max_sum, abs_sum);   // VAD.C:41-63
-                abs_sum /= (n_len / SR_FRAME_LEN);                             // VAD.C:65
-                max_sum /= (n_len / 240u);                                     // VAD.C:66
-                at.mid_val = m;
-                at.n_thl = (u16)max_sum;                                       // n_thl_ratio 1, VAD.C:68
-                at.s_thl = abs_sum * 11u / 10u;                                // s_thl_ratio 11/10, VAD.C:69
-                at.z_thl = 2;                                                  // 160*2/160/1, VAD.C:70
+                atap_finish(at, n_len, m, max_sum, abs_sum);
                 if (lane == 0) atap[b] = at;
                 mid = m; a_thl = mid + at.n_thl; b_thl = mid - at.n_thl;
             }

@@ -71,6 +71,16 @@ __device__ __forceinline__ void atap_stats(const u16 *x, bool vec_ok, u32 n_len,
     mid_out = mid; max_sum_out = max_sum; abs_sum_out = warp_sum(abs_sum);
 }
 
+// the rest of noise_atap (VAD.C:65-70) from atap_stats' results: averages over the window, thresholds into at
+__device__ __forceinline__ void atap_finish(atap_tag &at, u32 n_len, u32 mid, u32 max_sum, u32 abs_sum) {
+    abs_sum /= (n_len / SR_FRAME_LEN);                               // VAD.C:65
+    max_sum /= (n_len / 240u);                                       // VAD.C:66
+    at.mid_val = mid;
+    at.n_thl = (u16)max_sum;                                         // n_thl_ratio 1, VAD.C:68
+    at.s_thl = abs_sum * 11u / 10u;                                  // s_thl_ratio 11/10, VAD.C:69
+    at.z_thl = 2;                                                    // 160*2/160/1, VAD.C:70
+}
+
 // per-block summary: bs = sum |x-mid| over the 80 samples; flags = zc (bits 0..6, alternations inside the
 // block) | lc << 7 (class of last out-of-band sample, 0 none / 1 below / 2 above) | lcA << 9 (same over the
 // first 79 samples) | p0 << 11 (sample 0 is out of band)
