@@ -3,18 +3,11 @@
 // recognition path happens on the host: every result is produced by the kernels in sr_vad.cu,
 // sr_mfcc.cu and sr_dtw.cu. Without a CUDA device every entry point fails loudly.
 #include "sr_internal.h"
-#include <chrono>
-#include <condition_variable>
-#include <deque>
-#include <utility>
 #include "sr_pack_host.h"
 #include "sr_numa.h"
 #include <map>
 #include <algorithm>
-
-#ifndef SR_TRANSPORT_AUTO_DEFAULT
-#define SR_TRANSPORT_AUTO_DEFAULT 1      // what mode -1 (automatic) means: 1 = pack when this rank's share of the CPUs is >= 6
-#endif
+#include <type_traits>
 
 static int device_numa_node(int device) {
     char id[64] = {0};
@@ -76,16 +69,11 @@ int sr_destroy(sr_handle *h) {
     DeviceGuard g(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     sr_comm_destroy(h);
-    delete h->pool;
-    for (void *&st : h->stage) if (st) { cudaFreeHost(st); st = nullptr; }
-    DevBuf *bufs[] = {&h->dpacked, &h->bank_own, &h->pcm, &h->atap, &h->seg, &h->ftr, &h->score, &h->best, &h->best_alt, &h->status,
-                      &h->bidx, &h->bdis, &h->cmd, &h->misc0, &h->misc1, &h->misc2, &h->dtw_scratch, &h->bank_perm, &h->vad_work, &h->mfcc_work};
-    for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
     for (int i = 0; i < 2; ++i) { if (h->ev_h2d[i]) cudaEventDestroy(h->ev_h2d[i]); if (h->ev_done[i]) cudaEventDestroy(h->ev_done[i]); }
-    delete h;
+    delete h;                                           // frees the workspaces and stops the transport's workers, under g
     return 0;
 }
 
@@ -360,6 +348,43 @@ int sr_recognise_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32
 
 }  // extern "C"
 
+// sr_recog_out field by field: f(member, the handle's device mirror of it, bytes per utterance); score holds one word per
+// template of the handle's bank
+template <class F> static void for_each_output(sr_handle *h, F f) {
+    f(&sr_recog_out::atap, h->atap, sizeof(atap_tag));
+    f(&sr_recog_out::seg_off, h->seg, (size_t)24);
+    f(&sr_recog_out::ftr, h->ftr, (size_t)kFtrBytes);
+    f(&sr_recog_out::score, h->score, (size_t)h->n_slot * 4);
+    f(&sr_recog_out::best_idx, h->bidx, (size_t)4);
+    f(&sr_recog_out::best_dis, h->bdis, (size_t)4);
+    f(&sr_recog_out::cmd, h->cmd, (size_t)4);
+    f(&sr_recog_out::status, h->status, (size_t)1);
+}
+
+// the outputs of utterances [lo, ...) of o; NULL fields stay NULL
+static sr_recog_out recog_slice(sr_handle *h, const sr_recog_out &o, size_t lo) {
+    sr_recog_out s = o;
+    for_each_output(h, [&](auto m, DevBuf &, size_t bytes) { if (s.*m) s.*m += lo * bytes / sizeof *(s.*m); });
+    return s;
+}
+
+// get_mfcc (MFCC.C) and get_mdl (DTW.C) never write save_sign: copy back bytes [2, 2860) of each of n structs only
+static cudaError_t ftr_to_host(sr_handle *h, v_ftr_tag *dst, const void *src, size_t n) {
+    return cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(dst) + 2, kFtrBytes, static_cast<const unsigned char *>(src) + 2,
+                             kFtrBytes, kFtrBytes - 2, n, cudaMemcpyDeviceToHost, h->stream);
+}
+
+// the front end of spch_recg and save_mdl on B staged utterances: noise_atap, VAD, get_mfcc of segment 0, status
+static int front_end(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 n_len, atap_tag *atap, u32 *seg, void *ftr, u8 *status) {
+    // main.c:258-260 noise_atap + VAD (one fused launch on the staged utterance)
+    { TimedLaunch tl(h, TAG_VAD); SR_CK(h, launch_vad(pcm, U, B, n_len, U, 1, 1, atap, seg, h->num_sms, h->stream, vad_work(h))); }
+    // main.c:268 get_mfcc of segment 0
+    { TimedLaunch tl(h, TAG_MFCC); SR_CK(h, launch_mfcc_h(h, pcm, U, B, seg, 6, atap, ftr)); }
+    { TimedLaunch tl(h, TAG_STATUS); SR_CK(h, launch_status(seg, ftr, B, status, h->stream)); }
+    h->launches += 3;
+    return 0;
+}
+
 // wait_comm: order the template scan (the first kernel that rewrites score / best) after the handle's pending collective,
 // so that an all-gather of the previous batch overlaps this batch's VAD and MFCC (sr_comm.cu)
 int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, const sr_recog_out *o,
@@ -380,12 +405,7 @@ int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     if (!ftr) { SR_CK(h, ensure(h->ftr, (size_t)B * kFtrBytes)); ftr = static_cast<v_ftr_tag *>(h->ftr.p); }
     u8 *status = o->status;
     if (!status) { SR_CK(h, ensure(h->status, (size_t)B)); status = static_cast<u8 *>(h->status.p); }
-    // main.c:258-260 noise_atap + VAD (one fused launch on the staged utterance)
-    { TimedLaunch tl(h, TAG_VAD); SR_CK(h, launch_vad(pcm, U, B, n_len, U, 1, 1, atap, seg, h->num_sms, h->stream, vad_work(h))); }
-    // main.c:268 get_mfcc of segment 0
-    { TimedLaunch tl(h, TAG_MFCC); SR_CK(h, launch_mfcc_h(h, pcm, U, B, seg, 6, atap, ftr)); }
-    { TimedLaunch tl(h, TAG_STATUS); SR_CK(h, launch_status(seg, ftr, B, status, h->stream)); }
-    h->launches += 3;
+    if (const int rc = front_end(h, pcm, U, B, n_len, atap, seg, ftr, status)) return rc;
     if (h->comm) {                                       // collectives of earlier calls may still read score / the key buffer
         const int rc = wait_comm ? comm_wait_before_scan(h, o->score) : sr_comm_wait(h);
         if (rc) return rc;
@@ -447,10 +467,7 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
     int rc = sr_mfcc_batch_dev(h, static_cast<const u16 *>(h->pcm.p), U, B, static_cast<const u32 *>(h->seg.p), seg_stride,
                                static_cast<const atap_tag *>(h->atap.p), static_cast<v_ftr_tag *>(h->ftr.p));
     if (rc) return rc;
-    // MFCC.C never writes save_sign: copy back bytes [2, 2860) of every struct only
-    SR_CK(h, cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(ftr) + 2, kFtrBytes,
-                               static_cast<unsigned char *>(h->ftr.p) + 2, kFtrBytes, kFtrBytes - 2, B,
-                               cudaMemcpyDeviceToHost, h->stream));
+    SR_CK(h, ftr_to_host(h, ftr, h->ftr.p, B));
     SR_CK(h, cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -478,69 +495,17 @@ int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, 
     return 0;
 }
 
-// ranks of this node that share the host (torchrun exports LOCAL_WORLD_SIZE)
-static int local_world_size() {
-    static const int local_world = [] { const char *e = getenv("LOCAL_WORLD_SIZE"); const int v = e ? atoi(e) : 1; return v > 0 ? v : 1; }();
-    return local_world;
-}
-// CPUs this rank may count on: the process' usable CPUs (affinity capped by the cgroup quota) divided by those ranks
-static int rank_cpu_share() { return usable_cpus() / local_world_size(); }
-
-// local ranks whose GPU hangs off the same NUMA node as this handle's (torchrun convention: local rank r drives device r);
-// unknown topology counts everybody
-static int ranks_on_socket(const sr_handle *h) {
-    const int W = local_world_size();
-    if (W <= 1) return 1;
-    if (h->numa_node < 0) return W;
-    int n = 0;
-    for (int d = 0; d < W; ++d) if (device_numa_node(d) == h->numa_node) ++n;
-    return n < 1 ? 1 : n;
-}
-
-// 1 = forced on, 0 = forced off, -1 = automatic (decided per call by transport_auto_pick)
-static int transport_mode(const sr_handle *h) {
-    int mode = h->transport_mode;
-    if (mode < 0) {
-        static const int env_mode = [] { const char *e = getenv("SR_PACK12"); return e && *e ? atoi(e) : -1; }();
-        mode = env_mode;
-    }
-    // automatic: needs CPUs to pack with, and the socket's DRAM bandwidth to itself: with several GPUs per socket the DMA
-    // reads alone load it (4 x 54 GB/s at four) and packing measured 25.8 vs 19.5 ms at 4 and 8 ranks, 19.8-21.3 vs 19.5 with
-    // two ranks on one socket -- and ranks that probe at different moments talk each other into it. One rank per socket only.
-    if (mode < 0 && !(SR_TRANSPORT_AUTO_DEFAULT && rank_cpu_share() >= 6 && ranks_on_socket(h) <= 1)) mode = 0;
-    return mode;
-}
-
-// Automatic mode measures instead of guessing. Whether packing pays depends on what else loads the host's memory system:
-// one or two ranks per socket gain ~16 % (16.3 vs 19.4 ms per 1.05 GB), but with four ranks per socket the DMA reads
-// alone take ~216 GB/s of that socket's DRAM bandwidth and the packers' extra traffic makes the call SLOWER (25.8 vs
-// 19.5 ms, measured at 4 and 8 GPUs). So: the first qualifying call goes plain, the second packed, then the faster of
-// the two (ns per byte, exponentially averaged; packing must win by 7 %) is used, with the other re-probed every 32nd call.
-// With more than one rank on this GPU's socket the automatic mode stays plain (transport_mode above).
-static bool transport_auto_pick(sr_handle *h) {
-    const uint64_t n = h->auto_calls++;
-    if (h->auto_ns_per_byte[0] <= 0.0) return false;
-    if (h->auto_ns_per_byte[1] <= 0.0) return true;
-    const bool packed_better = h->auto_ns_per_byte[1] < 0.93 * h->auto_ns_per_byte[0];   // a clear win only (N = 1: 0.84)
-    if (n % 32 == 31) return !packed_better;                       // probe the loser now and then: conditions change
-    return packed_better;
-}
-static void transport_auto_record(sr_handle *h, bool packed, double ns_per_byte) {
-    double &v = h->auto_ns_per_byte[packed ? 1 : 0];
-    v = v <= 0.0 ? ns_per_byte : 0.75 * v + 0.25 * ns_per_byte;
-}
-
 int sr_set_transport(sr_handle *h, int mode) {
     SR_REQUIRE(h, h && mode >= -1 && mode <= 1);
-    h->transport_mode = mode;
+    h->transport.mode = mode;
     return 0;
 }
 
 int sr_transport_stats(const sr_handle *h, uint32_t *packed_chunks, uint32_t *plain_chunks, uint64_t *h2d_bytes) {
     if (!h) return -1;
-    if (packed_chunks) *packed_chunks = h->last_packed;
-    if (plain_chunks) *plain_chunks = h->last_plain;
-    if (h2d_bytes) *h2d_bytes = h->last_h2d;
+    if (packed_chunks) *packed_chunks = h->transport.last_packed;
+    if (plain_chunks) *plain_chunks = h->transport.last_plain;
+    if (h2d_bytes) *h2d_bytes = h->transport.last_h2d;
     return 0;
 }
 
@@ -572,187 +537,56 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
     if (B == 0) return 0;
     DeviceGuard g(h->device);
-    const size_t T = h->n_slot;
-    // chunk: ~32 MB of PCM (SR_CHUNK_MB overrides), a multiple of 8 utterances (keeps every chunk base 16-byte aligned)
-    static const size_t chunk_mb = [] { const char *e = getenv("SR_CHUNK_MB"); const long v = e ? atol(e) : 0; return (size_t)(v > 0 ? v : 32); }();
-    uint32_t chunk = (uint32_t)((chunk_mb << 20) / ((size_t)U * 2));
+    // chunk: ~32 MB of PCM, a multiple of 8 utterances (keeps every chunk base 16-byte aligned)
+    uint32_t chunk = (uint32_t)(((size_t)32 << 20) / ((size_t)U * 2));
     chunk = chunk < 8 ? 8 : (chunk & ~7u);
     if (chunk > B) chunk = B;
     const uint32_t nchunks = (B + chunk - 1) / chunk;
     const size_t chunk_bytes = (((size_t)chunk * U * 2 + 255) / 256) * 256;
     SR_CK(h, ensure(h->pcm, (nchunks > 1 ? 2 : 1) * chunk_bytes + 16));
-    sr_recog_out d;
+    sr_recog_out d;                                     // device mirrors of the non-NULL outputs
     memset(&d, 0, sizeof d);
-    if (o->atap) { SR_CK(h, ensure(h->atap, (size_t)B * sizeof(atap_tag))); d.atap = static_cast<atap_tag *>(h->atap.p);
-                   H2D(h, d.atap, o->atap, (size_t)B * sizeof(atap_tag)); }
-    if (o->seg_off) { SR_CK(h, ensure(h->seg, (size_t)B * 24)); d.seg_off = static_cast<u32 *>(h->seg.p); }
-    if (o->ftr) { SR_CK(h, ensure(h->ftr, (size_t)B * kFtrBytes)); d.ftr = static_cast<v_ftr_tag *>(h->ftr.p); }
-    if (o->score) { SR_CK(h, ensure(h->score, (size_t)B * T * 4 + 4)); d.score = static_cast<u32 *>(h->score.p); }
-    if (o->best_idx) { SR_CK(h, ensure(h->bidx, (size_t)B * 4)); d.best_idx = static_cast<u32 *>(h->bidx.p); }
-    if (o->best_dis) { SR_CK(h, ensure(h->bdis, (size_t)B * 4)); d.best_dis = static_cast<u32 *>(h->bdis.p); }
-    if (o->cmd) { SR_CK(h, ensure(h->cmd, (size_t)B * 4)); d.cmd = static_cast<u32 *>(h->cmd.p); }
-    if (o->status) { SR_CK(h, ensure(h->status, (size_t)B)); d.status = static_cast<u8 *>(h->status.p); }
-    // one chunk: H2D (plain u16, or 12-bit packed from a pinned staging slot + expansion on the device) -> kernels
-    auto issue_chunk = [&](uint32_t c, int buf, const void *packed_src) -> int {
+    cudaError_t e = cudaSuccess;
+    for_each_output(h, [&](auto m, DevBuf &buf, size_t bytes) {
+        if (o->*m && e == cudaSuccess && (e = ensure(buf, B * bytes)) == cudaSuccess)
+            d.*m = static_cast<std::remove_reference_t<decltype(d.*m)>>(buf.p);
+    });
+    if (e != cudaSuccess) return fail(h, "sr_recognise_batch: output buffers", e);
+    // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36)
+    if (o->atap) H2D(h, d.atap, o->atap, (size_t)B * sizeof(atap_tag));
+    uint32_t issued = 0;
+    // one chunk: H2D (plain u16, or 12-bit packed + expansion on the device) -> kernels on its slice of the outputs
+    auto step = [&](uint32_t c, int buf, const void *packed_src) -> int {
         const uint32_t b0 = c * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
         const size_t ns = (size_t)nb * U;
         u16 *dpcm = reinterpret_cast<u16 *>(static_cast<unsigned char *>(h->pcm.p) + (size_t)buf * chunk_bytes);
         cudaStream_t cs = nchunks > 1 ? h->copy_stream : h->stream;
-        if (nchunks > 1 && h->chunk_seq >= 2) SR_CK(h, cudaStreamWaitEvent(cs, h->ev_done[buf], 0));      // buffers free again
-        if (packed_src) {
-            unsigned char *dpk = static_cast<unsigned char *>(h->dpacked.p) + (size_t)buf * h->stage_cap;
-            SR_CK(h, cudaMemcpyAsync(dpk, packed_src, ns / 2 * 3, cudaMemcpyHostToDevice, cs));
-            h->last_h2d += ns / 2 * 3; ++h->last_packed;
-        } else {
-            SR_CK(h, cudaMemcpyAsync(dpcm, pcm + (size_t)b0 * U, ns * 2, cudaMemcpyHostToDevice, cs));
-            h->last_h2d += ns * 2; ++h->last_plain;
-        }
+        if (nchunks > 1 && issued >= 2) SR_CK(h, cudaStreamWaitEvent(cs, h->ev_done[buf], 0));      // buffers free again
+        if (packed_src) SR_CK(h, cudaMemcpyAsync(h->transport.device_stage(buf), packed_src, ns / 2 * 3, cudaMemcpyHostToDevice, cs));
+        else SR_CK(h, cudaMemcpyAsync(dpcm, pcm + (size_t)b0 * U, ns * 2, cudaMemcpyHostToDevice, cs));
         if (nchunks > 1) {
             SR_CK(h, cudaEventRecord(h->ev_h2d[buf], cs));
             SR_CK(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[buf], 0));
         }
         if (packed_src) {
-            SR_CK(h, launch_unpack12(static_cast<unsigned char *>(h->dpacked.p) + (size_t)buf * h->stage_cap, ns, dpcm, h->stream));
+            SR_CK(h, launch_unpack12(h->transport.device_stage(buf), ns, dpcm, h->stream));
             ++h->launches;
         }
-        sr_recog_out dc = d;
-        if (d.atap) dc.atap = d.atap + b0;
-        if (d.seg_off) dc.seg_off = d.seg_off + (size_t)b0 * 6;
-        if (d.ftr) dc.ftr = d.ftr + b0;
-        if (d.score) dc.score = d.score + (size_t)b0 * T;
-        if (d.best_idx) dc.best_idx = d.best_idx + b0;
-        if (d.best_dis) dc.best_dis = d.best_dis + b0;
-        if (d.cmd) dc.cmd = d.cmd + b0;
-        if (d.status) dc.status = d.status + b0;
-        int rc = sr_recognise_batch_dev(h, dpcm, U, nb, n_len, &dc);
-        if (rc) return rc;
+        const sr_recog_out dc = recog_slice(h, d, b0);
+        if (const int rc = sr_recognise_batch_dev(h, dpcm, U, nb, n_len, &dc)) return rc;
         if (nchunks > 1) SR_CK(h, cudaEventRecord(h->ev_done[buf], h->stream));
-        ++h->chunk_seq;
+        ++issued;
         return 0;
     };
-    h->chunk_seq = 0; h->last_packed = 0; h->last_plain = 0; h->last_h2d = 0;
-
-    const int tmode = nchunks >= 4 ? transport_mode(h) : 0;
-    const bool tauto = tmode < 0;
-    bool packed_transport = tmode > 0 || (tauto && transport_auto_pick(h));
-    const auto t_call0 = std::chrono::steady_clock::now();
-    bool did_setup = false;                              // this call created the pool / staging: its time is not a measurement
-    if (packed_transport) {                              // workers, pinned staging slots, device staging
-        const size_t pk = ((((size_t)chunk * U + 1) / 2 * 3 + 64 + 255) / 256) * 256;
-        did_setup = !h->pool || h->stage_cap < pk || h->dpacked.cap < 2 * pk;
-        ScopedNodeAffinity node_scope(h->numa_node);      // workers inherit it; staging pages are allocated from this node
-        if (!h->pool) {
-            // packers = this rank's CPU share minus room for the sender, the CUDA runtime's threads and the caller's own work
-            static const int env_nt = [] { const char *e = getenv("SR_PACK_THREADS"); return e && *e ? atoi(e) : 0; }();
-            // (measured on a 2 x 32-core host, 16-CPU quota: 8..12 packers all land at ~16.3 ms per 1.05 GB step; more only add
-            // memory traffic next to the DMA reads, which slows the link: 54 -> 47 GB/s at 14 packers)
-            int nt = env_nt > 0 ? env_nt : rank_cpu_share() - 3;
-            if (env_nt <= 0 && nt > 10) nt = 10;
-            nt = nt > 16 ? 16 : nt;
-            if (nt >= 2) h->pool = new (std::nothrow) PackPool(nt);
-        }
-        if (h->pool && h->stage_cap < pk) {
-            for (void *&st : h->stage) if (st) { cudaFreeHost(st); st = nullptr; }
-            h->stage_cap = 0;
-            bool ok = true;
-            // SR_PACK_WC=1: write-combined staging (the packers only ever stream whole cache lines into it and never read it back)
-            static const unsigned stage_flags = [] { const char *e = getenv("SR_PACK_WC"); return e && atoi(e) > 0 ? cudaHostAllocWriteCombined : cudaHostAllocDefault; }();
-            for (void *&st : h->stage) if (ok && cudaHostAlloc(&st, pk, stage_flags) != cudaSuccess) { st = nullptr; ok = false; }
-            if (ok) h->stage_cap = pk;
-            else { cudaGetLastError(); for (void *&st : h->stage) if (st) { cudaFreeHost(st); st = nullptr; } }
-        }
-        if (!h->pool || !h->stage_cap || ensure(h->dpacked, 2 * h->stage_cap) != cudaSuccess) { cudaGetLastError(); packed_transport = false; }
-    }
-
-    if (!packed_transport) {
-        for (uint32_t c = 0; c < nchunks; ++c) {
-            int rc = issue_chunk(c, (int)(c & 1), nullptr);
-            if (rc) return rc;
-        }
-    } else {
-        // The caller's thread sends chunks from the front as plain u16, paced by the copy engine; the worker pool packs
-        // chunks from the back into the staging slots and those are sent packed as soon as they are ready. The two
-        // meet in the middle, so the call is never slower than the plain path and approaches 3/4 of its PCIe time.
-        std::mutex m;
-        std::condition_variable cv_slot;
-        std::deque<std::pair<uint32_t, int>> ready;       // (chunk, staging slot)
-        std::vector<uint32_t> retry;                      // chunks that hold a sample >= 4096: sent plain
-        int lo = 0, hi = (int)nchunks - 1;                // unclaimed chunks [lo, hi]
-        unsigned free_mask = (1u << sr_handle::kStage) - 1u;
-        bool abort = false;
-        std::thread packer([&] {
-            ScopedNodeAffinity bind(h->numa_node);        // slice 0 of every chunk is packed by this thread
-            for (;;) {
-                int slot;
-                uint32_t c;
-                {
-                    std::unique_lock<std::mutex> lk(m);
-                    cv_slot.wait(lk, [&] { return abort || lo > hi || free_mask != 0; });
-                    if (abort || lo > hi) return;
-                    slot = __builtin_ctz(free_mask);
-                    free_mask &= ~(1u << slot);
-                    c = (uint32_t)hi--;
-                }
-                const uint32_t b0 = c * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
-                const size_t ns = (size_t)nb * U;
-                const uint32_t orb = (ns & 1) ? 0xFFFFu : h->pool->run(pcm + (size_t)b0 * U, ns, static_cast<uint8_t *>(h->stage[slot]));
-                {
-                    std::lock_guard<std::mutex> lk(m);
-                    if (orb & 0xF000u) { retry.push_back(c); free_mask |= 1u << slot; }
-                    else ready.emplace_back(c, slot);
-                }
-            }
-        });
-        int rc = 0;
-        int slot_of[2] = {-1, -1};                        // staging slot behind the copy last issued on each buffer
-        auto release = [&](int &sl) {
-            if (sl < 0) return;
-            { std::lock_guard<std::mutex> lk(m); free_mask |= 1u << sl; }
-            cv_slot.notify_one();
-            sl = -1;
-        };
-        uint32_t sent = 0;
-        while (sent < nchunks) {
-            int slot = -1;
-            long c = -1;
-            {
-                std::lock_guard<std::mutex> lk(m);
-                if (!ready.empty()) { c = ready.front().first; slot = ready.front().second; ready.pop_front(); }
-                else if (!retry.empty()) { c = retry.back(); retry.pop_back(); }
-                else if (lo <= hi) c = lo++;
-            }
-            if (c < 0) { std::this_thread::sleep_for(std::chrono::microseconds(50)); continue; }   // every chunk is claimed; the pool is still packing
-            const int buf = (int)(sent & 1);
-            if (sent >= 2) {                                               // at most two copies in flight: paces this thread
-                cudaError_t e = cudaEventSynchronize(h->ev_h2d[buf]);
-                if (e != cudaSuccess) { rc = fail(h, "cudaEventSynchronize", e); if (slot >= 0) release(slot); break; }
-                release(slot_of[buf]);
-            }
-            rc = issue_chunk((uint32_t)c, buf, slot >= 0 ? h->stage[slot] : nullptr);
-            if (rc) { if (slot >= 0) release(slot); break; }
-            slot_of[buf] = slot;
-            ++sent;
-        }
-        { std::lock_guard<std::mutex> lk(m); abort = true; }
-        cv_slot.notify_all();
-        packer.join();
-        if (rc) { cudaStreamSynchronize(h->copy_stream); return rc; }
-    }
-    if (o->atap) D2H(h, o->atap, d.atap, (size_t)B * sizeof(atap_tag));
-    if (o->seg_off) D2H(h, o->seg_off, d.seg_off, (size_t)B * 24);
-    if (o->ftr)
-        SR_CK(h, cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(o->ftr) + 2, kFtrBytes,
-                                   reinterpret_cast<unsigned char *>(d.ftr) + 2, kFtrBytes, kFtrBytes - 2, B,
-                                   cudaMemcpyDeviceToHost, h->stream));
-    if (o->score && T) D2H(h, o->score, d.score, (size_t)B * T * 4);
-    if (o->best_idx) D2H(h, o->best_idx, d.best_idx, (size_t)B * 4);
-    if (o->best_dis) D2H(h, o->best_dis, d.best_dis, (size_t)B * 4);
-    if (o->cmd) D2H(h, o->cmd, d.cmd, (size_t)B * 4);
-    if (o->status) D2H(h, o->status, d.status, (size_t)B);
+    if (const int rc = h->transport.send(h, pcm, U, B, chunk, step)) return rc;
+    for_each_output(h, [&](auto m, DevBuf &, size_t bytes) {
+        if (!(o->*m) || !bytes || e != cudaSuccess) return;
+        if constexpr (std::is_same_v<decltype(m), v_ftr_tag *sr_recog_out::*>) e = ftr_to_host(h, o->ftr, d.ftr, B);
+        else e = cudaMemcpyAsync(o->*m, d.*m, B * bytes, cudaMemcpyDeviceToHost, h->stream);
+    });
+    if (e != cudaSuccess) return fail(h, "sr_recognise_batch: copy back", e);
     SR_CK(h, cudaStreamSynchronize(h->stream));
-    if (tauto && !did_setup)
-        transport_auto_record(h, packed_transport && h->last_packed > 0,
-                              std::chrono::duration<double, std::nano>(std::chrono::steady_clock::now() - t_call0).count() / ((double)B * U * 2.0));
+    h->transport.call_done((uint64_t)B * U * 2);
     return 0;
 }
 
@@ -773,11 +607,10 @@ int sr_enrol_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, ui
     SR_CK(h, ensure(h->misc0, (size_t)B * slot_stride));
     H2D(h, h->pcm.p, pcm, (size_t)B * U * 2);
     SR_CK(h, cudaMemsetAsync(h->atap.p, 0, (size_t)B * sizeof(atap_tag), h->stream));
-    { TimedLaunch tl(h, TAG_VAD); SR_CK(h, launch_vad(static_cast<const u16 *>(h->pcm.p), U, B, n_len, U, 1, 1, static_cast<atap_tag *>(h->atap.p), static_cast<u32 *>(h->seg.p), h->num_sms, h->stream, vad_work(h))); }
-    { TimedLaunch tl(h, TAG_MFCC); SR_CK(h, launch_mfcc_h(h, static_cast<const u16 *>(h->pcm.p), U, B, static_cast<const u32 *>(h->seg.p), 6, static_cast<const atap_tag *>(h->atap.p), h->ftr.p)); }
-    SR_CK(h, launch_status(static_cast<const u32 *>(h->seg.p), h->ftr.p, B, static_cast<u8 *>(h->status.p), h->stream));
+    if (const int rc = front_end(h, static_cast<const u16 *>(h->pcm.p), U, B, n_len, static_cast<atap_tag *>(h->atap.p),
+                                 static_cast<u32 *>(h->seg.p), h->ftr.p, static_cast<u8 *>(h->status.p))) return rc;
     SR_CK(h, launch_pack_slots(h->ftr.p, static_cast<const u8 *>(h->status.p), B, h->misc0.p, slot_stride, h->stream));
-    h->launches += 4;
+    ++h->launches;
     D2H(h, bank_out, h->misc0.p, (size_t)B * slot_stride);
     if (status) D2H(h, status, h->status.p, (size_t)B);
     SR_CK(h, cudaStreamSynchronize(h->stream));
@@ -800,9 +633,7 @@ int sr_get_mdl_batch(sr_handle *h, const v_ftr_tag *in1, const v_ftr_tag *in2, u
     H2D(h, h->ftr.p, mdl, bytes);                                   // rejected pairs leave mdl as the caller passed it
     SR_CK(h, launch_get_mdl(h->misc0.p, h->misc1.p, h->ftr.p, n, static_cast<u32 *>(h->bdis.p), h->stream));
     ++h->launches;
-    // like get_mfcc, get_mdl never writes save_sign: copy back bytes [2, 2860) only
-    SR_CK(h, cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(mdl) + 2, kFtrBytes, static_cast<unsigned char *>(h->ftr.p) + 2,
-                               kFtrBytes, kFtrBytes - 2, n, cudaMemcpyDeviceToHost, h->stream));
+    SR_CK(h, ftr_to_host(h, mdl, h->ftr.p, n));
     if (dis) D2H(h, dis, h->bdis.p, (size_t)n * 4);
     SR_CK(h, cudaStreamSynchronize(h->stream));
     return 0;
@@ -818,20 +649,11 @@ int sr_recognise_batch_multi(sr_handle *const *handles, uint32_t n_handles, cons
     if (!handles || n_handles == 0 || !o) return fail(nullptr, "sr_recognise_batch_multi: bad arguments", cudaSuccess);
     for (uint32_t g = 0; g < n_handles; ++g)
         if (!handles[g] || handles[g]->n_slot != handles[0]->n_slot) return fail(nullptr, "sr_recognise_batch_multi: handles differ", cudaSuccess);
-    const size_t T = handles[0]->n_slot;
     std::vector<int> rc(n_handles, 0);
     std::vector<std::thread> th;
     for (uint32_t g = 0; g < n_handles; ++g) {
         const uint32_t lo = (uint32_t)((uint64_t)B * g / n_handles), hi = (uint32_t)((uint64_t)B * (g + 1) / n_handles);
-        sr_recog_out s = *o;
-        if (s.atap) s.atap += lo;
-        if (s.seg_off) s.seg_off += (size_t)lo * 6;
-        if (s.ftr) s.ftr += lo;
-        if (s.score) s.score += (size_t)lo * T;
-        if (s.best_idx) s.best_idx += lo;
-        if (s.best_dis) s.best_dis += lo;
-        if (s.cmd) s.cmd += lo;
-        if (s.status) s.status += lo;
+        const sr_recog_out s = recog_slice(handles[0], *o, lo);
         th.emplace_back([=, &rc]() { rc[g] = sr_recognise_batch(handles[g], pcm + (size_t)lo * U, U, hi - lo, n_len, &s); });
     }
     for (auto &t : th) t.join();

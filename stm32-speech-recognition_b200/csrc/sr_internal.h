@@ -1,6 +1,9 @@
 // sr_internal.h -- private to the library: the handle, workspaces and launch prototypes shared by sr_api.cu
 // and sr_stream.cu. Nothing here is part of the C-ABI.
 #pragma once
+#include <chrono>
+#include <functional>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <stdio.h>
@@ -47,10 +50,67 @@ using namespace srk;
 inline thread_local std::string g_tls_error;
 
 struct sr_comm;                                       // sr_comm.cu: NCCL communicator + its stream
+struct sr_handle;
 
+// grow-only device buffer (ensure), freed with its owner: owners are deleted under a DeviceGuard of their device
 struct DevBuf {
     void *p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+};
+
+// pinned host buffer, freed with its owner
+template <class T> struct Pinned {
+    T *p = nullptr;
+    Pinned() = default;
+    Pinned(const Pinned &) = delete;
+    Pinned &operator=(const Pinned &) = delete;
+    ~Pinned() { reset(); }
+    void reset() { if (p) cudaFreeHost(p); p = nullptr; }
+    cudaError_t alloc(size_t bytes) {
+        reset();
+        const cudaError_t e = cudaMallocHost(reinterpret_cast<void **>(&p), bytes);
+        if (e != cudaSuccess) p = nullptr;
+        return e;
+    }
+};
+
+// The packed PCM transport of sr_recognise_batch (sr_transport.cu). Chunks whose samples are all < 4096 cross PCIe as
+// 12 bits per sample: a worker pool packs them from the back of the batch into pinned staging slots while the caller's
+// thread sends plain u16 chunks from the front. Owns the pool, the pinned and device staging, the automatic mode's
+// measurements and the statistics of the last call.
+class PackedTransport {
+public:
+    // sends chunk c into device PCM buffer buf (0 or 1): from packed_src (12-bit, pinned staging) or, if NULL, plain
+    using Step = std::function<int(uint32_t c, int buf, const void *packed_src)>;
+    int mode = -1;                                      // sr_set_transport: 0 off, 1 on, -1 automatic
+    uint32_t last_packed = 0, last_plain = 0;           // sr_transport_stats: chunks and bytes of the last call
+    uint64_t last_h2d = 0;
+    ~PackedTransport();
+    // every chunk of `chunk` utterances (the last one shorter) of pcm[B][U], once, through step
+    int send(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t chunk, const Step &step);
+    // call after the results of the call are on the host: the automatic mode times the whole call
+    void call_done(uint64_t pcm_bytes);
+    // device staging of buffer buf, where step copies a packed chunk to
+    unsigned char *device_stage(int buf) const { return static_cast<unsigned char *>(dpacked.p) + (size_t)buf * stage_cap; }
+
+private:
+    static constexpr int kStage = 4;
+    uint64_t auto_calls = 0;                            // automatic mode: calls seen, measured ns per PCM byte [plain, packed]
+    double auto_ns_per_byte[2] = {0.0, 0.0};
+    bool probe = false;                                 // the current call is a measurement of the automatic mode
+    std::chrono::steady_clock::time_point t_call0;
+    std::unique_ptr<PackPool> pool;
+    Pinned<uint8_t> stage[kStage];
+    size_t stage_cap = 0;
+    DevBuf dpacked;                                     // 2 x stage_cap
+    int resolved_mode(const sr_handle *h) const;
+    bool auto_pick();
+    bool setup(const sr_handle *h, size_t pk);
+    int send_packed(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t chunk, const Step &step);
 };
 
 struct sr_handle {
@@ -77,17 +137,7 @@ struct sr_handle {
     std::vector<cudaEvent_t> ev;
     std::vector<uint32_t> ev_tag;
     size_t ev_used = 0;
-    // packed PCM transport (sr_recognise_batch): worker pool, pinned staging slots, device staging
-    int transport_mode = -1;                            // 0 off, 1 on, -1 automatic
-    uint64_t auto_calls = 0;                            // automatic mode: calls seen, measured ns per PCM byte [plain, packed]
-    double auto_ns_per_byte[2] = {0.0, 0.0};
-    PackPool *pool = nullptr;
-    static constexpr int kStage = 4;
-    void *stage[kStage] = {nullptr, nullptr, nullptr, nullptr};
-    size_t stage_cap = 0;
-    uint32_t last_packed = 0, last_plain = 0, chunk_seq = 0;
-    uint64_t last_h2d = 0;
-    DevBuf dpacked;
+    PackedTransport transport;                          // of sr_recognise_batch
     // command labels (commstr, main.c:25-31): n_labels records of label_stride bytes, NUL-terminated
     std::vector<uint8_t> labels;
     u32 n_labels = 0, label_stride = 0;

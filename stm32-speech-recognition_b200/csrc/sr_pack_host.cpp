@@ -117,17 +117,10 @@ __attribute__((target("avx512f,avx512bw,avx512vbmi"))) static uint32_t pack12_vb
     return o | pack12_vbmi(src + i, n - i, dst + (i >> 1) * 3);
 }
 
-#ifndef SR_PACK_NT_DEFAULT
-#define SR_PACK_NT_DEFAULT 1
-#endif
 typedef uint32_t (*pack_fn)(const uint16_t *, size_t, uint8_t *);
 static pack_fn pick_pack() {
     __builtin_cpu_init();
-    // SR_PACK_NT=0: ordinary stores -- the packed bytes stay in the last-level cache, where the GPU's PCIe reads find them
-    // (inbound reads are coherent) without a trip to DRAM and back; SR_PACK_NT=1: non-temporal stores (no read-for-ownership)
-    const char *e = getenv("SR_PACK_NT");
-    const bool nt = e && *e ? atoi(e) != 0 : SR_PACK_NT_DEFAULT;
-    if (__builtin_cpu_supports("avx512vbmi") && __builtin_cpu_supports("avx512bw")) return nt ? pack12_vbmi_nt : pack12_vbmi;
+    if (__builtin_cpu_supports("avx512vbmi") && __builtin_cpu_supports("avx512bw")) return pack12_vbmi_nt;
     if (__builtin_cpu_supports("avx2")) return pack12_avx2;
     return pack12_scalar;
 }

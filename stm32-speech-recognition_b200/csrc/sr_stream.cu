@@ -196,8 +196,8 @@ struct sr_stream_pool {
     sr_handle *h = nullptr;
     u32 S = 0, L = 0, n_len = 0, cap = 0, info_stride = 0, stage_stride = 0;
     DevBuf pcm, state, info, stage, lens, ev, seg_ev, atap_ev, map_ev, n_ev, ftr, status, frm, out;
-    unsigned char *out_host = nullptr;             // pinned: [count u32, pad][records]
-    u32 *lens_host = nullptr;                      // pinned staging of a ragged push's lengths
+    Pinned<unsigned char> out_host;                // [count u32, pad][records]
+    Pinned<u32> lens_host;                         // staging of a ragged push's lengths
     std::deque<sr_stream_event> pending;           // events not yet handed to the caller (max_events too small)
     static constexpr u32 kQuick = 4096;            // records fetched with the count in the first D2H copy
 };
@@ -211,12 +211,7 @@ int sr_streams_destroy(sr_stream_pool *p) {
     if (!p) return 0;
     DeviceGuard g(p->h->device);
     cudaStreamSynchronize(p->h->stream);
-    DevBuf *bufs[] = {&p->pcm, &p->state, &p->info, &p->stage, &p->lens, &p->ev, &p->seg_ev, &p->atap_ev, &p->map_ev,
-                      &p->n_ev, &p->ftr, &p->status, &p->frm, &p->out};
-    for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
-    if (p->out_host) cudaFreeHost(p->out_host);
-    if (p->lens_host) cudaFreeHost(p->lens_host);
-    delete p;
+    delete p;                                      // frees its buffers, under g
     return 0;
 }
 
@@ -255,8 +250,8 @@ int sr_streams_create(sr_handle *h, uint32_t n_streams, uint32_t max_samples, ui
     need(p->status, cap);
     need(p->frm, cap * 4);
     need(p->out, 16 + cap * sizeof(sr_stream_event));
-    if (e == cudaSuccess) e = cudaMallocHost(&p->out_host, 16 + cap * sizeof(sr_stream_event));
-    if (e == cudaSuccess) e = cudaMallocHost(&p->lens_host, (size_t)n_streams * 4);
+    if (e == cudaSuccess) e = p->out_host.alloc(16 + cap * sizeof(sr_stream_event));
+    if (e == cudaSuccess) e = p->lens_host.alloc((size_t)n_streams * 4);
     if (e != cudaSuccess) { sr_streams_destroy(p); return fail(h, "sr_streams_create: allocation", e); }
     *out = p;
     return sr_streams_reset(p);
@@ -313,7 +308,7 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     u32 max_len = uniform_len;
     if (lens) {
         max_len = 0;
-        for (u32 s = 0; s < p->S; ++s) { p->lens_host[s] = lens[s]; if (lens[s] > max_len) max_len = lens[s]; }
+        for (u32 s = 0; s < p->S; ++s) { p->lens_host.p[s] = lens[s]; if (lens[s] > max_len) max_len = lens[s]; }
     }
     SR_REQUIRE(h, max_len == 0 || chunk != nullptr);
     SR_REQUIRE(h, max_len <= p->L && chunk_stride >= max_len);
@@ -341,7 +336,7 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
             SR_CK(h, cudaMemcpy2DAsync(p->stage.p, (size_t)sstride * 2, chunk, (size_t)chunk_stride * 2, (size_t)max_len * 2, p->S,
                                        cudaMemcpyHostToDevice, h->stream));
         }
-        if (lens) SR_CK(h, cudaMemcpyAsync(p->lens.p, p->lens_host, (size_t)p->S * 4, cudaMemcpyHostToDevice, h->stream));
+        if (lens) SR_CK(h, cudaMemcpyAsync(p->lens.p, p->lens_host.p, (size_t)p->S * 4, cudaMemcpyHostToDevice, h->stream));
     }
     SR_CK(h, cudaMemsetAsync(p->n_ev.p, 0, 4, h->stream));
     u32 *n_ev = static_cast<u32 *>(p->n_ev.p);
@@ -370,15 +365,15 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     SR_CK(h, cudaGetLastError());
     h->launches += 4 + (h->n_slot ? 1 : 0);
     const u32 quick = p->cap < sr_stream_pool::kQuick ? p->cap : sr_stream_pool::kQuick;
-    D2H(h, p->out_host, p->out.p, 16 + (size_t)quick * sizeof(sr_stream_event));
+    D2H(h, p->out_host.p, p->out.p, 16 + (size_t)quick * sizeof(sr_stream_event));
     SR_CK(h, cudaStreamSynchronize(h->stream));                       // the one synchronisation of a push
-    const u32 ne = *reinterpret_cast<const u32 *>(p->out_host);
+    const u32 ne = *reinterpret_cast<const u32 *>(p->out_host.p);
     if (ne > quick) {                                                 // rare: a burst of closings larger than the quick window
-        D2H(h, p->out_host + 16 + (size_t)quick * sizeof(sr_stream_event), static_cast<unsigned char *>(p->out.p) + 16 + (size_t)quick * sizeof(sr_stream_event),
+        D2H(h, p->out_host.p + 16 + (size_t)quick * sizeof(sr_stream_event), static_cast<unsigned char *>(p->out.p) + 16 + (size_t)quick * sizeof(sr_stream_event),
             (size_t)(ne - quick) * sizeof(sr_stream_event));
         SR_CK(h, cudaStreamSynchronize(h->stream));
     }
-    const sr_stream_event *rec = reinterpret_cast<const sr_stream_event *>(p->out_host + 16);
+    const sr_stream_event *rec = reinterpret_cast<const sr_stream_event *>(p->out_host.p + 16);
     u32 k = 0;
     // older queued events first, then this push's; whatever does not fit stays queued for sr_streams_fetch
     while (k < max_events && events && !p->pending.empty()) { events[k++] = p->pending.front(); p->pending.pop_front(); }

@@ -25,9 +25,23 @@ FTR_DTYPE = np.dtype([("save_sign", "<u2"), ("frm_num", "<u2"), ("mfcc_dat", "<i
 assert ATAP_DTYPE.itemsize == 12 and FTR_DTYPE.itemsize == FTR_BYTES
 
 
+RECOG_FIELDS = ("atap", "seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status")
+
+
 class RecogOut(C.Structure):
-    _fields_ = [("atap", C.c_void_p), ("seg_off", C.c_void_p), ("ftr", C.c_void_p), ("score", C.c_void_p),
-                ("best_idx", C.c_void_p), ("best_dis", C.c_void_p), ("cmd", C.c_void_p), ("status", C.c_void_p)]
+    _fields_ = [(k, C.c_void_p) for k in RECOG_FIELDS]
+
+
+def _recog_out(ptrs):
+    """sr_recog_out of the fields in `ptrs` (numpy arrays or device pointers); the others are NULL"""
+    return RecogOut(*[_p(ptrs.get(k)) for k in RECOG_FIELDS])
+
+
+def _recog_arrays(B, T, want):
+    """zeroed host arrays for the fields of sr_recog_out named in `want`, for B utterances and T templates"""
+    shape = {"atap": (B, ATAP_DTYPE), "seg_off": ((B, 3, 2), np.uint32), "ftr": (B, FTR_DTYPE), "score": ((B, T), np.uint32),
+             "best_idx": (B, np.uint32), "best_dis": (B, np.uint32), "cmd": (B, np.uint32), "status": (B, np.uint8)}
+    return {k: np.zeros(*shape[k]) for k in RECOG_FIELDS if k in want}
 
 
 class StreamEvent(C.Structure):
@@ -261,25 +275,10 @@ class Handle:
         self._ck(lib().sr_dtw_batch(self._h, _p(ftr_in), B, flags, band_r, _p(score), _p(bi), _p(bd)))
         return score, bi, bd
 
-    def recognise(self, pcm, n_len=2400, want=("atap", "seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status")):
+    def recognise(self, pcm, n_len=2400, want=RECOG_FIELDS):
         B, U = pcm.shape
-        out = {}
-        if "atap" in want:
-            out["atap"] = np.zeros(B, ATAP_DTYPE)
-        if "seg_off" in want:
-            out["seg_off"] = np.zeros((B, 3, 2), np.uint32)
-        if "ftr" in want:
-            out["ftr"] = np.zeros(B, FTR_DTYPE)
-        if "score" in want:
-            out["score"] = np.zeros((B, self.n_slot), np.uint32)
-        for k in ("best_idx", "best_dis", "cmd"):
-            if k in want:
-                out[k] = np.zeros(B, np.uint32)
-        if "status" in want:
-            out["status"] = np.zeros(B, np.uint8)
-        ro = RecogOut(*[(_p(out[k]) if k in out else None) for k in
-                        ("atap", "seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status")])
-        self._ck(lib().sr_recognise_batch(self._h, _p(pcm), U, B, n_len, C.byref(ro)))
+        out = _recog_arrays(B, self.n_slot, want)
+        self._ck(lib().sr_recognise_batch(self._h, _p(pcm), U, B, n_len, C.byref(_recog_out(out))))
         return out
 
     def enrol(self, pcm, n_len=2400, slot_stride=4096):
@@ -340,9 +339,7 @@ class Handle:
         self._ck(lib().sr_allgather_dev(self._h, _p(send_ptr), _p(recv_ptr), nbytes))
 
     def recognise_dev_allgather(self, pcm_ptr, U, B, n_len, gathered_score=None, gathered_best=None, **ptrs):
-        ro = RecogOut(*[_p(ptrs.get(k)) for k in
-                        ("atap", "seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status")])
-        self._ck(lib().sr_recognise_batch_dev_allgather(self._h, _p(pcm_ptr), U, B, n_len, C.byref(ro),
+        self._ck(lib().sr_recognise_batch_dev_allgather(self._h, _p(pcm_ptr), U, B, n_len, C.byref(_recog_out(ptrs)),
                                                          _p(gathered_score), _p(gathered_best)))
 
     def set_dtw_variant(self, v):
@@ -363,9 +360,7 @@ class Handle:
         self._ck(lib().sr_set_labels(self._h, raw, len(labels), stride))
 
     def recognise_dev(self, pcm_ptr, U, B, n_len, **ptrs):
-        ro = RecogOut(*[_p(ptrs.get(k)) for k in
-                        ("atap", "seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status")])
-        self._ck(lib().sr_recognise_batch_dev(self._h, _p(pcm_ptr), U, B, n_len, C.byref(ro)))
+        self._ck(lib().sr_recognise_batch_dev(self._h, _p(pcm_ptr), U, B, n_len, C.byref(_recog_out(ptrs))))
 
 
 def comm_unique_id():
@@ -380,23 +375,9 @@ def comm_unique_id():
 def recognise_multi(handles, pcm, n_len=2400, want=("best_idx", "best_dis", "cmd", "status", "score", "seg_off")):
     """sr_recognise_batch_multi: one host call over several handles (one per GPU); numpy in/out"""
     B, U = pcm.shape
-    T = handles[0].n_slot
-    out = {}
-    if "seg_off" in want:
-        out["seg_off"] = np.zeros((B, 3, 2), np.uint32)
-    if "ftr" in want:
-        out["ftr"] = np.zeros(B, FTR_DTYPE)
-    if "score" in want:
-        out["score"] = np.zeros((B, T), np.uint32)
-    for k in ("best_idx", "best_dis", "cmd"):
-        if k in want:
-            out[k] = np.zeros(B, np.uint32)
-    if "status" in want:
-        out["status"] = np.zeros(B, np.uint8)
-    ro = RecogOut(*[(_p(out[k]) if k in out else None) for k in
-                    ("atap", "seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status")])
+    out = _recog_arrays(B, handles[0].n_slot, want)
     arr = (C.c_void_p * len(handles))(*[h._h for h in handles])
-    rc = lib().sr_recognise_batch_multi(arr, len(handles), _p(pcm), U, B, n_len, C.byref(ro))
+    rc = lib().sr_recognise_batch_multi(arr, len(handles), _p(pcm), U, B, n_len, C.byref(_recog_out(out)))
     if rc != 0:
         raise SrError("sr_recognise_batch_multi failed (%d): %s" % (rc, lib().sr_last_error(None).decode()))
     return out
