@@ -147,7 +147,9 @@ int sr_noise_atap_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t 
 int sr_vad_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t buf_len,
                  const atap_tag *atap /* [B] */, uint32_t *seg_off /* [B][3][2] */);
 /* get_mfcc of one segment per utterance: seg[b*seg_stride + 0/1] = start/end sample offsets.
- * Only frm_num and the first frm_num rows of ftr[b] are written (MFCC.C never writes save_sign). */
+ * Only frm_num and the first frm_num rows of ftr[b] are written (MFCC.C never writes save_sign).
+ * A segment that starts at 0 reads x[-1] = atap[b].mid_val (as a 16-bit sample), not the previous utterance's last
+ * sample; every batched entry point does the same (the drop-in get_mfcc reads the caller's start[-1]). */
 int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *seg,
                   uint32_t seg_stride, const atap_tag *atap /* [B] */, v_ftr_tag *ftr /* [B] */);
 /* dtw of every input against every bank slot. flags bit0: honour save_sign like spch_recg

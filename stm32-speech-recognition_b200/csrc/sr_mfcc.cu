@@ -58,7 +58,8 @@ struct __align__(16) MfccSmem {
     u32 lg[kConsumerWarps][32];
     u64 full[kNBuf];
     u64 empty[kNBuf];
-    s32 meta[kNBuf][4];                      // {F (-1 = no more utterances), sample index of x[start-1] in the buffer, mid, utterance b}
+    s32 meta[kNBuf][5];                      // {F (-1 = no more utterances), sample index of x[start-1] in the buffer, mid, utterance b,
+                                             //  x[start-1] pinned to mid (start == 0)}
     int turn;                                // dynamic hand-out: number of the CTA's next claim (claims are made in ring order)
 };
 
@@ -67,6 +68,11 @@ static_assert(sizeof(MfccSmem<15, 3>) <= 232448, "w15 variant exceeds the 227 KB
 
 // Stage utterance number `it` of this CTA's walk (batch row b) into ring slot it % kNBuf: one warp, lane 0 issues
 // the bulk copy. Bytes [lo,hi) of the batch = samples start-1 .. start+80(F-1)+159 of the utterance.
+// x[-1] of a segment that starts at sample 0 (MFCC.C:119, i = 0) is not a sample of the utterance: it is the last
+// sample of the previous row, or lies before the batch. Every batched entry point pins it to the utterance's own mid
+// (its pre-emphasis term is then 0), so an utterance's features do not depend on its row, its chunk, its shard or
+// another stream. The slot only flags it (meta[s][4]); the warp that takes frame 0 writes mid over x[0] once the slot
+// is full. A store here could be overwritten by the bulk copy, which spans x[-1] when sample 0 is not 16-byte aligned.
 template <int kConsumerWarps, int kNBuf, bool kRelaxedWait>
 __device__ __forceinline__ void stage_utterance(MfccSmem<kConsumerWarps, kNBuf> &sm, int it, u32 b, const u16 *__restrict__ pcm,
                                                 u32 U, const u32 *__restrict__ seg, u32 seg_stride,
@@ -84,16 +90,19 @@ __device__ __forceinline__ void stage_utterance(MfccSmem<kConsumerWarps, kNBuf> 
     const int F = mfcc_frames<SR_FRAME_LEN>(st, en, U);
     if (lane == 0) *reinterpret_cast<u16 *>(ftr + (size_t)b * kFtrBytes + 2) = (u16)F;   // MFCC.C:106,189
     if (F == 0) {
-        if (lane == 0) { sm.meta[s][0] = 0; sm.meta[s][1] = 0; sm.meta[s][2] = (s32)mid; sm.meta[s][3] = (s32)b; mbar_arrive(&sm.full[s]); }
+        if (lane == 0) {
+            sm.meta[s][0] = 0; sm.meta[s][1] = 0; sm.meta[s][2] = (s32)mid; sm.meta[s][3] = (s32)b; sm.meta[s][4] = 0;
+            mbar_arrive(&sm.full[s]);
+        }
         return;
     }
-    long long first = row * U + st - 1;                    // may be -1 for row 0, start 0
+    if (lane == 0) sm.meta[s][4] = (st == 0);
+    long long first = row * U + st - 1;                    // -1 for row 0, start 0
     const long long last = row * U + st + 80ll * (F - 1) + 160;   // exclusive
     unsigned char *dst = sm.pcm[s];
     int off = 0;
-    if (first < 0) {                                       // x[-1] of the whole batch: reference reads
-        if (lane == 0) reinterpret_cast<u16 *>(dst)[7] = (u16)mid;   // out of bounds (MFCC.C:119); pinned to mid
-        first = 0; off = 8;                                // sample 0 lands at dst+16 (index 8), x[-1] at index 7
+    if (first < 0) {                                       // x[-1] would lie before the batch: copy from sample 0, which
+        first = 0; off = 8;                                // lands at dst+16 (index 8); x[-1] is index 7, written by a consumer
         dst += 16;
     }
     const size_t lo = (size_t)first * 2, hi = (size_t)last * 2;
@@ -263,8 +272,11 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
         const u32 b = (u32)sm.meta[s][3];
         const int off = sm.meta[s][1];
         const s32 mid = sm.meta[s][2];
-        const u16 *x = reinterpret_cast<const u16 *>(sm.pcm[s]) + off;   // x[0] = sample start-1
+        u16 *x = reinterpret_cast<u16 *>(sm.pcm[s]) + off;               // x[0] = sample start-1
         unsigned char *out_rows = ftr + (size_t)b * kFtrBytes + 4;
+        const int f0 = (int)((warp - (int)(gidx % kConsumerWarps) + kConsumerWarps) % kConsumerWarps);   // this warp's first frame
+        // start == 0: x[-1] := mid (see stage_utterance). Only frame 0 reads x[0], and only its lane 0.
+        if (f0 == 0 && lane == 0 && sm.meta[s][4]) x[0] = (u16)mid;
 
         // pre-emphasis + Hamming, MFCC.C:115-124, of the frame at xf (xf[i] = vc_dat[i-1]); keeps w>>2 (stage-0 output) in wq
         auto preemph = [&](const u16 *xf) {
@@ -275,8 +287,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
                 wq[i] = preemph_hamm(xf[i + 1], xf[i], (u32)mid, hm[k]) >> 2;   // BUTFLY4ZERO_OPT with B=C=D=0
             }
         };
-        for (int f = (int)((warp - (int)(gidx % kConsumerWarps) + kConsumerWarps) % kConsumerWarps); f < F;
-             f += kConsumerWarps) {
+        for (int f = f0; f < F; f += kConsumerWarps) {
             const u16 *xf = x + 80 * f;                                  // xf[i] = vc_dat[i-1]
             preemph(xf);
             __syncwarp();

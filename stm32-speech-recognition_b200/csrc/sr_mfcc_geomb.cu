@@ -43,8 +43,10 @@ mfcc_geomb_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
         const size_t row = row_map ? row_map[b] : b;
         const int F = mfcc_frames<kGbFrame>(st, en, U);
         if (threadIdx.x == 0) *reinterpret_cast<u16 *>(ftr + (size_t)b * kFtrBytes + 2) = (u16)F;
-        const u16 *xs = pcm + row * U + st;                        // xs[-1] is read (MFCC.C:119); pinned to mid at the very start
-        const bool at_origin = (row == 0 && st == 0);
+        // xs[-1] is read (MFCC.C:119). For start == 0 it is not a sample of the utterance (the previous row's last sample,
+        // or before the batch): pinned to mid, as in the reference geometry's kernel (sr_mfcc.cu, stage_utterance)
+        const u16 *xs = pcm + row * U + st;
+        const bool at_origin = (st == 0);
         unsigned char *out_rows = ftr + (size_t)b * kFtrBytes + 4;
         for (int f = warp; f < F; f += kGbWarps) {
             const u16 *xf = xs + 80 * f;

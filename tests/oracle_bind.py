@@ -213,6 +213,64 @@ class RefOracle(_Base):
         return out
 
 
+def pinned_rows(pcm, atap):
+    """rows of U + 1 samples, [mid_val, row...]: with every segment shifted by +1, x[-1] of a segment that starts at
+    sample 0 is the utterance's own mid_val (as a 16-bit sample), and every other segment reads its own samples"""
+    B, U = pcm.shape
+    rows = np.empty((B, U + 1), np.uint16)
+    rows[:, 0] = atap["mid_val"].astype(np.uint16)
+    rows[:, 1:] = pcm
+    return rows
+
+
+def plant_sample0(pcm, rows, seed, before=4095):
+    """make VAD open segment 0 of each of `rows` at sample 0 (in place): someone is already speaking when the capture
+    starts. The first 560..1400 samples alternate between m +- 1200 (+- 150 of noise), m = the level of the quiet that
+    follows. The burst lies inside the 2 400-sample noise window, whose n_thl is the MEAN of the per-240-sample maxima
+    (VAD.C:60-68): at most 6 of its 10 windows are loud, so n_thl stays below 900 and every sample of the burst crosses
+    the band (frm_zero > z_thl); frames 0-7 are active and the segment is back-dated to sample 0 (VAD.C:178). The quiet
+    after the burst closes it: 8..18 frames. The last sample of the row before each planted row is set to `before`, far
+    from m, so x[-1] read from the neighbour would change the features."""
+    rng = np.random.default_rng(seed)
+    for r in rows:
+        n = int(rng.integers(640, 1400))
+        m = int(round(float(pcm[r, 1400:2400].mean())))
+        burst = m + np.where(np.arange(n) % 2 == 0, 1200, -1200) + rng.integers(-150, 151, n)
+        pcm[r, :n] = np.clip(burst, 0, 4095)
+        if r > 0:
+            pcm[r - 1, -1] = before
+
+
+def recognise_pinned(ora, pcm, n_len, bank, n_slot, slot_stride, geom_b=False):
+    """recognise_batch composed from the oracle's own stages, one utterance at a time, with x[-1] of a segment that starts
+    at sample 0 pinned to that utterance's mid_val (the rule of every batched entry point): noise_atap and VAD on the row,
+    get_mfcc of segment 0 on pinned_rows, dtw with the save_sign check, the strict '<' first-wins argmin (main.c:276-294).
+    geom_b: the GEOM_B get_mfcc (the port's restatement only). Same dict as recognise_batch."""
+    B, U = pcm.shape
+    out = dict(atap=np.zeros(B, ATAP_DTYPE), seg_off=np.zeros((B, 3, 2), np.uint32), ftr=np.zeros(B, FTR_DTYPE),
+               score=np.full((B, n_slot), NULL, np.uint32), best_idx=np.zeros(B, np.uint32),
+               best_dis=np.full(B, NULL, np.uint32), cmd=np.zeros(B, np.uint32), status=np.ones(B, np.uint8))
+    for b in range(B):
+        out["atap"][b] = ora.noise_atap(pcm[b], n_len)[0]
+        out["seg_off"][b] = ora.vad(pcm[b], U, out["atap"][b:b + 1]).reshape(3, 2)
+    ok = out["seg_off"][:, 0, 1] != NULL                      # main.c:261-266: VAD found no segment -> status 1
+    if ok.any():
+        rows = pinned_rows(pcm[ok], out["atap"][ok])
+        seg = out["seg_off"][ok, 0, :] + 1
+        f = ora.mfcc_geom_b_batch(rows, seg, out["atap"][ok]) if geom_b else ora.mfcc_batch(rows, seg, out["atap"][ok])
+        out["ftr"][ok] = f
+    out["status"][ok] = np.where(out["ftr"]["frm_num"][ok] == 0, 2, 0)   # main.c:269-274
+    good = out["status"] == 0
+    if good.any() and n_slot:
+        sc, _ = ora.dtw_batch(out["ftr"][good], bank, n_slot, slot_stride, check_sign=1)
+        out["score"][good] = sc
+        i = np.argmin(sc, axis=1)                             # first of the minima == the strict '<' scan from DIS_ERR
+        out["best_idx"][good] = i
+        out["best_dis"][good] = sc[np.arange(sc.shape[0]), i]
+        out["cmd"][good] = i // 4
+    return out
+
+
 def have_ref():
     return os.path.exists(REF_SO)
 

@@ -185,21 +185,49 @@ def test_mfcc_batch_sizes_around_the_cta_count(handle, ora, B, mix):
         assert (handle.mfcc(pcm, nulls, atap)["frm_num"] == 0).all()
 
 
-def test_mfcc_segment_at_sample_zero_reads_previous_utterance(handle, ora):
-    """start == 0 makes MFCC.C:119 read vc_dat[-1]; for b > 0 that is the last sample of utterance b-1 in a
-    contiguous batch (same as the reference on the same memory); for b == 0 it is pinned to mid_val."""
-    B, U = 5, 4000
+def test_mfcc_segment_at_sample_zero_pins_mid_val(handle, ora):
+    """start == 0 makes MFCC.C:119 read vc_dat[-1], which is not a sample of the utterance (the last sample of row b-1,
+    or before the batch). The batched forms pin it to the utterance's own mid_val in every row: the features equal the
+    oracle on [mid_val, row...]. The rows before are made to end far from mid (0 / 4095), and the start-0 segments sit at
+    every 16-byte phase of the bulk copy (U = 4003) and, through device pointers 2, 6 and 14 bytes past a 16-byte
+    boundary, in the cooperative copy. Segments that start at 1 read their own sample 0."""
+    for U in (4000, 4003):
+        _check_sample_zero_pins_mid_val(handle, ora, U)
+
+
+def _check_sample_zero_pins_mid_val(handle, ora, U):
+    import torch
+    B = 11
     pcm = sr_b200.synth_pcm_host(B, U, 0x99)
+    pcm[:, -1] = np.where(np.arange(B) % 2 == 0, 0, 4095)
     seg = np.tile(np.array([0, 1600], np.uint32), (B, 1))
+    seg[3] = (0, U)
+    seg[5] = (1, 1601)
+    seg[6] = (0, 159)                                  # less than a frame
+    seg[8] = (0, 160)                                  # exactly one frame
     atap = np.zeros(B, sr_b200.ATAP_DTYPE)
     atap["mid_val"] = 2100
-    got = handle.mfcc(pcm, seg, atap)
-    # oracle on a buffer with one leading sample = mid_val: utterance 0 then sees x[-1] = mid
-    flat = np.concatenate([[np.uint16(2100)], pcm.reshape(-1)])
-    for b in range(B):
-        view = flat[b * U: b * U + 1 + U].copy().reshape(1, -1)
-        want = ora.mfcc_batch(view, np.array([[1, 1601]], np.uint32), atap[b:b + 1])
-        assert ob.ftr_equal(got[b:b + 1], want), b
+    atap["mid_val"][4] = 300
+    want = ora.mfcc_batch(ob.pinned_rows(pcm, atap), seg + 1, atap)
+    assert want["frm_num"][6] == 0 and want["frm_num"][8] == 1 and want["frm_num"][3] == (U - 160) // 80 + 1
+    assert ob.ftr_equal(handle.mfcc(pcm, seg, atap), want), U
+    dev = torch.device("cuda:0")
+    h = sr_b200.Handle(0)
+    st = torch.cuda.Stream(dev)
+    h.set_stream(st.cuda_stream)
+    with torch.cuda.stream(st):
+        buf = torch.zeros(B * U + 16, dtype=torch.int16, device=dev)
+        seg_d, atm_d = _to_dev(seg), _to_dev(atap)
+        for k in (0, 1, 3, 7):                         # 0: aligned base (bulk copy); else 2k bytes past a boundary
+            buf.fill_(4095)
+            buf[k:k + B * U] = torch.from_numpy(pcm.view(np.int16).reshape(-1)).to(dev)
+            ptr = buf.data_ptr() + 2 * k
+            assert (ptr % 16 == 0) == (k == 0)
+            ft = torch.full((B * sr_b200.FTR_BYTES,), 0x5A, dtype=torch.uint8, device=dev)
+            h.mfcc_dev(ptr, U, B, seg_d.data_ptr(), 2, atm_d.data_ptr(), ft.data_ptr())
+            st.synchronize()
+            assert ob.ftr_equal(ft.cpu().numpy().view(sr_b200.FTR_DTYPE), want), (U, k)
+    h.close()
 
 
 def _windowed(x, prv, mid, hamm):
@@ -773,9 +801,12 @@ def test_reference_named_entry_points(handle, ora):
 def test_large_batch_shard_invariance_and_sampled_parity(handle, ora):
     """BASELINE-size run (16 384 x 1 s here to bound host RAM/time): results do not depend on how the batch is
     sharded (what the multi-GPU split relies on), enrolment then recognition of the same audio gives
-    distance 0 against its own template, and a random sample agrees with the oracle bit-for-bit."""
+    distance 0 against its own template, and a random sample agrees with the oracle bit-for-bit. Utterances whose
+    segment starts at sample 0 sit on both sides of the chunk boundaries and of the cut."""
     B, U, T = 16384, 8000, 20
     pcm = sr_b200.synth_pcm_host(B, U, 0x5EED0000)
+    planted = [2095, 2096, 4191, 4192, 4999, 5000]      # the host call's 32 MB chunks are 2 096 utterances; cut below
+    ob.plant_sample0(pcm, planted, 0x5EED)
     handle.set_bank(np.zeros((1, 4096), np.uint8), 0, 4096)
     enrol = handle.recognise(pcm[:T], 2400, want=("ftr", "status"))
     assert (enrol["status"] == 0).all()
@@ -789,10 +820,264 @@ def test_large_batch_shard_invariance_and_sampled_parity(handle, ora):
     for k in ("seg_off", "score", "best_idx", "best_dis", "cmd", "status"):
         assert np.array_equal(full[k], np.concatenate([a[k], b[k]])), k
     assert ob.ftr_equal(full["ftr"], np.concatenate([a["ftr"], b["ftr"]]))
-    idx = np.random.default_rng(0).choice(B, 192, replace=False)
-    ref = ora.recognise_batch(np.ascontiguousarray(pcm[idx]), 2400, bank, T, 4096)
+    idx = np.union1d(np.random.default_rng(0).choice(B, 192, replace=False), planted)
+    ref = ob.recognise_pinned(ora, np.ascontiguousarray(pcm[idx]), 2400, bank, T, 4096)
+    assert (ref["seg_off"][np.isin(idx, planted), 0, 0] == 0).all()
     _cmp_recog({k: v[idx] for k, v in full.items()}, ref)
     assert (full["status"] == 0).mean() > 0.99
+
+
+# ---- x[-1] of a segment at sample 0: one rule for every batched path --------------------------------------
+# VAD opens a segment at sample 0 when someone already speaks as the capture starts; get_mfcc then reads x[-1]
+# (MFCC.C:119). Every batched entry point pins it to the utterance's own mid_val, so no result may depend on where
+# the utterance sits: its row, the host call's chunks, a slice, the handles a batch is sharded over, another stream.
+# Inputs: ob.plant_sample0 (reach and sensitivity are asserted in test_oracle.py); reference: ob.recognise_pinned.
+def _sample0_bank(ora, T, geom_b=False):
+    """T templates in flash layout, three of them short utterances whose segment starts at sample 0 (so planted
+    utterances of 8..18 frames pass the 2:1 guard of DTW.C:133 against some templates)"""
+    tpl = sr_b200.synth_pcm_host(T, 8000, 0x7E3A0000)
+    ob.plant_sample0(tpl, [1, 4, 7], 0x7E3A)
+    e = ob.recognise_pinned(ob.port() if geom_b else ora, tpl, 2400, None, 0, 4096, geom_b=geom_b)
+    assert (e["status"] == 0).all()
+    return sr_b200.make_bank(e["ftr"])
+
+
+def _same_recog(got, want, rows=None, what=""):
+    """every field both dicts hold, bit for bit (features: the frm_num rows get_mfcc defines); `rows` selects the
+    rows of `want` that `got` holds"""
+    keys = [k for k in sr_b200.RECOG_FIELDS if k in got and k in want]
+    assert {"seg_off", "ftr", "score", "best_idx", "best_dis", "cmd", "status"} <= set(keys), keys
+    for k in keys:
+        g, w = got[k], (want[k] if rows is None else want[k][rows])
+        assert g.shape == w.shape, (what, k, g.shape, w.shape)
+        if k == "ftr":
+            bad = [i for i in range(len(g)) if not ob.ftr_equal(g[i:i + 1], w[i:i + 1])]
+        elif k == "atap":
+            bad = _first_bad_rows(g.view(np.uint8).reshape(len(g), -1), w.view(np.uint8).reshape(len(w), -1))
+        else:
+            bad = _first_bad_rows(g, w)
+        assert not bad, (what, k, bad[:8])
+
+
+def _recognise_dev_np(h, pcm, n_len, T):
+    """one sr_recognise_batch_dev launch on the whole batch; every output field, as the host call returns it"""
+    import torch
+    dev = torch.device("cuda:0")
+    B, U = pcm.shape
+    st = torch.cuda.Stream(dev)
+    h.set_stream(st.cuda_stream)
+    with torch.cuda.stream(st):
+        pcm_d = torch.from_numpy(pcm.view(np.int16)).to(dev)
+        out = {"atap": torch.full((B * 12,), 0xA5, dtype=torch.uint8, device=dev),
+               "seg_off": torch.full((B * 6,), 0x5A5A5A5A, dtype=torch.int32, device=dev),
+               "ftr": torch.full((B * sr_b200.FTR_BYTES,), 0x5A, dtype=torch.uint8, device=dev),
+               "score": torch.full((B * max(T, 1),), 0x5A5A5A5A, dtype=torch.int32, device=dev),
+               "status": torch.full((B,), 0x5A, dtype=torch.uint8, device=dev)}
+        for key in ("best_idx", "best_dis", "cmd"):
+            out[key] = torch.full((B,), 0x5A5A5A5A, dtype=torch.int32, device=dev)
+        h.recognise_dev(pcm_d.data_ptr(), U, B, n_len, **{key: v.data_ptr() for key, v in out.items()})
+    st.synchronize()
+    got = {key: v.cpu().numpy() for key, v in out.items()}
+    got["atap"] = got["atap"].view(sr_b200.ATAP_DTYPE)
+    got["ftr"] = got["ftr"].view(sr_b200.FTR_DTYPE)
+    got["seg_off"] = got["seg_off"].view(np.uint32).reshape(B, 3, 2)
+    got["score"] = got["score"].view(np.uint32).reshape(B, -1)[:, :T]
+    for key in ("best_idx", "best_dis", "cmd"):
+        got[key] = got[key].view(np.uint32)
+    return got
+
+
+def _planted_and_pinned(ora, pcm, rows, seed, bank, T):
+    ob.plant_sample0(pcm, rows, seed)
+    want = ob.recognise_pinned(ora, pcm, 2400, bank, T, 4096)
+    planted = np.isin(np.arange(pcm.shape[0]), rows)
+    assert ((want["seg_off"][:, 0, 0] == 0) == planted).all() and (want["status"][rows] == 0).all()
+    return want
+
+
+def test_mfcc_sample0_host_chunks_plain_packed_and_one_device_launch_agree(ora):
+    """sr_recognise_batch runs a 32 MB chunk per launch: 256 utterances at U = 65 535, so 600 utterances are three
+    chunks. Start-0 utterances at the first and last row of every chunk and a few others: the plain and the packed
+    transport and one sr_recognise_batch_dev launch over the whole batch all equal recognise_pinned, every field"""
+    B, U, T = 600, 65535, 9
+    rng = np.random.default_rng(0x5A1)
+    rows = sorted({0, 1, 2, 255, 256, 257, 511, 512, 513, 598, 599} | set(rng.choice(np.arange(3, 598), 5, replace=False).tolist()))
+    pcm = sr_b200.synth_pcm_host(B, U, 0x5A100000)
+    bank = _sample0_bank(ora, T)
+    want = _planted_and_pinned(ora, pcm, rows, 0x5A1, bank, T)
+    h = sr_b200.Handle(0)
+    h.set_bank(bank, T, 4096)
+    try:
+        h.set_transport(0)
+        plain = h.recognise(pcm, 2400)
+        assert h.transport_stats()[:2] == (0, 3)
+        h.set_transport(1)
+        packed = h.recognise(pcm, 2400)
+        assert sum(h.transport_stats()[:2]) == 3
+    finally:
+        h.set_transport(-1)
+    hd = sr_b200.Handle(0)
+    hd.set_bank(bank, T, 4096)
+    one = _recognise_dev_np(hd, pcm, 2400, T)
+    _same_recog(plain, one, what="plain vs one launch")
+    _same_recog(packed, plain, what="packed vs plain")
+    _same_recog(one, want, what="one launch vs recognise_pinned")
+    assert (want["best_dis"][rows] != ob.NULL).any()
+    h.close()
+    hd.close()
+
+
+def test_mfcc_sample0_slices_and_single_utterances_equal_the_full_batch(handle, ora):
+    """recognise(pcm[i:j]) with cuts at and next to start-0 utterances, and each of them as a batch of 1, equal the
+    rows of the full batch, which equals recognise_pinned"""
+    B, U, T = 64, 8000, 9
+    rows = [0, 1, 2, 7, 8, 31, 32, 33, 62, 63]
+    pcm = sr_b200.synth_pcm_host(B, U, 0x5A200000)
+    bank = _sample0_bank(ora, T)
+    want = _planted_and_pinned(ora, pcm, rows, 0x5A2, bank, T)
+    handle.set_bank(bank, T, 4096)
+    full = handle.recognise(pcm, 2400)
+    for i, j in ((1, 64), (2, 40), (7, 33), (8, 32), (9, 31), (31, 63), (32, 64), (33, 60)):
+        _same_recog(handle.recognise(pcm[i:j], 2400), full, rows=slice(i, j), what=(i, j))
+    for r in rows:
+        _same_recog(handle.recognise(pcm[r:r + 1], 2400), full, rows=slice(r, r + 1), what=r)
+    _same_recog(full, want, what="full vs recognise_pinned")
+
+
+def test_mfcc_sample0_multi_handle_shards_equal_one_handle(ora):
+    """sr_recognise_batch_multi over 2 and 3 handles (one GPU each when there are enough, else on GPU 0): shards start
+    at B*g/n = 200, 300, 400, each of which, and the rows around it, holds a start-0 utterance"""
+    import torch
+    ng = max(1, torch.cuda.device_count())
+    B, U, T = 600, 8000, 9
+    rows = [0, 1, 199, 200, 201, 299, 300, 301, 399, 400, 401, 598, 599]
+    pcm = sr_b200.synth_pcm_host(B, U, 0x5A300000)
+    bank = _sample0_bank(ora, T)
+    want = _planted_and_pinned(ora, pcm, rows, 0x5A3, bank, T)
+    h0 = sr_b200.Handle(0)
+    h0.set_bank(bank, T, 4096)
+    single = h0.recognise(pcm, 2400)
+    for n in (2, 3):
+        hs = [sr_b200.Handle(g % ng) for g in range(n)]
+        for h in hs:
+            h.set_bank(bank, T, 4096)
+        multi = sr_b200.recognise_multi(hs, pcm, 2400, want=sr_b200.RECOG_FIELDS)
+        _same_recog(multi, single, what=n)
+        for h in hs:
+            h.close()
+    _same_recog(single, want, what="single vs recognise_pinned")
+    h0.close()
+
+
+def test_mfcc_sample0_enrol_whole_batch_equals_one_at_a_time(handle, ora):
+    """sr_enrol_batch (pack_slots_kernel writes the flash slots): the whole batch gives the same slots and status as one
+    utterance at a time, and the slots of recognise_pinned's features"""
+    B, U = 40, 8000
+    rows = [0, 1, 2, 5, 6, 20, 38, 39]
+    pcm = sr_b200.synth_pcm_host(B, U, 0x5A400000)
+    pcm[10] = 2048                                     # VAD fails: the slot stays erased
+    want = _planted_and_pinned(ora, pcm, rows, 0x5A4, None, 0)
+    bank, status = handle.enrol(pcm, 2400)
+    for b in range(B):
+        one, st1 = handle.enrol(pcm[b:b + 1], 2400)
+        assert np.array_equal(one[0], bank[b]) and st1[0] == status[b], b
+    slots = sr_b200.make_bank(want["ftr"])
+    slots[want["status"] != 0] = 0xFF
+    assert np.array_equal(status, want["status"]) and status[10] == 1
+    assert not _first_bad_rows(bank, slots), _first_bad_rows(bank, slots)
+
+
+def _push_in_two_phases(pool, pcm, first, chunk=1000):
+    """streams in `first` receive all their samples (chunks of `chunk`) while the others receive none; then the others"""
+    S, L = pcm.shape
+    events = []
+    for group in (np.isin(np.arange(S), first), ~np.isin(np.arange(S), first)):
+        for n0 in range(0, L, chunk):
+            w = min(chunk, L - n0)
+            lens = np.where(group, w, 0).astype(np.uint32)
+            events += pool.push_ragged(np.ascontiguousarray(pcm[:, n0:n0 + w]), lens)
+    return events
+
+
+def _check_sample0_events(events, want, batch, planted):
+    """events == the closed segments of recognise_pinned's VAD; segment 0's results == recognise_pinned == the batch"""
+    S = want["status"].shape[0]
+    closed = [(s, k) for s in range(S) for k in range(3) if want["seg_off"][s, k, 1] != ob.NULL]
+    assert sorted((e["stream"], e["segment"]) for e in events) == closed
+    seen = set()
+    for e in events:
+        s, k = e["stream"], e["segment"]
+        assert (e["start"], e["end"]) == tuple(want["seg_off"][s, k])
+        if k == 0:
+            seen.add(s)
+            got = (e["frm_num"], e["status"], e["best_idx"], e["best_dis"], e["cmd"])
+            b = tuple(int(batch[q][s]) for q in ("status", "best_idx", "best_dis", "cmd"))
+            assert got[1:] == b, ("event vs batch", e, b)
+            w = (int(want["ftr"]["frm_num"][s]), int(want["status"][s]), int(want["best_idx"][s]), int(want["best_dis"][s]), int(want["cmd"][s]))
+            assert got == w, ("event vs recognise_pinned", e, w)
+    assert set(planted) <= seen
+
+
+@pytest.mark.parametrize("group", [False, True], ids=["one_handle", "group_of_two"])
+def test_mfcc_sample0_streaming_events_equal_pinned_and_batch(ora, group):
+    """one stream per utterance, start-0 utterances in streams s >= 1 (row s of the pool's [S][L] buffer, after stream
+    s-1's row). First the row before is still unfilled when the segment closes (stream s-1 is pushed after s), then,
+    after reset() and with other contents, it is already full. Events equal recognise_pinned and the batch call; with
+    a stream group of two handles the streams are sharded over both"""
+    S, L, T = 8, 8000, 9
+    bank = _sample0_bank(ora, T)
+    hs = [sr_b200.Handle(0) for _ in range(2 if group else 1)]
+    for h in hs:
+        h.set_bank(bank, T, 4096)
+    pool = sr_b200.StreamPool(hs if group else hs[0], S, L, 2400)
+    for run, (planted, first) in enumerate((([1, 3, 5, 7], [1, 3, 5, 7]),          # stream s-1 empty when s closes
+                                            ([2, 4, 6], [0, 1, 3, 5, 7]))):       # stream s-1 already full
+        if run:
+            pool.reset()
+        pcm = sr_b200.synth_pcm_host(S, L, 0x5A500000 + 0x100 * run)
+        want = _planted_and_pinned(ora, pcm, planted, 0x5A5 + run, bank, T)
+        batch = hs[0].recognise(pcm, 2400)
+        events = _push_in_two_phases(pool, pcm, first)
+        _check_sample0_events(events, want, batch, planted)
+        _same_recog(batch, want, what=run)
+        seg, atap = pool.segments()
+        assert np.array_equal(seg, want["seg_off"]) and atap.tobytes() == want["atap"].tobytes()
+    pool.close()
+    for h in hs:
+        h.close()
+
+
+def test_geom_b_sample0_batch_and_streaming_pin_mid_val():
+    """GEOM_B (mfcc_geomb_kernel) follows the same rule: get_mfcc of start-0 segments in every row, the recognise path
+    and streaming equal the port's GEOM_B restatement on [mid_val, row...] rows (parity unpinned, as for every GEOM_B
+    test)"""
+    po = ob.port()
+    h = sr_b200.Handle(0)
+    h.set_geometry(1)
+    B, U, T = 24, 8000, 9
+    pcm = sr_b200.synth_pcm_host(B, U, 0x5A600000)
+    pcm[:, -1] = np.where(np.arange(B) % 2 == 0, 0, 4095)
+    seg = np.tile(np.array([0, 1600], np.uint32), (B, 1))
+    seg[3] = (1, 1601)
+    atap = np.zeros(B, sr_b200.ATAP_DTYPE)
+    atap["mid_val"] = 2048
+    atap["mid_val"][5] = 300
+    want_f = po.mfcc_geom_b_batch(ob.pinned_rows(pcm, atap), seg + 1, atap)
+    assert (want_f["frm_num"] == 18).all()
+    assert ob.ftr_equal(h.mfcc(pcm, seg, atap), want_f)
+    bank = _sample0_bank(None, T, geom_b=True)
+    h.set_bank(bank, T, 4096)
+    rows = [0, 1, 2, 5, 11, 12, 17, 22, 23]
+    ob.plant_sample0(pcm, rows, 0x5A6)
+    want = ob.recognise_pinned(po, pcm, 2400, bank, T, 4096, geom_b=True)
+    assert (want["seg_off"][rows, 0, 0] == 0).all() and (want["status"][rows] == 0).all()
+    batch = h.recognise(pcm, 2400)
+    pool = sr_b200.StreamPool(h, B, U, 2400)
+    events = _push_in_two_phases(pool, pcm, rows)
+    pool.close()
+    _check_sample0_events(events, want, batch, rows)
+    _same_recog(batch, want, what="batch")
+    h.close()
 
 
 # ---- device-pointer variants on a torch stream ----------------------------------------------------------
@@ -848,7 +1133,7 @@ def _to_dev(a):
 def test_unaligned_device_pcm_vad_mfcc_recognise(ora, U):
     """the _dev entry points take pcm with 2-byte alignment (speech_recog.h). A batch base that is not 16-byte aligned makes
     vad_kernel stage with plain loads (chunk_issue) and mfcc_kernel with its cooperative copy (stage_utterance), which
-    pins x[-1] of a segment at sample 0 of row 0 to mid_val on its own; noise windows past 2 560 samples read global
+    must pin x[-1] of a segment at sample 0 to mid_val as the bulk copy does; noise windows past 2 560 samples read global
     memory from the unaligned base"""
     import torch
     dev = torch.device("cuda:0")

@@ -115,6 +115,56 @@ def test_port_get_mdl_equals_reference_build():
     assert np.array_equal(d1, d2) and ob.ftr_equal(m1, m2) and (d1 != ob.NULL).any() and (d1 == ob.NULL).any()
 
 
+@pytest.mark.parametrize("which", ["port", "ref"])
+def test_sample0_inputs_reach_the_case_and_recognise_pinned_is_recognise_batch(which):
+    """plant_sample0 and recognise_pinned are the inputs and the reference of the GPU tests of x[-1] at sample 0
+    (test_gpu_parity.py, *sample0*). Identity: on utterances none of whose segments starts at sample 0, recognise_pinned
+    equals the oracle's own recognise_batch in every field. Reach: VAD opens segment 0 of every planted utterance at
+    sample 0, with 1..119 frames, and no other. Sensitivity: every planted utterance's features differ between x[-1] =
+    mid_val, 0 and the preceding row's last sample, so a kernel that read either would fail those tests."""
+    if which == "ref":
+        _need_ref()
+    o = ob.port() if which == "port" else ob.ref()
+    B, U, T = 48, 8000, 10
+    tpl = sr_b200.synth_pcm_host(T, U, 0x5A0B0000)
+    ob.plant_sample0(tpl, [1, 4, 7], 3)
+    e = ob.recognise_pinned(o, tpl, 2400, None, 0, 4096)
+    assert (e["status"] == 0).all()
+    bank = sr_b200.make_bank(e["ftr"])
+    pcm = sr_b200.synth_pcm_host(B, U, 0x5A0A0000)
+    pcm[5] = 2048                                      # VAD fails: status 1
+    want = o.recognise_batch(pcm, 2400, bank, T, 4096)
+    got = ob.recognise_pinned(o, pcm, 2400, bank, T, 4096)
+    assert (want["seg_off"][:, :, 0] != 0).all() and set(want["status"].tolist()) == {0, 1}
+    for k in want:
+        if k == "ftr":
+            assert ob.ftr_equal(got[k], want[k])
+        else:
+            assert np.array_equal(got[k], want[k]), k
+    rows = [0, 1, 2, 9, 10, 23, 24, 46, 47]
+    ob.plant_sample0(pcm, rows, 4)
+    p = ob.recognise_pinned(o, pcm, 2400, bank, T, 4096)
+    planted = np.isin(np.arange(B), rows)
+    assert ((p["seg_off"][:, 0, 0] == 0) == planted).all()
+    assert (p["status"][rows] == 0).all() and (p["ftr"]["frm_num"][rows] >= 1).all() and (p["ftr"]["frm_num"][rows] <= 119).all()
+    assert (p["best_dis"][rows] != ob.NULL).any()      # the planted templates are in reach of the 2:1 guard (DTW.C:133)
+    seg = p["seg_off"][rows, 0, :] + 1
+    base = ob.pinned_rows(pcm[rows], p["atap"][rows])
+    feats = {}
+    for name, x1 in (("mid", None), ("zero", 0), ("before", "prev")):
+        r1 = base.copy()
+        if x1 == "prev":
+            r1[:, 0] = [pcm[r - 1, -1] if r else 4095 for r in rows]
+        elif x1 is not None:
+            r1[:, 0] = x1
+        feats[name] = o.mfcc_batch(r1, seg, p["atap"][rows])
+    assert ob.ftr_equal(feats["mid"], p["ftr"][rows])
+    for i, r in enumerate(rows):
+        assert r == 0 or pcm[r - 1, -1] == 4095
+        for a, b in (("mid", "zero"), ("mid", "before"), ("zero", "before")):
+            assert not ob.ftr_equal(feats[a][i:i + 1], feats[b][i:i + 1]), (r, a, b)
+
+
 def test_dtw_band_oracle_properties():
     """dtw_band is our own extension (parity unpinned by the reference): sanity properties only"""
     raw = sr_b200.synth_ftr_host(6, 0xD7A20000, 50, 100)
