@@ -7,7 +7,7 @@
 //     engine, cp.async.bulk + mbarrier complete_tx), one utterance ahead, as a side job that
 //     rotates over the warps -- every PCM sample is read from HBM exactly once although frames
 //     overlap by 50 %;
-//   * all 16 warps (see the variant table below) take frames round-robin from the CTA's concatenated frame stream,
+//   * all 16 warps take frames round-robin from the CTA's concatenated frame stream,
 //     one frame per warp: pre-emphasis + Hamming (MFCC.C:115-124), FFT, |.| (MFCC.C:49-60),
 //     energy (MFCC.C:128-133), 24 triangular filters (MFCC.C:136-162), log (MFCC.C:165-170),
 //     DCT (MFCC.C:173-183) -> 12 x s16.
@@ -29,13 +29,7 @@
 // and the sign-extending truncation is the identity (also no 32-bit overflow: 2*8209*16385 < 2^31).
 // The generic kernel below runs the shared core's FFT, which keeps the wrap because it accepts arbitrary complex input.
 #include <stdio.h>
-#include <stdlib.h>
-#include <type_traits>
 #include "sr_mfcc_core.cuh"
-
-#ifndef SR_MFCC_DEFAULT_WARPS
-#define SR_MFCC_DEFAULT_WARPS 16
-#endif
 
 namespace srk {
 
@@ -45,7 +39,9 @@ __host__ __device__ constexpr int padF(int e) { return e + ((e >> 6) << 2); }
 constexpr int kFftWords = 2 * (padF(1023) + 1);   // 2168
 static_assert(kFftWords >= kFftWordsTotal, "filter scratch must fit in the FFT buffer");
 
-template <int kConsumerWarps, int kNBuf>
+constexpr int kMfccWarps = 16;               // every warp takes frames and stages utterances as a side job
+constexpr int kNBuf = 3;                     // PCM ring depth
+
 struct __align__(16) MfccSmem {
     unsigned char pcm[kNBuf][kPcmBufBytes];
     int2 tw[340 * 3];
@@ -53,9 +49,9 @@ struct __align__(16) MfccSmem {
     u32 tri_even[512];                       // filter weights as 32-bit words: no unpacking in the frame loop
     u32 tri_odd[512];
     int4 dct[24 * 3];                        // DCT role of lane l < 24: its 12 weights as three 16-byte rows (12-word stride: conflict-free)
-    u32 fftbuf[kConsumerWarps][kFftWords];
-    s32 wq[kConsumerWarps][160];
-    u32 lg[kConsumerWarps][32];
+    u32 fftbuf[kMfccWarps][kFftWords];
+    s32 wq[kMfccWarps][160];
+    u32 lg[kMfccWarps][32];
     u64 full[kNBuf];
     u64 empty[kNBuf];
     s32 meta[kNBuf][5];                      // {F (-1 = no more utterances), sample index of x[start-1] in the buffer, mid, utterance b,
@@ -63,8 +59,7 @@ struct __align__(16) MfccSmem {
     int turn;                                // dynamic hand-out: number of the CTA's next claim (claims are made in ring order)
 };
 
-static_assert(sizeof(MfccSmem<16, 3>) <= 232448, "s16 variant exceeds the 227 KB shared-memory opt-in limit");
-static_assert(sizeof(MfccSmem<15, 3>) <= 232448, "w15 variant exceeds the 227 KB shared-memory opt-in limit");
+static_assert(sizeof(MfccSmem) <= 232448, "mfcc_kernel_s16 exceeds the 227 KB shared-memory opt-in limit");
 
 // Stage utterance number `it` of this CTA's walk (batch row b) into ring slot it % kNBuf: one warp, lane 0 issues
 // the bulk copy. Bytes [lo,hi) of the batch = samples start-1 .. start+80(F-1)+159 of the utterance.
@@ -73,8 +68,7 @@ static_assert(sizeof(MfccSmem<15, 3>) <= 232448, "w15 variant exceeds the 227 KB
 // (its pre-emphasis term is then 0), so an utterance's features do not depend on its row, its chunk, its shard or
 // another stream. The slot only flags it (meta[s][4]); the warp that takes frame 0 writes mid over x[0] once the slot
 // is full. A store here could be overwritten by the bulk copy, which spans x[-1] when sample 0 is not 16-byte aligned.
-template <int kConsumerWarps, int kNBuf, bool kRelaxedWait>
-__device__ __forceinline__ void stage_utterance(MfccSmem<kConsumerWarps, kNBuf> &sm, int it, u32 b, const u16 *__restrict__ pcm,
+__device__ __forceinline__ void stage_utterance(MfccSmem &sm, int it, u32 b, const u16 *__restrict__ pcm,
                                                 u32 U, const u32 *__restrict__ seg, u32 seg_stride,
                                                 const atap_tag *__restrict__ atap, unsigned char *__restrict__ ftr,
                                                 const u32 *__restrict__ row_map, size_t total_bytes, bool base_aligned,
@@ -83,10 +77,7 @@ __device__ __forceinline__ void stage_utterance(MfccSmem<kConsumerWarps, kNBuf> 
     const u32 st = seg[(size_t)b * seg_stride], en = seg[(size_t)b * seg_stride + 1];
     const u32 mid = atap[b].mid_val;
     const long long row = row_map ? (long long)row_map[b] : (long long)b;
-    if (it >= kNBuf) {
-        if (kRelaxedWait) mbar_wait_relaxed(&sm.empty[s], ((it / kNBuf) - 1) & 1);
-        else mbar_wait(&sm.empty[s], ((it / kNBuf) - 1) & 1);
-    }
+    if (it >= kNBuf) mbar_wait(&sm.empty[s], ((it / kNBuf) - 1) & 1);
     const int F = mfcc_frames<SR_FRAME_LEN>(st, en, U);
     if (lane == 0) *reinterpret_cast<u16 *>(ftr + (size_t)b * kFtrBytes + 2) = (u16)F;   // MFCC.C:106,189
     if (F == 0) {
@@ -143,25 +134,28 @@ __device__ __forceinline__ void stage_utterance(MfccSmem<kConsumerWarps, kNBuf> 
 }
 
 // end-of-work marker in ring slot it % kNBuf: consumers leave their loop when they meet it
-template <int kConsumerWarps, int kNBuf, bool kRelaxedWait>
-__device__ __forceinline__ void stage_end(MfccSmem<kConsumerWarps, kNBuf> &sm, int it, int lane) {
+__device__ __forceinline__ void stage_end(MfccSmem &sm, int it, int lane) {
     const int s = it % kNBuf;
-    if (it >= kNBuf) {
-        if (kRelaxedWait) mbar_wait_relaxed(&sm.empty[s], ((it / kNBuf) - 1) & 1);
-        else mbar_wait(&sm.empty[s], ((it / kNBuf) - 1) & 1);
-    }
+    if (it >= kNBuf) mbar_wait(&sm.empty[s], ((it / kNBuf) - 1) & 1);
     if (lane == 0) { sm.meta[s][0] = -1; mbar_arrive(&sm.full[s]); }
 }
 
-// kSelf = false: warp kConsumerWarps is a dedicated producer. kSelf = true: every warp is a consumer and the staging
-// of utterance it+kAhead is a side job of warp it % kConsumerWarps at the top of iteration it, so all four
+// One persistent CTA per SM (threads per CTA are capped at floor(65536 / regs / 128) * 128). Every warp is a consumer,
+// and the staging of utterance it+kAhead is a side job of warp it % kMfccWarps at the top of iteration it, so all four
 // schedulers of the SM carry the same number of working warps.
-template <int kConsumerWarps, int kNBuf, bool kSelf>
-__device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restrict__ seg,
-                                          u32 seg_stride, const atap_tag *__restrict__ atap,
-                                          unsigned char *__restrict__ ftr, const DevTables *__restrict__ tab,
-                                          const u32 *__restrict__ row_map, u32 rows_total, const u32 *__restrict__ B_dev,
-                                          u32 *__restrict__ work /* [0] next utterance to hand out, [1] CTAs finished; NULL: static */) {
+// Measured and dropped: the asm's 3-multiply twiddle form (one IMAD traded for a subtract: 4.91 ms vs 4.76), forcing the
+// C+-D sums of the butterflies onto the ALU pipe as three-input adds (4.86 vs 4.76), two 16-bit
+// stores instead of PRMT + one 32-bit store in block A (4.86 vs 4.80), 20 warps @ 96 regs (5.29 ms vs 5.31), 24 warps @ 80 regs (5.48 ms) -- the half-rate ALU and
+// FMA-heavy pipes, not occupancy, bound the kernel. On the H100 (400 W), no gain beyond run-to-run spread: storing w>>4 for
+// stage 1's A leg to skip its shift (4 SASS instructions per frame fewer), and log100 as one correction step each way
+// instead of the two loops (MFCC kernel 5.18 and 5.18 ms vs 5.20). Slower: 15 consumer warps plus a dedicated producer
+// warp, which leaves one scheduler with 3 working warps (5 % on the B200; on the H100 (700 W) MFCC kernel 4.97 ms vs 4.74,
+// step 6.01 ms vs 5.78).
+__global__ void __maxnreg__(128) mfcc_kernel_s16(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restrict__ seg,
+                                                 u32 seg_stride, const atap_tag *__restrict__ atap,
+                                                 unsigned char *__restrict__ ftr, const DevTables *__restrict__ tab,
+                                                 const u32 *__restrict__ row_map, u32 rows_total, const u32 *__restrict__ B_dev,
+                                                 u32 *__restrict__ work /* [0] next utterance to hand out, [1] CTAs finished; NULL: static */) {
     constexpr int kAhead = kNBuf - 2;                      // slot of it+kAhead was last used by utterance it-2
     if (B_dev) B = min(B, *B_dev);                         // batch size produced on the device (streaming: segments closed by this push)
     // the last CTA out re-arms the hand-out counters for the next launch on this stream
@@ -173,7 +167,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
     };
     if (blockIdx.x >= B) { cta_done(); return; }           // more CTAs than utterances (device-side batch size): these never claim
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    MfccSmem<kConsumerWarps, kNBuf> &sm = *reinterpret_cast<MfccSmem<kConsumerWarps, kNBuf> *>(smem_raw);
+    MfccSmem &sm = *reinterpret_cast<MfccSmem *>(smem_raw);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     // ---- one-time: tables to shared memory, barriers ------------------------------------------
@@ -188,7 +182,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
         sm.tri_odd[flt_word(i >> 4, i & 15)] = tab->tri_odd[i];
     }
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kNBuf; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], kConsumerWarps); }
+        for (int s = 0; s < kNBuf; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], kMfccWarps); }
         sm.turn = 0;
         mbar_fence_init();
     }
@@ -205,7 +199,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
     // the utterance numbers of a CTA grow with it_s and every slot behind an end marker holds an end marker too (a later
     // slot claimed EARLIER could hold a real utterance that the consumers, leaving at the first marker, would never see).
     // A claim waits only for the claim before it, which is made at the top of an earlier iteration: no cycle.
-    auto claim_stage = [&](int it_s, auto relaxed) {
+    auto claim_stage = [&](int it_s) {
         u32 b;
         if (work) {
             b = 0;
@@ -219,26 +213,11 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
             b = __shfl_sync(0xFFFFFFFFu, b, 0);
         }
         else b = blockIdx.x + (u32)it_s * gridDim.x;
-        if (b < B)
-            stage_utterance<kConsumerWarps, kNBuf, decltype(relaxed)::value>(sm, it_s, b, pcm, U, seg, seg_stride, atap, ftr, row_map,
-                                                                            total_bytes, base_aligned, lane);
-        else
-            stage_end<kConsumerWarps, kNBuf, decltype(relaxed)::value>(sm, it_s, lane);
-        return b < B;
+        if (b < B) stage_utterance(sm, it_s, b, pcm, U, seg, seg_stride, atap, ftr, row_map, total_bytes, base_aligned, lane);
+        else stage_end(sm, it_s, lane);
     };
-    if (!kSelf) {
-        // ============================ producer warp =============================================
-        // after its last claim it skips the consumer loop but does not return: every warp of the CTA must reach the
-        // final __syncthreads() (a CTA barrier that some threads never reach is undefined)
-        if (warp == kConsumerWarps) {
-            for (int it = 0;; ++it)
-                if (!claim_stage(it, std::true_type{})) break;
-        }
-    } else if (warp < kAhead) {                            // prologue: utterances 0 .. kAhead-1
-        claim_stage(warp, std::false_type{});
-    }
+    if (warp < kAhead) claim_stage(warp);                 // prologue: utterances 0 .. kAhead-1
 
-    // ================================ consumer warps ============================================
     u32 *fb = sm.fftbuf[warp];
     s32 *wq = sm.wq[warp];
     const int q1 = lane & 3;
@@ -263,8 +242,8 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
     const int4 *dctk4 = sm.dct + 3 * (lane < 24 ? lane : 0);
 
     u32 gidx = 0;   // frames of this CTA's stream before the current utterance
-    for (int it = 0; kSelf || warp < kConsumerWarps; ++it) {           // w15's producer warp never enters
-        if (kSelf && warp == it % kConsumerWarps) claim_stage(it + kAhead, std::false_type{});
+    for (int it = 0;; ++it) {
+        if (warp == it % kMfccWarps) claim_stage(it + kAhead);
         const int s = it % kNBuf;
         mbar_wait(&sm.full[s], (it / kNBuf) & 1);
         const int F = sm.meta[s][0];
@@ -274,7 +253,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
         const s32 mid = sm.meta[s][2];
         u16 *x = reinterpret_cast<u16 *>(sm.pcm[s]) + off;               // x[0] = sample start-1
         unsigned char *out_rows = ftr + (size_t)b * kFtrBytes + 4;
-        const int f0 = (int)((warp - (int)(gidx % kConsumerWarps) + kConsumerWarps) % kConsumerWarps);   // this warp's first frame
+        const int f0 = (int)((warp - (int)(gidx % kMfccWarps) + kMfccWarps) % kMfccWarps);   // this warp's first frame
         // start == 0: x[-1] := mid (see stage_utterance). Only frame 0 reads x[0], and only its lane 0.
         if (f0 == 0 && lane == 0 && sm.meta[s][4]) x[0] = (u16)mid;
 
@@ -287,7 +266,7 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
                 wq[i] = preemph_hamm(xf[i + 1], xf[i], (u32)mid, hm[k]) >> 2;   // BUTFLY4ZERO_OPT with B=C=D=0
             }
         };
-        for (int f = f0; f < F; f += kConsumerWarps) {
+        for (int f = f0; f < F; f += kMfccWarps) {
             const u16 *xf = x + 80 * f;                                  // xf[i] = vc_dat[i-1]
             preemph(xf);
             __syncwarp();
@@ -443,30 +422,6 @@ __device__ __forceinline__ void mfcc_body(const u16 *__restrict__ pcm, u32 U, u3
     cta_done();
 }
 
-// Variants (one persistent CTA per SM; threads per CTA are capped at floor(65536 / regs / 128) * 128):
-//   s16: 16 warps, all consumers, staging as a rotating side job, 3-deep ring   (default)
-//   w15: 15 consumers + 1 dedicated producer warp, 3-deep ring   (SR_MFCC_WARPS=15; 5 % slower: one scheduler
-//        carries only 3 working warps). Its producer warp used to return after its last claim, leaving the final
-//        __syncthreads() to the consumers alone, which is undefined; it now skips the consumer loop and joins it.
-// Measured and dropped: the asm's 3-multiply twiddle form (one IMAD traded for a subtract: 4.91 ms vs 4.76), forcing the
-// C+-D sums of the butterflies onto the ALU pipe as three-input adds (4.86 vs 4.76), two 16-bit
-// stores instead of PRMT + one 32-bit store in block A (4.86 vs 4.80), 20 warps @ 96 regs (5.29 ms vs 5.31), 24 warps @ 80 regs (5.48 ms) -- the half-rate ALU and
-// FMA-heavy pipes, not occupancy, bound the kernel. On the H100 (400 W), no gain beyond run-to-run spread: storing w>>4 for
-// stage 1's A leg to skip its shift (4 SASS instructions per frame fewer), and log100 as one correction step each way
-// instead of the two loops (MFCC kernel 5.18 and 5.18 ms vs 5.20).
-#define SR_MFCC_VARIANT(NAME, W, NB, SELF, NREG)                                                                     \
-    __global__ void __maxnreg__(NREG) mfcc_kernel_##NAME(const u16 *__restrict__ pcm, u32 U, u32 B,              \
-                                                         const u32 *__restrict__ seg, u32 seg_stride,            \
-                                                         const atap_tag *__restrict__ atap,                       \
-                                                         unsigned char *__restrict__ ftr,                         \
-                                                         const DevTables *__restrict__ tab,                       \
-                                                         const u32 *__restrict__ row_map, u32 rows_total,        \
-                                                         const u32 *__restrict__ B_dev, u32 *__restrict__ work) { \
-        mfcc_body<W, NB, SELF>(pcm, U, B, seg, seg_stride, atap, ftr, tab, row_map, rows_total, B_dev, work);     \
-    }
-SR_MFCC_VARIANT(s16, 16, 3, true, 128)
-SR_MFCC_VARIANT(w15, 15, 3, false, 128)
-
 // ---- generic (unpruned) FFT + magnitude: the reference's global `fft` (MFCC.C:27-62) -----------
 // One warp per frame, all five passes in shared memory exactly as the asm orders them. Not on the
 // hot path; it exists for the secondary drop-in symbol and as an on-device cross-check of the
@@ -494,41 +449,27 @@ fft_generic_kernel(const u32 *__restrict__ in /*[n][1024] packed or NULL*/, cons
 }
 
 // ---- host launchers -----------------------------------------------------------------------------
-template <int W, int NB, bool SELF, typename K>
-static cudaError_t launch_mfcc_variant(K kern, const u16 *pcm, u32 U, u32 B, const u32 *seg, u32 seg_stride,
-                                       const atap_tag *atap, void *ftr, int num_sms, const DevTables *tab, cudaStream_t st,
-                                       const u32 *row_map, u32 rows_total, const u32 *B_dev, u32 *work) {
-    const size_t smem = sizeof(MfccSmem<W, NB>);
-    const int threads = (SELF ? W : W + 1) * 32;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const u32 grid = B < (u32)num_sms ? B : (u32)num_sms;
-    kern<<<grid, threads, smem, st>>>(pcm, U, B, seg, seg_stride, atap, static_cast<unsigned char *>(ftr), tab, row_map,
-                                      rows_total, B_dev, work);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) {
-        cudaFuncAttributes fa;
-        if (cudaFuncGetAttributes(&fa, kern) == cudaSuccess)
-            fprintf(stderr, "mfcc kernel (%d warps) launch failed (%s): regs %d, maxThreads %d, static smem %zu, dyn smem %zu (max %d), threads %d\n",
-                    W, cudaGetErrorString(e), fa.numRegs, fa.maxThreadsPerBlock, fa.sharedSizeBytes, smem,
-                    fa.maxDynamicSharedSizeBytes, threads);
-    }
-    return e;
-}
-
 cudaError_t launch_mfcc(const u16 *pcm, u32 U, u32 B, const u32 *seg, u32 seg_stride, const atap_tag *atap,
                         void *ftr, int num_sms, cudaStream_t st, const u32 *row_map, u32 rows_total, const u32 *B_dev, u32 *work) {
     if (B == 0) return cudaSuccess;
     const DevTables *tab = dev_tables();
     if (!tab) return cudaErrorInitializationError;
-    static int variant = -1;                               // SR_MFCC_WARPS=15 selects the dedicated-producer variant (tuning knob)
-    if (variant < 0) {
-        const char *ev = getenv("SR_MFCC_WARPS");
-        variant = ev ? atoi(ev) : SR_MFCC_DEFAULT_WARPS;
+    const size_t smem = sizeof(MfccSmem);
+    const int threads = kMfccWarps * 32;
+    cudaError_t e = cudaFuncSetAttribute(mfcc_kernel_s16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const u32 grid = B < (u32)num_sms ? B : (u32)num_sms;
+    mfcc_kernel_s16<<<grid, threads, smem, st>>>(pcm, U, B, seg, seg_stride, atap, static_cast<unsigned char *>(ftr), tab,
+                                                 row_map, rows_total, B_dev, work);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        cudaFuncAttributes fa;
+        if (cudaFuncGetAttributes(&fa, mfcc_kernel_s16) == cudaSuccess)
+            fprintf(stderr, "mfcc kernel launch failed (%s): regs %d, maxThreads %d, static smem %zu, dyn smem %zu (max %d), threads %d\n",
+                    cudaGetErrorString(e), fa.numRegs, fa.maxThreadsPerBlock, fa.sharedSizeBytes, smem,
+                    fa.maxDynamicSharedSizeBytes, threads);
     }
-    if (variant == 15)
-        return launch_mfcc_variant<15, 3, false>(mfcc_kernel_w15, pcm, U, B, seg, seg_stride, atap, ftr, num_sms, tab, st, row_map, rows_total, B_dev, work);
-    return launch_mfcc_variant<16, 3, true>(mfcc_kernel_s16, pcm, U, B, seg, seg_stride, atap, ftr, num_sms, tab, st, row_map, rows_total, B_dev, work);
+    return e;
 }
 
 cudaError_t launch_fft_generic(const u32 *in_packed, const s16 *frames, u32 len, u32 n, u32 *raw_out, u32 *mag,

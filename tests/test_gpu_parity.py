@@ -294,24 +294,6 @@ def test_mfcc_largest_magnitude_frames(handle, ora):
     assert ob.ftr_equal(got, ora.mfcc_batch(pcm, seg, atap))
 
 
-def test_mfcc_tests_under_the_w15_variant():
-    """SR_MFCC_WARPS=15 selects mfcc_kernel_w15 (15 consumer warps + a dedicated producer warp, relaxed barrier waits).
-    The library reads the switch once per process, so this file's MFCC tests run again in a child pytest"""
-    import re
-    import subprocess
-    import sys
-    if os.environ.get("SR_MFCC_WARPS"):
-        pytest.skip("already running under a chosen MFCC variant")
-    env = dict(os.environ, SR_MFCC_WARPS="15", SR_NO_BUILD="1")
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.abspath(__file__), "-k", "mfcc and not geom"]
-    r = subprocess.run(cmd, cwd=os.path.dirname(HERE), env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
-                       timeout=1800)
-    assert r.returncode == 0, r.stdout[-4000:]
-    m = re.search(r"(\d+) passed", r.stdout)
-    assert m and int(m.group(1)) >= 100 and " failed" not in r.stdout, r.stdout[-4000:]
-
-
 # ---- noise_atap + VAD ---------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["stm32_123", "stm32_456", "stm32_noise", "stm32_voice_123", "v1"])
 def test_vad_on_board_captures_matches_golden(handle, name):
