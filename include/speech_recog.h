@@ -313,10 +313,13 @@ int sr_transport_stats(const sr_handle *h, uint32_t *packed_chunks, uint32_t *pl
 uint32_t sr_debug_pack12_host(int variant, const uint16_t *src, uint64_t n, uint8_t *dst);
 int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t *out);
 
-/* Per-kernel device timing: after sr_timing_enable(h, max_records) every kernel launch of this handle is
- * bracketed by a CUDA event pair on the launching stream; sr_timing_collect synchronises the stream and
- * returns (tag, milliseconds) per launch in issue order, then rearms. Tags: 0 noise_atap+VAD, 1 get_mfcc,
- * 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP). max_records = 0 disables. */
+/* Per-kernel device timing: after sr_timing_enable(h, max_records) every launch of the recognition-path kernels
+ * by this handle's noise_atap, VAD, MFCC, DTW, recognise and enrol calls (host-buffer and _dev forms) is bracketed
+ * by a CUDA event pair on the launching stream. Not timed: the test-hook kernels (FFT, get_dis, get_mdl, dtw_limit,
+ * sqrt check), the packed transport's 12-bit expander, enrol's slot packing and the streaming pool's kernels. Zero-size
+ * calls launch and record nothing. sr_timing_collect synchronises the
+ * stream and returns (tag, milliseconds) per timed launch in issue order, then rearms. Tags: 0 noise_atap+VAD,
+ * 1 get_mfcc, 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP). max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

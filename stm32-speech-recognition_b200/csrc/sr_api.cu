@@ -164,7 +164,10 @@ void sr_host_free(void *p) {
 
 int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 
-// ---- per-kernel timing: event pairs on the launching stream around every kernel -----------------------
+// ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
+enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
+       TAG_DTW_BAND = 6 };
+
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
     DeviceGuard g(h->device);
@@ -195,29 +198,111 @@ int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uin
     return 0;
 }
 
+}  // extern "C"
+
+// one kernel launch on the handle's stream, launch() returning its cudaError_t: bracketed by an event pair when tag is
+// not TAG_NONE and timing is enabled, counted when it succeeds
+template <class F> static int launch_on(sr_handle *h, int tag, const char *what, F launch) {
+    size_t slot = SIZE_MAX;
+    if (tag != TAG_NONE && h->timing && (h->ev_used + 1) * 2 <= h->ev.size()) {
+        slot = h->ev_used++;
+        h->ev_tag[slot] = tag;
+        cudaEventRecord(h->ev[2 * slot], h->stream);
+    }
+    const cudaError_t e = launch();
+    if (slot != SIZE_MAX) cudaEventRecord(h->ev[2 * slot + 1], h->stream);
+    if (e != cudaSuccess) return fail(h, what, e);
+    ++h->launches;
+    return 0;
+}
+#define SR_LAUNCH(h, tag, call)                                                                   \
+    do {                                                                                          \
+        if (const int rc__ = launch_on((h), (tag), #call, [&] { return (call); })) return rc__;   \
+    } while (0)
+
+// get_mfcc (MFCC.C) and get_mdl (DTW.C) never write save_sign: copy back bytes [2, 2860) of each of n structs only
+static cudaError_t ftr_to_host(sr_handle *h, v_ftr_tag *dst, const void *src, size_t n) {
+    return cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(dst) + 2, kFtrBytes, static_cast<const unsigned char *>(src) + 2,
+                             kFtrBytes, kFtrBytes - 2, n, cudaMemcpyDeviceToHost, h->stream);
+}
+
+// One host-buffer call: inputs staged into handle workspaces, kernels, outputs copied back, one synchronisation. The
+// first failure is kept (its message prefixed with the call's name) and every later step is skipped; finish() returns it.
+struct HostCall {
+    sr_handle *h;
+    const char *name;
+    DeviceGuard g;
+    int rc = 0;
+    struct Back { void *dst; const void *src; size_t bytes; bool ftr; } back[8];
+    int n_back = 0;
+
+    HostCall(sr_handle *hh, const char *nm) : h(hh), name(nm), g(hh->device) {}
+    void took(int r) {
+        if (!r || rc) return;
+        rc = r;
+        h->err = std::string(name) + ": " + h->err;
+        g_tls_error = h->err;
+    }
+    void ck(const char *what, cudaError_t e) { if (!rc && e != cudaSuccess) took(fail(h, what, e)); }
+    template <class F> void run(F f) { if (!rc) took(f()); }
+    template <class F> void launch(int tag, const char *what, F f) { if (!rc) took(launch_on(h, tag, what, f)); }
+    // workspace w, at least `bytes` long (NULL once the call has failed)
+    template <class T = void> T *ws(DevBuf &w, size_t bytes) {
+        if (!rc) ck("ensure", ensure(w, bytes));
+        return rc ? nullptr : static_cast<T *>(w.p);
+    }
+    void h2d(void *dst, const void *src, size_t bytes) {
+        if (!rc && bytes) ck("cudaMemcpyAsync host->device", cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
+    }
+    // `bytes` of host input src staged in workspace w (slack: extra bytes the kernel may read past the end)
+    template <class T> T *in(DevBuf &w, const T *src, size_t bytes, size_t slack = 0) {
+        T *d = ws<T>(w, bytes + slack);
+        h2d(d, src, bytes);
+        return d;
+    }
+    // workspace w for an output that finish() copies back to dst (if dst != NULL); v_ftr_tag outputs skip save_sign
+    template <class T> T *out(DevBuf &w, T *dst, size_t bytes, size_t slack = 0) {
+        T *d = ws<T>(w, bytes + slack);
+        if (d && dst && bytes) back[n_back++] = {dst, d, bytes, std::is_same_v<T, v_ftr_tag>};
+        return d;
+    }
+    int finish() {
+        for (int i = 0; i < n_back; ++i) {
+            const Back &b = back[i];
+            ck("copy back", b.ftr ? ftr_to_host(h, static_cast<v_ftr_tag *>(b.dst), b.src, b.bytes / kFtrBytes)
+                                  : cudaMemcpyAsync(b.dst, b.src, b.bytes, cudaMemcpyDeviceToHost, h->stream));
+        }
+        ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+        return rc;
+    }
+};
+
+extern "C" {
+
 // ---- template bank --------------------------------------------------------------------------------
 // Banks wider than one 32-template tile are walked in ascending frm_num order, so that the templates sharing a warp have
 // similar walk lengths (CPU model: mean/max walk length per tile 0.81 -> 0.88 at T = 200). The order is a hint: scores and
 // argmin keys carry the original slot numbers, and a stale order (bank rewritten in place) only costs efficiency.
 static int bank_order(sr_handle *h, const unsigned char *hdr_host /* n_slot headers, 4 bytes each, or NULL: fetch */) {
-    h->perm = nullptr;
-    const u32 T = h->n_slot;
-    if (T <= 32 || !h->bank) { h->perm_bank = h->bank; h->perm_n = T; h->perm_stride = h->slot_stride; return 0; }
+    BankView &b = h->bank;
+    b.order = nullptr;
+    const u32 T = b.n;
+    if (T <= 32 || !b.p) { h->perm_bank = b.p; h->perm_n = T; h->perm_stride = b.stride; return 0; }
     std::vector<u32> hdr(T);
     if (hdr_host) memcpy(hdr.data(), hdr_host, (size_t)T * 4);
     else {
-        SR_CK(h, cudaMemcpy2DAsync(hdr.data(), 4, h->bank, h->slot_stride, 4, T, cudaMemcpyDeviceToHost, h->stream));
+        SR_CK(h, cudaMemcpy2DAsync(hdr.data(), 4, b.p, b.stride, 4, T, cudaMemcpyDeviceToHost, h->stream));
         SR_CK(h, cudaStreamSynchronize(h->stream));
     }
     std::vector<u32> order(T);
     for (u32 i = 0; i < T; ++i) order[i] = i;
     auto key = [&](u32 i) { const u32 f = hdr[i] >> 16; return f > 119u ? 0xFFFFu : f; };   // garbage headers last
-    std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 b) { return key(a) < key(b); });
+    std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 c) { return key(a) < key(c); });
     SR_CK(h, ensure(h->bank_perm, (size_t)T * 4));
     SR_CK(h, cudaMemcpyAsync(h->bank_perm.p, order.data(), (size_t)T * 4, cudaMemcpyHostToDevice, h->stream));
     SR_CK(h, cudaStreamSynchronize(h->stream));                     // `order` is a local
-    h->perm = static_cast<const u32 *>(h->bank_perm.p);
-    h->perm_bank = h->bank; h->perm_n = T; h->perm_stride = h->slot_stride;
+    b.order = static_cast<const u32 *>(h->bank_perm.p);
+    h->perm_bank = b.p; h->perm_n = T; h->perm_stride = b.stride;
     return 0;
 }
 
@@ -226,7 +311,7 @@ int sr_set_bank_dev(sr_handle *h, const void *bank_dev, uint32_t n_slot, uint32_
     SR_REQUIRE(h, n_slot == 0 || (bank_dev != nullptr && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0));
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(bank_dev) & 3) == 0);
     const bool same = h->perm_bank == bank_dev && h->perm_n == n_slot && h->perm_stride == slot_stride;
-    h->bank = bank_dev; h->n_slot = n_slot; h->slot_stride = slot_stride;
+    h->bank = {bank_dev, n_slot, slot_stride, h->bank.order};
     if (same) return 0;                                   // same buffer as last time (callers re-set it per batch): keep the order
     DeviceGuard g(h->device);
     return bank_order(h, nullptr);
@@ -240,7 +325,7 @@ int sr_set_bank(sr_handle *h, const void *bank, uint32_t n_slot, uint32_t slot_s
     SR_CK(h, ensure(h->bank_own, bytes + 16));
     if (bytes) SR_CK(h, cudaMemcpyAsync(h->bank_own.p, bank, bytes, cudaMemcpyHostToDevice, h->stream));
     SR_CK(h, cudaStreamSynchronize(h->stream));
-    h->bank = h->bank_own.p; h->n_slot = n_slot; h->slot_stride = slot_stride;
+    h->bank = {h->bank_own.p, n_slot, slot_stride, nullptr};
     std::vector<u32> hdr(n_slot);
     for (u32 i = 0; i < n_slot; ++i) memcpy(&hdr[i], static_cast<const unsigned char *>(bank) + (size_t)i * slot_stride, 4);
     return bank_order(h, reinterpret_cast<const unsigned char *>(hdr.data()));
@@ -276,9 +361,9 @@ int sr_labels_batch(const sr_handle *h, const uint32_t *cmd, const uint8_t *stat
 int sr_noise_atap_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, atap_tag *atap) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && atap)));
     SR_REQUIRE(h, U <= 65535u && n_len <= 65535u);
+    if (B == 0) return 0;
     DeviceGuard g(h->device);
-    { TimedLaunch tl(h, TAG_VAD); SR_CK(h, launch_vad(pcm, U, B, n_len, 0, 1, 0, atap, nullptr, h->num_sms, h->stream, vad_work(h))); }
-    h->launches += B ? 1 : 0;
+    SR_LAUNCH(h, TAG_VAD, launch_vad(pcm, U, B, n_len, 0, 1, 0, atap, nullptr, h->num_sms, h->stream, vad_work(h)));
     return 0;
 }
 
@@ -286,9 +371,9 @@ int sr_vad_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, 
                      uint32_t *seg_off) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && atap && seg_off)));
     SR_REQUIRE(h, U <= 65535u && buf_len <= U);
+    if (B == 0) return 0;
     DeviceGuard g(h->device);
-    { TimedLaunch tl(h, TAG_VAD); SR_CK(h, launch_vad(pcm, U, B, 0, buf_len, 0, 1, const_cast<atap_tag *>(atap), seg_off, h->num_sms, h->stream, vad_work(h))); }
-    h->launches += B ? 1 : 0;
+    SR_LAUNCH(h, TAG_VAD, launch_vad(pcm, U, B, 0, buf_len, 0, 1, const_cast<atap_tag *>(atap), seg_off, h->num_sms, h->stream, vad_work(h)));
     return 0;
 }
 
@@ -296,14 +381,17 @@ int sr_mfcc_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
                       const atap_tag *atap, v_ftr_tag *ftr) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && seg && atap && ftr)));
     SR_REQUIRE(h, seg_stride >= 2 && (reinterpret_cast<uintptr_t>(ftr) & 3) == 0);
+    if (B == 0) return 0;
     DeviceGuard g(h->device);
-    { TimedLaunch tl(h, TAG_MFCC); SR_CK(h, launch_mfcc_h(h, pcm, U, B, seg, seg_stride, atap, ftr)); }
-    h->launches += B ? 1 : 0;
+    SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, B, seg, seg_stride, atap, ftr));
     return 0;
 }
 
-static int dtw_dev_impl(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
-                        uint32_t *best_idx, uint32_t *best_dis, uint32_t *cmd, const u8 *status) {
+}  // extern "C"
+
+// the template scan of B inputs against `bank`, then the argmin of each when one of best_idx / best_dis / cmd is wanted
+static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
+                        uint32_t *score, uint32_t *best_idx, uint32_t *best_dis, uint32_t *cmd, const u8 *status) {
     SR_REQUIRE(h, h && (B == 0 || in));
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
     if (B == 0) return 0;
@@ -313,40 +401,29 @@ static int dtw_dev_impl(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t 
         DevBuf &bb = h->best_sel ? h->best_alt : h->best;
         SR_CK(h, ensure(bb, (size_t)B * 8));
         best = static_cast<u64 *>(bb.p);
-        { TimedLaunch tl(h, TAG_BEST_INIT); SR_CK(h, launch_best_init(best, B, h->stream)); }
-        ++h->launches;
+        SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, B, h->stream));
     }
-    if (h->n_slot) {
-        if (flags & SR_DTW_BAND) {
-            SR_REQUIRE(h, band_r >= 0);
-            TimedLaunch tl(h, TAG_DTW_BAND);
-            SR_CK(h, launch_dtw_band(in, B, h->bank, h->n_slot, h->slot_stride, flags, band_r, score, best, h->num_sms, h->stream));
-        } else {
-            TimedLaunch tl(h, TAG_DTW);
-            SR_CK(h, launch_dtw_h(h, in, B, flags, score, best, status));
-        }
-        ++h->launches;
+    if (bank.n && (flags & SR_DTW_BAND)) {
+        SR_REQUIRE(h, band_r >= 0);
+        SR_LAUNCH(h, TAG_DTW_BAND, launch_dtw_band(in, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, h->num_sms, h->stream));
+    } else if (bank.n) {
+        SR_LAUNCH(h, TAG_DTW, launch_dtw_h(h, bank, in, B, flags, score, best, status));
     }
-    if (want_best) {
-        { TimedLaunch tl(h, TAG_BEST_FINAL); SR_CK(h, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream)); }
-        ++h->launches;
-    }
+    if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
     return 0;
 }
 
-int sr_dtw_batch_dev(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
-                     uint32_t *best_idx, uint32_t *best_dis) {
+extern "C" int sr_dtw_batch_dev(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
+                                uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h != nullptr);
     DeviceGuard g(h->device);
-    return dtw_dev_impl(h, in, B, flags, band_r, score, best_idx, best_dis, nullptr, nullptr);
+    return dtw_dev_impl(h, h->bank, in, B, flags, band_r, score, best_idx, best_dis, nullptr, nullptr);
 }
 
-int sr_recognise_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
-                           const sr_recog_out *o) {
+extern "C" int sr_recognise_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
+                                      const sr_recog_out *o) {
     return recognise_dev_impl(h, pcm, U, B, n_len, o, false);
 }
-
-}  // extern "C"
 
 // sr_recog_out field by field: f(member, the handle's device mirror of it, bytes per utterance); score holds one word per
 // template of the handle's bank
@@ -354,7 +431,7 @@ template <class F> static void for_each_output(sr_handle *h, F f) {
     f(&sr_recog_out::atap, h->atap, sizeof(atap_tag));
     f(&sr_recog_out::seg_off, h->seg, (size_t)24);
     f(&sr_recog_out::ftr, h->ftr, (size_t)kFtrBytes);
-    f(&sr_recog_out::score, h->score, (size_t)h->n_slot * 4);
+    f(&sr_recog_out::score, h->score, (size_t)h->bank.n * 4);
     f(&sr_recog_out::best_idx, h->bidx, (size_t)4);
     f(&sr_recog_out::best_dis, h->bdis, (size_t)4);
     f(&sr_recog_out::cmd, h->cmd, (size_t)4);
@@ -368,20 +445,13 @@ static sr_recog_out recog_slice(sr_handle *h, const sr_recog_out &o, size_t lo) 
     return s;
 }
 
-// get_mfcc (MFCC.C) and get_mdl (DTW.C) never write save_sign: copy back bytes [2, 2860) of each of n structs only
-static cudaError_t ftr_to_host(sr_handle *h, v_ftr_tag *dst, const void *src, size_t n) {
-    return cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(dst) + 2, kFtrBytes, static_cast<const unsigned char *>(src) + 2,
-                             kFtrBytes, kFtrBytes - 2, n, cudaMemcpyDeviceToHost, h->stream);
-}
-
 // the front end of spch_recg and save_mdl on B staged utterances: noise_atap, VAD, get_mfcc of segment 0, status
 static int front_end(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 n_len, atap_tag *atap, u32 *seg, void *ftr, u8 *status) {
     // main.c:258-260 noise_atap + VAD (one fused launch on the staged utterance)
-    { TimedLaunch tl(h, TAG_VAD); SR_CK(h, launch_vad(pcm, U, B, n_len, U, 1, 1, atap, seg, h->num_sms, h->stream, vad_work(h))); }
+    SR_LAUNCH(h, TAG_VAD, launch_vad(pcm, U, B, n_len, U, 1, 1, atap, seg, h->num_sms, h->stream, vad_work(h)));
     // main.c:268 get_mfcc of segment 0
-    { TimedLaunch tl(h, TAG_MFCC); SR_CK(h, launch_mfcc_h(h, pcm, U, B, seg, 6, atap, ftr)); }
-    { TimedLaunch tl(h, TAG_STATUS); SR_CK(h, launch_status(seg, ftr, B, status, h->stream)); }
-    h->launches += 3;
+    SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, B, seg, 6, atap, ftr));
+    SR_LAUNCH(h, TAG_STATUS, launch_status(seg, ftr, B, status, h->stream));
     return 0;
 }
 
@@ -411,7 +481,34 @@ int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
         if (rc) return rc;
     }
     // main.c:276-294 template scan, argmin, command index
-    return dtw_dev_impl(h, ftr, B, SR_DTW_CHECK_SIGN, 0, o->score, o->best_idx, o->best_dis, o->cmd, status);
+    return dtw_dev_impl(h, h->bank, ftr, B, SR_DTW_CHECK_SIGN, 0, o->score, o->best_idx, o->best_dis, o->cmd, status);
+}
+
+// sr_dtw_batch of B host inputs against `bank`, inside the host call c
+static int dtw_host(HostCall &c, const BankView &bank, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
+                    uint32_t *score, uint32_t *best_idx, uint32_t *best_dis) {
+    sr_handle *h = c.h;
+    const v_ftr_tag *d_in = c.in(h->ftr, in, (size_t)B * kFtrBytes);
+    u32 *d_score = score ? c.out(h->score, score, (size_t)B * bank.n * 4, 4) : nullptr;
+    u32 *d_idx = c.out(h->bidx, best_idx, (size_t)B * 4), *d_dis = c.out(h->bdis, best_dis, (size_t)B * 4);
+    c.run([&] { return dtw_dev_impl(h, bank, d_in, B, flags, band_r, d_score, best_idx ? d_idx : nullptr,
+                                    best_dis ? d_dis : nullptr, nullptr, nullptr); });
+    return c.finish();
+}
+
+// the FFT of n inputs, 1024-point packed (re | im<<16) or `len` real samples each: raw bins and / or magnitudes
+static int fft_host(HostCall &c, const uint32_t *packed, const int16_t *frames, uint32_t len, uint32_t n, uint32_t *raw,
+                    uint32_t *mag) {
+    sr_handle *h = c.h;
+    const void *d_in = packed ? (const void *)c.in(h->scratch[0], packed, (size_t)n * 4096)
+                              : (const void *)c.in(h->scratch[0], frames, (size_t)n * len * 2, 16);
+    u32 *d_raw = raw ? c.out(h->scratch[1], raw, (size_t)n * 4096) : nullptr;   // copied back before mag: see fft()
+    u32 *d_mag = mag ? c.out(h->scratch[2], mag, (size_t)n * 2048) : nullptr;
+    c.launch(TAG_NONE, "launch_fft_generic", [&] {
+        return launch_fft_generic(packed ? static_cast<const u32 *>(d_in) : nullptr, packed ? nullptr : static_cast<const s16 *>(d_in),
+                                  len, n, d_raw, d_mag, h->stream);
+    });
+    return c.finish();
 }
 
 extern "C" {
@@ -421,34 +518,24 @@ extern "C" {
 int sr_noise_atap_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, atap_tag *atap) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && atap)));
     if (B == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->pcm, (size_t)B * U * 2 + 16));
-    SR_CK(h, ensure(h->atap, (size_t)B * sizeof(atap_tag)));
-    H2D(h, h->pcm.p, pcm, (size_t)B * U * 2);
-    H2D(h, h->atap.p, atap, (size_t)B * sizeof(atap_tag));
-    int rc = sr_noise_atap_batch_dev(h, static_cast<const u16 *>(h->pcm.p), U, B, n_len, static_cast<atap_tag *>(h->atap.p));
-    if (rc) return rc;
-    D2H(h, atap, h->atap.p, (size_t)B * sizeof(atap_tag));
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_noise_atap_batch");
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    atap_tag *d_atap = c.in(h->atap, atap, (size_t)B * sizeof(atap_tag));      // in / out: untouched when n_len % 240 != 0
+    c.out(h->atap, atap, (size_t)B * sizeof(atap_tag));
+    c.run([&] { return sr_noise_atap_batch_dev(h, d_pcm, U, B, n_len, d_atap); });
+    return c.finish();
 }
 
 int sr_vad_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t buf_len, const atap_tag *atap,
                  uint32_t *seg_off) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && atap && seg_off)));
     if (B == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->pcm, (size_t)B * U * 2 + 16));
-    SR_CK(h, ensure(h->atap, (size_t)B * sizeof(atap_tag)));
-    SR_CK(h, ensure(h->seg, (size_t)B * 24));
-    H2D(h, h->pcm.p, pcm, (size_t)B * U * 2);
-    H2D(h, h->atap.p, atap, (size_t)B * sizeof(atap_tag));
-    int rc = sr_vad_batch_dev(h, static_cast<const u16 *>(h->pcm.p), U, B, buf_len, static_cast<const atap_tag *>(h->atap.p),
-                              static_cast<u32 *>(h->seg.p));
-    if (rc) return rc;
-    D2H(h, seg_off, h->seg.p, (size_t)B * 24);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_vad_batch");
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    const atap_tag *d_atap = c.in(h->atap, atap, (size_t)B * sizeof(atap_tag));
+    u32 *d_seg = c.out(h->seg, seg_off, (size_t)B * 24);
+    c.run([&] { return sr_vad_batch_dev(h, d_pcm, U, B, buf_len, d_atap, d_seg); });
+    return c.finish();
 }
 
 int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *seg, uint32_t seg_stride,
@@ -456,43 +543,21 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
     SR_REQUIRE(h, h && (B == 0 || (pcm && seg && atap && ftr)));
     SR_REQUIRE(h, seg_stride >= 2);
     if (B == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->pcm, (size_t)B * U * 2 + 16));
-    SR_CK(h, ensure(h->atap, (size_t)B * sizeof(atap_tag)));
-    SR_CK(h, ensure(h->seg, (size_t)B * seg_stride * 4));
-    SR_CK(h, ensure(h->ftr, (size_t)B * kFtrBytes));
-    H2D(h, h->pcm.p, pcm, (size_t)B * U * 2);
-    H2D(h, h->atap.p, atap, (size_t)B * sizeof(atap_tag));
-    H2D(h, h->seg.p, seg, (size_t)B * seg_stride * 4);
-    int rc = sr_mfcc_batch_dev(h, static_cast<const u16 *>(h->pcm.p), U, B, static_cast<const u32 *>(h->seg.p), seg_stride,
-                               static_cast<const atap_tag *>(h->atap.p), static_cast<v_ftr_tag *>(h->ftr.p));
-    if (rc) return rc;
-    SR_CK(h, ftr_to_host(h, ftr, h->ftr.p, B));
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_mfcc_batch");
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    const atap_tag *d_atap = c.in(h->atap, atap, (size_t)B * sizeof(atap_tag));
+    const u32 *d_seg = c.in(h->seg, seg, (size_t)B * seg_stride * 4);
+    v_ftr_tag *d_ftr = c.out(h->ftr, ftr, (size_t)B * kFtrBytes);
+    c.run([&] { return sr_mfcc_batch_dev(h, d_pcm, U, B, d_seg, seg_stride, d_atap, d_ftr); });
+    return c.finish();
 }
 
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                  uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h && (B == 0 || in));
     if (B == 0) return 0;
-    DeviceGuard g(h->device);
-    const size_t T = h->n_slot;
-    SR_CK(h, ensure(h->ftr, (size_t)B * kFtrBytes));
-    if (score) SR_CK(h, ensure(h->score, (size_t)B * T * 4 + 4));
-    SR_CK(h, ensure(h->bidx, (size_t)B * 4));
-    SR_CK(h, ensure(h->bdis, (size_t)B * 4));
-    H2D(h, h->ftr.p, in, (size_t)B * kFtrBytes);
-    int rc = dtw_dev_impl(h, static_cast<const v_ftr_tag *>(h->ftr.p), B, flags, band_r,
-                          score ? static_cast<u32 *>(h->score.p) : nullptr,
-                          best_idx ? static_cast<u32 *>(h->bidx.p) : nullptr,
-                          best_dis ? static_cast<u32 *>(h->bdis.p) : nullptr, nullptr, nullptr);
-    if (rc) return rc;
-    if (score && T) D2H(h, score, h->score.p, (size_t)B * T * 4);
-    if (best_idx) D2H(h, best_idx, h->bidx.p, (size_t)B * 4);
-    if (best_dis) D2H(h, best_dis, h->bdis.p, (size_t)B * 4);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_dtw_batch");
+    return dtw_host(c, h->bank, in, B, flags, band_r, score, best_idx, best_dis);
 }
 
 int sr_set_transport(sr_handle *h, int mode) {
@@ -518,15 +583,11 @@ uint32_t sr_debug_pack12_host(int variant, const uint16_t *src, uint64_t n, uint
 int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t *out) {
     SR_REQUIRE(h, h && packed && out && !(n & 1));
     if (n == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->misc0, (size_t)(n / 2 * 3) + 64));
-    SR_CK(h, ensure(h->misc1, (size_t)n * 2 + 64));
-    H2D(h, h->misc0.p, packed, (size_t)(n / 2 * 3));
-    SR_CK(h, launch_unpack12(h->misc0.p, n, static_cast<u16 *>(h->misc1.p), h->stream));
-    ++h->launches;
-    D2H(h, out, h->misc1.p, (size_t)n * 2);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_debug_unpack12");
+    const u8 *d_packed = c.in(h->scratch[0], packed, (size_t)(n / 2 * 3), 64);
+    u16 *d_out = c.out(h->scratch[1], out, (size_t)n * 2, 64);
+    c.launch(TAG_NONE, "launch_unpack12", [&] { return launch_unpack12(d_packed, n, d_out, h->stream); });
+    return c.finish();
 }
 
 // Host-buffer spch_recg for B utterances. Large batches are processed in chunks through two device PCM
@@ -536,28 +597,26 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
     SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
     if (B == 0) return 0;
-    DeviceGuard g(h->device);
+    HostCall c(h, "sr_recognise_batch");
     // chunk: ~32 MB of PCM, a multiple of 8 utterances (keeps every chunk base 16-byte aligned)
     uint32_t chunk = (uint32_t)(((size_t)32 << 20) / ((size_t)U * 2));
     chunk = chunk < 8 ? 8 : (chunk & ~7u);
     if (chunk > B) chunk = B;
     const uint32_t nchunks = (B + chunk - 1) / chunk;
     const size_t chunk_bytes = (((size_t)chunk * U * 2 + 255) / 256) * 256;
-    SR_CK(h, ensure(h->pcm, (nchunks > 1 ? 2 : 1) * chunk_bytes + 16));
+    c.ws(h->pcm, (nchunks > 1 ? 2 : 1) * chunk_bytes + 16);
     sr_recog_out d;                                     // device mirrors of the non-NULL outputs
     memset(&d, 0, sizeof d);
-    cudaError_t e = cudaSuccess;
     for_each_output(h, [&](auto m, DevBuf &buf, size_t bytes) {
-        if (o->*m && e == cudaSuccess && (e = ensure(buf, B * bytes)) == cudaSuccess)
-            d.*m = static_cast<std::remove_reference_t<decltype(d.*m)>>(buf.p);
+        if (!(o->*m)) return;
+        // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36)
+        if constexpr (std::is_same_v<decltype(m), atap_tag *sr_recog_out::*>) c.in(buf, o->*m, B * bytes);
+        d.*m = c.out(buf, o->*m, B * bytes);
     });
-    if (e != cudaSuccess) return fail(h, "sr_recognise_batch: output buffers", e);
-    // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36)
-    if (o->atap) H2D(h, d.atap, o->atap, (size_t)B * sizeof(atap_tag));
     uint32_t issued = 0;
     // one chunk: H2D (plain u16, or 12-bit packed + expansion on the device) -> kernels on its slice of the outputs
-    auto step = [&](uint32_t c, int buf, const void *packed_src) -> int {
-        const uint32_t b0 = c * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
+    auto step = [&](uint32_t ci, int buf, const void *packed_src) -> int {
+        const uint32_t b0 = ci * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
         const size_t ns = (size_t)nb * U;
         u16 *dpcm = reinterpret_cast<u16 *>(static_cast<unsigned char *>(h->pcm.p) + (size_t)buf * chunk_bytes);
         cudaStream_t cs = nchunks > 1 ? h->copy_stream : h->stream;
@@ -568,26 +627,17 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
             SR_CK(h, cudaEventRecord(h->ev_h2d[buf], cs));
             SR_CK(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[buf], 0));
         }
-        if (packed_src) {
-            SR_CK(h, launch_unpack12(h->transport.device_stage(buf), ns, dpcm, h->stream));
-            ++h->launches;
-        }
+        if (packed_src) SR_LAUNCH(h, TAG_NONE, launch_unpack12(h->transport.device_stage(buf), ns, dpcm, h->stream));
         const sr_recog_out dc = recog_slice(h, d, b0);
         if (const int rc = sr_recognise_batch_dev(h, dpcm, U, nb, n_len, &dc)) return rc;
         if (nchunks > 1) SR_CK(h, cudaEventRecord(h->ev_done[buf], h->stream));
         ++issued;
         return 0;
     };
-    if (const int rc = h->transport.send(h, pcm, U, B, chunk, step)) return rc;
-    for_each_output(h, [&](auto m, DevBuf &, size_t bytes) {
-        if (!(o->*m) || !bytes || e != cudaSuccess) return;
-        if constexpr (std::is_same_v<decltype(m), v_ftr_tag *sr_recog_out::*>) e = ftr_to_host(h, o->ftr, d.ftr, B);
-        else e = cudaMemcpyAsync(o->*m, d.*m, B * bytes, cudaMemcpyDeviceToHost, h->stream);
-    });
-    if (e != cudaSuccess) return fail(h, "sr_recognise_batch: copy back", e);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    h->transport.call_done((uint64_t)B * U * 2);
-    return 0;
+    c.run([&] { return h->transport.send(h, pcm, U, B, chunk, step); });
+    const int rc = c.finish();
+    if (rc == 0) h->transport.call_done((uint64_t)B * U * 2);
+    return rc;
 }
 
 // save_mdl (main.c:121-138) for B utterances: noise_atap -> VAD -> get_mfcc(seg 0) -> save_ftr_mdl into slot b of a
@@ -598,23 +648,17 @@ int sr_enrol_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, ui
     SR_REQUIRE(h, h && (B == 0 || (pcm && bank_out)));
     SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0);
     if (B == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->pcm, (size_t)B * U * 2 + 16));
-    SR_CK(h, ensure(h->atap, (size_t)B * sizeof(atap_tag)));
-    SR_CK(h, ensure(h->seg, (size_t)B * 24));
-    SR_CK(h, ensure(h->ftr, (size_t)B * kFtrBytes));
-    SR_CK(h, ensure(h->status, (size_t)B));
-    SR_CK(h, ensure(h->misc0, (size_t)B * slot_stride));
-    H2D(h, h->pcm.p, pcm, (size_t)B * U * 2);
-    SR_CK(h, cudaMemsetAsync(h->atap.p, 0, (size_t)B * sizeof(atap_tag), h->stream));
-    if (const int rc = front_end(h, static_cast<const u16 *>(h->pcm.p), U, B, n_len, static_cast<atap_tag *>(h->atap.p),
-                                 static_cast<u32 *>(h->seg.p), h->ftr.p, static_cast<u8 *>(h->status.p))) return rc;
-    SR_CK(h, launch_pack_slots(h->ftr.p, static_cast<const u8 *>(h->status.p), B, h->misc0.p, slot_stride, h->stream));
-    ++h->launches;
-    D2H(h, bank_out, h->misc0.p, (size_t)B * slot_stride);
-    if (status) D2H(h, status, h->status.p, (size_t)B);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_enrol_batch");
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    atap_tag *d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
+    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
+    void *d_ftr = c.ws(h->ftr, (size_t)B * kFtrBytes);
+    u8 *d_status = c.out(h->status, status, (size_t)B);
+    void *d_bank = c.out(h->scratch[0], bank_out, (size_t)B * slot_stride);
+    c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
+    c.run([&] { return front_end(h, d_pcm, U, B, n_len, d_atap, d_seg, d_ftr, d_status); });
+    c.launch(TAG_NONE, "launch_pack_slots", [&] { return launch_pack_slots(d_ftr, d_status, B, d_bank, slot_stride, h->stream); });
+    return c.finish();
 }
 
 // get_mdl (DTW.C:217-296) for n pairs: mdl[p] = average of in1[p], in2[p] along their greedy DTW path; dis[p] = the
@@ -622,21 +666,14 @@ int sr_enrol_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, ui
 int sr_get_mdl_batch(sr_handle *h, const v_ftr_tag *in1, const v_ftr_tag *in2, uint32_t n, v_ftr_tag *mdl, uint32_t *dis) {
     SR_REQUIRE(h, h && (n == 0 || (in1 && in2 && mdl)));
     if (n == 0) return 0;
-    DeviceGuard g(h->device);
+    HostCall c(h, "sr_get_mdl_batch");
     const size_t bytes = (size_t)n * kFtrBytes;
-    SR_CK(h, ensure(h->misc0, bytes));
-    SR_CK(h, ensure(h->misc1, bytes));
-    SR_CK(h, ensure(h->ftr, bytes));
-    SR_CK(h, ensure(h->bdis, (size_t)n * 4));
-    H2D(h, h->misc0.p, in1, bytes);
-    H2D(h, h->misc1.p, in2, bytes);
-    H2D(h, h->ftr.p, mdl, bytes);                                   // rejected pairs leave mdl as the caller passed it
-    SR_CK(h, launch_get_mdl(h->misc0.p, h->misc1.p, h->ftr.p, n, static_cast<u32 *>(h->bdis.p), h->stream));
-    ++h->launches;
-    SR_CK(h, ftr_to_host(h, mdl, h->ftr.p, n));
-    if (dis) D2H(h, dis, h->bdis.p, (size_t)n * 4);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    const v_ftr_tag *d_in1 = c.in(h->scratch[0], in1, bytes), *d_in2 = c.in(h->scratch[1], in2, bytes);
+    v_ftr_tag *d_mdl = c.in(h->ftr, mdl, bytes);                    // rejected pairs leave mdl as the caller passed it
+    c.out(h->ftr, mdl, bytes);
+    u32 *d_dis = c.out(h->bdis, dis, (size_t)n * 4);
+    c.launch(TAG_NONE, "launch_get_mdl", [&] { return launch_get_mdl(d_in1, d_in2, d_mdl, n, d_dis, h->stream); });
+    return c.finish();
 }
 
 // One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]
@@ -648,7 +685,7 @@ int sr_recognise_batch_multi(sr_handle *const *handles, uint32_t n_handles, cons
                              uint32_t n_len, const sr_recog_out *o) {
     if (!handles || n_handles == 0 || !o) return fail(nullptr, "sr_recognise_batch_multi: bad arguments", cudaSuccess);
     for (uint32_t g = 0; g < n_handles; ++g)
-        if (!handles[g] || handles[g]->n_slot != handles[0]->n_slot) return fail(nullptr, "sr_recognise_batch_multi: handles differ", cudaSuccess);
+        if (!handles[g] || handles[g]->bank.n != handles[0]->bank.n) return fail(nullptr, "sr_recognise_batch_multi: handles differ", cudaSuccess);
     std::vector<int> rc(n_handles, 0);
     std::vector<std::thread> th;
     for (uint32_t g = 0; g < n_handles; ++g) {
@@ -665,15 +702,8 @@ int sr_fft_mag_batch(sr_handle *h, const int16_t *frames, uint32_t len, uint32_t
     SR_REQUIRE(h, h && (n == 0 || (frames && mag)));
     SR_REQUIRE(h, len <= SR_FFT_POINT);                                   // MFCC.C:32-35
     if (n == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->misc0, (size_t)n * len * 2 + 16));
-    SR_CK(h, ensure(h->misc1, (size_t)n * 512 * 4));
-    if (len) H2D(h, h->misc0.p, frames, (size_t)n * len * 2);
-    SR_CK(h, launch_fft_generic(nullptr, static_cast<const s16 *>(h->misc0.p), len, n, nullptr, static_cast<u32 *>(h->misc1.p), h->stream));
-    ++h->launches;
-    D2H(h, mag, h->misc1.p, (size_t)n * 512 * 4);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_fft_mag_batch");
+    return fft_host(c, nullptr, frames, len, n, nullptr, mag);
 }
 
 // dtw_limit (DTW.C:76-109) for n points, explicit (I, M) per point instead of the reference's file statics
@@ -681,90 +711,74 @@ int sr_dtw_limit_batch(sr_handle *h, const uint16_t *x, const uint16_t *y, const
                        uint8_t *out) {
     SR_REQUIRE(h, h && (n == 0 || (x && y && I && M && out)));
     if (n == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->misc0, (size_t)n * 8 + 16));
-    SR_CK(h, ensure(h->misc2, (size_t)n + 16));
-    u16 *d = static_cast<u16 *>(h->misc0.p);
-    H2D(h, d, x, (size_t)n * 2); H2D(h, d + n, y, (size_t)n * 2); H2D(h, d + 2 * (size_t)n, I, (size_t)n * 2); H2D(h, d + 3 * (size_t)n, M, (size_t)n * 2);
-    SR_CK(h, launch_dtw_limit(d, d + n, d + 2 * (size_t)n, d + 3 * (size_t)n, n, static_cast<u8 *>(h->misc2.p), h->stream));
-    ++h->launches;
-    D2H(h, out, h->misc2.p, (size_t)n);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_dtw_limit_batch");
+    u16 *d = c.ws<u16>(h->scratch[0], (size_t)n * 8 + 16);          // x | y | I | M
+    const uint16_t *src[4] = {x, y, I, M};
+    for (int k = 0; k < 4; ++k) c.h2d(d + k * (size_t)n, src[k], (size_t)n * 2);
+    u8 *d_out = c.out(h->scratch[2], out, (size_t)n, 16);
+    c.launch(TAG_NONE, "launch_dtw_limit", [&] { return launch_dtw_limit(d, d + n, d + 2 * (size_t)n, d + 3 * (size_t)n, n, d_out, h->stream); });
+    return c.finish();
 }
 
 // raw FFT of packed (re | im<<16) 1024-point inputs -- test hook for the asm restatement parity
 int sr_fft_raw_batch(sr_handle *h, const uint32_t *in_packed, uint32_t n, uint32_t *out_packed) {
     SR_REQUIRE(h, h && (n == 0 || (in_packed && out_packed)));
     if (n == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->misc0, (size_t)n * 4096));
-    SR_CK(h, ensure(h->misc1, (size_t)n * 4096));
-    H2D(h, h->misc0.p, in_packed, (size_t)n * 4096);
-    SR_CK(h, launch_fft_generic(static_cast<const u32 *>(h->misc0.p), nullptr, 0, n, static_cast<u32 *>(h->misc1.p), nullptr, h->stream));
-    ++h->launches;
-    D2H(h, out_packed, h->misc1.p, (size_t)n * 4096);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_fft_raw_batch");
+    return fft_host(c, in_packed, nullptr, 0, n, out_packed, nullptr);
 }
 
 int sr_get_dis_batch(sr_handle *h, const int16_t *a, const int16_t *b, uint32_t n, uint32_t *dis) {
     SR_REQUIRE(h, h && (n == 0 || (a && b && dis)));
     if (n == 0) return 0;
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->misc0, (size_t)n * 24));
-    SR_CK(h, ensure(h->misc1, (size_t)n * 24));
-    SR_CK(h, ensure(h->misc2, (size_t)n * 4));
-    H2D(h, h->misc0.p, a, (size_t)n * 24);
-    H2D(h, h->misc1.p, b, (size_t)n * 24);
-    SR_CK(h, launch_get_dis(static_cast<const s16 *>(h->misc0.p), static_cast<const s16 *>(h->misc1.p), n, static_cast<u32 *>(h->misc2.p), h->stream));
-    ++h->launches;
-    D2H(h, dis, h->misc2.p, (size_t)n * 4);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_get_dis_batch");
+    const s16 *d_a = c.in(h->scratch[0], a, (size_t)n * 24), *d_b = c.in(h->scratch[1], b, (size_t)n * 24);
+    u32 *d_dis = c.out(h->scratch[2], dis, (size_t)n * 4);
+    c.launch(TAG_NONE, "launch_get_dis", [&] { return launch_get_dis(d_a, d_b, n, d_dis, h->stream); });
+    return c.finish();
 }
 
 // test hook: number of float bit patterns in [lo_bits, hi_bits) for which the branch-free sqrt differs from
 // the IEEE intrinsic (must be 0 over [1.0f, 2^33) = the range the kernels feed it)
 int sr_debug_sqrt_mismatches(sr_handle *h, uint32_t lo_bits, uint32_t hi_bits, uint64_t *mismatches) {
     SR_REQUIRE(h, h && mismatches);
-    DeviceGuard g(h->device);
-    SR_CK(h, ensure(h->misc2, 16));
-    SR_CK(h, cudaMemsetAsync(h->misc2.p, 0, 8, h->stream));
-    SR_CK(h, launch_sqrt_check(lo_bits, hi_bits, static_cast<unsigned long long *>(h->misc2.p), h->stream));
-    D2H(h, mismatches, h->misc2.p, 8);
-    SR_CK(h, cudaStreamSynchronize(h->stream));
-    return 0;
+    HostCall c(h, "sr_debug_sqrt_mismatches");
+    auto *bad = reinterpret_cast<unsigned long long *>(c.out(h->scratch[2], mismatches, 8, 8));
+    c.ck("cudaMemsetAsync", bad ? cudaMemsetAsync(bad, 0, 8, h->stream) : cudaSuccess);
+    c.launch(TAG_NONE, "launch_sqrt_check", [&] { return launch_sqrt_check(lo_bits, hi_bits, bad, h->stream); });
+    return c.finish();
 }
+
+}  // extern "C"
 
 // ---- (1) the reference's own entry points: batch-of-1 on a lazily created default handle -----------
 static std::mutex g_default_mu;
 static sr_handle *g_default = nullptr;
-static sr_handle *default_handle() {
+
+// f(default handle) under the default handle's lock, created on first use; `none` when there is no device
+template <class R, class F> static R on_default_handle(R none, F f) {
+    std::lock_guard<std::mutex> lk(g_default_mu);
     if (!g_default) {
         sr_handle *h = nullptr;
         if (sr_create(0, &h) == 0) g_default = h;
     }
-    return g_default;
+    return g_default ? f(g_default) : none;
 }
+
+extern "C" {
 
 // VAD.H:24 / VAD.C:22-71. On failure (no device) *atap is left untouched and sr_last_error(NULL) is set.
 void noise_atap(const uint16_t *noise, uint16_t n_len, atap_tag *atap) {
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    if (!h || !noise || !atap) return;
-    if (n_len == 0) return;
-    sr_noise_atap_batch(h, noise, n_len, 1, n_len, atap);
+    on_default_handle(0, [&](sr_handle *h) { return noise && atap && n_len ? sr_noise_atap_batch(h, noise, n_len, 1, n_len, atap) : 0; });
 }
 
 // VAD.H:25 / VAD.C:97-218. Segments come back as pointers into the caller's buffer.
 void VAD(const uint16_t *vc, uint16_t buf_len, valid_tag *valid_voice, atap_tag *atap_arg) {
     if (valid_voice) for (unsigned i = 0; i < SR_MAX_VC_CON; ++i) { valid_voice[i].start = nullptr; valid_voice[i].end = nullptr; }   // VAD.C:115-119
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    if (!h || !vc || !valid_voice || !atap_arg || buf_len == 0) return;
     uint32_t seg[6];
-    if (sr_vad_batch(h, vc, buf_len, 1, buf_len, atap_arg, seg) != 0) return;
+    if (on_default_handle(-1, [&](sr_handle *h) {
+            return vc && valid_voice && atap_arg && buf_len ? sr_vad_batch(h, vc, buf_len, 1, buf_len, atap_arg, seg) : -1;
+        }) != 0) return;
     for (unsigned i = 0; i < SR_MAX_VC_CON; ++i) {
         valid_voice[i].start = seg[2 * i] == SR_SEG_NULL ? nullptr : const_cast<uint16_t *>(vc) + seg[2 * i];
         valid_voice[i].end = seg[2 * i + 1] == SR_SEG_NULL ? nullptr : const_cast<uint16_t *>(vc) + seg[2 * i + 1];
@@ -774,16 +788,15 @@ void VAD(const uint16_t *vc, uint16_t buf_len, valid_tag *valid_voice, atap_tag 
 // MFCC.H:27 / MFCC.C:86-191. Like the reference this reads valid->start[-1] (MFCC.C:119, i=0).
 void get_mfcc(valid_tag *valid, v_ftr_tag *v_ftr, atap_tag *atap_arg) {
     if (!v_ftr) return;
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    if (!h || !valid || !atap_arg || !valid->start || !valid->end || valid->end < valid->start) { v_ftr->frm_num = 0; return; }
-    size_t len = (size_t)(valid->end - valid->start);
-    // more than vv_frm_max frames is rejected by the kernel (MFCC.C:103-107); cap what is shipped to the device
-    const size_t cap = 120 * 80 + 80;
-    if (len > cap) len = cap;
-    const uint32_t U = (uint32_t)len + 1;
-    const uint32_t seg[2] = {1u, U};
-    if (sr_mfcc_batch(h, valid->start - 1, U, 1, seg, 2, atap_arg, v_ftr) != 0) v_ftr->frm_num = 0;
+    const int rc = on_default_handle(-1, [&](sr_handle *h) {
+        if (!valid || !atap_arg || !valid->start || !valid->end || valid->end < valid->start) return -1;
+        // more than vv_frm_max frames is rejected by the kernel (MFCC.C:103-107); cap what is shipped to the device
+        const size_t len = std::min((size_t)(valid->end - valid->start), (size_t)(120 * 80 + 80));
+        const uint32_t U = (uint32_t)len + 1;
+        const uint32_t seg[2] = {1u, U};
+        return sr_mfcc_batch(h, valid->start - 1, U, 1, seg, 2, atap_arg, v_ftr);
+    });
+    if (rc != 0) v_ftr->frm_num = 0;
 }
 
 // the reference keeps in_frm_num / mdl_frm_num of the last dtw() call in file statics (DTW.C:65-68, set at :130-131);
@@ -792,31 +805,22 @@ static thread_local uint16_t g_last_I = 0, g_last_M = 0;
 
 // DTW.C:76-109 (global, no header): 0 = "ins", 1 = "outs", for the (I, M) of this thread's last dtw() call
 uint8_t dtw_limit(uint16_t x, uint16_t y) {
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    uint8_t r = 1;
-    if (!h) return r;
-    if (sr_dtw_limit_batch(h, &x, &y, &g_last_I, &g_last_M, 1, &r) != 0) return 1;
-    return r;
+    return on_default_handle<uint8_t>(1, [&](sr_handle *h) -> uint8_t {
+        uint8_t r = 1;
+        return sr_dtw_limit_batch(h, &x, &y, &g_last_I, &g_last_M, 1, &r) == 0 ? r : 1;
+    });
 }
 
-// DTW.H:7 / DTW.C:120-192
+// DTW.H:7 / DTW.C:120-192: the scan of sr_dtw_batch against a one-slot bank holding frt_mdl
 uint32_t dtw(v_ftr_tag *ftr_in, v_ftr_tag *frt_mdl) {
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    if (!h || !ftr_in || !frt_mdl) return SR_DIS_ERR;
-    g_last_I = ftr_in->frm_num; g_last_M = frt_mdl->frm_num;                  // DTW.C:130-131
-    const void *sv_bank = h->bank; const u32 sv_n = h->n_slot, sv_s = h->slot_stride;
-    const u32 *sv_perm = h->perm;
-    uint32_t score = SR_DIS_ERR;
-    DeviceGuard g(h->device);
-    if (ensure(h->misc2, kFtrBytes + 16) != cudaSuccess) return SR_DIS_ERR;
-    if (cudaMemcpyAsync(h->misc2.p, frt_mdl, kFtrBytes, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return SR_DIS_ERR;
-    h->bank = h->misc2.p; h->n_slot = 1; h->slot_stride = kFtrBytes;
-    h->perm = nullptr;                                              // the slot order belongs to the handle's real bank
-    const int rc = sr_dtw_batch(h, ftr_in, 1, 0, 0, &score, nullptr, nullptr);
-    h->bank = sv_bank; h->n_slot = sv_n; h->slot_stride = sv_s; h->perm = sv_perm;
-    return rc == 0 ? score : SR_DIS_ERR;
+    return on_default_handle<uint32_t>(SR_DIS_ERR, [&](sr_handle *h) -> uint32_t {
+        if (!ftr_in || !frt_mdl) return SR_DIS_ERR;
+        g_last_I = ftr_in->frm_num; g_last_M = frt_mdl->frm_num;                  // DTW.C:130-131
+        uint32_t score = SR_DIS_ERR;
+        HostCall c(h, "dtw");
+        const BankView one = {c.in(h->scratch[2], frt_mdl, kFtrBytes, 16), 1, (u32)kFtrBytes, nullptr};
+        return dtw_host(c, one, ftr_in, 1, 0, 0, &score, nullptr, nullptr) == 0 ? score : SR_DIS_ERR;
+    });
 }
 
 // MFCC.C:27-62: returns a pointer to a buffer owned by the library (thread-local instead of the
@@ -824,29 +828,18 @@ uint32_t dtw(v_ftr_tag *ftr_in, v_ftr_tag *frt_mdl) {
 uint32_t *fft(int16_t *dat_buf, uint16_t buf_len) {
     static thread_local uint32_t out[SR_FFT_POINT];
     if (buf_len > SR_FFT_POINT || !dat_buf) return nullptr;          // MFCC.C:32-35
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    if (!h) return nullptr;
-    DeviceGuard g(h->device);
-    if (ensure(h->misc0, 4096) != cudaSuccess || ensure(h->misc1, 4096) != cudaSuccess || ensure(h->misc2, 2048) != cudaSuccess) return nullptr;
-    if (buf_len && cudaMemcpyAsync(h->misc0.p, dat_buf, (size_t)buf_len * 2, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) return nullptr;
-    if (launch_fft_generic(nullptr, static_cast<const s16 *>(h->misc0.p), buf_len, 1, static_cast<u32 *>(h->misc1.p),
-                           static_cast<u32 *>(h->misc2.p), h->stream) != cudaSuccess) return nullptr;
-    ++h->launches;
-    if (cudaMemcpyAsync(out, h->misc2.p, 2048, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) return nullptr;
-    if (cudaMemcpyAsync(out + 512, static_cast<u32 *>(h->misc1.p) + 512, 2048, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) return nullptr;
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) return nullptr;
-    return out;
+    return on_default_handle<uint32_t *>(nullptr, [&](sr_handle *h) -> uint32_t * {
+        HostCall c(h, "fft");                                        // all raw bins, then the magnitudes over [0, 512)
+        return fft_host(c, nullptr, dat_buf, buf_len, 1, out, out) == 0 ? out : nullptr;
+    });
 }
 
 // DTW.C:45-62
 uint32_t get_dis(int16_t *frm_ftr1, int16_t *frm_ftr2) {
-    std::lock_guard<std::mutex> lk(g_default_mu);
-    sr_handle *h = default_handle();
-    if (!h || !frm_ftr1 || !frm_ftr2) return SR_DIS_ERR;
-    uint32_t d = SR_DIS_ERR;
-    if (sr_get_dis_batch(h, frm_ftr1, frm_ftr2, 1, &d) != 0) return SR_DIS_ERR;
-    return d;
+    return on_default_handle<uint32_t>(SR_DIS_ERR, [&](sr_handle *h) -> uint32_t {
+        uint32_t d = SR_DIS_ERR;
+        return frm_ftr1 && frm_ftr2 && sr_get_dis_batch(h, frm_ftr1, frm_ftr2, 1, &d) == 0 ? d : SR_DIS_ERR;
+    });
 }
 
 }  // extern "C"

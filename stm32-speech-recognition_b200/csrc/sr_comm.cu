@@ -221,7 +221,7 @@ int sr_recognise_batch_dev_allgather(sr_handle *h, const uint16_t *pcm, uint32_t
     if (rc) return rc;
     if (!gathered_score && !gathered_best) return 0;
     const void *keys = h->best_sel ? h->best_alt.p : h->best.p;     // the buffer this call's template scan just filled
-    return allgather2(h, gathered_score ? o.score : nullptr, gathered_score, gathered_score ? (size_t)B * h->n_slot * 4 : 0,
+    return allgather2(h, gathered_score ? o.score : nullptr, gathered_score, gathered_score ? (size_t)B * h->bank.n * 4 : 0,
                       gathered_best ? keys : nullptr, gathered_best, gathered_best ? (size_t)B * 8 : 0, o.score);
 }
 

@@ -113,6 +113,13 @@ private:
     int send_packed(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t chunk, const Step &step);
 };
 
+// a template bank on the device: n flash-layout slots of `stride` bytes at p, walked in `order` (NULL: slot order)
+struct BankView {
+    const void *p = nullptr;
+    u32 n = 0, stride = 0;
+    const u32 *order = nullptr;
+};
+
 struct sr_handle {
     int device = 0;
     int num_sms = 132;
@@ -122,14 +129,11 @@ struct sr_handle {
     cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
     uint64_t launches = 0;
     std::string err;
-    // template bank
-    const void *bank = nullptr;
-    DevBuf bank_own;
-    u32 n_slot = 0, slot_stride = 0;
-    // bank slots in ascending frm_num order (only for banks wider than one 32-template tile): an ordering hint for the
-    // greedy dtw kernels, recomputed when the bank pointer / geometry changes; correctness never depends on it
-    DevBuf bank_perm;
-    const u32 *perm = nullptr;
+    // template bank (sr_set_bank*). Its order lists the slots in ascending frm_num order (only for banks wider than one
+    // 32-template tile): a hint for the greedy dtw kernels, recomputed when the bank pointer / geometry changes;
+    // correctness never depends on it
+    BankView bank;
+    DevBuf bank_own, bank_perm;
     const void *perm_bank = nullptr;
     u32 perm_n = 0, perm_stride = 0;
     // optional per-kernel timing (sr_timing_enable): event pairs recorded around every launch
@@ -148,8 +152,9 @@ struct sr_handle {
     DevBuf dtw_scratch;                                // one word: max frm_num of the current inputs (dynamic kernel's slot size)
     int geom = 0;                                      // SR_GEOM_REF (160/80/1024) or SR_GEOM_B (200/80/256, extension)
     int numa_node = -1;                                // node the device hangs off (-1 unknown / single node)
-    // grow-only device workspaces
-    DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, misc0, misc1, misc2;
+    // grow-only device workspaces; scratch[] serves the secondary entry points (FFT, get_dis, get_mdl, dtw_limit, the
+    // 12-bit expander, the sqrt check, enrol's bank image, dtw()'s one-slot bank) and is never read by a recognise call
+    DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };
@@ -205,12 +210,12 @@ inline u32 *vad_work(sr_handle *h) {
     return static_cast<u32 *>(h->vad_work.p);
 }
 
-// greedy dtw of B inputs against the handle's bank with the handle's kernel variant
+// greedy dtw of B inputs against `bank` with the handle's kernel variant
 #ifndef SR_DTW_VARIANT_DEFAULT
 #define SR_DTW_VARIANT_DEFAULT 0
 #endif
-inline cudaError_t launch_dtw_h(sr_handle *h, const void *in_ftr, u32 B, u32 flags, u32 *score, u64 *best, const u8 *status,
-                                const u32 *B_dev = nullptr) {
+inline cudaError_t launch_dtw_h(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, u32 *score, u64 *best,
+                                const u8 *status, const u32 *B_dev = nullptr) {
     int v = h->dtw_variant;
     if (v < 0) {
         static const int env_v = [] { const char *e = getenv("SR_DTW_VARIANT"); return e && *e ? atoi(e) : SR_DTW_VARIANT_DEFAULT; }();
@@ -219,33 +224,15 @@ inline cudaError_t launch_dtw_h(sr_handle *h, const void *in_ftr, u32 B, u32 fla
     if (v == 1) {
         cudaError_t e = ensure(h->dtw_scratch, 16);
         if (e != cudaSuccess) return e;
-        return launch_dtw_dyn(in_ftr, B, h->bank, h->n_slot, h->slot_stride, flags, score, best, status, h->num_sms, h->stream,
-                              static_cast<u32 *>(h->dtw_scratch.p), B_dev, h->perm);
+        return launch_dtw_dyn(in_ftr, B, bank.p, bank.n, bank.stride, flags, score, best, status, h->num_sms, h->stream,
+                              static_cast<u32 *>(h->dtw_scratch.p), B_dev, bank.order);
     }
-    return launch_dtw(in_ftr, B, h->bank, h->n_slot, h->slot_stride, flags, score, best, status, h->num_sms, h->stream, B_dev, h->perm);
+    return launch_dtw(in_ftr, B, bank.p, bank.n, bank.stride, flags, score, best, status, h->num_sms, h->stream, B_dev, bank.order);
 }
 
 int comm_wait_before_scan(sr_handle *h, const void *score);   // sr_comm.cu
 int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, const sr_recog_out *o,
                        bool wait_comm);             // sr_api.cu
-
-// records a (start,end) event pair around one kernel launch when timing is enabled
-struct TimedLaunch {
-    sr_handle *h;
-    size_t slot = (size_t)-1;
-    TimedLaunch(sr_handle *hh, uint32_t tag) : h(hh) {
-        if (h->timing && (h->ev_used + 1) * 2 <= h->ev.size()) {
-            slot = h->ev_used++;
-            h->ev_tag[slot] = tag;
-            cudaEventRecord(h->ev[2 * slot], h->stream);
-        }
-    }
-    ~TimedLaunch() {
-        if (slot != (size_t)-1) cudaEventRecord(h->ev[2 * slot + 1], h->stream);
-    }
-};
-enum { TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5, TAG_DTW_BAND = 6,
-       TAG_FFT = 7, TAG_GET_DIS = 8 };
 
 struct DeviceGuard {
     int prev = -1;
@@ -258,5 +245,4 @@ struct DeviceGuard {
 };
 
 
-#define H2D(h, dst, src, bytes) SR_CK(h, cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyHostToDevice, (h)->stream))
 #define D2H(h, dst, src, bytes) SR_CK(h, cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyDeviceToHost, (h)->stream))

@@ -355,15 +355,15 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     stream_status_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const unsigned char *>(p->ftr.p), n_ev, p->cap,
                                                    static_cast<u8 *>(p->status.p), static_cast<u32 *>(p->frm.p), best);
     SR_CK(h, cudaGetLastError());
-    if (h->n_slot)
-        SR_CK(h, launch_dtw_h(h, p->ftr.p, p->cap, SR_DTW_CHECK_SIGN, nullptr, best, static_cast<const u8 *>(p->status.p), n_ev));
+    if (h->bank.n)
+        SR_CK(h, launch_dtw_h(h, h->bank, p->ftr.p, p->cap, SR_DTW_CHECK_SIGN, nullptr, best, static_cast<const u8 *>(p->status.p), n_ev));
     u32 *out_count = static_cast<u32 *>(p->out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(p->out.p) + 16);
     stream_finish_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const StreamEventDev *>(p->ev.p), n_ev, p->cap,
                                                    static_cast<const u8 *>(p->status.p), static_cast<const u32 *>(p->frm.p),
                                                    best, out_rec, out_count);
     SR_CK(h, cudaGetLastError());
-    h->launches += 4 + (h->n_slot ? 1 : 0);
+    h->launches += 4 + (h->bank.n ? 1 : 0);
     const u32 quick = p->cap < sr_stream_pool::kQuick ? p->cap : sr_stream_pool::kQuick;
     D2H(h, p->out_host.p, p->out.p, 16 + (size_t)quick * sizeof(sr_stream_event));
     SR_CK(h, cudaStreamSynchronize(h->stream));                       // the one synchronisation of a push
