@@ -290,6 +290,10 @@ int sr_dtw_limit_batch(sr_handle *h, const uint16_t *x, const uint16_t *y, const
  * u32[n][1024]) -> packed outputs; exists so tests can pin the FFT kernel code against the asm restatement
  * on arbitrary complex data */
 int sr_fft_raw_batch(sr_handle *h, const uint32_t *in_packed, uint32_t n, uint32_t *out_packed);
+/* test hook: the radix-4 FFT device code the MFCC kernels share, alone, at N = 256 (the GEOM_B FFT) or N = 1024, on n
+ * packed N-point inputs (u32[n][N]) -> packed outputs; lets tests drive the 256-point FFT with complex, full-length
+ * data, which the GEOM_B front end never feeds it. N must be 256 or 1024. */
+int sr_debug_fft_raw_n(sr_handle *h, const uint32_t *in_packed, uint32_t N, uint32_t n, uint32_t *out_packed);
 
 /* test hook: count of float bit patterns in [lo_bits, hi_bits) where the kernels' branch-free sqrt differs
  * from the IEEE sqrt.rn.f32 (0 over [1.0f, 2^33), the range the path can produce) */

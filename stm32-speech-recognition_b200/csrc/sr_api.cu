@@ -738,6 +738,17 @@ int sr_get_dis_batch(sr_handle *h, const int16_t *a, const int16_t *b, uint32_t 
     return c.finish();
 }
 
+// test hook: the shared MFCC core's FFT alone at N = 256 (GEOM_B) or 1024, on n packed N-point inputs
+int sr_debug_fft_raw_n(sr_handle *h, const uint32_t *in_packed, uint32_t N, uint32_t n, uint32_t *out_packed) {
+    SR_REQUIRE(h, h && (N == 256 || N == 1024) && (n == 0 || (in_packed && out_packed)));
+    if (n == 0) return 0;
+    HostCall c(h, "sr_debug_fft_raw_n");
+    const u32 *d_in = c.in(h->scratch[0], in_packed, (size_t)n * N * 4);
+    u32 *d_out = c.out(h->scratch[1], out_packed, (size_t)n * N * 4);
+    c.launch(TAG_NONE, "launch_fft_raw_n", [&] { return launch_fft_raw_n(d_in, N, n, d_out, h->stream); });
+    return c.finish();
+}
+
 // test hook: number of float bit patterns in [lo_bits, hi_bits) for which the branch-free sqrt differs from
 // the IEEE intrinsic (must be 0 over [1.0f, 2^33) = the range the kernels feed it)
 int sr_debug_sqrt_mismatches(sr_handle *h, uint32_t lo_bits, uint32_t hi_bits, uint64_t *mismatches) {

@@ -24,6 +24,7 @@ cudaError_t launch_mfcc_geomb(const u16 *pcm, u32 U, u32 B, const u32 *seg, u32 
                               int num_sms, cudaStream_t st, const u32 *row_map = nullptr, const u32 *B_dev = nullptr);
 cudaError_t launch_fft_generic(const u32 *in_packed, const s16 *frames, u32 len, u32 n, u32 *raw_out, u32 *mag,
                                cudaStream_t st);
+cudaError_t launch_fft_raw_n(const u32 *in, u32 N, u32 n, u32 *out, cudaStream_t st);
 cudaError_t launch_dtw(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
                        u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev = nullptr,
                        const u32 *perm = nullptr);

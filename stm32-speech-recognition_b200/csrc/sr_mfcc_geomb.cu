@@ -7,7 +7,8 @@
 // Matlab/matlab仿真/speech_recog.m:217-313), the FFT is the radix-4 routine of cr4_fft_1024_stm32.s:95-281 with three
 // twiddled passes instead of four (the twiddle table is cumulative: its first 84 triples serve N = 256), and every
 // integer rule of MFCC.C (pre-emphasis 95/100, hamm/1000, sqrtf*10, u32 energies, tri/100, log*100, DCT/100 into an
-// s16) is kept. Its only checker is oracle/sr_oracle.c::sro_mfcc_geom_b.
+// s16) is kept. Its checker is oracle/sr_oracle.c::sro_mfcc_geom_b, whose FFT and tables tests/test_extension_refs.py
+// holds to the exact DFT and to the tables' float64 formulas.
 //
 // One CTA per utterance (persistent over the batch), one frame per warp. The FFT is the N = 256 instance of the shared
 // core's fft_radix4 (sr_mfcc_core.cuh), the device code the drop-in fft runs at N = 1024 (s16 wrap on every store kept:
@@ -93,6 +94,35 @@ cudaError_t launch_mfcc_geomb(const u16 *pcm, u32 U, u32 B, const u32 *seg, u32 
     if (grid > B) grid = B;
     mfcc_geomb_kernel<<<grid, kGbWarps * 32, 0, st>>>(pcm, U, B, seg, seg_stride, atap, static_cast<unsigned char *>(ftr), tab,
                                                      row_map, B_dev);
+    return cudaGetLastError();
+}
+
+// ---- test hook: the shared core's fft_radix4<N> alone, on n packed (re | im << 16) N-point inputs, one frame per warp.
+// At N = 256 it is the only way to drive the GEOM_B FFT with complex, full-length input (the front end feeds it real,
+// windowed 200-sample frames). Not part of recognition.
+template <int N>
+__global__ void __launch_bounds__(128)
+fft_raw_n_kernel(const u32 *__restrict__ in, u32 n, u32 *__restrict__ out, const DevTables *__restrict__ tab) {
+    __shared__ u32 xs[4][N];
+    __shared__ u32 ys[4][N];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const u32 fr = blockIdx.x * 4 + warp;
+    if (fr >= n) return;
+    u32 *x = xs[warp], *y = ys[warp];
+    for (int i = lane; i < N; i += 32) x[i] = in[(size_t)fr * N + i];
+    __syncwarp();
+    fft_radix4<N>(x, y, tab, lane);
+    for (int i = lane; i < N; i += 32) out[(size_t)fr * N + i] = y[i];
+}
+
+cudaError_t launch_fft_raw_n(const u32 *in, u32 N, u32 n, u32 *out, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const DevTables *tab = dev_tables();
+    if (!tab) return cudaErrorInitializationError;
+    const u32 grid = (n + 3) / 4;
+    if (N == 256) fft_raw_n_kernel<256><<<grid, 128, 0, st>>>(in, n, out, tab);
+    else if (N == 1024) fft_raw_n_kernel<1024><<<grid, 128, 0, st>>>(in, n, out, tab);
+    else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 

@@ -132,6 +132,7 @@ def lib():
         L.sr_recognise_batch_multi.argtypes = [C.POINTER(vp), u32, vp, u32, u32, u32, C.POINTER(RecogOut)]
         L.sr_fft_mag_batch.argtypes = [vp, vp, u32, u32, vp]
         L.sr_fft_raw_batch.argtypes = [vp, vp, u32, vp]
+        L.sr_debug_fft_raw_n.argtypes = [vp, vp, u32, u32, vp]
         L.sr_get_dis_batch.argtypes = [vp, vp, vp, u32, vp]
         L.sr_dtw_limit_batch.argtypes = [vp, vp, vp, vp, vp, u32, vp]
         L.dtw_limit.argtypes = [C.c_uint16, C.c_uint16]
@@ -306,6 +307,15 @@ class Handle:
         n = packed.shape[0]
         out = np.zeros((n, 1024), np.uint32)
         self._ck(lib().sr_fft_raw_batch(self._h, _p(packed), n, _p(out)))
+        return out
+
+    def fft_raw_n(self, packed, N):
+        """the MFCC kernels' shared FFT alone at N = 256 or 1024 (test hook): packed [n, N] -> packed [n, N]"""
+        packed = np.ascontiguousarray(packed, np.uint32)
+        n = packed.shape[0]
+        assert packed.shape == (n, N)
+        out = np.zeros((n, N), np.uint32)
+        self._ck(lib().sr_debug_fft_raw_n(self._h, _p(packed), N, n, _p(out)))
         return out
 
     def get_dis(self, a, b):

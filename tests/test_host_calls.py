@@ -92,6 +92,7 @@ def test_host_buffer_call_accounting(h, data):
     assert _account(h, lambda: h.get_mdl(ftr, f2)) == (1, [])
     assert _account(h, lambda: h.fft_mag(np.ones((B, 160), np.int16))) == (1, [])
     assert _account(h, lambda: h.fft_raw(np.ones((B, 1024), np.uint32))) == (1, [])
+    assert _account(h, lambda: h.fft_raw_n(np.ones((B, 256), np.uint32), 256)) == (1, [])
     rows = ftr["mfcc_dat"][:, :12].copy()
     assert _account(h, lambda: h.get_dis(rows, rows[::-1].copy())) == (1, [])
     v = np.arange(B, dtype=np.uint16)
@@ -165,6 +166,7 @@ def test_null_pointer_with_work_fails(h):
              ("sr_get_mdl_batch", (a, None, 1, a, a)), ("sr_get_mdl_batch", (a, a, 1, None, a)),
              ("sr_fft_mag_batch", (None, 160, 1, a)), ("sr_fft_mag_batch", (a, 160, 1, None)),
              ("sr_fft_raw_batch", (a, 1, None)), ("sr_get_dis_batch", (a, None, 1, a)),
+             ("sr_debug_fft_raw_n", (None, 256, 1, a)), ("sr_debug_fft_raw_n", (a, 1024, 1, None)),
              ("sr_dtw_limit_batch", (a, a, None, a, 1, a)), ("sr_debug_unpack12", (a, 2, None)),
              ("sr_debug_sqrt_mismatches", (0, 1, None)),
              ("sr_noise_atap_batch_dev", (None, U, 1, 2400, a)), ("sr_vad_batch_dev", (a, U, 1, U, a, None)),
@@ -184,6 +186,7 @@ def test_zero_size_calls_do_nothing(h):
              ("sr_recognise_batch", (None, U, 0, 2400, o)), ("sr_enrol_batch", (None, U, 0, 2400, None, 4096, None)),
              ("sr_get_mdl_batch", (None, None, 0, None, None)), ("sr_fft_mag_batch", (None, 160, 0, None)),
              ("sr_fft_raw_batch", (None, 0, None)), ("sr_get_dis_batch", (None, None, 0, None)),
+             ("sr_debug_fft_raw_n", (None, 256, 0, None)),
              ("sr_dtw_limit_batch", (None, None, None, None, 0, None)),
              ("sr_dtw_batch_dev", (None, 0, 0, 0, None, None, None)), ("sr_recognise_batch_dev", (None, U, 0, 2400, o)),
              # checks that come after the early return
@@ -219,6 +222,7 @@ def test_checks_before_the_zero_size_early_return(h):
              ("sr_enrol_batch", (None, U, 0, 2400, None, 2048, None)),              # slot_stride < sizeof(v_ftr_tag)
              ("sr_enrol_batch", (None, U, 0, 2400, None, 4098, None)),              # slot_stride % 4 != 0
              ("sr_fft_mag_batch", (None, 1025, 0, None)),                           # len > SR_FFT_POINT
+             ("sr_debug_fft_raw_n", (None, 512, 0, None)),                          # N not 256 or 1024
              ("sr_debug_unpack12", (None, 0, None)),                                # NULL even when n == 0
              ("sr_debug_unpack12", (a, 3, a))]                                      # odd n
     for fn, args in cases:

@@ -40,13 +40,21 @@ def test_twiddles_equal_reference_asm_table():
 
 
 def test_committed_header_is_current():
-    """sr_tables.h in the tree is what the generator produces now"""
+    """sr_tables.h in the tree is what the generator produces now, including the GEOM_B tables (kernel and oracle both read
+    the header, so a stale one would pass every parity test)"""
     path = os.path.join(ROOT, "stm32-speech-recognition_b200", "csrc", "sr_tables.h")
     text = open(path).read()
-    hamm = [int(x) for x in re.search(r"sr_tab_hamm\[160\] = \{([^}]*)\}", text).group(1).replace("\n", "").split(",") if x.strip()]
-    assert hamm == gen_tables.hamm_table()
-    tw = [int(x) for x in re.search(r"sr_tab_twiddle\[2040\] = \{([^}]*)\}", text).group(1).replace("\n", "").split(",") if x.strip()]
-    assert tw == gen_tables.twiddle_table()
+
+    def table(name, n):
+        return [int(x) for x in re.search(r"\b%s\[%d\] = \{([^}]*)\}" % (name, n), text).group(1).replace("\n", "").split(",")
+                if x.strip()]
+    assert table("sr_tab_hamm", 160) == gen_tables.hamm_table()
+    assert table("sr_tab_twiddle", 2040) == gen_tables.twiddle_table()
+    cen_b, odd_b, even_b = gen_tables.tri_tables(gen_tables.FRQ_MAX_B)
+    assert table("sr_tab_b_hamm", 200) == gen_tables.hamm_table(gen_tables.FRAME_LEN_B)
+    assert table("sr_tab_b_tri_cen", 24) == cen_b
+    assert table("sr_tab_b_tri_odd", 128) == odd_b
+    assert table("sr_tab_b_tri_even", 128) == even_b
 
 
 def test_log_threshold_table_matches_libm_expression():
