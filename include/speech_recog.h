@@ -157,11 +157,26 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
  * best_idx/best_dis follow main.c:276-291 (strict '<', first wins, start 0 / 0xFFFFFFFF). */
 #define SR_DTW_CHECK_SIGN 1u
 #define SR_DTW_BAND       2u          /* use the Sakoe-Chiba banded DP (extension, not in the reference) */
+/* With SR_DTW_BAND, band_r is any radius >= 0 (a negative one fails): D(i,j) = get_dis(i,j) + min(D(i-1,j), D(i,j-1),
+ * D(i-1,j-1)) over the band |j - floor(i*M/I)| <= band_r, score D(I-1,M-1) / (I+M), SR_DIS_ERR when that cell lies
+ * outside the band or the 2:1 length guard of DTW.C:133 rejects the pair. Every band_r >= 118 is the unconstrained DTW
+ * over the whole matrix (feature sets have <= 119 frames). Parity unpinned: the reference has no DP; the checker is this
+ * project's own CPU restatement. The explicit flags and band_r of sr_dtw_batch decide, never the handle's sr_set_match. */
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                  uint32_t *score /* [B][n_slot] or NULL */, uint32_t *best_idx /* [B] or NULL */,
                  uint32_t *best_dis /* [B] or NULL */);
+/* The matcher of this handle's recognition calls: sr_recognise_batch, _dev, _dev_allgather, _multi and every streaming
+ * push, each reading it when it starts. flags = 0: the reference's greedy walk (dtw, DTW.C:120-192), the default;
+ * flags = SR_DTW_BAND: the banded DP above at radius band_r >= 0 (up to the full matrix). Recognition keeps honouring
+ * save_sign (SR_DTW_CHECK_SIGN, main.c:283) either way. Any other flag bit or a negative band_r fails and leaves the
+ * setting unchanged. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers;
+ * the ranks of an all-gather cannot be checked without a collective, so every rank must set the same one. Enrolment,
+ * sr_get_mdl_batch and the drop-in dtw() keep the greedy walk. */
+int sr_set_match(sr_handle *h, uint32_t flags, int band_r);
+int sr_get_match(const sr_handle *h, uint32_t *flags, int *band_r);
 /* spch_recg (main.c:249-296) for B utterances: noise_atap(first n_len) -> VAD(U) -> get_mfcc(seg 0)
- * -> dtw against the bank -> argmin -> cmd = idx / SR_FTR_PER_COMM. Any output pointer may be NULL. */
+ * -> dtw against the bank (the handle's matcher, sr_set_match) -> argmin -> cmd = idx / SR_FTR_PER_COMM. Any output
+ * pointer may be NULL. */
 typedef struct {
     atap_tag  *atap;       /* [B]            */
     uint32_t  *seg_off;    /* [B][3][2]      */
@@ -186,7 +201,7 @@ int            sr_labels_batch(const sr_handle *h, const uint32_t *cmd, const ui
 
 /* The same call spread over several GPUs of one box: contiguous shards, one host thread per handle, results
  * written straight into the caller's host arrays (no collective needed for host outputs). handles[g] must be
- * handles on different devices with the same bank set. */
+ * handles on different devices with the same bank set and the same matcher (sr_set_match). */
 int sr_recognise_batch_multi(sr_handle *const *handles, uint32_t n_handles, const uint16_t *pcm, uint32_t U, uint32_t B,
                              uint32_t n_len, const sr_recog_out *out);
 
@@ -241,7 +256,8 @@ int sr_get_mdl_batch(sr_handle *h, const v_ftr_tag *in1, const v_ftr_tag *in2, u
  * n_streams concurrent captures of max_samples samples each, fed in chunks -- in lock step (sr_streams_push) or every
  * stream at its own pace (sr_streams_push_ragged). Each push advances noise_atap (once the first n_len samples of a
  * stream are in) and VAD with the reference's carried state, and recognises every segment that closes (get_mfcc + dtw
- * + argmin against the handle's bank): one H2D copy, five kernels, one D2H copy and ONE synchronisation per push.
+ * with the handle's matcher + argmin against the handle's bank): one H2D copy, five kernels, one D2H copy and ONE
+ * synchronisation per push.
  * After the last chunk the events equal the batch results on the complete buffers; the reference itself only ever
  * recognises segment 0 (main.c:268), here all <= 3 segments of a stream produce an event.
  * Events are never dropped: what does not fit max_events stays queued (oldest first) and is handed out by the next
@@ -323,7 +339,8 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
  * sqrt check), the packed transport's 12-bit expander, enrol's slot packing and the streaming pool's kernels. Zero-size
  * calls launch and record nothing. sr_timing_collect synchronises the
  * stream and returns (tag, milliseconds) per timed launch in issue order, then rearms. Tags: 0 noise_atap+VAD,
- * 1 get_mfcc, 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP). max_records = 0 disables. */
+ * 1 get_mfcc, 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP, in sr_dtw_batch* and in recognise
+ * calls under the SR_DTW_BAND matcher). max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

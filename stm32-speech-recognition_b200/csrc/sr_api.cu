@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 2; }
+int sr_abi_version(void) { return 3; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -107,6 +107,19 @@ int sr_get_geometry(const sr_handle *h) { return h ? h->geom : SR_GEOM_REF; }
 int sr_set_dtw_variant(sr_handle *h, int variant) {
     SR_REQUIRE(h, h && variant >= -1 && variant <= 1);
     h->dtw_variant = variant;
+    return 0;
+}
+
+int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
+    SR_REQUIRE(h, h && (flags == 0 || flags == SR_DTW_BAND) && band_r >= 0);
+    h->match_flags = flags;
+    h->match_r = band_r;
+    return 0;
+}
+int sr_get_match(const sr_handle *h, uint32_t *flags, int *band_r) {
+    if (!h || !flags || !band_r) return fail(nullptr, "sr_get_match: bad arguments", cudaSuccess);
+    *flags = h->match_flags;
+    *band_r = h->match_r;
     return 0;
 }
 
@@ -403,11 +416,10 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
         best = static_cast<u64 *>(bb.p);
         SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, B, h->stream));
     }
-    if (bank.n && (flags & SR_DTW_BAND)) {
-        SR_REQUIRE(h, band_r >= 0);
-        SR_LAUNCH(h, TAG_DTW_BAND, launch_dtw_band(in, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, h->num_sms, h->stream));
-    } else if (bank.n) {
-        SR_LAUNCH(h, TAG_DTW, launch_dtw_h(h, bank, in, B, flags, score, best, status));
+    if (bank.n) {
+        const bool band = (flags & SR_DTW_BAND) != 0;
+        if (band) SR_REQUIRE(h, band_r >= 0);
+        SR_LAUNCH(h, band ? TAG_DTW_BAND : TAG_DTW, launch_scan(h, bank, in, B, flags, band_r, score, best, status));
     }
     if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
     return 0;
@@ -480,8 +492,9 @@ int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
         const int rc = wait_comm ? comm_wait_before_scan(h, o->score) : sr_comm_wait(h);
         if (rc) return rc;
     }
-    // main.c:276-294 template scan, argmin, command index
-    return dtw_dev_impl(h, h->bank, ftr, B, SR_DTW_CHECK_SIGN, 0, o->score, o->best_idx, o->best_dis, o->cmd, status);
+    // main.c:276-294 template scan (the handle's matcher, save_sign honoured as main.c:283 does), argmin, command index
+    return dtw_dev_impl(h, h->bank, ftr, B, SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, o->score, o->best_idx,
+                        o->best_dis, o->cmd, status);
 }
 
 // sr_dtw_batch of B host inputs against `bank`, inside the host call c
@@ -680,12 +693,14 @@ int sr_get_mdl_batch(sr_handle *h, const v_ftr_tag *in1, const v_ftr_tag *in2, u
 // from its own host thread, and every shard writes its results straight into its slice of the caller's host
 // arrays -- with host outputs the "gather" is the D2H copies themselves, no collective is needed. (Device-resident
 // multi-GPU use is one process per GPU with a NCCL all-gather of the score blocks, see bench.py.)
-// All handles must have the same template bank set. Returns the first non-zero shard status.
+// All handles must have the same template bank set and the same matcher. Returns the first non-zero shard status.
 int sr_recognise_batch_multi(sr_handle *const *handles, uint32_t n_handles, const uint16_t *pcm, uint32_t U, uint32_t B,
                              uint32_t n_len, const sr_recog_out *o) {
     if (!handles || n_handles == 0 || !o) return fail(nullptr, "sr_recognise_batch_multi: bad arguments", cudaSuccess);
     for (uint32_t g = 0; g < n_handles; ++g)
         if (!handles[g] || handles[g]->bank.n != handles[0]->bank.n) return fail(nullptr, "sr_recognise_batch_multi: handles differ", cudaSuccess);
+    for (uint32_t g = 0; g < n_handles; ++g)
+        if (!same_match(handles[g], handles[0])) return fail(nullptr, "sr_recognise_batch_multi: handles differ in their matcher", cudaSuccess);
     std::vector<int> rc(n_handles, 0);
     std::vector<std::thread> th;
     for (uint32_t g = 0; g < n_handles; ++g) {

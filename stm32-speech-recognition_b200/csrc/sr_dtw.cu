@@ -304,82 +304,173 @@ cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStre
 // BASELINE.json configs[2] names it; checked against our own CPU DP oracle sro_dtw_band -- parity unpinned
 // by the reference). D(i,j) = d(i,j) + min(D(i-1,j), D(i,j-1), D(i-1,j-1)), band |j - floor(i*M/I)| <= r,
 // local distance = get_dis, result D(I-1,M-1)/(I+M), same 2:1 length guard as DTW.C:133.
-// One WARP per (utterance, template) cost matrix: lane = band offset (2r+1 <= 32). The in-row dependency
+// Three kernels, chosen from r alone (launch_dtw_band): dtw_band_thread_kernel<10> for r = 10, dtw_band_kernel for the
+// other r <= 15, dtw_wide_kernel for r >= 16 up to the full matrix. On the recognition path all three take the
+// per-utterance status gate, a batch size produced on the device (streaming) and the bank order; scores and argmin keys
+// stay under the original slot number.
+// dtw_band_kernel: one WARP per (utterance, template) cost matrix, lane = band offset (2r+1 <= 32). The in-row dependency
 // x_j = d_j + min(A_j, x_{j-1}) is a (min,+) linear recurrence, solved per row with two warp scans:
 //   P = prefix-sum(d),  x_j = P_j + prefix-min_k( A_k - P_{k-1} );  A comes from the previous row by shuffles.
 namespace srk {
 
 constexpr s32 kInf = 0x3FFFFFFF;
 
-__global__ void __launch_bounds__(kDtwWarps * 32)
-dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best) {
+// The warp-per-pair tile scan of dtw_band_kernel and dtw_wide_kernel. A CTA stages a tile of Tt <= 32 templates (bank
+// slot perm[t] when a bank order is given); each warp stages one utterance at a time and scores it against the Tt
+// templates one after another, the whole warp on one cost matrix: pair(I, M, urow, trow, lane) returns, in every lane, the
+// score of a pair that passed pair_walks. Lane tt keeps the score of template tt; one score row and one atomicMin of the
+// warp's smallest key per utterance. An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in lane_packed_scan.
+template <class Pair>
+__device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
+                                               u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status,
+                                               const u32 *B_dev, const u32 *perm, Pair pair) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
+    if (B_dev) B = min(B, *B_dev);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const u32 t0 = blockIdx.x * kTileT;
     const int Tt = (int)min((u32)kTileT, T - t0);
     unsigned char *tile = smem_raw;                                               // byte-plane slots, as in dtw_kernel
-    u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)kTileT * kSlotBytes);
-    unsigned char *uslot = smem_raw + (size_t)kTileT * kSlotBytes + 128 + (size_t)warp * kSlotBytes;
-    stage_tile(tile, kSlotBytes, kNrm119, tfrm, nullptr, bank, slot_stride, flags, nullptr, t0, Tt, warp, lane, kDtwWarps);
+    u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)kTileT * kSlotBytes);  // [32] frame counts, [32] slot numbers
+    unsigned char *uslot = smem_raw + (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)warp * kSlotBytes;
+    stage_tile(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kDtwWarps);
     __syncthreads();
     for (u32 u = blockIdx.y * kDtwWarps + warp; u < B; u += gridDim.y * kDtwWarps) {
         const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
-        const int I = (int)((*reinterpret_cast<const u32 *>(uf)) >> 16);
+        u32 Iraw = kNoWalk;                               // VAD/MFCC failed: spch_recg returns before dtw
+        if (!(status && status[u] != SR_ST_OK)) Iraw = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
         __syncwarp();
-        if (I <= 119) stage_planes(uslot, kNrm119, uf, I, lane, 32);
+        stage_planes(uslot, kNrm119, uf, staged_rows(Iraw), lane, 32);
         __syncwarp();
         u32 my_result = SR_DIS_ERR;                       // lane tt keeps the result of template tt
         for (int tt = 0; tt < Tt; ++tt) {
             const u32 Mraw = tfrm[tt];
-            const int M = (int)Mraw;
             u32 result = SR_DIS_ERR;
-            if (I >= 1 && I <= 119 && pair_walks((u32)I, Mraw)) {
-                const unsigned char *trow = tile + (size_t)tt * kSlotBytes;
-                s32 Dprev = kInf;
-                int cprev = 0;
-                for (int i = 0; i < I; ++i) {
-                    const int c = (i * M) / I, j = c - r + lane;
-                    const bool valid = lane <= 2 * r && j >= 0 && j < M;
-                    PRow a, b;
-                    load_row(a, uslot, kNrm119, i);                            // broadcast read
-                    load_row(b, trow, kNrm119, valid ? j : 0);
-                    const s32 d = valid ? (s32)pdist(a, b) : 0;
-                    const int sft = c - cprev;
-                    const int su = lane + sft, sd = lane + sft - 1;
-                    s32 up = __shfl_sync(0xFFFFFFFFu, Dprev, su & 31);
-                    s32 dg = __shfl_sync(0xFFFFFFFFu, Dprev, sd & 31);
-                    if (su > 31) up = kInf;
-                    if (sd < 0 || sd > 31) dg = kInf;
-                    s32 A = min(up, dg);
-                    if (i == 0) A = (j == 0) ? 0 : kInf;
-                    if (!valid) A = kInf;
-                    s32 P = d;                                                 // inclusive prefix sum over lanes
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) { const s32 v = __shfl_up_sync(0xFFFFFFFFu, P, o); if (lane >= o) P += v; }
-                    s32 m = A - (P - d);                                       // A_k - P_{k-1}
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) { const s32 v = __shfl_up_sync(0xFFFFFFFFu, m, o); if (lane >= o) m = min(m, v); }
-                    s32 x = P + m;
-                    if (!valid || x >= kInf / 2) x = kInf;
-                    Dprev = x;
-                    cprev = c;
-                }
-                const int lend = (M - 1) - (cprev - r);                        // lane holding column M-1 in the last row
-                const s32 fin = __shfl_sync(0xFFFFFFFFu, Dprev, lend & 31);
-                if (lend >= 0 && lend <= 2 * r && fin < kInf / 2) result = (u32)fin / (u32)(I + M);
-            }
+            if (Iraw >= 1 && pair_walks(Iraw, Mraw))
+                result = pair((int)Iraw, (int)Mraw, uslot, tile + (size_t)tt * kSlotBytes, lane);
             if (lane == tt) my_result = result;
         }
-        const u32 t = t0 + lane;
-        if (t < T && score) score[(size_t)u * T + t] = my_result;
+        const bool has_t = lane < Tt;
+        const u32 t = !has_t ? 0u : perm ? tfrm[kTileT + lane] : t0 + (u32)lane;   // the original slot number
+        if (has_t && score) score[(size_t)u * T + t] = my_result;
         if (best) {
-            u64 key = t < T ? (((u64)my_result << 32) | (u64)t) : ~0ull;
+            u64 key = has_t ? (((u64)my_result << 32) | (u64)t) : ~0ull;
 #pragma unroll
             for (int o = 16; o; o >>= 1) { const u64 other = __shfl_xor_sync(0xFFFFFFFFu, key, o); key = other < key ? other : key; }
             if (lane == 0) atomicMin(reinterpret_cast<unsigned long long *>(&best[u]), (unsigned long long)key);
         }
     }
+}
+
+__global__ void __launch_bounds__(kDtwWarps * 32)
+dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
+                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
+                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
+    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
+                   [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
+        s32 Dprev = kInf;
+        int cprev = 0;
+        for (int i = 0; i < I; ++i) {
+            const int c = (i * M) / I, j = c - r + lane;
+            const bool valid = lane <= 2 * r && j >= 0 && j < M;
+            PRow a, b;
+            load_row(a, uslot, kNrm119, i);                            // broadcast read
+            load_row(b, trow, kNrm119, valid ? j : 0);
+            const s32 d = valid ? (s32)pdist(a, b) : 0;
+            const int sft = c - cprev;
+            const int su = lane + sft, sd = lane + sft - 1;
+            s32 up = __shfl_sync(0xFFFFFFFFu, Dprev, su & 31);
+            s32 dg = __shfl_sync(0xFFFFFFFFu, Dprev, sd & 31);
+            if (su > 31) up = kInf;
+            if (sd < 0 || sd > 31) dg = kInf;
+            s32 A = min(up, dg);
+            if (i == 0) A = (j == 0) ? 0 : kInf;
+            if (!valid) A = kInf;
+            s32 P = d;                                                 // inclusive prefix sum over lanes
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const s32 v = __shfl_up_sync(0xFFFFFFFFu, P, o); if (lane >= o) P += v; }
+            s32 m = A - (P - d);                                       // A_k - P_{k-1}
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const s32 v = __shfl_up_sync(0xFFFFFFFFu, m, o); if (lane >= o) m = min(m, v); }
+            s32 x = P + m;
+            if (!valid || x >= kInf / 2) x = kInf;
+            Dprev = x;
+            cprev = c;
+        }
+        const int lend = (M - 1) - (cprev - r);                        // lane holding column M-1 in the last row
+        const s32 fin = __shfl_sync(0xFFFFFFFFu, Dprev, lend & 31);
+        return (lend >= 0 && lend <= 2 * r && fin < kInf / 2) ? (u32)fin / (u32)(I + M) : SR_DIS_ERR;
+    });
+}
+
+// ---- K3w: the same DP for r >= 16 up to the full matrix: one WARP per pair, a whole ROW across the warp ---------------
+// A row never has more than M <= 119 valid columns, whatever r is, so lane l holds the fixed columns 4l .. 4l+3 (32 x 4 =
+// 128 >= 119) and the cost of a pair does not depend on r: r >= 118 is the unconstrained DTW (the host clamps r to 118).
+// The band of row i is the column interval [max(c-r, 0), min(c+r, M-1)], c = floor(i*M/I); cells outside it are +inf.
+// Per row: up and diag come from the lane's own previous row (diag of its first column by one shuffle); the in-row
+// recurrence x_j = d_j + min(A_j, x_{j-1}), A_j = min(up, diag), maps a lane's incoming x to its outgoing one as
+// f(x) = min(x + a, b) (a = the lane's sum of d, b = its outgoing x for an incoming +inf); one warp scan composes these
+// maps, f2(f1(x)) = min(x + a1 + a2, min(b1 + a2, b2)), giving every lane its incoming x, and a serial pass over the
+// lane's four cells writes the row. The template's four rows stay in registers for the whole pair.
+// Headroom of kInf = 2^30 - 1: a path to cell (i,j) has at most i+j+1 cells of at most 65 536, so every reachable cell
+// is below 237 * 65 536 = 15 532 032 and a full-matrix optimum at most max(I,M) * 65 536; +inf sums (b1 + a2 <= kInf +
+// 119 * 65 536) stay below 2^31 and are cut back to kInf, so a cell is reachable exactly when it is below kInf / 2.
+constexpr int kWideCells = 4;
+
+__global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
+dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
+                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
+                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
+    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
+                   [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
+        const int j0 = lane * kWideCells;
+        PRow b[kWideCells];
+        s32 D[kWideCells];
+#pragma unroll
+        for (int k = 0; k < kWideCells; ++k) {
+            load_row(b[k], trow, kNrm119, j0 + k < M ? j0 + k : 0);
+            D[k] = kInf;
+        }
+        for (int i = 0; i < I; ++i) {
+            const int c = (i * M) / I, lo = max(c - r, 0), hi = min(c + r, M - 1);
+            PRow a;
+            load_row(a, uslot, kNrm119, i);                            // broadcast read
+            s32 dg = __shfl_up_sync(0xFFFFFFFFu, D[kWideCells - 1], 1);   // D(i-1, j0-1)
+            if (lane == 0) dg = kInf;
+            s32 d[kWideCells], A[kWideCells];
+            bool valid[kWideCells];
+            s32 x = kInf, sum = 0;                                     // serial pass for an incoming +inf: b and a
+#pragma unroll
+            for (int k = 0; k < kWideCells; ++k) {
+                const int j = j0 + k;
+                valid[k] = j >= lo && j <= hi;
+                d[k] = valid[k] ? (s32)pdist(a, b[k]) : 0;
+                A[k] = i == 0 ? (j == 0 ? 0 : kInf) : min(D[k], dg);
+                dg = D[k];
+                x = valid[k] ? min(d[k] + min(A[k], x), kInf) : kInf;
+                sum += d[k];
+            }
+            s32 fa = sum, fb = x;                                      // inclusive composition of the lanes' maps
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const s32 pa = __shfl_up_sync(0xFFFFFFFFu, fa, o), pb = __shfl_up_sync(0xFFFFFFFFu, fb, o);
+                if (lane >= o) { fb = min(min(pb + fa, fb), kInf); fa += pa; }
+            }
+            x = __shfl_up_sync(0xFFFFFFFFu, min(kInf + fa, fb), 1);   // x_{j0-1}: the previous lanes' maps applied to +inf
+            if (lane == 0) x = kInf;
+            x = min(x, kInf);
+#pragma unroll
+            for (int k = 0; k < kWideCells; ++k) {                     // serial fix-up with the true incoming x
+                x = valid[k] ? min(d[k] + min(A[k], x), kInf) : kInf;
+                D[k] = x;
+            }
+        }
+        const int kend = (M - 1) & (kWideCells - 1);
+        s32 e = D[0];
+#pragma unroll
+        for (int k = 1; k < kWideCells; ++k) if (k == kend) e = D[k];
+        const s32 fin = __shfl_sync(0xFFFFFFFFu, e, (M - 1) / kWideCells);
+        return fin < kInf / 2 ? (u32)fin / (u32)(I + M) : SR_DIS_ERR;
+    });
 }
 
 // ---- K3b: the same banded DP, one THREAD per pair, band in registers (compile-time radius) -----------------------
@@ -390,9 +481,10 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 template <int R>
 __global__ void __launch_bounds__(kK2Warps * 32)
 dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-                       u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best, int Wg, int NU, int G,
-                       u32 tile0, int tslots) {
-    lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, nullptr, Wg, NU, G, tile0, tslots, nullptr, nullptr,
+                       u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best,
+                       const u8 *__restrict__ status, int Wg, int NU, int G, u32 tile0, int tslots,
+                       const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
+    lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
                      [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
         constexpr int W = 2 * R + 1;
         if (I == 0) return SR_DIS_ERR;                     // empty feature sets (M == 0 too, by the 2:1 guard): no cell
@@ -445,30 +537,35 @@ dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const un
     });
 }
 
+// the banded DP of radius band_r >= 0, the kernel chosen from band_r alone: the thread form for r = 10, the warp-scan
+// form for the other r <= 15 (2r+1 lanes of one warp), the whole-row form for r >= 16. Every r >= 118 is the full matrix
+// (|j - c| <= 118 for any two columns), so r is clamped to 118 and no r reaches the kernels' c +- r.
 cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
-                            u32 *score, u64 *best, int num_sms, cudaStream_t st) {
+                            u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev,
+                            const u32 *perm) {
     if (B == 0 || T == 0) return cudaSuccess;
-    if (band_r < 0 || band_r > 15) return cudaErrorInvalidValue;               // 2r+1 lanes of one warp
-    if (band_r == 10) {                                                       // the BASELINE radius: thread-per-pair form
+    if (band_r < 0) return cudaErrorInvalidValue;
+    const int r = min(band_r, (int)kMaxFrm - 1);
+    const auto *in = static_cast<const unsigned char *>(in_ftr);
+    const auto *bk = static_cast<const unsigned char *>(bank);
+    if (r == 10) {                                                            // the BASELINE radius: thread-per-pair form
         cudaError_t e = cudaFuncSetAttribute(dtw_band_thread_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
         if (e != cudaSuccess) return e;
         return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
             const LanePlan p = plan_lanes(Tt);
             dtw_band_thread_kernel<10><<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32,
-                                         p.smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
-                                                       static_cast<const unsigned char *>(bank), T, slot_stride, flags,
-                                                       score, best, p.Wg, p.NU, p.G, tile0, Tt);
+                                         p.smem, st>>>(in, B, bk, T, slot_stride, flags, score, best, status, p.Wg, p.NU,
+                                                       p.G, tile0, Tt, B_dev, perm);
             return cudaGetLastError();
         });
     }
-    const size_t band_smem = (size_t)kTileT * kSlotBytes + 128 + (size_t)kDtwWarps * kSlotBytes;
-    cudaError_t e = cudaFuncSetAttribute(dtw_band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)band_smem);
+    auto *kernel = r <= 15 ? dtw_band_kernel : dtw_wide_kernel;
+    const size_t smem = (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)kDtwWarps * kSlotBytes;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const u32 tiles = (T + kTileT - 1) / kTileT;
     dim3 grid(tiles, grid_rows(num_sms, tiles, B, kDtwWarps));
-    dtw_band_kernel<<<grid, kDtwWarps * 32, band_smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
-                                                                  static_cast<const unsigned char *>(bank), T,
-                                                                  slot_stride, flags, band_r, score, best);
+    kernel<<<grid, kDtwWarps * 32, smem, st>>>(in, B, bk, T, slot_stride, flags, r, score, best, status, B_dev, perm);
     return cudaGetLastError();
 }
 

@@ -1,5 +1,5 @@
 // sr_dtw_core.cuh -- the template scan's shared core, used by the static kernels (sr_dtw.cu: greedy dtw_kernel, banded
-// dtw_band_kernel and dtw_band_thread_kernel) and the dynamic-pair kernel (sr_dtw_dyn.cu): byte-plane rows and their
+// dtw_band_kernel, dtw_band_thread_kernel and dtw_wide_kernel) and the dynamic-pair kernel (sr_dtw_dyn.cu): byte-plane rows and their
 // get_dis, the slot header decode, the template tile stager, the greedy walk step, the score/argmin epilogue and the
 // launch geometry.
 //

@@ -32,7 +32,8 @@ cudaError_t launch_dtw_dyn(const void *in_ftr, u32 B, const void *bank, u32 T, u
                            u64 *best, const u8 *status, int num_sms, cudaStream_t st, u32 *max_frm_scratch,
                            const u32 *B_dev = nullptr, const u32 *perm = nullptr);
 cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
-                            u32 *score, u64 *best, int num_sms, cudaStream_t st);
+                            u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st,
+                            const u32 *B_dev = nullptr, const u32 *perm = nullptr);
 cudaError_t launch_best_init(u64 *best, u32 B, cudaStream_t st);
 cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status,
                               cudaStream_t st);
@@ -148,6 +149,8 @@ struct sr_handle {
     u32 n_labels = 0, label_stride = 0;
     sr_comm *comm = nullptr;                           // the exchange step (sr_comm_create), optional
     int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cu), -1 default
+    u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk or SR_DTW_BAND
+    int match_r = 0;                                   // its band radius
     DevBuf mfcc_work;                                  // the same for mfcc_kernel (next utterance, CTAs finished)
     DevBuf vad_work;                                   // two words: dynamic utterance hand-out of vad_kernel (zeroed once, self re-arming)
     DevBuf dtw_scratch;                                // one word: max frm_num of the current inputs (dynamic kernel's slot size)
@@ -229,6 +232,22 @@ inline cudaError_t launch_dtw_h(sr_handle *h, const BankView &bank, const void *
                               static_cast<u32 *>(h->dtw_scratch.p), B_dev, bank.order);
     }
     return launch_dtw(in_ftr, B, bank.p, bank.n, bank.stride, flags, score, best, status, h->num_sms, h->stream, B_dev, bank.order);
+}
+
+// The template scan of B inputs against `bank` -- the one place a matcher becomes a kernel launch: with SR_DTW_BAND in
+// flags the banded DP of radius band_r (launch_dtw_band picks the kernel from r), else the greedy walk. sr_dtw_batch
+// passes its caller's flags and r; the recognition paths (recognise, streaming) pass the handle's matcher.
+inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, int band_r,
+                               u32 *score, u64 *best, const u8 *status, const u32 *B_dev = nullptr) {
+    if (flags & SR_DTW_BAND)
+        return launch_dtw_band(in_ftr, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, status, h->num_sms,
+                               h->stream, B_dev, bank.order);
+    return launch_dtw_h(h, bank, in_ftr, B, flags, score, best, status, B_dev);
+}
+
+// the two handles' recognition calls score alike: both greedy, or both the banded DP at the same radius
+inline bool same_match(const sr_handle *a, const sr_handle *b) {
+    return a->match_flags == b->match_flags && (a->match_flags == 0 || a->match_r == b->match_r);
 }
 
 int comm_wait_before_scan(sr_handle *h, const void *score);   // sr_comm.cu

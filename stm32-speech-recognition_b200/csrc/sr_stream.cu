@@ -355,8 +355,9 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     stream_status_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const unsigned char *>(p->ftr.p), n_ev, p->cap,
                                                    static_cast<u8 *>(p->status.p), static_cast<u32 *>(p->frm.p), best);
     SR_CK(h, cudaGetLastError());
-    if (h->bank.n)
-        SR_CK(h, launch_dtw_h(h, h->bank, p->ftr.p, p->cap, SR_DTW_CHECK_SIGN, nullptr, best, static_cast<const u8 *>(p->status.p), n_ev));
+    if (h->bank.n)                                                    // the handle's matcher, read at every push
+        SR_CK(h, launch_scan(h, h->bank, p->ftr.p, p->cap, SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, nullptr, best,
+                             static_cast<const u8 *>(p->status.p), n_ev));
     u32 *out_count = static_cast<u32 *>(p->out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(p->out.p) + 16);
     stream_finish_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const StreamEventDev *>(p->ev.p), n_ev, p->cap,
@@ -468,6 +469,10 @@ int sr_stream_group_reset(sr_stream_group *gr) {
 static int group_push(sr_stream_group *gr, const uint16_t *chunk, uint32_t stride, uint32_t ulen, const uint32_t *lens,
                       sr_stream_event *events, uint32_t max_events, uint32_t *n_events) {
     if (!gr || !n_events) return fail(nullptr, "sr_stream_group_push: bad arguments", cudaSuccess);
+    *n_events = 0;
+    for (auto *sh : gr->shards)                                       // every shard must recognise with the same matcher
+        if (!same_match(sh->pool->h, gr->shards[0]->pool->h))
+            return fail(nullptr, "sr_stream_group_push: handles differ in their matcher", cudaSuccess);
     for (auto *sh : gr->shards) {
         std::lock_guard<std::mutex> lk(sh->m);
         sh->chunk = chunk ? chunk + (size_t)sh->s0 * stride : nullptr;

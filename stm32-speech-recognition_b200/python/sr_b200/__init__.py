@@ -112,6 +112,8 @@ def lib():
         L.sr_allgather_dev.argtypes = [vp, vp, vp, C.c_size_t]
         L.sr_recognise_batch_dev_allgather.argtypes = [vp, vp, u32, u32, u32, C.POINTER(RecogOut), vp, vp]
         L.sr_set_dtw_variant.argtypes = [vp, i32]
+        L.sr_set_match.argtypes = [vp, u32, i32]
+        L.sr_get_match.argtypes = [vp, vp, vp]
         L.sr_set_geometry.argtypes = [vp, i32]
         L.sr_get_geometry.argtypes = [vp]
         L.sr_set_labels.argtypes = [vp, vp, u32, u32]
@@ -355,6 +357,16 @@ class Handle:
     def set_dtw_variant(self, v):
         """greedy dtw kernel: 0 static lane = pair, 1 dynamic pair scheduling, -1 library default"""
         self._ck(lib().sr_set_dtw_variant(self._h, int(v)))
+
+    def set_match(self, flags, band_r=0):
+        """matcher of the recognition calls: 0 = the reference's greedy walk, DTW_BAND = the banded DP at radius band_r"""
+        self._ck(lib().sr_set_match(self._h, int(flags), int(band_r)))
+
+    def match(self):
+        """(flags, band_r) of the recognition calls' matcher"""
+        f, r = C.c_uint32(0), C.c_int(0)
+        self._ck(lib().sr_get_match(self._h, C.byref(f), C.byref(r)))
+        return int(f.value), int(r.value)
 
     def set_geometry(self, geom):
         """0 = reference 160/80/1024, 1 = GEOM_B 200/80/256 (extension, parity unpinned)"""
