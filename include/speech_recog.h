@@ -252,6 +252,34 @@ int sr_enrol_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, ui
  * (the reference writes out of bounds there). */
 int sr_get_mdl_batch(sr_handle *h, const v_ftr_tag *in1, const v_ftr_tag *in2, uint32_t n, v_ftr_tag *mdl, uint32_t *dis);
 
+/* ---- alignment along the banded DP (extension, parity unpinned: the reference has no DP) ---------------------------
+ * sr_dtw_path_batch: the SR_DTW_BAND DP of sr_dtw_batch for n (in[p], mdl[p]) pairs, with its optimal warping path.
+ * dis[p] equals sr_dtw_batch's band score of the same pair bit for bit. The path is traced back from (I-1, M-1) to (0, 0);
+ * at each cell the predecessor is the neighbour with the smallest D, ties to the diagonal (i-1, j-1), then (i, j-1) (only
+ * the template advances), then (i-1, j) (only the input advances), so a self-match's path is the diagonal. It is written
+ * in forward order as (i, j) byte pairs, path_len[p] = L with max(I, M) <= L <= I + M - 1, entries past L are 0xFF. A
+ * rejected pair (2:1 guard, I or M = 0 or > 119, end cell outside the band) has L = 0, all 0xFF and SR_DIS_ERR. path
+ * and path_len may be NULL; band_r >= 0 as in sr_dtw_batch (a negative one fails). The handle's sr_set_match is not read. */
+#define SR_PATH_MAX 237u   /* 2 * SR_VV_FRM_MAX - 1 */
+int sr_dtw_path_batch(sr_handle *h, const v_ftr_tag *in, const v_ftr_tag *mdl, uint32_t n, int band_r,
+                      uint8_t *path /* [n][SR_PATH_MAX][2] or NULL */, uint32_t *path_len /* [n] or NULL */,
+                      uint32_t *dis /* [n] */);
+/* sr_average_bank: one template per group by DTW barycentre averaging. The bank image holds G groups of K consecutive
+ * slots (1 <= K <= 32) of slot_stride bytes, e.g. the SR_FTR_PER_COMM repetitions sr_enrol_batch wrote per command. A slot
+ * is a member when save_sign == SR_SAVE_MASK and 1 <= frm_num <= 119. The anchor is the member k with the smallest sum
+ * over the other members l of the band score S(l -> k) (u64, SR_DIS_ERR counted as 0xFFFFFFFF, lowest k on a tie); C_0 is
+ * its features. Each of `iters` updates aligns every member whose score against C_t is not SR_DIS_ERR along its path and
+ * sets C_{t+1}[j] = (sum of the member frames aligned to column j) / (their count), per coefficient, truncating toward
+ * zero; C keeps the anchor's frame count, and with no member aligned C_{t+1} = C_t. bank_out has the input's shape: slot
+ * g*K holds C_iters signed with SR_SAVE_MASK, the group's other K-1 slots are erased (0xFF), so recognition's
+ * cmd = idx / SR_FTR_PER_COMM still names the command. A group with no member gets K erased slots and anchor 0xFFFFFFFF.
+ * score[g][k] = S(member k -> C_iters), SR_DIS_ERR for a non-member: what sr_dtw_batch(SR_DTW_BAND | SR_DTW_CHECK_SIGN)
+ * returns for that slot against bank_out. score and anchor may be NULL. Every pass runs on the device: 2 * iters + 3
+ * launches (the anchor scores, an alignment and an update per iteration, the final scores, the packing), fewer when a
+ * pass has no pair (K = 1 has no anchor scores). The handle's sr_set_match is not read. */
+int sr_average_bank(sr_handle *h, const void *bank, uint32_t slot_stride, uint32_t K, uint32_t G, int band_r,
+                    uint32_t iters, void *bank_out, uint32_t *score /* [G][K] or NULL */, uint32_t *anchor /* [G] or NULL */);
+
 /* ---- streaming front end (stands in for record(), main.c:77-102 / ADC.C:11-103) ----------------------------
  * n_streams concurrent captures of max_samples samples each, fed in chunks -- in lock step (sr_streams_push) or every
  * stream at its own pace (sr_streams_push_ragged). Each push advances noise_atap (once the first n_len samples of a
@@ -334,13 +362,14 @@ uint32_t sr_debug_pack12_host(int variant, const uint16_t *src, uint64_t n, uint
 int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t *out);
 
 /* Per-kernel device timing: after sr_timing_enable(h, max_records) every launch of the recognition-path kernels
- * by this handle's noise_atap, VAD, MFCC, DTW, recognise and enrol calls (host-buffer and _dev forms) is bracketed
+ * by this handle's noise_atap, VAD, MFCC, DTW, recognise, enrol, path and averaging calls (host-buffer and _dev forms) is bracketed
  * by a CUDA event pair on the launching stream. Not timed: the test-hook kernels (FFT, get_dis, get_mdl, dtw_limit,
- * sqrt check), the packed transport's 12-bit expander, enrol's slot packing and the streaming pool's kernels. Zero-size
+ * sqrt check), the packed transport's 12-bit expander, the slot packing of enrol and averaging and the streaming pool's kernels. Zero-size
  * calls launch and record nothing. sr_timing_collect synchronises the
  * stream and returns (tag, milliseconds) per timed launch in issue order, then rearms. Tags: 0 noise_atap+VAD,
  * 1 get_mfcc, 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP, in sr_dtw_batch* and in recognise
- * calls under the SR_DTW_BAND matcher). max_records = 0 disables. */
+ * calls under the SR_DTW_BAND matcher), 7 the banded DP with its path (every pass of sr_dtw_path_batch and
+ * sr_average_bank that aligns), 8 sr_average_bank's template update. max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

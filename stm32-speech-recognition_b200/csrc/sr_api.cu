@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 3; }
+int sr_abi_version(void) { return 4; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -179,7 +179,7 @@ int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
-       TAG_DTW_BAND = 6 };
+       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8 };
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
@@ -686,6 +686,103 @@ int sr_get_mdl_batch(sr_handle *h, const v_ftr_tag *in1, const v_ftr_tag *in2, u
     c.out(h->ftr, mdl, bytes);
     u32 *d_dis = c.out(h->bdis, dis, (size_t)n * 4);
     c.launch(TAG_NONE, "launch_get_mdl", [&] { return launch_get_mdl(d_in1, d_in2, d_mdl, n, d_dis, h->stream); });
+    return c.finish();
+}
+
+// The banded DP of n (in[p], mdl[p]) pairs with its optimal warping path (dtw_align_kernel): dis[p] is the score of
+// sr_dtw_batch with SR_DTW_BAND, path[p] the (i, j) points from (0, 0) to (I-1, M-1), 0xFF past path_len[p].
+int sr_dtw_path_batch(sr_handle *h, const v_ftr_tag *in, const v_ftr_tag *mdl, uint32_t n, int band_r, uint8_t *path,
+                      uint32_t *path_len, uint32_t *dis) {
+    SR_REQUIRE(h, h && (n == 0 || (in && mdl && dis)));
+    SR_REQUIRE(h, band_r >= 0);
+    if (n == 0) return 0;
+    HostCall c(h, "sr_dtw_path_batch");
+    const size_t bytes = (size_t)n * kFtrBytes;
+    const v_ftr_tag *d_in = c.in(h->align[0], in, bytes), *d_mdl = c.in(h->align[1], mdl, bytes);
+    u8 *d_path = path ? c.out(h->align[2], path, (size_t)n * SR_PATH_MAX * 2) : nullptr;
+    u32 *d_len = path_len ? c.out(h->align[3], path_len, (size_t)n * 4) : nullptr;
+    u32 *d_dis = c.out(h->align[4], dis, (size_t)n * 4);
+    c.launch(TAG_ALIGN, "launch_dtw_align", [&] {
+        return launch_dtw_align(d_in, kFtrBytes, d_mdl, kFtrBytes, nullptr, n, band_r, d_path, d_len, d_dis, nullptr, nullptr,
+                                0, nullptr, nullptr, h->num_sms, h->stream);
+    });
+    return c.finish();
+}
+
+// DTW barycentre averaging of G groups of K consecutive slots of a flash-layout bank image. Membership, the pair lists and
+// the per-group status come from the slot headers on the host; then every pass runs on the device, in one stream order:
+// the anchor scores S(l -> k) of every member pair, per iteration an alignment of every member to the group's template
+// (the first one resolves the anchor from S and copies it in as C_0) and an update, the final scores, and the packing of
+// slot g*K (the template, signed) with the group's other K-1 slots erased: one pack of G slots K*slot_stride bytes wide.
+int sr_average_bank(sr_handle *h, const void *bank, uint32_t slot_stride, uint32_t K, uint32_t G, int band_r, uint32_t iters,
+                    void *bank_out, uint32_t *score, uint32_t *anchor) {
+    SR_REQUIRE(h, h && (G == 0 || (bank && bank_out)));
+    SR_REQUIRE(h, band_r >= 0 && K >= 1 && K <= 32 && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0);
+    SR_REQUIRE(h, (uint64_t)K * slot_stride <= 0xFFFFFFFFull);
+    if (G == 0) return 0;
+    const auto *b = static_cast<const unsigned char *>(bank);
+    const size_t slots = (size_t)G * K;
+    std::vector<u32> mask(G, 0), pairs, mpairs;          // pairs: (input slot, template slot, S index) of the anchor pass
+    std::vector<u8> gst(G, SR_ST_VAD_FAIL);              // a group without members packs as failed: all K slots erased
+    for (u32 g = 0; g < G; ++g) {
+        for (u32 k = 0; k < K; ++k) {
+            u32 hdr;
+            memcpy(&hdr, b + ((size_t)g * K + k) * slot_stride, 4);
+            const u32 frm = hdr >> 16;
+            if ((hdr & 0xFFFFu) == SR_SAVE_MASK && frm >= 1 && frm <= SR_VV_FRM_MAX) mask[g] |= 1u << k;   // decode_frm's rule
+        }
+        if (!mask[g]) continue;
+        gst[g] = SR_ST_OK;
+        for (u32 l = 0; l < K; ++l) {
+            if (!((mask[g] >> l) & 1u)) continue;
+            mpairs.insert(mpairs.end(), {g * K + l, g, g * K + l});
+            for (u32 k = 0; k < K; ++k)
+                if (k != l && ((mask[g] >> k) & 1u)) pairs.insert(pairs.end(), {g * K + l, g * K + k, (g * K + l) * K + k});
+        }
+    }
+    const u32 n_anchor = (u32)(pairs.size() / 3), n_member = (u32)(mpairs.size() / 3);
+    pairs.insert(pairs.end(), mpairs.begin(), mpairs.end());
+    HostCall c(h, "sr_average_bank");
+    const unsigned char *d_bank = c.in(h->align[0], b, slots * slot_stride);
+    void *d_out = c.out(h->align[1], bank_out, slots * slot_stride);
+    u8 *d_path = c.ws<u8>(h->align[2], slots * SR_PATH_MAX * 2);
+    const auto *d_pairs = c.in(h->align[3], pairs.data(), pairs.size() * 4, 16);
+    auto *d_tpl = c.ws<unsigned char>(h->align[4], (size_t)G * kFtrBytes);
+    auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t o_st = al((size_t)G * 4), o_S = o_st + al(G), o_len = o_S + al(slots * K * 4);
+    auto *misc = c.ws<unsigned char>(h->align[5], o_len + slots * 4);                 // mask | status | S | path_len
+    u32 *d_mask = misc ? reinterpret_cast<u32 *>(misc) : nullptr;
+    u8 *d_st = misc ? misc + o_st : nullptr;
+    u32 *d_S = misc ? reinterpret_cast<u32 *>(misc + o_S) : nullptr, *d_len = misc ? reinterpret_cast<u32 *>(misc + o_len) : nullptr;
+    u32 *d_score = c.out(h->score, score, slots * 4), *d_anchor = c.out(h->bidx, anchor, (size_t)G * 4);
+    c.h2d(d_mask, mask.data(), (size_t)G * 4);
+    c.h2d(d_st, gst.data(), G);
+    auto fill = [&](void *p, int v, size_t bytes) { c.ck("cudaMemsetAsync", p ? cudaMemsetAsync(p, v, bytes, h->stream) : cudaSuccess); };
+    fill(d_S, 0xFF, slots * K * 4);                      // non-member pairs: SR_DIS_ERR
+    fill(d_len, 0, slots * 4);
+    fill(d_score, 0xFF, slots * 4);
+    fill(d_anchor, 0xFF, (size_t)G * 4);                 // empty groups: no anchor
+    const u32 *d_mp = d_pairs + 3 * (size_t)n_anchor;
+    if (n_anchor)
+        c.launch(TAG_ALIGN, "launch_dtw_align (anchor scores)", [&] {
+            return launch_dtw_align(d_bank, slot_stride, d_bank, slot_stride, d_pairs, n_anchor, band_r, nullptr, nullptr, d_S,
+                                    nullptr, nullptr, K, nullptr, nullptr, h->num_sms, h->stream);
+        });
+    for (u32 t = 0; t < iters && n_member; ++t) {
+        c.launch(TAG_ALIGN, "launch_dtw_align (members to the template)", [&] {
+            return launch_dtw_align(d_bank, slot_stride, d_tpl, kFtrBytes, d_mp, n_member, band_r, d_path, d_len, nullptr,
+                                    t == 0 ? d_S : nullptr, d_mask, K, d_tpl, d_anchor, h->num_sms, h->stream);
+        });
+        c.launch(TAG_AVG_UPDATE, "launch_average_update", [&] {
+            return launch_average_update(d_bank, slot_stride, K, G, d_mask, d_path, d_len, d_tpl, h->stream);
+        });
+    }
+    if (n_member)
+        c.launch(TAG_ALIGN, "launch_dtw_align (final scores)", [&] {
+            return launch_dtw_align(d_bank, slot_stride, d_tpl, kFtrBytes, d_mp, n_member, band_r, nullptr, nullptr, d_score,
+                                    iters == 0 ? d_S : nullptr, d_mask, K, d_tpl, d_anchor, h->num_sms, h->stream);
+        });
+    c.launch(TAG_NONE, "launch_pack_slots", [&] { return launch_pack_slots(d_tpl, d_st, G, d_out, K * slot_stride, h->stream); });
     return c.finish();
 }
 

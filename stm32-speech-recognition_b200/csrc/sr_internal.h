@@ -42,6 +42,13 @@ cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStre
 cudaError_t launch_dtw_limit(const u16 *x, const u16 *y, const u16 *I, const u16 *M, u32 n, u8 *out, cudaStream_t st);
 cudaError_t launch_get_mdl(const void *in1, const void *in2, void *mdl, u32 n, u32 *dis, cudaStream_t st);
 cudaError_t launch_pack_slots(const void *ftr, const u8 *status, u32 B, void *bank, u32 slot_stride, cudaStream_t st);
+// the banded DP with its warping path over a list of (input, template, output) u32 triples (NULL: p, p, p), and the DBA
+// update of G groups of K bank slots (sr_dtw_align.cu)
+cudaError_t launch_dtw_align(const void *in_base, u32 in_stride, const void *tpl_base, u32 tpl_stride, const void *pairs,
+                             u32 n, int band_r, u8 *path, u32 *path_len, u32 *dis, const u32 *pick_S, const u32 *mask, u32 K,
+                             void *tpl_out, u32 *anchor_out, int num_sms, cudaStream_t st);
+cudaError_t launch_average_update(const void *bank, u32 slot_stride, u32 K, u32 G, const u32 *mask, const u8 *path,
+                                  const u32 *path_len, void *tpl, cudaStream_t st);
 cudaError_t launch_sqrt_check(u32 lo, u32 hi, unsigned long long *bad_dev, cudaStream_t st);
 cudaError_t launch_unpack12(const void *packed, u64 n_samples, u16 *out, cudaStream_t st);
 class PackPool;
@@ -159,6 +166,7 @@ struct sr_handle {
     // grow-only device workspaces; scratch[] serves the secondary entry points (FFT, get_dis, get_mdl, dtw_limit, the
     // 12-bit expander, the sqrt check, enrol's bank image, dtw()'s one-slot bank) and is never read by a recognise call
     DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
+    DevBuf align[6];                                   // sr_dtw_path_batch / sr_average_bank: pairs, paths, templates, scores
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };

@@ -19,6 +19,7 @@ SEG_NULL = 0xFFFFFFFF
 DIS_ERR = 0xFFFFFFFF
 SAVE_MASK = 12345
 DTW_CHECK_SIGN, DTW_BAND = 1, 2
+PATH_MAX = 237                 # SR_PATH_MAX: the longest warping path, 2 * VV_FRM_MAX - 1 points
 
 ATAP_DTYPE = np.dtype([("mid_val", "<u4"), ("n_thl", "<u2"), ("z_thl", "<u2"), ("s_thl", "<u4")])
 FTR_DTYPE = np.dtype([("save_sign", "<u2"), ("frm_num", "<u2"), ("mfcc_dat", "<i2", (VV_FRM_MAX * MFCC_NUM,))])
@@ -85,6 +86,8 @@ def lib():
         L.sr_debug_unpack12.argtypes = [vp, vp, u64, vp]
         L.sr_enrol_batch.argtypes = [vp, vp, u32, u32, u32, vp, u32, vp]
         L.sr_get_mdl_batch.argtypes = [vp, vp, vp, u32, vp, vp]
+        L.sr_dtw_path_batch.argtypes = [vp, vp, vp, u32, i32, vp, vp, vp]
+        L.sr_average_bank.argtypes = [vp, vp, u32, u32, u32, i32, u32, vp, vp, vp]
         L.sr_streams_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
         L.sr_streams_destroy.argtypes = [vp]
         L.sr_streams_reset.argtypes = [vp]
@@ -298,6 +301,30 @@ class Handle:
         dis = np.zeros(n, np.uint32)
         self._ck(lib().sr_get_mdl_batch(self._h, _p(in1), _p(in2), n, _p(mdl), _p(dis)))
         return mdl, dis
+
+    def dtw_path(self, a, b, band_r, with_path=True):
+        """banded DP of the pairs (a[p], b[p]) with its optimal warping path (sr_dtw_path_batch): (dis [n], path
+        [n, PATH_MAX, 2] of (i, j) points, 0xFF past path_len, path_len [n]); path and path_len are None without with_path"""
+        a, b = np.ascontiguousarray(a, FTR_DTYPE), np.ascontiguousarray(b, FTR_DTYPE)
+        n = a.shape[0]
+        assert b.shape[0] == n
+        dis = np.zeros(n, np.uint32)
+        path = np.zeros((n, PATH_MAX, 2), np.uint8) if with_path else None
+        plen = np.zeros(n, np.uint32) if with_path else None
+        self._ck(lib().sr_dtw_path_batch(self._h, _p(a), _p(b), n, int(band_r), _p(path), _p(plen), _p(dis)))
+        return dis, path, plen
+
+    def average_bank(self, bank, slot_stride, K, band_r, iters):
+        """one template per group of K consecutive slots by DTW barycentre averaging (sr_average_bank): bank [G*K,
+        slot_stride] u8 -> (bank_out of the same shape, score [G, K], anchor [G])"""
+        bank = np.ascontiguousarray(bank, np.uint8).reshape(-1, slot_stride)
+        assert bank.shape[0] % K == 0
+        G = bank.shape[0] // K
+        out = np.zeros_like(bank)
+        score, anchor = np.zeros((G, K), np.uint32), np.zeros(G, np.uint32)
+        self._ck(lib().sr_average_bank(self._h, _p(bank), slot_stride, K, G, int(band_r), iters, _p(out), _p(score),
+                                       _p(anchor)))
+        return out, score, anchor
 
     def fft_mag(self, frames):
         n, length = frames.shape
