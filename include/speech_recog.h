@@ -147,7 +147,9 @@ int sr_noise_atap_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t 
 int sr_vad_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t buf_len,
                  const atap_tag *atap /* [B] */, uint32_t *seg_off /* [B][3][2] */);
 /* get_mfcc of one segment per utterance: seg[b*seg_stride + 0/1] = start/end sample offsets.
- * Only frm_num and the first frm_num rows of ftr[b] are written (MFCC.C never writes save_sign).
+ * Only frm_num and the first frm_num rows of ftr[b] are written (MFCC.C never writes save_sign); in the host-buffer
+ * calls too (this one, sr_recognise_batch*, get_mfcc): save_sign and every row >= frm_num, all rows of a rejected
+ * segment (frm_num = 0), come back as the caller passed them.
  * A segment that starts at 0 reads x[-1] = atap[b].mid_val (as a 16-bit sample), not the previous utterance's last
  * sample; every batched entry point does the same (the drop-in get_mfcc reads the caller's start[-1]). */
 int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *seg,
@@ -176,7 +178,9 @@ int sr_set_match(sr_handle *h, uint32_t flags, int band_r);
 int sr_get_match(const sr_handle *h, uint32_t *flags, int *band_r);
 /* spch_recg (main.c:249-296) for B utterances: noise_atap(first n_len) -> VAD(U) -> get_mfcc(seg 0)
  * -> dtw against the bank (the handle's matcher, sr_set_match) -> argmin -> cmd = idx / SR_FTR_PER_COMM. Any output
- * pointer may be NULL. */
+ * pointer may be NULL. A call writes the fields' [B] records and nothing else of the caller's memory, with two
+ * exceptions in every form: atap[b] is left untouched when n_len % 240 != 0, and of ftr[b] only frm_num and its first
+ * frm_num rows are written (as sr_mfcc_batch). */
 typedef struct {
     atap_tag  *atap;       /* [B]            */
     uint32_t  *seg_off;    /* [B][3][2]      */

@@ -502,7 +502,7 @@ static int dtw_host(HostCall &c, const BankView &bank, const v_ftr_tag *in, uint
                     uint32_t *score, uint32_t *best_idx, uint32_t *best_dis) {
     sr_handle *h = c.h;
     const v_ftr_tag *d_in = c.in(h->ftr, in, (size_t)B * kFtrBytes);
-    u32 *d_score = score ? c.out(h->score, score, (size_t)B * bank.n * 4, 4) : nullptr;
+    u32 *d_score = score ? c.out(h->score, score, (size_t)B * bank.n * 4) : nullptr;
     u32 *d_idx = c.out(h->bidx, best_idx, (size_t)B * 4), *d_dis = c.out(h->bdis, best_dis, (size_t)B * 4);
     c.run([&] { return dtw_dev_impl(h, bank, d_in, B, flags, band_r, d_score, best_idx ? d_idx : nullptr,
                                     best_dis ? d_dis : nullptr, nullptr, nullptr); });
@@ -560,7 +560,8 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
     const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
     const atap_tag *d_atap = c.in(h->atap, atap, (size_t)B * sizeof(atap_tag));
     const u32 *d_seg = c.in(h->seg, seg, (size_t)B * seg_stride * 4);
-    v_ftr_tag *d_ftr = c.out(h->ftr, ftr, (size_t)B * kFtrBytes);
+    v_ftr_tag *d_ftr = c.in(h->ftr, ftr, (size_t)B * kFtrBytes);     // in / out: rows >= frm_num keep the caller's bytes
+    c.out(h->ftr, ftr, (size_t)B * kFtrBytes);
     c.run([&] { return sr_mfcc_batch_dev(h, d_pcm, U, B, d_seg, seg_stride, d_atap, d_ftr); });
     return c.finish();
 }
@@ -622,8 +623,10 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     memset(&d, 0, sizeof d);
     for_each_output(h, [&](auto m, DevBuf &buf, size_t bytes) {
         if (!(o->*m)) return;
-        // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36)
-        if constexpr (std::is_same_v<decltype(m), atap_tag *sr_recog_out::*>) c.in(buf, o->*m, B * bytes);
+        // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36); so is ftr: get_mfcc writes
+        // frm_num and rows < frm_num only (MFCC.C), the caller's other bytes must come back as they were
+        if constexpr (std::is_same_v<decltype(m), atap_tag *sr_recog_out::*> || std::is_same_v<decltype(m), v_ftr_tag *sr_recog_out::*>)
+            c.in(buf, o->*m, B * bytes);
         d.*m = c.out(buf, o->*m, B * bytes);
     });
     uint32_t issued = 0;
