@@ -284,6 +284,63 @@ int sr_dtw_path_batch(sr_handle *h, const v_ftr_tag *in, const v_ftr_tag *mdl, u
 int sr_average_bank(sr_handle *h, const void *bank, uint32_t slot_stride, uint32_t K, uint32_t G, int band_r,
                     uint32_t iters, void *bank_out, uint32_t *score /* [G][K] or NULL */, uint32_t *anchor /* [G] or NULL */);
 
+/* ---- connected words: one-pass DP over the template bank (extension) ------------------------------------------------
+ * sr_mfcc_long_batch: get_mfcc (MFCC.C:86-191) with vv_frm_max replaced by frm_cap (1 <= frm_cap <= SR_CONN_FRM_MAX), in
+ * the handle's geometry. With F the frame count of MFCC.C:102, F <= frm_cap writes rows 0..F-1 of feat[b] and
+ * frm_num[b] = F; otherwise frm_num[b] = 0 and no row is written. Rows at or past frm_num[b] keep the caller's bytes. NULL
+ * segments, and x[-1] = mid_val for a segment that starts at sample 0, behave as in sr_mfcc_batch. Each segment is cut into
+ * pieces of at most 119 frames, piece k starting at sample start + 80*119*k, and every piece runs through the get_mfcc
+ * kernel; a piece past the first reads its real preceding sample, so every frame is the reference's own frame: pinned to
+ * the reference piece by piece. With frm_cap = 119 the result equals sr_mfcc_batch byte for byte. */
+#define SR_CONN_FRM_MAX  818u   /* frames of a 65 535-sample segment: (65535 - 160) / 80 + 1 */
+#define SR_CONN_SLOT_MAX 128u   /* widest bank sr_connected_batch and sr_recognise_connected_batch accept */
+int sr_mfcc_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *seg, uint32_t seg_stride,
+                       const atap_tag *atap /* [B] */, uint32_t frm_cap, int16_t *feat /* [B][frm_cap][12] */,
+                       uint32_t *frm_num /* [B] */);
+/* sr_connected_batch: the best sequence of words for each of B feature sequences X = x_0..x_{N-1} (N = frm_num[b] <=
+ * SR_CONN_FRM_MAX, rows at feat + b*frm_stride*12) against the handle's bank. Members are the slots with save_sign ==
+ * SR_SAVE_MASK and 1 <= frm_num <= 119; d(i, t, j) = get_dis(x_i, y_{t,j}) (DTW.C:45-62). With E(-1) = 0 and D(-1,.,.) = inf:
+ *   D(i, t, 0)      = d + min(D(i-1, t, 0), E(i-1) + penalty)
+ *   D(i, t, j >= 1) = d + min(D(i-1, t, j), D(i, t, j-1), D(i-1, t, j-1))
+ *   E(i) = min over members t of D(i, t, M_t - 1),   total = E(N-1)
+ * so total = min over segmentations of X and words t_k of the sum of (unnormalised full-matrix DTW + penalty). Ties: every
+ * cell carries the input frame its word started at, and takes the predecessor with the smallest D, on equal D the one whose
+ * word started later (a new word wins a tie); E(i) ties to the lowest slot (main.c:285-289). The trace-back from frame
+ * N-1 gives the words in time order: dis = the word's own path sum (the unnormalised full DTW of its frames against the
+ * slot), sum(dis + penalty) = total. n_words[b] is the true count, only the first min(n_words, max_words) records of
+ * words[b] are written. N = 0: 0 words, total 0; no member: 0 words, total UINT64_MAX. No band, no 2:1 guard; the handle's
+ * sr_set_match is not read. A bank wider than SR_CONN_SLOT_MAX, a frm_num[b] above SR_CONN_FRM_MAX or frm_stride, or a NULL
+ * n_words with B > 0 fail the call before anything is written. Parity unpinned: the reference decodes one word per
+ * segment; the checker is this project's own CPU restatement. */
+typedef struct {
+    uint32_t slot, cmd;      /* bank slot of the word; cmd = slot / SR_FTR_PER_COMM (main.c:292)     */
+    uint32_t segment;        /* VAD segment it came from (0 in sr_connected_batch)                   */
+    uint32_t start, end;     /* input frames [start, end) of that segment                            */
+    uint32_t dis;            /* the word's own path sum: unnormalised full-matrix DTW of those frames */
+} sr_conn_word;
+int sr_connected_batch(sr_handle *h, const int16_t *feat /* [B][frm_stride][12] */, const uint32_t *frm_num /* [B] */,
+                       uint32_t frm_stride, uint32_t B, uint32_t penalty, uint32_t max_words,
+                       sr_conn_word *words /* [B][max_words] or NULL */, uint32_t *n_words /* [B] */,
+                       uint64_t *total /* [B] or NULL */);
+/* sr_recognise_connected_batch: noise_atap (first n_len) -> VAD(U) -> sr_mfcc_long_batch features (frm_cap =
+ * SR_CONN_FRM_MAX) of EVERY closed segment -> sr_connected_batch of each segment on its own -> the words concatenated in
+ * segment order, each keeping its segment. Word boundaries never cross a VAD pause. total = the saturating sum over the
+ * decoded segments (0 when none has frames). status follows spch_recg on segment 0: SR_ST_VAD_FAIL if it never closed,
+ * SR_ST_MFCC_FAIL if it has 0 frames, SR_ST_OK otherwise; later segments with 0 frames add no words. Any output pointer may
+ * be NULL. The call writes the fields' [B] records and nothing else, except that atap[b] is left untouched when
+ * n_len % 240 != 0 and only the first min(n_words, max_words) records of words[b] are written. */
+typedef struct {
+    atap_tag     *atap;      /* [B]                */
+    uint32_t     *seg_off;   /* [B][3][2]          */
+    uint32_t     *frm_num;   /* [B][3]             */
+    uint32_t     *n_words;   /* [B]                */
+    sr_conn_word *words;     /* [B][max_words]     */
+    uint64_t     *total;     /* [B]                */
+    uint8_t      *status;    /* [B] SR_ST_*        */
+} sr_conn_out;
+int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
+                                 uint32_t penalty, uint32_t max_words, const sr_conn_out *out);
+
 /* ---- streaming front end (stands in for record(), main.c:77-102 / ADC.C:11-103) ----------------------------
  * n_streams concurrent captures of max_samples samples each, fed in chunks -- in lock step (sr_streams_push) or every
  * stream at its own pace (sr_streams_push_ragged). Each push advances noise_atap (once the first n_len samples of a
@@ -373,7 +430,8 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
  * stream and returns (tag, milliseconds) per timed launch in issue order, then rearms. Tags: 0 noise_atap+VAD,
  * 1 get_mfcc, 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP, in sr_dtw_batch* and in recognise
  * calls under the SR_DTW_BAND matcher), 7 the banded DP with its path (every pass of sr_dtw_path_batch and
- * sr_average_bank that aligns), 8 sr_average_bank's template update. max_records = 0 disables. */
+ * sr_average_bank that aligns), 8 sr_average_bank's template update, 9 the connected-word decoder (sr_connected_batch,
+ * sr_recognise_connected_batch; their get_mfcc launches are tag 1). max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

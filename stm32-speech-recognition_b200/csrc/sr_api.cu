@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 4; }
+int sr_abi_version(void) { return 5; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -179,7 +179,7 @@ int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
-       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8 };
+       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9 };
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
@@ -787,6 +787,191 @@ int sr_average_bank(sr_handle *h, const void *bank, uint32_t slot_stride, uint32
         });
     c.launch(TAG_NONE, "launch_pack_slots", [&] { return launch_pack_slots(d_tpl, d_st, G, d_out, K * slot_stride, h->stream); });
     return c.finish();
+}
+
+}  // extern "C"
+
+// ---- long features and connected words ----------------------------------------------------------------------------
+// frame count of a segment, MFCC.C:102-107 as mfcc_frames (sr_mfcc_core.cuh) counts it, without the vv_frm_max cap
+static u32 long_frames(u32 st, u32 en, u32 U, u32 frame_len) {
+    if (st == SR_SEG_NULL || en == SR_SEG_NULL || en > U || st > en) return 0;
+    const u32 len = en - st;
+    return len < frame_len ? 0u : (len - frame_len) / SR_FRAME_MOV + 1u;
+}
+
+// get_mfcc pieces of long segments: piece k of a segment of F frames is frames [119k, min(119(k+1), F)), a segment of
+// its own that starts at sample start + 80*119*k of the utterance's row (so x[-1] is pinned only for a piece at sample 0)
+struct LongPieces {
+    std::vector<u32> seg, row, dst;       // [P][2] start / end sample, [P] PCM row, [P][2] first long feature row / frames
+    std::vector<atap_tag> atap;           // [P] the utterance's
+    void add(u32 st, u32 F, u32 frame_len, u32 r, const atap_tag &a, u32 row0) {
+        for (u32 f0 = 0; f0 < F; f0 += SR_VV_FRM_MAX) {
+            const u32 nf = std::min(F - f0, SR_VV_FRM_MAX), ps = st + f0 * SR_FRAME_MOV;
+            seg.insert(seg.end(), {ps, ps + (nf - 1) * SR_FRAME_MOV + frame_len});
+            row.push_back(r);
+            dst.insert(dst.end(), {row0 + f0, nf});
+            atap.push_back(a);
+        }
+    }
+    u32 size() const { return (u32)row.size(); }
+};
+
+constexpr u32 kPieceChunk = 8192;         // pieces per get_mfcc launch: 8192 x 2860 B of piece features
+
+// the pieces through get_mfcc in the handle's geometry (tag 1), kPieceChunk at a time, their rows gathered into d_feat
+static void run_pieces(HostCall &c, const u16 *d_pcm, u32 U, u32 n_rows, const LongPieces &pc, s16 *d_feat) {
+    sr_handle *h = c.h;
+    const u32 P = pc.size();
+    for (u32 p0 = 0; p0 < P && !c.rc; p0 += kPieceChunk) {
+        const u32 np = std::min(P - p0, kPieceChunk);
+        u32 *tab = c.ws<u32>(h->conn[0], (size_t)np * 5 * 4);
+        atap_tag *d_atap = c.ws<atap_tag>(h->conn[1], (size_t)np * sizeof(atap_tag));
+        void *d_pf = c.ws(h->conn[2], (size_t)np * kFtrBytes);
+        if (c.rc) return;
+        u32 *d_seg = tab, *d_row = tab + 2 * (size_t)np, *d_dst = tab + 3 * (size_t)np;
+        c.h2d(d_seg, pc.seg.data() + 2 * (size_t)p0, (size_t)np * 8);
+        c.h2d(d_row, pc.row.data() + p0, (size_t)np * 4);
+        c.h2d(d_dst, pc.dst.data() + 2 * (size_t)p0, (size_t)np * 8);
+        c.h2d(d_atap, pc.atap.data() + p0, (size_t)np * sizeof(atap_tag));
+        c.launch(TAG_MFCC, "launch_mfcc_h (pieces)", [&] { return launch_mfcc_h(h, d_pcm, U, np, d_seg, 2, d_atap, d_pf, d_row, n_rows); });
+        c.launch(TAG_NONE, "launch_conn_gather", [&] { return launch_conn_gather(d_pf, d_dst, np, d_feat, h->num_sms, h->stream); });
+    }
+}
+
+extern "C" {
+
+// get_mfcc with vv_frm_max replaced by frm_cap: the frame counts and the piece plan come from the segment offsets on the
+// host, every feature row from the get_mfcc kernel
+int sr_mfcc_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *seg, uint32_t seg_stride,
+                       const atap_tag *atap, uint32_t frm_cap, int16_t *feat, uint32_t *frm_num) {
+    SR_REQUIRE(h, h && (B == 0 || (pcm && seg && atap && feat && frm_num)));
+    SR_REQUIRE(h, seg_stride >= 2 && frm_cap >= 1 && frm_cap <= SR_CONN_FRM_MAX && (uint64_t)B * frm_cap < (1ull << 32));
+    if (B == 0) return 0;
+    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
+    std::vector<u32> F(B);
+    LongPieces pc;
+    for (u32 b = 0; b < B; ++b) {
+        const u32 st = seg[(size_t)b * seg_stride], f = long_frames(st, seg[(size_t)b * seg_stride + 1], U, frame_len);
+        F[b] = f <= frm_cap ? f : 0u;
+        pc.add(st, F[b], frame_len, b, atap[b], b * frm_cap);
+    }
+    HostCall c(h, "sr_mfcc_long_batch");
+    const size_t fbytes = (size_t)B * frm_cap * 24;
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    s16 *d_feat = c.in(h->conn[3], reinterpret_cast<const s16 *>(feat), fbytes);   // in / out: rows >= frm_num keep the caller's bytes
+    c.out(h->conn[3], feat, fbytes);
+    run_pieces(c, d_pcm, U, B, pc, d_feat);
+    const int rc = c.finish();
+    if (rc == 0) memcpy(frm_num, F.data(), (size_t)B * 4);
+    return rc;
+}
+
+// the one-pass DP of B feature sequences against the handle's bank (dtw_connected_kernel, tag 9)
+int sr_connected_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_num, uint32_t frm_stride, uint32_t B,
+                       uint32_t penalty, uint32_t max_words, sr_conn_word *words, uint32_t *n_words, uint64_t *total) {
+    SR_REQUIRE(h, h && (B == 0 || (feat && frm_num && n_words)));
+    if (B == 0) return 0;
+    SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
+    for (u32 b = 0; b < B; ++b) SR_REQUIRE(h, frm_num[b] <= SR_CONN_FRM_MAX && frm_num[b] <= frm_stride);
+    HostCall c(h, "sr_connected_batch");
+    const s16 *d_feat = c.in(h->conn[3], feat, (size_t)B * frm_stride * 24);
+    const u32 *d_frm = c.in(h->conn[4], frm_num, (size_t)B * 4);
+    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
+    sr_conn_word *d_words = nullptr;
+    if (words && max_words) {                            // in / out: records past n_words keep the caller's bytes
+        d_words = c.in(h->conn[7], words, wbytes);
+        c.out(h->conn[7], words, wbytes);
+    }
+    u32 *d_nw = c.out(h->conn[8], n_words, (size_t)B * 4);
+    u64 *d_total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
+    const BankView &bk = h->bank;
+    c.launch(TAG_CONN, "launch_dtw_connected", [&] {
+        return launch_dtw_connected(d_feat, frm_stride, d_frm, nullptr, B, bk.p, bk.n, bk.stride, penalty, max_words, d_words,
+                                    d_nw, d_total, h->stream);
+    });
+    return c.finish();
+}
+
+// noise_atap + VAD, then (after one synchronisation: the piece plan needs the segments) the long features of every closed
+// segment packed back to back, one decoder sequence per segment with frames, and the join of each capture's segments
+int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, uint32_t penalty,
+                                 uint32_t max_words, const sr_conn_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
+    if (B == 0) return 0;
+    SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
+    HostCall c(h, "sr_recognise_connected_batch");
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    atap_tag *d_atap;
+    if (o->atap) d_atap = c.in(h->atap, o->atap, (size_t)B * sizeof(atap_tag));   // in / out: untouched when n_len % 240 != 0
+    else {
+        d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
+        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
+    }
+    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
+    c.launch(TAG_VAD, "launch_vad", [&] { return launch_vad(d_pcm, U, B, n_len, U, 1, 1, d_atap, d_seg, h->num_sms, h->stream, vad_work(h)); });
+    std::vector<u32> seg((size_t)B * 6);
+    std::vector<atap_tag> atap(B);
+    if (d_seg) c.ck("copy back", cudaMemcpyAsync(seg.data(), d_seg, (size_t)B * 24, cudaMemcpyDeviceToHost, h->stream));
+    if (d_atap) c.ck("copy back", cudaMemcpyAsync(atap.data(), d_atap, (size_t)B * sizeof(atap_tag), cudaMemcpyDeviceToHost, h->stream));
+    c.ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+    if (c.rc) return c.finish();
+    // the plan: sequence q = the q-th closed segment with frames; rows and word records packed at seq_off[q][0] (frames)
+    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
+    std::vector<u32> frm((size_t)B * 3), seq_of((size_t)B * 3, 0xFFFFFFFFu), seq_off, seq_frm;
+    std::vector<u8> status(B);
+    LongPieces pc;
+    u32 rows = 0;
+    for (u32 b = 0; b < B; ++b) {
+        for (u32 k = 0; k < 3; ++k) {
+            const u32 st = seg[b * 6 + 2 * k], F = long_frames(st, seg[b * 6 + 2 * k + 1], U, frame_len);   // <= 818: U <= 65535
+            frm[b * 3 + k] = F;
+            if (!F) continue;
+            seq_of[b * 3 + k] = (u32)seq_frm.size();
+            seq_off.insert(seq_off.end(), {rows, rows});
+            seq_frm.push_back(F);
+            pc.add(st, F, frame_len, b, atap[b], rows);
+            rows += F;
+        }
+        status[b] = seg[b * 6 + 1] == SR_SEG_NULL ? SR_ST_VAD_FAIL : frm[b * 3] == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;   // main.c:261-274
+    }
+    const u32 nseq = (u32)seq_frm.size();
+    s16 *d_feat = c.ws<s16>(h->conn[3], (size_t)rows * 24);
+    run_pieces(c, d_pcm, U, B, pc, d_feat);
+    u32 *tab = c.ws<u32>(h->conn[4], ((size_t)nseq * 3 + (size_t)B * 3) * 4);         // seq_off | seq_frm | seq_of
+    sr_conn_word *d_sw = c.ws<sr_conn_word>(h->conn[5], (size_t)rows * sizeof(sr_conn_word));
+    u64 *d_stot = c.ws<u64>(h->conn[6], (size_t)nseq * 12);                           // seq totals | seq word counts
+    if (c.rc) return c.finish();
+    u32 *d_soff = tab, *d_sfrm = tab + 2 * (size_t)nseq, *d_sof = tab + 3 * (size_t)nseq;
+    u32 *d_snw = reinterpret_cast<u32 *>(d_stot + nseq);
+    c.h2d(d_soff, seq_off.data(), (size_t)nseq * 8);
+    c.h2d(d_sfrm, seq_frm.data(), (size_t)nseq * 4);
+    c.h2d(d_sof, seq_of.data(), (size_t)B * 12);
+    const BankView &bk = h->bank;
+    if (nseq)
+        c.launch(TAG_CONN, "launch_dtw_connected", [&] {
+            return launch_dtw_connected(d_feat, 0, d_sfrm, d_soff, nseq, bk.p, bk.n, bk.stride, penalty, 0, d_sw, d_snw, d_stot,
+                                        h->stream);
+        });
+    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
+    sr_conn_word *d_words = nullptr;
+    if (o->words && max_words) {                         // in / out: records past n_words keep the caller's bytes
+        d_words = c.in(h->conn[7], o->words, wbytes);
+        c.out(h->conn[7], o->words, wbytes);
+    }
+    u32 *d_nw = o->n_words ? c.out(h->conn[8], o->n_words, (size_t)B * 4) : nullptr;
+    u64 *d_total = o->total ? c.out(h->conn[9], reinterpret_cast<u64 *>(o->total), (size_t)B * 8) : nullptr;
+    if (d_words || d_nw || d_total)
+        c.launch(TAG_NONE, "launch_conn_concat", [&] {
+            return launch_conn_concat(d_sof, d_soff, d_sw, d_snw, d_stot, B, max_words, d_words, d_nw, d_total, h->stream);
+        });
+    const int rc = c.finish();
+    if (rc) return rc;
+    if (o->atap) memcpy(o->atap, atap.data(), (size_t)B * sizeof(atap_tag));
+    if (o->seg_off) memcpy(o->seg_off, seg.data(), (size_t)B * 24);
+    if (o->frm_num) memcpy(o->frm_num, frm.data(), (size_t)B * 12);
+    if (o->status) memcpy(o->status, status.data(), B);
+    return 0;
 }
 
 // One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]

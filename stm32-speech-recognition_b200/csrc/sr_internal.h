@@ -49,6 +49,15 @@ cudaError_t launch_dtw_align(const void *in_base, u32 in_stride, const void *tpl
                              void *tpl_out, u32 *anchor_out, int num_sms, cudaStream_t st);
 cudaError_t launch_average_update(const void *bank, u32 slot_stride, u32 K, u32 G, const u32 *mask, const u8 *path,
                                   const u32 *path_len, void *tpl, cudaStream_t st);
+// the connected-word decoder over B feature sequences (seq_off: [B][2] first row, first word record, or NULL: b * frm_stride,
+// b * max_words), the gather of get_mfcc pieces into long feature rows and the join of a capture's segments (sr_dtw_connected.cu)
+cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 B,
+                                 const void *bank, u32 T, u32 slot_stride, u32 penalty, u32 max_words, sr_conn_word *words,
+                                 u32 *n_words, u64 *total, cudaStream_t st);
+cudaError_t launch_conn_gather(const void *pf, const u32 *pdst, u32 P, s16 *feat, int num_sms, cudaStream_t st);
+cudaError_t launch_conn_concat(const u32 *seq_of, const u32 *seq_off, const sr_conn_word *seq_words, const u32 *seq_nw,
+                               const u64 *seq_total, u32 B, u32 max_words, sr_conn_word *words, u32 *n_words, u64 *total,
+                               cudaStream_t st);
 cudaError_t launch_sqrt_check(u32 lo, u32 hi, unsigned long long *bad_dev, cudaStream_t st);
 cudaError_t launch_unpack12(const void *packed, u64 n_samples, u16 *out, cudaStream_t st);
 class PackPool;
@@ -167,6 +176,7 @@ struct sr_handle {
     // 12-bit expander, the sqrt check, enrol's bank image, dtw()'s one-slot bank) and is never read by a recognise call
     DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
     DevBuf align[6];                                   // sr_dtw_path_batch / sr_average_bank: pairs, paths, templates, scores
+    DevBuf conn[10];                                   // long features and the connected-word decoder: pieces, features, words
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };

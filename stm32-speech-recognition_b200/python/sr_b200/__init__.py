@@ -45,6 +45,16 @@ def _recog_arrays(B, T, want):
     return {k: np.zeros(*shape[k]) for k in RECOG_FIELDS if k in want}
 
 
+CONN_FRM_MAX = 818             # SR_CONN_FRM_MAX: frames of a 65 535-sample segment
+CONN_SLOT_MAX = 128            # SR_CONN_SLOT_MAX: the widest bank of the connected-word decoder
+WORD_DTYPE = np.dtype([(k, "<u4") for k in ("slot", "cmd", "segment", "start", "end", "dis")])   # sr_conn_word
+CONN_FIELDS = ("atap", "seg_off", "frm_num", "n_words", "words", "total", "status")
+
+
+class ConnOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in CONN_FIELDS]
+
+
 class StreamEvent(C.Structure):
     _fields_ = [(k, C.c_uint32) for k in ("stream", "segment", "start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")]
 
@@ -88,6 +98,9 @@ def lib():
         L.sr_get_mdl_batch.argtypes = [vp, vp, vp, u32, vp, vp]
         L.sr_dtw_path_batch.argtypes = [vp, vp, vp, u32, i32, vp, vp, vp]
         L.sr_average_bank.argtypes = [vp, vp, u32, u32, u32, i32, u32, vp, vp, vp]
+        L.sr_mfcc_long_batch.argtypes = [vp, vp, u32, u32, vp, u32, vp, u32, vp, vp]
+        L.sr_connected_batch.argtypes = [vp, vp, vp, u32, u32, u32, u32, vp, vp, vp]
+        L.sr_recognise_connected_batch.argtypes = [vp, vp, u32, u32, u32, u32, u32, C.POINTER(ConnOut)]
         L.sr_streams_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
         L.sr_streams_destroy.argtypes = [vp]
         L.sr_streams_reset.argtypes = [vp]
@@ -325,6 +338,44 @@ class Handle:
         self._ck(lib().sr_average_bank(self._h, _p(bank), slot_stride, K, G, int(band_r), iters, _p(out), _p(score),
                                        _p(anchor)))
         return out, score, anchor
+
+    def mfcc_long(self, pcm, seg, atap, frm_cap=CONN_FRM_MAX, feat=None):
+        """get_mfcc with vv_frm_max replaced by frm_cap (sr_mfcc_long_batch): (feat [B, frm_cap, 12] i16, frm_num [B]);
+        rows at or past frm_num keep what `feat` held (zeros when it is None)"""
+        B, U = pcm.shape
+        seg = np.ascontiguousarray(seg, np.uint32).reshape(B, -1)
+        feat = np.zeros((B, frm_cap, 12), np.int16) if feat is None else feat
+        assert feat.shape == (B, frm_cap, 12) and feat.dtype == np.int16 and feat.flags["C_CONTIGUOUS"]
+        frm = np.zeros(B, np.uint32)
+        self._ck(lib().sr_mfcc_long_batch(self._h, _p(pcm), U, B, _p(seg), seg.shape[1], _p(atap), frm_cap, _p(feat), _p(frm)))
+        return feat, frm
+
+    def connected(self, feat, frm_num, penalty, max_words, words=None, want_total=True):
+        """connected words of feature sequences feat [B, frm_stride, 12] i16 of frm_num [B] frames against the bank
+        (sr_connected_batch): (words [B, max_words] WORD_DTYPE, n_words [B], total [B] u64 or None); records past n_words
+        keep what `words` held (zeros when it is None)"""
+        feat = np.ascontiguousarray(feat, np.int16)
+        B, stride = feat.shape[0], feat.shape[1]
+        frm_num = np.ascontiguousarray(frm_num, np.uint32)
+        words = np.zeros((B, max_words), WORD_DTYPE) if words is None else words
+        n_words = np.zeros(B, np.uint32)
+        total = np.zeros(B, np.uint64) if want_total else None
+        self._ck(lib().sr_connected_batch(self._h, _p(feat), _p(frm_num), stride, B, penalty, max_words, _p(words),
+                                          _p(n_words), _p(total)))
+        return words, n_words, total
+
+    def recognise_connected(self, pcm, penalty, max_words, n_len=2400, want=CONN_FIELDS, out=None):
+        """noise_atap -> VAD -> long features of every segment -> connected words (sr_recognise_connected_batch): a dict
+        of the sr_conn_out fields named in `want` (or the arrays of `out`, which the call fills in place)"""
+        B, U = pcm.shape
+        if out is None:
+            shape = {"atap": (B, ATAP_DTYPE), "seg_off": ((B, 3, 2), np.uint32), "frm_num": ((B, 3), np.uint32),
+                     "n_words": (B, np.uint32), "words": ((B, max_words), WORD_DTYPE), "total": (B, np.uint64),
+                     "status": (B, np.uint8)}
+            out = {k: np.zeros(*shape[k]) for k in CONN_FIELDS if k in want}
+        o = ConnOut(*[_p(out.get(k)) for k in CONN_FIELDS])
+        self._ck(lib().sr_recognise_connected_batch(self._h, _p(pcm), U, B, n_len, penalty, max_words, C.byref(o)))
+        return out
 
     def fft_mag(self, frames):
         n, length = frames.shape
