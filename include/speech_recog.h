@@ -341,6 +341,49 @@ typedef struct {
 int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
                                  uint32_t penalty, uint32_t max_words, const sr_conn_out *out);
 
+/* ---- connected words under a finite-state grammar (extension, ABI version 6) ------------------------------------------
+ * A grammar is a nondeterministic finite-state network over commands: n_states states (1 <= n_states <=
+ * SR_GRAM_STATE_MAX), state 0 the start state; bit s of final_mask set means state s may end the sequence (final_mask != 0,
+ * no bit >= n_states); n_arcs arcs {from, to, cmd_mask}, an arc letting a word whose command c = slot / SR_FTR_PER_COMM has
+ * bit c set in cmd_mask lead from `from` to `to` (a bank has at most 128 slots: commands 0..31). No epsilon arcs; arcs may
+ * share (from, to) or overlap.
+ * A COPY is a pair (state s', member slot t) such that some arc into s' carries cmd(t); members as in sr_connected_batch
+ * (signed, 1 <= frm_num <= 119). Copies are numbered state-major, then by slot; src(c) is the set of states s with an arc
+ * s -> s' carrying cmd(t). At most SR_GRAM_COPY_MAX copies. With E_s(-1) = 0 for s = 0 and +inf otherwise, D(-1,.,.) = inf
+ * and d = get_dis (DTW.C:45-62):
+ *   D(i, c, 0)      = d + min(D(i-1, c, 0), min_{s in src(c)} E_s(i-1) + penalty)
+ *   D(i, c, j >= 1) = d + min(D(i-1, c, j), D(i, c, j-1), D(i-1, c, j-1))
+ *   E_s'(i) = min over copies c of state s' of D(i, c, M_t - 1),   total = min over final states s of E_s(N-1)
+ * Ties as in sr_connected_batch: cells prefer the later word start, E_s ties to the lowest copy (within a state the lowest
+ * slot), the final state ties to the lowest state. Trace-back from the chosen final state at N-1: its record gives (copy
+ * c, start b); the word's source state is the argmin over s in src(c) of E_s(b-1) (D only, ties to the lowest s; state 0
+ * at b = 0). Words in time order, dis = E(end-1) - E_src(b-1) - penalty. N = 0: 0 words, total 0 if state 0 is final,
+ * else UINT64_MAX. No accepting path: 0 words, total UINT64_MAX. The one-state loop grammar (n_states 1, final_mask 1, one
+ * arc 0 -> 0 carrying every command) is exactly sr_connected_batch. */
+#define SR_GRAM_STATE_MAX 16u
+#define SR_GRAM_COPY_MAX  128u   /* = SR_CONN_SLOT_MAX: one decoder warp per copy */
+typedef struct { uint32_t from, to, cmd_mask; } sr_gram_arc;
+typedef struct { uint32_t n_states, final_mask, n_arcs; const sr_gram_arc *arcs; } sr_grammar;
+/* sr_connected_grammar_batch: sr_connected_batch under grammar g, with its argument rules and footprint (only the first
+ * min(n_words, max_words) records of words[b] are written), plus B * frm_stride < 2^32 (feature rows are 32-bit
+ * indices; the limit is 96 GB of features). A grammar without copies against the bank (no arcs, or arcs whose commands
+ * have no member) is valid: 0 words, total as for N = 0 or no accepting path. A NULL or malformed grammar (state count, final mask, an arc
+ * endpoint >= n_states, NULL arcs with n_arcs > 0) fails the call, and so does a grammar with more than SR_GRAM_COPY_MAX
+ * copies against the handle's bank, whose membership is read from the bank (device memory, 4 header bytes per slot) when
+ * the call runs: before any launch and before any caller byte is written. B = 0 launches nothing. */
+int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat /* [B][frm_stride][12] */, const uint32_t *frm_num /* [B] */,
+                               uint32_t frm_stride, uint32_t B, const sr_grammar *g, uint32_t penalty, uint32_t max_words,
+                               sr_conn_word *words /* [B][max_words] or NULL */, uint32_t *n_words /* [B] */,
+                               uint64_t *total /* [B] or NULL */);
+/* sr_recognise_connected_grammar_batch: noise_atap -> VAD -> long features of every closed segment, as
+ * sr_recognise_connected_batch, then ONE decode per capture under g: the capture's segments with frames are one sequence,
+ * their frames back to back, and at the first frame of a later segment every within-word cell is reset to +inf, so no word
+ * crosses a pause while E, and with it the grammar state, carries over. Words keep their segment and segment-relative
+ * start / end. status, atap and the footprint are those of sr_recognise_connected_batch; the grammar rules are those of
+ * sr_connected_grammar_batch. Under the loop grammar the result equals sr_recognise_connected_batch bit for bit. */
+int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
+                                         const sr_grammar *g, uint32_t penalty, uint32_t max_words, const sr_conn_out *out);
+
 /* ---- streaming front end (stands in for record(), main.c:77-102 / ADC.C:11-103) ----------------------------
  * n_streams concurrent captures of max_samples samples each, fed in chunks -- in lock step (sr_streams_push) or every
  * stream at its own pace (sr_streams_push_ragged). Each push advances noise_atap (once the first n_len samples of a
@@ -431,7 +474,8 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
  * 1 get_mfcc, 2 status, 3 best-init, 4 dtw (greedy), 5 best-final, 6 dtw (banded DP, in sr_dtw_batch* and in recognise
  * calls under the SR_DTW_BAND matcher), 7 the banded DP with its path (every pass of sr_dtw_path_batch and
  * sr_average_bank that aligns), 8 sr_average_bank's template update, 9 the connected-word decoder (sr_connected_batch,
- * sr_recognise_connected_batch; their get_mfcc launches are tag 1). max_records = 0 disables. */
+ * sr_recognise_connected_batch; their get_mfcc launches are tag 1), 10 the grammar decoder (sr_connected_grammar_batch,
+ * sr_recognise_connected_grammar_batch; their get_mfcc launches are tag 1). max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

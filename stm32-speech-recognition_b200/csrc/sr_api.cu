@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 5; }
+int sr_abi_version(void) { return 6; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -179,7 +179,8 @@ int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
-       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9 };
+       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
+       TAG_GRAM = 10 };
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
@@ -965,6 +966,177 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
         c.launch(TAG_NONE, "launch_conn_concat", [&] {
             return launch_conn_concat(d_sof, d_soff, d_sw, d_snw, d_stot, B, max_words, d_words, d_nw, d_total, h->stream);
         });
+    const int rc = c.finish();
+    if (rc) return rc;
+    if (o->atap) memcpy(o->atap, atap.data(), (size_t)B * sizeof(atap_tag));
+    if (o->seg_off) memcpy(o->seg_off, seg.data(), (size_t)B * 24);
+    if (o->frm_num) memcpy(o->frm_num, frm.data(), (size_t)B * 12);
+    if (o->status) memcpy(o->status, status.data(), B);
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- connected words under a grammar ------------------------------------------------------------------------------
+// g's copies against the handle's bank (sr_grammar in speech_recog.h): copy[c] = slot | state << 8 | src << 16, numbered
+// state-major, then by slot. Membership comes from the bank's 4-byte headers, read from the device (sr_set_bank_dev banks
+// are borrowed device memory). Fails, writing nothing, on a NULL or malformed grammar or more than SR_GRAM_COPY_MAX copies.
+static int gram_copies(sr_handle *h, const sr_grammar *g, std::vector<u32> &copy) {
+    SR_REQUIRE(h, g != nullptr);
+    SR_REQUIRE(h, g->n_states >= 1 && g->n_states <= SR_GRAM_STATE_MAX);
+    SR_REQUIRE(h, g->final_mask != 0 && (g->final_mask >> g->n_states) == 0);
+    SR_REQUIRE(h, g->n_arcs == 0 || g->arcs != nullptr);
+    for (u32 a = 0; a < g->n_arcs; ++a) SR_REQUIRE(h, g->arcs[a].from < g->n_states && g->arcs[a].to < g->n_states);
+    SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
+    const BankView &bk = h->bank;
+    std::vector<u32> hdr(bk.n);
+    if (bk.n && bk.p) {
+        SR_CK(h, cudaMemcpy2DAsync(hdr.data(), 4, bk.p, bk.stride, 4, bk.n, cudaMemcpyDeviceToHost, h->stream));
+        SR_CK(h, cudaStreamSynchronize(h->stream));
+    }
+    copy.clear();
+    for (u32 to = 0; to < g->n_states; ++to)
+        for (u32 t = 0; t < bk.n; ++t) {
+            const u32 frm = hdr[t] >> 16;
+            if ((hdr[t] & 0xFFFFu) != SR_SAVE_MASK || frm < 1 || frm > SR_VV_FRM_MAX) continue;   // decode_frm's rule
+            u32 src = 0;
+            for (u32 a = 0; a < g->n_arcs; ++a)
+                if (g->arcs[a].to == to && ((g->arcs[a].cmd_mask >> (t / SR_FTR_PER_COMM)) & 1u)) src |= 1u << g->arcs[a].from;
+            if (src) copy.push_back(t | to << 8 | src << 16);
+        }
+    SR_REQUIRE(h, copy.size() <= SR_GRAM_COPY_MAX);
+    return 0;
+}
+
+constexpr size_t kGramRecBytes = 256u << 20;   // records per launch: sum of N * n_states * 8 B over its sequences
+
+// the grammar decoder (tag 10) over B sequences of frames N[b]: seq [B][3] holds each first feature row and its segments
+// (the record rows are filled in here). Launches take consecutive sequences whose records fit kGramRecBytes.
+static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &N, std::vector<u32> &seq,
+                        const std::vector<u32> &copy, const sr_grammar *g, u32 penalty, u32 max_words, sr_conn_word *d_words,
+                        u32 *d_nw, u64 *d_total) {
+    sr_handle *h = c.h;
+    const u32 B = (u32)N.size(), S = g->n_states;
+    std::vector<u32> cut{0};                             // launch boundaries
+    size_t rows = 0, rows_max = 0;
+    for (u32 b = 0; b < B; ++b) {
+        if (rows && (rows + N[b]) * S * 8 > kGramRecBytes) { cut.push_back(b); rows = 0; }
+        seq[3 * (size_t)b + 1] = (u32)rows;
+        rows += N[b];
+        rows_max = std::max(rows_max, rows);
+    }
+    cut.push_back(B);
+    static const u32 kNoCopy = 0;                         // the one staged word of a grammar without copies (C = 0:
+    const u32 *ctab = copy.empty() ? &kNoCopy : copy.data();   // no warp walks, every sequence decodes to 0 words)
+    u32 *d_copy = c.in(h->gram[0], ctab, std::max<size_t>(copy.size(), 1) * 4);
+    u32 *d_seq = c.in(h->gram[1], seq.data(), (size_t)B * 12);
+    u32 *d_frm = c.in(h->gram[2], N.data(), (size_t)B * 4);
+    u64 *d_rec = c.ws<u64>(h->gram[3], std::max<size_t>(rows_max, 1) * S * 8);
+    const BankView &bk = h->bank;
+    for (size_t k = 0; k + 1 < cut.size(); ++k) {
+        const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
+        c.launch(TAG_GRAM, "launch_dtw_grammar", [&] {
+            return launch_dtw_grammar(d_feat, d_frm + b0, d_seq + 3 * (size_t)b0, nb, bk.p, bk.stride, d_copy, (u32)copy.size(), S,
+                                      g->final_mask, penalty, max_words, d_words ? d_words + (size_t)b0 * max_words : nullptr,
+                                      d_nw ? d_nw + b0 : nullptr, d_total ? d_total + b0 : nullptr, d_rec, h->stream);
+        });
+    }
+}
+
+extern "C" {
+
+// sr_connected_batch under a grammar: the copies from the bank's headers, then the decoder (dtw_grammar_kernel, tag 10)
+int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_num, uint32_t frm_stride, uint32_t B,
+                               const sr_grammar *g, uint32_t penalty, uint32_t max_words, sr_conn_word *words, uint32_t *n_words,
+                               uint64_t *total) {
+    SR_REQUIRE(h, h && (B == 0 || (feat && frm_num && n_words)));
+    if (B == 0) return 0;
+    SR_REQUIRE(h, (uint64_t)B * frm_stride < (1ull << 32));
+    for (u32 b = 0; b < B; ++b) SR_REQUIRE(h, frm_num[b] <= SR_CONN_FRM_MAX && frm_num[b] <= frm_stride);
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    std::vector<u32> N(frm_num, frm_num + B), seq((size_t)B * 3);
+    for (u32 b = 0; b < B; ++b) {                          // one segment at frame 0
+        seq[3 * (size_t)b] = b * frm_stride;
+        seq[3 * (size_t)b + 2] = 1023u << 10 | 1023u << 20;
+    }
+    HostCall c(h, "sr_connected_grammar_batch");
+    const s16 *d_feat = c.in(h->conn[3], feat, (size_t)B * frm_stride * 24);
+    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
+    sr_conn_word *d_words = nullptr;
+    if (words && max_words) {                            // in / out: records past n_words keep the caller's bytes
+        d_words = c.in(h->conn[7], words, wbytes);
+        c.out(h->conn[7], words, wbytes);
+    }
+    u32 *d_nw = c.out(h->conn[8], n_words, (size_t)B * 4);
+    u64 *d_total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
+    run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d_words, d_nw, d_total);
+    return c.finish();
+}
+
+// noise_atap + VAD, one synchronisation, the long features of every closed segment packed back to back (a capture's
+// segments adjacent), then one decoder sequence per capture whose words go straight to the caller's records
+int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
+                                         const sr_grammar *g, uint32_t penalty, uint32_t max_words, const sr_conn_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
+    if (B == 0) return 0;
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    HostCall c(h, "sr_recognise_connected_grammar_batch");
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+    atap_tag *d_atap;
+    if (o->atap) d_atap = c.in(h->atap, o->atap, (size_t)B * sizeof(atap_tag));   // in / out: untouched when n_len % 240 != 0
+    else {
+        d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
+        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
+    }
+    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
+    c.launch(TAG_VAD, "launch_vad", [&] { return launch_vad(d_pcm, U, B, n_len, U, 1, 1, d_atap, d_seg, h->num_sms, h->stream, vad_work(h)); });
+    std::vector<u32> seg((size_t)B * 6);
+    std::vector<atap_tag> atap(B);
+    if (d_seg) c.ck("copy back", cudaMemcpyAsync(seg.data(), d_seg, (size_t)B * 24, cudaMemcpyDeviceToHost, h->stream));
+    if (d_atap) c.ck("copy back", cudaMemcpyAsync(atap.data(), d_atap, (size_t)B * sizeof(atap_tag), cudaMemcpyDeviceToHost, h->stream));
+    c.ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+    if (c.rc) return c.finish();
+    // the plan: capture b is sequence b, its segments with frames back to back from row seq[b][0]; segment k's first
+    // frame in that sequence (1023: no frames) is field k of seq[b][2]
+    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
+    std::vector<u32> frm((size_t)B * 3), N(B), seq((size_t)B * 3);
+    std::vector<u8> status(B);
+    LongPieces pc;
+    u32 rows = 0;
+    for (u32 b = 0; b < B; ++b) {
+        seq[3 * (size_t)b] = rows;
+        u32 segs = 0;
+        for (u32 k = 0; k < 3; ++k) {
+            const u32 st = seg[b * 6 + 2 * k], F = long_frames(st, seg[b * 6 + 2 * k + 1], U, frame_len);
+            frm[b * 3 + k] = F;
+            segs |= (F ? N[b] : 1023u) << (10 * k);
+            if (!F) continue;
+            pc.add(st, F, frame_len, b, atap[b], rows);
+            rows += F;
+            N[b] += F;
+        }
+        seq[3 * (size_t)b + 2] = segs;
+        // VAD's segments are disjoint, so a capture of U <= 65 535 samples has at most 818 frames over its segments
+        if (N[b] > SR_CONN_FRM_MAX) c.took(fail(h, "a capture's segments exceed SR_CONN_FRM_MAX frames", cudaSuccess));
+        status[b] = seg[b * 6 + 1] == SR_SEG_NULL ? SR_ST_VAD_FAIL : frm[b * 3] == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;   // main.c:261-274
+    }
+    if (c.rc) return c.finish();
+    s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(rows, 1) * 24);
+    run_pieces(c, d_pcm, U, B, pc, d_feat);
+    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
+    sr_conn_word *d_words = nullptr;
+    if (o->words && max_words) {                         // in / out: records past n_words keep the caller's bytes
+        d_words = c.in(h->conn[7], o->words, wbytes);
+        c.out(h->conn[7], o->words, wbytes);
+    }
+    u32 *d_nw = o->n_words ? c.out(h->conn[8], o->n_words, (size_t)B * 4) : nullptr;
+    u64 *d_total = o->total ? c.out(h->conn[9], reinterpret_cast<u64 *>(o->total), (size_t)B * 8) : nullptr;
+    if (d_words || d_nw || d_total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d_words, d_nw, d_total);
     const int rc = c.finish();
     if (rc) return rc;
     if (o->atap) memcpy(o->atap, atap.data(), (size_t)B * sizeof(atap_tag));

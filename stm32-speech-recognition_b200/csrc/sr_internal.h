@@ -58,6 +58,11 @@ cudaError_t launch_conn_gather(const void *pf, const u32 *pdst, u32 P, s16 *feat
 cudaError_t launch_conn_concat(const u32 *seq_of, const u32 *seq_off, const sr_conn_word *seq_words, const u32 *seq_nw,
                                const u64 *seq_total, u32 B, u32 max_words, sr_conn_word *words, u32 *n_words, u64 *total,
                                cudaStream_t st);
+// the grammar decoder over B sequences (seq: [B][3] first feature row, first record row, segment first frames) against C
+// copies of bank slots (copy: [C] slot | state << 8 | src << 16), records in rec (sr_dtw_grammar.cu)
+cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 B, const void *bank, u32 slot_stride,
+                               const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
+                               u32 *n_words, u64 *total, u64 *rec, cudaStream_t st);
 cudaError_t launch_sqrt_check(u32 lo, u32 hi, unsigned long long *bad_dev, cudaStream_t st);
 cudaError_t launch_unpack12(const void *packed, u64 n_samples, u16 *out, cudaStream_t st);
 class PackPool;
@@ -177,6 +182,7 @@ struct sr_handle {
     DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
     DevBuf align[6];                                   // sr_dtw_path_batch / sr_average_bank: pairs, paths, templates, scores
     DevBuf conn[10];                                   // long features and the connected-word decoder: pieces, features, words
+    DevBuf gram[4];                                    // the grammar decoder: copy table, sequence table, frame counts, records
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };

@@ -55,6 +55,40 @@ class ConnOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in CONN_FIELDS]
 
 
+GRAM_STATE_MAX = 16            # SR_GRAM_STATE_MAX
+GRAM_COPY_MAX = 128            # SR_GRAM_COPY_MAX
+
+
+class GramArc(C.Structure):
+    _fields_ = [("from_", C.c_uint32), ("to", C.c_uint32), ("cmd_mask", C.c_uint32)]
+
+
+class Grammar(C.Structure):
+    _fields_ = [("n_states", C.c_uint32), ("final_mask", C.c_uint32), ("n_arcs", C.c_uint32), ("arcs", C.POINTER(GramArc))]
+
+
+def grammar(g):
+    """(n_states, final_mask, [(from, to, cmd_mask), ...]) -> an sr_grammar (its arcs kept alive on the struct); a Grammar
+    passes through, None stays None (NULL)"""
+    if g is None or isinstance(g, Grammar):
+        return g
+    n_states, final_mask, arcs = g
+    arr = (GramArc * max(len(arcs), 1))(*[GramArc(*a) for a in arcs])
+    out = Grammar(n_states, final_mask, len(arcs), C.cast(arr, C.POINTER(GramArc)))
+    out._arcs = arr
+    return out
+
+
+def loop_grammar(n_cmd=32):
+    """the one-state loop grammar: any command, any number of times (exactly sr_connected_batch)"""
+    return (1, 1, [(0, 0, (1 << n_cmd) - 1 if n_cmd < 32 else 0xFFFFFFFF)])
+
+
+def chain_grammar(L, cmd_mask=0x3FF):
+    """exactly L words, each a command of cmd_mask (default the ten digits): states 0..L, arcs k -> k+1, final state L"""
+    return (L + 1, 1 << L, [(k, k + 1, cmd_mask) for k in range(L)])
+
+
 class StreamEvent(C.Structure):
     _fields_ = [(k, C.c_uint32) for k in ("stream", "segment", "start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")]
 
@@ -101,6 +135,8 @@ def lib():
         L.sr_mfcc_long_batch.argtypes = [vp, vp, u32, u32, vp, u32, vp, u32, vp, vp]
         L.sr_connected_batch.argtypes = [vp, vp, vp, u32, u32, u32, u32, vp, vp, vp]
         L.sr_recognise_connected_batch.argtypes = [vp, vp, u32, u32, u32, u32, u32, C.POINTER(ConnOut)]
+        L.sr_connected_grammar_batch.argtypes = [vp, vp, vp, u32, u32, vp, u32, u32, vp, vp, vp]
+        L.sr_recognise_connected_grammar_batch.argtypes = [vp, vp, u32, u32, u32, vp, u32, u32, C.POINTER(ConnOut)]
         L.sr_streams_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
         L.sr_streams_destroy.argtypes = [vp]
         L.sr_streams_reset.argtypes = [vp]
@@ -375,6 +411,37 @@ class Handle:
             out = {k: np.zeros(*shape[k]) for k in CONN_FIELDS if k in want}
         o = ConnOut(*[_p(out.get(k)) for k in CONN_FIELDS])
         self._ck(lib().sr_recognise_connected_batch(self._h, _p(pcm), U, B, n_len, penalty, max_words, C.byref(o)))
+        return out
+
+    def connected_grammar(self, feat, frm_num, grammar_, penalty, max_words, words=None, want_total=True):
+        """connected words under a grammar (sr_connected_grammar_batch), given as (n_states, final_mask, [(from, to,
+        cmd_mask), ...]) or a Grammar: (words [B, max_words] WORD_DTYPE, n_words [B], total [B] u64 or None); records
+        past n_words keep what `words` held (zeros when it is None)"""
+        feat = np.ascontiguousarray(feat, np.int16)
+        B, stride = feat.shape[0], feat.shape[1]
+        frm_num = np.ascontiguousarray(frm_num, np.uint32)
+        words = np.zeros((B, max_words), WORD_DTYPE) if words is None else words
+        n_words = np.zeros(B, np.uint32)
+        total = np.zeros(B, np.uint64) if want_total else None
+        g = grammar(grammar_)
+        self._ck(lib().sr_connected_grammar_batch(self._h, _p(feat), _p(frm_num), stride, B, None if g is None else C.byref(g),
+                                                  penalty, max_words, _p(words), _p(n_words), _p(total)))
+        return words, n_words, total
+
+    def recognise_connected_grammar(self, pcm, grammar_, penalty, max_words, n_len=2400, want=CONN_FIELDS, out=None):
+        """noise_atap -> VAD -> long features -> one grammar decode per capture across its segments
+        (sr_recognise_connected_grammar_batch): a dict of the sr_conn_out fields named in `want` (or the arrays of `out`,
+        filled in place)"""
+        B, U = pcm.shape
+        if out is None:
+            shape = {"atap": (B, ATAP_DTYPE), "seg_off": ((B, 3, 2), np.uint32), "frm_num": ((B, 3), np.uint32),
+                     "n_words": (B, np.uint32), "words": ((B, max_words), WORD_DTYPE), "total": (B, np.uint64),
+                     "status": (B, np.uint8)}
+            out = {k: np.zeros(*shape[k]) for k in CONN_FIELDS if k in want}
+        o = ConnOut(*[_p(out.get(k)) for k in CONN_FIELDS])
+        g = grammar(grammar_)
+        self._ck(lib().sr_recognise_connected_grammar_batch(self._h, _p(pcm), U, B, n_len, None if g is None else C.byref(g),
+                                                            penalty, max_words, C.byref(o)))
         return out
 
     def fft_mag(self, frames):
