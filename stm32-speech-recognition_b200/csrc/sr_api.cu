@@ -886,10 +886,11 @@ int sr_connected_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_nu
     u32 *d_nw = c.out(h->conn[8], n_words, (size_t)B * 4);
     u64 *d_total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
     const BankView &bk = h->bank;
-    c.launch(TAG_CONN, "launch_dtw_connected", [&] {
-        return launch_dtw_connected(d_feat, frm_stride, d_frm, nullptr, B, bk.p, bk.n, bk.stride, penalty, max_words, d_words,
-                                    d_nw, d_total, h->stream);
-    });
+    for (u32 b0 = 0; b0 < B; b0 += kSeqChunk)
+        c.launch(TAG_CONN, "launch_dtw_connected", [&] {
+            return launch_dtw_connected(d_feat, frm_stride, d_frm, nullptr, b0, std::min(B - b0, kSeqChunk), bk.p, bk.n, bk.stride,
+                                        penalty, max_words, d_words, d_nw, d_total, h->stream);
+        });
     return c.finish();
 }
 
@@ -949,10 +950,10 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
     c.h2d(d_sfrm, seq_frm.data(), (size_t)nseq * 4);
     c.h2d(d_sof, seq_of.data(), (size_t)B * 12);
     const BankView &bk = h->bank;
-    if (nseq)
+    for (u32 b0 = 0; b0 < nseq; b0 += kSeqChunk)
         c.launch(TAG_CONN, "launch_dtw_connected", [&] {
-            return launch_dtw_connected(d_feat, 0, d_sfrm, d_soff, nseq, bk.p, bk.n, bk.stride, penalty, 0, d_sw, d_snw, d_stot,
-                                        h->stream);
+            return launch_dtw_connected(d_feat, 0, d_sfrm, d_soff, b0, std::min(nseq - b0, kSeqChunk), bk.p, bk.n, bk.stride,
+                                        penalty, 0, d_sw, d_snw, d_stot, h->stream);
         });
     const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
     sr_conn_word *d_words = nullptr;
@@ -1035,11 +1036,13 @@ static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &
     const BankView &bk = h->bank;
     for (size_t k = 0; k + 1 < cut.size(); ++k) {
         const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
-        c.launch(TAG_GRAM, "launch_dtw_grammar", [&] {
-            return launch_dtw_grammar(d_feat, d_frm + b0, d_seq + 3 * (size_t)b0, nb, bk.p, bk.stride, d_copy, (u32)copy.size(), S,
-                                      g->final_mask, penalty, max_words, d_words ? d_words + (size_t)b0 * max_words : nullptr,
-                                      d_nw ? d_nw + b0 : nullptr, d_total ? d_total + b0 : nullptr, d_rec, h->stream);
-        });
+        for (u32 q0 = 0; q0 < nb; q0 += kSeqChunk)
+            c.launch(TAG_GRAM, "launch_dtw_grammar", [&] {
+                return launch_dtw_grammar(d_feat, d_frm + b0, d_seq + 3 * (size_t)b0, q0, std::min(nb - q0, kSeqChunk), bk.p,
+                                          bk.stride, d_copy, (u32)copy.size(), S, g->final_mask, penalty, max_words,
+                                          d_words ? d_words + (size_t)b0 * max_words : nullptr, d_nw ? d_nw + b0 : nullptr,
+                                          d_total ? d_total + b0 : nullptr, d_rec, h->stream);
+            });
     }
 }
 

@@ -209,39 +209,35 @@ conn_concat_kernel(const u32 *__restrict__ seq_of, const u32 *__restrict__ seq_o
     if (total) total[b] = tot;
 }
 
-// B sequences against the bank's T <= SR_CONN_SLOT_MAX slots: one cluster of ceil(T / kConnWarps) CTAs per sequence
-// (launches of at most 2^20 sequences each)
-cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 B,
+// sequences [b0, b0 + nb) against the bank's T <= SR_CONN_SLOT_MAX slots in one launch: one cluster of
+// ceil(T / kConnWarps) CTAs per sequence
+cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 b0, u32 nb,
                                  const void *bank, u32 T, u32 slot_stride, u32 penalty, u32 max_words, sr_conn_word *words,
                                  u32 *n_words, u64 *total, cudaStream_t st) {
-    if (B == 0) return cudaSuccess;
-    if (T > SR_CONN_SLOT_MAX) return cudaErrorInvalidValue;
+    if (nb == 0) return cudaSuccess;
+    if (T > SR_CONN_SLOT_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
     const u32 nc = T ? (T + kConnWarps - 1) / kConnWarps : 1u;
     cudaError_t e = cudaFuncSetAttribute(dtw_connected_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kConnSmem);
     if (e == cudaSuccess && nc > 8) e = cudaFuncSetAttribute(dtw_connected_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e != cudaSuccess) return e;
-    constexpr u32 kChunk = 1u << 20;
-    for (u32 b0 = 0; b0 < B; b0 += kChunk) {
-        const u32 nb = B - b0 < kChunk ? B - b0 : kChunk;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(nb * nc);
-        cfg.blockDim = dim3(kConnWarps * 32);
-        cfg.dynamicSmemBytes = kConnSmem;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = nc;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        const s16 *f = seq_off ? feat : feat + (size_t)b0 * frm_stride * 12;
-        e = cudaLaunchKernelEx(&cfg, dtw_connected_kernel, f, frm_stride, frm_num + b0, seq_off ? seq_off + 2 * (size_t)b0 : nullptr,
-                               static_cast<const unsigned char *>(bank), T, slot_stride, penalty, max_words,
-                               words && !seq_off ? words + (size_t)b0 * max_words : words, n_words + b0,
-                               total ? total + b0 : nullptr);
-        if (e != cudaSuccess) return e;
-    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(nb * nc);
+    cfg.blockDim = dim3(kConnWarps * 32);
+    cfg.dynamicSmemBytes = kConnSmem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = nc;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const s16 *f = seq_off ? feat : feat + (size_t)b0 * frm_stride * 12;
+    e = cudaLaunchKernelEx(&cfg, dtw_connected_kernel, f, frm_stride, frm_num + b0, seq_off ? seq_off + 2 * (size_t)b0 : nullptr,
+                           static_cast<const unsigned char *>(bank), T, slot_stride, penalty, max_words,
+                           words && !seq_off ? words + (size_t)b0 * max_words : words, n_words + b0,
+                           total ? total + b0 : nullptr);
+    if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }
 

@@ -217,39 +217,35 @@ dtw_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ frm_num
     if (total) total[s] = fd;
 }
 
-// B sequences (the table seq gives each its first feature row, its first record row and its segments) against C <=
-// SR_GRAM_COPY_MAX copies of the bank's slots: one cluster of ceil(C / kGramWarps) CTAs per sequence. rec holds
-// (last record row + 1) * S records; the caller chunks its sequences to bound it.
-cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 B, const void *bank, u32 slot_stride,
+// sequences [b0, b0 + nb) (the table seq gives each its first feature row, its first record row and its segments) against
+// C <= SR_GRAM_COPY_MAX copies of the bank's slots in one launch: one cluster of ceil(C / kGramWarps) CTAs per sequence.
+// rec holds (last record row + 1) * S records; the caller chunks its sequences to bound it.
+cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 b0, u32 nb, const void *bank, u32 slot_stride,
                                const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
                                u32 *n_words, u64 *total, u64 *rec, cudaStream_t st) {
-    if (B == 0) return cudaSuccess;
-    if (C > SR_GRAM_COPY_MAX || S == 0 || S > SR_GRAM_STATE_MAX) return cudaErrorInvalidValue;
+    if (nb == 0) return cudaSuccess;
+    if (C > SR_GRAM_COPY_MAX || S == 0 || S > SR_GRAM_STATE_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
     const u32 nc = C ? (C + kGramWarps - 1) / kGramWarps : 1u;
     cudaError_t e = cudaFuncSetAttribute(dtw_grammar_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGramSmem);
     if (e == cudaSuccess && nc > 8) e = cudaFuncSetAttribute(dtw_grammar_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e != cudaSuccess) return e;
-    constexpr u32 kChunk = 1u << 20;
-    for (u32 b0 = 0; b0 < B; b0 += kChunk) {
-        const u32 nb = B - b0 < kChunk ? B - b0 : kChunk;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(nb * nc);
-        cfg.blockDim = dim3(kGramWarps * 32);
-        cfg.dynamicSmemBytes = kGramSmem;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = nc;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        e = cudaLaunchKernelEx(&cfg, dtw_grammar_kernel, feat, frm_num + b0, seq + 3 * (size_t)b0,
-                               static_cast<const unsigned char *>(bank), slot_stride, copy, C, S, final_mask, penalty, max_words,
-                               words ? words + (size_t)b0 * max_words : nullptr, n_words ? n_words + b0 : nullptr,
-                               total ? total + b0 : nullptr, rec);
-        if (e != cudaSuccess) return e;
-    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(nb * nc);
+    cfg.blockDim = dim3(kGramWarps * 32);
+    cfg.dynamicSmemBytes = kGramSmem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = nc;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    e = cudaLaunchKernelEx(&cfg, dtw_grammar_kernel, feat, frm_num + b0, seq + 3 * (size_t)b0,
+                           static_cast<const unsigned char *>(bank), slot_stride, copy, C, S, final_mask, penalty, max_words,
+                           words ? words + (size_t)b0 * max_words : nullptr, n_words ? n_words + b0 : nullptr,
+                           total ? total + b0 : nullptr, rec);
+    if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }
 

@@ -49,18 +49,20 @@ cudaError_t launch_dtw_align(const void *in_base, u32 in_stride, const void *tpl
                              void *tpl_out, u32 *anchor_out, int num_sms, cudaStream_t st);
 cudaError_t launch_average_update(const void *bank, u32 slot_stride, u32 K, u32 G, const u32 *mask, const u8 *path,
                                   const u32 *path_len, void *tpl, cudaStream_t st);
-// the connected-word decoder over B feature sequences (seq_off: [B][2] first row, first word record, or NULL: b * frm_stride,
-// b * max_words), the gather of get_mfcc pieces into long feature rows and the join of a capture's segments (sr_dtw_connected.cu)
-cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 B,
+// the connected-word decoder over sequences [b0, b0 + nb) of a batch, nb <= kSeqChunk (seq_off: [B][2] first row, first
+// word record, or NULL: b * frm_stride, b * max_words), the gather of get_mfcc pieces into long feature rows and the join
+// of a capture's segments (sr_dtw_connected.cu)
+cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 b0, u32 nb,
                                  const void *bank, u32 T, u32 slot_stride, u32 penalty, u32 max_words, sr_conn_word *words,
                                  u32 *n_words, u64 *total, cudaStream_t st);
 cudaError_t launch_conn_gather(const void *pf, const u32 *pdst, u32 P, s16 *feat, int num_sms, cudaStream_t st);
 cudaError_t launch_conn_concat(const u32 *seq_of, const u32 *seq_off, const sr_conn_word *seq_words, const u32 *seq_nw,
                                const u64 *seq_total, u32 B, u32 max_words, sr_conn_word *words, u32 *n_words, u64 *total,
                                cudaStream_t st);
-// the grammar decoder over B sequences (seq: [B][3] first feature row, first record row, segment first frames) against C
-// copies of bank slots (copy: [C] slot | state << 8 | src << 16), records in rec (sr_dtw_grammar.cu)
-cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 B, const void *bank, u32 slot_stride,
+// the grammar decoder over sequences [b0, b0 + nb) of a batch, nb <= kSeqChunk (seq: [B][3] first feature row, first
+// record row, segment first frames) against C copies of bank slots (copy: [C] slot | state << 8 | src << 16), records in
+// rec (sr_dtw_grammar.cu)
+cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 b0, u32 nb, const void *bank, u32 slot_stride,
                                const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
                                u32 *n_words, u64 *total, u64 *rec, cudaStream_t st);
 cudaError_t launch_sqrt_check(u32 lo, u32 hi, unsigned long long *bad_dev, cudaStream_t st);

@@ -6,8 +6,9 @@
   2. sr_recognise_connected_batch on synthetic 3-word captures at U = 16 000 against an enrolled 80-slot bank: wall time
      per call and the kernel time by tag (0 noise_atap + VAD, 1 get_mfcc pieces, 9 the decoder).
 
-Every row checks a sample against the oracles (tests/oracle_connected.c, the composed oracle stages). The card's name,
-power limit and SM clock limit are read in the same run.
+Every row checks a sample against the oracles (tests/oracle_connected.c, the composed oracle stages): the first and last
+sequence (capture) of every launch -- decoder launches of 2^20 sequences, get_mfcc piece launches of 8 192 pieces -- plus
+random ones, --sample in all. The card's name, power limit and SM clock limit are read in the same run.
 
     python tools/bench_connected.py [--steps 2] [--warmup 1] [--json FILE]
 """
@@ -28,9 +29,28 @@ import oracle_bind as ob  # noqa: E402
 import oracle_connected as oc  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
+from test_connected_launches import _pieces, launch_sample, piece_plan, seq_launches  # noqa: E402
 
 NPROC = os.cpu_count() or 1
 PENALTY = 4000
+
+
+def edges(ranges):
+    """the first and last index of every range [lo, hi)"""
+    return {i for lo, hi in ranges for i in (lo, hi - 1)}
+
+
+def e2e_edges(frm_num, seq_ranges=None):
+    """the captures holding the first and last get_mfcc piece of every piece launch and, given the decoder's launch ranges
+    over the captures' segments with frames (default: one sequence per segment, K6), of every decoder launch"""
+    B = len(frm_num)
+    e = piece_plan(_pieces(frm_num).sum(1))[1]
+    if seq_ranges is None:
+        owner = np.repeat(np.arange(B), (frm_num > 0).sum(1))
+        e |= {int(owner[i]) for i in edges(seq_launches([0, len(owner)]))}
+    else:
+        e |= edges(seq_ranges)
+    return e
 
 
 def timed(h, fn, reps):
@@ -58,7 +78,7 @@ def main():
     ap.add_argument("--e2e-batch", type=int, default=16384)
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=1)
-    ap.add_argument("--sample", type=int, default=8)
+    ap.add_argument("--sample", type=int, default=32)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
 
@@ -74,6 +94,7 @@ def main():
     pool = sr_b200.synth_ftr_host(2000, 0xB0C0000, 50, 100).view(ob.FTR_DTYPE).reshape(2000)
     rows = np.concatenate([pool["mfcc_dat"][k][:int(pool["frm_num"][k]) * 12].reshape(-1, 12) for k in range(2000)])
     rng = np.random.default_rng(0xB0C)
+    srng = np.random.default_rng(0xB0C5)                  # the oracle samples' random part
     for N in (119, 300, 818):
         start = rng.integers(0, len(rows) - N, B)
         feat = np.empty((B, N, 12), np.int16)
@@ -87,8 +108,9 @@ def main():
             for _ in range(args.warmup):
                 h.connected(feat, frm, PENALTY, 16)
             wall, ker, (words, nw, tot) = timed(h, lambda: h.connected(feat, frm, PENALTY, 16), args.steps)
-            ww, wn, wt = co.connected(feat[:n], frm[:n], bank, T, 4096, PENALTY, 16, nthreads=NPROC)
-            ok = bool(np.array_equal(nw[:n], wn) and np.array_equal(tot[:n], wt) and np.array_equal(words[:n], ww))
+            idx = launch_sample(edges(seq_launches([0, B])), B, n, srng)
+            ww, wn, wt = co.connected(feat[idx], frm[idx], bank, T, 4096, PENALTY, 16, nthreads=NPROC)
+            ok = bool(np.array_equal(nw[idx], wn) and np.array_equal(tot[idx], wt) and np.array_equal(words[idx], ww))
             cells = float(N) * float(bank[:, 2:4].copy().view(np.uint16)[:, 0].astype(np.int64).sum()) * B
             kms = ker[9]
             results["decoder"].append({"N": N, "slots": T, "sequences": B, "kernel_ms": kms, "wall_ms": wall,
@@ -104,8 +126,9 @@ def main():
     for _ in range(args.warmup):
         h.recognise_connected(pcm, PENALTY, 8)
     wall, ker, out = timed(h, lambda: h.recognise_connected(pcm, PENALTY, 8), args.steps)
-    want = oc.recognise_connected(ob.best_oracle(), co, pcm[:n], 2400, bank, 80, 4096, PENALTY, 8)
-    ok = all(np.array_equal(out[k][:n], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
+    idx = launch_sample(e2e_edges(out["frm_num"]), E, n, srng)
+    want = oc.recognise_connected(ob.best_oracle(), co, pcm[idx], 2400, bank, 80, 4096, PENALTY, 8)
+    ok = all(np.array_equal(out[k][idx], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
     results["end_to_end"].append({"U": U, "captures": E, "wall_ms": wall, "captures_per_s": E / (wall * 1e-3),
                                   "kernel_ms": {str(k): v for k, v in sorted(ker.items())},
                                   "mean_words": float(out["n_words"].mean()), "sample_equals_oracle": bool(ok)})

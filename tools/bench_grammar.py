@@ -6,8 +6,9 @@
   3. 11-digit chain: 12 states, 110 copies (11 digit states of 10 averaged digits), sequences of 818 frames;
   4. end to end: 16 384 two-second captures under the PIN grammar.
 Kernel time (tags 9 and 10), sequences/s and cells/s, cells = N * sum of the copies' frame counts. Every row checks a
-sample against the oracle (tests/oracle_grammar.c, the composed oracle stages). The card's name, power limit and SM
-clock limit are read in the same run.
+sample against the oracle (tests/oracle_grammar.c, the composed oracle stages): the first and last sequence (capture) of
+every launch -- decoder launches cut at 2^28 bytes of records and at 2^20 sequences, get_mfcc piece launches of 8 192
+pieces -- plus random ones, --sample in all. The card's name, power limit and SM clock limit are read in the same run.
 
     python tools/bench_grammar.py [--steps 2] [--warmup 1] [--json FILE]
 """
@@ -26,8 +27,9 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import oracle_bind as ob  # noqa: E402
 import oracle_grammar as og  # noqa: E402
 import sr_b200  # noqa: E402
-from bench_connected import synth_bank, timed  # noqa: E402
+from bench_connected import e2e_edges, edges, synth_bank, timed  # noqa: E402
 from bench_match import card  # noqa: E402
+from test_connected_launches import launch_sample, record_cuts, seq_launches  # noqa: E402
 
 NPROC = os.cpu_count() or 1
 PENALTY = 4000
@@ -66,7 +68,7 @@ def main():
     ap.add_argument("--e2e-batch", type=int, default=16384)
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=1)
-    ap.add_argument("--sample", type=int, default=8)
+    ap.add_argument("--sample", type=int, default=32)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
 
@@ -77,10 +79,12 @@ def main():
     h = sr_b200.Handle(0)
     go = og.grammar()
     rows = []
+    srng = np.random.default_rng(0xB6A5)                  # the oracle samples' random part
 
     def row(name, B, N, bank, T, grammar, kms, words, nw, tot, feat, frm):
-        ww, wn, wt = go.decode(feat[:n], frm[:n], bank, T, 4096, grammar, PENALTY, 16, nthreads=NPROC)
-        ok = bool(np.array_equal(nw[:n], wn) and np.array_equal(tot[:n], wt) and np.array_equal(words[:n], ww))
+        idx = launch_sample(edges(seq_launches(record_cuts(frm, grammar[0]))), B, n, srng)
+        ww, wn, wt = go.decode(feat[idx], frm[idx], bank, T, 4096, grammar, PENALTY, 16, nthreads=NPROC)
+        ok = bool(np.array_equal(nw[idx], wn) and np.array_equal(tot[idx], wt) and np.array_equal(words[idx], ww))
         cells = float(N) * copy_frames(bank, grammar) * B
         rows.append({"row": name, "sequences": B, "N": N, "states": grammar[0], "kernel_ms": kms,
                      "sequences_per_s": B / (kms * 1e-3), "cells_per_s": cells / (kms * 1e-3),
@@ -130,8 +134,9 @@ def main():
     for _ in range(args.warmup):
         h.recognise_connected_grammar(pcm, PIN, PENALTY, 8)
     wall, ker, out = timed(h, lambda: h.recognise_connected_grammar(pcm, PIN, PENALTY, 8), args.steps)
-    want = og.recognise_connected_grammar(ob.best_oracle(), go, pcm[:n], 2400, avg, 40, 4096, PIN, PENALTY, 8, nthreads=NPROC)
-    ok = all(np.array_equal(out[k][:n], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
+    idx = launch_sample(e2e_edges(out["frm_num"], seq_launches(record_cuts(out["frm_num"].sum(1), PIN[0]))), E, n, srng)
+    want = og.recognise_connected_grammar(ob.best_oracle(), go, pcm[idx], 2400, avg, 40, 4096, PIN, PENALTY, 8, nthreads=NPROC)
+    ok = all(np.array_equal(out[k][idx], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
     e2e = {"U": U, "captures": E, "wall_ms": wall, "captures_per_s": E / (wall * 1e-3),
            "kernel_ms": {str(k): v for k, v in sorted(ker.items())}, "mean_words": float(out["n_words"].mean()),
            "sample_equals_oracle": bool(ok)}
