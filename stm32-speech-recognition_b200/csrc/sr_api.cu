@@ -839,6 +839,54 @@ static void run_pieces(HostCall &c, const u16 *d_pcm, u32 U, u32 n_rows, const L
     }
 }
 
+// the device copies of a connected call's outputs, each NULL when the caller passes none: word records (in / out: records
+// past n_words keep the caller's bytes), word counts and totals
+struct ConnDev { sr_conn_word *words; u32 *nw; u64 *total; };
+static ConnDev conn_outputs(HostCall &c, u32 B, u32 max_words, sr_conn_word *words, u32 *n_words, uint64_t *total) {
+    sr_handle *h = c.h;
+    ConnDev d{nullptr, nullptr, nullptr};
+    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
+    if (words && max_words) {
+        d.words = c.in(h->conn[7], words, wbytes);
+        c.out(h->conn[7], words, wbytes);
+    }
+    d.nw = n_words ? c.out(h->conn[8], n_words, (size_t)B * 4) : nullptr;
+    d.total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
+    return d;
+}
+
+// noise_atap + VAD of B captures of U samples from d_pcm (o->atap in / out: untouched when n_len % 240 != 0, else zeros),
+// then one synchronisation: the plan needs the segments. seg [B][6] and atap [B] come back on the host.
+static void conn_vad(HostCall &c, const u16 *d_pcm, u32 U, u32 B, u32 n_len, const sr_conn_out *o, std::vector<u32> &seg,
+                     std::vector<atap_tag> &atap) {
+    sr_handle *h = c.h;
+    atap_tag *d_atap;
+    if (o->atap) d_atap = c.in(h->atap, o->atap, (size_t)B * sizeof(atap_tag));
+    else {
+        d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
+        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
+    }
+    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
+    c.launch(TAG_VAD, "launch_vad", [&] { return launch_vad(d_pcm, U, B, n_len, U, 1, 1, d_atap, d_seg, h->num_sms, h->stream, vad_work(h)); });
+    seg.assign((size_t)B * 6, 0);
+    atap.assign(B, atap_tag{});
+    if (d_seg) c.ck("copy back", cudaMemcpyAsync(seg.data(), d_seg, (size_t)B * 24, cudaMemcpyDeviceToHost, h->stream));
+    if (d_atap) c.ck("copy back", cudaMemcpyAsync(atap.data(), d_atap, (size_t)B * sizeof(atap_tag), cudaMemcpyDeviceToHost, h->stream));
+    c.ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+}
+
+// the end of a recognise-connected call: finish c, then the host-side outputs of the plan
+static int conn_finish(HostCall &c, const sr_conn_out *o, u32 B, const std::vector<atap_tag> &atap, const std::vector<u32> &seg,
+                       const std::vector<u32> &frm, const std::vector<u8> &status) {
+    const int rc = c.finish();
+    if (rc) return rc;
+    if (o->atap) memcpy(o->atap, atap.data(), (size_t)B * sizeof(atap_tag));
+    if (o->seg_off) memcpy(o->seg_off, seg.data(), (size_t)B * 24);
+    if (o->frm_num) memcpy(o->frm_num, frm.data(), (size_t)B * 12);
+    if (o->status) memcpy(o->status, status.data(), B);
+    return 0;
+}
+
 extern "C" {
 
 // get_mfcc with vv_frm_max replaced by frm_cap: the frame counts and the piece plan come from the segment offsets on the
@@ -877,19 +925,12 @@ int sr_connected_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_nu
     HostCall c(h, "sr_connected_batch");
     const s16 *d_feat = c.in(h->conn[3], feat, (size_t)B * frm_stride * 24);
     const u32 *d_frm = c.in(h->conn[4], frm_num, (size_t)B * 4);
-    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
-    sr_conn_word *d_words = nullptr;
-    if (words && max_words) {                            // in / out: records past n_words keep the caller's bytes
-        d_words = c.in(h->conn[7], words, wbytes);
-        c.out(h->conn[7], words, wbytes);
-    }
-    u32 *d_nw = c.out(h->conn[8], n_words, (size_t)B * 4);
-    u64 *d_total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
+    const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
     const BankView &bk = h->bank;
     for (u32 b0 = 0; b0 < B; b0 += kSeqChunk)
         c.launch(TAG_CONN, "launch_dtw_connected", [&] {
             return launch_dtw_connected(d_feat, frm_stride, d_frm, nullptr, b0, std::min(B - b0, kSeqChunk), bk.p, bk.n, bk.stride,
-                                        penalty, max_words, d_words, d_nw, d_total, h->stream);
+                                        penalty, max_words, d.words, d.nw, d.total, h->stream);
         });
     return c.finish();
 }
@@ -904,19 +945,9 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
     SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
     HostCall c(h, "sr_recognise_connected_batch");
     const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    atap_tag *d_atap;
-    if (o->atap) d_atap = c.in(h->atap, o->atap, (size_t)B * sizeof(atap_tag));   // in / out: untouched when n_len % 240 != 0
-    else {
-        d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
-        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
-    }
-    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
-    c.launch(TAG_VAD, "launch_vad", [&] { return launch_vad(d_pcm, U, B, n_len, U, 1, 1, d_atap, d_seg, h->num_sms, h->stream, vad_work(h)); });
-    std::vector<u32> seg((size_t)B * 6);
-    std::vector<atap_tag> atap(B);
-    if (d_seg) c.ck("copy back", cudaMemcpyAsync(seg.data(), d_seg, (size_t)B * 24, cudaMemcpyDeviceToHost, h->stream));
-    if (d_atap) c.ck("copy back", cudaMemcpyAsync(atap.data(), d_atap, (size_t)B * sizeof(atap_tag), cudaMemcpyDeviceToHost, h->stream));
-    c.ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+    std::vector<u32> seg;
+    std::vector<atap_tag> atap;
+    conn_vad(c, d_pcm, U, B, n_len, o, seg, atap);
     if (c.rc) return c.finish();
     // the plan: sequence q = the q-th closed segment with frames; rows and word records packed at seq_off[q][0] (frames)
     const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
@@ -955,25 +986,12 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
             return launch_dtw_connected(d_feat, 0, d_sfrm, d_soff, b0, std::min(nseq - b0, kSeqChunk), bk.p, bk.n, bk.stride,
                                         penalty, 0, d_sw, d_snw, d_stot, h->stream);
         });
-    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
-    sr_conn_word *d_words = nullptr;
-    if (o->words && max_words) {                         // in / out: records past n_words keep the caller's bytes
-        d_words = c.in(h->conn[7], o->words, wbytes);
-        c.out(h->conn[7], o->words, wbytes);
-    }
-    u32 *d_nw = o->n_words ? c.out(h->conn[8], o->n_words, (size_t)B * 4) : nullptr;
-    u64 *d_total = o->total ? c.out(h->conn[9], reinterpret_cast<u64 *>(o->total), (size_t)B * 8) : nullptr;
-    if (d_words || d_nw || d_total)
+    const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
+    if (d.words || d.nw || d.total)
         c.launch(TAG_NONE, "launch_conn_concat", [&] {
-            return launch_conn_concat(d_sof, d_soff, d_sw, d_snw, d_stot, B, max_words, d_words, d_nw, d_total, h->stream);
+            return launch_conn_concat(d_sof, d_soff, d_sw, d_snw, d_stot, B, max_words, d.words, d.nw, d.total, h->stream);
         });
-    const int rc = c.finish();
-    if (rc) return rc;
-    if (o->atap) memcpy(o->atap, atap.data(), (size_t)B * sizeof(atap_tag));
-    if (o->seg_off) memcpy(o->seg_off, seg.data(), (size_t)B * 24);
-    if (o->frm_num) memcpy(o->frm_num, frm.data(), (size_t)B * 12);
-    if (o->status) memcpy(o->status, status.data(), B);
-    return 0;
+    return conn_finish(c, o, B, atap, seg, frm, status);
 }
 
 }  // extern "C"
@@ -1014,8 +1032,7 @@ constexpr size_t kGramRecBytes = 256u << 20;   // records per launch: sum of N *
 // the grammar decoder (tag 10) over B sequences of frames N[b]: seq [B][3] holds each first feature row and its segments
 // (the record rows are filled in here). Launches take consecutive sequences whose records fit kGramRecBytes.
 static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &N, std::vector<u32> &seq,
-                        const std::vector<u32> &copy, const sr_grammar *g, u32 penalty, u32 max_words, sr_conn_word *d_words,
-                        u32 *d_nw, u64 *d_total) {
+                        const std::vector<u32> &copy, const sr_grammar *g, u32 penalty, u32 max_words, const ConnDev &d) {
     sr_handle *h = c.h;
     const u32 B = (u32)N.size(), S = g->n_states;
     std::vector<u32> cut{0};                             // launch boundaries
@@ -1040,8 +1057,8 @@ static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &
             c.launch(TAG_GRAM, "launch_dtw_grammar", [&] {
                 return launch_dtw_grammar(d_feat, d_frm + b0, d_seq + 3 * (size_t)b0, q0, std::min(nb - q0, kSeqChunk), bk.p,
                                           bk.stride, d_copy, (u32)copy.size(), S, g->final_mask, penalty, max_words,
-                                          d_words ? d_words + (size_t)b0 * max_words : nullptr, d_nw ? d_nw + b0 : nullptr,
-                                          d_total ? d_total + b0 : nullptr, d_rec, h->stream);
+                                          d.words ? d.words + (size_t)b0 * max_words : nullptr, d.nw ? d.nw + b0 : nullptr,
+                                          d.total ? d.total + b0 : nullptr, d_rec, h->stream);
             });
     }
 }
@@ -1066,15 +1083,8 @@ int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat, const uint32_t
     }
     HostCall c(h, "sr_connected_grammar_batch");
     const s16 *d_feat = c.in(h->conn[3], feat, (size_t)B * frm_stride * 24);
-    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
-    sr_conn_word *d_words = nullptr;
-    if (words && max_words) {                            // in / out: records past n_words keep the caller's bytes
-        d_words = c.in(h->conn[7], words, wbytes);
-        c.out(h->conn[7], words, wbytes);
-    }
-    u32 *d_nw = c.out(h->conn[8], n_words, (size_t)B * 4);
-    u64 *d_total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
-    run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d_words, d_nw, d_total);
+    const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
+    run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
     return c.finish();
 }
 
@@ -1090,19 +1100,9 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
     if (const int rc = gram_copies(h, g, copy)) return rc;
     HostCall c(h, "sr_recognise_connected_grammar_batch");
     const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    atap_tag *d_atap;
-    if (o->atap) d_atap = c.in(h->atap, o->atap, (size_t)B * sizeof(atap_tag));   // in / out: untouched when n_len % 240 != 0
-    else {
-        d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
-        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
-    }
-    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
-    c.launch(TAG_VAD, "launch_vad", [&] { return launch_vad(d_pcm, U, B, n_len, U, 1, 1, d_atap, d_seg, h->num_sms, h->stream, vad_work(h)); });
-    std::vector<u32> seg((size_t)B * 6);
-    std::vector<atap_tag> atap(B);
-    if (d_seg) c.ck("copy back", cudaMemcpyAsync(seg.data(), d_seg, (size_t)B * 24, cudaMemcpyDeviceToHost, h->stream));
-    if (d_atap) c.ck("copy back", cudaMemcpyAsync(atap.data(), d_atap, (size_t)B * sizeof(atap_tag), cudaMemcpyDeviceToHost, h->stream));
-    c.ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+    std::vector<u32> seg;
+    std::vector<atap_tag> atap;
+    conn_vad(c, d_pcm, U, B, n_len, o, seg, atap);
     if (c.rc) return c.finish();
     // the plan: capture b is sequence b, its segments with frames back to back from row seq[b][0]; segment k's first
     // frame in that sequence (1023: no frames) is field k of seq[b][2]
@@ -1131,22 +1131,9 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
     if (c.rc) return c.finish();
     s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(rows, 1) * 24);
     run_pieces(c, d_pcm, U, B, pc, d_feat);
-    const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
-    sr_conn_word *d_words = nullptr;
-    if (o->words && max_words) {                         // in / out: records past n_words keep the caller's bytes
-        d_words = c.in(h->conn[7], o->words, wbytes);
-        c.out(h->conn[7], o->words, wbytes);
-    }
-    u32 *d_nw = o->n_words ? c.out(h->conn[8], o->n_words, (size_t)B * 4) : nullptr;
-    u64 *d_total = o->total ? c.out(h->conn[9], reinterpret_cast<u64 *>(o->total), (size_t)B * 8) : nullptr;
-    if (d_words || d_nw || d_total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d_words, d_nw, d_total);
-    const int rc = c.finish();
-    if (rc) return rc;
-    if (o->atap) memcpy(o->atap, atap.data(), (size_t)B * sizeof(atap_tag));
-    if (o->seg_off) memcpy(o->seg_off, seg.data(), (size_t)B * 24);
-    if (o->frm_num) memcpy(o->frm_num, frm.data(), (size_t)B * 12);
-    if (o->status) memcpy(o->status, status.data(), B);
-    return 0;
+    const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
+    if (d.words || d.nw || d.total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
+    return conn_finish(c, o, B, atap, seg, frm, status);
 }
 
 // One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]

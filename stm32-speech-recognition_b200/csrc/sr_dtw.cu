@@ -406,27 +406,19 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 // A row never has more than M <= 119 valid columns, whatever r is, so lane l holds the fixed columns 4l .. 4l+3 (32 x 4 =
 // 128 >= 119) and the cost of a pair does not depend on r: r >= 118 is the unconstrained DTW (the host clamps r to 118).
 // The band of row i is the column interval [max(c-r, 0), min(c+r, M-1)], c = floor(i*M/I); cells outside it are +inf.
-// Per row: up and diag come from the lane's own previous row (diag of its first column by one shuffle); the in-row
-// recurrence x_j = d_j + min(A_j, x_{j-1}), A_j = min(up, diag), maps a lane's incoming x to its outgoing one as
-// f(x) = min(x + a, b) (a = the lane's sum of d, b = its outgoing x for an incoming +inf); one warp scan composes these
-// maps, f2(f1(x)) = min(x + a1 + a2, min(b1 + a2, b2)), giving every lane its incoming x, and a serial pass over the
-// lane's four cells writes the row. The template's four rows stay in registers for the whole pair.
-// Headroom of kInf = 2^30 - 1: a path to cell (i,j) has at most i+j+1 cells of at most 65 536, so every reachable cell
-// is below 237 * 65 536 = 15 532 032 and a full-matrix optimum at most max(I,M) * 65 536; +inf sums (b1 + a2 <= kInf +
-// 119 * 65 536) stay below 2^31 and are cut back to kInf, so a cell is reachable exactly when it is below kInf / 2.
-constexpr int kWideCells = 4;
-
+// Each row is one dp_column step (sr_dtw_core.cuh, which also gives the headroom of kInf); the template's four rows
+// stay in registers for the whole pair.
 __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
 dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                 u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                 const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
     warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
-        const int j0 = lane * kWideCells;
-        PRow b[kWideCells];
-        s32 D[kWideCells];
+        const int j0 = lane * 4;
+        PRow b[4];
+        s32 D[4];
 #pragma unroll
-        for (int k = 0; k < kWideCells; ++k) {
+        for (int k = 0; k < 4; ++k) {
             load_row(b[k], trow, kNrm119, j0 + k < M ? j0 + k : 0);
             D[k] = kInf;
         }
@@ -434,41 +426,14 @@ dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
             const int c = (i * M) / I, lo = max(c - r, 0), hi = min(c + r, M - 1);
             PRow a;
             load_row(a, uslot, kNrm119, i);                            // broadcast read
-            s32 dg = __shfl_up_sync(0xFFFFFFFFu, D[kWideCells - 1], 1);   // D(i-1, j0-1)
-            if (lane == 0) dg = kInf;
-            s32 d[kWideCells], A[kWideCells];
-            bool valid[kWideCells];
-            s32 x = kInf, sum = 0;                                     // serial pass for an incoming +inf: b and a
-#pragma unroll
-            for (int k = 0; k < kWideCells; ++k) {
+            dp_column<s32, kInf>(D, lane, [&](int k, s32 up, s32 dg, s32 &d, s32 &A, bool &valid) {
                 const int j = j0 + k;
-                valid[k] = j >= lo && j <= hi;
-                d[k] = valid[k] ? (s32)pdist(a, b[k]) : 0;
-                A[k] = i == 0 ? (j == 0 ? 0 : kInf) : min(D[k], dg);
-                dg = D[k];
-                x = valid[k] ? min(d[k] + min(A[k], x), kInf) : kInf;
-                sum += d[k];
-            }
-            s32 fa = sum, fb = x;                                      // inclusive composition of the lanes' maps
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const s32 pa = __shfl_up_sync(0xFFFFFFFFu, fa, o), pb = __shfl_up_sync(0xFFFFFFFFu, fb, o);
-                if (lane >= o) { fb = min(min(pb + fa, fb), kInf); fa += pa; }
-            }
-            x = __shfl_up_sync(0xFFFFFFFFu, min(kInf + fa, fb), 1);   // x_{j0-1}: the previous lanes' maps applied to +inf
-            if (lane == 0) x = kInf;
-            x = min(x, kInf);
-#pragma unroll
-            for (int k = 0; k < kWideCells; ++k) {                     // serial fix-up with the true incoming x
-                x = valid[k] ? min(d[k] + min(A[k], x), kInf) : kInf;
-                D[k] = x;
-            }
+                valid = j >= lo && j <= hi;
+                d = valid ? (s32)pdist(a, b[k]) : 0;
+                A = i == 0 ? (j == 0 ? 0 : kInf) : min(up, dg);
+            }, [](int, s32, s32) {});
         }
-        const int kend = (M - 1) & (kWideCells - 1);
-        s32 e = D[0];
-#pragma unroll
-        for (int k = 1; k < kWideCells; ++k) if (k == kend) e = D[k];
-        const s32 fin = __shfl_sync(0xFFFFFFFFu, e, (M - 1) / kWideCells);
+        const s32 fin = dp_end(D, (M - 1) & 3, (M - 1) / 4);
         return fin < kInf / 2 ? (u32)fin / (u32)(I + M) : SR_DIS_ERR;
     });
 }

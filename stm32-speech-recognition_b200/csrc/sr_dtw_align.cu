@@ -4,9 +4,10 @@
 //
 // dtw_align_kernel: one WARP per (input, template) pair, in the whole-row form of dtw_wide_kernel for EVERY r (the cost
 // does not depend on r, the band only masks cells): lane l owns columns 4l .. 4l+3, the template's four rows stay in
-// registers, one warp scan of the lanes' (min,+) maps and a serial fix-up pass write each row. During the fix-up pass each
-// cell records which neighbour its minimum came from, 2 bits (0 diagonal, 1 (i, j-1), 2 (i-1, j)), ties in that order:
-// one byte per lane per row, 119 x 32 B per warp in shared memory. After the last row lane 0 traces back from
+// registers, and each row is one dp_column step (sr_dtw_core.cuh): a warp scan of the lanes' (min,+) maps and a serial
+// fix-up pass. During the fix-up pass each cell records which neighbour its minimum came from, 2 bits (0 diagonal,
+// 1 (i, j-1), 2 (i-1, j)), ties in that order: one byte per lane per row, 119 x 32 B per warp in shared memory. After
+// the last row lane 0 traces back from
 // (I-1, M-1) to (0, 0) (at most I + M - 1 <= 237 steps) and the warp writes the path forward, (i, j) byte pairs, padded
 // with 0xFF. Pairs come as a list over two base pointers with their own strides (bank slots, v_ftr_tag rows), so the one
 // kernel serves sr_dtw_path_batch and every pass of sr_average_bank; in "pick" mode the template of a pair is the
@@ -24,7 +25,7 @@ constexpr int kPathMax = 2 * kMaxFrm - 1;                 // 237 = I + M - 1 at 
 constexpr int kChoiceBytes = kMaxFrm * 32;                // one byte per lane per row
 constexpr int kPathBuf = 480;                             // 237 u16 points, rounded up
 constexpr int kAlignWarpBytes = 2 * kSlotBytes + kChoiceBytes + kPathBuf;
-constexpr s32 kAlignInf = 0x3FFFFFFF;                     // same headroom argument as dtw_wide_kernel (sr_dtw.cu)
+constexpr s32 kAlignInf = 0x3FFFFFFF;                     // the s32 headroom of dp_column (sr_dtw_core.cuh)
 
 struct AlignPair { u32 in, tpl, out; };
 
@@ -60,47 +61,22 @@ __device__ __forceinline__ s32 align_dp(int I, int M, int r, const unsigned char
         const int c = (i * M) / I, lo = max(c - r, 0), hi = min(c + r, M - 1);
         PRow a;
         load_row(a, uslot, kNrm119, i);                              // broadcast read
-        s32 dg = __shfl_up_sync(0xFFFFFFFFu, D[kAlignCells - 1], 1);  // D(i-1, j0-1)
-        if (lane == 0) dg = kAlignInf;
-        s32 d[kAlignCells], A[kAlignCells];
-        bool valid[kAlignCells], dfirst[kAlignCells];
-        s32 x = kAlignInf, sum = 0;                                  // serial pass for an incoming +inf
-#pragma unroll
-        for (int k = 0; k < kAlignCells; ++k) {
-            const int j = j0 + k;
-            valid[k] = j >= lo && j <= hi;
-            d[k] = valid[k] ? (s32)pdist(a, b[k]) : 0;
-            dfirst[k] = dg <= D[k];                                  // the diagonal is at least as good as (i-1, j)
-            A[k] = i == 0 ? (j == 0 ? 0 : kAlignInf) : min(D[k], dg);
-            dg = D[k];
-            x = valid[k] ? min(d[k] + min(A[k], x), kAlignInf) : kAlignInf;
-            sum += d[k];
-        }
-        s32 fa = sum, fb = x;                                        // inclusive composition of the lanes' maps
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const s32 pa = __shfl_up_sync(0xFFFFFFFFu, fa, o), pb = __shfl_up_sync(0xFFFFFFFFu, fb, o);
-            if (lane >= o) { fb = min(min(pb + fa, fb), kAlignInf); fa += pa; }
-        }
-        x = __shfl_up_sync(0xFFFFFFFFu, min(kAlignInf + fa, fb), 1);
-        if (lane == 0) x = kAlignInf;
-        x = min(x, kAlignInf);
+        bool dfirst[kAlignCells];
         u32 byte = 0;
-#pragma unroll
-        for (int k = 0; k < kAlignCells; ++k) {                      // serial fix-up with the true incoming x = D(i, j-1)
+        dp_column<s32, kAlignInf>(D, lane, [&](int k, s32 up, s32 dg, s32 &d, s32 &A, bool &valid) {
+            const int j = j0 + k;
+            valid = j >= lo && j <= hi;
+            d = valid ? (s32)pdist(a, b[k]) : 0;
+            dfirst[k] = dg <= up;                                    // the diagonal is at least as good as (i-1, j)
+            A = i == 0 ? (j == 0 ? 0 : kAlignInf) : min(up, dg);
+        }, [&](int k, s32 A, s32 x) {
             // minimum of diagonal, (i, j-1), (i-1, j), ties in that order
-            const u32 ch = dfirst[k] ? (A[k] <= x ? 0u : 1u) : (x <= A[k] ? 1u : 2u);
+            const u32 ch = dfirst[k] ? (A <= x ? 0u : 1u) : (x <= A ? 1u : 2u);
             byte |= ch << (2 * k);
-            x = valid[k] ? min(d[k] + min(A[k], x), kAlignInf) : kAlignInf;
-            D[k] = x;
-        }
+        });
         if (choice) choice[i * 32 + lane] = (u8)byte;
     }
-    const int kend = (M - 1) & (kAlignCells - 1);
-    s32 e = D[0];
-#pragma unroll
-    for (int k = 1; k < kAlignCells; ++k) if (k == kend) e = D[k];
-    const s32 fin = __shfl_sync(0xFFFFFFFFu, e, (M - 1) / kAlignCells);
+    const s32 fin = dp_end(D, (M - 1) & (kAlignCells - 1), (M - 1) / kAlignCells);
     return fin < kAlignInf / 2 ? fin : kAlignInf;
 }
 

@@ -1,11 +1,12 @@
-// sr_dtw_connected.cu -- K6: connected words by one-pass DP over the template bank (one-stage DTW, Ney 1984)
-// (EXTENSION: the reference decodes one word per VAD segment; checked against this project's own CPU restatement and
-// plain Python references, parity unpinned).
+// sr_dtw_connected.cu -- K6: connected words by one-pass DP over the template bank (one-stage DTW, Ney 1984), and K6g:
+// the same decoder under a finite-state grammar, over a network of template copies (EXTENSION: the reference decodes one
+// word per VAD segment; both are checked against this project's own CPU restatements and plain Python references, parity
+// unpinned).
 //
 // dtw_connected_kernel: one thread-block CLUSTER per feature sequence, one WARP per bank slot (kConnWarps slots per CTA,
 // up to kConnCluster CTAs per cluster). A warp holds its template's rows in registers, lane l owning columns 4l .. 4l+3
-// as in dtw_wide_kernel / dtw_align_kernel, and advances one input frame per step: one warp scan of the lanes' (min,+)
-// maps and a serial fix-up pass write the template's column of D for that frame. Cells are 64-bit keys
+// as in dtw_wide_kernel / dtw_align_kernel, and advances one input frame per step: one dp_column step (sr_dtw_core.cuh,
+// which also gives the headroom of the keys) writes the template's column of D for that frame. Cells are 64-bit keys
 //   key = D << 10 | (1023 - start)        (start = the input frame the cell's word started at, < 1024)
 // so one unsigned min compares (D, -start) lexicographically: the smallest D, ties to the later start. Cell j = 0 also
 // takes E(i-1) + penalty, a new word starting at frame i. After each frame every warp sends its end cell, re-keyed as
@@ -16,32 +17,94 @@
 // per frame suffices: a CTA writes frame i+2's candidates only after every CTA has passed barrier i+1, i.e. has read
 // frame i's.
 //
-// Headroom: a word's path has at most len + M - 1 <= 818 + 118 cells of get_dis <= 65 535, and at most 818 words each add
-// the penalty (< 2^32): D < 119 * 818 * 65 536 + 818 * 2^32 < 2^42, so D << 17 | slot << 10 | start fits 59 bits and
-// D << 10 plus the row sums of one warp scan (< 128 * 2^26) stays below the infinity 2^62.
+// dtw_grammar_kernel is dtw_connected_kernel with the bank replaced by the grammar's COPIES: a copy c = (state s', member
+// slot t) exists when some arc into s' carries cmd(t), and enters from src(c), the states with such an arc. The host
+// numbers the copies state-major, then by slot, and hands the kernel one word per copy,
+//   copy[c] = slot | state << 8 | src << 16.
+// One warp per copy (ceil(C / kConnWarps) <= 16 CTAs), each frame's column and end-cell exchange exactly as in K6, the
+// copy index in the slot field of the ekey. After the cluster barrier
+//   - each warp reduces only the candidates whose copy's state is in its own src mask: min_{s in src} E_s(i) + P is the
+//     coupling term of its cell j = 0 at frame i + 1 (the state of every copy is kept in a shared byte table);
+//   - global warp g reduces E_s(i) for the states s = g (mod warps in the cluster) and stores it, as an ekey, to the
+//     sequence's record rows in global memory: rec[(rec0 + i) * S + s].
+// At the first frame of a later segment every within-word cell is reset to +inf, so no word crosses the pause, while E and
+// with it the grammar state carry over. After the last frame one lane of rank 0 picks the final state and traces back
+// through the records, writing each word with its segment and segment-relative frames.
 //
 // conn_gather_kernel copies the rows of get_mfcc pieces into their long feature rows; conn_concat_kernel joins the words
 // of the segments of one capture (sr_recognise_connected_batch).
 #include <cooperative_groups.h>
+#include <utility>
 #include "sr_dtw_core.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace srk {
 
-constexpr int kConnWarps = 8;                              // bank slots per CTA
-constexpr int kConnCluster = 16;                           // CTAs per cluster at most: SR_CONN_SLOT_MAX = 128 slots
+constexpr int kConnWarps = 8;                              // bank slots or copies per CTA
+constexpr int kConnCluster = 16;                           // CTAs per cluster at most: 128 slots or copies
 constexpr int kConnCand = kConnWarps * kConnCluster;       // candidates per frame buffer
 constexpr u32 kConnFrm = SR_CONN_FRM_MAX;                  // 818
 constexpr u32 kSeqNrm = kConnFrm * 24;                     // norm offset of the sequence's byte-plane slot
 constexpr int kSeqBytes = kConnFrm * 28;                   // 22 904
 constexpr int kConnSmem = kSeqBytes + kConnWarps * kSlotBytes + 2 * kConnCand * 8 + kConnFrm * 8;   // 58 184
+constexpr int kGramSmem = kSeqBytes + kConnWarps * kSlotBytes + 2 * kConnCand * 8 + kConnCand;      // 51 768
 constexpr u64 kKeyInf = 1ull << 62;
 constexpr u64 kEkeyNone = ~0ull;
-static_assert(kConnWarps * kConnCluster == SR_CONN_SLOT_MAX, "one warp per slot");
-static_assert(kConnFrm < 1024, "start frames are 10-bit fields of the keys");
+constexpr u32 kSegNone = 1023u;                            // segment field of a segment without frames
+static_assert(kConnCand == SR_CONN_SLOT_MAX && kConnCand == SR_GRAM_COPY_MAX, "one warp per slot or copy");
+static_assert(kConnFrm < kSegNone, "start frames and segment first frames are 10-bit fields");
 
 __device__ __forceinline__ u64 umin64(u64 a, u64 b) { return a < b ? a : b; }
+
+// The start of both kernels: the sequence's N rows as byte planes (stage_planes reads row r at src + 4 + 24 r: src is a
+// header-less row array shifted by 4), then member(M), which stages what
+// else the kernel needs and returns the warp's bank slot with M = its frame count (left 0: the warp walks nothing); that
+// template's planes, one cluster barrier (staging done, and every CTA of the cluster runs), then lane l's four template
+// rows in b and a column of +inf in D. Returns M.
+template <class Member>
+__device__ __forceinline__ u32 conn_prologue(cg::cluster_group &cl, unsigned char *smem, const unsigned char *src, u32 N, PRow (&b)[4],
+                                             u64 (&D)[4], Member member) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    unsigned char *tslot = smem + kSeqBytes + warp * kSlotBytes;
+    stage_planes(smem, kSeqNrm, src, (int)N, threadIdx.x, blockDim.x);
+    u32 M = 0;
+    const unsigned char *slot = member(M);
+    if (M) stage_planes(tslot, kNrm119, slot, (int)M, lane, 32);
+    cl.sync();
+    const int j0 = lane * 4;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (M) load_row(b[k], tslot, kNrm119, j0 + k < (int)M ? j0 + k : 0);
+        D[k] = kKeyInf;
+    }
+    return M;
+}
+
+// Frame i of a warp whose template has M frames (0: none): its column by one dp_column step, cell j = 0 entered from
+// `enter`, then its end cell as ekey = D << 17 | idx << 10 | start to candidate idx of every CTA of the cluster, and one
+// cluster barrier. Returns the frame's candidate buffer.
+__device__ __forceinline__ u64 *conn_frame(cg::cluster_group &cl, u32 nc, const unsigned char *smem, u64 *cand, u32 i, u32 M,
+                                           u64 enter, const PRow (&b)[4], u64 (&D)[4], u32 idx) {
+    const int lane = threadIdx.x & 31, j0 = lane * 4;
+    u64 mine = kEkeyNone;
+    if (M) {
+        PRow a;
+        load_row(a, smem, kSeqNrm, (int)i);                // broadcast read
+        dp_column<u64, kKeyInf>(D, lane, [&](int k, u64 up, u64 dg, u64 &d, u64 &A, bool &valid) {
+            const int j = j0 + k;
+            valid = j < (int)M;
+            d = (u64)pdist(a, b[k]) << 10;
+            A = umin64(up, j == 0 ? enter : dg);
+        }, [](int, u64, u64) {});
+        const u64 e = dp_end(D, ((int)M - 1) & 3, ((int)M - 1) >> 2);
+        if (e < kKeyInf) mine = ((e >> 10) << 17) | ((u64)idx << 10) | (u64)(1023u - (u32)(e & 1023u));
+    }
+    u64 *buf = cand + (i & 1) * kConnCand;
+    if ((u32)lane < nc) cl.map_shared_rank(buf, (unsigned)lane)[idx] = mine;
+    cl.sync();
+    return buf;
+}
 
 __global__ void __launch_bounds__(kConnWarps * 32, 2)
 dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__restrict__ frm_num,
@@ -53,10 +116,8 @@ dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__
     const u32 nc = cl.num_blocks(), rank = cl.block_rank();
     const u32 s = blockIdx.x / nc;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    unsigned char *seq = smem_raw;
-    unsigned char *tslot = seq + kSeqBytes + warp * kSlotBytes;
-    u64 *cand = reinterpret_cast<u64 *>(seq + kSeqBytes + kConnWarps * kSlotBytes);   // [2][kConnCand]
-    u64 *rec = cand + 2 * kConnCand;                                                   // [kConnFrm] E(i) as ekey
+    u64 *cand = reinterpret_cast<u64 *>(smem_raw + kSeqBytes + kConnWarps * kSlotBytes);   // [2][kConnCand]
+    u64 *rec = cand + 2 * kConnCand;                                                       // [kConnFrm] E(i) as ekey
     const u32 N = frm_num[s];
     if (N == 0) {                                          // the whole cluster leaves: no barrier, no remote store
         if (rank == 0 && threadIdx.x == 0) {
@@ -66,72 +127,22 @@ dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__
         return;
     }
     const size_t row0 = seq_off ? seq_off[2 * s] : (size_t)s * frm_stride;
-    // the sequence's rows as byte planes (stage_planes reads row r at src + 4 + 24 r: a header-less row array shifted by 4)
-    stage_planes(seq, kSeqNrm, reinterpret_cast<const unsigned char *>(feat + row0 * 12) - 4, (int)N, threadIdx.x, blockDim.x);
     const u32 t = rank * kConnWarps + warp;                // this warp's bank slot
-    u32 M = 0;                                             // 0: not a member, never walked
-    if (t < T) {
-        const unsigned char *slot = bank + (size_t)t * slot_stride;
-        const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);
-        if (frm != kNoWalk) M = frm;
-        if (M) stage_planes(tslot, kNrm119, slot, (int)M, lane, 32);
-    }
-    cl.sync();                                             // staging done, and every CTA of the cluster runs
-    const int j0 = lane * 4;
     PRow b[4];
     u64 D[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        if (M) load_row(b[k], tslot, kNrm119, j0 + k < (int)M ? j0 + k : 0);
-        D[k] = kKeyInf;
-    }
+    const u32 M = conn_prologue(cl, smem_raw, reinterpret_cast<const unsigned char *>(feat + row0 * 12) - 4, N, b, D, [&](u32 &M) {
+        const unsigned char *slot = bank + (size_t)t * slot_stride;
+        if (t < T) {
+            const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);
+            if (frm != kNoWalk) M = frm;
+        }
+        return slot;
+    });
     const u64 pen = penalty;
     u64 enter = (pen << 10) | 1023u;                       // E(-1) + penalty, a word starting at frame 0
     const u32 ncand = nc * kConnWarps;
-    const int lend = ((int)M - 1) >> 2, kend = ((int)M - 1) & 3;
     for (u32 i = 0; i < N; ++i) {
-        u64 mine = kEkeyNone;
-        if (M) {
-            PRow a;
-            load_row(a, seq, kSeqNrm, (int)i);             // broadcast read
-            u64 dg = __shfl_up_sync(0xFFFFFFFFu, D[3], 1); // D(i-1, j0-1)
-            if (lane == 0) dg = kKeyInf;
-            u64 dk[4], A[4];
-            bool valid[4];
-            u64 x = kKeyInf, sum = 0;                      // serial pass for an incoming +inf
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const int j = j0 + k;
-                valid[k] = j < (int)M;
-                dk[k] = (u64)pdist(a, b[k]) << 10;
-                A[k] = umin64(D[k], j == 0 ? enter : dg);
-                dg = D[k];
-                x = valid[k] ? umin64(dk[k] + umin64(A[k], x), kKeyInf) : kKeyInf;
-                sum += dk[k];
-            }
-            u64 fa = sum, fb = x;                          // inclusive composition of the lanes' maps min(x + fa, fb)
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const u64 pa = __shfl_up_sync(0xFFFFFFFFu, fa, o), pb = __shfl_up_sync(0xFFFFFFFFu, fb, o);
-                if (lane >= o) { fb = umin64(umin64(pb + fa, fb), kKeyInf); fa += pa; }
-            }
-            x = __shfl_up_sync(0xFFFFFFFFu, umin64(kKeyInf + fa, fb), 1);
-            if (lane == 0) x = kKeyInf;
-            x = umin64(x, kKeyInf);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {                  // serial fix-up with the true incoming x = D(i, j-1)
-                x = valid[k] ? umin64(dk[k] + umin64(A[k], x), kKeyInf) : kKeyInf;
-                D[k] = x;
-            }
-            u64 e = D[0];
-#pragma unroll
-            for (int k = 1; k < 4; ++k) if (k == kend) e = D[k];
-            e = __shfl_sync(0xFFFFFFFFu, e, lend);
-            if (e < kKeyInf) mine = ((e >> 10) << 17) | ((u64)t << 10) | (u64)(1023u - (u32)(e & 1023u));
-        }
-        u64 *buf = cand + (i & 1) * kConnCand;
-        if ((u32)lane < nc) cl.map_shared_rank(buf, (unsigned)lane)[t] = mine;
-        cl.sync();
+        const u64 *buf = conn_frame(cl, nc, smem_raw, cand, i, M, enter, b, D, t);
         u64 best = kEkeyNone;
         for (u32 q = lane; q < ncand; q += 32) best = umin64(best, buf[q]);
 #pragma unroll
@@ -167,6 +178,131 @@ dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__
     }
     n_words[s] = K;
     if (total) total[s] = last >> 17;
+}
+
+// argmin over the states of mask of E_s(f) (D only, ties to the lowest state); the records of frame f are at r
+__device__ __forceinline__ u32 gram_src(const u64 *r, u32 mask) {
+    u32 best = 0;
+    u64 bd = ~0ull;
+    for (u32 s = 0; mask; ++s, mask >>= 1)
+        if ((mask & 1u) && (__ldcg(r + s) >> 17) < bd) { bd = __ldcg(r + s) >> 17; best = s; }
+    return best;
+}
+
+__global__ void __launch_bounds__(kConnWarps * 32, 2)
+dtw_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ frm_num,
+                   const u32 *__restrict__ seq /* [.][3] first row, first record row, segment first frames (3 x 10 bits) */,
+                   const unsigned char *__restrict__ bank, u32 slot_stride, const u32 *__restrict__ copy, u32 C, u32 S,
+                   u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *__restrict__ words /* or NULL */,
+                   u32 *__restrict__ n_words /* or NULL */, u64 *__restrict__ total /* or NULL */, u64 *rec) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    cg::cluster_group cl = cg::this_cluster();
+    const u32 nc = cl.num_blocks(), rank = cl.block_rank();
+    const u32 s = blockIdx.x / nc;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    u64 *cand = reinterpret_cast<u64 *>(smem_raw + kSeqBytes + kConnWarps * kSlotBytes);   // [2][kConnCand]
+    unsigned char *cst = reinterpret_cast<unsigned char *>(cand + 2 * kConnCand);          // [kConnCand] state of each copy
+    const u32 N = frm_num[s];
+    if (N == 0) {                                          // the whole cluster leaves: no barrier, no remote store
+        if (rank == 0 && threadIdx.x == 0) {
+            if (n_words) n_words[s] = 0;
+            if (total) total[s] = (final_mask & 1u) ? 0ull : ~0ull;
+        }
+        return;
+    }
+    const u32 row0 = seq[3 * s], rec0 = seq[3 * s + 1], segs = seq[3 * s + 2];
+    const u32 f0 = segs & 1023u, f1 = (segs >> 10) & 1023u, f2 = segs >> 20;
+    const u32 ncand = nc * kConnWarps;
+    const u32 c = rank * kConnWarps + warp;                // this warp's copy
+    u32 src = 0;
+    PRow b[4];
+    u64 D[4];
+    const u32 M = conn_prologue(cl, smem_raw, reinterpret_cast<const unsigned char *>(feat + (size_t)row0 * 12) - 4, N, b, D, [&](u32 &M) {
+        for (u32 q = threadIdx.x; q < ncand; q += blockDim.x) cst[q] = q < C ? (unsigned char)((copy[q] >> 8) & 15u) : 0;
+        const unsigned char *slot = bank;
+        if (c < C) {
+            const u32 cw = copy[c];
+            src = cw >> 16;
+            slot = bank + (size_t)(cw & 255u) * slot_stride;
+            M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);   // the host only makes copies of members
+            if (M == kNoWalk) M = 0;
+        }
+        return slot;
+    });
+    const u64 pen = penalty;
+    u64 enter = (src & 1u) ? ((pen << 10) | 1023u) : kKeyInf;   // E_0(-1) + penalty: a word starting at frame 0 from state 0
+    const u32 gw = rank * kConnWarps + warp;
+    u64 *R = rec + (size_t)rec0 * S;
+    for (u32 i = 0; i < N; ++i) {
+        if (M && (i == f0 || i == f1 || i == f2)) {        // a segment's first frame: no word crosses the pause
+#pragma unroll
+            for (int k = 0; k < 4; ++k) D[k] = kKeyInf;
+        }
+        const u64 *buf = conn_frame(cl, nc, smem_raw, cand, i, M, enter, b, D, c);
+        u64 best = kEkeyNone;                              // min over the copies of the states in src: the entry term
+        for (u32 q = lane; q < ncand; q += 32)
+            if ((src >> cst[q]) & 1u) best = umin64(best, buf[q]);
+#pragma unroll
+        for (int o = 16; o; o >>= 1) best = umin64(best, __shfl_xor_sync(0xFFFFFFFFu, best, o));
+        enter = best == kEkeyNone ? kKeyInf : ((((best >> 17) + pen) << 10) | (u64)(1023u - (i + 1)));
+        for (u32 st = gw; st < S; st += ncand) {           // the records E_st(i) this warp owns
+            u64 r = kEkeyNone;
+            for (u32 q = lane; q < ncand; q += 32)
+                if (cst[q] == st) r = umin64(r, buf[q]);
+#pragma unroll
+            for (int o = 16; o; o >>= 1) r = umin64(r, __shfl_xor_sync(0xFFFFFFFFu, r, o));
+            if (lane == 0) R[(size_t)i * S + st] = r;
+        }
+    }
+    __threadfence();
+    cl.sync();                                             // every CTA's records are written
+    if (rank != 0 || threadIdx.x != 0) return;
+    // records are read from L2 (ld.global.cg): other CTAs of the cluster wrote them, and this SM's L1 may hold a line of
+    // them from an earlier sequence. The final state: the smallest E_s(N-1) over final states, ties to the lowest state
+    u32 fs = S;
+    u64 fd = ~0ull;
+    for (u32 st = 0; st < S; ++st) {
+        const u64 r = __ldcg(R + (size_t)(N - 1) * S + st);
+        if (((final_mask >> st) & 1u) && r != kEkeyNone && (r >> 17) < fd) { fd = r >> 17; fs = st; }
+    }
+    if (fs == S) {                                         // no accepting path
+        if (n_words) n_words[s] = 0;
+        if (total) total[s] = ~0ull;
+        return;
+    }
+    // trace-back: the word ending at frame i in state st is [start, i + 1) of its copy, entered from the source state with
+    // the smallest E(start - 1) (state 0 at start 0)
+    u32 K = 0;
+    for (int i = (int)N - 1, st = (int)fs; i >= 0;) {
+        const u64 r = __ldcg(R + (size_t)i * S + st);
+        const u32 b0 = (u32)(r & 1023u), cp = (u32)((r >> 10) & 127u);
+        if (b0) st = (int)gram_src(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
+        i = (int)b0 - 1;
+        ++K;
+    }
+    u32 k = K;
+    for (int i = (int)N - 1, st = (int)fs; i >= 0;) {
+        const u64 r = __ldcg(R + (size_t)i * S + st);
+        const u32 b0 = (u32)(r & 1023u), cp = (u32)((r >> 10) & 127u);
+        u64 prev = 0;
+        if (b0) {
+            st = (int)gram_src(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
+            prev = __ldcg(R + (size_t)(b0 - 1) * S + st) >> 17;
+        }
+        --k;
+        if (words && k < max_words) {
+            const u32 g = (f2 != kSegNone && b0 >= f2) ? 2u : (f1 != kSegNone && b0 >= f1) ? 1u : 0u;
+            const u32 fb = g == 2 ? f2 : g == 1 ? f1 : f0;
+            sr_conn_word w;
+            w.slot = copy[cp] & 255u; w.cmd = w.slot / SR_FTR_PER_COMM; w.segment = g;
+            w.start = b0 - fb; w.end = (u32)i + 1 - fb;
+            w.dis = (u32)((r >> 17) - prev - pen);
+            words[(size_t)s * max_words + k] = w;
+        }
+        i = (int)b0 - 1;
+    }
+    if (n_words) n_words[s] = K;
+    if (total) total[s] = fd;
 }
 
 // rows [0, nf) of piece p's feature set -> long feature rows dst_row .. dst_row + nf - 1; pdst[p] = (dst_row, nf)
@@ -209,21 +345,18 @@ conn_concat_kernel(const u32 *__restrict__ seq_of, const u32 *__restrict__ seq_o
     if (total) total[b] = tot;
 }
 
-// sequences [b0, b0 + nb) against the bank's T <= SR_CONN_SLOT_MAX slots in one launch: one cluster of
-// ceil(T / kConnWarps) CTAs per sequence
-cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 b0, u32 nb,
-                                 const void *bank, u32 T, u32 slot_stride, u32 penalty, u32 max_words, sr_conn_word *words,
-                                 u32 *n_words, u64 *total, cudaStream_t st) {
-    if (nb == 0) return cudaSuccess;
-    if (T > SR_CONN_SLOT_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
-    const u32 nc = T ? (T + kConnWarps - 1) / kConnWarps : 1u;
-    cudaError_t e = cudaFuncSetAttribute(dtw_connected_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kConnSmem);
-    if (e == cudaSuccess && nc > 8) e = cudaFuncSetAttribute(dtw_connected_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+// nb sequences, one cluster of ceil(n / kConnWarps) CTAs (one warp per slot or copy, at least one CTA) per sequence;
+// clusters of more than 8 CTAs need the non-portable size
+template <class... P, class... A>
+static cudaError_t launch_clusters(void (*kernel)(P...), int smem, u32 nb, u32 n, cudaStream_t st, A &&...args) {
+    const u32 nc = n ? (n + kConnWarps - 1) / kConnWarps : 1u;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess && nc > 8) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(nb * nc);
     cfg.blockDim = dim3(kConnWarps * 32);
-    cfg.dynamicSmemBytes = kConnSmem;
+    cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -232,13 +365,36 @@ cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    const s16 *f = seq_off ? feat : feat + (size_t)b0 * frm_stride * 12;
-    e = cudaLaunchKernelEx(&cfg, dtw_connected_kernel, f, frm_stride, frm_num + b0, seq_off ? seq_off + 2 * (size_t)b0 : nullptr,
-                           static_cast<const unsigned char *>(bank), T, slot_stride, penalty, max_words,
-                           words && !seq_off ? words + (size_t)b0 * max_words : words, n_words + b0,
-                           total ? total + b0 : nullptr);
+    e = cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
+}
+
+// sequences [b0, b0 + nb) against the bank's T <= SR_CONN_SLOT_MAX slots in one launch
+cudaError_t launch_dtw_connected(const s16 *feat, u32 frm_stride, const u32 *frm_num, const u32 *seq_off, u32 b0, u32 nb,
+                                 const void *bank, u32 T, u32 slot_stride, u32 penalty, u32 max_words, sr_conn_word *words,
+                                 u32 *n_words, u64 *total, cudaStream_t st) {
+    if (nb == 0) return cudaSuccess;
+    if (T > SR_CONN_SLOT_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
+    const s16 *f = seq_off ? feat : feat + (size_t)b0 * frm_stride * 12;
+    return launch_clusters(dtw_connected_kernel, kConnSmem, nb, T, st, f, frm_stride, frm_num + b0,
+                           seq_off ? seq_off + 2 * (size_t)b0 : nullptr, static_cast<const unsigned char *>(bank), T,
+                           slot_stride, penalty, max_words, words && !seq_off ? words + (size_t)b0 * max_words : words,
+                           n_words + b0, total ? total + b0 : nullptr);
+}
+
+// sequences [b0, b0 + nb) (the table seq gives each its first feature row, its first record row and its segments) against
+// C <= SR_GRAM_COPY_MAX copies of the bank's slots in one launch. rec holds (last record row + 1) * S records; the caller
+// chunks its sequences to bound it.
+cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 b0, u32 nb, const void *bank, u32 slot_stride,
+                               const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
+                               u32 *n_words, u64 *total, u64 *rec, cudaStream_t st) {
+    if (nb == 0) return cudaSuccess;
+    if (C > SR_GRAM_COPY_MAX || S == 0 || S > SR_GRAM_STATE_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
+    return launch_clusters(dtw_grammar_kernel, kGramSmem, nb, C, st, feat, frm_num + b0, seq + 3 * (size_t)b0,
+                           static_cast<const unsigned char *>(bank), slot_stride, copy, C, S, final_mask, penalty, max_words,
+                           words ? words + (size_t)b0 * max_words : nullptr, n_words ? n_words + b0 : nullptr,
+                           total ? total + b0 : nullptr, rec);
 }
 
 cudaError_t launch_conn_gather(const void *pf, const u32 *pdst, u32 P, s16 *feat, int num_sms, cudaStream_t st) {

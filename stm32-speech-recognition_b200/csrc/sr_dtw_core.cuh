@@ -149,6 +149,66 @@ __device__ __forceinline__ bool greedy_step(int I, int M, int X1, int X2, PRow &
     return true;
 }
 
+// ---- the whole-row (min,+) DP column step (dtw_wide_kernel, align_dp, dtw_connected_kernel, dtw_grammar_kernel) ------
+// One warp holds a template column of up to 128 cells, lane l the cells j = 4l .. 4l+3 in D[4]; a step turns the column
+// of the previous input row (or frame) into this one. Per cell x_j = d_j + min(A_j, x_{j-1}), A_j = min(up, diag): the
+// up and diag terms come from the lane's own D (diag of its first cell by one shuffle), so the in-row recurrence maps a
+// lane's incoming x to its outgoing one as f(x) = min(x + a, b) (a = the lane's sum of d, b = its outgoing x for an
+// incoming +inf). One warp scan composes these maps, f2(f1(x)) = min(x + a1 + a2, min(b1 + a2, b2)), giving every lane
+// its incoming x, and a serial fix-up pass over the lane's four cells writes the column.
+// cell(k, up, dg, d, A, valid) fills cell k's local distance d, its A (from up = D(i-1, j) and dg = D(i-1, j-1)) and
+// its validity; a cell that is not valid is +inf, and its d still enters the lane's a. fix(k, A, x) sees each cell's A and incoming x = D(i, j-1)
+// during the fix-up pass, before the cell is written.
+// Headroom of the s32 keys of dtw_wide_kernel and align_dp, +inf = 2^30 - 1: a path to cell (i,j) has at most i+j+1
+// cells of at most 65 536, so every reachable cell is below 237 * 65 536 = 15 532 032 and a full-matrix optimum at most
+// max(I,M) * 65 536; +inf sums (b1 + a2 <= +inf + 119 * 65 536) stay below 2^31 and are cut back to +inf, so a cell is
+// reachable exactly when it is below +inf / 2.
+// Headroom of the u64 keys D << 10 | (1023 - start) of dtw_connected_kernel and dtw_grammar_kernel, +inf = 2^62: a word's
+// path has at most len + M - 1 <= 818 + 118 cells of get_dis <= 65 535, and at most 818 words each add the penalty
+// (< 2^32): D < 119 * 818 * 65 536 + 818 * 2^32 < 2^42, so the end key D << 17 | index << 10 | start fits 59 bits and
+// D << 10 plus the row sums of one warp scan (< 128 * 2^26) stays below 2^62.
+__device__ __forceinline__ s32 dp_min(s32 a, s32 b) { return min(a, b); }
+__device__ __forceinline__ u64 dp_min(u64 a, u64 b) { return a < b ? a : b; }
+
+template <class K, K kInfK, class Cell, class Fix>
+__device__ __forceinline__ void dp_column(K (&D)[4], int lane, Cell cell, Fix fix) {
+    K dg = __shfl_up_sync(0xFFFFFFFFu, D[3], 1);                     // D(i-1, j0-1)
+    if (lane == 0) dg = kInfK;
+    K d[4], A[4];
+    bool valid[4];
+    K x = kInfK, sum = 0;                                            // serial pass for an incoming +inf: b and a
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        cell(k, D[k], dg, d[k], A[k], valid[k]);
+        dg = D[k];
+        x = valid[k] ? dp_min(d[k] + dp_min(A[k], x), kInfK) : kInfK;
+        sum += d[k];
+    }
+    K fa = sum, fb = x;                                              // inclusive composition of the lanes' maps
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const K pa = __shfl_up_sync(0xFFFFFFFFu, fa, o), pb = __shfl_up_sync(0xFFFFFFFFu, fb, o);
+        if (lane >= o) { fb = dp_min(dp_min(pb + fa, fb), kInfK); fa += pa; }
+    }
+    x = __shfl_up_sync(0xFFFFFFFFu, dp_min(kInfK + fa, fb), 1);     // x_{j0-1}: the previous lanes' maps applied to +inf
+    if (lane == 0) x = kInfK;
+    x = dp_min(x, kInfK);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {                                    // serial fix-up with the true incoming x
+        fix(k, A[k], x);
+        x = valid[k] ? dp_min(d[k] + dp_min(A[k], x), kInfK) : kInfK;
+        D[k] = x;
+    }
+}
+// the end cell D(., M-1) of a column, in every lane: cell kend = (M-1) & 3 of lane lend = (M-1) / 4
+template <class K>
+__device__ __forceinline__ K dp_end(const K (&D)[4], int kend, int lend) {
+    K e = D[0];
+#pragma unroll
+    for (int k = 1; k < 4; ++k) if (k == kend) e = D[k];
+    return __shfl_sync(0xFFFFFFFFu, e, lend);
+}
+
 // score[u][t] and the spch_recg argmin (main.c:276-291) as one 64-bit atomicMin of (result, bank slot t):
 // strict '<', first wins == lexicographic min
 __device__ __forceinline__ void emit_pair(u32 *score, u64 *best, u32 T, u32 u, u32 t, u32 result) {

@@ -61,7 +61,7 @@ cudaError_t launch_conn_concat(const u32 *seq_of, const u32 *seq_off, const sr_c
                                cudaStream_t st);
 // the grammar decoder over sequences [b0, b0 + nb) of a batch, nb <= kSeqChunk (seq: [B][3] first feature row, first
 // record row, segment first frames) against C copies of bank slots (copy: [C] slot | state << 8 | src << 16), records in
-// rec (sr_dtw_grammar.cu)
+// rec (sr_dtw_connected.cu)
 cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 b0, u32 nb, const void *bank, u32 slot_stride,
                                const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
                                u32 *n_words, u64 *total, u64 *rec, cudaStream_t st);
