@@ -475,7 +475,8 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
  * calls under the SR_DTW_BAND matcher), 7 the banded DP with its path (every pass of sr_dtw_path_batch and
  * sr_average_bank that aligns), 8 sr_average_bank's template update, 9 the connected-word decoder (sr_connected_batch,
  * sr_recognise_connected_batch; their get_mfcc launches are tag 1), 10 the grammar decoder (sr_connected_grammar_batch,
- * sr_recognise_connected_grammar_batch; their get_mfcc launches are tag 1). max_records = 0 disables. */
+ * sr_recognise_connected_grammar_batch; their get_mfcc launches are tag 1), 11 and 12 the long-form block and segment passes
+ * (include/sr_long.h). max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 6; }
+int sr_abi_version(void) { return 7; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -180,7 +180,7 @@ int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
        TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
-       TAG_GRAM = 10 };
+       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12 };
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
@@ -1134,6 +1134,168 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
     if (d.words || d.nw || d.total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
     return conn_finish(c, o, B, atap, seg, frm, status);
+}
+
+}  // extern "C"
+
+// ---- long-form VAD and per-segment recognition (sr_long.h) ----------------------------------------------------------
+static bool long_args_ok(u32 U, u32 B, u32 n_len, u32 max_segs) {
+    return U <= SR_LONG_U_MAX && n_len <= 65535u && (uint64_t)B * max_segs < (1ull << 32);
+}
+
+// the long-form noise_atap and VAD of B recordings at pcm (device): noise_atap and the block summaries (tag 11), the
+// segment pass (tag 12)
+static int vad_long_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, const u32 *lens, u32 n_len, u32 max_segs, atap_tag *atap,
+                         u32 *n_segs, u32 *seg_off) {
+    SR_CK(h, ensure(h->lng[0], (size_t)B * long_info_stride(U) * 4));
+    u32 *info = static_cast<u32 *>(h->lng[0].p);
+    SR_LAUNCH(h, TAG_LONG_BLOCKS, launch_long_atap(pcm, U, B, lens, n_len, atap, h->stream));
+    SR_LAUNCH(h, TAG_LONG_BLOCKS, launch_long_blocks(pcm, U, B, lens, atap, info, h->num_sms, h->stream));
+    SR_LAUNCH(h, TAG_LONG_SEGS, launch_long_segments(U, B, lens, atap, info, max_segs, n_segs, seg_off, h->stream));
+    return 0;
+}
+
+// spch_recg's decision on the first min(n_segs[b], max_segs) segments of each of B recordings (n_segs, seg_off
+// [B][max_segs][2], atap: device): the flat segment table (prefix sum, then the table), get_mfcc with a row map (tag 1),
+// status (2), best-init (3), the template scan with the handle's matcher (4 or 6) and the argmin scatter into rec (5).
+// Every kernel after the prefix sum reads the segment count from device memory; B * max_segs bounds the launches.
+static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 max_segs, const atap_tag *atap, const u32 *n_segs,
+                               const u32 *seg_off, sr_long_seg *rec) {
+    const u32 M = B * max_segs;
+    if (M == 0) return 0;
+    SR_CK(h, ensure(h->lng[2], ((size_t)B + 1) * 4));                  // first[B] | n_flat
+    SR_CK(h, ensure(h->lng[3], (size_t)M * 16));                       // seg2[M][2] | row[M] | slot[M]
+    SR_CK(h, ensure(h->lng[4], (size_t)M * sizeof(atap_tag)));
+    SR_CK(h, ensure(h->lng[5], (size_t)M));
+    SR_CK(h, ensure(h->lng[6], (size_t)M * 8));
+    SR_CK(h, ensure(h->lng[7], (size_t)M * kFtrBytes));
+    u32 *first = static_cast<u32 *>(h->lng[2].p), *n_flat = first + B;
+    u32 *seg2 = static_cast<u32 *>(h->lng[3].p), *row = seg2 + 2 * (size_t)M, *slot = row + M;
+    atap_tag *atap_seg = static_cast<atap_tag *>(h->lng[4].p);
+    u8 *status = static_cast<u8 *>(h->lng[5].p);
+    u64 *best = static_cast<u64 *>(h->lng[6].p);
+    void *ftr = h->lng[7].p;
+    SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 0));
+    SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 1));
+    SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, M, seg2, 2, atap_seg, ftr, row, B, n_flat));     // main.c:268
+    SR_LAUNCH(h, TAG_STATUS, launch_long_status(seg2, ftr, n_flat, M, status, h->stream));          // main.c:261-274
+    SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, M, h->stream));                               // main.c:276-278
+    if (h->bank.n) {                                                   // main.c:279-291, save_sign honoured (main.c:283)
+        const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags;
+        SR_LAUNCH(h, (flags & SR_DTW_BAND) ? TAG_DTW_BAND : TAG_DTW,
+                  launch_scan(h, h->bank, ftr, M, flags, h->match_r, nullptr, best, status, n_flat));
+    }
+    SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, best, n_flat, M, rec, h->stream));   // main.c:292-294
+    return 0;
+}
+
+constexpr size_t kLongGroupBytes = (size_t)256 << 20;   // PCM per staged group of the host calls
+
+// The host-buffer long-form calls: whole recordings staged in groups of at most kLongGroupBytes of PCM (at least one
+// recording) through two device buffers -- the copy of group g+1 (copy stream) overlaps the kernels of group g -- and
+// run(device PCM, first recording, recordings) per group. A recording is never split.
+template <class F> static int long_groups(HostCall &c, const uint16_t *pcm, u32 U, u32 B, F run) {
+    sr_handle *h = c.h;
+    u32 G = (u32)(kLongGroupBytes / ((size_t)U * 2));
+    G = std::max(1u, std::min(G, B));
+    const u32 ng = (B + G - 1) / G;
+    const size_t gbytes = (((size_t)G * U * 2 + 255) / 256) * 256;
+    c.ws(h->pcm, (ng > 1 ? 2 : 1) * gbytes + 16);
+    for (u32 g = 0; g < ng && !c.rc; ++g) {
+        const u32 b0 = g * G, nb = std::min(G, B - b0);
+        const int buf = g & 1;
+        u16 *dpcm = reinterpret_cast<u16 *>(static_cast<unsigned char *>(h->pcm.p) + (size_t)buf * gbytes);
+        cudaStream_t cs = ng > 1 ? h->copy_stream : h->stream;
+        if (ng > 1 && g >= 2) c.ck("cudaStreamWaitEvent", cudaStreamWaitEvent(cs, h->ev_done[buf], 0));   // buffer free again
+        c.ck("cudaMemcpyAsync host->device", cudaMemcpyAsync(dpcm, pcm + (size_t)b0 * U, (size_t)nb * U * 2, cudaMemcpyHostToDevice, cs));
+        if (ng > 1) {
+            c.ck("cudaEventRecord", cudaEventRecord(h->ev_h2d[buf], cs));
+            c.ck("cudaStreamWaitEvent", cudaStreamWaitEvent(h->stream, h->ev_h2d[buf], 0));
+        }
+        c.run([&] { return run(static_cast<const u16 *>(dpcm), b0, nb); });
+        if (ng > 1) c.ck("cudaEventRecord", cudaEventRecord(h->ev_done[buf], h->stream));
+    }
+    return c.finish();
+}
+
+extern "C" {
+
+int sr_vad_long_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens, uint32_t n_len,
+                          uint32_t max_segs, atap_tag *atap, uint32_t *n_segs, uint32_t *seg_off) {
+    SR_REQUIRE(h, h && (B == 0 || (pcm && atap && n_segs && (seg_off || max_segs == 0))));
+    SR_REQUIRE(h, long_args_ok(U, B, n_len, max_segs));
+    if (B == 0) return 0;
+    DeviceGuard g(h->device);
+    return vad_long_impl(h, pcm, U, B, lens, n_len, max_segs, atap, n_segs, seg_off);
+}
+
+int sr_recognise_long_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens, uint32_t n_len,
+                                uint32_t max_segs, const sr_long_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || (pcm && (o->segs || max_segs == 0))));
+    SR_REQUIRE(h, long_args_ok(U, B, n_len, max_segs));
+    if (B == 0) return 0;
+    DeviceGuard g(h->device);
+    atap_tag *atap = o->atap;
+    if (!atap) {                                        // as sr_recognise_batch_dev: noise_atap on a zeroed record
+        SR_CK(h, ensure(h->lng[8], (size_t)B * sizeof(atap_tag)));
+        atap = static_cast<atap_tag *>(h->lng[8].p);
+        SR_CK(h, cudaMemsetAsync(atap, 0, (size_t)B * sizeof(atap_tag), h->stream));
+    }
+    u32 *n_segs = o->n_segs;
+    if (!n_segs) { SR_CK(h, ensure(h->lng[9], (size_t)B * 4)); n_segs = static_cast<u32 *>(h->lng[9].p); }
+    SR_CK(h, ensure(h->lng[1], (size_t)B * max_segs * 8 + 8));
+    u32 *seg_off = static_cast<u32 *>(h->lng[1].p);
+    if (const int rc = vad_long_impl(h, pcm, U, B, lens, n_len, max_segs, atap, n_segs, seg_off)) return rc;
+    return recognise_segs_impl(h, pcm, U, B, max_segs, atap, n_segs, seg_off, o->segs);
+}
+
+int sr_vad_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens, uint32_t n_len,
+                      uint32_t max_segs, atap_tag *atap, uint32_t *n_segs, uint32_t *seg_off) {
+    SR_REQUIRE(h, h && (B == 0 || (pcm && atap && n_segs && (seg_off || max_segs == 0))));
+    SR_REQUIRE(h, (B == 0 || U > 0) && long_args_ok(U, B, n_len, max_segs));
+    for (u32 b = 0; lens && b < B; ++b) SR_REQUIRE(h, lens[b] <= U);
+    if (B == 0) return 0;
+    HostCall c(h, "sr_vad_long_batch");
+    const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
+    atap_tag *d_atap = c.in(h->lng[8], atap, (size_t)B * sizeof(atap_tag));      // in / out: untouched when noise_atap skips
+    c.out(h->lng[8], atap, (size_t)B * sizeof(atap_tag));
+    u32 *d_n = c.out(h->lng[9], n_segs, (size_t)B * 4);
+    const size_t sbytes = (size_t)B * max_segs * 8;
+    u32 *d_seg = nullptr;
+    if (sbytes) {                                                           // in / out: segments past n_segs keep the caller's bytes
+        d_seg = c.in(h->lng[10], seg_off, sbytes);
+        c.out(h->lng[10], seg_off, sbytes);
+    }
+    return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
+        return sr_vad_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, d_atap + b0, d_n + b0,
+                                     d_seg ? d_seg + (size_t)b0 * max_segs * 2 : nullptr);
+    });
+}
+
+int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens, uint32_t n_len,
+                            uint32_t max_segs, const sr_long_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || (pcm && (o->segs || max_segs == 0))));
+    SR_REQUIRE(h, (B == 0 || U > 0) && long_args_ok(U, B, n_len, max_segs));
+    for (u32 b = 0; lens && b < B; ++b) SR_REQUIRE(h, lens[b] <= U);
+    if (B == 0) return 0;
+    HostCall c(h, "sr_recognise_long_batch");
+    const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
+    atap_tag *d_atap = nullptr;
+    if (o->atap) {
+        d_atap = c.in(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
+        c.out(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
+    }
+    u32 *d_n = o->n_segs ? c.out(h->lng[9], o->n_segs, (size_t)B * 4) : nullptr;
+    const size_t rbytes = (size_t)B * max_segs * sizeof(sr_long_seg);
+    sr_long_seg *d_rec = nullptr;
+    if (rbytes) {                                                           // in / out: records past n_segs keep the caller's bytes
+        d_rec = c.in(h->lng[10], o->segs, rbytes);
+        c.out(h->lng[10], o->segs, rbytes);
+    }
+    return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
+        const sr_long_out od{d_atap ? d_atap + b0 : nullptr, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
+        return sr_recognise_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, &od);
+    });
 }
 
 // One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]

@@ -13,6 +13,7 @@
 #include <thread>
 #include <vector>
 #include "sr_common.cuh"
+#include "../../include/sr_long.h"
 
 namespace srk {
 cudaError_t launch_vad(const u16 *pcm, u32 U, u32 B, u32 n_len, u32 buf_len, int do_atap, int do_vad, atap_tag *atap,
@@ -67,6 +68,20 @@ cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *s
                                u32 *n_words, u64 *total, u64 *rec, cudaStream_t st);
 cudaError_t launch_sqrt_check(u32 lo, u32 hi, unsigned long long *bad_dev, cudaStream_t st);
 cudaError_t launch_unpack12(const void *packed, u64 n_samples, u16 *out, cudaStream_t st);
+// the long-form VAD and its per-segment recognition (sr_vad_long.cu): noise_atap, the block summaries into info
+// ([B][long_info_stride(U)] words), the segment pass, the flat segment table (step 0: the prefix sum into first / n_flat,
+// step 1: the table), the per-segment status and the scatter of the argmin into the records
+u32 long_info_stride(u32 U);
+cudaError_t launch_long_atap(const u16 *pcm, u32 U, u32 B, const u32 *lens, u32 n_len, atap_tag *atap, cudaStream_t st);
+cudaError_t launch_long_blocks(const u16 *pcm, u32 U, u32 B, const u32 *lens, const atap_tag *atap, u32 *info, int num_sms,
+                               cudaStream_t st);
+cudaError_t launch_long_segments(u32 U, u32 B, const u32 *lens, const atap_tag *atap, const u32 *info, u32 max_segs, u32 *n_segs,
+                                 u32 *seg_off, cudaStream_t st);
+cudaError_t launch_long_flatten(const u32 *n_segs, const u32 *seg_off, const atap_tag *atap, u32 B, u32 max_segs, u32 *first,
+                                u32 *n_flat, u32 *seg2, u32 *row, u32 *slot, atap_tag *atap_seg, cudaStream_t st, int step);
+cudaError_t launch_long_status(const u32 *seg2, const void *ftr, const u32 *n_flat, u32 M, u8 *status, cudaStream_t st);
+cudaError_t launch_long_scatter(const u32 *seg2, const u32 *slot, const void *ftr, const u8 *status, const u64 *best,
+                                const u32 *n_flat, u32 M, sr_long_seg *rec, cudaStream_t st);
 class PackPool;
 }  // namespace srk
 
@@ -185,6 +200,9 @@ struct sr_handle {
     DevBuf align[6];                                   // sr_dtw_path_batch / sr_average_bank: pairs, paths, templates, scores
     DevBuf conn[10];                                   // long features and the connected-word decoder: pieces, features, words
     DevBuf gram[4];                                    // the grammar decoder: copy table, sequence table, frame counts, records
+    DevBuf lng[12];                                    // long-form VAD and recognition (sr_long.h): block summaries, segments,
+                                                       // counts, the flat segment table, its atap, status, keys, features, lens
+                                                       // and the host calls' device outputs
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };

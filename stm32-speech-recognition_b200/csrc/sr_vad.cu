@@ -22,40 +22,6 @@ namespace srk {
 
 constexpr int kVadMaxWarps = 20;
 
-// start staging samples [first, first+count) of the batch into `buf` (bulk async copy when the batch base is 16-byte
-// aligned, plain loads otherwise); completion is one phase of `bar` either way. Returns the sample index of `first`
-// inside buf.
-__device__ __forceinline__ int chunk_issue(unsigned char *buf, const u16 *pcm, size_t total_bytes, bool base_aligned,
-                                           size_t first, u32 count, u64 *bar, int lane) {
-    const size_t lo = first * 2, hi = lo + (size_t)count * 2;
-    if (base_aligned) {
-        const size_t lo_al = lo & ~(size_t)15;
-        size_t hi_al = (hi + 15) & ~(size_t)15;
-        const size_t lim = total_bytes & ~(size_t)15;
-        if (hi_al > lim) hi_al = lim;
-        const int shift = (int)((lo - lo_al) >> 1);
-        if (hi > hi_al) {                                        // tail beyond the last whole 16-byte granule
-            const u16 *g = reinterpret_cast<const u16 *>(reinterpret_cast<const unsigned char *>(pcm) + hi_al);
-            u16 *d = reinterpret_cast<u16 *>(buf + (hi_al - lo_al));
-            const int n = (int)((hi - hi_al) >> 1);
-            if (lane < n) d[lane] = g[lane];
-        }
-        __syncwarp();
-        if (lane == 0) {
-            const u32 nbytes = (u32)(hi_al - lo_al);
-            mbar_arrive_expect_tx(bar, nbytes);
-            bulk_g2s(buf, reinterpret_cast<const unsigned char *>(pcm) + lo_al, nbytes, bar);
-        }
-        return shift;
-    }
-    const u16 *g = pcm + first;
-    u16 *d = reinterpret_cast<u16 *>(buf);
-    for (u32 i = lane; i < count; i += 32) d[i] = g[i];
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar);
-    return 0;
-}
-
 constexpr u32 kVadChunk = 32 * 80;                               // samples per staged chunk: one 80-sample block per lane
 
 __global__ void __launch_bounds__(kVadMaxWarps * 32)

@@ -89,6 +89,14 @@ def chain_grammar(L, cmd_mask=0x3FF):
     return (L + 1, 1 << L, [(k, k + 1, cmd_mask) for k in range(L)])
 
 
+LONG_U_MAX = 1 << 27           # SR_LONG_U_MAX: the longest recording of the long-form calls (include/sr_long.h)
+LONG_SEG_DTYPE = np.dtype([(k, "<u4") for k in ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")])
+
+
+class LongOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("atap", "n_segs", "segs")]
+
+
 class StreamEvent(C.Structure):
     _fields_ = [(k, C.c_uint32) for k in ("stream", "segment", "start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")]
 
@@ -137,6 +145,10 @@ def lib():
         L.sr_recognise_connected_batch.argtypes = [vp, vp, u32, u32, u32, u32, u32, C.POINTER(ConnOut)]
         L.sr_connected_grammar_batch.argtypes = [vp, vp, vp, u32, u32, vp, u32, u32, vp, vp, vp]
         L.sr_recognise_connected_grammar_batch.argtypes = [vp, vp, u32, u32, u32, vp, u32, u32, C.POINTER(ConnOut)]
+        L.sr_vad_long_batch.argtypes = [vp, vp, u32, u32, vp, u32, u32, vp, vp, vp]
+        L.sr_vad_long_batch_dev.argtypes = [vp, vp, u32, u32, vp, u32, u32, vp, vp, vp]
+        L.sr_recognise_long_batch.argtypes = [vp, vp, u32, u32, vp, u32, u32, C.POINTER(LongOut)]
+        L.sr_recognise_long_batch_dev.argtypes = [vp, vp, u32, u32, vp, u32, u32, C.POINTER(LongOut)]
         L.sr_streams_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
         L.sr_streams_destroy.argtypes = [vp]
         L.sr_streams_reset.argtypes = [vp]
@@ -443,6 +455,39 @@ class Handle:
         self._ck(lib().sr_recognise_connected_grammar_batch(self._h, _p(pcm), U, B, n_len, None if g is None else C.byref(g),
                                                             penalty, max_words, C.byref(o)))
         return out
+
+    # -- long-form VAD and per-segment recognition (include/sr_long.h)
+    def vad_long_batch(self, pcm, max_segs, n_len=2400, lens=None, atap=None, seg_off=None):
+        """long-form noise_atap + VAD of pcm [B, U] (lens [B] samples each, None = U): dict(atap [B], n_segs [B],
+        seg_off [B, max_segs, 2]); atap and seg_off are in / out (prefilled bytes stay where nothing is written)"""
+        B, U = pcm.shape
+        atap = np.zeros(B, ATAP_DTYPE) if atap is None else atap
+        seg_off = np.zeros((B, max_segs, 2), np.uint32) if seg_off is None else seg_off
+        lens = None if lens is None else np.ascontiguousarray(lens, np.uint32)
+        n_segs = np.zeros(B, np.uint32)
+        self._ck(lib().sr_vad_long_batch(self._h, _p(pcm), U, B, _p(lens), n_len, max_segs, _p(atap), _p(n_segs),
+                                         _p(seg_off) if max_segs else None))
+        return dict(atap=atap, n_segs=n_segs, seg_off=seg_off)
+
+    def recognise_long_batch(self, pcm, max_segs, n_len=2400, lens=None, atap=None, segs=None):
+        """long-form VAD, then spch_recg's decision on every segment: dict(atap [B], n_segs [B], segs [B, max_segs]
+        LONG_SEG_DTYPE); atap and segs are in / out"""
+        B, U = pcm.shape
+        atap = np.zeros(B, ATAP_DTYPE) if atap is None else atap
+        segs = np.zeros((B, max_segs), LONG_SEG_DTYPE) if segs is None else segs
+        lens = None if lens is None else np.ascontiguousarray(lens, np.uint32)
+        n_segs = np.zeros(B, np.uint32)
+        out = LongOut(_p(atap), _p(n_segs), _p(segs) if max_segs else None)
+        self._ck(lib().sr_recognise_long_batch(self._h, _p(pcm), U, B, _p(lens), n_len, max_segs, C.byref(out)))
+        return dict(atap=atap, n_segs=n_segs, segs=segs)
+
+    def vad_long_batch_dev(self, pcm_ptr, U, B, lens_ptr, n_len, max_segs, atap_ptr, n_segs_ptr, seg_ptr):
+        self._ck(lib().sr_vad_long_batch_dev(self._h, _p(pcm_ptr), U, B, _p(lens_ptr), n_len, max_segs, _p(atap_ptr),
+                                             _p(n_segs_ptr), _p(seg_ptr)))
+
+    def recognise_long_batch_dev(self, pcm_ptr, U, B, lens_ptr, n_len, max_segs, atap_ptr, n_segs_ptr, segs_ptr):
+        out = LongOut(_p(atap_ptr), _p(n_segs_ptr), _p(segs_ptr))
+        self._ck(lib().sr_recognise_long_batch_dev(self._h, _p(pcm_ptr), U, B, _p(lens_ptr), n_len, max_segs, C.byref(out)))
 
     def fft_mag(self, frames):
         n, length = frames.shape
