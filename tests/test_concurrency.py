@@ -7,8 +7,8 @@ against a run made alone. The job table below runs one fixed script per entry-po
 serial baseline runs each job alone (checked on a sample against its oracle), then every job runs R times at once, one
 thread per handle. ctypes releases the GIL during each C call, so the threads' library calls overlap. Each job alternates
 between two inputs, so a repetition that skips work and leaves the previous repetition's workspace contents behind
-cannot pass. The last test is a CPU test: every sr_* entry point of the header is either in the job table or excluded
-with a reason."""
+cannot pass. The last test is a CPU test: every sr_* entry point of the headers (speech_recog.h and sr_long.h) is either
+in the job table or excluded with a reason."""
 import ctypes as C
 import os
 import re
@@ -29,7 +29,7 @@ import sr_b200
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-HEADER = os.path.join(ROOT, "include", "speech_recog.h")
+HEADERS = (os.path.join(ROOT, "include", "speech_recog.h"), os.path.join(ROOT, "include", "sr_long.h"))
 
 R = 3                                    # repetitions of every job in the concurrent run
 TIMING_CAP = 512                         # timing records per handle: more than any job launches per repetition
@@ -520,6 +520,65 @@ class StreamGroup(Job):
         return _event_oracle(self.w, self.w.pcm(self.S, self.L, 0xC9000000 + v, 3), self.w.bank8, 8, out, (0, 18, 19, 36))
 
 
+class LongForm(Job):
+    """sr_vad_long_batch and sr_recognise_long_batch on host PCM with ragged lens (poison past them), then
+    sr_recognise_long_batch_dev on the same recordings on a torch stream of the job's own; device outputs prefilled"""
+    name = "long_form"
+    calls = ("sr_vad_long_batch", "sr_recognise_long_batch", "sr_recognise_long_batch_dev")
+    B, U, MS = 6, 150001, 16
+
+    def open(self):
+        import torch
+        import oracle_long as ol
+        self.torch, self.ol = torch, ol
+        self.h = self.handle()
+        self.h.set_bank(self.w.bank40, 40, 4096)
+        self.st = torch.cuda.Stream(torch.device("cuda:0"))
+        self.h.set_stream(self.st.cuda_stream)
+        self.inputs = []
+        for v in range(2):
+            pcm = ol.synth_long(self.B, self.U, 0xCC000000 + v)
+            lens = np.array([self.U, 161, 90000 + v, 2399, 120001, self.U - 80 * v], np.uint32)
+            for b, n in enumerate(lens):
+                pcm[b, n:] = np.where(np.arange(self.U - n) % 2, 4095, 0)
+            self.inputs.append((pcm, lens))
+        with torch.cuda.stream(self.st):
+            self.dev = [(torch.from_numpy(p.view(np.int16)).to("cuda:0"), torch.from_numpy(n.view(np.int32)).to("cuda:0"))
+                        for p, n in self.inputs]
+            self.out = {k: torch.empty(self.B * n, dtype=torch.uint8, device="cuda:0")
+                        for k, n in (("atap", 12), ("n_segs", 4), ("segs", 28 * self.MS))}
+        self.st.synchronize()
+
+    def run(self, v):
+        pcm, lens = self.inputs[v]
+        vad = self.h.vad_long_batch(pcm, self.MS, 2400, lens)
+        rec = self.h.recognise_long_batch(pcm, self.MS, 2400, lens)
+        d_pcm, d_lens = self.dev[v]
+        with self.torch.cuda.stream(self.st):
+            for k, t in self.out.items():
+                t.fill_(0 if k == "atap" else 0x5A)             # atap is in / out: rows noise_atap skips keep zeros
+            self.h.recognise_long_batch_dev(d_pcm.data_ptr(), self.U, self.B, d_lens.data_ptr(), 2400, self.MS,
+                                            *(self.out[k].data_ptr() for k in ("atap", "n_segs", "segs")))
+            self.h.sync()
+            o = {k: t.cpu().numpy() for k, t in self.out.items()}
+        return {"vad_atap": vad["atap"], "vad_n_segs": vad["n_segs"], "seg_off": vad["seg_off"], "atap": rec["atap"],
+                "n_segs": rec["n_segs"], "segs": rec["segs"], "dev_atap": o["atap"].view(sr_b200.ATAP_DTYPE),
+                "dev_n_segs": o["n_segs"].view(np.uint32), "dev_segs": o["segs"].view(self.ol.LONG_SEG_DTYPE).reshape(self.B, self.MS)}
+
+    def oracle(self, v, out):
+        pcm, lens = self.inputs[v]
+        ol = self.ol
+        want = ol.recognise_long(ol.long_oracle(), self.w.po, pcm, 2400, self.w.bank40, 40, 4096, self.MS, lens)
+        k = np.arange(self.MS)[None, :] < np.minimum(want["n_segs"], self.MS)[:, None]
+        got = {"vad_atap": out["vad_atap"], "vad_n_segs": out["vad_n_segs"], "seg_off": out["seg_off"][k],
+               "atap": out["atap"], "n_segs": out["n_segs"], "segs": out["segs"][k], "dev_atap": out["dev_atap"],
+               "dev_n_segs": out["dev_n_segs"], "dev_segs": out["dev_segs"][k]}
+        seg_off = np.stack([want["segs"]["start"], want["segs"]["end"]], -1)[k]
+        return diff_outputs(got, {"vad_atap": want["atap"], "vad_n_segs": want["n_segs"], "seg_off": seg_off, "atap": want["atap"],
+                                  "n_segs": want["n_segs"], "segs": want["segs"][k], "dev_atap": want["atap"],
+                                  "dev_n_segs": want["n_segs"], "dev_segs": want["segs"][k]})
+
+
 class _SharedBank:
     """one read-only device copy of the 200-slot bank that both bank_dev jobs borrow"""
     t = None
@@ -583,10 +642,10 @@ class BankDevDtw(Job):
 
 
 JOBS = (RecognisePacked, RecogniseDevBand, DtwDynamic, GeomB, EnrolAverageAlign, LongConnected, Grammar, StreamRagged,
-        StreamGroup, BankDevRecognise, BankDevDtw)
+        StreamGroup, BankDevRecognise, BankDevDtw, LongForm)
 RECREATED = "dtw_dynamic"                # the job whose thread destroys its handle and makes a new one halfway through
 
-# sr_* entry points of include/speech_recog.h that no job runs, each with the reason
+# sr_* entry points of include/speech_recog.h and include/sr_long.h that no job runs, each with the reason
 EXCLUDED = {
     "sr_comm_unique_id": "NCCL: needs two ranks, one per GPU",
     "sr_comm_create": "NCCL: needs two ranks, one per GPU",
@@ -608,6 +667,7 @@ EXCLUDED = {
     "sr_vad_batch_dev": "device-pointer form of the recognise front end; recognise_dev_band runs the same kernel",
     "sr_mfcc_batch_dev": "device-pointer form of the recognise front end; recognise_dev_band runs the same kernel",
     "sr_dtw_batch_dev": "device-pointer form of sr_dtw_batch, which dtw_dynamic and bank_dev_dtw run",
+    "sr_vad_long_batch_dev": "its three launches are the first of sr_recognise_long_batch_dev, which long_form runs",
     "sr_get_mdl_batch": "test-hook kernel of the unused get_mdl; stateless, no workspace of its own",
     "sr_connected_grammar_batch": "kernel-level form of sr_recognise_connected_grammar_batch, which connected_grammar runs",
     "sr_fft_mag_batch": "stateless test-hook kernel; the drop-in fft() runs it from 8 threads",
@@ -635,15 +695,18 @@ OTHER_CALLS = ("sr_create", "sr_destroy", "sr_use_own_stream", "sr_host_alloc_de
 
 
 def header_entry_points():
-    src = open(HEADER).read()
-    src = re.sub(r"/\*.*?\*/", " ", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(sr_\w+)\s*\(", src)))
+    names = set()
+    for hdr in HEADERS:
+        src = re.sub(r"/\*.*?\*/", " ", open(hdr).read(), flags=re.S)
+        names |= set(re.findall(r"\b(sr_\w+)\s*\(", src))
+    return sorted(names)
 
 
 def test_every_entry_point_is_in_the_job_table_or_excluded():
-    """a new sr_* entry point of the header cannot skip the concurrency check without an entry here"""
+    """a new sr_* entry point of the headers cannot skip the concurrency check without an entry here"""
     names = header_entry_points()
     assert len(names) > 60 and "sr_recognise_batch" in names and "sr_connected_grammar_batch" in names, names
+    assert "sr_vad_long_batch_dev" in names, names
     covered = {c for j in JOBS for c in j.calls} | set(OTHER_CALLS)
     assert not (covered & set(EXCLUDED)), covered & set(EXCLUDED)
     missing = [n for n in names if n not in covered and n not in EXCLUDED]

@@ -6,10 +6,12 @@ a call may read. Every test requires (a) results equal to the oracle (or the pla
 
 Write sets (include/speech_recog.h): ftr -- frm_num and rows < frm_num of each struct, host calls included (MFCC.C
 never writes save_sign); seg_off [B][3][2]; atap [B], only when n_len % 240 == 0; score [B][n_slot]; best_idx,
-best_dis, cmd, status [B]; get_mdl -- frm_num and rows < frm_num of accepted pairs, rejected pairs untouched.
+best_dis, cmd, status [B]; get_mdl -- frm_num and rows < frm_num of accepted pairs, rejected pairs untouched; the
+long-form calls (include/sr_long.h) -- n_segs [B], atap [B] only when n_len % 240 == 0 and n_len <= lens[b], segment
+slots and records k < min(n_segs[b], max_segs).
 Read sets: MFCC samples [start - 1, end), [start, end) when start == 0; noise_atap / VAD samples < n_len / buf_len;
 features rows < frm_num (the greedy walk: rows < max(frm_num + 1, 2)); banks the v_ftr_tag of the slots a scan walks;
-stream chunks lens[s] / chunk_len samples per row, up to max_samples per stream.
+stream chunks lens[s] / chunk_len samples per row, up to max_samples per stream; long-form recordings lens[b] samples.
 
 Guards and poison lie inside the allocation they surround: no access made here leaves an allocation."""
 import ctypes as C
@@ -444,6 +446,71 @@ def test_recognise_dev_writes_and_reads(bank):
         pd.unchanged("pcm")
     bd.unchanged("bank")
     h.close()
+
+
+# ---- the long-form calls (include/sr_long.h) -----------------------------------------------------------------------------
+def _long_slots(n_segs, max_segs, nbytes):
+    """[B * max_segs * nbytes] mask of the slots a long-form call writes: k < min(n_segs[b], max_segs)"""
+    k = np.arange(max_segs)[None, :] < np.minimum(n_segs, max_segs)[:, None]
+    return np.repeat(k.reshape(-1), nbytes)
+
+
+def test_long_dev_writes_and_reads(bank):
+    """sr_vad_long_batch_dev and sr_recognise_long_batch_dev into outputs 4 bytes past a 16-byte boundary between
+    sentinels, on a handle whose workspaces an earlier, larger call left full (more recordings, more segments, another U):
+    atap is written only for rows with n_len % 240 == 0 and n_len <= lens[b]; segment slots and records only below
+    min(n_segs, max_segs); lens[b] > U reads as U; loud band-crossing poison past lens[b] and after the last row changes
+    nothing. The host calls on the same handle equal those of a fresh handle and the oracle."""
+    import oracle_long as ol
+    lo, port = ol.long_oracle(), ob.port()
+    B, U = 8, 30011
+    lens = np.array([2399, 2400, 2401, 0, U, U + 1, 0xFFFFFFFF, 20000], np.uint32)   # n_len - 1, n_len, n_len + 1, 0, >= U
+    eff = np.minimum(lens, U)
+    pcm = ol.synth_long(B, U, 0x1A5)
+    for b in range(B):
+        pcm[b, eff[b]:] = np.where(np.arange(U - eff[b]) % 2, 4095, 0)
+    atap0 = np.zeros(B, ob.ATAP_DTYPE)
+    atap0["mid_val"], atap0["n_thl"], atap0["z_thl"], atap0["s_thl"] = 2000 + np.arange(B), 40, 2, 3000
+    h = _handle(bank)
+    stale = ol.synth_long(12, 50000, 0x1A6)
+    assert h.recognise_long_batch(stale, 64, 2400)["n_segs"].sum() > 40
+    for n_len, ms, phase in ((2400, 3, 0), (2400, 64, 2), (2401, 64, 0), (2400, 0, 2)):
+        what = "n_len %d max_segs %d phase %d" % (n_len, ms, phase)
+        want = ol.recognise_long(lo, port, pcm, n_len, bank, T, 4096, ms, eff, atap=atap0)
+        want_n, want_seg = lo.vad_long(pcm, want["atap"], ms, eff)
+        assert want["n_segs"].tolist() == want_n.tolist()
+        if n_len == 2400:
+            assert [want["atap"][b].tobytes() == atap0[b].tobytes() for b in range(4)] == [True, False, False, True]
+        pd, ld = _pcm_dev(pcm, phase, poison=[4095, 0]), Dev(lens.nbytes, data=lens)
+        ad, nd, sd = Dev(atap0.nbytes, data=atap0), Dev(B * 4), Dev(B * ms * 8)
+        h.vad_long_batch_dev(pd.ptr, U, B, ld.ptr, n_len, ms, ad.ptr, nd.ptr, sd.ptr if ms else None)
+        h.sync()
+        ad.check(want["atap"], what=what + " vad atap")
+        nd.check(want_n, what=what + " n_segs")
+        sd.check(want_seg, _long_slots(want_n, ms, 8), what + " seg_off")
+        ad, nd, rd = Dev(atap0.nbytes, data=atap0), Dev(B * 4), Dev(B * ms * 28)
+        h.recognise_long_batch_dev(pd.ptr, U, B, ld.ptr, n_len, ms, ad.ptr, nd.ptr, rd.ptr if ms else None)
+        h.sync()
+        ad.check(want["atap"], what=what + " recognise atap")
+        nd.check(want_n, what=what + " recognise n_segs")
+        rd.check(want["segs"], _long_slots(want_n, ms, 28), what + " records")
+        pd.unchanged("pcm")
+        ld.unchanged("lens")
+        assert (ms == 64 or (want_n > ms).any()) and (want["segs"]["status"] == 0).sum() >= min(ms, 3)
+    # the host calls (lens <= U) after all of that, against a fresh handle and the oracle
+    fresh = _handle(bank)
+    try:
+        for hh in (h, fresh):
+            got = hh.recognise_long_batch(pcm, 5, 2400, eff, atap=atap0.copy())
+            want = ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 5, eff, atap=atap0)
+            for k in ("atap", "n_segs", "segs"):
+                assert got[k].tobytes() == want[k].tobytes(), k
+            v = hh.vad_long_batch(pcm, 5, 2400, eff, atap=atap0.copy())
+            assert v["n_segs"].tolist() == want["n_segs"].tolist()
+            assert (v["seg_off"][..., 0] == want["segs"]["start"]).all() and (v["seg_off"][..., 1] == want["segs"]["end"]).all()
+    finally:
+        fresh.close()
+        h.close()
 
 
 # ---- reads: poison outside the read set changes no result -----------------------------------------------------------
