@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 7; }
+int sr_abi_version(void) { return 8; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -180,7 +180,7 @@ int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
        TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
-       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12 };
+       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13 };
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
@@ -1296,6 +1296,191 @@ int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint3
         const sr_long_out od{d_atap ? d_atap + b0 : nullptr, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
         return sr_recognise_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, &od);
     });
+}
+
+}  // extern "C"
+
+// ---- one grammar decode per long recording (sr_long_grammar.h) --------------------------------------------------------
+constexpr size_t kLongGramRecBytes = 256u << 20;   // records per launch: sum of N * n_states * 12 B over its sequences
+
+// the long-recording grammar decoder (tag 13) over the sequences of seq [B][4] (first segment, segments, frames; the first
+// record row is filled in here) and the flat segment table at d_row / d_frm. Launches take consecutive sequences whose
+// records fit kLongGramRecBytes; a sequence whose records alone exceed it runs in a launch of its own, the record
+// workspace grown to fit it.
+static void run_long_grammar(HostCall &c, const s16 *d_feat, std::vector<u32> &seq, const u32 *d_row, const u32 *d_frm,
+                             const std::vector<u32> &copy, const sr_grammar *g, u32 penalty, u32 max_words, const ConnDev &d) {
+    sr_handle *h = c.h;
+    const u32 B = (u32)(seq.size() / 4), S = g->n_states;
+    std::vector<u32> cut{0};                             // launch boundaries
+    size_t rows = 0, rows_max = 0;
+    for (u32 b = 0; b < B; ++b) {
+        const size_t n = seq[4 * (size_t)b + 2];
+        if (rows && (rows + n) * S * 12 > kLongGramRecBytes) { cut.push_back(b); rows = 0; }
+        seq[4 * (size_t)b + 3] = (u32)rows;
+        rows += n;
+        rows_max = std::max(rows_max, rows);
+    }
+    cut.push_back(B);
+    static const u32 kNoCopy = 0;                         // as run_grammar: a grammar without copies stages one word
+    const u32 *ctab = copy.empty() ? &kNoCopy : copy.data();
+    u32 *d_copy = c.in(h->lgram[5], ctab, std::max<size_t>(copy.size(), 1) * 4);
+    u32 *d_seq = c.in(h->lgram[0], seq.data(), (size_t)B * 16);
+    u64 *recD = c.ws<u64>(h->lgram[2], std::max<size_t>(rows_max, 1) * S * 8);
+    u32 *recS = c.ws<u32>(h->lgram[3], std::max<size_t>(rows_max, 1) * S * 4);
+    const BankView &bk = h->bank;
+    for (size_t k = 0; k + 1 < cut.size(); ++k) {
+        const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
+        for (u32 q0 = 0; q0 < nb; q0 += kSeqChunk)
+            c.launch(TAG_LONG_GRAM, "launch_dtw_long_grammar", [&] {
+                return launch_dtw_long_grammar(d_feat, d_seq + 4 * (size_t)b0, q0, std::min(nb - q0, kSeqChunk), d_row, d_frm, bk.p,
+                                               bk.stride, d_copy, (u32)copy.size(), S, g->final_mask, penalty, max_words,
+                                               d.words ? d.words + (size_t)b0 * max_words : nullptr, d.nw ? d.nw + b0 : nullptr,
+                                               d.total ? d.total + b0 : nullptr, recD, recS, h->stream);
+            });
+    }
+}
+
+// the segment slots the end-to-end call gives the VAD per recording: a closed segment spans at least 8 + 11 = 19 VAD
+// frames (8 active ones open it, 11 inactive ones close it, and the next needs 8 new active ones) and an open one at least
+// 8, so a recording of U samples, with ceil((U - 160) / 80) frames, has at most frames / 19 + 1 segments
+static u32 long_seg_bound(u32 U) {
+    const u32 nfr = U > SR_FRAME_LEN ? (U - SR_FRAME_LEN + SR_FRAME_MOV - 1) / SR_FRAME_MOV : 0u;
+    return nfr / 19u + 2u;
+}
+
+extern "C" {
+
+// the kernel-level form: the flat segment table's rows, then the decoder (tag 13)
+int sr_connected_grammar_segs_batch(sr_handle *h, const int16_t *feat, const uint32_t *seq_seg, const uint32_t *seg_frm, uint32_t B,
+                                    const sr_grammar *g, uint32_t penalty, uint32_t max_words, sr_conn_word *words,
+                                    uint32_t *n_words, uint64_t *total) {
+    SR_REQUIRE(h, h && (B == 0 || (seq_seg && n_words)));
+    if (B == 0) return 0;
+    for (u32 b = 0; b < B; ++b) SR_REQUIRE(h, seq_seg[b] <= seq_seg[b + 1]);
+    const u32 n_seg = seq_seg[B];
+    SR_REQUIRE(h, n_seg == 0 || seg_frm);
+    std::vector<u32> row(n_seg);
+    uint64_t rows = 0;
+    for (u32 k = 0; k < n_seg; ++k) {
+        SR_REQUIRE(h, seg_frm[k] <= SR_CONN_FRM_MAX);
+        row[k] = (u32)rows;
+        rows += seg_frm[k];
+    }
+    SR_REQUIRE(h, rows < (1ull << 32) && (rows == 0 || feat));
+    std::vector<u32> seq((size_t)B * 4);
+    for (u32 b = 0; b < B; ++b) {
+        uint64_t N = 0;
+        for (u32 k = seq_seg[b]; k < seq_seg[b + 1]; ++k) N += seg_frm[k];
+        SR_REQUIRE(h, N <= SR_LONG_GRAM_FRM_MAX);
+        seq[4 * (size_t)b] = seq_seg[b];
+        seq[4 * (size_t)b + 1] = seq_seg[b + 1] - seq_seg[b];
+        seq[4 * (size_t)b + 2] = (u32)N;
+    }
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    HostCall c(h, "sr_connected_grammar_segs_batch");
+    const s16 *d_feat = c.in(h->conn[3], feat, (size_t)rows * 24, 24);
+    u32 *tab = c.ws<u32>(h->lgram[1], std::max<size_t>(n_seg, 1) * 8);   // seg_row [n_seg] | seg_frm [n_seg]
+    if (tab) {
+        c.h2d(tab, row.data(), (size_t)n_seg * 4);
+        c.h2d(tab + n_seg, seg_frm, (size_t)n_seg * 4);
+    }
+    const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
+    run_long_grammar(c, d_feat, seq, tab, tab + n_seg, copy, g, penalty, max_words, d);
+    return c.finish();
+}
+
+// Per group of recordings (long_groups): the long-form VAD into long_seg_bound(U) slots per recording (tags 11, 12), one
+// synchronisation for the plan, the feature pieces of every decodable segment (tag 1) and one decoder sequence per
+// recording over all its segments (tag 13). The per-segment records are written on the host from the plan.
+int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens,
+                                    uint32_t n_len, const sr_grammar *g, uint32_t penalty, uint32_t max_segs, uint32_t max_words,
+                                    const sr_long_gram_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    SR_REQUIRE(h, (B == 0 || U > 0) && long_args_ok(U, B, n_len, max_segs));
+    for (u32 b = 0; lens && b < B; ++b) SR_REQUIRE(h, lens[b] <= U);
+    if (B == 0) return 0;
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN, cap = long_seg_bound(U);
+    HostCall c(h, "sr_recognise_long_grammar_batch");
+    const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
+    atap_tag *d_atap;
+    if (o->atap) {                                      // in / out: untouched when noise_atap skips
+        d_atap = c.in(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
+        c.out(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
+    } else {
+        d_atap = c.ws<atap_tag>(h->lng[8], (size_t)B * sizeof(atap_tag));
+        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
+    }
+    u32 *d_n = c.ws<u32>(h->lng[9], (size_t)B * 4);
+    const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
+    struct SegRec { u32 b, k, st, en, F; u8 status; };    // the records of segments k < max_segs
+    std::vector<SegRec> recs;
+    std::vector<u32> n_all(B), segv;
+    std::vector<atap_tag> av;
+    const int rc = long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) -> int {
+        u32 *d_seg = c.ws<u32>(h->lgram[4], (size_t)nb * cap * 8);
+        if (c.rc) return 0;
+        if (const int r = vad_long_impl(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, cap, d_atap + b0, d_n + b0, d_seg))
+            return r;
+        segv.resize((size_t)nb * cap * 2);
+        av.resize(nb);
+        c.ck("copy back", cudaMemcpyAsync(n_all.data() + b0, d_n + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, h->stream));
+        c.ck("copy back", cudaMemcpyAsync(segv.data(), d_seg, segv.size() * 4, cudaMemcpyDeviceToHost, h->stream));
+        c.ck("copy back", cudaMemcpyAsync(av.data(), d_atap + b0, (size_t)nb * sizeof(atap_tag), cudaMemcpyDeviceToHost, h->stream));
+        c.ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
+        if (c.rc) return 0;
+        // the plan: recording q is sequence q; its segments are consecutive entries of the flat table, a decodable one with
+        // its frames (rows packed back to back in segment order), any other with 0 frames
+        std::vector<u32> seq((size_t)nb * 4), row, frm;
+        LongPieces pc;
+        u32 rows = 0;
+        for (u32 q = 0; q < nb; ++q) {
+            const u32 b = b0 + q, n = n_all[b];
+            if (n > cap) return fail(h, "a recording has more segments than long_seg_bound", cudaSuccess);
+            seq[4 * (size_t)q] = (u32)row.size();
+            seq[4 * (size_t)q + 1] = n;
+            u32 N = 0;
+            for (u32 k = 0; k < n; ++k) {
+                const u32 st = segv[((size_t)q * cap + k) * 2], en = segv[((size_t)q * cap + k) * 2 + 1];
+                const u32 F = long_frames(st, en, U, frame_len);
+                const bool ok = F >= 1 && F <= SR_CONN_FRM_MAX;   // long_frames is 0 for an open segment
+                row.push_back(rows);
+                frm.push_back(ok ? F : 0u);
+                if (ok) {
+                    pc.add(st, F, frame_len, q, av[q], rows);
+                    rows += F;
+                    N += F;
+                }
+                if (k < max_segs)
+                    recs.push_back({b, k, st, en, ok ? F : 0u, (u8)(en == SR_SEG_NULL ? SR_ST_VAD_FAIL : ok ? SR_ST_OK : SR_ST_MFCC_FAIL)});
+            }
+            seq[4 * (size_t)q + 2] = N;
+        }
+        const u32 ns = (u32)row.size();
+        s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(rows, 1) * 24);
+        run_pieces(c, dpcm, U, nb, pc, d_feat);
+        u32 *tab = c.ws<u32>(h->lgram[1], std::max<size_t>(ns, 1) * 8);   // seg_row [ns] | seg_frm [ns]
+        if (c.rc) return 0;
+        c.h2d(tab, row.data(), (size_t)ns * 4);
+        c.h2d(tab + ns, frm.data(), (size_t)ns * 4);
+        const ConnDev dq{d.words ? d.words + (size_t)b0 * max_words : nullptr, d.nw ? d.nw + b0 : nullptr,
+                         d.total ? d.total + b0 : nullptr};
+        run_long_grammar(c, d_feat, seq, tab, tab + ns, copy, g, penalty, max_words, dq);
+        return 0;
+    });
+    if (rc) return rc;
+    if (o->n_segs) memcpy(o->n_segs, n_all.data(), (size_t)B * 4);
+    for (const SegRec &r : recs) {
+        const size_t i = (size_t)r.b * max_segs + r.k;
+        if (o->seg_off) { o->seg_off[2 * i] = r.st; o->seg_off[2 * i + 1] = r.en; }
+        if (o->frm_num) o->frm_num[i] = r.F;
+        if (o->seg_status) o->seg_status[i] = r.status;
+    }
+    return 0;
 }
 
 // One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]

@@ -397,6 +397,212 @@ cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *s
                            total ? total + b0 : nullptr, rec);
 }
 
+// ---- K13: one grammar decode per long recording, across any number of segments (include/sr_long_grammar.h) -----------
+// dtw_long_grammar_kernel is dtw_grammar_kernel's recurrence with three changes.
+//  - Segments: the sequence owns segments k0 .. k0 + nk - 1 of a flat table (first feature row, frames <= 818; 0: nothing
+//    to decode). Each segment with frames is staged in turn into the CTA's plane buffer, every within-word cell reset to
+//    +inf, then decoded frame by frame; E, and with it the grammar state, carries across. A CTA restages its own buffer
+//    only after the cluster barrier of the last frame of the segment before, which every warp passes after its last read
+//    of that buffer; one CTA barrier then publishes the new planes.
+//  - Keys, for D < 2^53 (headroom below): cells keep D << 10 | (1023 - start) with start the frame within the SEGMENT (a
+//    word never crosses one, so the segment-relative order of starts is the sequence-relative one), +inf = 2^63. The end
+//    cell is exchanged as D << 7 | copy (smallest D, ties to the lowest copy, as K6g's ekey orders them), and the start of
+//    each copy's end cell, as a sequence-relative frame, goes to a second candidate array beside it.
+//  - Records: per (frame, state) E_s(i) as D << 7 | copy (8 B) and its word's start frame (4 B), in two arrays.
+// Headroom: a recording has at most F_max = (2^27 - 160) / 80 + 1 = 1 677 720 frames. A word of n frames has a path of at
+// most n + 118 cells of get_dis <= 65 536, and there are at most F_max words, each adding the penalty (< 2^32):
+// D < F_max * (119 * 65 536 + 2^32) < 2^52.7 < 2^53. So a cell key D << 10 stays below 2^63, and adding the row sums of one
+// warp scan (< 128 * 2^26) to +inf = 2^63 stays below 2^64; the end key D << 7 | copy fits 60 bits.
+constexpr int kLgSmem = kSeqBytes + kConnWarps * kSlotBytes + 2 * kConnCand * 8 + 2 * kConnCand * 4 + kConnCand;   // 52 792
+constexpr u64 kLgInf = 1ull << 63;
+
+// Frame li of segment-relative frames (its segment's first frame is sequence frame f0) of a warp whose copy's template has
+// M frames: dp_column, cell j = 0 entered from `enter`, then the end cell as D << 7 | idx to candidate idx, and its word's
+// sequence-relative start to start candidate idx, of every CTA of the cluster; one cluster barrier.
+__device__ __forceinline__ void lg_frame(cg::cluster_group &cl, u32 nc, const unsigned char *smem, u64 *cand, u32 *cstart,
+                                         u32 li, u32 f0, u32 M, u64 enter, const PRow (&b)[4], u64 (&D)[4], u32 idx) {
+    const int lane = threadIdx.x & 31, j0 = lane * 4;
+    u64 mine = kEkeyNone;
+    u32 mst = 0;
+    if (M) {
+        PRow a;
+        load_row(a, smem, kSeqNrm, (int)li);               // broadcast read
+        dp_column<u64, kLgInf>(D, lane, [&](int k, u64 up, u64 dg, u64 &d, u64 &A, bool &valid) {
+            const int j = j0 + k;
+            valid = j < (int)M;
+            d = (u64)pdist(a, b[k]) << 10;
+            A = umin64(up, j == 0 ? enter : dg);
+        }, [](int, u64, u64) {});
+        const u64 e = dp_end(D, ((int)M - 1) & 3, ((int)M - 1) >> 2);
+        if (e < kLgInf) {
+            mine = ((e >> 10) << 7) | (u64)idx;
+            mst = f0 + 1023u - (u32)(e & 1023u);
+        }
+    }
+    if ((u32)lane < nc) {
+        cl.map_shared_rank(cand, (unsigned)lane)[idx] = mine;
+        cl.map_shared_rank(cstart, (unsigned)lane)[idx] = mst;
+    }
+    cl.sync();
+}
+
+// argmin over the states of mask of E_s(f) (D only, ties to the lowest state); the records of frame f are at r
+__device__ __forceinline__ u32 lg_src(const u64 *r, u32 mask) {
+    u32 best = 0;
+    u64 bd = ~0ull;
+    for (u32 s = 0; mask; ++s, mask >>= 1)
+        if ((mask & 1u) && (__ldcg(r + s) >> 7) < bd) { bd = __ldcg(r + s) >> 7; best = s; }
+    return best;
+}
+
+__global__ void __launch_bounds__(kConnWarps * 32, 3)   // 80 registers: three CTAs per SM, as dtw_grammar_kernel
+dtw_long_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ seq /* [.][4] first segment, segments, frames, first record row */,
+                        const u32 *__restrict__ seg_row, const u32 *__restrict__ seg_frm, const unsigned char *__restrict__ bank,
+                        u32 slot_stride, const u32 *__restrict__ copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words,
+                        sr_conn_word *__restrict__ words /* or NULL */, u32 *__restrict__ n_words /* or NULL */,
+                        u64 *__restrict__ total /* or NULL */, u64 *recD, u32 *recS) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    cg::cluster_group cl = cg::this_cluster();
+    const u32 nc = cl.num_blocks(), rank = cl.block_rank();
+    const u32 s = blockIdx.x / nc;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    u64 *cand = reinterpret_cast<u64 *>(smem_raw + kSeqBytes + kConnWarps * kSlotBytes);   // [2][kConnCand] end keys
+    u32 *cstart = reinterpret_cast<u32 *>(cand + 2 * kConnCand);                            // [2][kConnCand] their starts
+    unsigned char *cst = reinterpret_cast<unsigned char *>(cstart + 2 * kConnCand);         // [kConnCand] state of each copy
+    const u32 k0 = seq[4 * s], nk = seq[4 * s + 1], N = seq[4 * s + 2], rec0 = seq[4 * s + 3];
+    if (N == 0) {                                          // the whole cluster leaves: no barrier, no remote store
+        if (rank == 0 && threadIdx.x == 0) {
+            if (n_words) n_words[s] = 0;
+            if (total) total[s] = (final_mask & 1u) ? 0ull : ~0ull;
+        }
+        return;
+    }
+    const u32 ncand = nc * kConnWarps;
+    const u32 c = rank * kConnWarps + warp;                // this warp's copy
+    u32 src = 0, M = 0;
+    const unsigned char *slot = bank;
+    for (u32 q = threadIdx.x; q < ncand; q += blockDim.x) cst[q] = q < C ? (unsigned char)((copy[q] >> 8) & 15u) : 0;
+    if (c < C) {
+        const u32 cw = copy[c];
+        src = cw >> 16;
+        slot = bank + (size_t)(cw & 255u) * slot_stride;
+        M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);   // the host only makes copies of members
+        if (M == kNoWalk) M = 0;
+    }
+    unsigned char *tslot = smem_raw + kSeqBytes + warp * kSlotBytes;
+    if (M) stage_planes(tslot, kNrm119, slot, (int)M, lane, 32);
+    cl.sync();                                             // staging done, and every CTA of the cluster runs
+    PRow b[4];
+    u64 D[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        if (M) load_row(b[k], tslot, kNrm119, lane * 4 + k < (int)M ? lane * 4 + k : 0);
+    const u64 pen = penalty;
+    u64 eb = (src & 1u) ? 0ull : ~0ull;                    // min over src of E_s(i - 1): E_0(-1) = 0
+    const u32 gw = rank * kConnWarps + warp;
+    u64 *R = recD + (size_t)rec0 * S;
+    u32 *RS = recS + (size_t)rec0 * S;
+    u32 gi = 0;                                            // sequence-relative frame
+    for (u32 k = k0; k < k0 + nk; ++k) {
+        const u32 F = seg_frm[k];
+        if (F == 0) continue;
+        stage_planes(smem_raw, kSeqNrm, reinterpret_cast<const unsigned char *>(feat + (size_t)seg_row[k] * 12) - 4, (int)F,
+                     threadIdx.x, blockDim.x);
+        __syncthreads();
+#pragma unroll
+        for (int q = 0; q < 4; ++q) D[q] = kLgInf;         // a segment's first frame: no word crosses the pause
+        const u32 f0 = gi;
+        for (u32 li = 0; li < F; ++li, ++gi) {
+            const u64 enter = eb == ~0ull ? kLgInf : (((eb + pen) << 10) | (u64)(1023u - li));
+            u64 *buf = cand + (gi & 1) * kConnCand;
+            u32 *sb = cstart + (gi & 1) * kConnCand;
+            lg_frame(cl, nc, smem_raw, buf, sb, li, f0, M, enter, b, D, c);
+            u64 best = kEkeyNone;                          // min over the copies of the states in src: the entry term
+            for (u32 q = lane; q < ncand; q += 32)
+                if ((src >> cst[q]) & 1u) best = umin64(best, buf[q]);
+#pragma unroll
+            for (int o = 16; o; o >>= 1) best = umin64(best, __shfl_xor_sync(0xFFFFFFFFu, best, o));
+            eb = best == kEkeyNone ? ~0ull : best >> 7;
+            for (u32 st = gw; st < S; st += ncand) {       // the records E_st(gi) this warp owns
+                u64 r = kEkeyNone;
+                for (u32 q = lane; q < ncand; q += 32)
+                    if (cst[q] == st) r = umin64(r, buf[q]);
+#pragma unroll
+                for (int o = 16; o; o >>= 1) r = umin64(r, __shfl_xor_sync(0xFFFFFFFFu, r, o));
+                if (lane == 0) {
+                    R[(size_t)gi * S + st] = r;
+                    RS[(size_t)gi * S + st] = r == kEkeyNone ? 0u : sb[r & 127u];
+                }
+            }
+        }
+    }
+    __threadfence();
+    cl.sync();                                             // every CTA's records are written
+    if (rank != 0 || threadIdx.x != 0) return;
+    // records are read from L2 (ld.global.cg), as in dtw_grammar_kernel. The final state: the smallest E_s(N-1) over
+    // final states, ties to the lowest state
+    u32 fs = S;
+    u64 fd = ~0ull;
+    for (u32 st = 0; st < S; ++st) {
+        const u64 r = __ldcg(R + (size_t)(N - 1) * S + st);
+        if (((final_mask >> st) & 1u) && r != kEkeyNone && (r >> 7) < fd) { fd = r >> 7; fs = st; }
+    }
+    if (fs == S) {                                         // no accepting path
+        if (n_words) n_words[s] = 0;
+        if (total) total[s] = ~0ull;
+        return;
+    }
+    // trace-back: the word ending at frame i in state st is [start, i + 1) of its copy, entered from the source state with
+    // the smallest E(start - 1) (state 0 at start 0); frames map to (segment, frame within it) through the segment table
+    u32 K = 0;
+    for (long long i = (long long)N - 1, st = fs; i >= 0;) {
+        const u64 r = __ldcg(R + (size_t)i * S + st);
+        const u32 b0 = __ldcg(RS + (size_t)i * S + st);
+        if (b0) st = lg_src(R + (size_t)(b0 - 1) * S, copy[r & 127u] >> 16);
+        i = (long long)b0 - 1;
+        ++K;
+    }
+    const u32 row0 = seg_row[k0];
+    u32 kk = k0 + nk - 1, k = K;
+    for (long long i = (long long)N - 1, st = fs; i >= 0;) {
+        const u64 r = __ldcg(R + (size_t)i * S + st);
+        const u32 b0 = __ldcg(RS + (size_t)i * S + st), cp = (u32)(r & 127u);
+        u64 prev = 0;
+        if (b0) {
+            st = lg_src(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
+            prev = __ldcg(R + (size_t)(b0 - 1) * S + st) >> 7;
+        }
+        --k;
+        if (words && k < max_words) {
+            while (seg_frm[kk] == 0 || seg_row[kk] - row0 > b0) --kk;
+            const u32 fb = seg_row[kk] - row0;
+            sr_conn_word w;
+            w.slot = copy[cp] & 255u; w.cmd = w.slot / SR_FTR_PER_COMM; w.segment = kk - k0;
+            w.start = b0 - fb; w.end = (u32)i + 1 - fb;
+            w.dis = (u32)((r >> 7) - prev - pen);
+            words[(size_t)s * max_words + k] = w;
+        }
+        i = (long long)b0 - 1;
+    }
+    if (n_words) n_words[s] = K;
+    if (total) total[s] = fd;
+}
+
+// sequences [b0, b0 + nb) (seq: [.][4] first segment, segments, frames, first record row; seg_row / seg_frm: the flat
+// segment table) against C <= SR_GRAM_COPY_MAX copies in one launch. recD / recS hold (last record row + 1) * S records;
+// the caller cuts its sequences to bound them.
+cudaError_t launch_dtw_long_grammar(const s16 *feat, const u32 *seq, u32 b0, u32 nb, const u32 *seg_row, const u32 *seg_frm,
+                                    const void *bank, u32 slot_stride, const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty,
+                                    u32 max_words, sr_conn_word *words, u32 *n_words, u64 *total, u64 *recD, u32 *recS,
+                                    cudaStream_t st) {
+    if (nb == 0) return cudaSuccess;
+    if (C > SR_GRAM_COPY_MAX || S == 0 || S > SR_GRAM_STATE_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
+    return launch_clusters(dtw_long_grammar_kernel, kLgSmem, nb, C, st, feat, seq + 4 * (size_t)b0, seg_row, seg_frm,
+                           static_cast<const unsigned char *>(bank), slot_stride, copy, C, S, final_mask, penalty, max_words,
+                           words ? words + (size_t)b0 * max_words : nullptr, n_words ? n_words + b0 : nullptr,
+                           total ? total + b0 : nullptr, recD, recS);
+}
+
 cudaError_t launch_conn_gather(const void *pf, const u32 *pdst, u32 P, s16 *feat, int num_sms, cudaStream_t st) {
     if (P == 0) return cudaSuccess;
     const u32 grid = P < (u32)num_sms * 16u ? P : (u32)num_sms * 16u;

@@ -13,7 +13,7 @@
 #include <thread>
 #include <vector>
 #include "sr_common.cuh"
-#include "../../include/sr_long.h"
+#include "../../include/sr_long_grammar.h"
 
 namespace srk {
 cudaError_t launch_vad(const u16 *pcm, u32 U, u32 B, u32 n_len, u32 buf_len, int do_atap, int do_vad, atap_tag *atap,
@@ -66,6 +66,13 @@ cudaError_t launch_conn_concat(const u32 *seq_of, const u32 *seq_off, const sr_c
 cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *seq, u32 b0, u32 nb, const void *bank, u32 slot_stride,
                                const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
                                u32 *n_words, u64 *total, u64 *rec, cudaStream_t st);
+// the long-recording grammar decoder over sequences [b0, b0 + nb) (seq: [B][4] first segment, segments, frames, first
+// record row) of a flat segment table (seg_row: first feature row, seg_frm: frames), records in recD / recS
+// (sr_dtw_connected.cu)
+cudaError_t launch_dtw_long_grammar(const s16 *feat, const u32 *seq, u32 b0, u32 nb, const u32 *seg_row, const u32 *seg_frm,
+                                    const void *bank, u32 slot_stride, const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty,
+                                    u32 max_words, sr_conn_word *words, u32 *n_words, u64 *total, u64 *recD, u32 *recS,
+                                    cudaStream_t st);
 cudaError_t launch_sqrt_check(u32 lo, u32 hi, unsigned long long *bad_dev, cudaStream_t st);
 cudaError_t launch_unpack12(const void *packed, u64 n_samples, u16 *out, cudaStream_t st);
 // the long-form VAD and its per-segment recognition (sr_vad_long.cu): noise_atap, the block summaries into info
@@ -203,6 +210,8 @@ struct sr_handle {
     DevBuf lng[12];                                    // long-form VAD and recognition (sr_long.h): block summaries, segments,
                                                        // counts, the flat segment table, its atap, status, keys, features, lens
                                                        // and the host calls' device outputs
+    DevBuf lgram[6];                                   // the long-recording grammar decoder (sr_long_grammar.h): sequence table,
+                                                       // segment rows and frames, both record arrays, VAD segments of a group
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };

@@ -97,6 +97,14 @@ class LongOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ("atap", "n_segs", "segs")]
 
 
+LONG_GRAM_FRM_MAX = 1677720    # SR_LONG_GRAM_FRM_MAX: frames of a 2^27-sample recording (include/sr_long_grammar.h)
+LONG_GRAM_FIELDS = ("atap", "n_segs", "seg_off", "frm_num", "seg_status", "n_words", "words", "total")
+
+
+class LongGramOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in LONG_GRAM_FIELDS]
+
+
 class StreamEvent(C.Structure):
     _fields_ = [(k, C.c_uint32) for k in ("stream", "segment", "start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")]
 
@@ -149,6 +157,8 @@ def lib():
         L.sr_vad_long_batch_dev.argtypes = [vp, vp, u32, u32, vp, u32, u32, vp, vp, vp]
         L.sr_recognise_long_batch.argtypes = [vp, vp, u32, u32, vp, u32, u32, C.POINTER(LongOut)]
         L.sr_recognise_long_batch_dev.argtypes = [vp, vp, u32, u32, vp, u32, u32, C.POINTER(LongOut)]
+        L.sr_connected_grammar_segs_batch.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp, vp, vp]
+        L.sr_recognise_long_grammar_batch.argtypes = [vp, vp, u32, u32, vp, u32, vp, u32, u32, u32, C.POINTER(LongGramOut)]
         L.sr_streams_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
         L.sr_streams_destroy.argtypes = [vp]
         L.sr_streams_reset.argtypes = [vp]
@@ -488,6 +498,44 @@ class Handle:
     def recognise_long_batch_dev(self, pcm_ptr, U, B, lens_ptr, n_len, max_segs, atap_ptr, n_segs_ptr, segs_ptr):
         out = LongOut(_p(atap_ptr), _p(n_segs_ptr), _p(segs_ptr))
         self._ck(lib().sr_recognise_long_batch_dev(self._h, _p(pcm_ptr), U, B, _p(lens_ptr), n_len, max_segs, C.byref(out)))
+
+    # -- one grammar decode per long recording (include/sr_long_grammar.h)
+    def connected_grammar_segs(self, feat, seq_seg, seg_frm, grammar_, penalty, max_words, words=None, want_total=True):
+        """the grammar decoder over a flat segment table (sr_connected_grammar_segs_batch): feat [rows, 12] i16 (the
+        segments' rows back to back), seq_seg [B+1], seg_frm [n_seg] -> (words [B, max_words] WORD_DTYPE, n_words [B],
+        total [B] u64 or None); records past n_words keep what `words` held (zeros when it is None)"""
+        feat = np.ascontiguousarray(feat, np.int16)
+        seq_seg = np.ascontiguousarray(seq_seg, np.uint32)
+        seg_frm = np.ascontiguousarray(seg_frm, np.uint32)
+        B = len(seq_seg) - 1
+        words = np.zeros((B, max_words), WORD_DTYPE) if words is None else words
+        n_words = np.zeros(B, np.uint32)
+        total = np.zeros(B, np.uint64) if want_total else None
+        g = grammar(grammar_)
+        self._ck(lib().sr_connected_grammar_segs_batch(self._h, _p(feat) if feat.size else None, _p(seq_seg),
+                                                       _p(seg_frm) if seg_frm.size else None, B,
+                                                       None if g is None else C.byref(g), penalty, max_words, _p(words),
+                                                       _p(n_words), _p(total)))
+        return words, n_words, total
+
+    def recognise_long_grammar(self, pcm, grammar_, penalty, max_segs, max_words, n_len=2400, lens=None,
+                               want=LONG_GRAM_FIELDS, out=None):
+        """long-form VAD, long features of every decodable segment and one grammar decode per recording
+        (sr_recognise_long_grammar_batch): a dict of the sr_long_gram_out fields named in `want` (or the arrays of `out`,
+        filled in place)"""
+        B, U = pcm.shape
+        if out is None:
+            shape = {"atap": (B, ATAP_DTYPE), "n_segs": (B, np.uint32), "seg_off": ((B, max_segs, 2), np.uint32),
+                     "frm_num": ((B, max_segs), np.uint32), "seg_status": ((B, max_segs), np.uint8),
+                     "n_words": (B, np.uint32), "words": ((B, max_words), WORD_DTYPE), "total": (B, np.uint64)}
+            out = {k: np.zeros(*shape[k]) for k in LONG_GRAM_FIELDS if k in want}
+        lens = None if lens is None else np.ascontiguousarray(lens, np.uint32)
+        o = LongGramOut(*[_p(out.get(k)) for k in LONG_GRAM_FIELDS])
+        g = grammar(grammar_)
+        self._ck(lib().sr_recognise_long_grammar_batch(self._h, _p(pcm), U, B, _p(lens), n_len,
+                                                       None if g is None else C.byref(g), penalty, max_segs, max_words,
+                                                       C.byref(o)))
+        return out
 
     def fft_mag(self, frames):
         n, length = frames.shape
