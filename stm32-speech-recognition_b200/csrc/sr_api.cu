@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 8; }
+int sr_abi_version(void) { return 9; }
 
 int sr_device_count(void) {
     int n = 0;

@@ -2,6 +2,7 @@
 // and sr_stream.cu. Nothing here is part of the C-ABI.
 #pragma once
 #include <chrono>
+#include <deque>
 #include <functional>
 #include <memory>
 #include <mutex>
@@ -319,3 +320,34 @@ struct DeviceGuard {
 
 
 #define D2H(h, dst, src, bytes) SR_CK(h, cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyDeviceToHost, (h)->stream))
+
+// ---- the part every streaming pool shares (sr_stream.cu): K4's fixed captures and K14's live streams ----------------
+// A push's step kernel appends the chunk and lists the segments it closed in ev / seg_ev / atap_ev / map_ev (n_ev of them,
+// at most cap); stream_core_recognise then runs get_mfcc on seg_ev (offsets inside PCM row map_ev of a [S][row_len]
+// buffer), the status, the handle's matcher and the packing of one sr_stream_event per segment, copies them back with the
+// push's one synchronisation and hands them out behind any queued ones.
+namespace srk {
+struct StreamEventDev {         // work list of the segments closed by the current push
+    u32 stream, segment, start, end;
+};
+}  // namespace srk
+
+struct StreamCore {
+    sr_handle *h = nullptr;
+    u32 S = 0, cap = 0, stage_stride = 0;
+    DevBuf stage, lens, ev, seg_ev, atap_ev, map_ev, n_ev, ftr, status, frm, out;
+    Pinned<unsigned char> out_host;                // [count u32, pad][records]
+    Pinned<u32> lens_host;                         // staging of a ragged push's lengths
+    std::deque<sr_stream_event> pending;           // events not yet handed to the caller (max_events too small)
+    static constexpr u32 kQuick = 4096;            // records fetched with the count in the first D2H copy
+};
+// the per-push buffers for S streams and cap events
+cudaError_t stream_core_alloc(StreamCore &c, sr_handle *h, u32 S, u32 cap);
+// a ragged push's lengths into lens_host (lens NULL: uniform_len for every stream); returns the longest
+u32 stream_core_lens(StreamCore &c, const uint32_t *lens, u32 uniform_len);
+// the chunk as the step kernel reads it (pinned host memory in place, else a staging copy), the lengths (ragged) and
+// the event counter zeroed, on the handle's stream
+int stream_core_stage(StreamCore &c, const uint16_t *chunk, u32 chunk_stride, u32 max_len, bool ragged, const u16 **chunk_dev,
+                      u32 *chunk_dev_stride);
+int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_event *events, u32 max_events, u32 *n_events);
+void stream_core_fetch(StreamCore &c, sr_stream_event *events, u32 max_events, u32 *n_events);

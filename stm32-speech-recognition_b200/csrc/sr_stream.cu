@@ -32,10 +32,6 @@ struct StreamState {            // one per stream, device resident
     u32 aw[32];                 // activity bitmap, frame f = bit f&31 of word f>>5 (<= 1024 frames: U <= 65535)
 };
 
-struct StreamEventDev {         // work list of the segments closed by the current push
-    u32 stream, segment, start, end;
-};
-
 __global__ void stream_reset_kernel(StreamState *st, u32 S) {
     const u32 s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
@@ -192,14 +188,118 @@ __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, 
 
 }  // namespace srk
 
-struct sr_stream_pool {
-    sr_handle *h = nullptr;
-    u32 S = 0, L = 0, n_len = 0, cap = 0, info_stride = 0, stage_stride = 0;
-    DevBuf pcm, state, info, stage, lens, ev, seg_ev, atap_ev, map_ev, n_ev, ftr, status, frm, out;
-    Pinned<unsigned char> out_host;                // [count u32, pad][records]
-    Pinned<u32> lens_host;                         // staging of a ragged push's lengths
-    std::deque<sr_stream_event> pending;           // events not yet handed to the caller (max_events too small)
-    static constexpr u32 kQuick = 4096;            // records fetched with the count in the first D2H copy
+// ---- what every streaming pool shares: the chunk read, recognition of the closed segments, the event queue ----------
+cudaError_t stream_core_alloc(StreamCore &c, sr_handle *h, u32 S, u32 cap) {
+    c.h = h; c.S = S; c.cap = cap;
+    cudaError_t e = cudaSuccess;
+    auto need = [&](DevBuf &b, size_t bytes) { if (e == cudaSuccess) e = ensure(b, bytes); };
+    need(c.lens, (size_t)S * 4);
+    need(c.ev, (size_t)cap * sizeof(StreamEventDev));
+    need(c.seg_ev, (size_t)cap * 8);
+    need(c.atap_ev, (size_t)cap * sizeof(atap_tag));
+    need(c.map_ev, (size_t)cap * 4);
+    need(c.n_ev, 16);
+    need(c.ftr, (size_t)cap * kFtrBytes);
+    need(c.status, cap);
+    need(c.frm, (size_t)cap * 4);
+    need(c.out, 16 + (size_t)cap * sizeof(sr_stream_event));
+    if (e == cudaSuccess) e = c.out_host.alloc(16 + (size_t)cap * sizeof(sr_stream_event));
+    if (e == cudaSuccess) e = c.lens_host.alloc((size_t)S * 4);
+    return e;
+}
+
+u32 stream_core_lens(StreamCore &c, const uint32_t *lens, u32 uniform_len) {
+    if (!lens) return uniform_len;
+    u32 max_len = 0;
+    for (u32 s = 0; s < c.S; ++s) { c.lens_host.p[s] = lens[s]; if (lens[s] > max_len) max_len = lens[s]; }
+    return max_len;
+}
+
+int stream_core_stage(StreamCore &c, const uint16_t *chunk, u32 chunk_stride, u32 max_len, bool ragged, const u16 **chunk_dev_out,
+                      u32 *chunk_dev_stride_out) {
+    sr_handle *h = c.h;
+    if (h->comm) { const int rc = sr_comm_wait(h); if (rc) return rc; }   // a pending gather may still read the handle's key buffer
+    const u16 *chunk_dev = static_cast<const u16 *>(c.stage.p);
+    u32 chunk_dev_stride = c.stage_stride;
+    if (max_len) {
+        // Pinned (cudaHostAlloc / cudaHostRegister / sr_host_alloc*) chunks are read by the kernel straight from host memory:
+        // one coalesced 16-byte-per-lane read per stream row, no copy-engine descriptor per row (a strided [S][chunk] slice
+        // of a larger capture array is 8192 rows of a few hundred bytes: the 2-D copy alone took ~2 ms). Pageable memory
+        // goes through a device staging buffer.
+        cudaPointerAttributes attr;
+        bool zero_copy = false;
+        if (cudaPointerGetAttributes(&attr, chunk) == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer) {
+            chunk_dev = static_cast<const u16 *>(attr.devicePointer);
+            chunk_dev_stride = chunk_stride;
+            zero_copy = true;
+        } else cudaGetLastError();
+        if (!zero_copy) {
+            const u32 sstride = (max_len + 7u) & ~7u;                    // staging rows start 16-byte aligned
+            SR_CK(h, ensure(c.stage, (size_t)c.S * sstride * 2 + 64));
+            c.stage_stride = sstride;
+            chunk_dev = static_cast<const u16 *>(c.stage.p); chunk_dev_stride = sstride;
+            SR_CK(h, cudaMemcpy2DAsync(c.stage.p, (size_t)sstride * 2, chunk, (size_t)chunk_stride * 2, (size_t)max_len * 2, c.S,
+                                       cudaMemcpyHostToDevice, h->stream));
+        }
+        if (ragged) SR_CK(h, cudaMemcpyAsync(c.lens.p, c.lens_host.p, (size_t)c.S * 4, cudaMemcpyHostToDevice, h->stream));
+    }
+    SR_CK(h, cudaMemsetAsync(c.n_ev.p, 0, 4, h->stream));
+    *chunk_dev_out = chunk_dev;
+    *chunk_dev_stride_out = chunk_dev_stride;
+    return 0;
+}
+
+int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_event *events, u32 max_events, u32 *n_events) {
+    sr_handle *h = c.h;
+    u32 *n_ev = static_cast<u32 *>(c.n_ev.p);
+    // recognise the closed segments; every kernel reads the number of events from device memory (upper bound: cap)
+    SR_CK(h, launch_mfcc_h(h, pcm, row_len, c.cap, static_cast<const u32 *>(c.seg_ev.p), 2,
+                           static_cast<const atap_tag *>(c.atap_ev.p), c.ftr.p, static_cast<const u32 *>(c.map_ev.p), c.S, n_ev));
+    SR_CK(h, ensure(h->best, (size_t)c.cap * 8));
+    u64 *best = static_cast<u64 *>(h->best.p);
+    const u32 gb = (c.cap + 255) / 256;
+    stream_status_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const unsigned char *>(c.ftr.p), n_ev, c.cap,
+                                                   static_cast<u8 *>(c.status.p), static_cast<u32 *>(c.frm.p), best);
+    SR_CK(h, cudaGetLastError());
+    if (h->bank.n)                                                    // the handle's matcher, read at every push
+        SR_CK(h, launch_scan(h, h->bank, c.ftr.p, c.cap, SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, nullptr, best,
+                             static_cast<const u8 *>(c.status.p), n_ev));
+    u32 *out_count = static_cast<u32 *>(c.out.p);
+    sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(c.out.p) + 16);
+    stream_finish_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap,
+                                                   static_cast<const u8 *>(c.status.p), static_cast<const u32 *>(c.frm.p),
+                                                   best, out_rec, out_count);
+    SR_CK(h, cudaGetLastError());
+    h->launches += 4 + (h->bank.n ? 1 : 0);
+    const u32 quick = c.cap < StreamCore::kQuick ? c.cap : StreamCore::kQuick;
+    D2H(h, c.out_host.p, c.out.p, 16 + (size_t)quick * sizeof(sr_stream_event));
+    SR_CK(h, cudaStreamSynchronize(h->stream));                       // the one synchronisation of a push
+    const u32 ne = *reinterpret_cast<const u32 *>(c.out_host.p);
+    if (ne > quick) {                                                 // rare: a burst of closings larger than the quick window
+        D2H(h, c.out_host.p + 16 + (size_t)quick * sizeof(sr_stream_event), static_cast<unsigned char *>(c.out.p) + 16 + (size_t)quick * sizeof(sr_stream_event),
+            (size_t)(ne - quick) * sizeof(sr_stream_event));
+        SR_CK(h, cudaStreamSynchronize(h->stream));
+    }
+    const sr_stream_event *rec = reinterpret_cast<const sr_stream_event *>(c.out_host.p + 16);
+    u32 k = 0;
+    // older queued events first, then this push's; whatever does not fit stays queued for the pool's fetch call
+    while (k < max_events && events && !c.pending.empty()) { events[k++] = c.pending.front(); c.pending.pop_front(); }
+    u32 i = 0;
+    if (c.pending.empty()) for (; i < ne && k < max_events && events; ++i) events[k++] = rec[i];
+    for (; i < ne; ++i) c.pending.push_back(rec[i]);
+    *n_events = k;
+    return 0;
+}
+
+void stream_core_fetch(StreamCore &c, sr_stream_event *events, u32 max_events, u32 *n_events) {
+    u32 k = 0;
+    while (k < max_events && events && !c.pending.empty()) { events[k++] = c.pending.front(); c.pending.pop_front(); }
+    *n_events = k;
+}
+
+struct sr_stream_pool : StreamCore {
+    u32 L = 0, n_len = 0, info_stride = 0;
+    DevBuf pcm, state, info;
 };
 
 static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t chunk_stride, uint32_t uniform_len,
@@ -232,26 +332,13 @@ int sr_streams_create(sr_handle *h, uint32_t n_streams, uint32_t max_samples, ui
     DeviceGuard g(h->device);
     sr_stream_pool *p = new (std::nothrow) sr_stream_pool;
     SR_REQUIRE(h, p != nullptr);
-    p->h = h; p->S = n_streams; p->L = max_samples; p->n_len = n_len; p->cap = 3 * n_streams;
+    p->L = max_samples; p->n_len = n_len;
     p->info_stride = 2 * (max_samples / 80 + 2);
-    const size_t cap = p->cap;
-    cudaError_t e = cudaSuccess;
+    cudaError_t e = stream_core_alloc(*p, h, n_streams, 3 * n_streams);
     auto need = [&](DevBuf &b, size_t bytes) { if (e == cudaSuccess) e = ensure(b, bytes); };
     need(p->pcm, (size_t)n_streams * max_samples * 2 + 64);
     need(p->state, (size_t)n_streams * sizeof(StreamState));
     need(p->info, (size_t)n_streams * p->info_stride * 4);
-    need(p->lens, (size_t)n_streams * 4);
-    need(p->ev, cap * sizeof(StreamEventDev));
-    need(p->seg_ev, cap * 8);
-    need(p->atap_ev, cap * sizeof(atap_tag));
-    need(p->map_ev, cap * 4);
-    need(p->n_ev, 16);
-    need(p->ftr, cap * kFtrBytes);
-    need(p->status, cap);
-    need(p->frm, cap * 4);
-    need(p->out, 16 + cap * sizeof(sr_stream_event));
-    if (e == cudaSuccess) e = p->out_host.alloc(16 + cap * sizeof(sr_stream_event));
-    if (e == cudaSuccess) e = p->lens_host.alloc((size_t)n_streams * 4);
     if (e != cudaSuccess) { sr_streams_destroy(p); return fail(h, "sr_streams_create: allocation", e); }
     *out = p;
     return sr_streams_reset(p);
@@ -274,9 +361,7 @@ int sr_streams_push_ragged(sr_stream_pool *p, const uint16_t *chunk, uint32_t ch
 // events queued by earlier pushes whose caller buffer was too small (nothing is ever dropped)
 int sr_streams_fetch(sr_stream_pool *p, sr_stream_event *events, uint32_t max_events, uint32_t *n_events) {
     SR_REQUIRE(nullptr, p && n_events);
-    u32 k = 0;
-    while (k < max_events && events && !p->pending.empty()) { events[k++] = p->pending.front(); p->pending.pop_front(); }
-    *n_events = k;
+    stream_core_fetch(*p, events, max_events, n_events);
     return 0;
 }
 uint32_t sr_streams_pending(const sr_stream_pool *p) { return p ? (uint32_t)p->pending.size() : 0; }
@@ -305,40 +390,13 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     SR_REQUIRE(nullptr, p && n_events);
     sr_handle *h = p->h;
     *n_events = 0;
-    u32 max_len = uniform_len;
-    if (lens) {
-        max_len = 0;
-        for (u32 s = 0; s < p->S; ++s) { p->lens_host.p[s] = lens[s]; if (lens[s] > max_len) max_len = lens[s]; }
-    }
+    const u32 max_len = stream_core_lens(*p, lens, uniform_len);
     SR_REQUIRE(h, max_len == 0 || chunk != nullptr);
     SR_REQUIRE(h, max_len <= p->L && chunk_stride >= max_len);
     DeviceGuard g(h->device);
-    if (h->comm) { const int rc = sr_comm_wait(h); if (rc) return rc; }   // a pending gather may still read the handle's key buffer
-    const u16 *chunk_dev = static_cast<const u16 *>(p->stage.p);
-    u32 chunk_dev_stride = p->stage_stride;
-    if (max_len) {
-        // Pinned (cudaHostAlloc / cudaHostRegister / sr_host_alloc*) chunks are read by the kernel straight from host memory:
-        // one coalesced 16-byte-per-lane read per stream row, no copy-engine descriptor per row (a strided [S][chunk] slice
-        // of a larger capture array is 8192 rows of a few hundred bytes: the 2-D copy alone took ~2 ms). Pageable memory
-        // goes through a device staging buffer.
-        cudaPointerAttributes attr;
-        bool zero_copy = false;
-        if (cudaPointerGetAttributes(&attr, chunk) == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer) {
-            chunk_dev = static_cast<const u16 *>(attr.devicePointer);
-            chunk_dev_stride = chunk_stride;
-            zero_copy = true;
-        } else cudaGetLastError();
-        if (!zero_copy) {
-            const u32 sstride = (max_len + 7u) & ~7u;                    // staging rows start 16-byte aligned
-            SR_CK(h, ensure(p->stage, (size_t)p->S * sstride * 2 + 64));
-            p->stage_stride = sstride;
-            chunk_dev = static_cast<const u16 *>(p->stage.p); chunk_dev_stride = sstride;
-            SR_CK(h, cudaMemcpy2DAsync(p->stage.p, (size_t)sstride * 2, chunk, (size_t)chunk_stride * 2, (size_t)max_len * 2, p->S,
-                                       cudaMemcpyHostToDevice, h->stream));
-        }
-        if (lens) SR_CK(h, cudaMemcpyAsync(p->lens.p, p->lens_host.p, (size_t)p->S * 4, cudaMemcpyHostToDevice, h->stream));
-    }
-    SR_CK(h, cudaMemsetAsync(p->n_ev.p, 0, 4, h->stream));
+    const u16 *chunk_dev;
+    u32 chunk_dev_stride;
+    if (const int rc = stream_core_stage(*p, chunk, chunk_stride, max_len, lens != nullptr, &chunk_dev, &chunk_dev_stride)) return rc;
     u32 *n_ev = static_cast<u32 *>(p->n_ev.p);
     stream_step_kernel<<<(p->S + kStreamWarps - 1) / kStreamWarps, kStreamWarps * 32, 0, h->stream>>>(
         static_cast<u16 *>(p->pcm.p), p->L, p->S, chunk_dev, chunk_dev_stride, max_len ? uniform_len : 0u,
@@ -346,43 +404,7 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
         static_cast<u32 *>(p->info.p), p->info_stride, static_cast<StreamEventDev *>(p->ev.p), static_cast<u32 *>(p->seg_ev.p),
         static_cast<atap_tag *>(p->atap_ev.p), static_cast<u32 *>(p->map_ev.p), n_ev, p->cap);
     SR_CK(h, cudaGetLastError());
-    // recognise the closed segments; every kernel reads the number of events from device memory (upper bound: cap)
-    SR_CK(h, launch_mfcc_h(h, static_cast<const u16 *>(p->pcm.p), p->L, p->cap, static_cast<const u32 *>(p->seg_ev.p), 2,
-                           static_cast<const atap_tag *>(p->atap_ev.p), p->ftr.p, static_cast<const u32 *>(p->map_ev.p), p->S, n_ev));
-    SR_CK(h, ensure(h->best, (size_t)p->cap * 8));
-    u64 *best = static_cast<u64 *>(h->best.p);
-    const u32 gb = (p->cap + 255) / 256;
-    stream_status_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const unsigned char *>(p->ftr.p), n_ev, p->cap,
-                                                   static_cast<u8 *>(p->status.p), static_cast<u32 *>(p->frm.p), best);
-    SR_CK(h, cudaGetLastError());
-    if (h->bank.n)                                                    // the handle's matcher, read at every push
-        SR_CK(h, launch_scan(h, h->bank, p->ftr.p, p->cap, SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, nullptr, best,
-                             static_cast<const u8 *>(p->status.p), n_ev));
-    u32 *out_count = static_cast<u32 *>(p->out.p);
-    sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(p->out.p) + 16);
-    stream_finish_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const StreamEventDev *>(p->ev.p), n_ev, p->cap,
-                                                   static_cast<const u8 *>(p->status.p), static_cast<const u32 *>(p->frm.p),
-                                                   best, out_rec, out_count);
-    SR_CK(h, cudaGetLastError());
-    h->launches += 4 + (h->bank.n ? 1 : 0);
-    const u32 quick = p->cap < sr_stream_pool::kQuick ? p->cap : sr_stream_pool::kQuick;
-    D2H(h, p->out_host.p, p->out.p, 16 + (size_t)quick * sizeof(sr_stream_event));
-    SR_CK(h, cudaStreamSynchronize(h->stream));                       // the one synchronisation of a push
-    const u32 ne = *reinterpret_cast<const u32 *>(p->out_host.p);
-    if (ne > quick) {                                                 // rare: a burst of closings larger than the quick window
-        D2H(h, p->out_host.p + 16 + (size_t)quick * sizeof(sr_stream_event), static_cast<unsigned char *>(p->out.p) + 16 + (size_t)quick * sizeof(sr_stream_event),
-            (size_t)(ne - quick) * sizeof(sr_stream_event));
-        SR_CK(h, cudaStreamSynchronize(h->stream));
-    }
-    const sr_stream_event *rec = reinterpret_cast<const sr_stream_event *>(p->out_host.p + 16);
-    u32 k = 0;
-    // older queued events first, then this push's; whatever does not fit stays queued for sr_streams_fetch
-    while (k < max_events && events && !p->pending.empty()) { events[k++] = p->pending.front(); p->pending.pop_front(); }
-    u32 i = 0;
-    if (p->pending.empty()) for (; i < ne && k < max_events && events; ++i) events[k++] = rec[i];
-    for (; i < ne; ++i) p->pending.push_back(rec[i]);
-    *n_events = k;
-    return 0;
+    return stream_core_recognise(*p, static_cast<const u16 *>(p->pcm.p), p->L, events, max_events, n_events);
 }
 
 // ---- streams sharded over several handles / GPUs (BASELINE configs[4] on 8 GPUs) ---------------------------------

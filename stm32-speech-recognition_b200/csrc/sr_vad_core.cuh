@@ -283,12 +283,16 @@ __device__ __forceinline__ u32 bm_shr(u32 x, int s, int lane) {
 // block_flags). `cin` is the class of the last out-of-band sample in the blocks before k0 (0 at the start of a capture)
 // and is advanced to cover the blocks of the frames handled here (lanes with k >= kend contribute nothing), so passes
 // may start at any frame and stop anywhere: the streaming kernel resumes where the previous push ended.
+// Frames are absolute (k == 0 is the capture's first frame); info holds the summaries of blocks koff, koff + 1, ... (0: all
+// of them from block 0), so a caller may keep only the blocks of the frames at hand.
 // Returns the ballot of "frame active" (VAD.C:164) over the 32 lanes.
-__device__ __forceinline__ u32 frames_pass(const u32 *info, u32 k0, u32 kend, int lane, const atap_tag &at, u32 &cin) {
+__device__ __forceinline__ u32 frames_pass(const u32 *info, u32 k0, u32 kend, int lane, const atap_tag &at, u32 &cin,
+                                           u32 koff = 0) {
     const u32 k = k0 + (u32)lane;
     const bool ok = k < kend;
     u32 bs0 = 0, f0 = 0, bs1 = 0, f1 = 0;
-    if (ok) { bs0 = info[2 * k]; f0 = info[2 * k + 1]; bs1 = info[2 * k + 2]; f1 = info[2 * k + 3]; }
+    const u32 j = k - koff;
+    if (ok) { bs0 = info[2 * j]; f0 = info[2 * j + 1]; bs1 = info[2 * j + 2]; f1 = info[2 * j + 3]; }
     const u32 zc0 = f0 & 127u, lc0 = (f0 >> 7) & 3u, lcA0 = (f0 >> 9) & 3u, p00 = (f0 >> 11) & 1u;
     const u32 zc1 = f1 & 127u, lc1 = (f1 >> 7) & 3u;
     const u32 fc0 = lc0 ? ((zc0 & 1u) ? 3u - lc0 : lc0) : 0u;      // first class from last class + parity
@@ -338,6 +342,78 @@ __device__ __forceinline__ void fsm_segments(u32 aw, u32 nfr, int lane, u32 (&se
         if (q < 0) break;                                          // never closes: end stays NULL
         seg[2 * sgi + 1] = 80u * (u32)q + 80u;                     // VAD.C:201: i - 11*80 + 160 with i = 80*(q+10)
         cur = q + 11;
+    }
+}
+
+// ---- the long-form endpoint FSM, carried across windows (K12 recordings, K14 live streams) ------------------------
+// position of the last set bit in a bitmap held one 32-bit word per lane; -1 if none
+__device__ __forceinline__ int find_last(u32 word) {
+    const u32 bal = __ballot_sync(0xFFFFFFFFu, word != 0);
+    if (!bal) return -1;
+    const int L = 31 - __clz(bal);
+    const u32 mw = __shfl_sync(0xFFFFFFFFu, word, L);
+    return 32 * L + 31 - __clz(mw);
+}
+
+// The FSM's state between windows: open (a segment has opened and not closed), closed = the n segments before it, and
+// run = the length of the run at the end of the frames seen so far that the FSM is counting (active frames while
+// closed, inactive ones while open), always shorter than the 8 / 11 that would complete it.
+struct LongFsm {
+    bool open;
+    u32 n, run;
+};
+
+// The endpoint FSM (VAD.C:164-216) over one window of nw <= 1024 frames starting at frame `base` (activity bitmap aw,
+// one 32-frame word per lane), continuing from state f: a run carried in from the previous window completes at the
+// window's first frames, later runs are found with fsm_segments' bit tricks. Windows may have any length from 1 to
+// 1 024: a run longer than the window is carried on. Every lane calls act.open(lane, f.n, frame) when segment f.n
+// opens at `frame` (VAD.C:178: start = 80 * frame) and act.close(lane, f.n, frame) when it closes with its first
+// inactive frame at `frame` (VAD.C:201: end = 80 * frame + 80); f is updated after the call.
+template <class Act>
+__device__ __forceinline__ void long_fsm_window(u32 aw, u32 nw, u32 base, int lane, LongFsm &f, Act &act) {
+    const u32 fullw = nw >> 5, rem = nw & 31u;
+    const u32 vmask = (u32)lane < fullw ? 0xFFFFFFFFu : ((u32)lane == fullw ? ((1u << rem) - 1u) : 0u);
+    aw &= vmask;
+    const u32 z = ~aw & vmask;
+    u32 a8 = aw & bm_shr(aw, 1, lane);
+    a8 &= bm_shr(a8, 2, lane);
+    a8 &= bm_shr(a8, 4, lane);                                     // a8[i]: frames i..i+7 all active
+    u32 z8 = z & bm_shr(z, 1, lane);
+    z8 &= bm_shr(z8, 2, lane);
+    z8 &= bm_shr(z8, 4, lane);
+    const u32 z11 = z8 & bm_shr(z8, 3, lane);                      // z11[i]: frames i..i+10 all inactive
+    auto open_at = [&](u32 frame) {
+        act.open(lane, f.n, frame);
+        f.open = true;
+    };
+    auto close_at = [&](u32 frame) {
+        act.close(lane, f.n, frame);
+        ++f.n;
+        f.open = false;
+    };
+    int cur = 0;                                                   // where the search for the next event resumes
+    bool event = false;
+    if (f.run) {                                                   // a run that began in the previous window
+        const u32 need = (f.open ? 11u : 8u) - f.run, msk = (1u << need) - 1u;
+        const u32 w0 = __shfl_sync(0xFFFFFFFFu, f.open ? z : aw, 0);
+        if (need <= nw && (w0 & msk) == msk) {
+            if (f.open) close_at(base - f.run); else open_at(base - f.run);
+            cur = (int)need;                                       // the opening / closing frame + 8 / + 11
+            event = true;
+        }
+    }
+    for (;;) {
+        const int p = find_first(f.open ? z11 : a8, lane, cur);
+        if (p < 0) break;
+        if (f.open) { close_at(base + (u32)p); cur = p + 11; } else { open_at(base + (u32)p); cur = p + 8; }
+        event = true;
+    }
+    // the run at the end of the window: frames since the last one that breaks it (and since the last event)
+    const int last_brk = find_last(f.open ? aw : z);
+    if (!event && last_brk < 0) f.run += nw;
+    else {
+        const int from = max(last_brk + 1, cur);
+        f.run = from < (int)nw ? nw - (u32)from : 0u;
     }
 }
 

@@ -108,73 +108,17 @@ long_block_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
 }
 
 // ---- K12: segments ---------------------------------------------------------------------------------------------------
-// position of the last set bit in a bitmap held one 32-bit word per lane; -1 if none
-__device__ __forceinline__ int find_last(u32 word) {
-    const u32 bal = __ballot_sync(0xFFFFFFFFu, word != 0);
-    if (!bal) return -1;
-    const int L = 31 - __clz(bal);
-    const u32 mw = __shfl_sync(0xFFFFFFFFu, word, L);
-    return 32 * L + 31 - __clz(mw);
-}
-
-// The FSM's state between windows: open (a segment has opened and not closed), closed = the n segments before it, and
-// run = the length of the run at the end of the frames seen so far that the FSM is counting (active frames while
-// closed, inactive ones while open), always shorter than the 8 / 11 that would complete it.
-struct LongFsm {
-    bool open;
-    u32 n, run;
+// the FSM's actions on a recording: segment k < max_segs is written to out[2k], out[2k+1] (end SR_SEG_NULL until it closes)
+struct LongSegOut {
+    u32 max_segs;
+    u32 *out;
+    __device__ __forceinline__ void open(int lane, u32 n, u32 frame) {        // VAD.C:178: start = i - 7*80, i the 8th active
+        if (lane == 0 && n < max_segs) { out[2 * n] = 80u * frame; out[2 * n + 1] = SR_SEG_NULL; }
+    }
+    __device__ __forceinline__ void close(int lane, u32 n, u32 frame) {       // VAD.C:201: end = i - 11*80 + 160, i the 11th inactive
+        if (lane == 0 && n < max_segs) out[2 * n + 1] = 80u * frame + 80u;
+    }
 };
-
-// The endpoint FSM (VAD.C:164-216) over one window of nw <= 1024 frames starting at frame `base` (activity bitmap aw,
-// one 32-frame word per lane), continuing from state f: a run carried in from the previous window completes at the
-// window's first frames, later runs are found with fsm_segments' bit tricks. Segment k < max_segs is written to
-// out[2k], out[2k+1] (end SR_SEG_NULL until it closes).
-__device__ __forceinline__ void long_fsm_window(u32 aw, u32 nw, u32 base, int lane, LongFsm &f, u32 max_segs, u32 *out) {
-    const u32 fullw = nw >> 5, rem = nw & 31u;
-    const u32 vmask = (u32)lane < fullw ? 0xFFFFFFFFu : ((u32)lane == fullw ? ((1u << rem) - 1u) : 0u);
-    aw &= vmask;
-    const u32 z = ~aw & vmask;
-    u32 a8 = aw & bm_shr(aw, 1, lane);
-    a8 &= bm_shr(a8, 2, lane);
-    a8 &= bm_shr(a8, 4, lane);                                     // a8[i]: frames i..i+7 all active
-    u32 z8 = z & bm_shr(z, 1, lane);
-    z8 &= bm_shr(z8, 2, lane);
-    z8 &= bm_shr(z8, 4, lane);
-    const u32 z11 = z8 & bm_shr(z8, 3, lane);                      // z11[i]: frames i..i+10 all inactive
-    auto open_at = [&](u32 frame) {                                // VAD.C:178: start = i - 7*80, i the 8th active frame
-        if (lane == 0 && f.n < max_segs) { out[2 * f.n] = 80u * frame; out[2 * f.n + 1] = SR_SEG_NULL; }
-        f.open = true;
-    };
-    auto close_at = [&](u32 frame) {                               // VAD.C:201: end = i - 11*80 + 160, i the 11th inactive
-        if (lane == 0 && f.n < max_segs) out[2 * f.n + 1] = 80u * frame + 80u;
-        ++f.n;
-        f.open = false;
-    };
-    int cur = 0;                                                   // where the search for the next event resumes
-    bool event = false;
-    if (f.run) {                                                   // a run that began in the previous window
-        const u32 need = (f.open ? 11u : 8u) - f.run, msk = (1u << need) - 1u;
-        const u32 w0 = __shfl_sync(0xFFFFFFFFu, f.open ? z : aw, 0);
-        if (need <= nw && (w0 & msk) == msk) {
-            if (f.open) close_at(base - f.run); else open_at(base - f.run);
-            cur = (int)need;                                       // the opening / closing frame + 8 / + 11
-            event = true;
-        }
-    }
-    for (;;) {
-        const int p = find_first(f.open ? z11 : a8, lane, cur);
-        if (p < 0) break;
-        if (f.open) { close_at(base + (u32)p); cur = p + 11; } else { open_at(base + (u32)p); cur = p + 8; }
-        event = true;
-    }
-    // the run at the end of the window: frames since the last one that breaks it (and since the last event)
-    const int last_brk = find_last(f.open ? aw : z);
-    if (!event && last_brk < 0) f.run += nw;
-    else {
-        const int from = max(last_brk + 1, cur);
-        f.run = from < (int)nw ? nw - (u32)from : 0u;
-    }
-}
 
 __global__ void __launch_bounds__(kLongWarps * 32)
 long_segment_kernel(u32 U, u32 B, const u32 *__restrict__ lens, const atap_tag *__restrict__ atap, const u32 *__restrict__ info,
@@ -187,6 +131,7 @@ long_segment_kernel(u32 U, u32 B, const u32 *__restrict__ lens, const atap_tag *
     const u32 *inf = info + (size_t)b * info_stride;
     u32 *out = seg_off + (size_t)b * max_segs * 2;
     LongFsm f{false, 0u, 0u};
+    LongSegOut act{max_segs, out};
     u32 cin = 0;                                                   // class of the last out-of-band sample so far (last_sig)
     for (u32 base = 0; base < nfr; base += 1024u) {
         const u32 nw = min(1024u, nfr - base);
@@ -195,7 +140,7 @@ long_segment_kernel(u32 U, u32 B, const u32 *__restrict__ lens, const atap_tag *
             const u32 word = frames_pass(inf, base + 32u * j, base + nw, lane, at, cin);   // VAD.C:121-164
             if ((u32)lane == j) aw = word;
         }
-        long_fsm_window(aw, nw, base, lane, f, max_segs, out);
+        long_fsm_window(aw, nw, base, lane, f, act);
     }
     if (lane == 0) n_segs[b] = f.n + (f.open ? 1u : 0u);           // + the segment still open (end SR_SEG_NULL)
 }

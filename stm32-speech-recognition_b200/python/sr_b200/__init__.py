@@ -168,6 +168,19 @@ def lib():
         L.sr_streams_fetch.argtypes = [vp, vp, u32, vp]
         L.sr_streams_pending.argtypes = [vp]
         L.sr_streams_pending.restype = u32
+        L.sr_long_streams_create.argtypes = [vp, u32, u32, u32, vp, C.POINTER(vp)]
+        L.sr_long_streams_destroy.argtypes = [vp]
+        L.sr_long_streams_reset.argtypes = [vp, vp, vp]
+        L.sr_long_streams_push.argtypes = [vp, vp, u32, u32, vp, u32, vp]
+        L.sr_long_streams_push_ragged.argtypes = [vp, vp, u32, vp, vp, u32, vp]
+        L.sr_long_streams_fetch.argtypes = [vp, vp, u32, vp]
+        L.sr_long_streams_pending.argtypes = [vp]
+        L.sr_long_streams_pending.restype = u32
+        L.sr_long_streams_max_events.argtypes = [vp]
+        L.sr_long_streams_max_events.restype = u32
+        L.sr_long_streams_state.argtypes = [vp, vp, vp, vp, vp]
+        L.sr_long_streams_ring_len.argtypes = [vp]
+        L.sr_long_streams_ring_len.restype = u32
         L.sr_stream_group_create.argtypes = [C.POINTER(vp), u32, u32, u32, u32, C.POINTER(vp)]
         L.sr_stream_group_destroy.argtypes = [vp]
         L.sr_stream_group_reset.argtypes = [vp]
@@ -723,6 +736,89 @@ class StreamPool:
         f = lib().sr_stream_group_segments if self.group else lib().sr_streams_segments
         self._ck(f(self._p, _p(seg), _p(atap)))
         return seg, atap
+
+
+def _row_stride(chunk):
+    """row stride of a [S, n] u16 chunk in samples (numpy may report any stride for a dimension of size 1)"""
+    assert chunk.dtype == np.uint16
+    return chunk.strides[0] // 2 if chunk.shape[0] > 1 else chunk.shape[1]
+
+
+class LongStreamPool:
+    """sr_long_stream_pool wrapper (include/sr_long_stream.h): S live streams of any length, fed in chunks of at most
+    max_chunk samples, every segment decided as it closes. atap: [S] ATAP_DTYPE initial values or None (zeros)."""
+
+    def __init__(self, handle, n_streams, max_chunk, n_len=2400, atap=None):
+        self.S, self.h = n_streams, handle
+        self._p = C.c_void_p()
+        handle._ck(lib().sr_long_streams_create(handle._h, n_streams, max_chunk, n_len, _p(atap), C.byref(self._p)))
+        self.max_events = int(lib().sr_long_streams_max_events(self._p))
+        self._ev = (StreamEvent * self.max_events)()
+        self.ring_len = int(lib().sr_long_streams_ring_len(self._p))
+
+    def _ck(self, rc):
+        if rc != 0:
+            raise SrError("long streaming call failed (%d): %s" % (rc, (lib().sr_last_error(None) or b"").decode()))
+
+    def close(self):
+        if self._p:
+            lib().sr_long_streams_destroy(self._p)
+            self._p = C.c_void_p()
+
+    def reset(self, which=None, atap=None):
+        """restart the streams with which[s] != 0 (None: all) from atap[s] (None: zeros)"""
+        which = None if which is None else np.ascontiguousarray(which, np.uint8)
+        self._ck(lib().sr_long_streams_reset(self._p, _p(which), _p(atap)))
+
+    def _events(self, n, buf=None):
+        buf = self._ev if buf is None else buf
+        return [{k: getattr(buf[i], k) for k, _ in StreamEvent._fields_} for i in range(n)]
+
+    def _buf(self, max_events):
+        if max_events is None or max_events <= self.max_events:
+            return self._ev, self.max_events if max_events is None else max_events
+        return (StreamEvent * max_events)(), max_events
+
+    def push(self, chunk, chunk_len=None, stride=None, max_events=None, events=None):
+        """chunk: numpy [S, chunk_len] u16 (or a raw host pointer with chunk_len / stride). Returns the events as dicts;
+        events: a ctypes StreamEvent array to write them to instead (the count is returned)"""
+        if isinstance(chunk, np.ndarray):
+            chunk_len, stride, ptr = chunk.shape[1], _row_stride(chunk), chunk.ctypes.data_as(C.c_void_p)
+        else:
+            ptr = C.c_void_p(int(chunk))
+        n = C.c_uint32(0)
+        buf, m = (events, len(events) if max_events is None else max_events) if events is not None else self._buf(max_events)
+        self._ck(lib().sr_long_streams_push(self._p, ptr, chunk_len, stride, buf, m, C.byref(n)))
+        return n.value if events is not None else self._events(n.value, buf)
+
+    def push_ragged(self, chunk, lens, stride=None, max_events=None, events=None):
+        """chunk: numpy [S, >= max(lens)] u16 (or raw pointer + stride); lens: [S] samples for each stream"""
+        lens = np.ascontiguousarray(lens, np.uint32)
+        if isinstance(chunk, np.ndarray):
+            stride, ptr = _row_stride(chunk), chunk.ctypes.data_as(C.c_void_p)
+        else:
+            ptr = C.c_void_p(int(chunk))
+        n = C.c_uint32(0)
+        buf, m = (events, len(events) if max_events is None else max_events) if events is not None else self._buf(max_events)
+        self._ck(lib().sr_long_streams_push_ragged(self._p, ptr, stride, _p(lens), buf, m, C.byref(n)))
+        return n.value if events is not None else self._events(n.value, buf)
+
+    def fetch(self, max_events=None):
+        buf, m = self._buf(max_events)
+        n = C.c_uint32(0)
+        self._ck(lib().sr_long_streams_fetch(self._p, buf, m, C.byref(n)))
+        return self._events(n.value, buf)
+
+    def pending(self):
+        return int(lib().sr_long_streams_pending(self._p))
+
+    def state(self):
+        """dict(n_recv [S], n_closed [S], open_start [S] (NULL: none open), atap [S])"""
+        out = dict(n_recv=np.zeros(self.S, np.uint32), n_closed=np.zeros(self.S, np.uint32),
+                   open_start=np.zeros(self.S, np.uint32), atap=np.zeros(self.S, ATAP_DTYPE))
+        self._ck(lib().sr_long_streams_state(self._p, _p(out["n_recv"]), _p(out["n_closed"]), _p(out["open_start"]),
+                                             _p(out["atap"])))
+        return out
 
 
 def host_alloc_dev(device, nbytes):
