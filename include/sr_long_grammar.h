@@ -30,7 +30,8 @@
  * long-form VAD) and 1 (get_mfcc of the feature pieces). The decoder launches take consecutive sequences whose records
  * (12 B per frame and grammar state) fit 256 MB; a sequence whose records alone exceed that runs in a launch of its own,
  * with the record workspace grown to fit it: up to 322 MB for a 2^27-sample recording under 16 states.
- * Not in speech_recog.h or sr_long.h, whose entry points tests enumerate; see DESIGN.md section K13. */
+ * A header of its own, as each extension has; the concurrency test's job table covers its entry points like those of
+ * every other header. See DESIGN.md section K13. */
 #ifndef SR_LONG_GRAMMAR_H_
 #define SR_LONG_GRAMMAR_H_
 #include "sr_long.h"

@@ -42,8 +42,8 @@
  * (DESIGN.md, K14). 2 (R + 9 680) bytes per stream, plus about 2.9 kB per event slot.
  *
  * Per push: one read of the chunk (zero-copy when it is pinned host memory, else one staging copy), four kernels (five
- * with a bank), one D2H copy and ONE synchronisation -- as sr_streams_push. Not in speech_recog.h, whose entry points a
- * test enumerates. */
+ * with a bank), one D2H copy and ONE synchronisation -- as sr_streams_push. A header of its own, as each extension has;
+ * the concurrency test's job table covers its entry points like those of every other header. */
 #ifndef SR_LONG_STREAM_H_
 #define SR_LONG_STREAM_H_
 #include "speech_recog.h"

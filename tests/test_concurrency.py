@@ -7,9 +7,10 @@ against a run made alone. The job table below runs one fixed script per entry-po
 serial baseline runs each job alone (checked on a sample against its oracle), then every job runs R times at once, one
 thread per handle. ctypes releases the GIL during each C call, so the threads' library calls overlap. Each job alternates
 between two inputs, so a repetition that skips work and leaves the previous repetition's workspace contents behind
-cannot pass. The last test is a CPU test: every sr_* entry point of the headers (speech_recog.h and sr_long.h) is either
-in the job table or excluded with a reason."""
+cannot pass. The last test is a CPU test: every sr_* entry point of every header under include/ (found by glob, so a new
+header cannot stay out) is either in the job table or excluded with a reason."""
 import ctypes as C
+import glob
 import os
 import re
 import subprocess
@@ -25,11 +26,16 @@ import oracle_align as oa
 import oracle_bind as ob
 import oracle_connected as oc
 import oracle_grammar as og
+import oracle_long as ol
+import oracle_long_grammar as olg
 import sr_b200
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-HEADERS = (os.path.join(ROOT, "include", "speech_recog.h"), os.path.join(ROOT, "include", "sr_long.h"))
+# every public header (include/compat/ holds the reference's own headers, which glob does not enter); sr_synth.h declares
+# the synthetic-workload helpers the tests build inputs with, whose names may be listed but need no job
+SYNTH_HEADER = os.path.join(ROOT, "include", "sr_synth.h")
+HEADERS = tuple(sorted(h for h in glob.glob(os.path.join(ROOT, "include", "*.h")) if h != SYNTH_HEADER))
 
 R = 3                                    # repetitions of every job in the concurrent run
 TIMING_CAP = 512                         # timing records per handle: more than any job launches per repetition
@@ -641,11 +647,144 @@ class BankDevDtw(Job):
                             {"score": sc, "best_idx": bi, "best_dis": bd})
 
 
+class LongGrammar(Job):
+    """sr_recognise_long_grammar_batch on ragged lens (one past 65 535 samples) under a 5-state PIN chain and then a
+    2-state alternation, so the record workspace changes size between inputs; max_segs below n_segs, atap NULL on input
+    1; then sr_connected_grammar_segs_batch on a small flat segment table"""
+    name = "long_grammar"
+    calls = ("sr_recognise_long_grammar_batch", "sr_connected_grammar_segs_batch")
+    B, U, P, MS, MW = 5, 120000, 1000, 4, 48
+    GRAMS = (sr_b200.chain_grammar(4, 0x3FF), (2, 3, [(0, 1, 0x55), (1, 0, 0x2AA), (1, 1, 0x1)]))
+
+    def open(self):
+        self.h = self.handle()
+        self.h.set_bank(self.w.bank40, 40, 4096)
+        self.inputs = []
+        for v in range(2):
+            pcm = ol.synth_long(self.B, self.U, 0xCD000000 + v)
+            lens = np.array([self.U, 70001 + v, 2399, 40000, self.U - 160 * v], np.uint32)
+            rng = np.random.default_rng(0xCD + v)
+            seg_frm = np.array([30, 0, 119, 5, 64 + v, 818], np.uint32)
+            feat = rng.integers(-3000, 3001, (int(seg_frm.sum()), 12)).astype(np.int16)
+            self.inputs.append((pcm, lens, feat, np.array([0, 2, 3, 6], np.uint32), seg_frm))
+
+    def run(self, v):
+        pcm, lens, feat, seq_seg, seg_frm = self.inputs[v]
+        g = self.GRAMS[v]
+        want = sr_b200.LONG_GRAM_FIELDS if v == 0 else tuple(k for k in sr_b200.LONG_GRAM_FIELDS if k != "atap")
+        out = self.h.recognise_long_grammar(pcm, g, self.P, self.MS, self.MW, 2400, lens, want=want)
+        w, nw, tot = self.h.connected_grammar_segs(feat, seq_seg, seg_frm, g, self.P, self.MW)
+        out.update({"segs_words": w, "segs_n_words": nw, "segs_total": tot})
+        return out
+
+    def oracle(self, v, out):
+        pcm, lens, feat, seq_seg, seg_frm = self.inputs[v]
+        g, lg = self.GRAMS[v], olg.long_grammar()
+        want = olg.recognise_long_grammar(ol.long_oracle(), self.w.po, lg, pcm, 2400, self.w.bank40, 40, 4096, g, self.P,
+                                          self.MS, self.MW, lens)
+        if v == 1:
+            del want["atap"]
+        assert (want["n_segs"] > self.MS).any() and (want["n_words"] > 0).any()
+        w, nw, tot = lg.decode_segs(feat, seq_seg, seg_frm, self.w.bank40, 40, 4096, g, self.P, self.MW)
+        want.update({"segs_words": w, "segs_n_words": nw, "segs_total": tot})
+        return diff_outputs(out, want)
+
+
+class LongStream(Job):
+    """sr_long_streams_*: a pool of 24 streams made and destroyed in every repetition, ragged pushes of 0-1 600 samples
+    (every third with a caller buffer of 2 events, so events queue) and a lock-step push, pending / fetch, a subset
+    reset with the queue drained, then more pushes; events sorted by (stream, segment), state(), max_events, ring_len"""
+    name = "long_stream"
+    calls = ("sr_long_streams_create", "sr_long_streams_destroy", "sr_long_streams_reset", "sr_long_streams_push",
+             "sr_long_streams_push_ragged", "sr_long_streams_fetch", "sr_long_streams_pending",
+             "sr_long_streams_max_events", "sr_long_streams_ring_len", "sr_long_streams_state")
+    S, L, MC = 24, 36000, 1600
+    RESET = np.arange(24) % 5 == 1                    # the streams restarted halfway
+
+    def open(self):
+        self.h = self.handle()
+        self.h.set_bank(self.w.bank8, 8, 4096)
+        self.inputs = []
+        for v in range(2):
+            pcm = ol.synth_long(self.S, self.L, 0xCE000000 + v)
+            rng = np.random.default_rng(0xCE + v)
+            pos, pushes = np.zeros(self.S, np.int64), []
+            while (pos < self.L).any():
+                lens = rng.choice([0, 1, 79, 80, 81, 333, 800, self.MC], self.S).astype(np.int64)
+                lens = np.minimum(lens, self.L - pos)
+                if len(pushes) % 7 == 3:
+                    lens[:] = min(640, int((self.L - pos).min()))              # a lock-step push
+                chunk = np.zeros((self.S, max(1, int(lens.max()))), np.uint16)
+                for s in range(self.S):
+                    chunk[s, :lens[s]] = pcm[s, pos[s]:pos[s] + lens[s]]
+                pushes.append((chunk, lens.astype(np.uint32), pos.copy()))
+                pos += lens
+            self.inputs.append((pcm, pushes))
+
+    def run(self, v):
+        pcm, pushes = self.inputs[v]
+        pool = sr_b200.LongStreamPool(self.h, self.S, self.MC, 2400)
+        try:
+            before, after, queued, half = [], [], [], len(pushes) // 2
+            for i, (chunk, lens, _) in enumerate(pushes):
+                evs = before if i < half else after
+                m = 2 if i % 3 == 2 else None
+                if (lens == lens[0]).all() and lens[0]:
+                    evs += pool.push(np.ascontiguousarray(chunk[:, :lens[0]]), max_events=m)
+                else:
+                    evs += pool.push_ragged(chunk, lens, max_events=m)
+                queued.append(pool.pending())
+                if i == half - 1:
+                    evs += pool.fetch(max_events=pool.pending())    # all of it: the reset must find the queue empty
+                    assert pool.pending() == 0
+                    pool.reset(self.RESET.astype(np.uint8))
+            after += pool.fetch(max_events=pool.pending())
+            st = pool.state()
+            return {"before": events_array(before), "after": events_array(after), "n_recv": st["n_recv"],
+                    "n_closed": st["n_closed"], "open_start": st["open_start"], "atap": st["atap"],
+                    "queued": np.array(queued, np.uint32),
+                    "sizes": np.array([pool.max_events, pool.ring_len, pool.pending()], np.uint32)}
+        finally:
+            pool.close()
+
+    def _closed(self, x):
+        """sr_recognise_long_batch of one stream's samples from the oracles: (closed records, open start, atap)"""
+        r = ol.recognise_long(ol.long_oracle(), self.w.po, np.ascontiguousarray(x[None, :]), 2400, self.w.bank8, 8, 4096,
+                              len(x) // 1520 + 4)
+        recs = [tuple(int(q) for q in rec) for rec in r["segs"][0, :int(r["n_segs"][0])].tolist()]
+        op = recs[-1][0] if recs and recs[-1][2] == 1 else 0xFFFFFFFF
+        return [t for t in recs if t[2] != 1], op, r["atap"][0].tobytes()
+
+    def oracle(self, v, out):
+        pcm, pushes = self.inputs[v]
+        cut = pushes[len(pushes) // 2][2]                 # each stream's sample count at the reset
+        E = -(-(-(-(self.MC + 2400) // 80)) // 19)        # the header's bound, c = n_len
+        bad = diff_outputs({"sizes": out["sizes"]},
+                           {"sizes": np.array([self.S * E, -(-(10561 + self.MC) // 80) * 80, 0], np.uint32)})
+        if out["queued"].max() == 0:
+            bad.append(("queued", "no push left events queued"))
+        fields = ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")
+        for s in (0, 1, 6, self.S - 1):
+            pre = self._closed(pcm[s, :int(cut[s])])[0]
+            x = pcm[s, int(cut[s]):] if self.RESET[s] else pcm[s]
+            closed, op, atap = self._closed(x)
+            for part, want in (("before", pre), ("after", closed if self.RESET[s] else closed[len(pre):])):
+                ev = out[part][out[part]["stream"] == s]
+                got = [tuple(int(e[k]) for k in fields) for e in ev]
+                first = 0 if part == "before" or self.RESET[s] else len(pre)
+                if got != want or ev["segment"].tolist() != list(range(first, first + len(ev))):
+                    bad.append(("%s events of stream %d" % (part, s), "%d events, %d closed records" % (len(got), len(want))))
+            st = (int(out["n_recv"][s]), int(out["n_closed"][s]), int(out["open_start"][s]), out["atap"][s].tobytes())
+            if st != (len(x), len(closed), op, atap):
+                bad.append(("state of stream %d" % s, "%s" % (st[:3],)))
+        return bad
+
+
 JOBS = (RecognisePacked, RecogniseDevBand, DtwDynamic, GeomB, EnrolAverageAlign, LongConnected, Grammar, StreamRagged,
-        StreamGroup, BankDevRecognise, BankDevDtw, LongForm)
+        StreamGroup, BankDevRecognise, BankDevDtw, LongForm, LongGrammar, LongStream)
 RECREATED = "dtw_dynamic"                # the job whose thread destroys its handle and makes a new one halfway through
 
-# sr_* entry points of include/speech_recog.h and include/sr_long.h that no job runs, each with the reason
+# sr_* entry points of the headers that no job runs, each with the reason
 EXCLUDED = {
     "sr_comm_unique_id": "NCCL: needs two ranks, one per GPU",
     "sr_comm_create": "NCCL: needs two ranks, one per GPU",
@@ -707,11 +846,16 @@ def test_every_entry_point_is_in_the_job_table_or_excluded():
     names = header_entry_points()
     assert len(names) > 60 and "sr_recognise_batch" in names and "sr_connected_grammar_batch" in names, names
     assert "sr_vad_long_batch_dev" in names, names
+    newer = {"sr_connected_grammar_segs_batch", "sr_recognise_long_grammar_batch"} | {
+        "sr_long_streams_" + n for n in ("create", "destroy", "reset", "push", "push_ragged", "fetch", "pending", "max_events",
+                                         "ring_len", "state")}
+    assert newer <= set(names), newer - set(names)
+    assert {os.path.basename(h) for h in HEADERS} >= {"speech_recog.h", "sr_long.h", "sr_long_grammar.h", "sr_long_stream.h"}
     covered = {c for j in JOBS for c in j.calls} | set(OTHER_CALLS)
     assert not (covered & set(EXCLUDED)), covered & set(EXCLUDED)
     missing = [n for n in names if n not in covered and n not in EXCLUDED]
     assert not missing, "entry points neither in the job table nor excluded: %s" % missing
-    lib_syms = set(re.findall(r"\b(sr_\w+)\b", open(os.path.join(ROOT, "include", "sr_synth.h")).read()))
+    lib_syms = set(re.findall(r"\b(sr_\w+)\b", open(SYNTH_HEADER).read()))
     stale = [n for n in (covered | set(EXCLUDED)) if n not in names and n not in lib_syms]
     assert not stale, "listed but not declared: %s" % stale
     assert len({j.name for j in JOBS}) == len(JOBS) and RECREATED in {j.name for j in JOBS}

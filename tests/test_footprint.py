@@ -787,3 +787,328 @@ def test_stream_push_past_max_samples_drops_the_excess(bank, ragged):
     pool.close()
     _check_batch(h, np.ascontiguousarray(pcm[:, :L]), evs, seg, atap)
     h.close()
+
+
+# ---- one grammar decode per long recording (include/sr_long_grammar.h) ------------------------------------------------------
+G13 = (3, 5, [(0, 1, 0x3), (1, 2, 0x7), (2, 0, 0x7), (1, 1, 0x8)])    # 3 states over commands 0-3
+
+
+def _long_gram_oracle(pcm, n_len, bank_, n_slot, stride, g, P, max_segs, max_words, lens=None, geom_b=False, atap=None):
+    import oracle_long as ol
+    import oracle_long_grammar as olg
+    return olg.recognise_long_grammar(ol.long_oracle(), ob.port(), olg.long_grammar(), pcm, n_len, bank_, n_slot, stride, g,
+                                      P, max_segs, max_words, lens, geom_b, atap)
+
+
+def _same(got, want, what=""):
+    for k in want:
+        assert np.asarray(got[k]).tobytes() == np.asarray(want[k]).tobytes(), (what, k)
+
+
+@pytest.mark.parametrize("geom", [0, 1], ids=["ref", "geom_b"])
+def test_long_grammar_reads_only_lens_samples(bank, geom):
+    """sr_recognise_long_grammar_batch: loud band-crossing poison past lens[b] (it would open segments if read) gives the
+    results of the clean recordings, which equal the composed oracle"""
+    import oracle_long as ol
+    B, U = 5, 90001
+    lens = np.array([U, 70000, 2399, 161, 40000], np.uint32)
+    clean = ol.synth_long(B, U, 0x13A5)
+    bad = clean.copy()
+    for b, n in enumerate(lens):
+        bad[b, n:] = np.where(np.arange(U - n) % 2, 4095, 0)
+    want = _long_gram_oracle(clean, 2400, bank, T, 4096, G13, 1000, 64, 256, lens, geom == 1)
+    assert (want["n_segs"][[0, 1, 4]] >= 3).all() and (want["n_words"] > 0).sum() >= 3
+    h = _handle(bank, geom)
+    for pcm in (clean, bad):
+        _same(h.recognise_long_grammar(pcm, G13, 1000, 64, 256, 2400, lens), want, "poison" if pcm is bad else "clean")
+    h.close()
+
+
+def test_long_grammar_outputs_may_be_null(bank):
+    """each output pointer NULL in turn, and every one but n_words: the fields passed equal the full call's. With atap
+    NULL and n_len = 0 (no calibration overwrites it) the call starts from zeros although the previous call on the handle
+    left another atap in the workspace the NULL path uses"""
+    import oracle_long as ol
+    B, U, MS, MW = 4, 60001, 5, 40
+    lens = np.array([U, 2000, 50000, 30000], np.uint32)
+    pcm = ol.synth_long(B, U, 0x13A6)
+    h = _handle(bank)
+    full = h.recognise_long_grammar(pcm, G13, 1000, MS, MW, 2400, lens)
+    _same(full, _long_gram_oracle(pcm, 2400, bank, T, 4096, G13, 1000, MS, MW, lens))
+    assert (full["n_segs"] > MS).any() and (full["n_words"] > 0).sum() >= 2
+    F = sr_b200.LONG_GRAM_FIELDS
+    for want in [tuple(k for k in F if k != q) for q in F] + [("n_words",)]:
+        _same(h.recognise_long_grammar(pcm, G13, 1000, MS, MW, 2400, lens, want=want), {k: full[k] for k in want}, want)
+    # n_len = 0: atap is the one VAD uses from the first sample on
+    given = _front(pcm, U)
+    assert (given["mid_val"] != 0).all()
+    out = {k: np.zeros(full[k].shape, full[k].dtype) for k in F}
+    out["atap"] = given.copy()
+    with_given = h.recognise_long_grammar(pcm, G13, 1000, MS, MW, 0, lens, out=out)   # leaves `given` in the workspace
+    assert with_given["atap"].tobytes() == given.tobytes()
+    no_atap = tuple(k for k in F if k != "atap")
+    got = h.recognise_long_grammar(pcm, G13, 1000, MS, MW, 0, lens, want=no_atap)
+    want = _long_gram_oracle(pcm, 0, bank, T, 4096, G13, 1000, MS, MW, lens)
+    _same(got, {k: want[k] for k in no_atap}, "atap NULL after a call with another atap")
+    assert any(got[k].tobytes() != with_given[k].tobytes() for k in no_atap)      # stale bytes would show
+    h.close()
+
+
+def test_long_grammar_shares_workspaces_with_the_other_calls(ora):
+    """on one handle: a 16-state K13 decode of a 2^27-sample recording (its records grow the workspace past 256 MB), a
+    1-state sr_connected_grammar_segs_batch, a larger sr_recognise_long_batch, a small K13 call in each geometry, the
+    capture grammar and connected calls, then K13 with a larger batch. Each result equals a fresh handle's byte for
+    byte, and the fresh handle's equals the CPU oracles"""
+    import oracle_connected as oc
+    import oracle_grammar as og
+    import oracle_long as ol
+    import oracle_long_grammar as olg
+    from test_connected import _bank
+    from test_long_stream import plant_act, planted_atap
+    lo, port = ol.long_oracle(), ob.port()
+    bk = _bank(np.random.default_rng(0x13F1), 16, "small", plant=False)     # 16 slots of 1-8 frames, stride 2880
+    NS, ST = 16, bk.shape[1]
+    g16 = (16, 0xFFFF, [(k, (k + 1) % 16, 0x1) for k in range(16)])          # 16 states x the 4 slots of command 0
+    chain = sr_b200.chain_grammar(3, 0xF)
+    # 800 active frames, 11 inactive: segments of 800 frames, 98.6 % of the recording decodable
+    act = ((np.arange((1 << 27) // 80 - 1) % 811) < 800).astype(np.uint8)
+    big = np.ascontiguousarray(plant_act(act)[None, :1 << 27])
+    assert act.sum() * 16 * 12 > 256 << 20
+    rng = np.random.default_rng(0x13F2)
+    seg_frm = np.array([7, 0, 300, 1, 818], np.uint32)
+    feat = rng.integers(-3000, 3001, (int(seg_frm.sum()), 12)).astype(np.int16)
+    seq_seg = np.array([0, 2, 5], np.uint32)
+    pcm3 = ol.synth_long(12, 100000, 0x13F3)
+    pcm4 = ol.synth_long(3, 30000, 0x13F4)
+    pcm5 = sr_b200.synth_pcm_host(8, 16000, 0x13F5, 3)
+    lens6 = np.array([60000, 59000, 20000, 161, 60000, 45000, 2401, 60000], np.uint32)
+    pcm6 = ol.synth_long(8, 60000, 0x13F6)
+
+    def steps():
+        yield "big", lambda h: h.recognise_long_grammar(big, g16, 1000, 8, 32, 0, None,
+                                                        out=dict(_gram_out(1, 8, 32), atap=planted_atap(1)))
+        yield "segs", lambda h: dict(zip(("words", "n_words", "total"), h.connected_grammar_segs(feat, seq_seg, seg_frm,
+                                                                                                 sr_b200.loop_grammar(), 500, 64)))
+        yield "long_batch", lambda h: h.recognise_long_batch(pcm3, 96, 2400)
+        for geom in (0, 1):
+            yield "small_geom%d" % geom, lambda h, geom=geom: _in_geom(h, geom, lambda: h.recognise_long_grammar(pcm4, chain, 1000, 16, 16))
+        yield "capture", lambda h: dict([("g_" + k, a) for k, a in h.recognise_connected_grammar(pcm5, chain, 0, 8).items()] +
+                                        [("c_" + k, a) for k, a in h.recognise_connected(pcm5, 3000, 8).items()])
+        yield "k13_larger_b", lambda h: h.recognise_long_grammar(pcm6, chain, 1000, 24, 64, 2400, lens6)
+
+    def oracle(name, got):
+        if name == "big":
+            w = _long_gram_oracle(big, 0, bk, NS, ST, g16, 1000, 8, 32, atap=planted_atap(1))
+            assert int(w["n_segs"][0]) > 2000 and int(w["n_words"][0]) > 2000
+        elif name == "segs":
+            w = dict(zip(("words", "n_words", "total"), olg.long_grammar().decode_segs(feat, seq_seg, seg_frm, bk, NS, ST,
+                                                                                        sr_b200.loop_grammar(), 500, 64)))
+        elif name == "long_batch":
+            w = ol.recognise_long(lo, port, pcm3, 2400, bk, NS, ST, 96)
+        elif name.startswith("small"):
+            w = _long_gram_oracle(pcm4, 2400, bk, NS, ST, chain, 1000, 16, 16, geom_b=name.endswith("1"))
+        elif name == "capture":
+            a = og.recognise_connected_grammar(ora, og.grammar(), pcm5, 2400, bk, NS, ST, chain, 0, 8)
+            b = oc.recognise_connected(ora, oc.connected(), pcm5, 2400, bk, NS, ST, 3000, 8)
+            w = dict([("g_" + k, v) for k, v in a.items()] + [("c_" + k, v) for k, v in b.items()])
+        else:
+            w = _long_gram_oracle(pcm6, 2400, bk, NS, ST, chain, 1000, 24, 64, lens6)
+        _same(got, w, name + " (fresh handle) against the oracle")
+
+    shared = _handle()
+    shared.set_bank(bk, NS, ST)
+    try:
+        for name, run in steps():
+            got = run(shared)
+            fresh = _handle()
+            fresh.set_bank(bk, NS, ST)
+            want = run(fresh)
+            fresh.close()
+            _same(got, want, name + ": shared handle against a fresh one")
+            oracle(name, want)
+    finally:
+        shared.close()
+
+
+def _gram_out(B, max_segs, max_words):
+    shape = {"atap": (B, ob.ATAP_DTYPE), "n_segs": (B, np.uint32), "seg_off": ((B, max_segs, 2), np.uint32),
+             "frm_num": ((B, max_segs), np.uint32), "seg_status": ((B, max_segs), np.uint8), "n_words": (B, np.uint32),
+             "words": ((B, max_words), sr_b200.WORD_DTYPE), "total": (B, np.uint64)}
+    return {k: np.zeros(*shape[k]) for k in sr_b200.LONG_GRAM_FIELDS}
+
+
+def _in_geom(h, geom, f):
+    h.set_geometry(geom)
+    try:
+        return f()
+    finally:
+        h.set_geometry(0)
+
+
+# ---- live streams of any length (include/sr_long_stream.h) ---------------------------------------------------------------
+def _long_events(evs, S):
+    """each stream's event records in segment order"""
+    per = [[] for _ in range(S)]
+    for e in sorted(evs, key=lambda e: (e["stream"], e["segment"])):
+        assert e["segment"] == len(per[e["stream"]])
+        per[e["stream"]].append(tuple(int(e[k]) for k in ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")))
+    return per
+
+
+def _check_long_prefix(h, pcm, per, st, n_len=2400):
+    """prefix equality after the last push: each stream's events are the closed records of sr_recognise_long_batch on
+    what it was fed, open_start its open record, atap its atap"""
+    S, N = pcm.shape
+    r = h.recognise_long_batch(pcm, N // 1520 + 4, n_len)
+    for s in range(S):
+        recs = [tuple(int(v) for v in rec) for rec in r["segs"][s, :int(r["n_segs"][s])].tolist()]
+        assert per[s] == [t for t in recs if t[2] != 1], s
+        assert int(st["open_start"][s]) == (recs[-1][0] if recs and recs[-1][2] == 1 else ob.NULL), s
+        assert st["atap"][s].tobytes() == r["atap"][s].tobytes() and int(st["n_recv"][s]) == N
+    assert sum(len(p) for p in per) > S
+
+
+def test_long_stream_push_reads_only_lens_samples(bank):
+    """sr_long_streams_push_ragged with rows that carry poison past lens[s] (lens 0 next to long rows): the events and
+    state of clean pushes, which satisfy prefix equality"""
+    S, L = 25, 40000
+    pcm = sr_b200.synth_pcm_host(S, L, 0x5EEDD000, 2)
+    h = _handle(bank)
+    runs = []
+    for poison in ([0, 0], [0xFFFF, 0]):
+        pool = sr_b200.LongStreamPool(h, S, 4000, 2400)
+        evs = _ragged_run(pool, pcm, np.random.default_rng(14), poison)
+        st = pool.state()
+        pool.close()
+        runs.append((_long_events(evs, S), st))
+    assert runs[0][0] == runs[1][0] and all(runs[0][1][k].tobytes() == runs[1][1][k].tobytes() for k in runs[0][1])
+    _check_long_prefix(h, pcm, runs[1][0], runs[1][1])
+    h.close()
+
+
+def test_long_stream_lock_step_reads_only_chunk_len_from_pinned_strided_rows(bank):
+    """sr_long_streams_push from pinned host memory, rows chunk_stride > chunk_len apart with poison in between: the
+    events and state of pushes of clean rows"""
+    S, L, cl, stride = 24, 16000, 800, 808 + 13
+    pcm = sr_b200.synth_pcm_host(S, L, 0x5EEDE000, 2)
+    h = _handle(bank)
+    buf, p = sr_b200.host_alloc_dev(0, S * stride * 2)
+    runs = []
+    try:
+        rows = buf.view(np.uint16).reshape(S, stride)
+        for pinned in (False, True):
+            pool = sr_b200.LongStreamPool(h, S, cl, 2400)
+            evs = []
+            for n0 in range(0, L, cl):
+                if pinned:
+                    rows[:] = np.resize(np.array([0xFFFF, 0], np.uint16), stride)
+                    rows[:, :cl] = pcm[:, n0:n0 + cl]
+                    evs += pool.push(p, chunk_len=cl, stride=stride)
+                else:
+                    evs += pool.push(np.ascontiguousarray(pcm[:, n0:n0 + cl]))
+            runs.append((_long_events(evs, S), pool.state()))
+            pool.close()
+    finally:
+        sr_b200.host_free(p)
+    assert runs[0][0] == runs[1][0] and all(runs[0][1][k].tobytes() == runs[1][1][k].tobytes() for k in runs[0][1])
+    _check_long_prefix(h, pcm, runs[1][0], runs[1][1])
+    h.close()
+
+
+def test_long_stream_reset_leaves_no_stale_ring_content(bank):
+    """rings and mirrors filled with MARK / LOUD blocks, then a subset reset and planted audio pushed to the reset streams:
+    a segment at stream sample 0, one on ring slot 0 after the first wrap (x[-1] from the mirror's partner slot R - 1)
+    and one across the wrap, read through the mirror. Events and state() equal a fresh pool's"""
+    from test_long_stream import MARK, plant_segs, planted_atap
+    h = _handle(bank)
+    h.set_bank(bank, T, 4096)
+    S, mc = 6, 640
+    which = (np.arange(S) % 2 == 0).astype(np.uint8)
+    pool = sr_b200.LongStreamPool(h, S, mc, 0, planted_atap(S))
+    Rb = pool.ring_len // 80
+    x = plant_segs(4 * Rb, [(0, 30), (Rb, 40), (2 * Rb - 20, 60)])
+    stale = np.tile(np.repeat(np.array([MARK, 2148], np.uint16), 80), Rb + 200)[:2 * 80 * Rb + 777]
+    try:
+        for n0 in range(0, len(stale), mc):
+            pool.push(np.ascontiguousarray(np.tile(stale[n0:n0 + mc], (S, 1))))
+        kept = pool.state()
+        pool.reset(which, planted_atap(S))
+        fresh = sr_b200.LongStreamPool(h, S, mc, 0, planted_atap(S))
+        got, want = [], []
+        for n0 in range(0, len(x), mc):
+            k = min(mc, len(x) - n0)
+            chunk = np.zeros((S, k), np.uint16)
+            chunk[which == 1] = x[n0:n0 + k]
+            lens = np.where(which == 1, k, 0).astype(np.uint32)
+            got += pool.push_ragged(chunk, lens)
+            want += fresh.push_ragged(chunk, lens)
+        st, fs = pool.state(), fresh.state()
+        fresh.close()
+        r = which == 1
+        assert _long_events(got, S) == _long_events(want, S)
+        assert [len(p) for p in _long_events(got, S)] == [3 if w else 0 for w in which]
+        for k in st:
+            assert st[k][r].tobytes() == fs[k][r].tobytes(), k
+            assert st[k][~r].tobytes() == kept[k][~r].tobytes(), k
+    finally:
+        pool.close()
+    h.close()
+
+
+def test_long_stream_reset_drops_only_the_reset_streams_queued_events(bank):
+    """events queued for reset and kept streams at the reset: each kept stream's survive in order, the reset streams' are
+    gone. Compared per stream with the same pool without the reset: within one push the order across streams is that of
+    the step kernel's atomic event slots, so only each stream's own sequence is defined"""
+    S, L, mc = 6, 48000, 640
+    pcm = sr_b200.synth_pcm_host(S, L, 0x5EEDF000, 3)
+    h = _handle(bank)
+    which = np.array([1, 0, 0, 1, 0, 1], np.uint8)
+    out = []
+    for reset in (False, True):
+        pool = sr_b200.LongStreamPool(h, S, mc, 2400)
+        for n0 in range(0, L, mc):
+            assert pool.push(np.ascontiguousarray(pcm[:, n0:n0 + mc]), max_events=0) == []
+        queued = pool.pending()
+        if reset:
+            pool.reset(which)
+        out.append((queued, pool.fetch(max_events=max(queued, 1)), pool.pending()))
+        pool.close()
+    (q0, all_ev, p0), (q1, kept_ev, p1) = out
+    assert q0 == q1 and p0 == p1 == 0
+
+    def per_stream(evs):                                            # each stream's events in the order handed out
+        return [[e for e in evs if e["stream"] == s] for s in range(S)]
+    every, kept = per_stream(all_ev), per_stream(kept_ev)
+    assert all(every[s] for s in range(S))
+    for s in range(S):
+        if which[s]:
+            assert kept[s] == [], s
+        else:
+            assert kept[s] == every[s] and [e["segment"] for e in kept[s]] == list(range(len(kept[s]))), s
+    h.close()
+
+
+def test_long_stream_state_outputs_may_be_null(bank):
+    """sr_long_streams_state with each output NULL in turn equals the full query, and leaves the caller's arrays it was
+    not given alone"""
+    S = 9
+    pcm = sr_b200.synth_pcm_host(S, 24000, 0x5EEE0000, 3)
+    h = _handle(bank)
+    pool = sr_b200.LongStreamPool(h, S, 800, 2400)
+    try:
+        for n0 in range(0, 24000 - 333, 800):
+            pool.push(np.ascontiguousarray(pcm[:, n0:n0 + 800]))
+        full = pool.state()
+        assert (full["n_closed"] > 0).any() and (full["n_recv"] > 0).all()
+        keys = ("n_recv", "n_closed", "open_start", "atap")
+        for null in keys + (None,):
+            arr = {k: np.frombuffer(b"\xa5" * full[k].nbytes, full[k].dtype).copy() for k in keys}
+            assert sr_b200.lib().sr_long_streams_state(pool._p, *[None if k == null else arr[k].ctypes.data for k in keys]) == 0
+            for k in keys:
+                if k == null:
+                    assert set(arr[k].tobytes()) == {0xA5}, k
+                else:
+                    assert arr[k].tobytes() == full[k].tobytes(), (null, k)
+    finally:
+        pool.close()
+    h.close()

@@ -755,3 +755,196 @@ def test_threads_beside_a_long_batch_handle(bank):
     finally:
         for h in handles:
             h.close()
+
+
+# ---- the event buffer at its bound ---------------------------------------------------------------------------------------
+# Period-19 activity: 8 active frames, then 11 inactive. A run of 8 opens a segment on its 8th frame and the 11th inactive
+# frame after it closes the segment, so closings fall every 19 frames, the densest the FSM allows, and a push that
+# evaluates F new frames starting on a closing closes exactly ceil(F / 19) segments per stream: the header's E.
+def period_act(n_frames, offset):
+    """offset inactive frames, then runs of 8 active and 11 inactive frames"""
+    k = np.arange(n_frames) - offset
+    return ((k >= 0) & (k % 19 < 8)).astype(np.uint8)
+
+
+def period_closings(n_frames, offset):
+    """the frames on which period_act's segments close: the 11th inactive frame after each run"""
+    return np.arange(offset + 18, n_frames, 19)
+
+
+def closings_between(closings, n0, n1):
+    """segments a push from n0 to n1 samples closes: closing frames it evaluates, frames_of(n0) .. frames_of(n1) - 1"""
+    return int(((closings >= frames_of(n0)) & (closings < frames_of(n1))).sum())
+
+
+def test_period_19_string_closes_every_19_frames():
+    """the sequential FSM on period_act closes on period_closings for every offset, and the planted PCM realises the
+    string under planted_atap (the long-form VAD oracle on the PCM gives the FSM's segments)"""
+    lo = ol.long_oracle()
+    for j in range(19):
+        act = period_act(600, j)
+        x = plant_act(act)
+        segs = fsm_seq(act[:frames_of(len(x))])                     # the frames the PCM's length evaluates
+        closed = [s for s in segs if s[1] != NULL]
+        assert [(e - 160) // 80 + 11 for _, e in closed] == period_closings(frames_of(len(x)), j).tolist()
+        n, seg = lo.vad_long(x[None, :], planted_atap(), 64)
+        assert [tuple(s) for s in seg[0, :int(n[0])].tolist()] == segs, j
+    assert events_per_push(1 << 20, 0) == 690 and (-(-(1 << 20) // 80)) // 19 == 689    # ceil and floor differ here
+
+
+def _take_counts(f, lens, max_events=None):
+    """one ragged push of Feed f: (events handed out, per-stream events handed out)"""
+    before = [len(g) for g in f.got]
+    lens = np.asarray(lens, np.int64)
+    chunk = np.zeros((f.S, max(1, int(lens.max()))), np.uint16)
+    for s in range(f.S):
+        chunk[s, :lens[s]] = f.xs[s][f.n[s]:f.n[s] + lens[s]]
+    evs = f.pool.push_ragged(chunk, lens.astype(np.uint32), max_events=max_events)
+    f.take(evs)
+    f.n += lens
+    return len(evs), [len(g) - b for g, b in zip(f.got, before)]
+
+
+def _check_prefix(f):
+    """with events still queued, each stream's events so far are a prefix of the closed records, and n_closed counts
+    them all"""
+    st = f.pool.state()
+    want = expected(f.h, f.xs, f.n, f.n_len, f.atap0)
+    for s in range(f.S):
+        closed = want[s][0]
+        assert f.got[s] == closed[:len(f.got[s])], s
+        assert int(st["n_closed"][s]) == len(closed) and int(st["n_recv"][s]) == f.n[s]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("geom", [0, 1])
+def test_event_buffer_at_its_bound_without_calibration(handle, bank, geom):
+    """max_chunk = 2^20, n_len = 0: 19 streams of period-19 activity offset by 0 ... 18 frames (every phase of the carried
+    run meets every push and window edge), pushes of 2^20 samples and ragged shorter ones; each stream closes exactly the
+    segments its phase puts into each push, and prefix equality holds after every push"""
+    handle.set_bank(bank[0], bank[1], 4096)
+    handle.set_geometry(geom)
+    max_chunk, S = 1 << 20, 19
+    sched = [max_chunk, 80 * 4099 + 41, max_chunk, max_chunk - 1, 12345, max_chunk]
+    total = sum(sched) + 80 * 19
+    n_frames = total // 80 + 2
+    xs = [plant_act(period_act(n_frames, j)) for j in range(S)]
+    clos = [period_closings(n_frames, j) for j in range(S)]
+    f = Feed(handle, xs, max_chunk, 0, planted_atap(S))
+    try:
+        E = events_per_push(max_chunk, 0)
+        assert f.pool.max_events == S * E == S * 690
+        rng = np.random.default_rng(geom)
+        for i, c in enumerate(sched):
+            lens = np.full(S, c, np.int64)
+            if i == 4:                                              # ragged: a different edge for every stream
+                lens = rng.integers(0, c + 1, S)
+            want = [closings_between(clos[s], f.n[s], f.n[s] + lens[s]) for s in range(S)]
+            n, per = _take_counts(f, lens)
+            assert per == want and n == sum(want), (i, per, want)
+            f.check()
+        assert max(closings_between(clos[s], 0, f.n[s]) for s in range(S)) > 2000
+    finally:
+        handle.set_geometry(0)
+        f.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("small_buffer", [False, True])
+def test_event_buffer_filled_to_cap(handle, bank, small_buffer):
+    """every stream aligned: the first push ends just before a closing frame, so the next push of 2^20 samples evaluates
+    13 108 frames from a closing on and closes E = 690 segments per stream: it hands out exactly max_events events (the
+    device buffer full to cap). With a caller buffer of 1 000 events, more than cap events carry over to the next push and
+    to fetch, oldest first"""
+    handle.set_bank(bank[0], bank[1], 4096)
+    max_chunk, S = 1 << 20, 19
+    first = 80 * (19 * 10 + 18) + 160                               # frames_of(first) = 208: frame 208 closes
+    assert frames_of(first) == 208 and 208 in period_closings(300, 0)
+    n_frames = (first + 3 * max_chunk) // 80 + 2
+    x = plant_act(period_act(n_frames, 0))
+    f = Feed(handle, [x] * S, max_chunk, 0, planted_atap(S))
+    clos = period_closings(n_frames, 0)
+    try:
+        cap = f.pool.max_events
+        assert cap == S * 690
+        m = 1000 if small_buffer else None
+        produced = handed = 0
+        for i, c in enumerate((first, max_chunk, max_chunk)):
+            k = closings_between(clos, int(f.n[0]), int(f.n[0]) + c)
+            n, per = _take_counts(f, [c] * S, m)
+            produced, handed = produced + k * S, handed + n
+            assert k == (10, 690, 690)[i] and f.pool.pending() == produced - handed
+            if not small_buffer:
+                assert n == k * S and per == [k] * S
+                assert i != 1 or n == cap                           # the push that fills the device buffer
+                f.check()
+            else:
+                assert n == min(m, produced - handed + n)
+                _check_prefix(f)
+        if small_buffer:
+            assert f.pool.pending() > cap
+            f.take(f.pool.fetch(max_events=f.pool.pending()))
+            assert f.pool.pending() == 0
+            f.check()
+    finally:
+        f.close()
+
+
+# Calibration push: n_len = 65 520 and max_chunk = 800, so c = n_len is what lets the push that completes calibration close
+# its segments (E = ceil(829 / 19) = 44 against ceil(10 / 19) = 1 without c). The period-19 string cannot realise itself
+# under its own noise_atap: with 9 loud blocks in 19 and a mean at mid_val, the quiet blocks carry as much |x - mid| as
+# the loud ones, and a loud frame sums only 1.055 times the window's average frame (s_thl is 1.1 times it). So the window
+# starts with 40 quiet blocks and holds 41 periods; loud samples sit 450 above mid_val and quiet ones 369 below it, which
+# puts mid_val at exactly 2 048, n_thl between 369 and 450 (quiet samples in band, no low markers, so no crossing counts),
+# and s_thl just under a loud frame's sum (160 * 450) and well above a mixed frame's (80 * 450 + 80 * 369).
+CAL_LEN, CAL_CHUNK, CAL_LEAD = 65520, 800, 40
+CAL_LOUD, CAL_QUIET = 2048 + 450, 2048 - 369
+
+
+def calibration_stream(n_frames):
+    """CAL_LEAD quiet blocks, then period-19 activity at CAL_LOUD / CAL_QUIET"""
+    act = period_act(n_frames, CAL_LEAD)
+    return np.where(plant_act(act) == LOUD, CAL_LOUD, CAL_QUIET).astype(np.uint16), act
+
+
+def test_calibration_stream_realises_its_string_under_its_own_atap():
+    """on the CPU: noise_atap over the first 65 520 samples gives mid_val 2 048 and thresholds under which the long-form
+    VAD oracle finds exactly the string's segments, 41 of them closing in the calibration window's frames"""
+    lo, port = ol.long_oracle(), ob.port()
+    x, act = calibration_stream(900)
+    at = port.noise_atap(np.ascontiguousarray(x[:CAL_LEN]), CAL_LEN)
+    assert int(at["mid_val"][0]) == 2048 and 369 < int(at["n_thl"][0]) < 450, at
+    assert 80 * (450 + 369) < int(at["s_thl"][0]) < 160 * 450, at
+    n, seg = lo.vad_long(x[None, :], at, 128)
+    assert [tuple(s) for s in seg[0, :int(n[0])].tolist()] == fsm_seq(act[:frames_of(len(x))])
+    assert closings_between(period_closings(900, CAL_LEAD), 0, CAL_LEN + CAL_CHUNK - 1) == 41
+    assert 41 > -(-(-(-CAL_CHUNK // 80)) // 19) == 1 and events_per_push(CAL_CHUNK, CAL_LEN) == 44
+
+
+@pytest.mark.gpu
+def test_event_buffer_at_the_calibration_push(handle, bank):
+    """pushes of 799 samples: no frame is evaluated before n reaches 65 520; the push that completes calibration evaluates
+    the 827 frames so far and closes 41 segments per stream, more than a bound without c allows; prefix equality after
+    every push from then on"""
+    handle.set_bank(bank[0], bank[1], 4096)
+    S = 8
+    x, _ = calibration_stream(1400)
+    clos = period_closings(1400, CAL_LEAD)
+    f = Feed(handle, [x] * S, CAL_CHUNK, CAL_LEN)
+    try:
+        assert f.pool.max_events == S * events_per_push(CAL_CHUNK, CAL_LEN) == S * 44
+        cal_push = False
+        while f.n[0] + 799 <= len(x) - 80:
+            n0 = int(f.n[0])
+            n, per = _take_counts(f, [799] * S)
+            # no frame is evaluated before calibration completes; its push evaluates every frame so far
+            want = closings_between(clos, n0 if n0 >= CAL_LEN else 0, n0 + 799) if n0 + 799 >= CAL_LEN else 0
+            assert per == [want] * S, (n0, per, want)
+            if n0 < CAL_LEN <= n0 + 799:
+                assert want == 41 and n == 41 * S
+                cal_push = True
+            if n0 + 799 >= CAL_LEN:
+                f.check()
+        assert cal_push
+    finally:
+        f.close()
