@@ -415,7 +415,9 @@ int sr_streams_segments(sr_stream_pool *p, uint32_t *seg_off /* [n_streams][3][2
 
 /* The same over several GPUs of one box (BASELINE configs[4]): streams [S*g/G, S*(g+1)/G) live on handles[g]; one
  * persistent host thread per shard (bound to its GPU's NUMA node) runs that shard's push, so the G pushes overlap.
- * chunk / lens / seg_off / atap are indexed by GLOBAL stream number, events carry global stream numbers. */
+ * chunk / lens / seg_off / atap are indexed by GLOBAL stream number, events carry global stream numbers.
+ * A group has no fetch or pending call: events that do not fit max_events stay queued on their shard and come out with
+ * the group's next push (oldest first, shard after shard); a push of zero samples drains them. */
 typedef struct sr_stream_group sr_stream_group;
 int sr_stream_group_create(sr_handle *const *handles, uint32_t n_handles, uint32_t n_streams, uint32_t max_samples,
                            uint32_t n_len, sr_stream_group **out);

@@ -722,12 +722,17 @@ class StreamPool:
         return self._events(n.value)
 
     def fetch(self, max_events=None):
-        assert not self.group
+        if self.group:
+            raise SrError("fetch() is not defined for a stream group: push zero samples to drain its queue")
         n = C.c_uint32(0)
         self._ck(lib().sr_streams_fetch(self._p, self._ev, 3 * self.S if max_events is None else max_events, C.byref(n)))
         return self._events(n.value)
 
     def pending(self):
+        """events queued by a pool's earlier pushes; a group has no such call (its queued events come out with its next
+        push, and a push of zero samples drains them)"""
+        if self.group:
+            raise SrError("pending() is not defined for a stream group: push zero samples to drain its queue")
         return int(lib().sr_streams_pending(self._p))
 
     def segments(self):
