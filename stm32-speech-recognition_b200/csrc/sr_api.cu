@@ -1029,6 +1029,13 @@ static int gram_copies(sr_handle *h, const sr_grammar *g, std::vector<u32> &copy
 
 constexpr size_t kGramRecBytes = 256u << 20;   // records per launch: sum of N * n_states * 8 B over its sequences
 
+// the copy table of both grammar decoders staged in gram[5]; a grammar without copies stages one word (C = 0: no warp
+// walks, every sequence decodes to 0 words)
+static u32 *stage_copies(HostCall &c, const std::vector<u32> &copy) {
+    static const u32 kNoCopy = 0;
+    return c.in(c.h->gram[5], copy.empty() ? &kNoCopy : copy.data(), std::max<size_t>(copy.size(), 1) * 4);
+}
+
 // the grammar decoder (tag 10) over B sequences of frames N[b]: seq [B][3] holds each first feature row and its segments
 // (the record rows are filled in here). Launches take consecutive sequences whose records fit kGramRecBytes.
 static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &N, std::vector<u32> &seq,
@@ -1044,12 +1051,10 @@ static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &
         rows_max = std::max(rows_max, rows);
     }
     cut.push_back(B);
-    static const u32 kNoCopy = 0;                         // the one staged word of a grammar without copies (C = 0:
-    const u32 *ctab = copy.empty() ? &kNoCopy : copy.data();   // no warp walks, every sequence decodes to 0 words)
-    u32 *d_copy = c.in(h->gram[0], ctab, std::max<size_t>(copy.size(), 1) * 4);
-    u32 *d_seq = c.in(h->gram[1], seq.data(), (size_t)B * 12);
-    u32 *d_frm = c.in(h->gram[2], N.data(), (size_t)B * 4);
-    u64 *d_rec = c.ws<u64>(h->gram[3], std::max<size_t>(rows_max, 1) * S * 8);
+    u32 *d_copy = stage_copies(c, copy);
+    u32 *d_seq = c.in(h->gram[0], seq.data(), (size_t)B * 12);
+    u32 *d_frm = c.in(h->gram[1], N.data(), (size_t)B * 4);
+    u64 *d_rec = c.ws<u64>(h->gram[2], std::max<size_t>(rows_max, 1) * S * 8);
     const BankView &bk = h->bank;
     for (size_t k = 0; k + 1 < cut.size(); ++k) {
         const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
@@ -1321,12 +1326,10 @@ static void run_long_grammar(HostCall &c, const s16 *d_feat, std::vector<u32> &s
         rows_max = std::max(rows_max, rows);
     }
     cut.push_back(B);
-    static const u32 kNoCopy = 0;                         // as run_grammar: a grammar without copies stages one word
-    const u32 *ctab = copy.empty() ? &kNoCopy : copy.data();
-    u32 *d_copy = c.in(h->lgram[5], ctab, std::max<size_t>(copy.size(), 1) * 4);
-    u32 *d_seq = c.in(h->lgram[0], seq.data(), (size_t)B * 16);
-    u64 *recD = c.ws<u64>(h->lgram[2], std::max<size_t>(rows_max, 1) * S * 8);
-    u32 *recS = c.ws<u32>(h->lgram[3], std::max<size_t>(rows_max, 1) * S * 4);
+    u32 *d_copy = stage_copies(c, copy);
+    u32 *d_seq = c.in(h->gram[0], seq.data(), (size_t)B * 16);
+    u64 *recD = c.ws<u64>(h->gram[2], std::max<size_t>(rows_max, 1) * S * 8);
+    u32 *recS = c.ws<u32>(h->gram[3], std::max<size_t>(rows_max, 1) * S * 4);
     const BankView &bk = h->bank;
     for (size_t k = 0; k + 1 < cut.size(); ++k) {
         const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
@@ -1381,7 +1384,7 @@ int sr_connected_grammar_segs_batch(sr_handle *h, const int16_t *feat, const uin
     if (const int rc = gram_copies(h, g, copy)) return rc;
     HostCall c(h, "sr_connected_grammar_segs_batch");
     const s16 *d_feat = c.in(h->conn[3], feat, (size_t)rows * 24, 24);
-    u32 *tab = c.ws<u32>(h->lgram[1], std::max<size_t>(n_seg, 1) * 8);   // seg_row [n_seg] | seg_frm [n_seg]
+    u32 *tab = c.ws<u32>(h->gram[1], std::max<size_t>(n_seg, 1) * 8);   // seg_row [n_seg] | seg_frm [n_seg]
     if (tab) {
         c.h2d(tab, row.data(), (size_t)n_seg * 4);
         c.h2d(tab + n_seg, seg_frm, (size_t)n_seg * 4);
@@ -1422,7 +1425,7 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
     std::vector<u32> n_all(B), segv;
     std::vector<atap_tag> av;
     const int rc = long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) -> int {
-        u32 *d_seg = c.ws<u32>(h->lgram[4], (size_t)nb * cap * 8);
+        u32 *d_seg = c.ws<u32>(h->gram[4], (size_t)nb * cap * 8);
         if (c.rc) return 0;
         if (const int r = vad_long_impl(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, cap, d_atap + b0, d_n + b0, d_seg))
             return r;
@@ -1463,7 +1466,7 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
         const u32 ns = (u32)row.size();
         s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(rows, 1) * 24);
         run_pieces(c, dpcm, U, nb, pc, d_feat);
-        u32 *tab = c.ws<u32>(h->lgram[1], std::max<size_t>(ns, 1) * 8);   // seg_row [ns] | seg_frm [ns]
+        u32 *tab = c.ws<u32>(h->gram[1], std::max<size_t>(ns, 1) * 8);   // seg_row [ns] | seg_frm [ns]
         if (c.rc) return 0;
         c.h2d(tab, row.data(), (size_t)ns * 4);
         c.h2d(tab + ns, frm.data(), (size_t)ns * 4);

@@ -207,12 +207,12 @@ struct sr_handle {
     DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
     DevBuf align[6];                                   // sr_dtw_path_batch / sr_average_bank: pairs, paths, templates, scores
     DevBuf conn[10];                                   // long features and the connected-word decoder: pieces, features, words
-    DevBuf gram[4];                                    // the grammar decoder: copy table, sequence table, frame counts, records
     DevBuf lng[12];                                    // long-form VAD and recognition (sr_long.h): block summaries, segments,
                                                        // counts, the flat segment table, its atap, status, keys, features, lens
                                                        // and the host calls' device outputs
-    DevBuf lgram[6];                                   // the long-recording grammar decoder (sr_long_grammar.h): sequence table,
-                                                       // segment rows and frames, both record arrays, VAD segments of a group
+    DevBuf gram[6];                                    // both grammar decoders: sequence table, segment rows and frames (K6g: frame
+                                                       // counts), records (K13: both arrays), the long-form VAD segments of a
+                                                       // group, copy table
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };
