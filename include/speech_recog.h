@@ -164,14 +164,27 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
  * outside the band or the 2:1 length guard of DTW.C:133 rejects the pair. Every band_r >= 118 is the unconstrained DTW
  * over the whole matrix (feature sets have <= 119 frames). Parity unpinned: the reference has no DP; the checker is this
  * project's own CPU restatement. The explicit flags and band_r of sr_dtw_batch decide, never the handle's sr_set_match. */
+#define SR_DTW_SYM_P1     4u          /* use the symmetric slope-constrained DP of Sakoe & Chiba (extension, ABI version 10) */
+/* With SR_DTW_SYM_P1 (without SR_DTW_BAND: the two together fail before any launch and write nothing), band_r is any
+ * radius >= 0 and the band is SR_DTW_BAND's: cell (i, j) is in it iff |j - floor(i*M/I)| <= band_r, every band_r >= 118
+ * the whole matrix. With d(i,j) = get_dis(x_i, y_j) (DTW.C:45-62) and 0-based cells, g(0,0) = 2 d(0,0) and
+ *   g(i,j) = min(g(i-1,j-2) + 2 d(i,j-1) + d(i,j),  g(i-1,j-1) + 2 d(i,j),  g(i-2,j-1) + 2 d(i-1,j) + d(i,j)),
+ * the symmetric form with slope constraint P = 1 (Sakoe & Chiba 1978). A move counts only when its start cell is
+ * reachable and every cell it passes through (for a two-step move the intermediate cell and the end cell) lies inside the
+ * matrix and the band; any other cell is unreachable ((0,1), for one). Every complete path weighs exactly I + M, so the
+ * score g(I-1,M-1) / (I+M) (u32, truncating) is the weighted mean of get_dis along the path. SR_DIS_ERR when the end cell is
+ * unreachable, I or M is 0 or above 119, or the 2:1 length guard of DTW.C:133 rejects the pair; SR_DTW_CHECK_SIGN works
+ * as with the other matchers. Headroom: g <= (I+M) * 65 536 < 2^24 (get_dis can return 65 536), so 32-bit arithmetic is
+ * exact. Parity unpinned: the reference has no DP; the checker is this project's own CPU restatement. */
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                  uint32_t *score /* [B][n_slot] or NULL */, uint32_t *best_idx /* [B] or NULL */,
                  uint32_t *best_dis /* [B] or NULL */);
 /* The matcher of this handle's recognition calls: sr_recognise_batch, _dev, _dev_allgather, _multi and every streaming
  * push, each reading it when it starts. flags = 0: the reference's greedy walk (dtw, DTW.C:120-192), the default;
- * flags = SR_DTW_BAND: the banded DP above at radius band_r >= 0 (up to the full matrix). Recognition keeps honouring
- * save_sign (SR_DTW_CHECK_SIGN, main.c:283) either way. Any other flag bit or a negative band_r fails and leaves the
- * setting unchanged. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers;
+ * flags = SR_DTW_BAND: the banded DP above at radius band_r >= 0 (up to the full matrix); flags = SR_DTW_SYM_P1: the
+ * symmetric P = 1 DP above at radius band_r >= 0. Recognition keeps honouring save_sign (SR_DTW_CHECK_SIGN, main.c:283)
+ * under every matcher. Any other flag value (SR_DTW_SYM_P1 | SR_DTW_BAND among them) or a negative band_r fails and
+ * leaves the setting unchanged. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers;
  * the ranks of an all-gather cannot be checked without a collective, so every rank must set the same one. Enrolment,
  * sr_get_mdl_batch and the drop-in dtw() keep the greedy walk. */
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r);
@@ -478,7 +491,8 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
  * sr_average_bank that aligns), 8 sr_average_bank's template update, 9 the connected-word decoder (sr_connected_batch,
  * sr_recognise_connected_batch; their get_mfcc launches are tag 1), 10 the grammar decoder (sr_connected_grammar_batch,
  * sr_recognise_connected_grammar_batch; their get_mfcc launches are tag 1), 11 and 12 the long-form block and segment passes
- * (include/sr_long.h). max_records = 0 disables. */
+ * (include/sr_long.h), 14 dtw (the symmetric P = 1 DP, in sr_dtw_batch* and in recognise calls under the SR_DTW_SYM_P1
+ * matcher). max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);
 

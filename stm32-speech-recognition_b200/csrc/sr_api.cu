@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 9; }
+int sr_abi_version(void) { return 10; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -111,7 +111,7 @@ int sr_set_dtw_variant(sr_handle *h, int variant) {
 }
 
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
-    SR_REQUIRE(h, h && (flags == 0 || flags == SR_DTW_BAND) && band_r >= 0);
+    SR_REQUIRE(h, h && (flags == 0 || flags == SR_DTW_BAND || flags == SR_DTW_SYM_P1) && band_r >= 0);
     h->match_flags = flags;
     h->match_r = band_r;
     return 0;
@@ -180,7 +180,12 @@ int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
        TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
-       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13 };
+       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13, TAG_DTW_SYM = 14 };
+
+// the timing tag of the template scan under flags (launch_scan's choice)
+static int scan_tag(u32 flags) {
+    return (flags & SR_DTW_SYM_P1) ? TAG_DTW_SYM : (flags & SR_DTW_BAND) ? TAG_DTW_BAND : TAG_DTW;
+}
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
@@ -408,6 +413,7 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
                         uint32_t *score, uint32_t *best_idx, uint32_t *best_dis, uint32_t *cmd, const u8 *status) {
     SR_REQUIRE(h, h && (B == 0 || in));
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
+    SR_REQUIRE(h, !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)));
     if (B == 0) return 0;
     const bool want_best = best_idx || best_dis || cmd;
     u64 *best = nullptr;
@@ -418,9 +424,8 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
         SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, B, h->stream));
     }
     if (bank.n) {
-        const bool band = (flags & SR_DTW_BAND) != 0;
-        if (band) SR_REQUIRE(h, band_r >= 0);
-        SR_LAUNCH(h, band ? TAG_DTW_BAND : TAG_DTW, launch_scan(h, bank, in, B, flags, band_r, score, best, status));
+        if (flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) SR_REQUIRE(h, band_r >= 0);
+        SR_LAUNCH(h, scan_tag(flags), launch_scan(h, bank, in, B, flags, band_r, score, best, status));
     }
     if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
     return 0;
@@ -570,6 +575,7 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                  uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h && (B == 0 || in));
+    SR_REQUIRE(h, !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)));      // before any copy: nothing is written
     if (B == 0) return 0;
     HostCall c(h, "sr_dtw_batch");
     return dtw_host(c, h->bank, in, B, flags, band_r, score, best_idx, best_dis);
@@ -1187,7 +1193,7 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
     SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, M, h->stream));                               // main.c:276-278
     if (h->bank.n) {                                                   // main.c:279-291, save_sign honoured (main.c:283)
         const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags;
-        SR_LAUNCH(h, (flags & SR_DTW_BAND) ? TAG_DTW_BAND : TAG_DTW,
+        SR_LAUNCH(h, scan_tag(flags),
                   launch_scan(h, h->bank, ftr, M, flags, h->match_r, nullptr, best, status, n_flat));
     }
     SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, best, n_flat, M, rec, h->stream));   // main.c:292-294

@@ -502,6 +502,84 @@ dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const un
     });
 }
 
+// ---- K3s: the symmetric slope-constrained DP of Sakoe & Chiba (1978), P = 1 (EXTENSION, parity unpinned) -------------
+// g(0,0) = 2 d(0,0); g(i,j) = min(g(i-1,j-2) + 2 d(i,j-1) + d(i,j), g(i-1,j-1) + 2 d(i,j), g(i-2,j-1) + 2 d(i-1,j) + d(i,j))
+// over the band of dtw_wide_kernel. A move counts only when its start cell is reachable and the cells it passes through
+// (the intermediate cell of a two-step move, and its end) lie in the band; every complete path then weighs I + M, so
+// g(I-1, M-1) / (I + M) is a weighted mean of get_dis. Checked against tests/oracle_sym.c.
+// One WARP per pair, a whole ROW across the warp, lane l holding columns 4l .. 4l+3 as in dtw_wide_kernel. Row i reads
+// only rows i-1 and i-2 of g and row i-1 of d, so there is no in-row recurrence and no scan: a lane needs from the lane
+// before it g(i-1, 4l-1) and g(i-1, 4l-2) + 2 d(i, 4l-1) (two shuffles), and g(i-2, 4l-1) is the first of those from the
+// previous row. Cells outside the band, or past M, hold d = kSymInf; g is kept clamped to kSymInf. Every move sums at
+// most four terms of at most kSymInf = 2^26 (< 2^31), and a reachable g(i,j) <= (i + j + 2) * 65 536 <= 238 * 65 536 <
+// 2^24 < kSymInf, so a move is finite exactly when it is below kSymInf.
+constexpr s32 kSymInf = 1 << 26;
+
+__global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
+dtw_sym_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
+               u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
+               const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
+    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
+                   [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
+        const int j0 = lane * 4;
+        PRow b[4];
+        s32 g1[4], g2[4], dp[4];                                       // g(i-1, .), g(i-2, .), d(i-1, .) of the lane's columns
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            load_row(b[k], trow, kNrm119, j0 + k < M ? j0 + k : 0);
+            g1[k] = g2[k] = dp[k] = kSymInf;
+        }
+        s32 w1 = kSymInf;                                              // g(i-2, j0-1): last row's shuffle of g(i-1, j0-1)
+        for (int i = 0; i < I; ++i) {
+            const int c = (i * M) / I, lo = max(c - r, 0), hi = min(c + r, M - 1);
+            PRow a;
+            load_row(a, uslot, kNrm119, i);                            // broadcast read
+            s32 d[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int j = j0 + k;
+                d[k] = (j >= lo && j <= hi) ? (s32)pdist(a, b[k]) : kSymInf;
+            }
+            s32 v1 = __shfl_up_sync(0xFFFFFFFFu, g1[3], 1);                      // g(i-1, j0-1)
+            s32 v2 = __shfl_up_sync(0xFFFFFFFFu, g1[2] + 2 * d[3], 1);           // g(i-1, j0-2) + 2 d(i, j0-1)
+            if (lane == 0) v1 = v2 = kSymInf;
+            const s32 gd[4] = {v1, g1[0], g1[1], g1[2]};                                  // g(i-1, j-1)
+            const s32 ga[4] = {v2, v1 + 2 * d[0], g1[0] + 2 * d[1], g1[1] + 2 * d[2]};    // g(i-1, j-2) + 2 d(i, j-1)
+            const s32 gc[4] = {w1, g2[0], g2[1], g2[2]};                                  // g(i-2, j-1)
+            s32 g[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                s32 x = min(min(ga[k], gc[k] + 2 * dp[k]) + d[k], gd[k] + 2 * d[k]);
+                if (i == 0 && j0 + k == 0) x = 2 * d[0];
+                g[k] = d[k] < kSymInf ? min(x, kSymInf) : kSymInf;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { g2[k] = g1[k]; g1[k] = g[k]; dp[k] = d[k]; }
+            w1 = v1;
+        }
+        const s32 fin = dp_end(g1, (M - 1) & 3, (M - 1) / 4);
+        return fin < kSymInf ? (u32)fin / (u32)(I + M) : SR_DIS_ERR;
+    });
+}
+
+// the symmetric P = 1 DP at radius band_r >= 0: one kernel for every r, clamped to 118 as in launch_dtw_band
+cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
+                           u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev,
+                           const u32 *perm) {
+    if (B == 0 || T == 0) return cudaSuccess;
+    if (band_r < 0) return cudaErrorInvalidValue;
+    const int r = min(band_r, (int)kMaxFrm - 1);
+    const size_t smem = (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)kDtwWarps * kSlotBytes;
+    cudaError_t e = cudaFuncSetAttribute(dtw_sym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const u32 tiles = (T + kTileT - 1) / kTileT;
+    dim3 grid(tiles, grid_rows(num_sms, tiles, B, kDtwWarps));
+    dtw_sym_kernel<<<grid, kDtwWarps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
+                                                       static_cast<const unsigned char *>(bank), T, slot_stride, flags, r,
+                                                       score, best, status, B_dev, perm);
+    return cudaGetLastError();
+}
+
 // the banded DP of radius band_r >= 0, the kernel chosen from band_r alone: the thread form for r = 10, the warp-scan
 // form for the other r <= 15 (2r+1 lanes of one warp), the whole-row form for r >= 16. Every r >= 118 is the full matrix
 // (|j - c| <= 118 for any two columns), so r is clamped to 118 and no r reaches the kernels' c +- r.

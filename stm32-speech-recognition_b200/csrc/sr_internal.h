@@ -36,6 +36,9 @@ cudaError_t launch_dtw_dyn(const void *in_ftr, u32 B, const void *bank, u32 T, u
 cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
                             u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st,
                             const u32 *B_dev = nullptr, const u32 *perm = nullptr);
+cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
+                           u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st,
+                           const u32 *B_dev = nullptr, const u32 *perm = nullptr);
 cudaError_t launch_best_init(u64 *best, u32 B, cudaStream_t st);
 cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status,
                               cudaStream_t st);
@@ -195,7 +198,7 @@ struct sr_handle {
     u32 n_labels = 0, label_stride = 0;
     sr_comm *comm = nullptr;                           // the exchange step (sr_comm_create), optional
     int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cu), -1 default
-    u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk or SR_DTW_BAND
+    u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk, SR_DTW_BAND or SR_DTW_SYM_P1
     int match_r = 0;                                   // its band radius
     DevBuf mfcc_work;                                  // the same for mfcc_kernel (next utterance, CTAs finished)
     DevBuf vad_work;                                   // two words: dynamic utterance hand-out of vad_kernel (zeroed once, self re-arming)
@@ -288,18 +291,22 @@ inline cudaError_t launch_dtw_h(sr_handle *h, const BankView &bank, const void *
     return launch_dtw(in_ftr, B, bank.p, bank.n, bank.stride, flags, score, best, status, h->num_sms, h->stream, B_dev, bank.order);
 }
 
-// The template scan of B inputs against `bank` -- the one place a matcher becomes a kernel launch: with SR_DTW_BAND in
-// flags the banded DP of radius band_r (launch_dtw_band picks the kernel from r), else the greedy walk. sr_dtw_batch
-// passes its caller's flags and r; the recognition paths (recognise, streaming) pass the handle's matcher.
+// The template scan of B inputs against `bank` -- the one place a matcher becomes a kernel launch: with SR_DTW_SYM_P1 in
+// flags the symmetric P = 1 DP of radius band_r, with SR_DTW_BAND the banded DP of radius band_r (launch_dtw_band picks
+// the kernel from r), else the greedy walk. sr_dtw_batch passes its caller's flags and r; the recognition paths
+// (recognise, streaming) pass the handle's matcher. The callers refuse SR_DTW_SYM_P1 | SR_DTW_BAND.
 inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, int band_r,
                                u32 *score, u64 *best, const u8 *status, const u32 *B_dev = nullptr) {
+    if (flags & SR_DTW_SYM_P1)
+        return launch_dtw_sym(in_ftr, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, status, h->num_sms,
+                              h->stream, B_dev, bank.order);
     if (flags & SR_DTW_BAND)
         return launch_dtw_band(in_ftr, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, status, h->num_sms,
                                h->stream, B_dev, bank.order);
     return launch_dtw_h(h, bank, in_ftr, B, flags, score, best, status, B_dev);
 }
 
-// the two handles' recognition calls score alike: both greedy, or both the banded DP at the same radius
+// the two handles' recognition calls score alike: both greedy, or both the same DP at the same radius
 inline bool same_match(const sr_handle *a, const sr_handle *b) {
     return a->match_flags == b->match_flags && (a->match_flags == 0 || a->match_r == b->match_r);
 }

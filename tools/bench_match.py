@@ -1,12 +1,15 @@
-"""Recognition time under each template matcher: the reference's greedy walk and the banded DP (sr_set_match) at several
-radii, on BASELINE configs[1]'s shape (65 536 utterances x 1 s, 20 templates, synthetic PCM generated on the device).
+"""Recognition time under each template matcher: the reference's greedy walk, the banded DP and the symmetric P = 1 DP
+(sr_set_match) at several radii, on BASELINE configs[1]'s shape (65 536 utterances x 1 s, 20 templates, synthetic PCM
+generated on the device).
 
 Per matcher: W warm-up steps, then K steps of sr_recognise_batch_dev between CUDA events (ms/step), the DTW kernel's own
-time from the library's event pairs (sr_timing_*, tag 4 greedy / 6 banded), and lattice cells per second = the cells the
-oracle evaluates on a sample of utterances, scaled to the batch, over the DTW kernel time. r = 15 and r = 16 sit on either
-side of the kernel choice (warp-scan form / whole-row form) and are run alternately, several rounds. A sample of every
-matcher's outputs is checked against the oracle's own composition: its front end (recognise_pinned), its dtw_batch at the
-same matcher, the strict '<' first-wins argmin. The card's name, power limit and SM clock limit are read in the same run.
+time from the library's event pairs (sr_timing_*, tag 4 greedy / 6 banded / 14 symmetric), and lattice cells per second =
+the cells the banded oracle evaluates at the same radius on a sample of utterances, scaled to the batch, over the DTW kernel
+time. r = 15 and r = 16 sit on either side of the kernel choice (warp-scan form / whole-row form) and are run alternately,
+several rounds; the symmetric rows at r = 10, 16 and 118 alternate with the banded rows at the same radii. A sample of every
+matcher's outputs -- the first utterances of the launch and its last ones -- is checked against the oracle's own
+composition: its front end (recognise_pinned), its template scan under the same matcher (oracle_sym for the symmetric DP),
+the strict '<' first-wins argmin. The card's name, power limit and SM clock limit are read in the same run.
 
     python tools/bench_match.py [--steps 20] [--warmup 3] [--rounds 3] [--json FILE]
 """
@@ -23,6 +26,7 @@ sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python")
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import oracle_bind as ob  # noqa: E402
+import oracle_sym as osym  # noqa: E402
 import sr_b200  # noqa: E402
 
 U, N_LEN = 8000, 2400
@@ -47,7 +51,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=3, help="alternating rounds of r = 15 and r = 16")
-    ap.add_argument("--sample", type=int, default=256, help="utterances checked against the oracle")
+    ap.add_argument("--sample", type=int, default=256, help="first utterances checked against the oracle")
+    ap.add_argument("--tail", type=int, default=32, help="last utterances checked against the oracle")
     ap.add_argument("--json", default=None, help="also write the results to this file")
     args = ap.parse_args()
 
@@ -78,14 +83,22 @@ def main():
     h.set_bank_dev(bank.data_ptr(), T, 4096)
     ptrs = {k: v.data_ptr() for k, v in outs.items()}
 
-    # the oracle's composition on the sample: the front end once, the template scan per matcher
+    # the oracle's composition on the sample (the first n utterances and the last `tail`): the front end once, the
+    # template scan per matcher
     bank_h = bank.cpu().numpy()
-    front = ob.recognise_pinned(ob.best_oracle(), sr_b200.synth_pcm_host(n, U, SEED), N_LEN, None, 0, 4096)
+    tail = min(args.tail, B - n)
+    rows = np.concatenate([np.arange(n), np.arange(B - tail, B)])
+    sample_pcm = pcm[torch.from_numpy(rows).to(dev)].cpu().numpy().view(np.uint16)
+    front = ob.recognise_pinned(ob.best_oracle(), sample_pcm, N_LEN, None, 0, 4096)
     good = front["status"] == 0
+    SYM = sr_b200.DTW_SYM_P1
 
     def oracle(flags, r):
+        nth = os.cpu_count() or 1
         sc, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1,
-                                        band_r=r if flags else -1, nthreads=os.cpu_count() or 1)
+                                        band_r=r if flags else -1, nthreads=nth)
+        if flags == SYM:                    # the symmetric DP's scores; cells: the banded DP's at the same radius
+            sc = osym.sym_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
         return sc, cells
 
     def run(flags, r):
@@ -104,11 +117,12 @@ def main():
         stream.synchronize()
         recs = h.timing_collect()
         h.timing_enable(0)
-        tag = 6 if flags else 4
+        tag = 14 if flags == SYM else 6 if flags else 4
         dtw_ms = [ms for t, ms in recs if t == tag]
         assert len(dtw_ms) == args.steps, (flags, r, len(dtw_ms))
         # outputs of the last step against the oracle on the sample
-        got = {k: outs[k][:n].cpu().numpy() for k in ("score", "best_idx", "best_dis", "cmd", "status")}
+        idx = torch.from_numpy(rows).to(dev)
+        got = {k: outs[k][idx].cpu().numpy() for k in ("score", "best_idx", "best_dis", "cmd", "status")}
         got["score"] = got["score"].view(np.uint32)
         sc, cells = oracle(flags, r)
         i = np.argmin(sc, axis=1)
@@ -116,8 +130,8 @@ def main():
               and np.array_equal(got["best_idx"][good].view(np.uint32), i)
               and np.array_equal(got["best_dis"][good].view(np.uint32), sc[np.arange(len(i)), i])
               and np.array_equal(got["cmd"][good].view(np.uint32), i // 4))
-        cells_batch = cells * B / n
-        return {"matcher": "greedy" if not flags else "band", "r": r if flags else None,
+        cells_batch = cells * B / len(rows)
+        return {"matcher": "greedy" if not flags else "sym" if flags == SYM else "band", "r": r if flags else None,
                 "ms_per_step": ev0.elapsed_time(ev1) / args.steps,
                 "dtw_ms_mean": float(np.mean(dtw_ms)), "dtw_ms_min": float(np.min(dtw_ms)), "dtw_ms_max": float(np.max(dtw_ms)),
                 "oracle_cells_per_step": cells_batch, "cells_per_s": cells_batch / (float(np.mean(dtw_ms)) * 1e-3),
@@ -125,10 +139,11 @@ def main():
 
     band = sr_b200.DTW_BAND
     plan = [(0, 0), (band, 10)] + [(band, r) for _ in range(args.rounds) for r in (15, 16)] + [(band, 32), (band, 118), (0, 0)]
+    plan += [(f, r) for _ in range(args.rounds) for r in (10, 16, 118) for f in (band, SYM)]
     results = [run(f, r) for f, r in plan]
     h.set_match(0, 0)
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "batch": B, "templates": T,
-            "steps": args.steps, "warmup": args.warmup, "sample": n, "sample_ok_utterances": int(good.sum()),
+            "steps": args.steps, "warmup": args.warmup, "sample": n, "tail": tail, "sample_ok_utterances": int(good.sum()),
             "results": results}
     print("card: %s, power limit %s, max SM clock %s" % (info["card"].get("name"), info["card"].get("power.limit"),
                                                         info["card"].get("clocks.max.sm")))
