@@ -176,15 +176,28 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
  * unreachable, I or M is 0 or above 119, or the 2:1 length guard of DTW.C:133 rejects the pair; SR_DTW_CHECK_SIGN works
  * as with the other matchers. Headroom: g <= (I+M) * 65 536 < 2^24 (get_dis can return 65 536), so 32-bit arithmetic is
  * exact. Parity unpinned: the reference has no DP; the checker is this project's own CPU restatement. */
+#define SR_DTW_ANY_RATE   8u          /* SR_DTW_BAND without the 2:1 length guard (extension, ABI version 11) */
+/* SR_DTW_BAND | SR_DTW_ANY_RATE (optionally | SR_DTW_CHECK_SIGN) is the SR_DTW_BAND DP above exactly -- the same band
+ * |j - floor(i*M/I)| <= band_r, recurrence and score D(I-1,M-1) / (I+M) -- except that the 2:1 length guard of DTW.C:133
+ * is not applied, so an utterance spoken at twice or half a template's rate (or faster, or slower) is still scored.
+ * SR_DIS_ERR when I or M is 0 or above 119, or when the end cell lies outside the band: for M > I it is ceil(M/I) - 1
+ * columns past the band centre of the last row, so a narrow band still rejects extreme ratios, and every band_r >= 118
+ * scores every pair of 1..119 frames on both sides. A pair within the guard scores bit for bit what SR_DTW_BAND gives it
+ * at the same band_r. SR_DTW_ANY_RATE without SR_DTW_BAND, or with SR_DTW_SYM_P1, fails before any launch and writes
+ * nothing. The symmetric P = 1 DP keeps its guard: its slope constraint cannot reach an end cell past 2:1 anyway.
+ * Parity unpinned: the reference has no DP; the checker is this project's own CPU restatement. */
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                  uint32_t *score /* [B][n_slot] or NULL */, uint32_t *best_idx /* [B] or NULL */,
                  uint32_t *best_dis /* [B] or NULL */);
 /* The matcher of this handle's recognition calls: sr_recognise_batch, _dev, _dev_allgather, _multi and every streaming
  * push, each reading it when it starts. flags = 0: the reference's greedy walk (dtw, DTW.C:120-192), the default;
- * flags = SR_DTW_BAND: the banded DP above at radius band_r >= 0 (up to the full matrix); flags = SR_DTW_SYM_P1: the
+ * flags = SR_DTW_BAND: the banded DP above at radius band_r >= 0 (up to the full matrix); flags = SR_DTW_BAND |
+ * SR_DTW_ANY_RATE: the same DP without the 2:1 length guard; flags = SR_DTW_SYM_P1: the
  * symmetric P = 1 DP above at radius band_r >= 0. Recognition keeps honouring save_sign (SR_DTW_CHECK_SIGN, main.c:283)
- * under every matcher. Any other flag value (SR_DTW_SYM_P1 | SR_DTW_BAND among them) or a negative band_r fails and
- * leaves the setting unchanged. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers;
+ * under every matcher. Any other flag value (SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE alone among them) or a
+ * negative band_r fails and leaves the setting unchanged. sr_get_match returns the flags as set, SR_DTW_ANY_RATE
+ * included. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers (with
+ * and without SR_DTW_ANY_RATE differ);
  * the ranks of an all-gather cannot be checked without a collective, so every rank must set the same one. Enrolment,
  * sr_get_mdl_batch and the drop-in dtw() keep the greedy walk. */
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r);

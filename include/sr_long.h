@@ -18,7 +18,8 @@
  * Per-segment decision: spch_recg's decision (main.c:276-295) applied to every segment.
  *  - get_mfcc on [start, end) with vv_frm_max = 119, in the handle's geometry (sr_set_geometry). x[-1] is the real
  *    preceding sample, except that a segment at sample 0 reads mid_val, as in every batched call.
- *  - Then the handle's matcher (sr_set_match: the greedy walk, SR_DTW_BAND or SR_DTW_SYM_P1) against the bank, the
+ *  - Then the handle's matcher (sr_set_match: the greedy walk, SR_DTW_BAND with or without SR_DTW_ANY_RATE, or
+ *    SR_DTW_SYM_P1) against the bank, the
  *    strict-'<' first-wins argmin, and
  *    cmd = idx / SR_FTR_PER_COMM.
  *  - Status: SR_ST_VAD_FAIL for an unclosed segment, SR_ST_MFCC_FAIL for 0 frames (which includes segments over 119

@@ -15,7 +15,7 @@
  *        SR_SEG_NULL when it has none, and n_closed is the number of its closed records;
  *      * atap is the call's atap.
  *    The batch call is taken with the same n_len and the same initial atap, under the handle's geometry, matcher (any of
- *    sr_set_match's, SR_DTW_SYM_P1 included) and bank as they were at the push that closed each segment.
+ *    sr_set_match's, SR_DTW_BAND | SR_DTW_ANY_RATE and SR_DTW_SYM_P1 included) and bank as they were at the push that closed each segment.
  *  - Frame rule: frame k (samples 80k .. 80k + 159) is evaluated once n > 80k + 160, the long-form VAD's
  *    "i < len - 160". A segment [start, end) is therefore reported by the push after which n >= end + 881. This is one
  *    sample later than sr_streams_*, which reports a segment once n >= end + 880 (its frames run to the capture's end).

@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 10; }
+int sr_abi_version(void) { return 11; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -111,7 +111,8 @@ int sr_set_dtw_variant(sr_handle *h, int variant) {
 }
 
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
-    SR_REQUIRE(h, h && (flags == 0 || flags == SR_DTW_BAND || flags == SR_DTW_SYM_P1) && band_r >= 0);
+    SR_REQUIRE(h, h && (flags == 0 || flags == SR_DTW_BAND || flags == (SR_DTW_BAND | SR_DTW_ANY_RATE) ||
+                        flags == SR_DTW_SYM_P1) && band_r >= 0);
     h->match_flags = flags;
     h->match_r = band_r;
     return 0;
@@ -185,6 +186,11 @@ enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT =
 // the timing tag of the template scan under flags (launch_scan's choice)
 static int scan_tag(u32 flags) {
     return (flags & SR_DTW_SYM_P1) ? TAG_DTW_SYM : (flags & SR_DTW_BAND) ? TAG_DTW_BAND : TAG_DTW;
+}
+// the matcher bits of sr_dtw_batch* name one matcher: not SR_DTW_SYM_P1 with SR_DTW_BAND, and SR_DTW_ANY_RATE only
+// as a modifier of SR_DTW_BAND
+static bool scan_flags_ok(u32 flags) {
+    return !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)) && (!(flags & SR_DTW_ANY_RATE) || (flags & SR_DTW_BAND));
 }
 
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
@@ -413,7 +419,7 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
                         uint32_t *score, uint32_t *best_idx, uint32_t *best_dis, uint32_t *cmd, const u8 *status) {
     SR_REQUIRE(h, h && (B == 0 || in));
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
-    SR_REQUIRE(h, !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)));
+    SR_REQUIRE(h, scan_flags_ok(flags));
     if (B == 0) return 0;
     const bool want_best = best_idx || best_dis || cmd;
     u64 *best = nullptr;
@@ -575,8 +581,9 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                  uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h && (B == 0 || in));
-    SR_REQUIRE(h, !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)));      // before any copy: nothing is written
+    SR_REQUIRE(h, scan_flags_ok(flags));                                     // before any copy: nothing is written
     if (B == 0) return 0;
+    if (h->bank.n && (flags & (SR_DTW_BAND | SR_DTW_SYM_P1))) SR_REQUIRE(h, band_r >= 0);   // dtw_dev_impl's radius rule
     HostCall c(h, "sr_dtw_batch");
     return dtw_host(c, h->bank, in, B, flags, band_r, score, best_idx, best_dis);
 }

@@ -25,12 +25,12 @@ __device__ __forceinline__ void group_barrier(int id, int nthreads) {
 // The lane-packed tile scan of dtw_kernel and dtw_band_thread_kernel. A CTA stages a tile of Tt <= 32 templates; its
 // warps, in G groups of Wg, stage NU utterances at a time, and each lane of a group scores one fixed (utterance slot,
 // template) pair of the NU x Tt (flattened), so lanes stay busy when Tt < 32. pair(I, M, urow, trow) scores a pair
-// that passed pair_walks.
+// that passed pair_walks(guard).
 template <class Pair>
 __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
                                                  u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status, int Wg,
                                                  int NU, int G, u32 tile0, int tslots, const u32 *B_dev, const u32 *perm,
-                                                 Pair pair) {
+                                                 bool guard, Pair pair) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     if (B_dev) B = min(B, *B_dev);
     if (B == 0) return;
@@ -72,7 +72,7 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
         const u32 u = ubase + (u32)ul;
         if (lane_has_pair && u < B) {
             const u32 Iraw = gfrm[ul];
-            const u32 result = pair_walks(Iraw, Mraw) ? pair((int)Iraw, (int)Mraw, gslots + (size_t)ul * kSlotBytes, trow)
+            const u32 result = pair_walks(Iraw, Mraw, guard) ? pair((int)Iraw, (int)Mraw, gslots + (size_t)ul * kSlotBytes, trow)
                                                       : SR_DIS_ERR;
             const u32 t = perm ? tfrm[kTileT + tl] : t0 + (u32)tl;   // the original slot number: score column, argmin key
             emit_pair(score, best, T, u, t, result);
@@ -90,7 +90,7 @@ dtw_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char 
            const u32 *__restrict__ perm /* optional: bank slots in ascending frm_num order (templates of a tile then have
                                            similar walk lengths); results are indexed by the ORIGINAL slot number */) {
     lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
-                     [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+                     true, [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
                          PRow i0, i1, m0, m1;
                          u32 dis, steps;
                          int X1, X2, x, y, ya0, yb0, ya1, yb1;
@@ -303,7 +303,10 @@ cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStre
 // ---- K3: Sakoe-Chiba banded DP (EXTENSION: not in the reference, whose dtw() is the greedy walk above;
 // BASELINE.json configs[2] names it; checked against our own CPU DP oracle sro_dtw_band -- parity unpinned
 // by the reference). D(i,j) = d(i,j) + min(D(i-1,j), D(i,j-1), D(i-1,j-1)), band |j - floor(i*M/I)| <= r,
-// local distance = get_dis, result D(I-1,M-1)/(I+M), same 2:1 length guard as DTW.C:133.
+// local distance = get_dis, result D(I-1,M-1)/(I+M), same 2:1 length guard as DTW.C:133 unless flags has
+// SR_DTW_ANY_RATE. Without the guard the band centre c = floor(i*M/I) moves by up to 118 columns per row (M > 2I), not
+// 0..2, and stays put for several rows when M < I/2; every kernel below takes any shift, and a shift past 2r + 1 leaves
+// the new row unreachable.
 // Three kernels, chosen from r alone (launch_dtw_band): dtw_band_thread_kernel<10> for r = 10, dtw_band_kernel for the
 // other r <= 15, dtw_wide_kernel for r >= 16 up to the full matrix. On the recognition path all three take the
 // per-utterance status gate, a batch size produced on the device (streaming) and the bank order; scores and argmin keys
@@ -318,12 +321,13 @@ constexpr s32 kInf = 0x3FFFFFFF;
 // The warp-per-pair tile scan of dtw_band_kernel and dtw_wide_kernel. A CTA stages a tile of Tt <= 32 templates (bank
 // slot perm[t] when a bank order is given); each warp stages one utterance at a time and scores it against the Tt
 // templates one after another, the whole warp on one cost matrix: pair(I, M, urow, trow, lane) returns, in every lane, the
-// score of a pair that passed pair_walks. Lane tt keeps the score of template tt; one score row and one atomicMin of the
-// warp's smallest key per utterance. An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in lane_packed_scan.
+// score of a pair that passed pair_walks(guard). Lane tt keeps the score of template tt; one score row and one atomicMin
+// of the warp's smallest key per utterance. An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in
+// lane_packed_scan.
 template <class Pair>
 __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
                                                u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status,
-                                               const u32 *B_dev, const u32 *perm, Pair pair) {
+                                               const u32 *B_dev, const u32 *perm, bool guard, Pair pair) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     if (B_dev) B = min(B, *B_dev);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -345,7 +349,7 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
         for (int tt = 0; tt < Tt; ++tt) {
             const u32 Mraw = tfrm[tt];
             u32 result = SR_DIS_ERR;
-            if (Iraw >= 1 && pair_walks(Iraw, Mraw))
+            if (Iraw >= 1 && pair_walks(Iraw, Mraw, guard))
                 result = pair((int)Iraw, (int)Mraw, uslot, tile + (size_t)tt * kSlotBytes, lane);
             if (lane == tt) my_result = result;
         }
@@ -365,7 +369,9 @@ __global__ void __launch_bounds__(kDtwWarps * 32)
 dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                 u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                 const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
+    // the previous row's cell of column j sits in lane j - (cprev - r): up and diag come from lanes lane + sft and
+    // lane + sft - 1, and any lane past 31 or past 2r (those hold kInf) is out of the previous row's band, whatever sft is
+    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         s32 Dprev = kInf;
         int cprev = 0;
@@ -412,7 +418,7 @@ __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (sh
 dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                 u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                 const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
+    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         const int j0 = lane * 4;
         PRow b[4];
@@ -441,8 +447,10 @@ dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 // ---- K3b: the same banded DP, one THREAD per pair, band in registers (compile-time radius) -----------------------
 // 3.7x fewer issue slots per lattice cell than the warp-scan form: no scans, no idle lanes (21 of 32), and the
 // lane-packed tile scan of dtw_kernel. The band of row i sits at columns c_i-R..c_i+R with
-// c_i = floor(i*M/I); it slides by s = c_i - c_{i-1} in {0,1,2} per row, realised as two predicated shift-by-one
-// passes over the register array (no divergence between lanes whose templates have different lengths).
+// c_i = floor(i*M/I); it slides by s = c_i - c_{i-1} in {0,1,2} per row under the 2:1 guard, realised as two
+// predicated shift-by-one passes over the register array (no divergence between lanes whose templates have different
+// lengths). Under SR_DTW_ANY_RATE a row may slide further (M > 2I): those rows take a loop of min(s, W) - 2 more passes
+// after the two, so the passes of a pair total at most M - 1, and a slide past W leaves no cell of the old row.
 template <int R>
 __global__ void __launch_bounds__(kK2Warps * 32)
 dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
@@ -450,23 +458,33 @@ dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const un
                        const u8 *__restrict__ status, int Wg, int NU, int G, u32 tile0, int tslots,
                        const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
     lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
-                     [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+                     !(flags & SR_DTW_ANY_RATE), [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
         constexpr int W = 2 * R + 1;
-        if (I == 0) return SR_DIS_ERR;                     // empty feature sets (M == 0 too, by the 2:1 guard): no cell
+        if (I == 0 || M == 0) return SR_DIS_ERR;           // empty feature sets: no cell
         s32 D[W];
 #pragma unroll
         for (int k = 0; k < W; ++k) D[k] = kInf;
         int c = 0, cprev = 0, err = 0;                     // c = floor(i*M/I) kept incrementally: i*M = c*I + err
         for (int i = 0; i < I; ++i) {
-            const int sft = c - cprev;                     // 0, 1 or 2 (M <= 2I)
+            const int sft = c - cprev;                     // 0, 1 or 2 when M <= 2I; up to M - 1 otherwise
             // diag source of cell k=0 is the old element at index sft-1
             s32 dm1 = sft == 2 ? D[1] : (sft == 1 ? D[0] : kInf);
+            if (sft > 2) {                                 // only without the 2:1 guard
+                dm1 = kInf;
+#pragma unroll
+                for (int k = 2; k < W; ++k) if (k == sft - 1) dm1 = D[k];
+            }
             if (sft >= 1) {
 #pragma unroll
                 for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
                 D[W - 1] = kInf;
             }
             if (sft >= 2) {
+#pragma unroll
+                for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
+                D[W - 1] = kInf;
+            }
+            for (int s = 2; s < min(sft, W); ++s) {        // only without the 2:1 guard
 #pragma unroll
                 for (int k = 0; k < W - 1; ++k) D[k] = D[k + 1];
                 D[W - 1] = kInf;
@@ -493,6 +511,7 @@ dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const un
             err += M;                                      // advance c to floor((i+1)*M/I)
             if (err >= I) { err -= I; ++c; }
             if (err >= I) { err -= I; ++c; }
+            if (err >= I) { c += err / I; err %= I; }      // only without the 2:1 guard (M > 2I)
         }
         const int kend = (M - 1) - (cprev - R);            // cell holding column M-1 in the last row
         s32 fin = kInf;
@@ -519,7 +538,7 @@ __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (sh
 dtw_sym_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm,
+    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, true,
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         const int j0 = lane * 4;
         PRow b[4];

@@ -82,10 +82,12 @@ __device__ __forceinline__ u32 decode_frm(u32 hdr, u32 flags) {
 // rows to stage: the greedy do-while may touch row frm, and rows 0 and 1 are always read (DTW.C:146-160), also when
 // frm_num == 0. The banded DP reads rows [0, frm) only.
 __device__ __forceinline__ int staged_rows(u32 frm) { return frm == kNoWalk ? 0 : (int)min(max(frm + 1u, 2u), kMaxFrm); }
-// both sides walkable and within the 2:1 length ratio (DTW.C:133)
-__device__ __forceinline__ bool pair_walks(u32 Iraw, u32 Mraw) {
+// both sides walkable and, with guard, within the 2:1 length ratio (DTW.C:133). Without it (the banded DP under
+// SR_DTW_ANY_RATE) both sides must have at least one frame, which the guard implies for all but the 0:0 pair.
+__device__ __forceinline__ bool pair_walks(u32 Iraw, u32 Mraw, bool guard) {
     const int I = (int)Iraw, M = (int)Mraw;
-    return Iraw != kNoWalk && Mraw != kNoWalk && !(I > M * 2 || 2 * I < M);
+    if (Iraw == kNoWalk || Mraw == kNoWalk) return false;
+    return guard ? !(I > M * 2 || 2 * I < M) : (I >= 1 && M >= 1);
 }
 
 // stage bank templates t0 .. t0+Tt-1 (bank slot perm[t] when a bank order is given) into tile slots of slot_bytes each:

@@ -152,7 +152,7 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
                 pending = false;
                 out_u = blockIdx.y + pend_seq * gridDim.y; out_t = c.tslot_id[pend_tl];
                 const u32 Iraw = c.ufrm[slot], Mraw = c.tfrm[pend_tl];
-                if (!pair_walks(Iraw, Mraw)) finish(SR_DIS_ERR);
+                if (!pair_walks(Iraw, Mraw, true)) finish(SR_DIS_ERR);
                 else {
                     urow = ring + slot * uslot; trow = tile + pend_tl * tslot;
                     I = (int)Iraw; M = (int)Mraw;

@@ -198,7 +198,7 @@ struct sr_handle {
     u32 n_labels = 0, label_stride = 0;
     sr_comm *comm = nullptr;                           // the exchange step (sr_comm_create), optional
     int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cu), -1 default
-    u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk, SR_DTW_BAND or SR_DTW_SYM_P1
+    u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk, SR_DTW_BAND (| SR_DTW_ANY_RATE) or SR_DTW_SYM_P1
     int match_r = 0;                                   // its band radius
     DevBuf mfcc_work;                                  // the same for mfcc_kernel (next utterance, CTAs finished)
     DevBuf vad_work;                                   // two words: dynamic utterance hand-out of vad_kernel (zeroed once, self re-arming)
@@ -293,8 +293,9 @@ inline cudaError_t launch_dtw_h(sr_handle *h, const BankView &bank, const void *
 
 // The template scan of B inputs against `bank` -- the one place a matcher becomes a kernel launch: with SR_DTW_SYM_P1 in
 // flags the symmetric P = 1 DP of radius band_r, with SR_DTW_BAND the banded DP of radius band_r (launch_dtw_band picks
-// the kernel from r), else the greedy walk. sr_dtw_batch passes its caller's flags and r; the recognition paths
-// (recognise, streaming) pass the handle's matcher. The callers refuse SR_DTW_SYM_P1 | SR_DTW_BAND.
+// the kernel from r; its kernels read SR_DTW_ANY_RATE from flags and then skip the 2:1 guard), else the greedy walk.
+// sr_dtw_batch passes its caller's flags and r; the recognition paths (recognise, streaming) pass the handle's matcher.
+// The callers refuse SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE without SR_DTW_BAND.
 inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, int band_r,
                                u32 *score, u64 *best, const u8 *status, const u32 *B_dev = nullptr) {
     if (flags & SR_DTW_SYM_P1)
@@ -306,7 +307,8 @@ inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *i
     return launch_dtw_h(h, bank, in_ftr, B, flags, score, best, status, B_dev);
 }
 
-// the two handles' recognition calls score alike: both greedy, or both the same DP at the same radius
+// the two handles' recognition calls score alike: both greedy, or both the same DP (SR_DTW_ANY_RATE included) at the
+// same radius
 inline bool same_match(const sr_handle *a, const sr_handle *b) {
     return a->match_flags == b->match_flags && (a->match_flags == 0 || a->match_r == b->match_r);
 }

@@ -18,7 +18,7 @@ FTR_BYTES = 2860
 SEG_NULL = 0xFFFFFFFF
 DIS_ERR = 0xFFFFFFFF
 SAVE_MASK = 12345
-DTW_CHECK_SIGN, DTW_BAND, DTW_SYM_P1 = 1, 2, 4
+DTW_CHECK_SIGN, DTW_BAND, DTW_SYM_P1, DTW_ANY_RATE = 1, 2, 4, 8
 PATH_MAX = 237                 # SR_PATH_MAX: the longest warping path, 2 * VV_FRM_MAX - 1 points
 
 ATAP_DTYPE = np.dtype([("mid_val", "<u4"), ("n_thl", "<u2"), ("z_thl", "<u2"), ("s_thl", "<u4")])
@@ -358,8 +358,9 @@ class Handle:
         return ftr
 
     def dtw(self, ftr_in, flags=0, band_r=0, want_score=True, want_best=True):
-        """every input against the bank (sr_dtw_batch): flags 0 = the greedy walk, DTW_BAND = the banded DP, DTW_SYM_P1 =
-        the symmetric P = 1 DP, at radius band_r, each optionally | DTW_CHECK_SIGN -> (score [B, n_slot], best_idx [B],
+        """every input against the bank (sr_dtw_batch): flags 0 = the greedy walk, DTW_BAND = the banded DP (| DTW_ANY_RATE:
+        without the 2:1 length guard), DTW_SYM_P1 = the symmetric P = 1 DP, at radius band_r, each optionally |
+        DTW_CHECK_SIGN -> (score [B, n_slot], best_idx [B],
         best_dis [B]), None where not wanted"""
         B = ftr_in.shape[0]
         score = np.zeros((B, self.n_slot), np.uint32) if want_score else None
@@ -614,7 +615,7 @@ class Handle:
 
     def set_match(self, flags, band_r=0):
         """matcher of the recognition calls: 0 = the reference's greedy walk, DTW_BAND = the banded DP at radius band_r,
-        DTW_SYM_P1 = the symmetric slope-constrained (P = 1) DP at radius band_r"""
+        DTW_BAND | DTW_ANY_RATE = the same DP without the 2:1 length guard, DTW_SYM_P1 = the symmetric slope-constrained (P = 1) DP at radius band_r"""
         self._ck(lib().sr_set_match(self._h, int(flags), int(band_r)))
 
     def match(self):

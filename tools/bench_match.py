@@ -1,14 +1,17 @@
-"""Recognition time under each template matcher: the reference's greedy walk, the banded DP and the symmetric P = 1 DP
-(sr_set_match) at several radii, on BASELINE configs[1]'s shape (65 536 utterances x 1 s, 20 templates, synthetic PCM
+"""Recognition time under each template matcher: the reference's greedy walk, the banded DP with and without the 2:1
+length guard (SR_DTW_ANY_RATE) and the symmetric P = 1 DP (sr_set_match) at several radii, on BASELINE configs[1]'s shape (65 536 utterances x 1 s, 20 templates, synthetic PCM
 generated on the device).
 
 Per matcher: W warm-up steps, then K steps of sr_recognise_batch_dev between CUDA events (ms/step), the DTW kernel's own
 time from the library's event pairs (sr_timing_*, tag 4 greedy / 6 banded / 14 symmetric), and lattice cells per second =
 the cells the banded oracle evaluates at the same radius on a sample of utterances, scaled to the batch, over the DTW kernel
 time. r = 15 and r = 16 sit on either side of the kernel choice (warp-scan form / whole-row form) and are run alternately,
-several rounds; the symmetric rows at r = 10, 16 and 118 alternate with the banded rows at the same radii. A sample of every
+several rounds; the symmetric rows and the banded rows without the guard at r = 10, 16 and 118 alternate with the banded
+rows at the same radii. The cells of those rows are the guarded banded DP's, so their cells per second compare the same
+work. A sample of every
 matcher's outputs -- the first utterances of the launch and its last ones -- is checked against the oracle's own
-composition: its front end (recognise_pinned), its template scan under the same matcher (oracle_sym for the symmetric DP),
+composition: its front end (recognise_pinned), its template scan under the same matcher (oracle_sym for the symmetric DP,
+oracle_rate for the banded DP without the guard),
 the strict '<' first-wins argmin. The card's name, power limit and SM clock limit are read in the same run.
 
     python tools/bench_match.py [--steps 20] [--warmup 3] [--rounds 3] [--json FILE]
@@ -26,6 +29,7 @@ sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python")
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import oracle_bind as ob  # noqa: E402
+import oracle_rate as orate  # noqa: E402
 import oracle_sym as osym  # noqa: E402
 import sr_b200  # noqa: E402
 
@@ -92,6 +96,7 @@ def main():
     front = ob.recognise_pinned(ob.best_oracle(), sample_pcm, N_LEN, None, 0, 4096)
     good = front["status"] == 0
     SYM = sr_b200.DTW_SYM_P1
+    RATE = sr_b200.DTW_BAND | sr_b200.DTW_ANY_RATE
 
     def oracle(flags, r):
         nth = os.cpu_count() or 1
@@ -99,6 +104,8 @@ def main():
                                         band_r=r if flags else -1, nthreads=nth)
         if flags == SYM:                    # the symmetric DP's scores; cells: the banded DP's at the same radius
             sc = osym.sym_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
+        if flags == RATE:                   # without the 2:1 guard; cells as above
+            sc = orate.rate_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
         return sc, cells
 
     def run(flags, r):
@@ -131,7 +138,8 @@ def main():
               and np.array_equal(got["best_dis"][good].view(np.uint32), sc[np.arange(len(i)), i])
               and np.array_equal(got["cmd"][good].view(np.uint32), i // 4))
         cells_batch = cells * B / len(rows)
-        return {"matcher": "greedy" if not flags else "sym" if flags == SYM else "band", "r": r if flags else None,
+        name = "greedy" if not flags else "sym" if flags == SYM else "band-any" if flags == RATE else "band"
+        return {"matcher": name, "r": r if flags else None,
                 "ms_per_step": ev0.elapsed_time(ev1) / args.steps,
                 "dtw_ms_mean": float(np.mean(dtw_ms)), "dtw_ms_min": float(np.min(dtw_ms)), "dtw_ms_max": float(np.max(dtw_ms)),
                 "oracle_cells_per_step": cells_batch, "cells_per_s": cells_batch / (float(np.mean(dtw_ms)) * 1e-3),
@@ -139,7 +147,7 @@ def main():
 
     band = sr_b200.DTW_BAND
     plan = [(0, 0), (band, 10)] + [(band, r) for _ in range(args.rounds) for r in (15, 16)] + [(band, 32), (band, 118), (0, 0)]
-    plan += [(f, r) for _ in range(args.rounds) for r in (10, 16, 118) for f in (band, SYM)]
+    plan += [(f, r) for _ in range(args.rounds) for r in (10, 16, 118) for f in (band, SYM, RATE)]
     results = [run(f, r) for f, r in plan]
     h.set_match(0, 0)
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "batch": B, "templates": T,
@@ -147,9 +155,9 @@ def main():
             "results": results}
     print("card: %s, power limit %s, max SM clock %s" % (info["card"].get("name"), info["card"].get("power.limit"),
                                                         info["card"].get("clocks.max.sm")))
-    print("%-8s %5s %10s %12s %22s %10s %6s" % ("matcher", "r", "ms/step", "dtw ms mean", "dtw ms min-max", "Gcells/s", "oracle"))
+    print("%-9s %5s %10s %12s %22s %10s %6s" % ("matcher", "r", "ms/step", "dtw ms mean", "dtw ms min-max", "Gcells/s", "oracle"))
     for x in results:
-        print("%-8s %5s %10.3f %12.3f %10.3f-%-11.3f %10.2f %6s" % (
+        print("%-9s %5s %10.3f %12.3f %10.3f-%-11.3f %10.2f %6s" % (
             x["matcher"], "" if x["r"] is None else x["r"], x["ms_per_step"], x["dtw_ms_mean"], x["dtw_ms_min"],
             x["dtw_ms_max"], x["cells_per_s"] / 1e9, x["sample_equals_oracle"]))
     print(json.dumps(info))
