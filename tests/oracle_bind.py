@@ -213,14 +213,22 @@ class RefOracle(_Base):
         return out
 
 
+def segment_rows(pcm, atap, segs):
+    """get_mfcc rows of (b, start, end) segments of pcm [B, U], [x[-1], samples]: x[-1] is the sample before the segment,
+    or the recording's mid_val (as a 16-bit sample) for a segment that starts at sample 0; zeros past the segment. Returns
+    (rows [n, max(end - start) + 1] u16, seg [n, 2] u32 = [1, 1 + end - start])"""
+    rows = np.zeros((len(segs), max(en - st for _, st, en in segs) + 1), np.uint16)
+    for i, (b, st, en) in enumerate(segs):
+        rows[i, 0] = pcm[b, st - 1] if st else np.uint16(atap["mid_val"][b] & 0xFFFF)
+        rows[i, 1:1 + en - st] = pcm[b, st:en]
+    return rows, np.array([[1, 1 + en - st] for _, st, en in segs], np.uint32).reshape(-1, 2)
+
+
 def pinned_rows(pcm, atap):
     """rows of U + 1 samples, [mid_val, row...]: with every segment shifted by +1, x[-1] of a segment that starts at
     sample 0 is the utterance's own mid_val (as a 16-bit sample), and every other segment reads its own samples"""
     B, U = pcm.shape
-    rows = np.empty((B, U + 1), np.uint16)
-    rows[:, 0] = atap["mid_val"].astype(np.uint16)
-    rows[:, 1:] = pcm
-    return rows
+    return segment_rows(pcm, atap, [(b, 0, U) for b in range(B)])[0]
 
 
 def plant_sample0(pcm, rows, seed, before=4095):

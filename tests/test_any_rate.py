@@ -1,7 +1,7 @@
 """The banded DP without the 2:1 length guard (SR_DTW_BAND | SR_DTW_ANY_RATE, an extension the reference does not have;
 parity unpinned) in sr_dtw_batch and as the matcher of every recognition call (sr_set_match).
 
-CPU: the header and the binding define the bit; the C oracle (tests/oracle_rate.c) equals a plain Python DP on every shape
+CPU: the header and the binding define the bit; the C oracle (tests/oracle_ext/rate.c) equals a plain Python DP on every shape
 up to 12 x 12 and the oracle port's SR_DTW_BAND DP on every pair within 2:1; it reproduces the real-speech accuracy of the
 four digit recordings. GPU: the setter and flag rules; sr_dtw_batch equals the oracle bit for bit on every (I, M) in
 1..119 x 1..119 at radii that pick each band kernel, and plain SR_DTW_BAND on every pair within 2:1; every recognition
@@ -16,12 +16,11 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_long as ol
-import oracle_rate as orate
+import oracle_ext as ox
 import sr_b200
 from test_extension_refs import NTHREADS
 from test_sym_match import (DIGITS, INT32_MAX, _bank_planted, _cmp_long, _ftr, _inputs, _k14_events, _k4_events, _rows,
-                            _same, _wav, _want_best, get_dis)
+                            _same, _want_best, get_dis)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NULL = DIS_ERR = 0xFFFFFFFF
@@ -64,7 +63,7 @@ def rate_ref(x, y, r):
 def test_oracle_equals_plain_reference_on_every_small_shape():
     """sro_rate == rate_ref on every I, M in 1..12 (ratios up to 12:1 both ways) at every r in 0..12 and 118, and the end
     cell outside the band (ceil(M/I) - 1 > r) always scores SR_DIS_ERR"""
-    ro = orate.rate_oracle()
+    ro = ox.rate_oracle()
     rng = np.random.default_rng(0xA11)
     n_far = n_err = 0
     for k, (I, M) in enumerate(itertools.product(range(1, 13), range(1, 13))):
@@ -86,7 +85,7 @@ def test_oracle_equals_plain_reference_on_every_small_shape():
 def test_oracle_equals_band_oracle_within_the_guard():
     """on every pair of 1..119-frame sets within 2:1 (sampled per shape) the new oracle scores what the port's SR_DTW_BAND
     DP scores at the same r; outside 2:1 the port says SR_DIS_ERR and the new oracle scores every pair at r = 118"""
-    ro, po = orate.rate_oracle(), ob.port()
+    ro, po = ox.rate_oracle(), ob.port()
     rng = np.random.default_rng(0xA12)
     frms = [1, 2, 3, 59, 60, 61, 118, 119] + [int(v) for v in rng.integers(1, 120, 24)]
     fin = _inputs(rng, frms)
@@ -109,9 +108,9 @@ def _real_speech_pairs():
 
 def _digit_bank(port, lo, a):
     """template k = segment k of recording a, in slot 4k (the other slots unsigned)"""
-    ea = ol.recognise_long(lo, port, a[None], 2400, None, 0, 4096, 32)
+    ea = ox.recognise_long(lo, port, a[None], 2400, None, 0, 4096, 32)
     ma = int(ea["n_segs"][0])
-    ftr = ol.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
+    ftr = ox.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
                                                           else int(s["start"])) for s in ea["segs"][0, :ma]])
     ftr4 = np.zeros(4 * ma, ob.FTR_DTYPE)
     ftr4[0::4] = ftr
@@ -124,10 +123,10 @@ def test_real_speech_accuracy_on_the_oracles():
     """the digit recordings, each recognised against its twin's segments at r = 118: the band DP gets 6, 8, 3, 3 right
     (20 of 46), the same DP without the guard 4, 8, 9, 8 (29 of 46). A fixed computation on fixed data, not a claim about
     speech in general"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     got = []
     for a_name, b_name in _real_speech_pairs():
-        a, b = _wav(a_name), _wav(b_name)
+        a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
         bank, T, ma = _digit_bank(port, lo, a)
         row = []
         for flags in (BAND, RATE):
@@ -142,7 +141,7 @@ def test_real_speech_accuracy_on_the_oracles():
 def _scores(ftr, bank, T, flags, r):
     """the oracle's template scan under a matcher (0 greedy, BAND, RATE) with the save_sign check"""
     if flags == RATE:
-        return orate.rate_oracle().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r, nthreads=NTHREADS)
+        return ox.rate_oracle().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r, nthreads=NTHREADS)
     return ob.port().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r if flags else -1, nthreads=NTHREADS)[0]
 
 
@@ -164,14 +163,14 @@ def _compose(front, bank, T, flags, r):
 
 def long_oracle(pcm, bank, T, flags, r, max_segs, lens=None):
     """sr_recognise_long_batch composed from the oracles: the long-form VAD and front end, the scan under the matcher"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     if flags != RATE:
-        return ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, max_segs, lens, band_r=r if flags else -1)
-    want = ol.recognise_long(lo, port, pcm, 2400, bank, 0, 4096, max_segs, lens)
+        return ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, max_segs, lens, band_r=r if flags else -1)
+    want = ox.recognise_long(lo, port, pcm, 2400, bank, 0, 4096, max_segs, lens)
     segs = want["segs"]
     todo = [(b, k) for b in range(len(segs)) for k in range(min(int(want["n_segs"][b]), max_segs)) if segs[b, k]["status"] == 0]
     if todo and T:
-        ftr = ol.ftr_of_segments(port, pcm, want["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
+        ftr = ox.ftr_of_segments(port, pcm, want["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
                                                             for b, k in todo])
         sc = _scores(ftr, bank, T, RATE, r)
         for i, (b, k) in enumerate(todo):
@@ -240,7 +239,7 @@ def test_dtw_batch_every_shape_equals_oracle(kind):
     """score, best_idx and best_dis of sr_dtw_batch(BAND | ANY_RATE) on every (I, M) in 1..119 x 1..119 (1:119 and 119:1
     included) at every radius that picks a band kernel, bit for bit against the oracle; tie-heavy {0, 1} rows as a second
     case. Every pair within 2:1 scores what plain SR_DTW_BAND scores; outside it BAND says SR_DIS_ERR"""
-    ro = orate.rate_oracle()
+    ro = ox.rate_oracle()
     fin, bank = _every_shape_case(kind, 0xA30 + (kind == "tie"))
     I = np.arange(1, 120)[:, None]
     M = np.arange(119, 0, -1)[None, :]
@@ -270,7 +269,7 @@ def test_dtw_batch_every_shape_equals_oracle(kind):
 def test_dtw_batch_planted_slots_equal_oracle(T):
     """banks with erased, unsigned, frm_num 0 and frm_num 120 slots; inputs of 0..120 frames; with and without
     CHECK_SIGN, at every kernel radius and INT32_MAX"""
-    ro = orate.rate_oracle()
+    ro = ox.rate_oracle()
     rng = np.random.default_rng(0xA40 + T)
     bank = _bank_planted(rng, T)
     frms = [0, 120, 1, 119, 2, 118, 3, 100] + [int(x) for x in rng.integers(1, 120, 32)]
@@ -454,7 +453,7 @@ def test_long_batch_and_dev_equal_oracle(r):
     import torch
     lens = np.array([70001, 161, 123457, 99999, 200000], np.uint32)
     Ul = 200000
-    pcm = ol.synth_long(len(lens), Ul, 0xA610)
+    pcm = ox.synth_long(len(lens), Ul, 0xA610)
     for b, n in enumerate(lens):
         pcm[b, n:] = np.where(np.arange(Ul - n) % 2, 4095, 0)
     bank, T = _synth_stretched_bank()
@@ -475,7 +474,7 @@ def test_long_batch_and_dev_equal_oracle(r):
                                    d_segs.data_ptr())
         h.sync()
         _cmp_long(dict(n_segs=d_n.cpu().numpy().view(np.uint32),
-                       segs=d_segs.cpu().numpy().view(ol.LONG_SEG_DTYPE).reshape(len(lens), 64)), want)
+                       segs=d_segs.cpu().numpy().view(ox.LONG_SEG_DTYPE).reshape(len(lens), 64)), want)
     finally:
         h.close()
 
@@ -485,7 +484,7 @@ def test_k14_long_streams_equal_oracle_on_every_prefix():
     """a live long-stream pool under BAND | ANY_RATE: each closed segment's event, handed out by the push after which it
     closed, so on the prefix pushed so far, equals the composed oracle's record of the whole recording, and every closed
     segment is handed out once"""
-    xs = list(ol.synth_long(6, 120000, 0xA620))
+    xs = list(ox.synth_long(6, 120000, 0xA620))
     xs[2] = xs[2][:50000]
     bank, T = _synth_stretched_bank()
     h = _handle(bank, T, RATE, 16)
@@ -524,7 +523,7 @@ def test_launches_and_tags_equal_the_band_matchers(case):
     """recognise, long recognise and sr_dtw_batch under BAND | ANY_RATE launch what they launch under BAND, with the
     same tags (6 for the scan), for r on both sides of every band-kernel choice"""
     pcm, bank, T = case["pcm"][:64], case["bank"], case["T"]
-    lpcm = ol.synth_long(3, 100000, 0xA640)
+    lpcm = ox.synth_long(3, 100000, 0xA640)
     fin = case["front"]["ftr"][:64]
     h = _handle(bank, T, 0, 0)
     try:
@@ -578,11 +577,11 @@ def test_bytes_written_equal_the_band_matchers(case):
 def test_real_speech_decisions_reported():
     """enrol each digit recording's segments (template k in slot 4k) and recognise its twin with sr_recognise_long_batch
     under band r = 118 and BAND | ANY_RATE r = 118: decisions equal the oracle; accuracy is printed, not asserted"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     h = sr_b200.Handle(0)
     try:
         for a_name, b_name in _real_speech_pairs():
-            a, b = _wav(a_name), _wav(b_name)
+            a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
             bank, T, ma = _digit_bank(port, lo, a)
             h.set_bank(bank, T, 4096)
             line = []

@@ -22,12 +22,8 @@ import traceback
 import numpy as np
 import pytest
 
-import oracle_align as oa
 import oracle_bind as ob
-import oracle_connected as oc
-import oracle_grammar as og
-import oracle_long as ol
-import oracle_long_grammar as olg
+import oracle_ext as ox
 import sr_b200
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -348,7 +344,7 @@ class EnrolAverageAlign(Job):
         slots = sr_b200.make_bank(want["ftr"])
         slots[want["status"] != 0] = 0xFF
         bad = oracle_diff({"slots": out["bank"][rows], "status": out["status"][rows]}, {"slots": slots, "status": want["status"]})
-        al = oa.align()
+        al = ox.align()
         avg, score, anchor = al.average_bank(out["bank"], 4096, self.K, 118, 2)
         bad += oracle_diff({k: out[k] for k in ("avg", "score", "anchor")}, {"avg": avg, "score": score, "anchor": anchor})
         sel = [0, 5, 66, 127]
@@ -391,8 +387,8 @@ class LongConnected(Job):
     def oracle(self, v, out):
         pcm, seg, atap = self.inputs[v]
         rows = list(self.rows)
-        feat, frm = oc.mfcc_long(self.w.ora, np.ascontiguousarray(pcm[rows]), seg[rows], atap[rows], oc.CONN_FRM_MAX)
-        words, nw, total = oc.connected().connected(feat, frm, self.w.bank128, 128, 4096, self.P, self.MW)
+        feat, frm = ox.mfcc_long(self.w.ora, np.ascontiguousarray(pcm[rows]), seg[rows], atap[rows], ox.CONN_FRM_MAX)
+        words, nw, total = ox.connected().connected(feat, frm, self.w.bank128, 128, 4096, self.P, self.MW)
         return oracle_diff({k: out[k][rows] for k in ("feat", "frm_num", "words", "n_words", "total")},
                             {"feat": feat, "frm_num": frm, "words": words, "n_words": nw, "total": total})
 
@@ -421,8 +417,8 @@ class Grammar(Job):
     def oracle(self, v, out):
         rows = list(self.rows)
         pcm = np.ascontiguousarray(self.pcm(v)[rows])
-        g = og.recognise_connected_grammar(self.w.ora, og.grammar(), pcm, 2400, self.w.bank40, 40, 4096, self.PIN, 0, self.MW)
-        c = oc.recognise_connected(self.w.ora, oc.connected(), pcm, 2400, self.w.bank40, 40, 4096, 3000, self.MW)
+        g = ox.recognise_connected_grammar(self.w.ora, ox.grammar(), pcm, 2400, self.w.bank40, 40, 4096, self.PIN, 0, self.MW)
+        c = ox.recognise_connected(self.w.ora, ox.connected(), pcm, 2400, self.w.bank40, 40, 4096, 3000, self.MW)
         want = dict([("pin_" + k, a) for k, a in g.items()] + [("loop_" + k, a) for k, a in c.items()])
         return oracle_diff({k: out[k][rows] for k in want}, want)
 
@@ -535,15 +531,14 @@ class LongForm(Job):
 
     def open(self):
         import torch
-        import oracle_long as ol
-        self.torch, self.ol = torch, ol
+        self.torch = torch
         self.h = self.handle()
         self.h.set_bank(self.w.bank40, 40, 4096)
         self.st = torch.cuda.Stream(torch.device("cuda:0"))
         self.h.set_stream(self.st.cuda_stream)
         self.inputs = []
         for v in range(2):
-            pcm = ol.synth_long(self.B, self.U, 0xCC000000 + v)
+            pcm = ox.synth_long(self.B, self.U, 0xCC000000 + v)
             lens = np.array([self.U, 161, 90000 + v, 2399, 120001, self.U - 80 * v], np.uint32)
             for b, n in enumerate(lens):
                 pcm[b, n:] = np.where(np.arange(self.U - n) % 2, 4095, 0)
@@ -569,12 +564,11 @@ class LongForm(Job):
             o = {k: t.cpu().numpy() for k, t in self.out.items()}
         return {"vad_atap": vad["atap"], "vad_n_segs": vad["n_segs"], "seg_off": vad["seg_off"], "atap": rec["atap"],
                 "n_segs": rec["n_segs"], "segs": rec["segs"], "dev_atap": o["atap"].view(sr_b200.ATAP_DTYPE),
-                "dev_n_segs": o["n_segs"].view(np.uint32), "dev_segs": o["segs"].view(self.ol.LONG_SEG_DTYPE).reshape(self.B, self.MS)}
+                "dev_n_segs": o["n_segs"].view(np.uint32), "dev_segs": o["segs"].view(ox.LONG_SEG_DTYPE).reshape(self.B, self.MS)}
 
     def oracle(self, v, out):
         pcm, lens = self.inputs[v]
-        ol = self.ol
-        want = ol.recognise_long(ol.long_oracle(), self.w.po, pcm, 2400, self.w.bank40, 40, 4096, self.MS, lens)
+        want = ox.recognise_long(ox.long_oracle(), self.w.po, pcm, 2400, self.w.bank40, 40, 4096, self.MS, lens)
         k = np.arange(self.MS)[None, :] < np.minimum(want["n_segs"], self.MS)[:, None]
         got = {"vad_atap": out["vad_atap"], "vad_n_segs": out["vad_n_segs"], "seg_off": out["seg_off"][k],
                "atap": out["atap"], "n_segs": out["n_segs"], "segs": out["segs"][k], "dev_atap": out["dev_atap"],
@@ -661,7 +655,7 @@ class LongGrammar(Job):
         self.h.set_bank(self.w.bank40, 40, 4096)
         self.inputs = []
         for v in range(2):
-            pcm = ol.synth_long(self.B, self.U, 0xCD000000 + v)
+            pcm = ox.synth_long(self.B, self.U, 0xCD000000 + v)
             lens = np.array([self.U, 70001 + v, 2399, 40000, self.U - 160 * v], np.uint32)
             rng = np.random.default_rng(0xCD + v)
             seg_frm = np.array([30, 0, 119, 5, 64 + v, 818], np.uint32)
@@ -679,9 +673,9 @@ class LongGrammar(Job):
 
     def oracle(self, v, out):
         pcm, lens, feat, seq_seg, seg_frm = self.inputs[v]
-        g, lg = self.GRAMS[v], olg.long_grammar()
-        want = olg.recognise_long_grammar(ol.long_oracle(), self.w.po, lg, pcm, 2400, self.w.bank40, 40, 4096, g, self.P,
-                                          self.MS, self.MW, lens)
+        g, lg = self.GRAMS[v], ox.long_grammar()
+        want = ox.recognise_long_grammar(ox.long_oracle(), self.w.po, lg, pcm, 2400, self.w.bank40, 40, 4096, g, self.P,
+                                         self.MS, self.MW, lens)
         if v == 1:
             del want["atap"]
         assert (want["n_segs"] > self.MS).any() and (want["n_words"] > 0).any()
@@ -706,7 +700,7 @@ class LongStream(Job):
         self.h.set_bank(self.w.bank8, 8, 4096)
         self.inputs = []
         for v in range(2):
-            pcm = ol.synth_long(self.S, self.L, 0xCE000000 + v)
+            pcm = ox.synth_long(self.S, self.L, 0xCE000000 + v)
             rng = np.random.default_rng(0xCE + v)
             pos, pushes = np.zeros(self.S, np.int64), []
             while (pos < self.L).any():
@@ -749,7 +743,7 @@ class LongStream(Job):
 
     def _closed(self, x):
         """sr_recognise_long_batch of one stream's samples from the oracles: (closed records, open start, atap)"""
-        r = ol.recognise_long(ol.long_oracle(), self.w.po, np.ascontiguousarray(x[None, :]), 2400, self.w.bank8, 8, 4096,
+        r = ox.recognise_long(ox.long_oracle(), self.w.po, np.ascontiguousarray(x[None, :]), 2400, self.w.bank8, 8, 4096,
                               len(x) // 1520 + 4)
         recs = [tuple(int(q) for q in rec) for rec in r["segs"][0, :int(r["n_segs"][0])].tolist()]
         op = recs[-1][0] if recs and recs[-1][2] == 1 else 0xFFFFFFFF
@@ -913,7 +907,7 @@ def test_serial_baseline_matches_the_oracles(baseline):
     pin = baseline["connected_grammar"][0][0]
     assert (pin["pin_n_words"][pin["pin_status"] == 0] == 4).all() and (pin["pin_status"] == 0).sum() > 16
     lc = baseline["mfcc_long_connected"][0][0]
-    assert (lc["frm_num"] == oc.CONN_FRM_MAX).sum() == LongConnected.B // 4 and (lc["n_words"][lc["frm_num"] > 0] >= 1).all()
+    assert (lc["frm_num"] == ox.CONN_FRM_MAX).sum() == LongConnected.B // 4 and (lc["n_words"][lc["frm_num"] > 0] >= 1).all()
     tags = baseline["enrol_average_path"][0][2][0]
     assert {ALIGN, AVG_UPDATE} <= set(tags) and GRAM in baseline["connected_grammar"][0][2][0]
     assert CONN in baseline["mfcc_long_connected"][0][2][0] and DTW_BAND in baseline["recognise_dev_band"][0][2][0]

@@ -1,7 +1,7 @@
 """Connected words (K6, an extension the reference does not have; the decoder's parity is unpinned, the long front end is
 pinned to the reference piece by piece): sr_mfcc_long_batch, sr_connected_batch and sr_recognise_connected_batch.
 
-CPU: the decoder's C restatement (tests/oracle_connected.c) equals cell_ref, a plain Python cell-level reference written
+CPU: the decoder's C restatement (tests/oracle_ext/connected.c) equals cell_ref, a plain Python cell-level reference written
 here from the definition in speech_recog.h; its total equals a brute-force minimum over segmentations built on
 dist_matrix and dtw_full (which share no code with either); the P = 2^32 - 1 and the concatenated-templates properties
 hold; the piecewise long-feature oracle at frm_cap = 119 equals the oracle's get_mfcc. GPU: all three calls equal the
@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_connected as oc
+import oracle_ext as ox
 import sr_b200
 from test_extension_refs import MAX_A, MAX_B, MAX_FRM, NTHREADS, dist_matrix
 
@@ -139,7 +139,7 @@ def test_oracle_equals_cell_reference_and_brute_force():
     planted, N = 0..40 of tie-heavy {0, 1} and +-32 767 rows, P in {0, 1, 1000, 2^32 - 1}, and an empty / all-non-member
     bank; the total equals brute_total, every word's dis equals dtw_full of its frames, the words tile [0, N) in order
     and sum(dis + P) = total"""
-    co = oc.connected()
+    co = ox.connected()
     rng = np.random.default_rng(0xC0)
     n_cases = n_multi = 0
     for case in range(96):
@@ -158,7 +158,7 @@ def test_oracle_equals_cell_reference_and_brute_force():
             want_words, want_total = cell_ref(x, bank, T, bank.shape[1], P)
             got = _as_tuples(w[0], int(nw[0]))
             assert (got, int(tot[0])) == (want_words, want_total), (case, P)
-            assert (w[0][int(nw[0]):] == np.zeros(1, oc.WORD_DTYPE)).all()
+            assert (w[0][int(nw[0]):] == np.zeros(1, ox.WORD_DTYPE)).all()
             if N == 0 or not mem:
                 assert got == [] and int(tot[0]) == (0 if N == 0 else 2 ** 64 - 1)
                 continue
@@ -175,7 +175,7 @@ def test_oracle_equals_cell_reference_and_brute_force():
 
 def test_max_penalty_gives_the_argmin_word():
     """P = 2^32 - 1: exactly one word, the argmin of the unnormalised full DTW, the lowest slot on a tie"""
-    co = oc.connected()
+    co = ox.connected()
     rng = np.random.default_rng(0xC1)
     for case in range(60):
         kind = ("tie", "small", "equal")[case % 3]
@@ -195,7 +195,7 @@ def test_max_penalty_gives_the_argmin_word():
 
 def test_concatenated_templates_decode_back():
     """an input made of distinct templates back to back decodes, at P = 0, to total 0 and that sequence of slots"""
-    co = oc.connected()
+    co = ox.connected()
     rng = np.random.default_rng(0xC2)
     for case in range(40):
         T = int(rng.integers(2, 9))
@@ -223,18 +223,18 @@ def test_piecewise_long_features_at_119_equal_get_mfcc():
     en = st + 160 + 80 * rng.integers(-1, 240, B)
     seg = np.stack([st, en], 1).astype(np.uint32)
     seg[5] = ob.NULL
-    feat, frm = oc.mfcc_long(o, pcm, seg, atap, 119)
+    feat, frm = ox.mfcc_long(o, pcm, seg, atap, 119)
     want = o.mfcc_batch(ob.pinned_rows(pcm, atap), np.where(seg == ob.NULL, ob.NULL, seg + 1), atap)
     assert np.array_equal(frm, want["frm_num"])
     for b in range(B):
         n = int(frm[b])
         assert np.array_equal(feat[b, :n].reshape(-1), want["mfcc_dat"][b][:n * 12])
-    feat2, frm2 = oc.mfcc_long(o, pcm, seg, atap, 818)
+    feat2, frm2 = ox.mfcc_long(o, pcm, seg, atap, 818)
     for b in range(B):
         n = int(frm2[b])
         if n > 119:                                     # frames 119.. = the segment that starts 80 * 119 samples later
             s2 = np.array([[seg[b, 0] + 80 * 119, seg[b, 1]]], np.uint32)
-            f, k = oc.mfcc_long(o, pcm[b:b + 1], s2, atap[b:b + 1], 818)
+            f, k = ox.mfcc_long(o, pcm[b:b + 1], s2, atap[b:b + 1], 818)
             assert int(k[0]) == n - 119 and np.array_equal(feat2[b, 119:n], f[0, :n - 119])
 
 
@@ -273,7 +273,7 @@ def test_mfcc_long_equals_piecewise_oracle(geom):
     for cap in (818, 300, 119, 1):
         fill = np.full((B, cap, 12), -12345, np.int16)
         feat, frm = h.mfcc_long(pcm, seg, atap, cap, feat=fill.copy())
-        want, wfrm = oc.mfcc_long(o, pcm, seg, atap, cap, geom_b=bool(geom))
+        want, wfrm = ox.mfcc_long(o, pcm, seg, atap, cap, geom_b=bool(geom))
         assert np.array_equal(frm, wfrm), cap
         for b in range(B):
             n = int(frm[b])
@@ -296,7 +296,7 @@ def test_mfcc_long_equals_piecewise_oracle(geom):
 def _check_connected(h, co, feat, frm, bank, T, stride, P, max_words, prefill=0x5A):
     """the GPU decoder against the oracle, outputs prefilled: records past n_words keep their bytes; two launches agree"""
     h.set_bank(bank, T, stride)
-    w0 = np.frombuffer(bytes([prefill]) * (len(frm) * max_words * 24), oc.WORD_DTYPE).reshape(len(frm), max_words).copy()
+    w0 = np.frombuffer(bytes([prefill]) * (len(frm) * max_words * 24), ox.WORD_DTYPE).reshape(len(frm), max_words).copy()
     got = h.connected(feat, frm, P, max_words, words=w0.copy())
     again = h.connected(feat, frm, P, max_words, words=w0.copy())
     ww, wn, wt = co.connected(feat, frm, bank, T, stride, P, max_words, nthreads=NTHREADS)
@@ -314,7 +314,7 @@ def _check_connected(h, co, feat, frm, bank, T, stride, P, max_words, prefill=0x
 def test_connected_equals_oracle_over_lengths_and_banks():
     """N in {0, 1, 2, 118, 119, 120, 237, 238, 500, 818} against banks of 1, 20, 32, 33, 80 and 128 (the limit) slots with
     non-members mixed in, every penalty, max_words smaller and larger than the word counts"""
-    co = oc.connected()
+    co = ox.connected()
     h = sr_b200.Handle(0)
     h.timing_enable(64)
     rng = np.random.default_rng(0xC5)
@@ -335,7 +335,7 @@ def test_connected_equals_oracle_over_lengths_and_banks():
 def test_connected_ties_headroom_and_averaged_bank():
     """all-equal rows (every cell a tie); rows at the largest local distance at N = 818 against 119-frame templates (D
     beyond 32 bits); tie-heavy {0, 1} rows; a bank from sr_average_bank of enrolled groups"""
-    co = oc.connected()
+    co = ox.connected()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0xC6)
     eq = _bank(rng, 24, "equal", stride=4096, fmin=1, fmax=119, plant=True)
@@ -366,7 +366,7 @@ def test_connected_batch_position_and_argument_rules():
     """batch sizes around multiples of 132 and 264 clusters, every sequence equal to the oracle wherever it sits; an
     over-limit bank (129 slots), frm_num above 818 or frm_stride and a NULL n_words fail and write nothing; B = 0 launches
     nothing"""
-    co = oc.connected()
+    co = ox.connected()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0xC7)
     bank = _bank(rng, 12, "small", stride=4096, fmin=2, fmax=40)
@@ -410,7 +410,7 @@ def _check_recognise(h, co, pcm, bank, T, P, max_words, n_len=2400):
     out = {k: np.repeat(v, B, axis=0) for k, v in out.items()}
     pre = {k: v.copy() for k, v in out.items()}
     got = h.recognise_connected(pcm, P, max_words, n_len, out=out)
-    want = oc.recognise_connected(ob.best_oracle(), co, pcm, n_len, bank, T, 4096, P, max_words, atap0=pre["atap"])
+    want = ox.recognise_connected(ob.best_oracle(), co, pcm, n_len, bank, T, 4096, P, max_words, atap0=pre["atap"])
     for k in ("atap", "seg_off", "frm_num", "n_words", "total", "status"):
         assert np.array_equal(got[k], want[k]), k
     for b in range(B):
@@ -433,7 +433,7 @@ def _enrolled_bank(h, n_cmd, seed):
 def test_recognise_connected_equals_composed_oracle():
     """the five board captures and synthetic 3-word captures at U = 8 000, 16 000 and 65 535 against an enrolled bank"""
     import os
-    co = oc.connected()
+    co = ox.connected()
     h = sr_b200.Handle(0)
     bank, _, _ = _enrolled_bank(h, 20, 0xC80000)
     cap = np.load(os.path.join(os.path.dirname(__file__), "golden", "captures.npz"))
@@ -456,7 +456,7 @@ def test_recognise_connected_decodes_spliced_words():
     SR_ST_MFCC_FAIL on it, the connected call returns the spliced command sequence. Frames that straddle a join match no
     template exactly, so the splices are chosen on the CPU first: only those from which the oracle recovers the sequence
     are kept, and the call must equal the oracle on every candidate"""
-    co = oc.connected()
+    co = ox.connected()
     ora = ob.best_oracle()
     h = sr_b200.Handle(0)
     n_cmd = 10
@@ -478,7 +478,7 @@ def test_recognise_connected_decodes_spliced_words():
         cands.append(x)
         seqs.append(seq)
     pcm = np.stack(cands).astype(np.uint16)
-    want = oc.recognise_connected(ora, co, pcm, 2400, bank, 4 * n_cmd, 4096, 3000, 8)
+    want = ox.recognise_connected(ora, co, pcm, 2400, bank, 4 * n_cmd, 4096, 3000, 8)
     keep = [b for b in range(len(seqs)) if want["status"][b] == 0 and want["frm_num"][b, 0] > 119
             and [int(w["cmd"]) for w in want["words"][b, :want["n_words"][b]]] == seqs[b]]
     assert len(keep) >= 3, len(keep)

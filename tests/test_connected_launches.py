@@ -13,8 +13,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_connected as oc
-import oracle_grammar as og
+import oracle_ext as ox
 import sr_b200
 from test_connected import P_MAX, _bank, _draw, _enrolled_bank, _slot
 from test_extension_refs import MAX_FRM, NTHREADS
@@ -97,7 +96,7 @@ def _poisoned(rng, N, stride):
 
 
 def _prefill_words(B, max_words):
-    return np.frombuffer(b"\x5a" * (B * max_words * 24), oc.WORD_DTYPE).reshape(B, max_words).copy()
+    return np.frombuffer(b"\x5a" * (B * max_words * 24), ox.WORD_DTYPE).reshape(B, max_words).copy()
 
 
 def _check_words(got, want, n_words, pre):
@@ -177,7 +176,7 @@ def test_mfcc_long_across_piece_chunks(geom):
     rows = _long_rows(rng, fmax)
     B = len(rows)
     seg = _long_segments(rng, rows, U, frame_len)
-    F = np.array([oc.long_frames(int(s), int(e), U, frame_len) for s, e in seg], np.int64)
+    F = np.array([ox.long_frames(int(s), int(e), U, frame_len) for s, e in seg], np.int64)
     assert list(F) == [max(f, 0) for f, _ in rows]
     pcm = rng.integers(0, 65536, (B, U), dtype=np.uint16)
     pcm[1::2] &= 0x0FFF
@@ -199,7 +198,7 @@ def test_mfcc_long_across_piece_chunks(geom):
         past = np.arange(cap)[None, :] >= frm[:, None].astype(np.int64)
         assert (feat[past] == PREFILL).all()
         idx = sorted(edge | set(rng.choice(B, 4, replace=False).tolist()))
-        want, wfrm = oc.mfcc_long(o, pcm[idx], seg[idx], atap[idx], cap, geom_b=bool(geom))
+        want, wfrm = ox.mfcc_long(o, pcm[idx], seg[idx], atap[idx], cap, geom_b=bool(geom))
         assert np.array_equal(frm[idx], wfrm)
         for q, b in enumerate(idx):
             assert np.array_equal(feat[b, :frm[b]], want[q, :frm[b]]), (cap, b)
@@ -218,7 +217,7 @@ def test_recognise_connected_across_piece_chunks():
     and sr_recognise_connected_grammar_batch under the PIN chain and the loop grammar: the composed oracles on the
     captures at the piece boundary, the first and the last and a few at random; capture slices of one piece launch each
     equal the whole call on every capture; the loop grammar equals sr_recognise_connected_batch on the whole batch"""
-    co, go, ora = oc.connected(), og.grammar(), ob.best_oracle()
+    co, go, ora = ox.connected(), ox.grammar(), ob.best_oracle()
     h = sr_b200.Handle(0)
     bank, _, _ = _enrolled_bank(h, 20, 0xC1B0000)
     h.set_bank(bank, 80, 4096)
@@ -241,9 +240,9 @@ def test_recognise_connected_across_piece_chunks():
         assert launches >= 2 and _count(h, TAG_MFCC) == launches
         idx = sorted(edge | set(rng.choice(B, 3, replace=False).tolist()))
         if g is None:
-            want = oc.recognise_connected(ora, co, pcm[idx], 2400, bank, 80, 4096, P, mw, atap0=pre["atap"][idx])
+            want = ox.recognise_connected(ora, co, pcm[idx], 2400, bank, 80, 4096, P, mw, atap0=pre["atap"][idx])
         else:
-            want = og.recognise_connected_grammar(ora, go, pcm[idx], 2400, bank, 80, 4096, g, P, mw,
+            want = ox.recognise_connected_grammar(ora, go, pcm[idx], 2400, bank, 80, 4096, g, P, mw,
                                                   atap0=pre["atap"][idx], nthreads=NTHREADS)
         for k in ("atap", "seg_off", "frm_num", "n_words", "total", "status"):
             assert np.array_equal(got[k][idx], want[k]), (name, k)
@@ -289,7 +288,7 @@ def test_grammar_record_cuts(S):
     15 (a row limit of 2 236 962, not a power of two) against 16 members of 1-8 frames, one per command; N = 0 sequences
     at every cut; max_words below (P = 0) and above (P = 2^32 - 1) the word counts. The oracle on the whole batch; slices
     of one launch each equal the whole call"""
-    go = og.grammar()
+    go = ox.grammar()
     rng = np.random.default_rng(0xC1C0 + S)
     bank = _bank(rng, 64, "small", stride=4096, fmin=1, fmax=8, plant=False)
     bank[np.arange(64) % 4 != 0] = 0xFF                   # slot 4c holds command c's one member
@@ -352,7 +351,7 @@ def _check_plants(got, plant, mw):
 def test_connected_over_2_20_sequences():
     """sr_connected_batch on 2^20 + 5 sequences: two K6 launches; the whole batch equals the oracle, the planted
     sequences on both sides of the split decode to slots 1 then 6 at P = 0; [0, 2^20) and [2^20, B) alone equal it"""
-    co = oc.connected()
+    co = ox.connected()
     rng = np.random.default_rng(0xC1D)
     B, bank, N, feat, plant = _many_short(rng)
     h = sr_b200.Handle(0)
@@ -379,7 +378,7 @@ def test_grammar_over_2_20_sequences():
     """sr_connected_grammar_batch on the same 2^20 + 5 sequences under an 8-state grammar that accepts the planted pair:
     the records fit one run_grammar launch, which makes two K6g launches; at 16 states and N = 2 everywhere the record
     cut falls at 2^20 itself (two launches again). The whole batch equals the oracle; slices of one launch equal it"""
-    go = og.grammar()
+    go = ox.grammar()
     rng = np.random.default_rng(0xC1E)
     B, bank, N, feat, plant = _many_short(rng)
     h = sr_b200.Handle(0)

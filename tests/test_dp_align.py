@@ -1,14 +1,14 @@
 """Alignment along the banded DP (K3p, an extension the reference does not have; parity unpinned): the optimal warping
 path of sr_dtw_path_batch and the DTW barycentre averaging of sr_average_bank.
 
-CPU: the oracle's restatement (tests/oracle_align.c) equals band_path_ref and average_ref, plain numpy / Python references
+CPU: the oracle's restatement (tests/oracle_ext/align.c) equals band_path_ref and average_ref, plain numpy / Python references
 written here from the definitions in speech_recog.h that share no code with it; the paths' invariants and the averaging
 properties. GPU: both calls equal the oracle bit for bit, the scores equal sr_dtw_batch's band scores, and the averaged
 bank is one recognition accepts."""
 import numpy as np
 import pytest
 
-import oracle_align as oa
+import oracle_ext as ox
 import oracle_bind as ob
 import sr_b200
 from test_extension_refs import (DIS_ERR, MAX_FRM, NTHREADS, _band_cases, _ftr, _guard_edge_shapes,
@@ -156,7 +156,7 @@ def test_oracle_path_equals_plain_reference_on_guard_edges():
     the paths start at (0, 0), end at (I-1, M-1), step by (1,0), (0,1) or (1,1), stay in the band, sum get_dis to
     D(I-1, M-1), and the score equals sro_dtw_band. band_path_ref runs once per distinct band (r and min(r, M - 1) select
     the same cells)"""
-    ao, po = oa.align(), ob.port()
+    ao, po = ox.align(), ob.port()
     rng = np.random.default_rng(0xA1)
     kinds = ("small", "full", "equal")
     n_paths = n_err = 0
@@ -185,7 +185,7 @@ def test_oracle_path_equals_plain_reference_on_guard_edges():
 
 def test_oracle_self_match_path_is_the_diagonal():
     """a self-match's path is the diagonal at every radius, also for all-equal rows where every cell ties"""
-    ao = oa.align()
+    ao = ox.align()
     rng = np.random.default_rng(0xA2)
     for n in (1, 2, 7, 60, 119):
         for kind in ("small", "equal", "full"):
@@ -203,7 +203,7 @@ def test_oracle_self_match_path_is_the_diagonal():
 def test_oracle_average_equals_plain_reference(K):
     """sro_average_bank == average_ref (bank bytes, scores, anchors) on random groups with the invalid cases planted, for
     iters in {0, 1, 3} and r in {10, 118}"""
-    ao = oa.align()
+    ao = ox.align()
     rng = np.random.default_rng(0xA3 + K)
     stride = 2880
     bank = _random_groups(rng, 6, K, stride)
@@ -221,7 +221,7 @@ def test_oracle_average_equals_plain_reference(K):
 def test_averaging_properties():
     """K = 1 returns the member; K identical members return that member; iters = 0 returns the anchor; every output
     coefficient lies within the range of the frames aligned to it"""
-    ao = oa.align()
+    ao = ox.align()
     rng = np.random.default_rng(0xA4)
     stride = 4096
     bank = _random_groups(rng, 8, 1, stride, plant=False)
@@ -259,7 +259,7 @@ def test_path_batch_equals_oracle_on_every_shape():
     """sr_dtw_path_batch == the oracle bit for bit (path bytes, lengths, scores) on all 119 x 119 shapes of the four
     _band_cases at r in {0, 1, 7, 10, 15, 16, 59, 118, 1000} and INT32_MAX (against r = 118); the scores equal
     sr_dtw_batch with SR_DTW_BAND for the same pairs; a NULL path gives the same scores; self-matches walk the diagonal"""
-    ao = oa.align()
+    ao = ox.align()
     h = sr_b200.Handle(0)
     for name, utt, tpl in _band_cases():
         a, b = _all_pairs(utt, tpl)
@@ -305,7 +305,7 @@ def test_path_batch_does_not_depend_on_batch_position():
     every pair equals the oracle wherever it sits in the batch"""
     import torch
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    ao = oa.align()
+    ao = ox.align()
     rng = np.random.default_rng(0xA6)
     n = 2 * sms * 2 * 8 + 50
     lens_a, lens_b = rng.integers(1, 120, n), rng.integers(1, 120, n)
@@ -330,7 +330,7 @@ def _check_average(h, bank, stride, K, r, iters):
     l0 = h.launch_count()
     got = h.average_bank(bank, stride, K, r, iters)
     launches, tags = h.launch_count() - l0, [t for t, _ in h.timing_collect()]
-    want = oa.align().average_bank(bank, stride, K, r, iters, nthreads=NTHREADS)
+    want = ox.align().average_bank(bank, stride, K, r, iters, nthreads=NTHREADS)
     for a, b, what in zip(got, want, ("bank", "score", "anchor")):
         assert np.array_equal(a, b), (K, r, iters, what)
     out, score, anchor = got
@@ -375,7 +375,7 @@ def test_average_bank_random_groups_with_invalid_slots_equal_oracle():
     bank = _random_groups(np.random.default_rng(0xA8), 70, 1, 2880, plant=False)
     got = h.average_bank(bank, 2880, 1, 16, 2)
     assert np.array_equal(got[0], bank)
-    assert all(np.array_equal(a, b) for a, b in zip(got, oa.align().average_bank(bank, 2880, 1, 16, 2)))
+    assert all(np.array_equal(a, b) for a, b in zip(got, ox.align().average_bank(bank, 2880, 1, 16, 2)))
     with pytest.raises(sr_b200.SrError):
         h.average_bank(bank, 2880, 1, -1, 1)
     h.close()

@@ -19,7 +19,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import oracle_align as oa
+import oracle_ext as ox
 import oracle_bind as ob
 import sr_b200
 
@@ -242,7 +242,7 @@ def test_path_and_average_write_every_output_byte():
     from test_extension_refs import _ftr
     a = _ftr([rng.integers(-3000, 3001, (int(rng.integers(1, 120)), 12)) for _ in range(n)])
     b = _ftr([rng.integers(-3000, 3001, (int(rng.integers(1, 120)), 12)) for _ in range(n)])
-    want = oa.align().dtw_path(a, b, 10)
+    want = ox.align().dtw_path(a, b, 10)
     for fill in (P8, Q8):
         path, plen, dis = (np.full(s, fill, np.uint8) for s in (n * 237 * 2, n * 4, n * 4))
         assert L.sr_dtw_path_batch(h._h, a.ctypes.data, b.ctypes.data, n, 10, path.ctypes.data, plen.ctypes.data,
@@ -251,7 +251,7 @@ def test_path_and_average_write_every_output_byte():
         assert np.array_equal(path.reshape(n, 237, 2), want[1])
     K, G, stride = 4, 40, 4096
     bk = _random_groups(rng, G, K, stride, fmin=5, fmax=60)
-    want = oa.align().average_bank(bk, stride, K, 10, 2)
+    want = ox.align().average_bank(bk, stride, K, 10, 2)
     for fill in (P8, Q8):
         out, score, anchor = (np.full(s, fill, np.uint8) for s in (G * K * stride, G * K * 4, G * 4))
         assert L.sr_average_bank(h._h, bk.ctypes.data, stride, K, G, 10, 2, out.ctypes.data, score.ctypes.data,
@@ -461,22 +461,21 @@ def test_long_dev_writes_and_reads(bank):
     atap is written only for rows with n_len % 240 == 0 and n_len <= lens[b]; segment slots and records only below
     min(n_segs, max_segs); lens[b] > U reads as U; loud band-crossing poison past lens[b] and after the last row changes
     nothing. The host calls on the same handle equal those of a fresh handle and the oracle."""
-    import oracle_long as ol
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     B, U = 8, 30011
     lens = np.array([2399, 2400, 2401, 0, U, U + 1, 0xFFFFFFFF, 20000], np.uint32)   # n_len - 1, n_len, n_len + 1, 0, >= U
     eff = np.minimum(lens, U)
-    pcm = ol.synth_long(B, U, 0x1A5)
+    pcm = ox.synth_long(B, U, 0x1A5)
     for b in range(B):
         pcm[b, eff[b]:] = np.where(np.arange(U - eff[b]) % 2, 4095, 0)
     atap0 = np.zeros(B, ob.ATAP_DTYPE)
     atap0["mid_val"], atap0["n_thl"], atap0["z_thl"], atap0["s_thl"] = 2000 + np.arange(B), 40, 2, 3000
     h = _handle(bank)
-    stale = ol.synth_long(12, 50000, 0x1A6)
+    stale = ox.synth_long(12, 50000, 0x1A6)
     assert h.recognise_long_batch(stale, 64, 2400)["n_segs"].sum() > 40
     for n_len, ms, phase in ((2400, 3, 0), (2400, 64, 2), (2401, 64, 0), (2400, 0, 2)):
         what = "n_len %d max_segs %d phase %d" % (n_len, ms, phase)
-        want = ol.recognise_long(lo, port, pcm, n_len, bank, T, 4096, ms, eff, atap=atap0)
+        want = ox.recognise_long(lo, port, pcm, n_len, bank, T, 4096, ms, eff, atap=atap0)
         want_n, want_seg = lo.vad_long(pcm, want["atap"], ms, eff)
         assert want["n_segs"].tolist() == want_n.tolist()
         if n_len == 2400:
@@ -502,7 +501,7 @@ def test_long_dev_writes_and_reads(bank):
     try:
         for hh in (h, fresh):
             got = hh.recognise_long_batch(pcm, 5, 2400, eff, atap=atap0.copy())
-            want = ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 5, eff, atap=atap0)
+            want = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 5, eff, atap=atap0)
             for k in ("atap", "n_segs", "segs"):
                 assert got[k].tobytes() == want[k].tobytes(), k
             v = hh.vad_long_batch(pcm, 5, 2400, eff, atap=atap0.copy())
@@ -658,7 +657,7 @@ def test_path_and_average_read_only_member_rows():
     h = _handle()
     a, b = _ftr_set(rng, 120), _ftr_set(rng, 120)
     for r in (7, 10, 16):
-        want = oa.align().dtw_path(a, b, r)
+        want = ox.align().dtw_path(a, b, r)
         bad_a = _poison_rows(a, a["frm_num"], sign=True)
         bad_b = _poison_rows(b, b["frm_num"], sign=True)
         for x, y in ((bad_a, b), (a, bad_b), (bad_a, bad_b)):
@@ -669,7 +668,7 @@ def test_path_and_average_read_only_member_rows():
     hdr = np.frombuffer(bk[:, :4].tobytes(), np.uint16).reshape(-1, 2).astype(int)
     member = (hdr[:, 0] == sr_b200.SAVE_MASK) & (hdr[:, 1] >= 1) & (hdr[:, 1] <= 119)
     assert (~member).sum() >= 4
-    want = oa.align().average_bank(bk, stride, K, 10, 2)
+    want = ox.align().average_bank(bk, stride, K, 10, 2)
     got = h.average_bank(_poison_bank(bk, stride, np.where(member, hdr[:, 1], 0), member), stride, K, 10, 2)
     assert all(np.array_equal(g, w) for g, w in zip(got, want))
     h.close()
@@ -794,10 +793,8 @@ G13 = (3, 5, [(0, 1, 0x3), (1, 2, 0x7), (2, 0, 0x7), (1, 1, 0x8)])    # 3 states
 
 
 def _long_gram_oracle(pcm, n_len, bank_, n_slot, stride, g, P, max_segs, max_words, lens=None, geom_b=False, atap=None):
-    import oracle_long as ol
-    import oracle_long_grammar as olg
-    return olg.recognise_long_grammar(ol.long_oracle(), ob.port(), olg.long_grammar(), pcm, n_len, bank_, n_slot, stride, g,
-                                      P, max_segs, max_words, lens, geom_b, atap)
+    return ox.recognise_long_grammar(ox.long_oracle(), ob.port(), ox.long_grammar(), pcm, n_len, bank_, n_slot, stride, g,
+                                     P, max_segs, max_words, lens, geom_b, atap)
 
 
 def _same(got, want, what=""):
@@ -809,10 +806,9 @@ def _same(got, want, what=""):
 def test_long_grammar_reads_only_lens_samples(bank, geom):
     """sr_recognise_long_grammar_batch: loud band-crossing poison past lens[b] (it would open segments if read) gives the
     results of the clean recordings, which equal the composed oracle"""
-    import oracle_long as ol
     B, U = 5, 90001
     lens = np.array([U, 70000, 2399, 161, 40000], np.uint32)
-    clean = ol.synth_long(B, U, 0x13A5)
+    clean = ox.synth_long(B, U, 0x13A5)
     bad = clean.copy()
     for b, n in enumerate(lens):
         bad[b, n:] = np.where(np.arange(U - n) % 2, 4095, 0)
@@ -828,10 +824,9 @@ def test_long_grammar_outputs_may_be_null(bank):
     """each output pointer NULL in turn, and every one but n_words: the fields passed equal the full call's. With atap
     NULL and n_len = 0 (no calibration overwrites it) the call starts from zeros although the previous call on the handle
     left another atap in the workspace the NULL path uses"""
-    import oracle_long as ol
     B, U, MS, MW = 4, 60001, 5, 40
     lens = np.array([U, 2000, 50000, 30000], np.uint32)
-    pcm = ol.synth_long(B, U, 0x13A6)
+    pcm = ox.synth_long(B, U, 0x13A6)
     h = _handle(bank)
     full = h.recognise_long_grammar(pcm, G13, 1000, MS, MW, 2400, lens)
     _same(full, _long_gram_oracle(pcm, 2400, bank, T, 4096, G13, 1000, MS, MW, lens))
@@ -859,13 +854,9 @@ def test_long_grammar_shares_workspaces_with_the_other_calls(ora):
     1-state sr_connected_grammar_segs_batch, a larger sr_recognise_long_batch, a small K13 call in each geometry, the
     capture grammar and connected calls, then K13 with a larger batch. Each result equals a fresh handle's byte for
     byte, and the fresh handle's equals the CPU oracles"""
-    import oracle_connected as oc
-    import oracle_grammar as og
-    import oracle_long as ol
-    import oracle_long_grammar as olg
     from test_connected import _bank
     from test_long_stream import plant_act, planted_atap
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     bk = _bank(np.random.default_rng(0x13F1), 16, "small", plant=False)     # 16 slots of 1-8 frames, stride 2880
     NS, ST = 16, bk.shape[1]
     g16 = (16, 0xFFFF, [(k, (k + 1) % 16, 0x1) for k in range(16)])          # 16 states x the 4 slots of command 0
@@ -878,11 +869,11 @@ def test_long_grammar_shares_workspaces_with_the_other_calls(ora):
     seg_frm = np.array([7, 0, 300, 1, 818], np.uint32)
     feat = rng.integers(-3000, 3001, (int(seg_frm.sum()), 12)).astype(np.int16)
     seq_seg = np.array([0, 2, 5], np.uint32)
-    pcm3 = ol.synth_long(12, 100000, 0x13F3)
-    pcm4 = ol.synth_long(3, 30000, 0x13F4)
+    pcm3 = ox.synth_long(12, 100000, 0x13F3)
+    pcm4 = ox.synth_long(3, 30000, 0x13F4)
     pcm5 = sr_b200.synth_pcm_host(8, 16000, 0x13F5, 3)
     lens6 = np.array([60000, 59000, 20000, 161, 60000, 45000, 2401, 60000], np.uint32)
-    pcm6 = ol.synth_long(8, 60000, 0x13F6)
+    pcm6 = ox.synth_long(8, 60000, 0x13F6)
 
     def steps():
         yield "big", lambda h: h.recognise_long_grammar(big, g16, 1000, 8, 32, 0, None,
@@ -901,15 +892,15 @@ def test_long_grammar_shares_workspaces_with_the_other_calls(ora):
             w = _long_gram_oracle(big, 0, bk, NS, ST, g16, 1000, 8, 32, atap=planted_atap(1))
             assert int(w["n_segs"][0]) > 2000 and int(w["n_words"][0]) > 2000
         elif name == "segs":
-            w = dict(zip(("words", "n_words", "total"), olg.long_grammar().decode_segs(feat, seq_seg, seg_frm, bk, NS, ST,
-                                                                                        sr_b200.loop_grammar(), 500, 64)))
+            w = dict(zip(("words", "n_words", "total"), ox.long_grammar().decode_segs(feat, seq_seg, seg_frm, bk, NS, ST,
+                                                                                       sr_b200.loop_grammar(), 500, 64)))
         elif name == "long_batch":
-            w = ol.recognise_long(lo, port, pcm3, 2400, bk, NS, ST, 96)
+            w = ox.recognise_long(lo, port, pcm3, 2400, bk, NS, ST, 96)
         elif name.startswith("small"):
             w = _long_gram_oracle(pcm4, 2400, bk, NS, ST, chain, 1000, 16, 16, geom_b=name.endswith("1"))
         elif name == "capture":
-            a = og.recognise_connected_grammar(ora, og.grammar(), pcm5, 2400, bk, NS, ST, chain, 0, 8)
-            b = oc.recognise_connected(ora, oc.connected(), pcm5, 2400, bk, NS, ST, 3000, 8)
+            a = ox.recognise_connected_grammar(ora, ox.grammar(), pcm5, 2400, bk, NS, ST, chain, 0, 8)
+            b = ox.recognise_connected(ora, ox.connected(), pcm5, 2400, bk, NS, ST, 3000, 8)
             w = dict([("g_" + k, v) for k, v in a.items()] + [("c_" + k, v) for k, v in b.items()])
         else:
             w = _long_gram_oracle(pcm6, 2400, bk, NS, ST, chain, 1000, 24, 64, lens6)

@@ -1,9 +1,9 @@
 """Connected words under a finite-state grammar (K6g, an extension the reference does not have; parity unpinned):
 sr_connected_grammar_batch and sr_recognise_connected_grammar_batch.
 
-CPU: the decoder's C restatement (tests/oracle_grammar.c) equals gram_ref, a plain Python cell-level reference written here
-from the definition in speech_recog.h, on random NFAs with segments; its totals equal a minimum over accepted command
-sequences and segmentations built on the unnormalised full DTW of test_connected; the words are accepted, tile every
+CPU: the decoder's C restatement (tests/oracle_ext/long_grammar.c, capture form) equals gram_ref, a plain Python cell-level
+reference written here from the definition in speech_recog.h, on random NFAs with segments; its totals equal a minimum
+over accepted command sequences and segmentations built on the unnormalised full DTW of test_connected; the words are accepted, tile every
 segment and carry their own path sums; the loop grammar is the K6 restatement; a chain of L states gives L words. GPU:
 both calls equal the oracles bit for bit and write only their documented bytes; under the loop grammar they equal
 sr_connected_batch and sr_recognise_connected_batch; a chain grammar recovers digit strings spoken across VAD pauses."""
@@ -13,8 +13,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_connected as oc
-import oracle_grammar as og
+import oracle_ext as ox
 import sr_b200
 from test_connected import _bank, _draw, _enrolled_bank, _members, _slot, dtw_full
 from test_extension_refs import MAX_A, MAX_B, NTHREADS
@@ -24,7 +23,7 @@ PENALTIES = (0, 1, 1000, P_MAX)
 TAG_MFCC, TAG_GRAM = 1, 10
 INF64 = 2 ** 64 - 1
 LOOP = sr_b200.loop_grammar()
-NONE = og.SEG_NONE
+NONE = ox.SEG_NONE
 
 
 # ---- references ---------------------------------------------------------------------------------------------------
@@ -176,7 +175,7 @@ def test_oracle_equals_cell_reference_and_brute_force():
     erased, unsigned and frm_num 0 / 120 slots, N = 0..30 of tie-heavy {0, 1} and +-32 767 rows, every P, 1-3 segments;
     at N <= 8 the total equals brute_total (UINT64_MAX where nothing is accepted); the words' commands are accepted, the
     words tile every segment, each dis is the full DTW of its frames and sum(dis + P) = total"""
-    go = og.grammar()
+    go = ox.grammar()
     rng = np.random.default_rng(0x6A0)
     n_cases = n_multi = n_none = n_brute = 0
     for case in range(160):
@@ -222,7 +221,7 @@ def test_oracle_equals_cell_reference_and_brute_force():
 def test_loop_grammar_is_the_connected_decoder():
     """the one-state loop grammar equals sro_connected bit for bit (words, n_words, total) on one segment, and on 2-3
     segments equals sro_connected of each segment on its own, words joined in order, totals summed"""
-    go, co = og.grammar(), oc.connected()
+    go, co = ox.grammar(), ox.connected()
     rng = np.random.default_rng(0x6A1)
     for case in range(80):
         kind = ("tie", "full", "small")[case % 3]
@@ -256,7 +255,7 @@ def test_loop_grammar_is_the_connected_decoder():
 def test_chain_gives_exactly_L_words():
     """a chain of L + 1 states (arcs k -> k+1 over every command, final state L) gives exactly L words whenever a path
     exists (L <= N), none otherwise, and each word lands in the next state"""
-    go = og.grammar()
+    go = ox.grammar()
     rng = np.random.default_rng(0x6A2)
     n_path = 0
     for case in range(60):
@@ -282,7 +281,7 @@ def test_chain_gives_exactly_L_words():
 def _check_grammar(h, go, feat, frm, bank, T, stride, g, P, max_words, prefill=0x5A, seg=None):
     """the GPU decoder against the oracle, outputs prefilled: records past n_words keep their bytes; two launches agree"""
     h.set_bank(bank, T, stride)
-    w0 = np.frombuffer(bytes([prefill]) * (len(frm) * max_words * 24), oc.WORD_DTYPE).reshape(len(frm), max_words).copy()
+    w0 = np.frombuffer(bytes([prefill]) * (len(frm) * max_words * 24), ox.WORD_DTYPE).reshape(len(frm), max_words).copy()
     got = h.connected_grammar(feat, frm, g, P, max_words, words=w0.copy())
     again = h.connected_grammar(feat, frm, g, P, max_words, words=w0.copy())
     ww, wn, wt = go.decode(feat, frm, bank, T, stride, g, P, max_words, nthreads=NTHREADS)
@@ -313,7 +312,7 @@ def test_grammar_equals_oracle_over_lengths_copies_and_states():
     """N in {0, 1, 2, 119, 120, 500, 818}, copy counts 1, 8, 9, 64, 127 and 128 (every cluster width 1..16 occurs across
     the cases), 1, 2, 5, 12 and 16 states, more states than warps in the cluster (1 copy under 16 states, 8 under 12: a
     warp records several states), max_words below and above the word counts; tag 10 only"""
-    go = og.grammar()
+    go = ox.grammar()
     h = sr_b200.Handle(0)
     h.timing_enable(256)
     rng = np.random.default_rng(0x6A3)
@@ -341,7 +340,7 @@ def test_grammar_equals_oracle_over_lengths_copies_and_states():
 def test_grammar_ties_headroom_averaged_bank_and_batch_position():
     """all-equal rows; the largest local distance at N = 818 (totals beyond 32 bits); random NFAs on tie-heavy rows; an
     sr_average_bank bank under the PIN and command-digit grammars; batch sizes around one and two passes of 132 clusters"""
-    go = og.grammar()
+    go = ox.grammar()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0x6A4)
     eq = _bank(rng, 24, "equal", stride=4096, fmin=1, fmax=119)
@@ -393,7 +392,7 @@ def test_grammar_without_copies():
     have no member, no arcs at all -- decode to 0 words with total 0 or UINT64_MAX as the definition says, at N = 0 and
     N > 0, equal to the oracle; on an erased bank the loop grammar still equals sr_connected_batch, at kernel level and
     end to end"""
-    go = og.grammar()
+    go = ox.grammar()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0x6A9)
     Ns = np.array([0, 1, 5, 119, 818, 0], np.uint32)
@@ -444,7 +443,7 @@ def _twin_case(rng):
 
 def test_source_ties_go_to_the_lowest_state():
     """on _twin_case the restatement equals gram_ref and traces the first word to slot 0"""
-    go = og.grammar()
+    go = ox.grammar()
     rng = np.random.default_rng(0x6AA)
     for case in range(8):
         bank, g, feat, frm = _twin_case(rng)
@@ -459,7 +458,7 @@ def test_source_ties_go_to_the_lowest_state():
 @pytest.mark.gpu
 def test_grammar_source_ties_on_gpu():
     """_twin_case on the GPU equals the restatement: the first word is slot 0"""
-    go = og.grammar()
+    go = ox.grammar()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0x6AB)
     for case in range(8):
@@ -549,7 +548,7 @@ def test_chain_grammar_recovers_strings_across_pauses():
     """4 words spliced with pauses longer than 110 ms, one string over 2-3 VAD segments: the call equals the composed
     oracle on every candidate (outputs prefilled); on the cases where the oracle recovers the spliced sequence, a 4-word
     chain grammar returns exactly that command sequence across segments"""
-    go = og.grammar()
+    go = ox.grammar()
     ora = ob.best_oracle()
     h = sr_b200.Handle(0)
     h.timing_enable(64)
@@ -557,7 +556,7 @@ def test_chain_grammar_recovers_strings_across_pauses():
     rng = np.random.default_rng(0x6A7)
     pcm, seqs, bank = _paused_captures(h, ora, n_cmd, 0x6A70000, 24, rng)
     g = sr_b200.chain_grammar(4, (1 << n_cmd) - 1)
-    want = og.recognise_connected_grammar(ora, go, pcm, 2400, bank, 4 * n_cmd, 4096, g, 0, 8, nthreads=NTHREADS)
+    want = ox.recognise_connected_grammar(ora, go, pcm, 2400, bank, 4 * n_cmd, 4096, g, 0, 8, nthreads=NTHREADS)
     nseg = (want["frm_num"] > 0).sum(1)
     keep = [b for b in range(len(seqs)) if want["status"][b] == 0 and nseg[b] >= 2
             and [int(w["cmd"]) for w in want["words"][b, :want["n_words"][b]]] == seqs[b]]

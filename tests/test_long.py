@@ -1,7 +1,7 @@
 """Long-form VAD and per-segment recognition (include/sr_long.h): recordings of any length up to 2^27 samples, every
 segment, one decision per segment.
 
-CPU: the restatement sro_vad_long (tests/oracle_long.c) equals a plain Python transcription of VAD.C:97-218 with the
+CPU: the restatement sro_vad_long (tests/oracle_ext/long.c) equals a plain Python transcription of VAD.C:97-218 with the
 3-segment cap removed, written here, on planted activity patterns and random PCM; its first three segments equal the port's
 sro_vad and the reference's own VAD, and on any recording the segments that close before sample 65 535 equal the reference's
 VAD on the first 65 535 samples (VAD is causal). A guard parses include/sr_long.h for entry points this file does not run.
@@ -19,11 +19,10 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_long as ol
+import oracle_ext as ox
 import sr_b200
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 NULL = 0xFFFFFFFF
 FIXTURES = ("digits_1_10_a", "digits_1_10_b", "digits_1_9_units_a", "digits_1_9_units_b")
 GROUP_BYTES = 256 << 20            # kLongGroupBytes, csrc/sr_api.cu
@@ -104,7 +103,7 @@ def _check_vad_long(lo, pcm, atap, n=None):
 
 
 def test_vad_long_equals_python_transcription_on_planted_patterns():
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     a = _atap()
     cases = {                                            # (runs of loud / quiet blocks, first run loud)
         "8 active frames open, 7 do not": ([8, 20, 9, 20], True),
@@ -127,7 +126,7 @@ def test_vad_long_equals_python_transcription_on_planted_patterns():
 
 
 def test_vad_long_thousands_of_segments():
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     rng = np.random.default_rng(1)
     runs = []
     for _ in range(2000):
@@ -138,7 +137,7 @@ def test_vad_long_thousands_of_segments():
 
 
 def test_vad_long_equals_python_transcription_on_random_pcm():
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     rng = np.random.default_rng(2)
     for t in range(12):
         n = int(rng.integers(100, 12000))
@@ -153,18 +152,11 @@ def test_vad_long_equals_python_transcription_on_random_pcm():
         _check_vad_long(lo, pcm, a)
 
 
-def _wav(name):
-    with open(os.path.join(GOLDEN, name + ".wav"), "rb") as f:
-        pcm, rate = sr_b200.wav_to_adc12(f.read())
-    assert rate == 8000
-    return pcm
-
-
 def test_first_three_segments_equal_vad_and_reference():
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     ref = ob.ref() if ob.have_ref() else None
-    recs = [_wav(f)[:65535] for f in FIXTURES] + list(sr_b200.synth_pcm_host(6, 40000, 0x10E6, 6))
-    recs.append(ol.synth_long(1, 65535, 0x10E7)[0])
+    recs = [ox.golden_wav(f)[:65535] for f in FIXTURES] + list(sr_b200.synth_pcm_host(6, 40000, 0x10E6, 6))
+    recs.append(ox.synth_long(1, 65535, 0x10E7)[0])
     for pcm in recs:
         n = len(pcm)
         a = port.noise_atap(pcm, 2400)
@@ -181,9 +173,9 @@ def test_first_three_segments_equal_vad_and_reference():
 def test_segments_closing_before_65535_equal_reference_vad():
     """VAD is causal: on any recording, the long-form segments that close before sample 65 535 are the reference's VAD on
     the first 65 535 samples, up to its three segments"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     vad65 = (ob.ref() if ob.have_ref() else port).vad
-    recs = [_wav(f) for f in FIXTURES] + list(ol.synth_long(3, 300000, 0x10E8))
+    recs = [ox.golden_wav(f) for f in FIXTURES] + list(ox.synth_long(3, 300000, 0x10E8))
     for pcm in recs:
         a = port.noise_atap(pcm, 2400)
         cnt, seg = lo.vad_long(pcm[None], a, 256)
@@ -217,12 +209,6 @@ def _bank_of(ftr, valid_slots=None):
     return sr_b200.make_bank(ftr4, 4096, valid), 4 * K
 
 
-def _synth_bank(T=12, seed=0x7E3A0000):
-    tpl = sr_b200.synth_pcm_host(T, 8000, seed)
-    e = ob.port().recognise_batch(tpl, 2400, None, 0, 4096)
-    return sr_b200.make_bank(e["ftr"]), T
-
-
 def _cmp_recognise(got, want, rows=None):
     rows = range(len(want["n_segs"])) if rows is None else rows
     for b in rows:
@@ -234,27 +220,27 @@ def _cmp_recognise(got, want, rows=None):
 
 @pytest.mark.gpu
 def test_fixtures_bit_exact(handle):
-    lo, port = ol.long_oracle(), ob.port()
-    recs = [_wav(f) for f in FIXTURES]
+    lo, port = ox.long_oracle(), ob.port()
+    recs = [ox.golden_wav(f) for f in FIXTURES]
     U = max(len(r) for r in recs)
     pcm = np.zeros((4, U), np.uint16)
     lens = np.array([len(r) for r in recs], np.uint32)
     for b, r in enumerate(recs):
         pcm[b, :len(r)] = r
         pcm[b, len(r):] = 4095                                   # poison past lens[b]
-    bank, T = _synth_bank()
+    bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
     v = handle.vad_long_batch(pcm, 32, 2400, lens)
     n, seg = lo.vad_long(pcm, v["atap"], 32, lens)
     assert v["n_segs"].tolist() == n.tolist() and (v["seg_off"] == seg).all()
     assert v["n_segs"].tolist() == [10, 10, 13, 13], v["n_segs"]
     got = handle.recognise_long_batch(pcm, 32, 2400, lens)
-    _cmp_recognise(got, ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 32, lens))
+    _cmp_recognise(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 32, lens))
 
 
 def _synth_long(lengths, U, seed):
     """recordings of the given lengths (many words each) in rows of U samples, poisoned past their length"""
-    pcm = ol.synth_long(len(lengths), U, seed)
+    pcm = ox.synth_long(len(lengths), U, seed)
     for b, n in enumerate(lengths):
         pcm[b, n:] = np.where(np.arange(U - n) % 2, 4095, 0)
     return pcm
@@ -262,15 +248,15 @@ def _synth_long(lengths, U, seed):
 
 @pytest.mark.gpu
 def test_ragged_synthetic_lengths(handle):
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     lens = np.array([160, 161, 240, 65535, 65536, 1000003, 1 << 24], np.uint32)
     pcm = _synth_long(lens, 1 << 24, 0x10A0)
-    bank, T = _synth_bank()
+    bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
     for geom in (0, 1):
         handle.set_geometry(geom)
         got = handle.recognise_long_batch(pcm, 4096, 2400, lens)
-        want = ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, geom_b=geom == 1)
+        want = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, geom_b=geom == 1)
         _cmp_recognise(got, want)
     handle.set_geometry(0)
     assert int(got["n_segs"][-1]) > 1000
@@ -278,9 +264,9 @@ def test_ragged_synthetic_lengths(handle):
 
 @pytest.mark.gpu
 def test_one_recording_of_2_27_samples(handle):
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     U = 1 << 27
-    pcm = ol.synth_long(1, U, 0x10B0)
+    pcm = ox.synth_long(1, U, 0x10B0)
     v = handle.vad_long_batch(pcm, 40000, 2400)
     n, seg = lo.vad_long(pcm, v["atap"], 40000)
     assert int(v["n_segs"][0]) == int(n[0]) > 1000
@@ -289,32 +275,32 @@ def test_one_recording_of_2_27_samples(handle):
 
 @pytest.mark.gpu
 def test_4096_recordings_of_1_to_30_s(handle):
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     rng = np.random.default_rng(4)
     B, U = 4096, 240000
     lens = rng.integers(8000, U + 1, B).astype(np.uint32)
-    pcm = ol.synth_long(B, U, 0x10C0)
-    bank, T = _synth_bank()
+    pcm = ox.synth_long(B, U, 0x10C0)
+    bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
     got = handle.recognise_long_batch(pcm, 64, 2400, lens)
-    atap = ol.atap_long(port, pcm, 2400, lens)
+    atap = ox.atap_long(port, pcm, 2400, lens)
     n, seg = lo.vad_long(pcm, atap, 64, lens)
     assert got["n_segs"].tolist() == n.tolist()
     assert (got["segs"]["start"] == np.where(np.arange(64)[None] < n[:, None], seg[..., 0], 0)).all()
     rows = sorted({0, B - 1, *rng.integers(0, B, 14).tolist()})
-    _cmp_recognise(got, ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64, lens, rows=rows), rows)
+    _cmp_recognise(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64, lens, rows=rows), rows)
 
 
 @pytest.mark.gpu
 def test_max_segs_cuts_and_prefilled_outputs(handle):
-    lo, port = ol.long_oracle(), ob.port()
-    pcm = ol.synth_long(3, 200000, 0x10D0)
-    bank, T = _synth_bank()
+    lo, port = ox.long_oracle(), ob.port()
+    pcm = ox.synth_long(3, 200000, 0x10D0)
+    bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
-    full = ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64)
+    full = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64)
     assert (full["n_segs"] > 3).all()
     for ms in (0, 1, 3):
-        segs = np.zeros((3, ms), ol.LONG_SEG_DTYPE)
+        segs = np.zeros((3, ms), ox.LONG_SEG_DTYPE)
         segs.view(np.uint32)[...] = PREFILL
         got = handle.recognise_long_batch(pcm, ms, 2400, segs=segs)
         assert got["n_segs"].tolist() == full["n_segs"].tolist()
@@ -324,7 +310,7 @@ def test_max_segs_cuts_and_prefilled_outputs(handle):
         assert v["n_segs"].tolist() == full["n_segs"].tolist()
         assert (v["seg_off"][..., 0] == full["segs"]["start"][:, :ms]).all()
     # records past n_segs keep the caller's bytes
-    segs = np.zeros((3, 64), ol.LONG_SEG_DTYPE)
+    segs = np.zeros((3, 64), ox.LONG_SEG_DTYPE)
     segs.view(np.uint32)[...] = PREFILL
     got = handle.recognise_long_batch(pcm, 64, 2400, segs=segs)
     for b in range(3):
@@ -333,7 +319,7 @@ def test_max_segs_cuts_and_prefilled_outputs(handle):
 
 @pytest.mark.gpu
 def test_full_scale_samples_and_threshold_corners(handle):
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     rng = np.random.default_rng(5)
     U = 150000
     pcm = rng.integers(0, 65536, (6, U)).astype(np.uint16)
@@ -350,7 +336,7 @@ def test_full_scale_samples_and_threshold_corners(handle):
     assert v["n_segs"].tolist() == n.tolist() and (v["seg_off"] == seg).all()
     # noise_atap on full-scale samples
     v = handle.vad_long_batch(pcm, 4096, 2400)
-    assert v["atap"].tobytes() == ol.atap_long(ob.port(), pcm, 2400).tobytes()
+    assert v["atap"].tobytes() == ox.atap_long(ob.port(), pcm, 2400).tobytes()
     n, seg = lo.vad_long(pcm, v["atap"], 4096)
     assert v["n_segs"].tolist() == n.tolist() and (v["seg_off"] == seg).all()
 
@@ -358,13 +344,13 @@ def test_full_scale_samples_and_threshold_corners(handle):
 @pytest.mark.gpu
 def test_dev_forms_at_unaligned_pcm(handle):
     import torch
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     lens = np.array([70001, 161, 123457, 99999], np.uint32)
     U = 123457
     pcm = _synth_long(lens, U, 0x10E0)
-    bank, T = _synth_bank()
+    bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
-    want = ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 40, lens)
+    want = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 40, lens)
     dev = torch.device("cuda:0")
     for off in (2, 6, 14):
         raw = torch.zeros(pcm.nbytes + 64, dtype=torch.uint8, device=dev)
@@ -389,7 +375,7 @@ def test_dev_forms_at_unaligned_pcm(handle):
             m = min(int(n[b]), 40)
             assert (seg[b, :m, 0] == want["segs"]["start"][b, :m]).all() and (seg[b, :m, 1] == want["segs"]["end"][b, :m]).all()
         got = dict(atap=d_atap2.cpu().numpy().view(ob.ATAP_DTYPE), n_segs=d_n2.cpu().numpy().view(np.uint32),
-                   segs=d_segs.cpu().numpy().view(ol.LONG_SEG_DTYPE).reshape(4, 40))
+                   segs=d_segs.cpu().numpy().view(ox.LONG_SEG_DTYPE).reshape(4, 40))
         _cmp_recognise(got, want)
 
 
@@ -399,8 +385,8 @@ def test_composition_with_the_existing_calls(handle, geom):
     """for recordings of <= 65 535 samples: records 0-2 = sr_vad_batch, segment 0 = sr_recognise_batch, every segment =
     sr_mfcc_batch + sr_dtw_batch on its (row, segment), under the greedy walk and r in {10, 15, 118}"""
     B, U = 24, 65535
-    pcm = ol.synth_long(B, U, 0x10F0 + geom)
-    bank, T = _synth_bank()
+    pcm = ox.synth_long(B, U, 0x10F0 + geom)
+    bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
     handle.set_geometry(geom)
     try:
@@ -441,24 +427,24 @@ def test_composition_with_the_existing_calls(handle, geom):
 def test_real_speech_decisions():
     """enrol one digit recording's segments (template k in slot 4k) and recognise the other, both directions, both pairs:
     GPU decisions equal the oracle's. Accuracy is reported (DESIGN.md), not asserted."""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     h = sr_b200.Handle(0)
     try:
         for a_name, b_name in ((FIXTURES[0], FIXTURES[1]), (FIXTURES[1], FIXTURES[0]), (FIXTURES[2], FIXTURES[3]),
                                (FIXTURES[3], FIXTURES[2])):
-            a, b = _wav(a_name), _wav(b_name)
+            a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
             for flags, r in ((0, 0), (2, 118)):
                 h.set_match(flags, r)
                 h.set_bank(np.zeros((0, 4096), np.uint8), 0, 4096)
                 ea = h.recognise_long_batch(a[None], 32, 2400)
                 ma = int(ea["n_segs"][0])
                 at = ea["atap"]
-                ftr = ol.ftr_of_segments(port, a[None], at, [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL else int(s["start"]))
+                ftr = ox.ftr_of_segments(port, a[None], at, [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL else int(s["start"]))
                                                              for s in ea["segs"][0, :ma]])
                 bank, T = _bank_of(ftr)
                 h.set_bank(bank, T, 4096)
                 got = h.recognise_long_batch(b[None], 32, 2400)
-                want = ol.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, band_r=-1 if flags == 0 else r)
+                want = ox.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, band_r=-1 if flags == 0 else r)
                 _cmp_recognise(got, want)
                 m = min(int(got["n_segs"][0]), ma)
                 right = int((got["segs"][0, :m]["cmd"] == np.arange(m)).sum())
@@ -474,7 +460,7 @@ def test_threads_beside_a_recognise_handle():
     lens = np.array([90000, 150000, 40000], np.uint32)
     pcm = _synth_long(lens, 150000, 0x1100)
     short = sr_b200.synth_pcm_host(64, 16000, 0x1110, 3)
-    bank, T = _synth_bank()
+    bank, T = ox.synth_bank()
     dev = torch.device("cuda:0")
 
     def job_vad(h):
@@ -541,10 +527,10 @@ def test_groups_and_launches_are_counted():
     """groups of at most 256 MB of PCM (at least one recording), 3 VAD launches per group (tags 11, 11, 12) and, for
     recognition, 7 more (flat table 2 untimed, get_mfcc, status, best-init, scan, scatter); the segment count of a group
     past one grid pass of every recognition kernel"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     h = sr_b200.Handle(0)
     try:
-        bank, T = _synth_bank()
+        bank, T = ox.synth_bank()
         h.set_bank(bank, T, 4096)
         h.timing_enable(4096)
         U = 1 << 24
@@ -560,7 +546,7 @@ def test_groups_and_launches_are_counted():
                             TAG_BEST_INIT: groups, TAG_DTW: groups, TAG_BEST_FINAL: groups}
         assert int(got["n_segs"][:G].sum()) > 132 * 4 and int(got["n_segs"][G:].sum()) > 132
         rows = [0, G - 1, G, len(lens) - 1, 4]
-        _cmp_recognise(got, ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, rows=rows), rows)
+        _cmp_recognise(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, rows=rows), rows)
         # the same recordings one group at a time
         for g0 in range(0, len(lens), G):
             part = h.recognise_long_batch(pcm[g0:g0 + G], 4096, 2400, lens[g0:g0 + G])

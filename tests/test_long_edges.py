@@ -22,7 +22,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_long as ol
+import oracle_ext as ox
 import sr_b200
 
 NULL = 0xFFFFFFFF
@@ -313,7 +313,7 @@ def test_planted_pcm_realises_its_activity_string():
     """sro_vad_long on the planted PCM equals the sequential FSM on the string: random and run-structured strings, the
     whole edge table; on short strings also the plain transcription of VAD.C (test_long.py)"""
     from test_long import py_vad_long
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     rng = np.random.default_rng(0xED6E)
     acts = [rng.integers(0, 2, int(rng.integers(0, 400))).astype(np.uint8) for _ in range(100)]
     acts += [np.asarray(_runs(rng, int(rng.integers(1, 3000))), np.uint8) for _ in range(100)]
@@ -415,7 +415,7 @@ def _both_vad(h, lo, names, acts, max_segs, offs=(0,), U=None):
 def test_window_edges_bit_exact(handle, w):
     """the edge table with its edge at frame 1 024 w, plus sparse and random strings, through both VAD calls: every
     segment, then cut at MAX_SEGS (the cut cases hold segment MAX_SEGS - 1 or MAX_SEGS open at the edge)"""
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     cases = edge_cases(w) + (sparse_cases() + random_cases(0x5EED + w, 4) if w == 2 else [])
     names, acts = [c[0] for c in cases], [c[1] for c in cases]
     _, _, n = _both_vad(handle, lo, names, acts, 512, offs=(0, 2))
@@ -428,15 +428,15 @@ def test_window_edges_bit_exact(handle, w):
 @pytest.mark.gpu
 def test_window_edges_recognised(handle):
     """sr_recognise_long_batch on the edge table at window 1 against a small bank: every record equals the oracle's"""
-    from test_long import _cmp_recognise, _synth_bank
-    lo, port = ol.long_oracle(), ob.port()
+    from test_long import _cmp_recognise
+    lo, port = ox.long_oracle(), ob.port()
     cases = edge_cases(1)
     pcm, lens = _batch([a for _, a in cases])
-    bank, T = _synth_bank(4)
+    bank, T = ox.synth_bank(4)
     handle.set_bank(bank, T, 4096)
     B = len(cases)
     got = handle.recognise_long_batch(pcm, 128, 0, lens, atap=plant_atap(B))
-    want = ol.recognise_long(lo, port, pcm, 0, bank, T, 4096, 128, lens, atap=plant_atap(B))
+    want = ox.recognise_long(lo, port, pcm, 0, bank, T, 4096, 128, lens, atap=plant_atap(B))
     _cmp_recognise(got, want)
     assert want["n_segs"].max() <= 128 and (want["segs"]["status"] == 0).sum() > B
 
@@ -467,7 +467,7 @@ def _random_acts(rng, B, nfr):
 @pytest.mark.parametrize("U", [2559, 7679])
 def test_block_pass_grid_strides(handle, U):
     """B * cpr items at n W - 1, n W and n W + 1 (the nearest multiples of cpr) for n = 1, 2, W the grid's warps"""
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     c = cpr(U)
     assert c == (1 if U == 2559 else 3)
     W = 8 * block_grid(U, 1 << 20, _sms())
@@ -508,7 +508,7 @@ def test_short_last_items(U):
     """last items of 1-5 blocks, recordings at every staging parity (odd U: rows alternate; host PCM and _dev PCM at
     offset 0 stage at the row's parity, at offset 2 bytes through plain loads), on a handle whose block workspace holds
     an earlier, quiet call's summaries: a block the kernel skips keeps them and moves a segment"""
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     rng = np.random.default_rng(U)
     acts, names = [], []
     for cnb in range(1, 6):
@@ -532,7 +532,7 @@ def test_short_last_items(U):
 @pytest.mark.gpu
 def test_empty_items_are_skipped_over_several_strides(handle):
     """ragged lens: most items of the batch lie past their recording's end, so next_item skips several strides of them"""
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     U = 1 << 20
     c, W = cpr(U), 16 * _sms()
     rng = np.random.default_rng(0xE1)
@@ -557,15 +557,15 @@ def test_empty_items_are_skipped_over_several_strides(handle):
 def test_batch_sizes_recognised(handle, B):
     """recognition past 8 recordings per segment-kernel CTA and 1 024 per prefix-sum pass, max_segs = 2 cutting some rows
     and not others: every record equals the oracle's"""
-    from test_long import _cmp_recognise, _synth_bank
-    lo, port = ol.long_oracle(), ob.port()
+    from test_long import _cmp_recognise
+    lo, port = ox.long_oracle(), ob.port()
     rng = np.random.default_rng(B)
     acts = [np.asarray(_runs(rng, int(rng.integers(1, 200)), 1, 13), np.uint8) for _ in range(B)]
     pcm, lens = _batch(acts)
-    bank, T = _synth_bank(4)
+    bank, T = ox.synth_bank(4)
     handle.set_bank(bank, T, 4096)
     got = handle.recognise_long_batch(pcm, 2, 0, lens, atap=plant_atap(B))
-    want = ol.recognise_long(lo, port, pcm, 0, bank, T, 4096, 2, lens, atap=plant_atap(B))
+    want = ox.recognise_long(lo, port, pcm, 0, bank, T, 4096, 2, lens, atap=plant_atap(B))
     _cmp_recognise(got, want)
     n = want["n_segs"]
     if B > 100:

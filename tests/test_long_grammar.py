@@ -1,12 +1,12 @@
 """One grammar decode per long recording (K13, include/sr_long_grammar.h; an extension the reference does not have, parity
 unpinned): sr_connected_grammar_segs_batch and sr_recognise_long_grammar_batch.
 
-CPU: the decoder's C restatement (tests/oracle_long_grammar.c) equals long_gram_ref, a plain Python cell-level reference
+CPU: the decoder's C restatement (tests/oracle_ext/long_grammar.c) equals long_gram_ref, a plain Python cell-level reference
 written here from the header's definition, on random NFAs over 1-40 segments with 0-frame segments interleaved; its words
 are accepted, stay inside one segment, tile every decodable segment and sum with the penalties to the total; on <= 3
-segments it is the capture decoder's restatement (sro_grammar) and under the loop grammar the per-segment connected decoder
-(sro_connected), joined. GPU: both calls equal the oracles bit for bit, including the u64 headroom corner, launch cuts,
-threads and real speech; the loop grammar equals sr_connected_batch per segment and short recordings equal
+segments it is the capture decoder's restatement (sro_grammar_batch) and under the loop grammar the per-segment connected
+decoder (sro_connected), joined. GPU: both calls equal the oracles bit for bit, including the u64 headroom corner, launch
+cuts, threads and real speech; the loop grammar equals sr_connected_batch per segment and short recordings equal
 sr_recognise_connected_grammar_batch."""
 import os
 import re
@@ -16,14 +16,11 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_connected as oc
-import oracle_grammar as og
-import oracle_long as ol
-import oracle_long_grammar as olg
+import oracle_ext as ox
 import sr_b200
 from test_connected import _bank, _draw, _members, _slot
 from test_grammar import accepts, copies_of, random_grammar
-from test_long import FIXTURES, _bank_of, _synth_long, _wav
+from test_long import FIXTURES, _bank_of, _synth_long
 from test_long_edges import plant, plant_atap
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -131,7 +128,7 @@ def test_oracle_equals_python_reference():
     """sro_long_grammar == long_gram_ref on random NFAs of 1-5 states, banks of 1-6 templates with non-members planted,
     1-40 segments of 0-12 frames, tie-heavy {0, 1} and +-32 767 rows, every P; the words are accepted, stay inside their
     segment, tile every decodable segment and sum with P to the total"""
-    lg = olg.long_grammar()
+    lg = ox.long_grammar()
     rng = np.random.default_rng(0x13A)
     n_multi = 0
     for case in range(90):
@@ -152,8 +149,9 @@ def test_oracle_equals_python_reference():
 
 
 def test_oracle_equals_capture_decoder_on_three_segments():
-    """with <= 3 segments of <= 818 frames in all, sro_long_grammar equals sro_grammar given that segment table"""
-    lg, go = olg.long_grammar(), og.grammar()
+    """with <= 3 segments of <= 818 frames in all, sro_long_grammar equals sro_grammar_batch given the segments' first
+    frames: the adapter's three-entry table"""
+    lg, go = ox.long_grammar(), ox.grammar()
     rng = np.random.default_rng(0x13B)
     for case in range(60):
         kind = ("tie", "full", "small")[case % 3]
@@ -168,9 +166,9 @@ def test_oracle_equals_capture_decoder_on_three_segments():
         x = _draw(rng, N, kind)
         first, f = [], 0
         for n in segs:
-            first.append(f if n else og.SEG_NONE)
+            first.append(f if n else ox.SEG_NONE)
             f += n
-        first += [og.SEG_NONE] * (3 - nseg)
+        first += [ox.SEG_NONE] * (3 - nseg)
         feat = np.zeros((1, max(N, 1), 12), np.int16)
         feat[0, :N] = x
         for P in PENALTIES:
@@ -182,7 +180,7 @@ def test_oracle_equals_capture_decoder_on_three_segments():
 def test_loop_grammar_equals_connected_per_segment():
     """under the loop grammar sro_long_grammar is sro_connected of each decodable segment alone, joined in order (each
     word keeping its segment), the totals summed"""
-    lg, co = olg.long_grammar(), oc.connected()
+    lg, co = ox.long_grammar(), ox.connected()
     rng = np.random.default_rng(0x13C)
     for case in range(40):
         kind = ("tie", "full", "small")[case % 3]
@@ -253,7 +251,7 @@ def _partition_grammar(S, T, rng):
 def test_segs_every_cluster_width_and_state_count(handle):
     """copy counts covering every cluster width 1..16 (C = 8 w copies: w CTAs) at w states, sequences of 1 and 2
     segments of 0, 1, 119, 120 and 818 frames and sequences with no decodable frame or no segment, every P"""
-    lg = olg.long_grammar()
+    lg = ox.long_grammar()
     rng = np.random.default_rng(0x13D)
     for w in range(1, 17):
         T = 8 * w
@@ -271,7 +269,7 @@ def test_segs_every_cluster_width_and_state_count(handle):
 def test_segs_many_segments(handle):
     """sequences of 819, 10 000 and 100 000 segments of 0-12 frames beside ones of 1 and 2, under a random NFA and the
     loop grammar, with max_words below and above the word counts"""
-    lg = olg.long_grammar()
+    lg = ox.long_grammar()
     rng = np.random.default_rng(0x13E)
     bank = _bank(rng, 12, "small")
     handle.set_bank(bank, 12, bank.shape[1])
@@ -290,7 +288,7 @@ def test_segs_headroom(handle):
     """one sequence of 1 677 720 one-frame segments at P = 2^32 - 1 against a 119-frame template at the largest get_dis
     (65 536) from every input row: every frame is a forced word of dis 119 * 65 536 and the total is near 2^52.7. The total,
     every word and the word count equal the oracle's; beyond that sequence's frame limit the call fails"""
-    lg = olg.long_grammar()
+    lg = ox.long_grammar()
     x = np.zeros(12, np.int16)
     x[0] = 32767
     y = np.zeros(12, np.int16)
@@ -353,14 +351,6 @@ def test_segs_loop_grammar_equals_connected_per_segment(handle):
 
 
 # ---- GPU: the end-to-end form ----------------------------------------------------------------------------------------------
-def _synth_bank(h, T=12, seed=0x7E3A0000):
-    tpl = sr_b200.synth_pcm_host(T, 8000, seed)
-    e = ob.port().recognise_batch(tpl, 2400, None, 0, 4096)
-    bank = sr_b200.make_bank(e["ftr"])
-    h.set_bank(bank, T, 4096)
-    return bank, T
-
-
 def _cmp_e2e(got, want, max_segs, max_words, rows=None):
     rows = range(len(want["n_segs"])) if rows is None else rows
     for b in rows:
@@ -397,8 +387,9 @@ def test_recognise_long_grammar_equals_composed_oracle(handle, geom):
     """synthetic recordings of ragged lengths and planted-activity ones (segments over 818 frames, an open last segment),
     three grammars, max_segs 0, 1, below and above n_segs, max_words below and above the word counts, prefilled outputs:
     every record equals the composed oracle and nothing outside the declared records is written"""
-    lo, port, lg = ol.long_oracle(), ob.port(), olg.long_grammar()
-    bank, T = _synth_bank(handle)
+    lo, port, lg = ox.long_oracle(), ob.port(), ox.long_grammar()
+    bank, T = ox.synth_bank()
+    handle.set_bank(bank, T, 4096)
     handle.set_geometry(geom)
     try:
         lens = np.array([160, 161, 30000, 65535, 200001, 240000], np.uint32)
@@ -408,8 +399,8 @@ def test_recognise_long_grammar_equals_composed_oracle(handle, geom):
         grams = (LOOP, sr_b200.chain_grammar(4, 0x7), (2, 3, [(0, 1, 0x5), (1, 0, 0xA), (1, 1, 0x1)]))
         for ci, (x, ln, n_len, at) in enumerate(cases):
             for gi, g in enumerate(grams):
-                want = olg.recognise_long_grammar(lo, port, lg, x, n_len, bank, T, 4096, g, 1000, 64, 256, ln, geom == 1,
-                                                  None if at is None else at.copy())
+                want = ox.recognise_long_grammar(lo, port, lg, x, n_len, bank, T, 4096, g, 1000, 64, 256, ln, geom == 1,
+                                                 None if at is None else at.copy())
                 ns = int(want["n_segs"].max())
                 for max_segs, max_words in ((64, 256), (0, 3), (1, 1), (max(ns - 2, 1), 0)):
                     B = len(ln)
@@ -440,8 +431,9 @@ def test_recognise_long_grammar_equals_composed_oracle(handle, geom):
 def test_short_recordings_equal_the_capture_call(handle):
     """property 2: recordings of <= 65 535 samples (lens = U) whose long-form VAD finds <= 3 segments decode exactly as
     sr_recognise_connected_grammar_batch: words, n_words, total, atap, seg_off and frm_num"""
-    bank, T = _synth_bank(handle)
-    pcm = np.concatenate([sr_b200.synth_pcm_host(24, 40000, 0x1310, 3), ol.synth_long(8, 40000, 0x1311)])
+    bank, T = ox.synth_bank()
+    handle.set_bank(bank, T, 4096)
+    pcm = np.concatenate([sr_b200.synth_pcm_host(24, 40000, 0x1310, 3), ox.synth_long(8, 40000, 0x1311)])
     pcm = np.ascontiguousarray(pcm[:, :40000])
     for g in (LOOP, sr_b200.chain_grammar(3, 0x7), (2, 3, [(0, 1, 0x5), (1, 0, 0xA), (1, 1, 0x1)])):
         got = handle.recognise_long_grammar(pcm, g, 1000, 8, 64)
@@ -480,7 +472,7 @@ def _cuts(N, S):
 def test_record_cuts_and_launch_counts(handle):
     """a batch whose records cut into >= 3 decoder launches and a sequence whose records alone exceed the cap: launches
     per tag follow the host's rule, restated here, every row equals the oracle's and the one-launch slices of the batch"""
-    lg = olg.long_grammar()
+    lg = ox.long_grammar()
     rng = np.random.default_rng(0x141)
     bank = _bank(rng, 16, "small", plant=False)
     handle.set_bank(bank, 16, bank.shape[1])
@@ -515,7 +507,7 @@ def test_groups_and_launches_of_the_end_to_end_call():
     and the decoder's cuts of tag 13; rows equal a call per group"""
     h = sr_b200.Handle(0)
     try:
-        _synth_bank(h)
+        h.set_bank(*ox.synth_bank(), 4096)
         h.timing_enable(4096)
         U = 1 << 24
         lens = np.array([U, U - 7, 3 * 80000, U, 161, U, U - 1, U, 999999, U], np.uint32)
@@ -541,12 +533,13 @@ def test_groups_and_launches_of_the_end_to_end_call():
 @pytest.mark.gpu
 def test_one_recording_of_2_27_samples(handle):
     """one recording of 2^27 samples end to end under a random grammar: equal to the composed oracle"""
-    lo, port, lg = ol.long_oracle(), ob.port(), olg.long_grammar()
-    bank, T = _synth_bank(handle)
-    pcm = ol.synth_long(1, 1 << 27, 0x1330)
+    lo, port, lg = ox.long_oracle(), ob.port(), ox.long_grammar()
+    bank, T = ox.synth_bank()
+    handle.set_bank(bank, T, 4096)
+    pcm = ox.synth_long(1, 1 << 27, 0x1330)
     g = (3, 5, [(0, 1, 0x3), (1, 2, 0x7), (2, 0, 0x7), (1, 1, 0x8)])
     got = handle.recognise_long_grammar(pcm, g, 1000, 100000, 400000)
-    want = olg.recognise_long_grammar(lo, port, lg, pcm, 2400, bank, T, 4096, g, 1000, 100000, 400000)
+    want = ox.recognise_long_grammar(lo, port, lg, pcm, 2400, bank, T, 4096, g, 1000, 100000, 400000)
     assert int(want["n_segs"][0]) > 1000
     _cmp_e2e(got, want, 100000, 400000)
 
@@ -575,7 +568,7 @@ def test_threads_beside_a_recognise_long_handle():
     handles = [sr_b200.Handle(0) for _ in jobs]
     try:
         for h in handles:
-            _synth_bank(h)
+            h.set_bank(*ox.synth_bank(), 4096)
         serial = [j(h) for j, h in zip(jobs, handles)]
         results = [[None] * 3 for _ in jobs]
         errors = []
@@ -607,16 +600,16 @@ def test_real_speech_digit_strings():
     """enrol one digit recording's segments (template k in slot 4k) and decode the other under the loop grammar, a chain
     of "any digit" positions as long as the enrolled list and the ordered chain: GPU equals the oracle. The accuracy (words
     whose command is their position) is printed and recorded in DESIGN.md, not asserted"""
-    lo, port, lg = ol.long_oracle(), ob.port(), olg.long_grammar()
+    lo, port, lg = ox.long_oracle(), ob.port(), ox.long_grammar()
     h = sr_b200.Handle(0)
     try:
         for a_name, b_name in ((FIXTURES[0], FIXTURES[1]), (FIXTURES[1], FIXTURES[0]), (FIXTURES[2], FIXTURES[3]),
                                (FIXTURES[3], FIXTURES[2])):
-            a, b = _wav(a_name), _wav(b_name)
+            a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
             h.set_bank(np.zeros((0, 4096), np.uint8), 0, 4096)
             ea = h.recognise_long_batch(a[None], 32, 2400)
             ma = int(ea["n_segs"][0])
-            ftr = ol.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
+            ftr = ox.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
                                                                   else int(s["start"])) for s in ea["segs"][0, :ma]])
             bank, T = _bank_of(ftr)
             h.set_bank(bank, T, 4096)
@@ -631,7 +624,7 @@ def test_real_speech_digit_strings():
                     print("%s -> %s, %s: %d copies > %d" % (a_name, b_name, name, K * K, sr_b200.GRAM_COPY_MAX))
                     continue
                 got = h.recognise_long_grammar(b[None], g, 1000, 32, 64)
-                want = olg.recognise_long_grammar(lo, port, lg, b[None], 2400, bank, T, 4096, g, 1000, 32, 64)
+                want = ox.recognise_long_grammar(lo, port, lg, b[None], 2400, bank, T, 4096, g, 1000, 32, 64)
                 _cmp_e2e(got, want, 32, 64)
                 n = int(got["n_words"][0])
                 cmds = got["words"][0, :n]["cmd"].tolist()

@@ -23,11 +23,10 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_long as ol
+import oracle_ext as ox
 import sr_b200
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 FIXTURES = ("digits_1_10_a", "digits_1_10_b", "digits_1_9_units_a", "digits_1_9_units_b")
 NULL = 0xFFFFFFFF
 ST_OK, ST_VAD_FAIL, ST_MFCC_FAIL = 0, 1, 2
@@ -235,19 +234,6 @@ def plant_act(act):
     return np.repeat(np.where(loud, LOUD, QUIET).astype(np.uint16), 80)
 
 
-def _wav(name):
-    with open(os.path.join(GOLDEN, name + ".wav"), "rb") as f:
-        pcm, rate = sr_b200.wav_to_adc12(f.read())
-    assert rate == 8000
-    return pcm
-
-
-def _synth_bank(T=12, seed=0x7E3A0000):
-    tpl = sr_b200.synth_pcm_host(T, 8000, seed)
-    e = ob.port().recognise_batch(tpl, 2400, None, 0, 4096)
-    return sr_b200.make_bank(e["ftr"]), T
-
-
 # ---- the prefix definition -----------------------------------------------------------------------------------------------
 def expected(h, xs, ns, n_len, atap0, rows=None):
     """sr_recognise_long_batch on the prefix xs[s][:ns[s]] of each stream: per stream (closed records, open start, atap)"""
@@ -337,7 +323,7 @@ def _uniform(total, c):
 # ---- GPU ------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def bank():
-    return _synth_bank()
+    return ox.synth_bank()
 
 
 @pytest.mark.gpu
@@ -350,7 +336,7 @@ def test_chunk_lengths(handle, bank, c):
         f = Feed(handle, xs, max_chunk, 0, planted_atap(2))
         _drive(f, [[1, 1]] * len(xs[0]) + [[0, 1]] * (len(xs[1]) - len(xs[0])), every=7)
     else:
-        xs = list(ol.synth_long(3, 24000, 0x14C0 + c))
+        xs = list(ox.synth_long(3, 24000, 0x14C0 + c))
         f = Feed(handle, xs, max_chunk, 2400)
         _drive(f, [[k] * 3 for k in _uniform(24000, c)], every=1 if c >= 79 else 0)
     f.check()
@@ -363,7 +349,7 @@ def test_random_ragged_pushes(handle, bank):
     handle.set_bank(bank[0], bank[1], 4096)
     rng = np.random.default_rng(141)
     S, N, max_chunk = 8, 40000, 700
-    xs = list(ol.synth_long(S, N, 0x14D0))
+    xs = list(ox.synth_long(S, N, 0x14D0))
     f = Feed(handle, xs, max_chunk, 2400)
     start = np.zeros(S, int)
     start[3] = 20                                       # a stream that starts late
@@ -466,7 +452,7 @@ def test_frame_caps_and_ring_wrap(handle, bank, geom):
 def test_calibration_lengths(handle, bank, n_len, given):
     handle.set_bank(bank[0], bank[1], 4096)
     S, N, max_chunk = 3, 90000, 500
-    xs = list(ol.synth_long(S, N, 0x14E0 + n_len))
+    xs = list(ox.synth_long(S, N, 0x14E0 + n_len))
     atap0 = None
     if given:
         atap0 = np.zeros(S, sr_b200.ATAP_DTYPE)
@@ -488,7 +474,7 @@ def test_calibration_lengths(handle, bank, n_len, given):
 @pytest.mark.parametrize("c", [80, 640])
 def test_digit_recordings(handle, bank, c):
     handle.set_bank(bank[0], bank[1], 4096)
-    xs = [_wav(n) for n in FIXTURES]
+    xs = [ox.golden_wav(n) for n in FIXTURES]
     f = Feed(handle, xs, 640, 2400)
     N = np.array([len(x) for x in xs])
     while (f.n < N).any():
@@ -502,8 +488,8 @@ def test_digit_recordings(handle, bank, c):
 def test_one_stream_of_2_27_samples_beside_4095_short_ones(handle, bank):
     handle.set_bank(bank[0], bank[1], 4096)
     S, max_chunk, short = 4096, 1 << 16, 20000
-    big = ol.synth_long(1, 1 << 27, 0x14F0)[0]
-    small = ol.synth_long(S - 1, short, 0x14F1)
+    big = ox.synth_long(1, 1 << 27, 0x14F0)[0]
+    small = ox.synth_long(S - 1, short, 0x14F1)
     pool = sr_b200.LongStreamPool(handle, S, max_chunk, 2400)
     got = [[] for _ in range(S)]
     chunk = sr_b200.host_alloc_dev(0, S * max_chunk * 2)
@@ -543,7 +529,7 @@ def test_one_stream_of_2_27_samples_beside_4095_short_ones(handle, bank):
 def test_reset_a_subset_mid_stream(handle, bank):
     handle.set_bank(bank[0], bank[1], 4096)
     S, N, c = 6, 50000, 640
-    xs = list(ol.synth_long(S, N, 0x1500))
+    xs = list(ox.synth_long(S, N, 0x1500))
     atap_r = np.zeros(S, sr_b200.ATAP_DTYPE)
     atap_r["mid_val"] = 77
     f = Feed(handle, xs, c, 2400)
@@ -568,9 +554,9 @@ def test_reset_a_subset_mid_stream(handle, bank):
 
 @pytest.mark.gpu
 def test_matcher_bank_and_geometry_switched_between_pushes(handle, bank):
-    bank2 = _synth_bank(9, 0x7E3B0000)
+    bank2 = ox.synth_bank(9, 0x7E3B0000)
     S, N, c = 4, 60000, 800
-    xs = list(ol.synth_long(S, N, 0x1510))
+    xs = list(ox.synth_long(S, N, 0x1510))
     configs = [(0, 0, 0, bank), (1, 0, 0, bank2), (0, 2, 8, bank), (0, 0, 0, None), (1, 2, 118, bank2)]
     f = Feed(handle, xs, c, 2400)
     rng = np.random.default_rng(7)
@@ -643,7 +629,7 @@ def test_composition_with_fixed_capture_streams(handle, bank):
     """on streams of <= 65 535 samples, after the last push, segments 0-2 equal sr_streams_* events field for field"""
     handle.set_bank(bank[0], bank[1], 4096)
     S, N, c = 16, 65535, 800
-    xs = ol.synth_long(S, N, 0x1520)
+    xs = ox.synth_long(S, N, 0x1520)
     k4 = sr_b200.StreamPool(handle, S, N, 2400)
     f = Feed(handle, list(xs), c, 2400)
     old = []
@@ -666,7 +652,7 @@ def test_composition_with_fixed_capture_streams(handle, bank):
 def test_event_buffer_footprint_and_queue(handle, bank):
     handle.set_bank(bank[0], bank[1], 4096)
     S, N, c = 8, 40000, 640
-    xs = ol.synth_long(S, N, 0x1530)
+    xs = ox.synth_long(S, N, 0x1530)
     ref = sr_b200.LongStreamPool(handle, S, c, 2400)
     pool = sr_b200.LongStreamPool(handle, S, c, 2400)
     assert pool.max_events == S * events_per_push(c, 2400)
@@ -700,7 +686,7 @@ def test_event_buffer_footprint_and_queue(handle, bank):
 @pytest.mark.gpu
 def test_launches_per_push_are_fixed(handle, bank):
     S, c = 32, 640
-    xs = ol.synth_long(S, 32000, 0x1540)
+    xs = ox.synth_long(S, 32000, 0x1540)
     pool = sr_b200.LongStreamPool(handle, S, c, 2400)
     try:
         for with_bank in (True, False):
@@ -720,8 +706,8 @@ def test_launches_per_push_are_fixed(handle, bank):
 @pytest.mark.gpu
 def test_threads_beside_a_long_batch_handle(bank):
     S, N, c = 8, 30000, 640
-    xs = ol.synth_long(S, N, 0x1550)
-    rec = ol.synth_long(4, 200000, 0x1551)
+    xs = ox.synth_long(S, N, 0x1550)
+    rec = ox.synth_long(4, 200000, 0x1551)
 
     def job_pool(h):
         h.set_bank(bank[0], bank[1], 4096)
@@ -780,7 +766,7 @@ def closings_between(closings, n0, n1):
 def test_period_19_string_closes_every_19_frames():
     """the sequential FSM on period_act closes on period_closings for every offset, and the planted PCM realises the
     string under planted_atap (the long-form VAD oracle on the PCM gives the FSM's segments)"""
-    lo = ol.long_oracle()
+    lo = ox.long_oracle()
     for j in range(19):
         act = period_act(600, j)
         x = plant_act(act)
@@ -910,7 +896,7 @@ def calibration_stream(n_frames):
 def test_calibration_stream_realises_its_string_under_its_own_atap():
     """on the CPU: noise_atap over the first 65 520 samples gives mid_val 2 048 and thresholds under which the long-form
     VAD oracle finds exactly the string's segments, 41 of them closing in the calibration window's frames"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     x, act = calibration_stream(900)
     at = port.noise_atap(np.ascontiguousarray(x[:CAL_LEN]), CAL_LEN)
     assert int(at["mid_val"][0]) == 2048 and 369 < int(at["n_thl"][0]) < 450, at

@@ -1,10 +1,10 @@
 """The symmetric slope-constrained DP of Sakoe & Chiba (SR_DTW_SYM_P1, an extension the reference does not have; parity
 unpinned) in sr_dtw_batch and as the matcher of every recognition call (sr_set_match).
 
-CPU: the C oracle (tests/oracle_sym.c) equals a plain Python cell-level reference, and a brute-force enumeration of every
+CPU: the C oracle (tests/oracle_ext/sym.c) equals a plain Python cell-level reference, and a brute-force enumeration of every
 P = 1 path (each complete path weighs I + M, the cheapest one is g); a planted band-edge case and the 65 536 headroom.
 GPU: sr_dtw_batch under SR_DTW_SYM_P1 equals the oracle bit for bit at every radius, bank width and shape; the setter
-rules; every recognition path under the matcher equals the oracle composition (front end, oracle_sym scores, the strict
+rules; every recognition path under the matcher equals the oracle composition (front end, the C oracle's scores, the strict
 '<' first-wins argmin, cmd = idx / 4); the matcher switched between pushes; tag 14 where tag 6 is under the band matcher;
 threads; real speech, reported. sr_recognise_batch_dev_allgather is not run here: it needs two NCCL ranks.
 Every GPU test makes its own handles, so the session handle never carries a matcher."""
@@ -16,13 +16,11 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
-import oracle_long as ol
-import oracle_sym as osym
+import oracle_ext as ox
 import sr_b200
 from test_extension_refs import NTHREADS
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 DIGITS = ("digits_1_10_a", "digits_1_10_b", "digits_1_9_units_a", "digits_1_9_units_b")
 NULL = DIS_ERR = 0xFFFFFFFF
 SYM, BAND, SIGN = sr_b200.DTW_SYM_P1, sr_b200.DTW_BAND, sr_b200.DTW_CHECK_SIGN
@@ -107,7 +105,7 @@ def _ftr(rows_list, frm=None):
 def test_oracle_equals_plain_cell_reference():
     """sro_sym == sym_ref on every I, M in 1..12 (the 2:1 guard's rejects included), every r in 0..12 and 118, with tie-heavy
     {0, 1} rows, +-32 767 rows and small random rows"""
-    so = osym.sym_oracle()
+    so = ox.sym_oracle()
     rng = np.random.default_rng(0x5A1)
     n = n_err = 0
     for k, (I, M) in enumerate(itertools.product(range(1, 13), range(1, 13))):
@@ -128,7 +126,7 @@ def test_oracle_equals_plain_cell_reference():
 def test_brute_force_every_path_weighs_i_plus_m():
     """for I, M <= 7 and r in 0..6: every complete P = 1 path weighs exactly I + M, the cheapest weighted sum is g, and
     the end cell is unreachable exactly when there is no path"""
-    so = osym.sym_oracle()
+    so = ox.sym_oracle()
     rng = np.random.default_rng(0x5A2)
     n_paths = n_unreach = 0
     for I, M in itertools.product(range(1, 8), range(1, 8)):
@@ -174,9 +172,9 @@ def test_planted_band_edge_scores_dis_err():
     I, M, r = case
     rng = np.random.default_rng(0x5A3)
     x, y = _rows(rng, I, "small"), _rows(rng, M, "small")
-    assert sym_ref(x, y, r) is None and osym.sym_oracle().g(x, y, r) is None
+    assert sym_ref(x, y, r) is None and ox.sym_oracle().g(x, y, r) is None
     bank = sr_b200.make_bank(_ftr([y]), STRIDE)
-    assert int(osym.sym_oracle().dtw_batch(_ftr([x]), bank, 1, STRIDE, band_r=r)[0, 0]) == DIS_ERR
+    assert int(ox.sym_oracle().dtw_batch(_ftr([x]), bank, 1, STRIDE, band_r=r)[0, 0]) == DIS_ERR
     assert sym_ref(x, y, r + 1) is not None or not in_band(I - 1, M - 1, I, M, r + 1)
 
 
@@ -184,7 +182,7 @@ def test_headroom_every_get_dis_65536():
     """I = M = 119 with every get_dis 65 536: g = 238 * 65 536, score 65 536"""
     assert get_dis(ROW_HI, ROW_LO) == 65536
     x, y = np.tile(ROW_HI, (119, 1)), np.tile(ROW_LO, (119, 1))
-    so = osym.sym_oracle()
+    so = ox.sym_oracle()
     assert so.g(x, y, 118) == 238 * 65536
     bank = sr_b200.make_bank(_ftr([y]), STRIDE)
     assert int(so.dtw_batch(_ftr([x]), bank, 1, STRIDE, band_r=118)[0, 0]) == 65536
@@ -226,7 +224,7 @@ def _want_best(score):
 def test_dtw_batch_sym_equals_oracle(T):
     """score, best_idx and best_dis of sr_dtw_batch(SR_DTW_SYM_P1[, CHECK_SIGN]) bit for bit against the oracle: every
     radius of RADII, inputs of 0..120 frames (every I in 1..119 over the widths, and the 2:1 edges), planted slots"""
-    so = osym.sym_oracle()
+    so = ox.sym_oracle()
     rng = np.random.default_rng(0x5B0 + T)
     bank = _bank_planted(rng, T)
     M = bank.view(np.uint16)[:, 1].astype(np.int64)
@@ -264,7 +262,7 @@ def test_dtw_batch_sym_headroom_and_band_edge():
         x, y = _rows(rng, I, "small"), _rows(rng, M, "small")
         h.set_bank(sr_b200.make_bank(_ftr([y]), 4096), 1, 4096)
         assert int(h.dtw(_ftr([x]), SYM, r)[0][0, 0]) == DIS_ERR
-        assert int(h.dtw(_ftr([x]), SYM, r + 1)[0][0, 0]) == int(osym.sym_oracle().dtw_batch(
+        assert int(h.dtw(_ftr([x]), SYM, r + 1)[0][0, 0]) == int(ox.sym_oracle().dtw_batch(
             _ftr([x]), sr_b200.make_bank(_ftr([y]), 4096), 1, 4096, band_r=r + 1)[0, 0])
     finally:
         h.close()
@@ -274,7 +272,7 @@ def test_dtw_batch_sym_headroom_and_band_edge():
 @pytest.mark.parametrize("B", (2111, 2112, 2113, 4225))
 def test_dtw_batch_sym_grid_boundaries(B):
     """batches around one grid pass (132 CTAs x 16 warps = 2 112 inputs per tile column) and two, best-only calls"""
-    so = osym.sym_oracle()
+    so = ox.sym_oracle()
     rng = np.random.default_rng(0x5C0 + B)
     T = 32
     fin = _inputs(rng, [int(x) for x in rng.integers(8, 24, B)])
@@ -339,7 +337,7 @@ PLANTED = [0, 1, 1047, 1048, 1049, 2096, 3199]
 def _scores(ftr, bank, T, flags, r):
     """the oracle's template scan under a matcher (flags 0 greedy, BAND, SYM) with the save_sign check"""
     if flags == SYM:
-        return osym.sym_oracle().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r, nthreads=NTHREADS)
+        return ox.sym_oracle().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r, nthreads=NTHREADS)
     return ob.port().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r if flags else -1, nthreads=NTHREADS)[0]
 
 
@@ -431,7 +429,7 @@ def test_recognise_sym_equals_oracle_composition(case, r):
 
 @pytest.mark.gpu
 def test_geom_b_recognise_sym_equals_own_oracle():
-    """GEOM_B features (parity unpinned) under the sym matcher: the port's GEOM_B front end, then oracle_sym"""
+    """GEOM_B features (parity unpinned) under the sym matcher: the port's GEOM_B front end, then tests/oracle_ext/sym.c"""
     po = ob.port()
     h = sr_b200.Handle(0)
     try:
@@ -522,7 +520,7 @@ def _check_k4(events, pool, pcm, bank, T, matcher=None):
                          ids=["lockstep", "ragged", "group_of_two"])
 def test_k4_streams_sym_equal_oracle(case, arrival, group):
     """fixed-capture stream pushes under the sym matcher: every event equals the oracle's get_mfcc of its segment, then
-    oracle_sym and the argmin"""
+    tests/oracle_ext/sym.c and the argmin"""
     S, L, T = 24, 40000, 20
     bank = case["bank"]
     pcm = sr_b200.synth_pcm_host(S, L, 0x5EEDD000, 3)
@@ -570,14 +568,14 @@ LONG_REC = ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")
 
 def long_oracle(pcm, bank, T, flags, r, max_segs, lens=None, geom_b=False):
     """sr_recognise_long_batch composed from the oracles: the long-form VAD and front end, the scan under the matcher"""
-    lo, port = ol.long_oracle(), ob.port()
+    lo, port = ox.long_oracle(), ob.port()
     if flags != SYM:
-        return ol.recognise_long(lo, port, pcm, 2400, bank, T, 4096, max_segs, lens, band_r=r if flags else -1, geom_b=geom_b)
-    want = ol.recognise_long(lo, port, pcm, 2400, bank, 0, 4096, max_segs, lens, geom_b=geom_b)
+        return ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, max_segs, lens, band_r=r if flags else -1, geom_b=geom_b)
+    want = ox.recognise_long(lo, port, pcm, 2400, bank, 0, 4096, max_segs, lens, geom_b=geom_b)
     segs = want["segs"]
     todo = [(b, k) for b in range(len(segs)) for k in range(min(int(want["n_segs"][b]), max_segs)) if segs[b, k]["status"] == 0]
     if todo and T:
-        ftr = ol.ftr_of_segments(port, pcm, want["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
+        ftr = ox.ftr_of_segments(port, pcm, want["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
                                                             for b, k in todo], geom_b)
         sc = _scores(ftr, bank, T, SYM, r)
         for i, (b, k) in enumerate(todo):
@@ -594,22 +592,16 @@ def _cmp_long(got, want):
         assert got["segs"][b, :m].tobytes() == want["segs"][b, :m].tobytes(), (b, got["segs"][b, :m], want["segs"][b, :m])
 
 
-def _synth_bank(T=12, seed=0x7E3A0000):
-    tpl = sr_b200.synth_pcm_host(T, 8000, seed)
-    e = ob.port().recognise_batch(tpl, 2400, None, 0, 4096)
-    return sr_b200.make_bank(e["ftr"]), T
-
-
 @pytest.mark.gpu
 def test_long_batch_and_dev_sym_equal_oracle():
     """sr_recognise_long_batch and its _dev form under SR_DTW_SYM_P1 equal the composed oracle on ragged recordings"""
     import torch
     lens = np.array([70001, 161, 123457, 99999, 200000], np.uint32)
     Ul = 200000
-    pcm = ol.synth_long(len(lens), Ul, 0x5F10)
+    pcm = ox.synth_long(len(lens), Ul, 0x5F10)
     for b, n in enumerate(lens):
         pcm[b, n:] = np.where(np.arange(Ul - n) % 2, 4095, 0)
-    bank, T = _synth_bank()
+    bank, T = ox.synth_bank()
     h = _handle(bank, T, SYM, 10)
     try:
         want = long_oracle(pcm, bank, T, SYM, 10, 64, lens)
@@ -624,7 +616,7 @@ def test_long_batch_and_dev_sym_equal_oracle():
                                    d_segs.data_ptr())
         h.sync()
         _cmp_long(dict(n_segs=d_n.cpu().numpy().view(np.uint32),
-                       segs=d_segs.cpu().numpy().view(ol.LONG_SEG_DTYPE).reshape(len(lens), 64)), want)
+                       segs=d_segs.cpu().numpy().view(ox.LONG_SEG_DTYPE).reshape(len(lens), 64)), want)
     finally:
         h.close()
 
@@ -672,9 +664,9 @@ def _check_k14(events, xs, bank, T, matchers):
 @pytest.mark.gpu
 def test_k14_long_streams_sym_equal_oracle():
     """a live long-stream pool under the sym matcher: every closed segment's event equals the composed oracle"""
-    xs = list(ol.synth_long(6, 120000, 0x5F20))
+    xs = list(ox.synth_long(6, 120000, 0x5F20))
     xs[2] = xs[2][:50000]
-    bank, T = _synth_bank()
+    bank, T = ox.synth_bank()
     h = _handle(bank, T, SYM, 16)
     try:
         pool = sr_b200.LongStreamPool(h, len(xs), 4000, 2400)
@@ -689,8 +681,8 @@ def test_k14_long_streams_sym_equal_oracle():
 def test_k14_matcher_switched_between_pushes():
     """greedy -> sym -> band between the pushes of one live long-stream pool: each event equals the oracle under the
     matcher of the push that returned it"""
-    xs = list(ol.synth_long(4, 160000, 0x5F30))
-    bank, T = _synth_bank()
+    xs = list(ox.synth_long(4, 160000, 0x5F30))
+    bank, T = ox.synth_bank()
     h = _handle(bank, T, 0, 0)
     try:
         pool = sr_b200.LongStreamPool(h, len(xs), 3000, 2400)
@@ -717,7 +709,7 @@ def test_tag_14_where_tag_6_is_under_the_band_matcher(case):
     """the recognise, long-recognise and sr_dtw_batch calls under SYM launch what they launch under BAND, with tag 14 in
     place of tag 6, for r on both sides of every band-kernel choice"""
     pcm, bank = case["pcm"][:64], case["bank"]
-    lpcm = ol.synth_long(3, 100000, 0x5F40)
+    lpcm = ox.synth_long(3, 100000, 0x5F40)
     fin = case["front"]["ftr"][:64]
     h = _handle(bank, 20, 0, 0)
     try:
@@ -747,7 +739,7 @@ def test_threads_under_sym_band_and_greedy(case):
     """handles under sym, band and greedy (recognise and long recognise) run on threads released by one barrier; every
     repetition equals its serial run"""
     pcm, bank = case["pcm"][:256], case["bank"]
-    lpcm = ol.synth_long(3, 120000, 0x5F50)
+    lpcm = ox.synth_long(3, 120000, 0x5F50)
     jobs = []
     for flags, r in ((SYM, 16), (SYM, 4), (BAND, 16), (0, 0)):
         jobs.append((flags, r, "short"))
@@ -791,13 +783,6 @@ def test_threads_under_sym_band_and_greedy(case):
 
 
 # ---- real speech, reported ----------------------------------------------------------------------------------------------
-def _wav(name):
-    with open(os.path.join(GOLDEN, name + ".wav"), "rb") as f:
-        pcm, rate = sr_b200.wav_to_adc12(f.read())
-    assert rate == 8000
-    return pcm
-
-
 @pytest.mark.gpu
 def test_real_speech_sym_reported():
     """enrol each digit recording's segments (template k in slot 4k) and recognise its twin with sr_recognise_long_batch
@@ -807,12 +792,12 @@ def test_real_speech_sym_reported():
     h = sr_b200.Handle(0)
     try:
         for a_name, b_name in ((DIGITS[0], DIGITS[1]), (DIGITS[1], DIGITS[0]), (DIGITS[2], DIGITS[3]), (DIGITS[3], DIGITS[2])):
-            a, b = _wav(a_name), _wav(b_name)
+            a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
             h.set_match(0, 0)
             h.set_bank(np.zeros((0, 4096), np.uint8), 0, 4096)
             ea = h.recognise_long_batch(a[None], 32, 2400)
             ma = int(ea["n_segs"][0])
-            ftr = ol.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
+            ftr = ox.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
                                                                    else int(s["start"])) for s in ea["segs"][0, :ma]])
             ftr4 = np.zeros(4 * ma, ob.FTR_DTYPE)
             ftr4[0::4] = ftr

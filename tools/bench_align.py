@@ -9,7 +9,7 @@ on BASELINE configs[1]-sized inputs (65 536 one-second utterances of synthetic P
   3. sr_recognise_batch_dev at r = 118 against the 20-slot bank (4 per command) and against its averaged bank (one signed
      slot per command, the others erased): ms per step and the DTW kernel's time (tag 6).
 
-Every row checks a sample against the oracles (tests/oracle_align.c, oracle/sr_oracle.c). The card's name, power limit
+Every row checks a sample against the oracles (tests/oracle_ext/align.c, oracle/sr_oracle.c). The card's name, power limit
 and SM clock limit are read in the same run.
 
     python tools/bench_align.py [--steps 10] [--warmup 2] [--json FILE]
@@ -27,7 +27,7 @@ sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python")
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-import oracle_align as oa  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import oracle_bind as ob  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
@@ -87,7 +87,7 @@ def main():
     tf = tftr.cpu().numpy().view(ob.FTR_DTYPE).reshape(T)
     bank20 = sr_b200.make_bank(tf)
     results = {"path": [], "average": [], "recognise": []}
-    ao, po = oa.align(), ob.port()
+    ao, po = ox.align(), ob.port()
 
     # 1. paths: utterance p against template p % T
     mdl = tf[np.arange(B) % T]

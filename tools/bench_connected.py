@@ -6,7 +6,7 @@
   2. sr_recognise_connected_batch on synthetic 3-word captures at U = 16 000 against an enrolled 80-slot bank: wall time
      per call and the kernel time by tag (0 noise_atap + VAD, 1 get_mfcc pieces, 9 the decoder).
 
-Every row checks a sample against the oracles (tests/oracle_connected.c, the composed oracle stages): the first and last
+Every row checks a sample against the oracles (tests/oracle_ext/connected.c, the composed oracle stages): the first and last
 sequence (capture) of every launch -- decoder launches of 2^20 sequences, get_mfcc piece launches of 8 192 pieces -- plus
 random ones, --sample in all. The card's name, power limit and SM clock limit are read in the same run.
 
@@ -26,7 +26,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_connected as oc  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
 from test_connected_launches import _pieces, launch_sample, piece_plan, seq_launches  # noqa: E402
@@ -87,7 +87,7 @@ def main():
         raise SystemExit("bench_connected: no CUDA device (there is nothing to measure without one)")
     B, n = args.batch, args.sample
     h = sr_b200.Handle(0)
-    co = oc.connected()
+    co = ox.connected()
     results = {"decoder": [], "end_to_end": []}
 
     # 1. the decoder: sequences of synthetic feature rows (2 000 structs of 50..100 frames, rows drawn at random)
@@ -127,7 +127,7 @@ def main():
         h.recognise_connected(pcm, PENALTY, 8)
     wall, ker, out = timed(h, lambda: h.recognise_connected(pcm, PENALTY, 8), args.steps)
     idx = launch_sample(e2e_edges(out["frm_num"]), E, n, srng)
-    want = oc.recognise_connected(ob.best_oracle(), co, pcm[idx], 2400, bank, 80, 4096, PENALTY, 8)
+    want = ox.recognise_connected(ob.best_oracle(), co, pcm[idx], 2400, bank, 80, 4096, PENALTY, 8)
     ok = all(np.array_equal(out[k][idx], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
     results["end_to_end"].append({"U": U, "captures": E, "wall_ms": wall, "captures_per_s": E / (wall * 1e-3),
                                   "kernel_ms": {str(k): v for k, v in sorted(ker.items())},

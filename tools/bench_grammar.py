@@ -6,7 +6,7 @@
   3. 11-digit chain: 12 states, 110 copies (11 digit states of 10 averaged digits), sequences of 818 frames;
   4. end to end: 16 384 two-second captures under the PIN grammar.
 Kernel time (tags 9 and 10), sequences/s and cells/s, cells = N * sum of the copies' frame counts. Every row checks a
-sample against the oracle (tests/oracle_grammar.c, the composed oracle stages): the first and last sequence (capture) of
+sample against the oracle (tests/oracle_ext/long_grammar.c, the composed oracle stages): the first and last sequence (capture) of
 every launch -- decoder launches cut at 2^28 bytes of records and at 2^20 sequences, get_mfcc piece launches of 8 192
 pieces -- plus random ones, --sample in all. The card's name, power limit and SM clock limit are read in the same run.
 
@@ -25,7 +25,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_grammar as og  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_connected import e2e_edges, edges, synth_bank, timed  # noqa: E402
 from bench_match import card  # noqa: E402
@@ -77,7 +77,7 @@ def main():
         raise SystemExit("bench_grammar: no CUDA device (there is nothing to measure without one)")
     n = args.sample
     h = sr_b200.Handle(0)
-    go = og.grammar()
+    go = ox.grammar()
     rows = []
     srng = np.random.default_rng(0xB6A5)                  # the oracle samples' random part
 
@@ -135,7 +135,7 @@ def main():
         h.recognise_connected_grammar(pcm, PIN, PENALTY, 8)
     wall, ker, out = timed(h, lambda: h.recognise_connected_grammar(pcm, PIN, PENALTY, 8), args.steps)
     idx = launch_sample(e2e_edges(out["frm_num"], seq_launches(record_cuts(out["frm_num"].sum(1), PIN[0]))), E, n, srng)
-    want = og.recognise_connected_grammar(ob.best_oracle(), go, pcm[idx], 2400, avg, 40, 4096, PIN, PENALTY, 8, nthreads=NPROC)
+    want = ox.recognise_connected_grammar(ob.best_oracle(), go, pcm[idx], 2400, avg, 40, 4096, PIN, PENALTY, 8, nthreads=NPROC)
     ok = all(np.array_equal(out[k][idx], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
     e2e = {"U": U, "captures": E, "wall_ms": wall, "captures_per_s": E / (wall * 1e-3),
            "kernel_ms": {str(k): v for k, v in sorted(ker.items())}, "mean_words": float(out["n_words"].mean()),

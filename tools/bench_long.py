@@ -6,7 +6,7 @@
   2. end to end (sr_recognise_long_batch, host buffers): 4 096 recordings of 30 s against a 12-slot bank, segments/s.
 Kernel times come from the timing tags (11 block pass: its noise_atap launch, then the block summaries; 12 segment pass),
 wall times from a host clock around calls that end in a synchronisation. Every row checks the oracle: the VAD of every
-recording (tests/oracle_long.c), and the per-segment records of sampled recordings (tests/oracle_long.py). The card's
+recording (tests/oracle_ext/long.c), and the per-segment records of sampled recordings (tests/oracle_ext.py). The card's
 name, power limit and SM clock limit are read in the same run.
 
     python tools/bench_long.py [--steps 3] [--warmup 1] [--json FILE]
@@ -25,7 +25,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_long as ol  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
 
@@ -36,7 +36,7 @@ def vad_row(h, B, U, seed, steps, warmup, max_segs):
     """one VAD configuration on device-resident PCM: timings and the oracle check of every recording"""
     import torch
     dev = torch.device("cuda:0")
-    pcm = ol.synth_long(B, U, seed)
+    pcm = ox.synth_long(B, U, seed)
     d_pcm = torch.from_numpy(pcm.view(np.int16)).to(dev)
     d_atap = torch.zeros(B * 12, dtype=torch.uint8, device=dev)
     d_n = torch.zeros(B, dtype=torch.int32, device=dev)
@@ -61,10 +61,10 @@ def vad_row(h, B, U, seed, steps, warmup, max_segs):
     seg_ms = sum(ms for k, (_, ms) in enumerate(rec) if k % 3 == 2) / steps
     # oracle: every recording
     atap = d_atap.cpu().numpy().view(ob.ATAP_DTYPE)
-    n, seg = ol.long_oracle().vad_long(pcm, atap, max_segs)
+    n, seg = ox.long_oracle().vad_long(pcm, atap, max_segs)
     got_n = d_n.cpu().numpy().view(np.uint32)
     got_seg = d_seg.cpu().numpy().view(np.uint32).reshape(B, max_segs, 2)
-    want_atap = ol.atap_long(ob.port(), pcm[: min(B, 64)], 2400)
+    want_atap = ox.atap_long(ob.port(), pcm[: min(B, 64)], 2400)
     ok = (got_n == n).all() and (got_seg == seg).all() and atap[: min(B, 64)].tobytes() == want_atap.tobytes()
     hours = B * U / 8000 / 3600
     nblk = B * (U // 80 + 1)
@@ -76,7 +76,7 @@ def vad_row(h, B, U, seed, steps, warmup, max_segs):
 
 
 def e2e_row(h, B, U, seed, steps, warmup, max_segs, sample):
-    pcm = ol.synth_long(B, U, seed)
+    pcm = ox.synth_long(B, U, seed)
     tpl = sr_b200.synth_pcm_host(12, 8000, 0x7E3A0000)
     e = ob.port().recognise_batch(tpl, 2400, None, 0, 4096)
     bank = sr_b200.make_bank(e["ftr"])
@@ -90,8 +90,8 @@ def e2e_row(h, B, U, seed, steps, warmup, max_segs, sample):
     nseg = int(np.minimum(got["n_segs"], max_segs).sum())
     rng = np.random.default_rng(seed)
     rows = sorted({0, B - 1, *rng.integers(0, B, sample - 2).tolist()})
-    lo, port = ol.long_oracle(), ob.port()
-    want = ol.recognise_long(lo, port, pcm, 2400, bank, 12, 4096, max_segs, rows=rows)
+    lo, port = ox.long_oracle(), ob.port()
+    want = ox.recognise_long(lo, port, pcm, 2400, bank, 12, 4096, max_segs, rows=rows)
     n, _ = lo.vad_long(pcm, got["atap"], max_segs)
     ok = (got["n_segs"] == n).all() and all(
         got["segs"][b].tobytes() == want["segs"][b].tobytes() and got["atap"][b].tobytes() == want["atap"][b].tobytes() for b in rows)

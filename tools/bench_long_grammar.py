@@ -5,7 +5,7 @@ restricted to command k mod 5, which keeps its copies within SR_GRAM_COPY_MAX), 
 enrolments) and the averaged bank (sr_average_bank of each command's 4 enrolments); then one recording of 2^27 samples
 under the loop grammar. Each row reports the decoder's kernel time (timing tag 13), the call's wall time, decoded frames
 per second of decoder time and G cells per second (frames x the summed template lengths of the grammar's copies). Every
-row checks the composed oracle (tests/oracle_long_grammar.py) on the first and last recording of every decoder launch and
+row checks the composed oracle (tests/oracle_ext.py) on the first and last recording of every decoder launch and
 on random others. The card's name and power limit are read in the same run; the JSON goes to tools/results/.
 
     python tools/bench_long_grammar.py [--steps 2] [--warmup 1] [--json FILE]
@@ -24,8 +24,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_long as ol  # noqa: E402
-import oracle_long_grammar as olg  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
 
@@ -84,8 +83,8 @@ def row(h, pcm, bank, T, g, steps, warmup, sample, seed, max_segs=256, max_words
     cells = frames * copy_cells(g, members(bank, T))
     rng = np.random.default_rng(seed)
     rows = sorted(launch_edges(B, U, N, g[0]) | set(rng.integers(0, B, sample).tolist()))
-    want = olg.recognise_long_grammar(ol.long_oracle(), ob.port(), olg.long_grammar(), np.ascontiguousarray(pcm[rows]), 2400,
-                                      bank, T, 4096, g, 1000, max_segs, max_words)
+    want = ox.recognise_long_grammar(ox.long_oracle(), ob.port(), ox.long_grammar(), np.ascontiguousarray(pcm[rows]), 2400,
+                                     bank, T, 4096, g, 1000, max_segs, max_words)
     ok = True
     for i, b in enumerate(rows):
         ok &= int(got["n_words"][b]) == int(want["n_words"][i]) and int(got["total"][b]) == int(want["total"][i])
@@ -112,12 +111,12 @@ def main():
     grams = {"loop": sr_b200.loop_grammar(), "pin4": sr_b200.chain_grammar(4, 0x1F),
              "chain11": (12, 1 << 11, [(k, k + 1, 1 << (k % 5)) for k in range(11)])}
     res = dict(card=card(), rows={})
-    pcm = ol.synth_long(4096, 240000, 0xB30)
+    pcm = ox.synth_long(4096, 240000, 0xB30)
     for bname, bank in (("bank20", bank20), ("averaged", avg)):
         for gname, g in grams.items():
             res["rows"]["4096x30s_%s_%s" % (gname, bname)] = row(h, pcm, bank, 20, g, a.steps, a.warmup, a.sample, 0xB31)
     del pcm
-    big = ol.synth_long(1, 1 << 27, 0xB40)
+    big = ox.synth_long(1, 1 << 27, 0xB40)
     res["rows"]["1x2^27_loop_bank20"] = row(h, big, bank20, 20, grams["loop"], 1, 0, 0, 0xB41, max_segs=1 << 17,
                                              max_words=1 << 19)
     h.close()

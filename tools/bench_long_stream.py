@@ -26,7 +26,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_long as ol  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
 
@@ -114,7 +114,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_long_stream: no CUDA device (there is nothing to measure without one)")
     S, total = args.streams, 8000 * args.seconds
-    recs = ol.synth_long(NREC, 8000 * 60, 0x5EED1400)
+    recs = ox.synth_long(NREC, 8000 * 60, 0x5EED1400)
     tpl = sr_b200.synth_pcm_host(12, 8000, 0x7E3A0000)
     bank = sr_b200.make_bank(ob.port().recognise_batch(tpl, 2400, None, 0, 4096)["ftr"])
     h = sr_b200.Handle(0)

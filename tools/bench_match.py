@@ -10,8 +10,8 @@ several rounds; the symmetric rows and the banded rows without the guard at r = 
 rows at the same radii. The cells of those rows are the guarded banded DP's, so their cells per second compare the same
 work. A sample of every
 matcher's outputs -- the first utterances of the launch and its last ones -- is checked against the oracle's own
-composition: its front end (recognise_pinned), its template scan under the same matcher (oracle_sym for the symmetric DP,
-oracle_rate for the banded DP without the guard),
+composition: its front end (recognise_pinned), its template scan under the same matcher (oracle_ext/sym.c for the symmetric DP,
+oracle_ext/rate.c for the banded DP without the guard),
 the strict '<' first-wins argmin. The card's name, power limit and SM clock limit are read in the same run.
 
     python tools/bench_match.py [--steps 20] [--warmup 3] [--rounds 3] [--json FILE]
@@ -29,8 +29,7 @@ sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python")
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_rate as orate  # noqa: E402
-import oracle_sym as osym  # noqa: E402
+import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 
 U, N_LEN = 8000, 2400
@@ -103,9 +102,9 @@ def main():
         sc, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1,
                                         band_r=r if flags else -1, nthreads=nth)
         if flags == SYM:                    # the symmetric DP's scores; cells: the banded DP's at the same radius
-            sc = osym.sym_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
+            sc = ox.sym_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
         if flags == RATE:                   # without the 2:1 guard; cells as above
-            sc = orate.rate_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
+            sc = ox.rate_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
         return sc, cells
 
     def run(flags, r):
