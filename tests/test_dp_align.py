@@ -22,13 +22,10 @@ ALIGN, AVG_UPDATE = 7, 8                 # tags of sr_timing_collect
 
 
 # ---- references ---------------------------------------------------------------------------------------------------
-def band_path_ref(fin, fmdl, r):
-    """(score, path, D(I-1,M-1)): the whole I x M matrix in exact integers, +inf outside the band |j - floor(i*M/I)| <= r,
-    then the trace-back from (I-1, M-1): the neighbour with the smallest D, ties to the diagonal, then (i, j-1), then
-    (i-1, j). Rejected pairs: (DIS_ERR, [], None)"""
+def band_matrix(fin, fmdl, r):
+    """the whole I x M matrix D(i, j) = d(i, j) + min(D(i-1, j-1), D(i, j-1), D(i-1, j)), D(0, 0) = d(0, 0), in exact
+    integers (lists of lists), +inf outside the band |j - floor(i*M/I)| <= r and where unreachable; no length guard"""
     I, M = len(fin), len(fmdl)
-    if _guard_rejects(I, M) or I > MAX_FRM or M > MAX_FRM:
-        return DIS_ERR, [], None
     d = dist_matrix(fin, fmdl).tolist()
     inf = float("inf")
     D = [[inf] * M for _ in range(I)]
@@ -41,6 +38,17 @@ def band_path_ref(fin, fmdl, r):
             best = min(D[i - 1][j - 1] if i and j else inf, D[i][j - 1] if j else inf, D[i - 1][j] if i else inf)
             if best != inf:
                 D[i][j] = best + d[i][j]
+    return D
+
+
+def band_path_ref(fin, fmdl, r):
+    """(score, path, D(I-1,M-1)): band_matrix, then the trace-back from (I-1, M-1): the neighbour with the smallest D, ties
+    to the diagonal, then (i, j-1), then (i-1, j). Rejected pairs: (DIS_ERR, [], None)"""
+    I, M = len(fin), len(fmdl)
+    if _guard_rejects(I, M) or I > MAX_FRM or M > MAX_FRM:
+        return DIS_ERR, [], None
+    D = band_matrix(fin, fmdl, r)
+    inf = float("inf")
     end = D[I - 1][M - 1]
     if end == inf:
         return DIS_ERR, [], None
