@@ -59,6 +59,7 @@ extern "C" {
 #define SR_ST_OK         0u
 #define SR_ST_VAD_FAIL   1u
 #define SR_ST_MFCC_FAIL  2u
+#define SR_ST_REJECT     3u           /* decided, then turned down by the margin rule SR_DTW_REJECT (extension) */
 
 /* ---- the reference's types (VAD.H:10-22, MFCC.H:18-25), identical layout -------------------- */
 #ifndef SR_NO_REFERENCE_TYPES
@@ -186,6 +187,19 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
  * at the same band_r. SR_DTW_ANY_RATE without SR_DTW_BAND, or with SR_DTW_SYM_P1, fails before any launch and writes
  * nothing. The symmetric P = 1 DP keeps its guard: its slope constraint cannot reach an end cell past 2:1 anyway.
  * Parity unpinned: the reference has no DP; the checker is this project's own CPU restatement. */
+#define SR_DTW_REJECT(q)  ((uint32_t)(q) << 16)  /* runner-up margin rule of q per mille (extension, ABI version 12) */
+/* SR_DTW_REJECT(q), 1 <= q <= 65535 in bits 16-31 of sr_set_match's flags (q = 0, no bits: no rule), lets a recognition
+ * call say "none of these". The reference always names a command (main.c:276-295); the rule applies to each decision it
+ * would return, i.e. an utterance or segment whose status is SR_ST_OK. With d1 = best_dis and c1 = cmd as the call returns
+ * them and d2 the smallest score over the bank slots t with t / SR_FTR_PER_COMM != c1 (the same scores, save_sign
+ * honoured), the decision is rejected iff d2 != SR_DIS_ERR and 1000 * (d2 - d1) < q * d1, computed in 64 bits: the
+ * runner-up command is less than q per mille worse than the winner. With no other command, or only SR_DIS_ERR scores
+ * there, the decision stands. A rejected record gets status SR_ST_REJECT and keeps best_idx, best_dis, cmd and the scores
+ * the call writes without the rule, so a caller can see what was turned down (sr_labels_batch maps it to NULL). The rule
+ * goes with every matcher and applies wherever the handle's matcher is read: sr_recognise_batch (both transports), _dev,
+ * _dev_allgather (whose gathered keys stay the argmin keys), _multi, the fixed-capture stream pools and groups, the
+ * long-recording calls and the live long streams. sr_dtw_batch* have no status to report: any flag bit >= 16 there fails
+ * before any copy or launch and writes nothing. */
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                  uint32_t *score /* [B][n_slot] or NULL */, uint32_t *best_idx /* [B] or NULL */,
                  uint32_t *best_dis /* [B] or NULL */);
@@ -195,9 +209,10 @@ int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, 
  * SR_DTW_ANY_RATE: the same DP without the 2:1 length guard; flags = SR_DTW_SYM_P1: the
  * symmetric P = 1 DP above at radius band_r >= 0. Recognition keeps honouring save_sign (SR_DTW_CHECK_SIGN, main.c:283)
  * under every matcher. Any other flag value (SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE alone among them) or a
- * negative band_r fails and leaves the setting unchanged. sr_get_match returns the flags as set, SR_DTW_ANY_RATE
- * included. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers (with
- * and without SR_DTW_ANY_RATE differ);
+ * negative band_r fails and leaves the setting unchanged. Each of these four may carry SR_DTW_REJECT(q), the margin rule
+ * above. sr_get_match returns the flags as set, SR_DTW_ANY_RATE and the rule's bits included.
+ * sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers (with
+ * and without SR_DTW_ANY_RATE differ, and so do different rules);
  * the ranks of an all-gather cannot be checked without a collective, so every rank must set the same one. Enrolment,
  * sr_get_mdl_batch and the drop-in dtw() keep the greedy walk. */
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r);

@@ -24,6 +24,8 @@
  *    cmd = idx / SR_FTR_PER_COMM.
  *  - Status: SR_ST_VAD_FAIL for an unclosed segment, SR_ST_MFCC_FAIL for 0 frames (which includes segments over 119
  *    frames, as in the reference), SR_ST_OK otherwise. best_idx = 0, best_dis = SR_DIS_ERR, cmd = 0 unless SR_ST_OK.
+ *  - Under the margin rule SR_DTW_REJECT(q) of the handle's matcher (speech_recog.h), an SR_ST_OK segment the rule turns
+ *    down gets SR_ST_REJECT and keeps its best_idx, best_dis and cmd.
  *
  * Recordings are pcm + b*U, with U <= 2^27 and lens[b] <= U (lens NULL: every recording has U samples); no sample at or
  * past lens[b] is read. n_segs[b] is the true segment count; only the first min(n_segs[b], max_segs) records of

@@ -16,6 +16,7 @@
  *      * atap is the call's atap.
  *    The batch call is taken with the same n_len and the same initial atap, under the handle's geometry, matcher (any of
  *    sr_set_match's, SR_DTW_BAND | SR_DTW_ANY_RATE and SR_DTW_SYM_P1 included) and bank as they were at the push that closed each segment.
+ *    The matcher includes its margin rule SR_DTW_REJECT(q), so an event carries SR_ST_REJECT exactly where that call's record does.
  *  - Frame rule: frame k (samples 80k .. 80k + 159) is evaluated once n > 80k + 160, the long-form VAD's
  *    "i < len - 160". A segment [start, end) is therefore reported by the push after which n >= end + 881. This is one
  *    sample later than sr_streams_*, which reports a segment once n >= end + 880 (its frames run to the capture's end).

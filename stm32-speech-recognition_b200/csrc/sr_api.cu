@@ -17,7 +17,7 @@ static int device_numa_node(int device) {
 
 extern "C" {
 
-int sr_abi_version(void) { return 11; }
+int sr_abi_version(void) { return 12; }
 
 int sr_device_count(void) {
     int n = 0;
@@ -111,8 +111,9 @@ int sr_set_dtw_variant(sr_handle *h, int variant) {
 }
 
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
-    SR_REQUIRE(h, h && (flags == 0 || flags == SR_DTW_BAND || flags == (SR_DTW_BAND | SR_DTW_ANY_RATE) ||
-                        flags == SR_DTW_SYM_P1) && band_r >= 0);
+    const uint32_t m = flags & 0xFFFFu;                       // the matcher; bits 16-31 are the margin rule SR_DTW_REJECT(q)
+    SR_REQUIRE(h, h && (m == 0 || m == SR_DTW_BAND || m == (SR_DTW_BAND | SR_DTW_ANY_RATE) || m == SR_DTW_SYM_P1) &&
+                      band_r >= 0);
     h->match_flags = flags;
     h->match_r = band_r;
     return 0;
@@ -189,6 +190,7 @@ static int scan_tag(u32 flags) {
 }
 // the matcher bits of sr_dtw_batch* name one matcher: not SR_DTW_SYM_P1 with SR_DTW_BAND, and SR_DTW_ANY_RATE only
 // as a modifier of SR_DTW_BAND
+// (the margin rule's bits are the recognition calls' own: sr_dtw_batch* refuse them before this is asked)
 static bool scan_flags_ok(u32 flags) {
     return !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)) && (!(flags & SR_DTW_ANY_RATE) || (flags & SR_DTW_BAND));
 }
@@ -421,25 +423,34 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
     SR_REQUIRE(h, scan_flags_ok(flags));
     if (B == 0) return 0;
-    const bool want_best = best_idx || best_dis || cmd;
-    u64 *best = nullptr;
+    // under the margin rule (C > 0) the status is an output of the decision too, and the scan writes per-command keys
+    // after the B argmin keys
+    const u32 C = status ? rule_cols(flags, bank.n) : 0;
+    if (!C) flags &= 0xFFFFu;
+    const bool want_best = best_idx || best_dis || cmd || C;
+    u64 *best = nullptr, *keys = nullptr;
     if (want_best) {
         DevBuf &bb = h->best_sel ? h->best_alt : h->best;
-        SR_CK(h, ensure(bb, (size_t)B * 8));
+        SR_CK(h, ensure(bb, (size_t)B * (1 + C) * 8));
         best = static_cast<u64 *>(bb.p);
-        SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, B, h->stream));
+        keys = C ? best + B : best;
+        SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(keys, (u64)B * (C ? C : 1), h->stream));
     }
     if (bank.n) {
         if (flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) SR_REQUIRE(h, band_r >= 0);
-        SR_LAUNCH(h, scan_tag(flags), launch_scan(h, bank, in, B, flags, band_r, score, best, status));
+        SR_LAUNCH(h, scan_tag(flags), launch_scan(h, bank, in, B, flags, band_r, score, keys, status));
     }
-    if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
+    if (want_best && C)
+        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final_reject(best, keys, B, C, rule_q(flags), best_idx, best_dis, cmd,
+                                                              const_cast<u8 *>(status), h->stream));
+    else if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
     return 0;
 }
 
 extern "C" int sr_dtw_batch_dev(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                                 uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h != nullptr);
+    SR_REQUIRE(h, (flags >> 16) == 0);                                      // no status to report a rejection in
     DeviceGuard g(h->device);
     return dtw_dev_impl(h, h->bank, in, B, flags, band_r, score, best_idx, best_dis, nullptr, nullptr);
 }
@@ -581,7 +592,7 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                  uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h && (B == 0 || in));
-    SR_REQUIRE(h, scan_flags_ok(flags));                                     // before any copy: nothing is written
+    SR_REQUIRE(h, scan_flags_ok(flags) && (flags >> 16) == 0);             // before any copy: nothing is written
     if (B == 0) return 0;
     if (h->bank.n && (flags & (SR_DTW_BAND | SR_DTW_SYM_P1))) SR_REQUIRE(h, band_r >= 0);   // dtw_dev_impl's radius rule
     HostCall c(h, "sr_dtw_batch");
@@ -1185,7 +1196,8 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
     SR_CK(h, ensure(h->lng[3], (size_t)M * 16));                       // seg2[M][2] | row[M] | slot[M]
     SR_CK(h, ensure(h->lng[4], (size_t)M * sizeof(atap_tag)));
     SR_CK(h, ensure(h->lng[5], (size_t)M));
-    SR_CK(h, ensure(h->lng[6], (size_t)M * 8));
+    const u32 C = rule_cols(h->match_flags, h->bank.n);               // the margin rule's per-command keys follow the M keys
+    SR_CK(h, ensure(h->lng[6], (size_t)M * (1 + C) * 8));
     SR_CK(h, ensure(h->lng[7], (size_t)M * kFtrBytes));
     u32 *first = static_cast<u32 *>(h->lng[2].p), *n_flat = first + B;
     u32 *seg2 = static_cast<u32 *>(h->lng[3].p), *row = seg2 + 2 * (size_t)M, *slot = row + M;
@@ -1197,13 +1209,15 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
     SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 1));
     SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, M, seg2, 2, atap_seg, ftr, row, B, n_flat));     // main.c:268
     SR_LAUNCH(h, TAG_STATUS, launch_long_status(seg2, ftr, n_flat, M, status, h->stream));          // main.c:261-274
-    SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(best, M, h->stream));                               // main.c:276-278
+    u64 *keys = C ? best + M : best;
+    SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(keys, (u64)M * (C ? C : 1), h->stream));                  // main.c:276-278
     if (h->bank.n) {                                                   // main.c:279-291, save_sign honoured (main.c:283)
         const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags;
         SR_LAUNCH(h, scan_tag(flags),
-                  launch_scan(h, h->bank, ftr, M, flags, h->match_r, nullptr, best, status, n_flat));
+                  launch_scan(h, h->bank, ftr, M, flags, h->match_r, nullptr, keys, status, n_flat));
     }
-    SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, best, n_flat, M, rec, h->stream));   // main.c:292-294
+    SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, keys, n_flat, M, rec, C, rule_q(h->match_flags),
+                                                     h->stream));                                   // main.c:292-294
     return 0;
 }
 

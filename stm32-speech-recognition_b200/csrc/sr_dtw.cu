@@ -75,7 +75,7 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
             const u32 result = pair_walks(Iraw, Mraw, guard) ? pair((int)Iraw, (int)Mraw, gslots + (size_t)ul * kSlotBytes, trow)
                                                       : SR_DIS_ERR;
             const u32 t = perm ? tfrm[kTileT + tl] : t0 + (u32)tl;   // the original slot number: score column, argmin key
-            emit_pair(score, best, T, u, t, result);
+            emit_pair(score, best, T, u, t, result, flags);
         }
         group_barrier(1 + group, gthreads);                                                          // before restaging
     }
@@ -113,6 +113,25 @@ __global__ void best_final_kernel(const u64 *best, u32 B, u32 *best_idx, u32 *be
     u64 k = best[i];
     u32 idx = (u32)(k & 0xFFFFFFFFull), dis = (u32)(k >> 32);
     if (status && status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }            // main.c:261-274
+    if (best_idx) best_idx[i] = idx;
+    if (best_dis) best_dis[i] = dis;
+    if (cmd) cmd[i] = idx / SR_FTR_PER_COMM;
+}
+// The same under the margin rule SR_DTW_REJECT(q), from the per-command keys [B][C] (key_of): g = rule_group(C) threads
+// per utterance take the row's two smallest keys, the first thread writes the argmin key to best[i] (what an all-gather
+// reads), the fields best_final_kernel writes, and SR_ST_REJECT over an SR_ST_OK status the rule turns down.
+__global__ void best_final_reject_kernel(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 *best_idx, u32 *best_dis,
+                                         u32 *cmd, u8 *status) {
+    const int g = rule_group(C);
+    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
+    const int lane = (int)(threadIdx.x & (u32)(g - 1));
+    if (i >= B) return;                                                         // whole warps: B * g threads
+    const Top2 k = top2_row(keys + (size_t)i * C, C, lane, g);
+    if (lane) return;
+    best[i] = k.k1;
+    u32 idx = (u32)(k.k1 & 0xFFFFFFFFull), dis = (u32)(k.k1 >> 32);
+    if (status && status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }            // main.c:261-274
+    else if (status && margin_rejects(dis, (u32)(k.k2 >> 32), q)) status[i] = SR_ST_REJECT;
     if (best_idx) best_idx[i] = idx;
     if (best_dis) best_dis[i] = dis;
     if (cmd) cmd[i] = idx / SR_FTR_PER_COMM;
@@ -276,15 +295,23 @@ cudaError_t launch_dtw(const void *in_ftr, u32 B, const void *bank, u32 T, u32 s
         return cudaGetLastError();
     });
 }
-cudaError_t launch_best_init(u64 *best, u32 B, cudaStream_t st) {
-    if (B == 0) return cudaSuccess;
-    best_init_kernel<<<(B + 255) / 256, 256, 0, st>>>(best, B);
+cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    if (n > 0xFFFFFF00ull) return cudaErrorInvalidValue;            // 32 GB of keys: past any workspace anyway
+    best_init_kernel<<<(u32)((n + 255) / 256), 256, 0, st>>>(best, (u32)n);
     return cudaGetLastError();
 }
 cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status,
                               cudaStream_t st) {
     if (B == 0) return cudaSuccess;
     best_final_kernel<<<(B + 255) / 256, 256, 0, st>>>(best, B, best_idx, best_dis, cmd, status);
+    return cudaGetLastError();
+}
+cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 *best_idx, u32 *best_dis, u32 *cmd,
+                                     u8 *status, cudaStream_t st) {
+    if (B == 0) return cudaSuccess;
+    const u64 threads = (u64)B * (u32)rule_group(C);
+    best_final_reject_kernel<<<(u32)((threads + 255) / 256), 256, 0, st>>>(best, keys, B, C, q, best_idx, best_dis, cmd, status);
     return cudaGetLastError();
 }
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st) {
@@ -322,7 +349,7 @@ constexpr s32 kInf = 0x3FFFFFFF;
 // slot perm[t] when a bank order is given); each warp stages one utterance at a time and scores it against the Tt
 // templates one after another, the whole warp on one cost matrix: pair(I, M, urow, trow, lane) returns, in every lane, the
 // score of a pair that passed pair_walks(guard). Lane tt keeps the score of template tt; one score row and one atomicMin
-// of the warp's smallest key per utterance. An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in
+// of the warp's smallest key per utterance (under the margin rule, one per lane into its command's key). An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in
 // lane_packed_scan.
 template <class Pair>
 __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
@@ -356,7 +383,10 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
         const bool has_t = lane < Tt;
         const u32 t = !has_t ? 0u : perm ? tfrm[kTileT + lane] : t0 + (u32)lane;   // the original slot number
         if (has_t && score) score[(size_t)u * T + t] = my_result;
-        if (best) {
+        if (best && (flags >> 16)) {                       // margin rule: one key per command, each lane its own
+            if (has_t) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, flags, T, u, t)),
+                                 (unsigned long long)(((u64)my_result << 32) | (u64)t));
+        } else if (best) {
             u64 key = has_t ? (((u64)my_result << 32) | (u64)t) : ~0ull;
 #pragma unroll
             for (int o = 16; o; o >>= 1) { const u64 other = __shfl_xor_sync(0xFFFFFFFFu, key, o); key = other < key ? other : key; }

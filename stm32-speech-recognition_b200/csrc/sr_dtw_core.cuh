@@ -211,12 +211,49 @@ __device__ __forceinline__ K dp_end(const K (&D)[4], int kend, int lend) {
     return __shfl_sync(0xFFFFFFFFu, e, lend);
 }
 
-// score[u][t] and the spch_recg argmin (main.c:276-291) as one 64-bit atomicMin of (result, bank slot t):
-// strict '<', first wins == lexicographic min
-__device__ __forceinline__ void emit_pair(u32 *score, u64 *best, u32 T, u32 u, u32 t, u32 result) {
-    if (score) score[(size_t)u * T + t] = result;
-    if (best) atomicMin(reinterpret_cast<unsigned long long *>(&best[u]), (unsigned long long)(((u64)result << 32) | (u64)t));
+// The argmin key of a pair: (result, bank slot t), strict '<', first wins == lexicographic min. Without the margin rule
+// (flags >> 16 == 0) best has one key per utterance. Under SR_DTW_REJECT(q) the runner-up command depends on the winner,
+// so best is the per-(utterance, command) array [B][ceil(T / 4)] instead: the minimum over its row is the same argmin key,
+// and the second smallest entry of the row is the runner-up command's score.
+__device__ __forceinline__ u64 *key_of(u64 *best, u32 flags, u32 T, u32 u, u32 t) {
+    return (flags >> 16) ? best + (size_t)u * ((T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM) + t / SR_FTR_PER_COMM : best + u;
 }
+// score[u][t] and the spch_recg argmin (main.c:276-291) as one 64-bit atomicMin of the pair's key
+__device__ __forceinline__ void emit_pair(u32 *score, u64 *best, u32 T, u32 u, u32 t, u32 result, u32 flags) {
+    if (score) score[(size_t)u * T + t] = result;
+    if (best) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, flags, T, u, t)),
+                        (unsigned long long)(((u64)result << 32) | (u64)t));
+}
+
+// ---- the margin rule (SR_DTW_REJECT) over one utterance's per-command keys ----------------------------------------
+// The two smallest keys of a row of C per-command keys: k1 is the argmin key, k2 the runner-up command's best key
+// (~0 when there is no other command). A group of g threads (1, or the 32 lanes of a warp) folds a strided part each and
+// merges by shuffles; every lane of the group ends with the row's pair.
+struct Top2 { u64 k1, k2; };
+__device__ __forceinline__ void top2_add(Top2 &a, u64 k) {
+    if (k < a.k1) { a.k2 = a.k1; a.k1 = k; }
+    else if (k < a.k2) a.k2 = k;
+}
+__device__ __forceinline__ Top2 top2_row(const u64 *row, u32 C, int lane, int g) {
+    Top2 a{~0ull, ~0ull};
+    for (u32 c = (u32)lane; c < C; c += (u32)g) top2_add(a, row[c]);
+    if (g == 32) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const u64 b1 = __shfl_xor_sync(0xFFFFFFFFu, a.k1, o), b2 = __shfl_xor_sync(0xFFFFFFFFu, a.k2, o);
+            const u64 lo = a.k1 < b1 ? a.k1 : b1, hi = a.k1 < b1 ? b1 : a.k1, m2 = a.k2 < b2 ? a.k2 : b2;
+            a.k1 = lo;
+            a.k2 = hi < m2 ? hi : m2;
+        }
+    }
+    return a;
+}
+// reject a decision of score d1 whose runner-up command scores d2 (SR_DIS_ERR: none): 1000 (d2 - d1) < q d1 in u64
+__device__ __forceinline__ bool margin_rejects(u32 d1, u32 d2, u32 q) {
+    return d2 != SR_DIS_ERR && 1000ull * (u64)(d2 - d1) < (u64)q * (u64)d1;
+}
+// threads per utterance of the rule's finishers: one for banks of up to 32 commands, a warp for wider ones
+__host__ __device__ __forceinline__ int rule_group(u32 C) { return C > 32 ? 32 : 1; }
 
 // ---- launch geometry --------------------------------------------------------------------------------------------
 // CTA rows per tile column: one CTA per SM over all columns (never a second partial wave), no more than the batch needs

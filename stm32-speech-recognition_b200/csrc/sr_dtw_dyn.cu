@@ -120,7 +120,7 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
     u32 dis = 0, step = 0, slot = 0, out_u = 0, out_t = 0;
     int x = 0, y = 0, I = 0, M = 0, X1 = 0, X2 = 0, ya0 = 0, yb0 = 0, ya1 = 0, yb1 = 0;
     auto finish = [&](u32 result) {
-        emit_pair(score, best, T, out_u, out_t, result);
+        emit_pair(score, best, T, out_u, out_t, result, flags);
         red_release_add_s(&c.done[slot], 1u);
         active = false;
     };

@@ -15,6 +15,7 @@
 // from device memory (no host round trip between VAD and recognition), one D2H copy, ONE synchronisation.
 #include "sr_internal.h"
 #include "sr_vad_core.cuh"
+#include "sr_dtw_core.cuh"
 #include <condition_variable>
 #include <deque>
 
@@ -160,29 +161,49 @@ __global__ void stream_segments_kernel(const StreamState *st, u32 S, u32 *seg_of
     if (n_recv) n_recv[s] = st[s].n;
 }
 
-// status per event from the freshly computed features (MFCC fail = frm_num 0, main.c:269-274) + argmin initialiser
-__global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, u32 cap, u8 *status, u32 *frm, u64 *best) {
+// status per event from the freshly computed features (MFCC fail = frm_num 0, main.c:269-274) + argmin initialiser:
+// best[cap] without the margin rule, its C per-command keys per event under it (kRule)
+template <bool kRule>
+__global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, u32 cap, u8 *status, u32 *frm, u64 *best,
+                                     u32 C) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= min(*n_ev, cap)) return;
     const u32 f = (*reinterpret_cast<const u32 *>(ftr + (size_t)i * kFtrBytes)) >> 16;
     status[i] = f == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;
     frm[i] = f;
-    best[i] = ((u64)SR_DIS_MAX << 32) | 0ull;                        // main.c:276-278
+    if constexpr (kRule) {
+        for (u32 c = 0; c < C; ++c) best[(size_t)i * C + c] = ((u64)SR_DIS_MAX << 32) | 0ull;
+    } else {
+        best[i] = ((u64)SR_DIS_MAX << 32) | 0ull;                    // main.c:276-278
+    }
 }
 
-// final argmin (main.c:285-294) + one packed record per event for a single D2H copy: word 0 of `out` = event count
+// final argmin (main.c:285-294) + one packed record per event for a single D2H copy: word 0 of `out` = event count.
+// Under the margin rule (kRule) rule_group(C) threads per event take the argmin and the runner-up from its C keys, and a
+// decision the rule turns down gets SR_ST_REJECT.
+template <bool kRule>
 __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, u32 cap, const u8 *status, const u32 *frm,
-                                     const u64 *best, sr_stream_event *out_rec, u32 *out_count) {
-    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+                                     const u64 *best, sr_stream_event *out_rec, u32 *out_count, u32 C, u32 q) {
+    const int g = kRule ? rule_group(C) : 1;
+    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
     const u32 ne = min(*n_ev, cap);
     if (i == 0) *out_count = ne;
     if (i >= ne) return;
-    const u64 k = best[i];
+    u64 k;
+    u8 st = status[i];
+    if constexpr (kRule) {
+        const Top2 t2 = top2_row(best + (size_t)i * C, C, (int)(threadIdx.x & (u32)(g - 1)), g);
+        if (threadIdx.x & (u32)(g - 1)) return;
+        k = t2.k1;
+        if (st == SR_ST_OK && margin_rejects((u32)(k >> 32), (u32)(t2.k2 >> 32), q)) st = SR_ST_REJECT;
+    } else {
+        k = best[i];
+    }
     u32 idx = (u32)(k & 0xFFFFFFFFull), dis = (u32)(k >> 32);
     if (status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }
     sr_stream_event r;
     r.stream = ev[i].stream; r.segment = ev[i].segment; r.start = ev[i].start; r.end = ev[i].end;
-    r.status = status[i]; r.frm_num = frm[i]; r.best_idx = idx; r.best_dis = dis; r.cmd = idx / SR_FTR_PER_COMM;
+    r.status = st; r.frm_num = frm[i]; r.best_idx = idx; r.best_dis = dis; r.cmd = idx / SR_FTR_PER_COMM;
     out_rec[i] = r;
 }
 
@@ -255,20 +276,23 @@ int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_
     // recognise the closed segments; every kernel reads the number of events from device memory (upper bound: cap)
     SR_CK(h, launch_mfcc_h(h, pcm, row_len, c.cap, static_cast<const u32 *>(c.seg_ev.p), 2,
                            static_cast<const atap_tag *>(c.atap_ev.p), c.ftr.p, static_cast<const u32 *>(c.map_ev.p), c.S, n_ev));
-    SR_CK(h, ensure(h->best, (size_t)c.cap * 8));
+    const u32 match = h->match_flags, C = rule_cols(match, h->bank.n);   // the handle's matcher, read at every push
+    SR_CK(h, ensure(h->best, (size_t)c.cap * (C ? C : 1) * 8));
     u64 *best = static_cast<u64 *>(h->best.p);
     const u32 gb = (c.cap + 255) / 256;
-    stream_status_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const unsigned char *>(c.ftr.p), n_ev, c.cap,
-                                                   static_cast<u8 *>(c.status.p), static_cast<u32 *>(c.frm.p), best);
+    (C ? stream_status_kernel<true> : stream_status_kernel<false>)<<<gb, 256, 0, h->stream>>>(
+        static_cast<const unsigned char *>(c.ftr.p), n_ev, c.cap, static_cast<u8 *>(c.status.p), static_cast<u32 *>(c.frm.p),
+        best, C);
     SR_CK(h, cudaGetLastError());
-    if (h->bank.n)                                                    // the handle's matcher, read at every push
-        SR_CK(h, launch_scan(h, h->bank, c.ftr.p, c.cap, SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, nullptr, best,
+    if (h->bank.n)
+        SR_CK(h, launch_scan(h, h->bank, c.ftr.p, c.cap, SR_DTW_CHECK_SIGN | match, h->match_r, nullptr, best,
                              static_cast<const u8 *>(c.status.p), n_ev));
     u32 *out_count = static_cast<u32 *>(c.out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(c.out.p) + 16);
-    stream_finish_kernel<<<gb, 256, 0, h->stream>>>(static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap,
-                                                   static_cast<const u8 *>(c.status.p), static_cast<const u32 *>(c.frm.p),
-                                                   best, out_rec, out_count);
+    const u32 gf = C ? (u32)(((u64)c.cap * (u32)rule_group(C) + 255) / 256) : gb;
+    (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<gf, 256, 0, h->stream>>>(
+        static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap, static_cast<const u8 *>(c.status.p),
+        static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match));
     SR_CK(h, cudaGetLastError());
     h->launches += 4 + (h->bank.n ? 1 : 0);
     const u32 quick = c.cap < StreamCore::kQuick ? c.cap : StreamCore::kQuick;

@@ -19,6 +19,16 @@ SEG_NULL = 0xFFFFFFFF
 DIS_ERR = 0xFFFFFFFF
 SAVE_MASK = 12345
 DTW_CHECK_SIGN, DTW_BAND, DTW_SYM_P1, DTW_ANY_RATE = 1, 2, 4, 8
+ST_OK, ST_VAD_FAIL, ST_MFCC_FAIL, ST_REJECT = 0, 1, 2, 3
+
+
+def dtw_reject(q):
+    """SR_DTW_REJECT(q): the runner-up margin rule of q per mille (0 = no rule), OR'ed into set_match's flags"""
+    q = int(q)
+    if not 0 <= q <= 0xFFFF:
+        raise ValueError("margin %d per mille outside 0..65535" % q)
+    return q << 16
+
 PATH_MAX = 237                 # SR_PATH_MAX: the longest warping path, 2 * VV_FRM_MAX - 1 points
 
 ATAP_DTYPE = np.dtype([("mid_val", "<u4"), ("n_thl", "<u2"), ("z_thl", "<u2"), ("s_thl", "<u4")])
@@ -615,7 +625,8 @@ class Handle:
 
     def set_match(self, flags, band_r=0):
         """matcher of the recognition calls: 0 = the reference's greedy walk, DTW_BAND = the banded DP at radius band_r,
-        DTW_BAND | DTW_ANY_RATE = the same DP without the 2:1 length guard, DTW_SYM_P1 = the symmetric slope-constrained (P = 1) DP at radius band_r"""
+        DTW_BAND | DTW_ANY_RATE = the same DP without the 2:1 length guard, DTW_SYM_P1 = the symmetric slope-constrained (P = 1) DP at radius band_r;
+        any of them | dtw_reject(q) turns down (ST_REJECT) a decision whose runner-up command is less than q per mille worse"""
         self._ck(lib().sr_set_match(self._h, int(flags), int(band_r)))
 
     def match(self):
