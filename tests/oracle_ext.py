@@ -2,8 +2,9 @@
   ctypes bindings of oracle/_build/liboracle_ext.so, built by __graft_entry__.build() from tests/oracle_ext/*.c -- the CPU
   restatements of the alignment calls, the connected-word decoder, the grammar decoder (capture and segment-table forms),
   the long-form VAD, the symmetric P = 1 matcher and the banded DP without the 2:1 guard;
-  the end-to-end calls composed from them and the oracle port's stages (mfcc_long, recognise_connected,
-  recognise_connected_grammar, recognise_long, recognise_long_grammar); and the recordings and banks the tests share."""
+  recognition's template scan under every matcher (match_scores) and the end-to-end calls composed from them and the
+  oracle port's stages (compose_recognise, mfcc_long, recognise_connected, recognise_connected_grammar, recognise_long,
+  recognise_long_grammar); and the recordings and banks the tests share."""
 import ctypes as C
 import functools
 import os
@@ -11,6 +12,7 @@ import os
 import numpy as np
 
 from oracle_bind import ATAP_DTYPE, FTR_DTYPE, NULL, PortOracle, _p, segment_rows
+from refs import NTHREADS
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXT_SO = os.path.join(ROOT, "oracle", "_build", "liboracle_ext.so")
@@ -280,6 +282,36 @@ def _front_end(ora, pcm, n_len, atap0, geom_b):
 
 
 # ---- the composed calls ---------------------------------------------------------------------------------------------------
+def match_scores(ftr, bank, n_slot, flags, r, slot_stride=4096):
+    """score [B, n_slot] of recognition's template scan under the matcher set by sr_set_match(flags, r), with the
+    save_sign check: the port's greedy walk (flags 0) and SR_DTW_BAND DP, tests/oracle_ext/rate.c for SR_DTW_BAND |
+    SR_DTW_ANY_RATE, tests/oracle_ext/sym.c for SR_DTW_SYM_P1"""
+    import sr_b200
+    if flags == sr_b200.DTW_SYM_P1:
+        return sym_oracle().dtw_batch(ftr, bank, n_slot, slot_stride, check_sign=1, band_r=r, nthreads=NTHREADS)
+    if flags == sr_b200.DTW_BAND | sr_b200.DTW_ANY_RATE:
+        return rate_oracle().dtw_batch(ftr, bank, n_slot, slot_stride, check_sign=1, band_r=r, nthreads=NTHREADS)
+    return PortOracle().dtw_batch(ftr, bank, n_slot, slot_stride, check_sign=1, band_r=r if flags else -1,
+                                  nthreads=NTHREADS)[0]
+
+
+def compose_recognise(front, bank, T, flags, r):
+    """sr_recognise_batch under the matcher (flags, r) from a front end (oracle_bind.recognise_pinned's atap, seg_off,
+    ftr and status): match_scores on the OK rows, the strict '<' first-wins argmin (main.c:276-294), cmd = idx / 4"""
+    out = {k: front[k].copy() for k in ("atap", "seg_off", "ftr", "status")}
+    B = len(out["status"])
+    out["score"] = np.full((B, T), NULL, np.uint32)
+    out["best_idx"], out["best_dis"], out["cmd"] = np.zeros(B, np.uint32), np.full(B, NULL, np.uint32), np.zeros(B, np.uint32)
+    good = out["status"] == 0
+    sc = match_scores(out["ftr"][good], bank, T, flags, r)
+    out["score"][good] = sc
+    i = np.argmin(sc, axis=1)                # first of the minima == the strict '<' scan from DIS_ERR
+    out["best_idx"][good] = i
+    out["best_dis"][good] = sc[np.arange(len(i)), i]
+    out["cmd"][good] = i // 4
+    return out
+
+
 def recognise_connected(ora, co, pcm, n_len, bank, n_slot, slot_stride, penalty, max_words, geom_b=False, atap0=None):
     """sr_recognise_connected_batch composed from the oracle stages: noise_atap and VAD per row, mfcc_long of every segment
     at frm_cap = 818, the decoder on each segment with frames, the words joined in segment order (segment set), total the
@@ -329,10 +361,11 @@ def recognise_connected_grammar(ora, go, pcm, n_len, bank, n_slot, slot_stride, 
     return out
 
 
-def recognise_long(lo, port, pcm, n_len, bank, n_slot, slot_stride, max_segs, lens=None, band_r=-1, geom_b=False,
+def recognise_long(lo, port, pcm, n_len, bank, n_slot, slot_stride, max_segs, lens=None, match=(0, 0), geom_b=False,
                    atap=None, rows=None):
     """sr_recognise_long_batch from the oracles' stages: dict(atap, n_segs, segs [B, max_segs] LONG_SEG_DTYPE, zeros past
-    n_segs). rows: recordings whose segments get records (None: all; the others' records stay zero)."""
+    n_segs), each segment scored by match_scores under the matcher match = (flags, r). rows: recordings whose segments
+    get records (None: all; the others' records stay zero)."""
     B, U = pcm.shape
     atap = atap_long(port, pcm, n_len, lens, atap)
     n, seg = lo.vad_long(pcm, atap, max_segs, lens)
@@ -353,7 +386,7 @@ def recognise_long(lo, port, pcm, n_len, bank, n_slot, slot_stride, max_segs, le
         return dict(atap=atap, n_segs=n, segs=segs)
     ftr = ftr_of_segments(port, pcm, atap, [(b, st, en) for b, _, st, en in todo], geom_b)
     if n_slot:
-        sc, _ = port.dtw_batch(ftr, bank, n_slot, slot_stride, check_sign=1, band_r=band_r, nthreads=8)
+        sc = match_scores(ftr, bank, n_slot, *match, slot_stride=slot_stride)
     for i, (b, k, st, en) in enumerate(todo):
         r = segs[b, k]
         r["frm_num"] = ftr["frm_num"][i]

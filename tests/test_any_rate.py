@@ -18,14 +18,16 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_extension_refs import NTHREADS
-from test_sym_match import (DIGITS, INT32_MAX, _bank_planted, _cmp_long, _ftr, _inputs, _k14_events, _k4_events, _rows,
-                            _same, _want_best, get_dis)
+from cases import bank_planted, digit_bank, inputs, make_ftr, real_speech_pairs, synth_long_poisoned, tie_rows
+from drive import (check_k4, check_k14, cmp_long, handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np,
+                   same, tags)
+from refs import NTHREADS, rate_ref, want_best
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NULL = DIS_ERR = 0xFFFFFFFF
 BAND, SIGN, SYM, ANY = sr_b200.DTW_BAND, sr_b200.DTW_CHECK_SIGN, sr_b200.DTW_SYM_P1, sr_b200.DTW_ANY_RATE
 RATE = BAND | ANY
+INT32_MAX = 2 ** 31 - 1
 STRIDE = ob.FTR_DTYPE.itemsize
 KERNEL_RADII = (0, 1, 10, 15, 16, 40, 118)           # warp-scan (<= 15), thread form (10), whole row (>= 16)
 # tags of sr_timing_collect
@@ -44,22 +46,6 @@ def test_header_and_binding_define_the_bit():
     assert sr_b200.DTW_ANY_RATE == 8 and len({BAND, SIGN, SYM, ANY}) == 4
 
 
-def rate_ref(x, y, r):
-    """D(I-1, M-1) of the band DP, cell by cell, without any length guard, or None when unreachable"""
-    I, M = len(x), len(y)
-    D = {}
-    for i in range(I):
-        for j in range(M):
-            if abs(j - (i * M) // I) > r:
-                continue
-            prev = [D[c] for c in ((i - 1, j), (i, j - 1), (i - 1, j - 1)) if c in D]
-            if i == j == 0:
-                prev = [0]
-            if prev:
-                D[i, j] = min(prev) + get_dis(x[i], y[j])
-    return D.get((I - 1, M - 1))
-
-
 def test_oracle_equals_plain_reference_on_every_small_shape():
     """sro_rate == rate_ref on every I, M in 1..12 (ratios up to 12:1 both ways) at every r in 0..12 and 118, and the end
     cell outside the band (ceil(M/I) - 1 > r) always scores SR_DIS_ERR"""
@@ -68,12 +54,12 @@ def test_oracle_equals_plain_reference_on_every_small_shape():
     n_far = n_err = 0
     for k, (I, M) in enumerate(itertools.product(range(1, 13), range(1, 13))):
         kind = ("tie", "full", "small")[k % 3]
-        x, y = _rows(rng, I, kind), _rows(rng, M, kind)
-        bank = sr_b200.make_bank(_ftr([y]), STRIDE)
+        x, y = tie_rows(rng, I, kind), tie_rows(rng, M, kind)
+        bank = sr_b200.make_bank(make_ftr([y]), STRIDE)
         for r in list(range(13)) + [118]:
             d = rate_ref(x, y, r)
             assert ro.d(x, y, r) == d, (I, M, r)
-            got = int(ro.dtw_batch(_ftr([x]), bank, 1, STRIDE, band_r=r)[0, 0])
+            got = int(ro.dtw_batch(make_ftr([x]), bank, 1, STRIDE, band_r=r)[0, 0])
             assert got == (DIS_ERR if d is None else d // (I + M)), (I, M, r)
             if M > I and -(-M // I) - 1 > r:
                 assert got == DIS_ERR
@@ -88,8 +74,8 @@ def test_oracle_equals_band_oracle_within_the_guard():
     ro, po = ox.rate_oracle(), ob.port()
     rng = np.random.default_rng(0xA12)
     frms = [1, 2, 3, 59, 60, 61, 118, 119] + [int(v) for v in rng.integers(1, 120, 24)]
-    fin = _inputs(rng, frms)
-    bank = sr_b200.make_bank(_inputs(rng, frms[::-1]), 4096)
+    fin = inputs(rng, frms)
+    bank = sr_b200.make_bank(inputs(rng, frms[::-1]), 4096)
     I = np.array(frms)[:, None]
     M = np.array(frms[::-1])[None, :]
     inside = (I <= 2 * M) & (M <= 2 * I)
@@ -102,35 +88,18 @@ def test_oracle_equals_band_oracle_within_the_guard():
             assert (got != DIS_ERR).all()
 
 
-def _real_speech_pairs():
-    return ((DIGITS[0], DIGITS[1]), (DIGITS[1], DIGITS[0]), (DIGITS[2], DIGITS[3]), (DIGITS[3], DIGITS[2]))
-
-
-def _digit_bank(port, lo, a):
-    """template k = segment k of recording a, in slot 4k (the other slots unsigned)"""
-    ea = ox.recognise_long(lo, port, a[None], 2400, None, 0, 4096, 32)
-    ma = int(ea["n_segs"][0])
-    ftr = ox.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
-                                                          else int(s["start"])) for s in ea["segs"][0, :ma]])
-    ftr4 = np.zeros(4 * ma, ob.FTR_DTYPE)
-    ftr4[0::4] = ftr
-    valid = np.zeros(4 * ma, bool)
-    valid[0::4] = True
-    return sr_b200.make_bank(ftr4, 4096, valid), 4 * ma, ma
-
-
 def test_real_speech_accuracy_on_the_oracles():
     """the digit recordings, each recognised against its twin's segments at r = 118: the band DP gets 6, 8, 3, 3 right
     (20 of 46), the same DP without the guard 4, 8, 9, 8 (29 of 46). A fixed computation on fixed data, not a claim about
     speech in general"""
     lo, port = ox.long_oracle(), ob.port()
     got = []
-    for a_name, b_name in _real_speech_pairs():
+    for a_name, b_name in real_speech_pairs():
         a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
-        bank, T, ma = _digit_bank(port, lo, a)
+        bank, T, ma = digit_bank(port, lo, a)
         row = []
         for flags in (BAND, RATE):
-            w = long_oracle(b[None], bank, T, flags, 118, 32)
+            w = ox.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, match=(flags, 118))
             m = min(int(w["n_segs"][0]), ma)
             row.append(int((w["segs"][0, :m]["cmd"] == np.arange(m)).sum()))
         got.append(tuple(row) + (ma,))
@@ -138,48 +107,6 @@ def test_real_speech_accuracy_on_the_oracles():
 
 
 # ---- oracle compositions -----------------------------------------------------------------------------------------------
-def _scores(ftr, bank, T, flags, r):
-    """the oracle's template scan under a matcher (0 greedy, BAND, RATE) with the save_sign check"""
-    if flags == RATE:
-        return ox.rate_oracle().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r, nthreads=NTHREADS)
-    return ob.port().dtw_batch(ftr, bank, T, 4096, check_sign=1, band_r=r if flags else -1, nthreads=NTHREADS)[0]
-
-
-def _compose(front, bank, T, flags, r):
-    """the front end, then the scan under the matcher, the strict '<' first-wins argmin, cmd = idx / 4"""
-    out = {k: front[k].copy() for k in ("atap", "seg_off", "ftr", "status")}
-    B = len(out["status"])
-    out["score"] = np.full((B, T), NULL, np.uint32)
-    out["best_idx"], out["best_dis"], out["cmd"] = np.zeros(B, np.uint32), np.full(B, NULL, np.uint32), np.zeros(B, np.uint32)
-    good = out["status"] == 0
-    sc = _scores(out["ftr"][good], bank, T, flags, r)
-    out["score"][good] = sc
-    i = np.argmin(sc, axis=1)
-    out["best_idx"][good] = i
-    out["best_dis"][good] = sc[np.arange(len(i)), i]
-    out["cmd"][good] = i // 4
-    return out
-
-
-def long_oracle(pcm, bank, T, flags, r, max_segs, lens=None):
-    """sr_recognise_long_batch composed from the oracles: the long-form VAD and front end, the scan under the matcher"""
-    lo, port = ox.long_oracle(), ob.port()
-    if flags != RATE:
-        return ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, max_segs, lens, band_r=r if flags else -1)
-    want = ox.recognise_long(lo, port, pcm, 2400, bank, 0, 4096, max_segs, lens)
-    segs = want["segs"]
-    todo = [(b, k) for b in range(len(segs)) for k in range(min(int(want["n_segs"][b]), max_segs)) if segs[b, k]["status"] == 0]
-    if todo and T:
-        ftr = ox.ftr_of_segments(port, pcm, want["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
-                                                            for b, k in todo])
-        sc = _scores(ftr, bank, T, RATE, r)
-        for i, (b, k) in enumerate(todo):
-            j = int(np.argmin(sc[i]))
-            if sc[i, j] != NULL:
-                segs[b, k]["best_idx"], segs[b, k]["best_dis"], segs[b, k]["cmd"] = j, sc[i, j], j // 4
-    return want
-
-
 # ---- sr_dtw_batch (GPU) ------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 def test_set_match_and_flag_rules():
@@ -198,8 +125,8 @@ def test_set_match_and_flag_rules():
                 h.set_match(flags, r)
             assert h.match() == (RATE, 7)
         rng = np.random.default_rng(0xA20)
-        h.set_bank(_bank_planted(rng, 8), 8, 4096)
-        fin = _inputs(rng, [30, 40, 50])
+        h.set_bank(bank_planted(rng, 8), 8, 4096)
+        fin = inputs(rng, [30, 40, 50])
         score = np.full((3, 8), 0xA5A5A5A5, np.uint32)
         bi, bd = np.full(3, 0xA5A5A5A5, np.uint32), np.full(3, 0xA5A5A5A5, np.uint32)
         c0 = h.launch_count()
@@ -228,8 +155,8 @@ def _every_shape_case(kind, seed):
     """inputs of 1..119 frames against a 119-slot bank of 119..1 frames: every (I, M) in 1..119 x 1..119 once"""
     rng = np.random.default_rng(seed)
     frms = list(range(1, 120))
-    fin = _ftr([_rows(rng, f, kind) for f in frms])
-    bank = sr_b200.make_bank(_ftr([_rows(rng, f, kind) for f in frms[::-1]]), 4096)
+    fin = make_ftr([tie_rows(rng, f, kind) for f in frms])
+    bank = sr_b200.make_bank(make_ftr([tie_rows(rng, f, kind) for f in frms[::-1]]), 4096)
     return fin, bank
 
 
@@ -251,7 +178,7 @@ def test_dtw_batch_every_shape_equals_oracle(kind):
             want = ro.dtw_batch(fin, bank, 119, 4096, band_r=r, nthreads=NTHREADS)
             score, bi, bd = h.dtw(fin, flags=RATE, band_r=r)
             assert np.array_equal(score, want), (kind, r, np.argwhere(score != want)[:4].tolist())
-            wi, wd = _want_best(want)
+            wi, wd = want_best(want)
             assert np.array_equal(bi, wi) and np.array_equal(bd, wd), (kind, r)
             s2, bi2, bd2 = h.dtw(fin, flags=RATE, band_r=r, want_score=False)
             assert s2 is None and np.array_equal(bi2, wi) and np.array_equal(bd2, wd), (kind, r)
@@ -271,9 +198,9 @@ def test_dtw_batch_planted_slots_equal_oracle(T):
     CHECK_SIGN, at every kernel radius and INT32_MAX"""
     ro = ox.rate_oracle()
     rng = np.random.default_rng(0xA40 + T)
-    bank = _bank_planted(rng, T)
+    bank = bank_planted(rng, T)
     frms = [0, 120, 1, 119, 2, 118, 3, 100] + [int(x) for x in rng.integers(1, 120, 32)]
-    fin = _inputs(rng, frms)
+    fin = inputs(rng, frms)
     h = sr_b200.Handle(0)
     h.set_bank(bank, T, 4096)
     try:
@@ -282,7 +209,7 @@ def test_dtw_batch_planted_slots_equal_oracle(T):
                 want = ro.dtw_batch(fin, bank, T, 4096, check_sign=flags & SIGN, band_r=r, nthreads=NTHREADS)
                 score, bi, bd = h.dtw(fin, flags=flags, band_r=r)
                 assert np.array_equal(score, want), (T, r, flags, np.argwhere(score != want)[:4].tolist())
-                wi, wd = _want_best(want)
+                wi, wd = want_best(want)
                 assert np.array_equal(bi, wi) and np.array_equal(bd, wd), (T, r, flags)
             assert (want[:2] == DIS_ERR).all()
     finally:
@@ -306,7 +233,7 @@ def _stretched_bank():
         rows += [x, x[::3], np.repeat(x, 3, axis=0)[:119]]
     valid = np.ones(24, bool)
     valid[5] = False
-    return sr_b200.make_bank(_ftr(rows), 4096, valid), 24
+    return sr_b200.make_bank(make_ftr(rows), 4096, valid), 24
 
 
 @pytest.fixture(scope="module")
@@ -325,13 +252,6 @@ def case():
     return {"pcm": pcm, "front": front, "bank": bank, "T": T}
 
 
-def _handle(bank, T, flags=RATE, r=0):
-    h = sr_b200.Handle(0)
-    h.set_bank(bank, T, 4096)
-    h.set_match(flags, r)
-    return h
-
-
 def _two_devices():
     import torch
     return torch.cuda.device_count() > 1
@@ -343,26 +263,25 @@ def test_recognise_equals_oracle_composition(case, r):
     """set_match(BAND | ANY_RATE, r): the host call on the plain and the packed transport and sr_recognise_batch_dev on a
     torch stream equal the oracle; sr_recognise_batch_multi too when two devices are visible. The guard changes the
     decision of some utterances"""
-    from test_gpu_parity import _recognise_dev_np
     pcm, front, bank, T = case["pcm"], case["front"], case["bank"], case["T"]
-    want = _compose(front, bank, T, RATE, r)
-    band = _compose(front, bank, T, BAND, r)
+    want = ox.compose_recognise(front, bank, T, RATE, r)
+    band = ox.compose_recognise(front, bank, T, BAND, r)
     good = want["status"] == 0
     assert (want["best_idx"][good] != band["best_idx"][good]).sum() > 10, r
-    h = _handle(bank, T, RATE, r)
+    h = handle(bank, T, RATE, r)
     try:
         h.set_transport(0)
-        _same(h.recognise(pcm, 2400), want, "host plain")
+        same(h.recognise(pcm, 2400), want, "host plain")
         h.set_transport(1)
-        _same(h.recognise(pcm, 2400), want, "host packed")
+        same(h.recognise(pcm, 2400), want, "host packed")
         assert h.transport_stats()[0] > 0
-        _same(_recognise_dev_np(h, pcm, 2400, T), want, "device launch on a torch stream")
+        same(recognise_dev_np(h, pcm, 2400, T), want, "device launch on a torch stream")
         if _two_devices():
             h.use_own_stream()
             h2 = sr_b200.Handle(1)
             h2.set_bank(bank, T, 4096)
             h2.set_match(RATE, r)
-            _same(sr_b200.recognise_multi([h, h2], pcm, 2400, want=sr_b200.RECOG_FIELDS), want, "multi")
+            same(sr_b200.recognise_multi([h, h2], pcm, 2400, want=sr_b200.RECOG_FIELDS), want, "multi")
             h2.close()
     finally:
         h.close()
@@ -373,7 +292,7 @@ def test_multi_refuses_band_beside_any_rate(case):
     """the bit is part of the matcher: sr_recognise_batch_multi over two handles (two devices when visible) refuses BAND
     beside BAND | ANY_RATE at the same radius, and runs once both carry the bit"""
     bank, T, pcm = case["bank"], case["T"], case["pcm"][:64]
-    a = _handle(bank, T, RATE, 16)
+    a = handle(bank, T, RATE, 16)
     b = sr_b200.Handle(1 if _two_devices() else 0)
     b.set_bank(bank, T, 4096)
     b.set_match(BAND, 16)
@@ -386,24 +305,6 @@ def test_multi_refuses_band_beside_any_rate(case):
     finally:
         a.close()
         b.close()
-
-
-def _check_k4(events, pool, pcm, bank, T, matcher):
-    ora = ob.best_oracle()
-    seg, atap = pool.segments()
-    S = pcm.shape[0]
-    closed = [(s, k) for s in range(S) for k in range(3) if seg[s, k, 1] != NULL]
-    assert sorted((e["stream"], e["segment"]) for e, _ in events) == closed and len(closed) >= 2 * S
-    for e, _ in events:
-        s, k = e["stream"], e["segment"]
-        f = ora.mfcc_batch(pcm[s:s + 1], seg[s, k].reshape(1, 2), atap[s:s + 1])
-        assert e["frm_num"] == int(f["frm_num"][0]), e
-        if e["frm_num"] == 0:
-            assert (e["status"], e["best_idx"], e["best_dis"]) == (2, 0, NULL), e
-            continue
-        sc = _scores(f, bank, T, *matcher)
-        i = int(np.argmin(sc[0]))
-        assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (0, i, int(sc[0, i]), i // 4), e
 
 
 @pytest.mark.gpu
@@ -419,14 +320,14 @@ def test_k4_streams_equal_oracle(case, arrival, group):
     bank, T = case["bank"], case["T"]
     pcm = sr_b200.synth_pcm_host(S, L, 0xA5EDD000, 3)
     pcm[3] = 2048
-    hs = [_handle(bank, T, RATE, 16)] + ([sr_b200.Handle(1)] if group else [])
+    hs = [handle(bank, T, RATE, 16)] + ([sr_b200.Handle(1)] if group else [])
     if group:
         hs[1].set_bank(bank, T, 4096)
         hs[1].set_match(RATE, 16)
     try:
         pool = sr_b200.StreamPool(hs if group else hs[0], S, L, 2400)
-        events = _k4_events(pool, pcm, arrival, np.random.default_rng(0xA6))
-        _check_k4(events, pool, pcm, bank, T, (RATE, 16))
+        events = k4_events(pool, pcm, arrival, np.random.default_rng(0xA6))
+        check_k4(events, pool, pcm, bank, T, (RATE, 16))
         pool.close()
     finally:
         for h in hs:
@@ -442,7 +343,7 @@ def _synth_stretched_bank():
     for k, f in enumerate(e["ftr"]):
         x = f["mfcc_dat"][:int(f["frm_num"]) * 12].reshape(-1, 12)
         rows += [x[::3], np.repeat(x, 3, axis=0)[:119]] + ([x] if k % 3 == 0 else [])
-    return sr_b200.make_bank(_ftr(rows), 4096), len(rows)
+    return sr_b200.make_bank(make_ftr(rows), 4096), len(rows)
 
 
 @pytest.mark.gpu
@@ -450,31 +351,19 @@ def _synth_stretched_bank():
 def test_long_batch_and_dev_equal_oracle(r):
     """sr_recognise_long_batch and its _dev form under BAND | ANY_RATE equal the composed oracle on ragged recordings,
     and the guard changes some segments' decisions"""
-    import torch
     lens = np.array([70001, 161, 123457, 99999, 200000], np.uint32)
-    Ul = 200000
-    pcm = ox.synth_long(len(lens), Ul, 0xA610)
-    for b, n in enumerate(lens):
-        pcm[b, n:] = np.where(np.arange(Ul - n) % 2, 4095, 0)
+    pcm = synth_long_poisoned(lens, 200000, 0xA610)
     bank, T = _synth_stretched_bank()
-    h = _handle(bank, T, RATE, r)
+    h = handle(bank, T, RATE, r)
     try:
-        want = long_oracle(pcm, bank, T, RATE, r, 64, lens)
-        band = long_oracle(pcm, bank, T, BAND, r, 64, lens)
+        lo, port = ox.long_oracle(), ob.port()
+        want = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64, lens, match=(RATE, r))
+        band = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64, lens, match=(BAND, r))
         diff = sum((want["segs"][b, :int(want["n_segs"][b])]["best_idx"] != band["segs"][b, :int(band["n_segs"][b])]["best_idx"]).sum()
                    for b in range(len(lens)))
         assert diff > 0, r
-        _cmp_long(h.recognise_long_batch(pcm, 64, 2400, lens), want)
-        dev = torch.device("cuda:0")
-        d_pcm = torch.from_numpy(pcm.view(np.int16)).to(dev)
-        d_lens = torch.from_numpy(lens.view(np.int32)).to(dev)
-        d_n = torch.zeros(len(lens), dtype=torch.int32, device=dev)
-        d_segs = torch.zeros(len(lens) * 64 * 7, dtype=torch.int32, device=dev)
-        h.recognise_long_batch_dev(d_pcm.data_ptr(), Ul, len(lens), d_lens.data_ptr(), 2400, 64, None, d_n.data_ptr(),
-                                   d_segs.data_ptr())
-        h.sync()
-        _cmp_long(dict(n_segs=d_n.cpu().numpy().view(np.uint32),
-                       segs=d_segs.cpu().numpy().view(ox.LONG_SEG_DTYPE).reshape(len(lens), 64)), want)
+        cmp_long(h.recognise_long_batch(pcm, 64, 2400, lens), want)
+        cmp_long(recognise_long_dev_np(h, pcm, lens, 64), want)
     finally:
         h.close()
 
@@ -487,37 +376,17 @@ def test_k14_long_streams_equal_oracle_on_every_prefix():
     xs = list(ox.synth_long(6, 120000, 0xA620))
     xs[2] = xs[2][:50000]
     bank, T = _synth_stretched_bank()
-    h = _handle(bank, T, RATE, 16)
+    h = handle(bank, T, RATE, 16)
     try:
         pool = sr_b200.LongStreamPool(h, len(xs), 4000, 2400)
-        events = _k14_events(pool, xs, 4000)
+        events = k14_events(pool, xs, 4000)
         pool.close()
     finally:
         h.close()
-    S = len(xs)
-    pcm = np.zeros((S, max(len(x) for x in xs)), np.uint16)
-    lens = np.array([len(x) for x in xs], np.uint32)
-    for s, x in enumerate(xs):
-        pcm[s, :len(x)] = x
-    want = long_oracle(pcm, bank, T, RATE, 16, 256, lens)
-    per = [0] * S
-    keys = ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")
-    for e, _ in events:
-        s, k = e["stream"], e["segment"]
-        assert k == per[s]
-        per[s] += 1
-        rec = want["segs"][s, k]
-        assert tuple(int(e[q]) for q in keys) == tuple(int(rec[q]) for q in keys), (e, rec)
-    for s in range(S):
-        assert per[s] == sum(1 for k in range(int(want["n_segs"][s])) if want["segs"][s, k]["status"] != 1), s
-    assert sum(per) > 3 * S
+    check_k14(events, xs, bank, T, [(RATE, 16)])
 
 
 # ---- launches, tags and bytes written (GPU) ----------------------------------------------------------------------------
-def _tags(h):
-    return [t for t, _ in h.timing_collect()]
-
-
 @pytest.mark.gpu
 def test_launches_and_tags_equal_the_band_matchers(case):
     """recognise, long recognise and sr_dtw_batch under BAND | ANY_RATE launch what they launch under BAND, with the
@@ -525,7 +394,7 @@ def test_launches_and_tags_equal_the_band_matchers(case):
     pcm, bank, T = case["pcm"][:64], case["bank"], case["T"]
     lpcm = ox.synth_long(3, 100000, 0xA640)
     fin = case["front"]["ftr"][:64]
-    h = _handle(bank, T, 0, 0)
+    h = handle(bank, T, 0, 0)
     try:
         h.set_transport(0)
         h.timing_enable(4096)
@@ -537,7 +406,7 @@ def test_launches_and_tags_equal_the_band_matchers(case):
                 h.recognise(pcm, 2400)
                 h.recognise_long_batch(lpcm, 32, 2400)
                 h.dtw(fin, flags | SIGN, r)
-                runs[flags] = (h.launch_count() - c0, _tags(h))
+                runs[flags] = (h.launch_count() - c0, tags(h))
             assert runs[RATE] == runs[BAND], r
             assert runs[RATE][1].count(DTW_BAND) == 3 and DTW not in runs[RATE][1]
     finally:
@@ -551,7 +420,7 @@ def test_bytes_written_equal_the_band_matchers(case):
     bank, T = case["bank"], case["T"]
     fin = case["front"]["ftr"][:40]
     B = len(fin)
-    h = _handle(bank, T, RATE, 16)
+    h = handle(bank, T, RATE, 16)
     try:
         for flags in (BAND, RATE, RATE | SIGN):
             score = np.full((B + 1) * T, 0xA5A5A5A5, np.uint32)
@@ -567,7 +436,8 @@ def test_bytes_written_equal_the_band_matchers(case):
             outs[flags] = h.recognise(pcm, 2400)
         for k in outs[BAND]:
             assert np.asarray(outs[RATE][k]).shape == np.asarray(outs[BAND][k]).shape, k
-        _same(outs[RATE], _compose({k: v[:B] for k, v in case["front"].items()}, bank, T, RATE, 16), "recognise")
+        want = ox.compose_recognise({k: v[:B] for k, v in case["front"].items()}, bank, T, RATE, 16)
+        same(outs[RATE], want, "recognise")
     finally:
         h.close()
 
@@ -580,15 +450,15 @@ def test_real_speech_decisions_reported():
     lo, port = ox.long_oracle(), ob.port()
     h = sr_b200.Handle(0)
     try:
-        for a_name, b_name in _real_speech_pairs():
+        for a_name, b_name in real_speech_pairs():
             a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
-            bank, T, ma = _digit_bank(port, lo, a)
+            bank, T, ma = digit_bank(port, lo, a)
             h.set_bank(bank, T, 4096)
             line = []
             for flags, name in ((BAND, "band r=118"), (RATE, "band r=118 any rate")):
                 h.set_match(flags, 118)
                 got = h.recognise_long_batch(b[None], 32, 2400)
-                _cmp_long(got, long_oracle(b[None], bank, T, flags, 118, 32))
+                cmp_long(got, ox.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, match=(flags, 118)))
                 m = min(int(got["n_segs"][0]), ma)
                 line.append("%s %d/%d" % (name, int((got["segs"][0, :m]["cmd"] == np.arange(m)).sum()), m))
             print("%s -> %s: %s" % (a_name, b_name, ", ".join(line)))

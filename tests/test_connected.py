@@ -12,37 +12,22 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_extension_refs import MAX_A, MAX_B, MAX_FRM, NTHREADS, dist_matrix
+from cases import draw, make_slot, random_bank
+from drive import enrolled_bank
+from refs import MAX_A, MAX_B, NTHREADS, bank_members, dtw_full, get_dis
 
 P_MAX = 2 ** 32 - 1
 PENALTIES = (0, 1, 1000, P_MAX)
 TAG_MFCC, TAG_CONN = 1, 9
-SAVE = sr_b200.SAVE_MASK
 
 
 # ---- references ---------------------------------------------------------------------------------------------------
-def _get_dis(a, b):
-    """get_dis (DTW.C:45-62) of two rows: u32-wrapped sum of squares, float32 square root, truncated"""
-    s = sum((int(p) - int(q)) ** 2 for p, q in zip(a, b)) & 0xFFFFFFFF
-    return int(np.sqrt(np.float32(s)))
-
-
-def _members(bank, n_slot, stride):
-    """{slot: rows [M, 12]} of the members: save_sign == SR_SAVE_MASK and 1 <= frm_num <= 119"""
-    out = {}
-    for t in range(n_slot):
-        sign, n = np.frombuffer(bank[t, :4].tobytes(), np.uint16)
-        if sign == SAVE and 1 <= n <= MAX_FRM:
-            out[t] = bank[t, 4:4 + 24 * int(n)].view(np.int16).reshape(int(n), 12).astype(np.int64)
-    return out
-
-
 def cell_ref(x, bank, n_slot, stride, P):
     """the decoder from its definition, cell by cell: (words [(slot, cmd, start, end, dis)], total)"""
     N = len(x)
     if N == 0:
         return [], 0
-    mem = _members(bank, n_slot, stride)
+    mem = bank_members(bank, n_slot, stride)
     if not mem:
         return [], 2 ** 64 - 1
     inf = None
@@ -61,7 +46,7 @@ def cell_ref(x, bank, n_slot, stride, P):
                 diag = prev[j]
                 cands = [c for c in cands if c is not inf]
                 best = min(cands, key=lambda c: (c[0], -c[1])) if cands else inf
-                row.append(inf if best is inf else (best[0] + _get_dis(x[i], y[j]), best[1]))
+                row.append(inf if best is inf else (best[0] + get_dis(x[i], y[j]), best[1]))
             D[t] = row
         ends = [(D[t][-1][0], t, D[t][-1][1]) for t in mem if D[t][-1] is not inf]
         E.append(min(ends, key=lambda e: (e[0], e[1])))
@@ -75,20 +60,6 @@ def cell_ref(x, bank, n_slot, stride, P):
     return words[::-1], E[-1][0]
 
 
-def dtw_full(a, b):
-    """unnormalised DTW over the full matrix, no 2:1 guard: D(I-1, M-1)"""
-    d = dist_matrix(a, b)
-    I, M = d.shape
-    D = np.zeros((I, M), np.int64)
-    for i in range(I):
-        for j in range(M):
-            prev = [D[i - 1, j]] if i else []
-            prev += [D[i, j - 1]] if j else []
-            prev += [D[i - 1, j - 1]] if i and j else []
-            D[i, j] = d[i, j] + (min(prev) if prev else 0)
-    return int(D[I - 1, M - 1])
-
-
 def brute_total(x, mem, P):
     """min over segmentations 0 = b_0 < ... < b_K = N and words t_k of sum(dtw_full(x[b_k-1:b_k], y_t_k) + P)"""
     N = len(x)
@@ -99,36 +70,6 @@ def brute_total(x, mem, P):
 
 
 # ---- inputs -------------------------------------------------------------------------------------------------------
-def _slot(rows, stride, sign=SAVE, frm=None):
-    s = np.full(stride, 0xFF, np.uint8)
-    n = len(rows) if frm is None else frm
-    s[:4] = np.frombuffer(np.array([sign, n], np.uint16).tobytes(), np.uint8)
-    s[4:4 + rows.size * 2] = np.frombuffer(np.ascontiguousarray(rows, np.int16).tobytes(), np.uint8)
-    return s
-
-
-def _draw(rng, n, kind):
-    if kind == "tie":                                     # rows from {0, 1}: ties everywhere
-        return rng.integers(0, 2, (n, 12)).astype(np.int16)
-    if kind == "full":                                    # +-32767
-        return (rng.choice([-1, 1], (n, 12)) * 32767).astype(np.int16)
-    if kind == "equal":
-        return np.tile(np.array([7, -3, 11, 0, -25, 4, 9, -1, 2, 3, -8, 6], np.int16), (n, 1))
-    return rng.integers(-3000, 3001, (n, 12)).astype(np.int16)
-
-
-def _bank(rng, T, kind, stride=2880, fmin=1, fmax=8, plant=True):
-    """T slots of fmin..fmax frames; with plant, non-members mixed in: erased, unsigned, frm_num 0 and frm_num 120"""
-    bank = np.stack([_slot(_draw(rng, int(rng.integers(fmin, fmax + 1)), kind), stride) for _ in range(T)]) if T else \
-        np.zeros((0, stride), np.uint8)
-    if plant and T >= 3:
-        for t in rng.choice(T, min(T - 1, max(1, T // 4)), replace=False):
-            c = int(rng.integers(4))
-            bank[t] = (np.full(stride, 0xFF, np.uint8) if c == 0 else _slot(_draw(rng, 3, kind), stride, sign=0) if c == 1
-                       else _slot(np.zeros((0, 12)), stride, frm=0) if c == 2 else _slot(_draw(rng, 5, kind), stride, frm=120))
-    return bank
-
-
 def _as_tuples(words, n):
     return [(int(w["slot"]), int(w["cmd"]), int(w["start"]), int(w["end"]), int(w["dis"])) for w in words[:n]]
 
@@ -145,12 +86,12 @@ def test_oracle_equals_cell_reference_and_brute_force():
     for case in range(96):
         kind = ("tie", "full", "small")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind)
+        bank = random_bank(rng, T, kind)
         if case % 16 == 15:
             bank[:] = 0xFF                                # no member at all
         N = int(rng.integers(0, 41)) if case > 2 else case
-        x = _draw(rng, N, kind)
-        mem = _members(bank, T, bank.shape[1])
+        x = draw(rng, N, kind)
+        mem = bank_members(bank, T, bank.shape[1])
         for P in PENALTIES:
             feat = np.zeros((1, max(N, 1), 12), np.int16)
             feat[0, :N] = x
@@ -180,12 +121,12 @@ def test_max_penalty_gives_the_argmin_word():
     for case in range(60):
         kind = ("tie", "small", "equal")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind, fmax=10)
-        mem = _members(bank, T, bank.shape[1])
+        bank = random_bank(rng, T, kind, fmax=10)
+        mem = bank_members(bank, T, bank.shape[1])
         if not mem:
             continue
         N = int(rng.integers(1, 30))
-        x = _draw(rng, N, kind)
+        x = draw(rng, N, kind)
         w, nw, tot = co.connected(x[None], [N], bank, T, bank.shape[1], P_MAX, 4)
         scores = {t: dtw_full(x.astype(np.int64), y) for t, y in mem.items()}
         best = min(scores, key=lambda t: (scores[t], t))
@@ -199,7 +140,7 @@ def test_concatenated_templates_decode_back():
     rng = np.random.default_rng(0xC2)
     for case in range(40):
         T = int(rng.integers(2, 9))
-        bank = np.stack([_slot(_draw(rng, int(rng.integers(2, 9)), "small"), 2880) for _ in range(T)])
+        bank = np.stack([make_slot(draw(rng, int(rng.integers(2, 9)), "small"), 2880) for _ in range(T)])
         seq = rng.integers(0, T, int(rng.integers(1, 6)))
         parts = [bank[t, 4:4 + 24 * int(bank[t, 2:4].view(np.uint16)[0])].view(np.int16).reshape(-1, 12) for t in seq]
         x = np.concatenate(parts)
@@ -320,10 +261,10 @@ def test_connected_equals_oracle_over_lengths_and_banks():
     rng = np.random.default_rng(0xC5)
     Ns = [0, 1, 2, 118, 119, 120, 237, 238, 500, 818]
     for T in (1, 20, 32, 33, 80, 128):
-        bank = _bank(rng, T, "small", stride=4096, fmin=1, fmax=119)
+        bank = random_bank(rng, T, "small", stride=4096, fmin=1, fmax=119)
         feat = np.zeros((len(Ns), 818, 12), np.int16)
         for k, N in enumerate(Ns):
-            feat[k, :N] = _draw(rng, N, "small")
+            feat[k, :N] = draw(rng, N, "small")
         for P in ((0, 5000, P_MAX) if T < 80 else (3000,)):
             got = _check_connected(h, co, feat, np.array(Ns, np.uint32), bank, T, 4096, P, 6)
             assert (got[1][1:] >= 1).all() and got[1][0] == 0 and got[2][0] == 0
@@ -338,19 +279,19 @@ def test_connected_ties_headroom_and_averaged_bank():
     co = ox.connected()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0xC6)
-    eq = _bank(rng, 24, "equal", stride=4096, fmin=1, fmax=119, plant=True)
+    eq = random_bank(rng, 24, "equal", stride=4096, fmin=1, fmax=119, plant=True)
     feat = np.zeros((6, 818, 12), np.int16)
-    feat[:] = _draw(rng, 1, "equal")[0]
+    feat[:] = draw(rng, 1, "equal")[0]
     frm = np.array([818, 1, 119, 300, 2, 817], np.uint32)
     for P in (0, 1, P_MAX):
         _check_connected(h, co, feat, frm, eq, 24, 4096, P, 900)
-    big = np.stack([_slot(np.tile(MAX_B, (119, 1)), 4096) for _ in range(40)])
+    big = np.stack([make_slot(np.tile(MAX_B, (119, 1)), 4096) for _ in range(40)])
     hf = np.tile(MAX_A, (4, 818, 1))
     got = _check_connected(h, co, hf, np.full(4, 818, np.uint32), big, 40, 4096, P_MAX, 4)
     assert (got[2] > 2 ** 32).all()
     _check_connected(h, co, hf, np.full(4, 818, np.uint32), big, 40, 4096, 0, 900)
-    tie = _bank(rng, 50, "tie", stride=4096, fmin=1, fmax=30)
-    ft = np.stack([np.concatenate([_draw(rng, 400, "tie"), np.zeros((418, 12), np.int16)]) for _ in range(5)])
+    tie = random_bank(rng, 50, "tie", stride=4096, fmin=1, fmax=30)
+    ft = np.stack([np.concatenate([draw(rng, 400, "tie"), np.zeros((418, 12), np.int16)]) for _ in range(5)])
     for P in (0, 1, 7):
         _check_connected(h, co, ft, np.array([400, 399, 1, 37, 250], np.uint32), tie, 50, 4096, P, 500)
     enr = h.enrol(sr_b200.synth_pcm_host(80, 8000, 0xC60000), 2400)[0]
@@ -369,11 +310,11 @@ def test_connected_batch_position_and_argument_rules():
     co = ox.connected()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0xC7)
-    bank = _bank(rng, 12, "small", stride=4096, fmin=2, fmax=40)
+    bank = random_bank(rng, 12, "small", stride=4096, fmin=2, fmax=40)
     lens = rng.integers(0, 160, 400).astype(np.uint32)
     feat = np.zeros((400, 160, 12), np.int16)
     for b in range(400):
-        feat[b, :lens[b]] = _draw(rng, int(lens[b]), "small")
+        feat[b, :lens[b]] = draw(rng, int(lens[b]), "small")
     h.set_bank(bank, 12, 4096)
     ww, wn, wt = co.connected(feat, lens, bank, 12, 4096, 2500, 8, nthreads=NTHREADS)
     for lo, hi in ((0, 131), (131, 263), (0, 132), (5, 138), (100, 365), (0, 400), (399, 400)):
@@ -382,7 +323,7 @@ def test_connected_batch_position_and_argument_rules():
         for b in range(lo, hi):
             k = min(int(wn[b]), 8)
             assert np.array_equal(got[0][b - lo, :k], ww[b, :k])
-    wide = _bank(rng, 129, "small", stride=4096, fmin=2, fmax=40)
+    wide = random_bank(rng, 129, "small", stride=4096, fmin=2, fmax=40)
     L = sr_b200.lib()
     for bk, T, fr, stride, nw_null in ((wide, 129, lens[:4], 160, False), (bank, 12, np.array([819, 1, 1, 1], np.uint32), 900, False),
                                        (bank, 12, np.array([1, 161, 1, 1], np.uint32), 160, False), (bank, 12, lens[:4], 160, True)):
@@ -420,22 +361,13 @@ def _check_recognise(h, co, pcm, bank, T, P, max_words, n_len=2400):
     return got
 
 
-def _enrolled_bank(h, n_cmd, seed):
-    """one enrolled word per command at slot 4 * cmd (the other slots erased), from synthetic one-word captures"""
-    pcm = sr_b200.synth_pcm_host(n_cmd, 8000, seed)
-    enr, st = h.enrol(pcm, 2400)
-    bank = np.full((4 * n_cmd, 4096), 0xFF, np.uint8)
-    bank[::4] = enr
-    return bank, pcm, st
-
-
 @pytest.mark.gpu
 def test_recognise_connected_equals_composed_oracle():
     """the five board captures and synthetic 3-word captures at U = 8 000, 16 000 and 65 535 against an enrolled bank"""
     import os
     co = ox.connected()
     h = sr_b200.Handle(0)
-    bank, _, _ = _enrolled_bank(h, 20, 0xC80000)
+    bank, _, _ = enrolled_bank(h, 20, 0xC80000)
     cap = np.load(os.path.join(os.path.dirname(__file__), "golden", "captures.npz"))
     for U in (8000, 16000):
         rows = [cap[k][:U] for k in sorted(cap.files) if len(cap[k]) >= U]
@@ -460,7 +392,7 @@ def test_recognise_connected_decodes_spliced_words():
     ora = ob.best_oracle()
     h = sr_b200.Handle(0)
     n_cmd = 10
-    bank, words_pcm, st = _enrolled_bank(h, n_cmd, 0xC90000)
+    bank, words_pcm, st = enrolled_bank(h, n_cmd, 0xC90000)
     atap = [ora.noise_atap(words_pcm[c], 2400) for c in range(n_cmd)]
     segs = [ora.vad(words_pcm[c], 8000, atap[c]).reshape(3, 2)[0] for c in range(n_cmd)]
     mid = [int(a["mid_val"][0]) for a in atap]

@@ -15,72 +15,21 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_connected import P_MAX, _bank, _draw, _enrolled_bank, _slot
-from test_extension_refs import MAX_FRM, NTHREADS
-from test_grammar import LOOP, _prefilled, accepts, partition_grammar
+from cases import draw, make_slot, partition_grammar, random_bank
+from drive import enrolled_bank, prefilled
+from refs import GRAM_REC_BYTES, NTHREADS, PIECE_CHUNK, SEQ_CHUNK, accepts, piece_plan, pieces, record_cuts, seq_launches
 
-PIECE_CHUNK = 8192          # kPieceChunk, csrc/sr_api.cu
-GRAM_REC_BYTES = 1 << 28    # kGramRecBytes, csrc/sr_api.cu
-SEQ_CHUNK = 1 << 20         # kSeqChunk, csrc/sr_common.cuh
+P_MAX = 2 ** 32 - 1
+LOOP = sr_b200.loop_grammar()
 TAG_MFCC, TAG_CONN, TAG_GRAM = 1, 9, 10
 PREFILL = -12345
 # poison for feature rows at and past frm_num: +-32 767 in a checkerboard over frames and coefficients
 POISON = np.where((np.arange(818)[:, None] + np.arange(12)[None, :]) % 2, 32767, -32767).astype(np.int16)
 
 
-# ---- plans: the host's splitting rules, restated -----------------------------------------------------------------
-def _pieces(F):
-    """get_mfcc pieces of segments of F frames: ceil(F / 119)"""
-    return (np.asarray(F, np.int64) + MAX_FRM - 1) // MAX_FRM
-
-
-def piece_plan(counts):
-    """pieces counts[r] of each row (capture order, then segment order) through launches of PIECE_CHUNK: (launches, the
-    rows holding the last piece of a launch and the first of the next plus the first and last row with pieces, row
-    slices [lo, hi) of at most PIECE_CHUNK pieces each)"""
-    counts = np.asarray(counts, np.int64)
-    owner = np.repeat(np.arange(len(counts)), counts)
-    launches = -(-len(owner) // PIECE_CHUNK)
-    edge = {int(owner[0]), int(owner[-1])}
-    for k in range(1, launches):
-        edge |= {int(owner[k * PIECE_CHUNK - 1]), int(owner[k * PIECE_CHUNK])}
-    slices, lo, n = [], 0, 0
-    for r, c in enumerate(counts):
-        if n + c > PIECE_CHUNK:
-            slices.append((lo, r))
-            lo, n = r, 0
-        n += int(c)
-    slices.append((lo, len(counts)))
-    return launches, edge, slices
-
-
-def record_cuts(N, S):
-    """run_grammar's launch boundaries [0, ..., B]: a cut before sequence b when rows && (rows + N[b]) * S * 8 > 2^28"""
-    cuts, rows = [0], 0
-    for b, n in enumerate(np.asarray(N, np.int64).tolist()):
-        if rows and (rows + n) * S * 8 > GRAM_REC_BYTES:
-            cuts.append(b)
-            rows = 0
-        rows += n
-    return cuts + [len(N)]
-
-
-def seq_launches(cuts):
-    """the sequence ranges [lo, hi) of the kernel launches of a plan whose launch boundaries are cuts [0, ..., B] (K6:
-    [0, B]; K6g: record_cuts), each cut range launched in chunks of SEQ_CHUNK"""
-    return [(b0, min(b0 + SEQ_CHUNK, hi)) for lo, hi in zip(cuts[:-1], cuts[1:]) for b0 in range(lo, hi, SEQ_CHUNK)]
-
-
+# ---- plans: the host's splitting rules, restated in refs.py ------------------------------------------------------
 def gram_launches(cuts):
     return len(seq_launches(cuts))
-
-
-def launch_sample(edge, B, n, rng):
-    """the indices in edge plus random ones, n in all (or all of edge when it is larger), sorted"""
-    edge = sorted(set(int(e) for e in edge))
-    rest = np.setdiff1d(np.arange(B), edge)
-    pick = rng.choice(rest, min(max(n - len(edge), 0), len(rest)), replace=False)
-    return np.array(sorted(edge + [int(p) for p in pick]), np.int64)
 
 
 def _count(h, tag):
@@ -129,7 +78,7 @@ def _long_rows(rng, fmax):
         rows.append((int(rng.integers(119 * (p - 1) + 1, min(119 * p, fmax) + 1)), at0))
 
     def fill_to(target):
-        cum = int(_pieces([max(F, 0) for F, _ in rows]).sum())
+        cum = int(pieces([max(F, 0) for F, _ in rows]).sum())
         while target - cum > 14:
             if rng.random() < 0.01:
                 rows.append((int(rng.choice([-1, -2])), False))
@@ -187,9 +136,9 @@ def test_mfcc_long_across_piece_chunks(geom):
     h.timing_enable(64)
     for cap, want_launches in ((818, 3), (714, 2)):
         Fc = np.where(F <= cap, F, 0)
-        launches, edge, slices = piece_plan(_pieces(Fc))
+        launches, edge, slices = piece_plan(pieces(Fc))
         print("geom %d frm_cap %d: %d rows, %d pieces, %d launches, boundary rows %s, slices %s" % (
-            geom, cap, B, int(_pieces(Fc).sum()), launches, sorted(edge), slices))
+            geom, cap, B, int(pieces(Fc).sum()), launches, sorted(edge), slices))
         assert launches == want_launches
         fill = np.full((B, cap, 12), PREFILL, np.int16)
         feat, frm = h.mfcc_long(pcm, seg, atap, cap, feat=fill.copy())
@@ -219,7 +168,7 @@ def test_recognise_connected_across_piece_chunks():
     equal the whole call on every capture; the loop grammar equals sr_recognise_connected_batch on the whole batch"""
     co, go, ora = ox.connected(), ox.grammar(), ob.best_oracle()
     h = sr_b200.Handle(0)
-    bank, _, _ = _enrolled_bank(h, 20, 0xC1B0000)
+    bank, _, _ = enrolled_bank(h, 20, 0xC1B0000)
     h.set_bank(bank, 80, 4096)
     B, U, P, mw = 4400, 16000, 4000, 3
     pcm = sr_b200.synth_pcm_host(B, U, 0xC1B1000, 3)
@@ -228,15 +177,15 @@ def test_recognise_connected_across_piece_chunks():
     calls = (("connected", None), ("pin", sr_b200.chain_grammar(4)), ("loop", LOOP))
     whole = {}
     for name, g in calls:
-        out = _prefilled(h, pcm, LOOP, P, mw, 2400)
+        out = prefilled(h, pcm, P, mw, 2400)
         pre = {k: v.copy() for k, v in out.items()}
         run = (lambda x, o: h.recognise_connected(x, P, mw, out=o)) if g is None else \
             (lambda x, o, g=g: h.recognise_connected_grammar(x, g, P, mw, out=o))
         _count(h, TAG_MFCC)
         got = run(pcm, out)
-        launches, edge, slices = piece_plan(_pieces(got["frm_num"]).sum(1))
+        launches, edge, slices = piece_plan(pieces(got["frm_num"]).sum(1))
         print("%s: %d captures, %d pieces, %d launches, boundary captures %s, slices %s" % (
-            name, B, int(_pieces(got["frm_num"]).sum()), launches, sorted(edge), slices))
+            name, B, int(pieces(got["frm_num"]).sum()), launches, sorted(edge), slices))
         assert launches >= 2 and _count(h, TAG_MFCC) == launches
         idx = sorted(edge | set(rng.choice(B, 3, replace=False).tolist()))
         if g is None:
@@ -290,7 +239,7 @@ def test_grammar_record_cuts(S):
     of one launch each equal the whole call"""
     go = ox.grammar()
     rng = np.random.default_rng(0xC1C0 + S)
-    bank = _bank(rng, 64, "small", stride=4096, fmin=1, fmax=8, plant=False)
+    bank = random_bank(rng, 64, "small", stride=4096, fmin=1, fmax=8, plant=False)
     bank[np.arange(64) % 4 != 0] = 0xFF                   # slot 4c holds command c's one member
     g = partition_grammar(rng, S, n_cmd=16)
     N = _record_lengths(rng, S, 3)
@@ -329,9 +278,9 @@ def _many_short(rng):
     slots 1 and 6 hold distinct 1-frame templates; the sequences at 2^20 - 1, 2^20, 2^20 + 1 and B - 1 are those two
     templates back to back"""
     B = SEQ_CHUNK + 5
-    bank = _bank(rng, 13, "small", stride=4096, fmin=1, fmax=3)
-    ya, yb = _draw(rng, 1, "small"), _draw(rng, 1, "small")
-    bank[1], bank[6] = _slot(ya, 4096), _slot(yb, 4096)
+    bank = random_bank(rng, 13, "small", stride=4096, fmin=1, fmax=3)
+    ya, yb = draw(rng, 1, "small"), draw(rng, 1, "small")
+    bank[1], bank[6] = make_slot(ya, 4096), make_slot(yb, 4096)
     N = rng.integers(0, 3, B).astype(np.uint32)
     plant = [SEQ_CHUNK - 1, SEQ_CHUNK, SEQ_CHUNK + 1, B - 1]
     N[plant] = 2

@@ -1,8 +1,8 @@
 """Alignment along the banded DP (K3p, an extension the reference does not have; parity unpinned): the optimal warping
 path of sr_dtw_path_batch and the DTW barycentre averaging of sr_average_bank.
 
-CPU: the oracle's restatement (tests/oracle_ext/align.c) equals band_path_ref and average_ref, plain numpy / Python references
-written here from the definitions in speech_recog.h that share no code with it; the paths' invariants and the averaging
+CPU: the oracle's restatement (tests/oracle_ext/align.c) equals band_path_ref and average_ref, plain numpy / Python
+references of refs.py written from the definitions in speech_recog.h that share no code with it; the paths' invariants and the averaging
 properties. GPU: both calls equal the oracle bit for bit, the scores equal sr_dtw_batch's band scores, and the averaged
 bank is one recognition accepts."""
 import numpy as np
@@ -11,139 +11,13 @@ import pytest
 import oracle_ext as ox
 import oracle_bind as ob
 import sr_b200
-from test_extension_refs import (DIS_ERR, MAX_FRM, NTHREADS, _band_cases, _ftr, _guard_edge_shapes,
-                                 _guard_rejects, _rows, dist_matrix)
+from cases import band_cases, band_rows, guard_edge_shapes, make_ftr, random_groups
+from refs import DIS_ERR, MAX_FRM, NTHREADS, STRIDE, average_ref, band_path_ref, dist_matrix, slot_rows
 
 RADII = (0, 1, 7, 10, 15, 16, 59, 118, 1000)
 INT32_MAX = 2 ** 31 - 1
-STRIDE = ob.FTR_DTYPE.itemsize
 PATH_MAX = 237
 ALIGN, AVG_UPDATE = 7, 8                 # tags of sr_timing_collect
-
-
-# ---- references ---------------------------------------------------------------------------------------------------
-def band_matrix(fin, fmdl, r):
-    """the whole I x M matrix D(i, j) = d(i, j) + min(D(i-1, j-1), D(i, j-1), D(i-1, j)), D(0, 0) = d(0, 0), in exact
-    integers (lists of lists), +inf outside the band |j - floor(i*M/I)| <= r and where unreachable; no length guard"""
-    I, M = len(fin), len(fmdl)
-    d = dist_matrix(fin, fmdl).tolist()
-    inf = float("inf")
-    D = [[inf] * M for _ in range(I)]
-    for i in range(I):
-        c = i * M // I
-        for j in range(max(0, c - r), min(M - 1, c + r) + 1):
-            if i == 0 and j == 0:
-                D[i][j] = d[0][0]
-                continue
-            best = min(D[i - 1][j - 1] if i and j else inf, D[i][j - 1] if j else inf, D[i - 1][j] if i else inf)
-            if best != inf:
-                D[i][j] = best + d[i][j]
-    return D
-
-
-def band_path_ref(fin, fmdl, r):
-    """(score, path, D(I-1,M-1)): band_matrix, then the trace-back from (I-1, M-1): the neighbour with the smallest D, ties
-    to the diagonal, then (i, j-1), then (i-1, j). Rejected pairs: (DIS_ERR, [], None)"""
-    I, M = len(fin), len(fmdl)
-    if _guard_rejects(I, M) or I > MAX_FRM or M > MAX_FRM:
-        return DIS_ERR, [], None
-    D = band_matrix(fin, fmdl, r)
-    inf = float("inf")
-    end = D[I - 1][M - 1]
-    if end == inf:
-        return DIS_ERR, [], None
-    i, j, path = I - 1, M - 1, [(I - 1, M - 1)]
-    while (i, j) != (0, 0):
-        cand = [(D[i - 1][j - 1] if i and j else inf, 0), (D[i][j - 1] if j else inf, 1), (D[i - 1][j] if i else inf, 2)]
-        k = min(cand)[1]                     # smallest D, then the lowest rank: diagonal, (i, j-1), (i-1, j)
-        i, j = (i - 1, j - 1) if k == 0 else (i, j - 1) if k == 1 else (i - 1, j)
-        path.append((i, j))
-    return int(end) // (I + M), path[::-1], int(end)
-
-
-def _slot_rows(slot):
-    """(save_sign, frm_num, rows [frm_num, 12]) of a bank slot (rows only when frm_num <= 119)"""
-    f = slot[:STRIDE].view(ob.FTR_DTYPE)[0]
-    n = int(f["frm_num"])
-    return int(f["save_sign"]), n, (f["mfcc_dat"][: n * 12].reshape(n, 12).astype(np.int64) if n <= MAX_FRM else None)
-
-
-def average_ref(bank, slot_stride, K, r, iters, ranges=None):
-    """sr_average_bank from its definition: (bank_out, score [G, K], anchor [G]). ranges: a list that receives, per group
-    with members and iters >= 1, the (lo, hi) per template cell of the frames the last update averaged"""
-    bank = np.asarray(bank, np.uint8).reshape(-1, slot_stride)
-    G = bank.shape[0] // K
-    out = np.full_like(bank, 0xFF)
-    score, anchor = np.full((G, K), DIS_ERR, np.uint32), np.full(G, 0xFFFFFFFF, np.uint32)
-    for g in range(G):
-        rows = {}
-        for k in range(K):
-            sign, n, x = _slot_rows(bank[g * K + k])
-            if sign == sr_b200.SAVE_MASK and 1 <= n <= MAX_FRM:
-                rows[k] = x
-        if not rows:
-            continue
-        S = {(l, k): band_path_ref(rows[l], rows[k], r)[0] for l in rows for k in rows if l != k}
-        a = min(rows, key=lambda k: (sum(S[l, k] for l in rows if l != k), k))
-        C = rows[a].copy()
-        for _ in range(iters):
-            tot, cnt = np.zeros_like(C), np.zeros(len(C), np.int64)
-            lo, hi = np.full(C.shape, 1 << 20), np.full(C.shape, -(1 << 20))
-            for l, x in rows.items():
-                s, path, _ = band_path_ref(x, C, r)
-                if s == DIS_ERR:
-                    continue
-                for i, j in path:
-                    tot[j] += x[i]
-                    cnt[j] += 1
-                    lo[j], hi[j] = np.minimum(lo[j], x[i]), np.maximum(hi[j], x[i])
-            if cnt.any():
-                C = np.sign(tot) * (np.abs(tot) // cnt[:, None])         # C division truncates toward zero
-                if ranges is not None:
-                    ranges.append((g, lo, hi, C.copy()))
-        M = len(C)
-        out[g * K, :4] = np.frombuffer(np.array([sr_b200.SAVE_MASK, M], np.uint16).tobytes(), np.uint8)
-        out[g * K, 4:4 + 24 * M] = np.frombuffer(C.astype(np.int16).tobytes(), np.uint8)
-        for k, x in rows.items():
-            score[g, k] = band_path_ref(x, C, r)[0]
-        anchor[g] = a
-    return out, score, anchor
-
-
-# ---- inputs -------------------------------------------------------------------------------------------------------
-def _slot(rows, stride, sign=sr_b200.SAVE_MASK, frm=None):
-    s = np.full(stride, 0xFF, np.uint8)
-    n = len(rows) if frm is None else frm
-    s[:4] = np.frombuffer(np.array([sign, n], np.uint16).tobytes(), np.uint8)
-    s[4:4 + rows.size * 2] = np.frombuffer(np.ascontiguousarray(rows, np.int16).tobytes(), np.uint8)
-    return s
-
-
-def _random_groups(rng, G, K, stride, fmin=3, fmax=24, plant=True):
-    """G groups of K slots of random features (lengths fmin..fmax, some repetitions of one word plus noise); with plant,
-    the invalid cases go into the first groups: an erased slot, frm_num 0, frm_num 120, an unsigned slot, a member the
-    2:1 guard rejects against the others, and an all-empty group"""
-    bank = np.full((G * K, stride), 0xFF, np.uint8)
-    for g in range(G):
-        n0 = int(rng.integers(fmin, fmax + 1))
-        base = rng.integers(-3000, 3001, (n0, 12))
-        for k in range(K):
-            n = int(np.clip(n0 + rng.integers(-n0 // 3, n0 // 3 + 1), 1, MAX_FRM))
-            idx = np.minimum((np.arange(n) * n0) // n, n0 - 1)
-            rows = base[idx] + rng.integers(-400, 401, (n, 12))
-            bank[g * K + k] = _slot(rows, stride)
-    if plant and G >= 3:
-        k_last = K - 1
-        if K >= 2:
-            bank[0 * K + k_last] = 0xFF                                           # erased
-            bank[1 * K + k_last] = _slot(np.zeros((0, 12)), stride, frm=0)        # frm_num 0
-        if K >= 3:
-            bank[0 * K + 1] = _slot(rng.integers(-9, 9, (5, 12)), stride, frm=120)   # frm_num 120
-            bank[1 * K + 1] = _slot(rng.integers(-3000, 3001, (10, 12)), stride, sign=0)   # unsigned
-            n = _slot_rows(bank[2 * K])[1]
-            bank[2 * K + 1] = _slot(rng.integers(-3000, 3001, (min(2 * n + 3, MAX_FRM), 12)), stride)   # guard rejects
-        bank[(G - 1) * K:G * K] = 0xFF                                            # all empty
-    return bank
 
 
 # ---- CPU: the oracle against the references -------------------------------------------------------------------------
@@ -168,9 +42,9 @@ def test_oracle_path_equals_plain_reference_on_guard_edges():
     rng = np.random.default_rng(0xA1)
     kinds = ("small", "full", "equal")
     n_paths = n_err = 0
-    for k, (I, M) in enumerate(_guard_edge_shapes()):
-        fin, fmdl = _rows(rng, I, kinds[k % 3]), _rows(rng, M, kinds[k % 3])
-        fi, fm = _ftr([fin]), _ftr([fmdl])
+    for k, (I, M) in enumerate(guard_edge_shapes()):
+        fin, fmdl = band_rows(rng, I, kinds[k % 3]), band_rows(rng, M, kinds[k % 3])
+        fi, fm = make_ftr([fin]), make_ftr([fmdl])
         memo = {}
         for r in RADII:
             dis, path, plen = ao.dtw_path(fi, fm, r)
@@ -197,8 +71,8 @@ def test_oracle_self_match_path_is_the_diagonal():
     rng = np.random.default_rng(0xA2)
     for n in (1, 2, 7, 60, 119):
         for kind in ("small", "equal", "full"):
-            x = _rows(rng, n, kind)
-            f = _ftr([x])
+            x = band_rows(rng, n, kind)
+            f = make_ftr([x])
             for r in RADII:
                 dis, path, plen = ao.dtw_path(f, f, r)
                 assert dis[0] == 0 and plen[0] == n
@@ -214,7 +88,7 @@ def test_oracle_average_equals_plain_reference(K):
     ao = ox.align()
     rng = np.random.default_rng(0xA3 + K)
     stride = 2880
-    bank = _random_groups(rng, 6, K, stride)
+    bank = random_groups(rng, 6, K, stride)
     for r in (10, 118):
         for iters in (0, 1, 3):
             got = ao.average_bank(bank, stride, K, r, iters)
@@ -232,19 +106,19 @@ def test_averaging_properties():
     ao = ox.align()
     rng = np.random.default_rng(0xA4)
     stride = 4096
-    bank = _random_groups(rng, 8, 1, stride, plant=False)
+    bank = random_groups(rng, 8, 1, stride, plant=False)
     for iters in (0, 1, 3):
         out, score, anchor = ao.average_bank(bank, stride, 1, 16, iters)
         assert np.array_equal(out, bank) and (score == 0).all() and (anchor == 0).all()
-    one = _random_groups(rng, 5, 1, stride, plant=False)
+    one = random_groups(rng, 5, 1, stride, plant=False)
     same = np.repeat(one, 4, axis=0)
     out, score, anchor = ao.average_bank(same, stride, 4, 10, 3)
     assert np.array_equal(out[::4], one) and (out.reshape(5, 4, stride)[:, 1:] == 0xFF).all()
     assert (score == 0).all() and (anchor == 0).all()
-    bank = _random_groups(rng, 10, 4, stride, plant=False)
+    bank = random_groups(rng, 10, 4, stride, plant=False)
     out, score, anchor = ao.average_bank(bank, stride, 4, 118, 0)
     for g in range(10):
-        n = _slot_rows(bank[g * 4 + anchor[g]])[1]
+        n = slot_rows(bank[g * 4 + anchor[g]])[1]
         assert np.array_equal(out[g * 4, :4 + 24 * n], bank[g * 4 + anchor[g], :4 + 24 * n])
     ranges = []
     want = average_ref(bank, stride, 4, 15, 2, ranges=ranges)
@@ -256,22 +130,22 @@ def test_averaging_properties():
 
 # ---- GPU ----------------------------------------------------------------------------------------------------------
 def _all_pairs(utt, tpl):
-    """every (utterance u, template t) pair of a _band_cases case, u-major"""
+    """every (utterance u, template t) pair of a band_cases case, u-major"""
     n = len(utt)
-    fin, fm = _ftr(utt), _ftr(tpl)
+    fin, fm = make_ftr(utt), make_ftr(tpl)
     return np.repeat(fin, n), np.tile(fm, n)
 
 
 @pytest.mark.gpu
 def test_path_batch_equals_oracle_on_every_shape():
     """sr_dtw_path_batch == the oracle bit for bit (path bytes, lengths, scores) on all 119 x 119 shapes of the four
-    _band_cases at r in {0, 1, 7, 10, 15, 16, 59, 118, 1000} and INT32_MAX (against r = 118); the scores equal
+    band_cases at r in {0, 1, 7, 10, 15, 16, 59, 118, 1000} and INT32_MAX (against r = 118); the scores equal
     sr_dtw_batch with SR_DTW_BAND for the same pairs; a NULL path gives the same scores; self-matches walk the diagonal"""
     ao = ox.align()
     h = sr_b200.Handle(0)
-    for name, utt, tpl in _band_cases():
+    for name, utt, tpl in band_cases():
         a, b = _all_pairs(utt, tpl)
-        bank = _ftr(tpl)
+        bank = make_ftr(tpl)
         h.set_bank(bank.view(np.uint8).reshape(len(tpl), STRIDE), len(tpl), STRIDE)
         for r in RADII + (INT32_MAX,):
             dis, path, plen = h.dtw_path(a, b, r)
@@ -279,7 +153,7 @@ def test_path_batch_equals_oracle_on_every_shape():
             assert np.array_equal(dis, wdis), (name, r)
             assert np.array_equal(plen, wlen), (name, r)
             assert np.array_equal(path, wpath), (name, r)
-            score, _, _ = h.dtw(_ftr(utt), flags=sr_b200.DTW_BAND, band_r=r, want_best=False)
+            score, _, _ = h.dtw(make_ftr(utt), flags=sr_b200.DTW_BAND, band_r=r, want_best=False)
             assert np.array_equal(dis.reshape(len(utt), len(tpl)), score), (name, r)
             assert np.array_equal(h.dtw_path(a, b, r, with_path=False)[0], dis), (name, r)
             if name == "self":
@@ -295,7 +169,7 @@ def test_path_batch_argument_rules_and_timing():
     h = sr_b200.Handle(0)
     h.timing_enable(16)
     rng = np.random.default_rng(0xA5)
-    f = _ftr([_rows(rng, 20, "small"), _rows(rng, 33, "small")])
+    f = make_ftr([band_rows(rng, 20, "small"), band_rows(rng, 33, "small")])
     for r in (-1, -1000):
         with pytest.raises(sr_b200.SrError):
             h.dtw_path(f, f, r)
@@ -318,8 +192,8 @@ def test_path_batch_does_not_depend_on_batch_position():
     n = 2 * sms * 2 * 8 + 50
     lens_a, lens_b = rng.integers(1, 120, n), rng.integers(1, 120, n)
     lens_b = np.clip(lens_b, (lens_a + 1) // 2, 2 * lens_a).clip(1, 119)
-    a = _ftr([_rows(rng, int(x), "small") for x in lens_a])
-    b = _ftr([_rows(rng, int(x), "small") for x in lens_b])
+    a = make_ftr([band_rows(rng, int(x), "small") for x in lens_a])
+    b = make_ftr([band_rows(rng, int(x), "small") for x in lens_b])
     h = sr_b200.Handle(0)
     for r in (7, 118):
         wdis, wpath, wlen = ao.dtw_path(a, b, r, nthreads=NTHREADS)
@@ -377,10 +251,10 @@ def test_average_bank_random_groups_with_invalid_slots_equal_oracle():
     h = sr_b200.Handle(0)
     h.timing_enable(64)
     for K in (4, 7, 32):
-        bank = _random_groups(np.random.default_rng(0xA7 + K), 70, K, 4096, fmin=5, fmax=119)
+        bank = random_groups(np.random.default_rng(0xA7 + K), 70, K, 4096, fmin=5, fmax=119)
         for r, iters in ((10, 0), (118, 1), (15, 3)):
             _check_average(h, bank, 4096, K, r, iters)
-    bank = _random_groups(np.random.default_rng(0xA8), 70, 1, 2880, plant=False)
+    bank = random_groups(np.random.default_rng(0xA8), 70, 1, 2880, plant=False)
     got = h.average_bank(bank, 2880, 1, 16, 2)
     assert np.array_equal(got[0], bank)
     assert all(np.array_equal(a, b) for a, b in zip(got, ox.align().average_bank(bank, 2880, 1, 16, 2)))

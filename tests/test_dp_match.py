@@ -1,7 +1,7 @@
 """The banded dynamic-programming matcher (K3, an extension the reference does not have; parity unpinned) at every radius
 up to the full matrix, and as the matcher of the recognition paths (sr_set_match).
 
-CPU: the oracle's sro_dtw_band equals the plain band_dp_ref of test_extension_refs at the wide radii, and the textbook
+CPU: the oracle's sro_dtw_band equals the plain band_dp_ref of refs.py at the wide radii, and the textbook
 full_dp_ref where the band covers every column. GPU: sr_dtw_batch with SR_DTW_BAND equals the oracle at those radii (the
 whole-row kernel for r >= 16); recognition, streaming and the multi-handle call under the band matcher equal the oracle's
 own composition of the same stages. Every GPU test makes its own handles, so the session handle never carries a matcher."""
@@ -9,13 +9,16 @@ import numpy as np
 import pytest
 
 import oracle_bind as ob
+import oracle_ext as ox
 import sr_b200
-from test_extension_refs import (DIS_ERR, MAX_FRM, NTHREADS, _band_cases, _ftr, _guard_edge_shapes, _rows, band_dp_ref,
-                                 full_dp_ref)
+from cases import band_cases, band_rows, guard_edge_shapes, make_ftr
+from drive import handle, recognise_dev_np, same
+from refs import DIS_ERR, MAX_FRM, NTHREADS, band_dp_ref, full_dp_ref
 
 WIDE_RADII = (16, 31, 32, 59, 117, 118, 119, 1000)
 INT32_MAX = 2 ** 31 - 1
 STRIDE = ob.FTR_DTYPE.itemsize
+BAND = sr_b200.DTW_BAND
 # tags of sr_timing_collect
 VAD_, MFCC_, STATUS, BEST_INIT, DTW, BEST_FINAL, DTW_BAND = range(7)
 
@@ -30,9 +33,9 @@ def test_dtw_band_oracle_equals_plain_references_at_wide_radii():
     rng = np.random.default_rng(0xD9)
     kinds = ("small", "full", "equal")
     n_full = n_narrow = 0
-    for k, (I, M) in enumerate(_guard_edge_shapes()):
-        fin, fmdl = _rows(rng, I, kinds[k % 3]), _rows(rng, M, kinds[k % 3])
-        fi, fm = _ftr([fin]), _ftr([fmdl])
+    for k, (I, M) in enumerate(guard_edge_shapes()):
+        fin, fmdl = band_rows(rng, I, kinds[k % 3]), band_rows(rng, M, kinds[k % 3])
+        fi, fm = make_ftr([fin]), make_ftr([fmdl])
         got = {r: int(po.dtw_batch(fi, fm.view(np.uint8), 1, STRIDE, band_r=r)[0][0, 0]) for r in WIDE_RADII}
         want = {}
         for r in WIDE_RADII:
@@ -60,8 +63,8 @@ def test_dtw_batch_wide_band_equals_oracle_on_every_shape():
     rng = np.random.default_rng(0x3D)
     h = sr_b200.Handle(0)
     n_checked = 0
-    for name, utt, tpl in _band_cases():
-        fin, bank = _ftr(utt), _ftr(tpl)
+    for name, utt, tpl in band_cases():
+        fin, bank = make_ftr(utt), make_ftr(tpl)
         T = len(bank)
         I = fin["frm_num"].astype(np.int64)[:, None]
         M = bank["frm_num"].astype(np.int64)[None, :]
@@ -106,31 +109,6 @@ U = 16000
 PLANTED = [0, 1, 1047, 1048, 1049, 2096, 2500, 3199]     # segments from sample 0, at and next to the 1 048-utterance chunks
 
 
-def _compose(front, bank, T, r):
-    """recognise_pinned's front end, then the oracle's dtw_batch(check_sign=1, band_r=r) and the strict '<' first-wins
-    argmin with cmd = idx / 4 (main.c:276-294)"""
-    out = {k: front[k].copy() for k in ("atap", "seg_off", "ftr", "status")}
-    B = len(out["status"])
-    out["score"] = np.full((B, T), ob.NULL, np.uint32)
-    out["best_idx"], out["best_dis"], out["cmd"] = np.zeros(B, np.uint32), np.full(B, ob.NULL, np.uint32), np.zeros(B, np.uint32)
-    good = out["status"] == 0
-    sc, _ = ob.port().dtw_batch(out["ftr"][good], bank, T, 4096, check_sign=1, band_r=r, nthreads=NTHREADS)
-    out["score"][good] = sc
-    i = np.argmin(sc, axis=1)                # first of the minima == the strict '<' scan from DIS_ERR
-    out["best_idx"][good] = i
-    out["best_dis"][good] = sc[np.arange(len(i)), i]
-    out["cmd"][good] = i // 4
-    return out
-
-
-def _same(got, want, what):
-    for k in ("seg_off", "score", "best_idx", "best_dis", "cmd", "status"):
-        g, w = np.asarray(got[k]).reshape(len(want["status"]), -1), want[k].reshape(len(want["status"]), -1)
-        bad = np.flatnonzero((g != w).any(axis=1))
-        assert len(bad) == 0, (what, k, bad[:8].tolist())
-    assert ob.ftr_equal(got["ftr"], want["ftr"]), what
-
-
 def _bank(ora, slots, valid):
     """flash-layout bank of the given template indices (duplicates tie), with unsigned slots where valid is 0. The eight
     templates include two short ones whose segment starts at sample 0, so planted utterances pass the 2:1 guard"""
@@ -166,14 +144,6 @@ def recog_case():
     return {"pcm": pcm, "front": front, "bank20": _bank(ora, slots20, valid20), "bank70": _bank(ora, slots70, valid70)}
 
 
-def _handle(bank, T, r, match=True):
-    h = sr_b200.Handle(0)
-    h.set_bank(bank, T, 4096)
-    if match:
-        h.set_match(sr_b200.DTW_BAND, r)
-    return h
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("r", RADII)
 def test_recognise_band_matcher_equals_oracle_composition(recog_case, r):
@@ -181,29 +151,28 @@ def test_recognise_band_matcher_equals_oracle_composition(recog_case, r):
     launch and sr_recognise_batch_multi over three handles on one GPU all equal the oracle composition, every field; with
     VAD and MFCC failures, unsigned slots, duplicate templates (ties), utterances whose segment starts at sample 0, and a
     70-slot bank (bank order active)"""
-    from test_gpu_parity import _recognise_dev_np
     pcm, front = recog_case["pcm"], recog_case["front"]
     bank = recog_case["bank20"]
-    want = _compose(front, bank, 20, r)
+    want = ox.compose_recognise(front, bank, 20, BAND, r)
     assert (want["best_dis"][want["status"] == 0] != ob.NULL).sum() > 2000
-    h = _handle(bank, 20, r)
+    h = handle(bank, 20, BAND, r)
     assert h.match() == (sr_b200.DTW_BAND, r)
     h.set_transport(0)
-    _same(h.recognise(pcm, 2400), want, "host plain")
+    same(h.recognise(pcm, 2400), want, "host plain")
     assert h.transport_stats()[:2] == (0, 4)
     h.set_transport(1)
-    _same(h.recognise(pcm, 2400), want, "host packed")
+    same(h.recognise(pcm, 2400), want, "host packed")
     assert h.transport_stats()[0] > 0
-    _same(_recognise_dev_np(h, pcm, 2400, 20), want, "device launch")
+    same(recognise_dev_np(h, pcm, 2400, 20), want, "device launch")
     h.use_own_stream()
-    hs = [h] + [_handle(bank, 20, r) for _ in range(2)]
-    _same(sr_b200.recognise_multi(hs, pcm, 2400, want=sr_b200.RECOG_FIELDS), want, "multi")
+    hs = [h] + [handle(bank, 20, BAND, r) for _ in range(2)]
+    same(sr_b200.recognise_multi(hs, pcm, 2400, want=sr_b200.RECOG_FIELDS), want, "multi")
     for x in hs:
         x.close()
-    h70 = _handle(recog_case["bank70"], 70, r)
+    h70 = handle(recog_case["bank70"], 70, BAND, r)
     n = 640
-    _same(h70.recognise(pcm[:n], 2400), _compose({k: v[:n] for k, v in front.items()}, recog_case["bank70"], 70, r),
-          "70-slot bank")
+    same(h70.recognise(pcm[:n], 2400),
+         ox.compose_recognise({k: v[:n] for k, v in front.items()}, recog_case["bank70"], 70, BAND, r), "70-slot bank")
     h70.close()
 
 
@@ -214,11 +183,12 @@ def test_band_matcher_setting_and_greedy_round_trip(recog_case):
     greedy composition"""
     pcm = recog_case["pcm"][:512]
     bank = recog_case["bank20"]
-    h = _handle(bank, 20, 0, match=False)
+    h = sr_b200.Handle(0)
+    h.set_bank(bank, 20, 4096)
     assert h.match() == (0, 0)
     greedy = h.recognise(pcm, 2400)
     want = ob.recognise_pinned(ob.best_oracle(), pcm, 2400, bank, 20, 4096)
-    _same(greedy, want, "greedy")
+    same(greedy, want, "greedy")
     for flags, r in ((sr_b200.DTW_BAND, -1), (sr_b200.DTW_CHECK_SIGN, 0), (sr_b200.DTW_BAND | 4, 3), (8, 0), (0, -5)):
         with pytest.raises(sr_b200.SrError):
             h.set_match(flags, r)
@@ -239,7 +209,7 @@ def test_band_matcher_recognise_launches_are_tagged_dtw_band(recog_case):
     """timed recognise launches carry tag 6 for the band kernel at every kernel choice (r = 10, 15, 16, 118), tag 4 under
     the greedy walk"""
     pcm = recog_case["pcm"][:64]
-    h = _handle(recog_case["bank20"], 20, 0, match=False)
+    h = handle(recog_case["bank20"], 20)
     h.set_transport(0)
     h.timing_enable(64)
     h.recognise(pcm, 2400)
@@ -266,8 +236,8 @@ def test_geom_b_recognise_band_matcher_equals_own_oracle(r):
     pcm = sr_b200.synth_pcm_host(128, 8000, 0x5EED0000)
     ob.plant_sample0(pcm, [0, 5, 127], 0xB5)
     front = ob.recognise_pinned(po, pcm, 2400, None, 0, 4096, geom_b=True)
-    want = _compose(front, bank, T, r)
-    _same(h.recognise(pcm, 2400), want, "GEOM_B")
+    want = ox.compose_recognise(front, bank, T, BAND, r)
+    same(h.recognise(pcm, 2400), want, "GEOM_B")
     assert (want["status"] == 0).sum() > 100
     h.close()
 
@@ -307,7 +277,7 @@ def test_streaming_band_matcher_equals_batch(recog_case, arrival, group):
     pcm = sr_b200.synth_pcm_host(S, L, 0x5EEDD000, 3)
     pcm[3] = 2048                                            # a silent stream: no event
     for r in (16, 10):
-        hs = [_handle(bank, T, r) for _ in range(2 if group else 1)]
+        hs = [handle(bank, T, BAND, r) for _ in range(2 if group else 1)]
         pool = sr_b200.StreamPool(hs if group else hs[0], S, L, 2400)
         events = _stream_events(pool, pcm, arrival, np.random.default_rng(0xE5 + r))
         seg, atap = pool.segments()
@@ -341,7 +311,7 @@ def test_multi_and_group_calls_refuse_handles_with_different_matchers(recog_case
     bank = recog_case["bank20"]
     pcm = recog_case["pcm"][:64]
     for second in ((0, 0), (sr_b200.DTW_BAND, 15)):
-        a, b = _handle(bank, 20, 16), _handle(bank, 20, 0, match=False)
+        a, b = handle(bank, 20, BAND, 16), handle(bank, 20)
         b.set_match(*second)
         with pytest.raises(sr_b200.SrError):
             sr_b200.recognise_multi([a, b], pcm, 2400)

@@ -2,8 +2,9 @@
 numpy / Python and sharing no code with oracle/sr_oracle.c (whose restatements sro_dtw_band and sro_mfcc_geom_b read the
 same generated tables as the kernels, so a mistake common to both would pass every parity test):
 
-  K3  the Sakoe-Chiba banded DP (dtw_band_kernel for r != 10, dtw_band_thread_kernel<10>): band_dp_ref, itself checked
-      against a textbook full-matrix DTW where the band covers every column and against the closed form of r = 0;
+  K3  the Sakoe-Chiba banded DP (dtw_band_kernel for r != 10, dtw_band_thread_kernel<10>): band_dp_ref of refs.py,
+      itself checked against a textbook full-matrix DTW where the band covers every column and against the closed form
+      of r = 0;
   K5  the GEOM_B front end (mfcc_geomb_kernel): its tables from the float64 formulas, and the 256-point FFT (the oracle's
       cr4_fft_generic.c on the CPU, the shared core's fft_radix4<256> on the device) against the exact DFT / N.
 
@@ -16,72 +17,16 @@ import pytest
 
 import oracle_bind as ob
 import sr_b200
-
-DIS_ERR = 0xFFFFFFFF
-MAX_FRM = 119
-NTHREADS = max(1, min(16, os.cpu_count() or 1))
+from cases import band_cases, band_rows, guard_edge_shapes, make_ftr
+from refs import (DIS_ERR, MAX_A, MAX_B, MAX_FRM, NTHREADS, band_dp_ref, dist_matrix, full_dp_ref, guard_rejects)
 
 
 # ---- references --------------------------------------------------------------------------------------------------
-def dist_matrix(a, b):
-    """get_dis (DTW.C:45-62) of every row of a [I,12] against every row of b [M,12]: the sum of the 12 squared differences
-    wrapped to u32, converted to float32, IEEE square root in float32, truncated"""
-    dif = a.astype(np.int64)[:, None, :] - b.astype(np.int64)[None, :, :]
-    s = ((dif * dif).sum(axis=2) & 0xFFFFFFFF).astype(np.uint32)
-    return np.sqrt(s.astype(np.float32)).astype(np.uint32).astype(np.int64)
-
-
-def _guard_rejects(I, M):
-    """the 2:1 length guard of dtw (DTW.C:133), and the empty sets that have no cell"""
-    return I == 0 or M == 0 or I > 2 * M or M > 2 * I
-
-
-def band_dp_ref(fin, fmdl, r, with_d=False):
-    """D(i,j) = d(i,j) + min(D(i-1,j), D(i,j-1), D(i-1,j-1)), D(0,0) = d(0,0), over the whole I x M matrix in exact
-    integers, +inf outside the band |j - floor(i*M/I)| <= r; the result is D(I-1,M-1) // (I+M), dis_err when that cell is
-    unreachable. with_d: (result, D(I-1,M-1))"""
-    I, M = len(fin), len(fmdl)
-    if _guard_rejects(I, M):
-        return (DIS_ERR, None) if with_d else DIS_ERR
-    d = dist_matrix(fin, fmdl).tolist()
-    inf = float("inf")
-    D = [[inf] * M for _ in range(I)]
-    for i in range(I):
-        c = i * M // I
-        for j in range(M):
-            if abs(j - c) > r:
-                continue
-            if i == 0 and j == 0:
-                best = 0
-            else:
-                best = min(D[i - 1][j] if i else inf, D[i][j - 1] if j else inf, D[i - 1][j - 1] if i and j else inf)
-            D[i][j] = best + d[i][j]
-    end = D[I - 1][M - 1]
-    res = DIS_ERR if end == inf else int(end) // (I + M)
-    return (res, None if end == inf else int(end)) if with_d else res
-
-
-def full_dp_ref(fin, fmdl):
-    """textbook DTW over the full matrix (no band), same local distance, guard and normalisation"""
-    I, M = len(fin), len(fmdl)
-    if _guard_rejects(I, M):
-        return DIS_ERR
-    d = dist_matrix(fin, fmdl)
-    D = np.zeros((I, M), np.int64)
-    for i in range(I):
-        for j in range(M):
-            prev = [D[i - 1, j]] if i else []
-            prev += [D[i, j - 1]] if j else []
-            prev += [D[i - 1, j - 1]] if i and j else []
-            D[i, j] = d[i, j] + (min(prev) if prev else 0)
-    return int(D[I - 1, M - 1]) // (I + M)
-
-
 def band0_closed_form(fin, fmdl):
     """r = 0: row i holds only the cell (i, floor(i*M/I)), so the one possible path is those cells; it exists when every
     row-to-row shift is at most 1 (an up or a diagonal step) and the last row's cell is column M-1"""
     I, M = len(fin), len(fmdl)
-    if _guard_rejects(I, M):
+    if guard_rejects(I, M):
         return DIS_ERR
     cols = [i * M // I for i in range(I)]
     if cols[-1] != M - 1 or any(b - a > 1 for a, b in zip(cols, cols[1:])):
@@ -94,42 +39,6 @@ def dft_over_n(re, im):
     """the exact DFT / N of each row, in float64"""
     N = re.shape[1]
     return np.fft.fft(re.astype(np.float64) + 1j * im.astype(np.float64), axis=1) / N
-
-
-# ---- inputs ------------------------------------------------------------------------------------------------------
-def _ftr(rows_list):
-    """v_ftr_tag structs holding the given [n,12] row arrays"""
-    f = np.zeros(len(rows_list), ob.FTR_DTYPE)
-    for k, rows in enumerate(rows_list):
-        f["frm_num"][k] = len(rows)
-        f["mfcc_dat"][k, :rows.size] = rows.reshape(-1)
-    return f
-
-
-def _rows(rng, n, kind):
-    if kind == "small":                      # the range of real MFCC rows
-        return rng.integers(-3000, 3001, (n, 12)).astype(np.int16)
-    if kind == "full":                       # +-32767: d ~ 65 500 on all but 1 in 4096 cells
-        return (rng.choice([-1, 1], (n, 12)) * 32767).astype(np.int16)
-    if kind == "equal":                      # d = 0 everywhere: every min of the recurrence is a tie
-        return np.tile(np.array([7, -3, 11, 0, -25, 4, 9, -1, 2, 3, -8, 6], np.int16), (n, 1))
-    raise ValueError(kind)
-
-
-# rows with get_dis(MAX_A, MAX_B) = 65 536, the largest local distance: 65535^2 + 362^2 = 2^32 - 27 rounds to 2^32 in
-# float32. A pair of such constant feature sets has D(I-1,M-1) = max(I,M) * 65 536, the largest result any pair can have
-MAX_A = np.array([32767, 362] + [0] * 10, np.int16)
-MAX_B = np.array([-32768, 0] + [0] * 10, np.int16)
-
-
-def _guard_edge_shapes():
-    """every (I, M) on the edges of the 2:1 guard (M = 2I, I = 2M and one either side, both inside 1..119) and the corners"""
-    s = {(1, 1), (1, 2), (2, 1), (119, 119), (60, 119), (119, 60)}
-    for a in range(1, MAX_FRM + 1):
-        for b in (2 * a - 1, 2 * a, 2 * a + 1):
-            if 1 <= b <= MAX_FRM:
-                s |= {(a, b), (b, a)}
-    return sorted(s)
 
 
 # ---- K3 on the CPU: the reference against band-free references, then the oracle against the reference ------------
@@ -159,7 +68,7 @@ def test_band_dp_ref_equals_full_dp_and_the_r0_closed_form():
     n_full = n_finite0 = n_end_out = 0
     for k, (I, M) in enumerate(shapes):
         kind = ("small", "full", "equal")[k % 3]
-        fin, fmdl = _rows(rng, I, kind), _rows(rng, M, kind)
+        fin, fmdl = band_rows(rng, I, kind), band_rows(rng, M, kind)
         full = full_dp_ref(fin, fmdl)
         for r in range(max(0, M - 1), 16):
             assert band_dp_ref(fin, fmdl, r) == full, (I, M, r)
@@ -167,7 +76,7 @@ def test_band_dp_ref_equals_full_dp_and_the_r0_closed_form():
         r0 = band_dp_ref(fin, fmdl, 0)
         assert r0 == band0_closed_form(fin, fmdl), (I, M)
         n_finite0 += r0 != DIS_ERR
-        n_end_out += (r0 == DIS_ERR) and not _guard_rejects(I, M)
+        n_end_out += (r0 == DIS_ERR) and not guard_rejects(I, M)
         if I == M:
             assert r0 == int(np.trace(dist_matrix(fin, fmdl))) // (2 * I)
     assert n_full > 1000 and n_finite0 > 100 and n_end_out > 100
@@ -180,12 +89,12 @@ def test_dtw_band_oracle_equals_plain_reference_every_radius():
     po = ob.port()
     rng = np.random.default_rng(10)
     kinds = ("small", "full", "equal")
-    for k, (I, M) in enumerate(_guard_edge_shapes()):
+    for k, (I, M) in enumerate(guard_edge_shapes()):
         kind = kinds[k % 3]
-        fin, fmdl = _rows(rng, I, kind), _rows(rng, M, kind)
+        fin, fmdl = band_rows(rng, I, kind), band_rows(rng, M, kind)
         if (I, M) in ((119, 119), (60, 119), (119, 60)):
             fin, fmdl = np.tile(MAX_A, (I, 1)), np.tile(MAX_B, (M, 1))
-        fi, fm = _ftr([fin]), _ftr([fmdl])
+        fi, fm = make_ftr([fin]), make_ftr([fmdl])
         for r in range(16):
             got = int(po.dtw_batch(fi, fm.view(np.uint8), 1, ob.FTR_DTYPE.itemsize, band_r=r)[0][0, 0])
             want = band_dp_ref(fin, fmdl, r)
@@ -196,22 +105,6 @@ def test_dtw_band_oracle_equals_plain_reference_every_radius():
 
 
 # ---- K3 on the GPU: both band kernels, every radius --------------------------------------------------------------
-def _band_cases():
-    """(name, utterances, templates): utterance k and template k have k + 1 rows, so each case holds every (I, M) with
-    I, M in 1..119 (the guard edges among them) and 119 templates (three full 32-wide tiles and a remainder tile)"""
-    rng = np.random.default_rng(0xBA4D)
-    lens = range(1, MAX_FRM + 1)
-    small_u = [_rows(rng, n, "small") for n in lens]
-    full_u = [_rows(rng, n, "full") for n in lens]
-    full_t = [_rows(rng, n, "full") for n in lens]
-    for k in (59, 118):                      # 60 and 119 rows: the largest local distance on every cell
-        full_u[k], full_t[k] = np.tile(MAX_A, (k + 1, 1)), np.tile(MAX_B, (k + 1, 1))
-    return [("small", small_u, [_rows(rng, n, "small") for n in lens]),
-            ("full", full_u, full_t),
-            ("equal", [_rows(rng, n, "equal") for n in lens], [_rows(rng, n, "equal") for n in lens]),
-            ("self", small_u, [x.copy() for x in small_u])]
-
-
 @pytest.mark.gpu
 def test_dtw_band_kernels_equal_plain_reference_and_oracle_every_radius(handle):
     """sr_dtw_batch with SR_DTW_BAND for every r in 0..15 (the warp-scan kernel for 15 radii, the thread kernel for r = 10):
@@ -224,8 +117,8 @@ def test_dtw_band_kernels_equal_plain_reference_and_oracle_every_radius(handle):
     rng = np.random.default_rng(0x5EED)
     stride = ob.FTR_DTYPE.itemsize
     n_checked = 0
-    for name, utt, tpl in _band_cases():
-        fin, bank = _ftr(utt), _ftr(tpl)
+    for name, utt, tpl in band_cases():
+        fin, bank = make_ftr(utt), make_ftr(tpl)
         B, T = len(fin), len(bank)
         I = fin["frm_num"].astype(np.int64)[:, None]
         M = bank["frm_num"].astype(np.int64)[None, :]

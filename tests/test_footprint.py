@@ -22,6 +22,7 @@ import pytest
 import oracle_ext as ox
 import oracle_bind as ob
 import sr_b200
+from cases import MARK, make_ftr, plant_act, plant_segs, planted_atap, random_bank, random_groups
 
 pytestmark = pytest.mark.gpu
 
@@ -218,8 +219,7 @@ def test_get_mdl_keeps_rows_past_the_new_frm_num():
     fi = [rng.integers(-3000, 3001, (int(rng.integers(20, 60)), 12)) for _ in range(n)]
     fm = [rng.integers(-3000, 3001, (int(rng.integers(20, 60)), 12)) for _ in range(n)]
     fm[5] = rng.integers(-3000, 3001, (2 * len(fi[5]) + 1, 12))  # the 2:1 guard rejects the pair
-    from test_extension_refs import _ftr
-    a, b = _ftr(fi), _ftr(fm)
+    a, b = make_ftr(fi), make_ftr(fm)
     want, wdis = ob.port().get_mdl(a, b)
     h = _handle()
     _prime(h, n)
@@ -234,14 +234,12 @@ def test_get_mdl_keeps_rows_past_the_new_frm_num():
 def test_path_and_average_write_every_output_byte():
     """sr_dtw_path_batch and sr_average_bank called with outputs prefilled with two different patterns return the same
     bytes, those of the oracle: no byte of path, path_len, dis, bank_out, score or anchor is left as the caller had it"""
-    from test_dp_align import _random_groups
     L = sr_b200.lib()
     h = _handle()
     rng = np.random.default_rng(0x9A)
     n = 150
-    from test_extension_refs import _ftr
-    a = _ftr([rng.integers(-3000, 3001, (int(rng.integers(1, 120)), 12)) for _ in range(n)])
-    b = _ftr([rng.integers(-3000, 3001, (int(rng.integers(1, 120)), 12)) for _ in range(n)])
+    a = make_ftr([rng.integers(-3000, 3001, (int(rng.integers(1, 120)), 12)) for _ in range(n)])
+    b = make_ftr([rng.integers(-3000, 3001, (int(rng.integers(1, 120)), 12)) for _ in range(n)])
     want = ox.align().dtw_path(a, b, 10)
     for fill in (P8, Q8):
         path, plen, dis = (np.full(s, fill, np.uint8) for s in (n * 237 * 2, n * 4, n * 4))
@@ -250,7 +248,7 @@ def test_path_and_average_write_every_output_byte():
         assert np.array_equal(dis.view(np.uint32), want[0]) and np.array_equal(plen.view(np.uint32), want[2])
         assert np.array_equal(path.reshape(n, 237, 2), want[1])
     K, G, stride = 4, 40, 4096
-    bk = _random_groups(rng, G, K, stride, fmin=5, fmax=60)
+    bk = random_groups(rng, G, K, stride, fmin=5, fmax=60)
     want = ox.align().average_bank(bk, stride, K, 10, 2)
     for fill in (P8, Q8):
         out, score, anchor = (np.full(s, fill, np.uint8) for s in (G * K * stride, G * K * 4, G * 4))
@@ -593,15 +591,13 @@ def _poison_bank(bank, stride, first_row, walked):
 
 
 def _ftr_set(rng, B):
-    from test_extension_refs import _ftr
     lens = np.r_[[1, 2, 3, 59, 118, 119], rng.integers(1, 120, B - 6)]
-    return _ftr([rng.integers(-3000, 3001, (int(n), 12)) for n in lens])
+    return make_ftr([rng.integers(-3000, 3001, (int(n), 12)) for n in lens])
 
 
 def _test_bank(rng, stride):
     """T slots: signed ones of 1..119 frames, then an unsigned, an erased and a frm_num 120 one"""
-    from test_extension_refs import _ftr
-    f = _ftr([rng.integers(-3000, 3001, (int(n), 12)) for n in np.r_[[1, 2, 119], rng.integers(1, 120, T - 3)]])
+    f = make_ftr([rng.integers(-3000, 3001, (int(n), 12)) for n in np.r_[[1, 2, 119], rng.integers(1, 120, T - 3)]])
     bk = sr_b200.make_bank(f, stride)
     bk[T - 3, :2] = 0                                               # unsigned
     bk[T - 2] = 0xFF                                                # erased
@@ -652,7 +648,6 @@ def test_dtw_reads_only_the_rows_it_walks(ora, scan):
 def test_path_and_average_read_only_member_rows():
     """sr_dtw_path_batch: rows >= frm_num and save_sign of both sides; sr_average_bank: rows >= frm_num and padding of
     member slots, every byte after the header of a non-member slot"""
-    from test_dp_align import _random_groups
     rng = np.random.default_rng(0xA1)
     h = _handle()
     a, b = _ftr_set(rng, 120), _ftr_set(rng, 120)
@@ -664,7 +659,7 @@ def test_path_and_average_read_only_member_rows():
             got = h.dtw_path(x, y, r)
             assert all(np.array_equal(g, w) for g, w in zip(got, want)), r
     K, G, stride = 4, 30, 4096
-    bk = _random_groups(rng, G, K, stride, fmin=3, fmax=80)
+    bk = random_groups(rng, G, K, stride, fmin=3, fmax=80)
     hdr = np.frombuffer(bk[:, :4].tobytes(), np.uint16).reshape(-1, 2).astype(int)
     member = (hdr[:, 0] == sr_b200.SAVE_MASK) & (hdr[:, 1] >= 1) & (hdr[:, 1] <= 119)
     assert (~member).sum() >= 4
@@ -854,10 +849,8 @@ def test_long_grammar_shares_workspaces_with_the_other_calls(ora):
     1-state sr_connected_grammar_segs_batch, a larger sr_recognise_long_batch, a small K13 call in each geometry, the
     capture grammar and connected calls, then K13 with a larger batch. Each result equals a fresh handle's byte for
     byte, and the fresh handle's equals the CPU oracles"""
-    from test_connected import _bank
-    from test_long_stream import plant_act, planted_atap
     lo, port = ox.long_oracle(), ob.port()
-    bk = _bank(np.random.default_rng(0x13F1), 16, "small", plant=False)     # 16 slots of 1-8 frames, stride 2880
+    bk = random_bank(np.random.default_rng(0x13F1), 16, "small", plant=False)     # 16 slots of 1-8 frames, stride 2880
     NS, ST = 16, bk.shape[1]
     g16 = (16, 0xFFFF, [(k, (k + 1) % 16, 0x1) for k in range(16)])          # 16 states x the 4 slots of command 0
     chain = sr_b200.chain_grammar(3, 0xF)
@@ -1010,7 +1003,6 @@ def test_long_stream_reset_leaves_no_stale_ring_content(bank):
     """rings and mirrors filled with MARK / LOUD blocks, then a subset reset and planted audio pushed to the reset streams:
     a segment at stream sample 0, one on ring slot 0 after the first wrap (x[-1] from the mirror's partner slot R - 1)
     and one across the wrap, read through the mirror. Events and state() equal a fresh pool's"""
-    from test_long_stream import MARK, plant_segs, planted_atap
     h = _handle(bank)
     h.set_bank(bank, T, 4096)
     S, mc = 6, 640

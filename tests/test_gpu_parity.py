@@ -9,6 +9,7 @@ import pytest
 
 import oracle_bind as ob
 import sr_b200
+from drive import recognise_dev_np
 
 pytestmark = pytest.mark.gpu
 
@@ -841,34 +842,6 @@ def _same_recog(got, want, rows=None, what=""):
         assert not bad, (what, k, bad[:8])
 
 
-def _recognise_dev_np(h, pcm, n_len, T):
-    """one sr_recognise_batch_dev launch on the whole batch; every output field, as the host call returns it"""
-    import torch
-    dev = torch.device("cuda:0")
-    B, U = pcm.shape
-    st = torch.cuda.Stream(dev)
-    h.set_stream(st.cuda_stream)
-    with torch.cuda.stream(st):
-        pcm_d = torch.from_numpy(pcm.view(np.int16)).to(dev)
-        out = {"atap": torch.full((B * 12,), 0xA5, dtype=torch.uint8, device=dev),
-               "seg_off": torch.full((B * 6,), 0x5A5A5A5A, dtype=torch.int32, device=dev),
-               "ftr": torch.full((B * sr_b200.FTR_BYTES,), 0x5A, dtype=torch.uint8, device=dev),
-               "score": torch.full((B * max(T, 1),), 0x5A5A5A5A, dtype=torch.int32, device=dev),
-               "status": torch.full((B,), 0x5A, dtype=torch.uint8, device=dev)}
-        for key in ("best_idx", "best_dis", "cmd"):
-            out[key] = torch.full((B,), 0x5A5A5A5A, dtype=torch.int32, device=dev)
-        h.recognise_dev(pcm_d.data_ptr(), U, B, n_len, **{key: v.data_ptr() for key, v in out.items()})
-    st.synchronize()
-    got = {key: v.cpu().numpy() for key, v in out.items()}
-    got["atap"] = got["atap"].view(sr_b200.ATAP_DTYPE)
-    got["ftr"] = got["ftr"].view(sr_b200.FTR_DTYPE)
-    got["seg_off"] = got["seg_off"].view(np.uint32).reshape(B, 3, 2)
-    got["score"] = got["score"].view(np.uint32).reshape(B, -1)[:, :T]
-    for key in ("best_idx", "best_dis", "cmd"):
-        got[key] = got[key].view(np.uint32)
-    return got
-
-
 def _planted_and_pinned(ora, pcm, rows, seed, bank, T):
     ob.plant_sample0(pcm, rows, seed)
     want = ob.recognise_pinned(ora, pcm, 2400, bank, T, 4096)
@@ -900,7 +873,7 @@ def test_mfcc_sample0_host_chunks_plain_packed_and_one_device_launch_agree(ora):
         h.set_transport(-1)
     hd = sr_b200.Handle(0)
     hd.set_bank(bank, T, 4096)
-    one = _recognise_dev_np(hd, pcm, 2400, T)
+    one = recognise_dev_np(hd, pcm, 2400, T)
     _same_recog(plain, one, what="plain vs one launch")
     _same_recog(packed, plain, what="packed vs plain")
     _same_recog(one, want, what="one launch vs recognise_pinned")

@@ -3,8 +3,8 @@ sr_connected_grammar_batch and sr_recognise_connected_grammar_batch.
 
 CPU: the decoder's C restatement (tests/oracle_ext/long_grammar.c, capture form) equals gram_ref, a plain Python cell-level
 reference written here from the definition in speech_recog.h, on random NFAs with segments; its totals equal a minimum
-over accepted command sequences and segmentations built on the unnormalised full DTW of test_connected; the words are accepted, tile every
-segment and carry their own path sums; the loop grammar is the K6 restatement; a chain of L states gives L words. GPU:
+over accepted command sequences and segmentations built on the unnormalised full DTW of refs.py; the words are accepted,
+tile every segment and carry their own path sums; the loop grammar is the K6 restatement; a chain of L states gives L words. GPU:
 both calls equal the oracles bit for bit and write only their documented bytes; under the loop grammar they equal
 sr_connected_batch and sr_recognise_connected_batch; a chain grammar recovers digit strings spoken across VAD pauses."""
 import os
@@ -15,8 +15,9 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_connected import _bank, _draw, _enrolled_bank, _members, _slot, dtw_full
-from test_extension_refs import MAX_A, MAX_B, NTHREADS
+from cases import draw, make_slot, partition_grammar, random_bank, random_grammar
+from drive import enrolled_bank, prefilled
+from refs import MAX_A, MAX_B, NTHREADS, accepts, bank_members, copies_of, dtw_full, get_dis
 
 P_MAX = 2 ** 32 - 1
 PENALTIES = (0, 1, 1000, P_MAX)
@@ -27,26 +28,6 @@ NONE = ox.SEG_NONE
 
 
 # ---- references ---------------------------------------------------------------------------------------------------
-def _get_dis(a, b):
-    s = sum((int(p) - int(q)) ** 2 for p, q in zip(a, b)) & 0xFFFFFFFF
-    return int(np.sqrt(np.float32(s)))
-
-
-def copies_of(grammar, mem):
-    """[(state, slot, src mask)] state-major, then by slot"""
-    S, _, arcs = grammar
-    out = []
-    for s in range(S):
-        for t in sorted(mem):
-            src = 0
-            for a, b, m in arcs:
-                if b == s and (m >> (t // 4)) & 1:
-                    src |= 1 << a
-            if src:
-                out.append((s, t, src))
-    return out
-
-
 def _seg_of(seg, f):
     """(segment index, its first frame) of frame f"""
     g = max(k for k in range(3) if seg[k] != NONE and seg[k] <= f)
@@ -59,7 +40,7 @@ def gram_ref(x, bank, n_slot, grammar, P, seg=(0, NONE, NONE)):
     N = len(x)
     if N == 0:
         return [], (0 if F & 1 else INF64)
-    mem = _members(bank, n_slot, bank.shape[1])
+    mem = bank_members(bank, n_slot, bank.shape[1])
     cps = copies_of(grammar, mem)
     inf = None
     D = [[inf] * len(mem[t]) for _, t, _ in cps]          # (D, start) of frame i-1; a cell key is (D, -start)
@@ -82,7 +63,7 @@ def gram_ref(x, bank, n_slot, grammar, P, seg=(0, NONE, NONE)):
                 diag = prev[j]
                 cands = [q for q in cands if q is not inf]
                 best = min(cands, key=lambda q: (q[0], -q[1])) if cands else inf
-                row.append(inf if best is inf else (best[0] + _get_dis(x[i], y[j]), best[1]))
+                row.append(inf if best is inf else (best[0] + get_dis(x[i], y[j]), best[1]))
             D[c] = row
             if row[-1] is not inf and (Ei[s] is inf or row[-1][0] < Ei[s][0]):
                 Ei[s] = (row[-1][0], c, row[-1][1])
@@ -132,28 +113,6 @@ def brute_total(x, mem, grammar, P, seg=(0, NONE, NONE)):
     return min(fin) if fin else INF64
 
 
-def accepts(grammar, cmds):
-    """the grammar accepts the command sequence"""
-    S, F, arcs = grammar
-    cur = {0}
-    for c in cmds:
-        cur = {b for a, b, m in arcs if a in cur and (m >> c) & 1}
-    return any(F >> s & 1 for s in cur)
-
-
-def random_grammar(rng, S=None):
-    """an NFA of 1-5 states: overlapping arcs (shared endpoints, overlapping command masks), unreachable or dead states,
-    a random final mask"""
-    S = int(rng.integers(1, 6)) if S is None else S
-    arcs = []
-    for _ in range(int(rng.integers(1, 2 * S + 2))):
-        a, b = int(rng.integers(S)), int(rng.integers(S))
-        m = int(rng.integers(1, 4)) if rng.random() < 0.6 else int(rng.integers(0, 2 ** 32))
-        arcs.append((a, b, m))
-    F = int(rng.integers(1, 2 ** S))
-    return (S, F, arcs)
-
-
 def _tuples(words, n):
     return [tuple(int(w[k]) for k in ("slot", "cmd", "segment", "start", "end", "dis")) for w in words[:n]]
 
@@ -181,14 +140,14 @@ def test_oracle_equals_cell_reference_and_brute_force():
     for case in range(160):
         kind = ("tie", "full", "small")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind)
+        bank = random_bank(rng, T, kind)
         g = random_grammar(rng)
         N = int(rng.integers(0, 31)) if case > 2 else case
         if case % 4 == 1:
             N = min(N, 8)
-        x = _draw(rng, N, kind)
+        x = draw(rng, N, kind)
         seg = _random_segments(rng, N)
-        mem = _members(bank, T, bank.shape[1])
+        mem = bank_members(bank, T, bank.shape[1])
         for P in PENALTIES:
             feat = np.zeros((1, max(N, 1), 12), np.int16)
             feat[0, :N] = x
@@ -226,11 +185,11 @@ def test_loop_grammar_is_the_connected_decoder():
     for case in range(80):
         kind = ("tie", "full", "small")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind)
+        bank = random_bank(rng, T, kind)
         if case % 16 == 15:
             bank[:] = 0xFF
         N = int(rng.integers(0, 41))
-        x = _draw(rng, N, kind)
+        x = draw(rng, N, kind)
         feat = np.zeros((1, max(N, 1), 12), np.int16)
         feat[0, :N] = x
         for P in PENALTIES:
@@ -260,10 +219,10 @@ def test_chain_gives_exactly_L_words():
     n_path = 0
     for case in range(60):
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, ("tie", "small")[case % 2], plant=False)
+        bank = random_bank(rng, T, ("tie", "small")[case % 2], plant=False)
         L = int(rng.integers(1, 6))
         N = int(rng.integers(0, 16))
-        x = _draw(rng, N, "small")
+        x = draw(rng, N, "small")
         feat = np.zeros((1, max(N, 1), 12), np.int16)
         feat[0, :N] = x
         g = sr_b200.chain_grammar(L, 0xFFFFFFFF)
@@ -295,18 +254,6 @@ def _check_grammar(h, go, feat, frm, bank, T, stride, g, P, max_words, prefill=0
     return got
 
 
-def partition_grammar(rng, S, n_cmd=32):
-    """S states; every command is assigned to one state, whose incoming arcs (from state 0, from itself and from a random
-    state) carry exactly its commands: the copies are the bank's members, once each"""
-    own = rng.integers(0, S, n_cmd)
-    arcs = []
-    for s in range(S):
-        m = int(sum(1 << c for c in range(n_cmd) if own[c] == s))
-        if m:
-            arcs += [(0, s, m), (s, s, m), (int(rng.integers(S)), s, m)]
-    return (S, int(rng.integers(1, 2 ** S)) | 1 << (S - 1), arcs)
-
-
 @pytest.mark.gpu
 def test_grammar_equals_oracle_over_lengths_copies_and_states():
     """N in {0, 1, 2, 119, 120, 500, 818}, copy counts 1, 8, 9, 64, 127 and 128 (every cluster width 1..16 occurs across
@@ -320,14 +267,14 @@ def test_grammar_equals_oracle_over_lengths_copies_and_states():
     widths = set()
     for C, S in ((1, 1), (8, 2), (9, 5), (64, 12), (127, 16), (128, 16), (17, 5), (40, 2), (100, 12), (120, 1), (56, 16),
                  (25, 12), (90, 5), (72, 2), (112, 16), (80, 1), (44, 12), (88, 5), (1, 16), (8, 12)):
-        bank = _bank(rng, 128, "small", stride=4096, fmin=1, fmax=119, plant=False)
+        bank = random_bank(rng, 128, "small", stride=4096, fmin=1, fmax=119, plant=False)
         bank[rng.choice(128, 128 - C, replace=False)] = 0xFF
         g = partition_grammar(rng, S)
-        assert len(copies_of(g, _members(bank, 128, 4096))) == C
+        assert len(copies_of(g, bank_members(bank, 128, 4096))) == C
         widths.add((C + 7) // 8)
         feat = np.zeros((len(Ns), 818, 12), np.int16)
         for k, N in enumerate(Ns):
-            feat[k, :N] = _draw(rng, N, "small")
+            feat[k, :N] = draw(rng, N, "small")
         for P in ((0, 5000) if C < 64 else (3000,)):
             got = _check_grammar(h, go, feat, np.array(Ns, np.uint32), bank, 128, 4096, g, P, 6)
             assert got[1][0] == 0
@@ -343,20 +290,20 @@ def test_grammar_ties_headroom_averaged_bank_and_batch_position():
     go = ox.grammar()
     h = sr_b200.Handle(0)
     rng = np.random.default_rng(0x6A4)
-    eq = _bank(rng, 24, "equal", stride=4096, fmin=1, fmax=119)
+    eq = random_bank(rng, 24, "equal", stride=4096, fmin=1, fmax=119)
     feat = np.zeros((6, 818, 12), np.int16)
-    feat[:] = _draw(rng, 1, "equal")[0]
+    feat[:] = draw(rng, 1, "equal")[0]
     frm = np.array([818, 1, 119, 300, 2, 817], np.uint32)
     for P in (0, 1, P_MAX):
         for g in (LOOP, sr_b200.chain_grammar(3, 0xFF), random_grammar(rng, 5)):
             _check_grammar(h, go, feat, frm, eq, 24, 4096, g, P, 900)
-    big = np.stack([_slot(np.tile(MAX_B, (119, 1)), 4096) for _ in range(40)])
+    big = np.stack([make_slot(np.tile(MAX_B, (119, 1)), 4096) for _ in range(40)])
     hf = np.tile(MAX_A, (4, 818, 1))
     got = _check_grammar(h, go, hf, np.full(4, 818, np.uint32), big, 40, 4096, sr_b200.chain_grammar(3, 0x3FF), P_MAX, 4)
     assert (got[2] > 2 ** 32).all() and (got[1] == 3).all()             # 3 x 40 = 120 copies
     _check_grammar(h, go, hf, np.full(4, 818, np.uint32), big, 40, 4096, LOOP, 0, 900)
-    tie = _bank(rng, 50, "tie", stride=4096, fmin=1, fmax=30)
-    ft = np.stack([np.concatenate([_draw(rng, 400, "tie"), np.zeros((418, 12), np.int16)]) for _ in range(5)])
+    tie = random_bank(rng, 50, "tie", stride=4096, fmin=1, fmax=30)
+    ft = np.stack([np.concatenate([draw(rng, 400, "tie"), np.zeros((418, 12), np.int16)]) for _ in range(5)])
     for P in (0, 1, 7):
         for S in (1, 2, 2):                                 # 50 slots: at most 2 states stay within 128 copies
             _check_grammar(h, go, ft, np.array([400, 399, 1, 37, 250], np.uint32), tie, 50, 4096, random_grammar(rng, S), P, 500)
@@ -366,15 +313,15 @@ def test_grammar_ties_headroom_averaged_bank_and_batch_position():
     f, n = h.mfcc_long(pcm, np.array([[2400, 16000]] * 16, np.uint32), h.noise_atap(pcm, 2400), 818)
     pin = (5, 1 << 4, [(k, k + 1, 0x3FF) for k in range(4)])
     cmd_digit = (3, 1 << 2, [(0, 1, 0x3FC00), (1, 2, 0x3FF)])
-    assert len(copies_of(pin, _members(avg, 80, 4096))) == 40
+    assert len(copies_of(pin, bank_members(avg, 80, 4096))) == 40
     for g in (pin, cmd_digit, LOOP):
         _check_grammar(h, go, f, n, avg, 80, 4096, g, 2000, 10)
-    bank = _bank(rng, 12, "small", stride=4096, fmin=2, fmax=40)
+    bank = random_bank(rng, 12, "small", stride=4096, fmin=2, fmax=40)
     g = random_grammar(rng, 4)
     lens = rng.integers(0, 160, 400).astype(np.uint32)
     feat = np.zeros((400, 160, 12), np.int16)
     for b in range(400):
-        feat[b, :lens[b]] = _draw(rng, int(lens[b]), "small")
+        feat[b, :lens[b]] = draw(rng, int(lens[b]), "small")
     h.set_bank(bank, 12, 4096)
     ww, wn, wt = go.decode(feat, lens, bank, 12, 4096, g, 2500, 8, nthreads=NTHREADS)
     for lo, hi in ((0, 131), (131, 263), (0, 132), (5, 138), (100, 365), (0, 400), (399, 400)):
@@ -398,14 +345,14 @@ def test_grammar_without_copies():
     Ns = np.array([0, 1, 5, 119, 818, 0], np.uint32)
     feat = np.zeros((len(Ns), 818, 12), np.int16)
     for k, N in enumerate(Ns):
-        feat[k, :N] = _draw(rng, int(N), "small")
+        feat[k, :N] = draw(rng, int(N), "small")
     erased = np.full((12, 4096), 0xFF, np.uint8)
-    digits = _bank(rng, 12, "small", stride=4096, fmin=1, fmax=40, plant=False)   # commands 0..2 only
+    digits = random_bank(rng, 12, "small", stride=4096, fmin=1, fmax=40, plant=False)   # commands 0..2 only
     empty = np.zeros((0, 4096), np.uint8)
     cases = [(erased, 12, LOOP), (empty, 0, LOOP), (digits, 12, (3, 1 << 2, [(0, 1, 1 << 20), (1, 2, 1 << 21)])),
              (digits, 12, (2, 1, [(0, 1, 0xFFFFFFF8)])), (digits, 12, (2, 3, [])), (digits, 12, (2, 2, []))]
     for bank, T, g in cases:
-        assert not copies_of(g, _members(bank, T, 4096) if T else {})
+        assert not copies_of(g, bank_members(bank, T, 4096) if T else {})
         for P in (0, P_MAX):
             got = _check_grammar(h, go, feat, Ns, bank, T, 4096, g, P, 4)
             assert (got[1] == 0).all()
@@ -416,8 +363,8 @@ def test_grammar_without_copies():
     h.set_bank(erased, 12, 4096)
     pcm = sr_b200.synth_pcm_host(8, 16000, 0x6A91000, 3)
     for P in (0, 4000):
-        a = h.recognise_connected(pcm, P, 4, out=_prefilled(h, pcm, LOOP, P, 4, 2400))
-        b = h.recognise_connected_grammar(pcm, LOOP, P, 4, out=_prefilled(h, pcm, LOOP, P, 4, 2400))
+        a = h.recognise_connected(pcm, P, 4, out=prefilled(h, pcm, P, 4, 2400))
+        b = h.recognise_connected_grammar(pcm, LOOP, P, 4, out=prefilled(h, pcm, P, 4, 2400))
         for k in a:
             assert np.array_equal(a[k], b[k]), (P, k)
         assert (b["n_words"] == 0).all() and (b["total"][b["frm_num"].sum(1) > 0] == INF64).all()
@@ -429,15 +376,15 @@ def _twin_case(rng):
     same template, reached through states 1 and 2, and both states lead to state 3 through slot 8 (command 2). E_1 = E_2
     at every frame, so the word before the last comes from state 1 -- slot 0 -- only because source ties go to the
     lowest state"""
-    t, u = _draw(rng, 6, "small"), _draw(rng, 5, "small")
+    t, u = draw(rng, 6, "small"), draw(rng, 5, "small")
     bank = np.full((12, 4096), 0xFF, np.uint8)
-    bank[0], bank[4], bank[8] = _slot(t, 4096), _slot(t, 4096), _slot(u, 4096)
+    bank[0], bank[4], bank[8] = make_slot(t, 4096), make_slot(t, 4096), make_slot(u, 4096)
     g = (4, 1 << 3, [(0, 1, 1), (0, 2, 2), (1, 3, 4), (2, 3, 4)])
     feat = np.zeros((3, 40, 12), np.int16)
     frm = np.array([11, 40, 17], np.uint32)
     feat[0, :11] = np.concatenate([t, u])
-    feat[1] = _draw(rng, 40, "small")
-    feat[2, :17] = np.concatenate([t, _draw(rng, 3, "small"), u, _draw(rng, 3, "small")])
+    feat[1] = draw(rng, 40, "small")
+    feat[2, :17] = np.concatenate([t, draw(rng, 3, "small"), u, draw(rng, 3, "small")])
     return bank, g, feat, frm
 
 
@@ -477,21 +424,15 @@ def test_loop_grammar_equals_connected_batch():
     Ns = np.array([0, 1, 2, 118, 119, 120, 300, 818, 57, 3], np.uint32)
     feat = np.zeros((len(Ns), 818, 12), np.int16)
     for k, N in enumerate(Ns):
-        feat[k, :N] = _draw(rng, int(N), ("tie", "small")[k % 2])
+        feat[k, :N] = draw(rng, int(N), ("tie", "small")[k % 2])
     for T in (20, 128):
-        h.set_bank(_bank(rng, T, "small", stride=4096, fmin=1, fmax=119), T, 4096)
+        h.set_bank(random_bank(rng, T, "small", stride=4096, fmin=1, fmax=119), T, 4096)
         for P in (0, 4000, P_MAX):
             a = h.connected(feat, Ns, P, 12)
             b = h.connected_grammar(feat, Ns, LOOP, P, 12)
             for p, q in zip(a, b):
                 assert np.array_equal(p, q), (T, P)
     h.close()
-
-
-def _prefilled(h, pcm, g, P, max_words, n_len):
-    shape = h.recognise_connected(pcm[:1], P, max_words, n_len)
-    out = {k: np.frombuffer(b"\x5a" * a.nbytes, a.dtype).reshape(a.shape).copy() for k, a in shape.items()}
-    return {k: np.repeat(v, pcm.shape[0], axis=0) for k, v in out.items()}
 
 
 @pytest.mark.gpu
@@ -501,15 +442,15 @@ def test_loop_grammar_equals_recognise_connected(geom):
     prefilled) on the five board captures and synthetic captures at U = 8 000, 16 000 and 65 535"""
     h = sr_b200.Handle(0)
     h.set_geometry(geom)
-    bank, _, _ = _enrolled_bank(h, 20, 0x6A60000 + geom)
+    bank, _, _ = enrolled_bank(h, 20, 0x6A60000 + geom)
     h.set_bank(bank, 80, 4096)
     cap = np.load(os.path.join(os.path.dirname(__file__), "golden", "captures.npz"))
     cases = [np.stack([cap[k][:U] for k in sorted(cap.files) if len(cap[k]) >= U]) for U in (8000, 16000)]
     cases += [sr_b200.synth_pcm_host(B, U, 0x6A61000 + U, 3) for U, B in ((8000, 40), (16000, 40), (65535, 12))]
     for pcm in cases:
         for P, mw in ((0, 3), (4000, 8), (P_MAX, 2)):
-            a = h.recognise_connected(pcm, P, mw, out=_prefilled(h, pcm, LOOP, P, mw, 2400))
-            b = h.recognise_connected_grammar(pcm, LOOP, P, mw, out=_prefilled(h, pcm, LOOP, P, mw, 2400))
+            a = h.recognise_connected(pcm, P, mw, out=prefilled(h, pcm, P, mw, 2400))
+            b = h.recognise_connected_grammar(pcm, LOOP, P, mw, out=prefilled(h, pcm, P, mw, 2400))
             for k in a:
                 assert np.array_equal(a[k], b[k]), (pcm.shape, P, k)
     h.close()
@@ -519,7 +460,7 @@ def _paused_captures(h, ora, n_cmd, seed, n_cases, rng):
     """4 enrolled words, with pauses of 300 ms (the quiet tail of a capture) after some of them, so one string spans 2-3
     VAD segments; the later words at 85 % of their enrolled amplitude, so that no template matches exactly: (pcm
     [n_cases, U], command sequences, bank)"""
-    bank, words_pcm, st = _enrolled_bank(h, n_cmd, seed)
+    bank, words_pcm, st = enrolled_bank(h, n_cmd, seed)
     atap = [ora.noise_atap(words_pcm[c], 2400) for c in range(n_cmd)]
     segs = [ora.vad(words_pcm[c], 8000, atap[c]).reshape(3, 2)[0] for c in range(n_cmd)]
     mid = [int(a["mid_val"][0]) for a in atap]
@@ -562,7 +503,7 @@ def test_chain_grammar_recovers_strings_across_pauses():
             and [int(w["cmd"]) for w in want["words"][b, :want["n_words"][b]]] == seqs[b]]
     assert len(keep) >= 3, len(keep)
     h.set_bank(bank, 4 * n_cmd, 4096)
-    pre = _prefilled(h, pcm, g, 0, 8, 2400)
+    pre = prefilled(h, pcm, 0, 8, 2400)
     got = h.recognise_connected_grammar(pcm, g, 0, 8, out={k: v.copy() for k, v in pre.items()})
     for k in ("atap", "seg_off", "frm_num", "n_words", "total", "status"):
         assert np.array_equal(got[k], want[k]), k
@@ -585,20 +526,20 @@ def test_grammar_argument_rules():
     h = sr_b200.Handle(0)
     L = sr_b200.lib()
     rng = np.random.default_rng(0x6A8)
-    bank = _bank(rng, 128, "small", stride=4096, fmin=2, fmax=40, plant=False)
+    bank = random_bank(rng, 128, "small", stride=4096, fmin=2, fmax=40, plant=False)
     bank[1:4] = 0xFF                                        # 125 members: command 0 has one, command 1 four
     h.set_bank(bank, 128, 4096)
     one = (2, 2, [(0, 1, 1)])                               # 1 copy
     null_arcs = sr_b200.Grammar(2, 2, 1, C.cast(None, C.POINTER(sr_b200.GramArc)))
-    assert len(copies_of((2, 2, [(0, 1, 0xFFFFFFFF), (1, 0, 2)]), _members(bank, 128, 4096))) == 129
-    assert len(copies_of((2, 2, [(0, 1, 0xFFFFFFFF), (1, 0, 1), (0, 0, 4)]), _members(bank, 128, 4096))) == 130
+    assert len(copies_of((2, 2, [(0, 1, 0xFFFFFFFF), (1, 0, 2)]), bank_members(bank, 128, 4096))) == 129
+    assert len(copies_of((2, 2, [(0, 1, 0xFFFFFFFF), (1, 0, 1), (0, 0, 4)]), bank_members(bank, 128, 4096))) == 130
     bad = [(2, 2, [(0, 1, 0xFFFFFFFF), (1, 0, 2)]),          # 125 + 4 = 129 copies
            (2, 2, [(0, 1, 0xFFFFFFFF), (1, 0, 1), (0, 0, 4)]),   # 130 copies
            (17, 1, [(0, 1, 1)]), (0, 1, []), (2, 2, [(0, 2, 1)]), (2, 2, [(2, 1, 1)]), (2, 0, [(0, 1, 1)]),
            (2, 4, [(0, 1, 1)]), None, null_arcs]
     lens = np.array([30, 0, 5, 12], np.uint32)
     f = np.zeros((4, 40, 12), np.int16)
-    f[:] = _draw(rng, 40, "small")
+    f[:] = draw(rng, 40, "small")
     pcm = sr_b200.synth_pcm_host(4, 8000, 0x6A80000, 3)
     for g in bad:
         gg = sr_b200.grammar(g)

@@ -2,7 +2,7 @@
 segment, one decision per segment.
 
 CPU: the restatement sro_vad_long (tests/oracle_ext/long.c) equals a plain Python transcription of VAD.C:97-218 with the
-3-segment cap removed, written here, on planted activity patterns and random PCM; its first three segments equal the port's
+3-segment cap removed (refs.py), on planted activity patterns and random PCM; its first three segments equal the port's
 sro_vad and the reference's own VAD, and on any recording the segments that close before sample 65 535 equal the reference's
 VAD on the first 65 535 samples (VAD is causal). A guard parses include/sr_long.h for entry points this file does not run.
 
@@ -21,60 +21,18 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
+from cases import DIGITS, bank_of_ftr, real_speech_pairs, synth_long_poisoned
+from drive import cmp_long_atap, tag_counts
+from refs import py_vad_long
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NULL = 0xFFFFFFFF
-FIXTURES = ("digits_1_10_a", "digits_1_10_b", "digits_1_9_units_a", "digits_1_9_units_b")
 GROUP_BYTES = 256 << 20            # kLongGroupBytes, csrc/sr_api.cu
 TAG_MFCC, TAG_STATUS, TAG_BEST_INIT, TAG_DTW, TAG_BEST_FINAL, TAG_DTW_BAND, TAG_BLOCKS, TAG_SEGS = 1, 2, 3, 4, 5, 6, 11, 12
 PREFILL = 0xA5A5A5A5
 
 
-# ---- the definition, transcribed: VAD.C:97-218 without max_vc_con, u32 length ----------------------------------------
-def py_vad_long(vc, n, atap):
-    """[(start, end)], end = NULL for a segment still open when the frames run out"""
-    mid, n_thl, z_thl, s_thl = int(atap["mid_val"]), int(atap["n_thl"]), int(atap["z_thl"]), int(atap["s_thl"])
-    a_thl, b_thl = (mid + n_thl) & 0xFFFFFFFF, (mid - n_thl) & 0xFFFFFFFF       # VAD.C:112-113
-    vc = [int(v) for v in vc[:n]]
-    last_sig, cur, front, back, segs = 0, 0, 0, 0, []
-    i = 0
-    while n > 160 and i < n - 160:                                               # VAD.C:121
-        frm_sum = sum(abs(vc[i + h] - mid) for h in range(160))                  # VAD.C:126-129
-        frm_zero = 0
-        for h in range(159):                                                     # VAD.C:132-157
-            if vc[i + h] >= a_thl:
-                last_sig = 2
-            elif vc[i + h] < b_thl:
-                last_sig = 1
-            w = vc[i + h + 1]
-            if w >= a_thl:
-                frm_zero += last_sig == 1
-            elif w < b_thl:
-                frm_zero += last_sig == 2
-        if frm_sum > s_thl or frm_zero > z_thl:                                  # VAD.C:164-187
-            if cur == 0:
-                cur, front = 1, 1
-            elif cur == 1:
-                front += 1
-                if front >= 8:
-                    cur, front = 2, 0
-                    segs.append([i - 7 * 80, NULL])
-            elif cur == 3:
-                back, cur = 0, 2
-        else:                                                                    # VAD.C:188-216
-            if cur == 2:
-                cur, back = 3, 1
-            elif cur == 3:
-                back += 1
-                if back >= 11:
-                    cur, back = 0, 0
-                    segs[-1][1] = i - 11 * 80 + 160
-            elif cur == 1:
-                front, cur = 0, 0
-        i += 80
-    return [tuple(s) for s in segs]
-
-
+# ---- planted inputs --------------------------------------------------------------------------------------------------
 def _atap(mid=2048, n_thl=5000, z_thl=2, s_thl=15999):
     a = np.zeros(1, ob.ATAP_DTYPE)
     a["mid_val"], a["n_thl"], a["z_thl"], a["s_thl"] = mid, n_thl, z_thl, s_thl
@@ -155,7 +113,7 @@ def test_vad_long_equals_python_transcription_on_random_pcm():
 def test_first_three_segments_equal_vad_and_reference():
     lo, port = ox.long_oracle(), ob.port()
     ref = ob.ref() if ob.have_ref() else None
-    recs = [ox.golden_wav(f)[:65535] for f in FIXTURES] + list(sr_b200.synth_pcm_host(6, 40000, 0x10E6, 6))
+    recs = [ox.golden_wav(f)[:65535] for f in DIGITS] + list(sr_b200.synth_pcm_host(6, 40000, 0x10E6, 6))
     recs.append(ox.synth_long(1, 65535, 0x10E7)[0])
     for pcm in recs:
         n = len(pcm)
@@ -175,7 +133,7 @@ def test_segments_closing_before_65535_equal_reference_vad():
     the first 65 535 samples, up to its three segments"""
     lo, port = ox.long_oracle(), ob.port()
     vad65 = (ob.ref() if ob.have_ref() else port).vad
-    recs = [ox.golden_wav(f) for f in FIXTURES] + list(ox.synth_long(3, 300000, 0x10E8))
+    recs = [ox.golden_wav(f) for f in DIGITS] + list(ox.synth_long(3, 300000, 0x10E8))
     for pcm in recs:
         a = port.noise_atap(pcm, 2400)
         cnt, seg = lo.vad_long(pcm[None], a, 256)
@@ -198,30 +156,11 @@ def test_every_long_entry_point_is_run_here():
         assert src.count(py[n]) >= 2, n                  # in a correctness test and in the concurrency test
 
 
-# ---- GPU ---------------------------------------------------------------------------------------------------------------
-def _bank_of(ftr, valid_slots=None):
-    """one template per feature struct, template k in slot 4k (cmd = k); the other slots erased"""
-    K = len(ftr)
-    ftr4 = np.zeros(4 * K, ob.FTR_DTYPE)
-    ftr4[0::4] = ftr
-    valid = np.zeros(4 * K, bool)
-    valid[0::4] = True
-    return sr_b200.make_bank(ftr4, 4096, valid), 4 * K
-
-
-def _cmp_recognise(got, want, rows=None):
-    rows = range(len(want["n_segs"])) if rows is None else rows
-    for b in rows:
-        assert got["n_segs"][b] == want["n_segs"][b], b
-        assert got["atap"][b].tobytes() == want["atap"][b].tobytes(), b
-        m = min(int(want["n_segs"][b]), got["segs"].shape[1])
-        assert got["segs"][b, :m].tobytes() == want["segs"][b, :m].tobytes(), (b, got["segs"][b, :m], want["segs"][b, :m])
-
-
+# ---- GPU -------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 def test_fixtures_bit_exact(handle):
     lo, port = ox.long_oracle(), ob.port()
-    recs = [ox.golden_wav(f) for f in FIXTURES]
+    recs = [ox.golden_wav(f) for f in DIGITS]
     U = max(len(r) for r in recs)
     pcm = np.zeros((4, U), np.uint16)
     lens = np.array([len(r) for r in recs], np.uint32)
@@ -235,29 +174,21 @@ def test_fixtures_bit_exact(handle):
     assert v["n_segs"].tolist() == n.tolist() and (v["seg_off"] == seg).all()
     assert v["n_segs"].tolist() == [10, 10, 13, 13], v["n_segs"]
     got = handle.recognise_long_batch(pcm, 32, 2400, lens)
-    _cmp_recognise(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 32, lens))
-
-
-def _synth_long(lengths, U, seed):
-    """recordings of the given lengths (many words each) in rows of U samples, poisoned past their length"""
-    pcm = ox.synth_long(len(lengths), U, seed)
-    for b, n in enumerate(lengths):
-        pcm[b, n:] = np.where(np.arange(U - n) % 2, 4095, 0)
-    return pcm
+    cmp_long_atap(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 32, lens))
 
 
 @pytest.mark.gpu
 def test_ragged_synthetic_lengths(handle):
     lo, port = ox.long_oracle(), ob.port()
     lens = np.array([160, 161, 240, 65535, 65536, 1000003, 1 << 24], np.uint32)
-    pcm = _synth_long(lens, 1 << 24, 0x10A0)
+    pcm = synth_long_poisoned(lens, 1 << 24, 0x10A0)
     bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
     for geom in (0, 1):
         handle.set_geometry(geom)
         got = handle.recognise_long_batch(pcm, 4096, 2400, lens)
         want = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, geom_b=geom == 1)
-        _cmp_recognise(got, want)
+        cmp_long_atap(got, want)
     handle.set_geometry(0)
     assert int(got["n_segs"][-1]) > 1000
 
@@ -288,7 +219,7 @@ def test_4096_recordings_of_1_to_30_s(handle):
     assert got["n_segs"].tolist() == n.tolist()
     assert (got["segs"]["start"] == np.where(np.arange(64)[None] < n[:, None], seg[..., 0], 0)).all()
     rows = sorted({0, B - 1, *rng.integers(0, B, 14).tolist()})
-    _cmp_recognise(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64, lens, rows=rows), rows)
+    cmp_long_atap(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 64, lens, rows=rows), rows)
 
 
 @pytest.mark.gpu
@@ -347,7 +278,7 @@ def test_dev_forms_at_unaligned_pcm(handle):
     lo, port = ox.long_oracle(), ob.port()
     lens = np.array([70001, 161, 123457, 99999], np.uint32)
     U = 123457
-    pcm = _synth_long(lens, U, 0x10E0)
+    pcm = synth_long_poisoned(lens, U, 0x10E0)
     bank, T = ox.synth_bank()
     handle.set_bank(bank, T, 4096)
     want = ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 40, lens)
@@ -376,7 +307,7 @@ def test_dev_forms_at_unaligned_pcm(handle):
             assert (seg[b, :m, 0] == want["segs"]["start"][b, :m]).all() and (seg[b, :m, 1] == want["segs"]["end"][b, :m]).all()
         got = dict(atap=d_atap2.cpu().numpy().view(ob.ATAP_DTYPE), n_segs=d_n2.cpu().numpy().view(np.uint32),
                    segs=d_segs.cpu().numpy().view(ox.LONG_SEG_DTYPE).reshape(4, 40))
-        _cmp_recognise(got, want)
+        cmp_long_atap(got, want)
 
 
 @pytest.mark.gpu
@@ -430,8 +361,7 @@ def test_real_speech_decisions():
     lo, port = ox.long_oracle(), ob.port()
     h = sr_b200.Handle(0)
     try:
-        for a_name, b_name in ((FIXTURES[0], FIXTURES[1]), (FIXTURES[1], FIXTURES[0]), (FIXTURES[2], FIXTURES[3]),
-                               (FIXTURES[3], FIXTURES[2])):
+        for a_name, b_name in real_speech_pairs():
             a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
             for flags, r in ((0, 0), (2, 118)):
                 h.set_match(flags, r)
@@ -441,11 +371,11 @@ def test_real_speech_decisions():
                 at = ea["atap"]
                 ftr = ox.ftr_of_segments(port, a[None], at, [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL else int(s["start"]))
                                                              for s in ea["segs"][0, :ma]])
-                bank, T = _bank_of(ftr)
+                bank, T = bank_of_ftr(ftr)
                 h.set_bank(bank, T, 4096)
                 got = h.recognise_long_batch(b[None], 32, 2400)
-                want = ox.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, band_r=-1 if flags == 0 else r)
-                _cmp_recognise(got, want)
+                want = ox.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, match=(flags, r))
+                cmp_long_atap(got, want)
                 m = min(int(got["n_segs"][0]), ma)
                 right = int((got["segs"][0, :m]["cmd"] == np.arange(m)).sum())
                 print("%s -> %s, %s: %d/%d" % (a_name, b_name, "greedy" if flags == 0 else "r=%d" % r, right, m))
@@ -458,7 +388,7 @@ def test_real_speech_decisions():
 def test_threads_beside_a_recognise_handle():
     import torch
     lens = np.array([90000, 150000, 40000], np.uint32)
-    pcm = _synth_long(lens, 150000, 0x1100)
+    pcm = synth_long_poisoned(lens, 150000, 0x1100)
     short = sr_b200.synth_pcm_host(64, 16000, 0x1110, 3)
     bank, T = ox.synth_bank()
     dev = torch.device("cuda:0")
@@ -516,12 +446,7 @@ def test_threads_beside_a_recognise_handle():
             h.close()
 
 
-# ---- the host's plan, counted -------------------------------------------------------------------------------------------
-def _tags(h):
-    t = [tag for tag, _ in h.timing_collect()]
-    return {k: t.count(k) for k in set(t)}
-
-
+# ---- the host's plan, counted ----------------------------------------------------------------------------------------
 @pytest.mark.gpu
 def test_groups_and_launches_are_counted():
     """groups of at most 256 MB of PCM (at least one recording), 3 VAD launches per group (tags 11, 11, 12) and, for
@@ -535,18 +460,18 @@ def test_groups_and_launches_are_counted():
         h.timing_enable(4096)
         U = 1 << 24
         lens = np.array([U, U - 7, 3 * 80000, U, 161, U, U - 1, U, 999999, U, U], np.uint32)
-        pcm = _synth_long(lens, U, 0x1200)
+        pcm = synth_long_poisoned(lens, U, 0x1200)
         G = max(1, GROUP_BYTES // (2 * U))
         groups = -(-len(lens) // G)
         assert G == 8 and groups == 2
         c0 = h.launch_count()
         got = h.recognise_long_batch(pcm, 4096, 2400, lens)
         assert h.launch_count() - c0 == 10 * groups
-        assert _tags(h) == {TAG_BLOCKS: 2 * groups, TAG_SEGS: groups, TAG_MFCC: groups, TAG_STATUS: groups,
+        assert tag_counts(h) == {TAG_BLOCKS: 2 * groups, TAG_SEGS: groups, TAG_MFCC: groups, TAG_STATUS: groups,
                             TAG_BEST_INIT: groups, TAG_DTW: groups, TAG_BEST_FINAL: groups}
         assert int(got["n_segs"][:G].sum()) > 132 * 4 and int(got["n_segs"][G:].sum()) > 132
         rows = [0, G - 1, G, len(lens) - 1, 4]
-        _cmp_recognise(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, rows=rows), rows)
+        cmp_long_atap(got, ox.recognise_long(lo, port, pcm, 2400, bank, T, 4096, 4096, lens, rows=rows), rows)
         # the same recordings one group at a time
         for g0 in range(0, len(lens), G):
             part = h.recognise_long_batch(pcm[g0:g0 + G], 4096, 2400, lens[g0:g0 + G])
@@ -556,7 +481,7 @@ def test_groups_and_launches_are_counted():
         c0 = h.launch_count()
         h.vad_long_batch(pcm, 0, 2400, lens)
         assert h.launch_count() - c0 == 3 * groups
-        assert _tags(h) == {TAG_BLOCKS: 2 * groups, TAG_SEGS: groups}
+        assert tag_counts(h) == {TAG_BLOCKS: 2 * groups, TAG_SEGS: groups}
         c0 = h.launch_count()
         h.recognise_long_batch(pcm[:2], 0, 2400, lens[:2])                # max_segs = 0 counts only
         assert h.launch_count() - c0 == 3

@@ -24,38 +24,17 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
+from cases import frames_of, plant, plant_atap
+from drive import cmp_long_atap
+from refs import py_vad_long
 
 NULL = 0xFFFFFFFF
 WIN = 1024                                  # frames per K12 window
-PLANT_ATAP = (2048, 100, 0, 0xFFFFFFFF)     # mid, n_thl, z_thl, s_thl: a frame is active on one band crossing
 EDGES = (1, 2, 7)                           # the window edge under test, in windows
 MAX_SEGS = 6                                # the cut of the edge-table calls
 
 
-# ---- planted inputs ------------------------------------------------------------------------------------------------------
-def frames_of(n):
-    """frames i = 80k while i < n - 160 (VAD.C:121)"""
-    return -(-(n - 160) // 80) if n > 160 else 0
-
-
-def plant(act, n=None):
-    """PCM of n samples (default 80 N + 160) whose N = len(act) frames are active exactly where act is 1 under PLANT_ATAP"""
-    act = np.asarray(act, np.uint8)
-    n = 80 * len(act) + 160 if n is None else n
-    assert frames_of(n) == len(act)
-    pcm = np.full(n, 2048, np.uint16)
-    pcm[0] = 1947                                           # below the band: last_sig = 1 before frame 0
-    k = np.flatnonzero(act)
-    pcm[80 * (k + 1)] = np.where(np.arange(len(k)) % 2 == 0, 2148, 1947)
-    return pcm
-
-
-def plant_atap(B):
-    a = np.zeros(B, ob.ATAP_DTYPE)
-    a["mid_val"], a["n_thl"], a["z_thl"], a["s_thl"] = PLANT_ATAP
-    return a
-
-
+# ---- the FSM over planted strings (plant and plant_atap: cases.py) ---------------------------------------------------
 def fsm_trace(act):
     """the sequential FSM of VAD.C:164-216 over an activity string: (segments [(start, end)], states {edge frame: (open,
     run, closed segments)} at every multiple of WIN, events [(open?, frame of the 8th / 11th frame, segment index)])"""
@@ -132,7 +111,7 @@ def fsm_windowed(act, W):
     return [tuple(s) for s in segs]
 
 
-# ---- the edge table ------------------------------------------------------------------------------------------------------
+# ---- the edge table --------------------------------------------------------------------------------------------------
 def _runs(rng, n, lo=1, hi=14):
     """a run-structured activity string of n frames"""
     out, a = [], int(rng.integers(0, 2))
@@ -238,7 +217,7 @@ def random_cases(seed, n):
     return [("random %d" % i, np.asarray(_runs(rng, int(rng.integers(2 * WIN, 8 * WIN))), np.uint8)) for i in range(n)]
 
 
-# ---- coverage of the table -------------------------------------------------------------------------------------------------
+# ---- coverage of the table -------------------------------------------------------------------------------------------
 def _outcome(act, e, op, r):
     need, want = (11 if op else 8) - r, 0 if op else 1
     j = 0
@@ -296,7 +275,7 @@ def required_rows():
     return rows | {"long segment", "gap > 1 window", "gap > 2 windows", "opening after a gap", "window without a crossing"}
 
 
-# ---- CPU ---------------------------------------------------------------------------------------------------------------------
+# ---- CPU -------------------------------------------------------------------------------------------------------------
 def _oracle_segs(lo, acts, max_segs=4096):
     n = max(80 * len(a) + 160 for a in acts)
     pcm = np.full((len(acts), n), 2048, np.uint16)
@@ -312,7 +291,6 @@ def _oracle_segs(lo, acts, max_segs=4096):
 def test_planted_pcm_realises_its_activity_string():
     """sro_vad_long on the planted PCM equals the sequential FSM on the string: random and run-structured strings, the
     whole edge table; on short strings also the plain transcription of VAD.C (test_long.py)"""
-    from test_long import py_vad_long
     lo = ox.long_oracle()
     rng = np.random.default_rng(0xED6E)
     acts = [rng.integers(0, 2, int(rng.integers(0, 400))).astype(np.uint8) for _ in range(100)]
@@ -361,7 +339,7 @@ def test_edge_table_reaches_every_row():
     assert not missing, sorted(missing, key=str)
 
 
-# ---- GPU: window edges ------------------------------------------------------------------------------------------------------
+# ---- GPU: window edges -----------------------------------------------------------------------------------------------
 def _batch(acts, U=None):
     """planted recordings in rows of U samples (default: the longest), poisoned past their length with loud band
     crossings"""
@@ -428,7 +406,6 @@ def test_window_edges_bit_exact(handle, w):
 @pytest.mark.gpu
 def test_window_edges_recognised(handle):
     """sr_recognise_long_batch on the edge table at window 1 against a small bank: every record equals the oracle's"""
-    from test_long import _cmp_recognise
     lo, port = ox.long_oracle(), ob.port()
     cases = edge_cases(1)
     pcm, lens = _batch([a for _, a in cases])
@@ -437,11 +414,11 @@ def test_window_edges_recognised(handle):
     B = len(cases)
     got = handle.recognise_long_batch(pcm, 128, 0, lens, atap=plant_atap(B))
     want = ox.recognise_long(lo, port, pcm, 0, bank, T, 4096, 128, lens, atap=plant_atap(B))
-    _cmp_recognise(got, want)
+    cmp_long_atap(got, want)
     assert want["n_segs"].max() <= 128 and (want["segs"]["status"] == 0).sum() > B
 
 
-# ---- GPU: work splitting -------------------------------------------------------------------------------------------------------
+# ---- GPU: work splitting ---------------------------------------------------------------------------------------------
 def cpr(U):
     """K11b's chunks (work items of 32 blocks) per recording: its blocks never exceed U / 80 + 1"""
     return (U // 80 + 1 + 31) // 32
@@ -557,7 +534,6 @@ def test_empty_items_are_skipped_over_several_strides(handle):
 def test_batch_sizes_recognised(handle, B):
     """recognition past 8 recordings per segment-kernel CTA and 1 024 per prefix-sum pass, max_segs = 2 cutting some rows
     and not others: every record equals the oracle's"""
-    from test_long import _cmp_recognise
     lo, port = ox.long_oracle(), ob.port()
     rng = np.random.default_rng(B)
     acts = [np.asarray(_runs(rng, int(rng.integers(1, 200)), 1, 13), np.uint8) for _ in range(B)]
@@ -566,7 +542,7 @@ def test_batch_sizes_recognised(handle, B):
     handle.set_bank(bank, T, 4096)
     got = handle.recognise_long_batch(pcm, 2, 0, lens, atap=plant_atap(B))
     want = ox.recognise_long(lo, port, pcm, 0, bank, T, 4096, 2, lens, atap=plant_atap(B))
-    _cmp_recognise(got, want)
+    cmp_long_atap(got, want)
     n = want["n_segs"]
     if B > 100:
         assert (n > 2).sum() > B // 10 and ((n >= 1) & (n <= 2)).sum() > B // 10

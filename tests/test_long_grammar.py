@@ -18,10 +18,10 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_connected import _bank, _draw, _members, _slot
-from test_grammar import accepts, copies_of, random_grammar
-from test_long import FIXTURES, _bank_of, _synth_long
-from test_long_edges import plant, plant_atap
+from cases import (bank_of_ftr, draw, make_slot, plant, plant_atap, random_bank, random_grammar, real_speech_pairs,
+                   synth_long_poisoned)
+from drive import tag_counts
+from refs import accepts, bank_members, copies_of, get_dis
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P_MAX = 2 ** 32 - 1
@@ -36,11 +36,6 @@ F_MAX = 1677720                    # SR_LONG_GRAM_FRM_MAX
 
 
 # ---- the reference ------------------------------------------------------------------------------------------------------
-def _get_dis(a, b):
-    s = sum((int(p) - int(q)) ** 2 for p, q in zip(a, b)) & 0xFFFFFFFF
-    return int(np.sqrt(np.float32(s)))
-
-
 def long_gram_ref(x, seg_frm, bank, n_slot, grammar, P):
     """the decoder from sr_long_grammar.h's definition, cell by cell, over x = the segments' rows back to back: (words
     [(slot, cmd, segment, start, end, dis)], total)"""
@@ -48,7 +43,7 @@ def long_gram_ref(x, seg_frm, bank, n_slot, grammar, P):
     N = int(sum(seg_frm))
     if N == 0:
         return [], (0 if F & 1 else INF64)
-    mem = _members(bank, n_slot, bank.shape[1])
+    mem = bank_members(bank, n_slot, bank.shape[1])
     cps = copies_of(grammar, mem)
     seg_of, first = [], []                                # per frame: its segment, the segment's first frame
     for k, n in enumerate(seg_frm):
@@ -74,7 +69,7 @@ def long_gram_ref(x, seg_frm, bank, n_slot, grammar, P):
                 diag = prev[j]
                 cands = [q for q in cands if q is not inf]
                 best = min(cands, key=lambda q: (q[0], -q[1])) if cands else inf
-                row.append(inf if best is inf else (best[0] + _get_dis(x[i], y[j]), best[1]))
+                row.append(inf if best is inf else (best[0] + get_dis(x[i], y[j]), best[1]))
             D[c] = row
             if row[-1] is not inf and (Ei[s] is inf or row[-1][0] < Ei[s][0]):
                 Ei[s] = (row[-1][0], c, row[-1][1])
@@ -134,10 +129,10 @@ def test_oracle_equals_python_reference():
     for case in range(90):
         kind = ("tie", "full", "small")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind)
+        bank = random_bank(rng, T, kind)
         g = random_grammar(rng)
         segs = _random_segs(rng, 40 if case % 5 == 0 else 12, 12 if case % 5 == 0 else 6)
-        x = _draw(rng, sum(segs), kind)
+        x = draw(rng, sum(segs), kind)
         for P in PENALTIES:
             w, nw, tot = lg.decode_segs(x, [0, len(segs)], segs, bank, T, bank.shape[1], g, P, 600)
             want_words, want_total = long_gram_ref(x, segs, bank, T, g, P)
@@ -156,14 +151,14 @@ def test_oracle_equals_capture_decoder_on_three_segments():
     for case in range(60):
         kind = ("tie", "full", "small")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind)
+        bank = random_bank(rng, T, kind)
         g = random_grammar(rng)
         nseg = int(rng.integers(1, 4))
         segs = [int(rng.integers(0, 30)) for _ in range(nseg)]
         if case == 0:
             segs = [300, 0, 518]                           # 818 frames in all
         N = sum(segs)
-        x = _draw(rng, N, kind)
+        x = draw(rng, N, kind)
         first, f = [], 0
         for n in segs:
             first.append(f if n else ox.SEG_NONE)
@@ -185,11 +180,11 @@ def test_loop_grammar_equals_connected_per_segment():
     for case in range(40):
         kind = ("tie", "full", "small")[case % 3]
         T = int(rng.integers(1, 7))
-        bank = _bank(rng, T, kind)
-        if not _members(bank, T, bank.shape[1]):
+        bank = random_bank(rng, T, kind)
+        if not bank_members(bank, T, bank.shape[1]):
             continue
         segs = _random_segs(rng, 20, 15)
-        x = _draw(rng, sum(segs), kind)
+        x = draw(rng, sum(segs), kind)
         for P in PENALTIES:
             w, nw, tot = lg.decode_segs(x, [0, len(segs)], segs, bank, T, bank.shape[1], LOOP, P, 400)
             want, total, r = [], 0, 0
@@ -219,7 +214,7 @@ def _flat(rng, seqs, kind="small"):
     """sequences given as lists of segment frame counts -> (feat [rows, 12], seq_seg, seg_frm)"""
     seg_frm = [n for s in seqs for n in s]
     seq_seg = np.cumsum([0] + [len(s) for s in seqs]).astype(np.uint32)
-    return _draw(rng, int(sum(seg_frm)), kind), seq_seg, np.array(seg_frm, np.uint32)
+    return draw(rng, int(sum(seg_frm)), kind), seq_seg, np.array(seg_frm, np.uint32)
 
 
 def _check_segs(h, lg, feat, seq_seg, seg_frm, bank, T, g, P, max_words, prefill=0x5A):
@@ -255,10 +250,10 @@ def test_segs_every_cluster_width_and_state_count(handle):
     rng = np.random.default_rng(0x13D)
     for w in range(1, 17):
         T = 8 * w
-        bank = _bank(rng, T, ("small", "tie", "full")[w % 3], plant=False)
+        bank = random_bank(rng, T, ("small", "tie", "full")[w % 3], plant=False)
         handle.set_bank(bank, T, bank.shape[1])
         g = _partition_grammar(w, T, rng)
-        assert len(copies_of(g, _members(bank, T, bank.shape[1]))) == T
+        assert len(copies_of(g, bank_members(bank, T, bank.shape[1]))) == T
         seqs = [[int(rng.choice([0, 1, 119, 120, 7]))], [0, 0], [818], [1, 0, 120], [], [119, 0, 1]]
         feat, seq_seg, seg_frm = _flat(rng, seqs, ("small", "tie", "full")[w % 3])
         for P in (PENALTIES[w % 4], 1000):
@@ -271,7 +266,7 @@ def test_segs_many_segments(handle):
     loop grammar, with max_words below and above the word counts"""
     lg = ox.long_grammar()
     rng = np.random.default_rng(0x13E)
-    bank = _bank(rng, 12, "small")
+    bank = random_bank(rng, 12, "small")
     handle.set_bank(bank, 12, bank.shape[1])
     seqs = [[5], [3, 0], [int(rng.integers(0, 13)) for _ in range(819)], [int(rng.integers(0, 13)) for _ in range(10000)],
             [int(rng.integers(0, 4)) for _ in range(100000)], [0] * 1000]
@@ -293,8 +288,8 @@ def test_segs_headroom(handle):
     x[0] = 32767
     y = np.zeros(12, np.int16)
     y[0], y[1] = -32768, 362                                  # 65535^2 + 362^2 = 2^32 - 27: sqrtf rounds to 65 536
-    assert _get_dis(x, y) == 65536
-    bank = np.stack([_slot(np.tile(y, (119, 1)), 2880)])
+    assert get_dis(x, y) == 65536
+    bank = np.stack([make_slot(np.tile(y, (119, 1)), 2880)])
     handle.set_bank(bank, 1, 2880)
     feat = np.tile(x, (F_MAX, 1))
     seg_frm = np.ones(F_MAX, np.uint32)
@@ -313,9 +308,9 @@ def test_segs_headroom(handle):
 def test_segs_argument_rules(handle):
     """a segment over 818 frames, a decreasing seq_seg and a malformed grammar fail before anything is written"""
     rng = np.random.default_rng(0x13F)
-    bank = _bank(rng, 4, "small", plant=False)
+    bank = random_bank(rng, 4, "small", plant=False)
     handle.set_bank(bank, 4, bank.shape[1])
-    feat = _draw(rng, 900, "small")
+    feat = draw(rng, 900, "small")
     words = np.full((1, 4), 7, sr_b200.WORD_DTYPE)
     for seq_seg, seg_frm, g in (([0, 1], [819], LOOP), ([0, 2, 1], [1, 1], LOOP), ([0, 1], [5], (0, 1, []))):
         with pytest.raises(sr_b200.SrError):
@@ -328,7 +323,7 @@ def test_segs_loop_grammar_equals_connected_per_segment(handle):
     """property 1 on the GPU: under the loop grammar the kernel-level call equals sr_connected_batch on each decodable
     segment alone, joined in order, the totals summed"""
     rng = np.random.default_rng(0x140)
-    bank = _bank(rng, 20, "small")
+    bank = random_bank(rng, 20, "small")
     handle.set_bank(bank, 20, bank.shape[1])
     seqs = [[int(rng.choice([0, 1, 30, 119, 200, 818])) for _ in range(int(rng.integers(1, 12)))] for _ in range(40)]
     feat, seq_seg, seg_frm = _flat(rng, seqs)
@@ -393,7 +388,7 @@ def test_recognise_long_grammar_equals_composed_oracle(handle, geom):
     handle.set_geometry(geom)
     try:
         lens = np.array([160, 161, 30000, 65535, 200001, 240000], np.uint32)
-        pcm = _synth_long(lens, 240000, 0x1300)
+        pcm = synth_long_poisoned(lens, 240000, 0x1300)
         pp, pl = _planted_batch()
         cases = [(pcm, lens, 2400, None), (pp, pl, 0, plant_atap(len(pl)))]
         grams = (LOOP, sr_b200.chain_grammar(4, 0x7), (2, 3, [(0, 1, 0x5), (1, 0, 0xA), (1, 1, 0x1)]))
@@ -451,11 +446,6 @@ def test_short_recordings_equal_the_capture_call(handle):
 
 
 # ---- GPU: launches, scale and threads ------------------------------------------------------------------------------------
-def _tags(h):
-    t = [tag for tag, _ in h.timing_collect()]
-    return {k: t.count(k) for k in set(t)}
-
-
 def _cuts(N, S):
     """the host's rule: consecutive sequences while their records (N * S * 12 B) fit REC_BYTES, a sequence whose records
     alone exceed it on its own"""
@@ -474,7 +464,7 @@ def test_record_cuts_and_launch_counts(handle):
     per tag follow the host's rule, restated here, every row equals the oracle's and the one-launch slices of the batch"""
     lg = ox.long_grammar()
     rng = np.random.default_rng(0x141)
-    bank = _bank(rng, 16, "small", plant=False)
+    bank = random_bank(rng, 16, "small", plant=False)
     handle.set_bank(bank, 16, bank.shape[1])
     S = 16
     g = (S, 0xFFFF, [(k, (k + 1) % S, 0x1) for k in range(S)])   # 16 states x 4 slots of command 0: 64 copies
@@ -489,7 +479,7 @@ def test_record_cuts_and_launch_counts(handle):
     c0 = handle.launch_count()
     w, nw, tot = handle.connected_grammar_segs(feat, seq_seg, seg_frm, g, 1000, 16)
     assert handle.launch_count() - c0 == len(cuts) - 1
-    assert _tags(handle) == {TAG_LONG_GRAM: len(cuts) - 1}
+    assert tag_counts(handle) == {TAG_LONG_GRAM: len(cuts) - 1}
     ww, wn, wt = lg.decode_segs(feat, seq_seg, seg_frm, bank, 16, bank.shape[1], g, 1000, 16)
     assert nw.tolist() == wn.tolist() and tot.tolist() == wt.tolist() and w.tobytes() == ww.tobytes()
     row = np.cumsum(np.r_[0, seg_frm])
@@ -511,14 +501,14 @@ def test_groups_and_launches_of_the_end_to_end_call():
         h.timing_enable(4096)
         U = 1 << 24
         lens = np.array([U, U - 7, 3 * 80000, U, 161, U, U - 1, U, 999999, U], np.uint32)
-        pcm = _synth_long(lens, U, 0x1320)
+        pcm = synth_long_poisoned(lens, U, 0x1320)
         G = max(1, GROUP_BYTES // (2 * U))
         groups = -(-len(lens) // G)
         assert G == 8 and groups == 2
         c0 = h.launch_count()
         got = h.recognise_long_grammar(pcm, LOOP, 1000, 64, 64, 2400, lens)
         n = h.launch_count() - c0
-        t = _tags(h)
+        t = tag_counts(h)
         assert t[TAG_BLOCKS] == 2 * groups and t[TAG_SEGS] == groups and t[TAG_LONG_GRAM] == groups
         assert t[TAG_MFCC] >= groups and n == sum(t.values()) + t[TAG_MFCC]   # one untimed gather per get_mfcc launch
         for g0 in range(0, len(lens), G):
@@ -549,14 +539,14 @@ def test_threads_beside_a_recognise_long_handle():
     """two long-grammar handles and a sr_recognise_long_batch handle on one GPU in threads: every result equals the
     serial run"""
     lens = np.array([90000, 150000, 40000], np.uint32)
-    pcm = _synth_long(lens, 150000, 0x1340)
+    pcm = synth_long_poisoned(lens, 150000, 0x1340)
     chain = sr_b200.chain_grammar(5, 0x7)
 
     def job_a(h):
         return h.recognise_long_grammar(pcm, LOOP, 1000, 32, 64, 2400, lens)
 
     def job_b(h):
-        w, nw, tot = h.connected_grammar_segs(_draw(np.random.default_rng(1), 3000, "small"), [0, 3, 5],
+        w, nw, tot = h.connected_grammar_segs(draw(np.random.default_rng(1), 3000, "small"), [0, 3, 5],
                                               [818, 0, 500, 818, 864 - 818], chain, 7, 64)
         r = h.recognise_long_grammar(pcm, chain, 7, 32, 64, 2400, lens)
         return dict(w=w, nw=nw, tot=tot, **r)
@@ -603,15 +593,14 @@ def test_real_speech_digit_strings():
     lo, port, lg = ox.long_oracle(), ob.port(), ox.long_grammar()
     h = sr_b200.Handle(0)
     try:
-        for a_name, b_name in ((FIXTURES[0], FIXTURES[1]), (FIXTURES[1], FIXTURES[0]), (FIXTURES[2], FIXTURES[3]),
-                               (FIXTURES[3], FIXTURES[2])):
+        for a_name, b_name in real_speech_pairs():
             a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
             h.set_bank(np.zeros((0, 4096), np.uint8), 0, 4096)
             ea = h.recognise_long_batch(a[None], 32, 2400)
             ma = int(ea["n_segs"][0])
             ftr = ox.ftr_of_segments(port, a[None], ea["atap"], [(0, int(s["start"]), int(s["end"]) if s["end"] != NULL
                                                                   else int(s["start"])) for s in ea["segs"][0, :ma]])
-            bank, T = _bank_of(ftr)
+            bank, T = bank_of_ftr(ftr)
             h.set_bank(bank, T, 4096)
             K = T // 4
             any_digit = (1 << K) - 1

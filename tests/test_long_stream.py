@@ -25,9 +25,9 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
+from cases import DIGITS, LOUD, QUIET, frames_of, plant_act, plant_segs, planted_atap
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FIXTURES = ("digits_1_10_a", "digits_1_10_b", "digits_1_9_units_a", "digits_1_9_units_b")
 NULL = 0xFFFFFFFF
 ST_OK, ST_VAD_FAIL, ST_MFCC_FAIL = 0, 1, 2
 HEADER = open(os.path.join(ROOT, "include", "sr_long_stream.h")).read()
@@ -48,10 +48,6 @@ def window(max_chunk):
 def events_per_push(max_chunk, n_len):
     c = n_len if n_len and n_len % 240 == 0 else 0
     return -(-(-(-(max_chunk + c) // 80)) // 19)
-
-
-def frames_of(n):
-    return -(-(n - 160) // 80) if n > 160 else 0
 
 
 def decodable(length, geom):
@@ -195,43 +191,6 @@ def test_fsm_carried_over_windows_of_any_length():
         cuts = set(rng.choice(np.arange(1, n), size=min(k, n - 1), replace=False).tolist()) if n > 1 else set()
         assert fsm_cut(act, cuts) == fsm_seq(act), (act, cuts)
         assert fsm_cut(act, set(range(1, n))) == fsm_seq(act)
-
-
-# ---- planted inputs ------------------------------------------------------------------------------------------------------
-def planted_atap(S=1):
-    """under this atap every sample is below b_thl (mid - n_thl wraps), so no band crossing counts; a loud block (2 148)
-    sums |x - mid| = 8 000 and a frame is active exactly when both its blocks are loud (as planted() in test_long.py)"""
-    a = np.zeros(S, sr_b200.ATAP_DTYPE)
-    a["mid_val"], a["n_thl"], a["z_thl"], a["s_thl"] = 2048, 5000, 2, 15999
-    return a
-
-
-QUIET, LOUD, MARK = 2000, 2148, 4095
-
-
-def plant_segs(n_blocks, segs):
-    """n_blocks quiet blocks with loud blocks p .. p + a for each (p, a): a segment [80p, 80(p + a) + 80) of a active
-    frames, closed by the quiet blocks after it. Under planted_atap a frame sums 7 680 over two quiet blocks, 11 840 over a
-    quiet and a loud one and 16 000 over two loud ones (s_thl 15 999). Quiet samples differ from mid_val (2 048), and the
-    sample before each segment (its x[-1], in a quiet block) is MARK: get_mfcc's pre-emphasis of the segment's first sample
-    then tells the real x[-1] from the mid_val that is pinned at row offset 0. A marked quiet block sums 5 839, so a frame
-    over it stays inactive."""
-    x = np.full(80 * n_blocks, QUIET, np.uint16)
-    for p, a in segs:
-        x[80 * p:80 * (p + a + 1)] = LOUD
-        if p:
-            x[80 * p - 1] = MARK
-    return x
-
-
-def plant_act(act):
-    """PCM whose frames are active exactly where act is 1 (blocks k, k + 1 loud <=> frame k active), under planted_atap;
-    an isolated active frame is two loud blocks, so act is first widened into the frames it forces"""
-    act = np.asarray(act, bool)
-    loud = np.zeros(len(act) + 1, bool)
-    loud[:-1] |= act
-    loud[1:] |= act
-    return np.repeat(np.where(loud, LOUD, QUIET).astype(np.uint16), 80)
 
 
 # ---- the prefix definition -----------------------------------------------------------------------------------------------
@@ -474,7 +433,7 @@ def test_calibration_lengths(handle, bank, n_len, given):
 @pytest.mark.parametrize("c", [80, 640])
 def test_digit_recordings(handle, bank, c):
     handle.set_bank(bank[0], bank[1], 4096)
-    xs = [ox.golden_wav(n) for n in FIXTURES]
+    xs = [ox.golden_wav(n) for n in DIGITS]
     f = Feed(handle, xs, 640, 2400)
     N = np.array([len(x) for x in xs])
     while (f.n < N).any():

@@ -1,8 +1,8 @@
 """The template matchers at the inputs where a wrong kernel still passes random features: unique minima, the any-rate
 slides of the register band, first-wins ties across a reordered bank, the anchor and arithmetic edges of the averaging,
 and the path call's empty and oversized inputs. Each case is checked bit for bit against the oracles of tests/oracle_ext
-and the plain references of test_extension_refs.py, test_dp_align.py and test_any_rate.py; a CPU test proves that each
-plant reaches its case (the minimum is unique, the slide reaches s, the tie really ties) before the GPU relies on it.
+and the plain references of refs.py; a CPU test proves that each plant reaches its case (the minimum is unique, the slide
+reaches s, the tie really ties) before the GPU relies on it.
 DESIGN.md lists the mutants of K2, K3, K3p, K6 and the shared core, and the test that catches each."""
 import ctypes as C
 
@@ -12,12 +12,12 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_any_rate import rate_ref
-from test_dp_align import ALIGN, AVG_UPDATE, STRIDE, _slot, _slot_rows, average_ref, band_matrix, band_path_ref
-from test_extension_refs import DIS_ERR, MAX_FRM, NTHREADS, _ftr, band_dp_ref
-from test_sym_match import _want_best
+from cases import make_ftr, make_slot
+from refs import (DIS_ERR, MAX_FRM, NTHREADS, STRIDE, average_ref, band_dp_ref, band_matrix, band_path_ref, rate_ref,
+                  slot_rows, want_best)
 
 BAND, ANY = sr_b200.DTW_BAND, sr_b200.DTW_ANY_RATE
+ALIGN, AVG_UPDATE = 7, 8                     # tags of sr_timing_collect
 RADII = (0, 1, 9, 10, 11, 15, 16, 118)      # both edges of each band kernel: warp-scan (<= 15), thread (10), whole row
 R = 10                                       # the thread form's radius; its band holds W = 21 cells
 W = 2 * R + 1
@@ -74,7 +74,7 @@ def test_unique_minimum_features_every_band_kernel():
     """sr_dtw_batch(BAND) and (BAND | ANY_RATE) at r = 0, 1, 9, 10, 11, 15, 16, 118 on the unique-minimum case: scores and
     argmin against the port's band DP and the any-rate oracle, and every pair against band_dp_ref / rate_ref"""
     utt, tpl = unique_case()
-    fin, bank = _ftr(utt), sr_b200.make_bank(_ftr(tpl), STRIDE)
+    fin, bank = make_ftr(utt), sr_b200.make_bank(make_ftr(tpl), STRIDE)
     po, ro = ob.port(), ox.rate_oracle()
     h = sr_b200.Handle(0)
     h.set_bank(bank, len(tpl), STRIDE)
@@ -87,7 +87,7 @@ def test_unique_minimum_features_every_band_kernel():
                 else:
                     want, _ = po.dtw_batch(fin, bank, len(tpl), STRIDE, band_r=r, nthreads=NTHREADS)
                 assert np.array_equal(score, want), (r, flags, np.argwhere(score != want)[:4].tolist())
-                wi, wd = _want_best(want)
+                wi, wd = want_best(want)
                 assert np.array_equal(bi, wi) and np.array_equal(bd, wd), (r, flags)
                 for u, x in enumerate(utt):
                     for t, y in enumerate(tpl):
@@ -181,7 +181,7 @@ def test_thread_form_slides_equal_oracle_and_plain_reference():
     pairs, plants = slide_case()
     utt = [p[0] for p in pairs]
     tpl = [p[1] for p in pairs]
-    fin, bank = _ftr(utt), sr_b200.make_bank(_ftr(tpl), STRIDE)
+    fin, bank = make_ftr(utt), sr_b200.make_bank(make_ftr(tpl), STRIDE)
     T = len(tpl)
     h = sr_b200.Handle(0)
     h.set_bank(bank, T, STRIDE)
@@ -189,7 +189,7 @@ def test_thread_form_slides_equal_oracle_and_plain_reference():
         score, bi, bd = h.dtw(fin, flags=BAND | ANY, band_r=R)
         want = ox.rate_oracle().dtw_batch(fin, bank, T, STRIDE, band_r=R, nthreads=NTHREADS)
         assert np.array_equal(score, want), np.argwhere(score != want)[:4].tolist()
-        wi, wd = _want_best(want)
+        wi, wd = want_best(want)
         assert np.array_equal(bi, wi) and np.array_equal(bd, wd)
         for k, (x, y) in enumerate(pairs):
             d = rate_ref(x, y, R)
@@ -209,11 +209,11 @@ def tie_bank(T):
     duplicate the remainder tile"""
     row = np.array([7, -3, 11, 0, -25, 4, 9, -1, 2, 3, -8, 6], np.int16)
     lens = [MAX_FRM] + [60 + (k * 37) % 59 for k in range(1, T - 1)] + [MAX_FRM]
-    return sr_b200.make_bank(_ftr([np.tile(row, (n, 1)) for n in lens]), STRIDE), lens, row
+    return sr_b200.make_bank(make_ftr([np.tile(row, (n, 1)) for n in lens]), STRIDE), lens, row
 
 
 def tie_inputs(row):
-    return _ftr([np.tile(row, (n, 1)) for n in (60, 80, 100, 119)])
+    return make_ftr([np.tile(row, (n, 1)) for n in (60, 80, 100, 119)])
 
 
 def test_tie_bank_ties_everywhere_and_is_visited_out_of_order():
@@ -271,8 +271,8 @@ def failed_case():
     rng = np.random.default_rng(0xE7)
     pcm = sr_b200.synth_pcm_host(5, 8000, 0xFA11ED00)
     pcm[FAILED_U] = 2048
-    bank = sr_b200.make_bank(_ftr([rng.integers(-3000, 3001, (int(n), 12)) for n in rng.integers(20, 41, 6)]), 4096)
-    bank[ZERO_SLOT] = _slot(np.zeros((0, 12)), 4096, frm=0)
+    bank = sr_b200.make_bank(make_ftr([rng.integers(-3000, 3001, (int(n), 12)) for n in rng.integers(20, 41, 6)]), 4096)
+    bank[ZERO_SLOT] = make_slot(np.zeros((0, 12)), 4096, frm=0)
     return pcm, bank
 
 
@@ -284,7 +284,7 @@ def test_failed_case_plants():
     ref = ora.recognise_batch(pcm, 2400, bank, len(bank), 4096)
     assert ref["status"][FAILED_U] != 0 and (np.delete(ref["status"], FAILED_U) == 0).all()
     assert (ref["score"][FAILED_U] == DIS_ERR).all()
-    empty = _ftr([np.zeros((0, 12), np.int16)])
+    empty = make_ftr([np.zeros((0, 12), np.int16)])
     assert ora.dtw_batch(empty, bank, len(bank), 4096)[0][0, ZERO_SLOT] != DIS_ERR
 
 
@@ -322,7 +322,7 @@ def _group_slots(members, K, stride=STRIDE):
     """one group of K slots: members {k: rows}, the other slots erased"""
     g = np.full((K, stride), 0xFF, np.uint8)
     for k, rows in members.items():
-        g[k] = _slot(rows, stride)
+        g[k] = make_slot(rows, stride)
     return g
 
 
@@ -350,9 +350,9 @@ def test_anchor_bank_plants():
     bank = anchor_bank()
     out, score, anchor = average_ref(bank, STRIDE, 32, AVG_R, 1)
     assert anchor.tolist() == ANCHORS
-    same = _slot_rows(bank[0])[2]
+    same = slot_rows(bank[0])[2]
     assert band_path_ref(same, same, AVG_R)[0] == 0
-    chain = [_slot_rows(bank[34 * 32 + k])[2] for k in range(26, 32)]
+    chain = [slot_rows(bank[34 * 32 + k])[2] for k in range(26, 32)]
     for a in chain:
         for b in chain:
             if a is not b:
@@ -378,10 +378,10 @@ def arithmetic_bank():
 def _sums(bank, K, r, g):
     """(sum, count) per template cell of group g's first update, from band_path_ref paths against its anchor"""
     _, _, anchor = average_ref(bank, STRIDE, K, r, 0)
-    C0 = _slot_rows(bank[g * K + anchor[g]])[2]
+    C0 = slot_rows(bank[g * K + anchor[g]])[2]
     tot, cnt = np.zeros_like(C0), np.zeros(len(C0), np.int64)
     for k in range(K):
-        _, n, x = _slot_rows(bank[g * K + k])
+        _, n, x = slot_rows(bank[g * K + k])
         if x is None or n == 0:
             continue
         s, path, _ = band_path_ref(x, C0, r)
@@ -400,10 +400,10 @@ def test_arithmetic_bank_plants():
         q = tot / cnt[:, None]
         assert ((tot < 0) & (np.trunc(q) != np.floor(q))).any(), r
     _, _, anchor = average_ref(bank, STRIDE, 4, 118, 0)
-    C0 = _slot_rows(bank[2 * 4 + anchor[2]])[2]
-    _, path, _ = band_path_ref(_slot_rows(bank[2 * 4 + 2])[2], C0, 118)
+    C0 = slot_rows(bank[2 * 4 + anchor[2]])[2]
+    _, path, _ = band_path_ref(slot_rows(bank[2 * 4 + 2])[2], C0, 118)
     assert len(C0) == 30 and sum(1 for _, j in path if j == 0) == 60 - 30 + 1
-    assert (_slot_rows(bank[0])[2] == -32768).any() and (_slot_rows(bank[0])[2] == 32767).any()
+    assert (slot_rows(bank[0])[2] == -32768).any() and (slot_rows(bank[0])[2] == 32767).any()
 
 
 def _average_and_count(h, bank, K, r, iters):
@@ -444,9 +444,9 @@ def test_average_bank_pass_counts():
     rng = np.random.default_rng(0xE5)
     one = np.concatenate([_group_slots({0: rng.integers(-3000, 3001, (n, 12))}, 1) for n in (1, 2, 50, 119)])
     empty = np.full((3 * 4, STRIDE), 0xFF, np.uint8)
-    empty[1] = _slot(np.zeros((0, 12)), STRIDE, frm=0)
-    empty[2] = _slot(rng.integers(-9, 9, (5, 12)), STRIDE, frm=120)
-    empty[3] = _slot(rng.integers(-3000, 3001, (10, 12)), STRIDE, sign=0)
+    empty[1] = make_slot(np.zeros((0, 12)), STRIDE, frm=0)
+    empty[2] = make_slot(rng.integers(-9, 9, (5, 12)), STRIDE, frm=120)
+    empty[3] = make_slot(rng.integers(-3000, 3001, (10, 12)), STRIDE, sign=0)
     h = sr_b200.Handle(0)
     h.timing_enable(64)
     try:
@@ -466,8 +466,8 @@ def _path_inputs():
     """pairs 0 and 1 have 0 frames on one side; in pair 2 the input and in pair 4 the template says 120 frames (past
     vv_frm_max) against a partner the 2:1 guard admits (119 and 80 frames), so only the frame count rejects them"""
     rng = np.random.default_rng(0xE6)
-    a = _ftr([rng.integers(-3000, 3001, (n, 12)) for n in (0, 5, 119, 60, 80)])
-    b = _ftr([rng.integers(-3000, 3001, (n, 12)) for n in (5, 0, 119, 59, 80)])
+    a = make_ftr([rng.integers(-3000, 3001, (n, 12)) for n in (0, 5, 119, 60, 80)])
+    b = make_ftr([rng.integers(-3000, 3001, (n, 12)) for n in (5, 0, 119, 59, 80)])
     a["frm_num"][2] = 120
     b["frm_num"][4] = 120
     return a, b

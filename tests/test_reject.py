@@ -18,11 +18,8 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from test_any_rate import _digit_bank, _real_speech_pairs
-from test_any_rate import _scores as _scores_rate
-from test_any_rate import long_oracle as long_oracle_rate
-from test_sym_match import _bank_planted, _inputs, _k14_events, _k4_events
-from test_sym_match import _scores as _scores_sym
+from cases import bank_planted, digit_bank, inputs, real_speech_pairs, synth_long_poisoned
+from drive import handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NULL = DIS_ERR = 0xFFFFFFFF
@@ -130,18 +127,18 @@ def _margin_table(q):
     right, out-of-vocabulary words, rejected)"""
     lo, port = ox.long_oracle(), ob.port()
     rows = []
-    for a_name, b_name in _real_speech_pairs():
+    for a_name, b_name in real_speech_pairs():
         a, b = ox.golden_wav(a_name), ox.golden_wav(b_name)
-        bank, T, ma = _digit_bank(port, lo, a)
+        bank, T, ma = digit_bank(port, lo, a)
         half = ma // 2
         bank = bank.copy()
         bank[4 * half:, 0:2] = 0xFF                                  # words half .. ma - 1 not enrolled: unsigned slots
-        w = long_oracle_rate(b[None], bank, T, RATE, 118, 32)
+        w = ox.recognise_long(lo, port, b[None], 2400, bank, T, 4096, 32, match=(RATE, 118))
         m = min(int(w["n_segs"][0]), ma)
         segs = w["segs"][0, :m]
         todo = [k for k in range(m) if segs[k]["status"] == OK]
         ftr = ox.ftr_of_segments(port, b[None], w["atap"], [(0, int(segs[k]["start"]), int(segs[k]["end"])) for k in todo])
-        sc = _scores_rate(ftr, bank, T, RATE, 118)
+        sc = ox.match_scores(ftr, bank, T, RATE, 118)
         idx, _, rej = rule_ref(sc, q)
         inv = np.array([k < half for k in todo])
         right = idx // 4 == np.array(todo)
@@ -191,8 +188,8 @@ def test_dtw_batch_refuses_the_rule_bits():
     h = sr_b200.Handle(0)
     try:
         rng = np.random.default_rng(0x7E2)
-        h.set_bank(_bank_planted(rng, 8), 8, 4096)
-        fin = _inputs(rng, [30, 40, 50])
+        h.set_bank(bank_planted(rng, 8), 8, 4096)
+        fin = inputs(rng, [30, 40, 50])
         score = np.full((3, 8), 0xA5A5A5A5, np.uint32)
         bi, bd = np.full(3, 0xA5A5A5A5, np.uint32), np.full(3, 0xA5A5A5A5, np.uint32)
         dev = torch.device("cuda:0")
@@ -249,19 +246,6 @@ def case():
     return {"pcm": pcm, "front": front, "bank": _bank_of(80, 0x7E3A0000), "T": 80}
 
 
-def _oracle_scores(ftr, bank, T, flags, r):
-    if flags == RATE:
-        return _scores_rate(ftr, bank, T, RATE, r)
-    return _scores_sym(ftr, bank, T, flags, r)
-
-
-def _handle(bank, T, flags, r):
-    h = sr_b200.Handle(0)
-    h.set_bank(bank, T, 4096)
-    h.set_match(flags, r)
-    return h
-
-
 def _same_but_status(on, off, q, what):
     """the rule-on result equals the rule-off one field by field, except status, which is the rule on off's scores"""
     for k in ("seg_off", "score", "best_idx", "best_dis", "cmd"):
@@ -280,19 +264,18 @@ def test_recognise_paths_equal_oracle_and_rule(case, matcher):
     plain and the packed transport and sr_recognise_batch_dev on a torch stream equal it except for SR_ST_REJECT, which
     is exactly the rule on the oracle's scores; launch counts and timing tags are the rule-off call's. Rejections grow
     with q, and q = 100 keeps some decisions"""
-    from test_gpu_parity import _recognise_dev_np
     flags, r = matcher
     pcm, front, bank, T = case["pcm"], case["front"], case["bank"], case["T"]
     good = front["status"] == OK
-    sc = _oracle_scores(front["ftr"][good], bank, T, flags, r)
-    h = _handle(bank, T, flags, r)
+    sc = ox.match_scores(front["ftr"][good], bank, T, flags, r)
+    h = handle(bank, T, flags, r)
     try:
         h.set_transport(0)
         h.timing_enable(64)
         off = h.recognise(pcm, 2400)
         assert np.array_equal(off["score"][good], sc) and (off["status"] == front["status"]).all()
         tags_off = [t for t, _ in h.timing_collect()]
-        dev_off = _recognise_dev_np(h, pcm, 2400, T)
+        dev_off = recognise_dev_np(h, pcm, 2400, T)
         h.use_own_stream()
         h.timing_collect()
         n_rej = {}
@@ -307,7 +290,7 @@ def test_recognise_paths_equal_oracle_and_rule(case, matcher):
             h.set_transport(1)
             _same_but_status(h.recognise(pcm, 2400), off, q, "host packed")
             h.timing_collect()
-            _same_but_status(_recognise_dev_np(h, pcm, 2400, T), dev_off, q, "device")
+            _same_but_status(recognise_dev_np(h, pcm, 2400, T), dev_off, q, "device")
             h.use_own_stream()
             h.set_match(flags, r)
             h.set_transport(0)
@@ -325,7 +308,7 @@ def test_rule_boundary_and_runner_up_are_exact(case):
     """q chosen so that 1000 (d2 - d1) == q d1 exactly for some utterance: that decision stands (strict '<'); and every
     decision whose winner's own command holds the next slot is judged by the next command, not the next slot"""
     pcm, bank, T = case["pcm"], case["bank"], case["T"]
-    h = _handle(bank, T, 0, 0)
+    h = handle(bank, T, 0, 0)
     try:
         off = h.recognise(pcm, 2400)
         good = off["status"] == OK
@@ -355,19 +338,18 @@ def test_bank_widths_and_batch_edges(T):
     """banks of 1, 2, 5, 80 and 1024 slots (one thread per utterance up to 32 commands, a warp beyond), batches just
     below, at and above multiples of the scan's rows (132 and 2112 utterances), under the greedy walk and each band
     kernel: the rule-on device call equals the rule-off one except where the rule says"""
-    from test_gpu_parity import _recognise_dev_np
     bank = _bank_of(T, 0x7E3B0000 + T)
-    h = _handle(bank, T, 0, 0)
+    h = handle(bank, T, 0, 0)
     try:
         for B in ((131, 132, 133) if T != 1024 else (131, 2113)):
             pcm = sr_b200.synth_pcm_host(B, U, 0x7E360000 + B, 2)
             for flags, r in ((0, 0), (BAND, 5), (BAND, 10), (BAND, 16), (SYM, 10)):
                 h.set_match(flags, r)
-                off = _recognise_dev_np(h, pcm, 2400, T)
+                off = recognise_dev_np(h, pcm, 2400, T)
                 h.use_own_stream()
                 for q in (100, 65535):
                     h.set_match(flags | REJ(q), r)
-                    n = _same_but_status(_recognise_dev_np(h, pcm, 2400, T), off, q, (T, B, flags, r))
+                    n = _same_but_status(recognise_dev_np(h, pcm, 2400, T), off, q, (T, B, flags, r))
                     h.use_own_stream()
                     if T <= 4:
                         assert n == 0                                # one command: nothing to compare with
@@ -385,7 +367,7 @@ def _long_status(pcm, lens, bank, T, flags, r, q, max_segs, rec):
     if todo:
         ftr = ox.ftr_of_segments(ob.port(), pcm, w["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
                                                              for b, k in todo])
-        sc = _oracle_scores(ftr, bank, T, flags, r)
+        sc = ox.match_scores(ftr, bank, T, flags, r)
         idx, d1, rej = rule_ref(sc, q)
         for i, (b, k) in enumerate(todo):
             if sc[i].min() != DIS_ERR:
@@ -411,15 +393,11 @@ def _cmp_long_rule(on, off, want_status, what):
 def test_long_batch_and_dev_under_the_rule(matcher):
     """sr_recognise_long_batch and its _dev form: the rule-on records equal the rule-off ones except status, which is
     SR_ST_REJECT exactly where the rule on the oracle's scores says; same launches and tags"""
-    import torch
     flags, r = matcher
     lens = np.array([70001, 161, 123457, 99999, 200000], np.uint32)
-    Ul = 200000
-    pcm = ox.synth_long(len(lens), Ul, 0x7E40)
-    for b, n in enumerate(lens):
-        pcm[b, n:] = np.where(np.arange(Ul - n) % 2, 4095, 0)
+    pcm = synth_long_poisoned(lens, 200000, 0x7E40)
     bank, T = _bank_of(40, 0x7E3C0000), 40
-    h = _handle(bank, T, flags, r)
+    h = handle(bank, T, flags, r)
     try:
         h.timing_enable(64)
         off = h.recognise_long_batch(pcm, 64, 2400, lens)
@@ -431,17 +409,8 @@ def test_long_batch_and_dev_under_the_rule(matcher):
             on = h.recognise_long_batch(pcm, 64, 2400, lens)
             assert [t for t, _ in h.timing_collect()] == tags
             total += _cmp_long_rule(on, off, want, "host")
-            dev = torch.device("cuda:0")
-            d_pcm = torch.from_numpy(pcm.view(np.int16)).to(dev)
-            d_lens = torch.from_numpy(lens.view(np.int32)).to(dev)
-            d_n = torch.zeros(len(lens), dtype=torch.int32, device=dev)
-            d_segs = torch.zeros(len(lens) * 64 * 7, dtype=torch.int32, device=dev)
-            h.recognise_long_batch_dev(d_pcm.data_ptr(), Ul, len(lens), d_lens.data_ptr(), 2400, 64, None, d_n.data_ptr(),
-                                       d_segs.data_ptr())
-            h.sync()
+            got = recognise_long_dev_np(h, pcm, lens, 64)
             h.timing_collect()
-            got = dict(n_segs=d_n.cpu().numpy().view(np.uint32),
-                       segs=d_segs.cpu().numpy().view(ox.LONG_SEG_DTYPE).reshape(len(lens), 64))
             _cmp_long_rule(got, off, want, "dev")
         assert total > 0
     finally:
@@ -462,7 +431,7 @@ def test_k4_streams_under_the_rule():
     pcm[3] = 2048
     runs = {}
     for label, qs in (("off", None), ("on", (0, 100, 1000))):
-        h = _handle(bank, T, BAND, 10)
+        h = handle(bank, T, BAND, 10)
         try:
             pool = sr_b200.StreamPool(h, S, L, 2400)
 
@@ -472,7 +441,7 @@ def test_k4_streams_under_the_rule():
                 q = qs[p % 3]
                 h.set_match(BAND | REJ(q), 10)
                 return q
-            runs[label] = _k4_events(pool, pcm, "ragged", np.random.default_rng(0x7E4), on_push)
+            runs[label] = k4_events(pool, pcm, "ragged", np.random.default_rng(0x7E4), on_push)
             seg, atap = pool.segments()
             pool.close()
         finally:
@@ -488,7 +457,7 @@ def test_k4_streams_under_the_rule():
         if want == OK and q:
             s, k = _event_key(e)
             f = ora.mfcc_batch(pcm[s:s + 1], seg[s, k].reshape(1, 2), atap[s:s + 1])
-            sc = _oracle_scores(f, bank, T, BAND, 10)
+            sc = ox.match_scores(f, bank, T, BAND, 10)
             idx, d1, rej = rule_ref(sc, q)
             assert (idx[0], d1[0]) == (o["best_idx"], o["best_dis"])
             want = REJECT if rej[0] else OK
@@ -505,7 +474,7 @@ def test_k14_rule_switched_between_pushes():
     bank, T = _bank_of(40, 0x7E3E0000), 40
     runs = {}
     for label, qs in (("off", None), ("on", (0, 100, 65535))):
-        h = _handle(bank, T, 0, 0)
+        h = handle(bank, T, 0, 0)
         try:
             pool = sr_b200.LongStreamPool(h, len(xs), 3000, 2400)
 
@@ -515,7 +484,7 @@ def test_k14_rule_switched_between_pushes():
                 q = qs[p % 3]
                 h.set_match(REJ(q), 0)
                 return q
-            runs[label] = _k14_events(pool, xs, 3000, on_push)
+            runs[label] = k14_events(pool, xs, 3000, on_push)
             pool.close()
         finally:
             h.close()
@@ -536,7 +505,7 @@ def test_k14_rule_switched_between_pushes():
         if want == OK and q:
             s = int(e["stream"])
             f = ox.ftr_of_segments(ob.port(), pcm, w["atap"], [(s, int(e["start"]), int(e["end"]))])
-            sc = _oracle_scores(f, bank, T, 0, 0)
+            sc = ox.match_scores(f, bank, T, 0, 0)
             want = REJECT if rule_ref(sc, q)[2][0] else OK
         assert e["status"] == want, (e, o, q)
         n_rej += want == REJECT
@@ -552,7 +521,7 @@ def test_multi_and_groups_refuse_unequal_rules(case):
     import torch
     bank, T, pcm = case["bank"], case["T"], case["pcm"][:64]
     two = torch.cuda.device_count() > 1
-    a = _handle(bank, T, REJ(100), 0)
+    a = handle(bank, T, REJ(100), 0)
     b = sr_b200.Handle(1 if two else 0)
     b.set_bank(bank, T, 4096)
     try:
@@ -582,7 +551,7 @@ def test_two_threads_with_different_rules(case):
     """two handles on one GPU, q = 100 and q = 65535, recognising concurrently from two threads: each result equals its
     handle's result alone"""
     bank, T, pcm = case["bank"], case["T"], case["pcm"][:300]
-    hs = [_handle(bank, T, BAND | REJ(q), 10) for q in (100, 65535)]
+    hs = [handle(bank, T, BAND | REJ(q), 10) for q in (100, 65535)]
     try:
         alone = [h.recognise(pcm, 2400) for h in hs]
         assert not np.array_equal(alone[0]["status"], alone[1]["status"])

@@ -29,7 +29,7 @@ import oracle_bind as ob  # noqa: E402
 import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_match import card  # noqa: E402
-from test_connected_launches import _pieces, launch_sample, piece_plan, seq_launches  # noqa: E402
+from refs import launch_sample, piece_plan, pieces, seq_launches  # noqa: E402
 
 NPROC = os.cpu_count() or 1
 PENALTY = 4000
@@ -44,7 +44,7 @@ def e2e_edges(frm_num, seq_ranges=None):
     """the captures holding the first and last get_mfcc piece of every piece launch and, given the decoder's launch ranges
     over the captures' segments with frames (default: one sequence per segment, K6), of every decoder launch"""
     B = len(frm_num)
-    e = piece_plan(_pieces(frm_num).sum(1))[1]
+    e = piece_plan(pieces(frm_num).sum(1))[1]
     if seq_ranges is None:
         owner = np.repeat(np.arange(B), (frm_num > 0).sum(1))
         e |= {int(owner[i]) for i in edges(seq_launches([0, len(owner)]))}

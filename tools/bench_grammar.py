@@ -29,7 +29,7 @@ import oracle_ext as ox  # noqa: E402
 import sr_b200  # noqa: E402
 from bench_connected import e2e_edges, edges, synth_bank, timed  # noqa: E402
 from bench_match import card  # noqa: E402
-from test_connected_launches import launch_sample, record_cuts, seq_launches  # noqa: E402
+from refs import launch_sample, record_cuts, seq_launches  # noqa: E402
 
 NPROC = os.cpu_count() or 1
 PENALTY = 4000

@@ -98,14 +98,10 @@ def main():
     RATE = sr_b200.DTW_BAND | sr_b200.DTW_ANY_RATE
 
     def oracle(flags, r):
-        nth = os.cpu_count() or 1
-        sc, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1,
-                                        band_r=r if flags else -1, nthreads=nth)
-        if flags == SYM:                    # the symmetric DP's scores; cells: the banded DP's at the same radius
-            sc = ox.sym_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
-        if flags == RATE:                   # without the 2:1 guard; cells as above
-            sc = ox.rate_oracle().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r, nthreads=nth)
-        return sc, cells
+        """the matcher's scores, and the cells of the port's greedy or banded DP at the same radius"""
+        _, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r if flags else -1,
+                                       nthreads=os.cpu_count() or 1)
+        return ox.match_scores(front["ftr"][good], bank_h, T, flags, r), cells
 
     def run(flags, r):
         h.set_match(flags, r)
