@@ -179,11 +179,7 @@ void sr_host_free(void *p) {
 
 int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 
-// ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
-enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
-       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
-       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13, TAG_DTW_SYM = 14 };
-
+// ---- kernel launches (launch_on, sr_internal.h) --------------------------------------------------------------------
 // the timing tag of the template scan under flags (launch_scan's choice)
 static int scan_tag(u32 flags) {
     return (flags & SR_DTW_SYM_P1) ? TAG_DTW_SYM : (flags & SR_DTW_BAND) ? TAG_DTW_BAND : TAG_DTW;
@@ -227,30 +223,21 @@ int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uin
 
 }  // extern "C"
 
-// one kernel launch on the handle's stream, launch() returning its cudaError_t: bracketed by an event pair when tag is
-// not TAG_NONE and timing is enabled, counted when it succeeds
-template <class F> static int launch_on(sr_handle *h, int tag, const char *what, F launch) {
-    size_t slot = SIZE_MAX;
-    if (tag != TAG_NONE && h->timing && (h->ev_used + 1) * 2 <= h->ev.size()) {
-        slot = h->ev_used++;
-        h->ev_tag[slot] = tag;
-        cudaEventRecord(h->ev[2 * slot], h->stream);
-    }
-    const cudaError_t e = launch();
-    if (slot != SIZE_MAX) cudaEventRecord(h->ev[2 * slot + 1], h->stream);
-    if (e != cudaSuccess) return fail(h, what, e);
-    ++h->launches;
-    return 0;
-}
-#define SR_LAUNCH(h, tag, call)                                                                   \
-    do {                                                                                          \
-        if (const int rc__ = launch_on((h), (tag), #call, [&] { return (call); })) return rc__;   \
-    } while (0)
-
 // get_mfcc (MFCC.C) and get_mdl (DTW.C) never write save_sign: copy back bytes [2, 2860) of each of n structs only
 static cudaError_t ftr_to_host(sr_handle *h, v_ftr_tag *dst, const void *src, size_t n) {
     return cudaMemcpy2DAsync(reinterpret_cast<unsigned char *>(dst) + 2, kFtrBytes, static_cast<const unsigned char *>(src) + 2,
                              kFtrBytes, kFtrBytes - 2, n, cudaMemcpyDeviceToHost, h->stream);
+}
+
+// the captures of a host-buffer call: 1..65 535 samples each, the calibration window inside them
+static bool capture_args_ok(u32 U, u32 B, u32 n_len) { return (B == 0 || U > 0) && U <= 65535u && n_len <= U; }
+
+// the B atap records noise_atap runs on: the caller's (atap != NULL), else B zeroed ones in w
+static cudaError_t atap_or_zeroed(sr_handle *h, DevBuf &w, u32 B, atap_tag *&atap) {
+    if (atap) return cudaSuccess;
+    const cudaError_t e = ensure(w, (size_t)B * sizeof(atap_tag));
+    atap = static_cast<atap_tag *>(w.p);
+    return e != cudaSuccess ? e : cudaMemsetAsync(atap, 0, (size_t)B * sizeof(atap_tag), h->stream);
 }
 
 // One host-buffer call: inputs staged into handle workspaces, kernels, outputs copied back, one synchronisation. The
@@ -293,6 +280,15 @@ struct HostCall {
         if (d && dst && bytes) back[n_back++] = {dst, d, bytes, std::is_same_v<T, v_ftr_tag>};
         return d;
     }
+    // B atap records in w (atap_or_zeroed): the caller's host records staged in -- and copied back when `back`: noise_atap
+    // leaves them untouched when n_len % 240 != 0 -- or zeroed ones when src is NULL
+    atap_tag *atap(DevBuf &w, atap_tag *src, u32 B, bool back) {
+        const size_t bytes = (size_t)B * sizeof(atap_tag);
+        atap_tag *d = src ? in(w, src, bytes) : nullptr;
+        if (src && back) out(w, src, bytes);
+        if (!src && !rc) ck("atap_or_zeroed", atap_or_zeroed(h, w, B, d));
+        return rc ? nullptr : d;
+    }
     int finish() {
         for (int i = 0; i < n_back; ++i) {
             const Back &b = back[i];
@@ -302,6 +298,31 @@ struct HostCall {
         ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
         return rc;
     }
+};
+
+// Host PCM [B][U] of the host call c sent to the device in n groups of G recordings (the last one fewer) through the two
+// buffers of h->pcm: with more than one group, the copy of the next group (copy stream) overlaps the kernels of this one
+// (compute stream).
+struct PcmGroups {
+    sr_handle *h;
+    u32 G, n;
+    size_t bytes;                                       // one buffer: G recordings, 256-byte aligned
+    PcmGroups(HostCall &c, u32 U, u32 B, u32 g) : h(c.h), G(g), n((B + g - 1) / g), bytes((((size_t)g * U * 2 + 255) / 256) * 256) {
+        c.ws(h->pcm, (n > 1 ? 2 : 1) * bytes + 16);
+    }
+    u16 *buf(int i) const { return reinterpret_cast<u16 *>(static_cast<unsigned char *>(h->pcm.p) + (size_t)i * bytes); }
+    // the k-th group sent, into buffer k & 1: once the kernels of group k - 2 are done with it, `size` bytes from src to dst,
+    // then the compute stream waits for the copy
+    cudaError_t send(u32 k, void *dst, const void *src, size_t size) const {
+        if (n == 1) return cudaMemcpyAsync(dst, src, size, cudaMemcpyHostToDevice, h->stream);
+        cudaError_t e = k >= 2 ? cudaStreamWaitEvent(h->copy_stream, h->ev_done[k & 1], 0) : cudaSuccess;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src, size, cudaMemcpyHostToDevice, h->copy_stream);
+        if (e == cudaSuccess) e = cudaEventRecord(h->ev_h2d[k & 1], h->copy_stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(h->stream, h->ev_h2d[k & 1], 0);
+        return e;
+    }
+    // after the kernels of the k-th group: its buffer is free again
+    cudaError_t done(u32 k) const { return n > 1 ? cudaEventRecord(h->ev_done[k & 1], h->stream) : cudaSuccess; }
 };
 
 extern "C" {
@@ -416,6 +437,23 @@ int sr_mfcc_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
 
 }  // extern "C"
 
+// main.c:276-291 on n inputs (n_dev: n on the device): w's n argmin keys, then under the margin rule (C > 0) n * C
+// per-command keys, set to their start (tag 3), and the template scan into them (4, 6 or 14); no w: it writes scores only
+static int scan_to_keys(sr_handle *h, DevBuf *w, u32 C, const BankView &bank, const void *in, u32 n, u32 flags, int band_r,
+                        u32 *score, const u8 *status, u64 *&keys, const u32 *n_dev = nullptr) {
+    keys = nullptr;
+    if (w) {
+        SR_CK(h, ensure(*w, (size_t)n * (1 + C) * 8));
+        keys = static_cast<u64 *>(w->p) + (C ? n : 0);
+        SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(keys, (u64)n * (C ? C : 1), h->stream));
+    }
+    if (bank.n) {
+        if (flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) SR_REQUIRE(h, band_r >= 0);
+        SR_LAUNCH(h, scan_tag(flags), launch_scan(h, bank, in, n, flags, band_r, score, keys, status, n_dev));
+    }
+    return 0;
+}
+
 // the template scan of B inputs against `bank`, then the argmin of each when one of best_idx / best_dis / cmd is wanted
 static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                         uint32_t *score, uint32_t *best_idx, uint32_t *best_dis, uint32_t *cmd, const u8 *status) {
@@ -423,23 +461,14 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
     SR_REQUIRE(h, scan_flags_ok(flags));
     if (B == 0) return 0;
-    // under the margin rule (C > 0) the status is an output of the decision too, and the scan writes per-command keys
-    // after the B argmin keys
+    // under the margin rule (C > 0) the status is an output of the decision too
     const u32 C = status ? rule_cols(flags, bank.n) : 0;
     if (!C) flags &= 0xFFFFu;
     const bool want_best = best_idx || best_dis || cmd || C;
-    u64 *best = nullptr, *keys = nullptr;
-    if (want_best) {
-        DevBuf &bb = h->best_sel ? h->best_alt : h->best;
-        SR_CK(h, ensure(bb, (size_t)B * (1 + C) * 8));
-        best = static_cast<u64 *>(bb.p);
-        keys = C ? best + B : best;
-        SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(keys, (u64)B * (C ? C : 1), h->stream));
-    }
-    if (bank.n) {
-        if (flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) SR_REQUIRE(h, band_r >= 0);
-        SR_LAUNCH(h, scan_tag(flags), launch_scan(h, bank, in, B, flags, band_r, score, keys, status));
-    }
+    DevBuf &bb = h->best_sel ? h->best_alt : h->best;
+    u64 *keys;
+    if (const int rc = scan_to_keys(h, want_best ? &bb : nullptr, C, bank, in, B, flags, band_r, score, status, keys)) return rc;
+    u64 *best = static_cast<u64 *>(bb.p);
     if (want_best && C)
         SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final_reject(best, keys, B, C, rule_q(flags), best_idx, best_dis, cmd,
                                                               const_cast<u8 *>(status), h->stream));
@@ -499,11 +528,7 @@ int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     if (B == 0) return 0;
     DeviceGuard g(h->device);
     atap_tag *atap = o->atap;
-    if (!atap) {
-        SR_CK(h, ensure(h->atap, (size_t)B * sizeof(atap_tag)));
-        atap = static_cast<atap_tag *>(h->atap.p);
-        SR_CK(h, cudaMemsetAsync(atap, 0, (size_t)B * sizeof(atap_tag), h->stream));
-    }
+    SR_CK(h, atap_or_zeroed(h, h->atap, B, atap));
     u32 *seg = o->seg_off;
     if (!seg) { SR_CK(h, ensure(h->seg, (size_t)B * 24)); seg = static_cast<u32 *>(h->seg.p); }
     v_ftr_tag *ftr = o->ftr;
@@ -556,8 +581,7 @@ int sr_noise_atap_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t 
     if (B == 0) return 0;
     HostCall c(h, "sr_noise_atap_batch");
     const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    atap_tag *d_atap = c.in(h->atap, atap, (size_t)B * sizeof(atap_tag));      // in / out: untouched when n_len % 240 != 0
-    c.out(h->atap, atap, (size_t)B * sizeof(atap_tag));
+    atap_tag *d_atap = c.atap(h->atap, atap, B, true);
     c.run([&] { return sr_noise_atap_batch_dev(h, d_pcm, U, B, n_len, d_atap); });
     return c.finish();
 }
@@ -634,16 +658,14 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
 // with pinned host memory the call is bound by max(PCIe, compute) instead of their sum.
 int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, const sr_recog_out *o) {
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
-    SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
+    SR_REQUIRE(h, capture_args_ok(U, B, n_len));
     if (B == 0) return 0;
     HostCall c(h, "sr_recognise_batch");
     // chunk: ~32 MB of PCM, a multiple of 8 utterances (keeps every chunk base 16-byte aligned)
     uint32_t chunk = (uint32_t)(((size_t)32 << 20) / ((size_t)U * 2));
     chunk = chunk < 8 ? 8 : (chunk & ~7u);
     if (chunk > B) chunk = B;
-    const uint32_t nchunks = (B + chunk - 1) / chunk;
-    const size_t chunk_bytes = (((size_t)chunk * U * 2 + 255) / 256) * 256;
-    c.ws(h->pcm, (nchunks > 1 ? 2 : 1) * chunk_bytes + 16);
+    const PcmGroups pg(c, U, B, chunk);
     sr_recog_out d;                                     // device mirrors of the non-NULL outputs
     memset(&d, 0, sizeof d);
     for_each_output(h, [&](auto m, DevBuf &buf, size_t bytes) {
@@ -655,24 +677,18 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
         d.*m = c.out(buf, o->*m, B * bytes);
     });
     uint32_t issued = 0;
-    // one chunk: H2D (plain u16, or 12-bit packed + expansion on the device) -> kernels on its slice of the outputs
+    // one chunk: H2D (plain u16, or 12-bit packed + expansion on the device) -> kernels on its slice of the outputs. The
+    // transport sends the issued-th chunk through buffer issued & 1.
     auto step = [&](uint32_t ci, int buf, const void *packed_src) -> int {
         const uint32_t b0 = ci * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
         const size_t ns = (size_t)nb * U;
-        u16 *dpcm = reinterpret_cast<u16 *>(static_cast<unsigned char *>(h->pcm.p) + (size_t)buf * chunk_bytes);
-        cudaStream_t cs = nchunks > 1 ? h->copy_stream : h->stream;
-        if (nchunks > 1 && issued >= 2) SR_CK(h, cudaStreamWaitEvent(cs, h->ev_done[buf], 0));      // buffers free again
-        if (packed_src) SR_CK(h, cudaMemcpyAsync(h->transport.device_stage(buf), packed_src, ns / 2 * 3, cudaMemcpyHostToDevice, cs));
-        else SR_CK(h, cudaMemcpyAsync(dpcm, pcm + (size_t)b0 * U, ns * 2, cudaMemcpyHostToDevice, cs));
-        if (nchunks > 1) {
-            SR_CK(h, cudaEventRecord(h->ev_h2d[buf], cs));
-            SR_CK(h, cudaStreamWaitEvent(h->stream, h->ev_h2d[buf], 0));
-        }
+        u16 *dpcm = pg.buf(buf);
+        if (packed_src) SR_CK(h, pg.send(issued, h->transport.device_stage(buf), packed_src, ns / 2 * 3));
+        else SR_CK(h, pg.send(issued, dpcm, pcm + (size_t)b0 * U, ns * 2));
         if (packed_src) SR_LAUNCH(h, TAG_NONE, launch_unpack12(h->transport.device_stage(buf), ns, dpcm, h->stream));
         const sr_recog_out dc = recog_slice(h, d, b0);
         if (const int rc = sr_recognise_batch_dev(h, dpcm, U, nb, n_len, &dc)) return rc;
-        if (nchunks > 1) SR_CK(h, cudaEventRecord(h->ev_done[buf], h->stream));
-        ++issued;
+        SR_CK(h, pg.done(issued++));
         return 0;
     };
     c.run([&] { return h->transport.send(h, pcm, U, B, chunk, step); });
@@ -687,16 +703,15 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
 int sr_enrol_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, void *bank_out,
                    uint32_t slot_stride, uint8_t *status) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && bank_out)));
-    SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0);
+    SR_REQUIRE(h, capture_args_ok(U, B, n_len) && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0);
     if (B == 0) return 0;
     HostCall c(h, "sr_enrol_batch");
     const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    atap_tag *d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
+    atap_tag *d_atap = c.atap(h->atap, nullptr, B, false);
     u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
     void *d_ftr = c.ws(h->ftr, (size_t)B * kFtrBytes);
     u8 *d_status = c.out(h->status, status, (size_t)B);
     void *d_bank = c.out(h->scratch[0], bank_out, (size_t)B * slot_stride);
-    c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
     c.run([&] { return front_end(h, d_pcm, U, B, n_len, d_atap, d_seg, d_ftr, d_status); });
     c.launch(TAG_NONE, "launch_pack_slots", [&] { return launch_pack_slots(d_ftr, d_status, B, d_bank, slot_stride, h->stream); });
     return c.finish();
@@ -817,29 +832,35 @@ int sr_average_bank(sr_handle *h, const void *bank, uint32_t slot_stride, uint32
 }  // extern "C"
 
 // ---- long features and connected words ----------------------------------------------------------------------------
-// frame count of a segment, MFCC.C:102-107 as mfcc_frames (sr_mfcc_core.cuh) counts it, without the vv_frm_max cap
-static u32 long_frames(u32 st, u32 en, u32 U, u32 frame_len) {
-    if (st == SR_SEG_NULL || en == SR_SEG_NULL || en > U || st > en) return 0;
-    const u32 len = en - st;
-    return len < frame_len ? 0u : (len - frame_len) / SR_FRAME_MOV + 1u;
-}
-
 // get_mfcc pieces of long segments: piece k of a segment of F frames is frames [119k, min(119(k+1), F)), a segment of
 // its own that starts at sample start + 80*119*k of the utterance's row (so x[-1] is pinned only for a piece at sample 0)
 struct LongPieces {
+    u32 frame_len;                        // the handle's geometry
+    u32 rows = 0;                         // long feature row of the next segment's first frame
     std::vector<u32> seg, row, dst;       // [P][2] start / end sample, [P] PCM row, [P][2] first long feature row / frames
     std::vector<atap_tag> atap;           // [P] the utterance's
-    void add(u32 st, u32 F, u32 frame_len, u32 r, const atap_tag &a, u32 row0) {
+    explicit LongPieces(const sr_handle *h) : frame_len(::frame_len(h)) {}
+    // segment [st, en) of PCM row r of U samples: its F frames (MFCC.C:102-107 as mfcc_frames in sr_mfcc_core.cuh counts
+    // them, without the vv_frm_max cap; 0 when it has none or more than cap) as pieces at rows, which advances by F
+    u32 add(u32 st, u32 en, u32 U, u32 r, const atap_tag &a, u32 cap = 0xFFFFFFFFu) {
+        const bool framed = st != SR_SEG_NULL && en != SR_SEG_NULL && en <= U && st <= en && en - st >= frame_len;
+        u32 F = framed ? (en - st - frame_len) / SR_FRAME_MOV + 1u : 0u;
+        if (F > cap) F = 0;
         for (u32 f0 = 0; f0 < F; f0 += SR_VV_FRM_MAX) {
             const u32 nf = std::min(F - f0, SR_VV_FRM_MAX), ps = st + f0 * SR_FRAME_MOV;
             seg.insert(seg.end(), {ps, ps + (nf - 1) * SR_FRAME_MOV + frame_len});
             row.push_back(r);
-            dst.insert(dst.end(), {row0 + f0, nf});
+            dst.insert(dst.end(), {rows + f0, nf});
             atap.push_back(a);
         }
+        rows += F;
+        return F;
     }
     u32 size() const { return (u32)row.size(); }
 };
+
+// spch_recg's early returns on a segment ending at en with F frames (main.c:261-274)
+static u8 seg_status(u32 en, u32 F) { return en == SR_SEG_NULL ? SR_ST_VAD_FAIL : F == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK; }
 
 constexpr u32 kPieceChunk = 8192;         // pieces per get_mfcc launch: 8192 x 2860 B of piece features
 
@@ -865,7 +886,13 @@ static void run_pieces(HostCall &c, const u16 *d_pcm, u32 U, u32 n_rows, const L
 
 // the device copies of a connected call's outputs, each NULL when the caller passes none: word records (in / out: records
 // past n_words keep the caller's bytes), word counts and totals
-struct ConnDev { sr_conn_word *words; u32 *nw; u64 *total; };
+struct ConnDev {
+    sr_conn_word *words; u32 *nw; u64 *total;
+    // the outputs of sequences b0, ...
+    ConnDev at(u32 b0, u32 max_words) const {
+        return {words ? words + (size_t)b0 * max_words : nullptr, nw ? nw + b0 : nullptr, total ? total + b0 : nullptr};
+    }
+};
 static ConnDev conn_outputs(HostCall &c, u32 B, u32 max_words, sr_conn_word *words, u32 *n_words, uint64_t *total) {
     sr_handle *h = c.h;
     ConnDev d{nullptr, nullptr, nullptr};
@@ -884,12 +911,7 @@ static ConnDev conn_outputs(HostCall &c, u32 B, u32 max_words, sr_conn_word *wor
 static void conn_vad(HostCall &c, const u16 *d_pcm, u32 U, u32 B, u32 n_len, const sr_conn_out *o, std::vector<u32> &seg,
                      std::vector<atap_tag> &atap) {
     sr_handle *h = c.h;
-    atap_tag *d_atap;
-    if (o->atap) d_atap = c.in(h->atap, o->atap, (size_t)B * sizeof(atap_tag));
-    else {
-        d_atap = c.ws<atap_tag>(h->atap, (size_t)B * sizeof(atap_tag));
-        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
-    }
+    atap_tag *d_atap = c.atap(h->atap, o->atap, B, false);
     u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
     c.launch(TAG_VAD, "launch_vad", [&] { return launch_vad(d_pcm, U, B, n_len, U, 1, 1, d_atap, d_seg, h->num_sms, h->stream, vad_work(h)); });
     seg.assign((size_t)B * 6, 0);
@@ -920,13 +942,11 @@ int sr_mfcc_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     SR_REQUIRE(h, h && (B == 0 || (pcm && seg && atap && feat && frm_num)));
     SR_REQUIRE(h, seg_stride >= 2 && frm_cap >= 1 && frm_cap <= SR_CONN_FRM_MAX && (uint64_t)B * frm_cap < (1ull << 32));
     if (B == 0) return 0;
-    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
     std::vector<u32> F(B);
-    LongPieces pc;
+    LongPieces pc(h);
     for (u32 b = 0; b < B; ++b) {
-        const u32 st = seg[(size_t)b * seg_stride], f = long_frames(st, seg[(size_t)b * seg_stride + 1], U, frame_len);
-        F[b] = f <= frm_cap ? f : 0u;
-        pc.add(st, F[b], frame_len, b, atap[b], b * frm_cap);
+        pc.rows = b * frm_cap;
+        F[b] = pc.add(seg[(size_t)b * seg_stride], seg[(size_t)b * seg_stride + 1], U, b, atap[b], frm_cap);
     }
     HostCall c(h, "sr_mfcc_long_batch");
     const size_t fbytes = (size_t)B * frm_cap * 24;
@@ -964,7 +984,7 @@ int sr_connected_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_nu
 int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, uint32_t penalty,
                                  uint32_t max_words, const sr_conn_out *o) {
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
-    SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
+    SR_REQUIRE(h, capture_args_ok(U, B, n_len));
     if (B == 0) return 0;
     SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
     HostCall c(h, "sr_recognise_connected_batch");
@@ -974,25 +994,21 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
     conn_vad(c, d_pcm, U, B, n_len, o, seg, atap);
     if (c.rc) return c.finish();
     // the plan: sequence q = the q-th closed segment with frames; rows and word records packed at seq_off[q][0] (frames)
-    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
     std::vector<u32> frm((size_t)B * 3), seq_of((size_t)B * 3, 0xFFFFFFFFu), seq_off, seq_frm;
     std::vector<u8> status(B);
-    LongPieces pc;
-    u32 rows = 0;
+    LongPieces pc(h);
     for (u32 b = 0; b < B; ++b) {
         for (u32 k = 0; k < 3; ++k) {
-            const u32 st = seg[b * 6 + 2 * k], F = long_frames(st, seg[b * 6 + 2 * k + 1], U, frame_len);   // <= 818: U <= 65535
+            const u32 r0 = pc.rows, F = pc.add(seg[b * 6 + 2 * k], seg[b * 6 + 2 * k + 1], U, b, atap[b]);   // <= 818: U <= 65535
             frm[b * 3 + k] = F;
             if (!F) continue;
             seq_of[b * 3 + k] = (u32)seq_frm.size();
-            seq_off.insert(seq_off.end(), {rows, rows});
+            seq_off.insert(seq_off.end(), {r0, r0});
             seq_frm.push_back(F);
-            pc.add(st, F, frame_len, b, atap[b], rows);
-            rows += F;
         }
-        status[b] = seg[b * 6 + 1] == SR_SEG_NULL ? SR_ST_VAD_FAIL : frm[b * 3] == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;   // main.c:261-274
+        status[b] = seg_status(seg[b * 6 + 1], frm[b * 3]);
     }
-    const u32 nseq = (u32)seq_frm.size();
+    const u32 nseq = (u32)seq_frm.size(), rows = pc.rows;
     s16 *d_feat = c.ws<s16>(h->conn[3], (size_t)rows * 24);
     run_pieces(c, d_pcm, U, B, pc, d_feat);
     u32 *tab = c.ws<u32>(h->conn[4], ((size_t)nseq * 3 + (size_t)B * 3) * 4);         // seq_off | seq_frm | seq_of
@@ -1051,7 +1067,30 @@ static int gram_copies(sr_handle *h, const sr_grammar *g, std::vector<u32> &copy
     return 0;
 }
 
-constexpr size_t kGramRecBytes = 256u << 20;   // records per launch: sum of N * n_states * 8 B over its sequences
+constexpr size_t kGramRecBytes = 256u << 20;   // records per launch of either grammar decoder
+
+// The launches of a grammar decoder over B sequences: consecutive ones whose records (frames(b) x row_bytes each) fit
+// kGramRecBytes, or one alone, at most kSeqChunk per launch. first_row(b) = b's first record row; rows_max: of one launch.
+struct RecordCuts {
+    std::vector<u32> cut{0};                            // launch boundaries
+    size_t rows_max = 0;
+    template <class N, class R> RecordCuts(u32 B, size_t row_bytes, N frames, R first_row) {
+        size_t rows = 0;
+        for (u32 b = 0; b < B; ++b) {
+            const size_t n = frames(b);
+            if (rows && (rows + n) * row_bytes > kGramRecBytes) { cut.push_back(b); rows = 0; }
+            first_row(b) = (u32)rows;
+            rows += n;
+            rows_max = std::max(rows_max, rows);
+        }
+        cut.push_back(B);
+    }
+    // launch(b0, q0, nq): sequences [b0 + q0, b0 + q0 + nq), the cut's records from row 0
+    template <class F> void launches(F launch) const {
+        for (size_t k = 0; k + 1 < cut.size(); ++k)
+            for (u32 q0 = 0, nb = cut[k + 1] - cut[k]; q0 < nb; q0 += kSeqChunk) launch(cut[k], q0, std::min(nb - q0, kSeqChunk));
+    }
+};
 
 // the copy table of both grammar decoders staged in gram[5]; a grammar without copies stages one word (C = 0: no warp
 // walks, every sequence decodes to 0 words)
@@ -1061,35 +1100,24 @@ static u32 *stage_copies(HostCall &c, const std::vector<u32> &copy) {
 }
 
 // the grammar decoder (tag 10) over B sequences of frames N[b]: seq [B][3] holds each first feature row and its segments
-// (the record rows are filled in here). Launches take consecutive sequences whose records fit kGramRecBytes.
+// (the record rows are filled in here), records cut by RecordCuts.
 static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &N, std::vector<u32> &seq,
                         const std::vector<u32> &copy, const sr_grammar *g, u32 penalty, u32 max_words, const ConnDev &d) {
     sr_handle *h = c.h;
     const u32 B = (u32)N.size(), S = g->n_states;
-    std::vector<u32> cut{0};                             // launch boundaries
-    size_t rows = 0, rows_max = 0;
-    for (u32 b = 0; b < B; ++b) {
-        if (rows && (rows + N[b]) * S * 8 > kGramRecBytes) { cut.push_back(b); rows = 0; }
-        seq[3 * (size_t)b + 1] = (u32)rows;
-        rows += N[b];
-        rows_max = std::max(rows_max, rows);
-    }
-    cut.push_back(B);
+    const RecordCuts cuts(B, (size_t)S * 8, [&](u32 b) { return N[b]; }, [&](u32 b) -> u32 & { return seq[3 * (size_t)b + 1]; });
     u32 *d_copy = stage_copies(c, copy);
     u32 *d_seq = c.in(h->gram[0], seq.data(), (size_t)B * 12);
     u32 *d_frm = c.in(h->gram[1], N.data(), (size_t)B * 4);
-    u64 *d_rec = c.ws<u64>(h->gram[2], std::max<size_t>(rows_max, 1) * S * 8);
+    u64 *d_rec = c.ws<u64>(h->gram[2], std::max<size_t>(cuts.rows_max, 1) * S * 8);
     const BankView &bk = h->bank;
-    for (size_t k = 0; k + 1 < cut.size(); ++k) {
-        const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
-        for (u32 q0 = 0; q0 < nb; q0 += kSeqChunk)
-            c.launch(TAG_GRAM, "launch_dtw_grammar", [&] {
-                return launch_dtw_grammar(d_feat, d_frm + b0, d_seq + 3 * (size_t)b0, q0, std::min(nb - q0, kSeqChunk), bk.p,
-                                          bk.stride, d_copy, (u32)copy.size(), S, g->final_mask, penalty, max_words,
-                                          d.words ? d.words + (size_t)b0 * max_words : nullptr, d.nw ? d.nw + b0 : nullptr,
-                                          d.total ? d.total + b0 : nullptr, d_rec, h->stream);
-            });
-    }
+    cuts.launches([&](u32 b0, u32 q0, u32 nq) {
+        const ConnDev o = d.at(b0, max_words);
+        c.launch(TAG_GRAM, "launch_dtw_grammar", [&] {
+            return launch_dtw_grammar(d_feat, d_frm + b0, d_seq + 3 * (size_t)b0, q0, nq, bk.p, bk.stride, d_copy, (u32)copy.size(),
+                                      S, g->final_mask, penalty, max_words, o.words, o.nw, o.total, d_rec, h->stream);
+        });
+    });
 }
 
 extern "C" {
@@ -1122,7 +1150,7 @@ int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat, const uint32_t
 int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
                                          const sr_grammar *g, uint32_t penalty, uint32_t max_words, const sr_conn_out *o) {
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
-    SR_REQUIRE(h, (B == 0 || U > 0) && U <= 65535u && n_len <= U);
+    SR_REQUIRE(h, capture_args_ok(U, B, n_len));
     if (B == 0) return 0;
     DeviceGuard dg(h->device);
     std::vector<u32> copy;
@@ -1135,30 +1163,25 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
     if (c.rc) return c.finish();
     // the plan: capture b is sequence b, its segments with frames back to back from row seq[b][0]; segment k's first
     // frame in that sequence (1023: no frames) is field k of seq[b][2]
-    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN;
     std::vector<u32> frm((size_t)B * 3), N(B), seq((size_t)B * 3);
     std::vector<u8> status(B);
-    LongPieces pc;
-    u32 rows = 0;
+    LongPieces pc(h);
     for (u32 b = 0; b < B; ++b) {
-        seq[3 * (size_t)b] = rows;
+        seq[3 * (size_t)b] = pc.rows;
         u32 segs = 0;
         for (u32 k = 0; k < 3; ++k) {
-            const u32 st = seg[b * 6 + 2 * k], F = long_frames(st, seg[b * 6 + 2 * k + 1], U, frame_len);
+            const u32 F = pc.add(seg[b * 6 + 2 * k], seg[b * 6 + 2 * k + 1], U, b, atap[b]);
             frm[b * 3 + k] = F;
             segs |= (F ? N[b] : 1023u) << (10 * k);
-            if (!F) continue;
-            pc.add(st, F, frame_len, b, atap[b], rows);
-            rows += F;
             N[b] += F;
         }
         seq[3 * (size_t)b + 2] = segs;
         // VAD's segments are disjoint, so a capture of U <= 65 535 samples has at most 818 frames over its segments
         if (N[b] > SR_CONN_FRM_MAX) c.took(fail(h, "a capture's segments exceed SR_CONN_FRM_MAX frames", cudaSuccess));
-        status[b] = seg[b * 6 + 1] == SR_SEG_NULL ? SR_ST_VAD_FAIL : frm[b * 3] == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;   // main.c:261-274
+        status[b] = seg_status(seg[b * 6 + 1], frm[b * 3]);
     }
     if (c.rc) return c.finish();
-    s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(rows, 1) * 24);
+    s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(pc.rows, 1) * 24);
     run_pieces(c, d_pcm, U, B, pc, d_feat);
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
     if (d.words || d.nw || d.total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
@@ -1170,6 +1193,13 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
 // ---- long-form VAD and per-segment recognition (sr_long.h) ----------------------------------------------------------
 static bool long_args_ok(u32 U, u32 B, u32 n_len, u32 max_segs) {
     return U <= SR_LONG_U_MAX && n_len <= 65535u && (uint64_t)B * max_segs < (1ull << 32);
+}
+// the host-buffer calls' recordings also have samples, and their lengths (host memory) lie within U
+static bool long_host_args_ok(u32 U, u32 B, const u32 *lens, u32 n_len, u32 max_segs) {
+    if ((B && !U) || !long_args_ok(U, B, n_len, max_segs)) return false;
+    for (u32 b = 0; lens && b < B; ++b)
+        if (lens[b] > U) return false;
+    return true;
 }
 
 // the long-form noise_atap and VAD of B recordings at pcm (device): noise_atap and the block summaries (tag 11), the
@@ -1196,26 +1226,20 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
     SR_CK(h, ensure(h->lng[3], (size_t)M * 16));                       // seg2[M][2] | row[M] | slot[M]
     SR_CK(h, ensure(h->lng[4], (size_t)M * sizeof(atap_tag)));
     SR_CK(h, ensure(h->lng[5], (size_t)M));
-    const u32 C = rule_cols(h->match_flags, h->bank.n);               // the margin rule's per-command keys follow the M keys
-    SR_CK(h, ensure(h->lng[6], (size_t)M * (1 + C) * 8));
     SR_CK(h, ensure(h->lng[7], (size_t)M * kFtrBytes));
     u32 *first = static_cast<u32 *>(h->lng[2].p), *n_flat = first + B;
     u32 *seg2 = static_cast<u32 *>(h->lng[3].p), *row = seg2 + 2 * (size_t)M, *slot = row + M;
     atap_tag *atap_seg = static_cast<atap_tag *>(h->lng[4].p);
     u8 *status = static_cast<u8 *>(h->lng[5].p);
-    u64 *best = static_cast<u64 *>(h->lng[6].p);
     void *ftr = h->lng[7].p;
     SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 0));
     SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 1));
     SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, M, seg2, 2, atap_seg, ftr, row, B, n_flat));     // main.c:268
     SR_LAUNCH(h, TAG_STATUS, launch_long_status(seg2, ftr, n_flat, M, status, h->stream));          // main.c:261-274
-    u64 *keys = C ? best + M : best;
-    SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(keys, (u64)M * (C ? C : 1), h->stream));                  // main.c:276-278
-    if (h->bank.n) {                                                   // main.c:279-291, save_sign honoured (main.c:283)
-        const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags;
-        SR_LAUNCH(h, scan_tag(flags),
-                  launch_scan(h, h->bank, ftr, M, flags, h->match_r, nullptr, keys, status, n_flat));
-    }
+    // main.c:276-291, save_sign honoured (main.c:283); the margin rule's per-command keys in lng[6]
+    const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags, C = rule_cols(flags, h->bank.n);
+    u64 *keys;
+    if (const int rc = scan_to_keys(h, &h->lng[6], C, h->bank, ftr, M, flags, h->match_r, nullptr, status, keys, n_flat)) return rc;
     SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, keys, n_flat, M, rec, C, rule_q(h->match_flags),
                                                      h->stream));                                   // main.c:292-294
     return 0;
@@ -1224,28 +1248,15 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
 constexpr size_t kLongGroupBytes = (size_t)256 << 20;   // PCM per staged group of the host calls
 
 // The host-buffer long-form calls: whole recordings staged in groups of at most kLongGroupBytes of PCM (at least one
-// recording) through two device buffers -- the copy of group g+1 (copy stream) overlaps the kernels of group g -- and
-// run(device PCM, first recording, recordings) per group. A recording is never split.
+// recording) through PcmGroups, and run(device PCM, first recording, recordings) per group. A recording is never split.
 template <class F> static int long_groups(HostCall &c, const uint16_t *pcm, u32 U, u32 B, F run) {
-    sr_handle *h = c.h;
-    u32 G = (u32)(kLongGroupBytes / ((size_t)U * 2));
-    G = std::max(1u, std::min(G, B));
-    const u32 ng = (B + G - 1) / G;
-    const size_t gbytes = (((size_t)G * U * 2 + 255) / 256) * 256;
-    c.ws(h->pcm, (ng > 1 ? 2 : 1) * gbytes + 16);
-    for (u32 g = 0; g < ng && !c.rc; ++g) {
-        const u32 b0 = g * G, nb = std::min(G, B - b0);
-        const int buf = g & 1;
-        u16 *dpcm = reinterpret_cast<u16 *>(static_cast<unsigned char *>(h->pcm.p) + (size_t)buf * gbytes);
-        cudaStream_t cs = ng > 1 ? h->copy_stream : h->stream;
-        if (ng > 1 && g >= 2) c.ck("cudaStreamWaitEvent", cudaStreamWaitEvent(cs, h->ev_done[buf], 0));   // buffer free again
-        c.ck("cudaMemcpyAsync host->device", cudaMemcpyAsync(dpcm, pcm + (size_t)b0 * U, (size_t)nb * U * 2, cudaMemcpyHostToDevice, cs));
-        if (ng > 1) {
-            c.ck("cudaEventRecord", cudaEventRecord(h->ev_h2d[buf], cs));
-            c.ck("cudaStreamWaitEvent", cudaStreamWaitEvent(h->stream, h->ev_h2d[buf], 0));
-        }
+    const PcmGroups pg(c, U, B, std::max(1u, std::min((u32)(kLongGroupBytes / ((size_t)U * 2)), B)));
+    for (u32 g = 0; g < pg.n && !c.rc; ++g) {
+        const u32 b0 = g * pg.G, nb = std::min(pg.G, B - b0);
+        u16 *dpcm = pg.buf(g & 1);
+        c.ck("PcmGroups::send", pg.send(g, dpcm, pcm + (size_t)b0 * U, (size_t)nb * U * 2));
         c.run([&] { return run(static_cast<const u16 *>(dpcm), b0, nb); });
-        if (ng > 1) c.ck("cudaEventRecord", cudaEventRecord(h->ev_done[buf], h->stream));
+        c.ck("PcmGroups::done", pg.done(g));
     }
     return c.finish();
 }
@@ -1268,11 +1279,7 @@ int sr_recognise_long_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, u
     if (B == 0) return 0;
     DeviceGuard g(h->device);
     atap_tag *atap = o->atap;
-    if (!atap) {                                        // as sr_recognise_batch_dev: noise_atap on a zeroed record
-        SR_CK(h, ensure(h->lng[8], (size_t)B * sizeof(atap_tag)));
-        atap = static_cast<atap_tag *>(h->lng[8].p);
-        SR_CK(h, cudaMemsetAsync(atap, 0, (size_t)B * sizeof(atap_tag), h->stream));
-    }
+    SR_CK(h, atap_or_zeroed(h, h->lng[8], B, atap));
     u32 *n_segs = o->n_segs;
     if (!n_segs) { SR_CK(h, ensure(h->lng[9], (size_t)B * 4)); n_segs = static_cast<u32 *>(h->lng[9].p); }
     SR_CK(h, ensure(h->lng[1], (size_t)B * max_segs * 8 + 8));
@@ -1284,13 +1291,11 @@ int sr_recognise_long_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, u
 int sr_vad_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens, uint32_t n_len,
                       uint32_t max_segs, atap_tag *atap, uint32_t *n_segs, uint32_t *seg_off) {
     SR_REQUIRE(h, h && (B == 0 || (pcm && atap && n_segs && (seg_off || max_segs == 0))));
-    SR_REQUIRE(h, (B == 0 || U > 0) && long_args_ok(U, B, n_len, max_segs));
-    for (u32 b = 0; lens && b < B; ++b) SR_REQUIRE(h, lens[b] <= U);
+    SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
     if (B == 0) return 0;
     HostCall c(h, "sr_vad_long_batch");
     const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap = c.in(h->lng[8], atap, (size_t)B * sizeof(atap_tag));      // in / out: untouched when noise_atap skips
-    c.out(h->lng[8], atap, (size_t)B * sizeof(atap_tag));
+    atap_tag *d_atap = c.atap(h->lng[8], atap, B, true);
     u32 *d_n = c.out(h->lng[9], n_segs, (size_t)B * 4);
     const size_t sbytes = (size_t)B * max_segs * 8;
     u32 *d_seg = nullptr;
@@ -1307,16 +1312,11 @@ int sr_vad_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
 int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens, uint32_t n_len,
                             uint32_t max_segs, const sr_long_out *o) {
     SR_REQUIRE(h, h && o && (B == 0 || (pcm && (o->segs || max_segs == 0))));
-    SR_REQUIRE(h, (B == 0 || U > 0) && long_args_ok(U, B, n_len, max_segs));
-    for (u32 b = 0; lens && b < B; ++b) SR_REQUIRE(h, lens[b] <= U);
+    SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
     if (B == 0) return 0;
     HostCall c(h, "sr_recognise_long_batch");
     const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap = nullptr;
-    if (o->atap) {
-        d_atap = c.in(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
-        c.out(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
-    }
+    atap_tag *d_atap = c.atap(h->lng[8], o->atap, B, true);
     u32 *d_n = o->n_segs ? c.out(h->lng[9], o->n_segs, (size_t)B * 4) : nullptr;
     const size_t rbytes = (size_t)B * max_segs * sizeof(sr_long_seg);
     sr_long_seg *d_rec = nullptr;
@@ -1325,7 +1325,7 @@ int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint3
         c.out(h->lng[10], o->segs, rbytes);
     }
     return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
-        const sr_long_out od{d_atap ? d_atap + b0 : nullptr, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
+        const sr_long_out od{d_atap + b0, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
         return sr_recognise_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, &od);
     });
 }
@@ -1333,41 +1333,28 @@ int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint3
 }  // extern "C"
 
 // ---- one grammar decode per long recording (sr_long_grammar.h) --------------------------------------------------------
-constexpr size_t kLongGramRecBytes = 256u << 20;   // records per launch: sum of N * n_states * 12 B over its sequences
-
 // the long-recording grammar decoder (tag 13) over the sequences of seq [B][4] (first segment, segments, frames; the first
-// record row is filled in here) and the flat segment table at d_row / d_frm. Launches take consecutive sequences whose
-// records fit kLongGramRecBytes; a sequence whose records alone exceed it runs in a launch of its own, the record
-// workspace grown to fit it.
+// record row is filled in here) and the flat segment table at d_row / d_frm, records cut by RecordCuts: the record
+// workspaces grow to fit a sequence whose records alone exceed the budget.
 static void run_long_grammar(HostCall &c, const s16 *d_feat, std::vector<u32> &seq, const u32 *d_row, const u32 *d_frm,
                              const std::vector<u32> &copy, const sr_grammar *g, u32 penalty, u32 max_words, const ConnDev &d) {
     sr_handle *h = c.h;
     const u32 B = (u32)(seq.size() / 4), S = g->n_states;
-    std::vector<u32> cut{0};                             // launch boundaries
-    size_t rows = 0, rows_max = 0;
-    for (u32 b = 0; b < B; ++b) {
-        const size_t n = seq[4 * (size_t)b + 2];
-        if (rows && (rows + n) * S * 12 > kLongGramRecBytes) { cut.push_back(b); rows = 0; }
-        seq[4 * (size_t)b + 3] = (u32)rows;
-        rows += n;
-        rows_max = std::max(rows_max, rows);
-    }
-    cut.push_back(B);
+    const RecordCuts cuts(B, (size_t)S * 12, [&](u32 b) { return seq[4 * (size_t)b + 2]; },
+                        [&](u32 b) -> u32 & { return seq[4 * (size_t)b + 3]; });
     u32 *d_copy = stage_copies(c, copy);
     u32 *d_seq = c.in(h->gram[0], seq.data(), (size_t)B * 16);
-    u64 *recD = c.ws<u64>(h->gram[2], std::max<size_t>(rows_max, 1) * S * 8);
-    u32 *recS = c.ws<u32>(h->gram[3], std::max<size_t>(rows_max, 1) * S * 4);
+    u64 *recD = c.ws<u64>(h->gram[2], std::max<size_t>(cuts.rows_max, 1) * S * 8);
+    u32 *recS = c.ws<u32>(h->gram[3], std::max<size_t>(cuts.rows_max, 1) * S * 4);
     const BankView &bk = h->bank;
-    for (size_t k = 0; k + 1 < cut.size(); ++k) {
-        const u32 b0 = cut[k], nb = cut[k + 1] - cut[k];
-        for (u32 q0 = 0; q0 < nb; q0 += kSeqChunk)
-            c.launch(TAG_LONG_GRAM, "launch_dtw_long_grammar", [&] {
-                return launch_dtw_long_grammar(d_feat, d_seq + 4 * (size_t)b0, q0, std::min(nb - q0, kSeqChunk), d_row, d_frm, bk.p,
-                                               bk.stride, d_copy, (u32)copy.size(), S, g->final_mask, penalty, max_words,
-                                               d.words ? d.words + (size_t)b0 * max_words : nullptr, d.nw ? d.nw + b0 : nullptr,
-                                               d.total ? d.total + b0 : nullptr, recD, recS, h->stream);
-            });
-    }
+    cuts.launches([&](u32 b0, u32 q0, u32 nq) {
+        const ConnDev o = d.at(b0, max_words);
+        c.launch(TAG_LONG_GRAM, "launch_dtw_long_grammar", [&] {
+            return launch_dtw_long_grammar(d_feat, d_seq + 4 * (size_t)b0, q0, nq, d_row, d_frm, bk.p, bk.stride, d_copy,
+                                           (u32)copy.size(), S, g->final_mask, penalty, max_words, o.words, o.nw, o.total, recD,
+                                           recS, h->stream);
+        });
+    });
 }
 
 // the segment slots the end-to-end call gives the VAD per recording: a closed segment spans at least 8 + 11 = 19 VAD
@@ -1428,23 +1415,15 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
                                     uint32_t n_len, const sr_grammar *g, uint32_t penalty, uint32_t max_segs, uint32_t max_words,
                                     const sr_long_gram_out *o) {
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
-    SR_REQUIRE(h, (B == 0 || U > 0) && long_args_ok(U, B, n_len, max_segs));
-    for (u32 b = 0; lens && b < B; ++b) SR_REQUIRE(h, lens[b] <= U);
+    SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
     if (B == 0) return 0;
     DeviceGuard dg(h->device);
     std::vector<u32> copy;
     if (const int rc = gram_copies(h, g, copy)) return rc;
-    const u32 frame_len = h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN, cap = long_seg_bound(U);
+    const u32 cap = long_seg_bound(U);
     HostCall c(h, "sr_recognise_long_grammar_batch");
     const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap;
-    if (o->atap) {                                      // in / out: untouched when noise_atap skips
-        d_atap = c.in(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
-        c.out(h->lng[8], o->atap, (size_t)B * sizeof(atap_tag));
-    } else {
-        d_atap = c.ws<atap_tag>(h->lng[8], (size_t)B * sizeof(atap_tag));
-        c.ck("cudaMemsetAsync", d_atap ? cudaMemsetAsync(d_atap, 0, (size_t)B * sizeof(atap_tag), h->stream) : cudaSuccess);
-    }
+    atap_tag *d_atap = c.atap(h->lng[8], o->atap, B, true);
     u32 *d_n = c.ws<u32>(h->lng[9], (size_t)B * 4);
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
     struct SegRec { u32 b, k, st, en, F; u8 status; };    // the records of segments k < max_segs
@@ -1466,8 +1445,7 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
         // the plan: recording q is sequence q; its segments are consecutive entries of the flat table, a decodable one with
         // its frames (rows packed back to back in segment order), any other with 0 frames
         std::vector<u32> seq((size_t)nb * 4), row, frm;
-        LongPieces pc;
-        u32 rows = 0;
+        LongPieces pc(h);
         for (u32 q = 0; q < nb; ++q) {
             const u32 b = b0 + q, n = n_all[b];
             if (n > cap) return fail(h, "a recording has more segments than long_seg_bound", cudaSuccess);
@@ -1476,30 +1454,22 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
             u32 N = 0;
             for (u32 k = 0; k < n; ++k) {
                 const u32 st = segv[((size_t)q * cap + k) * 2], en = segv[((size_t)q * cap + k) * 2 + 1];
-                const u32 F = long_frames(st, en, U, frame_len);
-                const bool ok = F >= 1 && F <= SR_CONN_FRM_MAX;   // long_frames is 0 for an open segment
-                row.push_back(rows);
-                frm.push_back(ok ? F : 0u);
-                if (ok) {
-                    pc.add(st, F, frame_len, q, av[q], rows);
-                    rows += F;
-                    N += F;
-                }
-                if (k < max_segs)
-                    recs.push_back({b, k, st, en, ok ? F : 0u, (u8)(en == SR_SEG_NULL ? SR_ST_VAD_FAIL : ok ? SR_ST_OK : SR_ST_MFCC_FAIL)});
+                row.push_back(pc.rows);
+                const u32 F = pc.add(st, en, U, q, av[q], SR_CONN_FRM_MAX);   // 0 for an open segment
+                frm.push_back(F);
+                N += F;
+                if (k < max_segs) recs.push_back({b, k, st, en, F, seg_status(en, F)});
             }
             seq[4 * (size_t)q + 2] = N;
         }
         const u32 ns = (u32)row.size();
-        s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(rows, 1) * 24);
+        s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(pc.rows, 1) * 24);
         run_pieces(c, dpcm, U, nb, pc, d_feat);
         u32 *tab = c.ws<u32>(h->gram[1], std::max<size_t>(ns, 1) * 8);   // seg_row [ns] | seg_frm [ns]
         if (c.rc) return 0;
         c.h2d(tab, row.data(), (size_t)ns * 4);
         c.h2d(tab + ns, frm.data(), (size_t)ns * 4);
-        const ConnDev dq{d.words ? d.words + (size_t)b0 * max_words : nullptr, d.nw ? d.nw + b0 : nullptr,
-                         d.total ? d.total + b0 : nullptr};
-        run_long_grammar(c, d_feat, seq, tab, tab + ns, copy, g, penalty, max_words, dq);
+        run_long_grammar(c, d_feat, seq, tab, tab + ns, copy, g, penalty, max_words, d.at(b0, max_words));
         return 0;
     });
     if (rc) return rc;

@@ -246,6 +246,34 @@ inline int fail(sr_handle *h, const char *what, cudaError_t e) {
         if (!(cond)) return fail((h), "requirement failed: " #cond, cudaSuccess); \
     } while (0)
 
+// ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
+enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
+       TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
+       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13, TAG_DTW_SYM = 14 };
+
+// one kernel launch on the handle's stream, launch() returning its cudaError_t (for <<<a, b>>>: cudaGetLastError()):
+// bracketed by an event pair when tag is not TAG_NONE and timing is enabled, counted when it succeeds
+template <class F> inline int launch_on(sr_handle *h, int tag, const char *what, F launch) {
+    size_t slot = SIZE_MAX;
+    if (tag != TAG_NONE && h->timing && (h->ev_used + 1) * 2 <= h->ev.size()) {
+        slot = h->ev_used++;
+        h->ev_tag[slot] = tag;
+        cudaEventRecord(h->ev[2 * slot], h->stream);
+    }
+    const cudaError_t e = launch();
+    if (slot != SIZE_MAX) cudaEventRecord(h->ev[2 * slot + 1], h->stream);
+    if (e != cudaSuccess) return fail(h, what, e);
+    ++h->launches;
+    return 0;
+}
+#define SR_LAUNCH(h, tag, call)                                                                   \
+    do {                                                                                          \
+        if (const int rc__ = launch_on((h), (tag), #call, [&] { return (call); })) return rc__;   \
+    } while (0)
+
+// samples per frame in the handle's geometry
+inline u32 frame_len(const sr_handle *h) { return h->geom == SR_GEOM_B ? 200u : SR_FRAME_LEN; }
+
 inline cudaError_t ensure(DevBuf &b, size_t bytes) {
     if (bytes <= b.cap) return cudaSuccess;
     if (b.p) { cudaError_t e = cudaFree(b.p); b.p = nullptr; b.cap = 0; if (e != cudaSuccess) return e; }

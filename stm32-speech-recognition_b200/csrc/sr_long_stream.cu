@@ -203,13 +203,16 @@ static int long_streams_push_impl(sr_long_stream_pool *p, const uint16_t *chunk,
     const u16 *chunk_dev;
     u32 chunk_dev_stride;
     if (const int rc = stream_core_stage(*p, chunk, chunk_stride, max_len, lens != nullptr, &chunk_dev, &chunk_dev_stride)) return rc;
-    long_stream_step_kernel<<<(p->S + kLsWarps - 1) / kLsWarps, kLsWarps * 32, 0, h->stream>>>(
-        static_cast<u16 *>(p->pcm.p), p->R, SR_LONG_STREAM_MIRROR, p->row, p->S, chunk_dev, chunk_dev_stride,
-        max_len ? uniform_len : 0u, (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr, p->n_len,
-        static_cast<LongStreamState *>(p->state.p), static_cast<u32 *>(p->info.p), p->info_stride, p->W,
-        h->geom == 1 ? 200u : SR_FRAME_LEN, static_cast<StreamEventDev *>(p->ev.p), static_cast<u32 *>(p->seg_ev.p),
-        static_cast<atap_tag *>(p->atap_ev.p), static_cast<u32 *>(p->map_ev.p), static_cast<u32 *>(p->n_ev.p), p->cap);
-    SR_CK(h, cudaGetLastError());
+    if (const int rc = launch_on(h, TAG_NONE, "long_stream_step_kernel", [&] {
+            long_stream_step_kernel<<<(p->S + kLsWarps - 1) / kLsWarps, kLsWarps * 32, 0, h->stream>>>(
+                static_cast<u16 *>(p->pcm.p), p->R, SR_LONG_STREAM_MIRROR, p->row, p->S, chunk_dev, chunk_dev_stride,
+                max_len ? uniform_len : 0u, (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr, p->n_len,
+                static_cast<LongStreamState *>(p->state.p), static_cast<u32 *>(p->info.p), p->info_stride, p->W, frame_len(h),
+                static_cast<StreamEventDev *>(p->ev.p), static_cast<u32 *>(p->seg_ev.p), static_cast<atap_tag *>(p->atap_ev.p),
+                static_cast<u32 *>(p->map_ev.p), static_cast<u32 *>(p->n_ev.p), p->cap);
+            return cudaGetLastError();
+        }))
+        return rc;
     if (max_len)
         for (u32 s = 0; s < p->S; ++s) p->n_host[s] += lens ? lens[s] : uniform_len;
     return stream_core_recognise(*p, static_cast<const u16 *>(p->pcm.p), p->row, events, max_events, n_events);
@@ -231,11 +234,13 @@ int sr_long_streams_reset(sr_long_stream_pool *p, const uint8_t *which, const at
     DeviceGuard g(h->device);
     if (which) SR_CK(h, cudaMemcpyAsync(p->which.p, which, p->S, cudaMemcpyHostToDevice, h->stream));
     if (atap) SR_CK(h, cudaMemcpyAsync(p->atap0.p, atap, (size_t)p->S * sizeof(atap_tag), cudaMemcpyHostToDevice, h->stream));
-    long_stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<LongStreamState *>(p->state.p), p->S,
-                                                                       which ? static_cast<const u8 *>(p->which.p) : nullptr,
-                                                                       atap ? static_cast<const atap_tag *>(p->atap0.p) : nullptr);
-    SR_CK(h, cudaGetLastError());
-    ++h->launches;
+    if (const int rc = launch_on(h, TAG_NONE, "long_stream_reset_kernel", [&] {
+            long_stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(
+                static_cast<LongStreamState *>(p->state.p), p->S, which ? static_cast<const u8 *>(p->which.p) : nullptr,
+                atap ? static_cast<const atap_tag *>(p->atap0.p) : nullptr);
+            return cudaGetLastError();
+        }))
+        return rc;
     SR_CK(h, cudaStreamSynchronize(h->stream));    // the caller's arrays may go once this returns
     for (u32 s = 0; s < p->S; ++s)
         if (!which || which[s]) p->n_host[s] = 0;
@@ -306,10 +311,12 @@ int sr_long_streams_state(sr_long_stream_pool *p, uint32_t *n_recv, uint32_t *n_
     DeviceGuard g(h->device);
     u32 *q = static_cast<u32 *>(p->query.p);
     atap_tag *qa = reinterpret_cast<atap_tag *>(q + 3 * (size_t)p->S);
-    long_stream_query_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<const LongStreamState *>(p->state.p), p->S,
-                                                                       q, qa);
-    SR_CK(h, cudaGetLastError());
-    ++h->launches;
+    if (const int rc = launch_on(h, TAG_NONE, "long_stream_query_kernel", [&] {
+            long_stream_query_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<const LongStreamState *>(p->state.p),
+                                                                               p->S, q, qa);
+            return cudaGetLastError();
+        }))
+        return rc;
     if (n_recv) D2H(h, n_recv, q, (size_t)p->S * 4);
     if (n_closed) D2H(h, n_closed, q + p->S, (size_t)p->S * 4);
     if (open_start) D2H(h, open_start, q + 2 * (size_t)p->S, (size_t)p->S * 4);

@@ -274,27 +274,33 @@ int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_
     sr_handle *h = c.h;
     u32 *n_ev = static_cast<u32 *>(c.n_ev.p);
     // recognise the closed segments; every kernel reads the number of events from device memory (upper bound: cap)
-    SR_CK(h, launch_mfcc_h(h, pcm, row_len, c.cap, static_cast<const u32 *>(c.seg_ev.p), 2,
-                           static_cast<const atap_tag *>(c.atap_ev.p), c.ftr.p, static_cast<const u32 *>(c.map_ev.p), c.S, n_ev));
+    SR_LAUNCH(h, TAG_NONE, launch_mfcc_h(h, pcm, row_len, c.cap, static_cast<const u32 *>(c.seg_ev.p), 2,
+                                         static_cast<const atap_tag *>(c.atap_ev.p), c.ftr.p, static_cast<const u32 *>(c.map_ev.p),
+                                         c.S, n_ev));
     const u32 match = h->match_flags, C = rule_cols(match, h->bank.n);   // the handle's matcher, read at every push
     SR_CK(h, ensure(h->best, (size_t)c.cap * (C ? C : 1) * 8));
     u64 *best = static_cast<u64 *>(h->best.p);
     const u32 gb = (c.cap + 255) / 256;
-    (C ? stream_status_kernel<true> : stream_status_kernel<false>)<<<gb, 256, 0, h->stream>>>(
-        static_cast<const unsigned char *>(c.ftr.p), n_ev, c.cap, static_cast<u8 *>(c.status.p), static_cast<u32 *>(c.frm.p),
-        best, C);
-    SR_CK(h, cudaGetLastError());
+    if (const int rc = launch_on(h, TAG_NONE, "stream_status_kernel", [&] {
+            (C ? stream_status_kernel<true> : stream_status_kernel<false>)<<<gb, 256, 0, h->stream>>>(
+                static_cast<const unsigned char *>(c.ftr.p), n_ev, c.cap, static_cast<u8 *>(c.status.p),
+                static_cast<u32 *>(c.frm.p), best, C);
+            return cudaGetLastError();
+        }))
+        return rc;
     if (h->bank.n)
-        SR_CK(h, launch_scan(h, h->bank, c.ftr.p, c.cap, SR_DTW_CHECK_SIGN | match, h->match_r, nullptr, best,
-                             static_cast<const u8 *>(c.status.p), n_ev));
+        SR_LAUNCH(h, TAG_NONE, launch_scan(h, h->bank, c.ftr.p, c.cap, SR_DTW_CHECK_SIGN | match, h->match_r, nullptr, best,
+                                           static_cast<const u8 *>(c.status.p), n_ev));
     u32 *out_count = static_cast<u32 *>(c.out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(c.out.p) + 16);
     const u32 gf = C ? (u32)(((u64)c.cap * (u32)rule_group(C) + 255) / 256) : gb;
-    (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<gf, 256, 0, h->stream>>>(
-        static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap, static_cast<const u8 *>(c.status.p),
-        static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match));
-    SR_CK(h, cudaGetLastError());
-    h->launches += 4 + (h->bank.n ? 1 : 0);
+    if (const int rc = launch_on(h, TAG_NONE, "stream_finish_kernel", [&] {
+            (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<gf, 256, 0, h->stream>>>(
+                static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap, static_cast<const u8 *>(c.status.p),
+                static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match));
+            return cudaGetLastError();
+        }))
+        return rc;
     const u32 quick = c.cap < StreamCore::kQuick ? c.cap : StreamCore::kQuick;
     D2H(h, c.out_host.p, c.out.p, 16 + (size_t)quick * sizeof(sr_stream_event));
     SR_CK(h, cudaStreamSynchronize(h->stream));                       // the one synchronisation of a push
@@ -344,10 +350,12 @@ int sr_streams_reset(sr_stream_pool *p) {
     sr_handle *h = p->h;
     DeviceGuard g(h->device);
     p->pending.clear();
-    stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<StreamState *>(p->state.p), p->S);
-    SR_CK(h, cudaGetLastError());
+    if (const int rc = launch_on(h, TAG_NONE, "stream_reset_kernel", [&] {
+            stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<StreamState *>(p->state.p), p->S);
+            return cudaGetLastError();
+        }))
+        return rc;
     SR_CK(h, cudaMemsetAsync(p->pcm.p, 0, (size_t)p->S * p->L * 2, h->stream));
-    ++h->launches;
     return 0;
 }
 
@@ -397,10 +405,13 @@ int sr_streams_segments(sr_stream_pool *p, uint32_t *seg_off, atap_tag *atap) {
     DeviceGuard g(h->device);
     SR_CK(h, ensure(h->seg, (size_t)p->S * 24));
     SR_CK(h, ensure(h->atap, (size_t)p->S * sizeof(atap_tag)));
-    stream_segments_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<const StreamState *>(p->state.p), p->S,
-                                                                     static_cast<u32 *>(h->seg.p), static_cast<atap_tag *>(h->atap.p), nullptr);
-    SR_CK(h, cudaGetLastError());
-    ++h->launches;
+    if (const int rc = launch_on(h, TAG_NONE, "stream_segments_kernel", [&] {
+            stream_segments_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<const StreamState *>(p->state.p), p->S,
+                                                                             static_cast<u32 *>(h->seg.p),
+                                                                             static_cast<atap_tag *>(h->atap.p), nullptr);
+            return cudaGetLastError();
+        }))
+        return rc;
     if (seg_off) D2H(h, seg_off, h->seg.p, (size_t)p->S * 24);
     if (atap) D2H(h, atap, h->atap.p, (size_t)p->S * sizeof(atap_tag));
     SR_CK(h, cudaStreamSynchronize(h->stream));
@@ -422,12 +433,16 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     u32 chunk_dev_stride;
     if (const int rc = stream_core_stage(*p, chunk, chunk_stride, max_len, lens != nullptr, &chunk_dev, &chunk_dev_stride)) return rc;
     u32 *n_ev = static_cast<u32 *>(p->n_ev.p);
-    stream_step_kernel<<<(p->S + kStreamWarps - 1) / kStreamWarps, kStreamWarps * 32, 0, h->stream>>>(
-        static_cast<u16 *>(p->pcm.p), p->L, p->S, chunk_dev, chunk_dev_stride, max_len ? uniform_len : 0u,
-        (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr, p->n_len, static_cast<StreamState *>(p->state.p),
-        static_cast<u32 *>(p->info.p), p->info_stride, static_cast<StreamEventDev *>(p->ev.p), static_cast<u32 *>(p->seg_ev.p),
-        static_cast<atap_tag *>(p->atap_ev.p), static_cast<u32 *>(p->map_ev.p), n_ev, p->cap);
-    SR_CK(h, cudaGetLastError());
+    if (const int rc = launch_on(h, TAG_NONE, "stream_step_kernel", [&] {
+            stream_step_kernel<<<(p->S + kStreamWarps - 1) / kStreamWarps, kStreamWarps * 32, 0, h->stream>>>(
+                static_cast<u16 *>(p->pcm.p), p->L, p->S, chunk_dev, chunk_dev_stride, max_len ? uniform_len : 0u,
+                (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr, p->n_len, static_cast<StreamState *>(p->state.p),
+                static_cast<u32 *>(p->info.p), p->info_stride, static_cast<StreamEventDev *>(p->ev.p),
+                static_cast<u32 *>(p->seg_ev.p), static_cast<atap_tag *>(p->atap_ev.p), static_cast<u32 *>(p->map_ev.p), n_ev,
+                p->cap);
+            return cudaGetLastError();
+        }))
+        return rc;
     return stream_core_recognise(*p, static_cast<const u16 *>(p->pcm.p), p->L, events, max_events, n_events);
 }
 
