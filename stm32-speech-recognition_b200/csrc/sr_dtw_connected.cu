@@ -56,6 +56,11 @@ static_assert(kConnCand == SR_CONN_SLOT_MAX && kConnCand == SR_GRAM_COPY_MAX, "o
 static_assert(kConnFrm < kSegNone, "start frames and segment first frames are 10-bit fields");
 
 __device__ __forceinline__ u64 umin64(u64 a, u64 b) { return a < b ? a : b; }
+__device__ __forceinline__ u64 warp_min(u64 v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v = umin64(v, __shfl_xor_sync(0xFFFFFFFFu, v, o));
+    return v;
+}
 
 // The start of both kernels: the sequence's N rows as byte planes (stage_planes reads row r at src + 4 + 24 r: src is a
 // header-less row array shifted by 4), then member(M), which stages what
@@ -81,23 +86,32 @@ __device__ __forceinline__ u32 conn_prologue(cg::cluster_group &cl, unsigned cha
     return M;
 }
 
-// Frame i of a warp whose template has M frames (0: none): its column by one dp_column step, cell j = 0 entered from
-// `enter`, then its end cell as ekey = D << 17 | idx << 10 | start to candidate idx of every CTA of the cluster, and one
-// cluster barrier. Returns the frame's candidate buffer.
+// The column of input row a for a warp whose template has M >= 1 frames: one dp_column step on keys
+// D << 10 | (1023 - start) with +inf = kInf, cell j = 0 entered from `enter`. Returns the end cell's key (>= kInf:
+// unreached). The caller loads a: loaded in here, K6g's segment reset compiles to other code.
+template <u64 kInf>
+__device__ __forceinline__ u64 conn_column(const PRow &a, u32 M, u64 enter, const PRow (&b)[4], u64 (&D)[4]) {
+    const int lane = threadIdx.x & 31, j0 = lane * 4;
+    dp_column<u64, kInf>(D, lane, [&](int k, u64 up, u64 dg, u64 &d, u64 &A, bool &valid) {
+        const int j = j0 + k;
+        valid = j < (int)M;
+        d = (u64)pdist(a, b[k]) << 10;
+        A = umin64(up, j == 0 ? enter : dg);
+    }, [](int, u64, u64) {});
+    return dp_end(D, ((int)M - 1) & 3, ((int)M - 1) >> 2);
+}
+
+// Frame i of a warp whose template has M frames (0: none): its column by conn_column, then its end cell as
+// ekey = D << 17 | idx << 10 | start to candidate idx of every CTA of the cluster, and one cluster barrier. Returns the
+// frame's candidate buffer.
 __device__ __forceinline__ u64 *conn_frame(cg::cluster_group &cl, u32 nc, const unsigned char *smem, u64 *cand, u32 i, u32 M,
                                            u64 enter, const PRow (&b)[4], u64 (&D)[4], u32 idx) {
-    const int lane = threadIdx.x & 31, j0 = lane * 4;
+    const int lane = threadIdx.x & 31;
     u64 mine = kEkeyNone;
     if (M) {
         PRow a;
         load_row(a, smem, kSeqNrm, (int)i);                // broadcast read
-        dp_column<u64, kKeyInf>(D, lane, [&](int k, u64 up, u64 dg, u64 &d, u64 &A, bool &valid) {
-            const int j = j0 + k;
-            valid = j < (int)M;
-            d = (u64)pdist(a, b[k]) << 10;
-            A = umin64(up, j == 0 ? enter : dg);
-        }, [](int, u64, u64) {});
-        const u64 e = dp_end(D, ((int)M - 1) & 3, ((int)M - 1) >> 2);
+        const u64 e = conn_column<kKeyInf>(a, M, enter, b, D);
         if (e < kKeyInf) mine = ((e >> 10) << 17) | ((u64)idx << 10) | (u64)(1023u - (u32)(e & 1023u));
     }
     u64 *buf = cand + (i & 1) * kConnCand;
@@ -145,8 +159,7 @@ dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__
         const u64 *buf = conn_frame(cl, nc, smem_raw, cand, i, M, enter, b, D, t);
         u64 best = kEkeyNone;
         for (u32 q = lane; q < ncand; q += 32) best = umin64(best, buf[q]);
-#pragma unroll
-        for (int o = 16; o; o >>= 1) best = umin64(best, __shfl_xor_sync(0xFFFFFFFFu, best, o));
+        best = warp_min(best);
         if (rank == 0 && threadIdx.x == 0) rec[i] = best;
         enter = best == kEkeyNone ? kKeyInf : ((((best >> 17) + pen) << 10) | (u64)(1023u - (i + 1)));
     }
@@ -180,13 +193,86 @@ dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__
     if (total) total[s] = last >> 17;
 }
 
+// ---- the grammar decoders' shared steps (K6g below, K13 further down) ------------------------------------------------
+// Records are end keys D << kShift | copy << (kShift - 7) | ...: K6g's ekey (kShift = 17), K13's D << 7 | copy. They are
+// read from L2 (ld.global.cg): other CTAs of the cluster wrote them, and this SM's L1 may hold a line of them from an
+// earlier sequence.
+
+// A sequence of no frames: no words, total 0 if state 0 is final, else ~0. The whole cluster leaves: no barrier, no
+// remote store.
+__device__ __forceinline__ void gram_empty(u32 rank, u32 s, u32 final_mask, u32 *n_words, u64 *total) {
+    if (rank == 0 && threadIdx.x == 0) {
+        if (n_words) n_words[s] = 0;
+        if (total) total[s] = (final_mask & 1u) ? 0ull : ~0ull;
+    }
+}
+
+// A sequence no path accepts: no words, total ~0.
+__device__ __forceinline__ void gram_no_path(u32 s, u32 *n_words, u64 *total) {
+    if (n_words) n_words[s] = 0;
+    if (total) total[s] = ~0ull;
+}
+
+// Copy c's member from copy[c] = slot | state << 8 | src << 16: fills the state table cst of the ncand candidates, sets
+// src and M (0: no copy or no member) and returns the template's slot.
+__device__ __forceinline__ const unsigned char *copy_member(unsigned char *cst, const u32 *copy, u32 C, u32 ncand, u32 c,
+                                                            const unsigned char *bank, u32 slot_stride, u32 &src, u32 &M) {
+    for (u32 q = threadIdx.x; q < ncand; q += blockDim.x) cst[q] = q < C ? (unsigned char)((copy[q] >> 8) & 15u) : 0;
+    const unsigned char *slot = bank;
+    if (c < C) {
+        const u32 cw = copy[c];
+        src = cw >> 16;
+        slot = bank + (size_t)(cw & 255u) * slot_stride;
+        M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);   // the host only makes copies of members
+        if (M == kNoWalk) M = 0;
+    }
+    return slot;
+}
+
+// The entry term: the min over the candidates of the copies whose state is in src.
+__device__ __forceinline__ u64 src_min(const u64 *buf, const unsigned char *cst, u32 ncand, u32 src, int lane) {
+    u64 best = kEkeyNone;
+    for (u32 q = lane; q < ncand; q += 32)
+        if ((src >> cst[q]) & 1u) best = umin64(best, buf[q]);
+    return warp_min(best);
+}
+
+// The per-state records: global warp gw reduces E_st over the candidates for the states st = gw (mod ncand), and its
+// lane 0 hands each to store(st, E_st).
+template <class Store>
+__device__ __forceinline__ void state_records(const u64 *buf, const unsigned char *cst, u32 ncand, u32 S, u32 gw, int lane,
+                                              Store store) {
+    for (u32 st = gw; st < S; st += ncand) {
+        u64 r = kEkeyNone;
+        for (u32 q = lane; q < ncand; q += 32)
+            if (cst[q] == st) r = umin64(r, buf[q]);
+        r = warp_min(r);
+        if (lane == 0) store(st, r);
+    }
+}
+
 // argmin over the states of mask of E_s(f) (D only, ties to the lowest state); the records of frame f are at r
-__device__ __forceinline__ u32 gram_src(const u64 *r, u32 mask) {
+template <int kShift>
+__device__ __forceinline__ u32 state_argmin(const u64 *r, u32 mask) {
     u32 best = 0;
     u64 bd = ~0ull;
     for (u32 s = 0; mask; ++s, mask >>= 1)
-        if ((mask & 1u) && (__ldcg(r + s) >> 17) < bd) { bd = __ldcg(r + s) >> 17; best = s; }
+        if ((mask & 1u) && (__ldcg(r + s) >> kShift) < bd) { bd = __ldcg(r + s) >> kShift; best = s; }
     return best;
+}
+
+// The final state: the smallest E_s(N-1) over the final states, ties to the lowest state; S if none is reached. Its D
+// goes to fd.
+template <int kShift>
+__device__ __forceinline__ u32 final_state(const u64 *R, u32 S, u32 N, u32 final_mask, u64 &fd) {
+    u32 fs = S;
+    u64 d = ~0ull;
+    for (u32 st = 0; st < S; ++st) {
+        const u64 r = __ldcg(R + (size_t)(N - 1) * S + st);
+        if (((final_mask >> st) & 1u) && r != kEkeyNone && (r >> kShift) < d) { d = r >> kShift; fs = st; }
+    }
+    fd = d;
+    return fs;
 }
 
 __global__ void __launch_bounds__(kConnWarps * 32, 2)
@@ -203,13 +289,7 @@ dtw_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ frm_num
     u64 *cand = reinterpret_cast<u64 *>(smem_raw + kSeqBytes + kConnWarps * kSlotBytes);   // [2][kConnCand]
     unsigned char *cst = reinterpret_cast<unsigned char *>(cand + 2 * kConnCand);          // [kConnCand] state of each copy
     const u32 N = frm_num[s];
-    if (N == 0) {                                          // the whole cluster leaves: no barrier, no remote store
-        if (rank == 0 && threadIdx.x == 0) {
-            if (n_words) n_words[s] = 0;
-            if (total) total[s] = (final_mask & 1u) ? 0ull : ~0ull;
-        }
-        return;
-    }
+    if (N == 0) return gram_empty(rank, s, final_mask, n_words, total);
     const u32 row0 = seq[3 * s], rec0 = seq[3 * s + 1], segs = seq[3 * s + 2];
     const u32 f0 = segs & 1023u, f1 = (segs >> 10) & 1023u, f2 = segs >> 20;
     const u32 ncand = nc * kConnWarps;
@@ -217,18 +297,8 @@ dtw_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ frm_num
     u32 src = 0;
     PRow b[4];
     u64 D[4];
-    const u32 M = conn_prologue(cl, smem_raw, reinterpret_cast<const unsigned char *>(feat + (size_t)row0 * 12) - 4, N, b, D, [&](u32 &M) {
-        for (u32 q = threadIdx.x; q < ncand; q += blockDim.x) cst[q] = q < C ? (unsigned char)((copy[q] >> 8) & 15u) : 0;
-        const unsigned char *slot = bank;
-        if (c < C) {
-            const u32 cw = copy[c];
-            src = cw >> 16;
-            slot = bank + (size_t)(cw & 255u) * slot_stride;
-            M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);   // the host only makes copies of members
-            if (M == kNoWalk) M = 0;
-        }
-        return slot;
-    });
+    const u32 M = conn_prologue(cl, smem_raw, reinterpret_cast<const unsigned char *>(feat + (size_t)row0 * 12) - 4, N, b, D,
+                                [&](u32 &M) { return copy_member(cst, copy, C, ncand, c, bank, slot_stride, src, M); });
     const u64 pen = penalty;
     u64 enter = (src & 1u) ? ((pen << 10) | 1023u) : kKeyInf;   // E_0(-1) + penalty: a word starting at frame 0 from state 0
     const u32 gw = rank * kConnWarps + warp;
@@ -239,44 +309,23 @@ dtw_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ frm_num
             for (int k = 0; k < 4; ++k) D[k] = kKeyInf;
         }
         const u64 *buf = conn_frame(cl, nc, smem_raw, cand, i, M, enter, b, D, c);
-        u64 best = kEkeyNone;                              // min over the copies of the states in src: the entry term
-        for (u32 q = lane; q < ncand; q += 32)
-            if ((src >> cst[q]) & 1u) best = umin64(best, buf[q]);
-#pragma unroll
-        for (int o = 16; o; o >>= 1) best = umin64(best, __shfl_xor_sync(0xFFFFFFFFu, best, o));
+        const u64 best = src_min(buf, cst, ncand, src, lane);
         enter = best == kEkeyNone ? kKeyInf : ((((best >> 17) + pen) << 10) | (u64)(1023u - (i + 1)));
-        for (u32 st = gw; st < S; st += ncand) {           // the records E_st(i) this warp owns
-            u64 r = kEkeyNone;
-            for (u32 q = lane; q < ncand; q += 32)
-                if (cst[q] == st) r = umin64(r, buf[q]);
-#pragma unroll
-            for (int o = 16; o; o >>= 1) r = umin64(r, __shfl_xor_sync(0xFFFFFFFFu, r, o));
-            if (lane == 0) R[(size_t)i * S + st] = r;
-        }
+        state_records(buf, cst, ncand, S, gw, lane, [&](u32 st, u64 r) { R[(size_t)i * S + st] = r; });
     }
     __threadfence();
     cl.sync();                                             // every CTA's records are written
     if (rank != 0 || threadIdx.x != 0) return;
-    // records are read from L2 (ld.global.cg): other CTAs of the cluster wrote them, and this SM's L1 may hold a line of
-    // them from an earlier sequence. The final state: the smallest E_s(N-1) over final states, ties to the lowest state
-    u32 fs = S;
-    u64 fd = ~0ull;
-    for (u32 st = 0; st < S; ++st) {
-        const u64 r = __ldcg(R + (size_t)(N - 1) * S + st);
-        if (((final_mask >> st) & 1u) && r != kEkeyNone && (r >> 17) < fd) { fd = r >> 17; fs = st; }
-    }
-    if (fs == S) {                                         // no accepting path
-        if (n_words) n_words[s] = 0;
-        if (total) total[s] = ~0ull;
-        return;
-    }
+    u64 fd;
+    const u32 fs = final_state<17>(R, S, N, final_mask, fd);
+    if (fs == S) return gram_no_path(s, n_words, total);
     // trace-back: the word ending at frame i in state st is [start, i + 1) of its copy, entered from the source state with
     // the smallest E(start - 1) (state 0 at start 0)
     u32 K = 0;
     for (int i = (int)N - 1, st = (int)fs; i >= 0;) {
         const u64 r = __ldcg(R + (size_t)i * S + st);
         const u32 b0 = (u32)(r & 1023u), cp = (u32)((r >> 10) & 127u);
-        if (b0) st = (int)gram_src(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
+        if (b0) st = (int)state_argmin<17>(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
         i = (int)b0 - 1;
         ++K;
     }
@@ -286,7 +335,7 @@ dtw_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ frm_num
         const u32 b0 = (u32)(r & 1023u), cp = (u32)((r >> 10) & 127u);
         u64 prev = 0;
         if (b0) {
-            st = (int)gram_src(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
+            st = (int)state_argmin<17>(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
             prev = __ldcg(R + (size_t)(b0 - 1) * S + st) >> 17;
         }
         --k;
@@ -345,6 +394,11 @@ conn_concat_kernel(const u32 *__restrict__ seq_of, const u32 *__restrict__ seq_o
     if (total) total[b] = tot;
 }
 
+// C copies, 1 .. SR_GRAM_STATE_MAX states and nb sequences: what one grammar decoder launch takes
+static bool gram_launch_ok(u32 C, u32 S, u32 nb) {
+    return C <= SR_GRAM_COPY_MAX && S != 0 && S <= SR_GRAM_STATE_MAX && nb <= kSeqChunk;
+}
+
 // nb sequences, one cluster of ceil(n / kConnWarps) CTAs (one warp per slot or copy, at least one CTA) per sequence;
 // clusters of more than 8 CTAs need the non-portable size
 template <class... P, class... A>
@@ -390,7 +444,7 @@ cudaError_t launch_dtw_grammar(const s16 *feat, const u32 *frm_num, const u32 *s
                                const u32 *copy, u32 C, u32 S, u32 final_mask, u32 penalty, u32 max_words, sr_conn_word *words,
                                u32 *n_words, u64 *total, u64 *rec, cudaStream_t st) {
     if (nb == 0) return cudaSuccess;
-    if (C > SR_GRAM_COPY_MAX || S == 0 || S > SR_GRAM_STATE_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
+    if (!gram_launch_ok(C, S, nb)) return cudaErrorInvalidValue;
     return launch_clusters(dtw_grammar_kernel, kGramSmem, nb, C, st, feat, frm_num + b0, seq + 3 * (size_t)b0,
                            static_cast<const unsigned char *>(bank), slot_stride, copy, C, S, final_mask, penalty, max_words,
                            words ? words + (size_t)b0 * max_words : nullptr, n_words ? n_words + b0 : nullptr,
@@ -417,23 +471,17 @@ constexpr int kLgSmem = kSeqBytes + kConnWarps * kSlotBytes + 2 * kConnCand * 8 
 constexpr u64 kLgInf = 1ull << 63;
 
 // Frame li of segment-relative frames (its segment's first frame is sequence frame f0) of a warp whose copy's template has
-// M frames: dp_column, cell j = 0 entered from `enter`, then the end cell as D << 7 | idx to candidate idx, and its word's
+// M frames: conn_column, then the end cell as D << 7 | idx to candidate idx, and its word's
 // sequence-relative start to start candidate idx, of every CTA of the cluster; one cluster barrier.
 __device__ __forceinline__ void lg_frame(cg::cluster_group &cl, u32 nc, const unsigned char *smem, u64 *cand, u32 *cstart,
                                          u32 li, u32 f0, u32 M, u64 enter, const PRow (&b)[4], u64 (&D)[4], u32 idx) {
-    const int lane = threadIdx.x & 31, j0 = lane * 4;
+    const int lane = threadIdx.x & 31;
     u64 mine = kEkeyNone;
     u32 mst = 0;
     if (M) {
         PRow a;
         load_row(a, smem, kSeqNrm, (int)li);               // broadcast read
-        dp_column<u64, kLgInf>(D, lane, [&](int k, u64 up, u64 dg, u64 &d, u64 &A, bool &valid) {
-            const int j = j0 + k;
-            valid = j < (int)M;
-            d = (u64)pdist(a, b[k]) << 10;
-            A = umin64(up, j == 0 ? enter : dg);
-        }, [](int, u64, u64) {});
-        const u64 e = dp_end(D, ((int)M - 1) & 3, ((int)M - 1) >> 2);
+        const u64 e = conn_column<kLgInf>(a, M, enter, b, D);
         if (e < kLgInf) {
             mine = ((e >> 10) << 7) | (u64)idx;
             mst = f0 + 1023u - (u32)(e & 1023u);
@@ -444,15 +492,6 @@ __device__ __forceinline__ void lg_frame(cg::cluster_group &cl, u32 nc, const un
         cl.map_shared_rank(cstart, (unsigned)lane)[idx] = mst;
     }
     cl.sync();
-}
-
-// argmin over the states of mask of E_s(f) (D only, ties to the lowest state); the records of frame f are at r
-__device__ __forceinline__ u32 lg_src(const u64 *r, u32 mask) {
-    u32 best = 0;
-    u64 bd = ~0ull;
-    for (u32 s = 0; mask; ++s, mask >>= 1)
-        if ((mask & 1u) && (__ldcg(r + s) >> 7) < bd) { bd = __ldcg(r + s) >> 7; best = s; }
-    return best;
 }
 
 __global__ void __launch_bounds__(kConnWarps * 32, 3)   // 80 registers: three CTAs per SM, as dtw_grammar_kernel
@@ -470,23 +509,18 @@ dtw_long_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ se
     u32 *cstart = reinterpret_cast<u32 *>(cand + 2 * kConnCand);                            // [2][kConnCand] their starts
     unsigned char *cst = reinterpret_cast<unsigned char *>(cstart + 2 * kConnCand);         // [kConnCand] state of each copy
     const u32 k0 = seq[4 * s], nk = seq[4 * s + 1], N = seq[4 * s + 2], rec0 = seq[4 * s + 3];
-    if (N == 0) {                                          // the whole cluster leaves: no barrier, no remote store
-        if (rank == 0 && threadIdx.x == 0) {
-            if (n_words) n_words[s] = 0;
-            if (total) total[s] = (final_mask & 1u) ? 0ull : ~0ull;
-        }
-        return;
-    }
+    if (N == 0) return gram_empty(rank, s, final_mask, n_words, total);
     const u32 ncand = nc * kConnWarps;
     const u32 c = rank * kConnWarps + warp;                // this warp's copy
     u32 src = 0, M = 0;
+    // copy_member's decode written out: through copy_member this kernel compiles to other SASS (77 registers), not timed
     const unsigned char *slot = bank;
     for (u32 q = threadIdx.x; q < ncand; q += blockDim.x) cst[q] = q < C ? (unsigned char)((copy[q] >> 8) & 15u) : 0;
     if (c < C) {
         const u32 cw = copy[c];
         src = cw >> 16;
         slot = bank + (size_t)(cw & 255u) * slot_stride;
-        M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);   // the host only makes copies of members
+        M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);
         if (M == kNoWalk) M = 0;
     }
     unsigned char *tslot = smem_raw + kSeqBytes + warp * kSlotBytes;
@@ -517,48 +551,27 @@ dtw_long_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ se
             u64 *buf = cand + (gi & 1) * kConnCand;
             u32 *sb = cstart + (gi & 1) * kConnCand;
             lg_frame(cl, nc, smem_raw, buf, sb, li, f0, M, enter, b, D, c);
-            u64 best = kEkeyNone;                          // min over the copies of the states in src: the entry term
-            for (u32 q = lane; q < ncand; q += 32)
-                if ((src >> cst[q]) & 1u) best = umin64(best, buf[q]);
-#pragma unroll
-            for (int o = 16; o; o >>= 1) best = umin64(best, __shfl_xor_sync(0xFFFFFFFFu, best, o));
+            const u64 best = src_min(buf, cst, ncand, src, lane);
             eb = best == kEkeyNone ? ~0ull : best >> 7;
-            for (u32 st = gw; st < S; st += ncand) {       // the records E_st(gi) this warp owns
-                u64 r = kEkeyNone;
-                for (u32 q = lane; q < ncand; q += 32)
-                    if (cst[q] == st) r = umin64(r, buf[q]);
-#pragma unroll
-                for (int o = 16; o; o >>= 1) r = umin64(r, __shfl_xor_sync(0xFFFFFFFFu, r, o));
-                if (lane == 0) {
-                    R[(size_t)gi * S + st] = r;
-                    RS[(size_t)gi * S + st] = r == kEkeyNone ? 0u : sb[r & 127u];
-                }
-            }
+            state_records(buf, cst, ncand, S, gw, lane, [&](u32 st, u64 r) {
+                R[(size_t)gi * S + st] = r;
+                RS[(size_t)gi * S + st] = r == kEkeyNone ? 0u : sb[r & 127u];   // and the start of its word
+            });
         }
     }
     __threadfence();
     cl.sync();                                             // every CTA's records are written
     if (rank != 0 || threadIdx.x != 0) return;
-    // records are read from L2 (ld.global.cg), as in dtw_grammar_kernel. The final state: the smallest E_s(N-1) over
-    // final states, ties to the lowest state
-    u32 fs = S;
-    u64 fd = ~0ull;
-    for (u32 st = 0; st < S; ++st) {
-        const u64 r = __ldcg(R + (size_t)(N - 1) * S + st);
-        if (((final_mask >> st) & 1u) && r != kEkeyNone && (r >> 7) < fd) { fd = r >> 7; fs = st; }
-    }
-    if (fs == S) {                                         // no accepting path
-        if (n_words) n_words[s] = 0;
-        if (total) total[s] = ~0ull;
-        return;
-    }
+    u64 fd;
+    const u32 fs = final_state<7>(R, S, N, final_mask, fd);
+    if (fs == S) return gram_no_path(s, n_words, total);
     // trace-back: the word ending at frame i in state st is [start, i + 1) of its copy, entered from the source state with
     // the smallest E(start - 1) (state 0 at start 0); frames map to (segment, frame within it) through the segment table
     u32 K = 0;
     for (long long i = (long long)N - 1, st = fs; i >= 0;) {
         const u64 r = __ldcg(R + (size_t)i * S + st);
         const u32 b0 = __ldcg(RS + (size_t)i * S + st);
-        if (b0) st = lg_src(R + (size_t)(b0 - 1) * S, copy[r & 127u] >> 16);
+        if (b0) st = state_argmin<7>(R + (size_t)(b0 - 1) * S, copy[r & 127u] >> 16);
         i = (long long)b0 - 1;
         ++K;
     }
@@ -569,7 +582,7 @@ dtw_long_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ se
         const u32 b0 = __ldcg(RS + (size_t)i * S + st), cp = (u32)(r & 127u);
         u64 prev = 0;
         if (b0) {
-            st = lg_src(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
+            st = state_argmin<7>(R + (size_t)(b0 - 1) * S, copy[cp] >> 16);
             prev = __ldcg(R + (size_t)(b0 - 1) * S + st) >> 7;
         }
         --k;
@@ -596,7 +609,7 @@ cudaError_t launch_dtw_long_grammar(const s16 *feat, const u32 *seq, u32 b0, u32
                                     u32 max_words, sr_conn_word *words, u32 *n_words, u64 *total, u64 *recD, u32 *recS,
                                     cudaStream_t st) {
     if (nb == 0) return cudaSuccess;
-    if (C > SR_GRAM_COPY_MAX || S == 0 || S > SR_GRAM_STATE_MAX || nb > kSeqChunk) return cudaErrorInvalidValue;
+    if (!gram_launch_ok(C, S, nb)) return cudaErrorInvalidValue;
     return launch_clusters(dtw_long_grammar_kernel, kLgSmem, nb, C, st, feat, seq + 4 * (size_t)b0, seg_row, seg_frm,
                            static_cast<const unsigned char *>(bank), slot_stride, copy, C, S, final_mask, penalty, max_words,
                            words ? words + (size_t)b0 * max_words : nullptr, n_words ? n_words + b0 : nullptr,
