@@ -243,16 +243,20 @@ def accepts(grammar, cmds):
     return any(F >> s & 1 for s in cur)
 
 
-# ---- the definition of the long-form VAD, transcribed: VAD.C:97-218 without max_vc_con, u32 length -------------------
-def py_vad_long(vc, n, atap):
-    """[(start, end)], end = NULL for a segment still open when the frames run out"""
-    mid, n_thl, z_thl, s_thl = int(atap["mid_val"]), int(atap["n_thl"]), int(atap["z_thl"]), int(atap["s_thl"])
-    a_thl, b_thl = (mid + n_thl) & 0xFFFFFFFF, (mid - n_thl) & 0xFFFFFFFF       # VAD.C:112-113
+# ---- the definition of the VAD, transcribed: VAD.C:97-218, u32 length ----------------------------------------------
+def vad_frames(vc, n, atap):
+    """the per-frame arithmetic of VAD.C:112-157 over the first n samples: (frm_sum, frm_zero, last_sig entering the
+    frame), one int64 array each with one entry per frame i = 80k < n - 160. last_sig is never reset (VAD.C:99), so the
+    frame enters with the class of the last out-of-band sample among samples <= 80k + 78: the previous frame scanned
+    them."""
+    mid, n_thl = int(atap["mid_val"]), int(atap["n_thl"])
+    a_thl, b_thl = (mid + n_thl) & 0xFFFFFFFF, (mid - n_thl) & 0xFFFFFFFF       # VAD.C:112-113 (u32)
     vc = [int(v) for v in vc[:n]]
-    last_sig, cur, front, back, segs = 0, 0, 0, 0, []
-    i = 0
+    sums, zeros, entry = [], [], []
+    last_sig, i = 0, 0
     while n > 160 and i < n - 160:                                               # VAD.C:121
-        frm_sum = sum(abs(vc[i + h] - mid) for h in range(160))                  # VAD.C:126-129
+        entry.append(last_sig)
+        sums.append(sum(abs(vc[i + h] - mid) for h in range(160)))               # VAD.C:126-129
         frm_zero = 0
         for h in range(159):                                                     # VAD.C:132-157
             if vc[i + h] >= a_thl:
@@ -264,7 +268,24 @@ def py_vad_long(vc, n, atap):
                 frm_zero += last_sig == 1
             elif w < b_thl:
                 frm_zero += last_sig == 2
-        if frm_sum > s_thl or frm_zero > z_thl:                                  # VAD.C:164-187
+        zeros.append(frm_zero)
+        i += 80
+    return np.array(sums, np.int64), np.array(zeros, np.int64), np.array(entry, np.int64)
+
+
+def vad_active(frames, atap):
+    """VAD.C:164: a frame is active when frm_sum > s_thl or frm_zero > z_thl"""
+    frm_sum, frm_zero = frames[0], frames[1]
+    return (frm_sum > int(atap["s_thl"])) | (frm_zero > int(atap["z_thl"]))
+
+
+def vad_fsm(active, cap=None):
+    """the endpoint FSM of VAD.C:164-216 over a frame-activity sequence: [(start, end)], end = NULL for a segment still
+    open when the frames run out; cap: the VAD returns once cap segments have closed (max_vc_con = 3, VAD.C:202-205)"""
+    cur, front, back, segs = 0, 0, 0, []
+    for k, a in enumerate(active):
+        i = 80 * k
+        if a:                                                                    # VAD.C:164-187
             if cur == 0:
                 cur, front = 1, 1
             elif cur == 1:
@@ -282,10 +303,30 @@ def py_vad_long(vc, n, atap):
                 if back >= 11:
                     cur, back = 0, 0
                     segs[-1][1] = i - 11 * 80 + 160
+                    if cap is not None and len(segs) == cap:
+                        break
             elif cur == 1:
                 front, cur = 0, 0
-        i += 80
     return [tuple(s) for s in segs]
+
+
+def py_vad(vc, n, atap, cap=None):
+    """VAD.C:97-218 on the first n samples: [(start, end)] (see vad_fsm)"""
+    return vad_fsm(vad_active(vad_frames(vc, n, atap), atap), cap)
+
+
+def seg_table(segs, cap=3):
+    """a [cap, 2] u32 table of segment offsets as VAD writes them (NULL where no segment opened or closed)"""
+    t = np.full((cap, 2), NULL, np.uint32)
+    for j, s in enumerate(segs[:cap]):
+        t[j] = s
+    return t
+
+
+def py_vad_long(vc, n, atap):
+    """the long-form VAD (VAD.C:97-218 without max_vc_con): [(start, end)], end = NULL for a segment still open when the
+    frames run out"""
+    return py_vad(vc, n, atap)
 
 
 # ---- the host's launch plan of the connected-word calls, restated ----------------------------------------------------
