@@ -200,6 +200,21 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
  * _dev_allgather (whose gathered keys stay the argmin keys), _multi, the fixed-capture stream pools and groups, the
  * long-recording calls and the live long streams. sr_dtw_batch* have no status to report: any flag bit >= 16 there fails
  * before any copy or launch and writes nothing. */
+#define SR_DTW_KNN(k)     ((uint32_t)(k) << 8)   /* K-nearest-neighbour decision rule, 1 <= k <= SR_FTR_PER_COMM (extension) */
+/* SR_DTW_KNN(k), 1 <= k <= SR_FTR_PER_COMM in bits 8-10 of sr_set_match's flags (0: no rule), decides by each command's
+ * k nearest templates (Rabiner, Levinson, Rosenberg & Wilpon, IEEE TASSP 27(4), 1979) instead of the one nearest slot of
+ * main.c:276-292. It applies to an utterance or segment whose status is SR_ST_OK. With s_t the score the call returns for
+ * bank slot t (save_sign honoured), command c owns the slots t < n_slot with t / SR_FTR_PER_COMM == c (the last one may
+ * own fewer), V_c is the set of its scores that are not SR_DIS_ERR, n_c = |V_c| and m = min(k, n_c): a command with fewer
+ * signed templates competes on those it has. Its score is e_c = floor((sum of the m smallest of V_c) / m), the sum in 64
+ * bits, and SR_DIS_ERR when n_c = 0. cmd is the command with the smallest e_c (the lowest on ties), best_idx its slot with
+ * the smallest score (the lowest on ties, so cmd == best_idx / SR_FTR_PER_COMM) and best_dis = e_cmd; when every e_c is
+ * SR_DIS_ERR they are 0, SR_DIS_ERR and 0, as without the rule. The scores, and every record whose status is not SR_ST_OK,
+ * are what the call writes without the rule, and the rule rejects nothing by itself. SR_DTW_KNN(1) is the call without
+ * the rule, bit for bit. With SR_DTW_REJECT(q) as well, the margin rule takes d1 = e_cmd and d2 = the smallest e_c over
+ * the other commands. _dev_allgather gathers best_dis << 32 | best_idx of this decision. The rule applies where the margin
+ * rule does; sr_dtw_batch* accept bits 4-15 and ignore them. A build without the rule refuses these flags in
+ * sr_set_match, which is how a caller detects it. */
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                  uint32_t *score /* [B][n_slot] or NULL */, uint32_t *best_idx /* [B] or NULL */,
                  uint32_t *best_dis /* [B] or NULL */);
@@ -209,8 +224,9 @@ int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, 
  * SR_DTW_ANY_RATE: the same DP without the 2:1 length guard; flags = SR_DTW_SYM_P1: the
  * symmetric P = 1 DP above at radius band_r >= 0. Recognition keeps honouring save_sign (SR_DTW_CHECK_SIGN, main.c:283)
  * under every matcher. Any other flag value (SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE alone among them) or a
- * negative band_r fails and leaves the setting unchanged. Each of these four may carry SR_DTW_REJECT(q), the margin rule
- * above. sr_get_match returns the flags as set, SR_DTW_ANY_RATE and the rule's bits included.
+ * negative band_r fails and leaves the setting unchanged. Each of these four may carry SR_DTW_KNN(k), the KNN rule, and
+ * SR_DTW_REJECT(q), the margin rule above, alone or together; a KNN field of 5-7 or any other bit in 4-15 fails and leaves
+ * the setting unchanged. sr_get_match returns the flags as set, SR_DTW_ANY_RATE and the rules' bits included.
  * sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers (with
  * and without SR_DTW_ANY_RATE differ, and so do different rules);
  * the ranks of an all-gather cannot be checked without a collective, so every rank must set the same one. Enrolment,

@@ -111,9 +111,10 @@ int sr_set_dtw_variant(sr_handle *h, int variant) {
 }
 
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
-    const uint32_t m = flags & 0xFFFFu;                       // the matcher; bits 16-31 are the margin rule SR_DTW_REJECT(q)
+    // the matcher; bits 8-10 are the KNN rule SR_DTW_KNN(k), bits 16-31 the margin rule SR_DTW_REJECT(q)
+    const uint32_t m = flags & 0xFFFFu & ~SR_DTW_KNN(7);
     SR_REQUIRE(h, h && (m == 0 || m == SR_DTW_BAND || m == (SR_DTW_BAND | SR_DTW_ANY_RATE) || m == SR_DTW_SYM_P1) &&
-                      band_r >= 0);
+                      rule_knn(flags) <= SR_FTR_PER_COMM && band_r >= 0);
     h->match_flags = flags;
     h->match_r = band_r;
     return 0;
@@ -437,8 +438,8 @@ int sr_mfcc_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
 
 }  // extern "C"
 
-// main.c:276-291 on n inputs (n_dev: n on the device): w's n argmin keys, then under the margin rule (C > 0) n * C
-// per-command keys, set to their start (tag 3), and the template scan into them (4, 6 or 14); no w: it writes scores only
+// main.c:276-291 on n inputs (n_dev: n on the device): w's n argmin keys, then under a decision rule (C > 0) n * C
+// keys (rule_cols), set to their start (tag 3), and the template scan into them (4, 6 or 14); no w: it writes scores only
 static int scan_to_keys(sr_handle *h, DevBuf *w, u32 C, const BankView &bank, const void *in, u32 n, u32 flags, int band_r,
                         u32 *score, const u8 *status, u64 *&keys, const u32 *n_dev = nullptr) {
     keys = nullptr;
@@ -461,17 +462,18 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
     SR_REQUIRE(h, scan_flags_ok(flags));
     if (B == 0) return 0;
-    // under the margin rule (C > 0) the status is an output of the decision too
+    // under a decision rule (C > 0) the status is an output of the decision too. Without a status (sr_dtw_batch*) the
+    // rule bits, and bits 4-15 that they accept and ignore, never reach a kernel
     const u32 C = status ? rule_cols(flags, bank.n) : 0;
-    if (!C) flags &= 0xFFFFu;
+    if (!C) flags &= kMatcherBits;
     const bool want_best = best_idx || best_dis || cmd || C;
     DevBuf &bb = h->best_sel ? h->best_alt : h->best;
     u64 *keys;
     if (const int rc = scan_to_keys(h, want_best ? &bb : nullptr, C, bank, in, B, flags, band_r, score, status, keys)) return rc;
     u64 *best = static_cast<u64 *>(bb.p);
     if (want_best && C)
-        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final_reject(best, keys, B, C, rule_q(flags), best_idx, best_dis, cmd,
-                                                              const_cast<u8 *>(status), h->stream));
+        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final_reject(best, keys, B, C, rule_q(flags), rule_knn(flags), best_idx, best_dis,
+                                                              cmd, const_cast<u8 *>(status), h->stream));
     else if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
     return 0;
 }
@@ -1236,12 +1238,12 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
     SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 1));
     SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, M, seg2, 2, atap_seg, ftr, row, B, n_flat));     // main.c:268
     SR_LAUNCH(h, TAG_STATUS, launch_long_status(seg2, ftr, n_flat, M, status, h->stream));          // main.c:261-274
-    // main.c:276-291, save_sign honoured (main.c:283); the margin rule's per-command keys in lng[6]
+    // main.c:276-291, save_sign honoured (main.c:283); a decision rule's key rows in lng[6]
     const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags, C = rule_cols(flags, h->bank.n);
     u64 *keys;
     if (const int rc = scan_to_keys(h, &h->lng[6], C, h->bank, ftr, M, flags, h->match_r, nullptr, status, keys, n_flat)) return rc;
     SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, keys, n_flat, M, rec, C, rule_q(h->match_flags),
-                                                     h->stream));                                   // main.c:292-294
+                                                     rule_knn(h->match_flags), h->stream));                                   // main.c:292-294
     return 0;
 }
 

@@ -117,16 +117,17 @@ __global__ void best_final_kernel(const u64 *best, u32 B, u32 *best_idx, u32 *be
     if (best_dis) best_dis[i] = dis;
     if (cmd) cmd[i] = idx / SR_FTR_PER_COMM;
 }
-// The same under the margin rule SR_DTW_REJECT(q), from the per-command keys [B][C] (key_of): g = rule_group(C) threads
-// per utterance take the row's two smallest keys, the first thread writes the argmin key to best[i] (what an all-gather
-// reads), the fields best_final_kernel writes, and SR_ST_REJECT over an SR_ST_OK status the rule turns down.
-__global__ void best_final_reject_kernel(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 *best_idx, u32 *best_dis,
-                                         u32 *cmd, u8 *status) {
-    const int g = rule_group(C);
+// The same under a decision rule, from the rows of C keys (key_of): g = rule_group(rule_cmds(C, knn)) threads per
+// utterance take the row's decision and runner-up (rule_row: the margin rule's per-command keys, or SR_DTW_KNN's
+// per-slot keys), the first thread writes the decision's key to best[i] (what an all-gather reads), the fields
+// best_final_kernel writes, and SR_ST_REJECT over an SR_ST_OK status the margin rule q turns down (q = 0: none).
+__global__ void best_final_reject_kernel(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx,
+                                         u32 *best_dis, u32 *cmd, u8 *status) {
+    const int g = rule_group(rule_cmds(C, knn));
     const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
     const int lane = (int)(threadIdx.x & (u32)(g - 1));
     if (i >= B) return;                                                         // whole warps: B * g threads
-    const Top2 k = top2_row(keys + (size_t)i * C, C, lane, g);
+    const Top2 k = rule_row(keys + (size_t)i * C, C, knn, lane, g);
     if (lane) return;
     best[i] = k.k1;
     u32 idx = (u32)(k.k1 & 0xFFFFFFFFull), dis = (u32)(k.k1 >> 32);
@@ -307,11 +308,12 @@ cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_d
     best_final_kernel<<<(B + 255) / 256, 256, 0, st>>>(best, B, best_idx, best_dis, cmd, status);
     return cudaGetLastError();
 }
-cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 *best_idx, u32 *best_dis, u32 *cmd,
-                                     u8 *status, cudaStream_t st) {
+cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
+                                     u32 *cmd, u8 *status, cudaStream_t st) {
     if (B == 0) return cudaSuccess;
-    const u64 threads = (u64)B * (u32)rule_group(C);
-    best_final_reject_kernel<<<(u32)((threads + 255) / 256), 256, 0, st>>>(best, keys, B, C, q, best_idx, best_dis, cmd, status);
+    const u64 threads = (u64)B * (u32)rule_group(rule_cmds(C, knn));
+    best_final_reject_kernel<<<(u32)((threads + 255) / 256), 256, 0, st>>>(best, keys, B, C, q, knn, best_idx, best_dis, cmd,
+                                                                             status);
     return cudaGetLastError();
 }
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st) {
@@ -383,7 +385,7 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
         const bool has_t = lane < Tt;
         const u32 t = !has_t ? 0u : perm ? tfrm[kTileT + lane] : t0 + (u32)lane;   // the original slot number
         if (has_t && score) score[(size_t)u * T + t] = my_result;
-        if (best && (flags >> 16)) {                       // margin rule: one key per command, each lane its own
+        if (best && key_rows(flags)) {                     // a decision rule: each lane its own key of the row
             if (has_t) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, flags, T, u, t)),
                                  (unsigned long long)(((u64)my_result << 32) | (u64)t));
         } else if (best) {

@@ -211,13 +211,18 @@ __device__ __forceinline__ K dp_end(const K (&D)[4], int kend, int lend) {
     return __shfl_sync(0xFFFFFFFFu, e, lend);
 }
 
-// The argmin key of a pair: (result, bank slot t), strict '<', first wins == lexicographic min. Without the margin rule
-// (flags >> 16 == 0) best has one key per utterance. Under SR_DTW_REJECT(q) the runner-up command depends on the winner,
-// so best is the per-(utterance, command) array [B][ceil(T / 4)] instead: the minimum over its row is the same argmin key,
-// and the second smallest entry of the row is the runner-up command's score.
+// The argmin key of a pair: (result, bank slot t), strict '<', first wins == lexicographic min. Without a decision rule
+// (no bits 8-10 or 16-31 in flags) best has one key per utterance. Under SR_DTW_REJECT(q) the runner-up command depends
+// on the winner, so best is the per-(utterance, command) array [B][ceil(T / 4)] instead: the minimum over its row is the
+// same argmin key, and the second smallest entry of the row is the runner-up command's score. Under SR_DTW_KNN(k) a
+// command's score needs all of its templates' scores, so best is the per-(utterance, slot) array [B][T], each key written
+// once.
 __device__ __forceinline__ u64 *key_of(u64 *best, u32 flags, u32 T, u32 u, u32 t) {
+    if (rule_knn(flags)) return best + (size_t)u * T + t;
     return (flags >> 16) ? best + (size_t)u * ((T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM) + t / SR_FTR_PER_COMM : best + u;
 }
+// a scan under a decision rule writes a row of keys per utterance (key_of)
+__device__ __forceinline__ bool key_rows(u32 flags) { return rule_knn(flags) || (flags >> 16); }
 // score[u][t] and the spch_recg argmin (main.c:276-291) as one 64-bit atomicMin of the pair's key
 __device__ __forceinline__ void emit_pair(u32 *score, u64 *best, u32 T, u32 u, u32 t, u32 result, u32 flags) {
     if (score) score[(size_t)u * T + t] = result;
@@ -234,9 +239,11 @@ __device__ __forceinline__ void top2_add(Top2 &a, u64 k) {
     if (k < a.k1) { a.k2 = a.k1; a.k1 = k; }
     else if (k < a.k2) a.k2 = k;
 }
-__device__ __forceinline__ Top2 top2_row(const u64 *row, u32 C, int lane, int g) {
+// the same over C keys key(c)
+template <class Key>
+__device__ __forceinline__ Top2 top2_fold(u32 C, int lane, int g, Key key) {
     Top2 a{~0ull, ~0ull};
-    for (u32 c = (u32)lane; c < C; c += (u32)g) top2_add(a, row[c]);
+    for (u32 c = (u32)lane; c < C; c += (u32)g) top2_add(a, key(c));
     if (g == 32) {
 #pragma unroll
         for (int o = 16; o; o >>= 1) {
@@ -248,12 +255,47 @@ __device__ __forceinline__ Top2 top2_row(const u64 *row, u32 C, int lane, int g)
     }
     return a;
 }
+__device__ __forceinline__ Top2 top2_row(const u64 *row, u32 C, int lane, int g) {
+    return top2_fold(C, lane, g, [row](u32 c) { return row[c]; });
+}
 // reject a decision of score d1 whose runner-up command scores d2 (SR_DIS_ERR: none): 1000 (d2 - d1) < q d1 in u64
 __device__ __forceinline__ bool margin_rejects(u32 d1, u32 d2, u32 q) {
     return d2 != SR_DIS_ERR && 1000ull * (u64)(d2 - d1) < (u64)q * (u64)d1;
 }
 // threads per utterance of the rule's finishers: one for banks of up to 32 commands, a warp for wider ones
 __host__ __device__ __forceinline__ int rule_group(u32 C) { return C > 32 ? 32 : 1; }
+// commands of a row of C keys: C per-command keys, or under SR_DTW_KNN (knn > 0) C per-slot keys
+__host__ __device__ __forceinline__ u32 rule_cmds(u32 C, u32 knn) { return knn ? (C + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM : C; }
+
+// ---- the KNN rule (SR_DTW_KNN) over one utterance's per-slot keys [T] -----------------------------------------------
+// Command c's key: its score e_c = floor(sum of the m = min(k, n_c) smallest of its n_c scores that are not SR_DIS_ERR
+// / m) (sum in u64), then its slot with the smallest score (the lowest on ties); SR_DIS_ERR << 32 | 0 when n_c = 0.
+// A mean of scores below SR_DIS_ERR stays below it, so the lexicographic minimum of the command keys is the decision.
+__device__ __forceinline__ u64 knn_key(const u64 *row, u32 T, u32 k, u32 c) {
+    u32 s[SR_FTR_PER_COMM];
+    u32 t_min = 0, s_min = SR_DIS_ERR;
+#pragma unroll
+    for (u32 j = 0; j < SR_FTR_PER_COMM; ++j) {
+        const u32 t = c * SR_FTR_PER_COMM + j;
+        s[j] = t < T ? (u32)(row[t] >> 32) : SR_DIS_ERR;
+        if (s[j] < s_min) { s_min = s[j]; t_min = t; }
+    }
+    // ascending (SR_DIS_ERR, the largest u32, last): a 4-input sorting network
+    auto cs = [&](int a, int b) { const u32 lo = min(s[a], s[b]), hi = max(s[a], s[b]); s[a] = lo; s[b] = hi; };
+    cs(0, 1); cs(2, 3); cs(0, 2); cs(1, 3); cs(1, 2);
+    u32 m = 0;
+    u64 sum = 0;
+#pragma unroll
+    for (u32 j = 0; j < SR_FTR_PER_COMM; ++j)
+        if (j < k && s[j] != SR_DIS_ERR) { sum += s[j]; ++m; }
+    return m ? ((sum / m) << 32) | t_min : (u64)SR_DIS_ERR << 32;
+}
+// The decision row of a rule: knn = 0, the margin rule's C per-command keys (top2_row); else the KNN rule's C = T
+// per-slot keys, folded per command. k1 is the decision's key (score << 32 | slot), k2 >> 32 the runner-up command's score.
+__device__ __forceinline__ Top2 rule_row(const u64 *row, u32 C, u32 knn, int lane, int g) {
+    if (!knn) return top2_row(row, C, lane, g);
+    return top2_fold(rule_cmds(C, knn), lane, g, [=](u32 c) { return knn_key(row, C, knn, c); });
+}
 
 // ---- launch geometry --------------------------------------------------------------------------------------------
 // CTA rows per tile column: one CTA per SM over all columns (never a second partial wave), no more than the batch needs

@@ -39,17 +39,26 @@ cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, 
 cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
                            u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st,
                            const u32 *B_dev = nullptr, const u32 *perm = nullptr);
-// n keys (B argmin keys, or the margin rule's B * C per-command keys) set to main.c:276-278's start
+// n keys (B argmin keys, or a decision rule's B * C keys) set to main.c:276-278's start
 cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st);
 cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status,
                               cudaStream_t st);
-// best_final under the margin rule: argmin keys into best[B], the fields and SR_ST_REJECT from the keys [B][C] (sr_dtw.cu)
-cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 *best_idx, u32 *best_dis, u32 *cmd,
-                                     u8 *status, cudaStream_t st);
-// The margin rule SR_DTW_REJECT(q) rides in bits 16-31 of the matcher flags. Under it the template scan writes one key per
-// (input, command): C = ceil(T / SR_FTR_PER_COMM) columns per input, 0 when there is no rule or no bank (no runner-up).
+// best_final under a decision rule (margin q, KNN knn): the decision's keys into best[B], the fields and SR_ST_REJECT
+// from the keys [B][C] (sr_dtw.cu)
+cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
+                                     u32 *cmd, u8 *status, cudaStream_t st);
+// The margin rule SR_DTW_REJECT(q) rides in bits 16-31 of the matcher flags, the KNN rule SR_DTW_KNN(k) in bits 8-10
+// (rule_knn). Under the margin rule alone the template scan writes one key per (input, command): C = ceil(T /
+// SR_FTR_PER_COMM) columns per input; under the KNN rule one key per (input, slot): C = T. C = 0 when there is no rule or
+// no bank.
 inline u32 rule_q(u32 flags) { return flags >> 16; }
-inline u32 rule_cols(u32 flags, u32 T) { return rule_q(flags) && T ? (T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM : 0; }
+inline u32 rule_cols(u32 flags, u32 T) {
+    if (!T) return 0;
+    if (rule_knn(flags)) return T;
+    return rule_q(flags) ? (T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM : 0;
+}
+// the matcher bits 0-3 of the flags: what sr_dtw_batch* pass on to a kernel
+constexpr u32 kMatcherBits = 0xFu;
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st);
 cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStream_t st);
 cudaError_t launch_dtw_limit(const u16 *x, const u16 *y, const u16 *I, const u16 *M, u32 n, u8 *out, cudaStream_t st);
@@ -100,7 +109,7 @@ cudaError_t launch_long_flatten(const u32 *n_segs, const u32 *seg_off, const ata
                                 u32 *n_flat, u32 *seg2, u32 *row, u32 *slot, atap_tag *atap_seg, cudaStream_t st, int step);
 cudaError_t launch_long_status(const u32 *seg2, const void *ftr, const u32 *n_flat, u32 M, u8 *status, cudaStream_t st);
 cudaError_t launch_long_scatter(const u32 *seg2, const u32 *slot, const void *ftr, const u8 *status, const u64 *best,
-                                const u32 *n_flat, u32 M, sr_long_seg *rec, u32 C, u32 q, cudaStream_t st);
+                                const u32 *n_flat, u32 M, sr_long_seg *rec, u32 C, u32 q, u32 knn, cudaStream_t st);
 class PackPool;
 }  // namespace srk
 
@@ -207,7 +216,7 @@ struct sr_handle {
     sr_comm *comm = nullptr;                           // the exchange step (sr_comm_create), optional
     int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cu), -1 default
     u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk, SR_DTW_BAND (| SR_DTW_ANY_RATE) or SR_DTW_SYM_P1,
-                                                       // | SR_DTW_REJECT(q)
+                                                       // | SR_DTW_KNN(k) | SR_DTW_REJECT(q)
     int match_r = 0;                                   // its band radius
     DevBuf mfcc_work;                                  // the same for mfcc_kernel (next utterance, CTAs finished)
     DevBuf vad_work;                                   // two words: dynamic utterance hand-out of vad_kernel (zeroed once, self re-arming)
@@ -345,9 +354,9 @@ inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *i
 }
 
 // the two handles' recognition calls score and decide alike: both greedy, or both the same DP (SR_DTW_ANY_RATE included)
-// at the same radius, under the same margin rule
+// at the same radius, under the same decision rules
 inline bool same_match(const sr_handle *a, const sr_handle *b) {
-    return a->match_flags == b->match_flags && ((a->match_flags & 0xFFFFu) == 0 || a->match_r == b->match_r);
+    return a->match_flags == b->match_flags && ((a->match_flags & kMatcherBits) == 0 || a->match_r == b->match_r);
 }
 
 int comm_wait_before_scan(sr_handle *h, const void *score);   // sr_comm.cu

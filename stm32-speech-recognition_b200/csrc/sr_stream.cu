@@ -162,7 +162,7 @@ __global__ void stream_segments_kernel(const StreamState *st, u32 S, u32 *seg_of
 }
 
 // status per event from the freshly computed features (MFCC fail = frm_num 0, main.c:269-274) + argmin initialiser:
-// best[cap] without the margin rule, its C per-command keys per event under it (kRule)
+// best[cap] without a decision rule, its C keys per event (rule_cols) under one (kRule)
 template <bool kRule>
 __global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, u32 cap, u8 *status, u32 *frm, u64 *best,
                                      u32 C) {
@@ -179,12 +179,12 @@ __global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, 
 }
 
 // final argmin (main.c:285-294) + one packed record per event for a single D2H copy: word 0 of `out` = event count.
-// Under the margin rule (kRule) rule_group(C) threads per event take the argmin and the runner-up from its C keys, and a
-// decision the rule turns down gets SR_ST_REJECT.
+// Under a decision rule (kRule) rule_group(rule_cmds(C, knn)) threads per event take the decision and the runner-up from
+// its C keys (rule_row), and a decision the margin rule q turns down gets SR_ST_REJECT.
 template <bool kRule>
 __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, u32 cap, const u8 *status, const u32 *frm,
-                                     const u64 *best, sr_stream_event *out_rec, u32 *out_count, u32 C, u32 q) {
-    const int g = kRule ? rule_group(C) : 1;
+                                     const u64 *best, sr_stream_event *out_rec, u32 *out_count, u32 C, u32 q, u32 knn) {
+    const int g = kRule ? rule_group(rule_cmds(C, knn)) : 1;
     const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
     const u32 ne = min(*n_ev, cap);
     if (i == 0) *out_count = ne;
@@ -192,7 +192,7 @@ __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, 
     u64 k;
     u8 st = status[i];
     if constexpr (kRule) {
-        const Top2 t2 = top2_row(best + (size_t)i * C, C, (int)(threadIdx.x & (u32)(g - 1)), g);
+        const Top2 t2 = rule_row(best + (size_t)i * C, C, knn, (int)(threadIdx.x & (u32)(g - 1)), g);
         if (threadIdx.x & (u32)(g - 1)) return;
         k = t2.k1;
         if (st == SR_ST_OK && margin_rejects((u32)(k >> 32), (u32)(t2.k2 >> 32), q)) st = SR_ST_REJECT;
@@ -293,11 +293,12 @@ int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_
                                            static_cast<const u8 *>(c.status.p), n_ev));
     u32 *out_count = static_cast<u32 *>(c.out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(c.out.p) + 16);
-    const u32 gf = C ? (u32)(((u64)c.cap * (u32)rule_group(C) + 255) / 256) : gb;
+    const u32 gf = C ? (u32)(((u64)c.cap * (u32)rule_group(rule_cmds(C, rule_knn(match))) + 255) / 256) : gb;
     if (const int rc = launch_on(h, TAG_NONE, "stream_finish_kernel", [&] {
             (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<gf, 256, 0, h->stream>>>(
                 static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap, static_cast<const u8 *>(c.status.p),
-                static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match));
+                static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match),
+                rule_knn(match));
             return cudaGetLastError();
         }))
         return rc;

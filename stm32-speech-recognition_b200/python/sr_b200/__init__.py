@@ -18,6 +18,7 @@ FTR_BYTES = 2860
 SEG_NULL = 0xFFFFFFFF
 DIS_ERR = 0xFFFFFFFF
 SAVE_MASK = 12345
+FTR_PER_COMM = 4               # SR_FTR_PER_COMM: bank slots per command
 DTW_CHECK_SIGN, DTW_BAND, DTW_SYM_P1, DTW_ANY_RATE = 1, 2, 4, 8
 ST_OK, ST_VAD_FAIL, ST_MFCC_FAIL, ST_REJECT = 0, 1, 2, 3
 
@@ -28,6 +29,15 @@ def dtw_reject(q):
     if not 0 <= q <= 0xFFFF:
         raise ValueError("margin %d per mille outside 0..65535" % q)
     return q << 16
+
+
+def dtw_knn(k):
+    """SR_DTW_KNN(k): decide by the mean of each command's k best template scores, 1 <= k <= 4 (0 = no rule), OR'ed
+    into set_match's flags"""
+    k = int(k)
+    if not 0 <= k <= FTR_PER_COMM:
+        raise ValueError("k = %d outside 0..%d" % (k, FTR_PER_COMM))
+    return k << 8
 
 PATH_MAX = 237                 # SR_PATH_MAX: the longest warping path, 2 * VV_FRM_MAX - 1 points
 
@@ -626,7 +636,10 @@ class Handle:
     def set_match(self, flags, band_r=0):
         """matcher of the recognition calls: 0 = the reference's greedy walk, DTW_BAND = the banded DP at radius band_r,
         DTW_BAND | DTW_ANY_RATE = the same DP without the 2:1 length guard, DTW_SYM_P1 = the symmetric slope-constrained (P = 1) DP at radius band_r;
-        any of them | dtw_reject(q) turns down (ST_REJECT) a decision whose runner-up command is less than q per mille worse"""
+        any of them | dtw_knn(k) decides by each command's score e_c, the floor of the mean of its min(k, n_c) smallest
+        scores other than DIS_ERR (n_c of them), with the winner's nearest slot as best_idx and e_cmd as best_dis;
+        any of them | dtw_reject(q) turns down (ST_REJECT) a decision whose runner-up command is less than q per mille worse
+        (under dtw_knn, by the commands' e_c)"""
         self._ck(lib().sr_set_match(self._h, int(flags), int(band_r)))
 
     def match(self):
