@@ -471,10 +471,9 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
     u64 *keys;
     if (const int rc = scan_to_keys(h, want_best ? &bb : nullptr, C, bank, in, B, flags, band_r, score, status, keys)) return rc;
     u64 *best = static_cast<u64 *>(bb.p);
-    if (want_best && C)
-        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final_reject(best, keys, B, C, rule_q(flags), rule_knn(flags), best_idx, best_dis,
-                                                              cmd, const_cast<u8 *>(status), h->stream));
-    else if (want_best) SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, B, best_idx, best_dis, cmd, status, h->stream));
+    if (want_best)
+        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, keys, B, C, rule_q(flags), rule_knn(flags), best_idx, best_dis, cmd,
+                                                       const_cast<u8 *>(status), h->stream));
     return 0;
 }
 

@@ -202,7 +202,7 @@ extern "C" {
 
 // spch_recg for this rank's shard + the exchange step: gathered_score[world*B][n_slot] (u32, rank-major = global
 // utterance order for equal shards) and/or gathered_best[world*B] = (best_dis << 32 | best_idx), the key of the
-// strict-'<' first-wins argmin (main.c:285-289), or under SR_DTW_KNN(k) of the KNN decision (best_final_reject_kernel
+// strict-'<' first-wins argmin (main.c:285-289), or under SR_DTW_KNN(k) of the KNN decision (best_final_kernel<true>
 // writes it to the key buffer's first B words). All pointers are device memory; out_dev->score must be non-NULL when
 // gathered_score is wanted. Asynchronous: sr_comm_wait + sr_sync (or stream order after sr_comm_wait) to consume.
 int sr_recognise_batch_dev_allgather(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,

@@ -105,37 +105,27 @@ dtw_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char 
 // best[] initialiser and finaliser (main.c:276-278 min_comm=0, min_dis=dis_max; main.c:292-294)
 __global__ void best_init_kernel(u64 *best, u32 B) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < B) best[i] = ((u64)SR_DIS_MAX << 32) | 0ull;
+    if (i < B) best[i] = kKeyStart;
 }
-__global__ void best_final_kernel(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status) {
-    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B) return;
-    u64 k = best[i];
-    u32 idx = (u32)(k & 0xFFFFFFFFull), dis = (u32)(k >> 32);
-    if (status && status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }            // main.c:261-274
-    if (best_idx) best_idx[i] = idx;
-    if (best_dis) best_dis[i] = dis;
-    if (cmd) cmd[i] = idx / SR_FTR_PER_COMM;
-}
-// The same under a decision rule, from the rows of C keys (key_of): g = rule_group(rule_cmds(C, knn)) threads per
-// utterance take the row's decision and runner-up (rule_row: the margin rule's per-command keys, or SR_DTW_KNN's
-// per-slot keys), the first thread writes the decision's key to best[i] (what an all-gather reads), the fields
-// best_final_kernel writes, and SR_ST_REJECT over an SR_ST_OK status the margin rule q turns down (q = 0: none).
-__global__ void best_final_reject_kernel(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx,
-                                         u32 *best_dis, u32 *cmd, u8 *status) {
-    const int g = rule_group(rule_cmds(C, knn));
-    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
-    const int lane = (int)(threadIdx.x & (u32)(g - 1));
+// The decision of each of B utterances (decide) into the fields NULL does not mark as unwanted (NULL status: every
+// utterance OK). Without a rule the keys are best's; under one (kRule) they are rows of C keys (key_of), and the decision's
+// key goes to best[i] (what an all-gather reads) and SR_ST_REJECT into status. The rule's arguments come last.
+template <bool kRule>
+__global__ void best_final_kernel(const u64 *keys, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, u8 *status, u64 *best,
+                                  u32 C, u32 q, u32 knn) {
+    const u32 g = kRule ? rule_lanes(C, knn) : 1u;
+    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / g;
     if (i >= B) return;                                                         // whole warps: B * g threads
-    const Top2 k = rule_row(keys + (size_t)i * C, C, knn, lane, g);
-    if (lane) return;
-    best[i] = k.k1;
-    u32 idx = (u32)(k.k1 & 0xFFFFFFFFull), dis = (u32)(k.k1 >> 32);
-    if (status && status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }            // main.c:261-274
-    else if (status && margin_rejects(dis, (u32)(k.k2 >> 32), q)) status[i] = SR_ST_REJECT;
-    if (best_idx) best_idx[i] = idx;
-    if (best_dis) best_dis[i] = dis;
-    if (cmd) cmd[i] = idx / SR_FTR_PER_COMM;
+    const u32 st = status ? status[i] : SR_ST_OK;
+    Decision d;
+    if (!decide<kRule>(keys, i, st, C, q, knn, g, d)) return;
+    if constexpr (kRule) {
+        best[i] = d.key;
+        if (d.status != st) status[i] = (u8)d.status;
+    }
+    if (best_idx) best_idx[i] = d.idx;
+    if (best_dis) best_dis[i] = d.dis;
+    if (cmd) cmd[i] = d.cmd;
 }
 
 // status of the recognise pipeline from VAD/MFCC results (main.c:261-274)
@@ -302,18 +292,11 @@ cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st) {
     best_init_kernel<<<(u32)((n + 255) / 256), 256, 0, st>>>(best, (u32)n);
     return cudaGetLastError();
 }
-cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status,
-                              cudaStream_t st) {
+cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
+                              u32 *cmd, u8 *status, cudaStream_t st) {
     if (B == 0) return cudaSuccess;
-    best_final_kernel<<<(B + 255) / 256, 256, 0, st>>>(best, B, best_idx, best_dis, cmd, status);
-    return cudaGetLastError();
-}
-cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
-                                     u32 *cmd, u8 *status, cudaStream_t st) {
-    if (B == 0) return cudaSuccess;
-    const u64 threads = (u64)B * (u32)rule_group(rule_cmds(C, knn));
-    best_final_reject_kernel<<<(u32)((threads + 255) / 256), 256, 0, st>>>(best, keys, B, C, q, knn, best_idx, best_dis, cmd,
-                                                                             status);
+    (C ? best_final_kernel<true> : best_final_kernel<false>)<<<rule_grid(B, C, knn), 256, 0, st>>>(
+        keys, B, best_idx, best_dis, cmd, status, best, C, q, knn);
     return cudaGetLastError();
 }
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st) {

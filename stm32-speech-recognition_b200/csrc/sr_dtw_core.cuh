@@ -216,7 +216,8 @@ __device__ __forceinline__ K dp_end(const K (&D)[4], int kend, int lend) {
 // on the winner, so best is the per-(utterance, command) array [B][ceil(T / 4)] instead: the minimum over its row is the
 // same argmin key, and the second smallest entry of the row is the runner-up command's score. Under SR_DTW_KNN(k) a
 // command's score needs all of its templates' scores, so best is the per-(utterance, slot) array [B][T], each key written
-// once.
+// once. Every key starts at (SR_DIS_MAX, slot 0) (main.c:276-278).
+constexpr u64 kKeyStart = (u64)SR_DIS_MAX << 32;
 __device__ __forceinline__ u64 *key_of(u64 *best, u32 flags, u32 T, u32 u, u32 t) {
     if (rule_knn(flags)) return best + (size_t)u * T + t;
     return (flags >> 16) ? best + (size_t)u * ((T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM) + t / SR_FTR_PER_COMM : best + u;
@@ -295,6 +296,35 @@ __device__ __forceinline__ u64 knn_key(const u64 *row, u32 T, u32 k, u32 c) {
 __device__ __forceinline__ Top2 rule_row(const u64 *row, u32 C, u32 knn, int lane, int g) {
     if (!knn) return top2_row(row, C, lane, g);
     return top2_fold(rule_cmds(C, knn), lane, g, [=](u32 c) { return knn_key(row, C, knn, c); });
+}
+
+// ---- one record's decision: the step of every finisher (main.c:261-294) -------------------------------------------
+// threads per record of a finisher: one without a rule (C = 0), else rule_group of the row's commands
+__host__ __device__ __forceinline__ u32 rule_lanes(u32 C, u32 knn) { return C ? (u32)rule_group(rule_cmds(C, knn)) : 1u; }
+// a finisher's grid of 256-thread CTAs over n records
+inline u32 rule_grid(u64 n, u32 C, u32 knn) { return (u32)((n * rule_lanes(C, knn) + 255) / 256); }
+// Record i's decision from its keys and the status st it comes in with. Without a rule (kRule false) its key is keys[i];
+// under one the g lanes of its group fold its row of C keys (rule_row), and only lane 0 gets the decision (the others
+// return false). An SR_ST_OK decision the margin rule q turns down gets SR_ST_REJECT, and a record whose st is not
+// SR_ST_OK reports idx 0 and SR_DIS_ERR.
+struct Decision { u64 key; u32 idx, dis, cmd, status; };
+template <bool kRule>
+__device__ __forceinline__ bool decide(const u64 *keys, u32 i, u32 st, u32 C, u32 q, u32 knn, u32 g, Decision &d) {
+    d.status = st;
+    if constexpr (kRule) {
+        const u32 lane = threadIdx.x & (g - 1);
+        const Top2 t2 = rule_row(keys + (size_t)i * C, C, knn, (int)lane, (int)g);
+        if (lane) return false;
+        d.key = t2.k1;
+        if (st == SR_ST_OK && margin_rejects((u32)(d.key >> 32), (u32)(t2.k2 >> 32), q)) d.status = SR_ST_REJECT;
+    } else {
+        d.key = keys[i];
+    }
+    d.idx = (u32)(d.key & 0xFFFFFFFFull);
+    d.dis = (u32)(d.key >> 32);
+    if (st != SR_ST_OK) { d.idx = 0; d.dis = SR_DIS_ERR; }
+    d.cmd = d.idx / SR_FTR_PER_COMM;
+    return true;
 }
 
 // ---- launch geometry --------------------------------------------------------------------------------------------

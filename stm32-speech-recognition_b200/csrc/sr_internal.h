@@ -41,22 +41,11 @@ cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u
                            const u32 *B_dev = nullptr, const u32 *perm = nullptr);
 // n keys (B argmin keys, or a decision rule's B * C keys) set to main.c:276-278's start
 cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st);
-cudaError_t launch_best_final(const u64 *best, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, const u8 *status,
-                              cudaStream_t st);
-// best_final under a decision rule (margin q, KNN knn): the decision's keys into best[B], the fields and SR_ST_REJECT
-// from the keys [B][C] (sr_dtw.cu)
-cudaError_t launch_best_final_reject(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
-                                     u32 *cmd, u8 *status, cudaStream_t st);
-// The margin rule SR_DTW_REJECT(q) rides in bits 16-31 of the matcher flags, the KNN rule SR_DTW_KNN(k) in bits 8-10
-// (rule_knn). Under the margin rule alone the template scan writes one key per (input, command): C = ceil(T /
-// SR_FTR_PER_COMM) columns per input; under the KNN rule one key per (input, slot): C = T. C = 0 when there is no rule or
-// no bank.
-inline u32 rule_q(u32 flags) { return flags >> 16; }
-inline u32 rule_cols(u32 flags, u32 T) {
-    if (!T) return 0;
-    if (rule_knn(flags)) return T;
-    return rule_q(flags) ? (T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM : 0;
-}
+// The decision of B inputs into the fields (sr_dtw.cu): without a rule (C = 0) from the argmin keys keys = best; under
+// the rule of margin q and KNN knn from the keys [B][C] (rule_cols), with the decision's keys into best[B] and
+// SR_ST_REJECT into status
+cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
+                              u32 *cmd, u8 *status, cudaStream_t st);
 // the matcher bits 0-3 of the flags: what sr_dtw_batch* pass on to a kernel
 constexpr u32 kMatcherBits = 0xFu;
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st);

@@ -172,38 +172,27 @@ __global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, 
     status[i] = f == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;
     frm[i] = f;
     if constexpr (kRule) {
-        for (u32 c = 0; c < C; ++c) best[(size_t)i * C + c] = ((u64)SR_DIS_MAX << 32) | 0ull;
+        for (u32 c = 0; c < C; ++c) best[(size_t)i * C + c] = kKeyStart;
     } else {
-        best[i] = ((u64)SR_DIS_MAX << 32) | 0ull;                    // main.c:276-278
+        best[i] = kKeyStart;
     }
 }
 
-// final argmin (main.c:285-294) + one packed record per event for a single D2H copy: word 0 of `out` = event count.
-// Under a decision rule (kRule) rule_group(rule_cmds(C, knn)) threads per event take the decision and the runner-up from
-// its C keys (rule_row), and a decision the margin rule q turns down gets SR_ST_REJECT.
+// each event's decision (decide, under a decision rule when kRule) + one packed record per event for a single D2H copy:
+// word 0 of `out` = event count
 template <bool kRule>
 __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, u32 cap, const u8 *status, const u32 *frm,
                                      const u64 *best, sr_stream_event *out_rec, u32 *out_count, u32 C, u32 q, u32 knn) {
-    const int g = kRule ? rule_group(rule_cmds(C, knn)) : 1;
-    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
+    const u32 g = kRule ? rule_lanes(C, knn) : 1u;
+    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / g;
     const u32 ne = min(*n_ev, cap);
     if (i == 0) *out_count = ne;
     if (i >= ne) return;
-    u64 k;
-    u8 st = status[i];
-    if constexpr (kRule) {
-        const Top2 t2 = rule_row(best + (size_t)i * C, C, knn, (int)(threadIdx.x & (u32)(g - 1)), g);
-        if (threadIdx.x & (u32)(g - 1)) return;
-        k = t2.k1;
-        if (st == SR_ST_OK && margin_rejects((u32)(k >> 32), (u32)(t2.k2 >> 32), q)) st = SR_ST_REJECT;
-    } else {
-        k = best[i];
-    }
-    u32 idx = (u32)(k & 0xFFFFFFFFull), dis = (u32)(k >> 32);
-    if (status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }
+    Decision d;
+    if (!decide<kRule>(best, i, status[i], C, q, knn, g, d)) return;
     sr_stream_event r;
     r.stream = ev[i].stream; r.segment = ev[i].segment; r.start = ev[i].start; r.end = ev[i].end;
-    r.status = st; r.frm_num = frm[i]; r.best_idx = idx; r.best_dis = dis; r.cmd = idx / SR_FTR_PER_COMM;
+    r.status = (u8)d.status; r.frm_num = frm[i]; r.best_idx = d.idx; r.best_dis = d.dis; r.cmd = d.cmd;
     out_rec[i] = r;
 }
 
@@ -293,9 +282,9 @@ int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_
                                            static_cast<const u8 *>(c.status.p), n_ev));
     u32 *out_count = static_cast<u32 *>(c.out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(c.out.p) + 16);
-    const u32 gf = C ? (u32)(((u64)c.cap * (u32)rule_group(rule_cmds(C, rule_knn(match))) + 255) / 256) : gb;
     if (const int rc = launch_on(h, TAG_NONE, "stream_finish_kernel", [&] {
-            (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<gf, 256, 0, h->stream>>>(
+            (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<rule_grid(c.cap, C, rule_knn(match)), 256, 0,
+                                                                              h->stream>>>(
                 static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap, static_cast<const u8 *>(c.status.p),
                 static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match),
                 rule_knn(match));

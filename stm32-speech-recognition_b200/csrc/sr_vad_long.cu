@@ -201,32 +201,20 @@ __global__ void long_status_kernel(const u32 *__restrict__ seg2, const unsigned 
     status[i] = seg2[2 * (size_t)i + 1] == SR_SEG_NULL ? SR_ST_VAD_FAIL : frm == 0 ? SR_ST_MFCC_FAIL : SR_ST_OK;
 }
 
-// the argmin (main.c:285-294) of every flat segment into its record. Under a decision rule (kRule)
-// rule_group(rule_cmds(C, knn)) threads per segment take the decision and the runner-up from its C keys (rule_row), and a
-// decision the margin rule q turns down gets SR_ST_REJECT.
+// the decision (decide, under a decision rule when kRule) of every flat segment into its record
 template <bool kRule>
 __global__ void long_scatter_kernel(const u32 *__restrict__ seg2, const u32 *__restrict__ slot, const unsigned char *__restrict__ ftr,
                                     const u8 *__restrict__ status, const u64 *__restrict__ best, const u32 *__restrict__ n_flat,
                                     sr_long_seg *__restrict__ rec, u32 C, u32 q, u32 knn) {
-    const int g = kRule ? rule_group(rule_cmds(C, knn)) : 1;
-    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / (u32)g;
+    const u32 g = kRule ? rule_lanes(C, knn) : 1u;
+    const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / g;
     if (i >= *n_flat) return;
-    u64 key;
-    u32 st = status[i];
-    if constexpr (kRule) {
-        const Top2 t2 = rule_row(best + (size_t)i * C, C, knn, (int)(threadIdx.x & (u32)(g - 1)), g);
-        if (threadIdx.x & (u32)(g - 1)) return;
-        key = t2.k1;
-        if (st == SR_ST_OK && margin_rejects((u32)(key >> 32), (u32)(t2.k2 >> 32), q)) st = SR_ST_REJECT;
-    } else {
-        key = best[i];
-    }
-    u32 idx = (u32)(key & 0xFFFFFFFFull), dis = (u32)(key >> 32);
-    if (status[i] != SR_ST_OK) { idx = 0; dis = SR_DIS_ERR; }
+    Decision d;
+    if (!decide<kRule>(best, i, status[i], C, q, knn, g, d)) return;
     sr_long_seg r;
-    r.start = seg2[2 * (size_t)i]; r.end = seg2[2 * (size_t)i + 1]; r.status = st;
+    r.start = seg2[2 * (size_t)i]; r.end = seg2[2 * (size_t)i + 1]; r.status = d.status;
     r.frm_num = (*reinterpret_cast<const u32 *>(ftr + (size_t)i * kFtrBytes)) >> 16;
-    r.best_idx = idx; r.best_dis = dis; r.cmd = idx / SR_FTR_PER_COMM;
+    r.best_idx = d.idx; r.best_dis = d.dis; r.cmd = d.cmd;
     rec[slot[i]] = r;
 }
 
@@ -284,8 +272,7 @@ cudaError_t launch_long_status(const u32 *seg2, const void *ftr, const u32 *n_fl
 
 cudaError_t launch_long_scatter(const u32 *seg2, const u32 *slot, const void *ftr, const u8 *status, const u64 *best,
                                 const u32 *n_flat, u32 M, sr_long_seg *rec, u32 C, u32 q, u32 knn, cudaStream_t st) {
-    const u32 grid = (u32)(((u64)M * (C ? (u32)rule_group(rule_cmds(C, knn)) : 1u) + 255) / 256);
-    (C ? long_scatter_kernel<true> : long_scatter_kernel<false>)<<<grid, 256, 0, st>>>(
+    (C ? long_scatter_kernel<true> : long_scatter_kernel<false>)<<<rule_grid(M, C, knn), 256, 0, st>>>(
         seg2, slot, static_cast<const unsigned char *>(ftr), status, best, n_flat, rec, C, q, knn);
     return cudaGetLastError();
 }

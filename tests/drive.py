@@ -124,6 +124,11 @@ def cmp_long_atap(got, want, rows=None):
 
 
 # ---- streams ---------------------------------------------------------------------------------------------------------
+def event_key(e):
+    """(stream, segment) of a stream event"""
+    return (int(e["stream"]), int(e["segment"]))
+
+
 def k4_events(pool, pcm, arrival, rng, on_push=None):
     """fixed-capture pushes of pcm, "lockstep" (800 samples each) or ragged: (events, on_push(p) of the push that returned
     each); on_push(p) runs before push p"""

@@ -4,7 +4,8 @@
   the long-form VAD, the symmetric P = 1 matcher and the banded DP without the 2:1 guard;
   recognition's template scan under every matcher (match_scores) and the end-to-end calls composed from them and the
   oracle port's stages (compose_recognise, mfcc_long, recognise_connected, recognise_connected_grammar, recognise_long,
-  recognise_long_grammar); and the recordings and banks the tests share."""
+  recognise_long_grammar); a call's records under a decision rule (under_rule, long_under_rule); and the recordings and
+  banks the tests share."""
 import ctypes as C
 import functools
 import os
@@ -12,7 +13,7 @@ import os
 import numpy as np
 
 from oracle_bind import ATAP_DTYPE, FTR_DTYPE, NULL, PortOracle, _p, segment_rows
-from refs import NTHREADS
+from refs import NTHREADS, decide
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXT_SO = os.path.join(ROOT, "oracle", "_build", "liboracle_ext.so")
@@ -312,6 +313,18 @@ def compose_recognise(front, bank, T, flags, r):
     return out
 
 
+
+def under_rule(off, k, q):
+    """what a recognition call writes under SR_DTW_KNN(k) | SR_DTW_REJECT(q), from the same call without a rule (off):
+    refs.decide on the scores of its SR_ST_OK rows"""
+    out = {key: np.array(v, copy=True) for key, v in off.items()}
+    ok = np.flatnonzero(np.asarray(off["status"]) == 0)
+    if len(ok) and np.asarray(off["score"]).shape[1]:
+        idx, dis, cmd, rej = decide(np.asarray(off["score"])[ok], k, q)
+        out["best_idx"][ok], out["best_dis"][ok], out["cmd"][ok] = idx, dis, cmd
+        out["status"][ok] = np.where(rej, 3, 0)                            # SR_ST_REJECT, SR_ST_OK
+    return out
+
 def recognise_connected(ora, co, pcm, n_len, bank, n_slot, slot_stride, penalty, max_words, geom_b=False, atap0=None):
     """sr_recognise_connected_batch composed from the oracle stages: noise_atap and VAD per row, mfcc_long of every segment
     at frm_cap = 818, the decoder on each segment with frames, the words joined in segment order (segment set), total the
@@ -400,6 +413,23 @@ def recognise_long(lo, port, pcm, n_len, bank, n_slot, slot_stride, max_segs, le
                 r["best_idx"], r["best_dis"], r["cmd"] = j, sc[i, j], j // 4
     return dict(atap=atap, n_segs=n, segs=segs)
 
+
+
+def long_under_rule(off, pcm, n_len, lens, bank, n_slot, match, k, q):
+    """what sr_recognise_long_batch writes under SR_DTW_KNN(k) | SR_DTW_REJECT(q) and the matcher match = (flags, r), from
+    the same call's records without a rule (off): refs.decide on the oracles' scores of each SR_ST_OK segment"""
+    port = PortOracle()
+    w = recognise_long(long_oracle(), port, pcm, n_len, bank, 0, 4096, off["segs"].shape[1], lens)
+    segs = off["segs"].copy()
+    todo = [(b, j) for b in range(len(segs)) for j in range(min(int(off["n_segs"][b]), segs.shape[1]))
+            if segs[b, j]["status"] == 0]
+    if todo:
+        ftr = ftr_of_segments(port, pcm, w["atap"], [(b, int(segs[b, j]["start"]), int(segs[b, j]["end"])) for b, j in todo])
+        idx, dis, cmd, rej = decide(match_scores(ftr, bank, n_slot, *match), k, q)
+        for i, (b, j) in enumerate(todo):
+            r = segs[b, j]
+            r["best_idx"], r["best_dis"], r["cmd"], r["status"] = idx[i], dis[i], cmd[i], 3 if rej[i] else 0
+    return dict(off, segs=segs)
 
 def recognise_long_grammar(lo, port, lg, pcm, n_len, bank, n_slot, slot_stride, grammar, penalty, max_segs, max_words,
                            lens=None, geom_b=False, atap=None):

@@ -1,8 +1,8 @@
 """Plain references the tests share (TEST INFRASTRUCTURE, CPU only): the local distance, the banded, full-matrix,
-any-rate and path DPs, DTW barycentre averaging, the connected-word and grammar helpers, the long-form VAD transcribed
-from VAD.C, and the host's launch plan of the connected-word calls. Each is written from its definition and shares no code with
-oracle/sr_oracle.c or tests/oracle_ext, so that a mistake common to a kernel and its oracle still fails a test. Bare
-asserts here are not rewritten by pytest, so each one carries a message."""
+any-rate and path DPs, the decision rules, DTW barycentre averaging, the connected-word and grammar helpers, the
+long-form VAD transcribed from VAD.C, and the host's launch plan of the connected-word calls. Each is written from its
+definition and shares no code with oracle/sr_oracle.c or tests/oracle_ext, so that a mistake common to a kernel and its
+oracle still fails a test. Bare asserts here are not rewritten by pytest, so each one carries a message."""
 import os
 
 import numpy as np
@@ -103,6 +103,31 @@ def want_best(score):
     key = (score.astype(np.uint64) << np.uint64(32)) | np.arange(T, dtype=np.uint64)[None, :]
     k = key.min(axis=1)
     return (k & np.uint64(0xFFFFFFFF)).astype(np.uint32), (k >> np.uint64(32)).astype(np.uint32)
+
+
+def decide(score, k=0, q=0):
+    """(best_idx, best_dis, cmd, reject) of each row of score [N][T] under SR_DTW_KNN(k) | SR_DTW_REJECT(q); k = 0 is the
+    nearest-slot decision of main.c:276-292, and KNN(1) | REJECT(q) the margin rule"""
+    score = np.asarray(score, np.uint32)
+    N, T = score.shape
+    C = (T + 3) // 4
+    s = np.full((N, 4 * C), DIS_ERR, np.uint64)
+    s[:, :T] = score
+    s = s.reshape(N, C, 4)
+    n = (s != DIS_ERR).sum(axis=2)
+    m = np.minimum(max(k, 1), n)
+    srt = np.sort(s, axis=2)                                             # SR_DIS_ERR last
+    take = np.arange(4)[None, None, :] < m[:, :, None]
+    e = np.where(m > 0, np.where(take, srt, 0).sum(axis=2) // np.maximum(m, 1), DIS_ERR).astype(np.uint64)
+    slot = np.arange(C)[None, :] * 4 + np.argmin(s, axis=2)              # first of the command's minima
+    key = (e << np.uint64(32)) | np.where(m > 0, slot, 0).astype(np.uint64)
+    c1 = np.argmin(key, axis=1)
+    k1 = key[np.arange(N), c1]
+    idx, d1 = (k1 & np.uint64(DIS_ERR)).astype(np.uint32), k1 >> np.uint64(32)
+    others = np.where(np.arange(C)[None, :] == c1[:, None], np.uint64(DIS_ERR), e)
+    d2 = others.min(axis=1, initial=DIS_ERR)
+    rej = (q > 0) & (d2 != DIS_ERR) & (np.uint64(1000) * (d2 - d1) < np.uint64(q) * d1)
+    return idx, d1.astype(np.uint32), idx // 4, rej
 
 
 # ---- paths and averaging ---------------------------------------------------------------------------------------------

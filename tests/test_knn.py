@@ -19,7 +19,8 @@ import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
 from cases import synth_long_poisoned
-from drive import handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np
+from drive import cmp_long, event_key, handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np, same
+from refs import decide
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DIS_ERR = 0xFFFFFFFF
@@ -34,32 +35,7 @@ RULES = tuple((k, q) for k in (1, 2, 3, 4) for q in (0, 100))
 U = 16000
 
 
-# ---- the rule in numpy ---------------------------------------------------------------------------------------------------
-def knn_decide(score, k, q=0):
-    """(best_idx, best_dis, cmd, reject) of each row of score [N][T] under SR_DTW_KNN(k) | SR_DTW_REJECT(q); k = 0 is the
-    nearest-slot decision of main.c:276-292"""
-    score = np.asarray(score, np.uint32)
-    N, T = score.shape
-    C = (T + 3) // 4
-    s = np.full((N, 4 * C), DIS_ERR, np.uint64)
-    s[:, :T] = score
-    s = s.reshape(N, C, 4)
-    n = (s != DIS_ERR).sum(axis=2)
-    m = np.minimum(max(k, 1), n)
-    srt = np.sort(s, axis=2)                                             # SR_DIS_ERR last
-    take = np.arange(4)[None, None, :] < m[:, :, None]
-    e = np.where(m > 0, np.where(take, srt, 0).sum(axis=2) // np.maximum(m, 1), DIS_ERR).astype(np.uint64)
-    slot = np.arange(C)[None, :] * 4 + np.argmin(s, axis=2)              # first of the command's minima
-    key = (e << np.uint64(32)) | np.where(m > 0, slot, 0).astype(np.uint64)
-    c1 = np.argmin(key, axis=1)
-    k1 = key[np.arange(N), c1]
-    idx, d1 = (k1 & np.uint64(DIS_ERR)).astype(np.uint32), k1 >> np.uint64(32)
-    others = np.where(np.arange(C)[None, :] == c1[:, None], np.uint64(DIS_ERR), e)
-    d2 = others.min(axis=1, initial=DIS_ERR)
-    rej = (q > 0) & (d2 != DIS_ERR) & (np.uint64(1000) * (d2 - d1) < np.uint64(q) * d1)
-    return idx, d1.astype(np.uint32), idx // 4, rej
-
-
+# ---- the rule in Python --------------------------------------------------------------------------------------------------
 def knn_brute(row, k, q):
     """the rule on one score row with Python integers"""
     T = len(row)
@@ -76,25 +52,6 @@ def knn_brute(row, k, q):
     d2 = min([e[c] for c in range(len(e)) if c != c1], default=DIS_ERR)
     rej = q > 0 and d2 != DIS_ERR and 1000 * (d2 - e[c1]) < q * e[c1]
     return idx, e[c1], c1, rej
-
-
-def expect(off, k, q):
-    """what a recognition call writes under KNN(k) | REJ(q), from the same call without a rule (off)"""
-    out = {key: np.array(v, copy=True) for key, v in off.items()}
-    ok = np.flatnonzero(np.asarray(off["status"]) == OK)
-    if len(ok) and np.asarray(off["score"]).shape[1]:
-        idx, dis, cmd, rej = knn_decide(np.asarray(off["score"])[ok], k, q)
-        out["best_idx"][ok], out["best_dis"][ok], out["cmd"][ok] = idx, dis, cmd
-        out["status"][ok] = np.where(rej, REJECT, OK)
-    return out
-
-
-def same(got, want, what):
-    for key in ("seg_off", "score", "best_idx", "best_dis", "cmd", "status"):
-        g, w = np.asarray(got[key]), np.asarray(want[key])
-        bad = np.flatnonzero((g.reshape(len(g), -1) != w.reshape(len(w), -1)).any(axis=1))
-        assert len(bad) == 0, (what, key, bad[:8].tolist())
-    assert ob.ftr_equal(got["ftr"], want["ftr"]), what
 
 
 # ---- banks -----------------------------------------------------------------------------------------------------------------
@@ -167,8 +124,8 @@ def test_header_and_binding_define_the_rule():
 
 
 def test_rule_reference_equals_brute_force():
-    """random rows with SR_DIS_ERR, ties and widths that are not multiples of 4: knn_decide == knn_brute, and k = 0 and
-    k = 1 are the nearest-slot argmin"""
+    """random rows with SR_DIS_ERR, ties and widths that are not multiples of 4: refs.decide == knn_brute, and k = 0
+    and k = 1 are the nearest-slot argmin"""
     rng = np.random.default_rng(0x7E7)
     for T in (1, 3, 4, 5, 8, 13, 80, 150):
         for kind in range(3):
@@ -178,13 +135,13 @@ def test_rule_reference_equals_brute_force():
             sc[:5] = DIS_ERR
             for k in (0, 1, 2, 3, 4):
                 for q in (0, 1, 100, 65535):
-                    got = knn_decide(sc, k, q)
+                    got = decide(sc, k, q)
                     for i in range(0, 200, 7):
                         want = knn_brute(sc[i], max(k, 1), q)
                         assert tuple(int(np.asarray(g)[i]) for g in got) == tuple(int(w) for w in want), (T, k, q, i)
             nn = np.argmin(sc, axis=1)
             for k in (0, 1):
-                idx, dis, _, _ = knn_decide(sc, k)
+                idx, dis, _, _ = decide(sc, k)
                 assert np.array_equal(idx, nn) and np.array_equal(dis, sc[np.arange(200), nn])
 
 
@@ -197,13 +154,13 @@ def test_planted_case_turns_the_decision():
     """on the oracle's scores: the nearest slot names command 1, KNN(3) command 0; with q just above KNN(3)'s margin the
     margin rule rejects the KNN decision, while the nearest-slot decision (score 0) always stands"""
     _, _, sc = _planted_scores()
-    assert knn_decide(sc[None], 0)[2][0] == 1 and knn_decide(sc[None], 3)[2][0] == 0, sc.tolist()
-    d1 = int(knn_decide(sc[None], 3)[1][0])
+    assert decide(sc[None], 0)[2][0] == 1 and decide(sc[None], 3)[2][0] == 0, sc.tolist()
+    d1 = int(decide(sc[None], 3)[1][0])
     d2 = (int(sc[4]) + sorted(int(x) for x in sc[5:8])[0] + sorted(int(x) for x in sc[5:8])[1]) // 3
     q = 1000 * (d2 - d1) // d1 + 1
     assert 0 < q <= 65535, (d1, d2)
-    assert knn_decide(sc[None], 3, q)[3][0] and not knn_decide(sc[None], 0, q)[3][0]
-    assert not knn_decide(sc[None], 3, q - 1)[3][0]
+    assert decide(sc[None], 3, q)[3][0] and not decide(sc[None], 0, q)[3][0]
+    assert not decide(sc[None], 3, q - 1)[3][0]
 
 
 # ---- GPU: setter and flag rules ----------------------------------------------------------------------------------------
@@ -297,7 +254,7 @@ def test_recognise_paths_under_knn(batch, bank_kind, matcher):
         plain = {}
         for k, q in RULES:
             h.set_match(flags | KNN(k) | REJ(q), r)
-            want = expect(off, k, q)
+            want = ox.under_rule(off, k, q)
             h.set_transport(0)
             on = h.recognise(pcm, 2400)
             assert [t for t, _ in h.timing_collect()] == tags_off, (k, q)
@@ -305,7 +262,7 @@ def test_recognise_paths_under_knn(batch, bank_kind, matcher):
             h.set_transport(1)
             same(h.recognise(pcm, 2400), want, ("host packed", k, q))
             h.timing_collect()
-            same(recognise_dev_np(h, pcm, 2400, T), expect(dev_off, k, q), ("device", k, q))
+            same(recognise_dev_np(h, pcm, 2400, T), ox.under_rule(dev_off, k, q), ("device", k, q))
             h.use_own_stream()
             h.timing_collect()
             plain[k, q] = on
@@ -324,7 +281,7 @@ def test_planted_case_on_the_gpu():
     """the planted bank: the nearest slot names command 1, KNN(3) command 0; the margin rule at the q of
     test_planted_case_turns_the_decision rejects under KNN(3) only"""
     pcm, bank, sc = _planted_scores()
-    d1 = int(knn_decide(sc[None], 3)[1][0])
+    d1 = int(decide(sc[None], 3)[1][0])
     d2 = (int(sc[4]) + sum(sorted(int(x) for x in sc[5:8])[:2])) // 3
     q = 1000 * (d2 - d1) // d1 + 1
     h = handle(bank, 8)
@@ -334,7 +291,7 @@ def test_planted_case_on_the_gpu():
         for k, qq, cmd, st in ((3, 0, 0, OK), (3, q, 0, REJECT), (0, q, 1, OK)):
             h.set_match(KNN(k) | REJ(qq), 0)
             out = h.recognise(pcm, 2400)
-            same(out, expect(nn, k, qq), (k, qq))
+            same(out, ox.under_rule(nn, k, qq), (k, qq))
             assert (out["cmd"][1], out["status"][1]) == (cmd, st), (k, qq)
     finally:
         h.close()
@@ -389,7 +346,7 @@ def test_multi_under_knn_and_refusal_of_unequal_rules(batch):
         ref = off.recognise(pcm, 2400)
         off.close()
         out = sr_b200.recognise_multi([a, b], pcm, 2400)
-        want = expect(ref, 3, 100)
+        want = ox.under_rule(ref, 3, 100)
         for key in out:
             assert np.array_equal(np.asarray(out[key]), np.asarray(want[key])), key
         for other in (0, KNN(2) | REJ(100), KNN(3), KNN(1) | REJ(100), BAND | KNN(3) | REJ(100)):
@@ -404,30 +361,6 @@ def test_multi_under_knn_and_refusal_of_unequal_rules(batch):
 
 
 # ---- long recordings and streams ------------------------------------------------------------------------------------------
-def _long_want(pcm, lens, bank, T, matcher, max_segs, off, k, q):
-    """a long-form call's records under KNN(k) | REJ(q): off's records with the rule applied to the oracle's scores of
-    each OK segment"""
-    w = ox.recognise_long(ox.long_oracle(), ob.port(), pcm, 2400, bank, 0, 4096, max_segs, lens)
-    segs = off["segs"]
-    todo = [(b, j) for b in range(len(segs)) for j in range(min(int(off["n_segs"][b]), max_segs)) if segs[b, j]["status"] == OK]
-    want = segs.copy()
-    if todo:
-        ftr = ox.ftr_of_segments(ob.port(), pcm, w["atap"], [(b, int(segs[b, j]["start"]), int(segs[b, j]["end"]))
-                                                             for b, j in todo])
-        idx, dis, cmd, rej = knn_decide(ox.match_scores(ftr, bank, T, *matcher), k, q)
-        for i, (b, j) in enumerate(todo):
-            r = want[b, j]
-            r["best_idx"], r["best_dis"], r["cmd"], r["status"] = idx[i], dis[i], cmd[i], REJECT if rej[i] else OK
-    return want
-
-
-def _cmp_long(got, off, want, what):
-    assert np.array_equal(got["n_segs"], off["n_segs"]), what
-    for b in range(len(off["n_segs"])):
-        m = min(int(off["n_segs"][b]), off["segs"].shape[1])
-        assert got["segs"][b, :m].tobytes() == want[b, :m].tobytes(), (what, b)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("matcher", ((0, 0), (BAND, 10), (SYM, 10)), ids=lambda m: "%d_r%d" % m)
 def test_long_batch_and_dev_under_knn(matcher):
@@ -443,19 +376,15 @@ def test_long_batch_and_dev_under_knn(matcher):
         changed = 0
         for k, q in ((1, 0), (2, 0), (3, 100), (4, 0), (4, 1000)):
             h.set_match(flags | KNN(k) | REJ(q), r)
-            want = _long_want(pcm, lens, bank, T, matcher, 64, off, k, q)
-            _cmp_long(h.recognise_long_batch(pcm, 64, 2400, lens), off, want, ("host", k, q))
-            _cmp_long(recognise_long_dev_np(h, pcm, lens, 64), off, want, ("dev", k, q))
+            want = ox.long_under_rule(off, pcm, 2400, lens, bank, T, matcher, k, q)
+            cmp_long(h.recognise_long_batch(pcm, 64, 2400, lens), want)
+            cmp_long(recognise_long_dev_np(h, pcm, lens, 64), want)
             if k == 1 and q == 0:
-                _cmp_long(off, off, want, "identity")
-            changed += int((want["best_dis"] != off["segs"]["best_dis"]).sum())
+                cmp_long(off, want)
+            changed += int((want["segs"]["best_dis"] != off["segs"]["best_dis"]).sum())
         assert changed > 0
     finally:
         h.close()
-
-
-def _event_key(e):
-    return (int(e["stream"]), int(e["segment"]))
 
 
 # the settings a stream's pushes cycle through
@@ -486,13 +415,13 @@ def test_k4_streams_under_knn_switched_between_pushes():
     ora, seen = ob.best_oracle(), set()
     assert len(events) >= 2 * S
     for e, (k, q) in events:
-        s, j = _event_key(e)
+        s, j = event_key(e)
         f = ora.mfcc_batch(pcm[s:s + 1], seg[s, j].reshape(1, 2), atap[s:s + 1])
         assert e["frm_num"] == int(f["frm_num"][0]), e
         if e["frm_num"] == 0:
             assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (2, 0, DIS_ERR, 0), e
             continue
-        idx, dis, cmd, rej = knn_decide(ox.match_scores(f, bank, T, BAND, 10), k, q)
+        idx, dis, cmd, rej = decide(ox.match_scores(f, bank, T, BAND, 10), k, q)
         assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (REJECT if rej[0] else OK, idx[0], dis[0], cmd[0]), \
             (k, q, e)
         seen.add((k, q))
@@ -525,14 +454,14 @@ def test_k14_streams_under_knn_switched_between_pushes():
     w = ox.recognise_long(ox.long_oracle(), ob.port(), pcm, 2400, bank, T, 4096, 256, lens)
     seen = set()
     for e, (k, q) in events:
-        s, j = _event_key(e)
+        s, j = event_key(e)
         rec = w["segs"][s, j]
         assert (int(e["start"]), int(e["end"]), int(e["frm_num"])) == (int(rec["start"]), int(rec["end"]), int(rec["frm_num"]))
         if rec["status"] != OK:
             assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (rec["status"], 0, DIS_ERR, 0), e
             continue
         f = ox.ftr_of_segments(ob.port(), pcm, w["atap"], [(s, int(e["start"]), int(e["end"]))])
-        idx, dis, cmd, rej = knn_decide(ox.match_scores(f, bank, T, 0, 0), k, q)
+        idx, dis, cmd, rej = decide(ox.match_scores(f, bank, T, 0, 0), k, q)
         assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (REJECT if rej[0] else OK, idx[0], dis[0], cmd[0]), \
             (k, q, e)
         seen.add((k, q))

@@ -19,7 +19,8 @@ import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
 from cases import bank_planted, digit_bank, inputs, real_speech_pairs, synth_long_poisoned
-from drive import handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np
+from drive import event_key, handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np
+from refs import decide
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NULL = DIS_ERR = 0xFFFFFFFF
@@ -34,21 +35,6 @@ QS = (1, 100, 1000, 65535)
 
 
 # ---- the rule in Python --------------------------------------------------------------------------------------------------
-def rule_ref(score, q):
-    """(best_idx, best_dis, reject) of each row of score [B][T] under SR_DTW_REJECT(q), vectorised"""
-    score = np.asarray(score, np.uint32)
-    B, T = score.shape
-    slots = np.arange(T, dtype=np.uint64)
-    key = (score.astype(np.uint64) << np.uint64(32)) | slots[None, :]
-    k1 = key.min(axis=1)
-    idx = (k1 & np.uint64(0xFFFFFFFF)).astype(np.uint32)
-    d1 = (k1 >> np.uint64(32)).astype(np.uint64)
-    other = (slots[None, :] // 4) != (idx.astype(np.uint64) // 4)[:, None]
-    d2 = np.where(other, score, np.uint32(DIS_ERR)).min(axis=1, initial=DIS_ERR).astype(np.uint64)
-    rej = (d2 != DIS_ERR) & (np.uint64(1000) * (d2 - d1) < np.uint64(q) * d1)
-    return idx, d1.astype(np.uint32), rej
-
-
 def rule_brute(row, q):
     """the rule on one score row with Python integers: the winner, then every other command's best score"""
     T = len(row)
@@ -58,16 +44,6 @@ def rule_brute(row, q):
     if not runners or min(runners) == DIS_ERR:
         return False
     return 1000 * (min(runners) - d1) < q * d1
-
-
-def status_under_rule(score, status, q):
-    """the status a call writes under the rule: SR_ST_REJECT over an SR_ST_OK decision the rule turns down"""
-    out = np.array(status, np.uint8).copy()
-    ok = out == OK
-    if ok.any() and np.asarray(score).shape[1]:
-        _, _, rej = rule_ref(np.asarray(score)[ok], q)
-        out[np.flatnonzero(ok)[rej]] = REJECT
-    return out
 
 
 # ---- CPU -----------------------------------------------------------------------------------------------------------------
@@ -87,8 +63,8 @@ def test_header_and_binding_define_the_rule():
 
 
 def test_rule_reference_equals_brute_force():
-    """rule_ref == rule_brute on random rows: ties between commands, d1 = 0, all-SR_DIS_ERR runner-ups, T not a multiple
-    of 4, one-command banks, q = 1 and q = 65535"""
+    """refs.decide(score, 1, q) == rule_brute on random rows: ties between commands, d1 = 0, all-SR_DIS_ERR runner-ups,
+    T not a multiple of 4, one-command banks, q = 1 and q = 65535"""
     rng = np.random.default_rng(0x7E1)
     seen = dict(tie=0, zero=0, err_runner=0, one_cmd=0, rej=0, keep=0)
     for T in (1, 2, 3, 4, 5, 7, 8, 9, 13, 33, 80):
@@ -107,7 +83,7 @@ def test_rule_reference_equals_brute_force():
                     sc = rng.integers(1, 5000, (B, T))
                     sc[rng.random((B, T)) < 0.6] = DIS_ERR
                 sc = sc.astype(np.uint32)
-                _, d1, rej = rule_ref(sc, q)
+                _, d1, _, rej = decide(sc, 1, q)
                 for b in range(B):
                     assert bool(rej[b]) == rule_brute(sc[b], q), (T, q, kind, sc[b].tolist())
                 seen["one_cmd"] += T <= 4
@@ -139,7 +115,7 @@ def _margin_table(q):
         todo = [k for k in range(m) if segs[k]["status"] == OK]
         ftr = ox.ftr_of_segments(port, b[None], w["atap"], [(0, int(segs[k]["start"]), int(segs[k]["end"])) for k in todo])
         sc = ox.match_scores(ftr, bank, T, RATE, 118)
-        idx, _, rej = rule_ref(sc, q)
+        idx, _, _, rej = decide(sc, 1, q)
         inv = np.array([k < half for k in todo])
         right = idx // 4 == np.array(todo)
         rows.append((int(inv.sum()), int((inv & ~rej).sum()), int((inv & ~rej & right).sum()), int((~inv).sum()),
@@ -251,7 +227,7 @@ def _same_but_status(on, off, q, what):
     for k in ("seg_off", "score", "best_idx", "best_dis", "cmd"):
         assert np.array_equal(np.asarray(on[k]), np.asarray(off[k])), (what, q, k)
     assert ob.ftr_equal(on["ftr"], off["ftr"]), what
-    want = status_under_rule(off["score"], off["status"], q)
+    want = ox.under_rule(off, 1, q)["status"]
     bad = np.flatnonzero(np.asarray(on["status"]) != want)
     assert len(bad) == 0, (what, q, bad[:8].tolist())
     return int((want == REJECT).sum())
@@ -313,7 +289,7 @@ def test_rule_boundary_and_runner_up_are_exact(case):
         off = h.recognise(pcm, 2400)
         good = off["status"] == OK
         s = off["score"][good].astype(np.int64)
-        i1, d1, _ = rule_ref(off["score"][good], 1)
+        i1, d1, _, _ = decide(off["score"][good], 1, 1)
         d1 = d1.astype(np.int64)
         masked = np.where((np.arange(T)[None, :] // 4) == (i1 // 4)[:, None], DIS_ERR, s)
         d2 = masked.min(axis=1)
@@ -358,34 +334,18 @@ def test_bank_widths_and_batch_edges(T):
 
 
 # ---- long recordings and streams ------------------------------------------------------------------------------------------
-def _long_status(pcm, lens, bank, T, flags, r, q, max_segs, rec):
-    """what the rule makes of a long-form call's records rec, from the oracle's features and scores of each OK segment"""
-    w = ox.recognise_long(ox.long_oracle(), ob.port(), pcm, 2400, bank, 0, 4096, max_segs, lens)
-    segs = rec["segs"]
-    todo = [(b, k) for b in range(len(segs)) for k in range(min(int(rec["n_segs"][b]), max_segs)) if segs[b, k]["status"] == OK]
-    want = segs["status"].copy()
-    if todo:
-        ftr = ox.ftr_of_segments(ob.port(), pcm, w["atap"], [(b, int(segs[b, k]["start"]), int(segs[b, k]["end"]))
-                                                             for b, k in todo])
-        sc = ox.match_scores(ftr, bank, T, flags, r)
-        idx, d1, rej = rule_ref(sc, q)
-        for i, (b, k) in enumerate(todo):
-            if sc[i].min() != DIS_ERR:
-                assert (segs[b, k]["best_idx"], segs[b, k]["best_dis"]) == (idx[i], d1[i]), (b, k)
-            if rej[i]:
-                want[b, k] = REJECT
-    return want
-
-
-def _cmp_long_rule(on, off, want_status, what):
+def _cmp_long_rule(on, off, want, what):
+    """on's records are want's, and want's are the rule-off records off except status (the rule's decision is the
+    nearest slot's); the number of rejections"""
     assert np.array_equal(on["n_segs"], off["n_segs"]), what
+    kept = want["segs"].copy()
+    kept["status"] = off["segs"]["status"]
+    assert kept.tobytes() == off["segs"].tobytes(), what
     for b in range(len(off["n_segs"])):
         m = min(int(off["n_segs"][b]), off["segs"].shape[1])
-        a, o = on["segs"][b, :m].copy(), off["segs"][b, :m]
-        assert np.array_equal(a["status"], want_status[b, :m]), (what, b)
-        a["status"] = o["status"]
-        assert a.tobytes() == o.tobytes(), (what, b)
-    return sum(int((want_status[b, :min(int(off["n_segs"][b]), 64)] == REJECT).sum()) for b in range(len(off["n_segs"])))
+        assert np.array_equal(on["segs"][b, :m]["status"], want["segs"][b, :m]["status"]), (what, b)
+        assert on["segs"][b, :m].tobytes() == want["segs"][b, :m].tobytes(), (what, b)
+    return int((want["segs"]["status"] == REJECT).sum())
 
 
 @pytest.mark.gpu
@@ -405,7 +365,7 @@ def test_long_batch_and_dev_under_the_rule(matcher):
         total = 0
         for q in (100, 1000):
             h.set_match(flags | REJ(q), r)
-            want = _long_status(pcm, lens, bank, T, flags, r, q, 64, off)
+            want = ox.long_under_rule(off, pcm, 2400, lens, bank, T, matcher, 1, q)
             on = h.recognise_long_batch(pcm, 64, 2400, lens)
             assert [t for t, _ in h.timing_collect()] == tags
             total += _cmp_long_rule(on, off, want, "host")
@@ -415,10 +375,6 @@ def test_long_batch_and_dev_under_the_rule(matcher):
         assert total > 0
     finally:
         h.close()
-
-
-def _event_key(e):
-    return (int(e["stream"]), int(e["segment"]))
 
 
 @pytest.mark.gpu
@@ -446,19 +402,19 @@ def test_k4_streams_under_the_rule():
             pool.close()
         finally:
             h.close()
-    off = {_event_key(e): e for e, _ in runs["off"]}
-    assert sorted(off) == sorted(_event_key(e) for e, _ in runs["on"])
+    off = {event_key(e): e for e, _ in runs["off"]}
+    assert sorted(off) == sorted(event_key(e) for e, _ in runs["on"])
     ora, n_rej = ob.best_oracle(), 0
     for e, q in runs["on"]:
-        o = off[_event_key(e)]
+        o = off[event_key(e)]
         for k in ("start", "end", "frm_num", "best_idx", "best_dis", "cmd"):
             assert e[k] == o[k], (k, e, o)
         want = o["status"]
         if want == OK and q:
-            s, k = _event_key(e)
+            s, k = event_key(e)
             f = ora.mfcc_batch(pcm[s:s + 1], seg[s, k].reshape(1, 2), atap[s:s + 1])
             sc = ox.match_scores(f, bank, T, BAND, 10)
-            idx, d1, rej = rule_ref(sc, q)
+            idx, d1, _, rej = decide(sc, 1, q)
             assert (idx[0], d1[0]) == (o["best_idx"], o["best_dis"])
             want = REJECT if rej[0] else OK
         assert e["status"] == want, (e, o, q)
@@ -488,8 +444,8 @@ def test_k14_rule_switched_between_pushes():
             pool.close()
         finally:
             h.close()
-    off = {_event_key(e): e for e, _ in runs["off"]}
-    assert sorted(off) == sorted(_event_key(e) for e, _ in runs["on"])
+    off = {event_key(e): e for e, _ in runs["off"]}
+    assert sorted(off) == sorted(event_key(e) for e, _ in runs["on"])
     Ul = max(len(x) for x in xs)
     pcm = np.zeros((len(xs), Ul), np.uint16)
     lens = np.array([len(x) for x in xs], np.uint32)
@@ -498,7 +454,7 @@ def test_k14_rule_switched_between_pushes():
     w = ox.recognise_long(ox.long_oracle(), ob.port(), pcm, 2400, bank, 0, 4096, 256, lens)
     n_rej, seen_q = 0, set()
     for e, q in runs["on"]:
-        o = off[_event_key(e)]
+        o = off[event_key(e)]
         for k in ("start", "end", "frm_num", "best_idx", "best_dis", "cmd"):
             assert e[k] == o[k], (k, e, o)
         want = o["status"]
@@ -506,7 +462,7 @@ def test_k14_rule_switched_between_pushes():
             s = int(e["stream"])
             f = ox.ftr_of_segments(ob.port(), pcm, w["atap"], [(s, int(e["start"]), int(e["end"]))])
             sc = ox.match_scores(f, bank, T, 0, 0)
-            want = REJECT if rule_ref(sc, q)[2][0] else OK
+            want = REJECT if decide(sc, 1, q)[3][0] else OK
         assert e["status"] == want, (e, o, q)
         n_rej += want == REJECT
         seen_q.add(q)
