@@ -213,8 +213,21 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
  * are what the call writes without the rule, and the rule rejects nothing by itself. SR_DTW_KNN(1) is the call without
  * the rule, bit for bit. With SR_DTW_REJECT(q) as well, the margin rule takes d1 = e_cmd and d2 = the smallest e_c over
  * the other commands. _dev_allgather gathers best_dis << 32 | best_idx of this decision. The rule applies where the margin
- * rule does; sr_dtw_batch* accept bits 4-15 and ignore them. A build without the rule refuses these flags in
- * sr_set_match, which is how a caller detects it. */
+ * rule does; sr_dtw_batch* accept bits 4-15 other than SR_DTW_LIFTER and ignore them. A build without the rule refuses
+ * these flags in sr_set_match, which is how a caller detects it. */
+#define SR_DTW_LIFTER     (1u << 13)  /* weight the local distance with a bandpass lifter (extension) */
+#define SR_DTW_LIFTER_W   { 10, 16, 21, 25, 27, 28, 27, 25, 21, 16, 10, 4 }  /* W[k-1] = round(4 (1 + 6 sin(pi k / 12))) */
+/* SR_DTW_LIFTER scores with the raised-sine bandpass lifter w_k = 1 + 6 sin(pi k / 12) of Juang, Rabiner & Wilpon (IEEE
+ * TASSP 35(7), 1987) on the cepstra c1..c12, in integers: mfcc_dat coefficient c of a row (c_{c+1}, MFCC.C:173-183)
+ * becomes a'_c = sat16(trunc(a_c * W[c] / 16)) with W = SR_DTW_LIFTER_W, the product in 32 bits, the division truncating
+ * toward zero and sat16 clamping to [-32768, 32767] (only |a_c| > 18 724 saturates). The scale keeps every liftered value
+ * within 1.75x of the original. Under the bit every matcher scores the pair (x, y) exactly as it scores the liftered pair
+ * (L(x), L(y)) without it, L applied to every row of the input and of the template; frame counts, save_sign, the 2:1
+ * guard, the band, the normalisation and SR_DIS_ERR are unchanged, and get_dis is still the square root of a u32 sum.
+ * It combines with each of the four matchers of sr_set_match and with SR_DTW_KNN(k) and SR_DTW_REJECT(q), reaches every
+ * recognition call that reads the handle's matcher, and is honoured by sr_dtw_batch*. Enrolment, sr_dtw_path_batch,
+ * sr_average_bank, the connected-word and grammar decoders and the drop-in dtw() do not read it. The ABI version stays
+ * 12: a build without the lifter refuses the bit in sr_set_match, which is how a caller detects it. */
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                  uint32_t *score /* [B][n_slot] or NULL */, uint32_t *best_idx /* [B] or NULL */,
                  uint32_t *best_dis /* [B] or NULL */);
@@ -225,10 +238,10 @@ int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, 
  * symmetric P = 1 DP above at radius band_r >= 0. Recognition keeps honouring save_sign (SR_DTW_CHECK_SIGN, main.c:283)
  * under every matcher. Any other flag value (SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE alone among them) or a
  * negative band_r fails and leaves the setting unchanged. Each of these four may carry SR_DTW_KNN(k), the KNN rule, and
- * SR_DTW_REJECT(q), the margin rule above, alone or together; a KNN field of 5-7 or any other bit in 4-15 fails and leaves
- * the setting unchanged. sr_get_match returns the flags as set, SR_DTW_ANY_RATE and the rules' bits included.
- * sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different matchers (with
- * and without SR_DTW_ANY_RATE differ, and so do different rules);
+ * SR_DTW_REJECT(q), the margin rule above, alone or together, and SR_DTW_LIFTER; a KNN field of 5-7 or any other bit in
+ * 4-15 fails and leaves the setting unchanged. sr_get_match returns the flags as set, SR_DTW_ANY_RATE, SR_DTW_LIFTER and
+ * the rules' bits included. sr_recognise_batch_multi and sr_stream_group_push* fail when their handles have different
+ * matchers (with and without SR_DTW_ANY_RATE or SR_DTW_LIFTER differ, and so do different rules);
  * the ranks of an all-gather cannot be checked without a collective, so every rank must set the same one. Enrolment,
  * sr_get_mdl_batch and the drop-in dtw() keep the greedy walk. */
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r);

@@ -111,8 +111,8 @@ int sr_set_dtw_variant(sr_handle *h, int variant) {
 }
 
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
-    // the matcher; bits 8-10 are the KNN rule SR_DTW_KNN(k), bits 16-31 the margin rule SR_DTW_REJECT(q)
-    const uint32_t m = flags & 0xFFFFu & ~SR_DTW_KNN(7);
+    // the matcher; bits 8-10 are the KNN rule SR_DTW_KNN(k), bit 13 the lifter, bits 16-31 the margin rule SR_DTW_REJECT(q)
+    const uint32_t m = flags & 0xFFFFu & ~SR_DTW_KNN(7) & ~SR_DTW_LIFTER;
     SR_REQUIRE(h, h && (m == 0 || m == SR_DTW_BAND || m == (SR_DTW_BAND | SR_DTW_ANY_RATE) || m == SR_DTW_SYM_P1) &&
                       rule_knn(flags) <= SR_FTR_PER_COMM && band_r >= 0);
     h->match_flags = flags;
@@ -463,7 +463,7 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
     SR_REQUIRE(h, scan_flags_ok(flags));
     if (B == 0) return 0;
     // under a decision rule (C > 0) the status is an output of the decision too. Without a status (sr_dtw_batch*) the
-    // rule bits, and bits 4-15 that they accept and ignore, never reach a kernel
+    // rule bits, and the bits 4-15 other than SR_DTW_LIFTER that they accept and ignore, never reach a kernel
     const u32 C = status ? rule_cols(flags, bank.n) : 0;
     if (!C) flags &= kMatcherBits;
     const bool want_best = best_idx || best_dis || cmd || C;

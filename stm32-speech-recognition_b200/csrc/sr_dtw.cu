@@ -25,8 +25,8 @@ __device__ __forceinline__ void group_barrier(int id, int nthreads) {
 // The lane-packed tile scan of dtw_kernel and dtw_band_thread_kernel. A CTA stages a tile of Tt <= 32 templates; its
 // warps, in G groups of Wg, stage NU utterances at a time, and each lane of a group scores one fixed (utterance slot,
 // template) pair of the NU x Tt (flattened), so lanes stay busy when Tt < 32. pair(I, M, urow, trow) scores a pair
-// that passed pair_walks(guard).
-template <class Pair>
+// that passed pair_walks(guard). kLift: inputs and templates staged liftered (SR_DTW_LIFTER).
+template <bool kLift, class Pair>
 __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
                                                  u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status, int Wg,
                                                  int NU, int G, u32 tile0, int tslots, const u32 *B_dev, const u32 *perm,
@@ -42,7 +42,8 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
     unsigned char *uslots = smem_raw + (size_t)tslots * kSlotBytes + kTileHdr;     // G*NU slots
     u32 *ufrm = reinterpret_cast<u32 *>(uslots + (size_t)G * NU * kSlotBytes);     // [G*NU]
 
-    stage_tile(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kK2Warps);
+    stage_tile<kLift>(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane,
+                      kK2Warps);
     __syncthreads();
 
     const int group = warp / Wg, wig = warp - group * Wg;
@@ -63,7 +64,7 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
             if (u < B && !(status && status[u] != SR_ST_OK)) {        // VAD/MFCC failed: spch_recg returns before dtw
                 const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
                 frm = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
-                stage_planes(gslots + (size_t)s * kSlotBytes, kNrm119, uf, staged_rows(frm), gtid, gthreads);
+                stage_planes<kLift>(gslots + (size_t)s * kSlotBytes, kNrm119, uf, staged_rows(frm), gtid, gthreads);
             }
             if (gtid == 0) gfrm[s] = frm;
         }
@@ -81,6 +82,7 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
     }
 }
 
+template <bool kLift>
 __global__ void __launch_bounds__(kK2Warps * 32)
 dtw_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
            u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best,
@@ -89,8 +91,8 @@ dtw_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char 
            const u32 *__restrict__ B_dev /* optional: batch size produced on the device (streaming) */,
            const u32 *__restrict__ perm /* optional: bank slots in ascending frm_num order (templates of a tile then have
                                            similar walk lengths); results are indexed by the ORIGINAL slot number */) {
-    lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
-                     true, [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+    lane_packed_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
+                            true, [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
                          PRow i0, i1, m0, m1;
                          u32 dis, steps;
                          int X1, X2, x, y, ya0, yb0, ya1, yb1;
@@ -276,11 +278,12 @@ static LanePlan plan_lanes(int Tt) {
 cudaError_t launch_dtw(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
                        u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev, const u32 *perm) {
     if (B == 0 || T == 0) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    auto *kernel = (flags & SR_DTW_LIFTER) ? dtw_kernel<true> : dtw_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
     if (e != cudaSuccess) return e;
     return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
         const LanePlan p = plan_lanes(Tt);
-        dtw_kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32, p.smem, st>>>(
+        kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32, p.smem, st>>>(
             static_cast<const unsigned char *>(in_ftr), B, static_cast<const unsigned char *>(bank), T, slot_stride, flags,
             score, best, status, p.Wg, p.NU, p.G, tile0, Tt, B_dev, perm);
         return cudaGetLastError();
@@ -335,8 +338,8 @@ constexpr s32 kInf = 0x3FFFFFFF;
 // templates one after another, the whole warp on one cost matrix: pair(I, M, urow, trow, lane) returns, in every lane, the
 // score of a pair that passed pair_walks(guard). Lane tt keeps the score of template tt; one score row and one atomicMin
 // of the warp's smallest key per utterance (under the margin rule, one per lane into its command's key). An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in
-// lane_packed_scan.
-template <class Pair>
+// lane_packed_scan. kLift: inputs and templates staged liftered (SR_DTW_LIFTER).
+template <bool kLift, class Pair>
 __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
                                                u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status,
                                                const u32 *B_dev, const u32 *perm, bool guard, Pair pair) {
@@ -348,14 +351,15 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
     unsigned char *tile = smem_raw;                                               // byte-plane slots, as in dtw_kernel
     u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)kTileT * kSlotBytes);  // [32] frame counts, [32] slot numbers
     unsigned char *uslot = smem_raw + (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)warp * kSlotBytes;
-    stage_tile(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kDtwWarps);
+    stage_tile<kLift>(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane,
+                      kDtwWarps);
     __syncthreads();
     for (u32 u = blockIdx.y * kDtwWarps + warp; u < B; u += gridDim.y * kDtwWarps) {
         const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
         u32 Iraw = kNoWalk;                               // VAD/MFCC failed: spch_recg returns before dtw
         if (!(status && status[u] != SR_ST_OK)) Iraw = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
         __syncwarp();
-        stage_planes(uslot, kNrm119, uf, staged_rows(Iraw), lane, 32);
+        stage_planes<kLift>(uslot, kNrm119, uf, staged_rows(Iraw), lane, 32);
         __syncwarp();
         u32 my_result = SR_DIS_ERR;                       // lane tt keeps the result of template tt
         for (int tt = 0; tt < Tt; ++tt) {
@@ -380,13 +384,14 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
     }
 }
 
+template <bool kLift>
 __global__ void __launch_bounds__(kDtwWarps * 32)
 dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                 u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                 const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
     // the previous row's cell of column j sits in lane j - (cprev - r): up and diag come from lanes lane + sft and
     // lane + sft - 1, and any lane past 31 or past 2r (those hold kInf) is out of the previous row's band, whatever sft is
-    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
+    warp_pair_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         s32 Dprev = kInf;
         int cprev = 0;
@@ -429,11 +434,12 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 // The band of row i is the column interval [max(c-r, 0), min(c+r, M-1)], c = floor(i*M/I); cells outside it are +inf.
 // Each row is one dp_column step (sr_dtw_core.cuh, which also gives the headroom of kInf); the template's four rows
 // stay in registers for the whole pair.
+template <bool kLift>
 __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
 dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                 u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                 const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
+    warp_pair_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         const int j0 = lane * 4;
         PRow b[4];
@@ -466,14 +472,14 @@ dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 // predicated shift-by-one passes over the register array (no divergence between lanes whose templates have different
 // lengths). Under SR_DTW_ANY_RATE a row may slide further (M > 2I): those rows take a loop of min(s, W) - 2 more passes
 // after the two, so the passes of a pair total at most M - 1, and a slide past W leaves no cell of the old row.
-template <int R>
+template <int R, bool kLift>
 __global__ void __launch_bounds__(kK2Warps * 32)
 dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                        u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best,
                        const u8 *__restrict__ status, int Wg, int NU, int G, u32 tile0, int tslots,
                        const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    lane_packed_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
-                     !(flags & SR_DTW_ANY_RATE), [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+    lane_packed_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
+                            !(flags & SR_DTW_ANY_RATE), [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
         constexpr int W = 2 * R + 1;
         if (I == 0 || M == 0) return SR_DIS_ERR;           // empty feature sets: no cell
         s32 D[W];
@@ -549,11 +555,12 @@ dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const un
 // 2^24 < kSymInf, so a move is finite exactly when it is below kSymInf.
 constexpr s32 kSymInf = 1 << 26;
 
+template <bool kLift>
 __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
 dtw_sym_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, true,
+    warp_pair_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, true,
                    [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         const int j0 = lane * 4;
         PRow b[4];
@@ -604,11 +611,12 @@ cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u
     if (band_r < 0) return cudaErrorInvalidValue;
     const int r = min(band_r, (int)kMaxFrm - 1);
     const size_t smem = (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)kDtwWarps * kSlotBytes;
-    cudaError_t e = cudaFuncSetAttribute(dtw_sym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto *kernel = (flags & SR_DTW_LIFTER) ? dtw_sym_kernel<true> : dtw_sym_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const u32 tiles = (T + kTileT - 1) / kTileT;
     dim3 grid(tiles, grid_rows(num_sms, tiles, B, kDtwWarps));
-    dtw_sym_kernel<<<grid, kDtwWarps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
+    kernel<<<grid, kDtwWarps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
                                                        static_cast<const unsigned char *>(bank), T, slot_stride, flags, r,
                                                        score, best, status, B_dev, perm);
     return cudaGetLastError();
@@ -625,18 +633,21 @@ cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, 
     const int r = min(band_r, (int)kMaxFrm - 1);
     const auto *in = static_cast<const unsigned char *>(in_ftr);
     const auto *bk = static_cast<const unsigned char *>(bank);
+    const bool lift = flags & SR_DTW_LIFTER;
     if (r == 10) {                                                            // the BASELINE radius: thread-per-pair form
-        cudaError_t e = cudaFuncSetAttribute(dtw_band_thread_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+        auto *thread_kernel = lift ? dtw_band_thread_kernel<10, true> : dtw_band_thread_kernel<10, false>;
+        cudaError_t e = cudaFuncSetAttribute(thread_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
         if (e != cudaSuccess) return e;
         return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
             const LanePlan p = plan_lanes(Tt);
-            dtw_band_thread_kernel<10><<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32,
+            thread_kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32,
                                          p.smem, st>>>(in, B, bk, T, slot_stride, flags, score, best, status, p.Wg, p.NU,
                                                        p.G, tile0, Tt, B_dev, perm);
             return cudaGetLastError();
         });
     }
-    auto *kernel = r <= 15 ? dtw_band_kernel : dtw_wide_kernel;
+    auto *kernel = r <= 15 ? (lift ? dtw_band_kernel<true> : dtw_band_kernel<false>)
+                           : (lift ? dtw_wide_kernel<true> : dtw_wide_kernel<false>);
     const size_t smem = (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)kDtwWarps * kSlotBytes;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

@@ -45,7 +45,14 @@ __device__ __forceinline__ u32 pdist(const PRow &a, const PRow &b) {
     const u32 dot = hh * 65536u + mx * 256u + ll;
     return usqrt_trunc(a.n + b.n - 2u * dot);
 }
-// convert one v_ftr_tag's rows [0,nrows) into the byte-plane slot; threads tid, tid+nthr, ... of the caller
+// SR_DTW_LIFTER's transform of one coefficient: sat16(trunc(a * W[c] / 16)), the product in s32
+__device__ __forceinline__ u32 lifter16(u32 a, int c) {
+    constexpr s32 kW[12] = SR_DTW_LIFTER_W;
+    return (u32)min(max(((s32)a * kW[c]) / 16, -32768), 32767);
+}
+// convert one v_ftr_tag's rows [0,nrows) into the byte-plane slot; threads tid, tid+nthr, ... of the caller. kLift: the
+// rows liftered first (SR_DTW_LIFTER), the norms those of the liftered rows
+template <bool kLift = false>
 __device__ __forceinline__ void stage_planes(unsigned char *slot, u32 nrm, const unsigned char *src_ftr, int nrows, int tid,
                                              int nthr) {
     for (int r = tid; r < nrows; r += nthr) {
@@ -53,6 +60,10 @@ __device__ __forceinline__ void stage_planes(unsigned char *slot, u32 nrm, const
         u32 w[6];
 #pragma unroll
         for (int j = 0; j < 6; ++j) w[j] = s[j];
+        if constexpr (kLift) {
+#pragma unroll
+            for (int j = 0; j < 6; ++j) w[j] = pack16(lifter16(lo16s(w[j]), 2 * j), lifter16(hi16s(w[j]), 2 * j + 1));
+        }
         u32 lo[3], hi[3], n = 0;
 #pragma unroll
         for (int j = 0; j < 3; ++j) {                      // words 2j, 2j+1 hold dims 4j..4j+3
@@ -92,7 +103,8 @@ __device__ __forceinline__ bool pair_walks(u32 Iraw, u32 Mraw, bool guard) {
 
 // stage bank templates t0 .. t0+Tt-1 (bank slot perm[t] when a bank order is given) into tile slots of slot_bytes each:
 // planes and norms, frame counts to tfrm[], bank slot numbers to tslot[] unless it is NULL. Warp w of nwarps stages
-// templates w, w+nwarps, ...
+// templates w, w+nwarps, ... (kLift: liftered, as stage_planes)
+template <bool kLift>
 __device__ __forceinline__ void stage_tile(unsigned char *tile, u32 slot_bytes, u32 nrm, u32 *tfrm, u32 *tslot,
                                            const unsigned char *bank, u32 slot_stride, u32 flags, const u32 *perm, u32 t0,
                                            int Tt, int warp, int lane, int nwarps) {
@@ -100,7 +112,7 @@ __device__ __forceinline__ void stage_tile(unsigned char *tile, u32 slot_bytes, 
         const u32 ts = perm ? perm[t0 + tt] : t0 + (u32)tt;
         const unsigned char *slot = bank + (size_t)ts * slot_stride;
         const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), flags);
-        stage_planes(tile + (size_t)tt * slot_bytes, nrm, slot, staged_rows(frm), lane, 32);
+        stage_planes<kLift>(tile + (size_t)tt * slot_bytes, nrm, slot, staged_rows(frm), lane, 32);
         if (lane == 0) {
             tfrm[tt] = frm;
             if (tslot) tslot[tt] = ts;

@@ -52,6 +52,7 @@ struct DynCtrl {
 
 __host__ __device__ inline u32 dyn_slot_bytes(u32 rows) { return (rows * 28u + 7u) & ~7u; }
 
+template <bool kLift>
 __global__ void __launch_bounds__(kDynWarps * 32, 1)
 dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
                u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best,
@@ -87,7 +88,7 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
     u32 R = ring_cap / uslot;
     if (R > (u32)kDynRMax) R = kDynRMax;
 
-    stage_tile(tile, tslot, tnrm, c.tfrm, c.tslot_id, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kDynWarps);
+    stage_tile<kLift>(tile, tslot, tnrm, c.tfrm, c.tslot_id, bank, slot_stride, flags, perm, t0, Tt, warp, lane, kDynWarps);
     __syncthreads();
 
     const u32 nseq = (B - blockIdx.y + gridDim.y - 1) / gridDim.y;       // utterances of this CTA: blockIdx.y + seq*gridDim.y
@@ -105,7 +106,7 @@ dtw_dyn_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
             if (!(status && status[u] != SR_ST_OK)) {                    // VAD/MFCC failed: spch_recg returns before dtw
                 const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
                 frm = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
-                stage_planes(ring + (size_t)slot * uslot, unrm, uf, min(staged_rows(frm), (int)urows), lane, 32);
+                stage_planes<kLift>(ring + (size_t)slot * uslot, unrm, uf, min(staged_rows(frm), (int)urows), lane, 32);
             }
             __syncwarp();
             if (lane == 0) { c.ufrm[slot] = frm; st_release_s(&c.flag[slot], seq + 1u); }
@@ -197,10 +198,11 @@ cudaError_t launch_dtw_dyn(const void *in_ftr, u32 B, const void *bank, u32 T, u
         if (e != cudaSuccess) return e;
     }
     const u32 smem = 226 * 1024;
-    cudaError_t e = cudaFuncSetAttribute(dtw_dyn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto *kernel = (flags & SR_DTW_LIFTER) ? dtw_dyn_kernel<true> : dtw_dyn_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     return launch_tiles(T, [&](u32 tile0, u32 ntiles, int) {
-        dtw_dyn_kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, 1u)), kDynWarps * 32, smem, st>>>(
+        kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, 1u)), kDynWarps * 32, smem, st>>>(
             static_cast<const unsigned char *>(in_ftr), B, static_cast<const unsigned char *>(bank), T, slot_stride, flags,
             score, best, status, tile0, smem, max_frm_scratch, B_dev, perm);
         return cudaGetLastError();

@@ -46,8 +46,8 @@ cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st);
 // SR_ST_REJECT into status
 cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
                               u32 *cmd, u8 *status, cudaStream_t st);
-// the matcher bits 0-3 of the flags: what sr_dtw_batch* pass on to a kernel
-constexpr u32 kMatcherBits = 0xFu;
+// the matcher bits of the flags, 0-3 and SR_DTW_LIFTER: what sr_dtw_batch* pass on to a kernel
+constexpr u32 kMatcherBits = 0xFu | SR_DTW_LIFTER;
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st);
 cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStream_t st);
 cudaError_t launch_dtw_limit(const u16 *x, const u16 *y, const u16 *I, const u16 *M, u32 n, u8 *out, cudaStream_t st);
@@ -205,7 +205,7 @@ struct sr_handle {
     sr_comm *comm = nullptr;                           // the exchange step (sr_comm_create), optional
     int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cu), -1 default
     u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk, SR_DTW_BAND (| SR_DTW_ANY_RATE) or SR_DTW_SYM_P1,
-                                                       // | SR_DTW_KNN(k) | SR_DTW_REJECT(q)
+                                                       // | SR_DTW_LIFTER | SR_DTW_KNN(k) | SR_DTW_REJECT(q)
     int match_r = 0;                                   // its band radius
     DevBuf mfcc_work;                                  // the same for mfcc_kernel (next utterance, CTAs finished)
     DevBuf vad_work;                                   // two words: dynamic utterance hand-out of vad_kernel (zeroed once, self re-arming)
@@ -329,6 +329,7 @@ inline cudaError_t launch_dtw_h(sr_handle *h, const BankView &bank, const void *
 // The template scan of B inputs against `bank` -- the one place a matcher becomes a kernel launch: with SR_DTW_SYM_P1 in
 // flags the symmetric P = 1 DP of radius band_r, with SR_DTW_BAND the banded DP of radius band_r (launch_dtw_band picks
 // the kernel from r; its kernels read SR_DTW_ANY_RATE from flags and then skip the 2:1 guard), else the greedy walk.
+// Each launcher picks its kernel's liftered form when flags has SR_DTW_LIFTER.
 // sr_dtw_batch passes its caller's flags and r; the recognition paths (recognise, streaming) pass the handle's matcher.
 // The callers refuse SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE without SR_DTW_BAND.
 inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, int band_r,
@@ -343,9 +344,10 @@ inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *i
 }
 
 // the two handles' recognition calls score and decide alike: both greedy, or both the same DP (SR_DTW_ANY_RATE included)
-// at the same radius, under the same decision rules
+// at the same radius, with or without SR_DTW_LIFTER alike, under the same decision rules
 inline bool same_match(const sr_handle *a, const sr_handle *b) {
-    return a->match_flags == b->match_flags && ((a->match_flags & kMatcherBits) == 0 || a->match_r == b->match_r);
+    return a->match_flags == b->match_flags &&
+           ((a->match_flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) == 0 || a->match_r == b->match_r);
 }
 
 int comm_wait_before_scan(sr_handle *h, const void *score);   // sr_comm.cu

@@ -20,6 +20,8 @@ DIS_ERR = 0xFFFFFFFF
 SAVE_MASK = 12345
 FTR_PER_COMM = 4               # SR_FTR_PER_COMM: bank slots per command
 DTW_CHECK_SIGN, DTW_BAND, DTW_SYM_P1, DTW_ANY_RATE = 1, 2, 4, 8
+DTW_LIFTER = 1 << 13           # SR_DTW_LIFTER: score liftered rows, a' = sat16(trunc(a * DTW_LIFTER_W[c] / 16))
+DTW_LIFTER_W = (10, 16, 21, 25, 27, 28, 27, 25, 21, 16, 10, 4)   # SR_DTW_LIFTER_W
 ST_OK, ST_VAD_FAIL, ST_MFCC_FAIL, ST_REJECT = 0, 1, 2, 3
 
 
@@ -380,7 +382,7 @@ class Handle:
     def dtw(self, ftr_in, flags=0, band_r=0, want_score=True, want_best=True):
         """every input against the bank (sr_dtw_batch): flags 0 = the greedy walk, DTW_BAND = the banded DP (| DTW_ANY_RATE:
         without the 2:1 length guard), DTW_SYM_P1 = the symmetric P = 1 DP, at radius band_r, each optionally |
-        DTW_CHECK_SIGN -> (score [B, n_slot], best_idx [B],
+        DTW_CHECK_SIGN and | DTW_LIFTER (liftered rows) -> (score [B, n_slot], best_idx [B],
         best_dis [B]), None where not wanted"""
         B = ftr_in.shape[0]
         score = np.zeros((B, self.n_slot), np.uint32) if want_score else None
@@ -639,7 +641,7 @@ class Handle:
         any of them | dtw_knn(k) decides by each command's score e_c, the floor of the mean of its min(k, n_c) smallest
         scores other than DIS_ERR (n_c of them), with the winner's nearest slot as best_idx and e_cmd as best_dis;
         any of them | dtw_reject(q) turns down (ST_REJECT) a decision whose runner-up command is less than q per mille worse
-        (under dtw_knn, by the commands' e_c)"""
+        (under dtw_knn, by the commands' e_c); any of them | DTW_LIFTER scores the liftered rows of inputs and templates"""
         self._ck(lib().sr_set_match(self._h, int(flags), int(band_r)))
 
     def match(self):

@@ -8,13 +8,15 @@ the cells the banded oracle evaluates at the same radius on a sample of utteranc
 time. r = 15 and r = 16 sit on either side of the kernel choice (warp-scan form / whole-row form) and are run alternately,
 several rounds; the symmetric rows and the banded rows without the guard at r = 10, 16 and 118 alternate with the banded
 rows at the same radii. The cells of those rows are the guarded banded DP's, so their cells per second compare the same
-work. A sample of every
+work. The lifter rows (SR_DTW_LIFTER) run the greedy walk, the banded DP at r = 10 and 16, the banded DP without the guard
+at r = 118 and the symmetric DP at r = 10 with the bit off and on, alternately, several rounds; they do the same DP work,
+so their difference is the cost of liftering each staged row. --rows lifter runs those rows alone. A sample of every
 matcher's outputs -- the first utterances of the launch and its last ones -- is checked against the oracle's own
 composition: its front end (recognise_pinned), its template scan under the same matcher (oracle_ext/sym.c for the symmetric DP,
-oracle_ext/rate.c for the banded DP without the guard),
+oracle_ext/rate.c for the banded DP without the guard, under SR_DTW_LIFTER on liftered rows: tests/lifter_ref.py),
 the strict '<' first-wins argmin. The card's name, power limit and SM clock limit are read in the same run.
 
-    python tools/bench_match.py [--steps 20] [--warmup 3] [--rounds 3] [--json FILE]
+    python tools/bench_match.py [--steps 20] [--warmup 3] [--rounds 3] [--rows all|lifter] [--json FILE]
 """
 import argparse
 import json
@@ -29,7 +31,7 @@ sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python")
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
+import lifter_ref  # noqa: E402
 import sr_b200  # noqa: E402
 
 U, N_LEN = 8000, 2400
@@ -56,6 +58,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3, help="alternating rounds of r = 15 and r = 16")
     ap.add_argument("--sample", type=int, default=256, help="first utterances checked against the oracle")
     ap.add_argument("--tail", type=int, default=32, help="last utterances checked against the oracle")
+    ap.add_argument("--rows", choices=("all", "lifter"), default="all", help="every matcher's rows, or the lifter rows alone")
     ap.add_argument("--json", default=None, help="also write the results to this file")
     args = ap.parse_args()
 
@@ -96,12 +99,13 @@ def main():
     good = front["status"] == 0
     SYM = sr_b200.DTW_SYM_P1
     RATE = sr_b200.DTW_BAND | sr_b200.DTW_ANY_RATE
+    LIFT = sr_b200.DTW_LIFTER
 
     def oracle(flags, r):
         """the matcher's scores, and the cells of the port's greedy or banded DP at the same radius"""
-        _, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r if flags else -1,
+        _, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r if flags & ~LIFT else -1,
                                        nthreads=os.cpu_count() or 1)
-        return ox.match_scores(front["ftr"][good], bank_h, T, flags, r), cells
+        return lifter_ref.match_scores(front["ftr"][good], bank_h, T, flags, r), cells
 
     def run(flags, r):
         h.set_match(flags, r)
@@ -119,7 +123,7 @@ def main():
         stream.synchronize()
         recs = h.timing_collect()
         h.timing_enable(0)
-        tag = 14 if flags == SYM else 6 if flags else 4
+        tag = 14 if flags & SYM else 6 if flags & sr_b200.DTW_BAND else 4
         dtw_ms = [ms for t, ms in recs if t == tag]
         assert len(dtw_ms) == args.steps, (flags, r, len(dtw_ms))
         # outputs of the last step against the oracle on the sample
@@ -133,8 +137,9 @@ def main():
               and np.array_equal(got["best_dis"][good].view(np.uint32), sc[np.arange(len(i)), i])
               and np.array_equal(got["cmd"][good].view(np.uint32), i // 4))
         cells_batch = cells * B / len(rows)
-        name = "greedy" if not flags else "sym" if flags == SYM else "band-any" if flags == RATE else "band"
-        return {"matcher": name, "r": r if flags else None,
+        m = flags & ~LIFT
+        name = ("greedy" if not m else "sym" if m == SYM else "band-any" if m == RATE else "band") + ("+lift" if flags & LIFT else "")
+        return {"matcher": name, "r": r if m else None,
                 "ms_per_step": ev0.elapsed_time(ev1) / args.steps,
                 "dtw_ms_mean": float(np.mean(dtw_ms)), "dtw_ms_min": float(np.min(dtw_ms)), "dtw_ms_max": float(np.max(dtw_ms)),
                 "oracle_cells_per_step": cells_batch, "cells_per_s": cells_batch / (float(np.mean(dtw_ms)) * 1e-3),
@@ -143,6 +148,9 @@ def main():
     band = sr_b200.DTW_BAND
     plan = [(0, 0), (band, 10)] + [(band, r) for _ in range(args.rounds) for r in (15, 16)] + [(band, 32), (band, 118), (0, 0)]
     plan += [(f, r) for _ in range(args.rounds) for r in (10, 16, 118) for f in (band, SYM, RATE)]
+    lifter_plan = [(f | lift, r) for _ in range(args.rounds) for f, r in ((0, 0), (band, 10), (band, 16), (RATE, 118), (SYM, 10))
+                   for lift in (0, LIFT)]
+    plan = lifter_plan if args.rows == "lifter" else plan + lifter_plan
     results = [run(f, r) for f, r in plan]
     h.set_match(0, 0)
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "batch": B, "templates": T,
@@ -150,9 +158,9 @@ def main():
             "results": results}
     print("card: %s, power limit %s, max SM clock %s" % (info["card"].get("name"), info["card"].get("power.limit"),
                                                         info["card"].get("clocks.max.sm")))
-    print("%-9s %5s %10s %12s %22s %10s %6s" % ("matcher", "r", "ms/step", "dtw ms mean", "dtw ms min-max", "Gcells/s", "oracle"))
+    print("%-14s %5s %10s %12s %22s %10s %6s" % ("matcher", "r", "ms/step", "dtw ms mean", "dtw ms min-max", "Gcells/s", "oracle"))
     for x in results:
-        print("%-9s %5s %10.3f %12.3f %10.3f-%-11.3f %10.2f %6s" % (
+        print("%-14s %5s %10.3f %12.3f %10.3f-%-11.3f %10.2f %6s" % (
             x["matcher"], "" if x["r"] is None else x["r"], x["ms_per_step"], x["dtw_ms_mean"], x["dtw_ms_min"],
             x["dtw_ms_max"], x["cells_per_s"] / 1e9, x["sample_equals_oracle"]))
     print(json.dumps(info))
