@@ -111,10 +111,9 @@ int sr_set_dtw_variant(sr_handle *h, int variant) {
 }
 
 int sr_set_match(sr_handle *h, uint32_t flags, int band_r) {
-    // the matcher; bits 8-10 are the KNN rule SR_DTW_KNN(k), bit 13 the lifter, bits 16-31 the margin rule SR_DTW_REJECT(q)
-    const uint32_t m = flags & 0xFFFFu & ~SR_DTW_KNN(7) & ~SR_DTW_LIFTER;
-    SR_REQUIRE(h, h && (m == 0 || m == SR_DTW_BAND || m == (SR_DTW_BAND | SR_DTW_ANY_RATE) || m == SR_DTW_SYM_P1) &&
-                      rule_knn(flags) <= SR_FTR_PER_COMM && band_r >= 0);
+    // the matcher, the lifter and the decision rules; the recognition calls add SR_DTW_CHECK_SIGN themselves
+    ScanPlan p;
+    SR_REQUIRE(h, h && !(flags & SR_DTW_CHECK_SIGN) && scan_plan(flags, band_r, 0, true, &p));
     h->match_flags = flags;
     h->match_r = band_r;
     return 0;
@@ -181,17 +180,6 @@ void sr_host_free(void *p) {
 int sr_host_numa_node(const void *p) { return p ? numa_node_of_page(p) : -1; }
 
 // ---- kernel launches (launch_on, sr_internal.h) --------------------------------------------------------------------
-// the timing tag of the template scan under flags (launch_scan's choice)
-static int scan_tag(u32 flags) {
-    return (flags & SR_DTW_SYM_P1) ? TAG_DTW_SYM : (flags & SR_DTW_BAND) ? TAG_DTW_BAND : TAG_DTW;
-}
-// the matcher bits of sr_dtw_batch* name one matcher: not SR_DTW_SYM_P1 with SR_DTW_BAND, and SR_DTW_ANY_RATE only
-// as a modifier of SR_DTW_BAND
-// (the margin rule's bits are the recognition calls' own: sr_dtw_batch* refuse them before this is asked)
-static bool scan_flags_ok(u32 flags) {
-    return !((flags & SR_DTW_SYM_P1) && (flags & SR_DTW_BAND)) && (!(flags & SR_DTW_ANY_RATE) || (flags & SR_DTW_BAND));
-}
-
 int sr_timing_enable(sr_handle *h, uint32_t max_records) {
     SR_REQUIRE(h, h != nullptr);
     DeviceGuard g(h->device);
@@ -438,49 +426,46 @@ int sr_mfcc_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
 
 }  // extern "C"
 
-// main.c:276-291 on n inputs (n_dev: n on the device): w's n argmin keys, then under a decision rule (C > 0) n * C
-// keys (rule_cols), set to their start (tag 3), and the template scan into them (4, 6 or 14); no w: it writes scores only
-static int scan_to_keys(sr_handle *h, DevBuf *w, u32 C, const BankView &bank, const void *in, u32 n, u32 flags, int band_r,
-                        u32 *score, const u8 *status, u64 *&keys, const u32 *n_dev = nullptr) {
+// main.c:276-291 on n inputs (n_dev: n on the device) under plan p: w's n argmin keys, then under a decision rule
+// (p.rule.C > 0) n * C keys, set to their start (tag 3), and the template scan into them (p.tag); no w: it writes scores
+// only
+static int scan_to_keys(sr_handle *h, DevBuf *w, const ScanPlan &p, const BankView &bank, const void *in, u32 n, u32 *score,
+                        const u8 *status, u64 *&keys, const u32 *n_dev = nullptr) {
+    const u32 C = p.rule.C;
     keys = nullptr;
     if (w) {
         SR_CK(h, ensure(*w, (size_t)n * (1 + C) * 8));
         keys = static_cast<u64 *>(w->p) + (C ? n : 0);
         SR_LAUNCH(h, TAG_BEST_INIT, launch_best_init(keys, (u64)n * (C ? C : 1), h->stream));
     }
-    if (bank.n) {
-        if (flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) SR_REQUIRE(h, band_r >= 0);
-        SR_LAUNCH(h, scan_tag(flags), launch_scan(h, bank, in, n, flags, band_r, score, keys, status, n_dev));
-    }
+    if (bank.n) SR_LAUNCH(h, p.tag, launch_scan(h, p, scan_args(p, bank, in, n, score, keys, status, n_dev)));
     return 0;
 }
 
-// the template scan of B inputs against `bank`, then the argmin of each when one of best_idx / best_dis / cmd is wanted
+// the template scan of B inputs against `bank`, then the argmin of each when one of best_idx / best_dis / cmd is wanted.
+// With a status (the recognition calls) the flags may carry a decision rule, and the status is an output of its decision
+// too; without one (sr_dtw_batch*) they may not.
 static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r,
                         uint32_t *score, uint32_t *best_idx, uint32_t *best_dis, uint32_t *cmd, const u8 *status) {
     SR_REQUIRE(h, h && (B == 0 || in));
     SR_REQUIRE(h, (reinterpret_cast<uintptr_t>(in) & 3) == 0);
-    SR_REQUIRE(h, scan_flags_ok(flags));
+    ScanPlan p;                                                             // no input: no template is scanned
+    SR_REQUIRE(h, scan_plan(flags, band_r, B ? bank.n : 0, status != nullptr, &p));
     if (B == 0) return 0;
-    // under a decision rule (C > 0) the status is an output of the decision too. Without a status (sr_dtw_batch*) the
-    // rule bits, and the bits 4-15 other than SR_DTW_LIFTER that they accept and ignore, never reach a kernel
-    const u32 C = status ? rule_cols(flags, bank.n) : 0;
-    if (!C) flags &= kMatcherBits;
-    const bool want_best = best_idx || best_dis || cmd || C;
+    const bool want_best = best_idx || best_dis || cmd || p.rule.C;
     DevBuf &bb = h->best_sel ? h->best_alt : h->best;
     u64 *keys;
-    if (const int rc = scan_to_keys(h, want_best ? &bb : nullptr, C, bank, in, B, flags, band_r, score, status, keys)) return rc;
+    if (const int rc = scan_to_keys(h, want_best ? &bb : nullptr, p, bank, in, B, score, status, keys)) return rc;
     u64 *best = static_cast<u64 *>(bb.p);
     if (want_best)
-        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, keys, B, C, rule_q(flags), rule_knn(flags), best_idx, best_dis, cmd,
-                                                       const_cast<u8 *>(status), h->stream));
+        SR_LAUNCH(h, TAG_BEST_FINAL, launch_best_final(best, keys, B, p.rule, best_idx, best_dis, cmd, const_cast<u8 *>(status),
+                                                       h->stream));
     return 0;
 }
 
 extern "C" int sr_dtw_batch_dev(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                                 uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h != nullptr);
-    SR_REQUIRE(h, (flags >> 16) == 0);                                      // no status to report a rejection in
     DeviceGuard g(h->device);
     return dtw_dev_impl(h, h->bank, in, B, flags, band_r, score, best_idx, best_dis, nullptr, nullptr);
 }
@@ -617,9 +602,9 @@ int sr_mfcc_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, con
 int sr_dtw_batch(sr_handle *h, const v_ftr_tag *in, uint32_t B, uint32_t flags, int band_r, uint32_t *score,
                  uint32_t *best_idx, uint32_t *best_dis) {
     SR_REQUIRE(h, h && (B == 0 || in));
-    SR_REQUIRE(h, scan_flags_ok(flags) && (flags >> 16) == 0);             // before any copy: nothing is written
+    ScanPlan p;                                                             // before any copy: nothing is written
+    SR_REQUIRE(h, scan_plan(flags, band_r, B ? h->bank.n : 0, false, &p));
     if (B == 0) return 0;
-    if (h->bank.n && (flags & (SR_DTW_BAND | SR_DTW_SYM_P1))) SR_REQUIRE(h, band_r >= 0);   // dtw_dev_impl's radius rule
     HostCall c(h, "sr_dtw_batch");
     return dtw_host(c, h->bank, in, B, flags, band_r, score, best_idx, best_dis);
 }
@@ -1238,11 +1223,11 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
     SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, M, seg2, 2, atap_seg, ftr, row, B, n_flat));     // main.c:268
     SR_LAUNCH(h, TAG_STATUS, launch_long_status(seg2, ftr, n_flat, M, status, h->stream));          // main.c:261-274
     // main.c:276-291, save_sign honoured (main.c:283); a decision rule's key rows in lng[6]
-    const u32 flags = SR_DTW_CHECK_SIGN | h->match_flags, C = rule_cols(flags, h->bank.n);
+    ScanPlan p;
+    scan_plan(SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, h->bank.n, true, &p);    // flags sr_set_match accepted
     u64 *keys;
-    if (const int rc = scan_to_keys(h, &h->lng[6], C, h->bank, ftr, M, flags, h->match_r, nullptr, status, keys, n_flat)) return rc;
-    SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, keys, n_flat, M, rec, C, rule_q(h->match_flags),
-                                                     rule_knn(h->match_flags), h->stream));                                   // main.c:292-294
+    if (const int rc = scan_to_keys(h, &h->lng[6], p, h->bank, ftr, M, nullptr, status, keys, n_flat)) return rc;
+    SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, keys, n_flat, M, rec, p.rule, h->stream));   // main.c:292-294
     return 0;
 }
 

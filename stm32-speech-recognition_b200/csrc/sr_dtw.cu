@@ -9,7 +9,10 @@
 // (flattened), so lanes stay busy when Tt < 32 (the host picks NU/Wg for the tile width).
 // dtw_limit is evaluated as a per-column y interval (ya, yb) updated only when x moves. Rows, header decode, the walk and
 // the epilogue are the shared core of sr_dtw_core.cuh.
-#include "sr_dtw_core.cuh"
+// Every template-scan kernel takes one ScanArgs; scan_plan and launch_scan at the end of this file are the one place the
+// matcher flags are decoded and a matcher becomes a kernel launch.
+#include "sr_internal.h"
+#include "sr_dtw_dyn.cuh"
 
 namespace srk {
 
@@ -25,25 +28,26 @@ __device__ __forceinline__ void group_barrier(int id, int nthreads) {
 // The lane-packed tile scan of dtw_kernel and dtw_band_thread_kernel. A CTA stages a tile of Tt <= 32 templates; its
 // warps, in G groups of Wg, stage NU utterances at a time, and each lane of a group scores one fixed (utterance slot,
 // template) pair of the NU x Tt (flattened), so lanes stay busy when Tt < 32. pair(I, M, urow, trow) scores a pair
-// that passed pair_walks(guard). kLift: inputs and templates staged liftered (SR_DTW_LIFTER).
+// that passed pair_walks(guard). kLift: inputs and templates staged liftered (SR_DTW_LIFTER). tslots: template slots
+// allocated in shared memory. The pointers are the kernel's (SCAN_PTRS).
 template <bool kLift, class Pair>
-__device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
-                                                 u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status, int Wg,
-                                                 int NU, int G, u32 tile0, int tslots, const u32 *B_dev, const u32 *perm,
-                                                 bool guard, Pair pair) {
+__device__ __forceinline__ void lane_packed_scan(const ScanArgs &a, const unsigned char *in_ftr, const unsigned char *bank,
+                                                 const u8 *status, const u32 *B_dev, const u32 *perm, u32 *score, u64 *best,
+                                                 int Wg, int NU, int G, u32 tile0, int tslots, bool guard, Pair pair) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
+    u32 B = a.B;
     if (B_dev) B = min(B, *B_dev);
     if (B == 0) return;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const u32 t0 = (blockIdx.x + tile0) * kTileT;
-    const int Tt = (int)min((u32)kTileT, T - t0);
+    const int Tt = (int)min((u32)kTileT, a.T - t0);
     unsigned char *tile = smem_raw;                                                // Tt slots
     u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)tslots * kSlotBytes);
     unsigned char *uslots = smem_raw + (size_t)tslots * kSlotBytes + kTileHdr;     // G*NU slots
     u32 *ufrm = reinterpret_cast<u32 *>(uslots + (size_t)G * NU * kSlotBytes);     // [G*NU]
 
-    stage_tile<kLift>(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane,
-                      kK2Warps);
+    stage_tile<kLift>(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, a.slot_stride, a.check_sign, perm, t0, Tt, warp,
+                      lane, kK2Warps);
     __syncthreads();
 
     const int group = warp / Wg, wig = warp - group * Wg;
@@ -63,7 +67,7 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
             u32 frm = kNoWalk;
             if (u < B && !(status && status[u] != SR_ST_OK)) {        // VAD/MFCC failed: spch_recg returns before dtw
                 const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
-                frm = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
+                frm = decode_frm(*reinterpret_cast<const u32 *>(uf), false);
                 stage_planes<kLift>(gslots + (size_t)s * kSlotBytes, kNrm119, uf, staged_rows(frm), gtid, gthreads);
             }
             if (gtid == 0) gfrm[s] = frm;
@@ -76,7 +80,7 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
             const u32 result = pair_walks(Iraw, Mraw, guard) ? pair((int)Iraw, (int)Mraw, gslots + (size_t)ul * kSlotBytes, trow)
                                                       : SR_DIS_ERR;
             const u32 t = perm ? tfrm[kTileT + tl] : t0 + (u32)tl;   // the original slot number: score column, argmin key
-            emit_pair(score, best, T, u, t, result, flags);
+            emit_pair(score, best, a, u, t, result);
         }
         group_barrier(1 + group, gthreads);                                                          // before restaging
     }
@@ -84,15 +88,12 @@ __device__ __forceinline__ void lane_packed_scan(const unsigned char *in_ftr, u3
 
 template <bool kLift>
 __global__ void __launch_bounds__(kK2Warps * 32)
-dtw_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-           u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best,
-           const u8 *__restrict__ status /* may be NULL: per-utterance SR_ST_* gate of sr_recognise */,
-           int Wg, int NU, int G, u32 tile0, int tslots /* template slots allocated in shared memory */,
-           const u32 *__restrict__ B_dev /* optional: batch size produced on the device (streaming) */,
-           const u32 *__restrict__ perm /* optional: bank slots in ascending frm_num order (templates of a tile then have
-                                           similar walk lengths); results are indexed by the ORIGINAL slot number */) {
-    lane_packed_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
-                            true, [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+dtw_kernel(const __grid_constant__ ScanArgs a, const unsigned char *__restrict__ in_ftr, const unsigned char *__restrict__ bank,
+           const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm,
+           u32 *__restrict__ score, u64 *__restrict__ best, int Wg, int NU, int G, u32 tile0,
+           int tslots) {
+    lane_packed_scan<kLift>(a, in_ftr, bank, status, B_dev, perm, score, best, Wg, NU, G, tile0, tslots, true,
+                            [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
                          PRow i0, i1, m0, m1;
                          u32 dis, steps;
                          int X1, X2, x, y, ya0, yb0, ya1, yb1;
@@ -110,17 +111,17 @@ __global__ void best_init_kernel(u64 *best, u32 B) {
     if (i < B) best[i] = kKeyStart;
 }
 // The decision of each of B utterances (decide) into the fields NULL does not mark as unwanted (NULL status: every
-// utterance OK). Without a rule the keys are best's; under one (kRule) they are rows of C keys (key_of), and the decision's
-// key goes to best[i] (what an all-gather reads) and SR_ST_REJECT into status. The rule's arguments come last.
+// utterance OK). Without a rule the keys are best's; under one (kRule) they are rows of C keys (ScanArgs), and the
+// decision's key goes to best[i] (what an all-gather reads) and SR_ST_REJECT into status. The rule comes last.
 template <bool kRule>
 __global__ void best_final_kernel(const u64 *keys, u32 B, u32 *best_idx, u32 *best_dis, u32 *cmd, u8 *status, u64 *best,
-                                  u32 C, u32 q, u32 knn) {
-    const u32 g = kRule ? rule_lanes(C, knn) : 1u;
+                                  Rule rl) {
+    const u32 g = kRule ? rule_lanes(rl) : 1u;
     const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / g;
     if (i >= B) return;                                                         // whole warps: B * g threads
     const u32 st = status ? status[i] : SR_ST_OK;
     Decision d;
-    if (!decide<kRule>(keys, i, st, C, q, knn, g, d)) return;
+    if (!decide<kRule>(keys, i, st, rl, g, d)) return;
     if constexpr (kRule) {
         best[i] = d.key;
         if (d.status != st) status[i] = (u8)d.status;
@@ -275,31 +276,17 @@ static LanePlan plan_lanes(int Tt) {
     return p;
 }
 
-cudaError_t launch_dtw(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
-                       u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev, const u32 *perm) {
-    if (B == 0 || T == 0) return cudaSuccess;
-    auto *kernel = (flags & SR_DTW_LIFTER) ? dtw_kernel<true> : dtw_kernel<false>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e != cudaSuccess) return e;
-    return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
-        const LanePlan p = plan_lanes(Tt);
-        kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32, p.smem, st>>>(
-            static_cast<const unsigned char *>(in_ftr), B, static_cast<const unsigned char *>(bank), T, slot_stride, flags,
-            score, best, status, p.Wg, p.NU, p.G, tile0, Tt, B_dev, perm);
-        return cudaGetLastError();
-    });
-}
 cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (n > 0xFFFFFF00ull) return cudaErrorInvalidValue;            // 32 GB of keys: past any workspace anyway
     best_init_kernel<<<(u32)((n + 255) / 256), 256, 0, st>>>(best, (u32)n);
     return cudaGetLastError();
 }
-cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
-                              u32 *cmd, u8 *status, cudaStream_t st) {
+cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, const Rule &rl, u32 *best_idx, u32 *best_dis, u32 *cmd,
+                              u8 *status, cudaStream_t st) {
     if (B == 0) return cudaSuccess;
-    (C ? best_final_kernel<true> : best_final_kernel<false>)<<<rule_grid(B, C, knn), 256, 0, st>>>(
-        keys, B, best_idx, best_dis, cmd, status, best, C, q, knn);
+    (rl.C ? best_final_kernel<true> : best_final_kernel<false>)<<<rule_grid(B, rl), 256, 0, st>>>(
+        keys, B, best_idx, best_dis, cmd, status, best, rl);
     return cudaGetLastError();
 }
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st) {
@@ -318,11 +305,11 @@ cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStre
 // ---- K3: Sakoe-Chiba banded DP (EXTENSION: not in the reference, whose dtw() is the greedy walk above;
 // BASELINE.json configs[2] names it; checked against our own CPU DP oracle sro_dtw_band -- parity unpinned
 // by the reference). D(i,j) = d(i,j) + min(D(i-1,j), D(i,j-1), D(i-1,j-1)), band |j - floor(i*M/I)| <= r,
-// local distance = get_dis, result D(I-1,M-1)/(I+M), same 2:1 length guard as DTW.C:133 unless flags has
-// SR_DTW_ANY_RATE. Without the guard the band centre c = floor(i*M/I) moves by up to 118 columns per row (M > 2I), not
+// local distance = get_dis, result D(I-1,M-1)/(I+M), same 2:1 length guard as DTW.C:133 unless the plan turns it off
+// (SR_DTW_ANY_RATE). Without the guard the band centre c = floor(i*M/I) moves by up to 118 columns per row (M > 2I), not
 // 0..2, and stays put for several rows when M < I/2; every kernel below takes any shift, and a shift past 2r + 1 leaves
 // the new row unreachable.
-// Three kernels, chosen from r alone (launch_dtw_band): dtw_band_thread_kernel<10> for r = 10, dtw_band_kernel for the
+// Three kernels, chosen from r alone (launch_scan): dtw_band_thread_kernel<10> for r = 10, dtw_band_kernel for the
 // other r <= 15, dtw_wide_kernel for r >= 16 up to the full matrix. On the recognition path all three take the
 // per-utterance status gate, a batch size produced on the device (streaming) and the bank order; scores and argmin keys
 // stay under the original slot number.
@@ -337,27 +324,29 @@ constexpr s32 kInf = 0x3FFFFFFF;
 // slot perm[t] when a bank order is given); each warp stages one utterance at a time and scores it against the Tt
 // templates one after another, the whole warp on one cost matrix: pair(I, M, urow, trow, lane) returns, in every lane, the
 // score of a pair that passed pair_walks(guard). Lane tt keeps the score of template tt; one score row and one atomicMin
-// of the warp's smallest key per utterance (under the margin rule, one per lane into its command's key). An utterance whose status is not SR_ST_OK scores SR_DIS_ERR, as in
+// of the warp's smallest key per utterance (under a decision rule, one per lane into its key of the row). An utterance
+// whose status is not SR_ST_OK scores SR_DIS_ERR, as in
 // lane_packed_scan. kLift: inputs and templates staged liftered (SR_DTW_LIFTER).
 template <bool kLift, class Pair>
-__device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 B, const unsigned char *bank, u32 T,
-                                               u32 slot_stride, u32 flags, u32 *score, u64 *best, const u8 *status,
-                                               const u32 *B_dev, const u32 *perm, bool guard, Pair pair) {
+__device__ __forceinline__ void warp_pair_scan(const ScanArgs &a, const unsigned char *in_ftr, const unsigned char *bank,
+                                               const u8 *status, const u32 *B_dev, const u32 *perm, u32 *score, u64 *best,
+                                               bool guard, Pair pair) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
+    u32 B = a.B;
     if (B_dev) B = min(B, *B_dev);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const u32 t0 = blockIdx.x * kTileT;
-    const int Tt = (int)min((u32)kTileT, T - t0);
+    const int Tt = (int)min((u32)kTileT, a.T - t0);
     unsigned char *tile = smem_raw;                                               // byte-plane slots, as in dtw_kernel
     u32 *tfrm = reinterpret_cast<u32 *>(smem_raw + (size_t)kTileT * kSlotBytes);  // [32] frame counts, [32] slot numbers
     unsigned char *uslot = smem_raw + (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)warp * kSlotBytes;
-    stage_tile<kLift>(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, slot_stride, flags, perm, t0, Tt, warp, lane,
-                      kDtwWarps);
+    stage_tile<kLift>(tile, kSlotBytes, kNrm119, tfrm, tfrm + kTileT, bank, a.slot_stride, a.check_sign, perm, t0, Tt, warp,
+                      lane, kDtwWarps);
     __syncthreads();
     for (u32 u = blockIdx.y * kDtwWarps + warp; u < B; u += gridDim.y * kDtwWarps) {
         const unsigned char *uf = in_ftr + (size_t)u * kFtrBytes;
         u32 Iraw = kNoWalk;                               // VAD/MFCC failed: spch_recg returns before dtw
-        if (!(status && status[u] != SR_ST_OK)) Iraw = decode_frm(*reinterpret_cast<const u32 *>(uf), 0);
+        if (!(status && status[u] != SR_ST_OK)) Iraw = decode_frm(*reinterpret_cast<const u32 *>(uf), false);
         __syncwarp();
         stage_planes<kLift>(uslot, kNrm119, uf, staged_rows(Iraw), lane, 32);
         __syncwarp();
@@ -371,9 +360,9 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
         }
         const bool has_t = lane < Tt;
         const u32 t = !has_t ? 0u : perm ? tfrm[kTileT + lane] : t0 + (u32)lane;   // the original slot number
-        if (has_t && score) score[(size_t)u * T + t] = my_result;
-        if (best && key_rows(flags)) {                     // a decision rule: each lane its own key of the row
-            if (has_t) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, flags, T, u, t)),
+        if (has_t && score) score[(size_t)u * a.T + t] = my_result;
+        if (best && key_rows(a)) {                         // a decision rule: each lane its own key of the row
+            if (has_t) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, a, u, t)),
                                  (unsigned long long)(((u64)my_result << 32) | (u64)t));
         } else if (best) {
             u64 key = has_t ? (((u64)my_result << 32) | (u64)t) : ~0ull;
@@ -386,13 +375,13 @@ __device__ __forceinline__ void warp_pair_scan(const unsigned char *in_ftr, u32 
 
 template <bool kLift>
 __global__ void __launch_bounds__(kDtwWarps * 32)
-dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
-                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
+dtw_band_kernel(const __grid_constant__ ScanArgs a, const unsigned char *__restrict__ in_ftr, const unsigned char *__restrict__ bank,
+                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm,
+                u32 *__restrict__ score, u64 *__restrict__ best) {
     // the previous row's cell of column j sits in lane j - (cprev - r): up and diag come from lanes lane + sft and
     // lane + sft - 1, and any lane past 31 or past 2r (those hold kInf) is out of the previous row's band, whatever sft is
-    warp_pair_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
-                   [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
+    warp_pair_scan<kLift>(a, in_ftr, bank, status, B_dev, perm, score, best, a.guard,
+                          [r = a.r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         s32 Dprev = kInf;
         int cprev = 0;
         for (int i = 0; i < I; ++i) {
@@ -436,11 +425,11 @@ dtw_band_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 // stay in registers for the whole pair.
 template <bool kLift>
 __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
-dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-                u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
-                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, !(flags & SR_DTW_ANY_RATE),
-                   [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
+dtw_wide_kernel(const __grid_constant__ ScanArgs a, const unsigned char *__restrict__ in_ftr, const unsigned char *__restrict__ bank,
+                const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm,
+                u32 *__restrict__ score, u64 *__restrict__ best) {
+    warp_pair_scan<kLift>(a, in_ftr, bank, status, B_dev, perm, score, best, a.guard,
+                          [r = a.r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         const int j0 = lane * 4;
         PRow b[4];
         s32 D[4];
@@ -474,12 +463,12 @@ dtw_wide_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned 
 // after the two, so the passes of a pair total at most M - 1, and a slide past W leaves no cell of the old row.
 template <int R, bool kLift>
 __global__ void __launch_bounds__(kK2Warps * 32)
-dtw_band_thread_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-                       u32 slot_stride, u32 flags, u32 *__restrict__ score, u64 *__restrict__ best,
-                       const u8 *__restrict__ status, int Wg, int NU, int G, u32 tile0, int tslots,
-                       const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    lane_packed_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, Wg, NU, G, tile0, tslots, B_dev, perm,
-                            !(flags & SR_DTW_ANY_RATE), [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
+dtw_band_thread_kernel(const __grid_constant__ ScanArgs a, const unsigned char *__restrict__ in_ftr, const unsigned char *__restrict__ bank,
+                       const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm,
+                       u32 *__restrict__ score, u64 *__restrict__ best, int Wg, int NU,
+                       int G, u32 tile0, int tslots) {
+    lane_packed_scan<kLift>(a, in_ftr, bank, status, B_dev, perm, score, best, Wg, NU, G, tile0, tslots, a.guard,
+                            [](int I, int M, const unsigned char *urow, const unsigned char *trow) {
         constexpr int W = 2 * R + 1;
         if (I == 0 || M == 0) return SR_DIS_ERR;           // empty feature sets: no cell
         s32 D[W];
@@ -557,11 +546,11 @@ constexpr s32 kSymInf = 1 << 26;
 
 template <bool kLift>
 __global__ void __launch_bounds__(kDtwWarps * 32, 1)       // one CTA per SM (shared memory): up to 128 registers
-dtw_sym_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned char *__restrict__ bank, u32 T,
-               u32 slot_stride, u32 flags, int r, u32 *__restrict__ score, u64 *__restrict__ best,
-               const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm) {
-    warp_pair_scan<kLift>(in_ftr, B, bank, T, slot_stride, flags, score, best, status, B_dev, perm, true,
-                   [r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
+dtw_sym_kernel(const __grid_constant__ ScanArgs a, const unsigned char *__restrict__ in_ftr, const unsigned char *__restrict__ bank,
+               const u8 *__restrict__ status, const u32 *__restrict__ B_dev, const u32 *__restrict__ perm,
+               u32 *__restrict__ score, u64 *__restrict__ best) {
+    warp_pair_scan<kLift>(a, in_ftr, bank, status, B_dev, perm, score, best, true,
+                          [r = a.r](int I, int M, const unsigned char *uslot, const unsigned char *trow, int lane) {
         const int j0 = lane * 4;
         PRow b[4];
         s32 g1[4], g2[4], dp[4];                                       // g(i-1, .), g(i-2, .), d(i-1, .) of the lane's columns
@@ -603,58 +592,103 @@ dtw_sym_kernel(const unsigned char *__restrict__ in_ftr, u32 B, const unsigned c
     });
 }
 
-// the symmetric P = 1 DP at radius band_r >= 0: one kernel for every r, clamped to 118 as in launch_dtw_band
-cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
-                           u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev,
-                           const u32 *perm) {
-    if (B == 0 || T == 0) return cudaSuccess;
-    if (band_r < 0) return cudaErrorInvalidValue;
-    const int r = min(band_r, (int)kMaxFrm - 1);
-    const size_t smem = (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)kDtwWarps * kSlotBytes;
-    auto *kernel = (flags & SR_DTW_LIFTER) ? dtw_sym_kernel<true> : dtw_sym_kernel<false>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const u32 tiles = (T + kTileT - 1) / kTileT;
-    dim3 grid(tiles, grid_rows(num_sms, tiles, B, kDtwWarps));
-    kernel<<<grid, kDtwWarps * 32, smem, st>>>(static_cast<const unsigned char *>(in_ftr), B,
-                                                       static_cast<const unsigned char *>(bank), T, slot_stride, flags, r,
-                                                       score, best, status, B_dev, perm);
-    return cudaGetLastError();
+}  // namespace srk
+
+// ---- the one decode of the matcher flags, and the one launcher of the template scan ---------------------------------
+bool scan_plan(u32 flags, int band_r, u32 T, bool rules, ScanPlan *out) {
+    static_assert(SR_FTR_PER_COMM == 4, "the margin rule's key column is t >> 2");
+    // one matcher: the greedy walk, the banded DP with or without SR_DTW_ANY_RATE, or the symmetric DP
+    const u32 m = flags & (SR_DTW_BAND | SR_DTW_SYM_P1 | SR_DTW_ANY_RATE);
+    if (m != 0 && m != SR_DTW_BAND && m != (SR_DTW_BAND | SR_DTW_ANY_RATE) && m != SR_DTW_SYM_P1) return false;
+    const u32 knn = (flags >> 8) & 7u, q = flags >> 16;                // SR_DTW_KNN(k), SR_DTW_REJECT(q)
+    if (rules) {
+        // sr_set_match's word: of bits 4-15 only the KNN rule's (k <= SR_FTR_PER_COMM) and the lifter; a radius >= 0
+        if ((flags & 0xFFF0u & ~SR_DTW_KNN(7) & ~SR_DTW_LIFTER) || knn > SR_FTR_PER_COMM || band_r < 0) return false;
+    } else {
+        // sr_dtw_batch*: no status to report a rejection in, so no bit >= 16, and bits 4-15 other than the lifter are
+        // ignored; a DP's radius must be >= 0 once there are templates to scan
+        if (q || (m && T && band_r < 0)) return false;
+    }
+    ScanPlan &p = *out;
+    p.matcher = (m & SR_DTW_SYM_P1) ? ScanPlan::kSym : m ? ScanPlan::kBand : ScanPlan::kGreedy;
+    p.tag = (m & SR_DTW_SYM_P1) ? TAG_DTW_SYM : m ? TAG_DTW_BAND : TAG_DTW;
+    p.check_sign = flags & SR_DTW_CHECK_SIGN;
+    p.guard = !(flags & SR_DTW_ANY_RATE);
+    p.lift = flags & SR_DTW_LIFTER;
+    // every r >= 118 is the full matrix (|j - c| <= 118 for any two columns), so no r reaches the kernels' c +- r
+    p.r = min(band_r, (int)kMaxFrm - 1);
+    // under a rule the scan writes a row of C keys per input: one per command for the margin rule alone, one per slot for
+    // the KNN rule (ScanArgs); no rule without a status to decide into (rules false) or without a bank
+    const u32 C = !rules || !T ? 0 : knn ? T : q ? (T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM : 0;
+    p.rule = C ? Rule{C, q, knn} : Rule{0, 0, 0};
+    return true;
 }
 
-// the banded DP of radius band_r >= 0, the kernel chosen from band_r alone: the thread form for r = 10, the warp-scan
-// form for the other r <= 15 (2r+1 lanes of one warp), the whole-row form for r >= 16. Every r >= 118 is the full matrix
-// (|j - c| <= 118 for any two columns), so r is clamped to 118 and no r reaches the kernels' c +- r.
-cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
-                            u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev,
-                            const u32 *perm) {
-    if (B == 0 || T == 0) return cudaSuccess;
-    if (band_r < 0) return cudaErrorInvalidValue;
-    const int r = min(band_r, (int)kMaxFrm - 1);
-    const auto *in = static_cast<const unsigned char *>(in_ftr);
-    const auto *bk = static_cast<const unsigned char *>(bank);
-    const bool lift = flags & SR_DTW_LIFTER;
-    if (r == 10) {                                                            // the BASELINE radius: thread-per-pair form
-        auto *thread_kernel = lift ? dtw_band_thread_kernel<10, true> : dtw_band_thread_kernel<10, false>;
-        cudaError_t e = cudaFuncSetAttribute(thread_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+ScanArgs scan_args(const ScanPlan &p, const BankView &bank, const void *in_ftr, u32 B, u32 *score, u64 *best,
+                   const u8 *status, const u32 *B_dev) {
+    const u32 C = p.rule.C;                                             // the key layout of p.rule (ScanArgs)
+    return ScanArgs{static_cast<const unsigned char *>(in_ftr), B, B_dev, status, static_cast<const unsigned char *>(bank.p),
+                    bank.n, bank.stride, bank.order, score, best, p.check_sign, p.guard, p.r, C ? C : 1,
+                    !C ? 32u : p.rule.knn ? 0u : 2u};
+}
+
+#ifndef SR_DTW_VARIANT_DEFAULT
+#define SR_DTW_VARIANT_DEFAULT 0
+#endif
+// the scan under p with the kernels' liftered (kLift) or plain form
+template <bool kLift>
+static cudaError_t launch_scan_as(sr_handle *h, const ScanPlan &p, const ScanArgs &a) {
+    const int num_sms = h->num_sms;
+    const cudaStream_t st = h->stream;
+    int variant = h->dtw_variant;
+    if (variant < 0) {
+        static const int env_v = [] { const char *e = getenv("SR_DTW_VARIANT"); return e && *e ? atoi(e) : SR_DTW_VARIANT_DEFAULT; }();
+        variant = env_v;
+    }
+    if (p.matcher == ScanPlan::kGreedy && variant == 1) {
+        // dynamic pairs: the longest input (frm_max_kernel, into the handle's scratch word) sizes the ring slots
+        cudaError_t e = ensure(h->dtw_scratch, 16);
         if (e != cudaSuccess) return e;
-        return launch_tiles(T, [&](u32 tile0, u32 ntiles, int Tt) {
-            const LanePlan p = plan_lanes(Tt);
-            thread_kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, B, (u32)(p.G * p.NU))), kK2Warps * 32,
-                                         p.smem, st>>>(in, B, bk, T, slot_stride, flags, score, best, status, p.Wg, p.NU,
-                                                       p.G, tile0, Tt, B_dev, perm);
+        u32 *max_frm = static_cast<u32 *>(h->dtw_scratch.p);
+        e = cudaMemsetAsync(max_frm, 0, 4, st);
+        if (e != cudaSuccess) return e;
+        const u32 g = min((a.B + 255) / 256, (u32)num_sms * 4u);
+        frm_max_kernel<<<g, 256, 0, st>>>(a.in_ftr, a.B, a.status, max_frm, a.B_dev);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        const u32 smem = 226 * 1024;
+        e = cudaFuncSetAttribute(dtw_dyn_kernel<kLift>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        return launch_tiles(a.T, [&](u32 tile0, u32 ntiles, int) {
+            dtw_dyn_kernel<kLift><<<dim3(ntiles, grid_rows(num_sms, ntiles, a.B, 1u)), kDynWarps * 32, smem, st>>>(
+                a, SCAN_PTRS(a), tile0, smem, max_frm);
             return cudaGetLastError();
         });
     }
-    auto *kernel = r <= 15 ? (lift ? dtw_band_kernel<true> : dtw_band_kernel<false>)
-                           : (lift ? dtw_wide_kernel<true> : dtw_wide_kernel<false>);
+    if (p.matcher == ScanPlan::kGreedy || (p.matcher == ScanPlan::kBand && p.r == 10)) {
+        // lane-packed: one launch per tile width, each with the lane plan of its width
+        auto *kernel = p.matcher == ScanPlan::kGreedy ? dtw_kernel<kLift> : dtw_band_thread_kernel<10, kLift>;
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+        if (e != cudaSuccess) return e;
+        return launch_tiles(a.T, [&](u32 tile0, u32 ntiles, int Tt) {
+            const LanePlan lp = plan_lanes(Tt);
+            kernel<<<dim3(ntiles, grid_rows(num_sms, ntiles, a.B, (u32)(lp.G * lp.NU))), kK2Warps * 32, lp.smem, st>>>(
+                a, SCAN_PTRS(a), lp.Wg, lp.NU, lp.G, tile0, Tt);
+            return cudaGetLastError();
+        });
+    }
+    // warp per pair: the symmetric DP, the band's warp-scan form for the other r <= 15 (2r+1 lanes of one warp), its
+    // whole-row form for r >= 16
+    auto *kernel = p.matcher == ScanPlan::kSym ? dtw_sym_kernel<kLift> : p.r <= 15 ? dtw_band_kernel<kLift> : dtw_wide_kernel<kLift>;
     const size_t smem = (size_t)kTileT * kSlotBytes + kTileHdr + (size_t)kDtwWarps * kSlotBytes;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    const u32 tiles = (T + kTileT - 1) / kTileT;
-    dim3 grid(tiles, grid_rows(num_sms, tiles, B, kDtwWarps));
-    kernel<<<grid, kDtwWarps * 32, smem, st>>>(in, B, bk, T, slot_stride, flags, r, score, best, status, B_dev, perm);
+    const u32 tiles = (a.T + kTileT - 1) / kTileT;
+    kernel<<<dim3(tiles, grid_rows(num_sms, tiles, a.B, kDtwWarps)), kDtwWarps * 32, smem, st>>>(a, SCAN_PTRS(a));
     return cudaGetLastError();
 }
 
-}  // namespace srk
+cudaError_t launch_scan(sr_handle *h, const ScanPlan &p, const ScanArgs &a) {
+    if (a.B == 0 || a.T == 0) return cudaSuccess;
+    return p.lift ? launch_scan_as<true>(h, p, a) : launch_scan_as<false>(h, p, a);
+}

@@ -107,7 +107,7 @@ dtw_align_kernel(const unsigned char *__restrict__ in_base, u32 in_stride, const
         } else {
             tf = tpl_base + (size_t)pr.tpl * tpl_stride;
         }
-        const u32 Iraw = decode_frm(*reinterpret_cast<const u32 *>(uf), 0), Mraw = decode_frm(*reinterpret_cast<const u32 *>(tf), 0);
+        const u32 Iraw = decode_frm(*reinterpret_cast<const u32 *>(uf), false), Mraw = decode_frm(*reinterpret_cast<const u32 *>(tf), false);
         const bool walks = Iraw >= 1 && pair_walks(Iraw, Mraw, true);
         const int I = (int)Iraw, M = (int)Mraw;
         __syncwarp();                                                // the previous pair's readers are done

@@ -147,7 +147,7 @@ dtw_connected_kernel(const s16 *__restrict__ feat, u32 frm_stride, const u32 *__
     const u32 M = conn_prologue(cl, smem_raw, reinterpret_cast<const unsigned char *>(feat + row0 * 12) - 4, N, b, D, [&](u32 &M) {
         const unsigned char *slot = bank + (size_t)t * slot_stride;
         if (t < T) {
-            const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);
+            const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), true);
             if (frm != kNoWalk) M = frm;
         }
         return slot;
@@ -223,7 +223,7 @@ __device__ __forceinline__ const unsigned char *copy_member(unsigned char *cst, 
         const u32 cw = copy[c];
         src = cw >> 16;
         slot = bank + (size_t)(cw & 255u) * slot_stride;
-        M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);   // the host only makes copies of members
+        M = decode_frm(*reinterpret_cast<const u32 *>(slot), true);   // the host only makes copies of members
         if (M == kNoWalk) M = 0;
     }
     return slot;
@@ -520,7 +520,7 @@ dtw_long_grammar_kernel(const s16 *__restrict__ feat, const u32 *__restrict__ se
         const u32 cw = copy[c];
         src = cw >> 16;
         slot = bank + (size_t)(cw & 255u) * slot_stride;
-        M = decode_frm(*reinterpret_cast<const u32 *>(slot), SR_DTW_CHECK_SIGN);
+        M = decode_frm(*reinterpret_cast<const u32 *>(slot), true);
         if (M == kNoWalk) M = 0;
     }
     unsigned char *tslot = smem_raw + kSeqBytes + warp * kSlotBytes;

@@ -1,7 +1,9 @@
 // sr_dtw_core.cuh -- the template scan's shared core, used by the static kernels (sr_dtw.cu: greedy dtw_kernel, banded
-// dtw_band_kernel, dtw_band_thread_kernel and dtw_wide_kernel) and the dynamic-pair kernel (sr_dtw_dyn.cu): byte-plane rows and their
-// get_dis, the slot header decode, the template tile stager, the greedy walk step, the score/argmin epilogue and the
-// launch geometry.
+// dtw_band_kernel, dtw_band_thread_kernel and dtw_wide_kernel, symmetric dtw_sym_kernel) and the dynamic-pair kernel
+// (sr_dtw_dyn.cuh): byte-plane rows and their get_dis, the slot header decode, the template tile stager, the greedy walk
+// step, the scan's argument block ScanArgs, the score/argmin epilogue, the decision step of the finishers and the launch
+// geometry. No kernel here reads the matcher flags: scan_plan (sr_dtw.cu) decodes them once on the host into ScanArgs'
+// fields and a Rule, and launch_scan there picks the kernel.
 //
 // Rows are staged as BYTE PLANES (low bytes | high bytes of the 12 s16), so that
 //   sum (a-b)^2 = |a|^2 + |b|^2 - 2 a.b        (exact in Z/2^32, the ring the reference accumulates in)
@@ -83,11 +85,11 @@ __device__ __forceinline__ void stage_planes(unsigned char *slot, u32 nrm, const
 
 // ---- headers ----------------------------------------------------------------------------------------------------
 // frame count from a feature set's first word (save_sign | frm_num << 16), or kNoWalk: a bank slot that is unsigned or
-// erased under SR_DTW_CHECK_SIGN (main.c:283), or a frm_num > vv_frm_max, whose rows would lie past the struct.
-// Utterances pass flags = 0.
-__device__ __forceinline__ u32 decode_frm(u32 hdr, u32 flags) {
+// erased under check_sign (SR_DTW_CHECK_SIGN, main.c:283), or a frm_num > vv_frm_max, whose rows would lie past the
+// struct. Utterances pass check_sign = false.
+__device__ __forceinline__ u32 decode_frm(u32 hdr, bool check_sign) {
     const u32 frm = hdr >> 16;
-    const bool unsigned_slot = (flags & SR_DTW_CHECK_SIGN) && (hdr & 0xFFFFu) != SR_SAVE_MASK;
+    const bool unsigned_slot = check_sign && (hdr & 0xFFFFu) != SR_SAVE_MASK;
     return (unsigned_slot || frm > kMaxFrm) ? kNoWalk : frm;
 }
 // rows to stage: the greedy do-while may touch row frm, and rows 0 and 1 are always read (DTW.C:146-160), also when
@@ -101,17 +103,54 @@ __device__ __forceinline__ bool pair_walks(u32 Iraw, u32 Mraw, bool guard) {
     return guard ? !(I > M * 2 || 2 * I < M) : (I >= 1 && M >= 1);
 }
 
+// ---- the scan's arguments: one block for every template-scan kernel ----------------------------------------------------
+// B inputs of kFtrBytes at in_ftr (B_dev: a batch size produced on the device, streaming; status: the per-input SR_ST_*
+// gate of the recognition calls, or NULL) against the T bank slots of slot_stride bytes at bank (perm: the slots in
+// ascending frm_num order, whose templates of a tile then walk alike, or NULL; results stay under the ORIGINAL slot
+// number). score [B][T] and best may be NULL. check_sign, guard (the 2:1 length guard: off only under SR_DTW_ANY_RATE)
+// and r (the band radius, at most 118) are the plan's (scan_plan, sr_dtw.cu).
+// The argmin key of a pair is (result, bank slot t): strict '<', first wins == lexicographic min. The key of pair (u, t)
+// is best[u * key_stride + (t >> key_shift)], the layout the plan's Rule sized:
+//   no rule:             one key per input,             key_stride 1,             key_shift 32 (t >> 32 is 0);
+//   SR_DTW_REJECT(q):    [B][ceil(T / 4)] per command,  key_stride ceil(T / 4),   key_shift 2. The runner-up command
+//                        depends on the winner; the row's minimum is the same argmin key, its second smallest the
+//                        runner-up command's score;
+//   SR_DTW_KNN(k):       [B][T] per slot, each written once: key_stride T, key_shift 0. A command's score needs all of
+//                        its templates' scores.
+// Every key starts at (SR_DIS_MAX, slot 0) (main.c:276-278).
+// Every scan kernel also takes a's seven pointers as __restrict__ parameters (SCAN_PTRS), which its body reads and
+// writes through: only restrict KERNEL parameters keep the loads read-only (LDG.CONSTANT). Restrict-qualified members,
+// locals or device-function parameters lose it to the scans' 64-bit atomics and named barriers, and __ldg keeps it but
+// changes how the staging loops compile (registers, unrolling).
+struct ScanArgs {
+    const unsigned char *in_ftr;
+    u32 B;
+    const u32 *B_dev;
+    const u8 *status;
+    const unsigned char *bank;
+    u32 T, slot_stride;
+    const u32 *perm;
+    u32 *score;
+    u64 *best;
+    bool check_sign, guard;
+    int r;
+    u32 key_stride, key_shift;
+};
+
+// The pointers of a, in the order of the scan kernels' __restrict__ parameters
+#define SCAN_PTRS(a) (a).in_ftr, (a).bank, (a).status, (a).B_dev, (a).perm, (a).score, (a).best
+
 // stage bank templates t0 .. t0+Tt-1 (bank slot perm[t] when a bank order is given) into tile slots of slot_bytes each:
 // planes and norms, frame counts to tfrm[], bank slot numbers to tslot[] unless it is NULL. Warp w of nwarps stages
 // templates w, w+nwarps, ... (kLift: liftered, as stage_planes)
 template <bool kLift>
 __device__ __forceinline__ void stage_tile(unsigned char *tile, u32 slot_bytes, u32 nrm, u32 *tfrm, u32 *tslot,
-                                           const unsigned char *bank, u32 slot_stride, u32 flags, const u32 *perm, u32 t0,
-                                           int Tt, int warp, int lane, int nwarps) {
+                                           const unsigned char *bank, u32 slot_stride, bool check_sign, const u32 *perm,
+                                           u32 t0, int Tt, int warp, int lane, int nwarps) {
     for (int tt = warp; tt < Tt; tt += nwarps) {
         const u32 ts = perm ? perm[t0 + tt] : t0 + (u32)tt;
         const unsigned char *slot = bank + (size_t)ts * slot_stride;
-        const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), flags);
+        const u32 frm = decode_frm(*reinterpret_cast<const u32 *>(slot), check_sign);
         stage_planes<kLift>(tile + (size_t)tt * slot_bytes, nrm, slot, staged_rows(frm), lane, 32);
         if (lane == 0) {
             tfrm[tt] = frm;
@@ -223,23 +262,17 @@ __device__ __forceinline__ K dp_end(const K (&D)[4], int kend, int lend) {
     return __shfl_sync(0xFFFFFFFFu, e, lend);
 }
 
-// The argmin key of a pair: (result, bank slot t), strict '<', first wins == lexicographic min. Without a decision rule
-// (no bits 8-10 or 16-31 in flags) best has one key per utterance. Under SR_DTW_REJECT(q) the runner-up command depends
-// on the winner, so best is the per-(utterance, command) array [B][ceil(T / 4)] instead: the minimum over its row is the
-// same argmin key, and the second smallest entry of the row is the runner-up command's score. Under SR_DTW_KNN(k) a
-// command's score needs all of its templates' scores, so best is the per-(utterance, slot) array [B][T], each key written
-// once. Every key starts at (SR_DIS_MAX, slot 0) (main.c:276-278).
+// ---- the argmin keys -----------------------------------------------------------------------------------------------
 constexpr u64 kKeyStart = (u64)SR_DIS_MAX << 32;
-__device__ __forceinline__ u64 *key_of(u64 *best, u32 flags, u32 T, u32 u, u32 t) {
-    if (rule_knn(flags)) return best + (size_t)u * T + t;
-    return (flags >> 16) ? best + (size_t)u * ((T + SR_FTR_PER_COMM - 1) / SR_FTR_PER_COMM) + t / SR_FTR_PER_COMM : best + u;
+// a scan under a decision rule writes a row of keys per input
+__device__ __forceinline__ bool key_rows(const ScanArgs &a) { return a.key_shift < 32; }
+__device__ __forceinline__ u64 *key_of(u64 *best, const ScanArgs &a, u32 u, u32 t) {
+    return best + (size_t)u * a.key_stride + ((u64)t >> a.key_shift);
 }
-// a scan under a decision rule writes a row of keys per utterance (key_of)
-__device__ __forceinline__ bool key_rows(u32 flags) { return rule_knn(flags) || (flags >> 16); }
 // score[u][t] and the spch_recg argmin (main.c:276-291) as one 64-bit atomicMin of the pair's key
-__device__ __forceinline__ void emit_pair(u32 *score, u64 *best, u32 T, u32 u, u32 t, u32 result, u32 flags) {
-    if (score) score[(size_t)u * T + t] = result;
-    if (best) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, flags, T, u, t)),
+__device__ __forceinline__ void emit_pair(u32 *score, u64 *best, const ScanArgs &a, u32 u, u32 t, u32 result) {
+    if (score) score[(size_t)u * a.T + t] = result;
+    if (best) atomicMin(reinterpret_cast<unsigned long long *>(key_of(best, a, u, t)),
                         (unsigned long long)(((u64)result << 32) | (u64)t));
 }
 
@@ -311,24 +344,27 @@ __device__ __forceinline__ Top2 rule_row(const u64 *row, u32 C, u32 knn, int lan
 }
 
 // ---- one record's decision: the step of every finisher (main.c:261-294) -------------------------------------------
+// The decision rule of a recognition call, from its matcher flags (scan_plan, sr_dtw.cu): C keys per record (0: no rule,
+// one argmin key; else the scan's row, ScanArgs), the margin q of SR_DTW_REJECT(q) and the k of SR_DTW_KNN(k) (0: off).
+struct Rule { u32 C, q, knn; };
 // threads per record of a finisher: one without a rule (C = 0), else rule_group of the row's commands
-__host__ __device__ __forceinline__ u32 rule_lanes(u32 C, u32 knn) { return C ? (u32)rule_group(rule_cmds(C, knn)) : 1u; }
+__host__ __device__ __forceinline__ u32 rule_lanes(const Rule &rl) { return rl.C ? (u32)rule_group(rule_cmds(rl.C, rl.knn)) : 1u; }
 // a finisher's grid of 256-thread CTAs over n records
-inline u32 rule_grid(u64 n, u32 C, u32 knn) { return (u32)((n * rule_lanes(C, knn) + 255) / 256); }
+inline u32 rule_grid(u64 n, const Rule &rl) { return (u32)((n * rule_lanes(rl) + 255) / 256); }
 // Record i's decision from its keys and the status st it comes in with. Without a rule (kRule false) its key is keys[i];
 // under one the g lanes of its group fold its row of C keys (rule_row), and only lane 0 gets the decision (the others
 // return false). An SR_ST_OK decision the margin rule q turns down gets SR_ST_REJECT, and a record whose st is not
 // SR_ST_OK reports idx 0 and SR_DIS_ERR.
 struct Decision { u64 key; u32 idx, dis, cmd, status; };
 template <bool kRule>
-__device__ __forceinline__ bool decide(const u64 *keys, u32 i, u32 st, u32 C, u32 q, u32 knn, u32 g, Decision &d) {
+__device__ __forceinline__ bool decide(const u64 *keys, u32 i, u32 st, const Rule &rl, u32 g, Decision &d) {
     d.status = st;
     if constexpr (kRule) {
         const u32 lane = threadIdx.x & (g - 1);
-        const Top2 t2 = rule_row(keys + (size_t)i * C, C, knn, (int)lane, (int)g);
+        const Top2 t2 = rule_row(keys + (size_t)i * rl.C, rl.C, rl.knn, (int)lane, (int)g);
         if (lane) return false;
         d.key = t2.k1;
-        if (st == SR_ST_OK && margin_rejects((u32)(d.key >> 32), (u32)(t2.k2 >> 32), q)) d.status = SR_ST_REJECT;
+        if (st == SR_ST_OK && margin_rejects((u32)(d.key >> 32), (u32)(t2.k2 >> 32), rl.q)) d.status = SR_ST_REJECT;
     } else {
         d.key = keys[i];
     }

@@ -13,7 +13,7 @@
 #include <string>
 #include <thread>
 #include <vector>
-#include "sr_common.cuh"
+#include "sr_dtw_core.cuh"
 #include "../../include/sr_long_grammar.h"
 
 namespace srk {
@@ -27,27 +27,12 @@ cudaError_t launch_mfcc_geomb(const u16 *pcm, u32 U, u32 B, const u32 *seg, u32 
 cudaError_t launch_fft_generic(const u32 *in_packed, const s16 *frames, u32 len, u32 n, u32 *raw_out, u32 *mag,
                                cudaStream_t st);
 cudaError_t launch_fft_raw_n(const u32 *in, u32 N, u32 n, u32 *out, cudaStream_t st);
-cudaError_t launch_dtw(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
-                       u64 *best, const u8 *status, int num_sms, cudaStream_t st, const u32 *B_dev = nullptr,
-                       const u32 *perm = nullptr);
-cudaError_t launch_dtw_dyn(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, u32 *score,
-                           u64 *best, const u8 *status, int num_sms, cudaStream_t st, u32 *max_frm_scratch,
-                           const u32 *B_dev = nullptr, const u32 *perm = nullptr);
-cudaError_t launch_dtw_band(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
-                            u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st,
-                            const u32 *B_dev = nullptr, const u32 *perm = nullptr);
-cudaError_t launch_dtw_sym(const void *in_ftr, u32 B, const void *bank, u32 T, u32 slot_stride, u32 flags, int band_r,
-                           u32 *score, u64 *best, const u8 *status, int num_sms, cudaStream_t st,
-                           const u32 *B_dev = nullptr, const u32 *perm = nullptr);
 // n keys (B argmin keys, or a decision rule's B * C keys) set to main.c:276-278's start
 cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st);
-// The decision of B inputs into the fields (sr_dtw.cu): without a rule (C = 0) from the argmin keys keys = best; under
-// the rule of margin q and KNN knn from the keys [B][C] (rule_cols), with the decision's keys into best[B] and
-// SR_ST_REJECT into status
-cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, u32 C, u32 q, u32 knn, u32 *best_idx, u32 *best_dis,
-                              u32 *cmd, u8 *status, cudaStream_t st);
-// the matcher bits of the flags, 0-3 and SR_DTW_LIFTER: what sr_dtw_batch* pass on to a kernel
-constexpr u32 kMatcherBits = 0xFu | SR_DTW_LIFTER;
+// The decision of B inputs into the fields (sr_dtw.cu): without a rule (rl.C = 0) from the argmin keys keys = best;
+// under one from the keys [B][rl.C], with the decision's keys into best[B] and SR_ST_REJECT into status
+cudaError_t launch_best_final(u64 *best, const u64 *keys, u32 B, const Rule &rl, u32 *best_idx, u32 *best_dis, u32 *cmd,
+                              u8 *status, cudaStream_t st);
 cudaError_t launch_status(const u32 *seg_off, const void *ftr, u32 B, u8 *status, cudaStream_t st);
 cudaError_t launch_get_dis(const s16 *a, const s16 *b, u32 n, u32 *out, cudaStream_t st);
 cudaError_t launch_dtw_limit(const u16 *x, const u16 *y, const u16 *I, const u16 *M, u32 n, u8 *out, cudaStream_t st);
@@ -98,7 +83,7 @@ cudaError_t launch_long_flatten(const u32 *n_segs, const u32 *seg_off, const ata
                                 u32 *n_flat, u32 *seg2, u32 *row, u32 *slot, atap_tag *atap_seg, cudaStream_t st, int step);
 cudaError_t launch_long_status(const u32 *seg2, const void *ftr, const u32 *n_flat, u32 M, u8 *status, cudaStream_t st);
 cudaError_t launch_long_scatter(const u32 *seg2, const u32 *slot, const void *ftr, const u8 *status, const u64 *best,
-                                const u32 *n_flat, u32 M, sr_long_seg *rec, u32 C, u32 q, u32 knn, cudaStream_t st);
+                                const u32 *n_flat, u32 M, sr_long_seg *rec, const Rule &rl, cudaStream_t st);
 class PackPool;
 }  // namespace srk
 
@@ -203,7 +188,7 @@ struct sr_handle {
     std::vector<uint8_t> labels;
     u32 n_labels = 0, label_stride = 0;
     sr_comm *comm = nullptr;                           // the exchange step (sr_comm_create), optional
-    int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cu), -1 default
+    int dtw_variant = -1;                              // greedy dtw kernel: 0 static lane = pair (sr_dtw.cu), 1 dynamic pairs (sr_dtw_dyn.cuh), -1 default
     u32 match_flags = 0;                               // matcher of the recognition calls (sr_set_match): 0 greedy walk, SR_DTW_BAND (| SR_DTW_ANY_RATE) or SR_DTW_SYM_P1,
                                                        // | SR_DTW_LIFTER | SR_DTW_KNN(k) | SR_DTW_REJECT(q)
     int match_r = 0;                                   // its band radius
@@ -306,48 +291,35 @@ inline u32 *vad_work(sr_handle *h) {
     return static_cast<u32 *>(h->vad_work.p);
 }
 
-// greedy dtw of B inputs against `bank` with the handle's kernel variant
-#ifndef SR_DTW_VARIANT_DEFAULT
-#define SR_DTW_VARIANT_DEFAULT 0
-#endif
-inline cudaError_t launch_dtw_h(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, u32 *score, u64 *best,
-                                const u8 *status, const u32 *B_dev = nullptr) {
-    int v = h->dtw_variant;
-    if (v < 0) {
-        static const int env_v = [] { const char *e = getenv("SR_DTW_VARIANT"); return e && *e ? atoi(e) : SR_DTW_VARIANT_DEFAULT; }();
-        v = env_v;
-    }
-    if (v == 1) {
-        cudaError_t e = ensure(h->dtw_scratch, 16);
-        if (e != cudaSuccess) return e;
-        return launch_dtw_dyn(in_ftr, B, bank.p, bank.n, bank.stride, flags, score, best, status, h->num_sms, h->stream,
-                              static_cast<u32 *>(h->dtw_scratch.p), B_dev, bank.order);
-    }
-    return launch_dtw(in_ftr, B, bank.p, bank.n, bank.stride, flags, score, best, status, h->num_sms, h->stream, B_dev, bank.order);
-}
-
-// The template scan of B inputs against `bank` -- the one place a matcher becomes a kernel launch: with SR_DTW_SYM_P1 in
-// flags the symmetric P = 1 DP of radius band_r, with SR_DTW_BAND the banded DP of radius band_r (launch_dtw_band picks
-// the kernel from r; its kernels read SR_DTW_ANY_RATE from flags and then skip the 2:1 guard), else the greedy walk.
-// Each launcher picks its kernel's liftered form when flags has SR_DTW_LIFTER.
-// sr_dtw_batch passes its caller's flags and r; the recognition paths (recognise, streaming) pass the handle's matcher.
-// The callers refuse SR_DTW_SYM_P1 | SR_DTW_BAND and SR_DTW_ANY_RATE without SR_DTW_BAND.
-inline cudaError_t launch_scan(sr_handle *h, const BankView &bank, const void *in_ftr, u32 B, u32 flags, int band_r,
-                               u32 *score, u64 *best, const u8 *status, const u32 *B_dev = nullptr) {
-    if (flags & SR_DTW_SYM_P1)
-        return launch_dtw_sym(in_ftr, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, status, h->num_sms,
-                              h->stream, B_dev, bank.order);
-    if (flags & SR_DTW_BAND)
-        return launch_dtw_band(in_ftr, B, bank.p, bank.n, bank.stride, flags, band_r, score, best, status, h->num_sms,
-                               h->stream, B_dev, bank.order);
-    return launch_dtw_h(h, bank, in_ftr, B, flags, score, best, status, B_dev);
-}
+// The template scan's matcher, decoded once from the matcher flags and band radius (scan_plan): the matcher, the
+// kernels' check_sign, guard (the 2:1 length guard, off under SR_DTW_ANY_RATE) and lifter, the radius clamped to 118,
+// the timing tag (TAG_DTW, TAG_DTW_BAND or TAG_DTW_SYM) and the decision rule
+struct ScanPlan {
+    enum Matcher { kGreedy, kBand, kSym } matcher;
+    bool check_sign, guard, lift;
+    int r, tag;
+    Rule rule;
+};
+// The plan of a scan against T templates under flags and band_r, false for flags the library refuses. rules: the
+// recognition calls, whose flags are SR_DTW_CHECK_SIGN | sr_set_match's (any radius >= 0; a decision rule's C from T,
+// none when T is 0); else sr_dtw_batch*, which have no status to decide a rule into (no bit >= 16, bits 4-15 other
+// than SR_DTW_LIFTER ignored, a DP's radius >= 0 when T > 0, rule {0, 0, 0}).
+bool scan_plan(u32 flags, int band_r, u32 T, bool rules, ScanPlan *out);
+// the arguments of the scan of B inputs at in_ftr against bank under p (score, best, status and B_dev may be NULL)
+ScanArgs scan_args(const ScanPlan &p, const BankView &bank, const void *in_ftr, u32 B, u32 *score, u64 *best,
+                   const u8 *status, const u32 *B_dev = nullptr);
+// The template scan under p (sr_dtw.cu) -- the one place a matcher becomes a kernel launch: the greedy walk with the
+// handle's variant (sr_set_dtw_variant, else SR_DTW_VARIANT: 0 the static kernel, 1 the dynamic pairs), the banded DP
+// (the thread form at r = 10, the warp-scan form for the other r <= 15, the whole-row form for r >= 16) or the symmetric
+// DP, each in its liftered form under SR_DTW_LIFTER. One counted launch, also for the dynamic kernel's pre-pass.
+cudaError_t launch_scan(sr_handle *h, const ScanPlan &p, const ScanArgs &a);
 
 // the two handles' recognition calls score and decide alike: both greedy, or both the same DP (SR_DTW_ANY_RATE included)
 // at the same radius, with or without SR_DTW_LIFTER alike, under the same decision rules
 inline bool same_match(const sr_handle *a, const sr_handle *b) {
-    return a->match_flags == b->match_flags &&
-           ((a->match_flags & (SR_DTW_BAND | SR_DTW_SYM_P1)) == 0 || a->match_r == b->match_r);
+    ScanPlan p;
+    scan_plan(a->match_flags, a->match_r, 0, true, &p);               // flags and radius sr_set_match accepted
+    return a->match_flags == b->match_flags && (p.matcher == ScanPlan::kGreedy || a->match_r == b->match_r);
 }
 
 int comm_wait_before_scan(sr_handle *h, const void *score);   // sr_comm.cu

@@ -162,7 +162,7 @@ __global__ void stream_segments_kernel(const StreamState *st, u32 S, u32 *seg_of
 }
 
 // status per event from the freshly computed features (MFCC fail = frm_num 0, main.c:269-274) + argmin initialiser:
-// best[cap] without a decision rule, its C keys per event (rule_cols) under one (kRule)
+// best[cap] without a decision rule, its C keys per event (ScanArgs) under one (kRule)
 template <bool kRule>
 __global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, u32 cap, u8 *status, u32 *frm, u64 *best,
                                      u32 C) {
@@ -182,14 +182,14 @@ __global__ void stream_status_kernel(const unsigned char *ftr, const u32 *n_ev, 
 // word 0 of `out` = event count
 template <bool kRule>
 __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, u32 cap, const u8 *status, const u32 *frm,
-                                     const u64 *best, sr_stream_event *out_rec, u32 *out_count, u32 C, u32 q, u32 knn) {
-    const u32 g = kRule ? rule_lanes(C, knn) : 1u;
+                                     const u64 *best, sr_stream_event *out_rec, u32 *out_count, Rule rl) {
+    const u32 g = kRule ? rule_lanes(rl) : 1u;
     const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / g;
     const u32 ne = min(*n_ev, cap);
     if (i == 0) *out_count = ne;
     if (i >= ne) return;
     Decision d;
-    if (!decide<kRule>(best, i, status[i], C, q, knn, g, d)) return;
+    if (!decide<kRule>(best, i, status[i], rl, g, d)) return;
     sr_stream_event r;
     r.stream = ev[i].stream; r.segment = ev[i].segment; r.start = ev[i].start; r.end = ev[i].end;
     r.status = (u8)d.status; r.frm_num = frm[i]; r.best_idx = d.idx; r.best_dis = d.dis; r.cmd = d.cmd;
@@ -266,7 +266,9 @@ int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_
     SR_LAUNCH(h, TAG_NONE, launch_mfcc_h(h, pcm, row_len, c.cap, static_cast<const u32 *>(c.seg_ev.p), 2,
                                          static_cast<const atap_tag *>(c.atap_ev.p), c.ftr.p, static_cast<const u32 *>(c.map_ev.p),
                                          c.S, n_ev));
-    const u32 match = h->match_flags, C = rule_cols(match, h->bank.n);   // the handle's matcher, read at every push
+    ScanPlan p;                                                          // the handle's matcher, read at every push
+    scan_plan(SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, h->bank.n, true, &p);   // flags sr_set_match accepted
+    const u32 C = p.rule.C;
     SR_CK(h, ensure(h->best, (size_t)c.cap * (C ? C : 1) * 8));
     u64 *best = static_cast<u64 *>(h->best.p);
     const u32 gb = (c.cap + 255) / 256;
@@ -278,16 +280,14 @@ int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_
         }))
         return rc;
     if (h->bank.n)
-        SR_LAUNCH(h, TAG_NONE, launch_scan(h, h->bank, c.ftr.p, c.cap, SR_DTW_CHECK_SIGN | match, h->match_r, nullptr, best,
-                                           static_cast<const u8 *>(c.status.p), n_ev));
+        SR_LAUNCH(h, TAG_NONE, launch_scan(h, p, scan_args(p, h->bank, c.ftr.p, c.cap, nullptr, best,
+                                                           static_cast<const u8 *>(c.status.p), n_ev)));
     u32 *out_count = static_cast<u32 *>(c.out.p);
     sr_stream_event *out_rec = reinterpret_cast<sr_stream_event *>(static_cast<unsigned char *>(c.out.p) + 16);
     if (const int rc = launch_on(h, TAG_NONE, "stream_finish_kernel", [&] {
-            (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<rule_grid(c.cap, C, rule_knn(match)), 256, 0,
-                                                                              h->stream>>>(
+            (C ? stream_finish_kernel<true> : stream_finish_kernel<false>)<<<rule_grid(c.cap, p.rule), 256, 0, h->stream>>>(
                 static_cast<const StreamEventDev *>(c.ev.p), n_ev, c.cap, static_cast<const u8 *>(c.status.p),
-                static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, C, rule_q(match),
-                rule_knn(match));
+                static_cast<const u32 *>(c.frm.p), best, out_rec, out_count, p.rule);
             return cudaGetLastError();
         }))
         return rc;

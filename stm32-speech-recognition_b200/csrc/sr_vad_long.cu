@@ -205,12 +205,12 @@ __global__ void long_status_kernel(const u32 *__restrict__ seg2, const unsigned 
 template <bool kRule>
 __global__ void long_scatter_kernel(const u32 *__restrict__ seg2, const u32 *__restrict__ slot, const unsigned char *__restrict__ ftr,
                                     const u8 *__restrict__ status, const u64 *__restrict__ best, const u32 *__restrict__ n_flat,
-                                    sr_long_seg *__restrict__ rec, u32 C, u32 q, u32 knn) {
-    const u32 g = kRule ? rule_lanes(C, knn) : 1u;
+                                    sr_long_seg *__restrict__ rec, Rule rl) {
+    const u32 g = kRule ? rule_lanes(rl) : 1u;
     const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) / g;
     if (i >= *n_flat) return;
     Decision d;
-    if (!decide<kRule>(best, i, status[i], C, q, knn, g, d)) return;
+    if (!decide<kRule>(best, i, status[i], rl, g, d)) return;
     sr_long_seg r;
     r.start = seg2[2 * (size_t)i]; r.end = seg2[2 * (size_t)i + 1]; r.status = d.status;
     r.frm_num = (*reinterpret_cast<const u32 *>(ftr + (size_t)i * kFtrBytes)) >> 16;
@@ -271,9 +271,9 @@ cudaError_t launch_long_status(const u32 *seg2, const void *ftr, const u32 *n_fl
 }
 
 cudaError_t launch_long_scatter(const u32 *seg2, const u32 *slot, const void *ftr, const u8 *status, const u64 *best,
-                                const u32 *n_flat, u32 M, sr_long_seg *rec, u32 C, u32 q, u32 knn, cudaStream_t st) {
-    (C ? long_scatter_kernel<true> : long_scatter_kernel<false>)<<<rule_grid(M, C, knn), 256, 0, st>>>(
-        seg2, slot, static_cast<const unsigned char *>(ftr), status, best, n_flat, rec, C, q, knn);
+                                const u32 *n_flat, u32 M, sr_long_seg *rec, const Rule &rl, cudaStream_t st) {
+    (rl.C ? long_scatter_kernel<true> : long_scatter_kernel<false>)<<<rule_grid(M, rl), 256, 0, st>>>(
+        seg2, slot, static_cast<const unsigned char *>(ftr), status, best, n_flat, rec, rl);
     return cudaGetLastError();
 }
 

@@ -598,7 +598,7 @@ def test_dtw_empty_feature_sets_are_deterministic(handle, ora):
 @pytest.mark.parametrize("T,B,fr", [(1, 70, (1, 119)), (5, 333, (20, 45)), (20, 1500, (23, 43)), (32, 257, (50, 100)),
                                     (33, 640, (1, 119)), (70, 200, (30, 119)), (200, 300, (50, 100))])
 def test_dtw_dynamic_pair_scheduling_equals_static_and_reference(ora, T, B, fr):
-    """sr_dtw_dyn.cu (pairs pulled dynamically from a ring of staged utterances) == the static kernel == the reference's
+    """sr_dtw_dyn.cuh (pairs pulled dynamically from a ring of staged utterances) == the static kernel == the reference's
     dtw, scores and first-wins argmin, over bank widths around the 32-template tile, all frame counts, mixed save_sign,
     the 2:1 guard, garbage headers; run twice so the second launch sees a dirty ring"""
     h = sr_b200.Handle(0)
