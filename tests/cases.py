@@ -127,6 +127,44 @@ def random_groups(rng, G, K, stride, fmin=3, fmax=24, plant=True):
     return bank
 
 
+def word_bank(T, seed, erase=(), dup=(), trunc=None):
+    """T slots of 4 096 bytes from synthetic one-word templates: command c's four slots are one word with one row dropped each (row
+    k * 7, none for k = 0), optionally cut to trunc(t) frames; dup (a, b) copies slot a into slot b; erase: unsigned"""
+    n_cmd = (T + 3) // 4
+    e = ob.recognise_pinned(ob.best_oracle(), sr_b200.synth_pcm_host(n_cmd, 8000, seed), 2400, None, 0, 4096)
+    ftr = np.zeros(4 * n_cmd, ob.FTR_DTYPE)
+    for t in range(4 * n_cmd):
+        f = e["ftr"][t // 4]
+        n = int(f["frm_num"])
+        rows = f["mfcc_dat"][:n * 12].reshape(n, 12)
+        x = rows if t % 4 == 0 else np.delete(rows, min((t % 4) * 7, n - 1), axis=0)
+        if trunc:
+            x = x[:trunc(t)]
+        ftr[t]["frm_num"] = len(x)
+        ftr[t]["mfcc_dat"][:x.size] = x.reshape(-1)
+    for a, b in dup:
+        ftr[b] = ftr[a]
+    valid = np.ones(T, bool)
+    valid[list(erase)] = False
+    return sr_b200.make_bank(ftr[:T], 4096, valid)
+
+
+def headroom_bank(seed):
+    """8 slots of word_bank(8, seed) (slot 6 unsigned, slot 3 a copy of slot 0) with +32 767 and -32 767 in
+    coefficients 0 and 1 of every row, and command 1's rows +32 767 in coefficient 2 as well: every greedy and symmetric
+    score of a synthetic utterance is above 32 768 (a margin rule's q d1 passes 2^31 at q = 65 535), and command 1, the
+    runner-up, scores about a quarter more than command 0"""
+    T = 8
+    f = np.ascontiguousarray(word_bank(T, seed)[:, :ob.FTR_DTYPE.itemsize]).view(ob.FTR_DTYPE).reshape(T).copy()
+    f[3] = f[0]
+    rows = f["mfcc_dat"].reshape(T, MAX_FRM, 12)
+    rows[:, :, 0], rows[:, :, 1] = 32767, -32767
+    rows[4:, :, 2] = 32767
+    valid = np.ones(T, bool)
+    valid[6] = False
+    return sr_b200.make_bank(f, 4096, valid)
+
+
 # ---- connected words and grammars ------------------------------------------------------------------------------------
 def draw(rng, n, kind):
     """n feature rows: "tie" from {0, 1}, "full" +-32 767, "equal" one repeated row, otherwise -3000 .. 3000"""

@@ -5,9 +5,11 @@ functions, so that CPU-only runs never import it. Bare asserts here are not rewr
 message."""
 import numpy as np
 
+import lifter_ref
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
+from refs import decide
 
 NULL = 0xFFFFFFFF
 LONG_REC = ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")
@@ -50,32 +52,63 @@ def prefilled(h, pcm, P, max_words, n_len):
 
 
 # ---- the device forms on torch buffers -------------------------------------------------------------------------------
-def recognise_dev_np(h, pcm, n_len, T):
-    """one sr_recognise_batch_dev launch on the whole batch; every output field, as the host call returns it"""
+def recognise_dev_launch(h, pcm, n_len, T, fields=sr_b200.RECOG_FIELDS, gather=()):
+    """one sr_recognise_batch_dev launch of pcm [B, U] on the handle's stream, which must be the current torch stream,
+    into fresh torch buffers prefilled with 0x5A / 0xA5 bytes for the fields named in `fields` (the others NULL). gather
+    names the gathered outputs of a world of one rank ("score": [B][T] u32, "best": [B] u64 keys): then the call is
+    sr_recognise_batch_dev_allgather, into buffers of their own. Returns the buffers, nothing synchronised"""
     import torch
     dev = torch.device("cuda:0")
     B, U = pcm.shape
-    st = torch.cuda.Stream(dev)
+    out = {"pcm": torch.from_numpy(pcm.view(np.int16)).to(dev)}
+    full = {"atap": (B * 12, 0xA5, torch.uint8), "seg_off": (B * 6, 0x5A5A5A5A, torch.int32),
+            "ftr": (B * sr_b200.FTR_BYTES, 0x5A, torch.uint8), "score": (B * max(T, 1), 0x5A5A5A5A, torch.int32),
+            "status": (B, 0x5A, torch.uint8), "best_idx": (B, 0x5A5A5A5A, torch.int32),
+            "best_dis": (B, 0x5A5A5A5A, torch.int32), "cmd": (B, 0x5A5A5A5A, torch.int32),
+            "gathered_score": (B * max(T, 1), 0x5A5A5A5A, torch.int32), "gathered_best": (B, 0x5A5A5A5A5A5A5A5A, torch.int64)}
+    for key in list(fields) + ["gathered_" + g for g in gather]:
+        n, fill, dt = full[key]
+        out[key] = torch.full((n,), fill, dtype=dt, device=dev)
+    ptrs = {key: out[key].data_ptr() for key in fields}
+    if gather:
+        gs, gb = (out["gathered_" + g].data_ptr() if g in gather else None for g in ("score", "best"))
+        h.recognise_dev_allgather(out["pcm"].data_ptr(), U, B, n_len, gathered_score=gs, gathered_best=gb, **ptrs)
+    else:
+        h.recognise_dev(out["pcm"].data_ptr(), U, B, n_len, **ptrs)
+    return dict(out, B=B, T=T)
+
+
+def recognise_dev_read(bufs):
+    """the buffers of recognise_dev_launch, once their work is done, as the host call returns the fields (gathered_score
+    [B, T] u32, gathered_best [B] u64)"""
+    B, T = bufs["B"], bufs["T"]
+    got = {key: v.cpu().numpy() for key, v in bufs.items() if key not in ("B", "T", "pcm")}
+    if "atap" in got:
+        got["atap"] = got["atap"].view(sr_b200.ATAP_DTYPE)
+    if "ftr" in got:
+        got["ftr"] = got["ftr"].view(sr_b200.FTR_DTYPE)
+    if "seg_off" in got:
+        got["seg_off"] = got["seg_off"].view(np.uint32).reshape(B, 3, 2)
+    for key in ("score", "gathered_score"):
+        if key in got:
+            got[key] = got[key].view(np.uint32).reshape(B, -1)[:, :T]
+    for key in ("best_idx", "best_dis", "cmd"):
+        if key in got:
+            got[key] = got[key].view(np.uint32)
+    if "gathered_best" in got:
+        got["gathered_best"] = got["gathered_best"].view(np.uint64)
+    return got
+
+
+def recognise_dev_np(h, pcm, n_len, T):
+    """one sr_recognise_batch_dev launch on the whole batch; every output field, as the host call returns it"""
+    import torch
+    st = torch.cuda.Stream(torch.device("cuda:0"))
     h.set_stream(st.cuda_stream)
     with torch.cuda.stream(st):
-        pcm_d = torch.from_numpy(pcm.view(np.int16)).to(dev)
-        out = {"atap": torch.full((B * 12,), 0xA5, dtype=torch.uint8, device=dev),
-               "seg_off": torch.full((B * 6,), 0x5A5A5A5A, dtype=torch.int32, device=dev),
-               "ftr": torch.full((B * sr_b200.FTR_BYTES,), 0x5A, dtype=torch.uint8, device=dev),
-               "score": torch.full((B * max(T, 1),), 0x5A5A5A5A, dtype=torch.int32, device=dev),
-               "status": torch.full((B,), 0x5A, dtype=torch.uint8, device=dev)}
-        for key in ("best_idx", "best_dis", "cmd"):
-            out[key] = torch.full((B,), 0x5A5A5A5A, dtype=torch.int32, device=dev)
-        h.recognise_dev(pcm_d.data_ptr(), U, B, n_len, **{key: v.data_ptr() for key, v in out.items()})
+        bufs = recognise_dev_launch(h, pcm, n_len, T)
     st.synchronize()
-    got = {key: v.cpu().numpy() for key, v in out.items()}
-    got["atap"] = got["atap"].view(sr_b200.ATAP_DTYPE)
-    got["ftr"] = got["ftr"].view(sr_b200.FTR_DTYPE)
-    got["seg_off"] = got["seg_off"].view(np.uint32).reshape(B, 3, 2)
-    got["score"] = got["score"].view(np.uint32).reshape(B, -1)[:, :T]
-    for key in ("best_idx", "best_dis", "cmd"):
-        got[key] = got[key].view(np.uint32)
-    return got
+    return recognise_dev_read(bufs)
 
 
 def recognise_long_dev_np(h, pcm, lens, max_segs):
@@ -155,7 +188,8 @@ def k4_events(pool, pcm, arrival, rng, on_push=None):
 
 def check_k4(events, pool, pcm, bank, T, matcher=None):
     """every closed segment has one event, and each equals the oracle's get_mfcc of its segment, then the scan under the
-    matcher of its push (matcher when the pushes did not switch it) and the first-wins argmin"""
+    matcher of its push (matcher when the pushes did not switch it) and its decision: a matcher (flags, r) decides by the
+    first-wins argmin, (flags, r, k, q) by SR_DTW_KNN(k) | SR_DTW_REJECT(q) (refs.decide); flags may hold SR_DTW_LIFTER"""
     ora = ob.best_oracle()
     seg, atap = pool.segments()
     S = pcm.shape[0]
@@ -163,16 +197,17 @@ def check_k4(events, pool, pcm, bank, T, matcher=None):
     got = sorted((e["stream"], e["segment"]) for e, _ in events)
     assert got == closed and len(closed) >= 2 * S, (got[:8], closed[:8], len(got), len(closed), S)
     for e, m in events:
-        flags, r = m if m is not None else matcher
+        m = m if m is not None else matcher
+        flags, r = m[:2]
         s, k = e["stream"], e["segment"]
         f = ora.mfcc_batch(pcm[s:s + 1], seg[s, k].reshape(1, 2), atap[s:s + 1])
         assert e["frm_num"] == int(f["frm_num"][0]), e
         if e["frm_num"] == 0:
             assert (e["status"], e["best_idx"], e["best_dis"]) == (2, 0, NULL), e
             continue
-        sc = ox.match_scores(f, bank, T, flags, r)
-        i = int(np.argmin(sc[0]))
-        assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == (0, i, int(sc[0, i]), i // 4), (m, e)
+        idx, dis, cmd, rej = decide(lifter_ref.match_scores(f, bank, T, flags, r), *m[2:])
+        want = (3 if rej[0] else 0, int(idx[0]), int(dis[0]), int(cmd[0]))
+        assert (e["status"], e["best_idx"], e["best_dis"], e["cmd"]) == want, (m, e)
 
 
 def k14_events(pool, xs, c, on_push=None):
@@ -193,17 +228,26 @@ def k14_events(pool, xs, c, on_push=None):
     return out
 
 
+def long_records(pcm, lens, bank, T, m, max_segs=256):
+    """the composed oracle's sr_recognise_long_batch records of pcm under the matcher m: (flags, r), or (flags, r, k, q)
+    with SR_DTW_KNN(k) | SR_DTW_REJECT(q); flags may hold SR_DTW_LIFTER"""
+    w = lifter_ref.recognise_long(ox.long_oracle(), ob.port(), pcm, 2400, bank, T, 4096, max_segs, lens, match=m[:2])
+    if len(m) == 2:
+        return w
+    return ox.long_under_rule(w, pcm, 2400, lens, bank, T, m[:2], *m[2:], scores=lifter_ref.match_scores)
+
+
 def check_k14(events, xs, bank, T, matchers):
     """each event equals the composed oracle's record of its whole recording under the matcher of its push (matchers[0]
-    when the pushes did not switch it), in segment order, and every closed segment is handed out once"""
+    when the pushes did not switch it; a matcher as long_records takes it), in segment order, and every closed segment is
+    handed out once"""
     S = len(xs)
     Ul = max(len(x) for x in xs)
     pcm = np.zeros((S, Ul), np.uint16)
     lens = np.array([len(x) for x in xs], np.uint32)
     for s, x in enumerate(xs):
         pcm[s, :len(x)] = x
-    want = {m: ox.recognise_long(ox.long_oracle(), ob.port(), pcm, 2400, bank, T, 4096, 256, lens, match=m)
-            for m in matchers}
+    want = {m: long_records(pcm, lens, bank, T, m) for m in matchers}
     per = [0] * S
     for e, m in events:
         m = m if m is not None else matchers[0]                 # pushes without a switch: the pool's one matcher

@@ -415,9 +415,10 @@ def recognise_long(lo, port, pcm, n_len, bank, n_slot, slot_stride, max_segs, le
 
 
 
-def long_under_rule(off, pcm, n_len, lens, bank, n_slot, match, k, q):
+def long_under_rule(off, pcm, n_len, lens, bank, n_slot, match, k, q, scores=match_scores):
     """what sr_recognise_long_batch writes under SR_DTW_KNN(k) | SR_DTW_REJECT(q) and the matcher match = (flags, r), from
-    the same call's records without a rule (off): refs.decide on the oracles' scores of each SR_ST_OK segment"""
+    the same call's records without a rule (off): refs.decide on the oracles' scores of each SR_ST_OK segment (scores:
+    the matcher's oracle, e.g. lifter_ref.match_scores for flags with SR_DTW_LIFTER)"""
     port = PortOracle()
     w = recognise_long(long_oracle(), port, pcm, n_len, bank, 0, 4096, off["segs"].shape[1], lens)
     segs = off["segs"].copy()
@@ -425,7 +426,7 @@ def long_under_rule(off, pcm, n_len, lens, bank, n_slot, match, k, q):
             if segs[b, j]["status"] == 0]
     if todo:
         ftr = ftr_of_segments(port, pcm, w["atap"], [(b, int(segs[b, j]["start"]), int(segs[b, j]["end"])) for b, j in todo])
-        idx, dis, cmd, rej = decide(match_scores(ftr, bank, n_slot, *match), k, q)
+        idx, dis, cmd, rej = decide(scores(ftr, bank, n_slot, *match), k, q)
         for i, (b, j) in enumerate(todo):
             r = segs[b, j]
             r["best_idx"], r["best_dis"], r["cmd"], r["status"] = idx[i], dis[i], cmd[i], 3 if rej[i] else 0

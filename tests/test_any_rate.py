@@ -7,7 +7,7 @@ four digit recordings. GPU: the setter and flag rules; sr_dtw_batch equals the o
 1..119 x 1..119 at radii that pick each band kernel, and plain SR_DTW_BAND on every pair within 2:1; every recognition
 path under the matcher equals the oracle composition, and a bank of stretched and shrunk templates makes the guard change
 decisions; bytes written and timing tags are the band matcher's; real speech, reported.
-sr_recognise_batch_dev_allgather is not run here: it needs two NCCL ranks. Every GPU test makes its own handles."""
+sr_recognise_batch_dev_allgather is run on a one-rank communicator by test_decision_paths.py. Every GPU test makes its own handles."""
 import itertools
 import os
 import re

@@ -780,15 +780,15 @@ RECREATED = "dtw_dynamic"                # the job whose thread destroys its han
 
 # sr_* entry points of the headers that no job runs, each with the reason
 EXCLUDED = {
-    "sr_comm_unique_id": "NCCL: needs two ranks, one per GPU",
-    "sr_comm_create": "NCCL: needs two ranks, one per GPU",
-    "sr_comm_destroy": "NCCL: needs two ranks, one per GPU",
-    "sr_comm_rank": "NCCL: needs two ranks, one per GPU",
-    "sr_comm_world": "NCCL: needs two ranks, one per GPU",
-    "sr_comm_nccl_version": "NCCL: needs two ranks, one per GPU",
-    "sr_comm_wait": "NCCL: needs two ranks, one per GPU",
-    "sr_allgather_dev": "NCCL: needs two ranks, one per GPU",
-    "sr_recognise_batch_dev_allgather": "NCCL: needs two ranks, one per GPU",
+    "sr_comm_unique_id": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_comm_create": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_comm_destroy": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_comm_rank": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_comm_world": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_comm_nccl_version": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_comm_wait": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_allgather_dev": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
+    "sr_recognise_batch_dev_allgather": "NCCL: a communicator of its own; test_decision_paths.py runs it on one rank",
     "sr_recognise_batch_multi": "requires handles on different devices",
     "sr_stream_group_push_ragged": "the group's ragged push is the pool's ragged push per shard; the stream_pool job runs it",
     "sr_streams_push": "the lock-step push is a ragged push with equal lengths; stream_pool and stream_group run both forms",

@@ -9,7 +9,8 @@ path (host plain and packed, _dev, _multi, the long-form host and _dev calls, fi
 under each matcher, k = 1 .. 4, with and without the margin rule, on banks with erased slots, a width that is not a
 multiple of 4, planted ties, rows without a score and more than 32 commands, equals the numpy rule applied to the
 oracle-checked scores; KNN(1) equals no rule bit for bit; bytes written; unequal rules refused by _multi.
-sr_recognise_batch_dev_allgather and stream groups over two devices are not run here: they need two ranks or two GPUs."""
+sr_recognise_batch_dev_allgather is run on a one-rank communicator by test_decision_paths.py; stream groups over two
+devices are not run here: they need two GPUs."""
 import os
 
 import numpy as np
@@ -18,7 +19,7 @@ import pytest
 import oracle_bind as ob
 import oracle_ext as ox
 import sr_b200
-from cases import synth_long_poisoned
+from cases import synth_long_poisoned, word_bank
 from drive import cmp_long, event_key, handle, k4_events, k14_events, recognise_dev_np, recognise_long_dev_np, same
 from refs import decide
 
@@ -55,37 +56,15 @@ def knn_brute(row, k, q):
 
 
 # ---- banks -----------------------------------------------------------------------------------------------------------------
-def _bank(T, seed, erase=(), dup=(), trunc=None):
-    """T slots from synthetic one-word templates: command c's four slots are one word with one row dropped each (row
-    k * 7, none for k = 0), optionally cut to trunc(t) frames; dup (a, b) copies slot a into slot b; erase: unsigned"""
-    n_cmd = (T + 3) // 4
-    e = ob.recognise_pinned(ob.best_oracle(), sr_b200.synth_pcm_host(n_cmd, 8000, seed), 2400, None, 0, 4096)
-    ftr = np.zeros(4 * n_cmd, ob.FTR_DTYPE)
-    for t in range(4 * n_cmd):
-        f = e["ftr"][t // 4]
-        n = int(f["frm_num"])
-        rows = f["mfcc_dat"][:n * 12].reshape(n, 12)
-        x = rows if t % 4 == 0 else np.delete(rows, min((t % 4) * 7, n - 1), axis=0)
-        if trunc:
-            x = x[:trunc(t)]
-        ftr[t]["frm_num"] = len(x)
-        ftr[t]["mfcc_dat"][:x.size] = x.reshape(-1)
-    for a, b in dup:
-        ftr[b] = ftr[a]
-    valid = np.ones(T, bool)
-    valid[list(erase)] = False
-    return sr_b200.make_bank(ftr[:T], 4096, valid)
-
-
 # signed: every slot signed; erased: n_c < k and n_c = 0, 78 slots, ties inside a command (16 = 17) and between commands
 # (command 6 = command 5); short: templates of 13 .. 20 frames, so that the longer inputs score SR_DIS_ERR against every
 # slot under the 2:1 guard; wide: 38 commands (the warp-per-utterance finishers), 150 slots
 BANKS = {
-    "signed": lambda: (_bank(80, 0x7E700000), 80),
-    "erased": lambda: (_bank(78, 0x7E710000, erase=(5, 6, 7, 8, 9, 10, 11, 13, 30, 31, 77),
-                             dup=((16, 17), (20, 24), (21, 25), (22, 26), (23, 27))), 78),
-    "short": lambda: (_bank(40, 0x7E720000, trunc=lambda t: 13 + t % 8), 40),
-    "wide": lambda: (_bank(150, 0x7E730000, erase=(1, 2, 3, 40, 41, 42, 43, 149)), 150),
+    "signed": lambda: (word_bank(80, 0x7E700000), 80),
+    "erased": lambda: (word_bank(78, 0x7E710000, erase=(5, 6, 7, 8, 9, 10, 11, 13, 30, 31, 77),
+                                  dup=((16, 17), (20, 24), (21, 25), (22, 26), (23, 27))), 78),
+    "short": lambda: (word_bank(40, 0x7E720000, trunc=lambda t: 13 + t % 8), 40),
+    "wide": lambda: (word_bank(150, 0x7E730000, erase=(1, 2, 3, 40, 41, 42, 43, 149)), 150),
 }
 
 

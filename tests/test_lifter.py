@@ -11,7 +11,8 @@ under all four matchers at radii that pick each band kernel, on every (I, M) in 
 every recognition path (host plain and packed, _dev, _multi, the long-form host and _dev calls, fixed-capture pools and
 live long streams) under each matcher with the bit, and with the decision rules on top, equals the oracle composition;
 _multi refuses a lifter/plain mix; launches, timing tags and bytes written are the flag-off matcher's.
-sr_recognise_batch_dev_allgather and stream groups over two devices are not run here: they need two ranks or two GPUs.
+sr_recognise_batch_dev_allgather is run on a one-rank communicator by test_decision_paths.py; stream groups over two
+devices are not run here: they need two GPUs.
 Every GPU test makes its own handles."""
 import os
 import re

@@ -7,7 +7,7 @@ flag rules; sr_dtw_batch* refuse the rule's bits before anything runs; every rec
 q equals the same call without the rule except for SR_ST_REJECT, which appears exactly where the rule, applied to the
 oracle-checked scores, says; banks of 1 .. 1024 slots and batches around the grid's row count; launches, timing tags and
 bytes written are the rule-off call's; unequal rules are refused by _multi and groups; two threads with different rules.
-sr_recognise_batch_dev_allgather is not run here: it needs two NCCL ranks."""
+sr_recognise_batch_dev_allgather is run on a one-rank communicator by test_decision_paths.py."""
 import os
 import re
 import threading

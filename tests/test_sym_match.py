@@ -6,7 +6,7 @@ P = 1 path (each complete path weighs I + M, the cheapest one is g); a planted b
 GPU: sr_dtw_batch under SR_DTW_SYM_P1 equals the oracle bit for bit at every radius, bank width and shape; the setter
 rules; every recognition path under the matcher equals the oracle composition (front end, the C oracle's scores, the strict
 '<' first-wins argmin, cmd = idx / 4); the matcher switched between pushes; tag 14 where tag 6 is under the band matcher;
-threads; real speech, reported. sr_recognise_batch_dev_allgather is not run here: it needs two NCCL ranks.
+threads; real speech, reported. sr_recognise_batch_dev_allgather is run on a one-rank communicator by test_decision_paths.py.
 Every GPU test makes its own handles, so the session handle never carries a matcher."""
 import itertools
 import os
