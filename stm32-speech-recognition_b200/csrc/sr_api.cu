@@ -224,8 +224,7 @@ static bool capture_args_ok(u32 U, u32 B, u32 n_len) { return (B == 0 || U > 0) 
 // the B atap records noise_atap runs on: the caller's (atap != NULL), else B zeroed ones in w
 static cudaError_t atap_or_zeroed(sr_handle *h, DevBuf &w, u32 B, atap_tag *&atap) {
     if (atap) return cudaSuccess;
-    const cudaError_t e = ensure(w, (size_t)B * sizeof(atap_tag));
-    atap = static_cast<atap_tag *>(w.p);
+    const cudaError_t e = ensure(w, (size_t)B * sizeof(atap_tag), atap);
     return e != cudaSuccess ? e : cudaMemsetAsync(atap, 0, (size_t)B * sizeof(atap_tag), h->stream);
 }
 
@@ -236,8 +235,8 @@ struct HostCall {
     const char *name;
     DeviceGuard g;
     int rc = 0;
-    struct Back { void *dst; const void *src; size_t bytes; bool ftr; } back[8];
-    int n_back = 0;
+    struct Back { void *dst; const void *src; size_t bytes; bool ftr; };
+    std::vector<Back> back;
 
     HostCall(sr_handle *hh, const char *nm) : h(hh), name(nm), g(hh->device) {}
     void took(int r) {
@@ -266,7 +265,7 @@ struct HostCall {
     // workspace w for an output that finish() copies back to dst (if dst != NULL); v_ftr_tag outputs skip save_sign
     template <class T> T *out(DevBuf &w, T *dst, size_t bytes, size_t slack = 0) {
         T *d = ws<T>(w, bytes + slack);
-        if (d && dst && bytes) back[n_back++] = {dst, d, bytes, std::is_same_v<T, v_ftr_tag>};
+        if (d && dst && bytes) back.push_back({dst, d, bytes, std::is_same_v<T, v_ftr_tag>});
         return d;
     }
     // B atap records in w (atap_or_zeroed): the caller's host records staged in -- and copied back when `back`: noise_atap
@@ -279,11 +278,9 @@ struct HostCall {
         return rc ? nullptr : d;
     }
     int finish() {
-        for (int i = 0; i < n_back; ++i) {
-            const Back &b = back[i];
+        for (const Back &b : back)
             ck("copy back", b.ftr ? ftr_to_host(h, static_cast<v_ftr_tag *>(b.dst), b.src, b.bytes / kFtrBytes)
                                   : cudaMemcpyAsync(b.dst, b.src, b.bytes, cudaMemcpyDeviceToHost, h->stream));
-        }
         ck("cudaStreamSynchronize", cudaStreamSynchronize(h->stream));
         return rc;
     }
@@ -453,7 +450,7 @@ static int dtw_dev_impl(sr_handle *h, const BankView &bank, const v_ftr_tag *in,
     SR_REQUIRE(h, scan_plan(flags, band_r, B ? bank.n : 0, status != nullptr, &p));
     if (B == 0) return 0;
     const bool want_best = best_idx || best_dis || cmd || p.rule.C;
-    DevBuf &bb = h->best_sel ? h->best_alt : h->best;
+    DevBuf &bb = key_buf(h);
     u64 *keys;
     if (const int rc = scan_to_keys(h, want_best ? &bb : nullptr, p, bank, in, B, score, status, keys)) return rc;
     u64 *best = static_cast<u64 *>(bb.p);
@@ -516,11 +513,11 @@ int recognise_dev_impl(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     atap_tag *atap = o->atap;
     SR_CK(h, atap_or_zeroed(h, h->atap, B, atap));
     u32 *seg = o->seg_off;
-    if (!seg) { SR_CK(h, ensure(h->seg, (size_t)B * 24)); seg = static_cast<u32 *>(h->seg.p); }
+    SR_CK(h, caller_or_ws(h->seg, (size_t)B * 24, seg));
     v_ftr_tag *ftr = o->ftr;
-    if (!ftr) { SR_CK(h, ensure(h->ftr, (size_t)B * kFtrBytes)); ftr = static_cast<v_ftr_tag *>(h->ftr.p); }
+    SR_CK(h, caller_or_ws(h->ftr, (size_t)B * kFtrBytes, ftr));
     u8 *status = o->status;
-    if (!status) { SR_CK(h, ensure(h->status, (size_t)B)); status = static_cast<u8 *>(h->status.p); }
+    SR_CK(h, caller_or_ws(h->status, (size_t)B, status));
     if (const int rc = front_end(h, pcm, U, B, n_len, atap, seg, ftr, status)) return rc;
     if (h->comm) {                                       // collectives of earlier calls may still read score / the key buffer
         const int rc = wait_comm ? comm_wait_before_scan(h, o->score) : sr_comm_wait(h);
@@ -727,10 +724,10 @@ int sr_dtw_path_batch(sr_handle *h, const v_ftr_tag *in, const v_ftr_tag *mdl, u
     if (n == 0) return 0;
     HostCall c(h, "sr_dtw_path_batch");
     const size_t bytes = (size_t)n * kFtrBytes;
-    const v_ftr_tag *d_in = c.in(h->align[0], in, bytes), *d_mdl = c.in(h->align[1], mdl, bytes);
-    u8 *d_path = path ? c.out(h->align[2], path, (size_t)n * SR_PATH_MAX * 2) : nullptr;
-    u32 *d_len = path_len ? c.out(h->align[3], path_len, (size_t)n * 4) : nullptr;
-    u32 *d_dis = c.out(h->align[4], dis, (size_t)n * 4);
+    const v_ftr_tag *d_in = c.in(h->align.in_bank, in, bytes), *d_mdl = c.in(h->align.mdl_out, mdl, bytes);
+    u8 *d_path = path ? c.out(h->align.path, path, (size_t)n * SR_PATH_MAX * 2) : nullptr;
+    u32 *d_len = path_len ? c.out(h->align.len_pairs, path_len, (size_t)n * 4) : nullptr;
+    u32 *d_dis = c.out(h->align.dis_tpl, dis, (size_t)n * 4);
     c.launch(TAG_ALIGN, "launch_dtw_align", [&] {
         return launch_dtw_align(d_in, kFtrBytes, d_mdl, kFtrBytes, nullptr, n, band_r, d_path, d_len, d_dis, nullptr, nullptr,
                                 0, nullptr, nullptr, h->num_sms, h->stream);
@@ -772,20 +769,15 @@ int sr_average_bank(sr_handle *h, const void *bank, uint32_t slot_stride, uint32
     const u32 n_anchor = (u32)(pairs.size() / 3), n_member = (u32)(mpairs.size() / 3);
     pairs.insert(pairs.end(), mpairs.begin(), mpairs.end());
     HostCall c(h, "sr_average_bank");
-    const unsigned char *d_bank = c.in(h->align[0], b, slots * slot_stride);
-    void *d_out = c.out(h->align[1], bank_out, slots * slot_stride);
-    u8 *d_path = c.ws<u8>(h->align[2], slots * SR_PATH_MAX * 2);
-    const auto *d_pairs = c.in(h->align[3], pairs.data(), pairs.size() * 4, 16);
-    auto *d_tpl = c.ws<unsigned char>(h->align[4], (size_t)G * kFtrBytes);
-    auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t o_st = al((size_t)G * 4), o_S = o_st + al(G), o_len = o_S + al(slots * K * 4);
-    auto *misc = c.ws<unsigned char>(h->align[5], o_len + slots * 4);                 // mask | status | S | path_len
-    u32 *d_mask = misc ? reinterpret_cast<u32 *>(misc) : nullptr;
-    u8 *d_st = misc ? misc + o_st : nullptr;
-    u32 *d_S = misc ? reinterpret_cast<u32 *>(misc + o_S) : nullptr, *d_len = misc ? reinterpret_cast<u32 *>(misc + o_len) : nullptr;
+    const unsigned char *d_bank = c.in(h->align.in_bank, b, slots * slot_stride);
+    void *d_out = c.out(h->align.mdl_out, bank_out, slots * slot_stride);
+    u8 *d_path = c.ws<u8>(h->align.path, slots * SR_PATH_MAX * 2);
+    const auto *d_pairs = c.in(h->align.len_pairs, pairs.data(), pairs.size() * 4, 16);
+    auto *d_tpl = c.ws<unsigned char>(h->align.dis_tpl, (size_t)G * kFtrBytes);
+    u32 *d_mask = c.in(h->align.mask, mask.data(), (size_t)G * 4);
+    u8 *d_st = c.in(h->align.group_status, gst.data(), G);
+    u32 *d_S = c.ws<u32>(h->align.anchor_S, slots * K * 4), *d_len = c.ws<u32>(h->align.slot_len, slots * 4);
     u32 *d_score = c.out(h->score, score, slots * 4), *d_anchor = c.out(h->bidx, anchor, (size_t)G * 4);
-    c.h2d(d_mask, mask.data(), (size_t)G * 4);
-    c.h2d(d_st, gst.data(), G);
     auto fill = [&](void *p, int v, size_t bytes) { c.ck("cudaMemsetAsync", p ? cudaMemsetAsync(p, v, bytes, h->stream) : cudaSuccess); };
     fill(d_S, 0xFF, slots * K * 4);                      // non-member pairs: SR_DIS_ERR
     fill(d_len, 0, slots * 4);
@@ -856,15 +848,11 @@ static void run_pieces(HostCall &c, const u16 *d_pcm, u32 U, u32 n_rows, const L
     const u32 P = pc.size();
     for (u32 p0 = 0; p0 < P && !c.rc; p0 += kPieceChunk) {
         const u32 np = std::min(P - p0, kPieceChunk);
-        u32 *tab = c.ws<u32>(h->conn[0], (size_t)np * 5 * 4);
-        atap_tag *d_atap = c.ws<atap_tag>(h->conn[1], (size_t)np * sizeof(atap_tag));
-        void *d_pf = c.ws(h->conn[2], (size_t)np * kFtrBytes);
-        if (c.rc) return;
-        u32 *d_seg = tab, *d_row = tab + 2 * (size_t)np, *d_dst = tab + 3 * (size_t)np;
-        c.h2d(d_seg, pc.seg.data() + 2 * (size_t)p0, (size_t)np * 8);
-        c.h2d(d_row, pc.row.data() + p0, (size_t)np * 4);
-        c.h2d(d_dst, pc.dst.data() + 2 * (size_t)p0, (size_t)np * 8);
-        c.h2d(d_atap, pc.atap.data() + p0, (size_t)np * sizeof(atap_tag));
+        const u32 *d_seg = c.in(h->pieces.seg, pc.seg.data() + 2 * (size_t)p0, (size_t)np * 8);
+        const u32 *d_row = c.in(h->pieces.row, pc.row.data() + p0, (size_t)np * 4);
+        const u32 *d_dst = c.in(h->pieces.dst, pc.dst.data() + 2 * (size_t)p0, (size_t)np * 8);
+        const atap_tag *d_atap = c.in(h->pieces.atap, pc.atap.data() + p0, (size_t)np * sizeof(atap_tag));
+        void *d_pf = c.ws(h->pieces.ftr, (size_t)np * kFtrBytes);
         c.launch(TAG_MFCC, "launch_mfcc_h (pieces)", [&] { return launch_mfcc_h(h, d_pcm, U, np, d_seg, 2, d_atap, d_pf, d_row, n_rows); });
         c.launch(TAG_NONE, "launch_conn_gather", [&] { return launch_conn_gather(d_pf, d_dst, np, d_feat, h->num_sms, h->stream); });
     }
@@ -884,11 +872,11 @@ static ConnDev conn_outputs(HostCall &c, u32 B, u32 max_words, sr_conn_word *wor
     ConnDev d{nullptr, nullptr, nullptr};
     const size_t wbytes = (size_t)B * max_words * sizeof(sr_conn_word);
     if (words && max_words) {
-        d.words = c.in(h->conn[7], words, wbytes);
-        c.out(h->conn[7], words, wbytes);
+        d.words = c.in(h->conn.words, words, wbytes);
+        c.out(h->conn.words, words, wbytes);
     }
-    d.nw = n_words ? c.out(h->conn[8], n_words, (size_t)B * 4) : nullptr;
-    d.total = total ? c.out(h->conn[9], reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
+    d.nw = n_words ? c.out(h->conn.n_words, n_words, (size_t)B * 4) : nullptr;
+    d.total = total ? c.out(h->conn.total, reinterpret_cast<u64 *>(total), (size_t)B * 8) : nullptr;
     return d;
 }
 
@@ -937,8 +925,8 @@ int sr_mfcc_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     HostCall c(h, "sr_mfcc_long_batch");
     const size_t fbytes = (size_t)B * frm_cap * 24;
     const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    s16 *d_feat = c.in(h->conn[3], reinterpret_cast<const s16 *>(feat), fbytes);   // in / out: rows >= frm_num keep the caller's bytes
-    c.out(h->conn[3], feat, fbytes);
+    s16 *d_feat = c.in(h->conn.feat, reinterpret_cast<const s16 *>(feat), fbytes);   // in / out: rows >= frm_num keep the caller's bytes
+    c.out(h->conn.feat, feat, fbytes);
     run_pieces(c, d_pcm, U, B, pc, d_feat);
     const int rc = c.finish();
     if (rc == 0) memcpy(frm_num, F.data(), (size_t)B * 4);
@@ -953,8 +941,8 @@ int sr_connected_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_nu
     SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
     for (u32 b = 0; b < B; ++b) SR_REQUIRE(h, frm_num[b] <= SR_CONN_FRM_MAX && frm_num[b] <= frm_stride);
     HostCall c(h, "sr_connected_batch");
-    const s16 *d_feat = c.in(h->conn[3], feat, (size_t)B * frm_stride * 24);
-    const u32 *d_frm = c.in(h->conn[4], frm_num, (size_t)B * 4);
+    const s16 *d_feat = c.in(h->conn.feat, feat, (size_t)B * frm_stride * 24);
+    const u32 *d_frm = c.in(h->conn.seq_frm, frm_num, (size_t)B * 4);
     const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
     const BankView &bk = h->bank;
     for (u32 b0 = 0; b0 < B; b0 += kSeqChunk)
@@ -995,17 +983,14 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
         status[b] = seg_status(seg[b * 6 + 1], frm[b * 3]);
     }
     const u32 nseq = (u32)seq_frm.size(), rows = pc.rows;
-    s16 *d_feat = c.ws<s16>(h->conn[3], (size_t)rows * 24);
+    s16 *d_feat = c.ws<s16>(h->conn.feat, (size_t)rows * 24);
     run_pieces(c, d_pcm, U, B, pc, d_feat);
-    u32 *tab = c.ws<u32>(h->conn[4], ((size_t)nseq * 3 + (size_t)B * 3) * 4);         // seq_off | seq_frm | seq_of
-    sr_conn_word *d_sw = c.ws<sr_conn_word>(h->conn[5], (size_t)rows * sizeof(sr_conn_word));
-    u64 *d_stot = c.ws<u64>(h->conn[6], (size_t)nseq * 12);                           // seq totals | seq word counts
-    if (c.rc) return c.finish();
-    u32 *d_soff = tab, *d_sfrm = tab + 2 * (size_t)nseq, *d_sof = tab + 3 * (size_t)nseq;
-    u32 *d_snw = reinterpret_cast<u32 *>(d_stot + nseq);
-    c.h2d(d_soff, seq_off.data(), (size_t)nseq * 8);
-    c.h2d(d_sfrm, seq_frm.data(), (size_t)nseq * 4);
-    c.h2d(d_sof, seq_of.data(), (size_t)B * 12);
+    const u32 *d_soff = c.in(h->conn.seq_off, seq_off.data(), (size_t)nseq * 8);
+    const u32 *d_sfrm = c.in(h->conn.seq_frm, seq_frm.data(), (size_t)nseq * 4);
+    const u32 *d_sof = c.in(h->conn.seq_of, seq_of.data(), (size_t)B * 12);
+    sr_conn_word *d_sw = c.ws<sr_conn_word>(h->conn.seq_words, (size_t)rows * sizeof(sr_conn_word));
+    u64 *d_stot = c.ws<u64>(h->conn.seq_total, (size_t)nseq * 8);
+    u32 *d_snw = c.ws<u32>(h->conn.seq_n_words, (size_t)nseq * 4);
     const BankView &bk = h->bank;
     for (u32 b0 = 0; b0 < nseq; b0 += kSeqChunk)
         c.launch(TAG_CONN, "launch_dtw_connected", [&] {
@@ -1078,11 +1063,11 @@ struct RecordCuts {
     }
 };
 
-// the copy table of both grammar decoders staged in gram[5]; a grammar without copies stages one word (C = 0: no warp
+// the copy table of both grammar decoders staged in gram.copy; a grammar without copies stages one word (C = 0: no warp
 // walks, every sequence decodes to 0 words)
 static u32 *stage_copies(HostCall &c, const std::vector<u32> &copy) {
     static const u32 kNoCopy = 0;
-    return c.in(c.h->gram[5], copy.empty() ? &kNoCopy : copy.data(), std::max<size_t>(copy.size(), 1) * 4);
+    return c.in(c.h->gram.copy, copy.empty() ? &kNoCopy : copy.data(), std::max<size_t>(copy.size(), 1) * 4);
 }
 
 // the grammar decoder (tag 10) over B sequences of frames N[b]: seq [B][3] holds each first feature row and its segments
@@ -1093,9 +1078,9 @@ static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &
     const u32 B = (u32)N.size(), S = g->n_states;
     const RecordCuts cuts(B, (size_t)S * 8, [&](u32 b) { return N[b]; }, [&](u32 b) -> u32 & { return seq[3 * (size_t)b + 1]; });
     u32 *d_copy = stage_copies(c, copy);
-    u32 *d_seq = c.in(h->gram[0], seq.data(), (size_t)B * 12);
-    u32 *d_frm = c.in(h->gram[1], N.data(), (size_t)B * 4);
-    u64 *d_rec = c.ws<u64>(h->gram[2], std::max<size_t>(cuts.rows_max, 1) * S * 8);
+    u32 *d_seq = c.in(h->gram.seq, seq.data(), (size_t)B * 12);
+    u32 *d_frm = c.in(h->gram.frm, N.data(), (size_t)B * 4);
+    u64 *d_rec = c.ws<u64>(h->gram.rec, std::max<size_t>(cuts.rows_max, 1) * S * 8);
     const BankView &bk = h->bank;
     cuts.launches([&](u32 b0, u32 q0, u32 nq) {
         const ConnDev o = d.at(b0, max_words);
@@ -1125,7 +1110,7 @@ int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat, const uint32_t
         seq[3 * (size_t)b + 2] = 1023u << 10 | 1023u << 20;
     }
     HostCall c(h, "sr_connected_grammar_batch");
-    const s16 *d_feat = c.in(h->conn[3], feat, (size_t)B * frm_stride * 24);
+    const s16 *d_feat = c.in(h->conn.feat, feat, (size_t)B * frm_stride * 24);
     const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
     run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
     return c.finish();
@@ -1167,7 +1152,7 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
         status[b] = seg_status(seg[b * 6 + 1], frm[b * 3]);
     }
     if (c.rc) return c.finish();
-    s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(pc.rows, 1) * 24);
+    s16 *d_feat = c.ws<s16>(h->conn.feat, std::max<size_t>(pc.rows, 1) * 24);
     run_pieces(c, d_pcm, U, B, pc, d_feat);
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
     if (d.words || d.nw || d.total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
@@ -1192,8 +1177,8 @@ static bool long_host_args_ok(u32 U, u32 B, const u32 *lens, u32 n_len, u32 max_
 // segment pass (tag 12)
 static int vad_long_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, const u32 *lens, u32 n_len, u32 max_segs, atap_tag *atap,
                          u32 *n_segs, u32 *seg_off) {
-    SR_CK(h, ensure(h->lng[0], (size_t)B * long_info_stride(U) * 4));
-    u32 *info = static_cast<u32 *>(h->lng[0].p);
+    u32 *info;
+    SR_CK(h, ensure(h->lng.info, (size_t)B * long_info_stride(U) * 4, info));
     SR_LAUNCH(h, TAG_LONG_BLOCKS, launch_long_atap(pcm, U, B, lens, n_len, atap, h->stream));
     SR_LAUNCH(h, TAG_LONG_BLOCKS, launch_long_blocks(pcm, U, B, lens, atap, info, h->num_sms, h->stream));
     SR_LAUNCH(h, TAG_LONG_SEGS, launch_long_segments(U, B, lens, atap, info, max_segs, n_segs, seg_off, h->stream));
@@ -1208,25 +1193,27 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
                                const u32 *seg_off, sr_long_seg *rec) {
     const u32 M = B * max_segs;
     if (M == 0) return 0;
-    SR_CK(h, ensure(h->lng[2], ((size_t)B + 1) * 4));                  // first[B] | n_flat
-    SR_CK(h, ensure(h->lng[3], (size_t)M * 16));                       // seg2[M][2] | row[M] | slot[M]
-    SR_CK(h, ensure(h->lng[4], (size_t)M * sizeof(atap_tag)));
-    SR_CK(h, ensure(h->lng[5], (size_t)M));
-    SR_CK(h, ensure(h->lng[7], (size_t)M * kFtrBytes));
-    u32 *first = static_cast<u32 *>(h->lng[2].p), *n_flat = first + B;
-    u32 *seg2 = static_cast<u32 *>(h->lng[3].p), *row = seg2 + 2 * (size_t)M, *slot = row + M;
-    atap_tag *atap_seg = static_cast<atap_tag *>(h->lng[4].p);
-    u8 *status = static_cast<u8 *>(h->lng[5].p);
-    void *ftr = h->lng[7].p;
+    u32 *first, *n_flat, *seg2, *row, *slot;
+    atap_tag *atap_seg;
+    u8 *status;
+    void *ftr;
+    SR_CK(h, ensure(h->lng.first, (size_t)B * 4, first));
+    SR_CK(h, ensure(h->lng.n_flat, 4, n_flat));
+    SR_CK(h, ensure(h->lng.seg2, (size_t)M * 8, seg2));
+    SR_CK(h, ensure(h->lng.row, (size_t)M * 4, row));
+    SR_CK(h, ensure(h->lng.slot, (size_t)M * 4, slot));
+    SR_CK(h, ensure(h->lng.atap_seg, (size_t)M * sizeof(atap_tag), atap_seg));
+    SR_CK(h, ensure(h->lng.status, (size_t)M, status));
+    SR_CK(h, ensure(h->lng.ftr, (size_t)M * kFtrBytes, ftr));
     SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 0));
     SR_LAUNCH(h, TAG_NONE, launch_long_flatten(n_segs, seg_off, atap, B, max_segs, first, n_flat, seg2, row, slot, atap_seg, h->stream, 1));
     SR_LAUNCH(h, TAG_MFCC, launch_mfcc_h(h, pcm, U, M, seg2, 2, atap_seg, ftr, row, B, n_flat));     // main.c:268
     SR_LAUNCH(h, TAG_STATUS, launch_long_status(seg2, ftr, n_flat, M, status, h->stream));          // main.c:261-274
-    // main.c:276-291, save_sign honoured (main.c:283); a decision rule's key rows in lng[6]
+    // main.c:276-291, save_sign honoured (main.c:283); a decision rule's key rows in lng.keys
     ScanPlan p;
     scan_plan(SR_DTW_CHECK_SIGN | h->match_flags, h->match_r, h->bank.n, true, &p);    // flags sr_set_match accepted
     u64 *keys;
-    if (const int rc = scan_to_keys(h, &h->lng[6], p, h->bank, ftr, M, nullptr, status, keys, n_flat)) return rc;
+    if (const int rc = scan_to_keys(h, &h->lng.keys, p, h->bank, ftr, M, nullptr, status, keys, n_flat)) return rc;
     SR_LAUNCH(h, TAG_BEST_FINAL, launch_long_scatter(seg2, slot, ftr, status, keys, n_flat, M, rec, p.rule, h->stream));   // main.c:292-294
     return 0;
 }
@@ -1265,11 +1252,11 @@ int sr_recognise_long_batch_dev(sr_handle *h, const uint16_t *pcm, uint32_t U, u
     if (B == 0) return 0;
     DeviceGuard g(h->device);
     atap_tag *atap = o->atap;
-    SR_CK(h, atap_or_zeroed(h, h->lng[8], B, atap));
+    SR_CK(h, atap_or_zeroed(h, h->lng.atap, B, atap));
     u32 *n_segs = o->n_segs;
-    if (!n_segs) { SR_CK(h, ensure(h->lng[9], (size_t)B * 4)); n_segs = static_cast<u32 *>(h->lng[9].p); }
-    SR_CK(h, ensure(h->lng[1], (size_t)B * max_segs * 8 + 8));
-    u32 *seg_off = static_cast<u32 *>(h->lng[1].p);
+    SR_CK(h, caller_or_ws(h->lng.n_segs, (size_t)B * 4, n_segs));
+    u32 *seg_off;
+    SR_CK(h, ensure(h->lng.seg_off, (size_t)B * max_segs * 8 + 8, seg_off));
     if (const int rc = vad_long_impl(h, pcm, U, B, lens, n_len, max_segs, atap, n_segs, seg_off)) return rc;
     return recognise_segs_impl(h, pcm, U, B, max_segs, atap, n_segs, seg_off, o->segs);
 }
@@ -1280,14 +1267,14 @@ int sr_vad_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
     SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
     if (B == 0) return 0;
     HostCall c(h, "sr_vad_long_batch");
-    const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap = c.atap(h->lng[8], atap, B, true);
-    u32 *d_n = c.out(h->lng[9], n_segs, (size_t)B * 4);
+    const u32 *d_lens = lens ? c.in(h->lng.lens, lens, (size_t)B * 4) : nullptr;
+    atap_tag *d_atap = c.atap(h->lng.atap, atap, B, true);
+    u32 *d_n = c.out(h->lng.n_segs, n_segs, (size_t)B * 4);
     const size_t sbytes = (size_t)B * max_segs * 8;
     u32 *d_seg = nullptr;
     if (sbytes) {                                                           // in / out: segments past n_segs keep the caller's bytes
-        d_seg = c.in(h->lng[10], seg_off, sbytes);
-        c.out(h->lng[10], seg_off, sbytes);
+        d_seg = c.in(h->lng.per_seg, seg_off, sbytes);
+        c.out(h->lng.per_seg, seg_off, sbytes);
     }
     return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
         return sr_vad_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, d_atap + b0, d_n + b0,
@@ -1301,14 +1288,14 @@ int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint3
     SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
     if (B == 0) return 0;
     HostCall c(h, "sr_recognise_long_batch");
-    const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap = c.atap(h->lng[8], o->atap, B, true);
-    u32 *d_n = o->n_segs ? c.out(h->lng[9], o->n_segs, (size_t)B * 4) : nullptr;
+    const u32 *d_lens = lens ? c.in(h->lng.lens, lens, (size_t)B * 4) : nullptr;
+    atap_tag *d_atap = c.atap(h->lng.atap, o->atap, B, true);
+    u32 *d_n = o->n_segs ? c.out(h->lng.n_segs, o->n_segs, (size_t)B * 4) : nullptr;
     const size_t rbytes = (size_t)B * max_segs * sizeof(sr_long_seg);
     sr_long_seg *d_rec = nullptr;
     if (rbytes) {                                                           // in / out: records past n_segs keep the caller's bytes
-        d_rec = c.in(h->lng[10], o->segs, rbytes);
-        c.out(h->lng[10], o->segs, rbytes);
+        d_rec = c.in(h->lng.per_seg, o->segs, rbytes);
+        c.out(h->lng.per_seg, o->segs, rbytes);
     }
     return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
         const sr_long_out od{d_atap + b0, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
@@ -1329,9 +1316,9 @@ static void run_long_grammar(HostCall &c, const s16 *d_feat, std::vector<u32> &s
     const RecordCuts cuts(B, (size_t)S * 12, [&](u32 b) { return seq[4 * (size_t)b + 2]; },
                         [&](u32 b) -> u32 & { return seq[4 * (size_t)b + 3]; });
     u32 *d_copy = stage_copies(c, copy);
-    u32 *d_seq = c.in(h->gram[0], seq.data(), (size_t)B * 16);
-    u64 *recD = c.ws<u64>(h->gram[2], std::max<size_t>(cuts.rows_max, 1) * S * 8);
-    u32 *recS = c.ws<u32>(h->gram[3], std::max<size_t>(cuts.rows_max, 1) * S * 4);
+    u32 *d_seq = c.in(h->gram.seq, seq.data(), (size_t)B * 16);
+    u64 *recD = c.ws<u64>(h->gram.rec, std::max<size_t>(cuts.rows_max, 1) * S * 8);
+    u32 *recS = c.ws<u32>(h->gram.rec_state, std::max<size_t>(cuts.rows_max, 1) * S * 4);
     const BankView &bk = h->bank;
     cuts.launches([&](u32 b0, u32 q0, u32 nq) {
         const ConnDev o = d.at(b0, max_words);
@@ -1383,14 +1370,13 @@ int sr_connected_grammar_segs_batch(sr_handle *h, const int16_t *feat, const uin
     std::vector<u32> copy;
     if (const int rc = gram_copies(h, g, copy)) return rc;
     HostCall c(h, "sr_connected_grammar_segs_batch");
-    const s16 *d_feat = c.in(h->conn[3], feat, (size_t)rows * 24, 24);
-    u32 *tab = c.ws<u32>(h->gram[1], std::max<size_t>(n_seg, 1) * 8);   // seg_row [n_seg] | seg_frm [n_seg]
-    if (tab) {
-        c.h2d(tab, row.data(), (size_t)n_seg * 4);
-        c.h2d(tab + n_seg, seg_frm, (size_t)n_seg * 4);
-    }
+    const s16 *d_feat = c.in(h->conn.feat, feat, (size_t)rows * 24, 24);
+    u32 *d_row = c.ws<u32>(h->gram.seg_row, std::max<size_t>(n_seg, 1) * 4);
+    u32 *d_frm = c.ws<u32>(h->gram.frm, std::max<size_t>(n_seg, 1) * 4);
+    c.h2d(d_row, row.data(), (size_t)n_seg * 4);
+    c.h2d(d_frm, seg_frm, (size_t)n_seg * 4);
     const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
-    run_long_grammar(c, d_feat, seq, tab, tab + n_seg, copy, g, penalty, max_words, d);
+    run_long_grammar(c, d_feat, seq, d_row, d_frm, copy, g, penalty, max_words, d);
     return c.finish();
 }
 
@@ -1408,16 +1394,16 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
     if (const int rc = gram_copies(h, g, copy)) return rc;
     const u32 cap = long_seg_bound(U);
     HostCall c(h, "sr_recognise_long_grammar_batch");
-    const u32 *d_lens = lens ? c.in(h->lng[11], lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap = c.atap(h->lng[8], o->atap, B, true);
-    u32 *d_n = c.ws<u32>(h->lng[9], (size_t)B * 4);
+    const u32 *d_lens = lens ? c.in(h->lng.lens, lens, (size_t)B * 4) : nullptr;
+    atap_tag *d_atap = c.atap(h->lng.atap, o->atap, B, true);
+    u32 *d_n = c.ws<u32>(h->lng.n_segs, (size_t)B * 4);
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
     struct SegRec { u32 b, k, st, en, F; u8 status; };    // the records of segments k < max_segs
     std::vector<SegRec> recs;
     std::vector<u32> n_all(B), segv;
     std::vector<atap_tag> av;
     const int rc = long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) -> int {
-        u32 *d_seg = c.ws<u32>(h->gram[4], (size_t)nb * cap * 8);
+        u32 *d_seg = c.ws<u32>(h->gram.vad_segs, (size_t)nb * cap * 8);
         if (c.rc) return 0;
         if (const int r = vad_long_impl(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, cap, d_atap + b0, d_n + b0, d_seg))
             return r;
@@ -1449,13 +1435,13 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
             seq[4 * (size_t)q + 2] = N;
         }
         const u32 ns = (u32)row.size();
-        s16 *d_feat = c.ws<s16>(h->conn[3], std::max<size_t>(pc.rows, 1) * 24);
+        s16 *d_feat = c.ws<s16>(h->conn.feat, std::max<size_t>(pc.rows, 1) * 24);
         run_pieces(c, dpcm, U, nb, pc, d_feat);
-        u32 *tab = c.ws<u32>(h->gram[1], std::max<size_t>(ns, 1) * 8);   // seg_row [ns] | seg_frm [ns]
-        if (c.rc) return 0;
-        c.h2d(tab, row.data(), (size_t)ns * 4);
-        c.h2d(tab + ns, frm.data(), (size_t)ns * 4);
-        run_long_grammar(c, d_feat, seq, tab, tab + ns, copy, g, penalty, max_words, d.at(b0, max_words));
+        u32 *d_row = c.ws<u32>(h->gram.seg_row, std::max<size_t>(ns, 1) * 4);
+        u32 *d_frm = c.ws<u32>(h->gram.frm, std::max<size_t>(ns, 1) * 4);
+        c.h2d(d_row, row.data(), (size_t)ns * 4);
+        c.h2d(d_frm, frm.data(), (size_t)ns * 4);
+        run_long_grammar(c, d_feat, seq, d_row, d_frm, copy, g, penalty, max_words, d.at(b0, max_words));
         return 0;
     });
     if (rc) return rc;

@@ -211,17 +211,14 @@ int sr_recognise_batch_dev_allgather(sr_handle *h, const uint16_t *pcm, uint32_t
     SR_REQUIRE(h, !gathered_score || out_dev->score);
     DeviceGuard g(h->device);
     sr_recog_out o = *out_dev;
-    if (gathered_best && !o.best_idx) {                              // force the argmin so that h->best holds the keys
-        SR_CK(h, ensure(h->bidx, (size_t)B * 4));
-        o.best_idx = static_cast<u32 *>(h->bidx.p);
-    }
+    if (gathered_best) SR_CK(h, caller_or_ws(h->bidx, (size_t)B * 4, o.best_idx));   // the argmin forced: keys in key_buf
     // A gather issued earlier may still be reading score / best. Only the template scan rewrites them, so only it waits
     // (comm_wait_before_scan inside recognise_dev_impl) -- and with alternating buffers it waits for the gather of two calls
     // ago, so nothing on the handle's stream ever waits for the previous batch's collective.
     int rc = recognise_dev_impl(h, pcm, U, B, n_len, &o, true);
     if (rc) return rc;
     if (!gathered_score && !gathered_best) return 0;
-    const void *keys = h->best_sel ? h->best_alt.p : h->best.p;     // the buffer this call's template scan just filled
+    const void *keys = key_buf(h).p;                                 // the buffer this call's template scan just filled
     return allgather2(h, gathered_score ? o.score : nullptr, gathered_score, gathered_score ? (size_t)B * h->bank.n * 4 : 0,
                       gathered_best ? keys : nullptr, gathered_best, gathered_best ? (size_t)B * 8 : 0, o.score);
 }

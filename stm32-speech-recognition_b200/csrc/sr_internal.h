@@ -200,17 +200,63 @@ struct sr_handle {
     // grow-only device workspaces; scratch[] serves the secondary entry points (FFT, get_dis, get_mdl, dtw_limit, the
     // 12-bit expander, the sqrt check, enrol's bank image, dtw()'s one-slot bank) and is never read by a recognise call
     DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
-    DevBuf align[6];                                   // sr_dtw_path_batch / sr_average_bank: pairs, paths, templates, scores
-    DevBuf conn[10];                                   // long features and the connected-word decoder: pieces, features, words
-    DevBuf lng[12];                                    // long-form VAD and recognition (sr_long.h): block summaries, segments,
-                                                       // counts, the flat segment table, its atap, status, keys, features, lens
-                                                       // and the host calls' device outputs
-    DevBuf gram[6];                                    // both grammar decoders: sequence table, segment rows and frames (K6g: frame
-                                                       // counts), records (K13: both arrays), the long-form VAD segments of a
-                                                       // group, copy table
+    // The workspace table of the other call families: one buffer per thing held, each listed with what it holds and the
+    // calls that use it. Where calls put different things in one buffer, each call's contents are named.
+    //
+    // get_mfcc pieces of long segments, at most kPieceChunk per launch (run_pieces): sr_mfcc_long_batch,
+    // sr_recognise_connected_batch, sr_recognise_connected_grammar_batch, sr_recognise_long_grammar_batch
+    // - seg, row, dst: [P][2] start / end sample, [P] PCM row, [P][2] first long feature row / frames
+    // - atap, ftr: [P] the recording's atap, [P] the piece's features
+    struct { DevBuf seg, row, dst, atap, ftr; } pieces;
+    // connected words
+    // - feat: long feature rows. sr_mfcc_long_batch, sr_connected_batch, sr_recognise_connected_batch,
+    //   sr_connected_grammar_batch, sr_recognise_connected_grammar_batch, sr_connected_grammar_segs_batch,
+    //   sr_recognise_long_grammar_batch
+    // - seq_frm: frames per sequence. sr_connected_batch (the caller's frm_num), sr_recognise_connected_batch
+    // - seq_off, seq_of: [n][2] each sequence's first row and first word record, [B][3] each capture segment's sequence.
+    //   sr_recognise_connected_batch
+    // - seq_words, seq_total, seq_n_words: each sequence's word records, total and word count. sr_recognise_connected_batch
+    // - words, n_words, total: the caller's outputs (conn_outputs). sr_connected_batch, sr_recognise_connected_batch,
+    //   sr_connected_grammar_batch, sr_recognise_connected_grammar_batch, sr_connected_grammar_segs_batch,
+    //   sr_recognise_long_grammar_batch
+    struct { DevBuf feat, seq_frm, seq_off, seq_of, seq_words, seq_total, seq_n_words, words, n_words, total; } conn;
+    // both grammar decoders: run_grammar (sr_connected_grammar_batch, sr_recognise_connected_grammar_batch) and K13's
+    // run_long_grammar (sr_connected_grammar_segs_batch, sr_recognise_long_grammar_batch)
+    // - seq: the sequence table. run_grammar: [B][3]; K13: [B][4]
+    // - frm: run_grammar: frames per sequence; K13: frames per segment
+    // - seg_row: each segment's first feature row. K13
+    // - rec: records. run_grammar's; K13's 64-bit ones
+    // - rec_state: K13's 32-bit records
+    // - copy: the copy table (stage_copies). Both decoders
+    // - vad_segs: a group's long-form VAD segments. sr_recognise_long_grammar_batch
+    struct { DevBuf seq, frm, seg_row, rec, rec_state, copy, vad_segs; } gram;
+    // long-form VAD and recognition (sr_long.h)
+    // - info: block summaries (vad_long_impl). sr_vad_long_batch(_dev), sr_recognise_long_batch(_dev),
+    //   sr_recognise_long_grammar_batch
+    // - seg_off: the segments [B][max_segs][2]. sr_recognise_long_batch(_dev)
+    // - first, n_flat, seg2, row, slot, atap_seg, status, keys, ftr: the flat segment table (recognise_segs_impl): [B]
+    //   each recording's first flat segment, their count, [M][2] start / end sample, [M] PCM row, [M] record slot,
+    //   [M] atap, status, argmin or decision-rule keys, features. sr_recognise_long_batch(_dev)
+    // - atap, n_segs: [B] atap records and segment counts. sr_recognise_long_batch_dev (when the caller passes none),
+    //   sr_vad_long_batch, sr_recognise_long_batch, sr_recognise_long_grammar_batch
+    // - per_seg: the caller's per-segment output. sr_vad_long_batch: seg_off; sr_recognise_long_batch: the records
+    // - lens: the caller's lens. sr_vad_long_batch, sr_recognise_long_batch, sr_recognise_long_grammar_batch
+    struct { DevBuf info, seg_off, first, n_flat, seg2, row, slot, atap_seg, status, keys, ftr, atap, n_segs, per_seg, lens; } lng;
+    // alignment: sr_dtw_path_batch and sr_average_bank
+    // - in_bank: sr_dtw_path_batch: in; sr_average_bank: the bank image
+    // - mdl_out: sr_dtw_path_batch: mdl; sr_average_bank: the output bank image
+    // - path: the warping paths. Both
+    // - len_pairs: sr_dtw_path_batch: path_len; sr_average_bank: the pair list
+    // - dis_tpl: sr_dtw_path_batch: dis; sr_average_bank: the group templates
+    // - mask, group_status, anchor_S, slot_len: [G] member masks, [G] group status, [slots][K] anchor scores, [slots] path
+    //   lengths. sr_average_bank
+    struct { DevBuf in_bank, mdl_out, path, len_pairs, dis_tpl, mask, group_status, anchor_S, slot_len; } align;
     int best_sel = 0;                                  // which of best / best_alt the current recognise call uses (alternates when a
                                                        // communicator is attached: the previous call's keys may still be being gathered)
 };
+
+// the key buffer of the current recognise call
+inline DevBuf &key_buf(sr_handle *h) { return h->best_sel ? h->best_alt : h->best; }
 
 inline int fail(sr_handle *h, const char *what, cudaError_t e) {
     char buf[512];
@@ -266,6 +312,14 @@ inline cudaError_t ensure(DevBuf &b, size_t bytes) {
     b.cap = want;
     return cudaSuccess;
 }
+// ensure, with p set to the workspace
+template <class T> inline cudaError_t ensure(DevBuf &b, size_t bytes, T *&p) {
+    const cudaError_t e = ensure(b, bytes);
+    p = static_cast<T *>(b.p);
+    return e;
+}
+// the caller's buffer p, or when it is NULL workspace b grown to `bytes`
+template <class T> inline cudaError_t caller_or_ws(DevBuf &b, size_t bytes, T *&p) { return p ? cudaSuccess : ensure(b, bytes, p); }
 
 inline u32 *mfcc_work(sr_handle *h) {
     if (!h->mfcc_work.p) {
