@@ -397,13 +397,8 @@ struct DeviceGuard {
 // A push's step kernel appends the chunk and lists the segments it closed in ev / seg_ev / atap_ev / map_ev (n_ev of them,
 // at most cap); stream_core_recognise then runs get_mfcc on seg_ev (offsets inside PCM row map_ev of a [S][row_len]
 // buffer), the status, the handle's matcher and the packing of one sr_stream_event per segment, copies them back with the
-// push's one synchronisation and hands them out behind any queued ones.
-namespace srk {
-struct StreamEventDev {         // work list of the segments closed by the current push
-    u32 stream, segment, start, end;
-};
-}  // namespace srk
-
+// push's one synchronisation and hands them out behind any queued ones. The step kernels list them through
+// srk::StreamEvents (sr_vad_core.cuh).
 struct StreamCore {
     sr_handle *h = nullptr;
     u32 S = 0, cap = 0, stage_stride = 0;

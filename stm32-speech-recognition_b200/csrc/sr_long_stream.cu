@@ -5,13 +5,14 @@
 // One WARP per stream, built from the shared cores (sr_vad_core.cuh):
 //   * the chunk is appended to the stream's ring of R samples; a sample that lands in the ring's first M slots is also
 //     written to the mirror behind the ring, so every segment that can still be decoded is contiguous in the row;
-//   * noise_atap runs once the calibration window is complete (atap_stats / atap_finish);
+//   * noise_atap runs once the calibration window is complete (noise_atap_warp);
 //   * the new frames are evaluated in windows of at most W frames: the window's blocks are summarised into a per-stream
-//     scratch (block_scan / block_scan_split8; one block is summarised again by the next window), frames_pass runs over
-//     them with last_sig (`cin`) carried in device state, and long_fsm_window continues the endpoint FSM from its carried
-//     state (open or closed, the run at the edge) -- K12's loop, cut at push boundaries instead of every 1 024 frames;
-//   * a closed segment goes to the push's event list (one atomicAdd): its ring offsets, or SR_SEG_NULL when it has more
-//     than 119 frames (get_mfcc then gives frm_num 0 and SR_ST_MFCC_FAIL, as the batch call does).
+//     scratch (block_pass over ring slots; one block is summarised again by the next window), then vad_window runs
+//     frames_pass over them with last_sig (`cin`) and continues the endpoint FSM from its carried state (open or closed,
+//     the run at the edge), both kept in device state (StreamVad, as K4 keeps them) -- K12's loop, cut at push
+//     boundaries instead of every 1 024 frames;
+//   * a closed segment goes to the push's event list (StreamEvents, shared with K4): its ring offsets, or SR_SEG_NULL
+//     when it has more than 119 frames (get_mfcc then gives frm_num 0 and SR_ST_MFCC_FAIL, as the batch call does).
 // Recognition is K4's: get_mfcc on the event list with its row map, the status kernel, the handle's matcher and the
 // finish kernel, then one D2H copy and one synchronisation (stream_core_recognise, sr_stream.cu).
 #include "sr_internal.h"
@@ -23,11 +24,8 @@ namespace srk {
 struct LongStreamState {        // one per stream, device resident
     atap_tag atap;
     u32 n;                      // samples received since the last reset
-    u32 frames;                 // frames evaluated: frames < this one are final
-    u32 cin;                    // class of the last out-of-band sample in blocks < frames (carried last_sig, VAD.C:99)
     u32 calibrated;
-    u32 open, closed, run;      // LongFsm
-    u32 open_start;             // start of the open segment, SR_SEG_NULL when none is open
+    StreamVad vad;
 };
 
 __global__ void long_stream_reset_kernel(LongStreamState *st, u32 S, const u8 *which, const atap_tag *atap) {
@@ -36,7 +34,7 @@ __global__ void long_stream_reset_kernel(LongStreamState *st, u32 S, const u8 *w
     LongStreamState z;
     memset(&z, 0, sizeof z);
     if (atap) z.atap = atap[s];
-    z.open_start = SR_SEG_NULL;
+    z.vad.open_start = SR_SEG_NULL;
     st[s] = z;
 }
 
@@ -45,28 +43,16 @@ __global__ void long_stream_query_kernel(const LongStreamState *st, u32 S, u32 *
     if (s >= S) return;
     const LongStreamState v = st[s];
     out[s] = v.n;
-    out[S + s] = v.closed;
-    out[2 * S + s] = v.open ? v.open_start : SR_SEG_NULL;
+    out[S + s] = v.vad.f.n;
+    out[2 * S + s] = v.vad.f.open ? v.vad.open_start : SR_SEG_NULL;
     atap[s] = v.atap;
-}
-
-__device__ __forceinline__ void warp_copy(u16 *dst, const u16 *src, u32 len, int lane) {
-    if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
-        const u32 nv = len >> 3;
-        for (u32 i = lane; i < nv; i += 32) reinterpret_cast<uint4 *>(dst)[i] = reinterpret_cast<const uint4 *>(src)[i];
-        for (u32 i = 8 * nv + lane; i < len; i += 32) dst[i] = src[i];
-    } else {
-        for (u32 i = lane; i < len; i += 32) dst[i] = src[i];
-    }
 }
 
 // the FSM's actions on a live stream: remember where the open segment starts; list a closed one as an event
 struct StreamCloseAct {
-    u32 s, R, frame_len, cap, open_start;
+    u32 s, R, frame_len, open_start;
     atap_tag at;
-    StreamEventDev *ev;
-    u32 *seg_ev, *map_ev, *n_ev;
-    atap_tag *atap_ev;
+    StreamEvents q;
     __device__ __forceinline__ void open(int, u32, u32 frame) { open_start = 80u * frame; }          // VAD.C:178
     __device__ __forceinline__ void close(int lane, u32 n, u32 frame) {
         if (lane == 0) {
@@ -80,13 +66,7 @@ struct StreamCloseAct {
                 if (ms == 0 && st != 0) ms = R;
                 me = ms + len;
             }
-            const u32 e = atomicAdd(n_ev, 1u);
-            if (e < cap) {
-                StreamEventDev d; d.stream = s; d.segment = n; d.start = st; d.end = end;
-                ev[e] = d;
-                seg_ev[2 * e] = ms; seg_ev[2 * e + 1] = me;
-                atap_ev[e] = at; map_ev[e] = s;
-            }
+            q.emit(s, n, st, end, ms, me, at);
         }
         open_start = SR_SEG_NULL;
     }
@@ -132,51 +112,32 @@ long_stream_step_kernel(u16 *__restrict__ pcm, u32 R, u32 M, u32 row, u32 S, con
     if (!calibrated) {
         if (n_len != 0 && n_len % 240u == 0) {                        // else atap stays as given (VAD.C:33-36)
             if (n < n_len) { if (lane == 0) sp->n = n; return; }
-            u32 m, max_sum, abs_sum;
-            atap_stats(x, true, n_len, lane, m, max_sum, abs_sum);
-            atap_finish(at, n_len, m, max_sum, abs_sum);
+            noise_atap_warp(x, true, n_len, lane, at);
         }
         calibrated = 1;
     }
     const u32 mid = at.mid_val, a_thl = mid + at.n_thl, b_thl = mid - at.n_thl;          // VAD.C:112-113 (u32 wrap)
 
     // ---- the frames that became complete: frame k once n > 80k + 160 (VAD.C:121), in windows of <= W frames ---------
-    const u32 nfr = n > SR_FRAME_LEN ? (n - SR_FRAME_LEN + SR_FRAME_MOV - 1) / SR_FRAME_MOV : 0u;
-    u32 k = sp->frames, cin = sp->cin;
-    LongFsm f{sp->open != 0, sp->closed, sp->run};
-    StreamCloseAct act{s, R, frame_len, cap, sp->open_start, at, ev, seg_ev, map_ev, n_ev, atap_ev};
-    while (k < nfr) {
-        const u32 nw = min(W, nfr - k), nb = nw + 1;                 // frame j = blocks j, j + 1
-        for (u32 b0 = 0; b0 < nb; b0 += 32) {                         // blocks k + b0 .. into info[2 (b0 + i)]
-            const u32 left = nb - b0;
-            const u32 i0 = (u32)((80ull * (k + b0)) % R);             // R is a multiple of 80: no block straddles the wrap
-            if (left <= 4u && i0 + 80u * left <= R) {                 // few contiguous blocks: eight lanes per block
-                u32 bs, fl;
-                block_scan_split8(x + i0, lane, left, mid, a_thl, b_thl, bs, fl);
-                const u32 bi = b0 + (u32)(lane >> 3);
-                if ((lane & 7) == 0 && (u32)(lane >> 3) < left) { info[2 * bi] = bs; info[2 * bi + 1] = fl; }
-            } else if ((u32)lane < left) {
-                VadWarpView v;
-                v.x = x + (u32)((80ull * (k + b0 + (u32)lane)) % R);
-                v.vec_ok = true;                                      // rows and blocks are 16-byte aligned
-                u32 bs, fl;
-                block_scan(v, 0u, mid, a_thl, b_thl, bs, fl);
-                info[2 * (b0 + lane)] = bs; info[2 * (b0 + lane) + 1] = fl;
-            }
-        }
+    const u32 nfr = frames_of(n);
+    StreamVad v = sp->vad;
+    StreamCloseAct act{s, R, frame_len, v.open_start, at, {ev, seg_ev, map_ev, n_ev, atap_ev, cap}};
+    while (v.frames < nfr) {
+        const u32 k = v.frames, nw = min(W, nfr - k), nb = nw + 1;  // frame j = blocks j, j + 1
+        // block k + i at its ring slot: R is a multiple of 80, so no block straddles the wrap; rows and blocks are 16-byte
+        // aligned. The last pass's blocks may run eight lanes per block when they do not wrap.
+        auto blk = [&](u32 i) { return x + (u32)((80ull * (k + i)) % R); };
+        const u32 last = (nb - 1u) & ~31u;
+        block_pass(blk, nb, blk(last) + 80u * (nb - last) <= x + R, true, mid, a_thl, b_thl, info, lane);
         __syncwarp();
-        u32 aw = 0;                                                   // lane j: activity of frames k + 32j .. + 31
-        for (u32 j = 0; 32u * j < nw; ++j) {
-            const u32 word = frames_pass(info, k + 32u * j, k + nw, lane, at, cin, k);      // VAD.C:121-164
-            if ((u32)lane == j) aw = word;
-        }
-        long_fsm_window(aw, nw, k, lane, f, act);                     // VAD.C:164-216
+        vad_window(info, k, k, nw, lane, at, v.cin, v.f, act);
         __syncwarp();                                                 // the next window rewrites info
-        k += nw;
+        v.frames += nw;
     }
+    v.open_start = act.open_start;
     if (lane == 0) {
-        sp->atap = at; sp->n = n; sp->frames = k; sp->cin = cin; sp->calibrated = calibrated;
-        sp->open = f.open ? 1u : 0u; sp->closed = f.n; sp->run = f.run; sp->open_start = act.open_start;
+        sp->atap = at; sp->n = n; sp->calibrated = calibrated;
+        sp->vad = v;
     }
 }
 

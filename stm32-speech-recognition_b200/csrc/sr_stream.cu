@@ -7,12 +7,12 @@
 // result on the complete buffers (segments of sr_vad_batch; segment 0 = sr_recognise_batch). The reference only
 // ever recognises segment 0 (main.c:268); here all <= 3 segments are (SURVEY 8f-3).
 //
-// One WARP per stream, built from the batch kernel's pieces (sr_vad_core.cuh): the new samples are appended to the
-// stream's device row, the 80-sample blocks that became complete are summarised lane-parallel (16-byte loads, packed
-// compares), the summaries are kept per stream, the frames that became complete are evaluated from them and the
-// endpoint FSM is re-evaluated on the activity bitmap of the frames seen so far (a prefix of the capture yields exactly
-// the decisions the sequential FSM has taken by then). One push = one H2D copy, five kernels whose batch sizes are read
-// from device memory (no host round trip between VAD and recognition), one D2H copy, ONE synchronisation.
+// One WARP per stream, built from the shared VAD steps (sr_vad_core.cuh): the new samples are appended to the stream's
+// device row (warp_copy), the 80-sample blocks that became complete are summarised (block_pass) and kept per stream, and
+// the frames that became complete are evaluated from them (vad_window), with last_sig and the endpoint FSM's state
+// carried from push to push at frame granularity (StreamVad, as K14 carries them). After any push the FSM holds exactly
+// the decisions the sequential FSM has taken on the frames seen so far. One push = one H2D copy, five kernels whose batch
+// sizes are read from device memory (no host round trip between VAD and recognition), one D2H copy, ONE synchronisation.
 #include "sr_internal.h"
 #include "sr_vad_core.cuh"
 #include "sr_dtw_core.cuh"
@@ -25,12 +25,9 @@ struct StreamState {            // one per stream, device resident
     atap_tag atap;
     u32 n;                      // samples received
     u32 blocks_done;            // 80-sample blocks summarised
-    u32 word_base;              // frames < word_base are final (multiple of 32): their activity word is complete
-    u32 cin_base;               // class of the last out-of-band sample in blocks < word_base (carried last_sig, VAD.C:99)
     u32 calibrated;
-    u32 emitted;                // segments already reported
-    u32 seg[6];
-    u32 aw[32];                 // activity bitmap, frame f = bit f&31 of word f>>5 (<= 1024 frames: U <= 65535)
+    u32 seg[6];                 // segments so far, as sr_vad_batch gives them
+    StreamVad vad;
 };
 
 __global__ void stream_reset_kernel(StreamState *st, u32 S) {
@@ -39,13 +36,33 @@ __global__ void stream_reset_kernel(StreamState *st, u32 S) {
     StreamState z;
     memset(&z, 0, sizeof z);
     for (int i = 0; i < 6; ++i) z.seg[i] = SR_SEG_NULL;
+    z.vad.open_start = SR_SEG_NULL;
     st[s] = z;
 }
 
+// The FSM's actions on a capture: K0's segments in lanes, and an event for each of the first SR_MAX_VC_CON segments as it
+// closes, with the capture's own offsets
+struct CaptureAct : SegLanes {
+    u32 s, open_start;
+    atap_tag at;
+    StreamEvents q;
+    __device__ __forceinline__ void open(int lane, u32 n, u32 frame) {
+        SegLanes::open(lane, n, frame);
+        open_start = 80u * frame;
+    }
+    __device__ __forceinline__ void close(int lane, u32 n, u32 frame) {
+        SegLanes::close(lane, n, frame);
+        const u32 end = 80u * frame + 80u;
+        if (lane == 0 && n < SR_MAX_VC_CON) q.emit(s, n, open_start, end, open_start, end, at);
+        open_start = SR_SEG_NULL;
+    }
+};
+
 constexpr int kStreamWarps = 8;
 
-// lens == NULL: every stream receives uniform_len samples; else stream s receives lens[s] (0 = nothing this time)
-__global__ void __launch_bounds__(kStreamWarps * 32)
+// lens == NULL: every stream receives uniform_len samples; else stream s receives lens[s] (0 = nothing this time).
+// Three CTAs per SM: without that bound ptxas gives the kernel 128 registers (two CTAs); with it 80, no spills.
+__global__ void __launch_bounds__(kStreamWarps * 32, 3)
 stream_step_kernel(u16 *__restrict__ pcm, u32 L, u32 S, const u16 *__restrict__ chunk, u32 chunk_stride,
                    u32 uniform_len, const u32 *__restrict__ lens, u32 n_len, StreamState *__restrict__ state,
                    u32 *__restrict__ info_all, u32 info_stride, StreamEventDev *__restrict__ ev,
@@ -63,15 +80,7 @@ stream_step_kernel(u16 *__restrict__ pcm, u32 L, u32 S, const u16 *__restrict__ 
     {
         u32 len = lens ? lens[s] : uniform_len;
         if (len > L - n) len = L - n;                                 // the capture buffer is full (ADC.H:9 VcBuf_Len)
-        const u16 *src = chunk + (size_t)s * chunk_stride;
-        u16 *dst = x + n;
-        if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
-            const u32 nv = len >> 3;
-            for (u32 i = lane; i < nv; i += 32) reinterpret_cast<uint4 *>(dst)[i] = reinterpret_cast<const uint4 *>(src)[i];
-            for (u32 i = 8 * nv + lane; i < len; i += 32) dst[i] = src[i];
-        } else {
-            for (u32 i = lane; i < len; i += 32) dst[i] = src[i];
-        }
+        warp_copy(x + n, chunk + (size_t)s * chunk_stride, len, lane);
         n += len;
         __syncwarp();
     }
@@ -83,74 +92,34 @@ stream_step_kernel(u16 *__restrict__ pcm, u32 L, u32 S, const u16 *__restrict__ 
     if (!calibrated) {
         if (n < n_len) { if (lane == 0) sp->n = n; return; }
         calibrated = 1;
-        if (n_len != 0 && n_len % 240u == 0) {                        // else atap stays untouched (VAD.C:33-36)
-            u32 m, max_sum, abs_sum;
-            atap_stats(x, vec_ok, n_len, lane, m, max_sum, abs_sum);
-            atap_finish(at, n_len, m, max_sum, abs_sum);
-        }
+        if (n_len != 0 && n_len % 240u == 0) noise_atap_warp(x, vec_ok, n_len, lane, at);   // else untouched (VAD.C:33-36)
     }
     const u32 mid = at.mid_val, a_thl = mid + at.n_thl, b_thl = mid - at.n_thl;          // VAD.C:112-113 (u32 wrap)
 
     // frames i = 80k while i < L-160 (VAD.C:121) over the FINAL buffer length L; frame k = blocks k, k+1
-    const u32 nfr_total = L > SR_FRAME_LEN ? (L - SR_FRAME_LEN + SR_FRAME_MOV - 1) / SR_FRAME_MOV : 0;
-    const u32 nblk_total = nfr_total ? nfr_total + 1 : 0;
-    const u32 nb_avail = min(n / 80u, nblk_total);
+    const u32 nfr_total = frames_of(L);
+    const u32 nb_avail = min(n / 80u, nfr_total ? nfr_total + 1 : 0u);
 
-    // ---- summaries of the blocks that became complete -------------------------------------------------------------
-    u32 blocks_done = sp->blocks_done;
-    for (u32 blk0 = blocks_done; blk0 < nb_avail; blk0 += 32) {
-        const u32 left = nb_avail - blk0;
-        const u16 *xb = x + 80u * blk0;
-        if (left <= 4u && (reinterpret_cast<uintptr_t>(xb) & 3) == 0) {            // few blocks: eight lanes per block
-            u32 bs, fl;
-            block_scan_split8(xb, lane, left, mid, a_thl, b_thl, bs, fl);
-            const u32 blk = blk0 + (u32)(lane >> 3);
-            if ((lane & 7) == 0 && blk < nb_avail) { info[2 * blk] = bs; info[2 * blk + 1] = fl; }
-        } else if ((u32)lane < left) {
-            VadWarpView v;
-            v.x = xb; v.vec_ok = (reinterpret_cast<uintptr_t>(xb) & 15) == 0;
-            u32 bs, fl;
-            block_scan(v, 80u * (u32)lane, mid, a_thl, b_thl, bs, fl);
-            info[2 * (blk0 + lane)] = bs; info[2 * (blk0 + lane) + 1] = fl;
-        }
-    }
-    blocks_done = max(blocks_done, nb_avail);
+    // ---- summaries of the blocks that became complete (rows and blocks share their alignment: 80 samples = 160 B) ---
+    const u32 blocks_done = sp->blocks_done;                           // <= nb_avail: n never decreases
+    block_pass([&](u32 i) { return x + 80u * (blocks_done + i); }, nb_avail - blocks_done,
+               (reinterpret_cast<uintptr_t>(x) & 3) == 0, vec_ok, mid, a_thl, b_thl, info + 2 * blocks_done, lane);
     __syncwarp();
 
-    // ---- frames that became complete: activity bitmap (the partial 32-frame word is simply re-evaluated) ------------
+    // ---- the frames that became complete, the FSM carried from the previous push; events for the segments closed ----
     const u32 ready = nb_avail ? min(nfr_total, nb_avail - 1u) : 0u;
-    u32 aw = sp->aw[lane];
-    u32 k0 = sp->word_base, cin = sp->cin_base;
-    while (k0 < ready) {
-        const u32 kend = min(ready, k0 + 32u);
-        u32 c = cin;
-        const u32 word = frames_pass(info, k0, kend, lane, at, c);
-        if ((u32)lane == (k0 >> 5)) aw = word;
-        if (kend != k0 + 32u) break;                                   // partial word: base and carry stay where they are
-        cin = c; k0 += 32u;
+    StreamVad v = sp->vad;
+    CaptureAct act{{lane < 6 ? sp->seg[lane] : SR_SEG_NULL}, s, v.open_start, at, {ev, seg_ev, map_ev, n_ev, atap_ev, cap}};
+    if (v.frames < ready) {
+        vad_window(info, 0u, v.frames, ready - v.frames, lane, at, v.cin, v.f, act);   // <= 818 frames: L <= 65535
+        v.frames = ready;
     }
-
-    // ---- endpoint FSM on the frames seen so far; report the segments that closed in this push -----------------------
-    u32 seg[6] = {SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL};
-    if (ready) fsm_segments(aw, ready, lane, seg);
-    u32 emitted = sp->emitted;
+    v.open_start = act.open_start;
     if (lane == 0) {
-        for (u32 sgi = emitted; sgi < SR_MAX_VC_CON && seg[2 * sgi + 1] != SR_SEG_NULL; ++sgi) {
-            const u32 e = atomicAdd(n_ev, 1u);
-            if (e < cap) {
-                StreamEventDev d; d.stream = s; d.segment = sgi; d.start = seg[2 * sgi]; d.end = seg[2 * sgi + 1];
-                ev[e] = d;
-                seg_ev[2 * e] = d.start; seg_ev[2 * e + 1] = d.end;
-                atap_ev[e] = at; map_ev[e] = s;
-            }
-            ++emitted;
-        }
-        sp->atap = at; sp->n = n; sp->blocks_done = blocks_done; sp->word_base = k0; sp->cin_base = cin;
-        sp->calibrated = calibrated; sp->emitted = emitted;
-#pragma unroll
-        for (int i = 0; i < 6; ++i) sp->seg[i] = seg[i];
+        sp->atap = at; sp->n = n; sp->blocks_done = nb_avail; sp->calibrated = calibrated;
+        sp->vad = v;
     }
-    sp->aw[lane] = aw;
+    if (lane < 6) sp->seg[lane] = act.seg;
 }
 
 __global__ void stream_segments_kernel(const StreamState *st, u32 S, u32 *seg_off, atap_tag *atap, u32 *n_recv) {

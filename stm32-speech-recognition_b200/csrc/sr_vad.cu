@@ -4,8 +4,10 @@
 // that start late take fewer). A warp's utterances form one stream of 32-block chunks (2560 samples)
 // through two shared-memory buffers: 1-D bulk async copies (TMA engine) keep the next chunk in flight while the
 // current one is scanned, so HBM traffic is the algorithmic 2*U bytes per utterance.
-//   * noise_atap: from the first staged chunk, three lanes per 240-sample block (IDP.2A sums, 16-byte loads);
-//   * VAD features: frames overlap by 50 %, so the scan works on 80-sample BLOCKS (each sample is
+// Each chunk runs the shared steps of sr_vad_core.cuh on the staged samples:
+//   * noise_atap (noise_atap_warp): from the first staged chunk, three lanes per 240-sample block (IDP.2A sums, 16-byte
+//     loads);
+//   * VAD features (block_pass): frames overlap by 50 %, so the scan works on 80-sample BLOCKS (each sample is
 //     touched once) and frame k = block k + block k+1. A block summary is a small monoid element:
 //     sum |x-mid|, number of class alternations among its out-of-band samples, class of the last
 //     out-of-band sample (the first one follows from the parity of the alternations). The band-
@@ -13,9 +15,10 @@
 //     (VAD.C:99): entering frame k it is the class of the last out-of-band sample at index <= i_k+78.
 //     Only ONE pair per frame can see that carried-in state (the pair ending at the frame's first
 //     out-of-band sample), so it is applied as a +1 correction; the carry itself is a warp scan.
-//   * endpoint FSM (VAD.C:164-216): 8 consecutive active frames open a segment at the first of
-//     them, 11 consecutive inactive frames close it at the first of those -- evaluated with bit
-//     tricks on the per-frame activity bitmap (one 32-frame word per lane) instead of a serial walk.
+//   * frames and endpoint FSM (vad_window, once per utterance from a fresh FSM state): 8 consecutive active frames open
+//     a segment at the first of them, 11 consecutive inactive frames close it at the first of those -- evaluated with
+//     bit tricks on the per-frame activity bitmap (one 32-frame word per lane) instead of a serial walk. The segments
+//     are held in lanes (SegLanes): lane j < 6 is seg_off[j], so segments past the third are dropped without a branch.
 #include "sr_vad_core.cuh"
 
 namespace srk {
@@ -42,9 +45,7 @@ vad_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, u32 n_len, u32 buf_len, in
 
     // the same for every utterance of the launch
     const bool atap_on = do_atap && n_len != 0 && (n_len % 240u) == 0 && n_len <= U;   // VAD.C:33-36: else untouched
-    // frames i = 0,80,.. while i < buf_len-160 (VAD.C:121); buf_len <= 160 reads past the buffer in the reference
-    // (int -> u32 compare) -- here: no frames.
-    const u32 nfr = (do_vad && buf_len > SR_FRAME_LEN && buf_len <= U) ? (buf_len - SR_FRAME_LEN + SR_FRAME_MOV - 1) / SR_FRAME_MOV : 0;
+    const u32 nfr = (do_vad && buf_len <= U) ? frames_of(buf_len) : 0;
     const u32 nblk = nfr ? nfr + 1 : 0;                            // frame k = blocks k, k+1
     const u32 vad_samples = 80u * nblk;                            // <= buf_len
     const bool atap_staged = atap_on && n_len <= kVadChunk;        // noise_atap from the first staged chunk
@@ -75,9 +76,7 @@ vad_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, u32 n_len, u32 buf_len, in
 
         // ---- noise_atap, VAD.C:22-71, when the window does not fit the first chunk: straight from global ------------
         if (atap_on && !atap_staged) {
-            u32 m, max_sum, abs_sum;
-            atap_stats(pcm + ubase, false, n_len, lane, m, max_sum, abs_sum);
-            atap_finish(at, n_len, m, max_sum, abs_sum);
+            noise_atap_warp(pcm + ubase, false, n_len, lane, at);
             if (lane == 0) atap[b] = at;
         }
         u32 mid = at.mid_val, a_thl = mid + at.n_thl, b_thl = mid - at.n_thl;            // VAD.C:112-113 (u32 wrap)
@@ -97,53 +96,27 @@ vad_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, u32 n_len, u32 buf_len, in
                                             min(kVadChunk, total - nc0), &bars[warp][odd ? 0 : 1], lane);
             }
             const int shift = shift_cur;
-            VadWarpView v;
-            v.x = reinterpret_cast<const u16 *>(buf) + shift;
-            v.vec_ok = (shift & 7) == 0;
+            const u16 *x = reinterpret_cast<const u16 *>(buf) + shift;
             if (c0 == 0 && atap_staged) {
-                u32 m, max_sum, abs_sum;
-                atap_stats(v.x, v.vec_ok, n_len, lane, m, max_sum, abs_sum);   // VAD.C:41-63
-                atap_finish(at, n_len, m, max_sum, abs_sum);
+                noise_atap_warp(x, (shift & 7) == 0, n_len, lane, at);
                 if (lane == 0) atap[b] = at;
-                mid = m; a_thl = mid + at.n_thl; b_thl = mid - at.n_thl;
+                mid = at.mid_val; a_thl = mid + at.n_thl; b_thl = mid - at.n_thl;
             }
             const u32 blk0 = c0 / 80u;
-            const u32 left = nblk > blk0 ? nblk - blk0 : 0u;                   // blocks of this chunk
-            if (left <= 4u && (shift & 1) == 0) {                              // few blocks: eight lanes per block
-                if (left) {
-                    u32 bs, fl;
-                    block_scan_split8(v.x, lane, left, mid, a_thl, b_thl, bs, fl);
-                    const u32 blk = blk0 + (u32)(lane >> 3);
-                    if ((lane & 7) == 0 && blk < nblk) { info[2 * blk] = bs; info[2 * blk + 1] = fl; }
-                }
-            } else if ((u32)lane < left) {
-                const u32 blk = blk0 + (u32)lane;
-                u32 bs, fl;
-                block_scan(v, 80u * (u32)lane, mid, a_thl, b_thl, bs, fl);
-                info[2 * blk] = bs; info[2 * blk + 1] = fl;
-            }
+            const u32 left = nblk > blk0 ? min(32u, nblk - blk0) : 0u;         // blocks of this chunk
+            block_pass([&](u32 i) { return x + 80u * i; }, left, (shift & 1) == 0, (shift & 7) == 0, mid, a_thl, b_thl,
+                       info + 2 * blk0, lane);
             __syncwarp();                                                      // this buffer is re-staged one chunk later
             shift_cur = shift_nxt;
         }
 
         // ---- VAD, VAD.C:97-218: frames from the block summaries ---------------------------------------------------
         if (do_vad) {
-            u32 seg[6] = {SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL, SR_SEG_NULL};
-            if (nfr > 0) {
-                u32 aw = 0;                                                    // lane j: activity of frames 32j..32j+31
-                u32 cin = 0;                                                   // class of last out-of-band sample before this pass
-                for (u32 k0 = 0, j = 0; k0 < nfr; k0 += 32, ++j) {
-                    const u32 word = frames_pass(info, k0, nfr, lane, at, cin);
-                    if ((u32)lane == j) aw = word;
-                }
-                fsm_segments(aw, nfr, lane, seg);                             // endpoint FSM on the bitmap
-            }
-            if (lane < 6) {
-                u32 val = seg[0];
-#pragma unroll
-                for (int j = 1; j < 6; ++j) if (lane == j) val = seg[j];
-                seg_off[(size_t)b * 6 + lane] = val;
-            }
+            u32 cin = 0;                                                       // last_sig before the first frame
+            LongFsm f{false, 0u, 0u};
+            SegLanes act{SR_SEG_NULL};
+            vad_window(info, 0u, 0u, nfr, lane, at, cin, f, act);             // nfr <= 818: U <= 65535
+            if (lane < 6) seg_off[(size_t)b * 6 + lane] = act.seg;
         }
         __syncwarp();
         b = have_next ? b_next : (work ? claim() : b + stride);
@@ -160,7 +133,7 @@ cudaError_t launch_vad(const u16 *pcm, u32 U, u32 B, u32 n_len, u32 buf_len, int
                        atap_tag *atap, u32 *seg_off, int num_sms, cudaStream_t st, u32 *work) {
     if (B == 0) return cudaSuccess;
     const u32 buf_bytes = kVadChunk * 2 + 32;                          // one 32-block chunk + alignment slack (16-byte multiple)
-    const u32 max_frames = 2 * ((buf_len > 160 ? (buf_len - 160 + 79) / 80 : 0) + 2);   // 2 words per 80-sample block
+    const u32 max_frames = 2 * (frames_of(buf_len) + 2);                // 2 words per 80-sample block
     const size_t per_warp = 2 * (size_t)buf_bytes + (size_t)max_frames * 4;   // two chunk buffers + block summaries
     int warps = (int)((220 * 1024) / per_warp);
     if (warps < 1) return cudaErrorInvalidValue;

@@ -1,16 +1,21 @@
-// sr_vad_core.cuh -- warp-level building blocks of noise_atap (VAD.C:22-71) and VAD (VAD.C:97-218), shared by the
-// batch kernel (sr_vad.cu: samples staged in shared memory), the long-form kernels (sr_vad_long.cu: the same staging)
-// and the streaming kernel (sr_stream.cu: samples read from the streams' device rows): bulk-copy staging, block
-// summaries, the frame pass over summaries, and the endpoint FSM on the activity bitmap.
+// sr_vad_core.cuh -- one warp's noise_atap (VAD.C:22-71) and VAD (VAD.C:97-218), shared by the four VAD kernels: the
+// batch kernel K0 (sr_vad.cu: samples staged in shared memory), the long-form kernels K11/K12 (sr_vad_long.cu: the same
+// staging), the fixed-capture streams K4 (sr_stream.cu: samples read from the streams' device rows) and the live streams
+// K14 (sr_long_stream.cu: samples in a ring). Each kernel runs the same three steps:
+//   * noise_atap_warp: the thresholds from the calibration window;
+//   * block_pass: the summaries of 80-sample blocks, wherever the caller keeps the samples;
+//   * vad_window: up to 1 024 frames from those summaries (frames_pass, last_sig carried in `cin`), then the endpoint FSM
+//     continued from its carried state (long_fsm_window); the caller's act says what an opening and a closing do.
 #pragma once
 #include "sr_common.cuh"
 
 namespace srk {
 
-struct VadWarpView {
-    const u16 *x;       // staged samples, x[0] = first sample of the utterance
-    bool vec_ok;        // 16-byte aligned -> uint4 shared loads
-};
+// frames i = 80k while i < len - 160 (VAD.C:121); none for len <= 160 (the reference compares as u32 and reads past the
+// buffer). Frame k = blocks k, k + 1.
+__host__ __device__ __forceinline__ u32 frames_of(u32 len) {
+    return len > SR_FRAME_LEN ? (len - SR_FRAME_LEN + SR_FRAME_MOV - 1) / SR_FRAME_MOV : 0u;
+}
 
 __device__ __forceinline__ u32 warp_sum(u32 v) {
 #pragma unroll
@@ -23,11 +28,11 @@ __device__ __forceinline__ u32 warp_max(u32 v) {
     return v;
 }
 
-// noise_atap's three sums (VAD.C:41-63) over staged samples x[0, n_len), n_len % 240 == 0: mid = sum/n_len,
-// max_sum = sum over 240-sample blocks of max|x-mid|, abs_sum = sum |x-mid|. Vector form: lane l owns samples
-// [80l, 80l+80) (three lanes per 240-block, n_len <= 2560), 16-byte loads, IDP.2A for the plain sum.
-__device__ __forceinline__ void atap_stats(const u16 *x, bool vec_ok, u32 n_len, int lane, u32 &mid_out, u32 &max_sum_out,
-                                           u32 &abs_sum_out) {
+// noise_atap (VAD.C:22-71) over samples x[0, n_len), n_len % 240 == 0, into at. Its three sums (VAD.C:41-63): mid =
+// sum/n_len, max_sum = sum over 240-sample blocks of max|x-mid|, abs_sum = sum |x-mid|. Vector form (x 16-byte aligned,
+// n_len <= 2560): lane l owns samples [80l, 80l+80) (three lanes per 240-block), 16-byte loads, IDP.2A for the plain sum.
+__device__ __forceinline__ void noise_atap_warp(const u16 *x, bool vec_ok, u32 n_len, int lane, atap_tag &at) {
+    u32 mid, max_sum = 0, abs_sum = 0;
     if (vec_ok && n_len <= 2560u) {
         const bool act = 80u * (u32)lane < n_len;
         const uint4 *p = reinterpret_cast<const uint4 *>(x + (act ? 80 * lane : 0));
@@ -38,7 +43,7 @@ __device__ __forceinline__ void atap_stats(const u16 *x, bool vec_ok, u32 n_len,
             s = __dp2a_lo(q.x, 0x0101u, s); s = __dp2a_lo(q.y, 0x0101u, s);
             s = __dp2a_lo(q.z, 0x0101u, s); s = __dp2a_lo(q.w, 0x0101u, s);
         }
-        const u32 mid = warp_sum(act ? s : 0u) / n_len;
+        mid = warp_sum(act ? s : 0u) / n_len;
         u32 mx = 0, sm = 0;
 #pragma unroll
         for (int c = 0; c < 10; ++c) {
@@ -54,26 +59,20 @@ __device__ __forceinline__ void atap_stats(const u16 *x, bool vec_ok, u32 n_len,
         if (!act) { mx = 0; sm = 0; }
         const u32 m1 = __shfl_down_sync(0xFFFFFFFFu, mx, 1), m2 = __shfl_down_sync(0xFFFFFFFFu, mx, 2);
         const u32 bmax = (act && lane % 3 == 0) ? max(mx, max(m1, m2)) : 0u;      // lanes 3k..3k+2 = block k
-        mid_out = mid;
-        max_sum_out = warp_sum(bmax);
-        abs_sum_out = warp_sum(sm);
-        return;
+        max_sum = warp_sum(bmax);
+        abs_sum = warp_sum(sm);
+    } else {
+        u32 s = 0;
+        for (u32 i = lane; i < n_len; i += 32) s += x[i];
+        mid = warp_sum(s) / n_len;                                   // VAD.C:41-45
+        for (u32 i = 0; i < n_len; i += 240u) {                      // VAD.C:48-63
+            u32 mx = 0, sm = 0;
+            for (u32 h = lane; h < 240u; h += 32) { const u32 v = x[i + h], a = v > mid ? v - mid : mid - v; mx = max(mx, a); sm += a; }
+            max_sum += warp_max(mx);
+            abs_sum += sm;
+        }
+        abs_sum = warp_sum(abs_sum);
     }
-    u32 s = 0;
-    for (u32 i = lane; i < n_len; i += 32) s += x[i];
-    const u32 mid = warp_sum(s) / n_len;                             // VAD.C:41-45
-    u32 max_sum = 0, abs_sum = 0;
-    for (u32 i = 0; i < n_len; i += 240u) {                          // VAD.C:48-63
-        u32 mx = 0, sm = 0;
-        for (u32 h = lane; h < 240u; h += 32) { const u32 v = x[i + h], a = v > mid ? v - mid : mid - v; mx = max(mx, a); sm += a; }
-        max_sum += warp_max(mx);
-        abs_sum += sm;
-    }
-    mid_out = mid; max_sum_out = max_sum; abs_sum_out = warp_sum(abs_sum);
-}
-
-// the rest of noise_atap (VAD.C:65-70) from atap_stats' results: averages over the window, thresholds into at
-__device__ __forceinline__ void atap_finish(atap_tag &at, u32 n_len, u32 mid, u32 max_sum, u32 abs_sum) {
     abs_sum /= (n_len / SR_FRAME_LEN);                               // VAD.C:65
     max_sum /= (n_len / 240u);                                       // VAD.C:66
     at.mid_val = mid;
@@ -116,11 +115,11 @@ __device__ __forceinline__ u32 block_flags(u32 (&H)[3], u32 (&L)[3]) {
 // (w << 16) + (0 - (t << 16)) (low sample, one LEA), shifted MSB-first into the bitmaps by IMAD.X (x*2 + carry, FMA pipe):
 // per sample 3 ALU-pipe and 3 FMA-pipe instructions -- the ALU pipe is what bounds this kernel. t == 0 and t > 0xFFFF
 // are patched after the loop; mid > 0xFFFF (only possible with a caller-supplied atap_tag) takes the plain loop.
-__device__ __forceinline__ void block_scan(const VadWarpView &v, u32 i0, u32 mid, u32 a_thl, u32 b_thl, u32 &bs_out,
+// p = the block's first sample; vec_ok: p is 16-byte aligned (uint4 loads).
+__device__ __forceinline__ void block_scan(const u16 *p, bool vec_ok, u32 mid, u32 a_thl, u32 b_thl, u32 &bs_out,
                                            u32 &flags_out) {
     u32 bs = 0;
     u32 H[3], L[3];
-    const u16 *p = v.x + i0;
     if (mid <= 0xFFFFu) {
         u32 gA[3] = {0, 0, 0}, gB[3] = {0, 0, 0};      // "s >= a_thl", "s >= b_thl"; samples 0..31, 32..63, 64..79
         u32 bsx = 0, bsn = 0;
@@ -128,7 +127,7 @@ __device__ __forceinline__ void block_scan(const VadWarpView &v, u32 i0, u32 mid
 #pragma unroll
         for (int c = 0; c < 10; ++c) {
             u32 w[4];
-            if (v.vec_ok) {
+            if (vec_ok) {
                 const uint4 q = *reinterpret_cast<const uint4 *>(p + 8 * c);
                 w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w;
             } else {
@@ -225,6 +224,38 @@ __device__ __forceinline__ void block_scan_split8(const u16 *x, int lane, u32 nb
     flags_out = block_flags(H, L);
 }
 
+// The summaries of blocks 0 .. n-1 into info[2i] (sum |x-mid|) and info[2i+1] (flags), block i starting at blk(i): passes
+// of 32 blocks, one lane per block. A last pass of at most four blocks runs eight lanes per block (block_scan_split8)
+// when split_ok: those blocks lie one after another from a 4-byte aligned blk(i). vec_ok: every blk(i) is 16-byte aligned.
+template <class Blk>
+__device__ __forceinline__ void block_pass(Blk blk, u32 n, bool split_ok, bool vec_ok, u32 mid, u32 a_thl, u32 b_thl, u32 *info,
+                                           int lane) {
+    for (u32 i0 = 0; i0 < n; i0 += 32) {
+        const u32 left = n - i0;
+        u32 bs, fl;
+        if (left <= 4u && split_ok) {
+            block_scan_split8(blk(i0), lane, left, mid, a_thl, b_thl, bs, fl);
+            const u32 i = i0 + (u32)(lane >> 3);
+            if ((lane & 7) == 0 && (u32)(lane >> 3) < left) { info[2 * i] = bs; info[2 * i + 1] = fl; }
+        } else if ((u32)lane < left) {
+            const u32 i = i0 + (u32)lane;
+            block_scan(blk(i), vec_ok, mid, a_thl, b_thl, bs, fl);
+            info[2 * i] = bs; info[2 * i + 1] = fl;
+        }
+    }
+}
+
+// dst[0, len) = src[0, len) by one warp: 16-byte copies when both sides are 16-byte aligned
+__device__ __forceinline__ void warp_copy(u16 *dst, const u16 *src, u32 len, int lane) {
+    if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
+        const u32 nv = len >> 3;
+        for (u32 i = lane; i < nv; i += 32) reinterpret_cast<uint4 *>(dst)[i] = reinterpret_cast<const uint4 *>(src)[i];
+        for (u32 i = 8 * nv + lane; i < len; i += 32) dst[i] = src[i];
+    } else {
+        for (u32 i = lane; i < len; i += 32) dst[i] = src[i];
+    }
+}
+
 // Start staging samples [first, first+count) of the batch into `buf` (bulk async copy when the batch base is 16-byte
 // aligned, plain loads otherwise); completion is one phase of `bar` either way. Returns the sample index of `first`
 // inside buf.
@@ -282,12 +313,11 @@ __device__ __forceinline__ u32 bm_shr(u32 x, int s, int lane) {
 // One pass over up to 32 frames k0 + lane (frame k = blocks k, k+1; info[2*blk] = sum |x-mid|, info[2*blk+1] = flags of
 // block_flags). `cin` is the class of the last out-of-band sample in the blocks before k0 (0 at the start of a capture)
 // and is advanced to cover the blocks of the frames handled here (lanes with k >= kend contribute nothing), so passes
-// may start at any frame and stop anywhere: the streaming kernel resumes where the previous push ended.
+// may start at any frame and stop anywhere: the streaming kernels resume where the previous push ended.
 // Frames are absolute (k == 0 is the capture's first frame); info holds the summaries of blocks koff, koff + 1, ... (0: all
 // of them from block 0), so a caller may keep only the blocks of the frames at hand.
 // Returns the ballot of "frame active" (VAD.C:164) over the 32 lanes.
-__device__ __forceinline__ u32 frames_pass(const u32 *info, u32 k0, u32 kend, int lane, const atap_tag &at, u32 &cin,
-                                           u32 koff = 0) {
+__device__ __forceinline__ u32 frames_pass(const u32 *info, u32 k0, u32 kend, int lane, const atap_tag &at, u32 &cin, u32 koff) {
     const u32 k = k0 + (u32)lane;
     const bool ok = k < kend;
     u32 bs0 = 0, f0 = 0, bs1 = 0, f1 = 0;
@@ -317,35 +347,7 @@ __device__ __forceinline__ u32 frames_pass(const u32 *info, u32 k0, u32 kend, in
     return __ballot_sync(0xFFFFFFFFu, active);
 }
 
-// Endpoint FSM (VAD.C:164-216) on the activity bitmap of frames [0, nfr) held one 32-frame word per lane (nfr <= 1024):
-// 8 consecutive active frames open a segment at the first of them, 11 consecutive inactive frames close it at the first
-// of those; at most SR_MAX_VC_CON segments. Frames >= nfr are unknown (neither active nor inactive), so the result for a
-// prefix of a capture is exactly the set of decisions the sequential FSM has taken after frame nfr-1.
-__device__ __forceinline__ void fsm_segments(u32 aw, u32 nfr, int lane, u32 (&seg)[6]) {
-    const u32 fullw = nfr >> 5, rem = nfr & 31u;
-    const u32 vmask = (u32)lane < fullw ? 0xFFFFFFFFu : ((u32)lane == fullw ? ((1u << rem) - 1u) : 0u);
-    aw &= vmask;
-    u32 a8 = aw & bm_shr(aw, 1, lane);
-    a8 &= bm_shr(a8, 2, lane);
-    a8 &= bm_shr(a8, 4, lane);                                     // a8[i]: frames i..i+7 all active
-    u32 z = ~aw & vmask;
-    u32 z8 = z & bm_shr(z, 1, lane);
-    z8 &= bm_shr(z8, 2, lane);
-    z8 &= bm_shr(z8, 4, lane);
-    const u32 z11 = z8 & bm_shr(z8, 3, lane);                      // z11[i]: frames i..i+10 all inactive
-    int cur = 0;
-    for (int sgi = 0; sgi < (int)SR_MAX_VC_CON; ++sgi) {
-        const int pfr = find_first(a8, lane, cur);
-        if (pfr < 0) break;
-        seg[2 * sgi] = 80u * (u32)pfr;                             // VAD.C:178: i - 7*80 with i = 80*(pfr+7)
-        const int q = find_first(z11, lane, pfr + 8);
-        if (q < 0) break;                                          // never closes: end stays NULL
-        seg[2 * sgi + 1] = 80u * (u32)q + 80u;                     // VAD.C:201: i - 11*80 + 160 with i = 80*(q+10)
-        cur = q + 11;
-    }
-}
-
-// ---- the long-form endpoint FSM, carried across windows (K12 recordings, K14 live streams) ------------------------
+// ---- the endpoint FSM, carried across windows ------------------------------------------------------------------
 // position of the last set bit in a bitmap held one 32-bit word per lane; -1 if none
 __device__ __forceinline__ int find_last(u32 word) {
     const u32 bal = __ballot_sync(0xFFFFFFFFu, word != 0);
@@ -364,11 +366,14 @@ struct LongFsm {
 };
 
 // The endpoint FSM (VAD.C:164-216) over one window of nw <= 1024 frames starting at frame `base` (activity bitmap aw,
-// one 32-frame word per lane), continuing from state f: a run carried in from the previous window completes at the
-// window's first frames, later runs are found with fsm_segments' bit tricks. Windows may have any length from 1 to
-// 1 024: a run longer than the window is carried on. Every lane calls act.open(lane, f.n, frame) when segment f.n
-// opens at `frame` (VAD.C:178: start = 80 * frame) and act.close(lane, f.n, frame) when it closes with its first
-// inactive frame at `frame` (VAD.C:201: end = 80 * frame + 80); f is updated after the call.
+// one 32-frame word per lane), continuing from state f: 8 consecutive active frames open a segment at the first of them,
+// 11 consecutive inactive frames close it at the first of those. A run carried in from the previous window completes at
+// the window's first frames; later runs are found with bit tricks (a8 / z11 below, find_first). Windows may have any
+// length up to 1 024: a run longer than the window is carried on, and frames past the window are unknown, so after any
+// window f holds exactly the decisions the sequential FSM has taken by its last frame. Every lane calls
+// act.open(lane, f.n, frame) when segment f.n opens at `frame` (VAD.C:178: start = 80 * frame) and act.close(lane, f.n,
+// frame) when it closes with its first inactive frame at `frame` (VAD.C:201: end = 80 * frame + 80); f is updated after
+// the call. There is no limit on the number of segments: an act that keeps SR_MAX_VC_CON ignores the later ones.
 template <class Act>
 __device__ __forceinline__ void long_fsm_window(u32 aw, u32 nw, u32 base, int lane, LongFsm &f, Act &act) {
     const u32 fullw = nw >> 5, rem = nw & 31u;
@@ -416,5 +421,63 @@ __device__ __forceinline__ void long_fsm_window(u32 aw, u32 nw, u32 base, int la
         f.run = from < (int)nw ? nw - (u32)from : 0u;
     }
 }
+
+// ---- one window of frames: summaries -> activity -> FSM ----------------------------------------------------------
+// Frames [k, k + nw), nw <= 1024, from the block summaries at info (block j at info[2 (j - koff)]): the activity words by
+// frames_pass with last_sig carried in cin (VAD.C:121-164), then the endpoint FSM from state f (VAD.C:164-216).
+template <class Act>
+__device__ __forceinline__ void vad_window(const u32 *info, u32 koff, u32 k, u32 nw, int lane, const atap_tag &at, u32 &cin,
+                                           LongFsm &f, Act &act) {
+    u32 aw = 0;                                                    // lane j: activity of frames k + 32j .. + 31
+    for (u32 j = 0; 32u * j < nw; ++j) {
+        const u32 word = frames_pass(info, k + 32u * j, k + nw, lane, at, cin, koff);
+        if ((u32)lane == j) aw = word;
+    }
+    long_fsm_window(aw, nw, k, lane, f, act);
+}
+
+// The FSM's actions for a capture of at most SR_MAX_VC_CON segments (K0, K4): lane j < 6 holds seg_off[j], the start of
+// segment n in lane 2n and its end in lane 2n + 1. Later segments land in lanes that are never stored, or in none.
+struct SegLanes {
+    u32 seg;
+    __device__ __forceinline__ void open(int lane, u32 n, u32 frame) {        // VAD.C:178
+        if ((u32)lane == 2u * n) seg = 80u * frame;
+    }
+    __device__ __forceinline__ void close(int lane, u32 n, u32 frame) {       // VAD.C:201
+        if ((u32)lane == 2u * n + 1u) seg = 80u * frame + 80u;
+    }
+};
+
+// ---- what a streaming kernel carries and reports (K4 fixed captures, K14 live streams) ----------------------------
+// The VAD state a stream carries from push to push: frames < `frames` are evaluated, cin is the class of the last
+// out-of-band sample in blocks < frames (last_sig, VAD.C:99), f the endpoint FSM's state and open_start the start of the
+// open segment (SR_SEG_NULL when none is open).
+struct StreamVad {
+    u32 frames, cin;
+    LongFsm f;
+    u32 open_start;
+};
+
+struct StreamEventDev {         // work list of the segments closed by the current push
+    u32 stream, segment, start, end;
+};
+
+// A push's event list: one atomicAdd per closed segment, at most cap events kept
+struct StreamEvents {
+    StreamEventDev *ev;
+    u32 *seg_ev, *map_ev, *n_ev;
+    atap_tag *atap_ev;
+    u32 cap;
+    // segment n = [start, end) of stream s, which get_mfcc reads at offsets [ms, me) of PCM row s under at
+    __device__ __forceinline__ void emit(u32 s, u32 n, u32 start, u32 end, u32 ms, u32 me, const atap_tag &at) const {
+        const u32 e = atomicAdd(n_ev, 1u);
+        if (e < cap) {
+            StreamEventDev d; d.stream = s; d.segment = n; d.start = start; d.end = end;
+            ev[e] = d;
+            seg_ev[2 * e] = ms; seg_ev[2 * e + 1] = me;
+            atap_ev[e] = at; map_ev[e] = s;
+        }
+    }
+};
 
 }  // namespace srk

@@ -1,14 +1,14 @@
 // sr_vad_long.cu -- long-form VAD and per-segment recognition (include/sr_long.h): noise_atap (VAD.C:22-71) and the
 // loop of VAD.C:97-218 with max_vc_con removed, over recordings of up to 2^27 samples, then spch_recg's decision
 // (main.c:276-295) on every segment. Built on the batch kernel's pieces (sr_vad_core.cuh):
-//   * K11a noise_atap: one warp per recording over its first n_len samples (atap_stats / atap_finish);
-//   * K11b block pass: the 80-sample block summaries (block_scan) of every recording, in work items of 32 blocks spread
+//   * K11a noise_atap: one warp per recording over its first n_len samples (noise_atap_warp);
+//   * K11b block pass: the 80-sample block summaries (block_pass) of every recording, in work items of 32 blocks spread
 //     over the whole grid rather than one warp per recording, so one 30-minute recording fills the GPU as well as a
 //     batch of short ones. Each warp streams its items through two shared-memory buffers with bulk async copies
 //     (chunk_issue): PCM is read once (2 B per sample) and 8 B per block are written to a workspace;
-//   * K12 segment pass: one warp per recording walks windows of 1024 frames: frames_pass over the summaries, its `cin`
-//     (the carried last_sig) handed from pass to pass and window to window, then the endpoint FSM on the window's
-//     activity bitmap -- fsm_segments' bit tricks, with the FSM's state (open or closed, and the length of the run that
+//   * K12 segment pass: one warp per recording walks windows of 1024 frames (vad_window): frames_pass over the summaries,
+//     its `cin` (the carried last_sig) handed from pass to pass and window to window, then the endpoint FSM on the
+//     window's activity bitmap (long_fsm_window), with the FSM's state (open or closed, and the length of the run that
 //     crosses the window edge) carried into the next window and any number of segments emitted;
 //   * recognition: a prefix sum over min(n_segs, max_segs) flattens the segments into one table (segment, PCM row,
 //     atap), and the unchanged get_mfcc, template-scan and argmin kernels run on it with the segment count read from
@@ -20,10 +20,6 @@
 
 namespace srk {
 
-// frames i = 80k while i < len - 160 (VAD.C:121); none for len <= 160
-__device__ __forceinline__ u32 long_frames_of(u32 len) {
-    return len > SR_FRAME_LEN ? (len - SR_FRAME_LEN + SR_FRAME_MOV - 1) / SR_FRAME_MOV : 0u;
-}
 __device__ __forceinline__ u32 rec_len(const u32 *lens, u32 b, u32 U) { return lens ? min(lens[b], U) : U; }
 
 // ---- K11a: noise_atap over the first n_len samples; atap[b] untouched when n_len % 240 != 0 or n_len > lens[b] -------
@@ -35,10 +31,8 @@ long_atap_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restric
     const u32 b = blockIdx.x * kLongWarps + (threadIdx.x >> 5);
     if (b >= B || n_len == 0 || n_len % 240u != 0 || n_len > rec_len(lens, b, U)) return;   // VAD.C:33-36
     const u16 *x = pcm + (size_t)b * U;
-    u32 m, max_sum, abs_sum;
-    atap_stats(x, (reinterpret_cast<uintptr_t>(x) & 15) == 0, n_len, lane, m, max_sum, abs_sum);   // VAD.C:41-63
-    atap_tag at = atap[b];
-    atap_finish(at, n_len, m, max_sum, abs_sum);                                                 // VAD.C:65-70
+    atap_tag at;
+    noise_atap_warp(x, (reinterpret_cast<uintptr_t>(x) & 15) == 0, n_len, lane, at);
     if (lane == 0) atap[b] = at;
 }
 
@@ -66,7 +60,7 @@ long_block_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
     auto item = [&](u64 i, u32 &b, u32 &blk0, u32 &nb) {
         b = (u32)(i / cpr);
         blk0 = (u32)(i % cpr) * 32u;
-        const u32 nfr = long_frames_of(rec_len(lens, b, U)), nblk = nfr ? nfr + 1 : 0;   // frame k = blocks k, k+1
+        const u32 nfr = frames_of(rec_len(lens, b, U)), nblk = nfr ? nfr + 1 : 0;   // frame k = blocks k, k+1
         nb = blk0 < nblk ? min(32u, nblk - blk0) : 0u;
     };
     auto next_item = [&](u64 i, u32 &b, u32 &blk0, u32 &nb) {
@@ -88,20 +82,9 @@ long_block_kernel(const u16 *__restrict__ pcm, u32 U, u32 B, const u32 *__restri
                                     &bars[warp][s ^ 1], lane);
         const atap_tag at = atap[cb];
         const u32 mid = at.mid_val, a_thl = mid + at.n_thl, b_thl = mid - at.n_thl;    // VAD.C:112-113 (u32 wrap)
-        u32 *inf = info + (size_t)cb * info_stride;
-        VadWarpView v;
-        v.x = reinterpret_cast<const u16 *>(buf0 + s * kLongBuf) + shift_cur;
-        v.vec_ok = (shift_cur & 7) == 0;
-        if (cnb <= 4u && (shift_cur & 1) == 0) {                               // few blocks: eight lanes per block
-            u32 bs, fl;
-            block_scan_split8(v.x, lane, cnb, mid, a_thl, b_thl, bs, fl);
-            const u32 blk = cblk0 + (u32)(lane >> 3);
-            if ((lane & 7) == 0 && (u32)(lane >> 3) < cnb) { inf[2 * blk] = bs; inf[2 * blk + 1] = fl; }
-        } else if ((u32)lane < cnb) {
-            u32 bs, fl;
-            block_scan(v, 80u * (u32)lane, mid, a_thl, b_thl, bs, fl);
-            inf[2 * (cblk0 + lane)] = bs; inf[2 * (cblk0 + lane) + 1] = fl;
-        }
+        const u16 *x = reinterpret_cast<const u16 *>(buf0 + s * kLongBuf) + shift_cur;
+        block_pass([&](u32 i) { return x + 80u * i; }, cnb, (shift_cur & 1) == 0, (shift_cur & 7) == 0, mid, a_thl, b_thl,
+                   info + (size_t)cb * info_stride + 2u * cblk0, lane);
         __syncwarp();                                                          // this buffer is re-staged one item later
         shift_cur = shift_nxt;
         it = nx;
@@ -127,22 +110,14 @@ long_segment_kernel(u32 U, u32 B, const u32 *__restrict__ lens, const atap_tag *
     const int lane = threadIdx.x & 31;
     const u32 b = blockIdx.x * kLongWarps + (threadIdx.x >> 5);
     if (b >= B) return;
-    const u32 nfr = long_frames_of(rec_len(lens, b, U));
+    const u32 nfr = frames_of(rec_len(lens, b, U));
     const atap_tag at = atap[b];
     const u32 *inf = info + (size_t)b * info_stride;
     u32 *out = seg_off + (size_t)b * max_segs * 2;
     LongFsm f{false, 0u, 0u};
     LongSegOut act{max_segs, out};
     u32 cin = 0;                                                   // class of the last out-of-band sample so far (last_sig)
-    for (u32 base = 0; base < nfr; base += 1024u) {
-        const u32 nw = min(1024u, nfr - base);
-        u32 aw = 0;                                                // lane j: activity of frames base + 32j .. + 31
-        for (u32 j = 0; 32u * j < nw; ++j) {
-            const u32 word = frames_pass(inf, base + 32u * j, base + nw, lane, at, cin);   // VAD.C:121-164
-            if ((u32)lane == j) aw = word;
-        }
-        long_fsm_window(aw, nw, base, lane, f, act);
-    }
+    for (u32 base = 0; base < nfr; base += 1024u) vad_window(inf, 0u, base, min(1024u, nfr - base), lane, at, cin, f, act);
     if (lane == 0) n_segs[b] = f.n + (f.open ? 1u : 0u);           // + the segment still open (end SR_SEG_NULL)
 }
 

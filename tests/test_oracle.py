@@ -207,11 +207,12 @@ def test_generic_radix4_fft_reproduces_the_1024_point_restatement():
 
 
 def test_bitmap_endpoint_fsm_equals_sequential_fsm_on_every_prefix():
-    """The endpoint FSM of VAD.C:164-216 as the kernels evaluate it (sr_vad_core.cuh::fsm_segments: 8 consecutive active
-    frames open a segment at the first of them, 11 consecutive inactive frames close it at the first of those, at most 3
-    segments) against the sequential state machine -- on random activity patterns and on EVERY prefix of them, which is the
-    property the streaming kernel relies on: re-running the bitmap form on the frames seen so far yields exactly the
-    decisions the sequential FSM has taken by then."""
+    """The endpoint FSM of VAD.C:164-216 as the kernels evaluate it on one window from a fresh state
+    (sr_vad_core.cuh::long_fsm_window's a8 / z11 bitmaps and find_first, as K0 runs it through vad_window: 8 consecutive
+    active frames open a segment at the first of them, 11 consecutive inactive frames close it at the first of those,
+    the first 3 segments kept) against the sequential state machine -- on random activity patterns and on EVERY prefix of
+    them: a window that ends at any frame yields exactly the decisions the sequential FSM has taken by then, which is
+    what lets the streaming kernels carry the FSM's state from push to push."""
     rng = np.random.default_rng(164)
 
     def sequential(act):

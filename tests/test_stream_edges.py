@@ -3,8 +3,8 @@
 Every case is checked after EVERY push, not only at the end, against the CPU oracle on the full buffer:
   - an event arrives in the push that delivers sample max(end + 879, n_len - 1): the frame that closes a segment is
     evaluated once n >= end + 880, and nothing is evaluated before the calibration window is complete;
-  - segments() is the oracle's VAD on the whole capture, masked: a start is shown once n >= start + 720 (fsm_segments opens
-    at frame start/80 + 7, frame k is evaluated once n >= 80k + 160) and an end once n >= end + 880; the reference FSM never
+  - segments() is the oracle's VAD on the whole capture, masked: a start is shown once n >= start + 720 (long_fsm_window
+    opens at frame start/80 + 7, frame k is evaluated once n >= 80k + 160) and an end once n >= end + 880; the reference FSM never
     abandons an opened segment, so a shown start is final;
   - atap is zero until the first n_len samples are in, then the oracle's noise_atap (zero for ever when n_len is 0 or not
     a multiple of 240: VAD.C:33-36 leaves it untouched);
@@ -15,7 +15,7 @@ Events are compared per stream: within one push their order across streams follo
 CPU: a header guard; the planted recordings of the GPU tests realise what they claim under the oracle (zero-atap runs of
 exact lengths, a segment that opens only through last_sig carried over a 32-frame word edge).
 GPU: capture lengths 161 ... 65 535 at every row alignment with lock-step chunks 1 ... 881 and ragged schedules (empty
-pushes and pushes past the end included); calibration windows 0 ... 65 520 (scalar atap_stats, catch-up pushes,
+pushes and pushes past the end included); calibration windows 0 ... 65 520 (scalar noise_atap_warp, catch-up pushes,
 full-scale rows); last_sig carried across pushes cut around word edges; 119- and 120-frame segments in both geometries,
 a fourth and fifth word, no bank and an all-unsigned bank; bursts of 6 144 events in one push (the second D2H copy) on a
 pool, through fetch and on a group; the matcher, bank, DTW variant and geometry switched between pushes; reset with
@@ -391,7 +391,7 @@ def test_capture_lengths_at_every_row_alignment(ora, L):
 @pytest.mark.parametrize("n_len", [0, 160, 240, 2400, 2560, 2640, 4800, 64800, 65520, "L"])
 def test_calibration_windows(ora, n_len):
     """n_len 0, 160 and 2 560 leave the zero atap (exact-zero runs open and close segments, one at sample 0); 2 640 is
-    the first window the scalar atap_stats sums; 64 800 and 65 520 make the calibration push a catch-up over ~810 blocks,
+    the first window the scalar noise_atap_warp sums; 64 800 and 65 520 make the calibration push a catch-up over ~810 blocks,
     and 65 520 sums full-scale rows to 4 293 853 200, just under 2^32; n_len = L = 24 000 calibrates on the whole
     capture. Stream S - 1 never receives n_len samples: no event, NULL segments, zero atap"""
     L = 24000 if n_len == "L" else 65535
