@@ -518,6 +518,14 @@ int sr_debug_fft_raw_n(sr_handle *h, const uint32_t *in_packed, uint32_t N, uint
 /* test hook: count of float bit patterns in [lo_bits, hi_bits) where the kernels' branch-free sqrt differs
  * from the IEEE sqrt.rn.f32 (0 over [1.0f, 2^33), the range the path can produce) */
 int sr_debug_sqrt_mismatches(sr_handle *h, uint32_t lo_bits, uint32_t hi_bits, uint64_t *mismatches);
+/* test hook: count of v in [lo, hi) (hi <= 2^32) where the MFCC kernels' log100 (a float estimate and two correction
+ * loops) differs from a binary search over the same threshold table (0 over [0, 2^32)) */
+int sr_debug_log100_mismatches(sr_handle *h, uint64_t lo, uint64_t hi, uint64_t *mismatches);
+/* test hook: count of (re, im) pairs of index [lo, hi) where the MFCC kernels' magnitude step differs from
+ * (u32)(sqrtf((float)pw) * 10), pw = re^2 + im^2 as an s32, 0 for pw <= 0. which = 0: mag10_small over |re|, |im| <= 8209,
+ * index (re + 8209) * 16419 + im + 8209 < 16419^2; which = 1: mag10 over every s16 pair, index (u16)re | (u16)im << 16
+ * < 2^32 (0 over each whole domain) */
+int sr_debug_mag10_mismatches(sr_handle *h, int which, uint64_t lo, uint64_t hi, uint64_t *mismatches);
 
 /* Packed PCM transport of sr_recognise_batch (host buffers): chunks whose samples are all < 4096 (the reference's
  * 12-bit ADC range) may cross PCIe as 12 bits per sample, packed by host worker threads and expanded on the

@@ -1541,6 +1541,28 @@ int sr_debug_sqrt_mismatches(sr_handle *h, uint32_t lo_bits, uint32_t hi_bits, u
     return c.finish();
 }
 
+// test hook: number of v in [lo, hi) for which the MFCC kernels' log100 differs from a binary search over the same
+// threshold table (must be 0 over [0, 2^32))
+int sr_debug_log100_mismatches(sr_handle *h, uint64_t lo, uint64_t hi, uint64_t *mismatches) {
+    SR_REQUIRE(h, h && mismatches && hi <= (1ull << 32));
+    HostCall c(h, "sr_debug_log100_mismatches");
+    auto *bad = reinterpret_cast<unsigned long long *>(c.out(h->scratch[2], mismatches, 8, 8));
+    c.ck("cudaMemsetAsync", bad ? cudaMemsetAsync(bad, 0, 8, h->stream) : cudaSuccess);
+    c.launch(TAG_NONE, "launch_log100_check", [&] { return launch_log100_check(lo, hi, bad, h->stream); });
+    return c.finish();
+}
+
+// test hook: number of (re, im) pairs of index [lo, hi) for which the MFCC kernels' magnitude step differs from IEEE
+// (u32)(sqrtf(pw) * 10); which = 0: mag10_small, i < 16419^2; which = 1: mag10, i < 2^32 (must be 0 over each domain)
+int sr_debug_mag10_mismatches(sr_handle *h, int which, uint64_t lo, uint64_t hi, uint64_t *mismatches) {
+    SR_REQUIRE(h, h && mismatches && (which == 0 || which == 1) && hi <= (which ? 1ull << 32 : 16419ull * 16419ull));
+    HostCall c(h, "sr_debug_mag10_mismatches");
+    auto *bad = reinterpret_cast<unsigned long long *>(c.out(h->scratch[2], mismatches, 8, 8));
+    c.ck("cudaMemsetAsync", bad ? cudaMemsetAsync(bad, 0, 8, h->stream) : cudaSuccess);
+    c.launch(TAG_NONE, "launch_mag10_check", [&] { return launch_mag10_check(which, lo, hi, bad, h->stream); });
+    return c.finish();
+}
+
 }  // extern "C"
 
 // ---- (1) the reference's own entry points: batch-of-1 on a lazily created default handle -----------

@@ -27,6 +27,8 @@ cudaError_t launch_mfcc_geomb(const u16 *pcm, u32 U, u32 B, const u32 *seg, u32 
 cudaError_t launch_fft_generic(const u32 *in_packed, const s16 *frames, u32 len, u32 n, u32 *raw_out, u32 *mag,
                                cudaStream_t st);
 cudaError_t launch_fft_raw_n(const u32 *in, u32 N, u32 n, u32 *out, cudaStream_t st);
+cudaError_t launch_log100_check(u64 lo, u64 hi, unsigned long long *bad_dev, cudaStream_t st);
+cudaError_t launch_mag10_check(int which, u64 lo, u64 hi, unsigned long long *bad_dev, cudaStream_t st);
 // n keys (B argmin keys, or a decision rule's B * C keys) set to main.c:276-278's start
 cudaError_t launch_best_init(u64 *best, u64 n, cudaStream_t st);
 // The decision of B inputs into the fields (sr_dtw.cu): without a rule (rl.C = 0) from the argmin keys keys = best;

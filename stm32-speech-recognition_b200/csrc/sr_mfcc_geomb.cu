@@ -126,4 +126,56 @@ cudaError_t launch_fft_raw_n(const u32 *in, u32 N, u32 n, u32 *out, cudaStream_t
     return cudaGetLastError();
 }
 
+// ---- test hooks: whole-domain checks of the float estimates under the MFCC kernels' exact integer steps. Each thread
+// counts its mismatches over a grid-strided range; the device code is the kernels' own inline functions.
+// log100 (float estimate + two correction loops) against the last L with thr[L] <= v, found by binary search, for v in
+// [lo, hi), hi <= 2^32
+__global__ void log100_check_kernel(u64 lo, u64 hi, const DevTables *__restrict__ tab, unsigned long long *bad) {
+    unsigned long long n = 0;
+    for (u64 i = lo + blockIdx.x * (u64)blockDim.x + threadIdx.x; i < hi; i += (u64)gridDim.x * blockDim.x) {
+        const u32 v = (u32)i;
+        int L = 0;
+        if (v != 0) {
+            int a = 0, b = 2218;                          // thr[a] <= v < thr[b + 1] (thr[2219] = 2^32 - 1 bounds nothing)
+            while (a < b) {
+                const int m = (a + b + 1) >> 1;
+                if (tab->log_thr[m] <= v) a = m;
+                else b = m - 1;
+            }
+            L = a;
+        }
+        if (log100(v, tab->log_thr) != (u32)L) ++n;
+    }
+    if (n) atomicAdd(bad, n);
+}
+
+// mag10_small over every (re, im) with |re|, |im| <= 8209 (which = 0; index i = (re + 8209) * 16419 + im + 8209, i <
+// 16419^2), or mag10 over every s16 pair (which = 1; re = low half of i, im = high half, i < 2^32), against
+// (u32)(sqrtf((float)pw) * 10) with pw = re^2 + im^2 as an s32: every step IEEE round-to-nearest, 0 for pw <= 0
+__global__ void mag10_check_kernel(int which, u64 lo, u64 hi, unsigned long long *bad) {
+    unsigned long long n = 0;
+    for (u64 i = lo + blockIdx.x * (u64)blockDim.x + threadIdx.x; i < hi; i += (u64)gridDim.x * blockDim.x) {
+        s32 re, im;
+        if (which == 0) { re = (s32)(i / 16419) - 8209; im = (s32)(i % 16419) - 8209; }
+        else { re = (s32)(s16)(u16)i; im = (s32)(s16)(u16)(i >> 16); }
+        const s32 pw = (s32)(u32)((long long)re * re + (long long)im * im);
+        const u32 want = pw <= 0 ? 0u : __float2uint_rz(__fmul_rn(__fsqrt_rn(__int2float_rn(pw)), 10.0f));
+        const u32 got = which == 0 ? mag10_small((u32)re, (u32)im) : mag10((u32)re, (u32)im);
+        if (got != want) ++n;
+    }
+    if (n) atomicAdd(bad, n);
+}
+
+cudaError_t launch_log100_check(u64 lo, u64 hi, unsigned long long *bad_dev, cudaStream_t st) {
+    const DevTables *tab = dev_tables();
+    if (!tab) return cudaErrorInitializationError;
+    log100_check_kernel<<<132 * 8, 256, 0, st>>>(lo, hi, tab, bad_dev);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mag10_check(int which, u64 lo, u64 hi, unsigned long long *bad_dev, cudaStream_t st) {
+    mag10_check_kernel<<<132 * 8, 256, 0, st>>>(which, lo, hi, bad_dev);
+    return cudaGetLastError();
+}
+
 }  // namespace srk

@@ -161,6 +161,8 @@ def lib():
         L.sr_timing_enable.argtypes = [vp, u32]
         L.sr_timing_collect.argtypes = [vp, vp, vp, u32, vp]
         L.sr_debug_sqrt_mismatches.argtypes = [vp, u32, u32, vp]
+        L.sr_debug_log100_mismatches.argtypes = [vp, u64, u64, vp]
+        L.sr_debug_mag10_mismatches.argtypes = [vp, C.c_int, u64, u64, vp]
         L.sr_set_transport.argtypes = [vp, C.c_int]
         L.sr_transport_stats.argtypes = [vp, vp, vp, vp]
         L.sr_debug_pack12_host.argtypes = [C.c_int, vp, u64, vp]

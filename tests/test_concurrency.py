@@ -809,6 +809,8 @@ EXCLUDED = {
     "sr_fft_raw_batch": "stateless test-hook kernel",
     "sr_debug_fft_raw_n": "stateless test-hook kernel",
     "sr_debug_sqrt_mismatches": "stateless test-hook kernel",
+    "sr_debug_log100_mismatches": "stateless test-hook kernel",
+    "sr_debug_mag10_mismatches": "stateless test-hook kernel",
     "sr_debug_pack12_host": "host only, no handle",
     "sr_debug_unpack12": "stateless test-hook kernel; recognise_packed runs the expander",
     "sr_set_labels": "host-side table of the handle; no device state",

@@ -7,6 +7,7 @@ import os
 import numpy as np
 import pytest
 
+import mfcc_ref as mr
 import oracle_bind as ob
 import sr_b200
 from drive import recognise_dev_np
@@ -92,6 +93,10 @@ def test_mfcc_extreme_inputs_and_ragged_segments(handle, ora):
     seg[15] = [1, 1 + 159]                             # one sample short of a frame
     atap = np.zeros(B, sr_b200.ATAP_DTYPE)
     atap["mid_val"] = rng.integers(0, 4096, B)
+    atap["mid_val"][10] = 2048                         # row 10 at its own mid_val: every windowed sample and bin is 0
+    seg[10] = [100, 100 + 9 * 80 + 160]
+    _, sums, _ = mr.mfcc_batch(pcm[10:11], seg[10:11], atap[10:11], mr.GEOM_A)
+    assert len(sums) == 10 and (sums == 0).all()
     got = handle.mfcc(pcm, seg, atap)
     valid = (seg[:, 0] != ob.NULL) & (seg[:, 1] != ob.NULL)
     want = ora.mfcc_batch(pcm[valid], seg[valid], atap[valid])

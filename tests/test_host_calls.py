@@ -104,6 +104,13 @@ def test_host_buffer_call_accounting(h, data):
     bad = C.c_uint64(7)
     n, tags = _account(h, lambda: _rc(h, "sr_debug_sqrt_mismatches", 0x3F800000, 0x3F810000, C.byref(bad)))
     assert tags == [] and bad.value == 0
+    bad = C.c_uint64(7)
+    n, tags = _account(h, lambda: _rc(h, "sr_debug_log100_mismatches", 0, 1 << 16, C.byref(bad)))
+    assert tags == [] and bad.value == 0
+    for which in (0, 1):
+        bad = C.c_uint64(7)
+        n, tags = _account(h, lambda: _rc(h, "sr_debug_mag10_mismatches", which, 0, 1 << 16, C.byref(bad)))
+        assert tags == [] and bad.value == 0
 
 
 def test_dtw_without_templates_launches_only_the_argmin(data):
@@ -168,7 +175,10 @@ def test_null_pointer_with_work_fails(h):
              ("sr_fft_raw_batch", (a, 1, None)), ("sr_get_dis_batch", (a, None, 1, a)),
              ("sr_debug_fft_raw_n", (None, 256, 1, a)), ("sr_debug_fft_raw_n", (a, 1024, 1, None)),
              ("sr_dtw_limit_batch", (a, a, None, a, 1, a)), ("sr_debug_unpack12", (a, 2, None)),
-             ("sr_debug_sqrt_mismatches", (0, 1, None)),
+             ("sr_debug_sqrt_mismatches", (0, 1, None)), ("sr_debug_log100_mismatches", (0, 1, None)),
+             ("sr_debug_log100_mismatches", (0, (1 << 32) + 1, a)), ("sr_debug_mag10_mismatches", (0, 0, 1, None)),
+             ("sr_debug_mag10_mismatches", (2, 0, 1, a)), ("sr_debug_mag10_mismatches", (0, 0, 16419 ** 2 + 1, a)),
+             ("sr_debug_mag10_mismatches", (1, 0, (1 << 32) + 1, a)),
              ("sr_noise_atap_batch_dev", (None, U, 1, 2400, a)), ("sr_vad_batch_dev", (a, U, 1, U, a, None)),
              ("sr_mfcc_batch_dev", (a, U, 1, None, 2, a, a)), ("sr_dtw_batch_dev", (None, 1, 0, 0, a, a, a)),
              ("sr_recognise_batch_dev", (None, U, 1, 2400, C.byref(sr_b200.RecogOut())))]
