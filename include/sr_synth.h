@@ -31,6 +31,23 @@ int sr_synth_ftr_host(void *out, uint32_t stride, uint32_t B, uint64_t seed_base
  * x -> (x-128)*16 + 2048. Host only (input adaptation, like the generator above). Returns the number of samples
  * written (<= max_samples), or -1 on a malformed / unsupported file; *sample_rate receives the file's rate. */
 long sr_wav_to_adc12(const void *wav, size_t wav_bytes, uint16_t *out, size_t max_samples, uint32_t *sample_rate);
+/* Polyphase resampling of 12-bit codes at `rate` to the 8 kHz every other call takes (DESIGN.md section 8). With
+ * (L, M) = (8000, rate) / gcd and the rate's odd-length s32 table h[0..N-1] (csrc/sr_resample_taps.h, centre
+ * c = (N-1)/2), u[i] = x[i/L] - 2048 when i % L == 0 and i/L < len, else 0 (outside the recording reads as mid-code):
+ *   acc[n] = sum_k h[k] * u[n*M + c - k]  (exact in s32),  y[n] = clamp(2048 + ((acc[n] + 2^14) >> 15), 0, 4095),
+ *   out_len = ceil(len * L / M), 0 when len = 0. At 8000 Hz, h = {32768}: the output is the input.
+ * Recordings are in + b*U_in with len = lens[b] (lens[b] > U_in is read as U_in; lens NULL: U_in); no sample at or past
+ * len is read. Output b is out + b*U_out; only out[b][0, out_len) and out_lens[b] (when out_lens is not NULL) are
+ * written. All pointers are device (or managed) memory on the current device, 2-byte aligned (lens and out_lens
+ * 4-byte). Asynchronous on `cuda_stream` (NULL: the legacy default stream). Returns 0, or -1 with nothing launched on a
+ * rate outside SR_RESAMPLE_RATES, U_in > SR_RESAMPLE_U_MAX, U_out < ceil(U_in * L / M) (the longest out_len a
+ * recording of U_in samples can have), a NULL or unusable pointer, or a failed launch. B = 0 does nothing. */
+#define SR_RESAMPLE_RATES { 8000, 11025, 16000, 22050, 32000, 44100, 48000 }
+#define SR_RESAMPLE_U_MAX (1u << 30)   /* longest input: 6.2 h at 48 kHz, more than 2^27 samples (SR_LONG_U_MAX) out */
+int sr_resample_adc12_dev(const uint16_t *in /* [B][U_in] 12-bit codes at `rate` */, uint32_t U_in, uint32_t B,
+                          const uint32_t *lens /* [B] device, or NULL = U_in */, uint32_t rate,
+                          uint16_t *out /* [B][U_out] 12-bit codes at 8 kHz */, uint32_t U_out,
+                          uint32_t *out_lens /* [B] device, or NULL */, void *cuda_stream);
 #ifdef __cplusplus
 }
 #endif

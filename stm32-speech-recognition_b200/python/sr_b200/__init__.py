@@ -255,6 +255,7 @@ def lib():
         L.sr_synth_ftr_host.argtypes = [vp, u32, u32, u64, u32, u32]
         L.sr_wav_to_adc12.argtypes = [vp, C.c_size_t, vp, C.c_size_t, vp]
         L.sr_wav_to_adc12.restype = C.c_long
+        L.sr_resample_adc12_dev.argtypes = [vp, u32, u32, vp, u32, vp, u32, vp, vp]
         L.noise_atap.argtypes = [vp, C.c_uint16, vp]
         L.noise_atap.restype = None
         L.VAD.argtypes = [vp, C.c_uint16, vp, vp]
@@ -905,6 +906,19 @@ def wav_to_adc12(wav_bytes, max_samples=1 << 24):
     if n < 0:
         raise SrError("not a supported PCM WAV file")
     return out[:n].copy(), rate.value
+
+
+RESAMPLE_RATES = (8000, 11025, 16000, 22050, 32000, 44100, 48000)   # SR_RESAMPLE_RATES
+RESAMPLE_U_MAX = 1 << 30       # SR_RESAMPLE_U_MAX: the longest input of resample_adc12_dev
+
+
+def resample_adc12_dev(in_ptr, U_in, B, lens_ptr, rate, out_ptr, U_out, out_lens_ptr=None, stream_ptr=None):
+    """sr_resample_adc12_dev: B recordings of 12-bit codes at `rate` (device [B, U_in], lengths [B] or None) -> device
+    [B, U_out] codes at 8 kHz and their lengths [B] (or None), asynchronous on `stream_ptr` (include/sr_synth.h)"""
+    rc = lib().sr_resample_adc12_dev(_p(in_ptr), U_in, B, _p(lens_ptr), rate, _p(out_ptr), U_out, _p(out_lens_ptr),
+                                     _p(stream_ptr))
+    if rc != 0:
+        raise SrError("sr_resample_adc12_dev failed (rate %d, U_in %d, B %d, U_out %d)" % (rate, U_in, B, U_out))
 
 
 def make_bank(ftr, slot_stride=4096, valid=None):
