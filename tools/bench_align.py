@@ -15,40 +15,15 @@ and SM clock limit are read in the same run.
     python tools/bench_align.py [--steps 10] [--warmup 2] [--json FILE]
 """
 import argparse
-import json
-import os
-import sys
-import time
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-import oracle_ext as ox  # noqa: E402
-import oracle_bind as ob  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
-
-U, N_LEN = 8000, 2400
-SEED, TPL_SEED = 0x5EED0000, 0x7E3A0000       # bench.py's inputs
-NPROC = os.cpu_count() or 1
-
-
-def timed(h, fn, reps):
-    """(wall ms per call, {tag: kernel ms per call}) of fn() repeated reps times"""
-    h.timing_enable(64 * reps)
-    t0 = time.perf_counter()
-    for _ in range(reps):
-        out = fn()
-    wall = (time.perf_counter() - t0) * 1e3 / reps
-    ker = {}
-    for t, ms in h.timing_collect():
-        ker[t] = ker.get(t, 0.0) + ms / reps
-    h.timing_enable(0)
-    return wall, ker, out
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import N_LEN, NPROC, SEED, TPL_SEED, U, card, cuda_device, event_steps, per_call, report, timed
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
 
 
 def main():
@@ -61,10 +36,7 @@ def main():
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
 
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_align: no CUDA device (there is nothing to measure without one)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_align")
     B, T, n = args.batch, args.templates, args.sample
     h = sr_b200.Handle(0)
     stream = torch.cuda.Stream(dev)
@@ -95,12 +67,15 @@ def main():
     for r in (10, 15, 16, 118):
         for _ in range(args.warmup):
             h.dtw_path(fin, mdl, r)
-        wall, ker, (dis, path, plen) = timed(h, lambda: h.dtw_path(fin, mdl, r), args.steps)
+        wall, recs, (dis, path, plen) = timed(h, lambda: h.dtw_path(fin, mdl, r), args.steps, 64 * args.steps)
+        ker = per_call(recs, args.steps)
         wd, wp, wl = ao.dtw_path(fin[:n], mdl[:n], r, nthreads=NPROC)
         ok = bool(np.array_equal(dis[:n], wd) and np.array_equal(path[:n], wp) and np.array_equal(plen[:n], wl))
         cells = sum(po.dtw_batch(fin[p:p + 1], sr_b200.make_bank(mdl[p:p + 1]), 1, 4096, band_r=r)[1] for p in range(n))
         cells_b = cells * B / n
-        _, kscan, _ = timed(h, lambda: h.dtw(fin, flags=sr_b200.DTW_BAND, band_r=r, want_best=False), args.steps)
+        _, recs, _ = timed(h, lambda: h.dtw(fin, flags=sr_b200.DTW_BAND, band_r=r, want_best=False), args.steps,
+                           64 * args.steps)
+        kscan = per_call(recs, args.steps)
         scan_cells = po.dtw_batch(fin[:n], bank20, T, 4096, band_r=r, nthreads=NPROC)[1] * B / n
         results["path"].append({"r": r, "pairs": B, "kernel_ms": ker[7], "wall_ms": wall, "pairs_per_s": B / (ker[7] * 1e-3),
                                 "cells_per_s": cells_b / (ker[7] * 1e-3), "scan_kernel_ms": kscan[6],
@@ -116,7 +91,9 @@ def main():
     ng = min(G, 64)
     for iters in (1, 3):
         h.average_bank(bank[:4 * K], 4096, K, 118, iters)
-        wall, ker, (out, score, anchor) = timed(h, lambda: h.average_bank(bank, 4096, K, 118, iters), max(1, args.steps // 5))
+        reps = max(1, args.steps // 5)
+        wall, recs, (out, score, anchor) = timed(h, lambda: h.average_bank(bank, 4096, K, 118, iters), reps, 64 * reps)
+        ker = per_call(recs, reps)
         wo, ws, wa = ao.average_bank(bank[:ng * K], 4096, K, 118, iters, nthreads=NPROC)
         ok = bool(np.array_equal(out[:ng * K], wo) and np.array_equal(score[:ng], ws) and np.array_equal(anchor[:ng], wa))
         results["average"].append({"G": G, "K": K, "r": 118, "iters": iters, "wall_ms": wall, "align_ms": ker.get(7, 0.0),
@@ -133,34 +110,23 @@ def main():
     for name, bk in (("4 per command", bank20), ("averaged", avg20)):
         h.set_bank(bk, T, 4096)
         h.set_match(sr_b200.DTW_BAND, 118)
-        for _ in range(args.warmup):
-            h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs)
-        h.sync()
-        h.timing_enable(6 * args.steps + 8)
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         h.set_stream(stream.cuda_stream)
-        with torch.cuda.stream(stream):
-            ev0.record(stream)
-            for _ in range(args.steps):
-                h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs)
-            ev1.record(stream)
-        stream.synchronize()
-        dtw_ms = [ms for t, ms in h.timing_collect() if t == 6]
-        h.timing_enable(0)
+        step_ms, recs = event_steps(h, stream, lambda: h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs), args.steps,
+                                    args.warmup, 6 * args.steps + 8)
         h.use_own_stream()
+        dtw_ms = [ms for t, ms in recs if t == 6]
         sc, _ = po.dtw_batch(front["ftr"][good], bk, T, 4096, check_sign=1, band_r=118, nthreads=NPROC)
         got = outs["score"][:n].cpu().numpy().view(np.uint32)
         i = np.argmin(sc, axis=1)
         ok = bool(np.array_equal(got[good], sc) and np.array_equal(outs["best_idx"][:n].cpu().numpy().view(np.uint32)[good], i))
         results["recognise"].append({"bank": name, "signed_slots": int((bk[:, :2].copy().view(np.uint16)[:, 0] == 12345).sum()),
-                                     "ms_per_step": ev0.elapsed_time(ev1) / args.steps,
+                                     "ms_per_step": step_ms,
                                      "dtw_ms_mean": float(np.mean(dtw_ms)), "sample_equals_oracle": ok})
     h.set_match(0, 0)
+    h.close()
 
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "batch": B, "templates": T,
             "steps": args.steps, "sample": n, "results": results}
-    c = info["card"]
-    print("card: %s, power limit %s, max SM clock %s" % (c.get("name"), c.get("power.limit"), c.get("clocks.max.sm")))
     for x in results["path"]:
         print("path r=%-4d kernel %8.3f ms  wall %8.1f ms  %6.2f Mpairs/s  %6.2f Gcells/s | scan %8.3f ms %6.2f Gcells/s  oracle %s" % (
             x["r"], x["kernel_ms"], x["wall_ms"], x["pairs_per_s"] / 1e6, x["cells_per_s"] / 1e9, x["scan_kernel_ms"],
@@ -171,13 +137,7 @@ def main():
     for x in results["recognise"]:
         print("recognise r=118 %-14s (%2d signed slots)  %8.3f ms/step  dtw %8.3f ms  oracle %s" % (
             x["bank"], x["signed_slots"], x["ms_per_step"], x["dtw_ms_mean"], x["sample_equals_oracle"]))
-    print(json.dumps(info))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(info, f, indent=1)
-    h.close()
-    if not all(x["sample_equals_oracle"] for v in results.values() for x in v):
-        raise SystemExit("bench_align: a sample differs from the oracle")
+    report("bench_align", info, all(x["sample_equals_oracle"] for v in results.values() for x in v), args.json)
 
 
 if __name__ == "__main__":

@@ -13,63 +13,18 @@ random ones, --sample in all. The card's name, power limit and SM clock limit ar
     python tools/bench_connected.py [--steps 2] [--warmup 1] [--json FILE]
 """
 import argparse
-import json
-import os
-import sys
-import time
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import NPROC, card, cuda_device, e2e_edges, edges, per_call, report, synth_bank, timed
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
+from refs import launch_sample, seq_launches
 
-import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
-from refs import launch_sample, piece_plan, pieces, seq_launches  # noqa: E402
-
-NPROC = os.cpu_count() or 1
 PENALTY = 4000
-
-
-def edges(ranges):
-    """the first and last index of every range [lo, hi)"""
-    return {i for lo, hi in ranges for i in (lo, hi - 1)}
-
-
-def e2e_edges(frm_num, seq_ranges=None):
-    """the captures holding the first and last get_mfcc piece of every piece launch and, given the decoder's launch ranges
-    over the captures' segments with frames (default: one sequence per segment, K6), of every decoder launch"""
-    B = len(frm_num)
-    e = piece_plan(pieces(frm_num).sum(1))[1]
-    if seq_ranges is None:
-        owner = np.repeat(np.arange(B), (frm_num > 0).sum(1))
-        e |= {int(owner[i]) for i in edges(seq_launches([0, len(owner)]))}
-    else:
-        e |= edges(seq_ranges)
-    return e
-
-
-def timed(h, fn, reps):
-    """(wall ms per call, {tag: kernel ms per call}, last result) of fn() repeated reps times"""
-    h.timing_enable(4096 * reps)
-    t0 = time.perf_counter()
-    for _ in range(reps):
-        out = fn()
-    wall = (time.perf_counter() - t0) * 1e3 / reps
-    ker = {}
-    for t, ms in h.timing_collect():
-        ker[t] = ker.get(t, 0.0) + ms / reps
-    h.timing_enable(0)
-    return wall, ker, out
-
-
-def synth_bank(T, seed):
-    ftr = sr_b200.synth_ftr_host(T, seed, 50, 100).view(ob.FTR_DTYPE).reshape(T)
-    return sr_b200.make_bank(ftr)
 
 
 def main():
@@ -82,9 +37,7 @@ def main():
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
 
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_connected: no CUDA device (there is nothing to measure without one)")
+    cuda_device("bench_connected")
     B, n = args.batch, args.sample
     h = sr_b200.Handle(0)
     co = ox.connected()
@@ -107,12 +60,13 @@ def main():
             h.set_bank(bank, T, 4096)
             for _ in range(args.warmup):
                 h.connected(feat, frm, PENALTY, 16)
-            wall, ker, (words, nw, tot) = timed(h, lambda: h.connected(feat, frm, PENALTY, 16), args.steps)
+            wall, recs, (words, nw, tot) = timed(h, lambda: h.connected(feat, frm, PENALTY, 16), args.steps,
+                                                 4096 * args.steps)
             idx = launch_sample(edges(seq_launches([0, B])), B, n, srng)
             ww, wn, wt = co.connected(feat[idx], frm[idx], bank, T, 4096, PENALTY, 16, nthreads=NPROC)
             ok = bool(np.array_equal(nw[idx], wn) and np.array_equal(tot[idx], wt) and np.array_equal(words[idx], ww))
             cells = float(N) * float(bank[:, 2:4].copy().view(np.uint16)[:, 0].astype(np.int64).sum()) * B
-            kms = ker[9]
+            kms = per_call(recs, args.steps)[9]
             results["decoder"].append({"N": N, "slots": T, "sequences": B, "kernel_ms": kms, "wall_ms": wall,
                                        "sequences_per_s": B / (kms * 1e-3), "cells_per_s": cells / (kms * 1e-3),
                                        "mean_words": float(nw.mean()), "sample_equals_oracle": ok})
@@ -125,18 +79,17 @@ def main():
     pcm = sr_b200.synth_pcm_host(E, U, 0xB0C3000, 3)
     for _ in range(args.warmup):
         h.recognise_connected(pcm, PENALTY, 8)
-    wall, ker, out = timed(h, lambda: h.recognise_connected(pcm, PENALTY, 8), args.steps)
+    wall, recs, out = timed(h, lambda: h.recognise_connected(pcm, PENALTY, 8), args.steps, 4096 * args.steps)
     idx = launch_sample(e2e_edges(out["frm_num"]), E, n, srng)
     want = ox.recognise_connected(ob.best_oracle(), co, pcm[idx], 2400, bank, 80, 4096, PENALTY, 8)
     ok = all(np.array_equal(out[k][idx], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
     results["end_to_end"].append({"U": U, "captures": E, "wall_ms": wall, "captures_per_s": E / (wall * 1e-3),
-                                  "kernel_ms": {str(k): v for k, v in sorted(ker.items())},
+                                  "kernel_ms": {str(k): v for k, v in sorted(per_call(recs, args.steps).items())},
                                   "mean_words": float(out["n_words"].mean()), "sample_equals_oracle": bool(ok)})
 
+    h.close()
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "penalty": PENALTY, "steps": args.steps,
             "sample": n, "results": results}
-    c = info["card"]
-    print("card: %s, power limit %s, max SM clock %s" % (c.get("name"), c.get("power.limit"), c.get("clocks.max.sm")))
     for x in results["decoder"]:
         print("decoder N=%-4d slots=%-3d kernel %9.2f ms  wall %9.1f ms  %8.3f Mseq/s  %7.2f Gcells/s  %.2f words  oracle %s" % (
             x["N"], x["slots"], x["kernel_ms"], x["wall_ms"], x["sequences_per_s"] / 1e6, x["cells_per_s"] / 1e9,
@@ -144,13 +97,7 @@ def main():
     for x in results["end_to_end"]:
         print("end to end U=%d B=%d  wall %9.1f ms  %9.0f captures/s  kernels %s  %.2f words  oracle %s" % (
             x["U"], x["captures"], x["wall_ms"], x["captures_per_s"], x["kernel_ms"], x["mean_words"], x["sample_equals_oracle"]))
-    print(json.dumps(info))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(info, f, indent=1)
-    h.close()
-    if not all(x["sample_equals_oracle"] for v in results.values() for x in v):
-        raise SystemExit("bench_connected: a sample differs from the oracle")
+    report("bench_connected", info, all(x["sample_equals_oracle"] for v in results.values() for x in v), args.json)
 
 
 if __name__ == "__main__":

@@ -13,25 +13,17 @@ pieces -- plus random ones, --sample in all. The card's name, power limit and SM
     python tools/bench_grammar.py [--steps 2] [--warmup 1] [--json FILE]
 """
 import argparse
-import json
-import os
-import sys
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import NPROC, card, cuda_device, e2e_edges, edges, per_call, report, synth_bank, timed
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
+from refs import launch_sample, record_cuts, seq_launches
 
-import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_connected import e2e_edges, edges, synth_bank, timed  # noqa: E402
-from bench_match import card  # noqa: E402
-from refs import launch_sample, record_cuts, seq_launches  # noqa: E402
-
-NPROC = os.cpu_count() or 1
 PENALTY = 4000
 PIN = (5, 1 << 4, [(k, k + 1, 0x3FF) for k in range(4)])
 PHONE = (12, 1 << 11, [(k, k + 1, 0x3FF) for k in range(11)])
@@ -72,9 +64,7 @@ def main():
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
 
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_grammar: no CUDA device (there is nothing to measure without one)")
+    cuda_device("bench_grammar")
     n = args.sample
     h = sr_b200.Handle(0)
     go = ox.grammar()
@@ -102,10 +92,10 @@ def main():
         h.connected_grammar(feat, frm, loop, PENALTY, 16)
     k6, k6g = [], []
     for _ in range(args.steps):
-        _, ker, out_k6 = timed(h, lambda: h.connected(feat, frm, PENALTY, 16), 1)
-        k6.append(ker[9])
-        _, ker, out = timed(h, lambda: h.connected_grammar(feat, frm, loop, PENALTY, 16), 1)
-        k6g.append(ker[10])
+        _, recs, out_k6 = timed(h, lambda: h.connected(feat, frm, PENALTY, 16), 1, 4096)
+        k6.append(per_call(recs, 1)[9])
+        _, recs, out = timed(h, lambda: h.connected_grammar(feat, frm, loop, PENALTY, 16), 1, 4096)
+        k6g.append(per_call(recs, 1)[10])
     same = all(np.array_equal(a, b) for a, b in zip(out_k6, out))
     row("loop grammar", B, 119, bank, 20, loop, float(np.median(k6g)), *out, feat, frm)
     rows[-1]["k6_kernel_ms"] = float(np.median(k6))
@@ -124,8 +114,8 @@ def main():
         frm = np.full(B, N, np.uint32)
         for _ in range(args.warmup):
             h.connected_grammar(feat, frm, g, PENALTY, 16)
-        _, ker, out = timed(h, lambda: h.connected_grammar(feat, frm, g, PENALTY, 16), args.steps)
-        row(name, B, N, avg, 40, g, ker[10], *out, feat, frm)
+        _, recs, out = timed(h, lambda: h.connected_grammar(feat, frm, g, PENALTY, 16), args.steps, 4096 * args.steps)
+        row(name, B, N, avg, 40, g, per_call(recs, args.steps)[10], *out, feat, frm)
         del feat
 
     # 4. end to end under the PIN grammar
@@ -133,18 +123,18 @@ def main():
     pcm = sr_b200.synth_pcm_host(E, U, 0xB6A4000, 3)
     for _ in range(args.warmup):
         h.recognise_connected_grammar(pcm, PIN, PENALTY, 8)
-    wall, ker, out = timed(h, lambda: h.recognise_connected_grammar(pcm, PIN, PENALTY, 8), args.steps)
+    wall, recs, out = timed(h, lambda: h.recognise_connected_grammar(pcm, PIN, PENALTY, 8), args.steps, 4096 * args.steps)
     idx = launch_sample(e2e_edges(out["frm_num"], seq_launches(record_cuts(out["frm_num"].sum(1), PIN[0]))), E, n, srng)
     want = ox.recognise_connected_grammar(ob.best_oracle(), go, pcm[idx], 2400, avg, 40, 4096, PIN, PENALTY, 8, nthreads=NPROC)
     ok = all(np.array_equal(out[k][idx], want[k]) for k in ("seg_off", "frm_num", "n_words", "total", "status", "words"))
     e2e = {"U": U, "captures": E, "wall_ms": wall, "captures_per_s": E / (wall * 1e-3),
-           "kernel_ms": {str(k): v for k, v in sorted(ker.items())}, "mean_words": float(out["n_words"].mean()),
+           "kernel_ms": {str(k): v for k, v in sorted(per_call(recs, args.steps).items())},
+           "mean_words": float(out["n_words"].mean()),
            "sample_equals_oracle": bool(ok)}
 
+    h.close()
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "penalty": PENALTY, "steps": args.steps,
             "sample": n, "decoder": rows, "end_to_end": e2e}
-    c = info["card"]
-    print("card: %s, power limit %s, max SM clock %s" % (c.get("name"), c.get("power.limit"), c.get("clocks.max.sm")))
     for x in rows:
         extra = "  K6 %.2f ms, overhead %+.1f %%" % (x["k6_kernel_ms"], 100 * x["overhead"]) if "overhead" in x else ""
         print("%-15s B=%-6d N=%-4d S=%-2d kernel %9.2f ms  %8.3f Mseq/s  %7.2f Gcells/s  %.2f words  oracle %s%s" % (
@@ -153,13 +143,7 @@ def main():
     print("end to end U=%d B=%d  wall %9.1f ms  %9.0f captures/s  kernels %s  %.2f words  oracle %s" % (
         e2e["U"], e2e["captures"], e2e["wall_ms"], e2e["captures_per_s"], e2e["kernel_ms"], e2e["mean_words"],
         e2e["sample_equals_oracle"]))
-    print(json.dumps(info))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(info, f, indent=1)
-    h.close()
-    if not (all(x["sample_equals_oracle"] for x in rows) and e2e["sample_equals_oracle"]):
-        raise SystemExit("bench_grammar: a sample differs from the oracle")
+    report("bench_grammar", info, all(x["sample_equals_oracle"] for x in rows) and e2e["sample_equals_oracle"], args.json)
 
 
 if __name__ == "__main__":

@@ -13,28 +13,20 @@ name, power limit and SM clock limit are read in the same run.
 """
 import argparse
 import json
-import os
-import sys
 import time
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
-
-HBM_PEAK = 3.35e12           # bytes/s, H100 SXM data sheet
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import HBM_PEAK, card, cuda_device, report, timed
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
 
 
 def vad_row(h, B, U, seed, steps, warmup, max_segs):
     """one VAD configuration on device-resident PCM: timings and the oracle check of every recording"""
-    import torch
     dev = torch.device("cuda:0")
     pcm = ox.synth_long(B, U, seed)
     d_pcm = torch.from_numpy(pcm.view(np.int16)).to(dev)
@@ -46,15 +38,7 @@ def vad_row(h, B, U, seed, steps, warmup, max_segs):
         h.vad_long_batch_dev(d_pcm.data_ptr(), U, B, None, 2400, max_segs, d_atap.data_ptr(), d_n.data_ptr(), d_seg.data_ptr())
     for _ in range(warmup):
         call()
-    h.sync()
-    h.timing_enable(8 * steps)
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        call()
-    h.sync()
-    wall = (time.perf_counter() - t0) / steps
-    rec = h.timing_collect()
-    h.timing_enable(0)
+    wall, rec, _ = timed(h, call, steps, 8 * steps)
     assert [t for t, _ in rec] == [11, 11, 12] * steps, rec
     atap_ms = sum(ms for k, (_, ms) in enumerate(rec) if k % 3 == 0) / steps
     block_ms = sum(ms for k, (_, ms) in enumerate(rec) if k % 3 == 1) / steps
@@ -69,7 +53,7 @@ def vad_row(h, B, U, seed, steps, warmup, max_segs):
     hours = B * U / 8000 / 3600
     nblk = B * (U // 80 + 1)
     block_bytes = B * U * 2 + nblk * 8
-    return dict(B=B, U=U, segments=int(got_n.sum()), wall_ms=wall * 1e3, atap_ms=atap_ms, block_ms=block_ms, segment_ms=seg_ms,
+    return dict(B=B, U=U, segments=int(got_n.sum()), wall_ms=wall, atap_ms=atap_ms, block_ms=block_ms, segment_ms=seg_ms,
                 vad_hours_per_s=hours / ((atap_ms + block_ms + seg_ms) / 1e3),
                 block_GBps=block_bytes / (block_ms / 1e3) / 1e9, block_share_of_hbm=block_bytes / (block_ms / 1e3) / HBM_PEAK,
                 oracle_ok=bool(ok), oracle_rows=B)
@@ -106,6 +90,7 @@ def main():
     ap.add_argument("--sample", type=int, default=16)
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
+    cuda_device("bench_long")
     h = sr_b200.Handle(0)
     res = dict(card=card(), rows={})
     res["rows"]["vad_1x2^27"] = vad_row(h, 1, 1 << 27, 0xB10, a.steps, a.warmup, 32768)
@@ -114,12 +99,7 @@ def main():
     h.close()
     for k, v in res["rows"].items():
         print(k, json.dumps(v))
-    print(json.dumps(res))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
-    if not all(v["oracle_ok"] for v in res["rows"].values()):
-        sys.exit(1)
+    report("bench_long", res, all(v["oracle_ok"] for v in res["rows"].values()), a.json)
 
 
 if __name__ == "__main__":

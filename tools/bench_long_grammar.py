@@ -13,20 +13,14 @@ on random others. The card's name and power limit are read in the same run; the 
 import argparse
 import json
 import os
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import ROOT, card, cuda_device, per_call, report, timed
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
 
 GROUP_BYTES = 256 << 20      # kLongGroupBytes: PCM per staged group
 REC_BYTES = 256 << 20        # kLongGramRecBytes: records per decoder launch
@@ -69,14 +63,8 @@ def row(h, pcm, bank, T, g, steps, warmup, sample, seed, max_segs=256, max_words
     B, U = pcm.shape
     for _ in range(warmup):
         h.recognise_long_grammar(pcm, g, 1000, max_segs, max_words)
-    h.timing_enable(1 << 16)
-    h.timing_collect()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        got = h.recognise_long_grammar(pcm, g, 1000, max_segs, max_words)
-    wall = (time.perf_counter() - t0) / steps
-    dec_ms = sum(ms for t, ms in h.timing_collect() if t == TAG_LONG_GRAM) / steps
-    h.timing_enable(0)
+    wall, recs, got = timed(h, lambda: h.recognise_long_grammar(pcm, g, 1000, max_segs, max_words), steps, 1 << 16)
+    dec_ms = per_call(recs, steps).get(TAG_LONG_GRAM, 0.0)
     N = got["frm_num"].sum(axis=1).astype(np.int64)
     assert (got["n_segs"] <= max_segs).all()
     frames = int(N.sum())
@@ -91,7 +79,7 @@ def row(h, pcm, bank, T, g, steps, warmup, sample, seed, max_segs=256, max_words
         m = min(int(want["n_words"][i]), max_words)
         ok &= got["words"][b, :m].tobytes() == want["words"][i, :m].tobytes()
         ok &= int(got["n_segs"][b]) == int(want["n_segs"][i])
-    return dict(B=B, U=U, states=g[0], frames=frames, decoder_ms=dec_ms, wall_ms=wall * 1e3,
+    return dict(B=B, U=U, states=g[0], frames=frames, decoder_ms=dec_ms, wall_ms=wall,
                 frames_per_s=frames / (dec_ms / 1e3), Gcells_per_s=cells / (dec_ms / 1e3) / 1e9,
                 words=int(got["n_words"].sum()), oracle_ok=bool(ok), oracle_rows=len(rows))
 
@@ -103,6 +91,7 @@ def main():
     ap.add_argument("--sample", type=int, default=8)
     ap.add_argument("--json", default=os.path.join(ROOT, "tools", "results", "bench_long_grammar_h100_700w.json"))
     a = ap.parse_args()
+    cuda_device("bench_long_grammar")
     h = sr_b200.Handle(0)
     tpl = sr_b200.synth_pcm_host(20, 8000, 0x7E3A0000)
     e = ob.port().recognise_batch(tpl, 2400, None, 0, 4096)
@@ -122,13 +111,7 @@ def main():
     h.close()
     for k, v in res["rows"].items():
         print(k, json.dumps(v))
-    print(json.dumps(res))
-    if a.json:
-        os.makedirs(os.path.dirname(a.json), exist_ok=True)
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
-    if not all(v["oracle_ok"] for v in res["rows"].values()):
-        sys.exit(1)
+    report("bench_long_grammar", res, all(v["oracle_ok"] for v in res["rows"].values()), a.json)
 
 
 if __name__ == "__main__":

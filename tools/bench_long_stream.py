@@ -14,21 +14,15 @@ The card's name, power limit and SM clock limit are read in the same run.
 """
 import argparse
 import json
-import os
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import card, cuda_device, report
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
 
 NREC = 64
 REC_KEYS = ("start", "end", "status", "frm_num", "best_idx", "best_dis", "cmd")
@@ -110,9 +104,7 @@ def main():
     ap.add_argument("--chunks", default="80,640", help="chunk lengths in samples (10 ms, 80 ms)")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_long_stream: no CUDA device (there is nothing to measure without one)")
+    cuda_device("bench_long_stream")
     S, total = args.streams, 8000 * args.seconds
     recs = ox.synth_long(NREC, 8000 * 60, 0x5EED1400)
     tpl = sr_b200.synth_pcm_host(12, 8000, 0x7E3A0000)
@@ -134,11 +126,7 @@ def main():
     finally:
         h.close()
         sr_b200.host_free(ptr)
-    res = dict(card=card(), streams=S, seconds=args.seconds, rows=rows)
-    print(json.dumps(res))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(res, f, indent=1)
+    report("bench_long_stream", dict(card=card(), streams=S, seconds=args.seconds, rows=rows), True, args.json)
 
 
 if __name__ == "__main__":

@@ -19,34 +19,15 @@ the strict '<' first-wins argmin. The card's name, power limit and SM clock limi
     python tools/bench_match.py [--steps 20] [--warmup 3] [--rounds 3] [--rows all|lifter] [--json FILE]
 """
 import argparse
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-import oracle_bind as ob  # noqa: E402
-import lifter_ref  # noqa: E402
-import sr_b200  # noqa: E402
-
-U, N_LEN = 8000, 2400
-SEED, TPL_SEED = 0x5EED0000, 0x7E3A0000       # bench.py's inputs
-
-
-def card():
-    """name, power limit and max SM clock of GPU 0, as nvidia-smi reports them (read only)"""
-    q = "name,power.limit,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=" + q, "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip()
-        return dict(zip(q.split(","), [x.strip() for x in out.split(",")]))
-    except (OSError, subprocess.SubprocessError) as e:
-        return {"error": str(e)}
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import N_LEN, NPROC, SEED, U, card, cuda_device, device_bank, event_steps, report, sample_rows
+import lifter_ref
+import oracle_bind as ob
+import sr_b200
 
 
 def main():
@@ -62,10 +43,7 @@ def main():
     ap.add_argument("--json", default=None, help="also write the results to this file")
     args = ap.parse_args()
 
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_match: no CUDA device (there is nothing to measure without one)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_match")
     B, T, n = args.batch, args.templates, min(args.sample, args.batch)
     stream = torch.cuda.Stream(dev)
     h = sr_b200.Handle(0)
@@ -73,27 +51,18 @@ def main():
     with torch.cuda.stream(stream):
         pcm = torch.empty((B, U), dtype=torch.int16, device=dev)
         sr_b200.synth_pcm_dev(pcm.data_ptr(), B, U, SEED, 1, stream.cuda_stream)
-        tpl = torch.empty((T, U), dtype=torch.int16, device=dev)
-        sr_b200.synth_pcm_dev(tpl.data_ptr(), T, U, TPL_SEED, 1, stream.cuda_stream)
-        tftr = torch.zeros((T, 2860), dtype=torch.uint8, device=dev)
-        h.set_bank_dev(0, 0, 4096)
-        h.recognise_dev(tpl.data_ptr(), U, T, N_LEN, ftr=tftr.data_ptr())
-        bank = torch.full((T, 4096), 255, dtype=torch.uint8, device=dev)
-        bank[:, :2860] = tftr
-        bank[:, 0], bank[:, 1] = 12345 & 0xFF, 12345 >> 8
+    bank = device_bank(h, stream, T)
+    with torch.cuda.stream(stream):
         outs = {k: torch.zeros(shape, dtype=dt, device=dev) for k, shape, dt in
                 (("seg_off", (B, 6), torch.int32), ("ftr", (B, 2860), torch.uint8), ("score", (B, T), torch.int32),
                  ("best_idx", (B,), torch.int32), ("best_dis", (B,), torch.int32), ("cmd", (B,), torch.int32),
                  ("status", (B,), torch.uint8))}
-    stream.synchronize()
-    h.set_bank_dev(bank.data_ptr(), T, 4096)
     ptrs = {k: v.data_ptr() for k, v in outs.items()}
 
     # the oracle's composition on the sample (the first n utterances and the last `tail`): the front end once, the
     # template scan per matcher
     bank_h = bank.cpu().numpy()
-    tail = min(args.tail, B - n)
-    rows = np.concatenate([np.arange(n), np.arange(B - tail, B)])
+    rows = sample_rows(B, n, args.tail)
     sample_pcm = pcm[torch.from_numpy(rows).to(dev)].cpu().numpy().view(np.uint16)
     front = ob.recognise_pinned(ob.best_oracle(), sample_pcm, N_LEN, None, 0, 4096)
     good = front["status"] == 0
@@ -104,25 +73,13 @@ def main():
     def oracle(flags, r):
         """the matcher's scores, and the cells of the port's greedy or banded DP at the same radius"""
         _, cells = ob.port().dtw_batch(front["ftr"][good], bank_h, T, 4096, check_sign=1, band_r=r if flags & ~LIFT else -1,
-                                       nthreads=os.cpu_count() or 1)
+                                       nthreads=NPROC)
         return lifter_ref.match_scores(front["ftr"][good], bank_h, T, flags, r), cells
 
     def run(flags, r):
         h.set_match(flags, r)
-        with torch.cuda.stream(stream):
-            for _ in range(args.warmup):
-                h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs)
-        stream.synchronize()
-        h.timing_enable(6 * args.steps + 8)
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        with torch.cuda.stream(stream):
-            ev0.record(stream)
-            for _ in range(args.steps):
-                h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs)
-            ev1.record(stream)
-        stream.synchronize()
-        recs = h.timing_collect()
-        h.timing_enable(0)
+        step_ms, recs = event_steps(h, stream, lambda: h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs), args.steps,
+                                    args.warmup, 6 * args.steps + 8)
         tag = 14 if flags & SYM else 6 if flags & sr_b200.DTW_BAND else 4
         dtw_ms = [ms for t, ms in recs if t == tag]
         assert len(dtw_ms) == args.steps, (flags, r, len(dtw_ms))
@@ -140,7 +97,7 @@ def main():
         m = flags & ~LIFT
         name = ("greedy" if not m else "sym" if m == SYM else "band-any" if m == RATE else "band") + ("+lift" if flags & LIFT else "")
         return {"matcher": name, "r": r if m else None,
-                "ms_per_step": ev0.elapsed_time(ev1) / args.steps,
+                "ms_per_step": step_ms,
                 "dtw_ms_mean": float(np.mean(dtw_ms)), "dtw_ms_min": float(np.min(dtw_ms)), "dtw_ms_max": float(np.max(dtw_ms)),
                 "oracle_cells_per_step": cells_batch, "cells_per_s": cells_batch / (float(np.mean(dtw_ms)) * 1e-3),
                 "sample_equals_oracle": bool(ok)}
@@ -153,23 +110,16 @@ def main():
     plan = lifter_plan if args.rows == "lifter" else plan + lifter_plan
     results = [run(f, r) for f, r in plan]
     h.set_match(0, 0)
+    h.close()
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "batch": B, "templates": T,
-            "steps": args.steps, "warmup": args.warmup, "sample": n, "tail": tail, "sample_ok_utterances": int(good.sum()),
-            "results": results}
-    print("card: %s, power limit %s, max SM clock %s" % (info["card"].get("name"), info["card"].get("power.limit"),
-                                                        info["card"].get("clocks.max.sm")))
+            "steps": args.steps, "warmup": args.warmup, "sample": n, "tail": len(rows) - n,
+            "sample_ok_utterances": int(good.sum()), "results": results}
     print("%-14s %5s %10s %12s %22s %10s %6s" % ("matcher", "r", "ms/step", "dtw ms mean", "dtw ms min-max", "Gcells/s", "oracle"))
     for x in results:
         print("%-14s %5s %10.3f %12.3f %10.3f-%-11.3f %10.2f %6s" % (
             x["matcher"], "" if x["r"] is None else x["r"], x["ms_per_step"], x["dtw_ms_mean"], x["dtw_ms_min"],
             x["dtw_ms_max"], x["cells_per_s"] / 1e9, x["sample_equals_oracle"]))
-    print(json.dumps(info))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(info, f, indent=1)
-    h.close()
-    if not all(x["sample_equals_oracle"] for x in results):
-        raise SystemExit("bench_match: a matcher's sample differs from the oracle")
+    report("bench_match", info, all(x["sample_equals_oracle"] for x in results), args.json)
 
 
 if __name__ == "__main__":

@@ -11,25 +11,17 @@ limit and SM clock limit are read in the same run.
 """
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-import resample_ref as rr  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
-
-HBM_PEAK = 3.35e12           # bytes/s, H100 SXM data sheet
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import HBM_PEAK, card, cuda_device, event_steps, report
+import resample_ref as rr
+import sr_b200
 
 
 def row(rate, B, secs, steps, warmup, sample, seed):
-    import torch
     dev = torch.device("cuda:0")
     U_in = rate * secs
     L, M = rr.ratio(rate)
@@ -43,15 +35,7 @@ def row(rate, B, secs, steps, warmup, sample, seed):
 
     def call():
         sr_b200.resample_adc12_dev(x.data_ptr(), U_in, B, None, rate, out.data_ptr(), U_out, olens.data_ptr(), s.cuda_stream)
-    for _ in range(warmup):
-        call()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(s)
-    for _ in range(steps):
-        call()
-    e1.record(s)
-    e1.synchronize()
-    ms = e0.elapsed_time(e1) / steps
+    ms, _ = event_steps(None, s, call, steps, warmup)
     # sampled check: first, last and two random recordings; their first and last 4096 outputs and 4 random windows
     rng = np.random.default_rng(seed)
     rows = sorted({0, B - 1, *rng.integers(0, B, 2).tolist()})
@@ -81,17 +65,13 @@ def main():
     ap.add_argument("--sample", type=int, default=4)
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
+    cuda_device("bench_resample")
     res = dict(card=card(), rows={})
     for rate in (int(r) for r in a.rates.split(",")):
         res["rows"]["%dHz" % rate] = row(rate, a.recordings, a.seconds, a.steps, a.warmup, a.sample, 0x5E5A + rate)
     for k, v in res["rows"].items():
         print(k, json.dumps(v))
-    print(json.dumps(res))
-    if a.json:
-        with open(a.json, "w") as f:
-            json.dump(res, f, indent=1)
-    if not all(v["oracle_ok"] for v in res["rows"].values()):
-        sys.exit(1)
+    report("bench_resample", res, all(v["oracle_ok"] for v in res["rows"].values()), a.json)
 
 
 if __name__ == "__main__":

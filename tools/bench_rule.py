@@ -15,25 +15,17 @@ and SM clock limit are read in the same run.
                                [--rounds 2] [--json FILE]
 """
 import argparse
-import json
-import os
-import sys
 
 import numpy as np
+import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "stm32-speech-recognition_b200", "python"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+# benchlib first: it puts the package and tests/ on sys.path
+from benchlib import N_LEN, SEED, U, card, cuda_device, device_bank, event_steps, report, sample_rows
+import oracle_bind as ob
+import oracle_ext as ox
+import sr_b200
+from refs import decide
 
-import oracle_bind as ob  # noqa: E402
-import oracle_ext as ox  # noqa: E402
-import sr_b200  # noqa: E402
-from bench_match import card  # noqa: E402
-from refs import decide  # noqa: E402
-
-U, N_LEN = 8000, 2400
-SEED, TPL_SEED = 0x5EED0000, 0x7E3A0000       # bench.py's inputs
 MATCHERS = ((0, 0), (sr_b200.DTW_BAND, 10), (sr_b200.DTW_BAND, 118))
 
 
@@ -51,10 +43,7 @@ def main():
     args = ap.parse_args()
     rules = [tuple(int(v) for v in x.split(":")) for x in args.rules.split(",")]
 
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_rule: no CUDA device (there is nothing to measure without one)")
-    dev = torch.device("cuda:0")
+    dev = cuda_device("bench_rule")
     B, n = args.batch, min(args.sample, args.batch)
     stream = torch.cuda.Stream(dev)
     h = sr_b200.Handle(0)
@@ -62,49 +51,27 @@ def main():
     with torch.cuda.stream(stream):
         pcm = torch.empty((B, U), dtype=torch.int16, device=dev)
         sr_b200.synth_pcm_dev(pcm.data_ptr(), B, U, SEED, 1, stream.cuda_stream)
-    tail = min(args.tail, B - n)
-    rows = np.concatenate([np.arange(n), np.arange(B - tail, B)])
+    rows = sample_rows(B, n, args.tail)
     stream.synchronize()
     sample_pcm = pcm[torch.from_numpy(rows).to(dev)].cpu().numpy().view(np.uint16)
     front = ob.recognise_pinned(ob.best_oracle(), sample_pcm, N_LEN, None, 0, 4096)
     good = front["status"] == 0
     results = []
     for T in [int(x) for x in args.templates.split(",")]:
+        bank = device_bank(h, stream, T)
         with torch.cuda.stream(stream):
-            tpl = torch.empty((T, U), dtype=torch.int16, device=dev)
-            sr_b200.synth_pcm_dev(tpl.data_ptr(), T, U, TPL_SEED, 1, stream.cuda_stream)
-            tftr = torch.zeros((T, 2860), dtype=torch.uint8, device=dev)
-            h.set_bank_dev(0, 0, 4096)
-            h.recognise_dev(tpl.data_ptr(), U, T, N_LEN, ftr=tftr.data_ptr())
-            bank = torch.full((T, 4096), 255, dtype=torch.uint8, device=dev)
-            bank[:, :2860] = tftr
-            bank[:, 0], bank[:, 1] = 12345 & 0xFF, 12345 >> 8
             outs = {k: torch.zeros(shape, dtype=dt, device=dev) for k, shape, dt in
                     (("seg_off", (B, 6), torch.int32), ("ftr", (B, 2860), torch.uint8), ("score", (B, T), torch.int32),
                      ("best_idx", (B,), torch.int32), ("best_dis", (B,), torch.int32), ("cmd", (B,), torch.int32),
                      ("status", (B,), torch.uint8))}
-        stream.synchronize()
-        h.set_bank_dev(bank.data_ptr(), T, 4096)
         ptrs = {k: v.data_ptr() for k, v in outs.items()}
         bank_h = bank.cpu().numpy()
         scores = {}
 
         def run(flags, r, k, q):
             h.set_match(flags | sr_b200.dtw_knn(k) | sr_b200.dtw_reject(q), r)
-            with torch.cuda.stream(stream):
-                for _ in range(args.warmup):
-                    h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs)
-            stream.synchronize()
-            h.timing_enable(6 * args.steps + 8)
-            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            with torch.cuda.stream(stream):
-                ev0.record(stream)
-                for _ in range(args.steps):
-                    h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs)
-                ev1.record(stream)
-            stream.synchronize()
-            recs = h.timing_collect()
-            h.timing_enable(0)
+            step_ms, recs = event_steps(h, stream, lambda: h.recognise_dev(pcm.data_ptr(), U, B, N_LEN, **ptrs),
+                                        args.steps, args.warmup, 6 * args.steps + 8)
             scan = 6 if flags else 4
             per = {t: [ms for tt, ms in recs if tt == t] for t in (3, scan, 5)}
             assert all(len(v) == args.steps for v in per.values()), (flags, r, k, q, {t: len(v) for t, v in per.items()})
@@ -122,7 +89,7 @@ def main():
                   and np.array_equal(got["best_dis"][good].view(np.uint32), d1)
                   and np.array_equal(got["cmd"][good].view(np.uint32), cmd))
             return {"templates": T, "matcher": "band" if flags else "greedy", "r": r if flags else None, "k": k, "q": q,
-                    "ms_per_step": ev0.elapsed_time(ev1) / args.steps,
+                    "ms_per_step": step_ms,
                     "init_ms": float(np.mean(per[3])), "scan_ms": float(np.mean(per[scan])),
                     "final_ms": float(np.mean(per[5])), "sample_rejected": int(rej.sum()),
                     "sample_cmd_changed": int((cmd != decide(sc)[2]).sum()), "sample_equals_oracle": bool(ok)}
@@ -134,24 +101,17 @@ def main():
             for s in settings:
                 results.append(run(*s))
     h.set_match(0, 0)
+    h.close()
     info = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "batch": B, "steps": args.steps,
-            "warmup": args.warmup, "rounds": args.rounds, "sample": n, "tail": tail,
+            "warmup": args.warmup, "rounds": args.rounds, "sample": n, "tail": len(rows) - n,
             "sample_ok_utterances": int(good.sum()), "results": results}
-    print("card: %s, power limit %s, max SM clock %s" % (info["card"].get("name"), info["card"].get("power.limit"),
-                                                        info["card"].get("clocks.max.sm")))
     print("%4s %-7s %5s %3s %6s %10s %9s %9s %9s %9s %9s %6s" % (
         "T", "matcher", "r", "k", "q", "ms/step", "init ms", "scan ms", "final ms", "rejected", "cmd diff", "oracle"))
     for x in results:
         print("%4d %-7s %5s %3d %6d %10.3f %9.4f %9.3f %9.4f %9d %9d %6s" % (
             x["templates"], x["matcher"], "" if x["r"] is None else x["r"], x["k"], x["q"], x["ms_per_step"], x["init_ms"],
             x["scan_ms"], x["final_ms"], x["sample_rejected"], x["sample_cmd_changed"], x["sample_equals_oracle"]))
-    print(json.dumps(info))
-    if args.json:
-        with open(args.json, "w") as f:
-            json.dump(info, f, indent=1)
-    h.close()
-    if not all(x["sample_equals_oracle"] for x in results):
-        raise SystemExit("bench_rule: a sample differs from the oracle")
+    report("bench_rule", info, all(x["sample_equals_oracle"] for x in results), args.json)
 
 
 if __name__ == "__main__":
