@@ -15,6 +15,7 @@
 #define SR_SYNTH_H_
 #include <stddef.h>
 #include <stdint.h>
+#include "sr_long_stream.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -48,6 +49,26 @@ int sr_resample_adc12_dev(const uint16_t *in /* [B][U_in] 12-bit codes at `rate`
                           const uint32_t *lens /* [B] device, or NULL = U_in */, uint32_t rate,
                           uint16_t *out /* [B][U_out] 12-bit codes at 8 kHz */, uint32_t U_out,
                           uint32_t *out_lens /* [B] device, or NULL */, void *cuda_stream);
+/* Live streams at any rate of SR_RESAMPLE_RATES: a pool of sr_long_stream.h whose streams are fed codes at `rate`, each
+ * resampled to 8 kHz on the GPU as it arrives (DESIGN.md, K14 at a rate). With (L, M), N and c = (N-1)/2 the rate's as
+ * above, a stream that has received n_in input samples since its reset has the 8 kHz stream
+ *   n8(n_in) = max(0, ceil((n_in*L - c) / M)) samples long -- exactly the outputs k whose newest input
+ *   (k*M + c) / L is below n_in -- holding the first n8(n_in) outputs of sr_resample_adc12_dev on those n_in samples
+ *   (inputs before sample 0 read as mid-code). They never change when more input arrives.
+ * Everything sr_long_stream.h says holds on that 8 kHz stream with n = n8(n_in): prefix equality with
+ * sr_recognise_long_batch (events, open_start, atap), the frame rule, calibration over its first n_len samples, event
+ * numbering and the matcher, bank and geometry rules. Every other sr_long_streams_* call takes the pool as it is:
+ *  - chunk_len, chunk_stride, lens and max_chunk (1 .. 2^20) count input samples at `rate`; event positions, n_recv
+ *    (sr_long_streams_state) and open_start are 8 kHz positions;
+ *  - ring_len and max_events follow sr_long_stream.h's formulas with max_chunk replaced by max8 = ceil(max_chunk*L/M),
+ *    the most 8 kHz samples one push can complete (n8(a + b) - n8(a) <= ceil(b*L/M));
+ *  - a push that would take a stream's input count past 2^32 - 1, or with lens[s] > max_chunk, fails before any stream
+ *    changes; a push runs one kernel more than at 8 kHz (five, six with a bank), still with one synchronisation.
+ * Refused before anything is allocated: a rate outside SR_RESAMPLE_RATES and every argument sr_long_streams_create
+ * refuses. rate = 8000 creates exactly the pool sr_long_streams_create creates. */
+int sr_long_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t max_chunk /* input samples */,
+                                   uint32_t n_len /* 8 kHz samples */, const atap_tag *atap /* [n_streams] or NULL */,
+                                   uint32_t rate, sr_long_stream_pool **out);
 #ifdef __cplusplus
 }
 #endif

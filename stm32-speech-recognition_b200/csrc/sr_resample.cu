@@ -6,12 +6,15 @@
 // memory, and hands out work items of one phase each: 32 lanes x R outputs L apart, so every lane of a warp reads the
 // same tap (one uniform load from the phase table in global memory serves R multiply-adds per lane). All arithmetic is
 // integer, and the tables keep |acc| < 2^31, so the s32 sums are exact. Results go through shared memory so that the
-// stores to the output row are coalesced.
+// stores to the output row are coalesced. The phase tables, the centring and the rounding are sr_resample_core.cuh's,
+// shared with K14's live streams at a rate.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <algorithm>
 #include <mutex>
 #include <vector>
 #include "../../include/sr_synth.h"
+#include "sr_resample_core.cuh"
 #include "sr_resample_taps.h"
 
 namespace {
@@ -59,7 +62,7 @@ __global__ void __launch_bounds__(kThreads) resample_kernel(const uint16_t *__re
     const uint16_t *x = in + (size_t)b * U_in;
     for (uint32_t i = threadIdx.x; i < p.span; i += kThreads) {
         const int64_t j = jlo + i;
-        s[i] = (j >= 0 && j < (int64_t)len) ? (int16_t)((int32_t)__ldg(x + j) - 2048) : (int16_t)0;
+        s[i] = (j >= 0 && j < (int64_t)len) ? resample_centre(__ldg(x + j)) : (int16_t)0;
     }
     __syncthreads();
 
@@ -82,22 +85,13 @@ __global__ void __launch_bounds__(kThreads) resample_kernel(const uint16_t *__re
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             const uint32_t nl = (qb * 32u * R + lane + 32u * r) * p.L + ph0;
-            int32_t y = 2048 + (int32_t)(((int64_t)acc[r] + (1 << 14)) >> 15);
-            y = y < 0 ? 0 : (y > 4095 ? 4095 : y);
-            if (nl < nt) o[nl] = (uint16_t)y;
+            if (nl < nt) o[nl] = resample_code(acc[r]);
         }
     }
     __syncthreads();
     uint16_t *dst = out + (size_t)b * U_out + n0;
     for (uint32_t i = threadIdx.x; i < nt; i += kThreads) dst[i] = o[i];
 }
-
-// per device: every rate's table as [L][K] phases (zero-padded to K taps) in one allocation, and the kernels' shared
-// memory limit raised to what the largest tile needs
-struct DeviceTables {
-    int32_t *hp = nullptr;
-    size_t off[kRates];
-};
 
 bool usable(const void *ptr, int dev, unsigned align) {
     if (!ptr || ((uintptr_t)ptr & (align - 1))) return false;
@@ -110,6 +104,47 @@ bool usable(const void *ptr, int dev, unsigned align) {
 }
 
 }  // namespace
+
+bool resample_rate(uint32_t rate, ResampleRate *out) {
+    for (const sr_resample_rate &r : sr_resample_rates)
+        if (r.rate == rate) {
+            *out = {r.rate, r.L, r.M, (r.N + r.L - 1) / r.L, (r.N - 1) / 2};
+            return true;
+        }
+    return false;
+}
+
+// per device: every rate's table as [L][K] phases (zero-padded to K taps) in one allocation
+const int32_t *resample_phases(uint32_t rate, int dev) {
+    static int32_t *tabs[64];
+    static std::mutex mu;
+    int k = 0;
+    while (k < kRates && sr_resample_rates[k].rate != rate) ++k;
+    if (k == kRates || dev < 0 || dev >= 64) return nullptr;
+    std::lock_guard<std::mutex> lk(mu);
+    size_t off[kRates], total = 0;
+    for (int r = 0; r < kRates; ++r) {
+        const sr_resample_rate &rr = sr_resample_rates[r];
+        off[r] = total;
+        total += (size_t)rr.L * ((rr.N + rr.L - 1) / rr.L);
+    }
+    if (!tabs[dev]) {
+        std::vector<int32_t> all(total, 0);
+        for (int r = 0; r < kRates; ++r) {
+            const sr_resample_rate &rr = sr_resample_rates[r];
+            const uint32_t K = (rr.N + rr.L - 1) / rr.L;
+            for (uint32_t i = 0; i < rr.N; ++i) all[off[r] + (size_t)(i % rr.L) * K + i / rr.L] = rr.h[i];
+        }
+        int32_t *d = nullptr;
+        if (cudaMalloc(&d, total * sizeof(int32_t)) != cudaSuccess) return nullptr;
+        if (cudaMemcpy(d, all.data(), total * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(d);
+            return nullptr;
+        }
+        tabs[dev] = d;
+    }
+    return tabs[dev] + off[k];
+}
 
 extern "C" int sr_resample_adc12_dev(const uint16_t *in, uint32_t U_in, uint32_t B, const uint32_t *lens, uint32_t rate,
                                      uint16_t *out, uint32_t U_out, uint32_t *out_lens, void *cuda_stream) {
@@ -128,37 +163,24 @@ extern "C" int sr_resample_adc12_dev(const uint16_t *in, uint32_t U_in, uint32_t
         (out_lens && !usable(out_lens, dev, 4)))
         return -1;
 
-    static DeviceTables tabs[64];
+    // the kernels' shared memory limit raised, once per device, to what the largest tile needs
+    static bool smem_set[64];
     static std::mutex mu;
     {
         std::lock_guard<std::mutex> lk(mu);
-        DeviceTables &t = tabs[dev];
-        if (!t.hp) {
-            std::vector<int32_t> all;
+        if (!smem_set[dev]) {
             size_t smem_max = 0;
-            for (int r = 0; r < kRates; ++r) {
-                const sr_resample_rate &rr = sr_resample_rates[r];
-                const Plan q = plan_of(rr);
-                t.off[r] = all.size();
-                all.resize(all.size() + (size_t)q.L * q.K, 0);
-                for (uint32_t i = 0; i < rr.N; ++i) all[t.off[r] + (size_t)(i % q.L) * q.K + i / q.L] = rr.h[i];
-                if (q.smem > smem_max) smem_max = q.smem;
-            }
+            for (const sr_resample_rate &rr : sr_resample_rates) smem_max = std::max(smem_max, plan_of(rr).smem);
             if (cudaFuncSetAttribute(resample_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) !=
                     cudaSuccess ||
                 cudaFuncSetAttribute(resample_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) !=
                     cudaSuccess)
                 return -1;
-            int32_t *d = nullptr;
-            if (cudaMalloc(&d, all.size() * sizeof(int32_t)) != cudaSuccess) return -1;
-            if (cudaMemcpy(d, all.data(), all.size() * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) {
-                cudaFree(d);
-                return -1;
-            }
-            t.hp = d;
+            smem_set[dev] = true;
         }
     }
-    const int32_t *hp = tabs[dev].hp + tabs[dev].off[k];
+    const int32_t *hp = resample_phases(rate, dev);
+    if (!hp) return -1;
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     const uint32_t grid = (uint32_t)(tiles * B);
     if (p.R == 4)

@@ -193,6 +193,7 @@ def lib():
         L.sr_streams_pending.argtypes = [vp]
         L.sr_streams_pending.restype = u32
         L.sr_long_streams_create.argtypes = [vp, u32, u32, u32, vp, C.POINTER(vp)]
+        L.sr_long_streams_create_at_rate.argtypes = [vp, u32, u32, u32, vp, u32, C.POINTER(vp)]
         L.sr_long_streams_destroy.argtypes = [vp]
         L.sr_long_streams_reset.argtypes = [vp, vp, vp]
         L.sr_long_streams_push.argtypes = [vp, vp, u32, u32, vp, u32, vp]
@@ -785,12 +786,19 @@ def _row_stride(chunk):
 
 class LongStreamPool:
     """sr_long_stream_pool wrapper (include/sr_long_stream.h): S live streams of any length, fed in chunks of at most
-    max_chunk samples, every segment decided as it closes. atap: [S] ATAP_DTYPE initial values or None (zeros)."""
+    max_chunk samples, every segment decided as it closes. atap: [S] ATAP_DTYPE initial values or None (zeros).
+    rate: None (8 kHz input, sr_long_streams_create), or the input rate of sr_long_streams_create_at_rate
+    (include/sr_synth.h; any of RESAMPLE_RATES, 8000 included): chunks and max_chunk then count samples at that rate,
+    while events, n_recv and open_start stay 8 kHz positions."""
 
-    def __init__(self, handle, n_streams, max_chunk, n_len=2400, atap=None):
-        self.S, self.h = n_streams, handle
+    def __init__(self, handle, n_streams, max_chunk, n_len=2400, atap=None, rate=None):
+        self.S, self.h, self.rate = n_streams, handle, rate
         self._p = C.c_void_p()
-        handle._ck(lib().sr_long_streams_create(handle._h, n_streams, max_chunk, n_len, _p(atap), C.byref(self._p)))
+        if rate is None:
+            handle._ck(lib().sr_long_streams_create(handle._h, n_streams, max_chunk, n_len, _p(atap), C.byref(self._p)))
+        else:
+            handle._ck(lib().sr_long_streams_create_at_rate(handle._h, n_streams, max_chunk, n_len, _p(atap), rate,
+                                                            C.byref(self._p)))
         self.max_events = int(lib().sr_long_streams_max_events(self._p))
         self._ev = (StreamEvent * self.max_events)()
         self.ring_len = int(lib().sr_long_streams_ring_len(self._p))
