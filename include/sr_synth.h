@@ -69,6 +69,34 @@ int sr_resample_adc12_dev(const uint16_t *in /* [B][U_in] 12-bit codes at `rate`
 int sr_long_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t max_chunk /* input samples */,
                                    uint32_t n_len /* 8 kHz samples */, const atap_tag *atap /* [n_streams] or NULL */,
                                    uint32_t rate, sr_long_stream_pool **out);
+/* Fixed captures at any rate of SR_RESAMPLE_RATES: a pool of speech_recog.h's streaming front end (sr_streams_*) whose
+ * streams are fed codes at `rate`, each resampled to 8 kHz on the GPU as it arrives (DESIGN.md, K4 at a rate). With n8
+ * as above, a stream that has received n_in input samples since the last reset has the 8 kHz stream of the first
+ * n8(n_in) = max(0, ceil((n_in*L - c) / M)) outputs of sr_resample_adc12_dev on those samples.
+ * Equivalence: after any sequence of pushes and resets, the pool is indistinguishable from the 8 kHz pool
+ * sr_streams_create(h, n_streams, max_samples, n_len) that is handed, at each push, every stream's outputs
+ * [n8(before), n8(after)) as one ragged push, under the same handle settings (geometry, matcher, bank) at each push:
+ * the same events from every push and from sr_streams_fetch, in the same order, the same sr_streams_pending and the same
+ * sr_streams_segments (seg_off and atap). So every rule of the 8 kHz pool applies to the 8 kHz stream: the capture of
+ * max_samples samples, the three segments, calibration over its first n_len samples, and positions in 8 kHz samples.
+ * As the 8 kHz pool drops the samples that arrive once its capture holds max_samples, this pool drops the 8 kHz outputs
+ * past max_samples (they are never computed); the push that brings them is accepted.
+ *  - chunk_len, chunk_stride and lens count input samples at `rate`. A push fails before any stream changes when one of
+ *    its lengths exceeds max_in = floor(max_samples*M/L), the longest chunk that never completes more than max_samples
+ *    8 kHz samples (n8(a + b) - n8(a) <= ceil(b*L/M)), or when it would take a stream's input count past 2^32 - 1;
+ *  - sr_streams_reset restarts the input counts and the filter's history too; a push runs one kernel more than at
+ *    8 kHz, still with one staging, one D2H copy of the events and one synchronisation;
+ *  - the last ceil(c/L) input samples of a capture complete no output until more input arrives (about 2 ms at every
+ *    rate): push a few milliseconds of audio after the end of speech so the VAD sees its last frames.
+ * Refused before anything is allocated: a rate outside SR_RESAMPLE_RATES and every argument sr_streams_create refuses.
+ * rate = 8000 creates exactly the pool sr_streams_create creates (max_in = max_samples, no input-count limit).
+ * A group at a rate is sr_stream_group_create with every shard created by sr_streams_create_at_rate; its push, drain and
+ * segment rules are unchanged, and chunk and lens are indexed by global stream. */
+int sr_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t max_samples /* 8 kHz */, uint32_t n_len /* 8 kHz */,
+                              uint32_t rate, sr_stream_pool **out);
+int sr_stream_group_create_at_rate(sr_handle *const *handles, uint32_t n_handles, uint32_t n_streams,
+                                   uint32_t max_samples /* 8 kHz */, uint32_t n_len /* 8 kHz */, uint32_t rate,
+                                   sr_stream_group **out);
 #ifdef __cplusplus
 }
 #endif

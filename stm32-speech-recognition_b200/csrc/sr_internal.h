@@ -14,6 +14,7 @@
 #include <thread>
 #include <vector>
 #include "sr_dtw_core.cuh"
+#include "sr_resample_core.cuh"
 #include "../../include/sr_long_grammar.h"
 
 namespace srk {
@@ -420,3 +421,30 @@ int stream_core_stage(StreamCore &c, const uint16_t *chunk, u32 chunk_stride, u3
                       u32 *chunk_dev_stride);
 int stream_core_recognise(StreamCore &c, const u16 *pcm, u32 row_len, sr_stream_event *events, u32 max_events, u32 *n_events);
 void stream_core_fetch(StreamCore &c, sr_stream_event *events, u32 max_events, u32 *n_events);
+
+// ---- a streaming pool's input at a rate other than 8 kHz (sr_stream.cu), for K4 and K14 alike ------------------------
+// Each push runs stream_resample_kernel before the pool's step kernel: it turns every stream's chunk into the 8 kHz
+// outputs whose filter support has arrived (resample_ready, sr_resample_core.cuh) and carries the stream's input count
+// and last K - 1 inputs to the next push. The step kernel reads the outputs through its ragged path. At 8 kHz there is
+// no stage (hp == NULL) and the pool is the plain one.
+struct ResampleStage {
+    ResampleRate rate{8000, 1, 1, 1, 0};
+    const int32_t *hp = nullptr;                   // the rate's [L][K] phase table on the pool's device
+    u32 T = 0, out_stride = 0, hist_stride = 0, grid = 0;   // outputs per window, row strides, launch width
+    size_t smem = 0;
+    DevBuf out, lens, n, hist;                     // 8 kHz staging [S][out_stride] and its counts [S]; input counts [S]
+                                                   // and carried inputs [S][hist_stride]
+};
+// the stage of S streams at `rate` whose pushes hold at most max_in input samples (nothing at 8 kHz); sets the kernel's
+// dynamic shared-memory limit to what the largest rate needs, the same value whichever pool sets it
+cudaError_t resample_stage_alloc(ResampleStage &r, sr_handle *h, u32 S, u32 rate, u32 max_in);
+// one launch on the handle's stream: the chunk (*chunk, *stride; *lens, or *uniform_len when NULL) becomes each stream's
+// new 8 kHz outputs below index `keep`, and *chunk .. *uniform_len then describe those outputs. Nothing at 8 kHz.
+int resample_stage_push(ResampleStage &r, sr_handle *h, u32 S, u32 keep, const u16 **chunk, u32 *stride, const u32 **lens,
+                        u32 *uniform_len);
+// in a reset kernel: stream s back to no input received, its carried inputs mid-code (no-op without a stage: n NULL)
+__device__ __forceinline__ void resample_stage_restart(u32 s, u32 *n, int16_t *hist, u32 hist_stride) {
+    if (!n) return;
+    n[s] = 0;
+    for (u32 i = 0; i < hist_stride; ++i) hist[(size_t)s * hist_stride + i] = 0;
+}

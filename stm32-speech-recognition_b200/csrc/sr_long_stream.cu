@@ -17,14 +17,14 @@
 // finish kernel, then one D2H copy and one synchronisation (stream_core_recognise, sr_stream.cu).
 //
 // A pool at a rate other than 8 kHz (sr_long_streams_create_at_rate, include/sr_synth.h) runs one more kernel before the
-// step kernel: long_stream_resample_kernel turns each stream's chunk into the 8 kHz outputs whose filter support has
-// arrived, n8(n_in) = resample_ready(n_in) of them in all, with K15's phases and arithmetic (sr_resample_core.cuh). The
-// stream's last K - 1 input samples are carried across pushes, so those outputs are the first n8 of sr_resample_adc12_dev
-// on everything pushed so far. The step kernel then takes them through its ragged path, unchanged.
+// step kernel: the resample stage K4 shares (ResampleStage, sr_stream.cu) turns each stream's chunk into the 8 kHz
+// outputs whose filter support has arrived, n8(n_in) = resample_ready(n_in) of them in all, with K15's phases and
+// arithmetic (sr_resample_core.cuh). The stream's last K - 1 input samples are carried across pushes, so those outputs
+// are the first n8 of sr_resample_adc12_dev on everything pushed so far. The step kernel then takes them through its
+// ragged path, unchanged.
 #include "sr_internal.h"
 #include "../../include/sr_long_stream.h"
 #include "../../include/sr_synth.h"
-#include "sr_resample_core.cuh"
 #include "sr_vad_core.cuh"
 
 namespace srk {
@@ -36,8 +36,7 @@ struct LongStreamState {        // one per stream, device resident
     StreamVad vad;
 };
 
-// rs_n / rs_hist (pools at a rate, else NULL): the input count and the hist_stride carried input samples of each stream,
-// back to none received and mid-code
+// rs_n / rs_hist: the pool's resample stage (at a rate, else NULL), restarted with the stream
 __global__ void long_stream_reset_kernel(LongStreamState *st, u32 S, const u8 *which, const atap_tag *atap, u32 *rs_n,
                                          int16_t *rs_hist, u32 hist_stride) {
     const u32 s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -47,10 +46,7 @@ __global__ void long_stream_reset_kernel(LongStreamState *st, u32 S, const u8 *w
     if (atap) z.atap = atap[s];
     z.vad.open_start = SR_SEG_NULL;
     st[s] = z;
-    if (rs_n) {
-        rs_n[s] = 0;
-        for (u32 i = 0; i < hist_stride; ++i) rs_hist[(size_t)s * hist_stride + i] = 0;
-    }
+    resample_stage_restart(s, rs_n, rs_hist, hist_stride);
 }
 
 __global__ void long_stream_query_kernel(const LongStreamState *st, u32 S, u32 *out /* [4][S] */, atap_tag *atap) {
@@ -156,94 +152,13 @@ long_stream_step_kernel(u16 *__restrict__ pcm, u32 R, u32 M, u32 row, u32 S, con
     }
 }
 
-// ---- K14 at a rate: the chunk -> the 8 kHz outputs it completes ------------------------------------------------------
-constexpr int kRsWarps = 16;
-constexpr u32 kRsSpan = 1024;                      // staged input samples per warp and window
-constexpr u32 kRsHistMax = 192;                    // K - 1 of the longest phase (48 kHz: 193 taps)
-constexpr uint32_t kRates[] = SR_RESAMPLE_RATES;
-
-// outputs per window: T, a multiple of 32, with ceil((T - 1) M / L) + K <= kRsSpan
-inline u32 rs_window(const ResampleRate &g) {
-    return (u32)(((uint64_t)(kRsSpan - g.K) * g.L / g.M + 1) / 32 * 32);
-}
-
-// One warp per stream (a grid-stride loop over streams), lanes over outputs. Stream s has received n0 = rs_n[s] input
-// samples and receives len more (lens == NULL: uniform_len); rs_hist holds inputs n0 - H .. n0 - 1 (H = K - 1, centred,
-// 0 before sample 0). Outputs [n8(n0), n8(n0 + len)) go to out[s][0, count), count to out_lens[s]; then the history
-// moves on to the last H inputs. Output k's newest input is j = (kM + c) / L >= n0, its oldest j - H >= n0 - H, so
-// history and chunk hold all it reads. The block's shared memory: the rate's [L][K] table, then per warp kRsSpan
-// centred inputs of one window of T outputs.
-__global__ void __launch_bounds__(kRsWarps * 32)
-long_stream_resample_kernel(const u16 *__restrict__ chunk, u32 chunk_stride, u32 uniform_len, const u32 *__restrict__ lens,
-                            u32 S, const int32_t *__restrict__ hp, ResampleRate g, u32 T, u32 *__restrict__ rs_n,
-                            int16_t *__restrict__ rs_hist, u32 hist_stride, u16 *__restrict__ out, u32 out_stride,
-                            u32 *__restrict__ out_lens) {
-    extern __shared__ int32_t rs_smem[];
-    int32_t *tab = rs_smem;                                                   // [L][K]
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int16_t *sx = reinterpret_cast<int16_t *>(rs_smem + g.L * g.K) + warp * kRsSpan;
-    for (u32 i = threadIdx.x; i < g.L * g.K; i += blockDim.x) tab[i] = __ldg(hp + i);
-    __syncthreads();
-    const u32 H = g.K - 1;
-    for (u32 s = blockIdx.x * kRsWarps + warp; s < S; s += gridDim.x * kRsWarps) {
-        const u32 n0 = rs_n[s], len = lens ? lens[s] : uniform_len;
-        const u16 *src = chunk + (size_t)s * chunk_stride;
-        int16_t *hist = rs_hist + (size_t)s * hist_stride;
-        const uint64_t k0 = resample_ready(n0, g.L, g.M, g.c), k1 = resample_ready((uint64_t)n0 + len, g.L, g.M, g.c);
-        u16 *dst = out + (size_t)s * out_stride;
-        for (uint64_t kb = k0; kb < k1; kb += T) {
-            const u32 nt = (u32)min((uint64_t)T, k1 - kb);
-            const uint64_t tb = kb * g.M + g.c;
-            const u32 pb = (u32)(tb % g.L);
-            const int64_t jb = (int64_t)(tb / g.L), jlo = jb - H;            // newest input of output kb, oldest staged
-            const u32 span = (u32)(((uint64_t)(nt - 1) * g.M + pb) / g.L) + g.K;
-            for (u32 i = lane; i < span; i += 32) {
-                const int64_t d = jlo + i - (int64_t)n0;                      // >= -H
-                sx[i] = d < 0 ? hist[d + H] : resample_centre(src[d]);
-            }
-            __syncwarp();
-            for (u32 q = lane; q < nt; q += 32) {
-                const u32 u = pb + q * g.M, p = u % g.L;
-                const int32_t *h = tab + p * g.K;
-                const int16_t *x = sx + H + u / g.L;                           // input jb + u / L
-                int32_t acc = 0;
-#pragma unroll 4
-                for (u32 m = 0; m < g.K; ++m) acc += h[m] * (int32_t)x[-(int32_t)m];
-                dst[kb - k0 + q] = resample_code(acc);
-            }
-            __syncwarp();
-        }
-        if (lane == 0) { out_lens[s] = (u32)(k1 - k0); rs_n[s] = n0 + len; }
-        if (len) {                                                            // inputs n0 + len - H .. n0 + len - 1
-            int16_t v[kRsHistMax / 32];
-#pragma unroll
-            for (u32 t = 0; t < kRsHistMax / 32; ++t) {
-                const u32 i = lane + 32 * t;
-                const int64_t d = (int64_t)len - H + i;                       // its offset from n0
-                v[t] = i >= H ? (int16_t)0 : d < 0 ? hist[d + H] : resample_centre(src[d]);
-            }
-            __syncwarp();
-#pragma unroll
-            for (u32 t = 0; t < kRsHistMax / 32; ++t)
-                if (lane + 32 * t < H) hist[lane + 32 * t] = v[t];
-        }
-        __syncwarp();
-    }
-}
-
 }  // namespace srk
 
 struct sr_long_stream_pool : StreamCore {
     u32 max_chunk = 0, n_len = 0, R = 0, row = 0, W = 0, info_stride = 0;
     DevBuf pcm, state, info, which, atap0, query;
     std::vector<uint64_t> n_host;                  // samples per stream since its reset, for the 2^32 - 1 limit
-    // at a rate other than 8 kHz: the rate, its phase table, outputs per window, the 8 kHz staging [S][rs_stride] with
-    // its counts, and each stream's input count and last K - 1 inputs ([S][hist_stride])
-    ResampleRate rate{8000, 1, 1, 1, 0};
-    const int32_t *rs_hp = nullptr;
-    u32 rs_T = 0, rs_stride = 0, hist_stride = 0, rs_grid = 0;
-    size_t rs_smem = 0;
-    DevBuf rs_out, rs_lens, rs_n, rs_hist;
+    ResampleStage rs;                              // at a rate other than 8 kHz
 };
 
 static int long_streams_push_impl(sr_long_stream_pool *p, const uint16_t *chunk, uint32_t chunk_stride, uint32_t uniform_len,
@@ -263,20 +178,8 @@ static int long_streams_push_impl(sr_long_stream_pool *p, const uint16_t *chunk,
     if (const int rc = stream_core_stage(*p, chunk, chunk_stride, max_len, lens != nullptr, &chunk_dev, &chunk_dev_stride)) return rc;
     const u32 *step_lens = (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr;
     u32 step_uniform = max_len ? uniform_len : 0u;
-    if (p->rs_hp) {                                   // at a rate: the step kernel takes the 8 kHz outputs instead
-        if (const int rc = launch_on(h, TAG_NONE, "long_stream_resample_kernel", [&] {
-                long_stream_resample_kernel<<<p->rs_grid, kRsWarps * 32, p->rs_smem, h->stream>>>(
-                    chunk_dev, chunk_dev_stride, step_uniform, step_lens, p->S, p->rs_hp, p->rate, p->rs_T,
-                    static_cast<u32 *>(p->rs_n.p), static_cast<int16_t *>(p->rs_hist.p), p->hist_stride,
-                    static_cast<u16 *>(p->rs_out.p), p->rs_stride, static_cast<u32 *>(p->rs_lens.p));
-                return cudaGetLastError();
-            }))
-            return rc;
-        chunk_dev = static_cast<const u16 *>(p->rs_out.p);
-        chunk_dev_stride = p->rs_stride;
-        step_lens = static_cast<const u32 *>(p->rs_lens.p);
-        step_uniform = 0;
-    }
+    if (const int rc = resample_stage_push(p->rs, h, p->S, 0xFFFFFFFFu, &chunk_dev, &chunk_dev_stride, &step_lens, &step_uniform))
+        return rc;                                    // at a rate: the step kernel takes the 8 kHz outputs instead
     if (const int rc = launch_on(h, TAG_NONE, "long_stream_step_kernel", [&] {
             long_stream_step_kernel<<<(p->S + kLsWarps - 1) / kLsWarps, kLsWarps * 32, 0, h->stream>>>(
                 static_cast<u16 *>(p->pcm.p), p->R, SR_LONG_STREAM_MIRROR, p->row, p->S, chunk_dev, chunk_dev_stride,
@@ -311,8 +214,8 @@ int sr_long_streams_reset(sr_long_stream_pool *p, const uint8_t *which, const at
     if (const int rc = launch_on(h, TAG_NONE, "long_stream_reset_kernel", [&] {
             long_stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(
                 static_cast<LongStreamState *>(p->state.p), p->S, which ? static_cast<const u8 *>(p->which.p) : nullptr,
-                atap ? static_cast<const atap_tag *>(p->atap0.p) : nullptr, static_cast<u32 *>(p->rs_n.p),
-                static_cast<int16_t *>(p->rs_hist.p), p->hist_stride);
+                atap ? static_cast<const atap_tag *>(p->atap0.p) : nullptr, static_cast<u32 *>(p->rs.n.p),
+                static_cast<int16_t *>(p->rs.hist.p), p->rs.hist_stride);
             return cudaGetLastError();
         }))
         return rc;
@@ -344,11 +247,6 @@ int sr_long_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t ma
     const u32 F = (max8 + c + SR_FRAME_MOV - 1) / SR_FRAME_MOV, E = (F + 18) / 19;
     SR_REQUIRE(h, (uint64_t)n_streams * E < (1ull << 31));
     DeviceGuard g_dev(h->device);
-    const int32_t *hp = nullptr;
-    if (rate != 8000) {
-        hp = resample_phases(rate, h->device);
-        if (!hp) return fail(h, "sr_long_streams_create_at_rate: phase table", cudaErrorMemoryAllocation);
-    }
     sr_long_stream_pool *p = new (std::nothrow) sr_long_stream_pool;
     SR_REQUIRE(h, p != nullptr);
     p->max_chunk = max_chunk; p->n_len = n_len;
@@ -367,27 +265,7 @@ int sr_long_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t ma
     need(p->which, n_streams);
     need(p->atap0, (size_t)n_streams * sizeof(atap_tag));
     need(p->query, (size_t)n_streams * (12 + sizeof(atap_tag)));
-    if (hp) {
-        p->rate = g; p->rs_hp = hp;
-        p->rs_T = rs_window(g);
-        p->rs_stride = (max8 + 7u) & ~7u;                             // staging rows start 16-byte aligned
-        p->hist_stride = (g.K - 1 + 7u) & ~7u;
-        p->rs_smem = (size_t)g.L * g.K * 4 + (size_t)kRsWarps * kRsSpan * 2;
-        const u32 blocks = (n_streams + kRsWarps - 1) / kRsWarps, per_sm = (u32)(200u * 1024u / p->rs_smem);
-        p->rs_grid = std::min(blocks, (u32)h->num_sms * std::max(per_sm, 1u));
-        need(p->rs_out, (size_t)n_streams * p->rs_stride * 2 + 64);
-        need(p->rs_lens, (size_t)n_streams * 4);
-        need(p->rs_n, (size_t)n_streams * 4);
-        need(p->rs_hist, (size_t)n_streams * p->hist_stride * 2);
-        // the limit every rate needs, the same value whichever pool sets it: pools at other rates may be launching
-        size_t smem_max = 0;
-        for (const uint32_t r : kRates) {
-            ResampleRate q;
-            if (resample_rate(r, &q)) smem_max = std::max(smem_max, (size_t)q.L * q.K * 4 + (size_t)kRsWarps * kRsSpan * 2);
-        }
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(long_stream_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
-    }
+    if (e == cudaSuccess) e = resample_stage_alloc(p->rs, h, n_streams, rate, max_chunk);
     if (e == cudaSuccess) e = cudaMemsetAsync(p->pcm.p, 0, (size_t)n_streams * p->row * 2 + 64, h->stream);
     if (e != cudaSuccess) { p->h = h; sr_long_streams_destroy(p); return fail(h, "sr_long_streams_create: allocation", e); }
     *out = p;

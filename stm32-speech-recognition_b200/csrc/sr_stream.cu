@@ -13,7 +13,14 @@
 // carried from push to push at frame granularity (StreamVad, as K14 carries them). After any push the FSM holds exactly
 // the decisions the sequential FSM has taken on the frames seen so far. One push = one H2D copy, five kernels whose batch
 // sizes are read from device memory (no host round trip between VAD and recognition), one D2H copy, ONE synchronisation.
+//
+// A pool at a rate other than 8 kHz (sr_streams_create_at_rate, include/sr_synth.h) runs one more kernel before the step
+// kernel: stream_resample_kernel, the resample stage it shares with K14 (ResampleStage, below), turns each stream's chunk
+// into the 8 kHz outputs whose filter support has arrived, carrying the stream's last K - 1 inputs across pushes. The
+// step kernel takes them through its ragged path, unchanged; outputs past the capture's end are not computed, as the
+// step kernel would drop them.
 #include "sr_internal.h"
+#include "../../include/sr_synth.h"
 #include "sr_vad_core.cuh"
 #include "sr_dtw_core.cuh"
 #include <condition_variable>
@@ -30,7 +37,8 @@ struct StreamState {            // one per stream, device resident
     StreamVad vad;
 };
 
-__global__ void stream_reset_kernel(StreamState *st, u32 S) {
+// rs_n / rs_hist: the pool's resample stage (at a rate, else NULL), restarted with the stream
+__global__ void stream_reset_kernel(StreamState *st, u32 S, u32 *rs_n, int16_t *rs_hist, u32 hist_stride) {
     const u32 s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
     StreamState z;
@@ -38,6 +46,7 @@ __global__ void stream_reset_kernel(StreamState *st, u32 S) {
     for (int i = 0; i < 6; ++i) z.seg[i] = SR_SEG_NULL;
     z.vad.open_start = SR_SEG_NULL;
     st[s] = z;
+    resample_stage_restart(s, rs_n, rs_hist, hist_stride);
 }
 
 // The FSM's actions on a capture: K0's segments in lanes, and an event for each of the first SR_MAX_VC_CON segments as it
@@ -165,6 +174,82 @@ __global__ void stream_finish_kernel(const StreamEventDev *ev, const u32 *n_ev, 
     out_rec[i] = r;
 }
 
+// ---- the resample stage of a pool at a rate: the chunk -> the 8 kHz outputs it completes (K4 and K14) ---------------
+constexpr int kRsWarps = 16;
+constexpr u32 kRsSpan = 1024;                      // staged input samples per warp and window
+constexpr u32 kRsHistMax = 192;                    // K - 1 of the longest phase (48 kHz: 193 taps)
+constexpr uint32_t kRates[] = SR_RESAMPLE_RATES;
+
+// outputs per window: T, a multiple of 32, with ceil((T - 1) M / L) + K <= kRsSpan
+inline u32 rs_window(const ResampleRate &g) {
+    return (u32)(((uint64_t)(kRsSpan - g.K) * g.L / g.M + 1) / 32 * 32);
+}
+
+// One warp per stream (a grid-stride loop over streams), lanes over outputs. Stream s has received n0 = rs_n[s] input
+// samples and receives len more (lens == NULL: uniform_len); rs_hist holds inputs n0 - H .. n0 - 1 (H = K - 1, centred,
+// 0 before sample 0). Outputs [n8(n0), n8(n0 + len)) below index `keep` go to out[s][0, count), count to out_lens[s];
+// then the history moves on to the last H inputs. Output k's newest input is j = (kM + c) / L >= n0, its oldest
+// j - H >= n0 - H, so history and chunk hold all it reads. The block's shared memory: the rate's [L][K] table, then per
+// warp kRsSpan centred inputs of one window of T outputs.
+__global__ void __launch_bounds__(kRsWarps * 32)
+stream_resample_kernel(const u16 *__restrict__ chunk, u32 chunk_stride, u32 uniform_len, const u32 *__restrict__ lens,
+                       u32 S, const int32_t *__restrict__ hp, ResampleRate g, u32 T, u32 keep, u32 *__restrict__ rs_n,
+                       int16_t *__restrict__ rs_hist, u32 hist_stride, u16 *__restrict__ out, u32 out_stride,
+                       u32 *__restrict__ out_lens) {
+    extern __shared__ int32_t rs_smem[];
+    int32_t *tab = rs_smem;                                                   // [L][K]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int16_t *sx = reinterpret_cast<int16_t *>(rs_smem + g.L * g.K) + warp * kRsSpan;
+    for (u32 i = threadIdx.x; i < g.L * g.K; i += blockDim.x) tab[i] = __ldg(hp + i);
+    __syncthreads();
+    const u32 H = g.K - 1;
+    for (u32 s = blockIdx.x * kRsWarps + warp; s < S; s += gridDim.x * kRsWarps) {
+        const u32 n0 = rs_n[s], len = lens ? lens[s] : uniform_len;
+        const u16 *src = chunk + (size_t)s * chunk_stride;
+        int16_t *hist = rs_hist + (size_t)s * hist_stride;
+        const uint64_t k0 = min(resample_ready(n0, g.L, g.M, g.c), (uint64_t)keep),
+                       k1 = min(resample_ready((uint64_t)n0 + len, g.L, g.M, g.c), (uint64_t)keep);
+        u16 *dst = out + (size_t)s * out_stride;
+        for (uint64_t kb = k0; kb < k1; kb += T) {
+            const u32 nt = (u32)min((uint64_t)T, k1 - kb);
+            const uint64_t tb = kb * g.M + g.c;
+            const u32 pb = (u32)(tb % g.L);
+            const int64_t jb = (int64_t)(tb / g.L), jlo = jb - H;            // newest input of output kb, oldest staged
+            const u32 span = (u32)(((uint64_t)(nt - 1) * g.M + pb) / g.L) + g.K;
+            for (u32 i = lane; i < span; i += 32) {
+                const int64_t d = jlo + i - (int64_t)n0;                      // >= -H
+                sx[i] = d < 0 ? hist[d + H] : resample_centre(src[d]);
+            }
+            __syncwarp();
+            for (u32 q = lane; q < nt; q += 32) {
+                const u32 u = pb + q * g.M, p = u % g.L;
+                const int32_t *h = tab + p * g.K;
+                const int16_t *x = sx + H + u / g.L;                           // input jb + u / L
+                int32_t acc = 0;
+#pragma unroll 4
+                for (u32 m = 0; m < g.K; ++m) acc += h[m] * (int32_t)x[-(int32_t)m];
+                dst[kb - k0 + q] = resample_code(acc);
+            }
+            __syncwarp();
+        }
+        if (lane == 0) { out_lens[s] = (u32)(k1 - k0); rs_n[s] = n0 + len; }
+        if (len) {                                                            // inputs n0 + len - H .. n0 + len - 1
+            int16_t v[kRsHistMax / 32];
+#pragma unroll
+            for (u32 t = 0; t < kRsHistMax / 32; ++t) {
+                const u32 i = lane + 32 * t;
+                const int64_t d = (int64_t)len - H + i;                       // its offset from n0
+                v[t] = i >= H ? (int16_t)0 : d < 0 ? hist[d + H] : resample_centre(src[d]);
+            }
+            __syncwarp();
+#pragma unroll
+            for (u32 t = 0; t < kRsHistMax / 32; ++t)
+                if (lane + 32 * t < H) hist[lane + 32 * t] = v[t];
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace srk
 
 // ---- what every streaming pool shares: the chunk read, recognition of the closed segments, the event queue ----------
@@ -286,9 +371,60 @@ void stream_core_fetch(StreamCore &c, sr_stream_event *events, u32 max_events, u
     *n_events = k;
 }
 
+cudaError_t resample_stage_alloc(ResampleStage &r, sr_handle *h, u32 S, u32 rate, u32 max_in) {
+    ResampleRate g;
+    if (rate == 8000 || !resample_rate(rate, &g)) return cudaSuccess;
+    const int32_t *hp = resample_phases(rate, h->device);
+    if (!hp) return cudaErrorMemoryAllocation;
+    r.rate = g; r.hp = hp;
+    r.T = rs_window(g);
+    const u32 max8 = (u32)(((uint64_t)max_in * g.L + g.M - 1) / g.M);  // the most 8 kHz samples one push completes
+    r.out_stride = (max8 + 7u) & ~7u;                                   // staging rows start 16-byte aligned
+    r.hist_stride = (g.K - 1 + 7u) & ~7u;
+    r.smem = (size_t)g.L * g.K * 4 + (size_t)kRsWarps * kRsSpan * 2;
+    const u32 blocks = (S + kRsWarps - 1) / kRsWarps, per_sm = (u32)(200u * 1024u / r.smem);
+    r.grid = std::min(blocks, (u32)h->num_sms * std::max(per_sm, 1u));
+    cudaError_t e = cudaSuccess;
+    auto need = [&](DevBuf &b, size_t bytes) { if (e == cudaSuccess) e = ensure(b, bytes); };
+    need(r.out, (size_t)S * r.out_stride * 2 + 64);
+    need(r.lens, (size_t)S * 4);
+    need(r.n, (size_t)S * 4);
+    need(r.hist, (size_t)S * r.hist_stride * 2);
+    // the limit every rate needs, the same value whichever pool sets it: pools at other rates may be launching
+    size_t smem_max = 0;
+    for (const uint32_t v : kRates) {
+        ResampleRate q;
+        if (resample_rate(v, &q)) smem_max = std::max(smem_max, (size_t)q.L * q.K * 4 + (size_t)kRsWarps * kRsSpan * 2);
+    }
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(stream_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+    return e;
+}
+
+int resample_stage_push(ResampleStage &r, sr_handle *h, u32 S, u32 keep, const u16 **chunk, u32 *stride, const u32 **lens,
+                        u32 *uniform_len) {
+    if (!r.hp) return 0;
+    if (const int rc = launch_on(h, TAG_NONE, "stream_resample_kernel", [&] {
+            stream_resample_kernel<<<r.grid, kRsWarps * 32, r.smem, h->stream>>>(
+                *chunk, *stride, *uniform_len, *lens, S, r.hp, r.rate, r.T, keep, static_cast<u32 *>(r.n.p),
+                static_cast<int16_t *>(r.hist.p), r.hist_stride, static_cast<u16 *>(r.out.p), r.out_stride,
+                static_cast<u32 *>(r.lens.p));
+            return cudaGetLastError();
+        }))
+        return rc;
+    *chunk = static_cast<const u16 *>(r.out.p);
+    *stride = r.out_stride;
+    *lens = static_cast<const u32 *>(r.lens.p);
+    *uniform_len = 0;
+    return 0;
+}
+
 struct sr_stream_pool : StreamCore {
     u32 L = 0, n_len = 0, info_stride = 0;
+    u32 max_in = 0;                                // the longest chunk in input samples: L at 8 kHz
     DevBuf pcm, state, info;
+    ResampleStage rs;                              // at a rate other than 8 kHz
+    std::vector<uint64_t> n_in;                    // at a rate: input samples per stream since the reset, for 2^32 - 1
 };
 
 static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t chunk_stride, uint32_t uniform_len,
@@ -310,26 +446,40 @@ int sr_streams_reset(sr_stream_pool *p) {
     DeviceGuard g(h->device);
     p->pending.clear();
     if (const int rc = launch_on(h, TAG_NONE, "stream_reset_kernel", [&] {
-            stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<StreamState *>(p->state.p), p->S);
+            stream_reset_kernel<<<(p->S + 127) / 128, 128, 0, h->stream>>>(static_cast<StreamState *>(p->state.p), p->S,
+                                                                          static_cast<u32 *>(p->rs.n.p),
+                                                                          static_cast<int16_t *>(p->rs.hist.p), p->rs.hist_stride);
             return cudaGetLastError();
         }))
         return rc;
+    std::fill(p->n_in.begin(), p->n_in.end(), 0);
     SR_CK(h, cudaMemsetAsync(p->pcm.p, 0, (size_t)p->S * p->L * 2, h->stream));
     return 0;
 }
 
 int sr_streams_create(sr_handle *h, uint32_t n_streams, uint32_t max_samples, uint32_t n_len, sr_stream_pool **out) {
+    return sr_streams_create_at_rate(h, n_streams, max_samples, n_len, 8000, out);
+}
+
+int sr_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t max_samples, uint32_t n_len, uint32_t rate,
+                              sr_stream_pool **out) {
     SR_REQUIRE(h, h && out && n_streams > 0 && max_samples > 0 && max_samples <= 65535u && n_len <= max_samples);
+    ResampleRate rg;
+    SR_REQUIRE(h, resample_rate(rate, &rg));
     DeviceGuard g(h->device);
     sr_stream_pool *p = new (std::nothrow) sr_stream_pool;
     SR_REQUIRE(h, p != nullptr);
     p->L = max_samples; p->n_len = n_len;
+    // the longest chunk completes at most max_samples 8 kHz samples: n8(a + b) - n8(a) <= ceil(b L / M) <= max_samples
+    p->max_in = (u32)(((uint64_t)max_samples * rg.M) / rg.L);
     p->info_stride = 2 * (max_samples / 80 + 2);
     cudaError_t e = stream_core_alloc(*p, h, n_streams, 3 * n_streams);
     auto need = [&](DevBuf &b, size_t bytes) { if (e == cudaSuccess) e = ensure(b, bytes); };
     need(p->pcm, (size_t)n_streams * max_samples * 2 + 64);
     need(p->state, (size_t)n_streams * sizeof(StreamState));
     need(p->info, (size_t)n_streams * p->info_stride * 4);
+    if (e == cudaSuccess) e = resample_stage_alloc(p->rs, h, n_streams, rate, p->max_in);
+    if (e == cudaSuccess && p->rs.hp) { try { p->n_in.assign(n_streams, 0); } catch (...) { e = cudaErrorMemoryAllocation; } }
     if (e != cudaSuccess) { sr_streams_destroy(p); return fail(h, "sr_streams_create: allocation", e); }
     *out = p;
     return sr_streams_reset(p);
@@ -386,22 +536,32 @@ static int streams_push_impl(sr_stream_pool *p, const uint16_t *chunk, uint32_t 
     *n_events = 0;
     const u32 max_len = stream_core_lens(*p, lens, uniform_len);
     SR_REQUIRE(h, max_len == 0 || chunk != nullptr);
-    SR_REQUIRE(h, max_len <= p->L && chunk_stride >= max_len);
+    SR_REQUIRE(h, max_len <= p->max_in && chunk_stride >= max_len);
+    if (p->rs.hp)                                                     // no input count past 2^32 - 1; nothing changes
+        for (u32 s = 0; s < p->S; ++s)
+            if (p->n_in[s] + (lens ? lens[s] : uniform_len) > 0xFFFFFFFFull)
+                return fail(h, "sr_streams_push: a stream would pass 2^32 - 1 input samples", cudaSuccess);
     DeviceGuard g(h->device);
     const u16 *chunk_dev;
     u32 chunk_dev_stride;
     if (const int rc = stream_core_stage(*p, chunk, chunk_stride, max_len, lens != nullptr, &chunk_dev, &chunk_dev_stride)) return rc;
+    const u32 *step_lens = (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr;
+    u32 step_uniform = max_len ? uniform_len : 0u;
+    // at a rate: the step kernel takes the 8 kHz outputs instead, none past the capture's end (it would drop them)
+    if (const int rc = resample_stage_push(p->rs, h, p->S, p->L, &chunk_dev, &chunk_dev_stride, &step_lens, &step_uniform))
+        return rc;
     u32 *n_ev = static_cast<u32 *>(p->n_ev.p);
     if (const int rc = launch_on(h, TAG_NONE, "stream_step_kernel", [&] {
             stream_step_kernel<<<(p->S + kStreamWarps - 1) / kStreamWarps, kStreamWarps * 32, 0, h->stream>>>(
-                static_cast<u16 *>(p->pcm.p), p->L, p->S, chunk_dev, chunk_dev_stride, max_len ? uniform_len : 0u,
-                (lens && max_len) ? static_cast<const u32 *>(p->lens.p) : nullptr, p->n_len, static_cast<StreamState *>(p->state.p),
-                static_cast<u32 *>(p->info.p), p->info_stride, static_cast<StreamEventDev *>(p->ev.p),
-                static_cast<u32 *>(p->seg_ev.p), static_cast<atap_tag *>(p->atap_ev.p), static_cast<u32 *>(p->map_ev.p), n_ev,
-                p->cap);
+                static_cast<u16 *>(p->pcm.p), p->L, p->S, chunk_dev, chunk_dev_stride, step_uniform, step_lens, p->n_len,
+                static_cast<StreamState *>(p->state.p), static_cast<u32 *>(p->info.p), p->info_stride,
+                static_cast<StreamEventDev *>(p->ev.p), static_cast<u32 *>(p->seg_ev.p), static_cast<atap_tag *>(p->atap_ev.p),
+                static_cast<u32 *>(p->map_ev.p), n_ev, p->cap);
             return cudaGetLastError();
         }))
         return rc;
+    if (p->rs.hp && max_len)
+        for (u32 s = 0; s < p->S; ++s) p->n_in[s] += lens ? lens[s] : uniform_len;
     return stream_core_recognise(*p, static_cast<const u16 *>(p->pcm.p), p->L, events, max_events, n_events);
 }
 
@@ -462,7 +622,14 @@ int sr_stream_group_destroy(sr_stream_group *gr) {
 
 int sr_stream_group_create(sr_handle *const *handles, uint32_t n_handles, uint32_t n_streams, uint32_t max_samples,
                            uint32_t n_len, sr_stream_group **out) {
-    if (!handles || !out || n_handles == 0 || n_streams < n_handles) return fail(nullptr, "sr_stream_group_create: bad arguments", cudaSuccess);
+    return sr_stream_group_create_at_rate(handles, n_handles, n_streams, max_samples, n_len, 8000, out);
+}
+
+int sr_stream_group_create_at_rate(sr_handle *const *handles, uint32_t n_handles, uint32_t n_streams, uint32_t max_samples,
+                                   uint32_t n_len, uint32_t rate, sr_stream_group **out) {
+    ResampleRate rg;
+    if (!handles || !out || n_handles == 0 || n_streams < n_handles || !resample_rate(rate, &rg))
+        return fail(nullptr, "sr_stream_group_create: bad arguments", cudaSuccess);
     sr_stream_group *gr = new (std::nothrow) sr_stream_group;
     if (!gr) return fail(nullptr, "sr_stream_group_create: out of memory", cudaErrorMemoryAllocation);
     gr->S = n_streams;
@@ -471,7 +638,7 @@ int sr_stream_group_create(sr_handle *const *handles, uint32_t n_handles, uint32
         sh->s0 = (u32)((uint64_t)n_streams * g / n_handles);
         sh->S = (u32)((uint64_t)n_streams * (g + 1) / n_handles) - sh->s0;
         gr->shards.push_back(sh);
-        const int rc = sr_streams_create(handles[g], sh->S, max_samples, n_len, &sh->pool);
+        const int rc = sr_streams_create_at_rate(handles[g], sh->S, max_samples, n_len, rate, &sh->pool);
         if (rc) { sr_stream_group_destroy(gr); return rc; }
         sh->ev.resize(3 * (size_t)sh->S);
         sh->th = std::thread(group_worker, sh);

@@ -207,6 +207,8 @@ def lib():
         L.sr_long_streams_ring_len.argtypes = [vp]
         L.sr_long_streams_ring_len.restype = u32
         L.sr_stream_group_create.argtypes = [C.POINTER(vp), u32, u32, u32, u32, C.POINTER(vp)]
+        L.sr_streams_create_at_rate.argtypes = [vp, u32, u32, u32, u32, C.POINTER(vp)]
+        L.sr_stream_group_create_at_rate.argtypes = [C.POINTER(vp), u32, u32, u32, u32, u32, C.POINTER(vp)]
         L.sr_stream_group_destroy.argtypes = [vp]
         L.sr_stream_group_reset.argtypes = [vp]
         L.sr_stream_group_push.argtypes = [vp, vp, u32, u32, vp, u32, vp]
@@ -694,20 +696,29 @@ def recognise_multi(handles, pcm, n_len=2400, want=("best_idx", "best_dis", "cmd
 class StreamPool:
     """sr_stream_pool / sr_stream_group wrapper: chunked capture of S streams, in lock step or ragged
     (include/speech_recog.h, streaming section). `handle` may be a list of handles: the streams are then sharded over
-    them (one GPU each)."""
+    them (one GPU each).
+    rate: None (8 kHz input, sr_streams_create / sr_stream_group_create), or the input rate of sr_streams_create_at_rate /
+    sr_stream_group_create_at_rate (include/sr_synth.h; any of RESAMPLE_RATES, 8000 included): chunks then count samples
+    at that rate, while max_samples, n_len and event positions stay 8 kHz samples."""
 
-    def __init__(self, handle, n_streams, max_samples, n_len=2400):
-        self.S, self.L = n_streams, max_samples
+    def __init__(self, handle, n_streams, max_samples, n_len=2400, rate=None):
+        self.S, self.L, self.rate = n_streams, max_samples, rate
         self._p = C.c_void_p()
         self.group = isinstance(handle, (list, tuple))
         self.h = handle[0] if self.group else handle
         if self.group:
             arr = (C.c_void_p * len(handle))(*[h._h for h in handle])
-            rc = lib().sr_stream_group_create(arr, len(handle), n_streams, max_samples, n_len, C.byref(self._p))
+            if rate is None:
+                rc = lib().sr_stream_group_create(arr, len(handle), n_streams, max_samples, n_len, C.byref(self._p))
+            else:
+                rc = lib().sr_stream_group_create_at_rate(arr, len(handle), n_streams, max_samples, n_len, rate,
+                                                          C.byref(self._p))
             if rc != 0:
                 raise SrError("sr_stream_group_create failed (%d): %s" % (rc, lib().sr_last_error(None).decode()))
-        else:
+        elif rate is None:
             handle._ck(lib().sr_streams_create(handle._h, n_streams, max_samples, n_len, C.byref(self._p)))
+        else:
+            handle._ck(lib().sr_streams_create_at_rate(handle._h, n_streams, max_samples, n_len, rate, C.byref(self._p)))
         self._ev = (StreamEvent * (3 * n_streams))()
 
     def _ck(self, rc):
