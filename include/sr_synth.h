@@ -16,6 +16,7 @@
 #include <stddef.h>
 #include <stdint.h>
 #include "sr_long_stream.h"
+#include "sr_long_grammar.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -97,6 +98,29 @@ int sr_streams_create_at_rate(sr_handle *h, uint32_t n_streams, uint32_t max_sam
 int sr_stream_group_create_at_rate(sr_handle *const *handles, uint32_t n_handles, uint32_t n_streams,
                                    uint32_t max_samples /* 8 kHz */, uint32_t n_len /* 8 kHz */, uint32_t rate,
                                    sr_stream_group **out);
+/* The host-buffer long-form calls at any rate of SR_RESAMPLE_RATES (DESIGN.md, long-form calls at a rate): recordings in
+ * host memory, rows of U_in codes at `rate` (sr_wav_to_adc12's output, say), resampled to 8 kHz on the GPU group by group.
+ * With (L, M) the rate's as above and U8 = ceil(U_in*L/M), recording b has len_b = lens[b] (U_in when lens is NULL) input
+ * samples and the 8 kHz recording y_b = the out_len_b = ceil(len_b*L/M) outputs of sr_resample_adc12_dev on them.
+ * Equivalence: the call writes exactly what sr_recognise_long_batch (sr_long.h), resp. sr_recognise_long_grammar_batch
+ * (sr_long_grammar.h), writes when given the recordings y_b at stride U8 with lens8[b] = out_len_b and the same n_len,
+ * initial atap, max_segs, grammar, penalty and max_words, under the handle's geometry, matcher and bank as they are when
+ * the call starts: every output field, and nothing else of the caller's memory. Segment offsets, n_len and atap are in
+ * 8 kHz samples, as in every other call.
+ *  - Staging: whole recordings in groups of at most 256 MB of input at the rate (at least one recording per group) through
+ *    the two device buffers of the 8 kHz calls, the copy of one group overlapping the work on the one before. Per group, on
+ *    the handle's stream, one K15 launch (timing tag 15) into an 8 kHz group buffer, then the 8 kHz call's per-group work.
+ *  - Refused before any copy or launch, with nothing written: a rate outside SR_RESAMPLE_RATES, U_in > SR_RESAMPLE_U_MAX,
+ *    U8 > SR_LONG_U_MAX, lens[b] > U_in, and every argument (with U8 and lens8 for U and lens) or grammar the 8 kHz call
+ *    refuses.
+ * rate = 8000 is the 8 kHz call: the same bytes and launches, no resample launch. */
+int sr_recognise_long_batch_at_rate(sr_handle *h, const uint16_t *pcm /* host [B][U_in] at rate */, uint32_t U_in, uint32_t B,
+                                    const uint32_t *lens /* host [B] input samples, or NULL = U_in */, uint32_t rate,
+                                    uint32_t n_len /* 8 kHz */, uint32_t max_segs, const sr_long_out *out);
+int sr_recognise_long_grammar_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B,
+                                            const uint32_t *lens, uint32_t rate, uint32_t n_len, const sr_grammar *g,
+                                            uint32_t penalty, uint32_t max_segs, uint32_t max_words,
+                                            const sr_long_gram_out *out);
 #ifdef __cplusplus
 }
 #endif

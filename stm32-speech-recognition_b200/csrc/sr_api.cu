@@ -3,6 +3,7 @@
 // recognition path happens on the host: every result is produced by the kernels in sr_vad.cu,
 // sr_mfcc.cu and sr_dtw.cu. Without a CUDA device every entry point fails loudly.
 #include "sr_internal.h"
+#include "../../include/sr_synth.h"
 #include "sr_pack_host.h"
 #include "sr_numa.h"
 #include <map>
@@ -1220,10 +1221,14 @@ static int recognise_segs_impl(sr_handle *h, const u16 *pcm, u32 U, u32 B, u32 m
 
 constexpr size_t kLongGroupBytes = (size_t)256 << 20;   // PCM per staged group of the host calls
 
-// The host-buffer long-form calls: whole recordings staged in groups of at most kLongGroupBytes of PCM (at least one
-// recording) through PcmGroups, and run(device PCM, first recording, recordings) per group. A recording is never split.
-template <class F> static int long_groups(HostCall &c, const uint16_t *pcm, u32 U, u32 B, F run) {
-    const PcmGroups pg(c, U, B, std::max(1u, std::min((u32)(kLongGroupBytes / ((size_t)U * 2)), B)));
+// recordings per staged group: as many rows of U samples as fit kLongGroupBytes, at least one, at most B
+static u32 long_group_size(u32 U, u32 B) { return std::max(1u, std::min((u32)(kLongGroupBytes / ((size_t)U * 2)), B)); }
+
+// The host-buffer long-form calls: whole recordings staged in groups of G (long_group_size: at most kLongGroupBytes of
+// PCM, at least one recording) through PcmGroups, and run(device PCM, first recording, recordings) per group. A recording
+// is never split.
+template <class F> static int long_groups(HostCall &c, const uint16_t *pcm, u32 U, u32 B, u32 G, F run) {
+    const PcmGroups pg(c, U, B, G);
     for (u32 g = 0; g < pg.n && !c.rc; ++g) {
         const u32 b0 = g * pg.G, nb = std::min(pg.G, B - b0);
         u16 *dpcm = pg.buf(g & 1);
@@ -1232,6 +1237,76 @@ template <class F> static int long_groups(HostCall &c, const uint16_t *pcm, u32 
         c.ck("PcmGroups::done", pg.done(g));
     }
     return c.finish();
+}
+
+// The 8 kHz recordings the per-group body of a host-buffer long-form call runs on. The caller's rows of U_in samples
+// (lens: host, or NULL) are staged by long_groups in groups of G recordings, at most kLongGroupBytes of input each, the
+// caller's lens in lng.lens. At 8 kHz the body takes each staged group as it is. At another rate, group() first runs K15
+// (tag 15) from the staged group into lng.pcm8, rows of U8 = ceil(U_in * L / M) samples, and its 8 kHz lengths into
+// lng.lens8, and the body takes those.
+struct LongSource {
+    HostCall &c;
+    u32 U_in, U8, G;
+    uint32_t rate;
+    const u32 *d_lens = nullptr;        // the caller's lens, staged (NULL: U_in)
+    u16 *pcm8 = nullptr;                // at a rate: [G][U8], G recordings per staged group
+    u32 *lens8 = nullptr;               // at a rate: [B]
+    LongSource(HostCall &cc, u32 U, u32 B, const u32 *lens, const ResampleRate &r)
+        : c(cc), U_in(U), U8((u32)(((uint64_t)U * r.L + r.M - 1) / r.M)), G(long_group_size(U, B)), rate(r.rate) {
+        d_lens = lens ? c.in(c.h->lng.lens, lens, (size_t)B * 4) : nullptr;
+        if (rate == 8000) return;
+        pcm8 = c.ws<u16>(c.h->lng.pcm8, (size_t)G * U8 * 2);
+        lens8 = c.ws<u32>(c.h->lng.lens8, (size_t)B * 4);
+    }
+    // recordings [b0, b0 + nb) staged at dpcm (rows of U_in samples) as the body reads them: pcm, row length U8, lens
+    int group(const u16 *dpcm, u32 b0, u32 nb, const u16 *&pcm, const u32 *&lens) const {
+        if (rate == 8000) {
+            pcm = dpcm;
+            lens = d_lens ? d_lens + b0 : nullptr;
+            return 0;
+        }
+        // grid: a group holds at most 2^27 rows, or rows of 2^27 samples together, and a tile at least 2 048 outputs
+        sr_handle *h = c.h;
+        SR_LAUNCH(h, TAG_RESAMPLE, launch_resample_adc12(dpcm, U_in, nb, d_lens ? d_lens + b0 : nullptr, rate, pcm8, U8,
+                                                         lens8 + b0, h->device, h->stream));
+        pcm = pcm8;
+        lens = lens8 + b0;
+        return 0;
+    }
+};
+
+// the argument rules of a host-buffer long-form call at a rate: the rate, U_in within K15's limit, and the 8 kHz call's
+// rules on U8 (lens8 <= U8 follows from lens <= U_in)
+static bool long_rate_args_ok(uint32_t rate, u32 U_in, u32 B, const u32 *lens, u32 n_len, u32 max_segs, ResampleRate *r) {
+    if (!resample_rate(rate, r) || U_in > SR_RESAMPLE_U_MAX) return false;
+    const uint64_t U8 = ((uint64_t)U_in * r->L + r->M - 1) / r->M;
+    if (U8 > SR_LONG_U_MAX || !long_host_args_ok((u32)U8, B, nullptr, n_len, max_segs)) return false;
+    for (u32 b = 0; lens && b < B; ++b)
+        if (lens[b] > U_in) return false;
+    return true;
+}
+
+static const ResampleRate kRate8k{8000, 1, 1, 1, 0};
+
+// sr_recognise_long_batch on the recordings of src, per staged group
+static int recognise_long_host(HostCall &c, const uint16_t *pcm, u32 B, const LongSource &src, u32 n_len, u32 max_segs,
+                               const sr_long_out *o) {
+    sr_handle *h = c.h;
+    atap_tag *d_atap = c.atap(h->lng.atap, o->atap, B, true);
+    u32 *d_n = o->n_segs ? c.out(h->lng.n_segs, o->n_segs, (size_t)B * 4) : nullptr;
+    const size_t rbytes = (size_t)B * max_segs * sizeof(sr_long_seg);
+    sr_long_seg *d_rec = nullptr;
+    if (rbytes) {                                                           // in / out: records past n_segs keep the caller's bytes
+        d_rec = c.in(h->lng.per_seg, o->segs, rbytes);
+        c.out(h->lng.per_seg, o->segs, rbytes);
+    }
+    return long_groups(c, pcm, src.U_in, B, src.G, [&](const u16 *dpcm, u32 b0, u32 nb) {
+        const u16 *p8;
+        const u32 *l8;
+        if (const int rc = src.group(dpcm, b0, nb, p8, l8)) return rc;
+        const sr_long_out od{d_atap + b0, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
+        return sr_recognise_long_batch_dev(h, p8, src.U8, nb, l8, n_len, max_segs, &od);
+    });
 }
 
 extern "C" {
@@ -1276,7 +1351,7 @@ int sr_vad_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B,
         d_seg = c.in(h->lng.per_seg, seg_off, sbytes);
         c.out(h->lng.per_seg, seg_off, sbytes);
     }
-    return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
+    return long_groups(c, pcm, U, B, long_group_size(U, B), [&](const u16 *dpcm, u32 b0, u32 nb) {
         return sr_vad_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, d_atap + b0, d_n + b0,
                                      d_seg ? d_seg + (size_t)b0 * max_segs * 2 : nullptr);
     });
@@ -1288,19 +1363,21 @@ int sr_recognise_long_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint3
     SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
     if (B == 0) return 0;
     HostCall c(h, "sr_recognise_long_batch");
-    const u32 *d_lens = lens ? c.in(h->lng.lens, lens, (size_t)B * 4) : nullptr;
-    atap_tag *d_atap = c.atap(h->lng.atap, o->atap, B, true);
-    u32 *d_n = o->n_segs ? c.out(h->lng.n_segs, o->n_segs, (size_t)B * 4) : nullptr;
-    const size_t rbytes = (size_t)B * max_segs * sizeof(sr_long_seg);
-    sr_long_seg *d_rec = nullptr;
-    if (rbytes) {                                                           // in / out: records past n_segs keep the caller's bytes
-        d_rec = c.in(h->lng.per_seg, o->segs, rbytes);
-        c.out(h->lng.per_seg, o->segs, rbytes);
-    }
-    return long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) {
-        const sr_long_out od{d_atap + b0, d_n ? d_n + b0 : nullptr, d_rec ? d_rec + (size_t)b0 * max_segs : nullptr};
-        return sr_recognise_long_batch_dev(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, max_segs, &od);
-    });
+    const LongSource src(c, U, B, lens, kRate8k);
+    return recognise_long_host(c, pcm, B, src, n_len, max_segs, o);
+}
+
+// at 8000 the 8 kHz call itself; else LongSource's K15 before each group's body
+int sr_recognise_long_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, const uint32_t *lens,
+                                    uint32_t rate, uint32_t n_len, uint32_t max_segs, const sr_long_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || (pcm && (o->segs || max_segs == 0))));
+    ResampleRate r;
+    SR_REQUIRE(h, long_rate_args_ok(rate, U_in, B, lens, n_len, max_segs, &r));
+    if (rate == 8000) return sr_recognise_long_batch(h, pcm, U_in, B, lens, n_len, max_segs, o);
+    if (B == 0) return 0;
+    HostCall c(h, "sr_recognise_long_batch_at_rate");
+    const LongSource src(c, U_in, B, lens, r);
+    return recognise_long_host(c, pcm, B, src, n_len, max_segs, o);
 }
 
 }  // extern "C"
@@ -1380,21 +1457,17 @@ int sr_connected_grammar_segs_batch(sr_handle *h, const int16_t *feat, const uin
     return c.finish();
 }
 
-// Per group of recordings (long_groups): the long-form VAD into long_seg_bound(U) slots per recording (tags 11, 12), one
+}  // extern "C"
+
+// sr_recognise_long_grammar_batch on the recordings of src under the copy table of gram_copies. Per group of recordings
+// (long_groups, then LongSource::group): the long-form VAD into long_seg_bound(U8) slots per recording (tags 11, 12), one
 // synchronisation for the plan, the feature pieces of every decodable segment (tag 1) and one decoder sequence per
 // recording over all its segments (tag 13). The per-segment records are written on the host from the plan.
-int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens,
-                                    uint32_t n_len, const sr_grammar *g, uint32_t penalty, uint32_t max_segs, uint32_t max_words,
-                                    const sr_long_gram_out *o) {
-    SR_REQUIRE(h, h && o && (B == 0 || pcm));
-    SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
-    if (B == 0) return 0;
-    DeviceGuard dg(h->device);
-    std::vector<u32> copy;
-    if (const int rc = gram_copies(h, g, copy)) return rc;
-    const u32 cap = long_seg_bound(U);
-    HostCall c(h, "sr_recognise_long_grammar_batch");
-    const u32 *d_lens = lens ? c.in(h->lng.lens, lens, (size_t)B * 4) : nullptr;
+static int recognise_long_grammar_host(HostCall &c, const uint16_t *pcm, u32 B, const LongSource &src,
+                                       const std::vector<u32> &copy, u32 n_len, const sr_grammar *g, u32 penalty,
+                                       u32 max_segs, u32 max_words, const sr_long_gram_out *o) {
+    sr_handle *h = c.h;
+    const u32 U = src.U8, cap = long_seg_bound(U);
     atap_tag *d_atap = c.atap(h->lng.atap, o->atap, B, true);
     u32 *d_n = c.ws<u32>(h->lng.n_segs, (size_t)B * 4);
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
@@ -1402,10 +1475,13 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
     std::vector<SegRec> recs;
     std::vector<u32> n_all(B), segv;
     std::vector<atap_tag> av;
-    const int rc = long_groups(c, pcm, U, B, [&](const u16 *dpcm, u32 b0, u32 nb) -> int {
+    const int rc = long_groups(c, pcm, src.U_in, B, src.G, [&](const u16 *dpcm_in, u32 b0, u32 nb) -> int {
         u32 *d_seg = c.ws<u32>(h->gram.vad_segs, (size_t)nb * cap * 8);
         if (c.rc) return 0;
-        if (const int r = vad_long_impl(h, dpcm, U, nb, d_lens ? d_lens + b0 : nullptr, n_len, cap, d_atap + b0, d_n + b0, d_seg))
+        const u16 *dpcm;
+        const u32 *d_lens;
+        if (const int r = src.group(dpcm_in, b0, nb, dpcm, d_lens)) return r;
+        if (const int r = vad_long_impl(h, dpcm, U, nb, d_lens, n_len, cap, d_atap + b0, d_n + b0, d_seg))
             return r;
         segv.resize((size_t)nb * cap * 2);
         av.resize(nb);
@@ -1453,6 +1529,39 @@ int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t 
         if (o->seg_status) o->seg_status[i] = r.status;
     }
     return 0;
+}
+
+extern "C" {
+
+int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens,
+                                    uint32_t n_len, const sr_grammar *g, uint32_t penalty, uint32_t max_segs, uint32_t max_words,
+                                    const sr_long_gram_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    SR_REQUIRE(h, long_host_args_ok(U, B, lens, n_len, max_segs));
+    if (B == 0) return 0;
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    HostCall c(h, "sr_recognise_long_grammar_batch");
+    const LongSource src(c, U, B, lens, kRate8k);
+    return recognise_long_grammar_host(c, pcm, B, src, copy, n_len, g, penalty, max_segs, max_words, o);
+}
+
+// at 8000 the 8 kHz call itself; else LongSource's K15 before each group's body
+int sr_recognise_long_grammar_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, const uint32_t *lens,
+                                            uint32_t rate, uint32_t n_len, const sr_grammar *g, uint32_t penalty,
+                                            uint32_t max_segs, uint32_t max_words, const sr_long_gram_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    ResampleRate r;
+    SR_REQUIRE(h, long_rate_args_ok(rate, U_in, B, lens, n_len, max_segs, &r));
+    if (rate == 8000) return sr_recognise_long_grammar_batch(h, pcm, U_in, B, lens, n_len, g, penalty, max_segs, max_words, o);
+    if (B == 0) return 0;
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    HostCall c(h, "sr_recognise_long_grammar_batch_at_rate");
+    const LongSource src(c, U_in, B, lens, r);
+    return recognise_long_grammar_host(c, pcm, B, src, copy, n_len, g, penalty, max_segs, max_words, o);
 }
 
 // One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]

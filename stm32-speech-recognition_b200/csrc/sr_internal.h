@@ -243,8 +243,11 @@ struct sr_handle {
     // - atap, n_segs: [B] atap records and segment counts. sr_recognise_long_batch_dev (when the caller passes none),
     //   sr_vad_long_batch, sr_recognise_long_batch, sr_recognise_long_grammar_batch
     // - per_seg: the caller's per-segment output. sr_vad_long_batch: seg_off; sr_recognise_long_batch: the records
-    // - lens: the caller's lens. sr_vad_long_batch, sr_recognise_long_batch, sr_recognise_long_grammar_batch
-    struct { DevBuf info, seg_off, first, n_flat, seg2, row, slot, atap_seg, status, keys, ftr, atap, n_segs, per_seg, lens; } lng;
+    // - lens: the caller's lens. sr_vad_long_batch, sr_recognise_long_batch, sr_recognise_long_grammar_batch and their
+    //   _at_rate forms (there in input samples)
+    // - pcm8, lens8: one staged group resampled to 8 kHz ([G][U8] samples) and every recording's 8 kHz length [B].
+    //   sr_recognise_long_batch_at_rate, sr_recognise_long_grammar_batch_at_rate
+    struct { DevBuf info, seg_off, first, n_flat, seg2, row, slot, atap_seg, status, keys, ftr, atap, n_segs, per_seg, lens, pcm8, lens8; } lng;
     // alignment: sr_dtw_path_batch and sr_average_bank
     // - in_bank: sr_dtw_path_batch: in; sr_average_bank: the bank image
     // - mdl_out: sr_dtw_path_batch: mdl; sr_average_bank: the output bank image
@@ -281,7 +284,7 @@ inline int fail(sr_handle *h, const char *what, cudaError_t e) {
 // ---- kernel launches: every one is counted (sr_launch_count); the tagged ones are timed ----------------------------
 enum { TAG_NONE = -1, TAG_VAD = 0, TAG_MFCC = 1, TAG_STATUS = 2, TAG_BEST_INIT = 3, TAG_DTW = 4, TAG_BEST_FINAL = 5,
        TAG_DTW_BAND = 6, TAG_ALIGN = 7, TAG_AVG_UPDATE = 8, TAG_CONN = 9,
-       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13, TAG_DTW_SYM = 14 };
+       TAG_GRAM = 10, TAG_LONG_BLOCKS = 11, TAG_LONG_SEGS = 12, TAG_LONG_GRAM = 13, TAG_DTW_SYM = 14, TAG_RESAMPLE = 15 };
 
 // one kernel launch on the handle's stream, launch() returning its cudaError_t (for <<<a, b>>>: cudaGetLastError()):
 // bracketed by an event pair when tag is not TAG_NONE and timing is enabled, counted when it succeeds

@@ -146,6 +146,41 @@ const int32_t *resample_phases(uint32_t rate, int dev) {
     return tabs[dev] + off[k];
 }
 
+// K15 on B recordings as one launch on st (declared in sr_resample_core.cuh); the caller has checked the rate, U_in, U_out,
+// the grid (tiles * B < 2^31) and the pointers
+cudaError_t launch_resample_adc12(const uint16_t *in, uint32_t U_in, uint32_t B, const uint32_t *lens, uint32_t rate,
+                                  uint16_t *out, uint32_t U_out, uint32_t *out_lens, int dev, cudaStream_t st) {
+    int k = 0;
+    while (k < kRates && sr_resample_rates[k].rate != rate) ++k;
+    if (k == kRates || dev < 0 || dev >= 64) return cudaErrorInvalidValue;
+    const Plan p = plan_of(sr_resample_rates[k]);
+    const uint64_t max_out = ((uint64_t)U_in * p.L + p.M - 1) / p.M;
+    const uint64_t tiles = max_out ? (max_out + p.T - 1) / p.T : 1;
+    // the kernels' shared memory limit raised, once per device, to what the largest tile needs
+    static bool smem_set[64];
+    static std::mutex mu;
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        if (!smem_set[dev]) {
+            size_t smem_max = 0;
+            for (const sr_resample_rate &rr : sr_resample_rates) smem_max = std::max(smem_max, plan_of(rr).smem);
+            cudaError_t e = cudaFuncSetAttribute(resample_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+            if (e == cudaSuccess)
+                e = cudaFuncSetAttribute(resample_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+            if (e != cudaSuccess) return e;
+            smem_set[dev] = true;
+        }
+    }
+    const int32_t *hp = resample_phases(rate, dev);
+    if (!hp) return cudaErrorMemoryAllocation;
+    const uint32_t grid = (uint32_t)(tiles * B);
+    if (p.R == 4)
+        resample_kernel<4><<<grid, kThreads, p.smem, st>>>(in, U_in, lens, out, U_out, out_lens, hp, p, (uint32_t)tiles);
+    else
+        resample_kernel<2><<<grid, kThreads, p.smem, st>>>(in, U_in, lens, out, U_out, out_lens, hp, p, (uint32_t)tiles);
+    return cudaGetLastError();
+}
+
 extern "C" int sr_resample_adc12_dev(const uint16_t *in, uint32_t U_in, uint32_t B, const uint32_t *lens, uint32_t rate,
                                      uint16_t *out, uint32_t U_out, uint32_t *out_lens, void *cuda_stream) {
     int k = 0;
@@ -162,30 +197,8 @@ extern "C" int sr_resample_adc12_dev(const uint16_t *in, uint32_t U_in, uint32_t
     if (!usable(in, dev, 2) || !usable(out, dev, 2) || (lens && !usable(lens, dev, 4)) ||
         (out_lens && !usable(out_lens, dev, 4)))
         return -1;
-
-    // the kernels' shared memory limit raised, once per device, to what the largest tile needs
-    static bool smem_set[64];
-    static std::mutex mu;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        if (!smem_set[dev]) {
-            size_t smem_max = 0;
-            for (const sr_resample_rate &rr : sr_resample_rates) smem_max = std::max(smem_max, plan_of(rr).smem);
-            if (cudaFuncSetAttribute(resample_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) !=
-                    cudaSuccess ||
-                cudaFuncSetAttribute(resample_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) !=
-                    cudaSuccess)
-                return -1;
-            smem_set[dev] = true;
-        }
-    }
-    const int32_t *hp = resample_phases(rate, dev);
-    if (!hp) return -1;
-    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    const uint32_t grid = (uint32_t)(tiles * B);
-    if (p.R == 4)
-        resample_kernel<4><<<grid, kThreads, p.smem, st>>>(in, U_in, lens, out, U_out, out_lens, hp, p, (uint32_t)tiles);
-    else
-        resample_kernel<2><<<grid, kThreads, p.smem, st>>>(in, U_in, lens, out, U_out, out_lens, hp, p, (uint32_t)tiles);
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+    return launch_resample_adc12(in, U_in, B, lens, rate, out, U_out, out_lens, dev, static_cast<cudaStream_t>(cuda_stream)) ==
+                   cudaSuccess
+               ? 0
+               : -1;
 }

@@ -18,6 +18,10 @@ bool resample_rate(uint32_t rate, ResampleRate *out);
 // the [L][K] phase table of `rate` (zero-padded to K taps per phase) on device dev, built on first use for every rate at
 // once; NULL when the rate is unknown or the table could not be built
 const int32_t *resample_phases(uint32_t rate, int dev);
+// K15 (sr_resample_adc12_dev) on B recordings of device dev as one launch on st, for callers that have checked the rate,
+// U_in, U_out and the pointers: the public call, and the host-buffer long-form calls at a rate under SR_LAUNCH
+cudaError_t launch_resample_adc12(const uint16_t *in, uint32_t U_in, uint32_t B, const uint32_t *lens, uint32_t rate,
+                                  uint16_t *out, uint32_t U_out, uint32_t *out_lens, int dev, cudaStream_t st);
 
 // an input code as the tables' sums take it
 __device__ __forceinline__ int16_t resample_centre(uint16_t x) { return (int16_t)((int32_t)x - 2048); }

@@ -183,6 +183,9 @@ def lib():
         L.sr_recognise_long_batch_dev.argtypes = [vp, vp, u32, u32, vp, u32, u32, C.POINTER(LongOut)]
         L.sr_connected_grammar_segs_batch.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp, vp, vp]
         L.sr_recognise_long_grammar_batch.argtypes = [vp, vp, u32, u32, vp, u32, vp, u32, u32, u32, C.POINTER(LongGramOut)]
+        L.sr_recognise_long_batch_at_rate.argtypes = [vp, vp, u32, u32, vp, u32, u32, u32, C.POINTER(LongOut)]
+        L.sr_recognise_long_grammar_batch_at_rate.argtypes = [vp, vp, u32, u32, vp, u32, u32, vp, u32, u32, u32,
+                                                              C.POINTER(LongGramOut)]
         L.sr_streams_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
         L.sr_streams_destroy.argtypes = [vp]
         L.sr_streams_reset.argtypes = [vp]
@@ -524,16 +527,22 @@ class Handle:
                                          _p(seg_off) if max_segs else None))
         return dict(atap=atap, n_segs=n_segs, seg_off=seg_off)
 
-    def recognise_long_batch(self, pcm, max_segs, n_len=2400, lens=None, atap=None, segs=None):
+    def recognise_long_batch(self, pcm, max_segs, n_len=2400, lens=None, atap=None, segs=None, rate=None):
         """long-form VAD, then spch_recg's decision on every segment: dict(atap [B], n_segs [B], segs [B, max_segs]
-        LONG_SEG_DTYPE); atap and segs are in / out"""
+        LONG_SEG_DTYPE); atap and segs are in / out. rate: None (8 kHz input, sr_recognise_long_batch), or the input rate
+        of sr_recognise_long_batch_at_rate (include/sr_synth.h; any of RESAMPLE_RATES): pcm and lens then count samples
+        at that rate, while n_len and the segment offsets stay in 8 kHz samples"""
         B, U = pcm.shape
         atap = np.zeros(B, ATAP_DTYPE) if atap is None else atap
         segs = np.zeros((B, max_segs), LONG_SEG_DTYPE) if segs is None else segs
         lens = None if lens is None else np.ascontiguousarray(lens, np.uint32)
         n_segs = np.zeros(B, np.uint32)
         out = LongOut(_p(atap), _p(n_segs), _p(segs) if max_segs else None)
-        self._ck(lib().sr_recognise_long_batch(self._h, _p(pcm), U, B, _p(lens), n_len, max_segs, C.byref(out)))
+        if rate is None:
+            self._ck(lib().sr_recognise_long_batch(self._h, _p(pcm), U, B, _p(lens), n_len, max_segs, C.byref(out)))
+        else:
+            self._ck(lib().sr_recognise_long_batch_at_rate(self._h, _p(pcm), U, B, _p(lens), rate, n_len, max_segs,
+                                                           C.byref(out)))
         return dict(atap=atap, n_segs=n_segs, segs=segs)
 
     def vad_long_batch_dev(self, pcm_ptr, U, B, lens_ptr, n_len, max_segs, atap_ptr, n_segs_ptr, seg_ptr):
@@ -564,10 +573,11 @@ class Handle:
         return words, n_words, total
 
     def recognise_long_grammar(self, pcm, grammar_, penalty, max_segs, max_words, n_len=2400, lens=None,
-                               want=LONG_GRAM_FIELDS, out=None):
+                               want=LONG_GRAM_FIELDS, out=None, rate=None):
         """long-form VAD, long features of every decodable segment and one grammar decode per recording
         (sr_recognise_long_grammar_batch): a dict of the sr_long_gram_out fields named in `want` (or the arrays of `out`,
-        filled in place)"""
+        filled in place). rate: None (8 kHz input), or the input rate of sr_recognise_long_grammar_batch_at_rate
+        (include/sr_synth.h), as in recognise_long_batch"""
         B, U = pcm.shape
         if out is None:
             shape = {"atap": (B, ATAP_DTYPE), "n_segs": (B, np.uint32), "seg_off": ((B, max_segs, 2), np.uint32),
@@ -577,9 +587,14 @@ class Handle:
         lens = None if lens is None else np.ascontiguousarray(lens, np.uint32)
         o = LongGramOut(*[_p(out.get(k)) for k in LONG_GRAM_FIELDS])
         g = grammar(grammar_)
-        self._ck(lib().sr_recognise_long_grammar_batch(self._h, _p(pcm), U, B, _p(lens), n_len,
-                                                       None if g is None else C.byref(g), penalty, max_segs, max_words,
-                                                       C.byref(o)))
+        if rate is None:
+            self._ck(lib().sr_recognise_long_grammar_batch(self._h, _p(pcm), U, B, _p(lens), n_len,
+                                                           None if g is None else C.byref(g), penalty, max_segs, max_words,
+                                                           C.byref(o)))
+        else:
+            self._ck(lib().sr_recognise_long_grammar_batch_at_rate(self._h, _p(pcm), U, B, _p(lens), rate, n_len,
+                                                                   None if g is None else C.byref(g), penalty, max_segs,
+                                                                   max_words, C.byref(o)))
         return out
 
     def fft_mag(self, frames):
