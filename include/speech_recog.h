@@ -557,7 +557,8 @@ int sr_debug_unpack12(sr_handle *h, const uint8_t *packed, uint64_t n, uint16_t 
  * sr_recognise_connected_batch; their get_mfcc launches are tag 1), 10 the grammar decoder (sr_connected_grammar_batch,
  * sr_recognise_connected_grammar_batch; their get_mfcc launches are tag 1), 11 and 12 the long-form block and segment passes
  * (include/sr_long.h), 14 dtw (the symmetric P = 1 DP, in sr_dtw_batch* and in recognise calls under the SR_DTW_SYM_P1
- * matcher), 15 the resampling of a staged group to 8 kHz (the long-form calls at a rate of include/sr_synth.h).
+ * matcher), 15 the resampling of a staged group to 8 kHz (the long-form calls at a rate of include/sr_synth.h), of a
+ * chunk (sr_recognise_batch_at_rate) or of a whole batch (the other capture calls at a rate of include/sr_synth.h).
  * max_records = 0 disables. */
 int sr_timing_enable(sr_handle *h, uint32_t max_records);
 int sr_timing_collect(sr_handle *h, uint32_t *tags, float *ms, uint32_t cap, uint32_t *n);

@@ -121,6 +121,36 @@ int sr_recognise_long_grammar_batch_at_rate(sr_handle *h, const uint16_t *pcm, u
                                             const uint32_t *lens, uint32_t rate, uint32_t n_len, const sr_grammar *g,
                                             uint32_t penalty, uint32_t max_segs, uint32_t max_words,
                                             const sr_long_gram_out *out);
+/* The host-buffer capture calls at any rate of SR_RESAMPLE_RATES (DESIGN.md, capture calls at a rate): save_mdl and
+ * spch_recg (speech_recog.h) on captures in host memory, rows of U_in codes at `rate`, resampled to 8 kHz on the GPU.
+ * With (L, M) the rate's as above and U8 = ceil(U_in*L/M), capture b becomes y_b = the U8 outputs of
+ * sr_resample_adc12_dev on its U_in samples (captures have no lens: every y_b is U8 long).
+ * Equivalence: the call writes exactly what the 8 kHz call -- sr_recognise_batch, sr_recognise_batch_multi,
+ * sr_enrol_batch, sr_recognise_connected_batch, sr_recognise_connected_grammar_batch -- writes when given the captures y_b
+ * at stride U8 with the same n_len, initial atap, bank, penalty, grammar and max_words, under the handle's geometry,
+ * matcher, lifter and decision rules as they are when the call starts: every output field, and nothing else of the
+ * caller's memory. As there, atap is left untouched when n_len % 240 != 0, and only frm_num and the first frm_num rows of
+ * a feature struct are written. n_len, seg_off, atap and word frames are in 8 kHz samples, as in every other call.
+ *  - sr_recognise_batch_at_rate keeps the 8 kHz call's chunk pipeline and packed transport: chunks of about 32 MB of
+ *    input (a multiple of 8 captures), each staged, expanded when packed, then one K15 launch (timing tag 15) and the 8 kHz
+ *    recognition of the chunk. sr_transport_stats counts input bytes. sr_recognise_batch_multi_at_rate shards the batch
+ *    as sr_recognise_batch_multi does, each shard running sr_recognise_batch_at_rate.
+ *  - The other three stage the whole batch in one copy, then one K15 launch (tag 15), then the 8 kHz call's work.
+ *  - Refused before any copy or launch, with nothing written: a rate outside SR_RESAMPLE_RATES, U8 > 65535 (so U_in is
+ *    at most floor(65535*M/L): 393 210 at 48 kHz, 361 261 at 44.1 kHz, 131 070 at 16 kHz), n_len > U8, and every
+ *    argument (with U8 for U), bank or grammar the 8 kHz call refuses.
+ * rate = 8000 is the 8 kHz call: the same bytes, launches, tags and transport statistics, no resample launch. */
+int sr_recognise_batch_at_rate(sr_handle *h, const uint16_t *pcm /* host [B][U_in] at rate */, uint32_t U_in, uint32_t B,
+                               uint32_t rate, uint32_t n_len /* 8 kHz */, const sr_recog_out *out);
+int sr_recognise_batch_multi_at_rate(sr_handle *const *handles, uint32_t n_handles, const uint16_t *pcm, uint32_t U_in,
+                                     uint32_t B, uint32_t rate, uint32_t n_len, const sr_recog_out *out);
+int sr_enrol_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate, uint32_t n_len,
+                           void *bank_out, uint32_t slot_stride, uint8_t *status);
+int sr_recognise_connected_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate,
+                                         uint32_t n_len, uint32_t penalty, uint32_t max_words, const sr_conn_out *out);
+int sr_recognise_connected_grammar_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate,
+                                                 uint32_t n_len, const sr_grammar *g, uint32_t penalty, uint32_t max_words,
+                                                 const sr_conn_out *out);
 #ifdef __cplusplus
 }
 #endif

@@ -312,6 +312,36 @@ struct PcmGroups {
     cudaError_t done(u32 k) const { return n > 1 ? cudaEventRecord(h->ev_done[k & 1], h->stream) : cudaSuccess; }
 };
 
+// ---- input at another rate (include/sr_synth.h) ------------------------------------------------------------------------
+static const ResampleRate kRate8k{8000, 1, 1, 1, 0};
+
+// ceil(n * L / M): the 8 kHz samples K15 makes of n input samples at the rate r
+static uint64_t rate_len(uint64_t n, const ResampleRate &r) { return (n * r.L + r.M - 1) / r.M; }
+
+// the argument rules of a capture call at a rate: the rate, and the 8 kHz call's rules with U8 = ceil(U_in * L / M) for U
+static bool capture_rate_args_ok(uint32_t rate, u32 U_in, u32 B, u32 n_len, ResampleRate *r) {
+    if (!resample_rate(rate, r)) return false;
+    const uint64_t U8 = rate_len(U_in, *r);
+    return U8 <= 65535u && capture_args_ok((u32)U8, B, n_len);
+}
+
+// The B captures of a whole-batch capture call staged in one copy, as the 8 kHz body reads them: at 8 kHz the caller's
+// rows in pcm. At another rate the rows of U_in samples go to pcm, then one K15 launch (tag 15) writes rows of
+// U8 = ceil(U_in * L / M) samples to pcm8, and the body reads those. Both carry the 16 bytes of slack of the 8 kHz staging.
+// K15's grid (B * tiles < 2^31, at most 32 tiles of 2 048 outputs per capture) holds for any batch whose features fit
+// device memory; a larger one fails at the launch.
+static const u16 *stage_captures(HostCall &c, const uint16_t *pcm, u32 U_in, u32 B, const ResampleRate &r) {
+    sr_handle *h = c.h;
+    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U_in * 2, 16);
+    if (r.rate == 8000) return d_pcm;
+    const u32 U8 = (u32)rate_len(U_in, r);
+    u16 *d_pcm8 = c.ws<u16>(h->pcm8, (size_t)B * U8 * 2 + 16);
+    c.launch(TAG_RESAMPLE, "launch_resample_adc12", [&] {
+        return launch_resample_adc12(d_pcm, U_in, B, nullptr, r.rate, d_pcm8, U8, nullptr, h->device, h->stream);
+    });
+    return d_pcm8;
+}
+
 extern "C" {
 
 // ---- template bank --------------------------------------------------------------------------------
@@ -556,6 +586,69 @@ static int fft_host(HostCall &c, const uint32_t *packed, const int16_t *frames, 
     return c.finish();
 }
 
+// sr_recognise_batch on B captures of U_in samples at the rate r (host memory; checked by the caller): chunks of about
+// 32 MB of input through PcmGroups and the transport, which count input bytes. At another rate each chunk, once staged
+// (and expanded, when it came packed), gets one K15 launch (tag 15) into pcm8, rows of U8 = ceil(U_in * L / M) samples, and
+// is recognised there. One pcm8 chunk is enough: on the handle's stream K15 of chunk c + 1 follows the recognition of c.
+static int recognise_host(sr_handle *h, const char *name, const uint16_t *pcm, u32 U_in, u32 B, const ResampleRate &r,
+                          u32 n_len, const sr_recog_out *o) {
+    HostCall c(h, name);
+    const u32 U = (u32)rate_len(U_in, r);               // the 8 kHz row
+    // chunk: ~32 MB of input PCM, a multiple of 8 utterances (keeps every chunk base 16-byte aligned)
+    uint32_t chunk = (uint32_t)(((size_t)32 << 20) / ((size_t)U_in * 2));
+    chunk = chunk < 8 ? 8 : (chunk & ~7u);
+    if (chunk > B) chunk = B;
+    const PcmGroups pg(c, U_in, B, chunk);
+    u16 *pcm8 = r.rate == 8000 ? nullptr : c.ws<u16>(h->pcm8, (size_t)chunk * U * 2 + 16);
+    sr_recog_out d;                                     // device mirrors of the non-NULL outputs
+    memset(&d, 0, sizeof d);
+    for_each_output(h, [&](auto m, DevBuf &buf, size_t bytes) {
+        if (!(o->*m)) return;
+        // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36); so is ftr: get_mfcc writes
+        // frm_num and rows < frm_num only (MFCC.C), the caller's other bytes must come back as they were
+        if constexpr (std::is_same_v<decltype(m), atap_tag *sr_recog_out::*> || std::is_same_v<decltype(m), v_ftr_tag *sr_recog_out::*>)
+            c.in(buf, o->*m, B * bytes);
+        d.*m = c.out(buf, o->*m, B * bytes);
+    });
+    uint32_t issued = 0;
+    // one chunk: H2D (plain u16, or 12-bit packed + expansion on the device) -> K15 at a rate -> kernels on its slice of
+    // the outputs. The transport sends the issued-th chunk through buffer issued & 1.
+    auto step = [&](uint32_t ci, int buf, const void *packed_src) -> int {
+        const uint32_t b0 = ci * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
+        const size_t ns = (size_t)nb * U_in;
+        u16 *dpcm = pg.buf(buf);
+        if (packed_src) SR_CK(h, pg.send(issued, h->transport.device_stage(buf), packed_src, ns / 2 * 3));
+        else SR_CK(h, pg.send(issued, dpcm, pcm + (size_t)b0 * U_in, ns * 2));
+        if (packed_src) SR_LAUNCH(h, TAG_NONE, launch_unpack12(h->transport.device_stage(buf), ns, dpcm, h->stream));
+        const u16 *p8 = dpcm;
+        if (pcm8) {
+            SR_LAUNCH(h, TAG_RESAMPLE, launch_resample_adc12(dpcm, U_in, nb, nullptr, r.rate, pcm8, U, nullptr, h->device, h->stream));
+            p8 = pcm8;
+        }
+        const sr_recog_out dc = recog_slice(h, d, b0);
+        if (const int rc = sr_recognise_batch_dev(h, p8, U, nb, n_len, &dc)) return rc;
+        SR_CK(h, pg.done(issued++));
+        return 0;
+    };
+    c.run([&] { return h->transport.send(h, pcm, U_in, B, chunk, step); });
+    const int rc = c.finish();
+    if (rc == 0) h->transport.call_done((uint64_t)B * U_in * 2);
+    return rc;
+}
+
+// save_mdl's body on B staged captures of U samples at 8 kHz (d_pcm, stage_captures): sr_enrol_batch and its form at a rate
+static int enrol_host(HostCall &c, const u16 *d_pcm, u32 U, u32 B, u32 n_len, void *bank_out, u32 slot_stride, u8 *status) {
+    sr_handle *h = c.h;
+    atap_tag *d_atap = c.atap(h->atap, nullptr, B, false);
+    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
+    void *d_ftr = c.ws(h->ftr, (size_t)B * kFtrBytes);
+    u8 *d_status = c.out(h->status, status, (size_t)B);
+    void *d_bank = c.out(h->scratch[0], bank_out, (size_t)B * slot_stride);
+    c.run([&] { return front_end(h, d_pcm, U, B, n_len, d_atap, d_seg, d_ftr, d_status); });
+    c.launch(TAG_NONE, "launch_pack_slots", [&] { return launch_pack_slots(d_ftr, d_status, B, d_bank, slot_stride, h->stream); });
+    return c.finish();
+}
+
 extern "C" {
 
 // ---- host-buffer entry points ---------------------------------------------------------------------
@@ -644,41 +737,18 @@ int sr_recognise_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
     SR_REQUIRE(h, capture_args_ok(U, B, n_len));
     if (B == 0) return 0;
-    HostCall c(h, "sr_recognise_batch");
-    // chunk: ~32 MB of PCM, a multiple of 8 utterances (keeps every chunk base 16-byte aligned)
-    uint32_t chunk = (uint32_t)(((size_t)32 << 20) / ((size_t)U * 2));
-    chunk = chunk < 8 ? 8 : (chunk & ~7u);
-    if (chunk > B) chunk = B;
-    const PcmGroups pg(c, U, B, chunk);
-    sr_recog_out d;                                     // device mirrors of the non-NULL outputs
-    memset(&d, 0, sizeof d);
-    for_each_output(h, [&](auto m, DevBuf &buf, size_t bytes) {
-        if (!(o->*m)) return;
-        // atap is in/out: noise_atap leaves it untouched when n_len % 240 != 0 (VAD.C:33-36); so is ftr: get_mfcc writes
-        // frm_num and rows < frm_num only (MFCC.C), the caller's other bytes must come back as they were
-        if constexpr (std::is_same_v<decltype(m), atap_tag *sr_recog_out::*> || std::is_same_v<decltype(m), v_ftr_tag *sr_recog_out::*>)
-            c.in(buf, o->*m, B * bytes);
-        d.*m = c.out(buf, o->*m, B * bytes);
-    });
-    uint32_t issued = 0;
-    // one chunk: H2D (plain u16, or 12-bit packed + expansion on the device) -> kernels on its slice of the outputs. The
-    // transport sends the issued-th chunk through buffer issued & 1.
-    auto step = [&](uint32_t ci, int buf, const void *packed_src) -> int {
-        const uint32_t b0 = ci * chunk, nb = (b0 + chunk <= B) ? chunk : B - b0;
-        const size_t ns = (size_t)nb * U;
-        u16 *dpcm = pg.buf(buf);
-        if (packed_src) SR_CK(h, pg.send(issued, h->transport.device_stage(buf), packed_src, ns / 2 * 3));
-        else SR_CK(h, pg.send(issued, dpcm, pcm + (size_t)b0 * U, ns * 2));
-        if (packed_src) SR_LAUNCH(h, TAG_NONE, launch_unpack12(h->transport.device_stage(buf), ns, dpcm, h->stream));
-        const sr_recog_out dc = recog_slice(h, d, b0);
-        if (const int rc = sr_recognise_batch_dev(h, dpcm, U, nb, n_len, &dc)) return rc;
-        SR_CK(h, pg.done(issued++));
-        return 0;
-    };
-    c.run([&] { return h->transport.send(h, pcm, U, B, chunk, step); });
-    const int rc = c.finish();
-    if (rc == 0) h->transport.call_done((uint64_t)B * U * 2);
-    return rc;
+    return recognise_host(h, "sr_recognise_batch", pcm, U, B, kRate8k, n_len, o);
+}
+
+// at 8000 the 8 kHz call itself; else recognise_host's K15 on each chunk before its recognition
+int sr_recognise_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate, uint32_t n_len,
+                               const sr_recog_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    ResampleRate r;
+    SR_REQUIRE(h, capture_rate_args_ok(rate, U_in, B, n_len, &r));
+    if (rate == 8000) return sr_recognise_batch(h, pcm, U_in, B, n_len, o);
+    if (B == 0) return 0;
+    return recognise_host(h, "sr_recognise_batch_at_rate", pcm, U_in, B, r, n_len, o);
 }
 
 // save_mdl (main.c:121-138) for B utterances: noise_atap -> VAD -> get_mfcc(seg 0) -> save_ftr_mdl into slot b of a
@@ -690,15 +760,19 @@ int sr_enrol_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, ui
     SR_REQUIRE(h, capture_args_ok(U, B, n_len) && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0);
     if (B == 0) return 0;
     HostCall c(h, "sr_enrol_batch");
-    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    atap_tag *d_atap = c.atap(h->atap, nullptr, B, false);
-    u32 *d_seg = c.ws<u32>(h->seg, (size_t)B * 24);
-    void *d_ftr = c.ws(h->ftr, (size_t)B * kFtrBytes);
-    u8 *d_status = c.out(h->status, status, (size_t)B);
-    void *d_bank = c.out(h->scratch[0], bank_out, (size_t)B * slot_stride);
-    c.run([&] { return front_end(h, d_pcm, U, B, n_len, d_atap, d_seg, d_ftr, d_status); });
-    c.launch(TAG_NONE, "launch_pack_slots", [&] { return launch_pack_slots(d_ftr, d_status, B, d_bank, slot_stride, h->stream); });
-    return c.finish();
+    return enrol_host(c, stage_captures(c, pcm, U, B, kRate8k), U, B, n_len, bank_out, slot_stride, status);
+}
+
+// at 8000 the 8 kHz call itself; else stage_captures' K15 before the 8 kHz body
+int sr_enrol_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate, uint32_t n_len,
+                           void *bank_out, uint32_t slot_stride, uint8_t *status) {
+    SR_REQUIRE(h, h && (B == 0 || (pcm && bank_out)));
+    ResampleRate r;
+    SR_REQUIRE(h, capture_rate_args_ok(rate, U_in, B, n_len, &r) && slot_stride >= (uint32_t)kFtrBytes && slot_stride % 4 == 0);
+    if (rate == 8000) return sr_enrol_batch(h, pcm, U_in, B, n_len, bank_out, slot_stride, status);
+    if (B == 0) return 0;
+    HostCall c(h, "sr_enrol_batch_at_rate");
+    return enrol_host(c, stage_captures(c, pcm, U_in, B, r), (u32)rate_len(U_in, r), B, n_len, bank_out, slot_stride, status);
 }
 
 // get_mdl (DTW.C:217-296) for n pairs: mdl[p] = average of in1[p], in2[p] along their greedy DTW path; dis[p] = the
@@ -908,6 +982,54 @@ static int conn_finish(HostCall &c, const sr_conn_out *o, u32 B, const std::vect
     return 0;
 }
 
+// noise_atap + VAD of B staged captures of U samples at 8 kHz (d_pcm, stage_captures), then (after one synchronisation:
+// the piece plan needs the segments) the long features of every closed segment packed back to back, one decoder sequence
+// per segment with frames, and the join of each capture's segments: sr_recognise_connected_batch and its form at a rate
+static int connected_host(HostCall &c, const u16 *d_pcm, u32 U, u32 B, u32 n_len, u32 penalty, u32 max_words,
+                          const sr_conn_out *o) {
+    sr_handle *h = c.h;
+    std::vector<u32> seg;
+    std::vector<atap_tag> atap;
+    conn_vad(c, d_pcm, U, B, n_len, o, seg, atap);
+    if (c.rc) return c.finish();
+    // the plan: sequence q = the q-th closed segment with frames; rows and word records packed at seq_off[q][0] (frames)
+    std::vector<u32> frm((size_t)B * 3), seq_of((size_t)B * 3, 0xFFFFFFFFu), seq_off, seq_frm;
+    std::vector<u8> status(B);
+    LongPieces pc(h);
+    for (u32 b = 0; b < B; ++b) {
+        for (u32 k = 0; k < 3; ++k) {
+            const u32 r0 = pc.rows, F = pc.add(seg[b * 6 + 2 * k], seg[b * 6 + 2 * k + 1], U, b, atap[b]);   // <= 818: U <= 65535
+            frm[b * 3 + k] = F;
+            if (!F) continue;
+            seq_of[b * 3 + k] = (u32)seq_frm.size();
+            seq_off.insert(seq_off.end(), {r0, r0});
+            seq_frm.push_back(F);
+        }
+        status[b] = seg_status(seg[b * 6 + 1], frm[b * 3]);
+    }
+    const u32 nseq = (u32)seq_frm.size(), rows = pc.rows;
+    s16 *d_feat = c.ws<s16>(h->conn.feat, (size_t)rows * 24);
+    run_pieces(c, d_pcm, U, B, pc, d_feat);
+    const u32 *d_soff = c.in(h->conn.seq_off, seq_off.data(), (size_t)nseq * 8);
+    const u32 *d_sfrm = c.in(h->conn.seq_frm, seq_frm.data(), (size_t)nseq * 4);
+    const u32 *d_sof = c.in(h->conn.seq_of, seq_of.data(), (size_t)B * 12);
+    sr_conn_word *d_sw = c.ws<sr_conn_word>(h->conn.seq_words, (size_t)rows * sizeof(sr_conn_word));
+    u64 *d_stot = c.ws<u64>(h->conn.seq_total, (size_t)nseq * 8);
+    u32 *d_snw = c.ws<u32>(h->conn.seq_n_words, (size_t)nseq * 4);
+    const BankView &bk = h->bank;
+    for (u32 b0 = 0; b0 < nseq; b0 += kSeqChunk)
+        c.launch(TAG_CONN, "launch_dtw_connected", [&] {
+            return launch_dtw_connected(d_feat, 0, d_sfrm, d_soff, b0, std::min(nseq - b0, kSeqChunk), bk.p, bk.n, bk.stride,
+                                        penalty, 0, d_sw, d_snw, d_stot, h->stream);
+        });
+    const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
+    if (d.words || d.nw || d.total)
+        c.launch(TAG_NONE, "launch_conn_concat", [&] {
+            return launch_conn_concat(d_sof, d_soff, d_sw, d_snw, d_stot, B, max_words, d.words, d.nw, d.total, h->stream);
+        });
+    return conn_finish(c, o, B, atap, seg, frm, status);
+}
+
 extern "C" {
 
 // get_mfcc with vv_frm_max replaced by frm_cap: the frame counts and the piece plan come from the segment offsets on the
@@ -954,8 +1076,6 @@ int sr_connected_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_nu
     return c.finish();
 }
 
-// noise_atap + VAD, then (after one synchronisation: the piece plan needs the segments) the long features of every closed
-// segment packed back to back, one decoder sequence per segment with frames, and the join of each capture's segments
 int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len, uint32_t penalty,
                                  uint32_t max_words, const sr_conn_out *o) {
     SR_REQUIRE(h, h && o && (B == 0 || pcm));
@@ -963,47 +1083,20 @@ int sr_recognise_connected_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, 
     if (B == 0) return 0;
     SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
     HostCall c(h, "sr_recognise_connected_batch");
-    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
-    std::vector<u32> seg;
-    std::vector<atap_tag> atap;
-    conn_vad(c, d_pcm, U, B, n_len, o, seg, atap);
-    if (c.rc) return c.finish();
-    // the plan: sequence q = the q-th closed segment with frames; rows and word records packed at seq_off[q][0] (frames)
-    std::vector<u32> frm((size_t)B * 3), seq_of((size_t)B * 3, 0xFFFFFFFFu), seq_off, seq_frm;
-    std::vector<u8> status(B);
-    LongPieces pc(h);
-    for (u32 b = 0; b < B; ++b) {
-        for (u32 k = 0; k < 3; ++k) {
-            const u32 r0 = pc.rows, F = pc.add(seg[b * 6 + 2 * k], seg[b * 6 + 2 * k + 1], U, b, atap[b]);   // <= 818: U <= 65535
-            frm[b * 3 + k] = F;
-            if (!F) continue;
-            seq_of[b * 3 + k] = (u32)seq_frm.size();
-            seq_off.insert(seq_off.end(), {r0, r0});
-            seq_frm.push_back(F);
-        }
-        status[b] = seg_status(seg[b * 6 + 1], frm[b * 3]);
-    }
-    const u32 nseq = (u32)seq_frm.size(), rows = pc.rows;
-    s16 *d_feat = c.ws<s16>(h->conn.feat, (size_t)rows * 24);
-    run_pieces(c, d_pcm, U, B, pc, d_feat);
-    const u32 *d_soff = c.in(h->conn.seq_off, seq_off.data(), (size_t)nseq * 8);
-    const u32 *d_sfrm = c.in(h->conn.seq_frm, seq_frm.data(), (size_t)nseq * 4);
-    const u32 *d_sof = c.in(h->conn.seq_of, seq_of.data(), (size_t)B * 12);
-    sr_conn_word *d_sw = c.ws<sr_conn_word>(h->conn.seq_words, (size_t)rows * sizeof(sr_conn_word));
-    u64 *d_stot = c.ws<u64>(h->conn.seq_total, (size_t)nseq * 8);
-    u32 *d_snw = c.ws<u32>(h->conn.seq_n_words, (size_t)nseq * 4);
-    const BankView &bk = h->bank;
-    for (u32 b0 = 0; b0 < nseq; b0 += kSeqChunk)
-        c.launch(TAG_CONN, "launch_dtw_connected", [&] {
-            return launch_dtw_connected(d_feat, 0, d_sfrm, d_soff, b0, std::min(nseq - b0, kSeqChunk), bk.p, bk.n, bk.stride,
-                                        penalty, 0, d_sw, d_snw, d_stot, h->stream);
-        });
-    const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
-    if (d.words || d.nw || d.total)
-        c.launch(TAG_NONE, "launch_conn_concat", [&] {
-            return launch_conn_concat(d_sof, d_soff, d_sw, d_snw, d_stot, B, max_words, d.words, d.nw, d.total, h->stream);
-        });
-    return conn_finish(c, o, B, atap, seg, frm, status);
+    return connected_host(c, stage_captures(c, pcm, U, B, kRate8k), U, B, n_len, penalty, max_words, o);
+}
+
+// at 8000 the 8 kHz call itself; else stage_captures' K15 before the 8 kHz body
+int sr_recognise_connected_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate,
+                                         uint32_t n_len, uint32_t penalty, uint32_t max_words, const sr_conn_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    ResampleRate r;
+    SR_REQUIRE(h, capture_rate_args_ok(rate, U_in, B, n_len, &r));
+    if (rate == 8000) return sr_recognise_connected_batch(h, pcm, U_in, B, n_len, penalty, max_words, o);
+    if (B == 0) return 0;
+    SR_REQUIRE(h, h->bank.n <= SR_CONN_SLOT_MAX);
+    HostCall c(h, "sr_recognise_connected_batch_at_rate");
+    return connected_host(c, stage_captures(c, pcm, U_in, B, r), (u32)rate_len(U_in, r), B, n_len, penalty, max_words, o);
 }
 
 }  // extern "C"
@@ -1092,43 +1185,13 @@ static void run_grammar(HostCall &c, const s16 *d_feat, const std::vector<u32> &
     });
 }
 
-extern "C" {
-
-// sr_connected_batch under a grammar: the copies from the bank's headers, then the decoder (dtw_grammar_kernel, tag 10)
-int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_num, uint32_t frm_stride, uint32_t B,
-                               const sr_grammar *g, uint32_t penalty, uint32_t max_words, sr_conn_word *words, uint32_t *n_words,
-                               uint64_t *total) {
-    SR_REQUIRE(h, h && (B == 0 || (feat && frm_num && n_words)));
-    if (B == 0) return 0;
-    SR_REQUIRE(h, (uint64_t)B * frm_stride < (1ull << 32));
-    for (u32 b = 0; b < B; ++b) SR_REQUIRE(h, frm_num[b] <= SR_CONN_FRM_MAX && frm_num[b] <= frm_stride);
-    DeviceGuard dg(h->device);
-    std::vector<u32> copy;
-    if (const int rc = gram_copies(h, g, copy)) return rc;
-    std::vector<u32> N(frm_num, frm_num + B), seq((size_t)B * 3);
-    for (u32 b = 0; b < B; ++b) {                          // one segment at frame 0
-        seq[3 * (size_t)b] = b * frm_stride;
-        seq[3 * (size_t)b + 2] = 1023u << 10 | 1023u << 20;
-    }
-    HostCall c(h, "sr_connected_grammar_batch");
-    const s16 *d_feat = c.in(h->conn.feat, feat, (size_t)B * frm_stride * 24);
-    const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
-    run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
-    return c.finish();
-}
-
-// noise_atap + VAD, one synchronisation, the long features of every closed segment packed back to back (a capture's
-// segments adjacent), then one decoder sequence per capture whose words go straight to the caller's records
-int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
-                                         const sr_grammar *g, uint32_t penalty, uint32_t max_words, const sr_conn_out *o) {
-    SR_REQUIRE(h, h && o && (B == 0 || pcm));
-    SR_REQUIRE(h, capture_args_ok(U, B, n_len));
-    if (B == 0) return 0;
-    DeviceGuard dg(h->device);
-    std::vector<u32> copy;
-    if (const int rc = gram_copies(h, g, copy)) return rc;
-    HostCall c(h, "sr_recognise_connected_grammar_batch");
-    const u16 *d_pcm = c.in(h->pcm, pcm, (size_t)B * U * 2, 16);
+// noise_atap + VAD of B staged captures of U samples at 8 kHz (d_pcm, stage_captures), one synchronisation, the long
+// features of every closed segment packed back to back (a capture's segments adjacent), then one decoder sequence per
+// capture under g's copy table whose words go straight to the caller's records: sr_recognise_connected_grammar_batch and
+// its form at a rate
+static int connected_grammar_host(HostCall &c, const u16 *d_pcm, u32 U, u32 B, u32 n_len, const std::vector<u32> &copy,
+                                  const sr_grammar *g, u32 penalty, u32 max_words, const sr_conn_out *o) {
+    sr_handle *h = c.h;
     std::vector<u32> seg;
     std::vector<atap_tag> atap;
     conn_vad(c, d_pcm, U, B, n_len, o, seg, atap);
@@ -1158,6 +1221,60 @@ int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint
     const ConnDev d = conn_outputs(c, B, max_words, o->words, o->n_words, o->total);
     if (d.words || d.nw || d.total) run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
     return conn_finish(c, o, B, atap, seg, frm, status);
+}
+
+extern "C" {
+
+// sr_connected_batch under a grammar: the copies from the bank's headers, then the decoder (dtw_grammar_kernel, tag 10)
+int sr_connected_grammar_batch(sr_handle *h, const int16_t *feat, const uint32_t *frm_num, uint32_t frm_stride, uint32_t B,
+                               const sr_grammar *g, uint32_t penalty, uint32_t max_words, sr_conn_word *words, uint32_t *n_words,
+                               uint64_t *total) {
+    SR_REQUIRE(h, h && (B == 0 || (feat && frm_num && n_words)));
+    if (B == 0) return 0;
+    SR_REQUIRE(h, (uint64_t)B * frm_stride < (1ull << 32));
+    for (u32 b = 0; b < B; ++b) SR_REQUIRE(h, frm_num[b] <= SR_CONN_FRM_MAX && frm_num[b] <= frm_stride);
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    std::vector<u32> N(frm_num, frm_num + B), seq((size_t)B * 3);
+    for (u32 b = 0; b < B; ++b) {                          // one segment at frame 0
+        seq[3 * (size_t)b] = b * frm_stride;
+        seq[3 * (size_t)b + 2] = 1023u << 10 | 1023u << 20;
+    }
+    HostCall c(h, "sr_connected_grammar_batch");
+    const s16 *d_feat = c.in(h->conn.feat, feat, (size_t)B * frm_stride * 24);
+    const ConnDev d = conn_outputs(c, B, max_words, words, n_words, total);
+    run_grammar(c, d_feat, N, seq, copy, g, penalty, max_words, d);
+    return c.finish();
+}
+
+int sr_recognise_connected_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, uint32_t n_len,
+                                         const sr_grammar *g, uint32_t penalty, uint32_t max_words, const sr_conn_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    SR_REQUIRE(h, capture_args_ok(U, B, n_len));
+    if (B == 0) return 0;
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    HostCall c(h, "sr_recognise_connected_grammar_batch");
+    return connected_grammar_host(c, stage_captures(c, pcm, U, B, kRate8k), U, B, n_len, copy, g, penalty, max_words, o);
+}
+
+// at 8000 the 8 kHz call itself; else stage_captures' K15 before the 8 kHz body
+int sr_recognise_connected_grammar_batch_at_rate(sr_handle *h, const uint16_t *pcm, uint32_t U_in, uint32_t B, uint32_t rate,
+                                                 uint32_t n_len, const sr_grammar *g, uint32_t penalty, uint32_t max_words,
+                                                 const sr_conn_out *o) {
+    SR_REQUIRE(h, h && o && (B == 0 || pcm));
+    ResampleRate r;
+    SR_REQUIRE(h, capture_rate_args_ok(rate, U_in, B, n_len, &r));
+    if (rate == 8000) return sr_recognise_connected_grammar_batch(h, pcm, U_in, B, n_len, g, penalty, max_words, o);
+    if (B == 0) return 0;
+    DeviceGuard dg(h->device);
+    std::vector<u32> copy;
+    if (const int rc = gram_copies(h, g, copy)) return rc;
+    HostCall c(h, "sr_recognise_connected_grammar_batch_at_rate");
+    return connected_grammar_host(c, stage_captures(c, pcm, U_in, B, r), (u32)rate_len(U_in, r), B, n_len, copy, g, penalty,
+                                  max_words, o);
 }
 
 }  // extern "C"
@@ -1242,7 +1359,7 @@ template <class F> static int long_groups(HostCall &c, const uint16_t *pcm, u32 
 // The 8 kHz recordings the per-group body of a host-buffer long-form call runs on. The caller's rows of U_in samples
 // (lens: host, or NULL) are staged by long_groups in groups of G recordings, at most kLongGroupBytes of input each, the
 // caller's lens in lng.lens. At 8 kHz the body takes each staged group as it is. At another rate, group() first runs K15
-// (tag 15) from the staged group into lng.pcm8, rows of U8 = ceil(U_in * L / M) samples, and its 8 kHz lengths into
+// (tag 15) from the staged group into pcm8, rows of U8 = ceil(U_in * L / M) samples, and its 8 kHz lengths into
 // lng.lens8, and the body takes those.
 struct LongSource {
     HostCall &c;
@@ -1252,10 +1369,10 @@ struct LongSource {
     u16 *pcm8 = nullptr;                // at a rate: [G][U8], G recordings per staged group
     u32 *lens8 = nullptr;               // at a rate: [B]
     LongSource(HostCall &cc, u32 U, u32 B, const u32 *lens, const ResampleRate &r)
-        : c(cc), U_in(U), U8((u32)(((uint64_t)U * r.L + r.M - 1) / r.M)), G(long_group_size(U, B)), rate(r.rate) {
+        : c(cc), U_in(U), U8(rate_len(U, r)), G(long_group_size(U, B)), rate(r.rate) {
         d_lens = lens ? c.in(c.h->lng.lens, lens, (size_t)B * 4) : nullptr;
         if (rate == 8000) return;
-        pcm8 = c.ws<u16>(c.h->lng.pcm8, (size_t)G * U8 * 2);
+        pcm8 = c.ws<u16>(c.h->pcm8, (size_t)G * U8 * 2);
         lens8 = c.ws<u32>(c.h->lng.lens8, (size_t)B * 4);
     }
     // recordings [b0, b0 + nb) staged at dpcm (rows of U_in samples) as the body reads them: pcm, row length U8, lens
@@ -1279,14 +1396,12 @@ struct LongSource {
 // rules on U8 (lens8 <= U8 follows from lens <= U_in)
 static bool long_rate_args_ok(uint32_t rate, u32 U_in, u32 B, const u32 *lens, u32 n_len, u32 max_segs, ResampleRate *r) {
     if (!resample_rate(rate, r) || U_in > SR_RESAMPLE_U_MAX) return false;
-    const uint64_t U8 = ((uint64_t)U_in * r->L + r->M - 1) / r->M;
+    const uint64_t U8 = rate_len(U_in, *r);
     if (U8 > SR_LONG_U_MAX || !long_host_args_ok((u32)U8, B, nullptr, n_len, max_segs)) return false;
     for (u32 b = 0; lens && b < B; ++b)
         if (lens[b] > U_in) return false;
     return true;
 }
-
-static const ResampleRate kRate8k{8000, 1, 1, 1, 0};
 
 // sr_recognise_long_batch on the recordings of src, per staged group
 static int recognise_long_host(HostCall &c, const uint16_t *pcm, u32 B, const LongSource &src, u32 n_len, u32 max_segs,
@@ -1531,6 +1646,36 @@ static int recognise_long_grammar_host(HostCall &c, const uint16_t *pcm, u32 B, 
     return 0;
 }
 
+// One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]
+// from its own host thread, and every shard writes its results straight into its slice of the caller's host
+// arrays -- with host outputs the "gather" is the D2H copies themselves, no collective is needed. (Device-resident
+// multi-GPU use is one process per GPU with a NCCL all-gather of the score blocks, see bench.py.)
+// All handles must have the same template bank set and the same matcher. Returns the first non-zero shard status.
+// Shards of captures at 8000 Hz run sr_recognise_batch; at another rate sr_recognise_batch_at_rate, whose argument rules
+// every shard applies before any copy (sr_recognise_batch_multi and its form at a rate).
+static int recognise_multi(sr_handle *const *handles, uint32_t n_handles, const uint16_t *pcm, uint32_t U_in, uint32_t B,
+                           uint32_t rate, uint32_t n_len, const sr_recog_out *o, const char *name) {
+    const std::string nm(name);
+    if (!handles || n_handles == 0 || !o) return fail(nullptr, (nm + ": bad arguments").c_str(), cudaSuccess);
+    for (uint32_t g = 0; g < n_handles; ++g)
+        if (!handles[g] || handles[g]->bank.n != handles[0]->bank.n) return fail(nullptr, (nm + ": handles differ").c_str(), cudaSuccess);
+    for (uint32_t g = 0; g < n_handles; ++g)
+        if (!same_match(handles[g], handles[0])) return fail(nullptr, (nm + ": handles differ in their matcher").c_str(), cudaSuccess);
+    std::vector<int> rc(n_handles, 0);
+    std::vector<std::thread> th;
+    for (uint32_t g = 0; g < n_handles; ++g) {
+        const uint32_t lo = (uint32_t)((uint64_t)B * g / n_handles), hi = (uint32_t)((uint64_t)B * (g + 1) / n_handles);
+        const sr_recog_out s = recog_slice(handles[0], *o, lo);
+        th.emplace_back([=, &rc]() {
+            rc[g] = rate == 8000 ? sr_recognise_batch(handles[g], pcm + (size_t)lo * U_in, U_in, hi - lo, n_len, &s)
+                                 : sr_recognise_batch_at_rate(handles[g], pcm + (size_t)lo * U_in, U_in, hi - lo, rate, n_len, &s);
+        });
+    }
+    for (auto &t : th) t.join();
+    for (uint32_t g = 0; g < n_handles; ++g) if (rc[g]) return rc[g];
+    return 0;
+}
+
 extern "C" {
 
 int sr_recognise_long_grammar_batch(sr_handle *h, const uint16_t *pcm, uint32_t U, uint32_t B, const uint32_t *lens,
@@ -1564,28 +1709,16 @@ int sr_recognise_long_grammar_batch_at_rate(sr_handle *h, const uint16_t *pcm, u
     return recognise_long_grammar_host(c, pcm, B, src, copy, n_len, g, penalty, max_segs, max_words, o);
 }
 
-// One host call, several GPUs: the batch is cut into contiguous shards (SURVEY 8e), shard g runs on handles[g]
-// from its own host thread, and every shard writes its results straight into its slice of the caller's host
-// arrays -- with host outputs the "gather" is the D2H copies themselves, no collective is needed. (Device-resident
-// multi-GPU use is one process per GPU with a NCCL all-gather of the score blocks, see bench.py.)
-// All handles must have the same template bank set and the same matcher. Returns the first non-zero shard status.
 int sr_recognise_batch_multi(sr_handle *const *handles, uint32_t n_handles, const uint16_t *pcm, uint32_t U, uint32_t B,
                              uint32_t n_len, const sr_recog_out *o) {
-    if (!handles || n_handles == 0 || !o) return fail(nullptr, "sr_recognise_batch_multi: bad arguments", cudaSuccess);
-    for (uint32_t g = 0; g < n_handles; ++g)
-        if (!handles[g] || handles[g]->bank.n != handles[0]->bank.n) return fail(nullptr, "sr_recognise_batch_multi: handles differ", cudaSuccess);
-    for (uint32_t g = 0; g < n_handles; ++g)
-        if (!same_match(handles[g], handles[0])) return fail(nullptr, "sr_recognise_batch_multi: handles differ in their matcher", cudaSuccess);
-    std::vector<int> rc(n_handles, 0);
-    std::vector<std::thread> th;
-    for (uint32_t g = 0; g < n_handles; ++g) {
-        const uint32_t lo = (uint32_t)((uint64_t)B * g / n_handles), hi = (uint32_t)((uint64_t)B * (g + 1) / n_handles);
-        const sr_recog_out s = recog_slice(handles[0], *o, lo);
-        th.emplace_back([=, &rc]() { rc[g] = sr_recognise_batch(handles[g], pcm + (size_t)lo * U, U, hi - lo, n_len, &s); });
-    }
-    for (auto &t : th) t.join();
-    for (uint32_t g = 0; g < n_handles; ++g) if (rc[g]) return rc[g];
-    return 0;
+    return recognise_multi(handles, n_handles, pcm, U, B, 8000, n_len, o, "sr_recognise_batch_multi");
+}
+
+// at 8000 the 8 kHz call itself; else the same shards, each running sr_recognise_batch_at_rate
+int sr_recognise_batch_multi_at_rate(sr_handle *const *handles, uint32_t n_handles, const uint16_t *pcm, uint32_t U_in,
+                                     uint32_t B, uint32_t rate, uint32_t n_len, const sr_recog_out *o) {
+    if (rate == 8000) return sr_recognise_batch_multi(handles, n_handles, pcm, U_in, B, n_len, o);
+    return recognise_multi(handles, n_handles, pcm, U_in, B, rate, n_len, o, "sr_recognise_batch_multi_at_rate");
 }
 
 int sr_fft_mag_batch(sr_handle *h, const int16_t *frames, uint32_t len, uint32_t n, uint32_t *mag) {

@@ -203,6 +203,12 @@ struct sr_handle {
     // grow-only device workspaces; scratch[] serves the secondary entry points (FFT, get_dis, get_mdl, dtw_limit, the
     // 12-bit expander, the sqrt check, enrol's bank image, dtw()'s one-slot bank) and is never read by a recognise call
     DevBuf pcm, atap, seg, ftr, score, best, best_alt, status, bidx, bdis, cmd, scratch[3];
+    // pcm8: input staged in pcm at another rate, resampled to 8 kHz by K15 for the 8 kHz body to read. The capture calls
+    // at a rate: sr_recognise_batch_at_rate (one chunk, [nb][U8]), sr_enrol_batch_at_rate,
+    // sr_recognise_connected_batch_at_rate, sr_recognise_connected_grammar_batch_at_rate (the whole batch, [B][U8]);
+    // the long-form calls at a rate: sr_recognise_long_batch_at_rate, sr_recognise_long_grammar_batch_at_rate (one
+    // staged group, [G][U8])
+    DevBuf pcm8;
     // The workspace table of the other call families: one buffer per thing held, each listed with what it holds and the
     // calls that use it. Where calls put different things in one buffer, each call's contents are named.
     //
@@ -245,9 +251,9 @@ struct sr_handle {
     // - per_seg: the caller's per-segment output. sr_vad_long_batch: seg_off; sr_recognise_long_batch: the records
     // - lens: the caller's lens. sr_vad_long_batch, sr_recognise_long_batch, sr_recognise_long_grammar_batch and their
     //   _at_rate forms (there in input samples)
-    // - pcm8, lens8: one staged group resampled to 8 kHz ([G][U8] samples) and every recording's 8 kHz length [B].
-    //   sr_recognise_long_batch_at_rate, sr_recognise_long_grammar_batch_at_rate
-    struct { DevBuf info, seg_off, first, n_flat, seg2, row, slot, atap_seg, status, keys, ftr, atap, n_segs, per_seg, lens, pcm8, lens8; } lng;
+    // - lens8: every recording's 8 kHz length [B] (its samples are in pcm8). sr_recognise_long_batch_at_rate,
+    //   sr_recognise_long_grammar_batch_at_rate
+    struct { DevBuf info, seg_off, first, n_flat, seg2, row, slot, atap_seg, status, keys, ftr, atap, n_segs, per_seg, lens, lens8; } lng;
     // alignment: sr_dtw_path_batch and sr_average_bank
     // - in_bank: sr_dtw_path_batch: in; sr_average_bank: the bank image
     // - mdl_out: sr_dtw_path_batch: mdl; sr_average_bank: the output bank image

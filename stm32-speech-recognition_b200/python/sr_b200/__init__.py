@@ -249,6 +249,12 @@ def lib():
         for name in ("sr_recognise_batch", "sr_recognise_batch_dev"):
             getattr(L, name).argtypes = [vp, vp, u32, u32, u32, C.POINTER(RecogOut)]
         L.sr_recognise_batch_multi.argtypes = [C.POINTER(vp), u32, vp, u32, u32, u32, C.POINTER(RecogOut)]
+        L.sr_recognise_batch_at_rate.argtypes = [vp, vp, u32, u32, u32, u32, C.POINTER(RecogOut)]
+        L.sr_recognise_batch_multi_at_rate.argtypes = [C.POINTER(vp), u32, vp, u32, u32, u32, u32, C.POINTER(RecogOut)]
+        L.sr_enrol_batch_at_rate.argtypes = [vp, vp, u32, u32, u32, u32, vp, u32, vp]
+        L.sr_recognise_connected_batch_at_rate.argtypes = [vp, vp, u32, u32, u32, u32, u32, u32, C.POINTER(ConnOut)]
+        L.sr_recognise_connected_grammar_batch_at_rate.argtypes = [vp, vp, u32, u32, u32, u32, vp, u32, u32,
+                                                                   C.POINTER(ConnOut)]
         L.sr_fft_mag_batch.argtypes = [vp, vp, u32, u32, vp]
         L.sr_fft_raw_batch.argtypes = [vp, vp, u32, vp]
         L.sr_debug_fft_raw_n.argtypes = [vp, vp, u32, u32, vp]
@@ -400,17 +406,28 @@ class Handle:
         self._ck(lib().sr_dtw_batch(self._h, _p(ftr_in), B, flags, band_r, _p(score), _p(bi), _p(bd)))
         return score, bi, bd
 
-    def recognise(self, pcm, n_len=2400, want=RECOG_FIELDS):
+    def recognise(self, pcm, n_len=2400, want=RECOG_FIELDS, rate=None):
+        """spch_recg on captures pcm [B, U] (sr_recognise_batch). rate: None (8 kHz input), or the input rate of
+        sr_recognise_batch_at_rate (include/sr_synth.h; any of RESAMPLE_RATES): pcm then counts samples at that rate,
+        while n_len and the outputs stay in 8 kHz samples"""
         B, U = pcm.shape
         out = _recog_arrays(B, self.n_slot, want)
-        self._ck(lib().sr_recognise_batch(self._h, _p(pcm), U, B, n_len, C.byref(_recog_out(out))))
+        if rate is None:
+            self._ck(lib().sr_recognise_batch(self._h, _p(pcm), U, B, n_len, C.byref(_recog_out(out))))
+        else:
+            self._ck(lib().sr_recognise_batch_at_rate(self._h, _p(pcm), U, B, rate, n_len, C.byref(_recog_out(out))))
         return out
 
-    def enrol(self, pcm, n_len=2400, slot_stride=4096):
+    def enrol(self, pcm, n_len=2400, slot_stride=4096, rate=None):
+        """save_mdl on captures pcm [B, U] (sr_enrol_batch): (bank [B, slot_stride] u8, status [B]). rate: None (8 kHz
+        input), or the input rate of sr_enrol_batch_at_rate (include/sr_synth.h), as in recognise"""
         B, U = pcm.shape
         bank = np.zeros((B, slot_stride), np.uint8)
         status = np.zeros(B, np.uint8)
-        self._ck(lib().sr_enrol_batch(self._h, _p(pcm), U, B, n_len, _p(bank), slot_stride, _p(status)))
+        if rate is None:
+            self._ck(lib().sr_enrol_batch(self._h, _p(pcm), U, B, n_len, _p(bank), slot_stride, _p(status)))
+        else:
+            self._ck(lib().sr_enrol_batch_at_rate(self._h, _p(pcm), U, B, rate, n_len, _p(bank), slot_stride, _p(status)))
         return bank, status
 
     def get_mdl(self, in1, in2, mdl=None):
@@ -470,9 +487,10 @@ class Handle:
                                           _p(n_words), _p(total)))
         return words, n_words, total
 
-    def recognise_connected(self, pcm, penalty, max_words, n_len=2400, want=CONN_FIELDS, out=None):
+    def recognise_connected(self, pcm, penalty, max_words, n_len=2400, want=CONN_FIELDS, out=None, rate=None):
         """noise_atap -> VAD -> long features of every segment -> connected words (sr_recognise_connected_batch): a dict
-        of the sr_conn_out fields named in `want` (or the arrays of `out`, which the call fills in place)"""
+        of the sr_conn_out fields named in `want` (or the arrays of `out`, which the call fills in place). rate: None
+        (8 kHz input), or the input rate of sr_recognise_connected_batch_at_rate (include/sr_synth.h), as in recognise"""
         B, U = pcm.shape
         if out is None:
             shape = {"atap": (B, ATAP_DTYPE), "seg_off": ((B, 3, 2), np.uint32), "frm_num": ((B, 3), np.uint32),
@@ -480,7 +498,11 @@ class Handle:
                      "status": (B, np.uint8)}
             out = {k: np.zeros(*shape[k]) for k in CONN_FIELDS if k in want}
         o = ConnOut(*[_p(out.get(k)) for k in CONN_FIELDS])
-        self._ck(lib().sr_recognise_connected_batch(self._h, _p(pcm), U, B, n_len, penalty, max_words, C.byref(o)))
+        if rate is None:
+            self._ck(lib().sr_recognise_connected_batch(self._h, _p(pcm), U, B, n_len, penalty, max_words, C.byref(o)))
+        else:
+            self._ck(lib().sr_recognise_connected_batch_at_rate(self._h, _p(pcm), U, B, rate, n_len, penalty, max_words,
+                                                                C.byref(o)))
         return out
 
     def connected_grammar(self, feat, frm_num, grammar_, penalty, max_words, words=None, want_total=True):
@@ -498,10 +520,12 @@ class Handle:
                                                   penalty, max_words, _p(words), _p(n_words), _p(total)))
         return words, n_words, total
 
-    def recognise_connected_grammar(self, pcm, grammar_, penalty, max_words, n_len=2400, want=CONN_FIELDS, out=None):
+    def recognise_connected_grammar(self, pcm, grammar_, penalty, max_words, n_len=2400, want=CONN_FIELDS, out=None,
+                                    rate=None):
         """noise_atap -> VAD -> long features -> one grammar decode per capture across its segments
         (sr_recognise_connected_grammar_batch): a dict of the sr_conn_out fields named in `want` (or the arrays of `out`,
-        filled in place)"""
+        filled in place). rate: None (8 kHz input), or the input rate of sr_recognise_connected_grammar_batch_at_rate
+        (include/sr_synth.h), as in recognise"""
         B, U = pcm.shape
         if out is None:
             shape = {"atap": (B, ATAP_DTYPE), "seg_off": ((B, 3, 2), np.uint32), "frm_num": ((B, 3), np.uint32),
@@ -510,8 +534,14 @@ class Handle:
             out = {k: np.zeros(*shape[k]) for k in CONN_FIELDS if k in want}
         o = ConnOut(*[_p(out.get(k)) for k in CONN_FIELDS])
         g = grammar(grammar_)
-        self._ck(lib().sr_recognise_connected_grammar_batch(self._h, _p(pcm), U, B, n_len, None if g is None else C.byref(g),
-                                                            penalty, max_words, C.byref(o)))
+        if rate is None:
+            self._ck(lib().sr_recognise_connected_grammar_batch(self._h, _p(pcm), U, B, n_len,
+                                                                None if g is None else C.byref(g), penalty, max_words,
+                                                                C.byref(o)))
+        else:
+            self._ck(lib().sr_recognise_connected_grammar_batch_at_rate(self._h, _p(pcm), U, B, rate, n_len,
+                                                                        None if g is None else C.byref(g), penalty,
+                                                                        max_words, C.byref(o)))
         return out
 
     # -- long-form VAD and per-segment recognition (include/sr_long.h)
@@ -697,14 +727,21 @@ def comm_unique_id():
     return bytes(buf)
 
 
-def recognise_multi(handles, pcm, n_len=2400, want=("best_idx", "best_dis", "cmd", "status", "score", "seg_off")):
-    """sr_recognise_batch_multi: one host call over several handles (one per GPU); numpy in/out"""
+def recognise_multi(handles, pcm, n_len=2400, want=("best_idx", "best_dis", "cmd", "status", "score", "seg_off"),
+                    rate=None):
+    """sr_recognise_batch_multi: one host call over several handles (one per GPU); numpy in/out. rate: None (8 kHz
+    input), or the input rate of sr_recognise_batch_multi_at_rate (include/sr_synth.h), as in Handle.recognise"""
     B, U = pcm.shape
     out = _recog_arrays(B, handles[0].n_slot, want)
     arr = (C.c_void_p * len(handles))(*[h._h for h in handles])
-    rc = lib().sr_recognise_batch_multi(arr, len(handles), _p(pcm), U, B, n_len, C.byref(_recog_out(out)))
+    if rate is None:
+        name = "sr_recognise_batch_multi"
+        rc = lib().sr_recognise_batch_multi(arr, len(handles), _p(pcm), U, B, n_len, C.byref(_recog_out(out)))
+    else:
+        name = "sr_recognise_batch_multi_at_rate"
+        rc = lib().sr_recognise_batch_multi_at_rate(arr, len(handles), _p(pcm), U, B, rate, n_len, C.byref(_recog_out(out)))
     if rc != 0:
-        raise SrError("sr_recognise_batch_multi failed (%d): %s" % (rc, lib().sr_last_error(None).decode()))
+        raise SrError("%s failed (%d): %s" % (name, rc, lib().sr_last_error(None).decode()))
     return out
 
 
